@@ -25,10 +25,6 @@ NVCC_FLAGS = [
     "-Xcompiler", "-fPIC,-ffp-contract=off,-Wall",
     "-ccbin", "/usr/bin/g++",
 ]
-# Development knobs of the reweight kernel (defaults in csrc/kernels.cu).
-for _knob in ("BB200_RW_THREADS", "BB200_RW_UNROLL", "BB200_RW_BLOCKS", "BB200_BEAM_BLOCKS", "BB200_RS_UNROLL", "BB200_BEAM_RAYS", "BB200_QS_LARGE_ITEMS", "BB200_WALK_BLOCKS", "BB200_RS_BLOCKS", "BB200_RW_CHUNK"):
-    if os.environ.get(_knob):
-        NVCC_FLAGS.append(f"-D{_knob}=" + os.environ[_knob])
 
 
 def nvcc() -> str:

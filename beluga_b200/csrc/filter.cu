@@ -3,7 +3,6 @@
 #include <algorithm>
 #include <atomic>
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 #include <limits>
 
@@ -107,19 +106,6 @@ Filter::Filter(const bb200_filter_config& config) : config_(config) {
     return;
   }
   if (config_.global_count == 0) config_.global_count = config_.capacity;
-  if (const char* v = std::getenv("BB200_SCHEDULE")) schedule_enabled_ = std::atoi(v) != 0;  // development knob: 0 disables the pose-sorted schedule
-  if (const char* v = std::getenv("BB200_TILED")) tiled_layout_ = std::atoi(v) != 0;         // development knob: table layout
-  if (const char* v = std::getenv("BB200_PARAM_POINTS")) param_points_ = std::atoi(v) != 0;  // development knob: scan as kernel parameters
-  if (const char* v = std::getenv("BB200_BEAM_ETA_TABLE")) beam_eta_table_ = std::atoi(v) != 0;  // development knob: tabulated beam normalisers
-  if (const char* v = std::getenv("BB200_FIXED")) fixed_lookup_ = std::atoi(v) != 0;         // development knob: fixed-point lookup kernel
-  if (const char* v = std::getenv("BB200_POLL_COMPLETION")) poll_completion_ = std::atoi(v) != 0;  // development knob: 0 = cudaStreamSynchronize
-  if (const char* v = std::getenv("BB200_PREDICT_SCHEDULE")) predict_schedule_ = std::atoi(v) != 0;  // development knob: host-predicted pose bins
-  if (const char* v = std::getenv("BB200_PREFETCH_TABLE")) prefetch_table_ = std::atoi(v) != 0;  // development knob: L2 prefetch of the likelihood table
-  if (const char* v = std::getenv("BB200_BEAM_TWO_PASS")) beam_two_pass_ = std::atoi(v) != 0;  // development knob: walk + mixture kernels
-  if (const char* v = std::getenv("BB200_PER_BIN")) schedule_per_bin_ = std::atof(v);        // development knob: particles per pose bin
-  if (const char* v = std::getenv("BB200_X_SPLIT")) schedule_x_split_ = std::atof(v);        // development knob: bins per warp along x
-  if (const char* v = std::getenv("BB200_EQUAL_MASS")) schedule_equal_mass_ = std::atoi(v) != 0;  // development knob: 0 = equal-size bins
-  if (const char* v = std::getenv("BB200_LEVER")) schedule_lever_ = std::atof(v);            // development knob: heading lever arm / mean range
   capacity_ = config.capacity;
   first_index_ = config.first_index;
 #define BB_TRY(expr)                                \
@@ -214,7 +200,6 @@ Filter::~Filter() {
   cudaFree(kld_hashes_global_);
   cudaFree(points_);
   cudaFreeHost(points_host_);
-  cudaFree(table_);
   cudaFree(tiled_);
   cudaFree(bordered_);
   cudaFree(beam_eta_);
@@ -569,8 +554,8 @@ int Filter::step_phase(int phase) {
     case kPhaseReweight: {
       mark("begin_step");
       {
-        const bool scheduled = schedule_enabled_ && n_ >= kScheduleMinParticles;
-        const bool warm = prefetch_table_ && sensor_ != BB200_SENSOR_BEAM && field_.use_fixed && bordered_bytes_ <= (96ull << 20);
+        const bool scheduled = n_ >= kScheduleMinParticles;
+        const bool warm = sensor_ != BB200_SENSOR_BEAM && field_.use_fixed && bordered_bytes_ <= (96ull << 20);
         launch_begin_fused_step(scalars_, tile_state_, scan_tile_count(n_), sched_, scheduled ? counters_ : nullptr, schedule_max_bins(), sched_tiles_,
                                 schedule_tile_count(), warm ? bordered_ : nullptr, bordered_bytes_, stream_);
         BB_LAUNCHED("begin_step");
@@ -657,7 +642,7 @@ int Filter::step_phase(int phase) {
       }
       // the last block sums the moments (one GPU: straight into pinned host memory, with the step's completion ticket)
       step_.poll_seq = 0;
-      if (!sharded && poll_completion_ && !timing_) {
+      if (!sharded && !timing_) {
         step_seq_ = step_seq_ == 0x7fffffff ? 1 : step_seq_ + 1;
         step_.poll_seq = step_seq_;
         summary_host_->seq = 0;  // nothing of this filter is in flight: the previous step was seen to end
@@ -999,37 +984,23 @@ int Filter::set_likelihood_field_map(const bb200_likelihood_field_param& p, cons
   const size_t count = field_host_.size();
   // Per-cell f(pz) in double: pz^3 (likelihood_field_model.hpp:84-89) or log pz (prob model :84-86).
   if (count + 64 >= (1ull << 32)) return fail(BB200_ERR_CAPACITY, "map too large for 32-bit cell indices");
-  std::vector<double> table(count + 1);
+  std::vector<double> table(count);  // row-major: the source of the layout the map's kernel reads
   auto f = [prob](float pzf) {
     const double pz = static_cast<double>(pzf);
     return prob ? std::log(pz) : pz * pz * pz;
   };
   for (size_t i = 0; i < count; ++i) table[i] = f(field_host_[i]);
-  table[count] = f(static_cast<float>(1. / p.max_laser_distance));  // spare cell for out-of-grid end points
+  const double unknown = f(static_cast<float>(1. / p.max_laser_distance));  // what out-of-grid end points read
   BB_CHECK(cudaStreamSynchronize(stream_));
-  cudaFree(table_);
-  table_ = nullptr;
-  BB_CHECK(dev_alloc(&table_, count + 1));
-  BB_CHECK(cudaMemcpyAsync(table_, table.data(), (count + 1) * sizeof(double), cudaMemcpyHostToDevice, stream_));
-  BB_CHECK(cudaStreamSynchronize(stream_));
-  // Tiled copy (4x4-cell tiles, Z-order inside) for the beam-parallel lookup kernel.
-  const int tiles_x = (g.width + 3) / 4, tiles_y = (g.height + 3) / 4;
-  const double unknown = f(static_cast<float>(1. / p.max_laser_distance));
-  if (static_cast<size_t>(tiles_x) * tiles_y * 16 + 64 >= (1ull << 32)) return fail(BB200_ERR_CAPACITY, "map too large for 32-bit cell indices");
-  std::vector<double> tiled(static_cast<size_t>(tiles_x) * tiles_y * 16 + 1, unknown);
-  for (int yi = 0; yi < g.height; ++yi)
-    for (int xi = 0; xi < g.width; ++xi) tiled[tiled_index(xi, yi, tiles_x)] = table[static_cast<size_t>(yi) * g.width + xi];
-  cudaFree(tiled_);
-  tiled_ = nullptr;
-  BB_CHECK(dev_alloc(&tiled_, tiled.size()));
-  BB_CHECK(cudaMemcpyAsync(tiled_, tiled.data(), tiled.size() * sizeof(double), cudaMemcpyHostToDevice, stream_));
-  BB_CHECK(cudaStreamSynchronize(stream_));
-  // Bordered tile layout for the fixed-point kernel.
   field_.use_fixed = 0;
   field_.bordered = nullptr;
+  field_.tiled = nullptr;
   cudaFree(bordered_);
   bordered_ = nullptr;
-  if (fixed_lookup_ && g.width + 2 <= kFixedMaxSide && g.height + 2 <= kFixedMaxSide) {
+  cudaFree(tiled_);
+  tiled_ = nullptr;
+  if (g.width + 2 <= kFixedMaxSide && g.height + 2 <= kFixedMaxSide) {
+    // Bordered tile layout for the fixed-point kernel.
     int kx = 0;
     while ((1 << kx) < (g.width + 2 + 3) / 4) ++kx;
     const size_t tile_rows = static_cast<size_t>((g.height + 2 + 3) / 4);
@@ -1047,17 +1018,24 @@ int Filter::set_likelihood_field_map(const bb200_likelihood_field_param& p, cons
     field_.border_x_max = static_cast<uint32_t>(4 * (g.width + 1) + 3);
     field_.border_y_max = static_cast<uint32_t>(g.height + 1);
     field_.use_fixed = 1;
+  } else {
+    // Tiled layout (4x4-cell tiles, no border, spare cell at the end) for the general kernel.
+    const int tiles_x = (g.width + 3) / 4, tiles_y = (g.height + 3) / 4;
+    if (static_cast<size_t>(tiles_x) * tiles_y * 16 + 64 >= (1ull << 32)) return fail(BB200_ERR_CAPACITY, "map too large for 32-bit cell indices");
+    std::vector<double> tiled(static_cast<size_t>(tiles_x) * tiles_y * 16 + 1, unknown);
+    for (int yi = 0; yi < g.height; ++yi)
+      for (int xi = 0; xi < g.width; ++xi) tiled[tiled_index(xi, yi, tiles_x)] = table[static_cast<size_t>(yi) * g.width + xi];
+    BB_CHECK(dev_alloc(&tiled_, tiled.size()));
+    BB_CHECK(cudaMemcpyAsync(tiled_, tiled.data(), tiled.size() * sizeof(double), cudaMemcpyHostToDevice, stream_));
+    BB_CHECK(cudaStreamSynchronize(stream_));
+    field_.tiled = tiled_;
+    field_.tiles_x = tiles_x;
+    field_.spare_index = static_cast<uint32_t>(tiled.size() - 1);
   }
-  field_.tiled = tiled_;
-  field_.tiles_x = tiles_x;
-  field_.use_tiled = tiled_layout_ ? 1 : 0;
-  field_.spare_index = static_cast<uint32_t>(tiled_layout_ ? tiled.size() - 1 : count);
-
-  field_.table = table_;
   field_.width = g.width;
   field_.height = g.height;
   field_.inv_resolution = 1. / g.resolution;
-  field_.unknown_value = f(static_cast<float>(1. / p.max_laser_distance));
+  field_.unknown_value = unknown;
   field_.init = prob ? 0.0 : 1.0;
   field_.exp_epilogue = prob ? 1 : 0;
   field_.world_to_field = pose_inverse(pose_from_array(g.origin));
@@ -1120,7 +1098,7 @@ int Filter::set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& 
   beam_ = BeamParams{p.z_hit, p.z_short, p.z_max, p.z_rand, p.sigma_hit, p.lambda_short, p.beam_max_range, nullptr, 0};
   cudaFree(beam_eta_);
   beam_eta_ = nullptr;
-  if (const uint32_t entries = beam_eta_table_ ? beam_eta_entries(p.beam_max_range, g.resolution) : 0u) {
+  if (const uint32_t entries = beam_eta_entries(p.beam_max_range, g.resolution)) {
     BB_CHECK(dev_alloc(&beam_eta_, entries));
     launch_beam_eta_table(beam_, g.resolution, beam_eta_, entries, stream_);
     BB_LAUNCHED("beam_eta_table");
@@ -1260,7 +1238,7 @@ int Filter::upload_points(const double* points_xy, uint64_t n_points) {
 bool Filter::predict_schedule(const MotionSampling& s, Schedule* grid) const {
   // The cloud after this step's propagate, from what the host already knows: the last estimate (the particles carry unit
   // weights, so it describes the raw cloud) composed with the motion means, spread widened by the motion noise.
-  if (!cloud_known_ || !predict_schedule_) return false;
+  if (!cloud_known_) return false;
   const bb200_estimate& e = cloud_;
   const Pose2 mean = motion_apply(s.model, Pose2{e.mean[0], e.mean[1], e.mean[2], e.mean[3]}, s.mean[0], s.mean[1], s.mean[2], Rot2{s.first_c, s.first_s});
   double var_theta = std::max(e.cov[8], 0.0) + s.stddev[0] * s.stddev[0];
@@ -1271,13 +1249,12 @@ bool Filter::predict_schedule(const MotionSampling& s, Schedule* grid) const {
   const double vx = e.cov[0] + spread, vy = e.cov[4] + spread;
   if (!std::isfinite(var_theta) || !std::isfinite(vx) || !std::isfinite(vy) || !std::isfinite(mean.x) || !std::isfinite(mean.y)) return false;
   const double r = std::exp(-0.5 * var_theta);
-  schedule_from_moments(*grid, r * mean.c, r * mean.s, mean.x, mean.y, vx, vy, static_cast<double>(n_), schedule_lever_ * points_mean_range_,
-                        0.5 * grid_resolution_, schedule_per_bin_, schedule_x_split_, schedule_equal_mass_);
+  schedule_from_moments(*grid, r * mean.c, r * mean.s, mean.x, mean.y, vx, vy, static_cast<double>(n_), points_mean_range_, 0.5 * grid_resolution_);
   return true;
 }
 
 int Filter::enqueue_propagate_reweight(const MotionSampling* sampling, uint32_t step, bool do_reweight, uint64_t n_points, bool counters_reset) {
-  const bool scheduled = do_reweight && schedule_enabled_ && n_ >= kScheduleMinParticles;
+  const bool scheduled = do_reweight && n_ >= kScheduleMinParticles;
   Schedule grid{};
   const uint32_t* perm = nullptr;
   if (scheduled && counters_reset && sampling != nullptr && predict_schedule(*sampling, &grid)) {
@@ -1297,7 +1274,7 @@ int Filter::enqueue_propagate_reweight(const MotionSampling* sampling, uint32_t 
   }
   if (scheduled && perm == nullptr) {
     mark("schedule");
-    launch_build_schedule(states_[cur_], n_, sched_, bins_, counters_, perm_, sched_tiles_, schedule_lever_ * points_mean_range_, 0.5 * grid_resolution_, schedule_per_bin_, schedule_x_split_, schedule_equal_mass_, stream_);
+    launch_build_schedule(states_[cur_], n_, sched_, bins_, counters_, perm_, sched_tiles_, points_mean_range_, 0.5 * grid_resolution_, stream_);
     BB_LAUNCHED_N("schedule", 4);
     perm = perm_;
   }
@@ -1307,7 +1284,7 @@ int Filter::enqueue_propagate_reweight(const MotionSampling* sampling, uint32_t 
       uint64_t pass = 0;
       // spans of the walk's 32-bit arithmetic: far ends lie within beam_max_range of the source, sources inside the grid
       const double reach_cells = beam_.beam_max_range * occupancy_view_.inv_resolution + 4.0;
-      if (beam_two_pass_ && n_points > 0 && occupancy_view_.free_padded != nullptr && reach_cells < static_cast<double>(1 << 21)) {
+      if (n_points > 0 && occupancy_view_.free_padded != nullptr && reach_cells < static_cast<double>(1 << 21)) {
         // hit words of one pass: at most 3 GiB, whole warps of particles
         pass = std::min<uint64_t>(n_, std::max<uint64_t>(32, ((3ull << 30) / (4ull * n_points)) / 32 * 32));
         const uint64_t words = beam_hit_words(pass, static_cast<uint32_t>(n_points));
@@ -1337,7 +1314,7 @@ int Filter::enqueue_propagate_reweight(const MotionSampling* sampling, uint32_t 
       }
     } else {
       mark("reweight_lfm");
-      launch_reweight_lfm(states_[cur_], weights_, n_, perm, field_, points_, param_points_ ? points_host_ : nullptr, static_cast<uint32_t>(n_points),
+      launch_reweight_lfm(states_[cur_], weights_, n_, perm, field_, points_, points_host_, static_cast<uint32_t>(n_points),
                           points_radius_, scalars_, stream_);
       BB_LAUNCHED("reweight_lfm");
     }

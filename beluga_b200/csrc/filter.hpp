@@ -248,14 +248,6 @@ class Filter {
 
   // execution schedule (pose-sorted processing order of the reweight kernels)
   static constexpr uint64_t kScheduleMinParticles = 32768;
-  bool schedule_enabled_{true};
-  bool tiled_layout_{true};
-  bool fixed_lookup_{true};
-  bool param_points_{true};
-  double schedule_per_bin_{4.0};
-  double schedule_lever_{1.0};
-  double schedule_x_split_{8.0};
-  bool schedule_equal_mass_{true};
   Schedule* sched_{nullptr};
   uint32_t* bins_{nullptr};
   uint2* bin_rank_{nullptr};
@@ -266,11 +258,9 @@ class Filter {
   // maps
   int sensor_{-1};
   std::vector<float> field_host_;
-  double* table_{nullptr};
   double* tiled_{nullptr};
   double* bordered_{nullptr};
   uint64_t bordered_bytes_{0};
-  bool prefetch_table_{true};
   FieldView field_{};
   int8_t* occupancy_{nullptr};
   uint8_t* free_distance_{nullptr};
@@ -280,8 +270,6 @@ class Filter {
   double2* beam_eta_{nullptr};
   uint32_t* beam_hits_{nullptr};   // two-pass beam model: hit word per (beam, particle) of one pass
   uint64_t beam_hits_words_{0};
-  bool beam_two_pass_{true};
-  bool beam_eta_table_{true};
   uint32_t* free_cells_{nullptr};
   uint64_t n_free_{0};
   int grid_width_{0}, grid_height_{0};
@@ -291,8 +279,6 @@ class Filter {
   double pivot_[2]{0.0, 0.0};
   bb200_estimate cloud_{};     // last estimate, when it describes the raw (unit-weight) cloud
   bool cloud_known_{false};
-  bool predict_schedule_{true};
-  bool poll_completion_{true};
   int step_seq_{0};
 
   // timing

@@ -17,29 +17,7 @@
 // reference's operation order without FMA contraction (the file is compiled with -fmad=false).
 #include "kernels.cuh"
 
-#include <cstdlib>
 #include <cstring>
-
-// Tuning knobs of the reweight kernel (overridable with -D from beluga_b200/build.py).
-#ifndef BB200_RW_THREADS
-#define BB200_RW_THREADS 256
-#endif
-#ifndef BB200_RW_UNROLL
-#define BB200_RW_UNROLL 2
-#endif
-#ifndef BB200_RW_BLOCKS
-#define BB200_RW_BLOCKS 4
-#endif
-#ifndef BB200_RW_CHUNK
-#define BB200_RW_CHUNK 0  // > 0: experiment -- chunks of adjacent tasks per CTA instead of one global ticket per warp
-#endif
-#ifndef BB200_RS_UNROLL
-#define BB200_RS_UNROLL 2  // particles per thread and round in resample_scatter_kernel
-#endif
-#ifndef BB200_RS_BLOCKS
-#define BB200_RS_BLOCKS 3  // resident CTAs per SM the kernel is compiled for (register cap); (blocks, unroll) = (3, 2) was chosen
-                          // by a sweep at 1M on a B200, carried over to the H100 without re-measuring
-#endif
 
 #include <algorithm>
 #include <cfloat>
@@ -330,33 +308,25 @@ __global__ void schedule_reset_kernel(Schedule* sched) {
   sched->tile_ticket = 0;
 }
 
-__global__ void schedule_params_kernel(Schedule* sched, uint64_t n, double mean_range, double min_bin, double per_bin, double x_split,
-                                       bool equal_mass) {
+__global__ void schedule_params_kernel(Schedule* sched, uint64_t n, double mean_range, double min_bin) {
   const double inv_n = 1.0 / static_cast<double>(n);
   const double mx = sched->sums[2] * inv_n, my = sched->sums[3] * inv_n;
   schedule_from_moments(*sched, sched->sums[0] * inv_n, sched->sums[1] * inv_n, mx, my, sched->sums[4] * inv_n - mx * mx,
-                        sched->sums[5] * inv_n - my * my, static_cast<double>(n), mean_range, min_bin, per_bin, x_split, equal_mass);
+                        sched->sums[5] * inv_n - my * my, static_cast<double>(n), mean_range, min_bin);
 }
 
 __device__ __forceinline__ uint32_t schedule_bin(const Schedule& g, const Pose2& st) {
   // heading relative to the mean as u = 2 tan(dtheta / 2): monotone in dtheta, one division instead of an atan2
   const double cr = st.c * g.c0 + st.s * g.s0, sr = st.s * g.c0 - st.c * g.s0;
   const double u = cr > -0.4 ? 2.0 * sr / (1.0 + cr) : (sr >= 0.0 ? 1e6 : -1e6);
-  int bt, bx, by;
-  if (g.equal_mass != 0u) {
-    // CDF value of each coordinate (single precision: the bin only decides which thread handles the particle)
-    const float zt = static_cast<float>(u) * g.kt, zx = static_cast<float>(st.x - g.mx) * g.kx, zy = static_cast<float>(st.y - g.my) * g.ky;
-    const float ft = __fdividef(static_cast<float>(g.nt), 1.0f + __expf(-zt));  // exp overflow -> 0, underflow -> count: the edge bins
-    const float fx = __fdividef(static_cast<float>(g.nx), 1.0f + __expf(-zx));
-    const float fy = __fdividef(static_cast<float>(g.ny), 1.0f + __expf(-zy));
-    bt = min(max(__float2int_rz(ft), 0), static_cast<int>(g.nt) - 1);  // NaN converts to 0
-    bx = min(max(__float2int_rz(fx), 0), static_cast<int>(g.nx) - 1);
-    by = min(max(__float2int_rz(fy), 0), static_cast<int>(g.ny) - 1);
-  } else {
-    bt = min(max(static_cast<int>(fmin(fmax((u + g.half_u) * g.scale_t, 0.0), 1e6)), 0), static_cast<int>(g.nt) - 1);
-    bx = min(max(static_cast<int>(fmin(fmax((st.x - g.x0) * g.scale_x, 0.0), 1e6)), 0), static_cast<int>(g.nx) - 1);
-    by = min(max(static_cast<int>(fmin(fmax((st.y - g.y0) * g.scale_y, 0.0), 1e6)), 0), static_cast<int>(g.ny) - 1);
-  }
+  // CDF value of each coordinate (single precision: the bin only decides which thread handles the particle)
+  const float zt = static_cast<float>(u) * g.kt, zx = static_cast<float>(st.x - g.mx) * g.kx, zy = static_cast<float>(st.y - g.my) * g.ky;
+  const float ft = __fdividef(static_cast<float>(g.nt), 1.0f + __expf(-zt));  // exp overflow -> 0, underflow -> count: the edge bins
+  const float fx = __fdividef(static_cast<float>(g.nx), 1.0f + __expf(-zx));
+  const float fy = __fdividef(static_cast<float>(g.ny), 1.0f + __expf(-zy));
+  const int bt = min(max(__float2int_rz(ft), 0), static_cast<int>(g.nt) - 1);  // NaN converts to 0
+  int bx = min(max(__float2int_rz(fx), 0), static_cast<int>(g.nx) - 1);
+  int by = min(max(__float2int_rz(fy), 0), static_cast<int>(g.ny) - 1);
   // Boustrophedon order: every other row runs backwards in x and every other plane backwards in y, so that consecutive
   // bins are always neighbours (a warp crossing a row end would otherwise span the whole cloud).
   if (bt & 1) by = static_cast<int>(g.ny) - 1 - by;
@@ -419,15 +389,16 @@ __global__ void __launch_bounds__(256) schedule_scatter_kernel(const uint32_t* _
 
 // ---- reweight (likelihood field; a3 + a5) --------------------------------------------------------
 
-constexpr int kRwThreads = BB200_RW_THREADS;  // x kRwBlocksPerSm CTAs per SM
-constexpr int kRwBlocksPerSm = BB200_RW_BLOCKS;
-constexpr int kRwUnroll = BB200_RW_UNROLL;  // groups of four beams in flight per thread
+// (threads, CTAs per SM, unroll) = (256, 4, 2) were chosen by sweeps on a B200, not re-measured on the H100.
+constexpr int kRwThreads = 256;  // x kRwBlocksPerSm CTAs per SM
+constexpr int kRwBlocksPerSm = 4;
+constexpr int kRwUnroll = 2;  // groups of four beams in flight per thread
 constexpr uint32_t kChunkBeams = 2048; // beams staged per shared-memory chunk (32 KB), multiple of 4
 
 /// floor(g) as int32 for |g| < 2^31: one F2I.F64.FLOOR (saturating).
 __device__ __forceinline__ int floor_to_int_fast(double g) { return __double2int_rd(g); }
 
-template <bool kFast, bool kTiled>
+template <bool kFast>
 __device__ __forceinline__ double field_lookup(const FieldView& f, double px, double py, double c, double s, double tx, double ty) {
   // likelihood_field_model.hpp:82-83 -- two products, one difference/sum, one offset; each rounded.
   const double x = (px * c - py * s) + tx;
@@ -448,18 +419,13 @@ __device__ __forceinline__ double field_lookup(const FieldView& f, double px, do
   // dense_grid.hpp:92-96 contains().  Out-of-grid end points read the spare cell that holds
   // f(unknown_space_occupancy_prob), so the load is unconditional (no divergent branch).
   const bool inside = static_cast<unsigned>(xi) < static_cast<unsigned>(f.width) && static_cast<unsigned>(yi) < static_cast<unsigned>(f.height);
-  uint32_t idx;
-  if (kTiled) {
-    const uint32_t ux = static_cast<uint32_t>(xi), uy = static_cast<uint32_t>(yi);
-    idx = (((uy >> 2) * static_cast<uint32_t>(f.tiles_x) + (ux >> 2)) << 4) | ((uy & 3u) << 2) | (ux & 3u);
-  } else {
-    idx = static_cast<uint32_t>(yi) * static_cast<uint32_t>(f.width) + static_cast<uint32_t>(xi);  // linear_grid.hpp:73-75
-  }
+  const uint32_t ux = static_cast<uint32_t>(xi), uy = static_cast<uint32_t>(yi);
+  uint32_t idx = (((uy >> 2) * static_cast<uint32_t>(f.tiles_x) + (ux >> 2)) << 4) | ((uy & 3u) << 2) | (ux & 3u);
   idx = inside ? idx : f.spare_index;
-  return __ldg((kTiled ? f.tiled : f.table) + idx);
+  return __ldg(f.tiled + idx);
 }
 
-template <bool kFast, bool kTiled>
+template <bool kFast>
 __device__ __forceinline__ double accumulate_chunk(const FieldView& f, const double2* pts, uint32_t count, double acc, double c, double s,
                                                    double tx, double ty) {
   // libstdc++ std::transform_reduce (numeric:439-462): groups of four, init += ((f0+f1)+(f2+f3)).
@@ -467,13 +433,13 @@ __device__ __forceinline__ double accumulate_chunk(const FieldView& f, const dou
 #pragma unroll kRwUnroll
   for (; b + 4 <= count; b += 4) {
     const double2 p0 = pts[b], p1 = pts[b + 1], p2 = pts[b + 2], p3 = pts[b + 3];
-    const double f0 = field_lookup<kFast, kTiled>(f, p0.x, p0.y, c, s, tx, ty);
-    const double f1 = field_lookup<kFast, kTiled>(f, p1.x, p1.y, c, s, tx, ty);
-    const double f2 = field_lookup<kFast, kTiled>(f, p2.x, p2.y, c, s, tx, ty);
-    const double f3 = field_lookup<kFast, kTiled>(f, p3.x, p3.y, c, s, tx, ty);
+    const double f0 = field_lookup<kFast>(f, p0.x, p0.y, c, s, tx, ty);
+    const double f1 = field_lookup<kFast>(f, p1.x, p1.y, c, s, tx, ty);
+    const double f2 = field_lookup<kFast>(f, p2.x, p2.y, c, s, tx, ty);
+    const double f3 = field_lookup<kFast>(f, p3.x, p3.y, c, s, tx, ty);
     acc = acc + ((f0 + f1) + (f2 + f3));
   }
-  for (; b < count; ++b) acc = acc + field_lookup<kFast, kTiled>(f, pts[b].x, pts[b].y, c, s, tx, ty);
+  for (; b < count; ++b) acc = acc + field_lookup<kFast>(f, pts[b].x, pts[b].y, c, s, tx, ty);
   return acc;
 }
 
@@ -497,7 +463,6 @@ __device__ __forceinline__ void publish_weight_max(unsigned long long bits, unsi
   }
 }
 
-template <bool kTiled>
 __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
     reweight_lfm_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, const uint32_t* __restrict__ perm,
                         FieldView field, const double2* __restrict__ points, uint32_t n_points, double points_radius,
@@ -543,8 +508,8 @@ __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
     mbarrier_wait(&s_bar, phase);
     phase ^= 1u;
     if (active) {
-      acc = fast ? accumulate_chunk<true, kTiled>(field, s_pts, count, acc, t.c, t.s, t.x, t.y)
-                 : accumulate_chunk<false, kTiled>(field, s_pts, count, acc, t.c, t.s, t.x, t.y);
+      acc = fast ? accumulate_chunk<true>(field, s_pts, count, acc, t.c, t.s, t.x, t.y)
+                 : accumulate_chunk<false>(field, s_pts, count, acc, t.c, t.s, t.x, t.y);
     }
     if (base + kChunkBeams < n_points) __syncthreads();  // s_pts is about to be overwritten by the next chunk
   }
@@ -635,8 +600,6 @@ struct ScanParam {
   double2 p[kParamBeams];
 };
 
-#define BB200_PRAGMA_STR(x) _Pragma(#x)
-#define BB200_PRAGMA_UNROLL(n) BB200_PRAGMA_STR(unroll n)
 // libstdc++ transform_reduce (numeric:439-462): groups of four, init += ((f0+f1)+(f2+f3)), then one by one.
 #define BB200_FIXED_SUM(POINT, COUNT, LOOKUP, TABLE)                                                                       \
   do {                                                                                                        \
@@ -655,7 +618,7 @@ struct ScanParam {
         f3 = LOOKUP(TABLE, q, p3.x, p3.y, margin);                                                            \
       }                                                                                                       \
       b = 4;                                                                                                  \
-      BB200_PRAGMA_UNROLL(BB200_RW_UNROLL) for (; b + 4 <= (COUNT); b += 4) {                                 \
+      _Pragma("unroll kRwUnroll") for (; b + 4 <= (COUNT); b += 4) {                                          \
         const double2 p0 = POINT(b), p1 = POINT(b + 1), p2 = POINT(b + 2), p3 = POINT(b + 3);                 \
         const double g0 = LOOKUP(TABLE, q, p0.x, p0.y, margin);                                               \
         const double g1 = LOOKUP(TABLE, q, p1.x, p1.y, margin);                                               \
@@ -705,35 +668,6 @@ __device__ __forceinline__ void fixed_particle_setup(const FieldView& field, con
   q.row_pitch = 4u * field.border_pitch;
 }
 
-#if BB200_RW_CHUNK > 0
-/// Next task of the CTA's current chunk (see the experiment note in reweight_lfm_fixed_param_kernel).  Every branch is on a
-/// value broadcast from lane 0, so that the warp provably stays converged: a spin loop inside `if (lane == 0)` makes ptxas
-/// give up the uniform datapath (LDCU) for the scan points in the beam loop that follows (LDC through the ADU pipe instead,
-/// which alone cost more than the chunks saved on a B200).
-__device__ __forceinline__ unsigned long long take_chunk_ticket(unsigned long long* s_chunk, unsigned long long* ticket_counter, int lane) {
-  for (;;) {
-    unsigned long long old = 0;
-    if (lane == 0) old = atomicAdd(s_chunk, 1ull);
-    old = __shfl_sync(0xffffffffu, old, 0);
-    const unsigned long long idx = old & 0xFFull, chunk = old >> 8;
-    if (idx < BB200_RW_CHUNK) return chunk * BB200_RW_CHUNK + idx;
-    if (idx == BB200_RW_CHUNK) {  // this warp refills: the new chunk's task 0 is its own
-      unsigned long long fresh = 0;
-      if (lane == 0) fresh = atomicAdd(ticket_counter, 1ull);
-      fresh = __shfl_sync(0xffffffffu, fresh, 0);
-      if (lane == 0) atomicExch(s_chunk, (fresh << 8) | 1ull);
-      return fresh * BB200_RW_CHUNK;
-    }
-    for (;;) {  // another warp is fetching the next chunk
-      unsigned long long cur = 0;
-      if (lane == 0) cur = *reinterpret_cast<volatile unsigned long long*>(s_chunk);
-      cur = __shfl_sync(0xffffffffu, cur, 0);
-      if ((cur >> 8) != chunk) break;
-    }
-  }
-}
-#endif
-
 /// Scan in the constant bank: nothing is shared between the warps of a CTA, so the grid is persistent
 /// (CTAs/SM x SM count) and every WARP draws the next 32 particles of the schedule from a global
 /// ticket counter.  A CTA-per-256-particles grid loses time to its slowest warp (each CTA holds its
@@ -745,24 +679,11 @@ __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
   const int lane = threadIdx.x % kWarp;
   const unsigned long long n_tasks = (n + kWarp - 1) / kWarp;  // a task = the next 32 particles of the schedule
   unsigned long long* ticket_counter = &scalars->work_ticket;
-#if BB200_RW_CHUNK > 0
-  // Experiment (rejected, DESIGN.md §4): the CTA draws CHUNKS of BB200_RW_CHUNK adjacent tasks from the global
-  // counter and its warps take tasks from the current chunk through a shared-memory word (chunk id << 8 | next index), so that
-  // the warps of a CTA work on neighbouring particles without waiting for each other; the warp that finds the chunk
-  // exhausted fetches the next one, the others spin on the word for that round trip.
-  __shared__ unsigned long long s_chunk;
-  if (threadIdx.x == 0) s_chunk = atomicAdd(ticket_counter, 1ull) << 8;
-  __syncthreads();
-  unsigned long long ticket = take_chunk_ticket(&s_chunk, ticket_counter, lane);
-#else
   unsigned long long ticket = __shfl_sync(0xffffffffu, lane == 0 ? atomicAdd(ticket_counter, 1ull) : 0ull, 0);
-#endif
   unsigned long long best = 0ull;
   while (ticket < n_tasks) {
-#if BB200_RW_CHUNK == 0
     // Draw the next ticket now; its round trip to L2 hides behind this task's beams.
     const unsigned long long next = lane == 0 ? atomicAdd(ticket_counter, 1ull) : 0ull;
-#endif
     const uint64_t slot = ticket * kWarp + lane;
     const bool active = slot < n;  // idle lanes of the last task walk the beams with a dummy pose
     const uint64_t i = active ? (perm != nullptr ? perm[slot] : slot) : 0;
@@ -780,11 +701,7 @@ __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
       const unsigned long long bits = weight_order_bits(w);
       best = bits > best ? bits : best;
     }
-#if BB200_RW_CHUNK > 0
-    ticket = take_chunk_ticket(&s_chunk, ticket_counter, lane);
-#else
     ticket = __shfl_sync(0xffffffffu, next, 0);
-#endif
   }
 #pragma unroll
   for (int off = kWarp / 2; off > 0; off >>= 1) {
@@ -872,8 +789,8 @@ __device__ __forceinline__ int cell_near(double p, double inv_resolution) {
 }
 
 /// One ray of Ray2d::cast (raycasting.hpp:79-107) over the standard Bresenham2i iterator (bresenham.hpp:84-160) as a
-/// state machine, so that a thread can keep several rays in flight (ray_step is one dependent load of the
-/// free-distance map plus a closed-form advance of the iterator; the walk is bound by that load's latency).
+/// state machine (ray_step is one dependent load of the free-distance map plus a closed-form advance of the
+/// iterator; the walk is bound by that load's latency).
 struct RayWalk {
   int x, y;            // iterator position: x along the longer axis (swapped when `reversed`)
   int xstep, ystep;
@@ -1000,15 +917,8 @@ __global__ void __launch_bounds__(256) beam_eta_table_kernel(BeamParams p, doubl
   table[k] = beam_normalisers(p, z_mean);
 }
 
-#ifndef BB200_BEAM_BLOCKS
-#define BB200_BEAM_BLOCKS 3
-#endif
-#ifndef BB200_BEAM_RAYS
-#define BB200_BEAM_RAYS 1  // rays a thread walks together (1, 2 or 4); 1 chosen by a sweep at C3 on a B200, not re-measured on the H100
-#endif
-constexpr int kBeamRays = BB200_BEAM_RAYS;
 constexpr int kBeamThreads = 256;
-constexpr int kBeamBlocksPerSm = BB200_BEAM_BLOCKS;
+constexpr int kBeamBlocksPerSm = 3;  // chosen on a B200, not re-measured on the H100
 constexpr uint32_t kBeamChunk = 1024;  // rays staged per shared-memory chunk (32 KB), multiple of 4
 
 __global__ void __launch_bounds__(kBeamThreads, kBeamBlocksPerSm)
@@ -1053,6 +963,12 @@ __global__ void __launch_bounds__(kBeamThreads, kBeamBlocksPerSm)
     const double ey = (src.s * ray.far_x + src.c * ray.far_y) + src.y;
     ray_begin(walk, sx, sy, cell_near(ex, grid.inv_resolution), cell_near(ey, grid.inv_resolution));
   };
+  auto walk_ray = [&](const BeamRay& ray) {
+    RayWalk walk;
+    begin_walk(walk, ray);
+    while (walk.active) ray_step(walk, grid);
+    return beam_value(ray, walk);
+  };
 
   double acc = 0.0;
   for (uint32_t base = 0; base < n_points; base += kBeamChunk) {
@@ -1068,34 +984,10 @@ __global__ void __launch_bounds__(kBeamThreads, kBeamBlocksPerSm)
     if (active) {
       uint32_t b = 0;
       for (; b + 4 <= count; b += 4) {  // transform_reduce grouping (numeric:439-462)
-        // The four rays of a group are walked together: their free-distance loads are independent, so the thread
-        // keeps kBeamRays of them in flight instead of waiting out one dependent chain after the other.
-        double f[4];
-#pragma unroll
-        for (int g0 = 0; g0 < 4; g0 += kBeamRays) {
-          RayWalk walk[kBeamRays];
-#pragma unroll
-          for (int r = 0; r < kBeamRays; ++r) begin_walk(walk[r], s_rays[b + g0 + r]);
-          bool any = true;
-          while (any) {
-            any = false;
-#pragma unroll
-            for (int r = 0; r < kBeamRays; ++r) {
-              if (walk[r].active) ray_step(walk[r], grid);
-              any |= walk[r].active;
-            }
-          }
-#pragma unroll
-          for (int r = 0; r < kBeamRays; ++r) f[g0 + r] = beam_value(s_rays[b + g0 + r], walk[r]);
-        }
-        acc = acc + ((f[0] + f[1]) + (f[2] + f[3]));
+        const double f0 = walk_ray(s_rays[b]), f1 = walk_ray(s_rays[b + 1]), f2 = walk_ray(s_rays[b + 2]), f3 = walk_ray(s_rays[b + 3]);
+        acc = acc + ((f0 + f1) + (f2 + f3));
       }
-      for (; b < count; ++b) {
-        RayWalk walk;
-        begin_walk(walk, s_rays[b]);
-        while (walk.active) ray_step(walk, grid);
-        acc = acc + beam_value(s_rays[b], walk);
-      }
+      for (; b < count; ++b) acc = acc + walk_ray(s_rays[b]);
     }
   }
   if (active) {
@@ -1115,10 +1007,9 @@ __global__ void __launch_bounds__(kBeamThreads, kBeamBlocksPerSm)
 // and a branch-free mixture loop.  Hit words: 0xFFFFFFFF = miss, else cy << 16 | cx (grids up to 65535 cells a side).
 
 constexpr uint32_t kHitMiss = 0xFFFFFFFFu;
-#ifndef BB200_WALK_BLOCKS
-#define BB200_WALK_BLOCKS 8  // resident CTAs per SM the walk is compiled for (register cap; the loop is latency-bound, so warps beat
-                            // registers even with a few spills); 8 chosen by a sweep at C3 on a B200, not re-measured on the H100
-#endif
+constexpr int kWalkBlocksPerSm = 8;  // resident CTAs per SM the walk is compiled for (register cap; the loop is latency-bound, so
+                                     // warps beat registers even with a few spills); chosen by a sweep at C3 on a B200, not
+                                     // re-measured on the H100
 constexpr int kWalkThreads = 256;
 constexpr uint32_t kWalkChunk = 1024;  // far ends staged per shared-memory chunk (16 KB)
 
@@ -1130,7 +1021,7 @@ constexpr uint32_t kWalkChunk = 1024;  // far ends staged per shared-memory chun
 /// the 32-bit reciprocal quotient of ray_step is the only path.  16 instructions per iteration instead of 45.
 /// (Walking 2 or 4 rays per thread together was slower at C3 on a B200, not re-measured on the H100 --
 /// the per-ray state machine and its activity flags cost more than the second load chain hides.)
-__global__ void __launch_bounds__(kWalkThreads, BB200_WALK_BLOCKS)
+__global__ void __launch_bounds__(kWalkThreads, kWalkBlocksPerSm)
     beam_walk_kernel(const Pose2* __restrict__ states, uint64_t n, uint64_t slot_base, uint64_t slot_count, const uint32_t* __restrict__ perm,
                      OccupancyView grid, double beam_max_range, const double2* __restrict__ points, uint32_t n_points,
                      uint32_t* __restrict__ hits, uint64_t hit_stride) {
@@ -1323,8 +1214,8 @@ __global__ void prepare_cdf_kernel(Scalars* s, double host_wmax, int ceil_log2_c
 
 /// Inclusive scan of per-thread totals across the block (warp shuffles + one smem hop).
 template <int kThreads>
-__device__ __forceinline__ unsigned long long block_inclusive_scan_u64_n(unsigned long long v, unsigned long long* warp_sums,
-                                                                          unsigned long long& block_total) {
+__device__ __forceinline__ unsigned long long block_inclusive_scan_u64(unsigned long long v, unsigned long long* warp_sums,
+                                                                        unsigned long long& block_total) {
   const int lane = threadIdx.x % kWarp, warp = threadIdx.x / kWarp;
 #pragma unroll
   for (int off = 1; off < kWarp; off <<= 1) {
@@ -1344,30 +1235,6 @@ __device__ __forceinline__ unsigned long long block_inclusive_scan_u64_n(unsigne
   }
   __syncthreads();
   block_total = warp_sums[kThreads / kWarp - 1];
-  return v + (warp > 0 ? warp_sums[warp - 1] : 0ull);
-}
-
-__device__ __forceinline__ unsigned long long block_inclusive_scan_u64(unsigned long long v, unsigned long long* warp_sums,
-                                                                        unsigned long long& block_total) {
-  const int lane = threadIdx.x % kWarp, warp = threadIdx.x / kWarp;
-#pragma unroll
-  for (int off = 1; off < kWarp; off <<= 1) {
-    const unsigned long long o = __shfl_up_sync(0xffffffffu, v, off);
-    if (lane >= off) v += o;
-  }
-  if (lane == kWarp - 1) warp_sums[warp] = v;
-  __syncthreads();
-  if (warp == 0) {
-    unsigned long long ws = lane < kScanThreads / kWarp ? warp_sums[lane] : 0ull;
-#pragma unroll
-    for (int off = 1; off < kWarp; off <<= 1) {
-      const unsigned long long o = __shfl_up_sync(0xffffffffu, ws, off);
-      if (lane >= off) ws += o;
-    }
-    if (lane < kScanThreads / kWarp) warp_sums[lane] = ws;
-  }
-  __syncthreads();
-  block_total = warp_sums[kScanThreads / kWarp - 1];
   return v + (warp > 0 ? warp_sums[warp - 1] : 0ull);
 }
 
@@ -1411,12 +1278,8 @@ __device__ __forceinline__ unsigned long long lookback_exclusive_prefix(unsigned
 // 16-byte accesses).  The quantisation is a multiplication by 2^e (exact, like scalbn, wherever the result is >= 1),
 // split into two power-of-two factors so that each stays a normal double for any exponent.
 constexpr int kQsThreads = 256;
-constexpr int kQsItemsSmall = 8;   // up to a few million weights: more tiles than SM slots, shortest chain
-#ifndef BB200_QS_LARGE_ITEMS
-#define BB200_QS_LARGE_ITEMS 8  // 16 halves the tiles per byte but was slower at 12.5M on a B200 (not re-measured on the H100)
-#endif
-constexpr int kQsItemsLarge = BB200_QS_LARGE_ITEMS;
-constexpr uint32_t kQsTile = kQsThreads * kQsItemsSmall;  // the smaller tile sizes the look-back state
+constexpr int kQsItems = 8;  // 16 halves the tiles per byte but was slower at 12.5M on a B200 (not re-measured on the H100)
+constexpr uint32_t kQsTile = kQsThreads * kQsItems;
 
 __device__ __forceinline__ double pow2_double(int e) {  // |e| <= 1000
   return __longlong_as_double(static_cast<long long>(e + 1023) << 52);
@@ -1428,7 +1291,6 @@ __device__ __forceinline__ unsigned long long quantize_mul(double w, double f1, 
 
 /// derive_exponent: the fused step -- the exponent comes from scalars->wmax_bits here (no prepare_cdf launch; the
 /// tile holding element 0 publishes exponent / valid for the host); otherwise scalars->exponent / valid are given.
-template <int kQsItems>
 __global__ void __launch_bounds__(kQsThreads) quantize_scan_kernel(const double* __restrict__ weights, uint64_t n,
                                                                    unsigned long long* __restrict__ cdf, Scalars* scalars,
                                                                    unsigned long long* tile_state, int derive_exponent, int ceil_log2_count) {
@@ -1479,7 +1341,7 @@ __global__ void __launch_bounds__(kQsThreads) quantize_scan_kernel(const double*
     }
   }
   unsigned long long tile_total;
-  const unsigned long long inclusive = block_inclusive_scan_u64_n<kQsThreads>(local, s_warp, tile_total);
+  const unsigned long long inclusive = block_inclusive_scan_u64<kQsThreads>(local, s_warp, tile_total);
   const unsigned long long prefix = lookback_exclusive_prefix(tile_state, tile, tile_total, &s_prefix);
   unsigned long long running = prefix + inclusive - local;
   if (base + kQsItems <= n) {
@@ -1521,7 +1383,7 @@ __global__ void __launch_bounds__(kScanThreads) scan_u32_kernel(const uint32_t* 
     local += q[k];
   }
   unsigned long long tile_total;
-  const unsigned long long inclusive = block_inclusive_scan_u64(local, s_warp, tile_total);
+  const unsigned long long inclusive = block_inclusive_scan_u64<kScanThreads>(local, s_warp, tile_total);
   const unsigned long long prefix = lookback_exclusive_prefix(tile_state, tile, tile_total, &s_prefix);
   unsigned long long running = prefix + inclusive - local;
 #pragma unroll
@@ -1826,16 +1688,15 @@ __global__ void __launch_bounds__(kRsThreads) resample_kernel(ResampleArgs a, Sc
 // (the parity tests compare them with the oracle's lower_bound search); the raw moments are summed per
 // particle (count * term) instead of per slot, which moves the estimate at rounding level only.
 
-__device__ __forceinline__ uint64_t comb_slots_before(unsigned long long position, unsigned long long offset, unsigned long long stride,
-                                                     uint64_t total_slots) {
-  if (position <= offset) return 0;  // number of slots j with offset + j * stride < position
-  const unsigned long long j = (position - offset + stride - 1) / stride;
-  return j < total_slots ? j : total_slots;
-}
+// (CTAs per SM, particles per thread and round) = (3, 2) was chosen by a sweep at 1M on a B200, carried over to the H100
+// without re-measuring.
+constexpr int kRsBlocksPerSm = 3;  // resident CTAs per SM the kernel is compiled for (register cap)
+constexpr int kRsUnroll = 2;       // particles per thread and round
 
-/// The same with the division replaced by a multiplication with magic = floor((2^64 - 1) / stride): the high word of
-/// x * magic is the quotient or one below it (x < 2^64, so the error of the reciprocal costs less than 1); one
-/// remainder check makes it exact.  A 64-bit division is ~150 instructions; this is 8.
+/// Number of slots j with offset + j * stride < position, i.e. ceil((position - offset) / stride) capped at total_slots, with
+/// the division replaced by a multiplication with magic = floor((2^64 - 1) / stride): the high word of x * magic is the
+/// quotient or one below it (x < 2^64, so the error of the reciprocal costs less than 1); one remainder check makes it
+/// exact.  A 64-bit division is ~150 instructions; this is 8.
 __device__ __forceinline__ uint64_t comb_slots_before_magic(unsigned long long position, unsigned long long offset, unsigned long long stride,
                                                            unsigned long long magic, uint64_t total_slots) {
   if (position <= offset) return 0;
@@ -1845,7 +1706,7 @@ __device__ __forceinline__ uint64_t comb_slots_before_magic(unsigned long long p
   return j < total_slots ? j : total_slots;
 }
 
-__global__ void __launch_bounds__(kRsThreads, BB200_RS_BLOCKS) resample_scatter_kernel(ResampleArgs a, Scalars* __restrict__ scalars,
+__global__ void __launch_bounds__(kRsThreads, kRsBlocksPerSm) resample_scatter_kernel(ResampleArgs a, Scalars* __restrict__ scalars,
                                                                      double* __restrict__ moment_partials) {
   __shared__ double s_red[kMomentCount * kRsThreads / kWarp];
   __shared__ unsigned long long s_comb[3];
@@ -1889,7 +1750,6 @@ __global__ void __launch_bounds__(kRsThreads, BB200_RS_BLOCKS) resample_scatter_
   // kRsUnroll particles per thread and round: their CDF reads, divisions and state loads are independent, so one thread keeps
   // several 32-byte gathers in flight (the kernel is bound by the latency of cdf -> state -> store, not by bandwidth).
   // Every thread runs the same number of rounds: whole warps stay together for the cooperative stores.
-  constexpr int kRsUnroll = BB200_RS_UNROLL;
   constexpr uint64_t kOwnCopies = 4;  // up to this many copies a thread stores itself
   const uint64_t per_round = static_cast<uint64_t>(gridDim.x) * kRsThreads * kRsUnroll;
   const uint64_t rounds = (a.n_in + per_round - 1) / per_round;
@@ -2144,13 +2004,12 @@ uint32_t schedule_max_bins() { return kMaxBins; }
 uint32_t schedule_tile_count() { return (kMaxBins + kScanTile - 1) / kScanTile; }
 
 void launch_build_schedule(const Pose2* states, uint64_t n, Schedule* sched, uint32_t* bins, uint32_t* counters, uint32_t* perm,
-                           unsigned long long* tile_state, double mean_range, double min_bin, double per_bin, double x_split, bool equal_mass,
-                           cudaStream_t stream) {
+                           unsigned long long* tile_state, double mean_range, double min_bin, cudaStream_t stream) {
   if (n == 0) return;
   const unsigned blocks = static_cast<unsigned>((n + 255) / 256);
   cudaMemsetAsync(counters, 0, kMaxBins * sizeof(uint32_t), stream);
   cudaMemsetAsync(tile_state, 0, schedule_tile_count() * sizeof(unsigned long long), stream);
-  schedule_params_kernel<<<1, 1, 0, stream>>>(sched, n, mean_range, min_bin, per_bin, x_split, equal_mass);
+  schedule_params_kernel<<<1, 1, 0, stream>>>(sched, n, mean_range, min_bin);
   schedule_histogram_kernel<<<blocks, 256, 0, stream>>>(states, n, sched, bins, counters);
   scan_u32_kernel<<<schedule_tile_count(), kScanThreads, 0, stream>>>(counters, counters, kMaxBins, &sched->tile_ticket, tile_state, nullptr);
   schedule_scatter_kernel<<<blocks, 256, 0, stream>>>(bins, n, counters, perm);
@@ -2165,14 +2024,6 @@ void launch_finish_schedule(const uint2* bin_rank, uint64_t n, uint32_t n_bins, 
   const uint32_t tiles = (n_bins + kScanTile - 1) / kScanTile;
   scan_u32_kernel<<<tiles, kScanThreads, 0, stream>>>(counters, counters, n_bins, &sched->tile_ticket, tile_state, nullptr);
   schedule_place_kernel<<<blocks, 256, 0, stream>>>(bin_rank, n, counters, perm);
-}
-
-bool scatter_resample_enabled() {
-  static const bool enabled = [] {
-    const char* v = std::getenv("BB200_SCATTER_RESAMPLE");  // development knob
-    return v == nullptr || std::atoi(v) != 0;
-  }();
-  return enabled;
 }
 
 int sm_count() {
@@ -2203,10 +2054,8 @@ void launch_reweight_lfm(const Pose2* states, double* weights, uint64_t n, const
     } else {
       reweight_lfm_fixed_kernel<<<blocks, kRwThreads, smem, stream>>>(states, weights, n, perm, field, points, n_points, points_radius, scalars);
     }
-  } else if (field.use_tiled) {
-    reweight_lfm_kernel<true><<<blocks, kRwThreads, smem, stream>>>(states, weights, n, perm, field, points, n_points, points_radius, scalars);
   } else {
-    reweight_lfm_kernel<false><<<blocks, kRwThreads, smem, stream>>>(states, weights, n, perm, field, points, n_points, points_radius, scalars);
+    reweight_lfm_kernel<<<blocks, kRwThreads, smem, stream>>>(states, weights, n, perm, field, points, n_points, points_radius, scalars);
   }
 }
 
@@ -2254,7 +2103,7 @@ void launch_max_weight(const double* weights, uint64_t n, Scalars* scalars, cuda
   max_weight_kernel<<<blocks, 512, 0, stream>>>(weights, n, scalars);
 }
 
-uint32_t scan_tile_count(uint64_t n) { return static_cast<uint32_t>((n + kQsTile - 1) / kQsTile); }  // the smaller of the two tile sizes
+uint32_t scan_tile_count(uint64_t n) { return static_cast<uint32_t>((n + kQsTile - 1) / kQsTile); }
 
 void launch_prepare_cdf(Scalars* scalars, double host_wmax, uint64_t global_count, unsigned long long* tile_state, uint32_t n_tiles,
                         cudaStream_t stream) {
@@ -2265,14 +2114,8 @@ void launch_prepare_cdf(Scalars* scalars, double host_wmax, uint64_t global_coun
 void launch_quantize_scan(const double* weights, uint64_t n, unsigned long long* cdf, Scalars* scalars, unsigned long long* tile_state,
                           cudaStream_t stream, bool derive_exponent, uint64_t global_count) {
   if (n == 0) return;
-  if (n > (4u << 20)) {
-    constexpr uint32_t tile = kQsThreads * kQsItemsLarge;
-    quantize_scan_kernel<kQsItemsLarge><<<static_cast<unsigned>((n + tile - 1) / tile), kQsThreads, 0, stream>>>(
-        weights, n, cdf, scalars, tile_state, derive_exponent ? 1 : 0, ceil_log2_u64(global_count));
-  } else {
-    quantize_scan_kernel<kQsItemsSmall><<<static_cast<unsigned>((n + kQsTile - 1) / kQsTile), kQsThreads, 0, stream>>>(
-        weights, n, cdf, scalars, tile_state, derive_exponent ? 1 : 0, ceil_log2_u64(global_count));
-  }
+  quantize_scan_kernel<<<scan_tile_count(n), kQsThreads, 0, stream>>>(weights, n, cdf, scalars, tile_state, derive_exponent ? 1 : 0,
+                                                                     ceil_log2_u64(global_count));
 }
 
 void launch_normalize(double* weights, uint64_t n, const Scalars* scalars, unsigned long long global_total, double* partials,
@@ -2318,13 +2161,12 @@ uint32_t launch_resample(const ResampleArgs& args, Scalars* scalars, double* mom
   // (Sharded with peer memory and device-side totals: the same, every copy stored into its owner's buffer.)
   const bool plain = args.scheme == 1 && args.random_state_probability <= 0.0 && args.hashes == nullptr && args.span_filter == 0 &&
                      args.peer_hash_count == 0 && args.window_begin == 0 &&
-                     args.global_total == 0 && args.cdf_offset == 0 && args.slot_first == 0 && scatter_resample_enabled();
+                     args.global_total == 0 && args.cdf_offset == 0 && args.slot_first == 0;
   const bool scatter = plain && ((args.peer_count == 0 && args.rank_totals == nullptr && args.slot_count == args.total_slots) ||
                                  (args.peer_count > 0 && args.rank_totals != nullptr));
   if (scatter) {
     // one pass over the input particles; a few particles per thread amortise the block reduction of the moments
-    const uint32_t per_sm = BB200_RS_BLOCKS;  // resident CTAs at the kernel's register count
-    const uint32_t blocks = static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>((args.n_in + kRsThreads - 1) / kRsThreads, kSmCount * per_sm)));
+    const uint32_t blocks = static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>((args.n_in + kRsThreads - 1) / kRsThreads, kSmCount * kRsBlocksPerSm)));
     resample_scatter_kernel<<<blocks, kRsThreads, 0, stream>>>(args, scalars, moment_partials);
     return blocks;
   }

@@ -10,22 +10,10 @@
 namespace bb200 {
 
 /// Device view of the likelihood-field lookup table (LFM / LFM-prob).
+/// The fixed-point kernels' members come first.  With the general kernel's members in front, ptxas arranged the set-up of
+/// reweight_lfm_fixed_param_kernel differently (same beam loop) and the kernel took 1.48 instead of 1.19 ms at 1M x 1080
+/// beams on an H100 80GB HBM3 (SXM, 400 W power limit).
 struct FieldView {
-  // f(pz) per cell (f = pz^3 or log pz), row-major, followed by one spare cell holding
-  // unknown_value (index width*height) that out-of-grid end points read.
-  const double* table;
-  // The same values in 4x4-cell tiles (one 128-byte line per tile, row-major inside), padded to whole
-  // tiles with unknown_value, plus the spare cell at tiles_x*tiles_y*16.  Index: tiled_index().
-  const double* tiled;
-  int tiles_x;
-  int use_tiled;          // which of the two layouts the kernel gathers from
-  uint32_t spare_index;   // index of the spare cell in the selected layout
-  int width, height;
-  double inv_resolution;  // 1. / resolution  (regular_grid.hpp:76)
-  double unknown_value;   // f(float(1/max_laser_distance)) for out-of-grid end points
-  double init;            // transform_reduce init: 1.0 (LFM) or 0.0 (prob)
-  int exp_epilogue;       // prob model: weight = exp(sum)
-  Pose2 world_to_field;   // grid.origin().inverse()
   // Bordered 4x4-tile layout for the fixed-point lookup kernel (reweight_lfm_fixed_kernel): the grid
   // with a one-cell border of unknown_value, cell (xi, yi) stored at padded coordinates
   // (px, py) = (xi + 1, yi + 1), index bordered_index(px, py, border_kx); 2^border_kx tiles per row.
@@ -35,6 +23,18 @@ struct FieldView {
   uint32_t border_x_max;  // 4 (width + 1) + 3: largest 4 * padded x with its two fraction bits
   uint32_t border_y_max;  // height + 1: largest padded y
   int use_fixed;          // launch the fixed-point kernel (map small enough for 16.16 cell coordinates)
+  int width, height;
+  double inv_resolution;  // 1. / resolution  (regular_grid.hpp:76)
+  double unknown_value;   // f(float(1/max_laser_distance)) for out-of-grid end points
+  double init;            // transform_reduce init: 1.0 (LFM) or 0.0 (prob)
+  int exp_epilogue;       // prob model: weight = exp(sum)
+  Pose2 world_to_field;   // grid.origin().inverse()
+  // f(pz) per cell (f = pz^3 or log pz) in 4x4-cell tiles (one 128-byte line per tile, row-major inside), padded to
+  // whole tiles with unknown_value, plus one spare cell holding unknown_value at tiles_x*tiles_y*16 that out-of-grid
+  // end points read.  Index: tiled_index().  Uploaded only for maps the fixed-point kernel does not take (use_fixed = 0).
+  const double* tiled;
+  int tiles_x;
+  uint32_t spare_index;   // index of the spare cell
 };
 
 /// Offset of padded cell (px, py) in the bordered tile layout.
@@ -166,29 +166,28 @@ struct Schedule {
   double sums[6];  // sum cos, sin, x, y, x^2, y^2 of the propagated cloud (device-built schedules only)
   unsigned long long tile_ticket;
   double c0, s0;            // mean heading (unit complex)
-  double x0, y0, half_u;    // lower corner of the box; half extent of the heading coordinate u = 2 tan(dtheta / 2)
-  double scale_t, scale_x, scale_y;
-  double mx, my;            // cloud mean (equal-mass bins)
-  float kt, kx, ky;         // equal-mass bins: 1.702 / sigma of u, x, y (logistic stand-in for the normal CDF)
-  uint32_t equal_mass;      // bins of equal expected particle count instead of equal size
+  double half_u;            // half extent of the heading coordinate u = 2 tan(dtheta / 2)
+  double mx, my;            // cloud mean
+  float kt, kx, ky;         // 1.702 / sigma of u, x, y (logistic stand-in for the normal CDF)
   uint32_t nt, nx, ny;
   uint32_t n_bins;
 };
 constexpr uint32_t kScheduleMaxBins = 1u << 19;  // 4 particles per bin up to 2M particles per shard, coarser bins beyond
+constexpr double kSchedulePerBin = 4.0;          // particles per pose bin (expected)
+constexpr double kScheduleXSplit = 8.0;          // bins per warp along x
 
 /// The pose-bin grid for a cloud with mean resultant (cbar, sbar), mean position (mx, my) and position variances
-/// (vx, vy), about `per_bin` particles per bin.  Runs on the device (moments of the propagated cloud) or on the host
+/// (vx, vy), about kSchedulePerBin particles per bin.  Runs on the device (moments of the propagated cloud) or on the host
 /// (moments predicted from the last estimate and the motion means).  The schedule only decides WHICH THREAD handles a
 /// particle, never a result.
 ///
-/// equal_mass = false: bins of equal physical edge in (range * heading, x, y) covering +-3 sigma.
-/// equal_mass = true:  every coordinate goes through a sigmoid CDF (logistic with the normal's spread) first, so that bins
-///   hold the same EXPECTED number of particles: small where the cloud is dense, large in the tails.  A uniform grid over
-///   a normal cloud puts most particles into bins 13x over-full, and 32 schedule neighbours then span a whole bin.
-/// x_split: bins are x_split times thinner in x than in the other two coordinates; x is the fastest index of the bin
-///   order, so a warp (32 neighbours of the schedule) covers x_split bins of a row: a cube, whatever the bin boundaries.
+/// Every coordinate goes through a sigmoid CDF (logistic with the normal's spread) first, so that bins hold the same
+/// EXPECTED number of particles: small where the cloud is dense, large in the tails.  A uniform grid over a normal cloud
+/// puts most particles into bins 13x over-full, and 32 schedule neighbours then span a whole bin.
+/// Bins are kScheduleXSplit times thinner in x than in the other two coordinates; x is the fastest index of the bin
+/// order, so a warp (32 neighbours of the schedule) covers kScheduleXSplit bins of a row: a cube, whatever the bin boundaries.
 BB_HD void schedule_from_moments(Schedule& g, double cbar, double sbar, double mx, double my, double vx, double vy, double n,
-                                 double mean_range, double min_bin, double per_bin, double x_split = 1.0, bool equal_mass = false) {
+                                 double mean_range, double min_bin) {
   const double r = sqrt(cbar * cbar + sbar * sbar);
   const double pi = 3.14159265358979323846;
   double c0 = 1.0, s0 = 0.0, sigma_theta = pi;
@@ -201,29 +200,24 @@ BB_HD void schedule_from_moments(Schedule& g, double cbar, double sbar, double m
   const double half_u = 2.0 * tan(0.5 * half_theta);
   const double half_x = fmax(3.0 * sqrt(fmax(vx, 0.0)), min_bin), half_y = fmax(3.0 * sqrt(fmax(vy, 0.0)), min_bin);
   const double lever = fmax(mean_range, 1.0);
-  x_split = fmin(fmax(x_split, 1.0), 32.0);
-  // Extents in physical units.  Equal-size bins tile the +-3 sigma box; equal-mass bins tile the unit cube of CDF values,
-  // where a bin at the centre of the cloud is sigma / (density of the sigmoid at 0 = 1.702 / 4) / count wide.
-  const double centre = equal_mass ? 1.0 / (3.0 * 0.4255) : 2.0;
+  // Extents in physical units: the bins tile the unit cube of CDF values, where a bin at the centre of the cloud is
+  // sigma / (density of the sigmoid at 0 = 1.702 / 4) / count wide.
+  const double centre = 1.0 / (3.0 * 0.4255);
   const double ext_t = centre * half_u * lever, ext_x = centre * half_x, ext_y = centre * half_y;
-  double q = cbrt(x_split * ext_t * ext_x * ext_y / fmax(n / per_bin, 1.0));  // edge of x_split bins side by side
+  double q = cbrt(kScheduleXSplit * ext_t * ext_x * ext_y / fmax(n / kSchedulePerBin, 1.0));  // edge of kScheduleXSplit bins side by side
   q = fmax(q, min_bin);
   uint32_t nt, nx, ny;
   for (;;) {
     nt = static_cast<uint32_t>(fmin(fmax(ceil(ext_t / q), 1.0), 65536.0));
-    nx = static_cast<uint32_t>(fmin(fmax(ceil(x_split * ext_x / q), 1.0), 65536.0));
+    nx = static_cast<uint32_t>(fmin(fmax(ceil(kScheduleXSplit * ext_x / q), 1.0), 65536.0));
     ny = static_cast<uint32_t>(fmin(fmax(ceil(ext_y / q), 1.0), 65536.0));
     if (static_cast<uint64_t>(nt) * nx * ny <= kScheduleMaxBins) break;
     q = q * 1.3;
   }
   g.c0 = c0, g.s0 = s0;
-  g.x0 = mx - half_x, g.y0 = my - half_y, g.half_u = half_u;
-  g.scale_t = static_cast<double>(nt) / (2.0 * half_u);
-  g.scale_x = static_cast<double>(nx) / (2.0 * half_x);
-  g.scale_y = static_cast<double>(ny) / (2.0 * half_y);
+  g.half_u = half_u;
   g.mx = mx, g.my = my;
   g.kt = static_cast<float>(1.702 * 3.0 / half_u), g.kx = static_cast<float>(1.702 * 3.0 / half_x), g.ky = static_cast<float>(1.702 * 3.0 / half_y);
-  g.equal_mass = equal_mass ? 1u : 0u;
   g.nt = nt, g.nx = nx, g.ny = ny;
   g.n_bins = nt * nx * ny;
 }
@@ -246,8 +240,7 @@ uint32_t schedule_max_bins();
 uint32_t schedule_tile_count();
 /// Counting sort of the particle indices over pose bins -> perm (needs launch_propagate's moments).
 void launch_build_schedule(const Pose2* states, uint64_t n, Schedule* sched, uint32_t* bins, uint32_t* counters, uint32_t* perm,
-                           unsigned long long* tile_state, double mean_range, double min_bin, double per_bin, double x_split, bool equal_mass,
-                           cudaStream_t stream);
+                           unsigned long long* tile_state, double mean_range, double min_bin, cudaStream_t stream);
 /// reweight with the likelihood-field table in schedule order (perm may be null) | block max.
 /// points_xy_host (optional): the same points in host memory; scans of up to 1920 points then travel as
 /// kernel parameters (constant bank) instead of being staged through shared memory.

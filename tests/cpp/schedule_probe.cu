@@ -8,23 +8,21 @@
 int main() {
   using namespace bb200;
   struct Case {
-    double cbar, sbar, mx, my, vx, vy, n, mean_range, min_bin, per_bin, x_split;
-    bool equal_mass;
+    double cbar, sbar, mx, my, vx, vy, n, mean_range, min_bin;
   };
   const Case cases[] = {
-      {0.45, 0.87, 30.0, 40.0, 0.25, 0.30, 1e6, 21.0, 0.025, 16.0, 1.0, false},
-      {0.45, 0.87, 30.0, 40.0, 0.25, 0.30, 1e6, 21.0, 0.025, 4.0, 8.0, true},
-      {0.45, 0.87, 30.0, 40.0, 0.25, 0.30, 1.25e7, 21.0, 0.025, 4.0, 8.0, true},
-      {1.0, 0.0, 3.0, 4.0, 0.0, 0.0, 1e4, 10.0, 0.025, 4.0, 8.0, true},
-      {0.0, 0.0, 0.0, 0.0, 1.0, 1.0, 1e4, 10.0, 0.025, 4.0, 8.0, true},
-      {-0.2, 0.1, -5.0, 7.5, 4.0, 0.01, 125000.0, 3.0, 0.05, 8.0, 4.0, false},
+      {0.45, 0.87, 30.0, 40.0, 0.25, 0.30, 1e6, 21.0, 0.025},
+      {0.45, 0.87, 30.0, 40.0, 0.25, 0.30, 1.25e7, 21.0, 0.025},
+      {1.0, 0.0, 3.0, 4.0, 0.0, 0.0, 1e4, 10.0, 0.025},
+      {0.0, 0.0, 0.0, 0.0, 1.0, 1.0, 1e4, 10.0, 0.025},
+      {-0.2, 0.1, -5.0, 7.5, 4.0, 0.01, 32769.0, 3.0, 0.05},      // just above the scheduling threshold; heading spread clamped
+      {0.486, -0.648, 12.5, -3.0, 0.04, 2.25, 2.5e5, 8.0, 0.05},  // 3 sigma of the heading just inside the +-2 rad clamp
   };
   for (const Case& c : cases) {
     Schedule g{};
-    schedule_from_moments(g, c.cbar, c.sbar, c.mx, c.my, c.vx, c.vy, c.n, c.mean_range, c.min_bin, c.per_bin, c.x_split, c.equal_mass);
-    std::printf("grid %u %u %u %u %u %.17g %.17g %.17g %.17g %.17g %.17g %.17g %.17g %.9g %.9g %.9g\n", g.nt, g.nx, g.ny, g.n_bins, g.equal_mass, g.c0,
-                g.s0, g.x0, g.y0, g.half_u, g.scale_t, g.scale_x, g.scale_y, static_cast<double>(g.kt), static_cast<double>(g.kx),
-                static_cast<double>(g.ky));
+    schedule_from_moments(g, c.cbar, c.sbar, c.mx, c.my, c.vx, c.vy, c.n, c.mean_range, c.min_bin);
+    std::printf("grid %u %u %u %u %.17g %.17g %.17g %.9g %.9g %.9g\n", g.nt, g.nx, g.ny, g.n_bins, g.c0, g.s0, g.half_u,
+                static_cast<double>(g.kt), static_cast<double>(g.kx), static_cast<double>(g.ky));
   }
   for (int kx = 0; kx < 4; ++kx)
     for (uint32_t py = 0; py < 9; ++py)

@@ -241,6 +241,37 @@ def test_reweight_beam_matches_oracle(bb, orc, scene):
     assert np.allclose(got, exp, rtol=1e-11, atol=1e-300)  # erf/exp per beam differ by ulps between CUDA and glibc
 
 
+@pytest.mark.parametrize("shape, launches", [("wide_grid", 2), ("long_reach", 2), ("fine_cells", 3)])
+def test_reweight_beam_fallbacks_match_oracle(bb, orc, scene, shape, launches):
+    """Maps whose shape selects the fused beam kernel or the per-beam normalisers instead of the two-pass walk with the
+    normaliser table: a grid wider than 65534 cells (fused kernel, table), a reach of 2^21 cells or more (fused kernel,
+    per-beam normalisers), and a range / resolution ratio too large for the table (two-pass walk, per-beam normalisers).
+    The scene is scaled with the resolution (scan, sigma_hit, 1 / lambda_short) so that its rays hit at the usual ranges
+    in cells; beam_max_range stays in metres.  `launches`: begin_step plus 1 (fused) or 2 (walk + mixture)."""
+    rng = np.random.default_rng(23)
+    if shape == "wide_grid":
+        cells = np.where(rng.random((8, 70_000)) < 0.05, 100, 0).astype(np.int8)
+        res, max_range = scene.resolution, 20.0
+    else:
+        cells = scene.cells
+        res, max_range = (1e-5, 30.0) if shape == "long_reach" else (0.01, 30.0)
+    scale = res / scene.resolution
+    height, width = cells.shape
+    n = 300
+    states = np.array([orc.se2(x, y, t) for x, y, t in zip(rng.uniform(0.0, width * res, n), rng.uniform(0.0, height * res, n),
+                                                             rng.uniform(-PI, PI, n))])
+    pts = scene.scans[0][::3] * scale
+    bp = dict(sigma_hit=0.2 * scale, lambda_short=0.1 / scale, beam_max_range=max_range)
+    f = bb.Filter(capacity=n)
+    f.set_beam_map(bb.BeamModelParam(**bp), bb.OccupancyGrid(cells, res))
+    f.set_particles(states)
+    before = f.launch_count()
+    f.reweight(pts)
+    assert f.launch_count() - before == launches
+    exp = orc.sensor_weights(orc.BEAM, orc.BeamParam(**bp), orc.Grid(cells, res), pts, states)
+    assert np.allclose(f.particles()[1], exp, rtol=1e-11, atol=1e-300)
+
+
 def test_propagate_matches_oracle(bb, orc):
     rng = np.random.default_rng(11)
     states = random_states(orc, rng, 5000, 10.0)

@@ -10,6 +10,7 @@ C ABI used by the tests and by bench.py; names follow the reference:
     beluga::Amcl<...> (algorithm/amcl_core.hpp:81)          Amcl
     Amcl::initialize(pose, covariance)  (:145)              Amcl.initialize(mean_xytheta, cov)
     Amcl::update(control, measurement)  (:165)              Amcl.update(control_pose, points)
+    beluga_ros::Amcl::update(pose, laser_scan / cloud)      Amcl.update_scan(...) / Amcl.update_point_cloud(...)
     Amcl::update_map(map)               (:150)              Amcl.update_map(...)
     Amcl::particles()                   (:128)              Amcl.particles()
     DifferentialDriveModelParam                             DifferentialDriveModelParam
@@ -31,7 +32,7 @@ from ._capi import (RESAMPLE_MULTINOMIAL, RESAMPLE_SYSTEMATIC, SENSOR_BEAM, SENS
 
 __all__ = [
     "Amcl", "AmclParams", "BeamModelParam", "DifferentialDriveModelParam", "OmnidirectionalDriveModelParam", "StationaryModelParam",
-    "Filter", "LikelihoodFieldModelParam", "motion_sampling", "scan_to_points", "take_evenly_indices",
+    "Filter", "LikelihoodFieldModelParam", "motion_sampling", "scan_to_points", "point_cloud_to_points", "take_evenly_indices",
     "OccupancyGrid", "BelugaB200Error", "device_count", "se2",
     "RESAMPLE_MULTINOMIAL", "RESAMPLE_SYSTEMATIC", "SENSOR_BEAM", "SENSOR_LIKELIHOOD_FIELD", "SENSOR_LIKELIHOOD_FIELD_PROB",
 ]
@@ -151,6 +152,41 @@ def scan_to_points(ranges, angle_min: float, angle_increment: float, min_range: 
     st = _capi.load().bb200_scan_to_points(C.byref(scan), _dptr(out), len(out), C.byref(n))
     if st != _capi.OK:
         raise BelugaB200Error(st, "bb200_scan_to_points")
+    return out[: n.value]
+
+
+def _point_cloud(data, point_step: int, x_offset: int, dtype, origin, n_points):
+    if isinstance(data, np.ndarray):
+        raw = np.ascontiguousarray(data).reshape(-1).view(np.uint8)
+    else:
+        raw = np.frombuffer(data, dtype=np.uint8)
+    if n_points is None:
+        n_points = len(raw) // point_step if point_step > 0 else 0
+    if n_points * point_step > len(raw):
+        raise ValueError(f"{n_points} points of {point_step} bytes do not fit in {len(raw)} bytes")
+    if isinstance(dtype, (int, np.integer)):
+        datatype = int(dtype)
+    else:  # any other numpy type is not a coordinate type: 0 makes the library reject it
+        datatype = {np.dtype(np.float32): _capi.POINT_FLOAT32, np.dtype(np.float64): _capi.POINT_FLOAT64}.get(np.dtype(dtype), 0)
+    o = None if origin is None else _f64(origin).reshape(12)
+    cloud = _capi.PointCloud(raw.ctypes.data if len(raw) else None, n_points, point_step, x_offset, datatype,
+                             None if o is None else o.ctypes.data_as(C.POINTER(C.c_double)))
+    return cloud, (raw, o)  # keep the buffers alive
+
+
+def point_cloud_to_points(data, point_step: int, x_offset: int, dtype, origin=None, n_points: int | None = None) -> np.ndarray:
+    """beluga_ros::SparsePointCloud3f::points() moved into the base frame (beluga_ros/include/beluga_ros/sparse_point_cloud.hpp:102-125,
+    beluga_ros/src/amcl.cpp:67-81): the (x, y) of every point of a packed PointCloud2 buffer, in order, NaN points included.
+
+    `data`: the message's bytes (bytes, bytearray, memoryview or any contiguous numpy array, structured ones included);
+    `dtype`: the x/y/z field type, a PointField code (7 FLOAT32, 8 FLOAT64) or a numpy type; `origin`: 3x4 [R | t] of the cloud's
+    frame in the base frame, None for the identity; `n_points`: width * height, by default as many points as the buffer holds."""
+    cloud, keep = _point_cloud(data, point_step, x_offset, dtype, origin, n_points)
+    out = np.zeros((max(cloud.n_points, 1), 2))
+    n = C.c_uint64()
+    st = _capi.load().bb200_point_cloud_to_points(C.byref(cloud), _dptr(out), cloud.n_points, C.byref(n))
+    if st != _capi.OK:
+        raise BelugaB200Error(st, "bb200_point_cloud_to_points: datatype must be 7 (FLOAT32) or 8 (FLOAT64) and x, y, z must fit in point_step")
     return out[: n.value]
 
 
@@ -603,6 +639,14 @@ class Amcl:
         scan, keep = _laser_scan(ranges, angle_min, angle_increment, min_range, max_range, max_beams, laser_origin)
         res = _capi.UpdateResult()
         self._check(self._lib.bb200_amcl_update_scan(self._h, _dptr(_f64(control_pose)), C.byref(scan), C.byref(res)))
+        return res
+
+    def update_point_cloud(self, control_pose, data, point_step: int, x_offset: int, dtype, origin=None,
+                           n_points: int | None = None) -> _capi.UpdateResult:
+        """Amcl::update(base_pose_in_odom, point_cloud) (beluga_ros/src/amcl.cpp:67-81); arguments as point_cloud_to_points."""
+        cloud, keep = _point_cloud(data, point_step, x_offset, dtype, origin, n_points)
+        res = _capi.UpdateResult()
+        self._check(self._lib.bb200_amcl_update_point_cloud(self._h, _dptr(_f64(control_pose)), C.byref(cloud), C.byref(res)))
         return res
 
     def export_shard(self) -> bytes:

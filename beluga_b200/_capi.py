@@ -99,6 +99,14 @@ class LaserScan(C.Structure):
                 ("min_range", C.c_double), ("max_range", C.c_double), ("max_beams", C.c_uint64), ("laser_origin", C.POINTER(C.c_double))]
 
 
+POINT_FLOAT32, POINT_FLOAT64 = 7, 8  # sensor_msgs/PointField datatypes
+
+
+class PointCloud(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("n_points", C.c_uint64), ("point_step", C.c_uint32), ("x_offset", C.c_uint32), ("datatype", C.c_int),
+                ("origin", C.POINTER(C.c_double))]
+
+
 class MarkerVertex(C.Structure):
     _fields_ = [("x", C.c_double), ("y", C.c_double), ("z", C.c_double), ("r", C.c_float), ("g", C.c_float), ("b", C.c_float), ("a", C.c_float)]
 
@@ -182,6 +190,8 @@ SIGNATURES = {
     "bb200_scan_to_points": (C.c_int, [_P(LaserScan), _dbl, C.c_uint64, _P(C.c_uint64)]),
     "bb200_take_evenly_indices": (C.c_int, [C.c_uint64, C.c_uint64, _P(C.c_uint64), C.c_uint64, _P(C.c_uint64)]),
     "bb200_amcl_update_scan": (C.c_int, [_vp, _dbl, _P(LaserScan), _P(UpdateResult)]),
+    "bb200_point_cloud_to_points": (C.c_int, [_P(PointCloud), _dbl, C.c_uint64, _P(C.c_uint64)]),
+    "bb200_amcl_update_point_cloud": (C.c_int, [_vp, _dbl, _P(PointCloud), _P(UpdateResult)]),
     "bb200_sharded_amcl_create": (C.c_int, [_P(AmclParam), _P(MotionParam), C.c_int, _P(C.c_int), _P(_vp)]),
     "bb200_sharded_amcl_destroy": (None, [_vp]),
     "bb200_sharded_amcl_last_error": (C.c_char_p, [_vp]),

@@ -1,6 +1,7 @@
 // extern "C" surface of libbeluga_b200.so (declared in include/beluga_b200.h).
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <limits>
 #include <memory>
 #include <new>
@@ -77,6 +78,33 @@ template <class Body>
 int guarded_create(Body&& body) noexcept {
   CreateErrorContext c;
   return guarded(c, body);
+}
+
+/// One coordinate of a packed point cloud record.  The record has no alignment guarantee (PointCloud2 packs its fields),
+/// hence the copy.  float64 values are narrowed to float: SparsePointCloud3f casts them (sparse_point_cloud.hpp:106-116).
+template <class Scalar>
+double cloud_scalar(const unsigned char* p) {
+  Scalar v;
+  std::memcpy(&v, p, sizeof(Scalar));
+  return static_cast<double>(static_cast<float>(v));
+}
+
+/// SparsePointCloud3f::points() | transform(origin * p, keep (x, y))  (beluga_ros/src/amcl.cpp:73-78)
+template <class Scalar>
+void cloud_to_points(const bb200_point_cloud& c, double* points_xy) {
+  const unsigned char* base = static_cast<const unsigned char*>(c.data) + c.x_offset;
+  const double* m = c.origin;
+  for (uint64_t i = 0; i < c.n_points; ++i) {
+    const unsigned char* p = base + i * c.point_step;
+    const double x = cloud_scalar<Scalar>(p), y = cloud_scalar<Scalar>(p + sizeof(Scalar)), z = cloud_scalar<Scalar>(p + 2 * sizeof(Scalar));
+    double px = x, py = y;
+    if (m != nullptr) {
+      px = ((m[0] * x + m[1] * y) + m[2] * z) + m[3];
+      py = ((m[4] * x + m[5] * y) + m[6] * z) + m[7];
+    }
+    points_xy[2 * i] = px;
+    points_xy[2 * i + 1] = py;
+  }
 }
 }  // namespace
 
@@ -537,6 +565,37 @@ int bb200_amcl_update_scan(bb200_amcl* a, const double control_pose[4], const bb
     uint64_t n = 0;
     const int st = bb200_scan_to_points(scan, points.data(), scan->n_ranges + 1, &n);
     if (st != BB200_OK) return st;
+    return bb200_amcl_update(a, control_pose, points.data(), n, out);
+  });
+}
+
+int bb200_point_cloud_to_points(const bb200_point_cloud* cloud, double* points_xy, uint64_t capacity, uint64_t* n_points) {
+  BB_REQUIRE(cloud && n_points && (points_xy || capacity == 0));
+  const bool f32 = cloud->datatype == BB200_POINT_FLOAT32;
+  BB_REQUIRE(f32 || cloud->datatype == BB200_POINT_FLOAT64);
+  const uint64_t scalar = f32 ? sizeof(float) : sizeof(double);
+  BB_REQUIRE(static_cast<uint64_t>(cloud->x_offset) + 3 * scalar <= cloud->point_step);
+  BB_REQUIRE(cloud->data || cloud->n_points == 0);
+  if (cloud->n_points > capacity) return BB200_ERR_CAPACITY;
+  if (f32) {
+    cloud_to_points<float>(*cloud, points_xy);
+  } else {
+    cloud_to_points<double>(*cloud, points_xy);
+  }
+  *n_points = cloud->n_points;
+  return BB200_OK;
+}
+
+int bb200_amcl_update_point_cloud(bb200_amcl* a, const double control_pose[4], const bb200_point_cloud* cloud, bb200_update_result* out) {
+  BB_REQUIRE(a && control_pose && cloud && out);
+  return guarded(a->impl, [&] {
+    std::vector<double> points(2 * cloud->n_points);
+    uint64_t n = 0;
+    const int st = bb200_point_cloud_to_points(cloud, points.data(), cloud->n_points, &n);
+    if (st != BB200_OK) {
+      a->impl.record_error("point cloud: datatype must be 7 (FLOAT32) or 8 (FLOAT64), x, y and z must fit in point_step, data must be set");
+      return st;
+    }
     return bb200_amcl_update(a, control_pose, points.data(), n, out);
   });
 }

@@ -1,6 +1,7 @@
 """Synthetic localisation workload (SURVEY.md section 8(d)): occupancy map, closed trajectory with
 perfect odometry, and noisy 360-degree scans converted to base-frame cartesian points the way
-beluga_ros does (beluga/sensor/data/laser_scan.hpp:64-91 + beluga_ros/src/amcl.cpp:57-62).
+beluga_ros does (beluga/sensor/data/laser_scan.hpp:64-91 + beluga_ros/src/amcl.cpp:57-62), and lidar point clouds of the
+same scene as packed PointCloud2 records (make_point_cloud).
 
 Pure numpy; deterministic for a given configuration.  Used by bench.py and the tests to drive both
 the GPU backend and the CPU oracle with identical inputs.
@@ -104,3 +105,71 @@ def make_scenario(grid_size: int = 500, n_beams: int = 180, steps: int = 100, re
         scans.append(np.stack([r * np.cos(a), r * np.sin(a)], axis=1))  # laser_scan.hpp:64-70, laser at the base origin
     cov = np.diag([0.25, 0.25, 0.0685])  # likelihood_params.yaml:83-87
     return Scenario(cells, resolution, poses, scans, poses[0].copy(), cov)
+
+
+# A packed sensor_msgs/PointCloud2 record of a spinning lidar: x, y, z, intensity (FLOAT32), ring (UINT16), time (FLOAT32)
+# at offsets 0, 4, 8, 12, 16, 18, 22 bytes per point -- the Velodyne layout, no padding.  The float64 variant widens x, y, z.
+LIDAR_FIELDS = ("x", "y", "z", "intensity", "ring", "time")
+
+
+def lidar_record(coordinate_type=np.float32) -> np.dtype:
+    c = np.dtype(coordinate_type).newbyteorder("<")
+    w = c.itemsize
+    return np.dtype({"names": list(LIDAR_FIELDS), "formats": [c, c, c, "<f4", "<u2", "<f4"],
+                     "offsets": [0, w, 2 * w, 3 * w, 3 * w + 4, 3 * w + 6], "itemsize": 3 * w + 10})
+
+
+@dataclass
+class PointCloud:
+    data: np.ndarray           # structured [height * width] array of lidar_record(), row-major (one row per laser ring)
+    width: int                 # azimuths per ring
+    height: int                # rings
+    origin: np.ndarray         # 3x4 [R | t] of the sensor frame in the base frame
+
+    @property
+    def point_step(self) -> int:
+        return self.data.dtype.itemsize
+
+    @property
+    def x_offset(self) -> int:
+        return self.data.dtype.fields["x"][1]
+
+    @property
+    def datatype(self) -> int:  # sensor_msgs/PointField code of x, y, z
+        return 7 if self.data.dtype.fields["x"][0] == np.float32 else 8
+
+
+def sensor_origin(x: float = 0.2, y: float = -0.05, z: float = 0.8, roll: float = 0.01, pitch: float = -0.015, yaw: float = 0.03) -> np.ndarray:
+    """3x4 [R | t] with R = Rz(yaw) Ry(pitch) Rx(roll): a lidar mounted above the base, slightly tilted."""
+    cr, sr, cp, sp, cy, sy = np.cos(roll), np.sin(roll), np.cos(pitch), np.sin(pitch), np.cos(yaw), np.sin(yaw)
+    rot = np.array([[cy * cp, cy * sp * sr - sy * cr, cy * sp * cr + sy * sr],
+                    [sy * cp, sy * sp * sr + cy * cr, sy * sp * cr - cy * sr],
+                    [-sp, cp * sr, cp * cr]])
+    return np.concatenate([rot, np.array([[x], [y], [z]])], axis=1)
+
+
+def make_point_cloud(sc: Scenario, k: int, rows: int = 16, azimuths: int = 1024, seed: int = 7, origin=None, coordinate_type=np.float32,
+                     scan_max_range: float = 30.0, range_sigma: float = 0.02, vertical_fov: float = np.deg2rad(30.0)) -> PointCloud:
+    """The lidar cloud seen from pose k of the scenario: `rows` rings x `azimuths` beams over 360 degrees, expressed in the
+    sensor frame `origin` (default sensor_origin()).  The map is 2-D, so every ring hits the wall at the same horizontal
+    distance: the raycast range from the sensor's position plus the scans' noise (drawn per point), at the ring's
+    elevation, which gives each ring its own z.  The base-frame (x, y) of point (ring, j) is that hit; z is the sensor
+    height plus distance * tan(elevation).  Deterministic for given arguments."""
+    o = sensor_origin() if origin is None else np.asarray(origin, dtype=np.float64).reshape(3, 4)
+    rot, t = o[:, :3], o[:, 3]
+    yaw = np.arctan2(rot[1, 0], rot[0, 0])
+    x, y, theta = sc.poses[k]
+    sensor_pose = (x + np.cos(theta) * t[0] - np.sin(theta) * t[1], y + np.sin(theta) * t[0] + np.cos(theta) * t[1], theta + yaw)
+    d = raycast_ranges(sc.cells, sc.resolution, sensor_pose, azimuths, scan_max_range)
+    rng = np.random.Generator(np.random.MT19937(seed * 100003 + k))
+    d = np.clip(d[None, :] + rng.normal(0.0, range_sigma, (rows, azimuths)), 0.05, scan_max_range)
+    a = yaw + np.linspace(-np.pi, np.pi, azimuths, endpoint=False)  # beam directions in the base frame
+    elevation = np.linspace(-vertical_fov / 2, vertical_fov / 2, rows)[:, None]
+    base = np.stack([t[0] + d * np.cos(a), t[1] + d * np.sin(a), t[2] + d * np.tan(elevation)], axis=-1).reshape(-1, 3)
+    sensor = (base - t) @ rot  # R^T (p - t), row by row
+    out = np.zeros(rows * azimuths, dtype=lidar_record(coordinate_type))
+    out["x"], out["y"], out["z"] = sensor[:, 0], sensor[:, 1], sensor[:, 2]
+    out["intensity"] = (100.0 / (1.0 + d)).reshape(-1)
+    out["ring"] = np.repeat(np.arange(rows, dtype=np.uint16), azimuths)
+    out["time"] = np.tile(np.arange(azimuths, dtype=np.float32) / np.float32(azimuths * 10), rows)  # one sweep at 10 Hz
+    return PointCloud(out, azimuths, rows, o)

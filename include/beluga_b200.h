@@ -451,6 +451,34 @@ int bb200_scan_to_points(const bb200_laser_scan* scan, double* points_xy, uint64
 int bb200_take_evenly_indices(uint64_t size, uint64_t count, uint64_t* indices, uint64_t capacity, uint64_t* n_indices);
 /* Amcl::update(base_pose_in_odom, laser_scan) -- beluga_ros/src/amcl.cpp:54-64. */
 int bb200_amcl_update_scan(bb200_amcl* a, const double control_pose[4], const bb200_laser_scan* scan, bb200_update_result* out);
+/* The point-cloud input of the same step: a sensor_msgs/PointCloud2 read the way beluga_ros::SparsePointCloud3f reads it
+ * (beluga_ros/include/beluga_ros/sparse_point_cloud.hpp:102-125) and moved into the base frame by beluga_ros/src/amcl.cpp:67-81.
+ * Point i is the three consecutive scalars (x, y, z) at data + i * point_step + x_offset (no alignment required); float64
+ * coordinates are narrowed to float first (the alias is the non-strict float one), then every coordinate is widened to double
+ * and (x, y) = rows 0 and 1 of R * (x, y, z) + t, summed left to right.  `origin` is the 3x4 row-major [R | t] of the cloud's
+ * frame in the base frame (NULL: identity, coordinates pass unchanged), the convention of bb200_laser_scan::laser_origin; Sophus
+ * applies the rotation through its unit quaternion, so the two agree to rounding.  No point is dropped or reordered: NaN
+ * points go on to the sensor model, which treats them as out of the grid.  Checking the message's field names (x, y, z
+ * first, all of one type) is the caller's part. */
+typedef enum bb200_point_datatype {
+  BB200_POINT_FLOAT32 = 7, /* sensor_msgs/PointField FLOAT32 */
+  BB200_POINT_FLOAT64 = 8  /* sensor_msgs/PointField FLOAT64 */
+} bb200_point_datatype;
+typedef struct bb200_point_cloud {
+  const void* data;
+  uint64_t n_points;      /* width * height */
+  uint32_t point_step;    /* bytes from one point to the next */
+  uint32_t x_offset;      /* byte offset of x inside a point; y and z follow it */
+  int datatype;           /* bb200_point_datatype */
+  const double* origin;   /* 12 doubles or NULL */
+} bb200_point_cloud;
+/* Writes the n_points (x, y) pairs and their count.  BB200_ERR_INVALID_ARGUMENT for a datatype other than 7 or 8,
+ * x_offset + 3 * sizeof(scalar) > point_step, or data == NULL with n_points > 0 (the std::invalid_argument cases of the
+ * reference that reach this layer); BB200_ERR_CAPACITY when n_points > capacity.  On failure nothing is written. */
+int bb200_point_cloud_to_points(const bb200_point_cloud* cloud, double* points_xy, uint64_t capacity, uint64_t* n_points);
+/* Amcl::update(base_pose_in_odom, point_cloud) -- beluga_ros/src/amcl.cpp:67-81.  A sharded filter converts with
+ * bb200_point_cloud_to_points and calls bb200_sharded_amcl_update. */
+int bb200_amcl_update_point_cloud(bb200_amcl* a, const double control_pose[4], const bb200_point_cloud* cloud, bb200_update_result* out);
 
 /* ---------------------------------------------------------------------------------------------
  * One filter over several GPUs (SURVEY 8e).  Particles are split into equal contiguous global index

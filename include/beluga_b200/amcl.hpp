@@ -5,7 +5,8 @@
 // hasher,] params), same public methods -- particles(), initialize(pose, covariance),
 // update_map(map), update(control_action, measurement) -> std::optional<std::pair<pose, covariance>>,
 // force_update() -- and the same AmclParams members and defaults (:34-55).  The particle set lives
-// on the GPU; particles() copies it out on demand.
+// on the GPU; particles() copies it out on demand.  update() also takes a point cloud, as the second
+// overload of beluga_ros::Amcl::update does (beluga_ros/src/amcl.cpp:67-81).
 //
 // What differs from the template: the random state generator is always the map's free-cell uniform
 // distribution (what beluga_ros::Amcl passes, beluga_ros/include/beluga_ros/amcl.hpp:269), the
@@ -129,11 +130,25 @@ class Amcl {
     static_assert(sizeof(std::pair<double, double>) == 2 * sizeof(double), "measurement points must be packed");
     bb200_update_result r{};
     check(bb200_amcl_update(handle_, control_action.data(), token.points.empty() ? nullptr : &token.points.front().first, token.points.size(), &r));
-    if (!r.updated) return std::nullopt;
-    Matrix3d cov;
-    for (int i = 0; i < 9; ++i) cov[i] = r.estimate.cov[i];
-    return std::make_pair(state_type::from_data(r.estimate.mean), cov);
+    return estimate_of(r);
   }
+
+  /// beluga_ros::Amcl::update(base_pose_in_odom, point_cloud) (beluga_ros/src/amcl.cpp:67-81): the cloud's points moved
+  /// into the base frame, then the update above.  Throws Error(BB200_ERR_INVALID_ARGUMENT) on an unusable layout.
+  auto update(const state_type& control_action, const PointCloudView& cloud) -> std::optional<estimation_type> {
+    const bb200_point_cloud c = cloud.c_view();
+    bb200_update_result r{};
+    check(bb200_amcl_update_point_cloud(handle_, control_action.data(), &c, &r));
+    return estimate_of(r);
+  }
+#ifdef BELUGA_B200_WITH_SOPHUS
+  /// The same for any beluga::BaseSparsePointCloud-shaped cloud, e.g. beluga_ros::SparsePointCloud3f.
+  template <class SparsePointCloud, std::enable_if_t<is_sparse_point_cloud_v<SparsePointCloud>, int> = 0>
+  auto update(const state_type& control_action, const SparsePointCloud& cloud) -> std::optional<estimation_type> {
+    const PackedPointCloud packed{cloud};
+    return update(control_action, packed.view());
+  }
+#endif
 
   /// amcl_core.hpp:204
   void force_update() { bb200_amcl_force_update(handle_); }
@@ -143,6 +158,12 @@ class Amcl {
  private:
   void check(int status) const {
     if (status != BB200_OK) throw Error(status, bb200_amcl_last_error(handle_));
+  }
+  static auto estimate_of(const bb200_update_result& r) -> std::optional<estimation_type> {
+    if (!r.updated) return std::nullopt;
+    Matrix3d cov;
+    for (int i = 0; i < 9; ++i) cov[i] = r.estimate.cov[i];
+    return std::make_pair(state_type::from_data(r.estimate.mean), cov);
   }
 
   AmclParams params_;

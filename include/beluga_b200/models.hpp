@@ -29,6 +29,7 @@
 #ifdef BELUGA_B200_WITH_SOPHUS
 #include <Eigen/Core>
 #include <sophus/se2.hpp>
+#include <sophus/se3.hpp>
 #endif
 
 namespace beluga_b200 {
@@ -244,6 +245,72 @@ struct BeamModelParam {
 struct measurement_token {
   std::vector<std::pair<double, double>> points;
 };
+
+// ---- point clouds --------------------------------------------------------------------------------
+
+/// A sensor_msgs/PointCloud2 buffer as beluga_ros::SparsePointCloud3f reads it
+/// (beluga_ros/include/beluga_ros/sparse_point_cloud.hpp:102-125): point i is the three scalars x, y, z at
+/// data + i * point_step + x_offset.  `origin` is the cloud's frame in the base frame as a 3x4 row-major [R | t]
+/// (nullptr: the identity).  A view: the buffers must outlive it.
+struct PointCloudView {
+  const void* data = nullptr;
+  std::uint64_t size = 0;  // width * height
+  std::uint32_t point_step = 0;
+  std::uint32_t x_offset = 0;
+  bb200_point_datatype datatype = BB200_POINT_FLOAT32;
+  const double* origin = nullptr;
+
+  [[nodiscard]] bb200_point_cloud c_view() const { return bb200_point_cloud{data, size, point_step, x_offset, datatype, origin}; }
+};
+
+/// The base-frame (x, y) of every point, in order (beluga_ros/src/amcl.cpp:67-78); host only, needs no GPU.
+/// Throws Error(BB200_ERR_INVALID_ARGUMENT) where SparsePointCloud3 throws std::invalid_argument on the layout.
+[[nodiscard]] inline std::vector<std::pair<double, double>> point_cloud_points(const PointCloudView& cloud) {
+  static_assert(sizeof(std::pair<double, double>) == 2 * sizeof(double), "measurement points must be packed");
+  std::vector<std::pair<double, double>> out(cloud.size);
+  const bb200_point_cloud c = cloud.c_view();
+  std::uint64_t n = 0;
+  const int st = bb200_point_cloud_to_points(&c, out.empty() ? nullptr : &out.front().first, out.size(), &n);
+  if (st != BB200_OK) throw Error(st, "point cloud: datatype must be FLOAT32 or FLOAT64 and x, y, z must fit in point_step");
+  return out;
+}
+
+#ifdef BELUGA_B200_WITH_SOPHUS
+namespace detail {
+template <class T, class = void>
+struct is_sparse_point_cloud : std::false_type {};
+/// Shaped like beluga::BaseSparsePointCloud (beluga/sensor/data/sparse_point_cloud.hpp): points() is a range of 3-vectors
+/// with x(), y(), z(), and origin() is the Sophus::SE3d of the cloud's frame in the filter's base frame.
+template <class T>
+struct is_sparse_point_cloud<T, std::void_t<decltype((*std::declval<const T&>().points().begin()).z()),
+                                            decltype(std::declval<const T&>().origin().matrix3x4())>>
+    : std::is_convertible<decltype(std::declval<const T&>().origin()), Sophus::SE3d> {};
+}  // namespace detail
+template <class T>
+inline constexpr bool is_sparse_point_cloud_v = detail::is_sparse_point_cloud<T>::value;
+
+/// A BaseSparsePointCloud-shaped cloud packed into float32 x, y, z records plus its origin: the C-ABI view of it.
+/// Coordinates are narrowed to float, which is what beluga_ros's SparsePointCloud3f alias hands to Amcl::update.
+struct PackedPointCloud {
+  std::vector<float> xyz;
+  std::array<double, 12> origin{};
+
+  template <class SparsePointCloud, std::enable_if_t<is_sparse_point_cloud_v<SparsePointCloud>, int> = 0>
+  explicit PackedPointCloud(const SparsePointCloud& cloud) {
+    for (const auto& p : cloud.points()) {
+      xyz.push_back(static_cast<float>(p.x()));
+      xyz.push_back(static_cast<float>(p.y()));
+      xyz.push_back(static_cast<float>(p.z()));
+    }
+    const auto m = cloud.origin().matrix3x4();
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 4; ++c) origin[static_cast<std::size_t>(4 * r + c)] = m(r, c);
+  }
+  [[nodiscard]] PointCloudView view() const {
+    return PointCloudView{xyz.data(), xyz.size() / 3, 3 * sizeof(float), 0, BB200_POINT_FLOAT32, origin.data()};
+  }
+};
+#endif
 
 namespace detail {
 

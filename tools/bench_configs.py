@@ -1,9 +1,11 @@
 #!/usr/bin/env python
-"""Timings of the other BASELINE.json configurations (parity-test cases, not the bench.py line):
+"""Timings of the other BASELINE.json configurations (parity-test cases, not the bench.py line), and of point-cloud updates:
+`cloud`: 65 536-point lidar clouds at 10k and 1M particles.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import json
 import os
+import subprocess
 import sys
 import time
 
@@ -18,7 +20,8 @@ MOTION = (0.1, 0.05, 0.1, 0.05)
 LFM = dict(max_obstacle_distance=2.0, max_laser_distance=100.0, z_hit=0.5, z_random=0.5, sigma_hit=0.2)
 
 
-def run_gpu(sc, sensor, sensor_params, params, steps, warmup=2):
+def run_gpu(sc, sensor, sensor_params, params, steps, warmup=2, clouds=None):
+    """`clouds`: one synthetic.PointCloud per step, fed through Amcl.update_point_cloud (conversion included in the step time)."""
     a = bb.Amcl(bb.DifferentialDriveModelParam(*MOTION), params)
     a.update_map(sensor, sensor_params, bb.OccupancyGrid(sc.cells, sc.resolution))
     a.initialize(sc.initial_mean, sc.initial_cov)
@@ -26,8 +29,13 @@ def run_gpu(sc, sensor, sensor_params, params, steps, warmup=2):
     wall, sizes, kernels = [], [], {}
     for k in range(warmup + steps):
         a.filter.clear_timings()
+        pose = bb.se2(*sc.poses[k % 100])
         t0 = time.perf_counter()
-        r = a.update(bb.se2(*sc.poses[k % 100]), sc.scans[k % 100])
+        if clouds is None:
+            r = a.update(pose, sc.scans[k % 100])
+        else:
+            pc = clouds[k]
+            r = a.update_point_cloud(pose, pc.data, pc.point_step, pc.x_offset, pc.datatype, origin=pc.origin)
         dt = time.perf_counter() - t0
         assert r.updated == 1
         if k >= warmup:
@@ -37,6 +45,43 @@ def run_gpu(sc, sensor, sensor_params, params, steps, warmup=2):
                 kernels[name] = kernels.get(name, 0.0) + ms / steps
     return {"ms_per_step_e2e": float(np.mean(wall)), "steps_per_s_e2e": 1e3 / float(np.mean(wall)), "particles": sizes,
             "kernels_ms": {k: round(v, 4) for k, v in kernels.items()}}
+
+
+def device_record():
+    """Name and power limit of the card this process measures on (a read-only nvidia-smi query)."""
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, check=True)
+        name, power, clock = (q.stdout.strip().split(", ") + ["?", "?", "?"])[:3]
+    except (OSError, subprocess.CalledProcessError):
+        name, power, clock = "nvidia-smi unavailable", "?", "?"
+    return {"name": name, "power_limit": power, "clocks_max_sm": clock}
+
+
+def run_cloud():
+    """Point-cloud updates (Amcl.update_point_cloud) with 64 x 1024 synthetic lidar clouds: 10k particles on C1's 500^2 map (the
+    node-sized case) and 1M on C2's 2000^2 map, and beside them C2's 1M x 1080 scan in the same process, so that the reweight
+    kernel's lookup rate with 32 shared-memory chunks per particle can be read against the scan's."""
+    res = {}
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    cases = (("cloud_10k_x_65536_lfm_500", 500, 10_000, 20, 2), ("cloud_1M_x_65536_lfm_2000", 2000, 1_000_000, 5, 1))
+    for name, grid, n, steps, warmup in cases:
+        sc = synthetic.make_scenario(grid_size=grid, n_beams=1080, steps=100)
+        clouds = [synthetic.make_point_cloud(sc, k, rows=64, azimuths=1024) for k in range(warmup + steps)]
+        params = bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=1)
+        r = run_gpu(sc, bb.SENSOR_LIKELIHOOD_FIELD, lfm, params, steps=steps, warmup=warmup, clouds=clouds)
+        r["points"] = 64 * 1024
+        r["lookups_per_ns_reweight"] = n * r["points"] / (r["kernels_ms"]["reweight_lfm"] * 1e6)
+        res[name] = r
+        if grid == 2000:
+            scan = run_gpu(sc, bb.SENSOR_LIKELIHOOD_FIELD, lfm, params, steps=10, warmup=3)
+            scan["points"] = 1080
+            scan["lookups_per_ns_reweight"] = n * 1080 / (scan["kernels_ms"]["reweight_lfm"] * 1e6)
+            res["cloud_reference_1M_x_1080_scan_lfm_2000"] = scan
+    device = device_record()
+    for r in res.values():
+        r["device"] = device
+    return res
 
 
 def main():
@@ -90,6 +135,8 @@ def main():
         out["c4_kld_100k_10M_lfm"] = run_gpu(sc, bb.SENSOR_LIKELIHOOD_FIELD, bb.LikelihoodFieldModelParam(**LFM),
                                              bb.AmclParams(min_particles=100_000, max_particles=10_000_000, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=1,
                                                            spatial_resolution=(0.5, 0.5, float(np.deg2rad(10.0)))), steps=6, warmup=1)  # beluga_ros defaults (SURVEY 8d)
+    if "cloud" in which:
+        out.update(run_cloud())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}

@@ -31,7 +31,7 @@ from ._capi import (RESAMPLE_MULTINOMIAL, RESAMPLE_SYSTEMATIC, SENSOR_BEAM, SENS
                     SENSOR_LIKELIHOOD_FIELD_PROB)
 
 __all__ = [
-    "Amcl", "AmclParams", "BeamModelParam", "DifferentialDriveModelParam", "OmnidirectionalDriveModelParam", "StationaryModelParam",
+    "Amcl", "AmclBatch", "AmclParams", "BeamModelParam", "DifferentialDriveModelParam", "OmnidirectionalDriveModelParam", "StationaryModelParam",
     "Filter", "LikelihoodFieldModelParam", "motion_sampling", "scan_to_points", "point_cloud_to_points", "take_evenly_indices",
     "OccupancyGrid", "BelugaB200Error", "device_count", "se2",
     "RESAMPLE_MULTINOMIAL", "RESAMPLE_SYSTEMATIC", "SENSOR_BEAM", "SENSOR_LIKELIHOOD_FIELD", "SENSOR_LIKELIHOOD_FIELD_PROB",
@@ -752,3 +752,92 @@ class ShardedAmcl:
         if n:
             self._check(self._lib.bb200_sharded_amcl_get_particles(self._h, _dptr(st), _dptr(w), n))
         return st, w
+
+
+class AmclBatch:
+    """bb200_amcl_batch: K independent beluga::Amcl filters on one GPU, sharing one likelihood-field map; update() steps every
+    member with a new scan with a fixed number of kernel launches and one synchronisation.  Member m's results and particles
+    equal those of a standalone Amcl built from params[m] and motions[m] and fed the same inputs."""
+
+    def __init__(self, motions, params):
+        """`motions[m]`, `params[m]`: member m's motion model and AmclParams (min_particles == max_particles <= 32768)."""
+        self._lib = _capi.load()
+        k = len(params)
+        if len(motions) != k:
+            raise ValueError("one motion model per member")
+        p = (_capi.AmclParam * max(k, 1))(*[q.c() for q in params])
+        m = (_capi.MotionParam * max(k, 1))(*[q.c_motion() for q in motions])
+        h = C.c_void_p()
+        st = self._lib.bb200_amcl_batch_create(p, m, k, C.byref(h))
+        if st != _capi.OK:
+            raise BelugaB200Error(st, self._lib.bb200_create_error().decode())
+        self._h = h
+        self.params = list(params)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.bb200_amcl_batch_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        self.close()
+
+    def __len__(self) -> int:
+        return self._lib.bb200_amcl_batch_members(self._h)
+
+    def _check(self, st: int):
+        if st != _capi.OK:
+            raise BelugaB200Error(st, self._lib.bb200_amcl_batch_last_error(self._h).decode())
+
+    def set_likelihood_field_map(self, params: LikelihoodFieldModelParam, grid: OccupancyGrid, prob: bool = False):
+        p, g = params.c(), grid.c()
+        self._check(self._lib.bb200_amcl_batch_set_likelihood_field_map(self._h, C.byref(p), C.byref(g), int(prob)))
+
+    def initialize(self, member: int, mean_xytheta, cov):
+        self._check(self._lib.bb200_amcl_batch_initialize(self._h, member, _dptr(_f64(mean_xytheta)), _dptr(_f64(cov).reshape(9))))
+
+    def initialize_from_map(self, member: int):
+        self._check(self._lib.bb200_amcl_batch_initialize_from_map(self._h, member))
+
+    def initialize_states(self, member: int, states, weights=None):
+        st = _f64(states).reshape(-1, 4)
+        w = None if weights is None else _f64(weights)
+        self._check(self._lib.bb200_amcl_batch_initialize_states(self._h, member, _dptr(st), None if w is None else _dptr(w), len(st)))
+
+    def force_update(self, member: int):
+        self._check(self._lib.bb200_amcl_batch_force_update(self._h, member))
+
+    def particles(self, member: int):
+        n = self.params[member].max_particles
+        st = np.zeros((n, 4))
+        w = np.zeros(n)
+        self._check(self._lib.bb200_amcl_batch_get_particles(self._h, member, _dptr(st), _dptr(w), n))
+        return st, w
+
+    def ancestors(self, member: int) -> np.ndarray:
+        out = np.zeros(self.params[member].max_particles, dtype=np.int64)
+        self._check(self._lib.bb200_amcl_batch_ancestors(self._h, member, out.ctypes.data_as(C.POINTER(C.c_int64)), len(out)))
+        return out
+
+    def cluster_estimate(self, member: int, linear: float = 0.20, angular: float = 0.524, percentile: float = 0.90):
+        """beluga::cluster_based_estimate of one member -> (mean[4], cov[3, 3])."""
+        p = _capi.ClusterParam(linear, angular, percentile)
+        est = _capi.Estimate()
+        self._check(self._lib.bb200_amcl_batch_cluster_estimate(self._h, member, C.byref(p), C.byref(est)))
+        return np.array(est.mean), np.array(est.cov).reshape(3, 3)
+
+    def update(self, control_poses, points, present=None) -> list:
+        """Amcl::update for every member whose `present` entry is true (None: all).  `control_poses`: K poses [c, s, x, y];
+        `points[m]`: member m's (x, y) points.  Returns K UpdateResult blocks; `.updated == 0` for absent members."""
+        k = len(self.params)
+        poses = _f64(control_poses).reshape(k, 4)
+        pts = [_f64(p).reshape(-1, 2) for p in points]
+        ptrs = (C.POINTER(C.c_double) * k)(*[_dptr(p) if len(p) else None for p in pts])
+        counts = (C.c_uint64 * k)(*[len(p) for p in pts])
+        mask = None if present is None else (C.c_uint8 * k)(*[1 if x else 0 for x in present])
+        res = (_capi.UpdateResult * k)()
+        self._check(self._lib.bb200_amcl_batch_update(self._h, _dptr(poses), ptrs, counts, mask, res))
+        return list(res)
+
+    def launch_count(self) -> int:
+        return self._lib.bb200_amcl_batch_launch_count(self._h)

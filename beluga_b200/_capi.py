@@ -211,6 +211,20 @@ SIGNATURES = {
     "bb200_amcl_leave_shards": (C.c_int, [_vp]),
     "bb200_filter_export_shard": (C.c_int, [_vp, _vp]),
     "bb200_filter_join_shards": (C.c_int, [_vp, C.c_int, C.c_int, _vp]),
+    "bb200_amcl_batch_create": (C.c_int, [_P(AmclParam), _P(MotionParam), C.c_int, _P(_vp)]),
+    "bb200_amcl_batch_destroy": (None, [_vp]),
+    "bb200_amcl_batch_last_error": (C.c_char_p, [_vp]),
+    "bb200_amcl_batch_members": (C.c_int, [_vp]),
+    "bb200_amcl_batch_set_likelihood_field_map": (C.c_int, [_vp, _P(LikelihoodFieldParam), _P(OccupancyGrid), C.c_int]),
+    "bb200_amcl_batch_initialize": (C.c_int, [_vp, C.c_int, _dbl, _dbl]),
+    "bb200_amcl_batch_initialize_from_map": (C.c_int, [_vp, C.c_int]),
+    "bb200_amcl_batch_initialize_states": (C.c_int, [_vp, C.c_int, _dbl, _dbl, C.c_uint64]),
+    "bb200_amcl_batch_force_update": (C.c_int, [_vp, C.c_int]),
+    "bb200_amcl_batch_get_particles": (C.c_int, [_vp, C.c_int, _dbl, _dbl, C.c_uint64]),
+    "bb200_amcl_batch_ancestors": (C.c_int, [_vp, C.c_int, _P(C.c_int64), C.c_uint64]),
+    "bb200_amcl_batch_cluster_estimate": (C.c_int, [_vp, C.c_int, _P(ClusterParam), _P(Estimate)]),
+    "bb200_amcl_batch_update": (C.c_int, [_vp, _dbl, _P(_dbl), _P(C.c_uint64), _P(C.c_uint8), _P(UpdateResult)]),
+    "bb200_amcl_batch_launch_count": (C.c_uint64, [_vp]),
     "bb200_amcl_plan_update": (C.c_int, [_vp, _dbl, _P(StepPlan)]),
     "bb200_amcl_commit_update": (None, [_vp, C.c_int, C.c_double]),
     "bb200_amcl_create_with_motion": (C.c_int, [_P(AmclParam), _P(MotionParam), _P(_vp)]),

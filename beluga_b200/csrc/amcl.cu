@@ -87,6 +87,10 @@ bb200_motion_sampling motion_sampling(const bb200_motion_param& p, const Pose2& 
   return out;
 }
 
+Amcl::Amcl(const bb200_amcl_param& p, const bb200_motion_param& motion, HostOnly) : params_(p), motion_(motion) {
+  if (params_.resample_interval == 0) params_.resample_interval = 1;
+}
+
 Amcl::Amcl(const bb200_amcl_param& p, const bb200_motion_param& motion) : params_(p), motion_(motion) {
   bb200_filter_config c{};
   c.device = p.device;
@@ -135,7 +139,7 @@ int Amcl::plan_update(const double control[4], bb200_step_plan* plan) {
   *plan = bb200_step_plan{};
   const Pose2 pose{control[0], control[1], control[2], control[3]};
   // Sharded filters gate on the GLOBAL particle count, which never drops to zero once initialised.
-  const uint64_t n = sharded() ? (initialized_ ? filter_->global_size() : 0u) : filter_->size();
+  const uint64_t n = !filter_ ? host_size_ : sharded() ? (initialized_ ? filter_->global_size() : 0u) : filter_->size();
   if (n == 0) return BB200_OK;  // amcl_core.hpp:166-168 -> std::nullopt
 
   // update_policy_(control_action) -- on_motion vs the last ACCEPTED pose (on_motion.hpp:121-133)

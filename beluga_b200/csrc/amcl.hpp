@@ -19,11 +19,24 @@ bb200_motion_sampling motion_sampling(const bb200_motion_param& p, const Pose2& 
 class Amcl {
  public:
   Amcl(const bb200_amcl_param& p, const bb200_motion_param& motion);
+  /// The host half alone (policies, control window, recovery estimator) for a filter whose particles live elsewhere -- a
+  /// member of a batch (csrc/batch.hpp).  The owner reports the particle count through set_host_size().
+  struct HostOnly {};
+  Amcl(const bb200_amcl_param& p, const bb200_motion_param& motion, HostOnly);
 
   Filter& filter() { return *filter_; }
   bool ok() const { return filter_ && filter_->ok(); }
   int create_status() const { return filter_ ? filter_->create_status() : BB200_ERR_CUDA; }
-  const char* last_error() const { return error_.empty() ? filter_->last_error() : error_.c_str(); }
+  const char* last_error() const { return error_.empty() && filter_ ? filter_->last_error() : error_.c_str(); }
+  /// Host-only: what initialize*() records after the owner has placed n particles.
+  void host_initialized(uint64_t n) {
+    host_size_ = n;
+    force_update_ = true;
+    initialized_ = n > 0;
+  }
+  /// Host-only: the particle count after a step (a resample sets it to max_particles).
+  void set_host_size(uint64_t n) { host_size_ = n; }
+  uint64_t host_size() const { return host_size_; }
   void record_error(const std::string& message) const { error_ = message; }  // the C-ABI exception guard
 
   int initialize(const double mean[3], const double cov[9]);
@@ -62,7 +75,9 @@ class Amcl {
   bool force_update_{true};
   bool initialized_{false};
   uint32_t step_{0};
+  uint64_t host_size_{0};  // particle count of a host-only instance
 
+ public:
   /// Everything plan_update() advances.  The reference's update() is atomic: when the device half of a step
   /// fails, the host half is rolled back so that a retry sees the same motion delta, every_n phase and filters.
   struct HostState {
@@ -76,6 +91,8 @@ class Amcl {
   };
   HostState snapshot() const;
   void restore(const HostState& s);
+
+ private:
   int update_device(const double control[4], const double* points_xy, uint64_t n_points, bb200_update_result* out);
 };
 

@@ -1,0 +1,95 @@
+// K independent beluga::Amcl filters that share one device, one likelihood-field map and one sensor model, stepped
+// together: one call runs every updating member's step with a fixed sequence of launches (csrc/kernels.cuh:
+// launch_batch_step) and one host synchronisation, whatever K is.  Each member keeps the host half of a bb200_amcl
+// (policies, control window, recovery estimator: an Amcl without a Filter) and a slice of the batch's particle buffers.
+#pragma once
+
+#include <memory>
+#include <string>
+#include <vector>
+
+#include "amcl.hpp"
+#include "filter.hpp"
+
+namespace bb200 {
+
+/// Largest particle count of a batch member: one member's kernels then run in at most 128 CTAs of each launch.
+constexpr uint64_t kBatchMaxParticles = 32768;
+
+class Batch {
+ public:
+  Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members);
+  ~Batch();
+  Batch(const Batch&) = delete;
+  Batch& operator=(const Batch&) = delete;
+
+  /// The configurations a batch rejects, checked without touching a device (BB200_OK or BB200_ERR_INVALID_ARGUMENT).
+  static int validate(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, std::string* error);
+
+  bool ok() const { return created_; }
+  int create_status() const { return create_status_; }
+  const char* last_error() const { return error_.c_str(); }
+  void record_error(const std::string& message) const { error_ = message; }  // the C-ABI exception guard
+  int members() const { return static_cast<int>(members_.size()); }
+  uint64_t launch_count() const { return launches_; }
+
+  int set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob);
+  int initialize(int member, const double mean[3], const double cov[9]);
+  int initialize_from_map(int member);
+  int initialize_states(int member, const double* states, const double* weights, uint64_t n);
+  int force_update(int member);
+  int get_particles(int member, double* states, double* weights, uint64_t capacity);
+  int ancestors(int member, int64_t* out, uint64_t capacity);
+  int cluster_estimate(int member, const bb200_cluster_param& p, bb200_estimate* out);
+  /// Amcl::update for every member whose present[m] is non-zero (present == nullptr: all of them).  Atomic for the whole
+  /// batch: when the device half fails, every member's host state is rolled back.
+  int update(const double* control_poses, const double* const* points_xy, const uint64_t* n_points, const uint8_t* present,
+             bb200_update_result* out);
+
+ private:
+  struct Member {
+    std::unique_ptr<Amcl> host;
+    uint64_t offset{0};    // first particle in the batch buffers
+    uint64_t capacity{0};  // max_particles
+    uint64_t n{0};
+    int cur{0};            // state buffer holding the particles
+    double pivot[2]{0.0, 0.0};
+    uint64_t seed{0};
+    uint64_t ancestors_n{0};
+  };
+  int fail(int status, const std::string& message);
+  int check(cudaError_t e, const char* what);
+  int from_map(int status);  // forwards the map filter's message
+  int member_ok(int member) const;
+  int ensure_points(uint64_t n_points);
+
+  std::vector<Member> members_;
+  std::unique_ptr<Filter> map_;  // the map, the stream and the clusterizer scratch (sized for the largest member)
+  bool created_{false};
+  int create_status_{BB200_OK};
+  mutable std::string error_;
+  bool record_ancestors_{false};
+
+  uint64_t total_{0};
+  Pose2* states_[2]{nullptr, nullptr};
+  double* weights_{nullptr};
+  unsigned long long* cdf_{nullptr};
+  long long* ancestors_{nullptr};
+  Scalars* scalars_{nullptr};
+  unsigned long long* tile_state_{nullptr};
+  double* partials_{nullptr};
+  BatchMember* table_{nullptr};       // device
+  BatchMember* table_host_{nullptr};  // pinned
+  uint32_t* first_{nullptr};          // device: kBatchLaunches x (K + 1)
+  uint32_t* first_host_{nullptr};     // pinned
+  double* points_{nullptr};
+  double* points_host_{nullptr};      // pinned
+  uint64_t points_capacity_{0};       // points (pairs)
+  StepSummary* summary_host_{nullptr};  // pinned, one per member of the step's table
+  int* ticket_host_{nullptr};           // pinned
+  unsigned int* members_done_{nullptr};
+  int seq_{0};
+  uint64_t launches_{0};
+};
+
+}  // namespace bb200

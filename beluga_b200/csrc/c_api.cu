@@ -11,10 +11,12 @@
 
 #include "../../include/beluga_b200.h"
 #include "amcl.hpp"
+#include "batch.hpp"
 #include "cluster_host.hpp"
 #include "filter.hpp"
 
 using bb200::Amcl;
+using bb200::Batch;
 using bb200::Filter;
 
 struct bb200_filter {
@@ -26,6 +28,11 @@ struct bb200_amcl {
   Amcl impl;
   bb200_filter* filter_view;  // non-owning alias handed out by bb200_amcl_filter
   bb200_amcl(const bb200_amcl_param& p, const bb200_motion_param& m) : impl(p, m), filter_view(nullptr) {}
+};
+
+struct bb200_amcl_batch {
+  Batch impl;
+  bb200_amcl_batch(const bb200_amcl_param* p, const bb200_motion_param* m, int n) : impl(p, m, n) {}
 };
 
 /// One filter over several shards driven by ONE host thread (the shape of beluga_ros's single-process node).
@@ -804,6 +811,71 @@ int bb200_sharded_amcl_get_particles(bb200_sharded_amcl* g, double* states, doub
     return static_cast<int>(BB200_OK);
   });
 }
+
+// ---- batches ------------------------------------------------------------------------------------------
+
+int bb200_amcl_batch_create(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bb200_amcl_batch** out) {
+  if (out == nullptr) {
+    g_create_error = "null argument";
+    return BB200_ERR_INVALID_ARGUMENT;
+  }
+  *out = nullptr;
+  {
+    const int st = Batch::validate(params, motions, n_members, &g_create_error);  // before any device is touched
+    if (st != BB200_OK) return st;
+  }
+  return guarded_create([&] {
+    auto b = std::make_unique<bb200_amcl_batch>(params, motions, n_members);
+    if (!b->impl.ok()) {
+      g_create_error = b->impl.last_error();
+      return b->impl.create_status();
+    }
+    *out = b.release();
+    return static_cast<int>(BB200_OK);
+  });
+}
+void bb200_amcl_batch_destroy(bb200_amcl_batch* b) { delete b; }
+const char* bb200_amcl_batch_last_error(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.last_error() : "null batch"; }
+int bb200_amcl_batch_members(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.members() : 0; }
+int bb200_amcl_batch_set_likelihood_field_map(bb200_amcl_batch* b, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid,
+                                              int prob) {
+  BB_REQUIRE(b && p && grid);
+  return guarded(b->impl, [&] { return b->impl.set_likelihood_field_map(*p, *grid, prob != 0); });
+}
+int bb200_amcl_batch_initialize(bb200_amcl_batch* b, int member, const double mean_xytheta[3], const double cov[9]) {
+  BB_REQUIRE(b && mean_xytheta && cov);
+  return guarded(b->impl, [&] { return b->impl.initialize(member, mean_xytheta, cov); });
+}
+int bb200_amcl_batch_initialize_from_map(bb200_amcl_batch* b, int member) {
+  BB_REQUIRE(b);
+  return guarded(b->impl, [&] { return b->impl.initialize_from_map(member); });
+}
+int bb200_amcl_batch_initialize_states(bb200_amcl_batch* b, int member, const double* states, const double* weights, uint64_t n) {
+  BB_REQUIRE(b);
+  return guarded(b->impl, [&] { return b->impl.initialize_states(member, states, weights, n); });
+}
+int bb200_amcl_batch_force_update(bb200_amcl_batch* b, int member) {
+  BB_REQUIRE(b);
+  return b->impl.force_update(member);
+}
+int bb200_amcl_batch_get_particles(bb200_amcl_batch* b, int member, double* states, double* weights, uint64_t capacity) {
+  BB_REQUIRE(b);
+  return guarded(b->impl, [&] { return b->impl.get_particles(member, states, weights, capacity); });
+}
+int bb200_amcl_batch_ancestors(bb200_amcl_batch* b, int member, int64_t* out, uint64_t capacity) {
+  BB_REQUIRE(b && (out || capacity == 0));
+  return guarded(b->impl, [&] { return b->impl.ancestors(member, out, capacity); });
+}
+int bb200_amcl_batch_cluster_estimate(bb200_amcl_batch* b, int member, const bb200_cluster_param* p, bb200_estimate* out) {
+  BB_REQUIRE(b && p && out);
+  return guarded(b->impl, [&] { return b->impl.cluster_estimate(member, *p, out); });
+}
+int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, const double* const* points_xy, const uint64_t* n_points,
+                            const uint8_t* present, bb200_update_result* out) {
+  BB_REQUIRE(b && control_poses && points_xy && n_points && out);
+  return guarded(b->impl, [&] { return b->impl.update(control_poses, points_xy, n_points, present, out); });
+}
+uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.launch_count() : 0; }
 
 int bb200_amcl_plan_update(bb200_amcl* a, const double control_pose[4], bb200_step_plan* plan) {
   BB_REQUIRE(a && control_pose && plan);

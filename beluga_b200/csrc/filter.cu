@@ -20,6 +20,8 @@ cudaError_t dev_alloc(T** p, size_t count) {
 
 Pose2 pose_from_array(const double* d) { return Pose2{d[0], d[1], d[2], d[3]}; }
 
+}  // namespace
+
 MotionSampling to_kernel_sampling(const bb200_motion_sampling& s) {
   MotionSampling m{};
   m.model = s.model;
@@ -31,8 +33,6 @@ MotionSampling to_kernel_sampling(const bb200_motion_sampling& s) {
   m.first_s = s.first_rotation[1];
   return m;
 }
-
-}  // namespace
 
 bool normal_transform(const double cov[9], double transform[9], std::string* error) {
   // isApprox(transpose) of Eigen: ||C - C^T||_F^2 <= 1e-24 * ||C||_F^2
@@ -1510,7 +1510,8 @@ int Filter::ensure_cluster_scratch(uint32_t cells) {
   return BB200_OK;
 }
 
-int Filter::cell_records(double linear_resolution, double angular_resolution, std::vector<HostCell>* host) {
+int Filter::cell_records(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], double linear_resolution,
+                         double angular_resolution, std::vector<HostCell>* host) {
   // Per-particle half of the clusterizer, also the device-side histogram of the particle cloud: spatial hash ->
   // first-occurrence numbering of the occupied cells -> stable sort of the particle indices by cell -> one record per
   // cell (representative = first particle, count, weight summed in particle order, raw moments).
@@ -1520,7 +1521,7 @@ int Filter::cell_records(double linear_resolution, double angular_resolution, st
     if (st != BB200_OK) return st;
   }
   mark("cluster_cells");
-  launch_cluster_cells_begin(states_[cur_], n_, linear_resolution, angular_resolution, cluster_, stream_);
+  launch_cluster_cells_begin(states, n, linear_resolution, angular_resolution, cluster_, stream_);
   BB_LAUNCHED_N("cluster_cells_begin", 3);
   unsigned long long cells64 = 0;
   BB_CHECK(cudaMemcpyAsync(&cells64, cluster_.words + 1, sizeof(cells64), cudaMemcpyDeviceToHost, stream_));
@@ -1532,10 +1533,10 @@ int Filter::cell_records(double linear_resolution, double angular_resolution, st
   }
   mark("cluster_sort");
   int sort_launches = 0;
-  const uint32_t* sorted = launch_cluster_sort(n_, cells, cluster_, stream_, &sort_launches);
+  const uint32_t* sorted = launch_cluster_sort(n, cells, cluster_, stream_, &sort_launches);
   BB_LAUNCHED_N("cluster_sort", sort_launches);
   mark("cluster_records");
-  launch_cluster_records(states_[cur_], weights_, sorted, cells, pivot_[0], pivot_[1], cluster_, stream_);
+  launch_cluster_records(states, weights, sorted, cells, pivot[0], pivot[1], cluster_, stream_);
   BB_LAUNCHED("cluster_records");
   host->resize(cells);
   static_assert(sizeof(HostCell) == sizeof(CellRecord), "record layouts must agree");
@@ -1547,25 +1548,31 @@ int Filter::cell_records(double linear_resolution, double angular_resolution, st
 
 int Filter::cluster_estimate(const bb200_cluster_param& p, bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells,
                              uint32_t* n_clusters) {
-  if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
+  return cluster_estimate_of(states_[cur_], weights_, n_, pivot_, p, out, cluster_ids, ids_capacity, n_cells, n_clusters);
+}
+
+int Filter::cluster_estimate_of(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], const bb200_cluster_param& p,
+                                bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells, uint32_t* n_clusters) {
+  if (n == 0) return fail(BB200_ERR_STATE, "no particles");
+  if (n > capacity_) return fail(BB200_ERR_CAPACITY, "cluster estimate: more particles than the scratch holds");
   if (!(p.linear_hash_resolution > 0.0) || !(p.angular_hash_resolution > 0.0) || !(p.weight_cap_percentile >= 0.0) ||
       !(p.weight_cap_percentile < 1.0))
     return fail(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)");
-  if (cluster_ids != nullptr && ids_capacity < n_) return fail(BB200_ERR_CAPACITY, "cluster id buffer too small");
+  if (cluster_ids != nullptr && ids_capacity < n) return fail(BB200_ERR_CAPACITY, "cluster id buffer too small");
   std::vector<HostCell> host;
   {
-    const int st = cell_records(p.linear_hash_resolution, p.angular_hash_resolution, &host);
+    const int st = cell_records(states, weights, n, pivot, p.linear_hash_resolution, p.angular_hash_resolution, &host);
     if (st != BB200_OK) return st;
   }
   const uint32_t cells = static_cast<uint32_t>(host.size());
-  const ClusterSelection sel = select_cluster(host.data(), host.size(), n_, p.linear_hash_resolution, p.angular_hash_resolution, p.weight_cap_percentile);
-  if (out != nullptr) estimate_from_moments(sel.moments, out);
+  const ClusterSelection sel = select_cluster(host.data(), host.size(), n, p.linear_hash_resolution, p.angular_hash_resolution, p.weight_cap_percentile);
+  if (out != nullptr) estimate_from_moments_static(sel.moments, pivot, out);
   if (n_cells != nullptr) *n_cells = cells;
   if (n_clusters != nullptr) *n_clusters = sel.clusters;
   if (cluster_ids != nullptr) {
-    std::vector<uint32_t> cell_of(n_);
-    BB_CHECK(cudaMemcpy(cell_of.data(), cluster_.cell_of, n_ * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    for (uint64_t i = 0; i < n_; ++i) cluster_ids[i] = sel.cluster_of_cell[cell_of[i]];
+    std::vector<uint32_t> cell_of(n);
+    BB_CHECK(cudaMemcpy(cell_of.data(), cluster_.cell_of, n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    for (uint64_t i = 0; i < n; ++i) cluster_ids[i] = sel.cluster_of_cell[cell_of[i]];
   }
   return BB200_OK;
 }
@@ -1575,7 +1582,7 @@ int Filter::particle_histogram(double linear_resolution, double angular_resoluti
   if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
   if (!(linear_resolution > 0.0) || !(angular_resolution > 0.0)) return fail(BB200_ERR_INVALID_ARGUMENT, "histogram resolutions must be positive");
   std::vector<HostCell> host;
-  const int st = cell_records(linear_resolution, angular_resolution, &host);
+  const int st = cell_records(states_[cur_], weights_, n_, pivot_, linear_resolution, angular_resolution, &host);
   if (st != BB200_OK) return st;
   if (n_bins != nullptr) *n_bins = host.size();
   double top = 1e-3;  // beluga_ros/particle_cloud.hpp:197

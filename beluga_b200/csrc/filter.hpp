@@ -52,6 +52,10 @@ class Filter {
   /// (optional, one per particle) is the parity hook for ParticleClusterizer::operator() (:304-316).
   int cluster_estimate(const bb200_cluster_param& p, bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells,
                        uint32_t* n_clusters);
+  /// The same over n particles held outside this filter (a batch member's slice, on this filter's device), the moments
+  /// taken about `pivot`.  n must not exceed the capacity.
+  int cluster_estimate_of(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], const bb200_cluster_param& p,
+                          bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells, uint32_t* n_clusters);
   /// Device-side histogram of the particle cloud over spatial-hash buckets (beluga_ros/particle_cloud.hpp:197-210): one
   /// record per occupied bucket in first-occurrence order.  bins may be null (count only).
   int particle_histogram(double linear_resolution, double angular_resolution, bb200_cluster_cell* bins, uint64_t capacity, uint64_t* n_bins,
@@ -144,6 +148,20 @@ class Filter {
   void record_error(const std::string& message) const { error_ = message; }  // the C-ABI exception guard
   int fail_with(int status, const std::string& message) { return fail(status, message); }
   bool ok() const { return created_; }
+
+  /// What a batch of filters (csrc/batch.hpp) takes from the filter that holds its map.
+  struct MapView {
+    int sensor;  // -1: no map yet
+    FieldView field;
+    const uint32_t* free_cells;
+    uint64_t n_free;
+    int grid_width, grid_height;
+    double grid_resolution;
+    Pose2 grid_origin;
+  };
+  MapView map_view() const { return MapView{sensor_, field_, free_cells_, n_free_, grid_width_, grid_height_, grid_resolution_, grid_origin_}; }
+  cudaStream_t stream() const { return stream_; }
+  int device() const { return config_.device; }
   int create_status() const { return create_status_; }
 
  private:
@@ -225,7 +243,8 @@ class Filter {
 
   // clusterizer scratch (allocated on first use)
   int ensure_cluster_scratch(uint32_t cells);
-  int cell_records(double linear_resolution, double angular_resolution, std::vector<HostCell>* host);
+  int cell_records(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], double linear_resolution,
+                   double angular_resolution, std::vector<HostCell>* host);
   ClusterScratch cluster_{};
 
   // KLD scratch
@@ -293,6 +312,9 @@ class Filter {
   std::vector<std::pair<const char*, float>> timings_;
   uint64_t launches_{0};
 };
+
+/// bb200_motion_sampling -> the kernels' MotionSampling.
+MotionSampling to_kernel_sampling(const bb200_motion_sampling& s);
 
 /// Symmetric 3x3 covariance -> V * sqrt(Lambda) (multivariate_normal_distribution.hpp:109-126).
 /// Returns false with a message for non-symmetric / negative-eigenvalue input.

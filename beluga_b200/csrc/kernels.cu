@@ -463,17 +463,17 @@ __device__ __forceinline__ void publish_weight_max(unsigned long long bits, unsi
   }
 }
 
-__global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
-    reweight_lfm_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, const uint32_t* __restrict__ perm,
-                        FieldView field, const double2* __restrict__ points, uint32_t n_points, double points_radius,
-                        Scalars* __restrict__ scalars) {
+/// One CTA of the general likelihood-field reweight: the particles in schedule slots [slot_base, slot_base + kRwThreads).
+__device__ __forceinline__ void reweight_lfm_block(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n,
+                                                   const uint32_t* __restrict__ perm, const FieldView& field, const double2* __restrict__ points,
+                                                   uint32_t n_points, double points_radius, Scalars* __restrict__ scalars, uint64_t slot_base) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double2* s_pts = reinterpret_cast<double2*>(smem_raw);
   __shared__ __align__(8) uint64_t s_bar;
   __shared__ unsigned long long s_max;
   __shared__ unsigned int s_arrived;
 
-  const uint64_t slot = static_cast<uint64_t>(blockIdx.x) * kRwThreads + threadIdx.x;
+  const uint64_t slot = slot_base + threadIdx.x;
   const bool active = slot < n;
   const uint64_t i = active ? (perm != nullptr ? perm[slot] : slot) : 0;
 
@@ -519,6 +519,13 @@ __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
     weights[i] = w;
   }
   publish_weight_max(active ? weight_order_bits(w) : 0ull, &s_max, &s_arrived, kRwThreads / kWarp, scalars);
+}
+
+__global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
+    reweight_lfm_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, const uint32_t* __restrict__ perm,
+                        FieldView field, const double2* __restrict__ points, uint32_t n_points, double points_radius,
+                        Scalars* __restrict__ scalars) {
+  reweight_lfm_block(states, weights, n, perm, field, points, n_points, points_radius, scalars, static_cast<uint64_t>(blockIdx.x) * kRwThreads);
 }
 
 // ---- reweight, fixed-point cell lookup ----------------------------------------------------------------
@@ -719,18 +726,18 @@ __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
   }
 }
 
-/// Scan staged in shared memory by TMA (scans longer than kParamBeams points): one CTA per kRwThreads particles.
-__global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
-    reweight_lfm_fixed_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, const uint32_t* __restrict__ perm,
-                              FieldView field, const double2* __restrict__ points, uint32_t n_points, double points_radius,
-                              Scalars* __restrict__ scalars) {
+/// Scan staged in shared memory by TMA (scans longer than kParamBeams points): one CTA per kRwThreads particles, the
+/// schedule slots [slot_base, slot_base + kRwThreads).
+__device__ __forceinline__ void reweight_lfm_fixed_block(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n,
+                                                         const uint32_t* __restrict__ perm, const FieldView& field, const double2* __restrict__ points,
+                                                         uint32_t n_points, double points_radius, Scalars* __restrict__ scalars, uint64_t slot_base) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double2* s_pts = reinterpret_cast<double2*>(smem_raw);
   __shared__ __align__(8) uint64_t s_bar;
   __shared__ unsigned long long s_max;
   __shared__ unsigned int s_arrived;
 
-  const uint64_t slot = static_cast<uint64_t>(blockIdx.x) * kRwThreads + threadIdx.x;
+  const uint64_t slot = slot_base + threadIdx.x;
   const bool active = slot < n;
   const uint64_t i = active ? (perm != nullptr ? perm[slot] : slot) : 0;
   if (threadIdx.x == 0) {
@@ -769,6 +776,13 @@ __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
   publish_weight_max(active ? weight_order_bits(w) : 0ull, &s_max, &s_arrived, kRwThreads / kWarp, scalars);
 }
 #undef BB200_FIXED_SUM
+
+__global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
+    reweight_lfm_fixed_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, const uint32_t* __restrict__ perm,
+                              FieldView field, const double2* __restrict__ points, uint32_t n_points, double points_radius,
+                              Scalars* __restrict__ scalars) {
+  reweight_lfm_fixed_block(states, weights, n, perm, field, points, n_points, points_radius, scalars, static_cast<uint64_t>(blockIdx.x) * kRwThreads);
+}
 
 // ---- reweight (beam model; a4 + a5) -----------------------------------------------------------
 // BeamSensorModel (sensor/beam_model.hpp:104-150): one thread per particle, beams in the inner
@@ -1291,14 +1305,12 @@ __device__ __forceinline__ unsigned long long quantize_mul(double w, double f1, 
 
 /// derive_exponent: the fused step -- the exponent comes from scalars->wmax_bits here (no prepare_cdf launch; the
 /// tile holding element 0 publishes exponent / valid for the host); otherwise scalars->exponent / valid are given.
-__global__ void __launch_bounds__(kQsThreads) quantize_scan_kernel(const double* __restrict__ weights, uint64_t n,
-                                                                   unsigned long long* __restrict__ cdf, Scalars* scalars,
-                                                                   unsigned long long* tile_state, int derive_exponent, int ceil_log2_count) {
+/// One tile of the CDF build; `tile` counts from the set's first weight.
+__device__ __forceinline__ void quantize_scan_tile(const double* __restrict__ weights, uint64_t n, unsigned long long* __restrict__ cdf,
+                                                   Scalars* scalars, unsigned long long* tile_state, uint32_t tile, int derive_exponent,
+                                                   int ceil_log2_count) {
   __shared__ unsigned long long s_warp[kQsThreads / kWarp];
   __shared__ unsigned long long s_prefix;
-  // Tiles are taken in blockIdx order (CTAs are dispatched in that order, which is what the look-back's forward progress
-  // needs -- the same assumption CUB's decoupled look-back makes): no ticket atomic and no barrier before the loads.
-  const uint32_t tile = blockIdx.x;
   int exponent, valid_flag;
   if (derive_exponent) {  // every thread derives the exponent itself: a broadcast load and a few integer operations
     const double wmax = __longlong_as_double(static_cast<long long>(scalars->wmax_bits));
@@ -1364,6 +1376,14 @@ __global__ void __launch_bounds__(kQsThreads) quantize_scan_kernel(const double*
     }
   }
   if (base <= n - 1 && n - 1 < base + kQsItems) scalars->total = prefix + inclusive;  // thread holding the last element
+}
+
+__global__ void __launch_bounds__(kQsThreads) quantize_scan_kernel(const double* __restrict__ weights, uint64_t n,
+                                                                   unsigned long long* __restrict__ cdf, Scalars* scalars,
+                                                                   unsigned long long* tile_state, int derive_exponent, int ceil_log2_count) {
+  // Tiles are taken in blockIdx order (CTAs are dispatched in that order, which is what the look-back's forward progress
+  // needs -- the same assumption CUB's decoupled look-back makes): no ticket atomic and no barrier before the loads.
+  quantize_scan_tile(weights, n, cdf, scalars, tile_state, blockIdx.x, derive_exponent, ceil_log2_count);
 }
 
 /// Exclusive prefix sum of u32 values (bin counters, KLD first-occurrence flags) with the same
@@ -1544,15 +1564,38 @@ __device__ __forceinline__ void store_block_moments(double* m, double* scratch /
 /// arrival order) -- the reduce_partials launch and the read-back copies of the fused step folded into the resample.
 /// With tail.summary set (single GPU: pinned host memory, written straight over PCIe) the host finds the step's
 /// results after its one stream synchronisation.
-template <int kThreads>
+/// What the last block of a single filter's resample does with the summed moments (thread 0).
+__device__ __forceinline__ bool tail_enabled(const StepTail& tail) { return tail.enabled != 0; }
+__device__ __forceinline__ void tail_publish(const StepTail& tail, const double* v, Scalars* scalars) {
+#pragma unroll
+  for (int k = 0; k < kMomentCount; ++k) {
+    tail.results[k] = v[k];
+    if (tail.summary != nullptr) tail.summary->moments[k] = v[k];
+  }
+  scalars->blocks_done = 0;
+  if (tail.summary != nullptr) {
+    tail.summary->total = scalars->total;
+    tail.summary->exponent = scalars->exponent;
+    tail.summary->valid = scalars->valid;
+    tail.summary->error = 0;
+    __threadfence_system();
+    if (tail.seq != 0) {  // the host polls this word instead of synchronising with the stream
+      *reinterpret_cast<volatile int*>(&tail.summary->seq) = tail.seq;
+      __threadfence_system();
+    }
+  }
+}
+
+/// `block` of `grid` blocks that produce one particle set's moments (a batch member's blocks are a slice of the launch).
+template <int kThreads, class Tail>
 __device__ __forceinline__ void finish_block_moments(double* m, double* scratch, double* __restrict__ moment_partials, Scalars* scalars,
-                                                     const StepTail& tail) {
-  store_block_moments<kThreads>(m, scratch, moment_partials + static_cast<size_t>(blockIdx.x) * kMomentCount);
-  if (!tail.enabled) return;
+                                                     uint32_t block, uint32_t grid, const Tail& tail) {
+  store_block_moments<kThreads>(m, scratch, moment_partials + static_cast<size_t>(block) * kMomentCount);
+  if (!tail_enabled(tail)) return;
   __shared__ int s_last;
   if (threadIdx.x == 0) {
     __threadfence();  // the row above before the arrival count
-    s_last = atomicAdd(&scalars->blocks_done, 1u) + 1u == gridDim.x ? 1 : 0;
+    s_last = atomicAdd(&scalars->blocks_done, 1u) + 1u == grid ? 1 : 0;
   }
   __syncthreads();
   if (!s_last) return;
@@ -1560,36 +1603,19 @@ __device__ __forceinline__ void finish_block_moments(double* m, double* scratch,
   double v[kMomentCount];
 #pragma unroll
   for (int k = 0; k < kMomentCount; ++k) v[k] = 0.0;
-  for (uint32_t r = threadIdx.x; r < gridDim.x; r += kThreads) {
+  for (uint32_t r = threadIdx.x; r < grid; r += kThreads) {
     const double* row = moment_partials + static_cast<size_t>(r) * kMomentCount;
 #pragma unroll
     for (int k = 0; k < kMomentCount; ++k) v[k] = v[k] + __ldcg(row + k);  // nine independent loads per row
   }
   block_sum_many<kThreads, kMomentCount>(v, scratch);
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int k = 0; k < kMomentCount; ++k) {
-      tail.results[k] = v[k];
-      if (tail.summary != nullptr) tail.summary->moments[k] = v[k];
-    }
-  }
-  if (threadIdx.x == 0) {
-    scalars->blocks_done = 0;
-    if (tail.summary != nullptr) {
-      tail.summary->total = scalars->total;
-      tail.summary->exponent = scalars->exponent;
-      tail.summary->valid = scalars->valid;
-      tail.summary->error = 0;
-      __threadfence_system();
-      if (tail.seq != 0) {  // the host polls this word instead of synchronising with the stream
-        *reinterpret_cast<volatile int*>(&tail.summary->seq) = tail.seq;
-        __threadfence_system();
-      }
-    }
-  }
+  if (threadIdx.x == 0) tail_publish(tail, v, scalars);
 }
 
-__global__ void __launch_bounds__(kRsThreads) resample_kernel(ResampleArgs a, Scalars* __restrict__ scalars, double* __restrict__ moment_partials) {
+/// Block `block` of `grid` of the per-slot resample (resample_kernel).
+template <class Tail>
+__device__ __forceinline__ void resample_block(const ResampleArgs& a, Scalars* __restrict__ scalars, double* __restrict__ moment_partials,
+                                               uint32_t block, uint32_t grid, const Tail& tail) {
   __shared__ double s_red[kMomentCount * kRsThreads / kWarp];
   unsigned long long total = a.global_total != 0 ? a.global_total : scalars->total;
   unsigned long long cdf_offset = a.cdf_offset, span_end = 0;
@@ -1631,8 +1657,8 @@ __global__ void __launch_bounds__(kRsThreads) resample_kernel(ResampleArgs a, Sc
 #pragma unroll
   for (int k = 0; k < kMomentCount; ++k) m[k] = 0.0;
 
-  for (uint64_t local = static_cast<uint64_t>(blockIdx.x) * kRsThreads + threadIdx.x; local < slot_count;
-       local += static_cast<uint64_t>(gridDim.x) * kRsThreads) {
+  for (uint64_t local = static_cast<uint64_t>(block) * kRsThreads + threadIdx.x; local < slot_count;
+       local += static_cast<uint64_t>(grid) * kRsThreads) {
     const uint64_t j = slot_first + local;
     Pose2 st;
     long long ancestor = -1;
@@ -1677,7 +1703,11 @@ __global__ void __launch_bounds__(kRsThreads) resample_kernel(ResampleArgs a, Sc
     if (a.hashes != nullptr) a.hashes[local] = spatial_hash(st, a.hash_resolution[0], a.hash_resolution[1], a.hash_resolution[2]);
     accumulate_moments(m, st, 1.0, a.pivot_x, a.pivot_y);
   }
-  finish_block_moments<kRsThreads>(m, s_red, moment_partials, scalars, a.tail);
+  finish_block_moments<kRsThreads>(m, s_red, moment_partials, scalars, block, grid, tail);
+}
+
+__global__ void __launch_bounds__(kRsThreads) resample_kernel(ResampleArgs a, Scalars* __restrict__ scalars, double* __restrict__ moment_partials) {
+  resample_block(a, scalars, moment_partials, blockIdx.x, gridDim.x, a.tail);
 }
 
 // ---- resample, scatter form (systematic comb on one GPU) ----------------------------------------------
@@ -1706,8 +1736,10 @@ __device__ __forceinline__ uint64_t comb_slots_before_magic(unsigned long long p
   return j < total_slots ? j : total_slots;
 }
 
-__global__ void __launch_bounds__(kRsThreads, kRsBlocksPerSm) resample_scatter_kernel(ResampleArgs a, Scalars* __restrict__ scalars,
-                                                                     double* __restrict__ moment_partials) {
+/// Block `block` of `grid` of the scatter-form resample (resample_scatter_kernel).
+template <class Tail>
+__device__ __forceinline__ void resample_scatter_block(const ResampleArgs& a, Scalars* __restrict__ scalars, double* __restrict__ moment_partials,
+                                                       uint32_t block, uint32_t grid, const Tail& tail) {
   __shared__ double s_red[kMomentCount * kRsThreads / kWarp];
   __shared__ unsigned long long s_comb[3];
   // One GPU: the local CDF is the global one.  Sharded (rank_totals set): positions shift by the totals of
@@ -1751,10 +1783,10 @@ __global__ void __launch_bounds__(kRsThreads, kRsBlocksPerSm) resample_scatter_k
   // several 32-byte gathers in flight (the kernel is bound by the latency of cdf -> state -> store, not by bandwidth).
   // Every thread runs the same number of rounds: whole warps stay together for the cooperative stores.
   constexpr uint64_t kOwnCopies = 4;  // up to this many copies a thread stores itself
-  const uint64_t per_round = static_cast<uint64_t>(gridDim.x) * kRsThreads * kRsUnroll;
+  const uint64_t per_round = static_cast<uint64_t>(grid) * kRsThreads * kRsUnroll;
   const uint64_t rounds = (a.n_in + per_round - 1) / per_round;
   for (uint64_t round = 0; round < rounds; ++round) {
-    const uint64_t first = round * per_round + static_cast<uint64_t>(blockIdx.x) * kRsThreads * kRsUnroll + threadIdx.x;
+    const uint64_t first = round * per_round + static_cast<uint64_t>(block) * kRsThreads * kRsUnroll + threadIdx.x;
     uint64_t ja[kRsUnroll], copies[kRsUnroll];
 #pragma unroll
     for (int u = 0; u < kRsUnroll; ++u) {
@@ -1809,7 +1841,12 @@ __global__ void __launch_bounds__(kRsThreads, kRsBlocksPerSm) resample_scatter_k
       }
     }
   }
-  finish_block_moments<kRsThreads>(m, s_red, moment_partials, scalars, a.tail);
+  finish_block_moments<kRsThreads>(m, s_red, moment_partials, scalars, block, grid, tail);
+}
+
+__global__ void __launch_bounds__(kRsThreads, kRsBlocksPerSm) resample_scatter_kernel(ResampleArgs a, Scalars* __restrict__ scalars,
+                                                                     double* __restrict__ moment_partials) {
+  resample_scatter_block(a, scalars, moment_partials, blockIdx.x, gridDim.x, a.tail);
 }
 
 // ---- moments / reductions -------------------------------------------------------------------------
@@ -1838,6 +1875,172 @@ __global__ void __launch_bounds__(256) reduce_partials_kernel(const double* __re
 
 __global__ void __launch_bounds__(256) fill_kernel(double* __restrict__ out, uint64_t n, double value) {
   for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * 256 + threadIdx.x; i < n; i += static_cast<uint64_t>(gridDim.x) * 256) out[i] = value;
+}
+
+// ---- batches of filters ----------------------------------------------------------------------------------
+// Each kernel below runs, per CTA, the block body of the single-filter kernel it stands for, on the CTA's member.
+
+/// The member owning CTA `cta` of `launch` (the last one whose range starts at or before it: members without CTAs in this
+/// launch have empty ranges), the CTA's index inside that range and the range's length.
+__device__ __forceinline__ uint32_t batch_member_of(const BatchStepArgs& s, int launch, uint32_t cta, uint32_t& local, uint32_t& count) {
+  const uint32_t* first = s.first + static_cast<size_t>(launch) * (s.n_members + 1);
+  uint32_t lo = 0, hi = s.n_members;  // first[lo] <= cta < first[hi]
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (__ldg(first + mid) <= cta) {
+      lo = mid;
+    } else {
+      hi = mid;
+    }
+  }
+  const uint32_t begin = __ldg(first + lo);
+  local = cta - begin;
+  count = __ldg(first + lo + 1) - begin;
+  return lo;
+}
+
+/// A member's current (which = 0) or staging (which = 1) state buffer; a select, not an indexed load from the parameters.
+__device__ __forceinline__ Pose2* batch_states(const BatchStepArgs& s, const BatchMember& m, int which) {
+  return ((m.cur ^ which) != 0 ? s.states[1] : s.states[0]) + m.offset;
+}
+
+/// The per-step scalars of every member (what begin_fused_step_kernel resets for one filter) and the scan state.
+__global__ void __launch_bounds__(256) batch_begin_kernel(BatchStepArgs s) {
+  const uint32_t stride = gridDim.x * 256;
+  for (uint32_t t = blockIdx.x * 256 + threadIdx.x; t < s.n_members; t += stride) {
+    Scalars* sc = s.scalars + t;
+    sc->wmax_bits = 0;
+    sc->tile_ticket = 0;
+    sc->total = 0;
+    sc->exponent = 0;
+    sc->valid = 0;
+    sc->blocks_done = 0;
+  }
+  for (uint32_t t = blockIdx.x * 256 + threadIdx.x; t < s.ctas[kBatchScan]; t += stride) s.tile_state[t] = 0;
+}
+
+/// propagate_kernel's per-particle body (counter RNG keyed by the member's seed, local index and step).
+__global__ void __launch_bounds__(kPrThreads) batch_propagate_kernel(BatchStepArgs s) {
+  uint32_t local, count;
+  const BatchMember& m = s.members[batch_member_of(s, kBatchPropagate, blockIdx.x, local, count)];
+  const uint64_t i = static_cast<uint64_t>(local) * kPrThreads + threadIdx.x;
+  if (i < m.n) {
+    Pose2* states = batch_states(s, m, 0);
+    store_pose(states + i, propagate_one(load_pose(states + i), m.sampling, m.seed, i, m.step));
+  }
+}
+
+/// One CTA of reweight_lfm_fixed_kernel (or, for maps beyond kFixedMaxSide, reweight_lfm_kernel) per 256 particles of a
+/// member; each member's scan is staged into shared memory in kChunkBeams-point chunks.
+__global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm) batch_reweight_kernel(BatchStepArgs s) {
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kBatchReweight, blockIdx.x, local, count);
+  const BatchMember& m = s.members[k];
+  const Pose2* states = batch_states(s, m, 0);
+  const double2* points = reinterpret_cast<const double2*>(s.points) + m.point_offset;
+  const uint64_t slot_base = static_cast<uint64_t>(local) * kRwThreads;
+  if (s.field.use_fixed) {
+    reweight_lfm_fixed_block(states, s.weights + m.offset, m.n, nullptr, s.field, points, m.n_points, m.points_radius, s.scalars + k, slot_base);
+  } else {
+    reweight_lfm_block(states, s.weights + m.offset, m.n, nullptr, s.field, points, m.n_points, m.points_radius, s.scalars + k, slot_base);
+  }
+}
+
+/// quantize_scan_kernel per member: the exponent from the member's own largest weight, its own look-back state.
+__global__ void __launch_bounds__(kQsThreads) batch_scan_kernel(BatchStepArgs s) {
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kBatchScan, blockIdx.x, local, count);
+  const BatchMember& m = s.members[k];
+  quantize_scan_tile(s.weights + m.offset, m.n, s.cdf + m.offset, s.scalars + k, s.tile_state + (blockIdx.x - local), local, 1,
+                     m.ceil_log2_count);
+}
+
+/// The end of a member's step: its summary block, then -- from the last member to get there -- the step's ticket.
+struct BatchTail {
+  StepSummary* summary;
+  unsigned int* members_done;
+  uint32_t n_members;
+  int* ticket;
+  int seq;
+};
+__device__ __forceinline__ bool tail_enabled(const BatchTail&) { return true; }
+__device__ __forceinline__ void tail_publish(const BatchTail& tail, const double* v, Scalars* scalars) {
+#pragma unroll
+  for (int k = 0; k < kMomentCount; ++k) tail.summary->moments[k] = v[k];
+  scalars->blocks_done = 0;
+  tail.summary->total = scalars->total;
+  tail.summary->exponent = scalars->exponent;
+  tail.summary->valid = scalars->valid;
+  tail.summary->error = 0;
+  __threadfence_system();  // this member's summary before its arrival
+  if (atomicAdd(tail.members_done, 1u) + 1u == tail.n_members) {
+    __threadfence_system();  // every member's summary (each fenced before its arrival) before the ticket
+    *tail.members_done = 0;
+    *reinterpret_cast<volatile int*>(tail.ticket) = tail.seq;  // the host polls this word
+    __threadfence_system();
+  }
+}
+
+/// A step that keeps its particles: normalize_kernel's w /= S and moments_kernel's rows over the same partition
+/// (moments_block_count blocks), the rows summed like reduce_partials_kernel does.
+__device__ __forceinline__ void normalize_moments_block(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, double px,
+                                                        double py, Scalars* scalars, double* __restrict__ moment_partials, uint32_t block,
+                                                        uint32_t grid, const BatchTail& tail) {
+  __shared__ double s_red[kMomentCount * kStreamThreads / kWarp];
+  const double factor = scalbn(static_cast<double>(scalars->total), -scalars->exponent);
+  const bool valid = scalars->valid != 0 && factor > 0.0;
+  double m[kMomentCount];
+#pragma unroll
+  for (int k = 0; k < kMomentCount; ++k) m[k] = 0.0;
+  for (uint64_t i = static_cast<uint64_t>(block) * kStreamThreads + threadIdx.x; i < n; i += static_cast<uint64_t>(grid) * kStreamThreads) {
+    double w = weights[i];
+    if (valid) {
+      w = w / factor;  // actions/normalize.hpp:82
+      weights[i] = w;
+    }
+    accumulate_moments(m, load_pose(states + i), w, px, py);
+  }
+  finish_block_moments<kStreamThreads>(m, s_red, moment_partials, scalars, block, grid, tail);
+}
+
+/// Per member: resample_scatter_kernel or resample_kernel (recovery injection, multinomial draws) on a resampling step,
+/// normalisation otherwise; then the member's moments, summed by its last CTA.
+__global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs s) {
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kBatchFinish, blockIdx.x, local, count);
+  const BatchMember& m = s.members[k];
+  Scalars* scalars = s.scalars + k;
+  double* partials = s.partials + static_cast<size_t>(blockIdx.x - local) * kMomentCount;
+  const BatchTail tail{s.summary + k, s.members_done, s.n_members, s.ticket, s.seq};
+  if (!m.resample) {
+    normalize_moments_block(batch_states(s, m, 0), s.weights + m.offset, m.n, m.pivot_x, m.pivot_y, scalars, partials, local, count, tail);
+    return;
+  }
+  ResampleArgs a{};
+  a.states_in = batch_states(s, m, 0);
+  a.cdf = s.cdf + m.offset;
+  a.n_in = m.n;
+  a.states_out = batch_states(s, m, 1);
+  a.weights_out = s.weights + m.offset;
+  a.ancestors = s.ancestors != nullptr ? s.ancestors + m.offset : nullptr;
+  a.slot_count = m.slots;
+  a.total_slots = m.slots;
+  a.scheme = m.scheme;
+  a.seed = m.seed;
+  a.step = m.step;
+  a.random_state_probability = m.random_state_probability;
+  a.free_cells = s.free_cells;
+  a.n_free = s.n_free;
+  a.grid_width = s.grid_width;
+  a.grid_resolution = s.grid_resolution;
+  a.grid_origin = s.grid_origin;
+  a.pivot_x = m.pivot_x;
+  a.pivot_y = m.pivot_y;
+  if (m.scheme == 1 && m.random_state_probability <= 0.0) {  // systematic, nothing drawn per slot: launch_resample's scatter form
+    resample_scatter_block(a, scalars, partials, local, count, tail);
+  } else {
+    resample_block(a, scalars, partials, local, count, tail);
+  }
 }
 
 // ---- shard exchange ------------------------------------------------------------------------------------
@@ -2156,6 +2359,38 @@ uint32_t resample_block_count(uint64_t slots) {
   return static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>((slots + kRsThreads - 1) / kRsThreads, kSmCount * 16)));
 }
 
+uint32_t resample_scatter_block_count(uint64_t n_in) {
+  // one pass over the input particles; a few particles per thread amortise the block reduction of the moments
+  return static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>((n_in + kRsThreads - 1) / kRsThreads, kSmCount * kRsBlocksPerSm)));
+}
+
+uint32_t batch_scan_tiles(uint64_t n) { return scan_tile_count(n); }
+
+void batch_member_ctas(const BatchMember& m, uint32_t out[kBatchLaunches]) {
+  out[kBatchPropagate] = static_cast<uint32_t>((m.n + kPrThreads - 1) / kPrThreads);
+  out[kBatchReweight] = static_cast<uint32_t>((m.n + kRwThreads - 1) / kRwThreads);
+  out[kBatchScan] = scan_tile_count(m.n);
+  // the partition launch_resample / launch_moments would use for a single filter of this size
+  if (!m.resample) {
+    out[kBatchFinish] = moments_block_count(m.n);
+  } else if (m.scheme == 1 && m.random_state_probability <= 0.0) {
+    out[kBatchFinish] = resample_scatter_block_count(m.n);
+  } else {
+    out[kBatchFinish] = resample_block_count(m.slots);
+  }
+}
+
+int launch_batch_step(const BatchStepArgs& s, cudaStream_t stream) {
+  const uint32_t reset = std::max(s.n_members, s.ctas[kBatchScan]);
+  batch_begin_kernel<<<std::max(1u, std::min((reset + 255u) / 256u, kSmCount * 4u)), 256, 0, stream>>>(s);
+  batch_propagate_kernel<<<s.ctas[kBatchPropagate], kPrThreads, 0, stream>>>(s);
+  const size_t smem = static_cast<size_t>(std::min(s.max_points, kChunkBeams)) * sizeof(double2);
+  batch_reweight_kernel<<<s.ctas[kBatchReweight], kRwThreads, smem, stream>>>(s);
+  batch_scan_kernel<<<s.ctas[kBatchScan], kQsThreads, 0, stream>>>(s);
+  batch_finish_kernel<<<s.ctas[kBatchFinish], kRsThreads, 0, stream>>>(s);
+  return 5;
+}
+
 uint32_t launch_resample(const ResampleArgs& args, Scalars* scalars, double* moment_partials, cudaStream_t stream) {
   // The whole set on one GPU with the systematic comb and nothing per slot to draw: scatter form.
   // (Sharded with peer memory and device-side totals: the same, every copy stored into its owner's buffer.)
@@ -2165,8 +2400,7 @@ uint32_t launch_resample(const ResampleArgs& args, Scalars* scalars, double* mom
   const bool scatter = plain && ((args.peer_count == 0 && args.rank_totals == nullptr && args.slot_count == args.total_slots) ||
                                  (args.peer_count > 0 && args.rank_totals != nullptr));
   if (scatter) {
-    // one pass over the input particles; a few particles per thread amortise the block reduction of the moments
-    const uint32_t blocks = static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>((args.n_in + kRsThreads - 1) / kRsThreads, kSmCount * kRsBlocksPerSm)));
+    const uint32_t blocks = resample_scatter_block_count(args.n_in);
     resample_scatter_kernel<<<blocks, kRsThreads, 0, stream>>>(args, scalars, moment_partials);
     return blocks;
   }

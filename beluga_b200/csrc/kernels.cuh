@@ -343,6 +343,71 @@ uint32_t resample_block_count(uint64_t slots);
 /// blocks launched (= rows of moment_partials written).
 uint32_t launch_resample(const ResampleArgs& args, Scalars* scalars, double* moment_partials, cudaStream_t stream);
 
+/// Blocks of the scatter-form resample over n_in particles (launch_resample picks that form for a plain systematic comb).
+uint32_t resample_scatter_block_count(uint64_t n_in);
+
+// ---- batches: K independent filters stepped by one fixed sequence of launches ---------------------------------
+// The members' particles lie back to back in one set of buffers.  Every launch of a batch step gives each updating
+// member its own contiguous range of CTAs; a CTA finds its member by a binary search over the ranges' starts and then
+// runs the same block body the single-filter kernel runs, with its index inside the member's range as the block index
+// and the range's length as the grid.  Each member therefore sees the CTA partition -- and the moment partials, and so
+// the rounding -- of a single filter of its size.
+
+/// What one member does in a batch step (built on the host every step).
+struct BatchMember {
+  uint64_t offset;          // first particle of the member in the batch buffers
+  uint64_t n;               // particles before the step
+  uint64_t slots;           // max_particles: particles after a resample
+  uint64_t seed;
+  uint32_t step;
+  int resample;             // 1: resample (every_n fired); 0: normalise the weights and keep the particles
+  int scheme;               // bb200_resample_scheme
+  int cur;                  // state buffer holding the member's particles
+  int ceil_log2_count;      // of max_particles: the fixed-point exponent's headroom
+  int pad;
+  double random_state_probability;
+  double pivot_x, pivot_y;  // of the raw moments (the member's last estimate)
+  MotionSampling sampling;
+  uint64_t point_offset;    // first point of the member's scan in the batch's point buffer
+  uint32_t n_points;
+  double points_radius;     // largest |x| + |y| of the scan (NaN: some point is not finite)
+};
+
+/// Start of member m's CTA range in each launch: first[m] .. first[m + 1] (n_members + 1 entries per launch).
+enum BatchLaunch : int { kBatchPropagate = 0, kBatchReweight = 1, kBatchScan = 2, kBatchFinish = 3, kBatchLaunches = 4 };
+
+struct BatchStepArgs {
+  const BatchMember* members;     // device
+  const uint32_t* first;          // device: kBatchLaunches x (n_members + 1) CTA prefixes
+  uint32_t n_members;             // members that update in this step (the table lists only those)
+  uint32_t ctas[kBatchLaunches];  // total CTAs of each launch
+  uint32_t max_points;            // longest scan of the step (shared-memory staging of the reweight)
+  Pose2* states[2];
+  double* weights;
+  unsigned long long* cdf;
+  long long* ancestors;           // nullable
+  unsigned long long* tile_state; // one word per scan tile of the step
+  Scalars* scalars;               // one per member of the table
+  double* partials;               // kMomentCount per finish CTA
+  const double* points;           // (x, y) pairs
+  FieldView field;
+  const uint32_t* free_cells;
+  uint64_t n_free;
+  int grid_width;
+  double grid_resolution;
+  Pose2 grid_origin;
+  StepSummary* summary;           // one per member of the table (pinned host memory)
+  unsigned int* members_done;     // device word, zero between steps
+  int* ticket;                    // pinned: stores `seq` once every member's summary is complete
+  int seq;
+};
+/// Reset | propagate | reweight | quantise + scan | resample or normalise + moments.  Returns the number of launches.
+int launch_batch_step(const BatchStepArgs& args, cudaStream_t stream);
+/// Scan tiles of a member of n particles (the quantise-scan CTAs it needs).
+uint32_t batch_scan_tiles(uint64_t n);
+/// CTAs of a member in the launches of a batch step: propagate, reweight, scan, finish.
+void batch_member_ctas(const BatchMember& m, uint32_t out[kBatchLaunches]);
+
 /// Per-block raw weighted moments of (states, weights).
 uint32_t moments_block_count(uint64_t n);
 void launch_moments(const Pose2* states, const double* weights, uint64_t n, double pivot_x, double pivot_y, double* moment_partials,

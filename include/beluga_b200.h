@@ -544,6 +544,50 @@ int bb200_amcl_leave_shards(bb200_amcl* a);
 int bb200_filter_export_shard(bb200_filter* f, void* out256);
 int bb200_filter_join_shards(bb200_filter* f, int world, int rank, const void* handles);
 
+/* ---------------------------------------------------------------------------------------------
+ * Many independent filters on one GPU: a batch of K beluga::Amcl members that share one device, one
+ * likelihood-field map and one sensor model -- a fleet server localising many robots against one site
+ * map, a simulator with many agents.  bb200_amcl_batch_update steps every member that has a new scan
+ * with a fixed number of kernel launches and one host synchronisation, whatever K is; each member's
+ * result and particles are bit-identical to what a standalone bb200_amcl with the same parameters returns
+ * for the same inputs.
+ *
+ * Every member has its own parameter block (seed, policies, resampling scheme, recovery override) and
+ * motion model.  Members keep a fixed particle count: bb200_amcl_batch_create rejects, before touching a
+ * device, with BB200_ERR_INVALID_ARGUMENT: n_members < 1, min_particles != max_particles (KLD), selective
+ * resampling, non-zero shard fields, max_particles of 0 or above 32768, and members on different devices.
+ * Only the likelihood-field models are supported (no beam model).
+ * ------------------------------------------------------------------------------------------- */
+typedef struct bb200_amcl_batch bb200_amcl_batch;
+/* params[m] and motions[m] configure member m (params[m].device must be the same for all). */
+int bb200_amcl_batch_create(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bb200_amcl_batch** out);
+void bb200_amcl_batch_destroy(bb200_amcl_batch* b);
+const char* bb200_amcl_batch_last_error(const bb200_amcl_batch* b);
+int bb200_amcl_batch_members(const bb200_amcl_batch* b);
+/* One likelihood field (prob != 0: the prob model) for every member, built and uploaded once. */
+int bb200_amcl_batch_set_likelihood_field_map(bb200_amcl_batch* b, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid,
+                                              int prob);
+/* bb200_amcl_initialize / _initialize_from_map / _initialize_states / _force_update for member `member`. */
+int bb200_amcl_batch_initialize(bb200_amcl_batch* b, int member, const double mean_xytheta[3], const double cov[9]);
+int bb200_amcl_batch_initialize_from_map(bb200_amcl_batch* b, int member);
+int bb200_amcl_batch_initialize_states(bb200_amcl_batch* b, int member, const double* states, const double* weights, uint64_t n);
+int bb200_amcl_batch_force_update(bb200_amcl_batch* b, int member);
+/* Member m's particles (at most `capacity`; either output may be NULL). */
+int bb200_amcl_batch_get_particles(bb200_amcl_batch* b, int member, double* states, double* weights, uint64_t capacity);
+/* Resample indices of member m's last resample (params[m].record_ancestors must be set). */
+int bb200_amcl_batch_ancestors(bb200_amcl_batch* b, int member, int64_t* out, uint64_t capacity);
+/* beluga::cluster_based_estimate of member m's particles. */
+int bb200_amcl_batch_cluster_estimate(bb200_amcl_batch* b, int member, const bb200_cluster_param* p, bb200_estimate* out);
+/* Amcl::update for every member m with present[m] != 0 (present NULL: all members).  control_poses holds K poses of 4
+ * doubles, points_xy[m] member m's n_points[m] (x, y) pairs (NULL when n_points[m] == 0), out[m] its result.  An absent
+ * member is left untouched -- no policy is evaluated -- and gets out[m].updated = 0.  Present members go through their
+ * own on_motion / every_n / recovery-estimator logic exactly as in bb200_amcl_update.  The call is atomic: when it fails,
+ * every member's host state is as if it had not been made. */
+int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, const double* const* points_xy, const uint64_t* n_points,
+                            const uint8_t* present, bb200_update_result* out);
+/* Kernel launches issued by this batch so far. */
+uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b);
+
 /* The two host halves of bb200_amcl_update for callers that drive the filter themselves. */
 int bb200_amcl_plan_update(bb200_amcl* a, const double control_pose[4], bb200_step_plan* plan);
 void bb200_amcl_commit_update(bb200_amcl* a, int resampled, double random_state_probability);

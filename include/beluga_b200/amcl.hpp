@@ -44,6 +44,28 @@ struct AmclParams {
   int device = 0;
 };
 
+/// AmclParams as the C ABI's parameter block.
+inline bb200_amcl_param c_amcl_param(const AmclParams& params) {
+  bb200_amcl_param p{};
+  p.update_min_d = params.update_min_d;
+  p.update_min_a = params.update_min_a;
+  p.resample_interval = params.resample_interval;
+  p.selective_resampling = params.selective_resampling ? 1 : 0;
+  p.min_particles = params.min_particles;
+  p.max_particles = params.max_particles;
+  p.alpha_slow = params.alpha_slow;
+  p.alpha_fast = params.alpha_fast;
+  p.kld_epsilon = params.kld_epsilon;
+  p.kld_z = params.kld_z;
+  p.spatial_resolution[0] = params.spatial_resolution_x;
+  p.spatial_resolution[1] = params.spatial_resolution_y;
+  p.spatial_resolution[2] = params.spatial_resolution_theta;
+  p.resample_scheme = params.resample_scheme;
+  p.seed = params.seed;
+  p.device = params.device;
+  return p;
+}
+
 /// Particle set copy: the two vectors of beluga::TupleVector<std::tuple<SE2d, Weight>>.
 struct ParticleSet {
   std::vector<SE2d> states;
@@ -62,23 +84,7 @@ class Amcl {
 
   Amcl(MotionModel motion_model, SensorModel sensor_model, const AmclParams& params = AmclParams{}, ExecutionPolicy = ExecutionPolicy{})
       : params_{params}, motion_model_{std::move(motion_model)}, sensor_model_{std::move(sensor_model)} {
-    bb200_amcl_param p{};
-    p.update_min_d = params.update_min_d;
-    p.update_min_a = params.update_min_a;
-    p.resample_interval = params.resample_interval;
-    p.selective_resampling = params.selective_resampling ? 1 : 0;
-    p.min_particles = params.min_particles;
-    p.max_particles = params.max_particles;
-    p.alpha_slow = params.alpha_slow;
-    p.alpha_fast = params.alpha_fast;
-    p.kld_epsilon = params.kld_epsilon;
-    p.kld_z = params.kld_z;
-    p.spatial_resolution[0] = params.spatial_resolution_x;
-    p.spatial_resolution[1] = params.spatial_resolution_y;
-    p.spatial_resolution[2] = params.spatial_resolution_theta;
-    p.resample_scheme = params.resample_scheme;
-    p.seed = params.seed;
-    p.device = params.device;
+    const bb200_amcl_param p = c_amcl_param(params);
     const bb200_motion_param m = motion_model_.c_motion_param();
     const int st = bb200_amcl_create_with_motion(&p, &m, &handle_);
     if (st != BB200_OK) throw Error(st, bb200_create_error());
@@ -198,5 +204,102 @@ template <class MotionModel, class SensorModel, class ExecutionPolicy>
   for (int i = 0; i < 9; ++i) cov[i] = e.cov[i];
   return std::make_pair(SE2d::from_data(e.mean), cov);
 }
+
+/// K independent filters on one GPU that share one likelihood-field map (bb200_amcl_batch): update() steps every member
+/// with a new scan at once.  Member m behaves like an Amcl built from motions[m] and params[m]; members keep a fixed
+/// particle count (min_particles == max_particles <= 32768).  Results are returned per member, std::nullopt where the
+/// reference's update would return it or where the member had no scan this step.
+class AmclBatch {
+ public:
+  using estimation_type = std::pair<SE2d, Matrix3d>;
+
+  AmclBatch(const std::vector<bb200_motion_param>& motions, const std::vector<AmclParams>& params) {
+    if (motions.size() != params.size()) throw Error(BB200_ERR_INVALID_ARGUMENT, "one motion model per member");
+    std::vector<bb200_amcl_param> p;
+    for (const AmclParams& q : params) p.push_back(c_amcl_param(q));
+    const int st = bb200_amcl_batch_create(p.data(), motions.data(), static_cast<int>(p.size()), &handle_);
+    if (st != BB200_OK) throw Error(st, bb200_create_error());
+    sizes_.reserve(params.size());
+    for (const AmclParams& q : params) sizes_.push_back(q.max_particles);
+  }
+  ~AmclBatch() { bb200_amcl_batch_destroy(handle_); }
+  AmclBatch(const AmclBatch&) = delete;
+  AmclBatch& operator=(const AmclBatch&) = delete;
+
+  [[nodiscard]] std::size_t size() const { return sizes_.size(); }
+
+  /// One likelihood field for every member (prob: the LikelihoodFieldProb model).
+  void set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob = false) {
+    check(bb200_amcl_batch_set_likelihood_field_map(handle_, &p, &grid, prob ? 1 : 0));
+  }
+  void initialize(std::size_t member, const SE2d& pose, const Matrix3d& covariance) {
+    const double mean[3] = {pose.x(), pose.y(), pose.theta()};
+    check(bb200_amcl_batch_initialize(handle_, index(member), mean, covariance.data()));
+  }
+  void initialize_from_map(std::size_t member) { check(bb200_amcl_batch_initialize_from_map(handle_, index(member))); }
+  void force_update(std::size_t member) { check(bb200_amcl_batch_force_update(handle_, index(member))); }
+
+  /// controls[m] and points[m] are member m's odometry pose and scan points; present (optional) marks the members that
+  /// have a scan this step.
+  auto update(const std::vector<SE2d>& controls, const std::vector<std::vector<std::pair<double, double>>>& points,
+              const std::vector<bool>* present = nullptr) -> std::vector<std::optional<estimation_type>> {
+    const std::size_t k = size();
+    if (controls.size() != k || points.size() != k || (present != nullptr && present->size() != k))
+      throw Error(BB200_ERR_INVALID_ARGUMENT, "one control, one scan (and one presence flag) per member");
+    static_assert(sizeof(SE2d) == 4 * sizeof(double), "SE2d must be four packed doubles");
+    static_assert(sizeof(std::pair<double, double>) == 2 * sizeof(double), "measurement points must be packed");
+    std::vector<const double*> pts(k);
+    std::vector<std::uint64_t> counts(k);
+    std::vector<std::uint8_t> mask(present != nullptr ? k : 0);
+    for (std::size_t m = 0; m < k; ++m) {
+      pts[m] = points[m].empty() ? nullptr : &points[m].front().first;
+      counts[m] = points[m].size();
+      if (present != nullptr) mask[m] = (*present)[m] ? 1 : 0;
+    }
+    std::vector<bb200_update_result> r(k);
+    check(bb200_amcl_batch_update(handle_, controls.front().data(), pts.data(), counts.data(), present != nullptr ? mask.data() : nullptr, r.data()));
+    std::vector<std::optional<estimation_type>> out(k);
+    for (std::size_t m = 0; m < k; ++m) {
+      if (!r[m].updated) continue;
+      Matrix3d cov;
+      for (int i = 0; i < 9; ++i) cov[i] = r[m].estimate.cov[i];
+      out[m] = std::make_pair(SE2d::from_data(r[m].estimate.mean), cov);
+    }
+    return out;
+  }
+
+  /// Member m's particle set, copied from the device.
+  [[nodiscard]] ParticleSet particles(std::size_t member) const {
+    ParticleSet out;
+    out.states.resize(sizes_.at(member));
+    out.weights.resize(sizes_.at(member));
+    check(bb200_amcl_batch_get_particles(handle_, index(member), reinterpret_cast<double*>(out.states.data()), out.weights.data(), out.size()));
+    return out;
+  }
+
+  /// beluga::cluster_based_estimate of member m's particles.
+  [[nodiscard]] estimation_type cluster_based_estimate(std::size_t member, ParticleClusterizerParam parameters = {}) const {
+    const bb200_cluster_param p{parameters.linear_hash_resolution, parameters.angular_hash_resolution, parameters.weight_cap_percentile};
+    bb200_estimate e{};
+    check(bb200_amcl_batch_cluster_estimate(handle_, index(member), &p, &e));
+    Matrix3d cov;
+    for (int i = 0; i < 9; ++i) cov[i] = e.cov[i];
+    return std::make_pair(SE2d::from_data(e.mean), cov);
+  }
+
+  [[nodiscard]] bb200_amcl_batch* handle() const { return handle_; }
+
+ private:
+  int index(std::size_t member) const {
+    if (member >= size()) throw Error(BB200_ERR_INVALID_ARGUMENT, "member index out of range");
+    return static_cast<int>(member);
+  }
+  void check(int status) const {
+    if (status != BB200_OK) throw Error(status, bb200_amcl_batch_last_error(handle_));
+  }
+
+  bb200_amcl_batch* handle_{nullptr};
+  std::vector<std::size_t> sizes_;
+};
 
 }  // namespace beluga_b200

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Timings of the other BASELINE.json configurations (parity-test cases, not the bench.py line), and of point-cloud updates:
-`cloud`: 65 536-point lidar clouds at 10k and 1M particles.
+`cloud`: 65 536-point lidar clouds at 10k and 1M particles.  `batch`: K node-sized filters (2000 particles x 100 points) stepped as one
+AmclBatch against K standalone Amcl stepped one after another.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import json
@@ -84,6 +85,52 @@ def run_cloud():
     return res
 
 
+def run_batch():
+    """AmclBatch with K in {1, 16, 64, 256} members x 2000 particles x 100 points (the reference benchmark's max_beams) on the 2000^2
+    synthetic map, systematic resampling, every member updating every step; beside it, in the same process, K standalone Amcl
+    stepped one after another on the same inputs."""
+    res = {}
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=100, steps=100)
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    n, steps, warmup = 2000, 20, 3
+    device = device_record()
+    for k in (1, 16, 64, 256):
+        params = [bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m) for m in range(k)]
+        motions = [bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)]
+        batch = bb.AmclBatch(motions, params)
+        batch.set_likelihood_field_map(lfm, grid)
+        singles = []
+        for m in range(k):
+            batch.initialize(m, sc.initial_mean, sc.initial_cov)
+            a = bb.Amcl(motions[m], params[m])
+            a.update_map(bb.SENSOR_LIKELIHOOD_FIELD, lfm, grid)
+            a.initialize(sc.initial_mean, sc.initial_cov)
+            singles.append(a)
+        wall_batch, wall_single, launches = [], [], []
+        for t in range(warmup + steps):
+            pose = bb.se2(*sc.poses[t])
+            t0 = time.perf_counter()
+            before = batch.launch_count()
+            r = batch.update([pose] * k, [sc.scans[t]] * k)
+            t1 = time.perf_counter()
+            assert all(x.updated for x in r)
+            launches.append(batch.launch_count() - before)
+            for a in singles:
+                assert a.update(pose, sc.scans[t]).updated == 1
+            t2 = time.perf_counter()
+            if t >= warmup:
+                wall_batch.append((t1 - t0) * 1e3)
+                wall_single.append((t2 - t1) * 1e3)
+        mb, ms = float(np.median(wall_batch)), float(np.median(wall_single))
+        res[f"batch_{k}_x_2000_x_100_lfm_2000"] = {
+            "members": k, "particles": n, "points": 100, "steps": steps,
+            "ms_per_step_e2e": mb, "member_steps_per_s": k * 1e3 / mb, "launches_per_step": int(max(launches)),
+            "standalone_ms_per_round": ms, "standalone_member_steps_per_s": k * 1e3 / ms,
+            "kernels_ms": {}, "device": device}
+    return res
+
+
 def main():
     out = {}
     which = sys.argv[1:] or ["c1", "c3", "c4"]
@@ -137,6 +184,8 @@ def main():
                                                            spatial_resolution=(0.5, 0.5, float(np.deg2rad(10.0)))), steps=6, warmup=1)  # beluga_ros defaults (SURVEY 8d)
     if "cloud" in which:
         out.update(run_cloud())
+    if "batch" in which:
+        out.update(run_batch())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}

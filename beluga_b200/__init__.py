@@ -481,29 +481,6 @@ class Filter:
     def enqueue_moments(self, pivot):
         self._check(self._lib.bb200_filter_enqueue_moments(self._h, _dptr(_f64(pivot))))
 
-    def ipc_handles(self) -> bytes:
-        buf = C.create_string_buffer(128)
-        self._check(self._lib.bb200_filter_ipc_handles(self._h, buf))
-        return buf.raw
-
-    def open_peers(self, world: int, rank: int, handles: bytes):
-        buf = C.create_string_buffer(handles, len(handles))
-        self._check(self._lib.bb200_filter_open_peers(self._h, world, rank, buf))
-
-    def enqueue_resample_push_device(self, opts: _capi.ResampleOpts, rank_totals_ptr: int, rank: int, world: int, shard: int, pivot):
-        self._check(self._lib.bb200_filter_enqueue_resample_push_device(self._h, C.byref(opts), C.c_void_p(rank_totals_ptr), rank, world, shard,
-                                                                        _dptr(_f64(pivot))))
-
-    def enqueue_resample_push(self, opts: _capi.ResampleOpts, global_total: int, cdf_offset: int, slot_begin: int, slot_end: int, shard: int, pivot):
-        self._check(self._lib.bb200_filter_enqueue_resample_push(self._h, C.byref(opts), global_total, cdf_offset, slot_begin, slot_end, shard,
-                                                                 _dptr(_f64(pivot))))
-
-    def enqueue_reduce_moments(self):
-        self._check(self._lib.bb200_filter_enqueue_reduce_moments(self._h))
-
-    def enqueue_flip_adopt(self, n: int):
-        self._check(self._lib.bb200_filter_enqueue_flip_adopt(self._h, n))
-
     def ancestors(self) -> np.ndarray:
         out = np.zeros(self.size(), dtype=np.int64)
         self._check(self._lib.bb200_filter_ancestors(self._h, out.ctypes.data_as(C.POINTER(C.c_int64)), len(out)))

@@ -154,12 +154,6 @@ SIGNATURES = {
     "bb200_filter_enqueue_resample_range": (C.c_int, [_vp, _P(ResampleOpts), C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64]),
     "bb200_filter_enqueue_adopt": (C.c_int, [_vp, C.c_uint64]),
     "bb200_filter_enqueue_moments": (C.c_int, [_vp, _dbl]),
-    "bb200_filter_ipc_handles": (C.c_int, [_vp, _vp]),
-    "bb200_filter_open_peers": (C.c_int, [_vp, C.c_int, C.c_int, _vp]),
-    "bb200_filter_enqueue_resample_push_device": (C.c_int, [_vp, _P(ResampleOpts), C.c_void_p, C.c_int, C.c_int, C.c_uint64, _dbl]),
-    "bb200_filter_enqueue_resample_push": (C.c_int, [_vp, _P(ResampleOpts), C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, _dbl]),
-    "bb200_filter_enqueue_reduce_moments": (C.c_int, [_vp]),
-    "bb200_filter_enqueue_flip_adopt": (C.c_int, [_vp, C.c_uint64]),
     "bb200_filter_ancestors": (C.c_int, [_vp, _P(C.c_int64), C.c_uint64]),
     "bb200_filter_cdf": (C.c_int, [_vp, _P(C.c_uint64), C.c_uint64]),
     "bb200_filter_estimate": (C.c_int, [_vp, _P(Estimate)]),
@@ -209,8 +203,6 @@ SIGNATURES = {
     "bb200_amcl_export_shard": (C.c_int, [_vp, _vp]),
     "bb200_amcl_join_shards": (C.c_int, [_vp, C.c_int, C.c_int, _vp]),
     "bb200_amcl_leave_shards": (C.c_int, [_vp]),
-    "bb200_filter_export_shard": (C.c_int, [_vp, _vp]),
-    "bb200_filter_join_shards": (C.c_int, [_vp, C.c_int, C.c_int, _vp]),
     "bb200_amcl_batch_create": (C.c_int, [_P(AmclParam), _P(MotionParam), C.c_int, _P(_vp)]),
     "bb200_amcl_batch_destroy": (None, [_vp]),
     "bb200_amcl_batch_last_error": (C.c_char_p, [_vp]),

@@ -255,7 +255,7 @@ int bb200_filter_enqueue_propagate_reweight(bb200_filter* f, const bb200_motion_
 }
 int bb200_filter_enqueue_build_cdf(bb200_filter* f) {
   BB_REQUIRE(f);
-  return guarded(f->impl, [&] { return f->impl.enqueue_build_cdf(); });
+  return guarded(f->impl, [&] { return f->impl.enqueue_build_cdf(-1.0); });
 }
 int bb200_filter_enqueue_resample_range(bb200_filter* f, const bb200_resample_opts* o, uint64_t global_total, uint64_t cdf_offset, uint64_t slot_begin,
                                         uint64_t slot_end) {
@@ -269,32 +269,6 @@ int bb200_filter_enqueue_adopt(bb200_filter* f, uint64_t n) {
 int bb200_filter_enqueue_moments(bb200_filter* f, const double pivot_xy[2]) {
   BB_REQUIRE(f && pivot_xy);
   return guarded(f->impl, [&] { return f->impl.enqueue_moments(pivot_xy); });
-}
-int bb200_filter_ipc_handles(bb200_filter* f, void* out128) {
-  BB_REQUIRE(f && out128);
-  return guarded(f->impl, [&] { return f->impl.ipc_handles(out128); });
-}
-int bb200_filter_open_peers(bb200_filter* f, int world, int rank, const void* handles) {
-  BB_REQUIRE(f && handles);
-  return guarded(f->impl, [&] { return f->impl.open_peers(world, rank, handles); });
-}
-int bb200_filter_enqueue_resample_push(bb200_filter* f, const bb200_resample_opts* o, uint64_t global_total, uint64_t cdf_offset, uint64_t slot_begin,
-                                       uint64_t slot_end, uint64_t shard, const double pivot_xy[2]) {
-  BB_REQUIRE(f && o && pivot_xy && slot_end >= slot_begin && shard > 0);
-  return guarded(f->impl, [&] { return f->impl.enqueue_resample_push(*o, global_total, cdf_offset, slot_begin, slot_end, shard, pivot_xy); });
-}
-int bb200_filter_enqueue_resample_push_device(bb200_filter* f, const bb200_resample_opts* o, const uint64_t* rank_totals_device, int rank, int world,
-                                              uint64_t shard, const double pivot_xy[2]) {
-  BB_REQUIRE(f && o && rank_totals_device && pivot_xy && shard > 0);
-  return guarded(f->impl, [&] { return f->impl.enqueue_resample_push_device(*o, rank_totals_device, rank, world, shard, pivot_xy); });
-}
-int bb200_filter_enqueue_reduce_moments(bb200_filter* f) {
-  BB_REQUIRE(f);
-  return guarded(f->impl, [&] { return f->impl.enqueue_reduce_moments(); });
-}
-int bb200_filter_enqueue_flip_adopt(bb200_filter* f, uint64_t n) {
-  BB_REQUIRE(f);
-  return guarded(f->impl, [&] { return f->impl.enqueue_flip_adopt(n); });
 }
 int bb200_filter_ancestors(bb200_filter* f, int64_t* out, uint64_t capacity) {
   BB_REQUIRE(f && out);
@@ -620,14 +594,6 @@ int bb200_amcl_join_shards(bb200_amcl* a, int world, int rank, const void* handl
 int bb200_amcl_leave_shards(bb200_amcl* a) {
   BB_REQUIRE(a);
   return guarded(a->impl, [&] { return a->impl.filter().leave_shards(); });
-}
-int bb200_filter_export_shard(bb200_filter* f, void* out256) {
-  BB_REQUIRE(f && out256);
-  return guarded(f->impl, [&] { return f->impl.export_shard(out256); });
-}
-int bb200_filter_join_shards(bb200_filter* f, int world, int rank, const void* handles) {
-  BB_REQUIRE(f && handles);
-  return guarded(f->impl, [&] { return f->impl.join_shards_ipc(world, rank, handles); });
 }
 
 int bb200_sharded_amcl_create(const bb200_amcl_param* p, const bb200_motion_param* motion, int n_shards, const int* devices, bb200_sharded_amcl** out) {

@@ -281,29 +281,46 @@ int Filter::set_stream(void* stream) {
   return BB200_OK;
 }
 
+// ---- stream-ordered operations (the blocking ones further down add the synchronisation and read-back) ----------
+
 int Filter::enqueue_propagate_reweight(const bb200_motion_sampling* sampling, uint32_t step, const double* points_xy, uint64_t n_points) {
+  // points_xy == nullptr: propagate only.  The pinned point staging buffer is overwritten: the caller has synchronised
+  // since the previous upload.
   if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
-  if (points_xy == nullptr || sensor_ < 0) return fail(BB200_ERR_STATE, "no sensor model map set / no points");
-  if (n_points > 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, "too many points");
+  const bool do_reweight = points_xy != nullptr;
+  if (do_reweight && sensor_ < 0) return fail(BB200_ERR_STATE, "no sensor model map set");
+  if (do_reweight && n_points > 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, "too many points");
   BB_CHECK(cudaSetDevice(config_.device));
-  int st = upload_points(points_xy, n_points);  // the caller synchronised at the end of the previous step
-  if (st != BB200_OK) return st;
+  if (do_reweight) {
+    const int st = upload_points(points_xy, n_points);
+    if (st != BB200_OK) return st;
+  }
   MotionSampling s{};
   if (sampling != nullptr) s = to_kernel_sampling(*sampling);
   mark("begin_step");
   launch_begin_step(scalars_, stream_);
   BB_LAUNCHED("begin_step");
-  st = enqueue_propagate_reweight(sampling != nullptr ? &s : nullptr, step, true, n_points, false);
+  const int st = enqueue_propagate_reweight_kernels(sampling != nullptr ? &s : nullptr, step, do_reweight, n_points, false);
   cdf_valid_ = false;
   cloud_known_ = false;
   return st;
 }
 
-int Filter::enqueue_build_cdf() {
+int Filter::enqueue_max_weight() {
+  if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
+  BB_CHECK(cudaSetDevice(config_.device));
+  launch_begin_step(scalars_, stream_);
+  BB_LAUNCHED("begin_step");
+  launch_max_weight(weights_, n_, scalars_, stream_);
+  BB_LAUNCHED("max_weight");
+  return BB200_OK;
+}
+
+int Filter::enqueue_build_cdf(double global_wmax) {
   if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
   BB_CHECK(cudaSetDevice(config_.device));
   mark("prepare_cdf");
-  launch_prepare_cdf(scalars_, -1.0, config_.global_count, tile_state_, scan_tile_count(n_), stream_);
+  launch_prepare_cdf(scalars_, global_wmax, config_.global_count, tile_state_, scan_tile_count(n_), stream_);
   BB_LAUNCHED("prepare_cdf");
   mark("quantize_scan");
   launch_quantize_scan(weights_, n_, cdf_, scalars_, tile_state_, stream_);
@@ -313,18 +330,20 @@ int Filter::enqueue_build_cdf() {
 }
 
 int Filter::enqueue_resample_range(const bb200_resample_opts& o, uint64_t global_total, uint64_t cdf_offset, uint64_t slot_begin, uint64_t slot_end) {
+  // Sharded filter: this rank produces the output slots [slot_begin, slot_end) -- exactly those whose
+  // comb position falls inside its span of the global CDF -- into the staging buffer, in slot order.
   if (!cdf_valid_) return fail(BB200_ERR_STATE, "build_cdf must run before resample_range");
   if (o.scheme != BB200_RESAMPLE_SYSTEMATIC || o.min_particles < o.max_particles)
-    return fail(BB200_ERR_STATE, "range resampling supports the systematic comb without KLD (multinomial: bb200_filter_enqueue_resample_push)");
+    return fail(BB200_ERR_STATE, "range resampling supports the systematic comb without KLD (multinomial or KLD on shards: bb200_amcl_join_shards / bb200_sharded_amcl)");
   if (o.random_state_probability > 0.0 && n_free_ == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
   if (slot_end < slot_begin || slot_end - slot_begin > capacity_) return fail(BB200_ERR_CAPACITY, "slot range exceeds the staging buffer");
   BB_CHECK(cudaSetDevice(config_.device));
   if (slot_end > slot_begin) {
     ResampleArgs a = make_resample_args(o, 0, slot_end - slot_begin, false);
-    a.slot_first = slot_begin;
+    a.slot_first = slot_begin;  // global slot index
     a.global_total = global_total;
     a.cdf_offset = cdf_offset;
-    a.weights_out = nullptr;
+    a.weights_out = nullptr;  // the current weights stay untouched; adopt() writes the ones
     mark("resample_range");
     launch_resample(a, scalars_, partials_, stream_);
     BB_LAUNCHED("resample_range");
@@ -332,35 +351,34 @@ int Filter::enqueue_resample_range(const bb200_resample_opts& o, uint64_t global
   return BB200_OK;
 }
 
-int Filter::ipc_handles(void* out128) {
+int Filter::enqueue_adopt(uint64_t n) {
+  // The caller has placed n particle states into the current state buffer, e.g. through an all-to-all: make them
+  // the particle set with unit weights (make_from_state, particle_traits.hpp:105).
+  if (n > capacity_) return fail(BB200_ERR_CAPACITY, "more particles than the filter capacity");
   BB_CHECK(cudaSetDevice(config_.device));
-  static_assert(sizeof(cudaIpcMemHandle_t) == 64, "two IPC handles are exported as 128 bytes");
-  cudaIpcMemHandle_t h[2];
-  BB_CHECK(cudaIpcGetMemHandle(&h[0], states_[0]));
-  BB_CHECK(cudaIpcGetMemHandle(&h[1], states_[1]));
-  std::memcpy(out128, h, sizeof(h));
+  cloud_known_ = false;
+  n_ = n;
+  cdf_valid_ = false;
+  if (n > 0) {
+    mark("fill_weights");
+    launch_fill(weights_, n, 1.0, stream_);
+    BB_LAUNCHED("fill_weights");
+  }
   return BB200_OK;
 }
 
-int Filter::open_peers(int world, int rank, const void* handles) {
-  if (world < 1 || world > 8 || rank < 0 || rank >= world) return fail(BB200_ERR_INVALID_ARGUMENT, "peer groups hold 1..8 ranks");
+int Filter::enqueue_moments(const double pivot[2]) {
+  if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
   BB_CHECK(cudaSetDevice(config_.device));
-  if (peer_world_ != 0) return fail(BB200_ERR_STATE, "the peers' buffers are already mapped");
-  const auto* all = static_cast<const cudaIpcMemHandle_t*>(handles);
-  for (int r = 0; r < world; ++r) {
-    for (int b = 0; b < 2; ++b) {
-      if (r == rank) {
-        peer_states_[b][r] = states_[b];
-      } else {
-        void* p = nullptr;
-        BB_CHECK(cudaIpcOpenMemHandle(&p, all[2 * r + b], cudaIpcMemLazyEnablePeerAccess));
-        peer_states_[b][r] = static_cast<Pose2*>(p);
-      }
-    }
-  }
-  peer_world_ = world;
-  peer_rank_ = rank;
-  peers_ipc_ = true;
+  return enqueue_moment_kernels(pivot);
+}
+
+int Filter::enqueue_moment_kernels(const double pivot[2]) {
+  mark("moments");
+  launch_moments(states_[cur_], weights_, n_, pivot[0], pivot[1], partials_, stream_);
+  BB_LAUNCHED("moments");
+  launch_reduce_partials(partials_, moments_block_count(n_), kMomentCount, results_, stream_);
+  BB_LAUNCHED("reduce_partials");
   return BB200_OK;
 }
 
@@ -530,7 +548,6 @@ int Filter::step_begin(const bb200_motion_sampling& sampling, uint32_t step, con
   BB_CHECK(cudaSetDevice(config_.device));
   const int st = upload_points(points_xy, n_points);
   if (st != BB200_OK) return st;
-  if (world > 1 && peer_mail_[0] == nullptr) return fail(BB200_ERR_STATE, "shards joined without mail blocks (legacy open_peers): use join_shards");
   step_ = StepContext{};
   summary_host_->error = 0;
   step_.active = true;
@@ -559,7 +576,7 @@ int Filter::step_phase(int phase) {
         launch_begin_fused_step(scalars_, tile_state_, scan_tile_count(n_), sched_, scheduled ? counters_ : nullptr, schedule_max_bins(), sched_tiles_,
                                 schedule_tile_count(), warm ? bordered_ : nullptr, bordered_bytes_, stream_);
         BB_LAUNCHED("begin_step");
-        st = enqueue_propagate_reweight(&step_.sampling, step_.step, true, step_.n_points, scheduled);
+        st = enqueue_propagate_reweight_kernels(&step_.sampling, step_.step, true, step_.n_points, scheduled);
       }
       if (st != BB200_OK) return st;
       if (sharded) {
@@ -682,11 +699,8 @@ int Filter::step_phase(int phase) {
       mark("normalize");
       launch_normalize(weights_, n_, scalars_, sharded ? ~0ull : 0ull, partials_, &rows, stream_);  // actions/normalize.hpp:82
       BB_LAUNCHED("normalize");
-      mark("moments");
-      launch_moments(states_[cur_], weights_, n_, pivot_[0], pivot_[1], partials_, stream_);
-      BB_LAUNCHED("moments");
-      launch_reduce_partials(partials_, moments_block_count(n_), kMomentCount, results_, stream_);
-      BB_LAUNCHED("reduce_partials");
+      st = enqueue_moment_kernels(pivot_);  // a KLD-sized shard may be empty here
+      if (st != BB200_OK) return st;
       step_.normalized = true;
       if (sharded && split_posts_) {
         mark("exchange");
@@ -851,107 +865,6 @@ int Filter::step_end(bb200_estimate* est, double* weight_sum, uint64_t* new_size
   pivot_[1] = est->mean[3];
   cloud_ = *est;
   cloud_known_ = step_.resampled;  // unit weights: the estimate describes the raw cloud, the next step can predict its pose bins
-  return BB200_OK;
-}
-
-int Filter::enqueue_resample_push(const bb200_resample_opts& o, uint64_t global_total, uint64_t cdf_offset, uint64_t slot_begin, uint64_t slot_end,
-                                  uint64_t shard, const double pivot[2]) {
-  if (peer_world_ == 0) return fail(BB200_ERR_STATE, "open_peers must run before resample_push");
-  if (!cdf_valid_) return fail(BB200_ERR_STATE, "build_cdf must run before resample_push");
-  if (o.min_particles < o.max_particles) return fail(BB200_ERR_STATE, "sharded resampling does not support KLD");
-  if (o.random_state_probability > 0.0 && n_free_ == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
-  if (o.scheme != BB200_RESAMPLE_SYSTEMATIC && (slot_begin != 0 || slot_end != o.max_particles))
-    return fail(BB200_ERR_INVALID_ARGUMENT, "multinomial push walks all global slots: pass [0, max_particles)");
-  BB_CHECK(cudaSetDevice(config_.device));
-  ResampleArgs a = make_resample_args(o, 0, slot_end - slot_begin, false);
-  a.slot_first = slot_begin;
-  if (o.scheme != BB200_RESAMPLE_SYSTEMATIC) {  // draws are independent: every rank filters the global slots by its CDF span
-    a.span_filter = 1;
-    a.owner_first = first_index_;
-    a.owner_count = shard;
-  }
-  a.global_total = global_total;
-  a.cdf_offset = cdf_offset;
-  a.weights_out = nullptr;
-  a.ancestors = nullptr;
-  a.peer_count = peer_world_;
-  a.peer_shard = shard;
-  a.pivot_x = pivot[0];
-  a.pivot_y = pivot[1];
-  for (int r = 0; r < peer_world_; ++r) a.peer_out[r] = peer_states_[cur_ ^ 1][r];
-  mark("resample_push");
-  // slot_count may be 0 (a shard without weight): the kernel still writes its (zero) moment partials.
-  pushed_blocks_ = launch_resample(a, scalars_, partials_, stream_);
-  BB_LAUNCHED("resample_push");
-  return BB200_OK;
-}
-
-int Filter::enqueue_resample_push_device(const bb200_resample_opts& o, const uint64_t* rank_totals_device, int rank, int world, uint64_t shard,
-                                         const double pivot[2]) {
-  if (peer_world_ == 0) return fail(BB200_ERR_STATE, "open_peers must run before resample_push");
-  if (!cdf_valid_) return fail(BB200_ERR_STATE, "build_cdf must run before resample_push");
-  if (o.min_particles < o.max_particles) return fail(BB200_ERR_STATE, "sharded resampling does not support KLD");
-  if (o.random_state_probability > 0.0 && n_free_ == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
-  if (rank_totals_device == nullptr || world != peer_world_ || rank < 0 || rank >= world) return fail(BB200_ERR_INVALID_ARGUMENT, "rank totals / rank / world");
-  BB_CHECK(cudaSetDevice(config_.device));
-  // Systematic: the kernel derives this rank's slot range from the totals; the grid is sized for a shard and strides.
-  // Multinomial: all global slots, filtered by this rank's span.
-  const bool systematic = o.scheme == BB200_RESAMPLE_SYSTEMATIC;
-  ResampleArgs a = make_resample_args(o, 0, systematic ? shard : o.max_particles, false);
-  a.slot_first = 0;
-  a.weights_out = nullptr;
-  a.ancestors = nullptr;
-  a.peer_count = peer_world_;
-  a.peer_shard = shard;
-  a.pivot_x = pivot[0];
-  a.pivot_y = pivot[1];
-  a.rank_totals = reinterpret_cast<const unsigned long long*>(rank_totals_device);
-  a.rank = rank;
-  a.world = world;
-  if (!systematic) {
-    a.span_filter = 1;
-    a.owner_first = first_index_;
-    a.owner_count = shard;
-  }
-  for (int r = 0; r < peer_world_; ++r) a.peer_out[r] = peer_states_[cur_ ^ 1][r];
-  mark("resample_push");
-  pushed_blocks_ = launch_resample(a, scalars_, partials_, stream_);  // a.slot_count only sizes the grid here
-  BB_LAUNCHED("resample_push");
-  return BB200_OK;
-}
-
-int Filter::enqueue_reduce_moments() {
-  BB_CHECK(cudaSetDevice(config_.device));
-  launch_reduce_partials(partials_, pushed_blocks_, kMomentCount, results_, stream_);
-  BB_LAUNCHED("reduce_partials");
-  return BB200_OK;
-}
-
-int Filter::enqueue_flip_adopt(uint64_t n) {
-  cur_ ^= 1;  // the staging buffer, filled by the peers, becomes the particle set
-  return enqueue_adopt(n);
-}
-
-int Filter::enqueue_adopt(uint64_t n) {
-  if (n > capacity_) return fail(BB200_ERR_CAPACITY, "more particles than the filter capacity");
-  cloud_known_ = false;
-  BB_CHECK(cudaSetDevice(config_.device));
-  n_ = n;
-  cdf_valid_ = false;
-  mark("fill_weights");
-  launch_fill(weights_, n, 1.0, stream_);
-  BB_LAUNCHED("fill_weights");
-  return BB200_OK;
-}
-
-int Filter::enqueue_moments(const double pivot[2]) {
-  if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
-  BB_CHECK(cudaSetDevice(config_.device));
-  mark("moments");
-  launch_moments(states_[cur_], weights_, n_, pivot[0], pivot[1], partials_, stream_);
-  BB_LAUNCHED("moments");
-  launch_reduce_partials(partials_, moments_block_count(n_), kMomentCount, results_, stream_);
-  BB_LAUNCHED("reduce_partials");
   return BB200_OK;
 }
 
@@ -1253,7 +1166,7 @@ bool Filter::predict_schedule(const MotionSampling& s, Schedule* grid) const {
   return true;
 }
 
-int Filter::enqueue_propagate_reweight(const MotionSampling* sampling, uint32_t step, bool do_reweight, uint64_t n_points, bool counters_reset) {
+int Filter::enqueue_propagate_reweight_kernels(const MotionSampling* sampling, uint32_t step, bool do_reweight, uint64_t n_points, bool counters_reset) {
   const bool scheduled = do_reweight && n_ >= kScheduleMinParticles;
   Schedule grid{};
   const uint32_t* perm = nullptr;
@@ -1323,36 +1236,17 @@ int Filter::enqueue_propagate_reweight(const MotionSampling* sampling, uint32_t 
 }
 
 int Filter::propagate_reweight(const bb200_motion_sampling* sampling, uint32_t step, const double* points_xy, uint64_t n_points) {
-  if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
-  const bool do_reweight = points_xy != nullptr;
-  if (do_reweight && sensor_ < 0) return fail(BB200_ERR_STATE, "no sensor model map set");
-  if (do_reweight && n_points > 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, "too many points");
   BB_CHECK(cudaSetDevice(config_.device));
-  BB_CHECK(cudaStreamSynchronize(stream_));  // staging buffer reuse + keeps the fine-grained API simple
-  if (do_reweight) {
-    const int st = upload_points(points_xy, n_points);
-    if (st != BB200_OK) return st;
-  }
-  MotionSampling s{};
-  if (sampling != nullptr) s = to_kernel_sampling(*sampling);
-  mark("begin_step");
-  launch_begin_step(scalars_, stream_);
-  BB_LAUNCHED("begin_step");
-  const int st = enqueue_propagate_reweight(sampling != nullptr ? &s : nullptr, step, do_reweight, n_points, false);
+  BB_CHECK(cudaStreamSynchronize(stream_));  // the pinned point staging buffer may still be read by the previous upload
+  const int st = enqueue_propagate_reweight(sampling, step, points_xy, n_points);
   if (st != BB200_OK) return st;
-  cdf_valid_ = false;
-  cloud_known_ = false;
   finish_marks();
   return BB200_OK;
 }
 
 int Filter::max_weight(double* wmax) {
-  if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
-  BB_CHECK(cudaSetDevice(config_.device));
-  launch_begin_step(scalars_, stream_);
-  BB_LAUNCHED("begin_step");
-  launch_max_weight(weights_, n_, scalars_, stream_);
-  BB_LAUNCHED("max_weight");
+  const int st = enqueue_max_weight();
+  if (st != BB200_OK) return st;
   BB_CHECK(cudaMemcpyAsync(scalars_host_, scalars_, sizeof(Scalars), cudaMemcpyDeviceToHost, stream_));
   BB_CHECK(cudaStreamSynchronize(stream_));
   double v;
@@ -1362,24 +1256,13 @@ int Filter::max_weight(double* wmax) {
 }
 
 int Filter::build_cdf(double global_wmax, uint64_t* local_total, int* exponent) {
-  if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
-  BB_CHECK(cudaSetDevice(config_.device));
-  if (global_wmax < 0.0) {
-    launch_begin_step(scalars_, stream_);
-    BB_LAUNCHED("begin_step");
-    launch_max_weight(weights_, n_, scalars_, stream_);
-    BB_LAUNCHED("max_weight");
-  }
-  mark("prepare_cdf");
-  launch_prepare_cdf(scalars_, global_wmax, config_.global_count, tile_state_, scan_tile_count(n_), stream_);
-  BB_LAUNCHED("prepare_cdf");
-  mark("quantize_scan");
-  launch_quantize_scan(weights_, n_, cdf_, scalars_, tile_state_, stream_);
-  BB_LAUNCHED("quantize_scan");
+  int st = BB200_OK;
+  if (global_wmax < 0.0) st = enqueue_max_weight();  // no global value: the exponent from this filter's own largest weight
+  if (st == BB200_OK) st = enqueue_build_cdf(global_wmax);
+  if (st != BB200_OK) return st;
   BB_CHECK(cudaMemcpyAsync(scalars_host_, scalars_, sizeof(Scalars), cudaMemcpyDeviceToHost, stream_));
   BB_CHECK(cudaStreamSynchronize(stream_));
   finish_marks();
-  cdf_valid_ = true;
   if (local_total != nullptr) *local_total = scalars_host_->total;
   if (exponent != nullptr) *exponent = scalars_host_->exponent;
   // No positive finite weight (the reference would divide by zero in normalize.hpp:82): a uniform CDF
@@ -1449,13 +1332,8 @@ void Filter::estimate_from_moments_static(const double m[kMomentCount], const do
 void Filter::estimate_from_moments(const double m[kMomentCount], bb200_estimate* out) const { estimate_from_moments_static(m, pivot_, out); }
 
 int Filter::moments(const double pivot[2], double out[9]) {
-  if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
-  BB_CHECK(cudaSetDevice(config_.device));
-  mark("moments");
-  launch_moments(states_[cur_], weights_, n_, pivot[0], pivot[1], partials_, stream_);
-  BB_LAUNCHED("moments");
-  launch_reduce_partials(partials_, moments_block_count(n_), kMomentCount, results_, stream_);
-  BB_LAUNCHED("reduce_partials");
+  const int st = enqueue_moments(pivot);
+  if (st != BB200_OK) return st;
   BB_CHECK(cudaMemcpyAsync(results_host_, results_, kMomentCount * sizeof(double), cudaMemcpyDeviceToHost, stream_));
   BB_CHECK(cudaStreamSynchronize(stream_));
   finish_marks();
@@ -1678,43 +1556,19 @@ int Filter::resample(const bb200_resample_opts& o, uint64_t* new_size) {
 }
 
 int Filter::resample_range(const bb200_resample_opts& o, uint64_t global_total, uint64_t cdf_offset, uint64_t slot_begin, uint64_t slot_end) {
-  // Sharded filter: this rank produces the output slots [slot_begin, slot_end) -- exactly those whose
-  // comb position falls inside its span of the global CDF -- into the staging buffer, in slot order.
-  if (!cdf_valid_) return fail(BB200_ERR_STATE, "build_cdf must run before resample_range");
-  if (o.scheme != BB200_RESAMPLE_SYSTEMATIC || o.min_particles < o.max_particles)
-    return fail(BB200_ERR_STATE, "range resampling supports the systematic comb without KLD (multinomial: bb200_filter_enqueue_resample_push)");
-  if (o.random_state_probability > 0.0 && n_free_ == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
-  if (slot_end < slot_begin || slot_end - slot_begin > capacity_) return fail(BB200_ERR_CAPACITY, "slot range exceeds the staging buffer");
-  BB_CHECK(cudaSetDevice(config_.device));
-  if (slot_end > slot_begin) {
-    ResampleArgs a = make_resample_args(o, 0, slot_end - slot_begin, false);
-    a.slot_first = slot_begin;  // global slot index
-    a.global_total = global_total;
-    a.cdf_offset = cdf_offset;
-    a.weights_out = nullptr;  // the current weights stay untouched; adopt() writes the ones
-    mark("resample_range");
-    launch_resample(a, scalars_, partials_, stream_);
-    BB_LAUNCHED("resample_range");
-  }
+  const int st = enqueue_resample_range(o, global_total, cdf_offset, slot_begin, slot_end);
+  if (st != BB200_OK) return st;
   BB_CHECK(cudaStreamSynchronize(stream_));
   finish_marks();
   return BB200_OK;
 }
 
 int Filter::adopt(uint64_t n, int from_staging) {
-  // The caller has placed n particle states into the current (or staging) state buffer, e.g. through
-  // an all-to-all: make them the particle set with unit weights (make_from_state, particle_traits.hpp:105).
-  if (n > capacity_) return fail(BB200_ERR_CAPACITY, "more particles than the filter capacity");
-  BB_CHECK(cudaSetDevice(config_.device));
-  if (from_staging) cur_ ^= 1;
-  cloud_known_ = false;
-  n_ = n;
-  cdf_valid_ = false;
-  if (n > 0) {
-    launch_fill(weights_, n, 1.0, stream_);
-    BB_LAUNCHED("fill_weights");
-  }
+  const int st = enqueue_adopt(n);
+  if (st != BB200_OK) return st;
+  if (from_staging) cur_ ^= 1;  // the staging buffer holds the n states
   BB_CHECK(cudaStreamSynchronize(stream_));
+  finish_marks();
   return BB200_OK;
 }
 

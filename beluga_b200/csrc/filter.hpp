@@ -70,22 +70,15 @@ class Filter {
                     const bb200_resample_opts& o, bb200_estimate* est, double* weight_sum, uint64_t* new_size);
 
   // Stream-ordered variants for callers that interleave collectives on the same stream (sharded
-  // filters): nothing here synchronises with the host or reads results back.
+  // filters): nothing here synchronises with the host or reads results back.  Each blocking call
+  // above is its variant here followed by the synchronisation and the read-back.
   int set_stream(void* stream);
   int enqueue_propagate_reweight(const bb200_motion_sampling* sampling, uint32_t step, const double* points_xy, uint64_t n_points);
-  int enqueue_build_cdf();                      // exponent from the wmax in the device scalars (all-reduced by the caller)
+  /// global_wmax < 0: the exponent from the wmax in the device scalars (all-reduced by the caller).
+  int enqueue_build_cdf(double global_wmax);
   int enqueue_resample_range(const bb200_resample_opts& o, uint64_t global_total, uint64_t cdf_offset, uint64_t slot_begin, uint64_t slot_end);
   int enqueue_adopt(uint64_t n);
-  // Peer-to-peer redistribution (one process per GPU; CUDA IPC): handles of the two state buffers,
-  // mapping of the peers' buffers, and the fused produce-and-store step.
-  int ipc_handles(void* out128);
-  int open_peers(int world, int rank, const void* handles /* world x 128 bytes */);
-  int enqueue_resample_push(const bb200_resample_opts& o, uint64_t global_total, uint64_t cdf_offset, uint64_t slot_begin, uint64_t slot_end,
-                            uint64_t shard, const double pivot[2]);
-  int enqueue_resample_push_device(const bb200_resample_opts& o, const uint64_t* rank_totals_device, int rank, int world, uint64_t shard,
-                                   const double pivot[2]);
-  int enqueue_flip_adopt(uint64_t n);
-  int enqueue_reduce_moments();
+  int enqueue_moments(const double pivot[2]);   // raw moments stay in the device result block
 
   // ---- one filter over several shards, exchanges through peer memory (no NCCL, no host round trip) ----
   /// CUDA IPC handles of the two state buffers and the mail block (3 x 64 bytes) for peers in OTHER processes.
@@ -133,7 +126,6 @@ class Filter {
   /// Synchronises and closes the batch of phases enqueued so far.  After kPhaseNormalize a caller may still run
   /// kPhaseResample + kPhaseFinish + step_end (selective resampling: the decision needs the effective sample size).
   int step_end(bb200_estimate* est, double* weight_sum, uint64_t* new_size, double* sum_sq);
-  int enqueue_moments(const double pivot[2]);   // raw moments stay in the device result block
 
   int synchronize();
   int device_pointer(int which, void** ptr, uint64_t* bytes);
@@ -168,7 +160,11 @@ class Filter {
   int fail(int status, const std::string& message);
   int check(cudaError_t e, const char* what);
   int upload_points(const double* points_xy, uint64_t n_points);
-  int enqueue_propagate_reweight(const MotionSampling* sampling, uint32_t step, bool do_reweight, uint64_t n_points, bool counters_reset);
+  /// propagate | schedule | reweight on a staged step (points uploaded, scalars reset), no validation.
+  int enqueue_propagate_reweight_kernels(const MotionSampling* sampling, uint32_t step, bool do_reweight, uint64_t n_points, bool counters_reset);
+  int enqueue_max_weight();  // begin_step | max_weight: this filter's largest weight into the device scalars
+  /// moments | reduce_partials about `pivot` into the device result block; unlike enqueue_moments, also on an empty set.
+  int enqueue_moment_kernels(const double pivot[2]);
   bool predict_schedule(const MotionSampling& s, Schedule* grid) const;
   int ensure_cdf_ready();
   int resample_kld(const bb200_resample_opts& o, uint64_t* accepted);
@@ -206,7 +202,6 @@ class Filter {
   cudaStream_t stream_{nullptr};
   bool owns_stream_{true};
   int peer_world_{0}, peer_rank_{0};
-  uint32_t pushed_blocks_{1};
   Pose2* peer_states_[2][8]{};  // [buffer][rank]: the peers' ping-pong state buffers mapped into this process
   ShardMail* mail_{nullptr};                 // this rank's mail block
   ShardMail* peer_mail_[kMaxShards]{};       // every rank's mail block as seen from here ([rank] = mail_)

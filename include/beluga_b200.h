@@ -254,25 +254,6 @@ int bb200_filter_enqueue_resample_range(bb200_filter* f, const bb200_resample_op
                                         uint64_t slot_begin, uint64_t slot_end);
 int bb200_filter_enqueue_adopt(bb200_filter* f, uint64_t n);
 int bb200_filter_enqueue_moments(bb200_filter* f, const double pivot_xy[2]);
-/* Fused resample + redistribution over NVLink peer memory (one process per GPU, <= 8 ranks, equal
- * shards).  Each rank exports CUDA IPC handles of its two state buffers (128 bytes), the handles of all
- * ranks are gathered by the caller and opened with bb200_filter_open_peers.  bb200_filter_enqueue_resample_push
- * then produces this rank's slot range [slot_begin, slot_end) and stores every state straight into the
- * staging buffer of the rank that owns the slot (peer stores), accumulating the raw moments of what it
- * produced; bb200_filter_enqueue_reduce_moments leaves them in the result block for the caller's
- * all-reduce -- which is also the barrier after which every rank calls bb200_filter_enqueue_flip_adopt. */
-int bb200_filter_ipc_handles(bb200_filter* f, void* out128);
-int bb200_filter_open_peers(bb200_filter* f, int world, int rank, const void* handles);
-int bb200_filter_enqueue_resample_push(bb200_filter* f, const bb200_resample_opts* o, uint64_t global_total, uint64_t cdf_offset,
-                                       uint64_t slot_begin, uint64_t slot_end, uint64_t shard, const double pivot_xy[2]);
-/* The same with the bookkeeping on the device: rank_totals_device points at the `world` all-gathered
- * fixed-point totals (uint64, device memory, rank order).  The kernel derives the global total, this
- * rank's CDF offset and (systematic) its slot range from them, so the host need not read the totals
- * back before launching -- one host synchronisation per step instead of two. */
-int bb200_filter_enqueue_resample_push_device(bb200_filter* f, const bb200_resample_opts* o, const uint64_t* rank_totals_device, int rank,
-                                              int world, uint64_t shard, const double pivot_xy[2]);
-int bb200_filter_enqueue_reduce_moments(bb200_filter* f);
-int bb200_filter_enqueue_flip_adopt(bb200_filter* f, uint64_t n);
 /* Ancestor index of every particle produced by the last resample (-1: injected random state). */
 int bb200_filter_ancestors(bb200_filter* f, int64_t* out, uint64_t capacity);
 /* The local fixed-point CDF built by the last build_cdf / normalize (parity hook). */
@@ -541,8 +522,6 @@ int bb200_amcl_join_shards(bb200_amcl* a, int world, int rank, const void* handl
 /* Unmap the peers' buffers again.  CUDA IPC wants every importer to close before the exporter frees: call this on all
  * ranks, synchronise the ranks (barrier), then destroy. */
 int bb200_amcl_leave_shards(bb200_amcl* a);
-int bb200_filter_export_shard(bb200_filter* f, void* out256);
-int bb200_filter_join_shards(bb200_filter* f, int world, int rank, const void* handles);
 
 /* ---------------------------------------------------------------------------------------------
  * Many independent filters on one GPU: a batch of K beluga::Amcl members that share one device, one

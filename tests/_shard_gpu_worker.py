@@ -1,5 +1,10 @@
 """Worker of tests/test_gpu_sharded.py: one rank (one GPU) of a sharded filter; rank 0 also runs the
-same filter on a single GPU and compares -- results must not depend on the number of ranks."""
+same filter on a single GPU and compares -- results must not depend on the number of ranks.
+
+    python -m torch.distributed.run --nproc-per-node=R _shard_gpu_worker.py SHARD STEPS MODE
+
+MODE: nccl, nccl-recovery, nccl-selective (NCCL collectives from Python), p2p, p2p-recovery, p2p-multinomial,
+p2p-kld (the exchanges through peer memory inside the library)."""
 import os
 import sys
 
@@ -26,6 +31,8 @@ def main():
     scheme = bb.RESAMPLE_MULTINOMIAL if mode == "p2p-multinomial" else bb.RESAMPLE_SYSTEMATIC
     inject = 0.03 if mode.endswith("recovery") or mode == "p2p-multinomial" else None  # random_intersperse probability
     kld_min = 500 if mode == "p2p-kld" else None  # KLD-adaptive particle count on shards (peer-memory path)
+    # every other step keeps its particles, the others resample only when the effective sample size drops
+    selective = dict(selective_resampling=True, resample_interval=2) if mode == "nccl-selective" else {}
     total = shard * world
     sc = synthetic.make_scenario(grid_size=200, n_beams=181, steps=steps + 1)
     motion = bb.DifferentialDriveModelParam(0.1, 0.05, 0.1, 0.05)
@@ -33,22 +40,24 @@ def main():
     grid = bb.OccupancyGrid(sc.cells, sc.resolution)
 
     override = inject if (p2p and inject is not None) else 0.0  # the peer-memory path takes the injection probability as a parameter
-    sharded = ShardedAmcl(motion, bb.AmclParams(resample_scheme=scheme, seed=21, device=local_rank, recovery_probability_override=override),
+    sharded = ShardedAmcl(motion, bb.AmclParams(resample_scheme=scheme, seed=21, device=local_rank, recovery_probability_override=override, **selective),
                           shard=shard, p2p=p2p, kld_min_particles=kld_min)
     sharded.update_map(bb.SENSOR_LIKELIHOOD_FIELD, lfm, grid)
     sharded.initialize(sc.initial_mean, sc.initial_cov)
     single = None
     if rank == 0:
         single = bb.Amcl(motion, bb.AmclParams(min_particles=kld_min or total, max_particles=total, resample_scheme=scheme, seed=21, device=0,
-                                               recovery_probability_override=override))
+                                               recovery_probability_override=override, **selective))
         single.update_map(bb.SENSOR_LIKELIHOOD_FIELD, lfm, grid)
         single.initialize(sc.initial_mean, sc.initial_cov)
 
+    resampled = []
     for k in range(steps):
         pose = bb.se2(*sc.poses[k])
         out = sharded.update(pose, sc.scans[k], random_state_probability=None if p2p else inject)
         assert out is not None
         mean, cov, info = out
+        resampled.append(info["resampled"])
         # gather the sharded particle set on rank 0 (a KLD-sized filter holds fewer than `shard` particles per rank)
         states, weights = sharded.filter.particles()
         padded = np.zeros((shard, 4))
@@ -58,6 +67,9 @@ def main():
         gathered = [torch.zeros(shard, 4, dtype=torch.float64, device="cuda") for _ in range(world)]
         dist.all_gather(gathered, torch.from_numpy(padded).cuda())
         gathered = [g[: int(c.item())] for g, c in zip(gathered, counts)]
+        if selective:
+            gathered_weights = [torch.zeros(shard, dtype=torch.float64, device="cuda") for _ in range(world)]
+            dist.all_gather(gathered_weights, torch.from_numpy(weights).cuda())
         if rank == 0:
             if inject is None or p2p:
                 r = single.update(pose, sc.scans[k])
@@ -75,11 +87,18 @@ def main():
             all_states = torch.cat(gathered).cpu().numpy()
             assert len(all_states) == len(ref_states) == info["n_particles"], f"step {k}: {len(all_states)} particles on shards, {len(ref_states)} on one GPU"
             assert np.array_equal(all_states, ref_states), f"step {k}: sharded particle set differs from the single-GPU one"
-            assert np.all(weights == 1.0) and np.all(ref_w == 1.0)
+            if selective:  # a step that keeps its particles leaves them normalised weights
+                assert info["resampled"] == bool(r.resampled), f"step {k}: the sharded filter decided otherwise whether to resample"
+                all_weights = torch.cat(gathered_weights).cpu().numpy()
+                assert np.array_equal(all_weights, ref_w), f"step {k}: sharded weights differ from the single-GPU ones"
+            else:
+                assert np.all(weights == 1.0) and np.all(ref_w == 1.0)
             assert info["weight_sum"] == ref_sum
             tol = 1e-11 if kld_min else 1e-12  # KLD: the single filter re-reads its new set for the estimate, the shards sum what they produced
             assert np.abs(mean - ref_mean).max() < tol
             assert np.abs(cov - ref_cov).max() < tol
+    if selective:
+        assert any(resampled) and not all(resampled), f"selective resampling should both resample and keep: {resampled}"
     sharded.close()
     dist.barrier()
     if rank == 0:

@@ -1,4 +1,4 @@
-"""CPU-side checks of the drop-in boundary: the C-ABI library loads, exports every symbol that
+"""CPU-side checks of the drop-in boundary: the C-ABI library loads, exports exactly the symbols that
 include/beluga_b200.h declares, refuses to run without a GPU, and its host-only logic matches the oracle."""
 import ctypes as C
 import math
@@ -36,6 +36,8 @@ def test_header_symbols_are_exported(lib):
     assert len(declared) >= 35
     missing = [s for s in declared if s not in exported]
     assert not missing, f"declared in include/beluga_b200.h but not exported: {missing}"
+    undeclared = sorted(exported - set(declared))
+    assert not undeclared, f"exported but not declared in include/beluga_b200.h: {undeclared}"
     assert set(_capi.SIGNATURES) == set(declared), "ctypes table and header disagree"
     assert lib.bb200_abi_version() == 2
 

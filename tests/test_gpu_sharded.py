@@ -2,7 +2,7 @@
 estimate as the single-GPU filter with the same total particle count, step after step -- both with
 the NCCL all-to-all redistribution and with the fused kernel that stores over NVLink peer memory, with
 recovery injection (random_intersperse) and with multinomial sampling (every rank filters the global
-slots by its span of the CDF)."""
+slots by its span of the CDF).  The NCCL fallback also runs with one rank, so that one GPU exercises it."""
 import os
 import subprocess
 import sys
@@ -14,21 +14,34 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 MODES = ["nccl", "p2p", "nccl-recovery", "p2p-recovery", "p2p-multinomial", "p2p-kld"]
+ONE_GPU_MODES = ["nccl", "nccl-recovery", "nccl-selective"]
 
 
-@pytest.mark.parametrize("mode", MODES)
-def test_two_gpu_shards_match_single_gpu(mode):
+def _run_worker(ranks: int, port: int, mode: str):
     import beluga_b200 as bb
     from beluga_b200 import build as bb_build
 
     bb_build.build()
-    if bb.device_count() < 2:
-        pytest.skip("needs 2 GPUs")
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
-           "--master-port", str(29711 + 2 * MODES.index(mode)), os.path.join(ROOT, "tests", "_shard_gpu_worker.py"), "40000", "6", mode]
+    if bb.device_count() < ranks:
+        pytest.skip(f"needs {ranks} GPUs")
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={ranks}", "--master-addr", "127.0.0.1",
+           "--master-port", str(port), os.path.join(ROOT, "tests", "_shard_gpu_worker.py"), "40000", "6", mode]
     out = subprocess.run(cmd, capture_output=True, text=True, timeout=600, cwd=ROOT)
     assert out.returncode == 0, out.stdout[-2000:] + out.stderr[-4000:]
     assert "SHARD_GPU_WORKER_OK" in out.stdout
+
+
+@pytest.mark.parametrize("mode", MODES)
+def test_two_gpu_shards_match_single_gpu(mode):
+    _run_worker(2, 29711 + 2 * MODES.index(mode), mode)
+
+
+@pytest.mark.parametrize("mode", ONE_GPU_MODES)
+def test_one_rank_nccl_fallback_matches_single_gpu(mode):
+    """The NCCL fallback of ShardedAmcl with a single rank: the filter-level calls it composes (the stream-ordered ones on
+    a resampling step; the blocking ones, normalize_by and the effective-sample-size decision under selective resampling)
+    must reproduce the single-GPU filter."""
+    _run_worker(1, 29741 + 2 * ONE_GPU_MODES.index(mode), mode)
 
 
 @pytest.mark.parametrize("mode", ["systematic", "multinomial", "selective"])

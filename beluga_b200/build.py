@@ -14,8 +14,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbeluga_b200.so")
-SOURCES = ["kernels.cu", "cluster.cu", "filter.cu", "amcl.cu", "batch.cu", "c_api.cu", "map_host.cpp", "cluster_host.cpp"]
-HEADERS = ["kernels.cuh", "cluster.cuh", "cluster_host.hpp", "se2_math.cuh", "filter.hpp", "amcl.hpp", "batch.hpp", "map_host.hpp", os.path.join("..", "..", "include", "beluga_b200.h")]
+SOURCES = ["kernels.cu", "cluster.cu", "device_map.cu", "filter.cu", "amcl.cu", "batch.cu", "c_api.cu", "map_host.cpp", "cluster_host.cpp"]
+HEADERS = ["kernels.cuh", "cluster.cuh", "cluster_host.hpp", "se2_math.cuh", "device_map.hpp", "filter.hpp", "amcl.hpp", "batch.hpp", "map_host.hpp", os.path.join("..", "..", "include", "beluga_b200.h")]
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [

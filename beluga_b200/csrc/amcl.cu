@@ -87,60 +87,14 @@ bb200_motion_sampling motion_sampling(const bb200_motion_param& p, const Pose2& 
   return out;
 }
 
-Amcl::Amcl(const bb200_amcl_param& p, const bb200_motion_param& motion, HostOnly) : params_(p), motion_(motion) {
+AmclPolicy::AmclPolicy(const bb200_amcl_param& p, const bb200_motion_param& motion) : params_(p), motion_(motion) {
   if (params_.resample_interval == 0) params_.resample_interval = 1;
 }
 
-Amcl::Amcl(const bb200_amcl_param& p, const bb200_motion_param& motion) : params_(p), motion_(motion) {
-  bb200_filter_config c{};
-  c.device = p.device;
-  c.capacity = p.shard_capacity != 0 ? p.shard_capacity : p.max_particles;
-  c.seed = p.seed;
-  c.first_index = p.shard_first_index;
-  c.global_count = p.max_particles;
-  c.record_ancestors = p.record_ancestors;
-  filter_ = std::make_unique<Filter>(c);
-  if (params_.resample_interval == 0) params_.resample_interval = 1;
-  if (sharded() && params_.min_particles < params_.max_particles && filter_->ok()) (void)filter_->enable_shard_kld();
-}
-
-int Amcl::initialize(const double mean[3], const double cov[9]) {
-  error_.clear();
-  const int st = filter_->initialize_normal(mean, cov, sharded() ? params_.shard_capacity : params_.max_particles);
-  if (st == BB200_OK) {
-    force_update_ = true;  // amcl_core.hpp:136
-    initialized_ = true;
-  }
-  return st;
-}
-
-int Amcl::initialize_from_map() {
-  error_.clear();
-  const int st = filter_->initialize_uniform(sharded() ? params_.shard_capacity : params_.max_particles);
-  if (st == BB200_OK) {
-    force_update_ = true;  // beluga_ros/include/beluga_ros/amcl.hpp:193-199
-    initialized_ = true;
-  }
-  return st;
-}
-
-int Amcl::initialize_states(const double* states, const double* weights, uint64_t n) {
-  error_.clear();
-  const int st = filter_->set_particles(states, weights, n);
-  if (st == BB200_OK) {
-    force_update_ = true;
-    initialized_ = n > 0;
-  }
-  return st;
-}
-
-int Amcl::plan_update(const double control[4], bb200_step_plan* plan) {
-  error_.clear();
+void AmclPolicy::plan_update(const double control[4], uint64_t n, bb200_step_plan* plan) {
   *plan = bb200_step_plan{};
   const Pose2 pose{control[0], control[1], control[2], control[3]};
-  // Sharded filters gate on the GLOBAL particle count, which never drops to zero once initialised.
-  const uint64_t n = !filter_ ? host_size_ : sharded() ? (initialized_ ? filter_->global_size() : 0u) : filter_->size();
-  if (n == 0) return BB200_OK;  // amcl_core.hpp:166-168 -> std::nullopt
+  if (n == 0) return;  // amcl_core.hpp:166-168 -> std::nullopt
 
   // update_policy_(control_action) -- on_motion vs the last ACCEPTED pose (on_motion.hpp:121-133)
   bool moved;
@@ -153,7 +107,7 @@ int Amcl::plan_update(const double control[4], bb200_step_plan* plan) {
             std::fabs(rot_log(Rot2{delta.c, delta.s})) > params_.update_min_a;
     if (moved) latest_pose_ = pose;
   }
-  if (!moved && !force_update_) return BB200_OK;
+  if (!moved && !force_update_) return;
 
   // control_action_window_ << control (circular_array.hpp:473-480); reads clamp to size-1 (:353-361)
   window_[1] = window_[0];
@@ -191,28 +145,51 @@ int Amcl::plan_update(const double control[4], bb200_step_plan* plan) {
   for (int k = 0; k < 3; ++k) o.spatial_resolution[k] = params_.spatial_resolution[k];
   o.random_state_probability = random_state_probability;
   plan->update = 1;
-  return BB200_OK;
 }
 
-void Amcl::commit_update(int resampled, double random_state_probability) {
+void AmclPolicy::commit_update(int resampled, double random_state_probability) {
   if (resampled && random_state_probability > 0.0) fast_output_ = slow_output_ = 0.0;  // amcl_core.hpp:184-186
   force_update_ = false;
 }
 
-Amcl::HostState Amcl::snapshot() const {
-  return HostState{latest_pose_, every_n_current_, slow_output_, fast_output_, {window_[0], window_[1]}, window_size_, force_update_, step_};
+// ---------------------------------------------------------------------------------------------------
+
+Amcl::Amcl(const bb200_amcl_param& p, const bb200_motion_param& motion)
+    : policy_(p, motion),
+      filter_(bb200_filter_config{p.device, p.shard_capacity != 0 ? p.shard_capacity : p.max_particles, p.seed, p.shard_first_index, p.max_particles,
+                                  p.record_ancestors}) {
+  if (sharded() && p.min_particles < p.max_particles && filter_.ok()) (void)filter_.enable_shard_kld();
 }
 
-void Amcl::restore(const HostState& s) {
-  latest_pose_ = s.latest_pose;
-  every_n_current_ = s.every_n_current;
-  slow_output_ = s.slow_output;
-  fast_output_ = s.fast_output;
-  window_[0] = s.window[0];
-  window_[1] = s.window[1];
-  window_size_ = s.window_size;
-  force_update_ = s.force_update;
-  step_ = s.step;
+int Amcl::initialized(int status, bool has_particles) {
+  if (status == BB200_OK) {
+    policy_.force_update();  // amcl_core.hpp:136, beluga_ros/include/beluga_ros/amcl.hpp:193-199
+    initialized_ = has_particles;
+  }
+  return status;
+}
+
+int Amcl::initialize(const double mean[3], const double cov[9]) {
+  error_.clear();
+  return initialized(filter_.initialize_normal(mean, cov, sharded() ? params().shard_capacity : params().max_particles), true);
+}
+
+int Amcl::initialize_from_map() {
+  error_.clear();
+  return initialized(filter_.initialize_uniform(sharded() ? params().shard_capacity : params().max_particles), true);
+}
+
+int Amcl::initialize_states(const double* states, const double* weights, uint64_t n) {
+  error_.clear();
+  return initialized(filter_.set_particles(states, weights, n), n > 0);
+}
+
+int Amcl::plan_update(const double control[4], bb200_step_plan* plan) {
+  error_.clear();
+  // Sharded filters gate on the GLOBAL particle count, which never drops to zero once initialised.
+  const uint64_t n = sharded() ? (initialized_ ? filter_.global_size() : 0u) : filter_.size();
+  policy_.plan_update(control, n, plan);
+  return BB200_OK;
 }
 
 int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], const double* points_xy, uint64_t n_points,
@@ -220,21 +197,21 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
   *out = bb200_update_result{};
   if (ranks == nullptr || count < 1 || count > kMaxShards) return BB200_ERR_INVALID_ARGUMENT;
   Amcl& lead = *ranks[0];
-  const bool kld = lead.params_.min_particles < lead.params_.max_particles;
+  const bool kld = lead.params().min_particles < lead.params().max_particles;
   if (kld)
     for (int r = 0; r < count; ++r)
-      if (!ranks[r]->filter_->shard_kld())
-        return ranks[r]->filter_->fail_with(BB200_ERR_STATE, "KLD-adaptive resampling on shards: the hash arrays were not exported (create the shards with min_particles < max_particles before joining them)");
+      if (!ranks[r]->filter_.shard_kld())
+        return ranks[r]->filter_.fail_with(BB200_ERR_STATE, "KLD-adaptive resampling on shards: the hash arrays were not exported (create the shards with min_particles < max_particles before joining them)");
   for (int r = 0; r < count; ++r)
-    if (ranks[r]->sharded() && ranks[r]->filter_->shard_world() <= 1)
-      return ranks[r]->filter_->fail_with(BB200_ERR_STATE, "this shard has not joined its peers (bb200_amcl_join_shards / bb200_sharded_amcl_create)");
-  std::vector<HostState> before;
+    if (ranks[r]->sharded() && ranks[r]->filter_.shard_world() <= 1)
+      return ranks[r]->filter_.fail_with(BB200_ERR_STATE, "this shard has not joined its peers (bb200_amcl_join_shards / bb200_sharded_amcl_create)");
+  std::vector<AmclPolicy> before;
   before.reserve(static_cast<size_t>(count));
-  for (int r = 0; r < count; ++r) before.push_back(ranks[r]->snapshot());
+  for (int r = 0; r < count; ++r) before.push_back(ranks[r]->policy_);
   auto rollback = [&](int st) {
     for (int r = 0; r < count; ++r) {
-      ranks[r]->restore(before[static_cast<size_t>(r)]);
-      ranks[r]->filter_->step_abort();
+      ranks[r]->policy_ = before[static_cast<size_t>(r)];
+      ranks[r]->filter_.step_abort();
     }
     return st;
   };
@@ -245,7 +222,7 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
     const int st = ranks[r]->plan_update(control, &p);
     if (st != BB200_OK) return rollback(st);
     if (r == 0) plan = p;
-    if (p.update != plan.update || p.step != plan.step) return rollback(lead.filter_->fail_with(BB200_ERR_STATE, "the shards of a filter disagree on the step plan"));
+    if (p.update != plan.update || p.step != plan.step) return rollback(lead.filter_.fail_with(BB200_ERR_STATE, "the shards of a filter disagree on the step plan"));
   }
   if (!plan.update) return BB200_OK;
   out->random_state_probability = plan.random_state_probability;
@@ -253,7 +230,7 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
   auto run_phases = [&](std::initializer_list<int> phases) {
     for (const int phase : phases)
       for (int r = 0; r < count; ++r) {
-        const int st = ranks[r]->filter_->step_phase(phase);
+        const int st = ranks[r]->filter_.step_phase(phase);
         if (st != BB200_OK) return st;
       }
     return static_cast<int>(BB200_OK);
@@ -263,7 +240,7 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
       bb200_estimate est{};
       double weight_sum = 0.0, sq = 0.0;
       uint64_t n = 0;
-      const int st = ranks[r]->filter_->step_end(&est, &weight_sum, &n, &sq);
+      const int st = ranks[r]->filter_.step_end(&est, &weight_sum, &n, &sq);
       if (st != BB200_OK) return st;
       if (r == 0) {  // the exchanged sums are the same bits on every shard
         out->estimate = est;
@@ -277,40 +254,40 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
 
   const bool resample_now = plan.resample != 0 && plan.needs_ess == 0;
   for (int r = 0; r < count; ++r) {
-    const int st = ranks[r]->filter_->step_begin(plan.sampling, plan.step, points_xy, n_points, plan.opts, resample_now);
+    const int st = ranks[r]->filter_.step_begin(plan.sampling, plan.step, points_xy, n_points, plan.opts, resample_now);
     if (st != BB200_OK) return rollback(st);
   }
   // views::take_while_kld over the shards (take_while_kld.hpp:72-137): the candidate stream is ordered by output slot, and
   // every rank sees the spatial hash of every candidate, so all ranks count distinct buckets over the same stream and
   // stop at the same slot.  Windows of slots double like the single-GPU chunks; one host decision per window.
   auto kld_size = [&](uint64_t* accepted) {
-    const uint64_t max = lead.params_.max_particles;
+    const uint64_t max = lead.params().max_particles;
     for (int r = 0; r < count; ++r) {
-      const int st = ranks[r]->filter_->step_totals(nullptr, nullptr);  // enqueue the totals exchange on every shard
+      const int st = ranks[r]->filter_.step_totals(nullptr, nullptr);  // enqueue the totals exchange on every shard
       if (st != BB200_OK) return st;
     }
     uint64_t begin = 0, k_before = 0;
-    uint64_t end = std::min<uint64_t>(max, std::max<uint64_t>(2 * lead.params_.min_particles, 65536));
+    uint64_t end = std::min<uint64_t>(max, std::max<uint64_t>(2 * lead.params().min_particles, 65536));
     *accepted = max;
     while (begin < max) {
       for (int r = 0; r < count; ++r) {
-        const int st = ranks[r]->filter_->kld_sharded_candidates(begin, end);
+        const int st = ranks[r]->filter_.kld_sharded_candidates(begin, end);
         if (st != BB200_OK) return st;
       }
       for (int r = 0; r < count; ++r) {
-        const int st = ranks[r]->filter_->kld_sharded_count(begin, end, k_before);
+        const int st = ranks[r]->filter_.kld_sharded_count(begin, end, k_before);
         if (st != BB200_OK) return st;
       }
       uint64_t cutoff = ~0ull, fresh = 0;
       for (int r = 0; r < count; ++r) {
         uint64_t c = 0, f = 0;
-        const int st = ranks[r]->filter_->kld_sharded_read(&c, &f);
+        const int st = ranks[r]->filter_.kld_sharded_read(&c, &f);
         if (st != BB200_OK) return st;
         if (r == 0) {
           cutoff = c;
           fresh = f;
         } else if (c != cutoff || f != fresh) {
-          return lead.filter_->fail_with(BB200_ERR_STATE, "KLD on shards: the ranks disagree on the count");
+          return lead.filter_.fail_with(BB200_ERR_STATE, "KLD on shards: the ranks disagree on the count");
         }
       }
       if (cutoff != ~0ull) {
@@ -330,7 +307,7 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
     uint64_t accepted = 0;
     if (st == BB200_OK) st = kld_size(&accepted);
     if (st == BB200_OK) {
-      for (int r = 0; r < count; ++r) ranks[r]->filter_->step_set_kld_accepted(accepted);
+      for (int r = 0; r < count; ++r) ranks[r]->filter_.step_set_kld_accepted(accepted);
       st = run_phases({Filter::kPhaseResample, Filter::kPhaseFinish});
     }
   } else {
@@ -344,12 +321,12 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
   if (!resample_now && plan.resample != 0) {
     // on_effective_size_drop (on_effective_size_drop.hpp:45-49): ESS = 1 / sum w~^2 < N / 2
     const double ess = sum_sq > 0.0 ? 1.0 / sum_sq : 0.0;
-    if (ess < static_cast<double>(lead.filter_->global_size()) * 0.5) {
+    if (ess < static_cast<double>(lead.filter_.global_size()) * 0.5) {
       if (kld) {
         uint64_t accepted = 0;
         st = kld_size(&accepted);
         if (st != BB200_OK) return rollback(st);
-        for (int r = 0; r < count; ++r) ranks[r]->filter_->step_set_kld_accepted(accepted);
+        for (int r = 0; r < count; ++r) ranks[r]->filter_.step_set_kld_accepted(accepted);
       }
       st = run_phases({Filter::kPhaseResample, Filter::kPhaseFinish});
       if (st == BB200_OK) st = close_batch(nullptr);
@@ -358,9 +335,9 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
     }
   }
   out->resampled = resampled ? 1 : 0;
-  out->weights_degenerate = lead.filter_->last_weights_valid() ? 0 : 1;
+  out->weights_degenerate = lead.filter_.last_weights_valid() ? 0 : 1;
   for (int r = 0; r < count; ++r) {
-    ranks[r]->filter_->step_abort();
+    ranks[r]->filter_.step_abort();
     ranks[r]->commit_update(out->resampled, plan.random_state_probability);
   }
   out->updated = 1;
@@ -372,9 +349,9 @@ int Amcl::update(const double control[4], const double* points_xy, uint64_t n_po
     Amcl* self = this;
     return update_group(&self, 1, control, points_xy, n_points, out);
   }
-  const HostState before = snapshot();
+  const AmclPolicy before = policy_;
   const int st = update_device(control, points_xy, n_points, out);
-  if (st != BB200_OK) restore(before);  // policies, control window and recovery estimator as if the call had not happened
+  if (st != BB200_OK) policy_ = before;  // policies, control window and recovery estimator as if the call had not happened
   return st;
 }
 
@@ -384,21 +361,21 @@ int Amcl::update_device(const double control[4], const double* points_xy, uint64
   int st = plan_update(control, &plan);
   if (st != BB200_OK || !plan.update) return st;
   out->random_state_probability = plan.random_state_probability;
-  const uint64_t n = filter_->size();
+  const uint64_t n = filter_.size();
   bool do_resample = plan.resample != 0;
-  const bool kld_active = params_.min_particles < params_.max_particles;
+  const bool kld_active = params().min_particles < params().max_particles;
   if (do_resample && !plan.needs_ess && !kld_active) {
     // The whole step in one stream-ordered sequence with a single host synchronisation.
     uint64_t new_size = 0;
-    st = filter_->step_resample(plan.sampling, plan.step, points_xy, n_points, plan.opts, &out->estimate, &out->weight_sum, &new_size);
+    st = filter_.step_resample(plan.sampling, plan.step, points_xy, n_points, plan.opts, &out->estimate, &out->weight_sum, &new_size);
     if (st != BB200_OK) return st;
     out->resampled = 1;
     out->n_particles = new_size;
   } else {
-    st = filter_->propagate_reweight(&plan.sampling, plan.step, points_xy, n_points);
+    st = filter_.propagate_reweight(&plan.sampling, plan.step, points_xy, n_points);
     if (st != BB200_OK) return st;
     double factor = 0.0, sum_sq = 0.0;
-    st = filter_->normalize(&factor, &sum_sq);
+    st = filter_.normalize(&factor, &sum_sq);
     if (st != BB200_OK) return st;
     out->weight_sum = factor;
     if (plan.needs_ess) {
@@ -408,15 +385,15 @@ int Amcl::update_device(const double control[4], const double* points_xy, uint64
     }
     if (do_resample) {
       uint64_t new_size = 0;
-      st = filter_->resample(plan.opts, &new_size);
+      st = filter_.resample(plan.opts, &new_size);
       if (st != BB200_OK) return st;
       out->resampled = 1;
     }
-    st = filter_->estimate(&out->estimate);
+    st = filter_.estimate(&out->estimate);
     if (st != BB200_OK) return st;
-    out->n_particles = filter_->size();
+    out->n_particles = filter_.size();
   }
-  out->weights_degenerate = filter_->last_weights_valid() ? 0 : 1;
+  out->weights_degenerate = filter_.last_weights_valid() ? 0 : 1;
   commit_update(out->resampled, plan.random_state_probability);
   out->updated = 1;
   return BB200_OK;

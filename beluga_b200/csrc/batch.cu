@@ -1,28 +1,25 @@
 #include "batch.hpp"
 
 #include <algorithm>
-#include <atomic>
 #include <cmath>
 #include <cstring>
+#include <initializer_list>
 
 namespace bb200 {
 
 namespace {
-
-template <class T>
-cudaError_t dev_alloc(T** p, size_t count) {
-  return cudaMalloc(reinterpret_cast<void**>(p), std::max<size_t>(count, 1) * sizeof(T));
-}
-template <class T>
-cudaError_t host_alloc(T** p, size_t count) {
-  return cudaMallocHost(reinterpret_cast<void**>(p), std::max<size_t>(count, 1) * sizeof(T));
-}
 
 constexpr uint64_t kSliceAlign = 32;  // particles
 
 /// Moment-partial rows a member of `capacity` particles can need in the finish launch (whichever form it takes).
 uint64_t finish_rows(uint64_t capacity) {
   return std::max<uint64_t>({resample_scatter_block_count(capacity), resample_block_count(capacity), moments_block_count(capacity)});
+}
+
+uint64_t largest_member(const bb200_amcl_param* params, int n_members) {
+  uint64_t largest = 0;
+  for (int k = 0; params != nullptr && k < n_members; ++k) largest = std::max(largest, params[k].max_particles);
+  return largest;
 }
 
 }  // namespace
@@ -48,45 +45,31 @@ int Batch::validate(const bb200_amcl_param* params, const bb200_motion_param* mo
   return BB200_OK;
 }
 
-Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members) {
+Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members)
+    : clusterizer_(largest_member(params, n_members)) {
   create_status_ = validate(params, motions, n_members, &error_);
   if (create_status_ != BB200_OK) return;
-  uint64_t largest = 0, tiles = 0, rows = 0;
-  members_.resize(static_cast<size_t>(n_members));
+  uint64_t tiles = 0, rows = 0;
+  members_.reserve(static_cast<size_t>(n_members));
   for (int k = 0; k < n_members; ++k) {
-    Member& m = members_[static_cast<size_t>(k)];
-    m.host = std::make_unique<Amcl>(params[k], motions[k], Amcl::HostOnly{});
+    members_.push_back(Member{AmclPolicy(params[k], motions[k])});
+    Member& m = members_.back();
     // The CDF build reads weights and writes the CDF 16 bytes at a time from the slice's start: slices begin on whole
     // 256-byte lines.
     total_ = (total_ + kSliceAlign - 1) / kSliceAlign * kSliceAlign;
     m.offset = total_;
     m.capacity = params[k].max_particles;
-    m.seed = params[k].seed;
     total_ += m.capacity;
-    largest = std::max(largest, m.capacity);
     tiles += batch_scan_tiles(m.capacity);
     rows += finish_rows(m.capacity);
     record_ancestors_ = record_ancestors_ || params[k].record_ancestors != 0;
   }
-  bb200_filter_config c{};
-  c.device = params[0].device;
-  c.capacity = largest;
-  map_ = std::make_unique<Filter>(c);
-  if (!map_->ok()) {
-    create_status_ = map_->create_status();
-    error_ = map_->last_error();
-    return;
-  }
-#define BB_TRY(expr)                         \
-  do {                                       \
-    const int st = check((expr), #expr);     \
-    if (st != BB200_OK) {                    \
-      create_status_ = st;                   \
-      return;                                \
-    }                                        \
-  } while (0)
+  device_ = params[0].device;
+  create_status_ = check_device(device_, &error_);
+  if (create_status_ != BB200_OK) return;
   const size_t k1 = static_cast<size_t>(n_members) + 1;
-  BB_TRY(cudaSetDevice(c.device));
+  BB_TRY(cudaSetDevice(device_));
+  BB_TRY(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
   BB_TRY(dev_alloc(&states_[0], total_));
   BB_TRY(dev_alloc(&states_[1], total_));
   BB_TRY(dev_alloc(&weights_, total_));
@@ -103,47 +86,19 @@ Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, 
   BB_TRY(host_alloc(&ticket_host_, 1));
   BB_TRY(dev_alloc(&members_done_, 1));
   *ticket_host_ = 0;  // pinned allocations are recycled with their old contents
-  BB_TRY(cudaMemsetAsync(scalars_, 0, members_.size() * sizeof(Scalars), map_->stream()));
-  BB_TRY(cudaMemsetAsync(members_done_, 0, sizeof(unsigned int), map_->stream()));
-  BB_TRY(cudaStreamSynchronize(map_->stream()));
-#undef BB_TRY
+  BB_TRY(cudaMemsetAsync(scalars_, 0, members_.size() * sizeof(Scalars), stream_));
+  BB_TRY(cudaMemsetAsync(members_done_, 0, sizeof(unsigned int), stream_));
+  BB_TRY(cudaStreamSynchronize(stream_));
   created_ = true;
 }
 
 Batch::~Batch() {
-  if (map_ && map_->stream() != nullptr) cudaStreamSynchronize(map_->stream());
-  cudaFree(states_[0]);
-  cudaFree(states_[1]);
-  cudaFree(weights_);
-  cudaFree(cdf_);
-  cudaFree(ancestors_);
-  cudaFree(scalars_);
-  cudaFree(tile_state_);
-  cudaFree(partials_);
-  cudaFree(table_);
-  cudaFreeHost(table_host_);
-  cudaFree(first_);
-  cudaFreeHost(first_host_);
-  cudaFree(points_);
-  cudaFreeHost(points_host_);
-  cudaFreeHost(summary_host_);
-  cudaFreeHost(ticket_host_);
-  cudaFree(members_done_);
-}
-
-int Batch::fail(int status, const std::string& message) {
-  error_ = message;
-  return status;
-}
-
-int Batch::check(cudaError_t e, const char* what) {
-  if (e == cudaSuccess) return BB200_OK;
-  return fail(BB200_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-}
-
-int Batch::from_map(int status) {
-  if (status != BB200_OK) error_ = map_->last_error();
-  return status;
+  if (stream_ != nullptr) cudaStreamSynchronize(stream_);
+  for (void* p : std::initializer_list<void*>{states_[0], states_[1], weights_, cdf_, ancestors_, scalars_, tile_state_, partials_, table_, first_,
+                                              points_, members_done_})
+    cudaFree(p);
+  for (void* p : std::initializer_list<void*>{table_host_, first_host_, points_host_, summary_host_, ticket_host_}) cudaFreeHost(p);
+  if (stream_ != nullptr) cudaStreamDestroy(stream_);
 }
 
 int Batch::member_ok(int member) const {
@@ -154,21 +109,15 @@ int Batch::member_ok(int member) const {
   return BB200_OK;
 }
 
-#define BB_CHECK(expr)                    \
-  do {                                    \
-    const int st_ = check((expr), #expr); \
-    if (st_ != BB200_OK) return st_;      \
-  } while (0)
-#define BB_MEMBER(member)                     \
-  do {                                        \
-    error_.clear();                           \
-    const int st_ = member_ok(member);        \
-    if (st_ != BB200_OK) return st_;          \
-  } while (0)
+#define BB_MEMBER(member) do { error_.clear(); if (const int st_ = member_ok(member)) return st_; } while (0)
 
 int Batch::set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob) {
   error_.clear();
-  return from_map(map_->set_likelihood_field_map(p, grid, prob));
+  MapTables tables;
+  const int st = prepare_likelihood_field_map(p, grid, prob, &tables, &error_);
+  if (st != BB200_OK) return st;
+  BB_CHECK(cudaSetDevice(device_));
+  return map_.upload(tables, stream_, &error_);
 }
 
 int Batch::initialize(int member, const double mean[3], const double cov[9]) {
@@ -177,36 +126,32 @@ int Batch::initialize(int member, const double mean[3], const double cov[9]) {
   double transform[9];
   std::string message;
   if (!normal_transform(cov, transform, &message)) return fail(BB200_ERR_INVALID_ARGUMENT, message);
-  BB_CHECK(cudaSetDevice(map_->device()));
-  launch_initialize_normal(states_[m.cur] + m.offset, weights_ + m.offset, m.capacity, mean, transform, m.seed, 0, map_->stream());
+  BB_CHECK(cudaSetDevice(device_));
+  launch_initialize_normal(states_[m.cur] + m.offset, weights_ + m.offset, m.capacity, mean, transform, m.policy.params().seed, 0, stream_);
   ++launches_;
   BB_CHECK(cudaGetLastError());
-  BB_CHECK(cudaStreamSynchronize(map_->stream()));
+  BB_CHECK(cudaStreamSynchronize(stream_));
   m.n = m.capacity;
   m.pivot[0] = mean[0];
   m.pivot[1] = mean[1];
-  m.host->host_initialized(m.n);  // amcl_core.hpp:136: the next update is forced
+  m.policy.force_update();  // amcl_core.hpp:136
   return BB200_OK;
 }
 
 int Batch::initialize_from_map(int member) {
   BB_MEMBER(member);
   Member& m = members_[static_cast<size_t>(member)];
-  const Filter::MapView map = map_->map_view();
-  if (map.sensor < 0) return fail(BB200_ERR_STATE, "initialize_from_map needs a map (set the likelihood field first)");
-  if (map.n_free == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
-  BB_CHECK(cudaSetDevice(map_->device()));
-  launch_initialize_uniform(states_[m.cur] + m.offset, weights_ + m.offset, m.capacity, map.free_cells, map.n_free, map.grid_width, map.grid_resolution,
-                            map.grid_origin, m.seed, 0, map_->stream());
+  if (map_.sensor < 0) return fail(BB200_ERR_STATE, "initialize_from_map needs a map (set the likelihood field first)");
+  if (map_.n_free == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
+  BB_CHECK(cudaSetDevice(device_));
+  launch_initialize_uniform(states_[m.cur] + m.offset, weights_ + m.offset, m.capacity, map_.free_cells, map_.n_free, map_.grid_width,
+                            map_.grid_resolution, map_.grid_origin, m.policy.params().seed, 0, stream_);
   ++launches_;
   BB_CHECK(cudaGetLastError());
-  BB_CHECK(cudaStreamSynchronize(map_->stream()));
+  BB_CHECK(cudaStreamSynchronize(stream_));
   m.n = m.capacity;
-  // pivot of the raw moments: the middle of the map in the global frame (what Filter::initialize_uniform takes)
-  const double cx = 0.5 * map.grid_width * map.grid_resolution, cy = 0.5 * map.grid_height * map.grid_resolution;
-  m.pivot[0] = (map.grid_origin.c * cx - map.grid_origin.s * cy) + map.grid_origin.x;
-  m.pivot[1] = (map.grid_origin.s * cx + map.grid_origin.c * cy) + map.grid_origin.y;
-  m.host->host_initialized(m.n);
+  map_.centre(m.pivot);
+  m.policy.force_update();
   return BB200_OK;
 }
 
@@ -215,8 +160,8 @@ int Batch::initialize_states(int member, const double* states, const double* wei
   Member& m = members_[static_cast<size_t>(member)];
   if (n > m.capacity) return fail(BB200_ERR_CAPACITY, "more particles than the member's max_particles");
   if (n > 0 && states == nullptr) return fail(BB200_ERR_INVALID_ARGUMENT, "states is null");
-  BB_CHECK(cudaSetDevice(map_->device()));
-  BB_CHECK(cudaStreamSynchronize(map_->stream()));
+  BB_CHECK(cudaSetDevice(device_));
+  BB_CHECK(cudaStreamSynchronize(stream_));
   if (n > 0) {
     BB_CHECK(cudaMemcpy(states_[m.cur] + m.offset, states, n * sizeof(Pose2), cudaMemcpyHostToDevice));
     const std::vector<double> ones(weights == nullptr ? n : 0, 1.0);
@@ -225,21 +170,21 @@ int Batch::initialize_states(int member, const double* states, const double* wei
     m.pivot[1] = states[3];
   }
   m.n = n;
-  m.host->host_initialized(n);
+  m.policy.force_update();
   return BB200_OK;
 }
 
 int Batch::force_update(int member) {
   BB_MEMBER(member);
-  members_[static_cast<size_t>(member)].host->force_update();
+  members_[static_cast<size_t>(member)].policy.force_update();
   return BB200_OK;
 }
 
 int Batch::get_particles(int member, double* states, double* weights, uint64_t capacity) {
   BB_MEMBER(member);
   const Member& m = members_[static_cast<size_t>(member)];
-  BB_CHECK(cudaSetDevice(map_->device()));
-  BB_CHECK(cudaStreamSynchronize(map_->stream()));
+  BB_CHECK(cudaSetDevice(device_));
+  BB_CHECK(cudaStreamSynchronize(stream_));
   const uint64_t n = std::min(capacity, m.n);
   if (states != nullptr && n > 0) BB_CHECK(cudaMemcpy(states, states_[m.cur] + m.offset, n * sizeof(Pose2), cudaMemcpyDeviceToHost));
   if (weights != nullptr && n > 0) BB_CHECK(cudaMemcpy(weights, weights_ + m.offset, n * sizeof(double), cudaMemcpyDeviceToHost));
@@ -249,9 +194,9 @@ int Batch::get_particles(int member, double* states, double* weights, uint64_t c
 int Batch::ancestors(int member, int64_t* out, uint64_t capacity) {
   BB_MEMBER(member);
   const Member& m = members_[static_cast<size_t>(member)];
-  if (!m.host->params().record_ancestors) return fail(BB200_ERR_STATE, "the member was created without record_ancestors");
-  BB_CHECK(cudaSetDevice(map_->device()));
-  BB_CHECK(cudaStreamSynchronize(map_->stream()));
+  if (!m.policy.params().record_ancestors) return fail(BB200_ERR_STATE, "the member was created without record_ancestors");
+  BB_CHECK(cudaSetDevice(device_));
+  BB_CHECK(cudaStreamSynchronize(stream_));
   const uint64_t n = std::min(capacity, m.ancestors_n);
   if (out != nullptr && n > 0) BB_CHECK(cudaMemcpy(out, ancestors_ + m.offset, n * sizeof(int64_t), cudaMemcpyDeviceToHost));
   return BB200_OK;
@@ -260,20 +205,16 @@ int Batch::ancestors(int member, int64_t* out, uint64_t capacity) {
 int Batch::cluster_estimate(int member, const bb200_cluster_param& p, bb200_estimate* out) {
   BB_MEMBER(member);
   const Member& m = members_[static_cast<size_t>(member)];
-  return from_map(map_->cluster_estimate_of(states_[m.cur] + m.offset, weights_ + m.offset, m.n, m.pivot, p, out, nullptr, 0, nullptr, nullptr));
+  BB_CHECK(cudaSetDevice(device_));
+  return clusterizer_.estimate(states_[m.cur] + m.offset, weights_ + m.offset, m.n, m.pivot, p, stream_, out, nullptr, 0, nullptr, nullptr, &error_);
 }
 
 int Batch::ensure_points(uint64_t n_points) {
   if (n_points <= points_capacity_) return BB200_OK;
-  BB_CHECK(cudaStreamSynchronize(map_->stream()));
-  cudaFree(points_);
-  cudaFreeHost(points_host_);
-  points_ = nullptr;
-  points_host_ = nullptr;
+  BB_CHECK(cudaStreamSynchronize(stream_));
   points_capacity_ = 0;
   const uint64_t cap = std::max<uint64_t>(n_points + n_points / 2, 4096);
-  BB_CHECK(dev_alloc(&points_, 2 * cap));
-  BB_CHECK(host_alloc(&points_host_, 2 * cap));
+  BB_CHECK(realloc_staged(&points_, &points_host_, 2 * cap));
   points_capacity_ = cap;
   return BB200_OK;
 }
@@ -283,10 +224,11 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   error_.clear();
   const size_t count = members_.size();
   for (size_t k = 0; k < count; ++k) out[k] = bb200_update_result{};
-  std::vector<Amcl::HostState> before(count);
-  for (size_t k = 0; k < count; ++k) before[k] = members_[k].host->snapshot();
+  std::vector<AmclPolicy> before;
+  before.reserve(count);
+  for (const Member& m : members_) before.push_back(m.policy);
   auto rollback = [&](int st) {
-    for (size_t k = 0; k < count; ++k) members_[k].host->restore(before[k]);
+    for (size_t k = 0; k < count; ++k) members_[k].policy = before[k];
     return st;
   };
 
@@ -295,25 +237,23 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   std::vector<uint32_t> active;  // members that update in this step, in member order
   for (size_t k = 0; k < count; ++k) {
     if (present != nullptr && present[k] == 0) continue;
-    const int st = members_[k].host->plan_update(control_poses + 4 * k, &plans[k]);
-    if (st != BB200_OK) return rollback(fail(st, members_[k].host->last_error()));
+    members_[k].policy.plan_update(control_poses + 4 * k, members_[k].n, &plans[k]);
     if (plans[k].update) active.push_back(static_cast<uint32_t>(k));
   }
   if (active.empty()) return BB200_OK;
 
-  const Filter::MapView map = map_->map_view();
-  if (map.sensor < 0) return rollback(fail(BB200_ERR_STATE, "no likelihood-field map set"));
+  if (map_.sensor < 0) return rollback(fail(BB200_ERR_STATE, "no likelihood-field map set"));
   uint64_t points_total = 0;
   uint32_t max_points = 0;
   for (const uint32_t k : active) {
     if (n_points[k] > 0xffffffffull) return rollback(fail(BB200_ERR_INVALID_ARGUMENT, "too many points"));
     if (n_points[k] > 0 && points_xy[k] == nullptr) return rollback(fail(BB200_ERR_INVALID_ARGUMENT, "points_xy is null"));
-    if (plans[k].resample && plans[k].random_state_probability > 0.0 && map.n_free == 0)
+    if (plans[k].resample && plans[k].random_state_probability > 0.0 && map_.n_free == 0)
       return rollback(fail(BB200_ERR_STATE, "recovery injection needs a map with free cells"));
     points_total += n_points[k];
     max_points = std::max(max_points, static_cast<uint32_t>(n_points[k]));
   }
-  int st = check(cudaSetDevice(map_->device()), "cudaSetDevice");
+  int st = check(cudaSetDevice(device_), "cudaSetDevice");
   if (st == BB200_OK) st = ensure_points(points_total);  // the previous step has ended: the staging buffers are free
   if (st != BB200_OK) return rollback(st);
 
@@ -331,7 +271,7 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     b.offset = m.offset;
     b.n = m.n;
     b.slots = m.capacity;
-    b.seed = m.seed;
+    b.seed = m.policy.params().seed;
     b.step = plan.step;
     b.resample = plan.resample;
     b.scheme = plan.opts.scheme;
@@ -343,14 +283,8 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     b.sampling = to_kernel_sampling(plan.sampling);
     b.point_offset = point_offset;
     b.n_points = static_cast<uint32_t>(n_points[k]);
-    double radius = 0.0;  // as Filter::upload_points: NaN sticks (the exact lookup path)
-    const double* p = points_xy[k];
-    for (uint64_t i = 0; i < n_points[k]; ++i) {
-      const double r = std::fabs(p[2 * i]) + std::fabs(p[2 * i + 1]);
-      radius = (r > radius || std::isnan(r)) ? r : radius;
-    }
-    b.points_radius = radius;
-    if (n_points[k] > 0) std::memcpy(points_host_ + 2 * point_offset, p, 2 * n_points[k] * sizeof(double));
+    b.points_radius = scan_radius(points_xy[k], n_points[k]);
+    if (n_points[k] > 0) std::memcpy(points_host_ + 2 * point_offset, points_xy[k], 2 * n_points[k] * sizeof(double));
     point_offset += n_points[k];
     uint32_t ctas[kBatchLaunches];
     batch_member_ctas(b, ctas);
@@ -361,7 +295,7 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   }
   for (int l = 0; l < kBatchLaunches; ++l) first_host_[static_cast<size_t>(l) * (n_active + 1) + n_active] = a.ctas[l];
 
-  cudaStream_t stream = map_->stream();
+  cudaStream_t stream = stream_;
   seq_ = seq_ == 0x7fffffff ? 1 : seq_ + 1;
   *ticket_host_ = 0;
   st = check(cudaMemcpyAsync(table_, table_host_, n_active * sizeof(BatchMember), cudaMemcpyHostToDevice, stream), "upload member table");
@@ -382,12 +316,12 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   a.scalars = scalars_;
   a.partials = partials_;
   a.points = points_;
-  a.field = map.field;
-  a.free_cells = map.free_cells;
-  a.n_free = map.n_free;
-  a.grid_width = map.grid_width;
-  a.grid_resolution = map.grid_resolution;
-  a.grid_origin = map.grid_origin;
+  a.field = map_.field;
+  a.free_cells = map_.free_cells;
+  a.n_free = map_.n_free;
+  a.grid_width = map_.grid_width;
+  a.grid_resolution = map_.grid_resolution;
+  a.grid_origin = map_.grid_origin;
   a.summary = summary_host_;
   a.members_done = members_done_;
   a.ticket = ticket_host_;
@@ -396,21 +330,10 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   st = check(cudaGetLastError(), "batch step launch");
   if (st != BB200_OK) return rollback(st);
 
-  // The last member to finish stores the ticket into pinned memory; spinning on it sees the end of the step before a
-  // stream synchronisation would return.  The stream is queried now and then so that a failed launch cannot hang us.
-  bool done = false;
-  const volatile int* ticket = ticket_host_;
-  for (uint32_t spins = 1; !done; ++spins) {
-    if (*ticket == seq_) {
-      done = true;
-    } else if ((spins & 0x3fffu) == 0) {
-      const cudaError_t q = cudaStreamQuery(stream);
-      if (q != cudaErrorNotReady) break;
-    }
-  }
-  std::atomic_thread_fence(std::memory_order_acquire);
+  // The last member to finish stores the ticket into pinned memory.
+  const bool done = wait_for_ticket(ticket_host_, seq_, stream);
   if (!done) st = check(cudaStreamSynchronize(stream), "batch step");
-  if (st == BB200_OK && !done && *ticket != seq_) st = fail(BB200_ERR_CUDA, "the batch step ended without its completion ticket");
+  if (st == BB200_OK && !done && *static_cast<volatile int*>(ticket_host_) != seq_) st = fail(BB200_ERR_CUDA, "the batch step ended without its completion ticket");
   if (st != BB200_OK) return rollback(st);
 
   for (uint32_t j = 0; j < n_active; ++j) {
@@ -419,14 +342,13 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     const StepSummary& s = summary_host_[j];
     const bb200_step_plan& plan = plans[k];
     bb200_update_result& r = out[k];
-    Filter::estimate_from_moments_static(s.moments, m.pivot, &r.estimate);
+    estimate_from_moments(s.moments, m.pivot, &r.estimate);
     m.pivot[0] = r.estimate.mean[2];
     m.pivot[1] = r.estimate.mean[3];
     if (plan.resample) {
       m.cur ^= 1;
       m.n = m.capacity;
       m.ancestors_n = m.n;
-      m.host->set_host_size(m.n);  // the recovery estimator's 1 / N from the next step on
     }
     r.updated = 1;
     r.resampled = plan.resample;
@@ -434,7 +356,7 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     r.random_state_probability = plan.random_state_probability;
     r.weight_sum = std::ldexp(static_cast<double>(s.total), -s.exponent);
     r.weights_degenerate = s.valid != 0 ? 0 : 1;
-    m.host->commit_update(r.resampled, plan.random_state_probability);
+    m.policy.commit_update(r.resampled, plan.random_state_probability);
   }
   return BB200_OK;
 }

@@ -1,15 +1,15 @@
 // K independent beluga::Amcl filters that share one device, one likelihood-field map and one sensor model, stepped
 // together: one call runs every updating member's step with a fixed sequence of launches (csrc/kernels.cuh:
 // launch_batch_step) and one host synchronisation, whatever K is.  Each member keeps the host half of a bb200_amcl
-// (policies, control window, recovery estimator: an Amcl without a Filter) and a slice of the batch's particle buffers.
+// (AmclPolicy) and a slice of the batch's particle buffers.
 #pragma once
 
-#include <memory>
 #include <string>
 #include <vector>
 
 #include "amcl.hpp"
-#include "filter.hpp"
+#include "cluster.cuh"
+#include "device_map.hpp"
 
 namespace bb200 {
 
@@ -48,23 +48,27 @@ class Batch {
 
  private:
   struct Member {
-    std::unique_ptr<Amcl> host;
+    AmclPolicy policy;
     uint64_t offset{0};    // first particle in the batch buffers
     uint64_t capacity{0};  // max_particles
     uint64_t n{0};
     int cur{0};            // state buffer holding the particles
     double pivot[2]{0.0, 0.0};
-    uint64_t seed{0};
     uint64_t ancestors_n{0};
   };
-  int fail(int status, const std::string& message);
-  int check(cudaError_t e, const char* what);
-  int from_map(int status);  // forwards the map filter's message
+  int fail(int status, const std::string& message) {
+    error_ = message;
+    return status;
+  }
+  int check(cudaError_t e, const char* what) { return cuda_check(e, what, &error_); }
   int member_ok(int member) const;
   int ensure_points(uint64_t n_points);
 
   std::vector<Member> members_;
-  std::unique_ptr<Filter> map_;  // the map, the stream and the clusterizer scratch (sized for the largest member)
+  int device_{0};
+  cudaStream_t stream_{nullptr};
+  DeviceMap map_;
+  Clusterizer clusterizer_;  // sized for the largest member
   bool created_{false};
   int create_status_{BB200_OK};
   mutable std::string error_;

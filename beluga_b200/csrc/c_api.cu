@@ -113,6 +113,21 @@ void cloud_to_points(const bb200_point_cloud& c, double* points_xy) {
     points_xy[2 * i + 1] = py;
   }
 }
+
+/// Prepares the map's tables once and uploads them to every shard.  A failed preparation is reported by the first shard, as
+/// its own set_*_map call would.
+template <class Prepare>
+int set_sharded_map(bb200_sharded_amcl* g, Prepare&& prepare) {
+  g->error.clear();
+  return guarded(*g, [&] {
+    bb200::MapTables tables;
+    std::string message;
+    int st = prepare(&tables, &message);
+    if (st != BB200_OK) return g->ranks[0]->impl.filter().fail_with(st, message);
+    for (auto a = g->ranks.begin(); st == BB200_OK && a != g->ranks.end(); ++a) st = (*a)->impl.filter().set_map(tables);
+    return st;
+  });
+}
 }  // namespace
 
 extern "C" {
@@ -242,7 +257,7 @@ int bb200_systematic_comb(uint64_t seed, uint32_t step, uint64_t global_total, u
 int bb200_estimate_from_moments(const double moments[9], const double pivot_xy[2], bb200_estimate* out) {
   BB_REQUIRE(moments && pivot_xy && out);
   // Pure host arithmetic (estimation.hpp:436-475 from raw moments); needs no device.
-  bb200::Filter::estimate_from_moments_static(moments, pivot_xy, out);
+  bb200::estimate_from_moments(moments, pivot_xy, out);
   return BB200_OK;
 }
 int bb200_filter_set_stream(bb200_filter* f, void* cuda_stream) {
@@ -654,13 +669,14 @@ bb200_amcl* bb200_sharded_amcl_shard(bb200_sharded_amcl* g, int rank) {
     }                                                         \
     return static_cast<int>(BB200_OK);                        \
   })
+
 int bb200_sharded_amcl_set_likelihood_field_map(bb200_sharded_amcl* g, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid, int prob) {
-  BB_REQUIRE(p && grid);
-  BB_EACH_SHARD(a->impl.filter().set_likelihood_field_map(*p, *grid, prob != 0));
+  BB_REQUIRE(g && p && grid);
+  return set_sharded_map(g, [&](bb200::MapTables* t, std::string* e) { return bb200::prepare_likelihood_field_map(*p, *grid, prob != 0, t, e); });
 }
 int bb200_sharded_amcl_set_beam_map(bb200_sharded_amcl* g, const bb200_beam_param* p, const bb200_occupancy_grid* grid) {
-  BB_REQUIRE(p && grid);
-  BB_EACH_SHARD(a->impl.filter().set_beam_map(*p, *grid));
+  BB_REQUIRE(g && p && grid);
+  return set_sharded_map(g, [&](bb200::MapTables* t, std::string* e) { return bb200::prepare_beam_map(*p, *grid, t, e); });
 }
 int bb200_sharded_amcl_initialize(bb200_sharded_amcl* g, const double mean_xytheta[3], const double cov[9]) {
   BB_REQUIRE(mean_xytheta && cov);
@@ -754,7 +770,7 @@ int bb200_sharded_amcl_cluster_estimate(bb200_sharded_amcl* g, const bb200_clust
     static_assert(sizeof(bb200_cluster_cell) == sizeof(bb200::HostCell), "public and internal cell records must agree");
     const bb200::ClusterSelection sel = bb200::select_cluster(reinterpret_cast<const bb200::HostCell*>(merged.data()), n_merged, n_particles,
                                                               p->linear_hash_resolution, p->angular_hash_resolution, p->weight_cap_percentile);
-    bb200::Filter::estimate_from_moments_static(sel.moments, g->ranks[0]->impl.filter().pivot(), out);  // every shard accumulates about the same pivot
+    bb200::estimate_from_moments(sel.moments, g->ranks[0]->impl.filter().pivot(), out);  // every shard accumulates about the same pivot
     if (n_cells != nullptr) *n_cells = static_cast<uint32_t>(n_merged);
     if (n_clusters != nullptr) *n_clusters = sel.clusters;
     return static_cast<int>(BB200_OK);

@@ -8,6 +8,7 @@
 #include "cluster.cuh"
 
 #include <algorithm>
+#include <initializer_list>
 
 namespace bb200 {
 
@@ -272,5 +273,112 @@ void launch_cluster_records(const Pose2* states, const double* weights, const ui
   const unsigned cell_blocks = static_cast<unsigned>((static_cast<uint64_t>(cells) * kWarp + kCellThreads - 1) / kCellThreads);
   cluster_cells_kernel<<<cell_blocks, kCellThreads, 0, stream>>>(states, weights, s.hashes, sorted_idx, s.starts, cells, pivot_x, pivot_y, s.records);
 }
+
+// ---- Clusterizer -------------------------------------------------------------------------------------
+
+Clusterizer::~Clusterizer() {
+  for (void* p : std::initializer_list<void*>{s_.hashes, s_.keys, s_.first, s_.slot_of, s_.flags, s_.cell_of, s_.starts, s_.keys_a, s_.keys_b, s_.idx_a,
+                                              s_.idx_b, s_.histogram, s_.tile_state, s_.words, s_.records})
+    cudaFree(p);
+}
+
+int Clusterizer::ensure_scratch(uint32_t cells, std::string* error) {
+  auto check = [error](cudaError_t e, const char* what) { return cuda_check(e, what, error); };
+  ClusterScratch& c = s_;
+  if (c.hashes == nullptr) {
+    if (c.capacity >= (1ull << 31)) return reject(BB200_ERR_CAPACITY, "cluster estimate: more than 2^31 particles per filter", error);
+    uint64_t table = 2;
+    while (table < 2 * c.capacity) table <<= 1;
+    const uint32_t tiles = cluster_sort_tiles(c.capacity);
+    BB_CHECK(dev_alloc(&c.keys, table));
+    BB_CHECK(dev_alloc(&c.first, table));
+    BB_CHECK(dev_alloc(&c.slot_of, c.capacity));
+    BB_CHECK(dev_alloc(&c.flags, c.capacity));
+    BB_CHECK(dev_alloc(&c.cell_of, c.capacity));
+    BB_CHECK(dev_alloc(&c.starts, c.capacity + 1));
+    BB_CHECK(dev_alloc(&c.keys_a, c.capacity));
+    BB_CHECK(dev_alloc(&c.keys_b, c.capacity));
+    BB_CHECK(dev_alloc(&c.idx_a, c.capacity));
+    BB_CHECK(dev_alloc(&c.idx_b, c.capacity));
+    BB_CHECK(dev_alloc(&c.histogram, static_cast<size_t>(256) * tiles));
+    BB_CHECK(dev_alloc(&c.tile_state, static_cast<size_t>(scan_tile_count(std::max<uint64_t>(c.capacity + 1, 256ull * tiles)) + 1)));
+    BB_CHECK(dev_alloc(&c.words, 4));
+    BB_CHECK(dev_alloc(&c.hashes, c.capacity));  // last: marks the scratch as allocated
+    c.table_size = table;
+  }
+  if (cells > c.records_capacity) {
+    cudaFree(c.records);
+    c.records = nullptr;
+    c.records_capacity = 0;
+    const uint64_t want = std::min<uint64_t>(c.capacity, std::max<uint64_t>(1024, 2ull * cells));
+    BB_CHECK(dev_alloc(&c.records, want));
+    c.records_capacity = want;
+  }
+  return BB200_OK;
+}
+
+int Clusterizer::cell_records(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], double linear_resolution,
+                              double angular_resolution, cudaStream_t stream, std::vector<HostCell>* host, std::string* error) {
+  // spatial hash -> first-occurrence numbering of the occupied cells -> stable sort of the particle indices by cell -> one
+  // record per cell (representative = first particle, count, weight summed in particle order, raw moments).
+  auto check = [error](cudaError_t e, const char* what) { return cuda_check(e, what, error); };
+  auto stage = [this](const char* name) { if (mark) mark(name); };
+  {
+    const int st = ensure_scratch(0, error);
+    if (st != BB200_OK) return st;
+  }
+  stage("cluster_cells");
+  launch_cluster_cells_begin(states, n, linear_resolution, angular_resolution, s_, stream);
+  BB_LAUNCHED_N("cluster_cells_begin", 3);
+  unsigned long long cells64 = 0;
+  BB_CHECK(cudaMemcpyAsync(&cells64, s_.words + 1, sizeof(cells64), cudaMemcpyDeviceToHost, stream));
+  BB_CHECK(cudaStreamSynchronize(stream));
+  const uint32_t cells = static_cast<uint32_t>(cells64);
+  {
+    const int st = ensure_scratch(cells, error);
+    if (st != BB200_OK) return st;
+  }
+  stage("cluster_sort");
+  int sort_launches = 0;
+  const uint32_t* sorted = launch_cluster_sort(n, cells, s_, stream, &sort_launches);
+  BB_LAUNCHED_N("cluster_sort", sort_launches);
+  stage("cluster_records");
+  launch_cluster_records(states, weights, sorted, cells, pivot[0], pivot[1], s_, stream);
+  BB_LAUNCHED("cluster_records");
+  host->resize(cells);
+  static_assert(sizeof(HostCell) == sizeof(CellRecord), "record layouts must agree");
+  BB_CHECK(cudaMemcpyAsync(host->data(), s_.records, static_cast<size_t>(cells) * sizeof(CellRecord), cudaMemcpyDeviceToHost, stream));
+  BB_CHECK(cudaStreamSynchronize(stream));
+  stage("end");
+  return BB200_OK;
+}
+
+int Clusterizer::estimate(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], const bb200_cluster_param& p, cudaStream_t stream,
+                          bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells, uint32_t* n_clusters, std::string* error) {
+  auto check = [error](cudaError_t e, const char* what) { return cuda_check(e, what, error); };
+  if (n == 0) return reject(BB200_ERR_STATE, "no particles", error);
+  if (n > s_.capacity) return reject(BB200_ERR_CAPACITY, "cluster estimate: more particles than the scratch holds", error);
+  if (!(p.linear_hash_resolution > 0.0) || !(p.angular_hash_resolution > 0.0) || !(p.weight_cap_percentile >= 0.0) ||
+      !(p.weight_cap_percentile < 1.0))
+    return reject(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)", error);
+  if (cluster_ids != nullptr && ids_capacity < n) return reject(BB200_ERR_CAPACITY, "cluster id buffer too small", error);
+  std::vector<HostCell> host;
+  {
+    const int st = cell_records(states, weights, n, pivot, p.linear_hash_resolution, p.angular_hash_resolution, stream, &host, error);
+    if (st != BB200_OK) return st;
+  }
+  const uint32_t cells = static_cast<uint32_t>(host.size());
+  const ClusterSelection sel = select_cluster(host.data(), host.size(), n, p.linear_hash_resolution, p.angular_hash_resolution, p.weight_cap_percentile);
+  if (out != nullptr) estimate_from_moments(sel.moments, pivot, out);
+  if (n_cells != nullptr) *n_cells = cells;
+  if (n_clusters != nullptr) *n_clusters = sel.clusters;
+  if (cluster_ids != nullptr) {
+    std::vector<uint32_t> cell_of(n);
+    BB_CHECK(cudaMemcpy(cell_of.data(), s_.cell_of, n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    for (uint64_t i = 0; i < n; ++i) cluster_ids[i] = sel.cluster_of_cell[cell_of[i]];
+  }
+  return BB200_OK;
+}
+
 
 }  // namespace bb200

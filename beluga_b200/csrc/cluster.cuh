@@ -10,7 +10,11 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <functional>
+#include <string>
+#include <vector>
 
+#include "cluster_host.hpp"
 #include "kernels.cuh"
 
 namespace bb200 {
@@ -27,7 +31,7 @@ struct CellRecord {
 };
 static_assert(sizeof(CellRecord) == 128, "CellRecord is copied to the host as raw bytes");
 
-/// Scratch buffers of the clusterizer (owned by Filter, sized for `capacity` particles).
+/// Scratch buffers of the clusterizer (owned by Clusterizer, sized for `capacity` particles).
 struct ClusterScratch {
   uint64_t capacity{0};
   uint64_t table_size{0};              // power of two >= 2 * capacity
@@ -63,5 +67,35 @@ const uint32_t* launch_cluster_sort(uint64_t n, uint32_t cells, const ClusterScr
 /// One CellRecord per cell from the sorted indices.
 void launch_cluster_records(const Pose2* states, const double* weights, const uint32_t* sorted_idx, uint32_t cells, double pivot_x, double pivot_y,
                             const ClusterScratch& s, cudaStream_t stream);
+
+/// The clusterizer of a filter or a batch: scratch for up to `capacity` particles on one device, allocated on first use,
+/// run over any particle set of that size in that device's memory.  Every call works on the current device, ordered on
+/// `stream`, and returns a bb200_status with the message in *error.
+class Clusterizer {
+ public:
+  explicit Clusterizer(uint64_t capacity) { s_.capacity = capacity; }
+  ~Clusterizer();
+  Clusterizer(const Clusterizer&) = delete;
+  Clusterizer& operator=(const Clusterizer&) = delete;
+
+  /// Per-particle half of the clusterizer, also the device-side histogram of the particle cloud: one record per occupied
+  /// cell in first-occurrence order, raw moments about `pivot`, copied to *host.
+  int cell_records(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], double linear_resolution, double angular_resolution,
+                   cudaStream_t stream, std::vector<HostCell>* host, std::string* error);
+  /// beluga::cluster_based_estimate (algorithm/cluster_based_estimation.hpp:415-432) of the n particles, the moments taken
+  /// about `pivot`; cluster_ids (optional, one per particle) is the parity hook for ParticleClusterizer::operator() (:304-316).
+  int estimate(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], const bb200_cluster_param& p, cudaStream_t stream,
+               bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells, uint32_t* n_clusters, std::string* error);
+  uint64_t launches() const { return launches_; }
+
+  /// Called with each stage's timing label before its launches and with "end" after the last copy (a filter's timing marks).
+  std::function<void(const char*)> mark;
+
+ private:
+  int ensure_scratch(uint32_t cells, std::string* error);
+
+  ClusterScratch s_{};  // allocated once `hashes` is set
+  uint64_t launches_{0};
+};
 
 }  // namespace bb200

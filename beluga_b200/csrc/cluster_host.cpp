@@ -1,6 +1,8 @@
 #include "cluster_host.hpp"
 
 #include <algorithm>
+#include <cmath>
+#include <limits>
 #include <queue>
 #include <unordered_map>
 
@@ -118,6 +120,31 @@ ClusterSelection select_cluster(const HostCell* cells, std::size_t n_cells, std:
       for (int j = 0; j < 9; ++j) out.moments[j] += cells[k].moments[j];
   }
   return out;
+}
+
+void estimate_from_moments(const double m[9], const double pivot[2], bb200_estimate* out) {
+  // Normalised weights w/S: mean of (cos, sin, x, y); cov = (E[d d^T] - E[d] E[d]^T) / (1 - sum (w/S)^2).
+  const double sum = m[0];
+  const double mc = m[2] / sum, ms = m[3] / sum, mdx = m[4] / sum, mdy = m[5] / sum;
+  const double correction = 1.0 - m[1] / (sum * sum);
+  for (double& c : out->cov) c = 0.0;
+  out->cov[0] = (m[6] / sum - mdx * mdx) / correction;
+  out->cov[1] = (m[7] / sum - mdx * mdy) / correction;
+  out->cov[3] = out->cov[1];
+  out->cov[4] = (m[8] / sum - mdy * mdy) / correction;
+  out->mean[2] = pivot[0] + mdx;
+  out->mean[3] = pivot[1] + mdy;
+  const double norm = std::sqrt(mc * mc + ms * ms);
+  if (norm < std::numeric_limits<double>::epsilon()) {
+    out->cov[8] = std::numeric_limits<double>::infinity();
+    out->mean[0] = 1.0;
+    out->mean[1] = 0.0;
+  } else {
+    out->cov[8] = -2.0 * std::log(norm);
+    const double len = std::hypot(mc, ms);
+    out->mean[0] = mc / len;
+    out->mean[1] = ms / len;
+  }
 }
 
 }  // namespace bb200

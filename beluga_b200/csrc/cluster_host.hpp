@@ -8,6 +8,8 @@
 #include <cstdint>
 #include <vector>
 
+#include "../../include/beluga_b200.h"
+
 namespace bb200 {
 
 /// Host view of one device CellRecord (cluster.cuh), field for field.
@@ -33,5 +35,9 @@ struct ClusterSelection {
 /// n_particles sizes the map's initial reserve like make_cluster_map (:146).
 ClusterSelection select_cluster(const HostCell* cells, std::size_t n_cells, std::uint64_t n_particles, double linear_resolution,
                                 double angular_resolution, double weight_cap_percentile);
+
+/// Mean and covariance (estimation.hpp:436-475) from the nine raw moments about `pivot` (layout of kMomentCount in
+/// kernels.cuh): what every estimate ends with, of the whole set or of the selected cluster.
+void estimate_from_moments(const double m[9], const double pivot[2], bb200_estimate* out);
 
 }  // namespace bb200

@@ -1,0 +1,166 @@
+#include "device_map.hpp"
+
+#include <cmath>
+#include <cstring>
+
+#include "map_host.hpp"
+
+namespace bb200 {
+
+namespace {
+
+Pose2 pose_from_array(const double* d) { return Pose2{d[0], d[1], d[2], d[3]}; }
+
+/// Checks the grid and fills in what every sensor model has: the geometry and the free cells.
+int prepare_grid(const bb200_occupancy_grid& g, MapTables* t, std::string* error) {
+  if (g.cells == nullptr || g.width <= 0 || g.height <= 0 || !(g.resolution > 0.0)) return reject(BB200_ERR_INVALID_ARGUMENT, "invalid occupancy grid", error);
+  *t = MapTables{};
+  t->free_cells = make_free_cells(g);
+  t->n_free = t->free_cells.size();
+  t->grid_width = g.width;
+  t->grid_height = g.height;
+  t->grid_resolution = g.resolution;
+  t->grid_origin = pose_from_array(g.origin);
+  return BB200_OK;
+}
+
+}  // namespace
+
+int prepare_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& g, bool prob, MapTables* t, std::string* error) {
+  const int st = prepare_grid(g, t, error);
+  if (st != BB200_OK) return st;
+  if (!(p.sigma_hit > 0.0) || !(p.max_laser_distance > 0.0)) return reject(BB200_ERR_INVALID_ARGUMENT, "invalid likelihood field parameters", error);
+  const char* too_large = "map too large for 32-bit cell indices";
+  t->field_host = make_likelihood_field(p, g);
+  const size_t count = t->field_host.size();
+  if (count + 64 >= (1ull << 32)) return reject(BB200_ERR_CAPACITY, too_large, error);
+  // The lookup table the reweight kernel gathers from: f(pz) per cell as double, f = pz^3 (LikelihoodFieldModel) or
+  // log pz (LikelihoodFieldProbModel).  f is a pure function of the float cell value, so tabulating it is bit-identical to
+  // evaluating it per beam as likelihood_field_model.hpp:84-89 / likelihood_field_prob_model.hpp:84-86 do.
+  std::vector<double> table(count);  // row-major: the source of the layout the map's kernel reads
+  auto f = [prob](float pzf) {
+    const double pz = static_cast<double>(pzf);
+    return prob ? std::log(pz) : pz * pz * pz;
+  };
+  for (size_t i = 0; i < count; ++i) table[i] = f(t->field_host[i]);
+  const double unknown = f(static_cast<float>(1. / p.max_laser_distance));  // what out-of-grid end points read
+  FieldView& v = t->field;
+  if (g.width + 2 <= kFixedMaxSide && g.height + 2 <= kFixedMaxSide) {
+    // Bordered tile layout for the fixed-point kernel.
+    int kx = 0;
+    while ((1 << kx) < (g.width + 2 + 3) / 4) ++kx;
+    const size_t tile_rows = static_cast<size_t>((g.height + 2 + 3) / 4);
+    t->bordered.assign(tile_rows << (kx + 4), unknown);
+    for (int yi = 0; yi < g.height; ++yi)
+      for (int xi = 0; xi < g.width; ++xi)
+        t->bordered[bordered_index(static_cast<uint32_t>(xi + 1), static_cast<uint32_t>(yi + 1), kx)] = table[static_cast<size_t>(yi) * g.width + xi];
+    v.border_kx = kx;
+    v.border_pitch = 1u << kx;
+    v.border_x_max = static_cast<uint32_t>(4 * (g.width + 1) + 3);
+    v.border_y_max = static_cast<uint32_t>(g.height + 1);
+    v.use_fixed = 1;
+    t->bordered_bytes = t->bordered.size() * sizeof(double);
+  } else {
+    // Tiled layout (4x4-cell tiles, no border, spare cell at the end) for the general kernel.
+    const int tiles_x = (g.width + 3) / 4, tiles_y = (g.height + 3) / 4;
+    if (static_cast<size_t>(tiles_x) * tiles_y * 16 + 64 >= (1ull << 32)) return reject(BB200_ERR_CAPACITY, too_large, error);
+    t->tiled.assign(static_cast<size_t>(tiles_x) * tiles_y * 16 + 1, unknown);
+    for (int yi = 0; yi < g.height; ++yi)
+      for (int xi = 0; xi < g.width; ++xi) t->tiled[tiled_index(xi, yi, tiles_x)] = table[static_cast<size_t>(yi) * g.width + xi];
+    v.tiles_x = tiles_x;
+    v.spare_index = static_cast<uint32_t>(t->tiled.size() - 1);
+  }
+  v.width = g.width;
+  v.height = g.height;
+  v.inv_resolution = 1. / g.resolution;
+  v.unknown_value = unknown;
+  v.init = prob ? 0.0 : 1.0;
+  v.exp_epilogue = prob ? 1 : 0;
+  v.world_to_field = pose_inverse(pose_from_array(g.origin));
+  t->sensor = prob ? BB200_SENSOR_LIKELIHOOD_FIELD_PROB : BB200_SENSOR_LIKELIHOOD_FIELD;
+  return BB200_OK;
+}
+
+int prepare_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& g, MapTables* t, std::string* error) {
+  const int st = prepare_grid(g, t, error);
+  if (st != BB200_OK) return st;
+  t->cells.assign(g.cells, g.cells + static_cast<size_t>(g.width) * static_cast<size_t>(g.height));
+  t->free_distance = make_free_distance(g);
+  OccupancyView& v = t->occupancy;
+  // padded copy for the two-pass walk: a border of zeros, power-of-two pitch
+  int shift = 1;
+  while ((1 << shift) < g.width + 2) ++shift;
+  if (shift <= 16 && g.height <= 65535) {
+    t->free_padded.assign((static_cast<size_t>(g.height) + 2) << shift, 0);
+    for (int y = 0; y < g.height; ++y)
+      std::memcpy(t->free_padded.data() + ((static_cast<size_t>(y) + 1) << shift) + 1, t->free_distance.data() + static_cast<size_t>(y) * g.width,
+                  static_cast<size_t>(g.width));
+    v.pad_shift = shift;
+  }
+  v.width = g.width;
+  v.height = g.height;
+  v.resolution = g.resolution;
+  v.inv_resolution = 1. / g.resolution;
+  v.world_to_grid = pose_inverse(pose_from_array(g.origin));
+  t->beam = BeamParams{p.z_hit, p.z_short, p.z_max, p.z_rand, p.sigma_hit, p.lambda_short, p.beam_max_range, nullptr, 0};
+  t->sensor = BB200_SENSOR_BEAM;
+  return BB200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+
+void DeviceMap::release() {
+  for (void* p : buffers_) cudaFree(p);
+  buffers_.clear();
+  static_cast<MapLayout&>(*this) = MapLayout{};
+  field_host.clear();
+  free_cells = nullptr;
+}
+
+template <class T>
+cudaError_t DeviceMap::copy(const std::vector<T>& v, const T** out, cudaStream_t stream) {
+  T* p = nullptr;
+  *out = nullptr;
+  if (v.empty()) return cudaSuccess;
+  if (const cudaError_t e = dev_alloc(&p, v.size())) return e;
+  buffers_.push_back(p);
+  *out = p;
+  return cudaMemcpyAsync(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, stream);
+}
+
+int DeviceMap::upload(const MapTables& t, cudaStream_t stream, std::string* error) {
+  auto check = [error](cudaError_t e, const char* what) { return cuda_check(e, what, error); };
+  BB_CHECK(cudaStreamSynchronize(stream));  // nothing in flight reads the old tables any more
+  release();
+  static_cast<MapLayout&>(*this) = t;
+  sensor = -1;  // until every table is in place
+  BB_CHECK(copy(t.bordered, &field.bordered, stream));
+  BB_CHECK(copy(t.tiled, &field.tiled, stream));
+  BB_CHECK(copy(t.cells, &occupancy.cells, stream));
+  BB_CHECK(copy(t.free_distance, &occupancy.free_distance, stream));
+  BB_CHECK(copy(t.free_padded, &occupancy.free_padded, stream));
+  BB_CHECK(copy(t.free_cells, &free_cells, stream));
+  if (t.sensor == BB200_SENSOR_BEAM) {
+    if (const uint32_t entries = beam_eta_entries(beam.beam_max_range, grid_resolution)) {
+      double2* eta = nullptr;
+      BB_CHECK(dev_alloc(&eta, entries));
+      buffers_.push_back(eta);
+      launch_beam_eta_table(beam, grid_resolution, eta, entries, stream);
+      BB_LAUNCHED("beam_eta_table");
+      beam.eta = eta;
+      beam.eta_entries = entries;
+    }
+  }
+  BB_CHECK(cudaStreamSynchronize(stream));  // the host tables may go once this returns
+  field_host = t.field_host;
+  sensor = t.sensor;
+  return BB200_OK;
+}
+
+void DeviceMap::centre(double pivot[2]) const {
+  const double cx = 0.5 * grid_width * grid_resolution, cy = 0.5 * grid_height * grid_resolution;
+  pivot[0] = (grid_origin.c * cx - grid_origin.s * cy) + grid_origin.x;
+  pivot[1] = (grid_origin.s * cx + grid_origin.c * cy) + grid_origin.y;
+}
+
+}  // namespace bb200

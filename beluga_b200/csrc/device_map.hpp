@@ -1,0 +1,72 @@
+// The map a sensor model reads, in two halves: MapTables, prepared on the host once per map without touching a device,
+// and DeviceMap, one device's copy of those tables.  A filter holds one DeviceMap, a batch holds one for all its members,
+// and a sharded filter prepares the tables once and uploads them to every shard.
+#pragma once
+
+#include <cstdint>
+#include <string>
+#include <vector>
+
+#include "kernels.cuh"
+
+namespace bb200 {
+
+/// What the kernels are handed: the sensor model, its views and the grid geometry.  The views' device pointers are null
+/// in MapTables and set in DeviceMap.
+struct MapLayout {
+  int sensor{-1};  // -1: no map yet
+  FieldView field{};
+  OccupancyView occupancy{};
+  BeamParams beam{};
+  int grid_width{0}, grid_height{0};
+  double grid_resolution{1.0};
+  Pose2 grid_origin{1.0, 0.0, 0.0, 0.0};
+  uint64_t n_free{0};          // free cells
+  uint64_t bordered_bytes{0};  // size of the bordered table
+};
+
+/// Everything the device copy of a map is made from.
+struct MapTables : MapLayout {
+  std::vector<float> field_host;  // likelihood field (get_likelihood_field); empty for the beam model
+  std::vector<double> bordered;   // f(pz) in the bordered layout of the fixed-point kernel (maps up to kFixedMaxSide) ...
+  std::vector<double> tiled;      // ... or in the tiled layout of the general kernel
+  std::vector<int8_t> cells;      // beam model: the grid, its free distance and the padded copy of that
+  std::vector<uint8_t> free_distance;
+  std::vector<uint8_t> free_padded;
+  std::vector<uint32_t> free_cells;  // recovery injection and initialize_from_map
+};
+
+/// Host preparation of a likelihood-field map (LikelihoodFieldModel, or LikelihoodFieldProbModel when prob).  Returns a
+/// bb200_status; on failure *error holds the message.
+int prepare_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob, MapTables* out,
+                                 std::string* error);
+/// Host preparation of a beam-model map.
+int prepare_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid, MapTables* out, std::string* error);
+
+/// One device's copy of the current map.
+struct DeviceMap : MapLayout {
+  DeviceMap() = default;
+  ~DeviceMap() { release(); }
+  DeviceMap(const DeviceMap&) = delete;
+  DeviceMap& operator=(const DeviceMap&) = delete;
+
+  /// Replaces the map with `t` on the current device: waits for `stream`, copies the tables and, for the beam model,
+  /// builds the normaliser table there.  Returns a bb200_status; on failure *error holds the message.
+  int upload(const MapTables& t, cudaStream_t stream, std::string* error);
+  /// The middle of the map in the global frame: the pivot of the raw moments after initialize_from_map.
+  void centre(double pivot[2]) const;
+  uint64_t launches() const { return launches_; }  // the beam model's normaliser tables
+
+  std::vector<float> field_host;
+  const uint32_t* free_cells{nullptr};
+
+ private:
+  void release();
+  template <class T>
+  cudaError_t copy(const std::vector<T>& v, const T** out, cudaStream_t stream);
+
+  std::vector<void*> buffers_;  // every device allocation of the current map
+  uint64_t launches_{0};
+};
+
+}  // namespace bb200

@@ -4,23 +4,11 @@
 #include <atomic>
 #include <cmath>
 #include <cstring>
-#include <limits>
+#include <initializer_list>
 
 #include "cluster_host.hpp"
-#include "map_host.hpp"
 
 namespace bb200 {
-
-namespace {
-
-template <class T>
-cudaError_t dev_alloc(T** p, size_t count) {
-  return cudaMalloc(reinterpret_cast<void**>(p), std::max<size_t>(count, 1) * sizeof(T));
-}
-
-Pose2 pose_from_array(const double* d) { return Pose2{d[0], d[1], d[2], d[3]}; }
-
-}  // namespace
 
 MotionSampling to_kernel_sampling(const bb200_motion_sampling& s) {
   MotionSampling m{};
@@ -89,18 +77,36 @@ bool normal_transform(const double cov[9], double transform[9], std::string* err
   return true;
 }
 
+int check_device(int device, std::string* error) {
+  int count = 0;
+  if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0)
+    return reject(BB200_ERR_NO_DEVICE, "no CUDA device available (this backend has no CPU fallback)", error);
+  if (device < 0 || device >= count) return reject(BB200_ERR_INVALID_ARGUMENT, "device ordinal out of range", error);
+  return BB200_OK;
+}
+
+double scan_radius(const double* points_xy, uint64_t n_points) {
+  double radius = 0.0;
+  for (uint64_t i = 0; i < n_points; ++i) {
+    const double r = std::fabs(points_xy[2 * i]) + std::fabs(points_xy[2 * i + 1]);
+    radius = (r > radius || std::isnan(r)) ? r : radius;
+  }
+  return radius;
+}
+
+bool wait_for_ticket(const volatile int* word, int ticket, cudaStream_t stream) {
+  for (uint32_t spins = 1; *word != ticket; ++spins)
+    if ((spins & 0x3fffu) == 0 && cudaStreamQuery(stream) != cudaErrorNotReady) return false;  // ended without it, or failed
+  std::atomic_thread_fence(std::memory_order_acquire);
+  return true;
+}
+
 // ---------------------------------------------------------------------------------------------------
 
-Filter::Filter(const bb200_filter_config& config) : config_(config) {
-  int count = 0;
-  if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
-    create_status_ = fail(BB200_ERR_NO_DEVICE, "no CUDA device available (this backend has no CPU fallback)");
-    return;
-  }
-  if (config.device < 0 || config.device >= count) {
-    create_status_ = fail(BB200_ERR_INVALID_ARGUMENT, "device ordinal out of range");
-    return;
-  }
+Filter::Filter(const bb200_filter_config& config) : config_(config), cluster_(config.capacity) {
+  cluster_.mark = [this](const char* name) { mark(name); };
+  create_status_ = check_device(config.device, &error_);
+  if (create_status_ != BB200_OK) return;
   if (config.capacity == 0) {
     create_status_ = fail(BB200_ERR_INVALID_ARGUMENT, "capacity must be positive");
     return;
@@ -108,14 +114,6 @@ Filter::Filter(const bb200_filter_config& config) : config_(config) {
   if (config_.global_count == 0) config_.global_count = config_.capacity;
   capacity_ = config.capacity;
   first_index_ = config.first_index;
-#define BB_TRY(expr)                                \
-  do {                                              \
-    const int st = check((expr), #expr);            \
-    if (st != BB200_OK) {                           \
-      create_status_ = st;                          \
-      return;                                       \
-    }                                               \
-  } while (0)
   BB_TRY(cudaSetDevice(config.device));
   BB_TRY(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
   BB_TRY(dev_alloc(&states_[0], capacity_));
@@ -146,7 +144,6 @@ Filter::Filter(const bb200_filter_config& config) : config_(config) {
   BB_TRY(cudaMemsetAsync(summary_, 0, sizeof(StepSummary), stream_));
   BB_TRY(cudaMemsetAsync(scalars_, 0, sizeof(Scalars), stream_));
   BB_TRY(cudaStreamSynchronize(stream_));
-#undef BB_TRY
   global_size_ = config_.global_count;
   created_ = true;
 }
@@ -155,84 +152,13 @@ Filter::~Filter() {
   if (stream_ != nullptr) cudaStreamSynchronize(stream_);
   release_peers();
   for (auto& e : event_pool_) cudaEventDestroy(e);
-  cudaFree(mail_);
-  cudaFree(shard_totals_);
-  cudaFree(summary_);
-  cudaFreeHost(summary_host_);
-  cudaFree(states_[0]);
-  cudaFree(states_[1]);
-  cudaFree(weights_);
-  cudaFree(cdf_);
-  cudaFree(ancestors_);
-  cudaFree(hashes_);
-  cudaFree(scalars_);
-  cudaFree(sched_);
-  cudaFree(bins_);
-  cudaFree(bin_rank_);
-  cudaFree(perm_);
-  cudaFree(counters_);
-  cudaFree(sched_tiles_);
-  cudaFreeHost(scalars_host_);
-  cudaFree(tile_state_);
-  cudaFree(partials_);
-  cudaFree(results_);
-  cudaFreeHost(results_host_);
-  cudaFree(cluster_.hashes);
-  cudaFree(cluster_.keys);
-  cudaFree(cluster_.first);
-  cudaFree(cluster_.slot_of);
-  cudaFree(cluster_.flags);
-  cudaFree(cluster_.cell_of);
-  cudaFree(cluster_.starts);
-  cudaFree(cluster_.keys_a);
-  cudaFree(cluster_.keys_b);
-  cudaFree(cluster_.idx_a);
-  cudaFree(cluster_.idx_b);
-  cudaFree(cluster_.histogram);
-  cudaFree(cluster_.tile_state);
-  cudaFree(cluster_.words);
-  cudaFree(cluster_.records);
-  cudaFree(kld_keys_);
-  cudaFree(kld_vals_);
-  cudaFree(kld_flags_);
-  cudaFree(kld_scan_);
-  cudaFree(kld_tile_state_);
-  cudaFree(kld_hashes_global_);
-  cudaFree(points_);
-  cudaFreeHost(points_host_);
-  cudaFree(tiled_);
-  cudaFree(bordered_);
-  cudaFree(beam_eta_);
-  cudaFree(beam_hits_);
-  cudaFree(free_padded_);
-  cudaFree(occupancy_);
-  cudaFree(free_distance_);
-  cudaFree(free_cells_);
+  for (void* p : std::initializer_list<void*>{mail_, shard_totals_, summary_, states_[0], states_[1], weights_, cdf_, ancestors_, hashes_, scalars_,
+                                              sched_, bins_, bin_rank_, perm_, counters_, sched_tiles_, tile_state_, partials_, results_, kld_keys_,
+                                              kld_vals_, kld_flags_, kld_scan_, kld_tile_state_, kld_hashes_global_, points_, beam_hits_})
+    cudaFree(p);
+  for (void* p : std::initializer_list<void*>{summary_host_, scalars_host_, results_host_, points_host_}) cudaFreeHost(p);
   if (stream_ != nullptr && owns_stream_) cudaStreamDestroy(stream_);
 }
-
-int Filter::fail(int status, const std::string& message) {
-  error_ = message;
-  return status;
-}
-
-int Filter::check(cudaError_t e, const char* what) {
-  if (e == cudaSuccess) return BB200_OK;
-  return fail(BB200_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-}
-
-#define BB_CHECK(expr)                          \
-  do {                                          \
-    const int st_ = check((expr), #expr);       \
-    if (st_ != BB200_OK) return st_;            \
-  } while (0)
-#define BB_LAUNCHED_N(name, count)                          \
-  do {                                                      \
-    launches_ += (count);                                   \
-    const int st_ = check(cudaGetLastError(), name);        \
-    if (st_ != BB200_OK) return st_;                        \
-  } while (0)
-#define BB_LAUNCHED(name) BB_LAUNCHED_N(name, 1)
 
 void Filter::mark(const char* name) {
   if (!timing_) return;
@@ -288,7 +214,7 @@ int Filter::enqueue_propagate_reweight(const bb200_motion_sampling* sampling, ui
   // since the previous upload.
   if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
   const bool do_reweight = points_xy != nullptr;
-  if (do_reweight && sensor_ < 0) return fail(BB200_ERR_STATE, "no sensor model map set");
+  if (do_reweight && map_.sensor < 0) return fail(BB200_ERR_STATE, "no sensor model map set");
   if (do_reweight && n_points > 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, "too many points");
   BB_CHECK(cudaSetDevice(config_.device));
   if (do_reweight) {
@@ -335,7 +261,7 @@ int Filter::enqueue_resample_range(const bb200_resample_opts& o, uint64_t global
   if (!cdf_valid_) return fail(BB200_ERR_STATE, "build_cdf must run before resample_range");
   if (o.scheme != BB200_RESAMPLE_SYSTEMATIC || o.min_particles < o.max_particles)
     return fail(BB200_ERR_STATE, "range resampling supports the systematic comb without KLD (multinomial or KLD on shards: bb200_amcl_join_shards / bb200_sharded_amcl)");
-  if (o.random_state_probability > 0.0 && n_free_ == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
+  if (o.random_state_probability > 0.0 && map_.n_free == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
   if (slot_end < slot_begin || slot_end - slot_begin > capacity_) return fail(BB200_ERR_CAPACITY, "slot range exceeds the staging buffer");
   BB_CHECK(cudaSetDevice(config_.device));
   if (slot_end > slot_begin) {
@@ -535,10 +461,10 @@ int Filter::step_begin(const bb200_motion_sampling& sampling, uint32_t step, con
   const uint64_t world = peer_world_ > 1 ? static_cast<uint64_t>(peer_world_) : 1;
   const bool kld = o.min_particles < o.max_particles;
   if (n_ == 0 && !(world > 1 && shard_kld_)) return fail(BB200_ERR_STATE, "no particles");  // a KLD-sized filter may leave a shard empty
-  if (sensor_ < 0) return fail(BB200_ERR_STATE, "no sensor model map set");
+  if (map_.sensor < 0) return fail(BB200_ERR_STATE, "no sensor model map set");
   if (kld && !(world > 1 && shard_kld_)) return fail(BB200_ERR_STATE, "the fused step does not run KLD on one GPU; use resample()");
   if (n_points > 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, "too many points");
-  if (o.random_state_probability > 0.0 && n_free_ == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
+  if (o.random_state_probability > 0.0 && map_.n_free == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
   if (world > 1) {
     if ((!shard_kld_ && n_ != capacity_) || n_ > capacity_ || o.max_particles != world * capacity_)
       return fail(BB200_ERR_STATE, "a sharded filter keeps `capacity` particles on every rank (fewer only under KLD)");
@@ -572,9 +498,9 @@ int Filter::step_phase(int phase) {
       mark("begin_step");
       {
         const bool scheduled = n_ >= kScheduleMinParticles;
-        const bool warm = sensor_ != BB200_SENSOR_BEAM && field_.use_fixed && bordered_bytes_ <= (96ull << 20);
+        const bool warm = map_.sensor != BB200_SENSOR_BEAM && map_.field.use_fixed && map_.bordered_bytes <= (96ull << 20);
         launch_begin_fused_step(scalars_, tile_state_, scan_tile_count(n_), sched_, scheduled ? counters_ : nullptr, schedule_max_bins(), sched_tiles_,
-                                schedule_tile_count(), warm ? bordered_ : nullptr, bordered_bytes_, stream_);
+                                schedule_tile_count(), warm ? map_.field.bordered : nullptr, map_.bordered_bytes, stream_);
         BB_LAUNCHED("begin_step");
         st = enqueue_propagate_reweight_kernels(&step_.sampling, step_.step, true, step_.n_points, scheduled);
       }
@@ -806,23 +732,9 @@ void Filter::step_set_kld_accepted(uint64_t accepted) { step_.kld_accepted = acc
 int Filter::step_end(bb200_estimate* est, double* weight_sum, uint64_t* new_size, double* sum_sq) {
   if (!step_.active) return fail(BB200_ERR_STATE, "step_begin must run first");
   BB_CHECK(cudaSetDevice(config_.device));
-  bool done = false;
-  if (step_.poll_seq != 0 && step_.resampled) {
-    // The resample kernel's last block stored the summary to pinned memory and then the step's ticket: spinning on that
-    // word sees the end of the step a few microseconds before a stream synchronisation returns.  Everything later on this
-    // stream is ordered behind the kernel anyway.  The stream is queried now and then so that a failed launch cannot hang us.
-    const volatile int* seq = &summary_host_->seq;
-    for (uint32_t spins = 1; !done; ++spins) {
-      if (*seq == step_.poll_seq) {
-        done = true;
-      } else if ((spins & 0x3fffu) == 0) {
-        const cudaError_t q = cudaStreamQuery(stream_);
-        if (q == cudaSuccess) break;  // finished: the ticket is there (or the plain path below reports what went wrong)
-        if (q != cudaErrorNotReady) break;
-      }
-    }
-    std::atomic_thread_fence(std::memory_order_acquire);
-  }
+  // The resample kernel's last block stores the summary to pinned memory and then the step's ticket.  Everything later on
+  // this stream is ordered behind that kernel anyway.
+  const bool done = step_.poll_seq != 0 && step_.resampled && wait_for_ticket(&summary_host_->seq, step_.poll_seq, stream_);
   if (!done) BB_CHECK(cudaStreamSynchronize(stream_));
   step_.poll_seq = 0;
   finish_marks();
@@ -860,7 +772,7 @@ int Filter::step_end(bb200_estimate* est, double* weight_sum, uint64_t* new_size
   if (!weights_valid_) error_ = "no positive finite weight (uniform CDF substituted)";
   bb200_estimate local{};
   if (est == nullptr) est = &local;
-  estimate_from_moments(moments, est);
+  estimate_from_moments(moments, pivot_, est);
   pivot_[0] = est->mean[2];
   pivot_[1] = est->mean[3];
   cloud_ = *est;
@@ -890,155 +802,27 @@ int Filter::device_pointer(int which, void** ptr, uint64_t* bytes) {
 // ---- maps -----------------------------------------------------------------------------------------
 
 int Filter::set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& g, bool prob) {
-  if (g.cells == nullptr || g.width <= 0 || g.height <= 0 || !(g.resolution > 0.0)) return fail(BB200_ERR_INVALID_ARGUMENT, "invalid occupancy grid");
-  if (!(p.sigma_hit > 0.0) || !(p.max_laser_distance > 0.0)) return fail(BB200_ERR_INVALID_ARGUMENT, "invalid likelihood field parameters");
-  BB_CHECK(cudaSetDevice(config_.device));
-  field_host_ = make_likelihood_field(p, g);
-  const size_t count = field_host_.size();
-  // Per-cell f(pz) in double: pz^3 (likelihood_field_model.hpp:84-89) or log pz (prob model :84-86).
-  if (count + 64 >= (1ull << 32)) return fail(BB200_ERR_CAPACITY, "map too large for 32-bit cell indices");
-  std::vector<double> table(count);  // row-major: the source of the layout the map's kernel reads
-  auto f = [prob](float pzf) {
-    const double pz = static_cast<double>(pzf);
-    return prob ? std::log(pz) : pz * pz * pz;
-  };
-  for (size_t i = 0; i < count; ++i) table[i] = f(field_host_[i]);
-  const double unknown = f(static_cast<float>(1. / p.max_laser_distance));  // what out-of-grid end points read
-  BB_CHECK(cudaStreamSynchronize(stream_));
-  field_.use_fixed = 0;
-  field_.bordered = nullptr;
-  field_.tiled = nullptr;
-  cudaFree(bordered_);
-  bordered_ = nullptr;
-  cudaFree(tiled_);
-  tiled_ = nullptr;
-  if (g.width + 2 <= kFixedMaxSide && g.height + 2 <= kFixedMaxSide) {
-    // Bordered tile layout for the fixed-point kernel.
-    int kx = 0;
-    while ((1 << kx) < (g.width + 2 + 3) / 4) ++kx;
-    const size_t tile_rows = static_cast<size_t>((g.height + 2 + 3) / 4);
-    std::vector<double> bordered((tile_rows << (kx + 4)), unknown);
-    for (int yi = 0; yi < g.height; ++yi)
-      for (int xi = 0; xi < g.width; ++xi)
-        bordered[bordered_index(static_cast<uint32_t>(xi + 1), static_cast<uint32_t>(yi + 1), kx)] = table[static_cast<size_t>(yi) * g.width + xi];
-    BB_CHECK(dev_alloc(&bordered_, bordered.size()));
-    bordered_bytes_ = bordered.size() * sizeof(double);
-    BB_CHECK(cudaMemcpyAsync(bordered_, bordered.data(), bordered.size() * sizeof(double), cudaMemcpyHostToDevice, stream_));
-    BB_CHECK(cudaStreamSynchronize(stream_));
-    field_.bordered = bordered_;
-    field_.border_kx = kx;
-    field_.border_pitch = 1u << kx;
-    field_.border_x_max = static_cast<uint32_t>(4 * (g.width + 1) + 3);
-    field_.border_y_max = static_cast<uint32_t>(g.height + 1);
-    field_.use_fixed = 1;
-  } else {
-    // Tiled layout (4x4-cell tiles, no border, spare cell at the end) for the general kernel.
-    const int tiles_x = (g.width + 3) / 4, tiles_y = (g.height + 3) / 4;
-    if (static_cast<size_t>(tiles_x) * tiles_y * 16 + 64 >= (1ull << 32)) return fail(BB200_ERR_CAPACITY, "map too large for 32-bit cell indices");
-    std::vector<double> tiled(static_cast<size_t>(tiles_x) * tiles_y * 16 + 1, unknown);
-    for (int yi = 0; yi < g.height; ++yi)
-      for (int xi = 0; xi < g.width; ++xi) tiled[tiled_index(xi, yi, tiles_x)] = table[static_cast<size_t>(yi) * g.width + xi];
-    BB_CHECK(dev_alloc(&tiled_, tiled.size()));
-    BB_CHECK(cudaMemcpyAsync(tiled_, tiled.data(), tiled.size() * sizeof(double), cudaMemcpyHostToDevice, stream_));
-    BB_CHECK(cudaStreamSynchronize(stream_));
-    field_.tiled = tiled_;
-    field_.tiles_x = tiles_x;
-    field_.spare_index = static_cast<uint32_t>(tiled.size() - 1);
-  }
-  field_.width = g.width;
-  field_.height = g.height;
-  field_.inv_resolution = 1. / g.resolution;
-  field_.unknown_value = unknown;
-  field_.init = prob ? 0.0 : 1.0;
-  field_.exp_epilogue = prob ? 1 : 0;
-  field_.world_to_field = pose_inverse(pose_from_array(g.origin));
-  sensor_ = prob ? BB200_SENSOR_LIKELIHOOD_FIELD_PROB : BB200_SENSOR_LIKELIHOOD_FIELD;
-
-  // Free cells for the recovery random-state generator.
-  const std::vector<uint32_t> free = make_free_cells(g);
-  cudaFree(free_cells_);
-  free_cells_ = nullptr;
-  n_free_ = free.size();
-  BB_CHECK(dev_alloc(&free_cells_, free.size()));
-  if (!free.empty()) BB_CHECK(cudaMemcpy(free_cells_, free.data(), free.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-  grid_width_ = g.width;
-  grid_height_ = g.height;
-  grid_resolution_ = g.resolution;
-  grid_origin_ = pose_from_array(g.origin);
-  return BB200_OK;
+  MapTables tables;
+  const int st = prepare_likelihood_field_map(p, g, prob, &tables, &error_);
+  return st != BB200_OK ? st : set_map(tables);
 }
 
 int Filter::set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& g) {
-  if (g.cells == nullptr || g.width <= 0 || g.height <= 0 || !(g.resolution > 0.0)) return fail(BB200_ERR_INVALID_ARGUMENT, "invalid occupancy grid");
-  BB_CHECK(cudaSetDevice(config_.device));
-  const size_t count = static_cast<size_t>(g.width) * static_cast<size_t>(g.height);
-  BB_CHECK(cudaStreamSynchronize(stream_));
-  cudaFree(occupancy_);
-  occupancy_ = nullptr;
-  BB_CHECK(dev_alloc(&occupancy_, count));
-  BB_CHECK(cudaMemcpy(occupancy_, g.cells, count, cudaMemcpyHostToDevice));
-  const std::vector<uint8_t> free_distance = make_free_distance(g);
-  cudaFree(free_distance_);
-  free_distance_ = nullptr;
-  BB_CHECK(dev_alloc(&free_distance_, count));
-  BB_CHECK(cudaMemcpy(free_distance_, free_distance.data(), count, cudaMemcpyHostToDevice));
-  // padded copy for the two-pass walk: a border of zeros, power-of-two pitch
-  cudaFree(free_padded_);
-  free_padded_ = nullptr;
-  occupancy_view_.free_padded = nullptr;
-  occupancy_view_.pad_shift = 0;
-  {
-    int shift = 1;
-    while ((1 << shift) < g.width + 2) ++shift;
-    const size_t rows = static_cast<size_t>(g.height) + 2;
-    if (shift <= 16 && g.height <= 65535) {
-      std::vector<uint8_t> padded(rows << shift, 0);
-      for (int y = 0; y < g.height; ++y)
-        std::memcpy(padded.data() + ((static_cast<size_t>(y) + 1) << shift) + 1, free_distance.data() + static_cast<size_t>(y) * g.width, static_cast<size_t>(g.width));
-      BB_CHECK(dev_alloc(&free_padded_, padded.size()));
-      BB_CHECK(cudaMemcpy(free_padded_, padded.data(), padded.size(), cudaMemcpyHostToDevice));
-      occupancy_view_.free_padded = free_padded_;
-      occupancy_view_.pad_shift = shift;
-    }
-  }
-  occupancy_view_.cells = occupancy_;
-  occupancy_view_.free_distance = free_distance_;
-  occupancy_view_.width = g.width;
-  occupancy_view_.height = g.height;
-  occupancy_view_.resolution = g.resolution;
-  occupancy_view_.inv_resolution = 1. / g.resolution;
-  occupancy_view_.world_to_grid = pose_inverse(pose_from_array(g.origin));
-  beam_ = BeamParams{p.z_hit, p.z_short, p.z_max, p.z_rand, p.sigma_hit, p.lambda_short, p.beam_max_range, nullptr, 0};
-  cudaFree(beam_eta_);
-  beam_eta_ = nullptr;
-  if (const uint32_t entries = beam_eta_entries(p.beam_max_range, g.resolution)) {
-    BB_CHECK(dev_alloc(&beam_eta_, entries));
-    launch_beam_eta_table(beam_, g.resolution, beam_eta_, entries, stream_);
-    BB_LAUNCHED("beam_eta_table");
-    BB_CHECK(cudaStreamSynchronize(stream_));
-    beam_.eta = beam_eta_;
-    beam_.eta_entries = entries;
-  }
-  sensor_ = BB200_SENSOR_BEAM;
-  field_host_.clear();
+  MapTables tables;
+  const int st = prepare_beam_map(p, g, &tables, &error_);
+  return st != BB200_OK ? st : set_map(tables);
+}
 
-  const std::vector<uint32_t> free = make_free_cells(g);
-  cudaFree(free_cells_);
-  free_cells_ = nullptr;
-  n_free_ = free.size();
-  BB_CHECK(dev_alloc(&free_cells_, free.size()));
-  if (!free.empty()) BB_CHECK(cudaMemcpy(free_cells_, free.data(), free.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-  grid_width_ = g.width;
-  grid_height_ = g.height;
-  grid_resolution_ = g.resolution;
-  grid_origin_ = pose_from_array(g.origin);
-  return BB200_OK;
+int Filter::set_map(const MapTables& tables) {
+  BB_CHECK(cudaSetDevice(config_.device));
+  return map_.upload(tables, stream_, &error_);
 }
 
 int Filter::get_likelihood_field(float* out, uint64_t capacity) const {
-  if (field_host_.empty()) return BB200_ERR_STATE;
-  if (capacity < field_host_.size()) return BB200_ERR_CAPACITY;
-  std::memcpy(out, field_host_.data(), field_host_.size() * sizeof(float));
+  const std::vector<float>& field = map_.field_host;
+  if (field.empty()) return BB200_ERR_STATE;
+  if (capacity < field.size()) return BB200_ERR_CAPACITY;
+  std::memcpy(out, field.data(), field.size() * sizeof(float));
   return BB200_OK;
 }
 
@@ -1100,20 +884,17 @@ int Filter::initialize_normal(const double mean[3], const double cov[9], uint64_
 
 int Filter::initialize_uniform(uint64_t n) {
   if (n > capacity_) return fail(BB200_ERR_CAPACITY, "more particles than the filter capacity");
-  if (sensor_ < 0) return fail(BB200_ERR_STATE, "initialize_from_map needs a map (set_*_map first)");
-  if (n_free_ == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
+  if (map_.sensor < 0) return fail(BB200_ERR_STATE, "initialize_from_map needs a map (set_*_map first)");
+  if (map_.n_free == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
   BB_CHECK(cudaSetDevice(config_.device));
-  launch_initialize_uniform(states_[cur_], weights_, n, free_cells_, n_free_, grid_width_, grid_resolution_, grid_origin_, config_.seed,
-                            first_index_, stream_);
+  launch_initialize_uniform(states_[cur_], weights_, n, map_.free_cells, map_.n_free, map_.grid_width, map_.grid_resolution, map_.grid_origin,
+                            config_.seed, first_index_, stream_);
   BB_LAUNCHED("initialize_uniform");
   BB_CHECK(cudaStreamSynchronize(stream_));
   n_ = n;
   cdf_valid_ = false;
   cloud_known_ = false;
-  // pivot of the raw moments: the middle of the map in the global frame
-  const double cx = 0.5 * grid_width_ * grid_resolution_, cy = 0.5 * grid_height_ * grid_resolution_;
-  pivot_[0] = (grid_origin_.c * cx - grid_origin_.s * cy) + grid_origin_.x;
-  pivot_[1] = (grid_origin_.s * cx + grid_origin_.c * cy) + grid_origin_.y;
+  map_.centre(pivot_);
   return BB200_OK;
 }
 
@@ -1121,24 +902,17 @@ int Filter::initialize_uniform(uint64_t n) {
 
 int Filter::upload_points(const double* points_xy, uint64_t n_points) {
   if (n_points > points_capacity_) {
-    cudaFree(points_);
-    cudaFreeHost(points_host_);
-    points_ = nullptr;
-    points_host_ = nullptr;
     points_capacity_ = 0;
     const uint64_t cap = std::max<uint64_t>(n_points, 2048);
-    BB_CHECK(dev_alloc(&points_, 2 * cap));
-    BB_CHECK(cudaMallocHost(reinterpret_cast<void**>(&points_host_), 2 * cap * sizeof(double)));
+    BB_CHECK(realloc_staged(&points_, &points_host_, 2 * cap));
     points_capacity_ = cap;
   }
-  double radius = 0.0, range_sum = 0.0;
+  double range_sum = 0.0;
   for (uint64_t i = 0; i < n_points; ++i) {
-    const double r = std::fabs(points_xy[2 * i]) + std::fabs(points_xy[2 * i + 1]);
-    radius = (r > radius || std::isnan(r)) ? r : radius;  // NaN sticks -> general lookup path
     const double e = std::hypot(points_xy[2 * i], points_xy[2 * i + 1]);
     if (std::isfinite(e)) range_sum += e;
   }
-  points_radius_ = radius;
+  points_radius_ = scan_radius(points_xy, n_points);
   points_mean_range_ = n_points > 0 ? range_sum / static_cast<double>(n_points) : 1.0;  // lever arm of the heading in the schedule
   if (n_points > 0) {
     // The previous step's copy must have left the staging buffer before it is overwritten.
@@ -1162,7 +936,7 @@ bool Filter::predict_schedule(const MotionSampling& s, Schedule* grid) const {
   const double vx = e.cov[0] + spread, vy = e.cov[4] + spread;
   if (!std::isfinite(var_theta) || !std::isfinite(vx) || !std::isfinite(vy) || !std::isfinite(mean.x) || !std::isfinite(mean.y)) return false;
   const double r = std::exp(-0.5 * var_theta);
-  schedule_from_moments(*grid, r * mean.c, r * mean.s, mean.x, mean.y, vx, vy, static_cast<double>(n_), points_mean_range_, 0.5 * grid_resolution_);
+  schedule_from_moments(*grid, r * mean.c, r * mean.s, mean.x, mean.y, vx, vy, static_cast<double>(n_), points_mean_range_, 0.5 * map_.grid_resolution);
   return true;
 }
 
@@ -1187,17 +961,17 @@ int Filter::enqueue_propagate_reweight_kernels(const MotionSampling* sampling, u
   }
   if (scheduled && perm == nullptr) {
     mark("schedule");
-    launch_build_schedule(states_[cur_], n_, sched_, bins_, counters_, perm_, sched_tiles_, points_mean_range_, 0.5 * grid_resolution_, stream_);
+    launch_build_schedule(states_[cur_], n_, sched_, bins_, counters_, perm_, sched_tiles_, points_mean_range_, 0.5 * map_.grid_resolution, stream_);
     BB_LAUNCHED_N("schedule", 4);
     perm = perm_;
   }
   if (do_reweight) {
-    if (sensor_ == BB200_SENSOR_BEAM) {
+    if (map_.sensor == BB200_SENSOR_BEAM) {
       mark("reweight_beam");
       uint64_t pass = 0;
       // spans of the walk's 32-bit arithmetic: far ends lie within beam_max_range of the source, sources inside the grid
-      const double reach_cells = beam_.beam_max_range * occupancy_view_.inv_resolution + 4.0;
-      if (n_points > 0 && occupancy_view_.free_padded != nullptr && reach_cells < static_cast<double>(1 << 21)) {
+      const double reach_cells = map_.beam.beam_max_range * map_.occupancy.inv_resolution + 4.0;
+      if (n_points > 0 && map_.occupancy.free_padded != nullptr && reach_cells < static_cast<double>(1 << 21)) {
         // hit words of one pass: at most 3 GiB, whole warps of particles
         pass = std::min<uint64_t>(n_, std::max<uint64_t>(32, ((3ull << 30) / (4ull * n_points)) / 32 * 32));
         const uint64_t words = beam_hit_words(pass, static_cast<uint32_t>(n_points));
@@ -1218,16 +992,16 @@ int Filter::enqueue_propagate_reweight_kernels(const MotionSampling* sampling, u
         }
       }
       if (pass > 0) {
-        launch_reweight_beam_two_pass(states_[cur_], weights_, n_, perm, occupancy_view_, beam_, points_, static_cast<uint32_t>(n_points), beam_hits_, pass,
+        launch_reweight_beam_two_pass(states_[cur_], weights_, n_, perm, map_.occupancy, map_.beam, points_, static_cast<uint32_t>(n_points), beam_hits_, pass,
                                       scalars_, stream_);
         BB_LAUNCHED_N("reweight_beam", 2 * static_cast<int>((n_ + pass - 1) / pass));
       } else {
-        launch_reweight_beam(states_[cur_], weights_, n_, perm, occupancy_view_, beam_, points_, static_cast<uint32_t>(n_points), scalars_, stream_);
+        launch_reweight_beam(states_[cur_], weights_, n_, perm, map_.occupancy, map_.beam, points_, static_cast<uint32_t>(n_points), scalars_, stream_);
         BB_LAUNCHED("reweight_beam");
       }
     } else {
       mark("reweight_lfm");
-      launch_reweight_lfm(states_[cur_], weights_, n_, perm, field_, points_, points_host_, static_cast<uint32_t>(n_points),
+      launch_reweight_lfm(states_[cur_], weights_, n_, perm, map_.field, points_, points_host_, static_cast<uint32_t>(n_points),
                           points_radius_, scalars_, stream_);
       BB_LAUNCHED("reweight_lfm");
     }
@@ -1303,34 +1077,6 @@ int Filter::ensure_cdf_ready() {
   return build_cdf(-1.0, nullptr, nullptr);
 }
 
-void Filter::estimate_from_moments_static(const double m[kMomentCount], const double pivot[2], bb200_estimate* out) {
-  // estimation.hpp:436-475 from raw moments about the pivot: normalised weights w/S,
-  // mean of (cos, sin, x, y); cov = (E[d d^T] - E[d] E[d]^T) / (1 - sum (w/S)^2).
-  const double sum = m[0];
-  const double mc = m[2] / sum, ms = m[3] / sum, mdx = m[4] / sum, mdy = m[5] / sum;
-  const double correction = 1.0 - m[1] / (sum * sum);
-  for (double& c : out->cov) c = 0.0;
-  out->cov[0] = (m[6] / sum - mdx * mdx) / correction;
-  out->cov[1] = (m[7] / sum - mdx * mdy) / correction;
-  out->cov[3] = out->cov[1];
-  out->cov[4] = (m[8] / sum - mdy * mdy) / correction;
-  out->mean[2] = pivot[0] + mdx;
-  out->mean[3] = pivot[1] + mdy;
-  const double norm = std::sqrt(mc * mc + ms * ms);
-  if (norm < std::numeric_limits<double>::epsilon()) {
-    out->cov[8] = std::numeric_limits<double>::infinity();
-    out->mean[0] = 1.0;
-    out->mean[1] = 0.0;
-  } else {
-    out->cov[8] = -2.0 * std::log(norm);
-    const double len = std::hypot(mc, ms);
-    out->mean[0] = mc / len;
-    out->mean[1] = ms / len;
-  }
-}
-
-void Filter::estimate_from_moments(const double m[kMomentCount], bb200_estimate* out) const { estimate_from_moments_static(m, pivot_, out); }
-
 int Filter::moments(const double pivot[2], double out[9]) {
   const int st = enqueue_moments(pivot);
   if (st != BB200_OK) return st;
@@ -1345,7 +1091,7 @@ int Filter::estimate(bb200_estimate* out) {
   double m[kMomentCount];
   const int st = moments(pivot_, m);
   if (st != BB200_OK) return st;
-  estimate_from_moments(m, out);
+  estimate_from_moments(m, pivot_, out);
   pivot_[0] = out->mean[2];
   pivot_[1] = out->mean[3];
   return BB200_OK;
@@ -1353,115 +1099,23 @@ int Filter::estimate(bb200_estimate* out) {
 
 // ---- cluster-based estimate ---------------------------------------------------------------------
 
-int Filter::ensure_cluster_scratch(uint32_t cells) {
-  ClusterScratch& c = cluster_;
-  if (c.capacity == 0) {
-    if (capacity_ >= (1ull << 31)) return fail(BB200_ERR_CAPACITY, "cluster estimate: more than 2^31 particles per filter");
-    uint64_t table = 2;
-    while (table < 2 * capacity_) table <<= 1;
-    const uint32_t tiles = cluster_sort_tiles(capacity_);
-    BB_CHECK(dev_alloc(&c.hashes, capacity_));
-    BB_CHECK(dev_alloc(&c.keys, table));
-    BB_CHECK(dev_alloc(&c.first, table));
-    BB_CHECK(dev_alloc(&c.slot_of, capacity_));
-    BB_CHECK(dev_alloc(&c.flags, capacity_));
-    BB_CHECK(dev_alloc(&c.cell_of, capacity_));
-    BB_CHECK(dev_alloc(&c.starts, capacity_ + 1));
-    BB_CHECK(dev_alloc(&c.keys_a, capacity_));
-    BB_CHECK(dev_alloc(&c.keys_b, capacity_));
-    BB_CHECK(dev_alloc(&c.idx_a, capacity_));
-    BB_CHECK(dev_alloc(&c.idx_b, capacity_));
-    BB_CHECK(dev_alloc(&c.histogram, static_cast<size_t>(256) * tiles));
-    BB_CHECK(dev_alloc(&c.tile_state, static_cast<size_t>(scan_tile_count(std::max<uint64_t>(capacity_ + 1, 256ull * tiles)) + 1)));
-    BB_CHECK(dev_alloc(&c.words, 4));
-    c.table_size = table;
-    c.capacity = capacity_;
-  }
-  if (cells > c.records_capacity) {
-    cudaFree(c.records);
-    c.records = nullptr;
-    c.records_capacity = 0;
-    const uint64_t want = std::min<uint64_t>(capacity_, std::max<uint64_t>(1024, 2ull * cells));
-    BB_CHECK(dev_alloc(&c.records, want));
-    c.records_capacity = want;
-  }
-  return BB200_OK;
-}
-
-int Filter::cell_records(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], double linear_resolution,
-                         double angular_resolution, std::vector<HostCell>* host) {
-  // Per-particle half of the clusterizer, also the device-side histogram of the particle cloud: spatial hash ->
-  // first-occurrence numbering of the occupied cells -> stable sort of the particle indices by cell -> one record per
-  // cell (representative = first particle, count, weight summed in particle order, raw moments).
-  BB_CHECK(cudaSetDevice(config_.device));
-  {
-    const int st = ensure_cluster_scratch(0);
-    if (st != BB200_OK) return st;
-  }
-  mark("cluster_cells");
-  launch_cluster_cells_begin(states, n, linear_resolution, angular_resolution, cluster_, stream_);
-  BB_LAUNCHED_N("cluster_cells_begin", 3);
-  unsigned long long cells64 = 0;
-  BB_CHECK(cudaMemcpyAsync(&cells64, cluster_.words + 1, sizeof(cells64), cudaMemcpyDeviceToHost, stream_));
-  BB_CHECK(cudaStreamSynchronize(stream_));
-  const uint32_t cells = static_cast<uint32_t>(cells64);
-  {
-    const int st = ensure_cluster_scratch(cells);
-    if (st != BB200_OK) return st;
-  }
-  mark("cluster_sort");
-  int sort_launches = 0;
-  const uint32_t* sorted = launch_cluster_sort(n, cells, cluster_, stream_, &sort_launches);
-  BB_LAUNCHED_N("cluster_sort", sort_launches);
-  mark("cluster_records");
-  launch_cluster_records(states, weights, sorted, cells, pivot[0], pivot[1], cluster_, stream_);
-  BB_LAUNCHED("cluster_records");
-  host->resize(cells);
-  static_assert(sizeof(HostCell) == sizeof(CellRecord), "record layouts must agree");
-  BB_CHECK(cudaMemcpyAsync(host->data(), cluster_.records, static_cast<size_t>(cells) * sizeof(CellRecord), cudaMemcpyDeviceToHost, stream_));
-  BB_CHECK(cudaStreamSynchronize(stream_));
-  finish_marks();
-  return BB200_OK;
-}
-
 int Filter::cluster_estimate(const bb200_cluster_param& p, bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells,
                              uint32_t* n_clusters) {
-  return cluster_estimate_of(states_[cur_], weights_, n_, pivot_, p, out, cluster_ids, ids_capacity, n_cells, n_clusters);
-}
-
-int Filter::cluster_estimate_of(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], const bb200_cluster_param& p,
-                                bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells, uint32_t* n_clusters) {
-  if (n == 0) return fail(BB200_ERR_STATE, "no particles");
-  if (n > capacity_) return fail(BB200_ERR_CAPACITY, "cluster estimate: more particles than the scratch holds");
-  if (!(p.linear_hash_resolution > 0.0) || !(p.angular_hash_resolution > 0.0) || !(p.weight_cap_percentile >= 0.0) ||
-      !(p.weight_cap_percentile < 1.0))
-    return fail(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)");
-  if (cluster_ids != nullptr && ids_capacity < n) return fail(BB200_ERR_CAPACITY, "cluster id buffer too small");
-  std::vector<HostCell> host;
-  {
-    const int st = cell_records(states, weights, n, pivot, p.linear_hash_resolution, p.angular_hash_resolution, &host);
-    if (st != BB200_OK) return st;
-  }
-  const uint32_t cells = static_cast<uint32_t>(host.size());
-  const ClusterSelection sel = select_cluster(host.data(), host.size(), n, p.linear_hash_resolution, p.angular_hash_resolution, p.weight_cap_percentile);
-  if (out != nullptr) estimate_from_moments_static(sel.moments, pivot, out);
-  if (n_cells != nullptr) *n_cells = cells;
-  if (n_clusters != nullptr) *n_clusters = sel.clusters;
-  if (cluster_ids != nullptr) {
-    std::vector<uint32_t> cell_of(n);
-    BB_CHECK(cudaMemcpy(cell_of.data(), cluster_.cell_of, n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    for (uint64_t i = 0; i < n; ++i) cluster_ids[i] = sel.cluster_of_cell[cell_of[i]];
-  }
-  return BB200_OK;
+  BB_CHECK(cudaSetDevice(config_.device));
+  const int st = cluster_.estimate(states_[cur_], weights_, n_, pivot_, p, stream_, out, cluster_ids, ids_capacity, n_cells, n_clusters, &error_);
+  if (st == BB200_OK) finish_marks();
+  return st;
 }
 
 int Filter::particle_histogram(double linear_resolution, double angular_resolution, bb200_cluster_cell* bins, uint64_t capacity, uint64_t* n_bins,
                                double* max_bin_weight) {
   if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
   if (!(linear_resolution > 0.0) || !(angular_resolution > 0.0)) return fail(BB200_ERR_INVALID_ARGUMENT, "histogram resolutions must be positive");
+  BB_CHECK(cudaSetDevice(config_.device));
   std::vector<HostCell> host;
-  const int st = cell_records(states_[cur_], weights_, n_, pivot_, linear_resolution, angular_resolution, &host);
+  const int st = cluster_.cell_records(states_[cur_], weights_, n_, pivot_, linear_resolution, angular_resolution, stream_, &host, &error_);
   if (st != BB200_OK) return st;
+  finish_marks();
   if (n_bins != nullptr) *n_bins = host.size();
   double top = 1e-3;  // beluga_ros/particle_cloud.hpp:197
   for (const HostCell& c : host) top = c.weight > top ? c.weight : top;
@@ -1515,11 +1169,11 @@ ResampleArgs Filter::make_resample_args(const bb200_resample_opts& o, uint64_t s
   a.seed = config_.seed;
   a.step = o.step;
   a.random_state_probability = o.random_state_probability;
-  a.free_cells = free_cells_;
-  a.n_free = n_free_;
-  a.grid_width = grid_width_;
-  a.grid_resolution = grid_resolution_;
-  a.grid_origin = grid_origin_;
+  a.free_cells = map_.free_cells;
+  a.n_free = map_.n_free;
+  a.grid_width = map_.grid_width;
+  a.grid_resolution = map_.grid_resolution;
+  a.grid_origin = map_.grid_origin;
   for (int k = 0; k < 3; ++k) a.hash_resolution[k] = o.spatial_resolution[k];
   a.pivot_x = pivot_[0];
   a.pivot_y = pivot_[1];
@@ -1529,7 +1183,7 @@ ResampleArgs Filter::make_resample_args(const bb200_resample_opts& o, uint64_t s
 int Filter::resample(const bb200_resample_opts& o, uint64_t* new_size) {
   if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
   if (o.max_particles == 0 || o.max_particles > capacity_) return fail(BB200_ERR_CAPACITY, "max_particles exceeds the filter capacity");
-  if (o.random_state_probability > 0.0 && n_free_ == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
+  if (o.random_state_probability > 0.0 && map_.n_free == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
   int st = ensure_cdf_ready();
   if (st != BB200_OK && !cdf_valid_) return st;
   BB_CHECK(cudaSetDevice(config_.device));

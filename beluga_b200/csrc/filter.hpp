@@ -1,4 +1,4 @@
-// Device-resident particle set of the CUDA MCL backend: buffers, map uploads and the per-step
+// Device-resident particle set of the CUDA MCL backend: buffers, its map (device_map.hpp) and the per-step
 // kernel sequence behind the C ABI of include/beluga_b200.h.  Host-side counterpart of
 // beluga::TupleVector<std::tuple<SE2d, Weight>> (reference: containers/tuple_vector.hpp:50-223)
 // plus the actions/views that iterate it (propagate, reweight, normalize, sample, assign).
@@ -12,7 +12,7 @@
 
 #include "../../include/beluga_b200.h"
 #include "cluster.cuh"
-#include "cluster_host.hpp"
+#include "device_map.hpp"
 #include "kernels.cuh"
 
 namespace bb200 {
@@ -27,6 +27,8 @@ class Filter {
   // Every method returns a bb200_status and records the message for last_error().
   int set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob);
   int set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid);
+  /// Makes the prepared tables this filter's map (the upload half of set_*_map).
+  int set_map(const MapTables& tables);
   int get_likelihood_field(float* out, uint64_t capacity) const;
 
   int set_particles(const double* states, const double* weights, uint64_t n);
@@ -52,17 +54,12 @@ class Filter {
   /// (optional, one per particle) is the parity hook for ParticleClusterizer::operator() (:304-316).
   int cluster_estimate(const bb200_cluster_param& p, bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells,
                        uint32_t* n_clusters);
-  /// The same over n particles held outside this filter (a batch member's slice, on this filter's device), the moments
-  /// taken about `pivot`.  n must not exceed the capacity.
-  int cluster_estimate_of(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], const bb200_cluster_param& p,
-                          bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells, uint32_t* n_clusters);
   /// Device-side histogram of the particle cloud over spatial-hash buckets (beluga_ros/particle_cloud.hpp:197-210): one
   /// record per occupied bucket in first-occurrence order.  bins may be null (count only).
   int particle_histogram(double linear_resolution, double angular_resolution, bb200_cluster_cell* bins, uint64_t capacity, uint64_t* n_bins,
                          double* max_bin_weight);
   /// `count` states drawn by weight without touching the set (views::sample | take_exactly, particle_cloud.hpp:141-147).
   int sample_states(uint64_t count, uint32_t step, double* states_out);
-  static void estimate_from_moments_static(const double m[kMomentCount], const double pivot[2], bb200_estimate* out);
 
   /// Fused single-GPU step: propagate | reweight | normalize | resample | estimate with one
   /// host synchronisation at the end (the composition Amcl::update performs every step).
@@ -133,32 +130,21 @@ class Filter {
   void set_timing(bool on) { timing_ = on; }
   void clear_timings() { timings_.clear(); }
   int last_timings(const char** names, float* ms, int capacity) const;
-  uint64_t launch_count() const { return launches_; }
+  uint64_t launch_count() const { return launches_ + map_.launches() + cluster_.launches(); }
   /// False when the last CDF was built from a weight set without any positive finite weight (uniform CDF substituted).
   bool last_weights_valid() const { return weights_valid_; }
   const char* last_error() const { return error_.c_str(); }
   void record_error(const std::string& message) const { error_ = message; }  // the C-ABI exception guard
   int fail_with(int status, const std::string& message) { return fail(status, message); }
   bool ok() const { return created_; }
-
-  /// What a batch of filters (csrc/batch.hpp) takes from the filter that holds its map.
-  struct MapView {
-    int sensor;  // -1: no map yet
-    FieldView field;
-    const uint32_t* free_cells;
-    uint64_t n_free;
-    int grid_width, grid_height;
-    double grid_resolution;
-    Pose2 grid_origin;
-  };
-  MapView map_view() const { return MapView{sensor_, field_, free_cells_, n_free_, grid_width_, grid_height_, grid_resolution_, grid_origin_}; }
-  cudaStream_t stream() const { return stream_; }
-  int device() const { return config_.device; }
   int create_status() const { return create_status_; }
 
  private:
-  int fail(int status, const std::string& message);
-  int check(cudaError_t e, const char* what);
+  int fail(int status, const std::string& message) {
+    error_ = message;
+    return status;
+  }
+  int check(cudaError_t e, const char* what) { return cuda_check(e, what, &error_); }
   int upload_points(const double* points_xy, uint64_t n_points);
   /// propagate | schedule | reweight on a staged step (points uploaded, scalars reset), no validation.
   int enqueue_propagate_reweight_kernels(const MotionSampling* sampling, uint32_t step, bool do_reweight, uint64_t n_points, bool counters_reset);
@@ -169,7 +155,6 @@ class Filter {
   int ensure_cdf_ready();
   int resample_kld(const bb200_resample_opts& o, uint64_t* accepted);
   ResampleArgs make_resample_args(const bb200_resample_opts& o, uint64_t slot_begin, uint64_t slot_end, bool with_hashes) const;
-  void estimate_from_moments(const double m[kMomentCount], bb200_estimate* out) const;
   void mark(const char* name);  // timing: record an event before the next kernel
   void finish_marks();
   bool use_device() const;
@@ -236,11 +221,7 @@ class Filter {
   double* results_{nullptr};       // device: kMomentCount + extras
   double* results_host_{nullptr};  // pinned
 
-  // clusterizer scratch (allocated on first use)
-  int ensure_cluster_scratch(uint32_t cells);
-  int cell_records(const Pose2* states, const double* weights, uint64_t n, const double pivot[2], double linear_resolution,
-                   double angular_resolution, std::vector<HostCell>* host);
-  ClusterScratch cluster_{};
+  Clusterizer cluster_;
 
   // KLD scratch
   unsigned long long* kld_keys_{nullptr};
@@ -269,26 +250,9 @@ class Filter {
   uint32_t* counters_{nullptr};
   unsigned long long* sched_tiles_{nullptr};
 
-  // maps
-  int sensor_{-1};
-  std::vector<float> field_host_;
-  double* tiled_{nullptr};
-  double* bordered_{nullptr};
-  uint64_t bordered_bytes_{0};
-  FieldView field_{};
-  int8_t* occupancy_{nullptr};
-  uint8_t* free_distance_{nullptr};
-  uint8_t* free_padded_{nullptr};
-  OccupancyView occupancy_view_{};
-  BeamParams beam_{};
-  double2* beam_eta_{nullptr};
+  DeviceMap map_;
   uint32_t* beam_hits_{nullptr};   // two-pass beam model: hit word per (beam, particle) of one pass
   uint64_t beam_hits_words_{0};
-  uint32_t* free_cells_{nullptr};
-  uint64_t n_free_{0};
-  int grid_width_{0}, grid_height_{0};
-  double grid_resolution_{1.0};
-  Pose2 grid_origin_{1.0, 0.0, 0.0, 0.0};
 
   double pivot_[2]{0.0, 0.0};
   bb200_estimate cloud_{};     // last estimate, when it describes the raw (unit-weight) cloud
@@ -310,6 +274,18 @@ class Filter {
 
 /// bb200_motion_sampling -> the kernels' MotionSampling.
 MotionSampling to_kernel_sampling(const bb200_motion_sampling& s);
+
+/// BB200_ERR_NO_DEVICE without any CUDA device, BB200_ERR_INVALID_ARGUMENT for an ordinal out of range.
+int check_device(int device, std::string* error);
+
+/// Largest |x| + |y| of a scan's end points: bounds the cells the reweight kernels can reach.  A NaN sticks, which sends
+/// the scan down the exact lookup path.
+double scan_radius(const double* points_xy, uint64_t n_points);
+
+/// Spins until the kernel that ends a step stores `ticket` into the pinned word: the host sees the end of the step a few
+/// microseconds before a stream synchronisation would return.  The stream is queried now and then so that a failed launch
+/// cannot hang the caller.  False when the stream ended (or failed) without the ticket being seen: the caller synchronises.
+bool wait_for_ticket(const volatile int* word, int ticket, cudaStream_t stream);
 
 /// Symmetric 3x3 covariance -> V * sqrt(Lambda) (multivariate_normal_distribution.hpp:109-126).
 /// Returns false with a message for non-symmetric / negative-eigenvalue input.

@@ -4,7 +4,9 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <string>
 
+#include "../../include/beluga_b200.h"
 #include "se2_math.cuh"
 
 namespace bb200 {
@@ -142,6 +144,44 @@ constexpr int kMomentCount = 9;  // sum w, sum w^2, sum w c, sum w s, sum w dx, 
 /// SMs of the H100 SXM the grid-stride launches are sized for.  A fixed number, not the device's count, so
 /// that the per-block partial sums (and with them the rounding of the moments) do not depend on the part.
 constexpr uint32_t kSmCount = 132;
+
+// ---- host side of the owners of device buffers (Filter, Batch, DeviceMap, Clusterizer) ---------------------
+
+/// cudaMalloc / cudaMallocHost of `count` elements (at least one, so that an empty table still has an address).
+template <class T>
+cudaError_t dev_alloc(T** p, size_t count) {
+  return cudaMalloc(reinterpret_cast<void**>(p), (count > 1 ? count : 1) * sizeof(T));
+}
+template <class T>
+cudaError_t host_alloc(T** p, size_t count) {
+  return cudaMallocHost(reinterpret_cast<void**>(p), (count > 1 ? count : 1) * sizeof(T));
+}
+/// A device buffer and its pinned staging copy with room for `count` elements each; the old contents are dropped.
+template <class T>
+cudaError_t realloc_staged(T** dev, T** host, size_t count) {
+  cudaFree(*dev);
+  cudaFreeHost(*host);
+  *dev = *host = nullptr;
+  const cudaError_t e = dev_alloc(dev, count);
+  return e != cudaSuccess ? e : host_alloc(host, count);
+}
+/// `status` with `message` in *error.
+inline int reject(int status, const char* message, std::string* error) {
+  *error = message;
+  return status;
+}
+/// BB200_OK, or BB200_ERR_CUDA with "what: <CUDA error>" in *error.
+inline int cuda_check(cudaError_t e, const char* what, std::string* error) {
+  if (e == cudaSuccess) return BB200_OK;
+  *error = std::string(what) + ": " + cudaGetErrorString(e);
+  return BB200_ERR_CUDA;
+}
+// Early returns through the enclosing scope's check(cudaError_t, const char* what); BB_LAUNCHED_N also counts the launches
+// in launches_, BB_TRY (constructors) keeps the status in create_status_.
+#define BB_CHECK(expr) do { if (const int st_ = check((expr), #expr)) return st_; } while (0)
+#define BB_LAUNCHED_N(name, count) do { launches_ += (count); if (const int st_ = check(cudaGetLastError(), name)) return st_; } while (0)
+#define BB_LAUNCHED(name) BB_LAUNCHED_N(name, 1)
+#define BB_TRY(expr) do { if (const int st_ = check((expr), #expr)) { create_status_ = st_; return; } } while (0)
 
 // ---- launchers (all asynchronous on `stream`) ---------------------------------------------------
 

@@ -1,15 +1,12 @@
 // Host-side map preprocessing of the CUDA MCL backend (once per map, not per step).
 //
-// Builds what the device kernels index:
+// Computes the per-cell grids the map tables are made from (device_map.hpp lays them out for the kernels):
 //   * the likelihood field of LikelihoodFieldModelBase::make_likelihood_field
 //     (reference: sensor/likelihood_field_model_base.hpp:130-185), whose brushfire distance map
 //     (algorithm/distance_map.hpp:55-98) is order dependent -- the value of a cell depends on which
 //     equal-distance parent leaves the std::priority_queue first -- so it is computed with the same
 //     queue discipline on the host instead of an exact GPU distance transform;
-//   * the per-cell lookup table the reweight kernel gathers from: f(pz) as double, with
-//     f = pz^3 (LikelihoodFieldModel) or log(pz) (LikelihoodFieldProbModel).  f is a pure
-//     function of the float cell value, so tabulating it is bit-identical to evaluating it per
-//     beam as likelihood_field_model.hpp:84-89 / likelihood_field_prob_model.hpp:84-86 do;
+//   * the free distance of the beam model's ray cast;
 //   * the free-cell list of MultivariateUniformDistribution<SE2d, OccupancyGrid>
 //     (random/multivariate_uniform_distribution.hpp:158-160).
 #pragma once

@@ -135,6 +135,13 @@ int DeviceMap::upload(const MapTables& t, cudaStream_t stream, std::string* erro
   static_cast<MapLayout&>(*this) = t;
   sensor = -1;  // until every table is in place
   BB_CHECK(copy(t.bordered, &field.bordered, stream));
+  if (field.bordered != nullptr) {
+    // The biased index of element e is e + bias modulo 2^32; it equals e + bias, and the moved-back base then finds the
+    // element, only if no element's biased index passes 2^32.
+    const uint32_t bias = fixed_index_bias(field.border_pitch);
+    if (static_cast<uint64_t>(bias) + t.bordered.size() <= (1ull << 32))
+      field.bordered_biased = reinterpret_cast<const double*>(reinterpret_cast<uintptr_t>(field.bordered) - uintptr_t{bias} * sizeof(double));
+  }
   BB_CHECK(copy(t.tiled, &field.tiled, stream));
   BB_CHECK(copy(t.cells, &occupancy.cells, stream));
   BB_CHECK(copy(t.free_distance, &occupancy.free_distance, stream));

@@ -389,10 +389,16 @@ __global__ void __launch_bounds__(256) schedule_scatter_kernel(const uint32_t* _
 
 // ---- reweight (likelihood field; a3 + a5) --------------------------------------------------------
 
-// (threads, CTAs per SM, unroll) = (256, 4, 2) were chosen by sweeps on a B200, not re-measured on the H100.
+// Fixed-point kernels, measured with bench.py (reweight_lfm_fixed_param_kernel, 1M x 1080 beams) on an H100 80GB HBM3
+// (SXM): at a 400 W power limit 3 CTAs/SM -> 1.12 ms, 4 -> 1.47 ms, 5 -> 1.80 ms; at 700 W, 3 CTAs/SM with unroll 1 ->
+// 0.99 ms, unroll 2 -> 0.99 ms (slightly slower, and the shared-memory kernels spill).  6 CTAs/SM spills in every kernel.
+// kRwThreads is the B200's choice.
 constexpr int kRwThreads = 256;  // x kRwBlocksPerSm CTAs per SM
-constexpr int kRwBlocksPerSm = 4;
-constexpr int kRwUnroll = 2;  // groups of four beams in flight per thread
+constexpr int kRwBlocksPerSm = 3;
+constexpr int kRwUnroll = 1;  // iterations of the fixed-point kernels' eight-beam loop body unrolled
+// The general kernel (reweight_lfm_kernel, maps beyond kFixedMaxSide) keeps the B200 sweep's (4 CTAs/SM, unroll 2).
+constexpr int kRwGeneralBlocksPerSm = 4;
+constexpr int kRwGeneralUnroll = 2;  // groups of four beams in flight per thread
 constexpr uint32_t kChunkBeams = 2048; // beams staged per shared-memory chunk (32 KB), multiple of 4
 
 /// floor(g) as int32 for |g| < 2^31: one F2I.F64.FLOOR (saturating).
@@ -430,7 +436,7 @@ __device__ __forceinline__ double accumulate_chunk(const FieldView& f, const dou
                                                    double tx, double ty) {
   // libstdc++ std::transform_reduce (numeric:439-462): groups of four, init += ((f0+f1)+(f2+f3)).
   uint32_t b = 0;
-#pragma unroll kRwUnroll
+#pragma unroll kRwGeneralUnroll
   for (; b + 4 <= count; b += 4) {
     const double2 p0 = pts[b], p1 = pts[b + 1], p2 = pts[b + 2], p3 = pts[b + 3];
     const double f0 = field_lookup<kFast>(f, p0.x, p0.y, c, s, tx, ty);
@@ -521,7 +527,7 @@ __device__ __forceinline__ void reweight_lfm_block(const Pose2* __restrict__ sta
   publish_weight_max(active ? weight_order_bits(w) : 0ull, &s_max, &s_arrived, kRwThreads / kWarp, scalars);
 }
 
-__global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
+__global__ void __launch_bounds__(kRwThreads, kRwGeneralBlocksPerSm)
     reweight_lfm_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, const uint32_t* __restrict__ perm,
                         FieldView field, const double2* __restrict__ points, uint32_t n_points, double points_radius,
                         Scalars* __restrict__ scalars) {
@@ -543,7 +549,8 @@ __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
 // coordinate, about once every two steps among a million particles) or a particle out of the 2^13 range
 // redoes its beams with the reference's own operation sequence; nothing else in the loop branches.
 // Out-of-grid end points clamp (one DPX add-min per coordinate, which also strips the bias) to the
-// one-cell border holding the unknown-space value, so the load is unconditional.
+// one-cell border holding the unknown-space value, so the load is unconditional.  A warp whose particles all keep their
+// end points inside the grid (fixed_particle_setup) needs neither: it runs the loop with fixed_lookup<true>.
 
 constexpr double kFixedMagicX = 393216.0;   // 1.5 * 2^18: ulp 2^-34; high word = 0x41180000 + floor(4 g)    for |g| < 2^17
 constexpr double kFixedMagicY = 1572864.0;  // 1.5 * 2^20: ulp 2^-32; high word = 0x41380000 + floor(g)      for |g| < 2^19
@@ -563,24 +570,33 @@ struct FixedParticle {
   double ox, oy;         // field-frame position in cells, plus the border cell, plus magic constant and guard
   uint32_t x_max, y_max; // 4 (width + 1) + 3, height + 1: largest 4 * padded x (+ 2 fraction bits) and padded y
   uint32_t row_pitch;    // 4 * 2^kx: elements per row of cells (four rows of tiles' worth per tile row)
+  bool in_grid;          // warp-uniform: every end point of every particle of the warp lies inside the grid
 };
 
 /// `margin` collects the smallest fraction word seen (<= kFixedAmbiguous: a coordinate too close to a cell edge to call).
 /// x arrives as 4 * padded x with two fraction bits below it, y as padded y: the element index
 ///   (y >> 2) * 16 * tiles_per_row  +  (x >> 2) * 16 + (x & 3) * 4 + (y & 3)
 /// is then one bit-select (y's low two bits replace x's fraction bits), one mask and one multiply-add.
-__device__ __forceinline__ double fixed_lookup(const double* __restrict__ bordered, const FixedParticle& q, double px, double py, uint32_t& margin) {
+/// kInGrid: the warp's end points all lie inside the grid, so the clamp is the identity and is left out, and so is the
+/// bias: both bias words are multiples of 4, so the biased words give the index plus fixed_index_bias(pitch) (mod 2^32),
+/// and `table` is the base moved back by that much (FieldView::bordered_biased).
+template <bool kInGrid>
+__device__ __forceinline__ double fixed_lookup(const double* __restrict__ table, const FixedParticle& q, double px, double py, uint32_t& margin) {
   const double gx = fma(px, q.cx, fma(-py, q.sx, q.ox));  // gx + 1 + magic + guard
   const double gy = fma(px, q.sx, fma(py, q.cx, q.oy));   // gy + 1 + magic + guard
   margin = __vimin3_u32(margin, static_cast<uint32_t>(__double2loint(gx)), static_cast<uint32_t>(__double2loint(gy)));
-  // min(word - bias, max): a negative coordinate wraps to a huge unsigned and clamps to the far border,
-  // which holds the same unknown-space value as the near one.
-  const uint32_t ux = __viaddmin_u32(static_cast<uint32_t>(__double2hiint(gx)), 0u - kFixedBiasX, q.x_max);  // 4 * padded x + 2 fraction bits
-  const uint32_t uy = __viaddmin_u32(static_cast<uint32_t>(__double2hiint(gy)), 0u - kFixedBiasY, q.y_max);  // padded y
+  uint32_t ux = static_cast<uint32_t>(__double2hiint(gx));  // bias + 4 * padded x + 2 fraction bits
+  uint32_t uy = static_cast<uint32_t>(__double2hiint(gy));  // bias + padded y
+  if (!kInGrid) {
+    // min(word - bias, max): a negative coordinate wraps to a huge unsigned and clamps to the far border,
+    // which holds the same unknown-space value as the near one.
+    ux = __viaddmin_u32(ux, 0u - kFixedBiasX, q.x_max);
+    uy = __viaddmin_u32(uy, 0u - kFixedBiasY, q.y_max);
+  }
   uint32_t low;  // (ux & ~3) | (uy & 3) as ONE bit-select (the compiler splits it into two operations)
   asm("lop3.b32 %0, %1, 3, %2, 0xB8;" : "=r"(low) : "r"(ux), "r"(uy));
   const uint32_t idx = (uy & ~3u) * q.row_pitch + low;
-  return __ldg(bordered + idx);
+  return __ldg(table + idx);
 }
 
 /// The reference's operation sequence (field_lookup) against the bordered layout.
@@ -599,40 +615,45 @@ __device__ __forceinline__ Pose2 field_frame_pose(const FieldView& f, const Pose
   return pose_mul(f.world_to_field, active ? load_pose(states + i) : Pose2{1.0, 0.0, 0.0, 0.0});
 }
 
-/// Scan points as a kernel parameter: they sit in the constant bank and reach the FP64 instructions
-/// through uniform registers -- no shared-memory load per beam and no L1 data-pipe traffic.  30 KB of
-/// the 32 KB parameter space; longer scans take the shared-memory (TMA) variant.
+/// Scan points as a kernel parameter: they sit in the constant bank -- no shared-memory load per beam and no L1
+/// data-pipe traffic.  Both loops read them with register-indexed LDC.64, two per beam.  30 KB of the 32 KB parameter
+/// space; longer scans take the shared-memory (TMA) variant.
 constexpr uint32_t kParamBeams = 1920;
 struct ScanParam {
   double2 p[kParamBeams];
 };
 
 // libstdc++ transform_reduce (numeric:439-462): groups of four, init += ((f0+f1)+(f2+f3)), then one by one.
-#define BB200_FIXED_SUM(POINT, COUNT, LOOKUP, TABLE)                                                                       \
+#define BB200_FIXED_GROUP(F, B, POINT, LOOKUP, TABLE)                                                         \
   do {                                                                                                        \
-    const double acc_before = acc;                                                                            \
-    uint32_t margin = margin_start;                                                                           \
+    const double2 p0 = POINT(B), p1 = POINT((B) + 1), p2 = POINT((B) + 2), p3 = POINT((B) + 3);               \
+    F##0 = LOOKUP(TABLE, q, p0.x, p0.y, margin);                                                              \
+    F##1 = LOOKUP(TABLE, q, p1.x, p1.y, margin);                                                              \
+    F##2 = LOOKUP(TABLE, q, p2.x, p2.y, margin);                                                              \
+    F##3 = LOOKUP(TABLE, q, p3.x, p3.y, margin);                                                              \
+  } while (0)
+
+#define BB200_FIXED_BEAMS(POINT, COUNT, LOOKUP, TABLE)                                                        \
+  do {                                                                                                        \
     uint32_t b = 0;                                                                                           \
     if (4 <= (COUNT)) {                                                                                       \
       /* Software pipeline: the loads of the next four beams are issued before the previous four are summed */\
       /* (a warp issues in order: summing first would leave it with four loads in flight, then none).       */\
-      double f0, f1, f2, f3;                                                                                  \
-      {                                                                                                       \
-        const double2 p0 = POINT(0), p1 = POINT(1), p2 = POINT(2), p3 = POINT(3);                             \
-        f0 = LOOKUP(TABLE, q, p0.x, p0.y, margin);                                                            \
-        f1 = LOOKUP(TABLE, q, p1.x, p1.y, margin);                                                            \
-        f2 = LOOKUP(TABLE, q, p2.x, p2.y, margin);                                                            \
-        f3 = LOOKUP(TABLE, q, p3.x, p3.y, margin);                                                            \
-      }                                                                                                       \
+      /* Two groups per iteration, loaded alternately into f and g: no register copies between groups.      */\
+      double f0, f1, f2, f3, g0, g1, g2, g3;                                                                  \
+      BB200_FIXED_GROUP(f, 0, POINT, LOOKUP, TABLE);                                                          \
       b = 4;                                                                                                  \
-      _Pragma("unroll kRwUnroll") for (; b + 4 <= (COUNT); b += 4) {                                          \
-        const double2 p0 = POINT(b), p1 = POINT(b + 1), p2 = POINT(b + 2), p3 = POINT(b + 3);                 \
-        const double g0 = LOOKUP(TABLE, q, p0.x, p0.y, margin);                                               \
-        const double g1 = LOOKUP(TABLE, q, p1.x, p1.y, margin);                                               \
-        const double g2 = LOOKUP(TABLE, q, p2.x, p2.y, margin);                                               \
-        const double g3 = LOOKUP(TABLE, q, p3.x, p3.y, margin);                                               \
+      _Pragma("unroll kRwUnroll") for (; b + 8 <= (COUNT); b += 8) {                                          \
+        BB200_FIXED_GROUP(g, b, POINT, LOOKUP, TABLE);                                                        \
+        acc = acc + ((f0 + f1) + (f2 + f3));                                                                  \
+        BB200_FIXED_GROUP(f, b + 4, POINT, LOOKUP, TABLE);                                                    \
+        acc = acc + ((g0 + g1) + (g2 + g3));                                                                  \
+      }                                                                                                       \
+      if (b + 4 <= (COUNT)) {                                                                                 \
+        BB200_FIXED_GROUP(g, b, POINT, LOOKUP, TABLE);                                                        \
         acc = acc + ((f0 + f1) + (f2 + f3));                                                                  \
         f0 = g0, f1 = g1, f2 = g2, f3 = g3;                                                                   \
+        b += 4;                                                                                               \
       }                                                                                                       \
       acc = acc + ((f0 + f1) + (f2 + f3));                                                                    \
     }                                                                                                         \
@@ -640,10 +661,20 @@ struct ScanParam {
       const double2 p0 = POINT(b);                                                                            \
       acc = acc + LOOKUP(TABLE, q, p0.x, p0.y, margin);                                                       \
     }                                                                                                         \
+  } while (0)
+
+#define BB200_FIXED_SUM(POINT, COUNT)                                                                         \
+  do {                                                                                                        \
+    const double acc_before = acc;                                                                            \
+    uint32_t margin = margin_start;                                                                           \
+    if (q.in_grid)                                                                                            \
+      BB200_FIXED_BEAMS(POINT, COUNT, fixed_lookup<true>, field.bordered_biased);                             \
+    else                                                                                                      \
+      BB200_FIXED_BEAMS(POINT, COUNT, fixed_lookup<false>, field.bordered);                                   \
     if (margin <= kFixedAmbiguous) { /* a coordinate within ~2^-30 cells of a cell edge, or a particle out of range */ \
       const Pose2 te = field_frame_pose(field, states, i, active);                                            \
       acc = acc_before;                                                                                       \
-      b = 0;                                                                                                  \
+      uint32_t b = 0;                                                                                         \
       for (; b + 4 <= (COUNT); b += 4) {                                                                      \
         const double2 p0 = POINT(b), p1 = POINT(b + 1), p2 = POINT(b + 2), p3 = POINT(b + 3);                 \
         const double f0 = bordered_lookup_exact(field, p0.x, p0.y, te.c, te.s, te.x, te.y);                   \
@@ -673,6 +704,14 @@ __device__ __forceinline__ void fixed_particle_setup(const FieldView& field, con
   q.x_max = field.border_x_max;
   q.y_max = field.border_y_max;
   q.row_pitch = 4u * field.border_pitch;
+  // points_radius bounds |px| + |py|, so every end point lies within points_radius * inv cells of (t.x, t.y) in each
+  // coordinate, give or take rounding far below the two cells added.  A square inside [0, width) x [0, height) keeps every
+  // reference cell inside the grid (reach < 8100 then holds too: width, height <= kFixedMaxSide).  False for NaN.
+  const double cells = points_radius * inv + 2.0;
+  const double gx = t.x * inv, gy = t.y * inv;
+  const bool inside = gx - cells >= 0.0 && gx + cells < static_cast<double>(field.width) && gy - cells >= 0.0 &&
+                      gy + cells < static_cast<double>(field.height);
+  q.in_grid = __all_sync(0xffffffffu, inside) && field.bordered_biased != nullptr;
 }
 
 /// Scan in the constant bank: nothing is shared between the warps of a CTA, so the grid is persistent
@@ -699,7 +738,7 @@ __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
     fixed_particle_setup(field, states, i, active, points_radius, q, margin_start);
     double acc = field.init;
 #define BB200_POINT(k) scan.p[(k)]
-    BB200_FIXED_SUM(BB200_POINT, n_points, fixed_lookup, field.bordered);
+    BB200_FIXED_SUM(BB200_POINT, n_points);
 #undef BB200_POINT
     if (active) {
       const double likelihood = field.exp_epilogue ? exp(acc) : acc;
@@ -763,7 +802,7 @@ __device__ __forceinline__ void reweight_lfm_fixed_block(const Pose2* __restrict
     mbarrier_wait(&s_bar, phase);
     phase ^= 1u;
 #define BB200_POINT(k) s_pts[(k)]
-    BB200_FIXED_SUM(BB200_POINT, count, fixed_lookup, field.bordered);
+    BB200_FIXED_SUM(BB200_POINT, count);
 #undef BB200_POINT
     if (base + kChunkBeams < n_points) __syncthreads();
   }
@@ -776,6 +815,8 @@ __device__ __forceinline__ void reweight_lfm_fixed_block(const Pose2* __restrict
   publish_weight_max(active ? weight_order_bits(w) : 0ull, &s_max, &s_arrived, kRwThreads / kWarp, scalars);
 }
 #undef BB200_FIXED_SUM
+#undef BB200_FIXED_BEAMS
+#undef BB200_FIXED_GROUP
 
 __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
     reweight_lfm_fixed_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, const uint32_t* __restrict__ perm,
@@ -2151,6 +2192,8 @@ int ceil_log2_u64(uint64_t n) {
 constexpr uint32_t kStreamMaxBlocks = kSmCount * 8;
 
 }  // namespace
+
+uint32_t fixed_index_bias(uint32_t border_pitch) { return kFixedBiasY * (4u * border_pitch) + kFixedBiasX; }
 
 // ---- launchers -------------------------------------------------------------------------------------
 

@@ -20,6 +20,9 @@ struct FieldView {
   // with a one-cell border of unknown_value, cell (xi, yi) stored at padded coordinates
   // (px, py) = (xi + 1, yi + 1), index bordered_index(px, py, border_kx); 2^border_kx tiles per row.
   const double* bordered;
+  // bordered moved back by fixed_index_bias(border_pitch) elements: warps whose end points all lie inside the grid index
+  // it with the still-biased fixed-point words.  Null if a biased index could pass 2^32 (every warp then clamps).
+  const double* bordered_biased;
   int border_kx;
   uint32_t border_pitch;  // 2^border_kx
   uint32_t border_x_max;  // 4 (width + 1) + 3: largest 4 * padded x with its two fraction bits
@@ -45,6 +48,9 @@ BB_HD uint32_t bordered_index(uint32_t px, uint32_t py, int kx) {
 }
 /// Largest padded grid side the fixed-point kernel accepts (cell coordinates below 2^13).
 constexpr int kFixedMaxSide = 8000;
+/// What the fixed-point lookup's element index gains, modulo 2^32, when its coordinates keep the bias of their magic
+/// constants (kernels.cu, fixed_lookup).
+uint32_t fixed_index_bias(uint32_t border_pitch);
 
 /// Device view of the occupancy grid (beam model).
 struct OccupancyView {

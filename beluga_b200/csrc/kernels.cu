@@ -392,9 +392,12 @@ __global__ void __launch_bounds__(256) schedule_scatter_kernel(const uint32_t* _
 // Fixed-point kernels, measured with bench.py (reweight_lfm_fixed_param_kernel, 1M x 1080 beams) on an H100 80GB HBM3
 // (SXM): at a 400 W power limit 3 CTAs/SM -> 1.12 ms, 4 -> 1.47 ms, 5 -> 1.80 ms; at 700 W, 3 CTAs/SM with unroll 1 ->
 // 0.99 ms, unroll 2 -> 0.99 ms (slightly slower, and the shared-memory kernels spill).  6 CTAs/SM spills in every kernel.
-// kRwThreads is the B200's choice.
+// The two-particle param kernel (slots l, l + 32) at a 400 W power limit, 1M: 2 CTAs/SM -> 1.046-1.050 ms, 3 -> 1.069-1.072
+// ms, against 1.141-1.178 ms for the one-particle kernel (DESIGN section 4, item 8).  kRwThreads is the B200's choice.
 constexpr int kRwThreads = 256;  // x kRwBlocksPerSm CTAs per SM
 constexpr int kRwBlocksPerSm = 3;
+constexpr int kRwPairBlocksPerSm = 2;  // the two-particle variant of reweight_lfm_fixed_param_kernel (126 registers)
+constexpr uint64_t kRwPairFill = 6;      // pair tasks per resident warp below which one particle per thread is faster
 constexpr int kRwUnroll = 1;  // iterations of the fixed-point kernels' eight-beam loop body unrolled
 // The general kernel (reweight_lfm_kernel, maps beyond kFixedMaxSide) keeps the B200 sweep's (4 CTAs/SM, unroll 2).
 constexpr int kRwGeneralBlocksPerSm = 4;
@@ -565,9 +568,13 @@ constexpr double kFixedGuardX = 1.16415321826934814453125e-10; // 2^-33 = 2 ulp 
 constexpr double kFixedGuardY = 4.656612873077392578125e-10;   // 2^-31 = 2 ulp of kFixedMagicY
 constexpr uint32_t kFixedAmbiguous = 4u;  // fraction words 0..4: the cell is not decided (5 * 2^-32 per coordinate)
 
-struct FixedParticle {
+struct FixedPose {
   double cx, sx;         // cos, sin of the field-frame heading, times 1/resolution
   double ox, oy;         // field-frame position in cells, plus the border cell, plus magic constant and guard
+};
+
+/// The table geometry, held once per thread however many particles it weighs.
+struct FixedGrid {
   uint32_t x_max, y_max; // 4 (width + 1) + 3, height + 1: largest 4 * padded x (+ 2 fraction bits) and padded y
   uint32_t row_pitch;    // 4 * 2^kx: elements per row of cells (four rows of tiles' worth per tile row)
   bool in_grid;          // warp-uniform: every end point of every particle of the warp lies inside the grid
@@ -581,7 +588,8 @@ struct FixedParticle {
 /// bias: both bias words are multiples of 4, so the biased words give the index plus fixed_index_bias(pitch) (mod 2^32),
 /// and `table` is the base moved back by that much (FieldView::bordered_biased).
 template <bool kInGrid>
-__device__ __forceinline__ double fixed_lookup(const double* __restrict__ table, const FixedParticle& q, double px, double py, uint32_t& margin) {
+__device__ __forceinline__ double fixed_lookup(const double* __restrict__ table, const FixedGrid& g, const FixedPose& q, double px, double py,
+                                               uint32_t& margin) {
   const double gx = fma(px, q.cx, fma(-py, q.sx, q.ox));  // gx + 1 + magic + guard
   const double gy = fma(px, q.sx, fma(py, q.cx, q.oy));   // gy + 1 + magic + guard
   margin = __vimin3_u32(margin, static_cast<uint32_t>(__double2loint(gx)), static_cast<uint32_t>(__double2loint(gy)));
@@ -590,12 +598,12 @@ __device__ __forceinline__ double fixed_lookup(const double* __restrict__ table,
   if (!kInGrid) {
     // min(word - bias, max): a negative coordinate wraps to a huge unsigned and clamps to the far border,
     // which holds the same unknown-space value as the near one.
-    ux = __viaddmin_u32(ux, 0u - kFixedBiasX, q.x_max);
-    uy = __viaddmin_u32(uy, 0u - kFixedBiasY, q.y_max);
+    ux = __viaddmin_u32(ux, 0u - kFixedBiasX, g.x_max);
+    uy = __viaddmin_u32(uy, 0u - kFixedBiasY, g.y_max);
   }
   uint32_t low;  // (ux & ~3) | (uy & 3) as ONE bit-select (the compiler splits it into two operations)
   asm("lop3.b32 %0, %1, 3, %2, 0xB8;" : "=r"(low) : "r"(ux), "r"(uy));
-  const uint32_t idx = (uy & ~3u) * q.row_pitch + low;
+  const uint32_t idx = (uy & ~3u) * g.row_pitch + low;
   return __ldg(table + idx);
 }
 
@@ -623,76 +631,88 @@ struct ScanParam {
   double2 p[kParamBeams];
 };
 
-// libstdc++ transform_reduce (numeric:439-462): groups of four, init += ((f0+f1)+(f2+f3)), then one by one.
-#define BB200_FIXED_GROUP(F, B, POINT, LOOKUP, TABLE)                                                         \
+// libstdc++ transform_reduce (numeric:439-462): groups of four, init += ((f0+f1)+(f2+f3)), then one by one.  A thread
+// weighs P particles (q[k], acc[k], margin[k], i[k], active[k]; one FixedGrid `grid`) against every point it reads, each
+// particle's sum in that order.
+#define BB200_FIXED_GROUP(F, B, POINT, LOOKUP, TABLE, P)                                                      \
   do {                                                                                                        \
     const double2 p0 = POINT(B), p1 = POINT((B) + 1), p2 = POINT((B) + 2), p3 = POINT((B) + 3);               \
-    F##0 = LOOKUP(TABLE, q, p0.x, p0.y, margin);                                                              \
-    F##1 = LOOKUP(TABLE, q, p1.x, p1.y, margin);                                                              \
-    F##2 = LOOKUP(TABLE, q, p2.x, p2.y, margin);                                                              \
-    F##3 = LOOKUP(TABLE, q, p3.x, p3.y, margin);                                                              \
+    _Pragma("unroll") for (int k = 0; k < (P); ++k) {                                                         \
+      F##0[k] = LOOKUP(TABLE, grid, q[k], p0.x, p0.y, margin[k]);                                             \
+      F##1[k] = LOOKUP(TABLE, grid, q[k], p1.x, p1.y, margin[k]);                                             \
+      F##2[k] = LOOKUP(TABLE, grid, q[k], p2.x, p2.y, margin[k]);                                             \
+      F##3[k] = LOOKUP(TABLE, grid, q[k], p3.x, p3.y, margin[k]);                                             \
+    }                                                                                                         \
   } while (0)
 
-#define BB200_FIXED_BEAMS(POINT, COUNT, LOOKUP, TABLE)                                                        \
+#define BB200_FIXED_ADD(F, P) \
+  _Pragma("unroll") for (int k = 0; k < (P); ++k) acc[k] = acc[k] + ((F##0[k] + F##1[k]) + (F##2[k] + F##3[k]))
+
+#define BB200_FIXED_BEAMS(POINT, COUNT, LOOKUP, TABLE, P)                                                     \
   do {                                                                                                        \
     uint32_t b = 0;                                                                                           \
     if (4 <= (COUNT)) {                                                                                       \
       /* Software pipeline: the loads of the next four beams are issued before the previous four are summed */\
       /* (a warp issues in order: summing first would leave it with four loads in flight, then none).       */\
       /* Two groups per iteration, loaded alternately into f and g: no register copies between groups.      */\
-      double f0, f1, f2, f3, g0, g1, g2, g3;                                                                  \
-      BB200_FIXED_GROUP(f, 0, POINT, LOOKUP, TABLE);                                                          \
+      double f0[P], f1[P], f2[P], f3[P], g0[P], g1[P], g2[P], g3[P];                                          \
+      BB200_FIXED_GROUP(f, 0, POINT, LOOKUP, TABLE, P);                                                       \
       b = 4;                                                                                                  \
       _Pragma("unroll kRwUnroll") for (; b + 8 <= (COUNT); b += 8) {                                          \
-        BB200_FIXED_GROUP(g, b, POINT, LOOKUP, TABLE);                                                        \
-        acc = acc + ((f0 + f1) + (f2 + f3));                                                                  \
-        BB200_FIXED_GROUP(f, b + 4, POINT, LOOKUP, TABLE);                                                    \
-        acc = acc + ((g0 + g1) + (g2 + g3));                                                                  \
+        BB200_FIXED_GROUP(g, b, POINT, LOOKUP, TABLE, P);                                                     \
+        BB200_FIXED_ADD(f, P);                                                                                \
+        BB200_FIXED_GROUP(f, b + 4, POINT, LOOKUP, TABLE, P);                                                 \
+        BB200_FIXED_ADD(g, P);                                                                                \
       }                                                                                                       \
       if (b + 4 <= (COUNT)) {                                                                                 \
-        BB200_FIXED_GROUP(g, b, POINT, LOOKUP, TABLE);                                                        \
-        acc = acc + ((f0 + f1) + (f2 + f3));                                                                  \
-        f0 = g0, f1 = g1, f2 = g2, f3 = g3;                                                                   \
+        BB200_FIXED_GROUP(g, b, POINT, LOOKUP, TABLE, P);                                                     \
+        BB200_FIXED_ADD(f, P);                                                                                \
+        _Pragma("unroll") for (int k = 0; k < (P); ++k) f0[k] = g0[k], f1[k] = g1[k], f2[k] = g2[k], f3[k] = g3[k]; \
         b += 4;                                                                                               \
       }                                                                                                       \
-      acc = acc + ((f0 + f1) + (f2 + f3));                                                                    \
+      BB200_FIXED_ADD(f, P);                                                                                  \
     }                                                                                                         \
     for (; b < (COUNT); ++b) {                                                                                \
       const double2 p0 = POINT(b);                                                                            \
-      acc = acc + LOOKUP(TABLE, q, p0.x, p0.y, margin);                                                       \
+      _Pragma("unroll") for (int k = 0; k < (P); ++k) acc[k] = acc[k] + LOOKUP(TABLE, grid, q[k], p0.x, p0.y, margin[k]); \
     }                                                                                                         \
   } while (0)
 
-#define BB200_FIXED_SUM(POINT, COUNT)                                                                         \
+#define BB200_FIXED_SUM(POINT, COUNT, P)                                                                      \
   do {                                                                                                        \
-    const double acc_before = acc;                                                                            \
-    uint32_t margin = margin_start;                                                                           \
-    if (q.in_grid)                                                                                            \
-      BB200_FIXED_BEAMS(POINT, COUNT, fixed_lookup<true>, field.bordered_biased);                             \
+    double acc_before[P];                                                                                     \
+    uint32_t margin[P];                                                                                       \
+    _Pragma("unroll") for (int k = 0; k < (P); ++k) acc_before[k] = acc[k], margin[k] = margin_start[k];      \
+    if (grid.in_grid)                                                                                         \
+      BB200_FIXED_BEAMS(POINT, COUNT, fixed_lookup<true>, field.bordered_biased, P);                          \
     else                                                                                                      \
-      BB200_FIXED_BEAMS(POINT, COUNT, fixed_lookup<false>, field.bordered);                                   \
-    if (margin <= kFixedAmbiguous) { /* a coordinate within ~2^-30 cells of a cell edge, or a particle out of range */ \
-      const Pose2 te = field_frame_pose(field, states, i, active);                                            \
-      acc = acc_before;                                                                                       \
-      uint32_t b = 0;                                                                                         \
-      for (; b + 4 <= (COUNT); b += 4) {                                                                      \
-        const double2 p0 = POINT(b), p1 = POINT(b + 1), p2 = POINT(b + 2), p3 = POINT(b + 3);                 \
-        const double f0 = bordered_lookup_exact(field, p0.x, p0.y, te.c, te.s, te.x, te.y);                   \
-        const double f1 = bordered_lookup_exact(field, p1.x, p1.y, te.c, te.s, te.x, te.y);                   \
-        const double f2 = bordered_lookup_exact(field, p2.x, p2.y, te.c, te.s, te.x, te.y);                   \
-        const double f3 = bordered_lookup_exact(field, p3.x, p3.y, te.c, te.s, te.x, te.y);                   \
-        acc = acc + ((f0 + f1) + (f2 + f3));                                                                  \
-      }                                                                                                       \
-      for (; b < (COUNT); ++b) {                                                                              \
-        const double2 p0 = POINT(b);                                                                          \
-        acc = acc + bordered_lookup_exact(field, p0.x, p0.y, te.c, te.s, te.x, te.y);                         \
+      BB200_FIXED_BEAMS(POINT, COUNT, fixed_lookup<false>, field.bordered, P);                                \
+    _Pragma("unroll") for (int k = 0; k < (P); ++k) {                                                         \
+      if (margin[k] <= kFixedAmbiguous) { /* a coordinate within ~2^-30 cells of a cell edge, or a particle out of range */ \
+        const Pose2 te = field_frame_pose(field, states, i[k], active[k]);                                    \
+        double a = acc_before[k];                                                                             \
+        uint32_t b = 0;                                                                                       \
+        for (; b + 4 <= (COUNT); b += 4) {                                                                    \
+          const double2 p0 = POINT(b), p1 = POINT(b + 1), p2 = POINT(b + 2), p3 = POINT(b + 3);               \
+          const double f0 = bordered_lookup_exact(field, p0.x, p0.y, te.c, te.s, te.x, te.y);                 \
+          const double f1 = bordered_lookup_exact(field, p1.x, p1.y, te.c, te.s, te.x, te.y);                 \
+          const double f2 = bordered_lookup_exact(field, p2.x, p2.y, te.c, te.s, te.x, te.y);                 \
+          const double f3 = bordered_lookup_exact(field, p3.x, p3.y, te.c, te.s, te.x, te.y);                 \
+          a = a + ((f0 + f1) + (f2 + f3));                                                                    \
+        }                                                                                                     \
+        for (; b < (COUNT); ++b) {                                                                            \
+          const double2 p0 = POINT(b);                                                                        \
+          a = a + bordered_lookup_exact(field, p0.x, p0.y, te.c, te.s, te.x, te.y);                           \
+        }                                                                                                     \
+        acc[k] = a;                                                                                           \
       }                                                                                                       \
     }                                                                                                         \
   } while (0)
 
-/// Per-particle constants of the fixed-point evaluation.
-__device__ __forceinline__ void fixed_particle_setup(const FieldView& field, const Pose2* __restrict__ states, uint64_t i, bool active,
-                                                     double points_radius, FixedParticle& q, uint32_t& margin_start) {
+/// Per-particle constants of the fixed-point evaluation.  Returns whether every end point of the particle stays inside
+/// the grid.
+__device__ __forceinline__ bool fixed_pose_setup(const FieldView& field, const Pose2* __restrict__ states, uint64_t i, bool active,
+                                                 double points_radius, FixedPose& q, uint32_t& margin_start) {
   const Pose2 t = field_frame_pose(field, states, i, active);
   const double inv = field.inv_resolution;
   // The error bound above needs every term of g below 2^13 cells.
@@ -701,51 +721,75 @@ __device__ __forceinline__ void fixed_particle_setup(const FieldView& field, con
   q.cx = t.c * inv, q.sx = t.s * inv;
   q.ox = (t.x * inv + 1.0) + (kFixedMagicX + kFixedGuardX);
   q.oy = (t.y * inv + 1.0) + (kFixedMagicY + kFixedGuardY);
-  q.x_max = field.border_x_max;
-  q.y_max = field.border_y_max;
-  q.row_pitch = 4u * field.border_pitch;
   // points_radius bounds |px| + |py|, so every end point lies within points_radius * inv cells of (t.x, t.y) in each
   // coordinate, give or take rounding far below the two cells added.  A square inside [0, width) x [0, height) keeps every
   // reference cell inside the grid (reach < 8100 then holds too: width, height <= kFixedMaxSide).  False for NaN.
   const double cells = points_radius * inv + 2.0;
   const double gx = t.x * inv, gy = t.y * inv;
-  const bool inside = gx - cells >= 0.0 && gx + cells < static_cast<double>(field.width) && gy - cells >= 0.0 &&
-                      gy + cells < static_cast<double>(field.height);
-  q.in_grid = __all_sync(0xffffffffu, inside) && field.bordered_biased != nullptr;
+  return gx - cells >= 0.0 && gx + cells < static_cast<double>(field.width) && gy - cells >= 0.0 &&
+         gy + cells < static_cast<double>(field.height);
+}
+
+/// The table geometry, and whether every particle of the warp (`inside`: all of this thread's) keeps its end points in the grid.
+__device__ __forceinline__ FixedGrid fixed_grid_setup(const FieldView& field, bool inside) {
+  FixedGrid g;
+  g.x_max = field.border_x_max;
+  g.y_max = field.border_y_max;
+  g.row_pitch = 4u * field.border_pitch;
+  g.in_grid = __all_sync(0xffffffffu, inside) && field.bordered_biased != nullptr;
+  return g;
 }
 
 /// Scan in the constant bank: nothing is shared between the warps of a CTA, so the grid is persistent
 /// (CTAs/SM x SM count) and every WARP draws the next 32 particles of the schedule from a global
 /// ticket counter.  A CTA-per-256-particles grid loses time to its slowest warp (each CTA holds its
 /// SM slot until the last of its warps is through 1080 beams) and to the partial last wave.
-__global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
+/// P = 2: lane l of a 64-slot task weighs the particles of slots l and l + 32 in one loop: each scan point is read once
+/// for both, and the loop control is shared.  Each gather instruction still covers 32 consecutive slots (a few pose bins,
+/// so a few table lines); adjacent slots (2l, 2l + 1) spread one instruction over twice as many bins and are slower.
+template <int P>
+__global__ void __launch_bounds__(kRwThreads, P == 1 ? kRwBlocksPerSm : kRwPairBlocksPerSm)
     reweight_lfm_fixed_param_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, const uint32_t* __restrict__ perm,
                                     FieldView field, uint32_t n_points, double points_radius, Scalars* __restrict__ scalars,
                                     const __grid_constant__ ScanParam scan) {
   const int lane = threadIdx.x % kWarp;
-  const unsigned long long n_tasks = (n + kWarp - 1) / kWarp;  // a task = the next 32 particles of the schedule
+  constexpr int kTask = kWarp * P;  // a task = the next kWarp * P particles of the schedule
+  const unsigned long long n_tasks = (n + kTask - 1) / kTask;
   unsigned long long* ticket_counter = &scalars->work_ticket;
   unsigned long long ticket = __shfl_sync(0xffffffffu, lane == 0 ? atomicAdd(ticket_counter, 1ull) : 0ull, 0);
   unsigned long long best = 0ull;
   while (ticket < n_tasks) {
     // Draw the next ticket now; its round trip to L2 hides behind this task's beams.
     const unsigned long long next = lane == 0 ? atomicAdd(ticket_counter, 1ull) : 0ull;
-    const uint64_t slot = ticket * kWarp + lane;
-    const bool active = slot < n;  // idle lanes of the last task walk the beams with a dummy pose
-    const uint64_t i = active ? (perm != nullptr ? perm[slot] : slot) : 0;
-    uint32_t margin_start;
-    FixedParticle q;
-    fixed_particle_setup(field, states, i, active, points_radius, q, margin_start);
-    double acc = field.init;
+    bool active[P];  // idle slots of the last task walk the beams with a dummy pose
+    uint64_t i[P];
+    uint32_t margin_start[P];
+    FixedPose q[P];
+    double acc[P];
+#pragma unroll
+    for (int k = 0; k < P; ++k) {
+      const uint64_t slot = ticket * kTask + static_cast<uint64_t>(k) * kWarp + lane;
+      active[k] = slot < n;
+      i[k] = active[k] ? (perm != nullptr ? perm[slot] : slot) : 0;
+    }
+    bool inside = fixed_pose_setup(field, states, i[0], active[0], points_radius, q[0], margin_start[0]);
+#pragma unroll
+    for (int k = 1; k < P; ++k) inside &= fixed_pose_setup(field, states, i[k], active[k], points_radius, q[k], margin_start[k]);
+    const FixedGrid grid = fixed_grid_setup(field, inside);
+#pragma unroll
+    for (int k = 0; k < P; ++k) acc[k] = field.init;
 #define BB200_POINT(k) scan.p[(k)]
-    BB200_FIXED_SUM(BB200_POINT, n_points);
+    BB200_FIXED_SUM(BB200_POINT, n_points, P);
 #undef BB200_POINT
-    if (active) {
-      const double likelihood = field.exp_epilogue ? exp(acc) : acc;
-      const double w = weights[i] * likelihood;  // actions/reweight.hpp:54-60
-      weights[i] = w;
-      const unsigned long long bits = weight_order_bits(w);
-      best = bits > best ? bits : best;
+#pragma unroll
+    for (int k = 0; k < P; ++k) {
+      if (active[k]) {
+        const double likelihood = field.exp_epilogue ? exp(acc[k]) : acc[k];
+        const double w = weights[i[k]] * likelihood;  // actions/reweight.hpp:54-60
+        weights[i[k]] = w;
+        const unsigned long long bits = weight_order_bits(w);
+        best = bits > best ? bits : best;
+      }
     }
     ticket = __shfl_sync(0xffffffffu, next, 0);
   }
@@ -777,19 +821,19 @@ __device__ __forceinline__ void reweight_lfm_fixed_block(const Pose2* __restrict
   __shared__ unsigned int s_arrived;
 
   const uint64_t slot = slot_base + threadIdx.x;
-  const bool active = slot < n;
-  const uint64_t i = active ? (perm != nullptr ? perm[slot] : slot) : 0;
+  const bool active[1] = {slot < n};
+  const uint64_t i[1] = {active[0] ? (perm != nullptr ? perm[slot] : slot) : 0};
   if (threadIdx.x == 0) {
     s_max = 0ull;
     s_arrived = 0u;
     mbarrier_init(&s_bar, 1);
     mbarrier_init_fence();
   }
-  uint32_t margin_start;
-  FixedParticle q;
-  fixed_particle_setup(field, states, i, active, points_radius, q, margin_start);
+  uint32_t margin_start[1];
+  FixedPose q[1];
+  const FixedGrid grid = fixed_grid_setup(field, fixed_pose_setup(field, states, i[0], active[0], points_radius, q[0], margin_start[0]));
 
-  double acc = field.init;
+  double acc[1] = {field.init};
   __syncthreads();  // s_max and the barrier initialised
   uint32_t phase = 0;
   for (uint32_t base = 0; base < n_points; base += kChunkBeams) {
@@ -802,20 +846,21 @@ __device__ __forceinline__ void reweight_lfm_fixed_block(const Pose2* __restrict
     mbarrier_wait(&s_bar, phase);
     phase ^= 1u;
 #define BB200_POINT(k) s_pts[(k)]
-    BB200_FIXED_SUM(BB200_POINT, count);
+    BB200_FIXED_SUM(BB200_POINT, count, 1);
 #undef BB200_POINT
     if (base + kChunkBeams < n_points) __syncthreads();
   }
   double w = 0.0;
-  if (active) {
-    const double likelihood = field.exp_epilogue ? exp(acc) : acc;
-    w = weights[i] * likelihood;  // actions/reweight.hpp:54-60
-    weights[i] = w;
+  if (active[0]) {
+    const double likelihood = field.exp_epilogue ? exp(acc[0]) : acc[0];
+    w = weights[i[0]] * likelihood;  // actions/reweight.hpp:54-60
+    weights[i[0]] = w;
   }
-  publish_weight_max(active ? weight_order_bits(w) : 0ull, &s_max, &s_arrived, kRwThreads / kWarp, scalars);
+  publish_weight_max(active[0] ? weight_order_bits(w) : 0ull, &s_max, &s_arrived, kRwThreads / kWarp, scalars);
 }
 #undef BB200_FIXED_SUM
 #undef BB200_FIXED_BEAMS
+#undef BB200_FIXED_ADD
 #undef BB200_FIXED_GROUP
 
 __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
@@ -2294,9 +2339,19 @@ void launch_reweight_lfm(const Pose2* states, double* weights, uint64_t n, const
     static thread_local ScanParam scan;  // launch parameters are copied at launch time
     if (points_xy_host != nullptr && n_points <= kParamBeams) {
       std::memcpy(scan.p, points_xy_host, static_cast<size_t>(n_points) * sizeof(double2));
-      const unsigned ctas_needed = static_cast<unsigned>((n + kRwThreads - 1) / kRwThreads);
-      const unsigned persistent = std::min<unsigned>(static_cast<unsigned>(sm_count()) * kRwBlocksPerSm, ctas_needed);
-      reweight_lfm_fixed_param_kernel<<<persistent, kRwThreads, 0, stream>>>(states, weights, n, perm, field, n_points, points_radius, scalars, scan);
+      // Two particles per thread halve the warps with work: worth it only while the pair tasks still fill every resident
+      // warp kRwPairFill times over (811 009 particles and more on a 132-SM H100).
+      const uint64_t pair_tasks = (n + 2 * kWarp - 1) / (2 * kWarp);
+      const uint64_t pair_warps = static_cast<uint64_t>(sm_count()) * kRwPairBlocksPerSm * (kRwThreads / kWarp);
+      if (pair_tasks >= kRwPairFill * pair_warps) {
+        const unsigned ctas_needed = static_cast<unsigned>((n + 2 * kRwThreads - 1) / (2 * kRwThreads));
+        const unsigned persistent = std::min<unsigned>(static_cast<unsigned>(sm_count()) * kRwPairBlocksPerSm, ctas_needed);
+        reweight_lfm_fixed_param_kernel<2><<<persistent, kRwThreads, 0, stream>>>(states, weights, n, perm, field, n_points, points_radius, scalars, scan);
+      } else {
+        const unsigned ctas_needed = static_cast<unsigned>((n + kRwThreads - 1) / kRwThreads);
+        const unsigned persistent = std::min<unsigned>(static_cast<unsigned>(sm_count()) * kRwBlocksPerSm, ctas_needed);
+        reweight_lfm_fixed_param_kernel<1><<<persistent, kRwThreads, 0, stream>>>(states, weights, n, perm, field, n_points, points_radius, scalars, scan);
+      }
     } else {
       reweight_lfm_fixed_kernel<<<blocks, kRwThreads, smem, stream>>>(states, weights, n, perm, field, points, n_points, points_radius, scalars);
     }

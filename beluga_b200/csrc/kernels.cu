@@ -434,22 +434,39 @@ __device__ __forceinline__ double field_lookup(const FieldView& f, double px, do
   return __ldg(f.tiled + idx);
 }
 
-template <bool kFast>
-__device__ __forceinline__ double accumulate_chunk(const FieldView& f, const double2* pts, uint32_t count, double acc, double c, double s,
-                                                   double tx, double ty) {
-  // libstdc++ std::transform_reduce (numeric:439-462): groups of four, init += ((f0+f1)+(f2+f3)).
+/// acc + the sum of lookup(pts[b]) over b < count in libstdc++ std::transform_reduce's order (numeric:439-462): groups of
+/// four, acc + ((f0+f1)+(f2+f3)), then one at a time.  kUnroll: groups per unrolled iteration (1 compiles as no pragma does).
+template <int kUnroll, class Lookup>
+__device__ __forceinline__ double transform_reduce_exact(const double2* pts, uint32_t count, double acc, Lookup lookup) {
   uint32_t b = 0;
-#pragma unroll kRwGeneralUnroll
+#pragma unroll kUnroll
   for (; b + 4 <= count; b += 4) {
     const double2 p0 = pts[b], p1 = pts[b + 1], p2 = pts[b + 2], p3 = pts[b + 3];
-    const double f0 = field_lookup<kFast>(f, p0.x, p0.y, c, s, tx, ty);
-    const double f1 = field_lookup<kFast>(f, p1.x, p1.y, c, s, tx, ty);
-    const double f2 = field_lookup<kFast>(f, p2.x, p2.y, c, s, tx, ty);
-    const double f3 = field_lookup<kFast>(f, p3.x, p3.y, c, s, tx, ty);
+    const double f0 = lookup(p0), f1 = lookup(p1), f2 = lookup(p2), f3 = lookup(p3);
     acc = acc + ((f0 + f1) + (f2 + f3));
   }
-  for (; b < count; ++b) acc = acc + field_lookup<kFast>(f, pts[b].x, pts[b].y, c, s, tx, ty);
+  for (; b < count; ++b) acc = acc + lookup(pts[b]);
   return acc;
+}
+
+/// The particle in schedule slot `slot` (perm: the schedule's order, nullptr for the identity); idle slots read particle 0.
+__device__ __forceinline__ uint64_t slot_particle(const uint32_t* __restrict__ perm, uint64_t slot, bool active) {
+  return active ? (perm != nullptr ? perm[slot] : slot) : 0;
+}
+
+/// transform = world_to_likelihood_field * state (likelihood_field_model.hpp:70-74); idle threads use the identity.
+__device__ __forceinline__ Pose2 field_frame_pose(const FieldView& f, const Pose2* __restrict__ states, uint64_t i, bool active) {
+  return pose_mul(f.world_to_field, active ? load_pose(states + i) : Pose2{1.0, 0.0, 0.0, 0.0});
+}
+
+/// Stores particle i's new weight, its weight w times the likelihood its sum of field values gives (actions/reweight.hpp:54-60),
+/// and returns the new weight's order bits.  w is weights[i] itself or a copy read earlier.
+__device__ __forceinline__ unsigned long long store_reweighted(const FieldView& f, double* __restrict__ weights, uint64_t i, const double& w,
+                                                               double sum) {
+  const double likelihood = f.exp_epilogue ? exp(sum) : sum;
+  const double updated = w * likelihood;
+  weights[i] = updated;
+  return weight_order_bits(updated);
 }
 
 /// Block-wide max of the weight bit patterns without a closing barrier: every warp folds its max
@@ -472,62 +489,61 @@ __device__ __forceinline__ void publish_weight_max(unsigned long long bits, unsi
   }
 }
 
-/// One CTA of the general likelihood-field reweight: the particles in schedule slots [slot_base, slot_base + kRwThreads).
-__device__ __forceinline__ void reweight_lfm_block(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n,
-                                                   const uint32_t* __restrict__ perm, const FieldView& field, const double2* __restrict__ points,
-                                                   uint32_t n_points, double points_radius, Scalars* __restrict__ scalars, uint64_t slot_base) {
+/// The shared-memory body of one CTA's reweight: the scan goes to shared memory in kChunkBeams-point chunks by TMA bulk
+/// copy (completion on an mbarrier), `chunk(pts, count)` runs on each chunk, and the order bits that `weight_bits()`
+/// returns after the last one go into the block's weight max.
+template <class Chunk, class WeightBits>
+__device__ __forceinline__ void staged_scan_block(const double2* __restrict__ points, uint32_t n_points, Scalars* __restrict__ scalars,
+                                                  Chunk chunk, WeightBits weight_bits) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double2* s_pts = reinterpret_cast<double2*>(smem_raw);
   __shared__ __align__(8) uint64_t s_bar;
   __shared__ unsigned long long s_max;
   __shared__ unsigned int s_arrived;
-
-  const uint64_t slot = slot_base + threadIdx.x;
-  const bool active = slot < n;
-  const uint64_t i = active ? (perm != nullptr ? perm[slot] : slot) : 0;
-
   if (threadIdx.x == 0) {
     s_max = 0ull;
     s_arrived = 0u;
     mbarrier_init(&s_bar, 1);
     mbarrier_init_fence();
   }
-  Pose2 st{1.0, 0.0, 0.0, 0.0};
-  double w = 0.0;
-  if (active) {
-    st = load_pose(states + i);
-    w = weights[i];
-  }
-  // transform = world_to_likelihood_field * state (likelihood_field_model.hpp:70-74)
-  const Pose2 t = pose_mul(field.world_to_field, st);
-  // Fast floor is exact while every |coordinate * inv_resolution| stays below 2^30.
-  const double reach = (points_radius + fmax(fabs(t.x), fabs(t.y))) * field.inv_resolution;
-  const bool fast = reach < 1073741824.0;  // false for NaN
-  double acc = field.init;
-  uint32_t phase = 0;
   __syncthreads();  // barrier and s_max initialised
+  uint32_t phase = 0;
   for (uint32_t base = 0; base < n_points; base += kChunkBeams) {
     const uint32_t count = min(kChunkBeams, n_points - base);
     if (threadIdx.x == 0) {
-      // TMA bulk copy of the scan points into shared memory (UBLKCP), completion on the mbarrier.
       const uint32_t bytes = count * static_cast<uint32_t>(sizeof(double2));
       mbarrier_expect_tx(&s_bar, bytes);
       bulk_copy_g2s(s_pts, points + base, bytes, &s_bar);
     }
     mbarrier_wait(&s_bar, phase);
     phase ^= 1u;
-    if (active) {
-      acc = fast ? accumulate_chunk<true>(field, s_pts, count, acc, t.c, t.s, t.x, t.y)
-                 : accumulate_chunk<false>(field, s_pts, count, acc, t.c, t.s, t.x, t.y);
-    }
+    chunk(s_pts, count);
     if (base + kChunkBeams < n_points) __syncthreads();  // s_pts is about to be overwritten by the next chunk
   }
-  if (active) {
-    const double likelihood = field.exp_epilogue ? exp(acc) : acc;
-    w = w * likelihood;  // actions/reweight.hpp:54-60
-    weights[i] = w;
-  }
-  publish_weight_max(active ? weight_order_bits(w) : 0ull, &s_max, &s_arrived, kRwThreads / kWarp, scalars);
+  publish_weight_max(weight_bits(), &s_max, &s_arrived, kRwThreads / kWarp, scalars);
+}
+
+/// One CTA of the general likelihood-field reweight: the particles in schedule slots [slot_base, slot_base + kRwThreads).
+__device__ __forceinline__ void reweight_lfm_block(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n,
+                                                   const uint32_t* __restrict__ perm, const FieldView& field, const double2* __restrict__ points,
+                                                   uint32_t n_points, double points_radius, Scalars* __restrict__ scalars, uint64_t slot_base) {
+  const uint64_t slot = slot_base + threadIdx.x;
+  const bool active = slot < n;
+  const uint64_t i = slot_particle(perm, slot, active);
+  const double w = active ? weights[i] : 0.0;
+  const Pose2 t = field_frame_pose(field, states, i, active);
+  // Fast floor is exact while every |coordinate * inv_resolution| stays below 2^30.
+  const double reach = (points_radius + fmax(fabs(t.x), fabs(t.y))) * field.inv_resolution;
+  const bool fast = reach < 1073741824.0;  // false for NaN
+  double acc = field.init;
+  staged_scan_block(
+      points, n_points, scalars,
+      [&](const double2* pts, uint32_t count) {
+        if (!active) return;
+        acc = fast ? transform_reduce_exact<kRwGeneralUnroll>(pts, count, acc, [&](double2 p) { return field_lookup<true>(field, p.x, p.y, t.c, t.s, t.x, t.y); })
+                   : transform_reduce_exact<kRwGeneralUnroll>(pts, count, acc, [&](double2 p) { return field_lookup<false>(field, p.x, p.y, t.c, t.s, t.x, t.y); });
+      },
+      [&] { return active ? store_reweighted(field, weights, i, w, acc) : 0ull; });
 }
 
 __global__ void __launch_bounds__(kRwThreads, kRwGeneralBlocksPerSm)
@@ -553,7 +569,7 @@ __global__ void __launch_bounds__(kRwThreads, kRwGeneralBlocksPerSm)
 // redoes its beams with the reference's own operation sequence; nothing else in the loop branches.
 // Out-of-grid end points clamp (one DPX add-min per coordinate, which also strips the bias) to the
 // one-cell border holding the unknown-space value, so the load is unconditional.  A warp whose particles all keep their
-// end points inside the grid (fixed_particle_setup) needs neither: it runs the loop with fixed_lookup<true>.
+// end points inside the grid (fixed_pose_setup) needs neither: it runs the loop with fixed_lookup<true>.
 
 constexpr double kFixedMagicX = 393216.0;   // 1.5 * 2^18: ulp 2^-34; high word = 0x41180000 + floor(4 g)    for |g| < 2^17
 constexpr double kFixedMagicY = 1572864.0;  // 1.5 * 2^20: ulp 2^-32; high word = 0x41380000 + floor(g)      for |g| < 2^19
@@ -618,11 +634,6 @@ __device__ __forceinline__ double bordered_lookup_exact(const FieldView& f, doub
   return __ldg(f.bordered + bordered_index(static_cast<uint32_t>(xi + 1), static_cast<uint32_t>(yi + 1), f.border_kx));
 }
 
-/// transform = world_to_likelihood_field * state (likelihood_field_model.hpp:70-74); idle threads use the identity.
-__device__ __forceinline__ Pose2 field_frame_pose(const FieldView& f, const Pose2* __restrict__ states, uint64_t i, bool active) {
-  return pose_mul(f.world_to_field, active ? load_pose(states + i) : Pose2{1.0, 0.0, 0.0, 0.0});
-}
-
 /// Scan points as a kernel parameter: they sit in the constant bank -- no shared-memory load per beam and no L1
 /// data-pipe traffic.  Both loops read them with register-indexed LDC.64, two per beam.  30 KB of the 32 KB parameter
 /// space; longer scans take the shared-memory (TMA) variant.
@@ -631,83 +642,93 @@ struct ScanParam {
   double2 p[kParamBeams];
 };
 
-// libstdc++ transform_reduce (numeric:439-462): groups of four, init += ((f0+f1)+(f2+f3)), then one by one.  A thread
-// weighs P particles (q[k], acc[k], margin[k], i[k], active[k]; one FixedGrid `grid`) against every point it reads, each
-// particle's sum in that order.
-#define BB200_FIXED_GROUP(F, B, POINT, LOOKUP, TABLE, P)                                                      \
-  do {                                                                                                        \
-    const double2 p0 = POINT(B), p1 = POINT((B) + 1), p2 = POINT((B) + 2), p3 = POINT((B) + 3);               \
-    _Pragma("unroll") for (int k = 0; k < (P); ++k) {                                                         \
-      F##0[k] = LOOKUP(TABLE, grid, q[k], p0.x, p0.y, margin[k]);                                             \
-      F##1[k] = LOOKUP(TABLE, grid, q[k], p1.x, p1.y, margin[k]);                                             \
-      F##2[k] = LOOKUP(TABLE, grid, q[k], p2.x, p2.y, margin[k]);                                             \
-      F##3[k] = LOOKUP(TABLE, grid, q[k], p3.x, p3.y, margin[k]);                                             \
-    }                                                                                                         \
-  } while (0)
+// A thread weighs P particles (q[k], acc[k], margin[k]; one FixedGrid) against every point it reads, each particle's sum in
+// libstdc++ transform_reduce's order (transform_reduce_exact).
 
-#define BB200_FIXED_ADD(F, P) \
-  _Pragma("unroll") for (int k = 0; k < (P); ++k) acc[k] = acc[k] + ((F##0[k] + F##1[k]) + (F##2[k] + F##3[k]))
+/// f[j][k]: the table value at point b + j for particle k.
+template <int P, bool kInGrid>
+__device__ __forceinline__ void fixed_group(double (&f)[4][P], const double2* pts, uint32_t b, const FieldView& field,
+                                            const FixedGrid& grid, const FixedPose (&q)[P], uint32_t (&margin)[P]) {
+  const double* table = kInGrid ? field.bordered_biased : field.bordered;
+  const double2 p0 = pts[b], p1 = pts[b + 1], p2 = pts[b + 2], p3 = pts[b + 3];
+#pragma unroll
+  for (int k = 0; k < P; ++k) {
+    f[0][k] = fixed_lookup<kInGrid>(table, grid, q[k], p0.x, p0.y, margin[k]);
+    f[1][k] = fixed_lookup<kInGrid>(table, grid, q[k], p1.x, p1.y, margin[k]);
+    f[2][k] = fixed_lookup<kInGrid>(table, grid, q[k], p2.x, p2.y, margin[k]);
+    f[3][k] = fixed_lookup<kInGrid>(table, grid, q[k], p3.x, p3.y, margin[k]);
+  }
+}
 
-#define BB200_FIXED_BEAMS(POINT, COUNT, LOOKUP, TABLE, P)                                                     \
-  do {                                                                                                        \
-    uint32_t b = 0;                                                                                           \
-    if (4 <= (COUNT)) {                                                                                       \
-      /* Software pipeline: the loads of the next four beams are issued before the previous four are summed */\
-      /* (a warp issues in order: summing first would leave it with four loads in flight, then none).       */\
-      /* Two groups per iteration, loaded alternately into f and g: no register copies between groups.      */\
-      double f0[P], f1[P], f2[P], f3[P], g0[P], g1[P], g2[P], g3[P];                                          \
-      BB200_FIXED_GROUP(f, 0, POINT, LOOKUP, TABLE, P);                                                       \
-      b = 4;                                                                                                  \
-      _Pragma("unroll kRwUnroll") for (; b + 8 <= (COUNT); b += 8) {                                          \
-        BB200_FIXED_GROUP(g, b, POINT, LOOKUP, TABLE, P);                                                     \
-        BB200_FIXED_ADD(f, P);                                                                                \
-        BB200_FIXED_GROUP(f, b + 4, POINT, LOOKUP, TABLE, P);                                                 \
-        BB200_FIXED_ADD(g, P);                                                                                \
-      }                                                                                                       \
-      if (b + 4 <= (COUNT)) {                                                                                 \
-        BB200_FIXED_GROUP(g, b, POINT, LOOKUP, TABLE, P);                                                     \
-        BB200_FIXED_ADD(f, P);                                                                                \
-        _Pragma("unroll") for (int k = 0; k < (P); ++k) f0[k] = g0[k], f1[k] = g1[k], f2[k] = g2[k], f3[k] = g3[k]; \
-        b += 4;                                                                                               \
-      }                                                                                                       \
-      BB200_FIXED_ADD(f, P);                                                                                  \
-    }                                                                                                         \
-    for (; b < (COUNT); ++b) {                                                                                \
-      const double2 p0 = POINT(b);                                                                            \
-      _Pragma("unroll") for (int k = 0; k < (P); ++k) acc[k] = acc[k] + LOOKUP(TABLE, grid, q[k], p0.x, p0.y, margin[k]); \
-    }                                                                                                         \
-  } while (0)
+template <int P>
+__device__ __forceinline__ void fixed_add(double (&acc)[P], const double (&f)[4][P]) {
+#pragma unroll
+  for (int k = 0; k < P; ++k) acc[k] = acc[k] + ((f[0][k] + f[1][k]) + (f[2][k] + f[3][k]));
+}
 
-#define BB200_FIXED_SUM(POINT, COUNT, P)                                                                      \
-  do {                                                                                                        \
-    double acc_before[P];                                                                                     \
-    uint32_t margin[P];                                                                                       \
-    _Pragma("unroll") for (int k = 0; k < (P); ++k) acc_before[k] = acc[k], margin[k] = margin_start[k];      \
-    if (grid.in_grid)                                                                                         \
-      BB200_FIXED_BEAMS(POINT, COUNT, fixed_lookup<true>, field.bordered_biased, P);                          \
-    else                                                                                                      \
-      BB200_FIXED_BEAMS(POINT, COUNT, fixed_lookup<false>, field.bordered, P);                                \
-    _Pragma("unroll") for (int k = 0; k < (P); ++k) {                                                         \
-      if (margin[k] <= kFixedAmbiguous) { /* a coordinate within ~2^-30 cells of a cell edge, or a particle out of range */ \
-        const Pose2 te = field_frame_pose(field, states, i[k], active[k]);                                    \
-        double a = acc_before[k];                                                                             \
-        uint32_t b = 0;                                                                                       \
-        for (; b + 4 <= (COUNT); b += 4) {                                                                    \
-          const double2 p0 = POINT(b), p1 = POINT(b + 1), p2 = POINT(b + 2), p3 = POINT(b + 3);               \
-          const double f0 = bordered_lookup_exact(field, p0.x, p0.y, te.c, te.s, te.x, te.y);                 \
-          const double f1 = bordered_lookup_exact(field, p1.x, p1.y, te.c, te.s, te.x, te.y);                 \
-          const double f2 = bordered_lookup_exact(field, p2.x, p2.y, te.c, te.s, te.x, te.y);                 \
-          const double f3 = bordered_lookup_exact(field, p3.x, p3.y, te.c, te.s, te.x, te.y);                 \
-          a = a + ((f0 + f1) + (f2 + f3));                                                                    \
-        }                                                                                                     \
-        for (; b < (COUNT); ++b) {                                                                            \
-          const double2 p0 = POINT(b);                                                                        \
-          a = a + bordered_lookup_exact(field, p0.x, p0.y, te.c, te.s, te.x, te.y);                           \
-        }                                                                                                     \
-        acc[k] = a;                                                                                           \
-      }                                                                                                       \
-    }                                                                                                         \
-  } while (0)
+/// The fixed-point sums of pts[0, count) onto acc, from FieldView::bordered_biased for kInGrid, else from bordered.
+template <int P, bool kInGrid>
+__device__ __forceinline__ void fixed_beams(const double2* pts, uint32_t count, const FieldView& field, const FixedGrid& grid,
+                                            const FixedPose (&q)[P], double (&acc)[P], uint32_t (&margin)[P]) {
+  uint32_t b = 0;
+  if (4 <= count) {
+    // Software pipeline: the loads of the next four beams are issued before the previous four are summed (a warp issues
+    // in order: summing first would leave it with four loads in flight, then none).  Two groups per iteration, loaded
+    // alternately into f and g: no register copies between groups.
+    double f[4][P], g[4][P];
+    fixed_group<P, kInGrid>(f, pts, 0, field, grid, q, margin);
+    b = 4;
+#pragma unroll kRwUnroll
+    for (; b + 8 <= count; b += 8) {
+      fixed_group<P, kInGrid>(g, pts, b, field, grid, q, margin);
+      fixed_add<P>(acc, f);
+      fixed_group<P, kInGrid>(f, pts, b + 4, field, grid, q, margin);
+      fixed_add<P>(acc, g);
+    }
+    if (b + 4 <= count) {
+      fixed_group<P, kInGrid>(g, pts, b, field, grid, q, margin);
+      fixed_add<P>(acc, f);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int k = 0; k < P; ++k) f[j][k] = g[j][k];
+      }
+      b += 4;
+    }
+    fixed_add<P>(acc, f);
+  }
+  for (; b < count; ++b) {
+    const double2 p = pts[b];
+#pragma unroll
+    for (int k = 0; k < P; ++k) acc[k] = acc[k] + fixed_lookup<kInGrid>(kInGrid ? field.bordered_biased : field.bordered, grid, q[k], p.x, p.y, margin[k]);
+  }
+}
+
+/// Adds the field values of pts[0, count) to the P sums acc: the fixed-point loop, then the reference's own operation
+/// sequence from the sum it started with for a particle whose margin ends at or below kFixedAmbiguous.  `pts` is the
+/// ScanParam in the constant bank or a chunk in shared memory.
+template <int P>
+__device__ __forceinline__ void fixed_sum(const FieldView& field, const Pose2* __restrict__ states, const FixedGrid& grid,
+                                          const FixedPose (&q)[P], const uint32_t (&margin_start)[P], const uint64_t (&i)[P],
+                                          const bool (&active)[P], const double2* pts, uint32_t count, double (&acc)[P]) {
+  double acc_before[P];
+  uint32_t margin[P];
+#pragma unroll
+  for (int k = 0; k < P; ++k) acc_before[k] = acc[k], margin[k] = margin_start[k];
+  if (grid.in_grid) {
+    fixed_beams<P, true>(pts, count, field, grid, q, acc, margin);
+  } else {
+    fixed_beams<P, false>(pts, count, field, grid, q, acc, margin);
+  }
+#pragma unroll
+  for (int k = 0; k < P; ++k) {
+    if (margin[k] <= kFixedAmbiguous) {  // a coordinate within ~2^-30 cells of a cell edge, or a particle out of range
+      const Pose2 t = field_frame_pose(field, states, i[k], active[k]);
+      acc[k] = transform_reduce_exact<1>(pts, count, acc_before[k],
+                                         [&](double2 p) { return bordered_lookup_exact(field, p.x, p.y, t.c, t.s, t.x, t.y); });
+    }
+  }
+}
 
 /// Per-particle constants of the fixed-point evaluation.  Returns whether every end point of the particle stays inside
 /// the grid.
@@ -770,7 +791,7 @@ __global__ void __launch_bounds__(kRwThreads, P == 1 ? kRwBlocksPerSm : kRwPairB
     for (int k = 0; k < P; ++k) {
       const uint64_t slot = ticket * kTask + static_cast<uint64_t>(k) * kWarp + lane;
       active[k] = slot < n;
-      i[k] = active[k] ? (perm != nullptr ? perm[slot] : slot) : 0;
+      i[k] = slot_particle(perm, slot, active[k]);
     }
     bool inside = fixed_pose_setup(field, states, i[0], active[0], points_radius, q[0], margin_start[0]);
 #pragma unroll
@@ -778,16 +799,11 @@ __global__ void __launch_bounds__(kRwThreads, P == 1 ? kRwBlocksPerSm : kRwPairB
     const FixedGrid grid = fixed_grid_setup(field, inside);
 #pragma unroll
     for (int k = 0; k < P; ++k) acc[k] = field.init;
-#define BB200_POINT(k) scan.p[(k)]
-    BB200_FIXED_SUM(BB200_POINT, n_points, P);
-#undef BB200_POINT
+    fixed_sum<P>(field, states, grid, q, margin_start, i, active, scan.p, n_points, acc);
 #pragma unroll
     for (int k = 0; k < P; ++k) {
       if (active[k]) {
-        const double likelihood = field.exp_epilogue ? exp(acc[k]) : acc[k];
-        const double w = weights[i[k]] * likelihood;  // actions/reweight.hpp:54-60
-        weights[i[k]] = w;
-        const unsigned long long bits = weight_order_bits(w);
+        const unsigned long long bits = store_reweighted(field, weights, i[k], weights[i[k]], acc[k]);
         best = bits > best ? bits : best;
       }
     }
@@ -814,54 +830,18 @@ __global__ void __launch_bounds__(kRwThreads, P == 1 ? kRwBlocksPerSm : kRwPairB
 __device__ __forceinline__ void reweight_lfm_fixed_block(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n,
                                                          const uint32_t* __restrict__ perm, const FieldView& field, const double2* __restrict__ points,
                                                          uint32_t n_points, double points_radius, Scalars* __restrict__ scalars, uint64_t slot_base) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  double2* s_pts = reinterpret_cast<double2*>(smem_raw);
-  __shared__ __align__(8) uint64_t s_bar;
-  __shared__ unsigned long long s_max;
-  __shared__ unsigned int s_arrived;
-
   const uint64_t slot = slot_base + threadIdx.x;
   const bool active[1] = {slot < n};
-  const uint64_t i[1] = {active[0] ? (perm != nullptr ? perm[slot] : slot) : 0};
-  if (threadIdx.x == 0) {
-    s_max = 0ull;
-    s_arrived = 0u;
-    mbarrier_init(&s_bar, 1);
-    mbarrier_init_fence();
-  }
+  const uint64_t i[1] = {slot_particle(perm, slot, active[0])};
   uint32_t margin_start[1];
   FixedPose q[1];
   const FixedGrid grid = fixed_grid_setup(field, fixed_pose_setup(field, states, i[0], active[0], points_radius, q[0], margin_start[0]));
-
   double acc[1] = {field.init};
-  __syncthreads();  // s_max and the barrier initialised
-  uint32_t phase = 0;
-  for (uint32_t base = 0; base < n_points; base += kChunkBeams) {
-    const uint32_t count = min(kChunkBeams, n_points - base);
-    if (threadIdx.x == 0) {
-      const uint32_t bytes = count * static_cast<uint32_t>(sizeof(double2));
-      mbarrier_expect_tx(&s_bar, bytes);
-      bulk_copy_g2s(s_pts, points + base, bytes, &s_bar);
-    }
-    mbarrier_wait(&s_bar, phase);
-    phase ^= 1u;
-#define BB200_POINT(k) s_pts[(k)]
-    BB200_FIXED_SUM(BB200_POINT, count, 1);
-#undef BB200_POINT
-    if (base + kChunkBeams < n_points) __syncthreads();
-  }
-  double w = 0.0;
-  if (active[0]) {
-    const double likelihood = field.exp_epilogue ? exp(acc[0]) : acc[0];
-    w = weights[i[0]] * likelihood;  // actions/reweight.hpp:54-60
-    weights[i[0]] = w;
-  }
-  publish_weight_max(active[0] ? weight_order_bits(w) : 0ull, &s_max, &s_arrived, kRwThreads / kWarp, scalars);
+  staged_scan_block(
+      points, n_points, scalars,
+      [&](const double2* pts, uint32_t count) { fixed_sum<1>(field, states, grid, q, margin_start, i, active, pts, count, acc); },
+      [&] { return active[0] ? store_reweighted(field, weights, i[0], weights[i[0]], acc[0]) : 0ull; });
 }
-#undef BB200_FIXED_SUM
-#undef BB200_FIXED_BEAMS
-#undef BB200_FIXED_ADD
-#undef BB200_FIXED_GROUP
 
 __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm)
     reweight_lfm_fixed_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, const uint32_t* __restrict__ perm,

@@ -20,7 +20,7 @@ M32 = 1 << 32
 
 
 def in_grid(tx, ty, inv, radius, width, height):
-    """fixed_particle_setup: the square of points_radius * inv + 2 cells around the position lies inside the grid."""
+    """fixed_pose_setup: the square of points_radius * inv + 2 cells around the position lies inside the grid."""
     cells = radius * inv + 2.0
     gx, gy = tx * inv, ty * inv
     return gx - cells >= 0.0 and gx + cells < width and gy - cells >= 0.0 and gy + cells < height

@@ -803,6 +803,27 @@ class AmclBatch:
         self._check(self._lib.bb200_amcl_batch_cluster_estimate(self._h, member, C.byref(p), C.byref(est)))
         return np.array(est.mean), np.array(est.cov).reshape(3, 3)
 
+    def cluster_estimates(self, present=None, linear: float = 0.20, angular: float = 0.524, percentile: float = 0.90, with_counts: bool = False):
+        """beluga::cluster_based_estimate of every member whose `present` entry is true (None: all), in one call with a fixed
+        number of kernel launches -> one (mean[4], cov[3, 3]) per member, None for members not selected; with_counts makes
+        each entry (mean, cov, n_cells, n_clusters)."""
+        k = len(self.params)
+        if present is not None and len(present) != k:
+            raise ValueError("one presence flag per member")
+        p = _capi.ClusterParam(linear, angular, percentile)
+        mask = None if present is None else (C.c_uint8 * k)(*[1 if x else 0 for x in present])
+        est = (_capi.Estimate * k)()
+        cells, clusters = (C.c_uint32 * k)(), (C.c_uint32 * k)()
+        self._check(self._lib.bb200_amcl_batch_cluster_estimates(self._h, C.byref(p), mask, est, cells, clusters))
+        out = []
+        for m in range(k):
+            if present is not None and not present[m]:
+                out.append(None)
+                continue
+            e = (np.array(est[m].mean), np.array(est[m].cov).reshape(3, 3))
+            out.append((*e, cells[m], clusters[m]) if with_counts else e)
+        return out
+
     def update(self, control_poses, points, present=None) -> list:
         """Amcl::update for every member whose `present` entry is true (None: all).  `control_poses`: K poses [c, s, x, y];
         `points[m]`: member m's (x, y) points.  Returns K UpdateResult blocks; `.updated == 0` for absent members."""

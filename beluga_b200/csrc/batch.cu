@@ -10,16 +10,11 @@ namespace bb200 {
 namespace {
 
 constexpr uint64_t kSliceAlign = 32;  // particles
+static_assert(kBatchMaxParticles <= kBatchClusterMaxParticles, "the batch cluster estimate packs a member's particle index into 15 bits");
 
 /// Moment-partial rows a member of `capacity` particles can need in the finish launch (whichever form it takes).
 uint64_t finish_rows(uint64_t capacity) {
   return std::max<uint64_t>({resample_scatter_block_count(capacity), resample_block_count(capacity), moments_block_count(capacity)});
-}
-
-uint64_t largest_member(const bb200_amcl_param* params, int n_members) {
-  uint64_t largest = 0;
-  for (int k = 0; params != nullptr && k < n_members; ++k) largest = std::max(largest, params[k].max_particles);
-  return largest;
 }
 
 }  // namespace
@@ -45,8 +40,7 @@ int Batch::validate(const bb200_amcl_param* params, const bb200_motion_param* mo
   return BB200_OK;
 }
 
-Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members)
-    : clusterizer_(largest_member(params, n_members)) {
+Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members) {
   create_status_ = validate(params, motions, n_members, &error_);
   if (create_status_ != BB200_OK) return;
   uint64_t tiles = 0, rows = 0;
@@ -60,6 +54,10 @@ Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, 
     m.offset = total_;
     m.capacity = params[k].max_particles;
     total_ += m.capacity;
+    m.table_offset = table_total_;
+    m.table_slots = 2;
+    while (m.table_slots < 2 * m.capacity) m.table_slots <<= 1;
+    table_total_ += m.table_slots;
     tiles += batch_scan_tiles(m.capacity);
     rows += finish_rows(m.capacity);
     record_ancestors_ = record_ancestors_ || params[k].record_ancestors != 0;
@@ -95,9 +93,12 @@ Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, 
 Batch::~Batch() {
   if (stream_ != nullptr) cudaStreamSynchronize(stream_);
   for (void* p : std::initializer_list<void*>{states_[0], states_[1], weights_, cdf_, ancestors_, scalars_, tile_state_, partials_, table_, first_,
-                                              points_, members_done_})
+                                              points_, members_done_, cl_hashes_, cl_keys_, cl_first_, cl_ids_, cl_cell_of_, cl_sort_[0], cl_sort_[1],
+                                              cl_starts_, cl_records_, cl_table_, cl_cells_})
     cudaFree(p);
-  for (void* p : std::initializer_list<void*>{table_host_, first_host_, points_host_, summary_host_, ticket_host_}) cudaFreeHost(p);
+  for (void* p : std::initializer_list<void*>{table_host_, first_host_, points_host_, summary_host_, ticket_host_, cl_table_host_, cl_cells_host_,
+                                              cl_records_host_})
+    cudaFreeHost(p);
   if (stream_ != nullptr) cudaStreamDestroy(stream_);
 }
 
@@ -204,9 +205,118 @@ int Batch::ancestors(int member, int64_t* out, uint64_t capacity) {
 
 int Batch::cluster_estimate(int member, const bb200_cluster_param& p, bb200_estimate* out) {
   BB_MEMBER(member);
-  const Member& m = members_[static_cast<size_t>(member)];
+  std::vector<uint8_t> present(members_.size(), 0);
+  present[static_cast<size_t>(member)] = 1;
+  std::vector<bb200_estimate> all(members_.size());  // indexed by member
+  const int st = cluster_estimates(p, present.data(), all.data(), nullptr, nullptr);
+  if (st == BB200_OK) *out = all[static_cast<size_t>(member)];
+  return st;
+}
+
+int Batch::ensure_cluster_scratch() {
+  if (cl_cells_host_ != nullptr) return BB200_OK;
+  const size_t k = members_.size();
+  BB_CHECK(dev_alloc(&cl_hashes_, total_));
+  BB_CHECK(dev_alloc(&cl_keys_, table_total_));
+  BB_CHECK(dev_alloc(&cl_first_, table_total_));
+  BB_CHECK(dev_alloc(&cl_ids_, table_total_));
+  BB_CHECK(dev_alloc(&cl_cell_of_, total_));
+  BB_CHECK(dev_alloc(&cl_sort_[0], total_));
+  BB_CHECK(dev_alloc(&cl_sort_[1], total_));
+  BB_CHECK(dev_alloc(&cl_starts_, total_ + k));
+  BB_CHECK(dev_alloc(&cl_records_, total_));
+  BB_CHECK(dev_alloc(&cl_table_, k));
+  BB_CHECK(host_alloc(&cl_table_host_, k));
+  BB_CHECK(dev_alloc(&cl_cells_, k));
+  BB_CHECK(host_alloc(&cl_cells_host_, k));  // last: marks the scratch as allocated
+  return BB200_OK;
+}
+
+int Batch::ensure_cluster_records(uint64_t cells) {
+  if (cells <= cl_records_host_capacity_) return BB200_OK;
+  cudaFreeHost(cl_records_host_);
+  cl_records_host_ = nullptr;
+  cl_records_host_capacity_ = 0;
+  const uint64_t want = std::min<uint64_t>(total_, std::max<uint64_t>(4096, 2 * cells));
+  BB_CHECK(host_alloc(&cl_records_host_, want));
+  cl_records_host_capacity_ = want;
+  return BB200_OK;
+}
+
+int Batch::cluster_estimates(const bb200_cluster_param& p, const uint8_t* present, bb200_estimate* out, uint32_t* n_cells, uint32_t* n_clusters) {
+  error_.clear();
+  if (!(p.linear_hash_resolution > 0.0) || !(p.angular_hash_resolution > 0.0) || !(p.weight_cap_percentile >= 0.0) ||
+      !(p.weight_cap_percentile < 1.0))
+    return fail(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)");
+  std::vector<uint32_t> selected;  // in member order
+  for (size_t k = 0; k < members_.size(); ++k) {
+    if (present != nullptr && present[k] == 0) continue;
+    if (members_[k].n == 0) return fail(BB200_ERR_STATE, "member " + std::to_string(k) + ": no particles");
+    selected.push_back(static_cast<uint32_t>(k));
+  }
+  if (selected.empty()) return BB200_OK;
   BB_CHECK(cudaSetDevice(device_));
-  return clusterizer_.estimate(states_[m.cur] + m.offset, weights_ + m.offset, m.n, m.pivot, p, stream_, out, nullptr, 0, nullptr, nullptr, &error_);
+  if (const int st = ensure_cluster_scratch()) return st;  // every batch call ends synchronised: the pinned buffers are free
+
+  const uint32_t n_sel = static_cast<uint32_t>(selected.size());
+  for (uint32_t j = 0; j < n_sel; ++j) {
+    const uint32_t k = selected[j];
+    const Member& m = members_[k];
+    BatchClusterMember& c = cl_table_host_[j];
+    c = BatchClusterMember{};
+    c.offset = m.offset;
+    c.table_offset = m.table_offset;
+    c.starts_offset = m.offset + k;  // a member's cells + 1 starts end before the next member's slice begins
+    c.n = static_cast<uint32_t>(m.n);
+    c.table_mask = m.table_slots - 1;
+    c.cur = static_cast<uint32_t>(m.cur);
+    c.pivot_x = m.pivot[0];
+    c.pivot_y = m.pivot[1];
+  }
+  cudaStream_t stream = stream_;
+  BB_CHECK(cudaMemcpyAsync(cl_table_, cl_table_host_, n_sel * sizeof(BatchClusterMember), cudaMemcpyHostToDevice, stream));
+  BatchClusterArgs a{};
+  a.members = cl_table_;
+  a.states[0] = states_[0];
+  a.states[1] = states_[1];
+  a.weights = weights_;
+  a.linear = p.linear_hash_resolution;
+  a.angular = p.angular_hash_resolution;
+  a.hashes = cl_hashes_;
+  a.keys = cl_keys_;
+  a.first = cl_first_;
+  a.ids = cl_ids_;
+  a.cell_of = cl_cell_of_;
+  a.sort_a = cl_sort_[0];
+  a.sort_b = cl_sort_[1];
+  a.starts = cl_starts_;
+  a.records = cl_records_;
+  a.cells = cl_cells_;
+  launch_batch_cluster_cells(a, n_sel, stream);
+  BB_LAUNCHED("batch_cluster_cells");
+  BB_CHECK(cudaMemcpyAsync(cl_cells_host_, cl_cells_, n_sel * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+  BB_CHECK(cudaStreamSynchronize(stream));  // 1: the cell counts size the records' read-back
+  uint64_t total_cells = 0;
+  for (uint32_t j = 0; j < n_sel; ++j) total_cells += cl_cells_host_[j];
+  if (const int st = ensure_cluster_records(total_cells)) return st;
+  launch_batch_cluster_compact(cl_table_, cl_cells_, cl_records_, n_sel, cl_records_host_, stream);
+  BB_LAUNCHED("batch_cluster_compact");
+  BB_CHECK(cudaStreamSynchronize(stream));  // 2: every record is in pinned memory
+
+  // Host pass per member (Clusterizer::estimate's): the flood over the cells, then the estimate about the member's pivot.
+  static_assert(sizeof(HostCell) == sizeof(CellRecord), "record layouts must agree");
+  const HostCell* cells = reinterpret_cast<const HostCell*>(cl_records_host_);
+  for (uint32_t j = 0; j < n_sel; ++j) {
+    const uint32_t k = selected[j];
+    const Member& m = members_[k];
+    const uint32_t count = cl_cells_host_[j];
+    const ClusterSelection sel = select_cluster(cells, count, m.n, p.linear_hash_resolution, p.angular_hash_resolution, p.weight_cap_percentile);
+    if (out != nullptr) estimate_from_moments(sel.moments, m.pivot, &out[k]);
+    if (n_cells != nullptr) n_cells[k] = count;
+    if (n_clusters != nullptr) n_clusters[k] = sel.clusters;
+    cells += count;
+  }
+  return BB200_OK;
 }
 
 int Batch::ensure_points(uint64_t n_points) {

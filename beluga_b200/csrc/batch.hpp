@@ -40,7 +40,12 @@ class Batch {
   int force_update(int member);
   int get_particles(int member, double* states, double* weights, uint64_t capacity);
   int ancestors(int member, int64_t* out, uint64_t capacity);
+  /// The cluster estimate of one member: cluster_estimates with that member alone selected.
   int cluster_estimate(int member, const bb200_cluster_param& p, bb200_estimate* out);
+  /// beluga::cluster_based_estimate of every member whose present[m] is non-zero (present == nullptr: all of them): two
+  /// kernel launches and two host synchronisations whatever K and the cell counts are.  out[m], n_cells[m] and
+  /// n_clusters[m] (either may be nullptr) are written for selected members only.
+  int cluster_estimates(const bb200_cluster_param& p, const uint8_t* present, bb200_estimate* out, uint32_t* n_cells, uint32_t* n_clusters);
   /// Amcl::update for every member whose present[m] is non-zero (present == nullptr: all of them).  Atomic for the whole
   /// batch: when the device half fails, every member's host state is rolled back.
   int update(const double* control_poses, const double* const* points_xy, const uint64_t* n_points, const uint8_t* present,
@@ -55,6 +60,8 @@ class Batch {
     int cur{0};            // state buffer holding the particles
     double pivot[2]{0.0, 0.0};
     uint64_t ancestors_n{0};
+    uint64_t table_offset{0};  // its hash table in the cluster scratch
+    uint32_t table_slots{0};   // a power of two >= 2 * capacity
   };
   int fail(int status, const std::string& message) {
     error_ = message;
@@ -63,12 +70,13 @@ class Batch {
   int check(cudaError_t e, const char* what) { return cuda_check(e, what, &error_); }
   int member_ok(int member) const;
   int ensure_points(uint64_t n_points);
+  int ensure_cluster_scratch();
+  int ensure_cluster_records(uint64_t cells);
 
   std::vector<Member> members_;
   int device_{0};
   cudaStream_t stream_{nullptr};
   DeviceMap map_;
-  Clusterizer clusterizer_;  // sized for the largest member
   bool created_{false};
   int create_status_{BB200_OK};
   mutable std::string error_;
@@ -94,6 +102,24 @@ class Batch {
   unsigned int* members_done_{nullptr};
   int seq_{0};
   uint64_t launches_{0};
+
+  // Cluster estimate scratch (allocated on first use): per-member slices of the particle-sized buffers, and the hash
+  // tables back to back.
+  uint64_t table_total_{0};
+  unsigned long long* cl_hashes_{nullptr};
+  unsigned long long* cl_keys_{nullptr};
+  unsigned int* cl_first_{nullptr};
+  uint32_t* cl_ids_{nullptr};
+  uint32_t* cl_cell_of_{nullptr};
+  uint32_t* cl_sort_[2]{nullptr, nullptr};
+  uint32_t* cl_starts_{nullptr};
+  CellRecord* cl_records_{nullptr};
+  BatchClusterMember* cl_table_{nullptr};       // device
+  BatchClusterMember* cl_table_host_{nullptr};  // pinned
+  uint32_t* cl_cells_{nullptr};                 // device
+  uint32_t* cl_cells_host_{nullptr};            // pinned
+  CellRecord* cl_records_host_{nullptr};        // pinned, written by the compaction kernel
+  uint64_t cl_records_host_capacity_{0};
 };
 
 }  // namespace bb200

@@ -852,6 +852,11 @@ int bb200_amcl_batch_cluster_estimate(bb200_amcl_batch* b, int member, const bb2
   BB_REQUIRE(b && p && out);
   return guarded(b->impl, [&] { return b->impl.cluster_estimate(member, *p, out); });
 }
+int bb200_amcl_batch_cluster_estimates(bb200_amcl_batch* b, const bb200_cluster_param* p, const uint8_t* present, bb200_estimate* out,
+                                       uint32_t* n_cells, uint32_t* n_clusters) {
+  BB_REQUIRE(b && p && out);
+  return guarded(b->impl, [&] { return b->impl.cluster_estimates(*p, present, out, n_cells, n_clusters); });
+}
 int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, const double* const* points_xy, const uint64_t* n_points,
                             const uint8_t* present, bb200_update_result* out) {
   BB_REQUIRE(b && control_poses && points_xy && n_points && out);

@@ -3,6 +3,7 @@
 //   cluster_cell_of                 dense cell id per particle (cells numbered by first occurrence)
 //   radix_histogram / radix_scatter stable LSD radix sort of the particle indices by cell id
 //   cluster_cells                   one warp per cell: ordered weight sum, moments, representative
+//   batch_cluster_cells / _compact  the same stages for every selected member of a batch, one CTA per member
 // Nothing here uses floating-point atomics: every sum has a fixed order, so results are reproducible
 // run to run and the per-cell weight is the reference's sequential sum bit for bit.
 #include "cluster.cuh"
@@ -146,15 +147,13 @@ __global__ void __launch_bounds__(kSortThreads) radix_scatter_kernel(const uint3
 
 constexpr int kCellThreads = 128;
 
-__global__ void __launch_bounds__(kCellThreads) cluster_cells_kernel(const Pose2* __restrict__ states, const double* __restrict__ weights,
-                                                                    const unsigned long long* __restrict__ hashes,
-                                                                    const uint32_t* __restrict__ sorted_idx, const uint32_t* __restrict__ starts,
-                                                                    uint32_t cells, double px, double py, CellRecord* __restrict__ records) {
-  const uint32_t cell = (blockIdx.x * kCellThreads + threadIdx.x) / kWarp;
-  if (cell >= cells) return;  // whole warps leave together
+/// The record of one cell, built by one warp: sorted_idx[begin, end) are the cell's particles in particle order.  Each lane
+/// gathers every 32nd particle, the moments meet in a fixed xor-shuffle tree, and the weight is the reference's sequential
+/// sum.  The single-filter and the batch kernels both build their records here, so the two agree bit for bit.
+__device__ __forceinline__ void cell_record_warp(const Pose2* states, const double* weights, const unsigned long long* hashes,
+                                                 const uint32_t* sorted_idx, uint32_t begin, uint32_t end, double px, double py,
+                                                 CellRecord* record) {
   const int lane = threadIdx.x % kWarp;
-  const uint32_t begin = starts[cell], end = starts[cell + 1];
-
   double m[kMomentCount];
 #pragma unroll
   for (int k = 0; k < kMomentCount; ++k) m[k] = 0.0;
@@ -209,7 +208,7 @@ __global__ void __launch_bounds__(kCellThreads) cluster_cells_kernel(const Pose2
     }
   }
   if (lane == 0) {
-    const uint32_t first = sorted_idx[begin];  // stable sort: the cell's earliest particle
+    const uint32_t first = sorted_idx[begin];  // particle order inside the cell: the cell's earliest particle
     CellRecord r;
     r.hash = hashes[first];
     r.first_index = first;
@@ -218,8 +217,199 @@ __global__ void __launch_bounds__(kCellThreads) cluster_cells_kernel(const Pose2
     r.representative = load_state(states + first);
 #pragma unroll
     for (int k = 0; k < kMomentCount; ++k) r.moments[k] = m[k];
-    records[cell] = r;
+    *record = r;
   }
+}
+
+__global__ void __launch_bounds__(kCellThreads) cluster_cells_kernel(const Pose2* __restrict__ states, const double* __restrict__ weights,
+                                                                    const unsigned long long* __restrict__ hashes,
+                                                                    const uint32_t* __restrict__ sorted_idx, const uint32_t* __restrict__ starts,
+                                                                    uint32_t cells, double px, double py, CellRecord* __restrict__ records) {
+  const uint32_t cell = (blockIdx.x * kCellThreads + threadIdx.x) / kWarp;
+  if (cell >= cells) return;  // whole warps leave together
+  cell_record_warp(states, weights, hashes, sorted_idx, starts[cell], starts[cell + 1], px, py, records + cell);
+}
+
+// ---- every selected member of a batch: one CTA per member -------------------------------------------
+// The CTA runs the whole per-particle half of its member (at most kBatchClusterMaxParticles particles) with the
+// single-filter stages as block-wide loops: hash set, first-occurrence numbering in particle order, stable LSD sort of
+// the particle indices by cell, segment starts, one record per cell.  A member's scratch is its own slice of the batch
+// buffers, so no CTA waits for another.
+
+constexpr int kBatchCellThreads = 1024;
+constexpr int kBatchCellWarps = kBatchCellThreads / kWarp;
+constexpr int kIndexBits = 15;  // particle index inside a member: < kBatchClusterMaxParticles
+static_assert(kBatchClusterMaxParticles == (1u << kIndexBits), "sort values pack (cell, particle index) into 30 bits");
+
+__global__ void __launch_bounds__(kBatchCellThreads) batch_cluster_cells_kernel(const BatchClusterArgs a) {
+  __shared__ uint32_t s_warp[kBatchCellWarps];            // head flags per warp in the current chunk
+  __shared__ uint32_t s_base[kRadix];                     // digit counts, then the next free output position per digit
+  __shared__ uint32_t s_count[kBatchCellWarps][kRadix];   // keys per (warp, digit) in the current chunk
+  const BatchClusterMember mb = a.members[blockIdx.x];
+  const uint32_t n = mb.n;
+  const Pose2* states = (mb.cur != 0 ? a.states[1] : a.states[0]) + mb.offset;
+  const double* weights = a.weights + mb.offset;
+  unsigned long long* hashes = a.hashes + mb.offset;
+  unsigned long long* keys = a.keys + mb.table_offset;
+  unsigned int* first = a.first + mb.table_offset;
+  uint32_t* ids = a.ids + mb.table_offset;
+  uint32_t* cell_of = a.cell_of + mb.offset;
+  uint32_t* starts = a.starts + mb.starts_offset;
+  const uint64_t mask = mb.table_mask;
+  const int tid = threadIdx.x, lane = tid % kWarp, warp = tid / kWarp;
+  const unsigned lanes_below = (1u << lane) - 1u;
+
+  for (uint64_t s = tid; s <= mask; s += kBatchCellThreads) {
+    keys[s] = kEmpty;
+    first[s] = ~0u;
+  }
+  __syncthreads();
+  // spatial_hash<SE2d>{linear, linear, angular} of every state into the set "cell -> smallest particle index".
+  for (uint32_t i = tid; i < n; i += kBatchCellThreads) {
+    const unsigned long long hash = spatial_hash(load_state(states + i), a.linear, a.linear, a.angular);
+    hashes[i] = hash;
+    const unsigned long long key = hash == kEmpty ? kEmpty - 1 : hash;
+    uint64_t pos = probe_start(key, mask);
+    for (;;) {
+      const unsigned long long prev = atomicCAS(keys + pos, kEmpty, key);
+      if (prev == kEmpty || prev == key) {
+        atomicMin(first + pos, i);
+        break;
+      }
+      pos = (pos + 1) & mask;
+    }
+  }
+  __syncthreads();
+  // Cells numbered by first occurrence: chunk by chunk in particle order, a cell's first particle takes the next number.
+  uint32_t cells = 0;
+  for (uint32_t base = 0; base < n; base += kBatchCellThreads) {
+    const uint32_t i = base + tid;
+    uint32_t pos = 0;
+    bool head = false;
+    if (i < n) {
+      const unsigned long long hash = hashes[i];
+      const unsigned long long key = hash == kEmpty ? kEmpty - 1 : hash;
+      pos = static_cast<uint32_t>(probe_start(key, mask));
+      while (keys[pos] != key) pos = (pos + 1) & mask;
+      head = first[pos] == i;
+      cell_of[i] = pos;  // the slot for now, the cell id below
+    }
+    const unsigned heads = __ballot_sync(0xffffffffu, head);
+    if (lane == 0) s_warp[warp] = __popc(heads);
+    __syncthreads();
+    uint32_t before = cells;
+    for (int w = 0; w < kBatchCellWarps; ++w) {
+      const uint32_t c = s_warp[w];
+      if (w < warp) before += c;
+      cells += c;
+    }
+    if (head) ids[pos] = before + __popc(heads & lanes_below);
+    __syncthreads();
+  }
+  // Sort values (cell << 15 | particle index), in particle order.
+  uint32_t* in = a.sort_a + mb.offset;
+  uint32_t* out = a.sort_b + mb.offset;
+  for (uint32_t i = tid; i < n; i += kBatchCellThreads) {
+    const uint32_t cell = ids[cell_of[i]];
+    cell_of[i] = cell;
+    in[i] = cell << kIndexBits | i;
+  }
+  __syncthreads();
+  // Stable LSD radix sort by cell, 8 bits per pass: the order of a stable sort of the particle indices by cell, which is
+  // also the order of the unique keys cell * 2^15 + index.  The last pass keeps the particle index only.
+  const int passes = cells > kRadix ? 2 : 1;
+  for (int pass = 0; pass < passes; ++pass) {
+    const int shift = kIndexBits + 8 * pass;
+    const bool last = pass == passes - 1;
+    if (tid < kRadix) s_base[tid] = 0;
+    __syncthreads();
+    for (uint32_t i = tid; i < n; i += kBatchCellThreads) atomicAdd(&s_base[(in[i] >> shift) & (kRadix - 1)], 1u);
+    __syncthreads();
+    if (warp == 0) {  // exclusive scan of the 256 digit counts, 8 per lane
+      constexpr int kPer = kRadix / kWarp;
+      uint32_t v[kPer], sum = 0;
+#pragma unroll
+      for (int k = 0; k < kPer; ++k) {
+        v[k] = s_base[lane * kPer + k];
+        sum += v[k];
+      }
+      uint32_t incl = sum;
+#pragma unroll
+      for (int off = 1; off < kWarp; off <<= 1) {
+        const uint32_t o = __shfl_up_sync(0xffffffffu, incl, off);
+        if (lane >= off) incl += o;
+      }
+      uint32_t running = incl - sum;
+#pragma unroll
+      for (int k = 0; k < kPer; ++k) {
+        s_base[lane * kPer + k] = running;
+        running += v[k];
+      }
+    }
+    __syncthreads();
+    for (uint32_t base = 0; base < n; base += kBatchCellThreads) {
+      for (int k = tid; k < kBatchCellWarps * kRadix; k += kBatchCellThreads) (&s_count[0][0])[k] = 0;
+      __syncthreads();
+      const uint32_t e = base + tid;
+      const bool valid = e < n;
+      const uint32_t v = valid ? in[e] : 0u;
+      const uint32_t digit = valid ? ((v >> shift) & (kRadix - 1)) : kRadix;  // invalid lanes form their own group
+      const unsigned peers = __match_any_sync(0xffffffffu, digit);
+      const uint32_t rank = __popc(peers & lanes_below);
+      if (valid && rank == 0) s_count[warp][digit] = __popc(peers);
+      __syncthreads();
+      if (tid < kRadix) {  // thread d turns the per-warp counts of digit d into offsets (warp order = element order)
+        uint32_t running = s_base[tid];
+        for (int w = 0; w < kBatchCellWarps; ++w) {
+          const uint32_t c = s_count[w][tid];
+          s_count[w][tid] = running;
+          running += c;
+        }
+        s_base[tid] = running;
+      }
+      __syncthreads();
+      if (valid) out[s_count[warp][digit] + rank] = last ? (v & (kBatchClusterMaxParticles - 1)) : v;
+      __syncthreads();
+    }
+    uint32_t* t = in;
+    in = out;
+    out = t;
+  }
+  const uint32_t* sorted = in;
+  // Segment starts: a cell begins where the sorted sequence changes cell.
+  for (uint32_t p = tid; p < n; p += kBatchCellThreads) {
+    const uint32_t cell = cell_of[sorted[p]];
+    if (p == 0 || cell != cell_of[sorted[p - 1]]) starts[cell] = p;
+  }
+  if (tid == 0) starts[cells] = n;
+  __syncthreads();
+  CellRecord* records = a.records + mb.offset;
+  for (uint32_t c = warp; c < cells; c += kBatchCellWarps)
+    cell_record_warp(states, weights, hashes, sorted, starts[c], starts[c + 1], mb.pivot_x, mb.pivot_y, records + c);
+  if (tid == 0) a.cells[blockIdx.x] = cells;
+}
+
+/// Member j's records move from its slice to out[cells of members 0 .. j-1 ...]: one CTA per member, 16 bytes per thread.
+constexpr int kCompactThreads = 256;
+
+__global__ void __launch_bounds__(kCompactThreads) batch_cluster_compact_kernel(const BatchClusterMember* __restrict__ members,
+                                                                                 const uint32_t* __restrict__ cells, const CellRecord* __restrict__ records,
+                                                                                 CellRecord* __restrict__ out) {
+  __shared__ uint64_t s_sum[kCompactThreads / kWarp];
+  uint64_t sum = 0;
+  for (uint32_t j = threadIdx.x; j < blockIdx.x; j += kCompactThreads) sum += cells[j];
+#pragma unroll
+  for (int off = kWarp / 2; off > 0; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
+  if (threadIdx.x % kWarp == 0) s_sum[threadIdx.x / kWarp] = sum;
+  __syncthreads();
+  uint64_t dst = 0;
+#pragma unroll
+  for (int w = 0; w < kCompactThreads / kWarp; ++w) dst += s_sum[w];
+  constexpr int kWords = sizeof(CellRecord) / sizeof(double2);
+  const double2* src = reinterpret_cast<const double2*>(records + members[blockIdx.x].offset);
+  double2* to = reinterpret_cast<double2*>(out + dst);
+  const uint64_t words = static_cast<uint64_t>(cells[blockIdx.x]) * kWords;
+  for (uint64_t k = threadIdx.x; k < words; k += kCompactThreads) to[k] = src[k];
 }
 
 int bits_for(uint32_t values) {  // bits needed to represent 0 .. values-1
@@ -272,6 +462,15 @@ void launch_cluster_records(const Pose2* states, const double* weights, const ui
                             const ClusterScratch& s, cudaStream_t stream) {
   const unsigned cell_blocks = static_cast<unsigned>((static_cast<uint64_t>(cells) * kWarp + kCellThreads - 1) / kCellThreads);
   cluster_cells_kernel<<<cell_blocks, kCellThreads, 0, stream>>>(states, weights, s.hashes, sorted_idx, s.starts, cells, pivot_x, pivot_y, s.records);
+}
+
+void launch_batch_cluster_cells(const BatchClusterArgs& a, uint32_t n_members, cudaStream_t stream) {
+  batch_cluster_cells_kernel<<<n_members, kBatchCellThreads, 0, stream>>>(a);
+}
+
+void launch_batch_cluster_compact(const BatchClusterMember* members, const uint32_t* cells, const CellRecord* records, uint32_t n_members,
+                                  CellRecord* out, cudaStream_t stream) {
+  batch_cluster_compact_kernel<<<n_members, kCompactThreads, 0, stream>>>(members, cells, records, out);
 }
 
 // ---- Clusterizer -------------------------------------------------------------------------------------

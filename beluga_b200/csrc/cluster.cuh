@@ -68,7 +68,48 @@ const uint32_t* launch_cluster_sort(uint64_t n, uint32_t cells, const ClusterScr
 void launch_cluster_records(const Pose2* states, const double* weights, const uint32_t* sorted_idx, uint32_t cells, double pivot_x, double pivot_y,
                             const ClusterScratch& s, cudaStream_t stream);
 
-/// The clusterizer of a filter or a batch: scratch for up to `capacity` particles on one device, allocated on first use,
+// ---- every selected member of a batch at once ------------------------------------------------------------------------
+
+/// Largest member a batch cluster estimate handles: a member's particle index then fits in 15 bits.
+constexpr uint32_t kBatchClusterMaxParticles = 32768;
+
+/// One selected member of a batch cluster estimate.  Its scratch is its own slice of each buffer.
+struct BatchClusterMember {
+  uint64_t offset;         // first particle in the batch buffers; also its record slice (cells <= particles)
+  uint64_t table_offset;   // first slot of its hash table
+  uint64_t starts_offset;  // first of its cells + 1 segment starts
+  uint32_t n;              // particles (> 0)
+  uint32_t table_mask;     // table slots - 1 (a power of two minus one)
+  uint32_t cur;            // state buffer holding the particles
+  uint32_t pad;
+  double pivot_x, pivot_y; // the member's moment pivot
+};
+
+struct BatchClusterArgs {
+  const BatchClusterMember* members;  // one per CTA
+  const Pose2* states[2];
+  const double* weights;
+  double linear, angular;             // spatial-hash resolutions
+  unsigned long long* hashes;         // [particles]
+  unsigned long long* keys;           // [table slots]
+  unsigned int* first;                // [table slots] smallest particle index per key
+  uint32_t* ids;                      // [table slots] cell id of the key's cell
+  uint32_t* cell_of;                  // [particles]
+  uint32_t* sort_a;                   // [particles] sort ping-pong
+  uint32_t* sort_b;
+  uint32_t* starts;                   // [particles + members]
+  CellRecord* records;                // [particles] member slices
+  uint32_t* cells;                    // [selected members] occupied cells
+};
+
+/// One CTA per selected member: hash set, first-occurrence numbering, stable sort by cell and one CellRecord per cell,
+/// written to the member's record slice; cells[j] receives member j's cell count.  One launch.
+void launch_batch_cluster_cells(const BatchClusterArgs& a, uint32_t n_members, cudaStream_t stream);
+/// Member j's cells[j] records to out[cells[0] + ... + cells[j - 1]]: the records of all members back to back.  One launch.
+void launch_batch_cluster_compact(const BatchClusterMember* members, const uint32_t* cells, const CellRecord* records, uint32_t n_members,
+                                  CellRecord* out, cudaStream_t stream);
+
+/// The clusterizer of a filter: scratch for up to `capacity` particles on one device, allocated on first use,
 /// run over any particle set of that size in that device's memory.  Every call works on the current device, ordered on
 /// `stream`, and returns a bb200_status with the message in *error.
 class Clusterizer {

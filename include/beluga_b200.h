@@ -536,6 +536,10 @@ int bb200_amcl_leave_shards(bb200_amcl* a);
  * device, with BB200_ERR_INVALID_ARGUMENT: n_members < 1, min_particles != max_particles (KLD), selective
  * resampling, non-zero shard fields, max_particles of 0 or above 32768, and members on different devices.
  * Only the likelihood-field models are supported (no beam model).
+ *
+ * The fleet loop of a beluga_ros node per member is bb200_amcl_batch_update, then
+ * bb200_amcl_batch_cluster_estimates for the members that updated: the estimate every node publishes, for all of them
+ * with two kernel launches and two host synchronisations, whatever K and the members' cell counts are.
  * ------------------------------------------------------------------------------------------- */
 typedef struct bb200_amcl_batch bb200_amcl_batch;
 /* params[m] and motions[m] configure member m (params[m].device must be the same for all). */
@@ -555,8 +559,17 @@ int bb200_amcl_batch_force_update(bb200_amcl_batch* b, int member);
 int bb200_amcl_batch_get_particles(bb200_amcl_batch* b, int member, double* states, double* weights, uint64_t capacity);
 /* Resample indices of member m's last resample (params[m].record_ancestors must be set). */
 int bb200_amcl_batch_ancestors(bb200_amcl_batch* b, int member, int64_t* out, uint64_t capacity);
-/* beluga::cluster_based_estimate of member m's particles. */
+/* beluga::cluster_based_estimate of member m's particles (bb200_amcl_batch_cluster_estimates with member m alone). */
 int bb200_amcl_batch_cluster_estimate(bb200_amcl_batch* b, int member, const bb200_cluster_param* p, bb200_estimate* out);
+/* beluga::cluster_based_estimate of every member m with present[m] != 0 (present NULL: all members), with one set of
+ * clusterizer parameters for all of them.  out[m] receives member m's estimate.  n_cells and n_clusters may be NULL;
+ * when they are not, entry m receives member m's occupied cells and clusters.  Entries of members not selected are not
+ * written.  The number of kernel launches does not depend on K or on the members' cell counts.  Every selected member's
+ * result is bit-identical to bb200_amcl_batch_cluster_estimate(b, m, p, ...) and to a standalone filter's
+ * bb200_filter_cluster_estimate over the same particles.  Fails before any launch with BB200_ERR_INVALID_ARGUMENT for
+ * bad parameters and with BB200_ERR_STATE when a selected member holds no particles. */
+int bb200_amcl_batch_cluster_estimates(bb200_amcl_batch* b, const bb200_cluster_param* p, const uint8_t* present,
+                                       bb200_estimate* out, uint32_t* n_cells, uint32_t* n_clusters);
 /* Amcl::update for every member m with present[m] != 0 (present NULL: all members).  control_poses holds K poses of 4
  * doubles, points_xy[m] member m's n_points[m] (x, y) pairs (NULL when n_points[m] == 0), out[m] its result.  An absent
  * member is left untouched -- no policy is evaluated -- and gets out[m].updated = 0.  Present members go through their
@@ -564,7 +577,7 @@ int bb200_amcl_batch_cluster_estimate(bb200_amcl_batch* b, int member, const bb2
  * every member's host state is as if it had not been made. */
 int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, const double* const* points_xy, const uint64_t* n_points,
                             const uint8_t* present, bb200_update_result* out);
-/* Kernel launches issued by this batch so far. */
+/* Kernel launches issued by this batch so far (steps, initialisations and cluster estimates). */
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b);
 
 /* The two host halves of bb200_amcl_update for callers that drive the filter themselves. */

@@ -287,6 +287,27 @@ class AmclBatch {
     return std::make_pair(SE2d::from_data(e.mean), cov);
   }
 
+  /// beluga::cluster_based_estimate of every member whose present[m] is true (present == nullptr: all of them) in one call
+  /// with a fixed number of kernel launches; std::nullopt for members not selected.
+  [[nodiscard]] auto cluster_based_estimates(const std::vector<bool>* present = nullptr, ParticleClusterizerParam parameters = {}) const
+      -> std::vector<std::optional<estimation_type>> {
+    const std::size_t k = size();
+    if (present != nullptr && present->size() != k) throw Error(BB200_ERR_INVALID_ARGUMENT, "one presence flag per member");
+    const bb200_cluster_param p{parameters.linear_hash_resolution, parameters.angular_hash_resolution, parameters.weight_cap_percentile};
+    std::vector<std::uint8_t> mask(present != nullptr ? k : 0);
+    for (std::size_t m = 0; m < mask.size(); ++m) mask[m] = (*present)[m] ? 1 : 0;
+    std::vector<bb200_estimate> e(k);
+    check(bb200_amcl_batch_cluster_estimates(handle_, &p, present != nullptr ? mask.data() : nullptr, e.data(), nullptr, nullptr));
+    std::vector<std::optional<estimation_type>> out(k);
+    for (std::size_t m = 0; m < k; ++m) {
+      if (present != nullptr && !(*present)[m]) continue;
+      Matrix3d cov;
+      for (int i = 0; i < 9; ++i) cov[i] = e[m].cov[i];
+      out[m] = std::make_pair(SE2d::from_data(e[m].mean), cov);
+    }
+    return out;
+  }
+
   [[nodiscard]] bb200_amcl_batch* handle() const { return handle_; }
 
  private:

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Timings of the other BASELINE.json configurations (parity-test cases, not the bench.py line), and of point-cloud updates:
 `cloud`: 65 536-point lidar clouds at 10k and 1M particles.  `batch`: K node-sized filters (2000 particles x 100 points) stepped as one
-AmclBatch against K standalone Amcl stepped one after another.
+AmclBatch against K standalone Amcl stepped one after another.  `batch_cluster`: the same batches with the beluga_ros-shaped round
+update + cluster estimate, the estimate taken for all members in one call and member by member.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import json
@@ -131,6 +132,92 @@ def run_batch():
     return res
 
 
+def select_host_ms(states, weights, repeats=50):
+    """Host time of the select_cluster pass alone (bb200_cluster_select_host) on the cells of one member's particles at the
+    default clusterizer parameters; the records come from a standalone filter's device histogram."""
+    import ctypes as C
+
+    from beluga_b200 import _capi
+
+    lib = _capi.load()
+    f = bb.Filter(capacity=len(states))
+    f.set_particles(states, weights)
+    n_bins, top = C.c_uint64(0), C.c_double(0.0)
+    lib.bb200_filter_particle_histogram(f._h, 0.20, 0.524, None, 0, C.byref(n_bins), C.byref(top))
+    m = n_bins.value
+    cells = (_capi.ClusterCell * max(m, 1))()
+    assert lib.bb200_filter_particle_histogram(f._h, 0.20, 0.524, cells, m, C.byref(n_bins), C.byref(top)) == 0
+    p = _capi.ClusterParam(0.20, 0.524, 0.90)
+    ids = (C.c_uint32 * max(m, 1))()
+    n_clusters, found, best = C.c_uint32(0), C.c_int(0), C.c_uint32(0)
+    out = np.zeros(9)
+    times = []
+    for _ in range(repeats):
+        t0 = time.perf_counter()
+        lib.bb200_cluster_select_host(cells, m, len(states), C.byref(p), ids, C.byref(n_clusters), C.byref(found), C.byref(best),
+                                      out.ctypes.data_as(C.POINTER(C.c_double)))
+        times.append((time.perf_counter() - t0) * 1e3)
+    return float(np.median(times)), m
+
+
+def run_batch_cluster():
+    """The `batch` workload (K in {1, 16, 64, 256} members x 2000 particles x 100 points, 2000^2 map, systematic resampling, every
+    member updating every step) and K = 1 x 32 768 particles, timed as beluga_ros-shaped rounds: update, then the cluster-based
+    estimate of every member, once as one cluster_estimates call and once as K cluster_estimate(m) calls, on the same particles.
+    On a build without AmclBatch.cluster_estimates only the per-member form is timed."""
+    res = {}
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=100, steps=100)
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    steps, warmup = 20, 3
+    batched = hasattr(bb.AmclBatch, "cluster_estimates")
+    device = device_record()
+    for k, n in ((1, 2000), (16, 2000), (64, 2000), (256, 2000), (1, 32768)):
+        params = [bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m) for m in range(k)]
+        batch = bb.AmclBatch([bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)], params)
+        batch.set_likelihood_field_map(lfm, grid)
+        for m in range(k):
+            batch.initialize(m, sc.initial_mean, sc.initial_cov)
+        update_ms, all_ms, each_ms, all_launches, each_launches = [], [], [], [], []
+        for t in range(warmup + steps):
+            pose = bb.se2(*sc.poses[t])
+            t0 = time.perf_counter()
+            r = batch.update([pose] * k, [sc.scans[t]] * k)
+            t1 = time.perf_counter()
+            assert all(x.updated for x in r)
+            if batched:
+                before = batch.launch_count()
+                t2 = time.perf_counter()
+                together = batch.cluster_estimates()
+                t3 = time.perf_counter()
+                all_launches.append(batch.launch_count() - before)
+            before = batch.launch_count()
+            t4 = time.perf_counter()
+            each = [batch.cluster_estimate(m) for m in range(k)]
+            t5 = time.perf_counter()
+            each_launches.append(batch.launch_count() - before)
+            if batched:
+                assert all(a[0].tobytes() == b[0].tobytes() and a[1].tobytes() == b[1].tobytes() for a, b in zip(together, each))
+            if t >= warmup:
+                update_ms.append((t1 - t0) * 1e3)
+                each_ms.append((t5 - t4) * 1e3)
+                if batched:
+                    all_ms.append((t3 - t2) * 1e3)
+        states, weights = batch.particles(0)
+        select_ms, cells = select_host_ms(states, weights)
+        row = {"members": k, "particles": n, "points": 100, "steps": steps, "update_ms": float(np.median(update_ms)),
+               "per_member_estimates_ms": float(np.median(each_ms)),
+               "round_ms_per_member_form": float(np.median(np.add(update_ms, each_ms))),
+               "launches_per_member_call": int(max(each_launches)) / k,
+               "select_cluster_host_ms_one_member": select_ms, "cells_member_0": cells,
+               "ms_per_step_e2e": float(np.median(np.add(update_ms, all_ms if batched else each_ms))), "kernels_ms": {}, "device": device}
+        if batched:
+            row.update({"batched_estimates_ms": float(np.median(all_ms)), "round_ms_batched_form": float(np.median(np.add(update_ms, all_ms))),
+                        "launches_per_batched_call": int(max(all_launches))})
+        res[f"batch_cluster_{k}_x_{n}_x_100_lfm_2000"] = row
+    return res
+
+
 def main():
     out = {}
     which = sys.argv[1:] or ["c1", "c3", "c4"]
@@ -186,6 +273,8 @@ def main():
         out.update(run_cloud())
     if "batch" in which:
         out.update(run_batch())
+    if "batch_cluster" in which:
+        out.update(run_batch_cluster())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}

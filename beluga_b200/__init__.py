@@ -732,9 +732,10 @@ class ShardedAmcl:
 
 
 class AmclBatch:
-    """bb200_amcl_batch: K independent beluga::Amcl filters on one GPU, sharing one likelihood-field map; update() steps every
-    member with a new scan with a fixed number of kernel launches and one synchronisation.  Member m's results and particles
-    equal those of a standalone Amcl built from params[m] and motions[m] and fed the same inputs."""
+    """bb200_amcl_batch: K independent beluga::Amcl filters on one GPU, sharing one map -- a likelihood field
+    (set_likelihood_field_map) or a beam-model map (set_beam_map); update() steps every member with a new scan with a fixed
+    number of kernel launches and one synchronisation.  Member m's results and particles equal those of a standalone Amcl
+    built from params[m] and motions[m] and fed the same inputs."""
 
     def __init__(self, motions, params):
         """`motions[m]`, `params[m]`: member m's motion model and AmclParams (min_particles == max_particles <= 32768)."""
@@ -769,6 +770,11 @@ class AmclBatch:
     def set_likelihood_field_map(self, params: LikelihoodFieldModelParam, grid: OccupancyGrid, prob: bool = False):
         p, g = params.c(), grid.c()
         self._check(self._lib.bb200_amcl_batch_set_likelihood_field_map(self._h, C.byref(p), C.byref(g), int(prob)))
+
+    def set_beam_map(self, params: BeamModelParam, grid: OccupancyGrid):
+        """The beam model (BeamSensorModel) on `grid` for every member; replaces the map set before, of either model."""
+        p, g = params.c(), grid.c()
+        self._check(self._lib.bb200_amcl_batch_set_beam_map(self._h, C.byref(p), C.byref(g)))
 
     def initialize(self, member: int, mean_xytheta, cov):
         self._check(self._lib.bb200_amcl_batch_initialize(self._h, member, _dptr(_f64(mean_xytheta)), _dptr(_f64(cov).reshape(9))))

@@ -208,6 +208,7 @@ SIGNATURES = {
     "bb200_amcl_batch_last_error": (C.c_char_p, [_vp]),
     "bb200_amcl_batch_members": (C.c_int, [_vp]),
     "bb200_amcl_batch_set_likelihood_field_map": (C.c_int, [_vp, _P(LikelihoodFieldParam), _P(OccupancyGrid), C.c_int]),
+    "bb200_amcl_batch_set_beam_map": (C.c_int, [_vp, _P(BeamParam), _P(OccupancyGrid)]),
     "bb200_amcl_batch_initialize": (C.c_int, [_vp, C.c_int, _dbl, _dbl]),
     "bb200_amcl_batch_initialize_from_map": (C.c_int, [_vp, C.c_int]),
     "bb200_amcl_batch_initialize_states": (C.c_int, [_vp, C.c_int, _dbl, _dbl, C.c_uint64]),

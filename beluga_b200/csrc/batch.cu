@@ -93,7 +93,7 @@ Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, 
 Batch::~Batch() {
   if (stream_ != nullptr) cudaStreamSynchronize(stream_);
   for (void* p : std::initializer_list<void*>{states_[0], states_[1], weights_, cdf_, ancestors_, scalars_, tile_state_, partials_, table_, first_,
-                                              points_, members_done_, cl_hashes_, cl_keys_, cl_first_, cl_ids_, cl_cell_of_, cl_sort_[0], cl_sort_[1],
+                                              points_, hits_, members_done_, cl_hashes_, cl_keys_, cl_first_, cl_ids_, cl_cell_of_, cl_sort_[0], cl_sort_[1],
                                               cl_starts_, cl_records_, cl_table_, cl_cells_})
     cudaFree(p);
   for (void* p : std::initializer_list<void*>{table_host_, first_host_, points_host_, summary_host_, ticket_host_, cl_table_host_, cl_cells_host_,
@@ -116,7 +116,17 @@ int Batch::set_likelihood_field_map(const bb200_likelihood_field_param& p, const
   error_.clear();
   MapTables tables;
   const int st = prepare_likelihood_field_map(p, grid, prob, &tables, &error_);
-  if (st != BB200_OK) return st;
+  return st != BB200_OK ? st : set_map(tables);
+}
+
+int Batch::set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid) {
+  error_.clear();
+  MapTables tables;
+  const int st = prepare_beam_map(p, grid, &tables, &error_);
+  return st != BB200_OK ? st : set_map(tables);
+}
+
+int Batch::set_map(const MapTables& tables) {
   BB_CHECK(cudaSetDevice(device_));
   return map_.upload(tables, stream_, &error_);
 }
@@ -142,7 +152,7 @@ int Batch::initialize(int member, const double mean[3], const double cov[9]) {
 int Batch::initialize_from_map(int member) {
   BB_MEMBER(member);
   Member& m = members_[static_cast<size_t>(member)];
-  if (map_.sensor < 0) return fail(BB200_ERR_STATE, "initialize_from_map needs a map (set the likelihood field first)");
+  if (map_.sensor < 0) return fail(BB200_ERR_STATE, "initialize_from_map needs a map (set_*_map first)");
   if (map_.n_free == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
   BB_CHECK(cudaSetDevice(device_));
   launch_initialize_uniform(states_[m.cur] + m.offset, weights_ + m.offset, m.capacity, map_.free_cells, map_.n_free, map_.grid_width,
@@ -329,6 +339,22 @@ int Batch::ensure_points(uint64_t n_points) {
   return BB200_OK;
 }
 
+bool Batch::ensure_hits(uint64_t words) {
+  if (words <= hits_capacity_) return true;
+  // Every batch call ends synchronised: nothing in flight reads the old buffer.
+  cudaFree(hits_);
+  hits_ = nullptr;
+  hits_capacity_ = 0;
+  // words is at most one pass's worth (the caller checks), so the slack never takes the buffer past that
+  const uint64_t want = std::min<uint64_t>(std::max<uint64_t>(words + words / 2, 4096), kBeamHitPassBytes / sizeof(uint32_t));
+  if (dev_alloc(&hits_, want) != cudaSuccess) {
+    (void)cudaGetLastError();  // no room for the hit words: the fused kernel needs none
+    return false;
+  }
+  hits_capacity_ = want;
+  return true;
+}
+
 int Batch::update(const double* control_poses, const double* const* points_xy, const uint64_t* n_points, const uint8_t* present,
                   bb200_update_result* out) {
   error_.clear();
@@ -352,7 +378,7 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   }
   if (active.empty()) return BB200_OK;
 
-  if (map_.sensor < 0) return rollback(fail(BB200_ERR_STATE, "no likelihood-field map set"));
+  if (map_.sensor < 0) return rollback(fail(BB200_ERR_STATE, "no map set"));
   uint64_t points_total = 0;
   uint32_t max_points = 0;
   for (const uint32_t k : active) {
@@ -371,7 +397,7 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   const uint32_t n_active = static_cast<uint32_t>(active.size());
   BatchStepArgs a{};
   a.n_members = n_active;
-  uint64_t point_offset = 0;
+  uint64_t point_offset = 0, hit_words = 0;
   for (uint32_t j = 0; j < n_active; ++j) {
     const uint32_t k = active[j];
     const Member& m = members_[k];
@@ -396,6 +422,9 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     b.points_radius = scan_radius(points_xy[k], n_points[k]);
     if (n_points[k] > 0) std::memcpy(points_host_ + 2 * point_offset, points_xy[k], 2 * n_points[k] * sizeof(double));
     point_offset += n_points[k];
+    b.hit_offset = hit_words;
+    b.hit_stride = (m.n + 31) / 32 * 32;
+    hit_words += b.hit_stride * n_points[k];
     uint32_t ctas[kBatchLaunches];
     batch_member_ctas(b, ctas);
     for (int l = 0; l < kBatchLaunches; ++l) {
@@ -404,6 +433,13 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     }
   }
   for (int l = 0; l < kBatchLaunches; ++l) first_host_[static_cast<size_t>(l) * (n_active + 1) + n_active] = a.ctas[l];
+  // The beam model walks every member's rays in one pass when the map allows it (the rule of the single filter) and the
+  // step's hit words fit under the single filter's bound for one pass and in device memory; otherwise the fused kernel.
+  a.path = kBatchField;
+  if (map_.sensor == BB200_SENSOR_BEAM) {
+    const bool two_pass = beam_two_pass_map(map_) && hit_words <= kBeamHitPassBytes / sizeof(uint32_t) && ensure_hits(hit_words);
+    a.path = two_pass ? kBatchBeamTwoPass : kBatchBeamFused;
+  }
 
   cudaStream_t stream = stream_;
   seq_ = seq_ == 0x7fffffff ? 1 : seq_ + 1;
@@ -432,6 +468,9 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   a.grid_width = map_.grid_width;
   a.grid_resolution = map_.grid_resolution;
   a.grid_origin = map_.grid_origin;
+  a.occupancy = map_.occupancy;
+  a.beam = map_.beam;
+  a.hits = hits_;
   a.summary = summary_host_;
   a.members_done = members_done_;
   a.ticket = ticket_host_;

@@ -1,5 +1,5 @@
-// K independent beluga::Amcl filters that share one device, one likelihood-field map and one sensor model, stepped
-// together: one call runs every updating member's step with a fixed sequence of launches (csrc/kernels.cuh:
+// K independent beluga::Amcl filters that share one device, one map and one sensor model (either likelihood-field model
+// or the beam model), stepped together: one call runs every updating member's step with a fixed sequence of launches (csrc/kernels.cuh:
 // launch_batch_step) and one host synchronisation, whatever K is.  Each member keeps the host half of a bb200_amcl
 // (AmclPolicy) and a slice of the batch's particle buffers.
 #pragma once
@@ -31,9 +31,11 @@ class Batch {
   const char* last_error() const { return error_.c_str(); }
   void record_error(const std::string& message) const { error_ = message; }  // the C-ABI exception guard
   int members() const { return static_cast<int>(members_.size()); }
-  uint64_t launch_count() const { return launches_; }
+  uint64_t launch_count() const { return launches_ + map_.launches(); }  // the map's: the beam model's normaliser table
 
+  /// The map every member reads; a later set_*_map call replaces it, whichever sensor model either is for.
   int set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob);
+  int set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid);
   int initialize(int member, const double mean[3], const double cov[9]);
   int initialize_from_map(int member);
   int initialize_states(int member, const double* states, const double* weights, uint64_t n);
@@ -70,6 +72,8 @@ class Batch {
   int check(cudaError_t e, const char* what) { return cuda_check(e, what, &error_); }
   int member_ok(int member) const;
   int ensure_points(uint64_t n_points);
+  bool ensure_hits(uint64_t words);
+  int set_map(const MapTables& tables);
   int ensure_cluster_scratch();
   int ensure_cluster_records(uint64_t cells);
 
@@ -97,6 +101,8 @@ class Batch {
   double* points_{nullptr};
   double* points_host_{nullptr};      // pinned
   uint64_t points_capacity_{0};       // points (pairs)
+  uint32_t* hits_{nullptr};           // beam model, two-pass form: the step's hit words (grows only)
+  uint64_t hits_capacity_{0};         // words
   StepSummary* summary_host_{nullptr};  // pinned, one per member of the step's table
   int* ticket_host_{nullptr};           // pinned
   unsigned int* members_done_{nullptr};

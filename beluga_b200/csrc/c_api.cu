@@ -824,6 +824,10 @@ int bb200_amcl_batch_set_likelihood_field_map(bb200_amcl_batch* b, const bb200_l
   BB_REQUIRE(b && p && grid);
   return guarded(b->impl, [&] { return b->impl.set_likelihood_field_map(*p, *grid, prob != 0); });
 }
+int bb200_amcl_batch_set_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p, const bb200_occupancy_grid* grid) {
+  BB_REQUIRE(b && p && grid);
+  return guarded(b->impl, [&] { return b->impl.set_beam_map(*p, *grid); });
+}
 int bb200_amcl_batch_initialize(bb200_amcl_batch* b, int member, const double mean_xytheta[3], const double cov[9]) {
   BB_REQUIRE(b && mean_xytheta && cov);
   return guarded(b->impl, [&] { return b->impl.initialize(member, mean_xytheta, cov); });

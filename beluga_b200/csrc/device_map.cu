@@ -107,6 +107,12 @@ int prepare_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& g, M
   return BB200_OK;
 }
 
+bool beam_two_pass_map(const MapLayout& map) {
+  // spans of the walk's 32-bit arithmetic: far ends lie within beam_max_range of the source, sources inside the grid
+  const double reach_cells = map.beam.beam_max_range * map.occupancy.inv_resolution + 4.0;
+  return map.occupancy.free_padded != nullptr && reach_cells < static_cast<double>(1 << 21);
+}
+
 // ---------------------------------------------------------------------------------------------------
 
 void DeviceMap::release() {

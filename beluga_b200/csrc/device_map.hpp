@@ -42,6 +42,9 @@ int prepare_likelihood_field_map(const bb200_likelihood_field_param& p, const bb
                                  std::string* error);
 /// Host preparation of a beam-model map.
 int prepare_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid, MapTables* out, std::string* error);
+/// Whether the beam model's two-pass walk can take this map: it has the padded free-distance copy (grids up to 65534
+/// cells wide and 65535 high) and its rays stay short enough for the walk's 32-bit span arithmetic.  Filter and Batch both decide by it.
+bool beam_two_pass_map(const MapLayout& map);
 
 /// One device's copy of the current map.
 struct DeviceMap : MapLayout {

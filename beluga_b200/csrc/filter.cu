@@ -969,11 +969,9 @@ int Filter::enqueue_propagate_reweight_kernels(const MotionSampling* sampling, u
     if (map_.sensor == BB200_SENSOR_BEAM) {
       mark("reweight_beam");
       uint64_t pass = 0;
-      // spans of the walk's 32-bit arithmetic: far ends lie within beam_max_range of the source, sources inside the grid
-      const double reach_cells = map_.beam.beam_max_range * map_.occupancy.inv_resolution + 4.0;
-      if (n_points > 0 && map_.occupancy.free_padded != nullptr && reach_cells < static_cast<double>(1 << 21)) {
-        // hit words of one pass: at most 3 GiB, whole warps of particles
-        pass = std::min<uint64_t>(n_, std::max<uint64_t>(32, ((3ull << 30) / (4ull * n_points)) / 32 * 32));
+      if (n_points > 0 && beam_two_pass_map(map_)) {
+        // hit words of one pass: at most kBeamHitPassBytes, whole warps of particles
+        pass = std::min<uint64_t>(n_, std::max<uint64_t>(32, (kBeamHitPassBytes / (4ull * n_points)) / 32 * 32));
         const uint64_t words = beam_hit_words(pass, static_cast<uint32_t>(n_points));
         if (words > beam_hits_words_) {
           BB_CHECK(cudaStreamSynchronize(stream_));
@@ -981,7 +979,7 @@ int Filter::enqueue_propagate_reweight_kernels(const MotionSampling* sampling, u
           beam_hits_ = nullptr;
           beam_hits_words_ = 0;
           // sized for the filter's capacity so that a growing particle count (KLD) does not reallocate every step
-          const uint64_t pass_cap = std::min<uint64_t>(capacity_, std::max<uint64_t>(32, ((3ull << 30) / (4ull * n_points)) / 32 * 32));
+          const uint64_t pass_cap = std::min<uint64_t>(capacity_, std::max<uint64_t>(32, (kBeamHitPassBytes / (4ull * n_points)) / 32 * 32));
           const uint64_t want = beam_hit_words(std::max(pass, pass_cap), static_cast<uint32_t>(n_points));
           if (dev_alloc(&beam_hits_, want) == cudaSuccess) {
             beam_hits_words_ = want;

@@ -1001,13 +1001,14 @@ constexpr int kBeamThreads = 256;
 constexpr int kBeamBlocksPerSm = 3;  // chosen on a B200, not re-measured on the H100
 constexpr uint32_t kBeamChunk = 1024;  // rays staged per shared-memory chunk (32 KB), multiple of 4
 
-__global__ void __launch_bounds__(kBeamThreads, kBeamBlocksPerSm)
-    reweight_beam_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, const uint32_t* __restrict__ perm,
-                         OccupancyView grid, BeamParams params, const double2* __restrict__ points, uint32_t n_points,
-                         Scalars* __restrict__ scalars) {
+/// One CTA of the fused beam reweight: the particles in schedule slots [block * kBeamThreads, (block + 1) * kBeamThreads).
+__device__ __forceinline__ void reweight_beam_block(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n,
+                                                    const uint32_t* __restrict__ perm, const OccupancyView& grid, const BeamParams& params,
+                                                    const double2* __restrict__ points, uint32_t n_points, Scalars* __restrict__ scalars,
+                                                    uint32_t block) {
   __shared__ BeamRay s_rays[kBeamChunk];
   __shared__ unsigned long long s_red[kBeamThreads / kWarp];
-  const uint64_t slot = static_cast<uint64_t>(blockIdx.x) * kBeamThreads + threadIdx.x;
+  const uint64_t slot = static_cast<uint64_t>(block) * kBeamThreads + threadIdx.x;
   const bool active = slot < n;
   const uint64_t i = active ? (perm != nullptr ? perm[slot] : slot) : 0;
 
@@ -1078,6 +1079,13 @@ __global__ void __launch_bounds__(kBeamThreads, kBeamBlocksPerSm)
   if (threadIdx.x == 0 && m != 0) atomicMax(&scalars->wmax_bits, m);
 }
 
+__global__ void __launch_bounds__(kBeamThreads, kBeamBlocksPerSm)
+    reweight_beam_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, const uint32_t* __restrict__ perm,
+                         OccupancyView grid, BeamParams params, const double2* __restrict__ points, uint32_t n_points,
+                         Scalars* __restrict__ scalars) {
+  reweight_beam_block(states, weights, n, perm, grid, params, points, n_points, scalars, blockIdx.x);
+}
+
 // ---- beam model in two passes ----------------------------------------------------------------------
 // The fused kernel above carries the ray walk (integer, one dependent load per iteration) and the mixture (FP64:
 // sqrt, exp, three dozen constants) in one register allocation: 78 registers and a long instruction stream per
@@ -1101,12 +1109,14 @@ constexpr uint32_t kWalkChunk = 1024;  // far ends staged per shared-memory chun
 /// the 32-bit reciprocal quotient of ray_step is the only path.  16 instructions per iteration instead of 45.
 /// (Walking 2 or 4 rays per thread together was slower at C3 on a B200, not re-measured on the H100 --
 /// the per-ray state machine and its activity flags cost more than the second load chain hides.)
-__global__ void __launch_bounds__(kWalkThreads, kWalkBlocksPerSm)
-    beam_walk_kernel(const Pose2* __restrict__ states, uint64_t n, uint64_t slot_base, uint64_t slot_count, const uint32_t* __restrict__ perm,
-                     OccupancyView grid, double beam_max_range, const double2* __restrict__ points, uint32_t n_points,
-                     uint32_t* __restrict__ hits, uint64_t hit_stride) {
+/// One CTA of the walk: pass-local particles [block * kWalkThreads, (block + 1) * kWalkThreads) of the pass at slot_base.
+/// `grid` by value: taken by reference, ptxas schedules beam_walk_kernel differently (same registers and spills).
+__device__ __forceinline__ void beam_walk_block(const Pose2* __restrict__ states, uint64_t n, uint64_t slot_base, uint64_t slot_count,
+                                                const uint32_t* __restrict__ perm, OccupancyView grid, double beam_max_range,
+                                                const double2* __restrict__ points, uint32_t n_points, uint32_t* __restrict__ hits,
+                                                uint64_t hit_stride, uint32_t block) {
   __shared__ double2 s_far[kWalkChunk];
-  const uint64_t local = static_cast<uint64_t>(blockIdx.x) * kWalkThreads + threadIdx.x;
+  const uint64_t local = static_cast<uint64_t>(block) * kWalkThreads + threadIdx.x;
   const uint64_t slot = slot_base + local;
   const bool active = local < slot_count && slot < n;
   const uint64_t i = active ? (perm != nullptr ? perm[slot] : slot) : 0;
@@ -1183,16 +1193,25 @@ __global__ void __launch_bounds__(kWalkThreads, kWalkBlocksPerSm)
   }
 }
 
+__global__ void __launch_bounds__(kWalkThreads, kWalkBlocksPerSm)
+    beam_walk_kernel(const Pose2* __restrict__ states, uint64_t n, uint64_t slot_base, uint64_t slot_count, const uint32_t* __restrict__ perm,
+                     OccupancyView grid, double beam_max_range, const double2* __restrict__ points, uint32_t n_points,
+                     uint32_t* __restrict__ hits, uint64_t hit_stride) {
+  beam_walk_block(states, n, slot_base, slot_count, perm, grid, beam_max_range, points, n_points, hits, hit_stride, blockIdx.x);
+}
+
 constexpr int kMixThreads = 256;
 constexpr uint32_t kMixChunk = 2048;
 
-__global__ void __launch_bounds__(kMixThreads)
-    beam_mixture_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, uint64_t slot_base, uint64_t slot_count,
-                        const uint32_t* __restrict__ perm, OccupancyView grid, BeamParams params, const double2* __restrict__ points,
-                        uint32_t n_points, const uint32_t* __restrict__ hits, uint64_t hit_stride, Scalars* __restrict__ scalars) {
+/// One CTA of the mixture over the hit words beam_walk_block wrote for the same block of the same pass.
+__device__ __forceinline__ void beam_mixture_block(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, uint64_t slot_base,
+                                                   uint64_t slot_count, const uint32_t* __restrict__ perm, const OccupancyView& grid,
+                                                   const BeamParams& params, const double2* __restrict__ points, uint32_t n_points,
+                                                   const uint32_t* __restrict__ hits, uint64_t hit_stride, Scalars* __restrict__ scalars,
+                                                   uint32_t block) {
   __shared__ double2 s_beam[kMixChunk];  // {z, exp(-lambda_short * z)}
   __shared__ unsigned long long s_red[kMixThreads / kWarp];
-  const uint64_t local = static_cast<uint64_t>(blockIdx.x) * kMixThreads + threadIdx.x;
+  const uint64_t local = static_cast<uint64_t>(block) * kMixThreads + threadIdx.x;
   const uint64_t slot = slot_base + local;
   const bool active = local < slot_count && slot < n;
   const uint64_t i = active ? (perm != nullptr ? perm[slot] : slot) : 0;
@@ -1249,6 +1268,13 @@ __global__ void __launch_bounds__(kMixThreads)
   }
   const unsigned long long m = block_max_u64<kMixThreads>(active ? weight_order_bits(w) : 0ull, s_red);
   if (threadIdx.x == 0 && m != 0) atomicMax(&scalars->wmax_bits, m);
+}
+
+__global__ void __launch_bounds__(kMixThreads)
+    beam_mixture_kernel(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, uint64_t slot_base, uint64_t slot_count,
+                        const uint32_t* __restrict__ perm, OccupancyView grid, BeamParams params, const double2* __restrict__ points,
+                        uint32_t n_points, const uint32_t* __restrict__ hits, uint64_t hit_stride, Scalars* __restrict__ scalars) {
+  beam_mixture_block(states, weights, n, slot_base, slot_count, perm, grid, params, points, n_points, hits, hit_stride, scalars, blockIdx.x);
 }
 
 __global__ void __launch_bounds__(512) max_weight_kernel(const double* __restrict__ weights, uint64_t n, Scalars* scalars) {
@@ -2012,6 +2038,38 @@ __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm) batch_reweight_ker
   }
 }
 
+// The beam model's kernels take their CTAs from the kBatchReweight range too: one CTA per 256 particles in all of them.
+static_assert(kWalkThreads == kRwThreads && kMixThreads == kRwThreads && kBeamThreads == kRwThreads,
+              "every reweight form of a batch step shares the kBatchReweight CTA range");
+
+/// beam_walk_kernel per member: the whole member in one pass, its hit words beam-major at hits + hit_offset.
+__global__ void __launch_bounds__(kWalkThreads, kWalkBlocksPerSm) batch_beam_walk_kernel(BatchStepArgs s) {
+  uint32_t local, count;
+  const BatchMember& m = s.members[batch_member_of(s, kBatchReweight, blockIdx.x, local, count)];
+  const double2* points = reinterpret_cast<const double2*>(s.points) + m.point_offset;
+  beam_walk_block(batch_states(s, m, 0), m.n, 0, m.n, nullptr, s.occupancy, s.beam.beam_max_range, points, m.n_points, s.hits + m.hit_offset,
+                  m.hit_stride, local);
+}
+
+/// beam_mixture_kernel per member over the words batch_beam_walk_kernel wrote; the largest weight into the member's scalars.
+__global__ void __launch_bounds__(kMixThreads) batch_beam_mixture_kernel(BatchStepArgs s) {
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kBatchReweight, blockIdx.x, local, count);
+  const BatchMember& m = s.members[k];
+  const double2* points = reinterpret_cast<const double2*>(s.points) + m.point_offset;
+  beam_mixture_block(batch_states(s, m, 0), s.weights + m.offset, m.n, 0, m.n, nullptr, s.occupancy, s.beam, points, m.n_points,
+                     s.hits + m.hit_offset, m.hit_stride, s.scalars + k, local);
+}
+
+/// reweight_beam_kernel per member (maps the walk cannot take, or a step whose hit words would not fit).
+__global__ void __launch_bounds__(kBeamThreads, kBeamBlocksPerSm) batch_reweight_beam_kernel(BatchStepArgs s) {
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kBatchReweight, blockIdx.x, local, count);
+  const BatchMember& m = s.members[k];
+  const double2* points = reinterpret_cast<const double2*>(s.points) + m.point_offset;
+  reweight_beam_block(batch_states(s, m, 0), s.weights + m.offset, m.n, nullptr, s.occupancy, s.beam, points, m.n_points, s.scalars + k, local);
+}
+
 /// quantize_scan_kernel per member: the exponent from the member's own largest weight, its own look-back state.
 __global__ void __launch_bounds__(kQsThreads) batch_scan_kernel(BatchStepArgs s) {
   uint32_t local, count;
@@ -2462,11 +2520,20 @@ int launch_batch_step(const BatchStepArgs& s, cudaStream_t stream) {
   const uint32_t reset = std::max(s.n_members, s.ctas[kBatchScan]);
   batch_begin_kernel<<<std::max(1u, std::min((reset + 255u) / 256u, kSmCount * 4u)), 256, 0, stream>>>(s);
   batch_propagate_kernel<<<s.ctas[kBatchPropagate], kPrThreads, 0, stream>>>(s);
-  const size_t smem = static_cast<size_t>(std::min(s.max_points, kChunkBeams)) * sizeof(double2);
-  batch_reweight_kernel<<<s.ctas[kBatchReweight], kRwThreads, smem, stream>>>(s);
+  int launches = 5;
+  if (s.path == kBatchBeamTwoPass) {
+    batch_beam_walk_kernel<<<s.ctas[kBatchReweight], kWalkThreads, 0, stream>>>(s);
+    batch_beam_mixture_kernel<<<s.ctas[kBatchReweight], kMixThreads, 0, stream>>>(s);
+    launches = 6;
+  } else if (s.path == kBatchBeamFused) {
+    batch_reweight_beam_kernel<<<s.ctas[kBatchReweight], kBeamThreads, 0, stream>>>(s);
+  } else {
+    const size_t smem = static_cast<size_t>(std::min(s.max_points, kChunkBeams)) * sizeof(double2);
+    batch_reweight_kernel<<<s.ctas[kBatchReweight], kRwThreads, smem, stream>>>(s);
+  }
   batch_scan_kernel<<<s.ctas[kBatchScan], kQsThreads, 0, stream>>>(s);
   batch_finish_kernel<<<s.ctas[kBatchFinish], kRsThreads, 0, stream>>>(s);
-  return 5;
+  return launches;
 }
 
 uint32_t launch_resample(const ResampleArgs& args, Scalars* scalars, double* moment_partials, cudaStream_t stream) {

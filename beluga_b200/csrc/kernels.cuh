@@ -300,6 +300,8 @@ void launch_reweight_beam(const Pose2* states, double* weights, uint64_t n, cons
 /// The same in two passes over `pass_particles` particles at a time: ray walk -> one 32-bit hit word per (beam, particle)
 /// in `hits` (beam_hit_words(pass_particles, n_points) words), then the mixture.  Grids up to 65535 cells a side.
 uint64_t beam_hit_words(uint64_t particles, uint32_t n_points);
+/// Largest hit-word buffer of one pass (a batch step is one pass: beyond this it takes the fused kernel).
+constexpr uint64_t kBeamHitPassBytes = 3ull << 30;
 void launch_reweight_beam_two_pass(const Pose2* states, double* weights, uint64_t n, const uint32_t* perm, const OccupancyView& grid,
                                    const BeamParams& params, const double* points_xy_device, uint32_t n_points, uint32_t* hits,
                                    uint64_t pass_particles, Scalars* scalars, cudaStream_t stream);
@@ -417,6 +419,8 @@ struct BatchMember {
   uint64_t point_offset;    // first point of the member's scan in the batch's point buffer
   uint32_t n_points;
   double points_radius;     // largest |x| + |y| of the scan (NaN: some point is not finite)
+  uint64_t hit_offset;      // beam model, two-pass form: first hit word of the member in the batch's hit buffer ...
+  uint64_t hit_stride;      // ... beam-major, round_up(n, 32) words per beam (the single filter's layout)
 };
 
 /// Start of member m's CTA range in each launch: first[m] .. first[m + 1] (n_members + 1 entries per launch).
@@ -446,8 +450,18 @@ struct BatchStepArgs {
   unsigned int* members_done;     // device word, zero between steps
   int* ticket;                    // pinned: stores `seq` once every member's summary is complete
   int seq;
+  // The beam model (after the likelihood-field members so that those kernels keep their parameter offsets).
+  int path;                       // BatchReweightPath
+  OccupancyView occupancy;
+  BeamParams beam;
+  uint32_t* hits;                 // two-pass form: every member's hit words (BatchMember::hit_offset)
 };
-/// Reset | propagate | reweight | quantise + scan | resample or normalise + moments.  Returns the number of launches.
+static_assert(sizeof(BatchStepArgs) <= 1024, "the step's arguments travel as one kernel parameter block (4 KB at most)");
+/// Reweight | scan | finish: the likelihood field in one launch, the beam model's walk and mixture in two (two-pass form)
+/// or in one (fused form).
+enum BatchReweightPath : int { kBatchField = 0, kBatchBeamTwoPass = 1, kBatchBeamFused = 2 };
+/// Reset | propagate | reweight | quantise + scan | resample or normalise + moments.  Returns the number of launches: 5, or
+/// 6 for the beam model's two-pass form, whatever the members, their particle counts and their scans are.
 int launch_batch_step(const BatchStepArgs& args, cudaStream_t stream);
 /// Scan tiles of a member of n particles (the quantise-scan CTAs it needs).
 uint32_t batch_scan_tiles(uint64_t n);

@@ -525,7 +525,7 @@ int bb200_amcl_leave_shards(bb200_amcl* a);
 
 /* ---------------------------------------------------------------------------------------------
  * Many independent filters on one GPU: a batch of K beluga::Amcl members that share one device, one
- * likelihood-field map and one sensor model -- a fleet server localising many robots against one site
+ * map and one sensor model -- a fleet server localising many robots against one site
  * map, a simulator with many agents.  bb200_amcl_batch_update steps every member that has a new scan
  * with a fixed number of kernel launches and one host synchronisation, whatever K is; each member's
  * result and particles are bit-identical to what a standalone bb200_amcl with the same parameters returns
@@ -535,7 +535,12 @@ int bb200_amcl_leave_shards(bb200_amcl* a);
  * motion model.  Members keep a fixed particle count: bb200_amcl_batch_create rejects, before touching a
  * device, with BB200_ERR_INVALID_ARGUMENT: n_members < 1, min_particles != max_particles (KLD), selective
  * resampling, non-zero shard fields, max_particles of 0 or above 32768, and members on different devices.
- * Only the likelihood-field models are supported (no beam model).
+ * The map chooses the sensor model: either likelihood-field model (bb200_amcl_batch_set_likelihood_field_map)
+ * or the beam model (bb200_amcl_batch_set_beam_map).  A step takes 5 kernel launches, or 6 for the beam model
+ * on maps where a standalone filter walks its rays in two passes; there the batch does the same unless the
+ * step's hit words (sum over the updating members of round_up(n, 32) x scan points x 4 bytes) exceed 3 GiB
+ * or cannot be allocated, and then takes the fused beam kernel in 5 launches.  Either way every member's results stay
+ * bit-identical to its standalone twin's.
  *
  * The fleet loop of a beluga_ros node per member is bb200_amcl_batch_update, then
  * bb200_amcl_batch_cluster_estimates for the members that updated: the estimate every node publishes, for all of them
@@ -547,9 +552,13 @@ int bb200_amcl_batch_create(const bb200_amcl_param* params, const bb200_motion_p
 void bb200_amcl_batch_destroy(bb200_amcl_batch* b);
 const char* bb200_amcl_batch_last_error(const bb200_amcl_batch* b);
 int bb200_amcl_batch_members(const bb200_amcl_batch* b);
-/* One likelihood field (prob != 0: the prob model) for every member, built and uploaded once. */
+/* One likelihood field (prob != 0: the prob model) for every member, built and uploaded once.  Replaces any earlier
+ * map, whichever sensor model it was for. */
 int bb200_amcl_batch_set_likelihood_field_map(bb200_amcl_batch* b, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid,
                                               int prob);
+/* One beam-model map (BeamSensorModel) for every member, built and uploaded once; replaces any earlier map the same way.
+ * BB200_ERR_INVALID_ARGUMENT for a null handle or argument. */
+int bb200_amcl_batch_set_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p, const bb200_occupancy_grid* grid);
 /* bb200_amcl_initialize / _initialize_from_map / _initialize_states / _force_update for member `member`. */
 int bb200_amcl_batch_initialize(bb200_amcl_batch* b, int member, const double mean_xytheta[3], const double cov[9]);
 int bb200_amcl_batch_initialize_from_map(bb200_amcl_batch* b, int member);
@@ -577,7 +586,8 @@ int bb200_amcl_batch_cluster_estimates(bb200_amcl_batch* b, const bb200_cluster_
  * every member's host state is as if it had not been made. */
 int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, const double* const* points_xy, const uint64_t* n_points,
                             const uint8_t* present, bb200_update_result* out);
-/* Kernel launches issued by this batch so far (steps, initialisations and cluster estimates). */
+/* Kernel launches issued by this batch so far (steps, initialisations, cluster estimates and the beam model's map
+ * uploads). */
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b);
 
 /* The two host halves of bb200_amcl_update for callers that drive the filter themselves. */

@@ -205,8 +205,8 @@ template <class MotionModel, class SensorModel, class ExecutionPolicy>
   return std::make_pair(SE2d::from_data(e.mean), cov);
 }
 
-/// K independent filters on one GPU that share one likelihood-field map (bb200_amcl_batch): update() steps every member
-/// with a new scan at once.  Member m behaves like an Amcl built from motions[m] and params[m]; members keep a fixed
+/// K independent filters on one GPU that share one map (bb200_amcl_batch), for a likelihood-field model or the beam model:
+/// update() steps every member with a new scan at once.  Member m behaves like an Amcl built from motions[m] and params[m]; members keep a fixed
 /// particle count (min_particles == max_particles <= 32768).  Results are returned per member, std::nullopt where the
 /// reference's update would return it or where the member had no scan this step.
 class AmclBatch {
@@ -232,6 +232,8 @@ class AmclBatch {
   void set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob = false) {
     check(bb200_amcl_batch_set_likelihood_field_map(handle_, &p, &grid, prob ? 1 : 0));
   }
+  /// One beam-model map (BeamSensorModel) for every member; replaces the map set before, whichever model it was for.
+  void set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid) { check(bb200_amcl_batch_set_beam_map(handle_, &p, &grid)); }
   void initialize(std::size_t member, const SE2d& pose, const Matrix3d& covariance) {
     const double mean[3] = {pose.x(), pose.y(), pose.theta()};
     check(bb200_amcl_batch_initialize(handle_, index(member), mean, covariance.data()));

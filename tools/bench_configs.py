@@ -2,7 +2,8 @@
 """Timings of the other BASELINE.json configurations (parity-test cases, not the bench.py line), and of point-cloud updates:
 `cloud`: 65 536-point lidar clouds at 10k and 1M particles.  `batch`: K node-sized filters (2000 particles x 100 points) stepped as one
 AmclBatch against K standalone Amcl stepped one after another.  `batch_cluster`: the same batches with the beluga_ros-shaped round
-update + cluster estimate, the estimate taken for all members in one call and member by member.
+update + cluster estimate, the estimate taken for all members in one call and member by member.  `batch_beam`: AmclBatch with the
+beam model (60 and 720 points per member) against the same members stepped as standalone Amcl.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import json
@@ -129,6 +130,60 @@ def run_batch():
             "ms_per_step_e2e": mb, "member_steps_per_s": k * 1e3 / mb, "launches_per_step": int(max(launches)),
             "standalone_ms_per_round": ms, "standalone_member_steps_per_s": k * 1e3 / ms,
             "kernels_ms": {}, "device": device}
+    return res
+
+
+def run_batch_beam():
+    """AmclBatch with the beam model (beam_max_range 60 m as in C3): K in {1, 16, 64, 256} members x 2000 particles x 60 points
+    (beluga_amcl's default max_beams) and 256 x 2000 x 720 points on the 2000^2 synthetic map, systematic resampling, every
+    member updating every step; beside it, in the same process, K standalone Amcl stepped one after another on the same inputs.
+    On a build without AmclBatch.set_beam_map only the standalone filters are timed."""
+    res = {}
+    beam = bb.BeamModelParam(beam_max_range=60.0)
+    n, steps, warmup = 2000, 20, 3
+    batched = hasattr(bb.AmclBatch, "set_beam_map")
+    device = device_record()
+    for points, ks in ((60, (1, 16, 64, 256)), (720, (256,))):
+        sc = synthetic.make_scenario(grid_size=2000, n_beams=points, steps=warmup + steps)
+        grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+        for k in ks:
+            params = [bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m) for m in range(k)]
+            motions = [bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)]
+            batch = bb.AmclBatch(motions, params) if batched else None
+            if batched:
+                batch.set_beam_map(beam, grid)
+            singles = []
+            for m in range(k):
+                if batched:
+                    batch.initialize(m, sc.initial_mean, sc.initial_cov)
+                a = bb.Amcl(motions[m], params[m])
+                a.update_map(bb.SENSOR_BEAM, beam, grid)
+                a.initialize(sc.initial_mean, sc.initial_cov)
+                singles.append(a)
+            wall_batch, wall_single, launches = [], [], []
+            for t in range(warmup + steps):
+                pose = bb.se2(*sc.poses[t])
+                t0 = time.perf_counter()
+                if batched:
+                    before = batch.launch_count()
+                    r = batch.update([pose] * k, [sc.scans[t]] * k)
+                    assert all(x.updated for x in r)
+                    launches.append(batch.launch_count() - before)
+                t1 = time.perf_counter()
+                for a in singles:
+                    assert a.update(pose, sc.scans[t]).updated == 1
+                t2 = time.perf_counter()
+                if t >= warmup:
+                    wall_batch.append((t1 - t0) * 1e3)
+                    wall_single.append((t2 - t1) * 1e3)
+            ms = float(np.median(wall_single))
+            row = {"members": k, "particles": n, "points": points, "beam_max_range": 60.0, "steps": steps,
+                   "standalone_ms_per_round": ms, "standalone_member_steps_per_s": k * 1e3 / ms, "ms_per_step_e2e": ms, "kernels_ms": {},
+                   "device": device}
+            if batched:
+                mb = float(np.median(wall_batch))
+                row.update({"ms_per_step_e2e": mb, "member_steps_per_s": k * 1e3 / mb, "launches_per_step": int(max(launches))})
+            res[f"batch_beam_{k}_x_{n}_x_{points}_beam_2000"] = row
     return res
 
 
@@ -275,6 +330,8 @@ def main():
         out.update(run_batch())
     if "batch_cluster" in which:
         out.update(run_batch_cluster())
+    if "batch_beam" in which:
+        out.update(run_batch_beam())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}

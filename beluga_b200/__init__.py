@@ -732,8 +732,9 @@ class ShardedAmcl:
 
 
 class AmclBatch:
-    """bb200_amcl_batch: K independent beluga::Amcl filters on one GPU, sharing one map -- a likelihood field
-    (set_likelihood_field_map) or a beam-model map (set_beam_map); update() steps every member with a new scan with a fixed
+    """bb200_amcl_batch: K independent beluga::Amcl filters on one GPU, each reading one of the batch's maps -- a
+    likelihood field or a beam-model map, one for every member (set_*_map) or several (add_*_map and update_map, which
+    moves a member to another map as a node's Amcl::update_map does); update() steps every member with a new scan with a fixed
     number of kernel launches and one synchronisation.  Member m's results and particles equal those of a standalone Amcl
     built from params[m] and motions[m] and fed the same inputs."""
 
@@ -751,6 +752,7 @@ class AmclBatch:
             raise BelugaB200Error(st, self._lib.bb200_create_error().decode())
         self._h = h
         self.params = list(params)
+        self._field_shapes = {}  # (height, width) of each likelihood-field map, by id
 
     def close(self):
         if getattr(self, "_h", None):
@@ -768,13 +770,53 @@ class AmclBatch:
             raise BelugaB200Error(st, self._lib.bb200_amcl_batch_last_error(self._h).decode())
 
     def set_likelihood_field_map(self, params: LikelihoodFieldModelParam, grid: OccupancyGrid, prob: bool = False):
+        """One likelihood field for every member: removes every map, adds this one and assigns every member to it."""
         p, g = params.c(), grid.c()
         self._check(self._lib.bb200_amcl_batch_set_likelihood_field_map(self._h, C.byref(p), C.byref(g), int(prob)))
+        self._field_shapes = {self.member_map(0): grid.cells.shape}
 
     def set_beam_map(self, params: BeamModelParam, grid: OccupancyGrid):
         """The beam model (BeamSensorModel) on `grid` for every member; replaces the map set before, of either model."""
         p, g = params.c(), grid.c()
         self._check(self._lib.bb200_amcl_batch_set_beam_map(self._h, C.byref(p), C.byref(g)))
+        self._field_shapes = {}
+
+    def add_likelihood_field_map(self, params: LikelihoodFieldModelParam, grid: OccupancyGrid, prob: bool = False) -> int:
+        """Adds a likelihood-field map that no member reads yet; returns its id (0, 1, ... never reused)."""
+        p, g = params.c(), grid.c()
+        i = C.c_int(-1)
+        self._check(self._lib.bb200_amcl_batch_add_likelihood_field_map(self._h, C.byref(p), C.byref(g), int(prob), C.byref(i)))
+        self._field_shapes[i.value] = grid.cells.shape
+        return i.value
+
+    def add_beam_map(self, params: BeamModelParam, grid: OccupancyGrid) -> int:
+        """Adds a beam-model map that no member reads yet; returns its id."""
+        p, g = params.c(), grid.c()
+        i = C.c_int(-1)
+        self._check(self._lib.bb200_amcl_batch_add_beam_map(self._h, C.byref(p), C.byref(g), C.byref(i)))
+        return i.value
+
+    def update_map(self, member: int, map_id: int):
+        """Amcl::update_map for one member: it keeps its particles and policies and reads `map_id` from its next step."""
+        self._check(self._lib.bb200_amcl_batch_update_map(self._h, member, map_id))
+
+    def member_map(self, member: int) -> int:
+        """The id of the map member `member` reads (-1: none)."""
+        i = C.c_int(-1)
+        self._check(self._lib.bb200_amcl_batch_member_map(self._h, member, C.byref(i)))
+        return i.value
+
+    def remove_map(self, map_id: int):
+        """Frees a map that no member reads."""
+        self._check(self._lib.bb200_amcl_batch_remove_map(self._h, map_id))
+        self._field_shapes.pop(map_id, None)
+
+    def likelihood_field(self, map_id: int) -> np.ndarray:
+        """likelihood_field() of a likelihood-field map as a (height, width) float32 array."""
+        out = np.zeros(self._field_shapes.get(map_id, (1, 1)), dtype=np.float32)
+        size = out.size if map_id in self._field_shapes else 0
+        self._check(self._lib.bb200_amcl_batch_get_likelihood_field(self._h, map_id, out.ctypes.data_as(C.POINTER(C.c_float)), size))
+        return out
 
     def initialize(self, member: int, mean_xytheta, cov):
         self._check(self._lib.bb200_amcl_batch_initialize(self._h, member, _dptr(_f64(mean_xytheta)), _dptr(_f64(cov).reshape(9))))

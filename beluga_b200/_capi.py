@@ -209,6 +209,12 @@ SIGNATURES = {
     "bb200_amcl_batch_members": (C.c_int, [_vp]),
     "bb200_amcl_batch_set_likelihood_field_map": (C.c_int, [_vp, _P(LikelihoodFieldParam), _P(OccupancyGrid), C.c_int]),
     "bb200_amcl_batch_set_beam_map": (C.c_int, [_vp, _P(BeamParam), _P(OccupancyGrid)]),
+    "bb200_amcl_batch_add_likelihood_field_map": (C.c_int, [_vp, _P(LikelihoodFieldParam), _P(OccupancyGrid), C.c_int, _P(C.c_int)]),
+    "bb200_amcl_batch_add_beam_map": (C.c_int, [_vp, _P(BeamParam), _P(OccupancyGrid), _P(C.c_int)]),
+    "bb200_amcl_batch_update_map": (C.c_int, [_vp, C.c_int, C.c_int]),
+    "bb200_amcl_batch_member_map": (C.c_int, [_vp, C.c_int, _P(C.c_int)]),
+    "bb200_amcl_batch_remove_map": (C.c_int, [_vp, C.c_int]),
+    "bb200_amcl_batch_get_likelihood_field": (C.c_int, [_vp, C.c_int, _P(C.c_float), C.c_uint64]),
     "bb200_amcl_batch_initialize": (C.c_int, [_vp, C.c_int, _dbl, _dbl]),
     "bb200_amcl_batch_initialize_from_map": (C.c_int, [_vp, C.c_int]),
     "bb200_amcl_batch_initialize_states": (C.c_int, [_vp, C.c_int, _dbl, _dbl, C.c_uint64]),

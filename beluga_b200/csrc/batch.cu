@@ -93,7 +93,7 @@ Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, 
 Batch::~Batch() {
   if (stream_ != nullptr) cudaStreamSynchronize(stream_);
   for (void* p : std::initializer_list<void*>{states_[0], states_[1], weights_, cdf_, ancestors_, scalars_, tile_state_, partials_, table_, first_,
-                                              points_, hits_, members_done_, cl_hashes_, cl_keys_, cl_first_, cl_ids_, cl_cell_of_, cl_sort_[0], cl_sort_[1],
+                                              points_, hits_, map_table_, members_done_, cl_hashes_, cl_keys_, cl_first_, cl_ids_, cl_cell_of_, cl_sort_[0], cl_sort_[1],
                                               cl_starts_, cl_records_, cl_table_, cl_cells_})
     cudaFree(p);
   for (void* p : std::initializer_list<void*>{table_host_, first_host_, points_host_, summary_host_, ticket_host_, cl_table_host_, cl_cells_host_,
@@ -112,6 +112,13 @@ int Batch::member_ok(int member) const {
 
 #define BB_MEMBER(member) do { error_.clear(); if (const int st_ = member_ok(member)) return st_; } while (0)
 
+const Batch::MapEntry* Batch::find_map(int id) const {
+  const auto it = maps_.find(id);
+  if (it != maps_.end()) return &it->second;
+  error_ = "unknown map id " + std::to_string(id);
+  return nullptr;
+}
+
 int Batch::set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob) {
   error_.clear();
   MapTables tables;
@@ -126,9 +133,115 @@ int Batch::set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& g
   return st != BB200_OK ? st : set_map(tables);
 }
 
+int Batch::add_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob, int* id) {
+  error_.clear();
+  MapTables tables;
+  const int st = prepare_likelihood_field_map(p, grid, prob, &tables, &error_);
+  return st != BB200_OK ? st : add_map(tables, id);
+}
+
+int Batch::add_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid, int* id) {
+  error_.clear();
+  MapTables tables;
+  const int st = prepare_beam_map(p, grid, &tables, &error_);
+  return st != BB200_OK ? st : add_map(tables, id);
+}
+
 int Batch::set_map(const MapTables& tables) {
+  // The old maps go before the new one is uploaded, so that the device never holds both; a failed upload leaves the
+  // batch without a map.
   BB_CHECK(cudaSetDevice(device_));
-  return map_.upload(tables, stream_, &error_);
+  BB_CHECK(cudaStreamSynchronize(stream_));
+  maps_.clear();
+  map_table_current_ = false;
+  for (Member& m : members_) m.map = -1;
+  int id = -1;
+  const int st = add_map(tables, &id);
+  if (st != BB200_OK) return st;
+  for (Member& m : members_) m.map = id;
+  return BB200_OK;
+}
+
+int Batch::add_map(const MapTables& tables, int* id) {
+  BB_CHECK(cudaSetDevice(device_));
+  const int new_id = next_map_id_;
+  MapEntry& e = maps_[new_id];
+  const int st = e.map.upload(tables, stream_, &error_);
+  launches_ += e.map.launches();
+  if (st != BB200_OK) {
+    maps_.erase(new_id);
+    return st;
+  }
+  map_table_current_ = false;
+  ++next_map_id_;
+  *id = new_id;
+  return BB200_OK;
+}
+
+int Batch::update_map(int member, int id) {
+  BB_MEMBER(member);
+  if (find_map(id) == nullptr) return BB200_ERR_INVALID_ARGUMENT;
+  members_[static_cast<size_t>(member)].map = id;
+  return BB200_OK;
+}
+
+int Batch::member_map(int member, int* id) const {
+  error_.clear();
+  if (const int st = member_ok(member)) return st;
+  *id = members_[static_cast<size_t>(member)].map;
+  return BB200_OK;
+}
+
+int Batch::remove_map(int id) {
+  error_.clear();
+  if (find_map(id) == nullptr) return BB200_ERR_INVALID_ARGUMENT;
+  for (size_t k = 0; k < members_.size(); ++k)
+    if (members_[k].map == id) return fail(BB200_ERR_STATE, "member " + std::to_string(k) + " reads map " + std::to_string(id));
+  BB_CHECK(cudaSetDevice(device_));
+  BB_CHECK(cudaStreamSynchronize(stream_));  // nothing in flight reads its tables
+  maps_.erase(id);
+  map_table_current_ = false;
+  return BB200_OK;
+}
+
+int Batch::get_likelihood_field(int id, float* out, uint64_t capacity) const {
+  error_.clear();
+  const MapEntry* e = find_map(id);
+  if (e == nullptr) return BB200_ERR_INVALID_ARGUMENT;
+  const std::vector<float>& field = e->map.field_host;
+  if (field.empty()) {
+    error_ = "map " + std::to_string(id) + " is not a likelihood-field map";
+    return BB200_ERR_STATE;
+  }
+  if (capacity < field.size()) {
+    error_ = "capacity below the field's cells";
+    return BB200_ERR_CAPACITY;
+  }
+  std::memcpy(out, field.data(), field.size() * sizeof(float));
+  return BB200_OK;
+}
+
+int Batch::ensure_map_table() {
+  if (map_table_current_) return BB200_OK;
+  std::vector<BatchMap> host;
+  host.reserve(maps_.size());
+  for (auto& [id, e] : maps_) {
+    const DeviceMap& d = e.map;
+    e.slot = static_cast<int>(host.size());
+    host.push_back(BatchMap{d.field, d.occupancy, d.beam, d.free_cells, d.n_free, d.grid_width, d.grid_resolution, d.grid_origin});
+  }
+  if (host.size() > map_table_capacity_) {
+    BB_CHECK(cudaFree(map_table_));  // every batch call ends synchronised: no step reads the old table
+    map_table_ = nullptr;
+    map_table_capacity_ = 0;
+    BB_CHECK(dev_alloc(&map_table_, host.size()));
+    map_table_capacity_ = host.size();
+  }
+  // On the batch's stream, so that the step's launches follow the copy in order; the pageable source is staged before the
+  // call returns.
+  BB_CHECK(cudaMemcpyAsync(map_table_, host.data(), host.size() * sizeof(BatchMap), cudaMemcpyHostToDevice, stream_));
+  map_table_current_ = true;
+  return BB200_OK;
 }
 
 int Batch::initialize(int member, const double mean[3], const double cov[9]) {
@@ -152,16 +265,17 @@ int Batch::initialize(int member, const double mean[3], const double cov[9]) {
 int Batch::initialize_from_map(int member) {
   BB_MEMBER(member);
   Member& m = members_[static_cast<size_t>(member)];
-  if (map_.sensor < 0) return fail(BB200_ERR_STATE, "initialize_from_map needs a map (set_*_map first)");
-  if (map_.n_free == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
+  if (m.map < 0) return fail(BB200_ERR_STATE, "initialize_from_map needs a map (set_*_map or update_map first)");
+  const DeviceMap& map = maps_.at(m.map).map;
+  if (map.n_free == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
   BB_CHECK(cudaSetDevice(device_));
-  launch_initialize_uniform(states_[m.cur] + m.offset, weights_ + m.offset, m.capacity, map_.free_cells, map_.n_free, map_.grid_width,
-                            map_.grid_resolution, map_.grid_origin, m.policy.params().seed, 0, stream_);
+  launch_initialize_uniform(states_[m.cur] + m.offset, weights_ + m.offset, m.capacity, map.free_cells, map.n_free, map.grid_width,
+                            map.grid_resolution, map.grid_origin, m.policy.params().seed, 0, stream_);
   ++launches_;
   BB_CHECK(cudaGetLastError());
   BB_CHECK(cudaStreamSynchronize(stream_));
   m.n = m.capacity;
-  map_.centre(m.pivot);
+  map.centre(m.pivot);
   m.policy.force_update();
   return BB200_OK;
 }
@@ -378,22 +492,31 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   }
   if (active.empty()) return BB200_OK;
 
-  if (map_.sensor < 0) return rollback(fail(BB200_ERR_STATE, "no map set"));
   uint64_t points_total = 0;
   uint32_t max_points = 0;
+  int step_map = -1;            // the map every updating member reads, or -1 when they read several
+  std::vector<int> forms(count, kBatchField);
+  for (const uint32_t k : active)
+    if (members_[k].map < 0) return rollback(fail(BB200_ERR_STATE, maps_.empty() ? "no map set" : "member " + std::to_string(k) + " has no map"));
   for (const uint32_t k : active) {
     if (n_points[k] > 0xffffffffull) return rollback(fail(BB200_ERR_INVALID_ARGUMENT, "too many points"));
     if (n_points[k] > 0 && points_xy[k] == nullptr) return rollback(fail(BB200_ERR_INVALID_ARGUMENT, "points_xy is null"));
-    if (plans[k].resample && plans[k].random_state_probability > 0.0 && map_.n_free == 0)
+    const int id = members_[k].map;
+    const DeviceMap& map = maps_.at(id).map;
+    if (plans[k].resample && plans[k].random_state_probability > 0.0 && map.n_free == 0)
       return rollback(fail(BB200_ERR_STATE, "recovery injection needs a map with free cells"));
+    // The beam model walks a member's rays in two passes when its map allows it (the rule of the single filter).
+    if (map.sensor == BB200_SENSOR_BEAM) forms[k] = beam_two_pass_map(map) ? kBatchBeamTwoPass : kBatchBeamFused;
+    step_map = k == active.front() || step_map == id ? id : -1;
     points_total += n_points[k];
     max_points = std::max(max_points, static_cast<uint32_t>(n_points[k]));
   }
   int st = check(cudaSetDevice(device_), "cudaSetDevice");
   if (st == BB200_OK) st = ensure_points(points_total);  // the previous step has ended: the staging buffers are free
+  if (st == BB200_OK && step_map < 0) st = ensure_map_table();
   if (st != BB200_OK) return rollback(st);
 
-  // The step's member table, the CTA ranges of every launch and the concatenated scans.
+  // The step's member table and the concatenated scans.
   const uint32_t n_active = static_cast<uint32_t>(active.size());
   BatchStepArgs a{};
   a.n_members = n_active;
@@ -413,6 +536,7 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     b.scheme = plan.opts.scheme;
     b.cur = m.cur;
     b.ceil_log2_count = ceil_log2_count(m.capacity);
+    b.map = step_map < 0 ? maps_.at(m.map).slot : 0;
     b.random_state_probability = plan.random_state_probability;
     b.pivot_x = m.pivot[0];
     b.pivot_y = m.pivot[1];
@@ -422,24 +546,29 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     b.points_radius = scan_radius(points_xy[k], n_points[k]);
     if (n_points[k] > 0) std::memcpy(points_host_ + 2 * point_offset, points_xy[k], 2 * n_points[k] * sizeof(double));
     point_offset += n_points[k];
-    b.hit_offset = hit_words;
     b.hit_stride = (m.n + 31) / 32 * 32;
-    hit_words += b.hit_stride * n_points[k];
+    if (forms[k] == kBatchBeamTwoPass) {
+      b.hit_offset = hit_words;
+      hit_words += b.hit_stride * n_points[k];
+    }
+  }
+  // The two-pass members keep that form when their hit words fit under the single filter's bound for one pass and in
+  // device memory; otherwise they take the fused kernel.
+  if (hit_words > 0 && !(hit_words <= kBeamHitPassBytes / sizeof(uint32_t) && ensure_hits(hit_words)))
+    for (const uint32_t k : active)
+      if (forms[k] == kBatchBeamTwoPass) forms[k] = kBatchBeamFused;
+  // The CTA ranges of every row: each member in the reweight row of its form.
+  for (uint32_t j = 0; j < n_active; ++j) {
+    const int form = forms[active[j]];
+    a.forms |= 1 << form;
     uint32_t ctas[kBatchLaunches];
-    batch_member_ctas(b, ctas);
+    batch_member_ctas(table_host_[j], form, ctas);
     for (int l = 0; l < kBatchLaunches; ++l) {
       first_host_[static_cast<size_t>(l) * (n_active + 1) + j] = a.ctas[l];
       a.ctas[l] += ctas[l];
     }
   }
   for (int l = 0; l < kBatchLaunches; ++l) first_host_[static_cast<size_t>(l) * (n_active + 1) + n_active] = a.ctas[l];
-  // The beam model walks every member's rays in one pass when the map allows it (the rule of the single filter) and the
-  // step's hit words fit under the single filter's bound for one pass and in device memory; otherwise the fused kernel.
-  a.path = kBatchField;
-  if (map_.sensor == BB200_SENSOR_BEAM) {
-    const bool two_pass = beam_two_pass_map(map_) && hit_words <= kBeamHitPassBytes / sizeof(uint32_t) && ensure_hits(hit_words);
-    a.path = two_pass ? kBatchBeamTwoPass : kBatchBeamFused;
-  }
 
   cudaStream_t stream = stream_;
   seq_ = seq_ == 0x7fffffff ? 1 : seq_ + 1;
@@ -462,14 +591,19 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   a.scalars = scalars_;
   a.partials = partials_;
   a.points = points_;
-  a.field = map_.field;
-  a.free_cells = map_.free_cells;
-  a.n_free = map_.n_free;
-  a.grid_width = map_.grid_width;
-  a.grid_resolution = map_.grid_resolution;
-  a.grid_origin = map_.grid_origin;
-  a.occupancy = map_.occupancy;
-  a.beam = map_.beam;
+  if (step_map >= 0) {
+    const DeviceMap& map = maps_.at(step_map).map;
+    a.field = map.field;
+    a.free_cells = map.free_cells;
+    a.n_free = map.n_free;
+    a.grid_width = map.grid_width;
+    a.grid_resolution = map.grid_resolution;
+    a.grid_origin = map.grid_origin;
+    a.occupancy = map.occupancy;
+    a.beam = map.beam;
+  } else {
+    a.maps = map_table_;
+  }
   a.hits = hits_;
   a.summary = summary_host_;
   a.members_done = members_done_;

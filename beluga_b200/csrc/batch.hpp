@@ -1,9 +1,10 @@
-// K independent beluga::Amcl filters that share one device, one map and one sensor model (either likelihood-field model
-// or the beam model), stepped together: one call runs every updating member's step with a fixed sequence of launches (csrc/kernels.cuh:
-// launch_batch_step) and one host synchronisation, whatever K is.  Each member keeps the host half of a bb200_amcl
-// (AmclPolicy) and a slice of the batch's particle buffers.
+// K independent beluga::Amcl filters that share one device, stepped together: one call runs every updating member's step
+// with a fixed sequence of launches (csrc/kernels.cuh: launch_batch_step) and one host synchronisation, whatever K is.
+// Each member keeps the host half of a bb200_amcl (AmclPolicy) and a slice of the batch's particle buffers, and reads one
+// of the batch's maps (each a grid with its sensor model: likelihood-field model or the beam model).
 #pragma once
 
+#include <map>
 #include <string>
 #include <vector>
 
@@ -31,11 +32,20 @@ class Batch {
   const char* last_error() const { return error_.c_str(); }
   void record_error(const std::string& message) const { error_ = message; }  // the C-ABI exception guard
   int members() const { return static_cast<int>(members_.size()); }
-  uint64_t launch_count() const { return launches_ + map_.launches(); }  // the map's: the beam model's normaliser table
+  uint64_t launch_count() const { return launches_; }  // including the map uploads' (the beam model's normaliser tables)
 
-  /// The map every member reads; a later set_*_map call replaces it, whichever sensor model either is for.
+  /// One map for every member: removes every map, adds this one and assigns every member to it.
   int set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob);
   int set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid);
+  /// Adds a map without assigning it; *id receives its id (0, 1, ... over the batch's life, never reused).
+  int add_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob, int* id);
+  int add_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid, int* id);
+  /// Amcl::update_map for one member: its particles and policies stay; its later steps read map `id`.
+  int update_map(int member, int id);
+  int member_map(int member, int* id) const;
+  /// Frees map `id` (BB200_ERR_STATE while a member reads it).
+  int remove_map(int id);
+  int get_likelihood_field(int id, float* out, uint64_t capacity) const;
   int initialize(int member, const double mean[3], const double cov[9]);
   int initialize_from_map(int member);
   int initialize_states(int member, const double* states, const double* weights, uint64_t n);
@@ -64,6 +74,11 @@ class Batch {
     uint64_t ancestors_n{0};
     uint64_t table_offset{0};  // its hash table in the cluster scratch
     uint32_t table_slots{0};   // a power of two >= 2 * capacity
+    int map{-1};               // id of the map it reads (-1: none)
+  };
+  struct MapEntry {
+    DeviceMap map;
+    int slot{0};  // its entry in the device map table
   };
   int fail(int status, const std::string& message) {
     error_ = message;
@@ -71,16 +86,23 @@ class Batch {
   }
   int check(cudaError_t e, const char* what) { return cuda_check(e, what, &error_); }
   int member_ok(int member) const;
+  const MapEntry* find_map(int id) const;
   int ensure_points(uint64_t n_points);
   bool ensure_hits(uint64_t words);
   int set_map(const MapTables& tables);
+  int add_map(const MapTables& tables, int* id);
+  int ensure_map_table();
   int ensure_cluster_scratch();
   int ensure_cluster_records(uint64_t cells);
 
   std::vector<Member> members_;
   int device_{0};
   cudaStream_t stream_{nullptr};
-  DeviceMap map_;
+  std::map<int, MapEntry> maps_;  // by id
+  int next_map_id_{0};
+  BatchMap* map_table_{nullptr};  // device: one entry per map (MapEntry::slot), for steps whose members read several maps
+  size_t map_table_capacity_{0};
+  bool map_table_current_{false};  // the table and the slots match maps_
   bool created_{false};
   int create_status_{BB200_OK};
   mutable std::string error_;

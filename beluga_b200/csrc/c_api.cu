@@ -828,6 +828,31 @@ int bb200_amcl_batch_set_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p
   BB_REQUIRE(b && p && grid);
   return guarded(b->impl, [&] { return b->impl.set_beam_map(*p, *grid); });
 }
+int bb200_amcl_batch_add_likelihood_field_map(bb200_amcl_batch* b, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid,
+                                              int prob, int* map_id) {
+  BB_REQUIRE(b && p && grid && map_id);
+  return guarded(b->impl, [&] { return b->impl.add_likelihood_field_map(*p, *grid, prob != 0, map_id); });
+}
+int bb200_amcl_batch_add_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p, const bb200_occupancy_grid* grid, int* map_id) {
+  BB_REQUIRE(b && p && grid && map_id);
+  return guarded(b->impl, [&] { return b->impl.add_beam_map(*p, *grid, map_id); });
+}
+int bb200_amcl_batch_update_map(bb200_amcl_batch* b, int member, int map_id) {
+  BB_REQUIRE(b);
+  return guarded(b->impl, [&] { return b->impl.update_map(member, map_id); });
+}
+int bb200_amcl_batch_member_map(const bb200_amcl_batch* b, int member, int* map_id) {
+  BB_REQUIRE(b && map_id);
+  return guarded(b->impl, [&] { return b->impl.member_map(member, map_id); });
+}
+int bb200_amcl_batch_remove_map(bb200_amcl_batch* b, int map_id) {
+  BB_REQUIRE(b);
+  return guarded(b->impl, [&] { return b->impl.remove_map(map_id); });
+}
+int bb200_amcl_batch_get_likelihood_field(const bb200_amcl_batch* b, int map_id, float* out, uint64_t capacity) {
+  BB_REQUIRE(b && out);
+  return guarded(b->impl, [&] { return b->impl.get_likelihood_field(map_id, out, capacity); });
+}
 int bb200_amcl_batch_initialize(bb200_amcl_batch* b, int member, const double mean_xytheta[3], const double cov[9]) {
   BB_REQUIRE(b && mean_xytheta && cov);
   return guarded(b->impl, [&] { return b->impl.initialize(member, mean_xytheta, cov); });

@@ -1996,6 +1996,42 @@ __device__ __forceinline__ Pose2* batch_states(const BatchStepArgs& s, const Bat
   return ((m.cur ^ which) != 0 ? s.states[1] : s.states[0]) + m.offset;
 }
 
+// Where a member's map views come from: the parameter block when every member of the step reads one map (kTable false:
+// the views stay in the constant bank, as in the single-filter kernels), the batch's map table otherwise.
+template <bool kTable>
+__device__ __forceinline__ const FieldView& batch_field(const BatchStepArgs& s, const BatchMember& m) {
+  if constexpr (kTable) return s.maps[m.map].field;
+  else return s.field;
+}
+template <bool kTable>
+__device__ __forceinline__ const OccupancyView& batch_occupancy(const BatchStepArgs& s, const BatchMember& m) {
+  if constexpr (kTable) return s.maps[m.map].occupancy;
+  else return s.occupancy;
+}
+template <bool kTable>
+__device__ __forceinline__ const BeamParams& batch_beam(const BatchStepArgs& s, const BatchMember& m) {
+  if constexpr (kTable) return s.maps[m.map].beam;
+  else return s.beam;
+}
+/// Recovery injection's free cells and grid geometry.
+template <bool kTable>
+__device__ __forceinline__ void batch_recovery_map(const BatchStepArgs& s, const BatchMember& m, ResampleArgs& a) {
+  if constexpr (kTable) {
+    const BatchMap& map = s.maps[m.map];
+    a.free_cells = map.free_cells;
+    a.n_free = map.n_free;
+    a.grid_width = map.grid_width;
+    a.grid_resolution = map.grid_resolution;
+    a.grid_origin = map.grid_origin;
+  } else {
+    a.free_cells = s.free_cells;
+    a.n_free = s.n_free;
+    a.grid_width = s.grid_width;
+    a.grid_resolution = s.grid_resolution;
+    a.grid_origin = s.grid_origin;
+  }
+}
+
 /// The per-step scalars of every member (what begin_fused_step_kernel resets for one filter) and the scan state.
 __global__ void __launch_bounds__(256) batch_begin_kernel(BatchStepArgs s) {
   const uint32_t stride = gridDim.x * 256;
@@ -2023,7 +2059,9 @@ __global__ void __launch_bounds__(kPrThreads) batch_propagate_kernel(BatchStepAr
 }
 
 /// One CTA of reweight_lfm_fixed_kernel (or, for maps beyond kFixedMaxSide, reweight_lfm_kernel) per 256 particles of a
-/// member; each member's scan is staged into shared memory in kChunkBeams-point chunks.
+/// member; each member's scan is staged into shared memory in kChunkBeams-point chunks.  The kernel is chosen per member
+/// (by its map), so it is uniform within a CTA.
+template <bool kTable>
 __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm) batch_reweight_kernel(BatchStepArgs s) {
   uint32_t local, count;
   const uint32_t k = batch_member_of(s, kBatchReweight, blockIdx.x, local, count);
@@ -2031,43 +2069,49 @@ __global__ void __launch_bounds__(kRwThreads, kRwBlocksPerSm) batch_reweight_ker
   const Pose2* states = batch_states(s, m, 0);
   const double2* points = reinterpret_cast<const double2*>(s.points) + m.point_offset;
   const uint64_t slot_base = static_cast<uint64_t>(local) * kRwThreads;
-  if (s.field.use_fixed) {
-    reweight_lfm_fixed_block(states, s.weights + m.offset, m.n, nullptr, s.field, points, m.n_points, m.points_radius, s.scalars + k, slot_base);
+  const FieldView& field = batch_field<kTable>(s, m);
+  if (field.use_fixed) {
+    reweight_lfm_fixed_block(states, s.weights + m.offset, m.n, nullptr, field, points, m.n_points, m.points_radius, s.scalars + k, slot_base);
   } else {
-    reweight_lfm_block(states, s.weights + m.offset, m.n, nullptr, s.field, points, m.n_points, m.points_radius, s.scalars + k, slot_base);
+    reweight_lfm_block(states, s.weights + m.offset, m.n, nullptr, field, points, m.n_points, m.points_radius, s.scalars + k, slot_base);
   }
 }
 
-// The beam model's kernels take their CTAs from the kBatchReweight range too: one CTA per 256 particles in all of them.
+// batch_member_ctas sizes every reweight row (kBatchReweight, kBatchReweightWalk, kBatchReweightBeam) with kRwThreads: one
+// CTA per 256 particles in every reweight form.
 static_assert(kWalkThreads == kRwThreads && kMixThreads == kRwThreads && kBeamThreads == kRwThreads,
-              "every reweight form of a batch step shares the kBatchReweight CTA range");
+              "batch_member_ctas sizes every reweight row of a batch step with kRwThreads");
 
 /// beam_walk_kernel per member: the whole member in one pass, its hit words beam-major at hits + hit_offset.
+template <bool kTable>
 __global__ void __launch_bounds__(kWalkThreads, kWalkBlocksPerSm) batch_beam_walk_kernel(BatchStepArgs s) {
   uint32_t local, count;
-  const BatchMember& m = s.members[batch_member_of(s, kBatchReweight, blockIdx.x, local, count)];
+  const BatchMember& m = s.members[batch_member_of(s, kBatchReweightWalk, blockIdx.x, local, count)];
   const double2* points = reinterpret_cast<const double2*>(s.points) + m.point_offset;
-  beam_walk_block(batch_states(s, m, 0), m.n, 0, m.n, nullptr, s.occupancy, s.beam.beam_max_range, points, m.n_points, s.hits + m.hit_offset,
-                  m.hit_stride, local);
+  beam_walk_block(batch_states(s, m, 0), m.n, 0, m.n, nullptr, batch_occupancy<kTable>(s, m), batch_beam<kTable>(s, m).beam_max_range, points,
+                  m.n_points, s.hits + m.hit_offset, m.hit_stride, local);
 }
 
 /// beam_mixture_kernel per member over the words batch_beam_walk_kernel wrote; the largest weight into the member's scalars.
+template <bool kTable>
 __global__ void __launch_bounds__(kMixThreads) batch_beam_mixture_kernel(BatchStepArgs s) {
   uint32_t local, count;
-  const uint32_t k = batch_member_of(s, kBatchReweight, blockIdx.x, local, count);
+  const uint32_t k = batch_member_of(s, kBatchReweightWalk, blockIdx.x, local, count);
   const BatchMember& m = s.members[k];
   const double2* points = reinterpret_cast<const double2*>(s.points) + m.point_offset;
-  beam_mixture_block(batch_states(s, m, 0), s.weights + m.offset, m.n, 0, m.n, nullptr, s.occupancy, s.beam, points, m.n_points,
-                     s.hits + m.hit_offset, m.hit_stride, s.scalars + k, local);
+  beam_mixture_block(batch_states(s, m, 0), s.weights + m.offset, m.n, 0, m.n, nullptr, batch_occupancy<kTable>(s, m), batch_beam<kTable>(s, m),
+                     points, m.n_points, s.hits + m.hit_offset, m.hit_stride, s.scalars + k, local);
 }
 
 /// reweight_beam_kernel per member (maps the walk cannot take, or a step whose hit words would not fit).
+template <bool kTable>
 __global__ void __launch_bounds__(kBeamThreads, kBeamBlocksPerSm) batch_reweight_beam_kernel(BatchStepArgs s) {
   uint32_t local, count;
-  const uint32_t k = batch_member_of(s, kBatchReweight, blockIdx.x, local, count);
+  const uint32_t k = batch_member_of(s, kBatchReweightBeam, blockIdx.x, local, count);
   const BatchMember& m = s.members[k];
   const double2* points = reinterpret_cast<const double2*>(s.points) + m.point_offset;
-  reweight_beam_block(batch_states(s, m, 0), s.weights + m.offset, m.n, nullptr, s.occupancy, s.beam, points, m.n_points, s.scalars + k, local);
+  reweight_beam_block(batch_states(s, m, 0), s.weights + m.offset, m.n, nullptr, batch_occupancy<kTable>(s, m), batch_beam<kTable>(s, m), points,
+                      m.n_points, s.scalars + k, local);
 }
 
 /// quantize_scan_kernel per member: the exponent from the member's own largest weight, its own look-back state.
@@ -2129,6 +2173,7 @@ __device__ __forceinline__ void normalize_moments_block(const Pose2* __restrict_
 
 /// Per member: resample_scatter_kernel or resample_kernel (recovery injection, multinomial draws) on a resampling step,
 /// normalisation otherwise; then the member's moments, summed by its last CTA.
+template <bool kTable>
 __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs s) {
   uint32_t local, count;
   const uint32_t k = batch_member_of(s, kBatchFinish, blockIdx.x, local, count);
@@ -2153,11 +2198,7 @@ __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs 
   a.seed = m.seed;
   a.step = m.step;
   a.random_state_probability = m.random_state_probability;
-  a.free_cells = s.free_cells;
-  a.n_free = s.n_free;
-  a.grid_width = s.grid_width;
-  a.grid_resolution = s.grid_resolution;
-  a.grid_origin = s.grid_origin;
+  batch_recovery_map<kTable>(s, m, a);
   a.pivot_x = m.pivot_x;
   a.pivot_y = m.pivot_y;
   if (m.scheme == 1 && m.random_state_probability <= 0.0) {  // systematic, nothing drawn per slot: launch_resample's scatter form
@@ -2502,9 +2543,10 @@ uint32_t resample_scatter_block_count(uint64_t n_in) {
 
 uint32_t batch_scan_tiles(uint64_t n) { return scan_tile_count(n); }
 
-void batch_member_ctas(const BatchMember& m, uint32_t out[kBatchLaunches]) {
+void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunches]) {
   out[kBatchPropagate] = static_cast<uint32_t>((m.n + kPrThreads - 1) / kPrThreads);
-  out[kBatchReweight] = static_cast<uint32_t>((m.n + kRwThreads - 1) / kRwThreads);
+  out[kBatchReweight] = out[kBatchReweightWalk] = out[kBatchReweightBeam] = 0;
+  out[batch_reweight_row(form)] = static_cast<uint32_t>((m.n + kRwThreads - 1) / kRwThreads);
   out[kBatchScan] = scan_tile_count(m.n);
   // the partition launch_resample / launch_moments would use for a single filter of this size
   if (!m.resample) {
@@ -2516,24 +2558,35 @@ void batch_member_ctas(const BatchMember& m, uint32_t out[kBatchLaunches]) {
   }
 }
 
-int launch_batch_step(const BatchStepArgs& s, cudaStream_t stream) {
+namespace {
+template <bool kTable>
+int launch_batch_step_from(const BatchStepArgs& s, cudaStream_t stream) {
   const uint32_t reset = std::max(s.n_members, s.ctas[kBatchScan]);
   batch_begin_kernel<<<std::max(1u, std::min((reset + 255u) / 256u, kSmCount * 4u)), 256, 0, stream>>>(s);
   batch_propagate_kernel<<<s.ctas[kBatchPropagate], kPrThreads, 0, stream>>>(s);
-  int launches = 5;
-  if (s.path == kBatchBeamTwoPass) {
-    batch_beam_walk_kernel<<<s.ctas[kBatchReweight], kWalkThreads, 0, stream>>>(s);
-    batch_beam_mixture_kernel<<<s.ctas[kBatchReweight], kMixThreads, 0, stream>>>(s);
-    launches = 6;
-  } else if (s.path == kBatchBeamFused) {
-    batch_reweight_beam_kernel<<<s.ctas[kBatchReweight], kBeamThreads, 0, stream>>>(s);
-  } else {
+  int launches = 4;
+  if (s.forms & (1 << kBatchField)) {
     const size_t smem = static_cast<size_t>(std::min(s.max_points, kChunkBeams)) * sizeof(double2);
-    batch_reweight_kernel<<<s.ctas[kBatchReweight], kRwThreads, smem, stream>>>(s);
+    batch_reweight_kernel<kTable><<<s.ctas[kBatchReweight], kRwThreads, smem, stream>>>(s);
+    launches += 1;
+  }
+  if (s.forms & (1 << kBatchBeamTwoPass)) {
+    batch_beam_walk_kernel<kTable><<<s.ctas[kBatchReweightWalk], kWalkThreads, 0, stream>>>(s);
+    batch_beam_mixture_kernel<kTable><<<s.ctas[kBatchReweightWalk], kMixThreads, 0, stream>>>(s);
+    launches += 2;
+  }
+  if (s.forms & (1 << kBatchBeamFused)) {
+    batch_reweight_beam_kernel<kTable><<<s.ctas[kBatchReweightBeam], kBeamThreads, 0, stream>>>(s);
+    launches += 1;
   }
   batch_scan_kernel<<<s.ctas[kBatchScan], kQsThreads, 0, stream>>>(s);
-  batch_finish_kernel<<<s.ctas[kBatchFinish], kRsThreads, 0, stream>>>(s);
+  batch_finish_kernel<kTable><<<s.ctas[kBatchFinish], kRsThreads, 0, stream>>>(s);
   return launches;
+}
+}  // namespace
+
+int launch_batch_step(const BatchStepArgs& s, cudaStream_t stream) {
+  return s.maps != nullptr ? launch_batch_step_from<true>(s, stream) : launch_batch_step_from<false>(s, stream);
 }
 
 uint32_t launch_resample(const ResampleArgs& args, Scalars* scalars, double* moment_partials, cudaStream_t stream) {

@@ -412,7 +412,7 @@ struct BatchMember {
   int scheme;               // bb200_resample_scheme
   int cur;                  // state buffer holding the member's particles
   int ceil_log2_count;      // of max_particles: the fixed-point exponent's headroom
-  int pad;
+  int map;                  // the member's entry in BatchStepArgs::maps (read only when that table is set)
   double random_state_probability;
   double pivot_x, pivot_y;  // of the raw moments (the member's last estimate)
   MotionSampling sampling;
@@ -423,8 +423,35 @@ struct BatchMember {
   uint64_t hit_stride;      // ... beam-major, round_up(n, 32) words per beam (the single filter's layout)
 };
 
-/// Start of member m's CTA range in each launch: first[m] .. first[m + 1] (n_members + 1 entries per launch).
-enum BatchLaunch : int { kBatchPropagate = 0, kBatchReweight = 1, kBatchScan = 2, kBatchFinish = 3, kBatchLaunches = 4 };
+/// Start of member m's CTA range in each row: first[m] .. first[m + 1] (n_members + 1 entries per row).  The three
+/// reweight forms have a row each; a member has CTAs in the row of its own form and an empty range in the other two.
+enum BatchLaunch : int {
+  kBatchPropagate = 0,
+  kBatchReweight = 1,      // likelihood field
+  kBatchScan = 2,
+  kBatchFinish = 3,
+  kBatchReweightWalk = 4,  // beam model, two-pass form (walk and mixture)
+  kBatchReweightBeam = 5,  // beam model, fused form
+  kBatchLaunches = 6
+};
+/// The reweight forms of a batch step; BatchStepArgs::forms has bit f set when some member takes form f.
+enum BatchReweightPath : int { kBatchField = 0, kBatchBeamTwoPass = 1, kBatchBeamFused = 2 };
+/// The CTA-range row of each reweight form.
+constexpr int batch_reweight_row(int form) {
+  return form == kBatchField ? kBatchReweight : form == kBatchBeamTwoPass ? kBatchReweightWalk : kBatchReweightBeam;
+}
+
+/// One map of a batch: the views and grid geometry the batch kernels read, one entry of Batch's device map table.
+struct BatchMap {
+  FieldView field;
+  OccupancyView occupancy;
+  BeamParams beam;
+  const uint32_t* free_cells;
+  uint64_t n_free;
+  int grid_width;
+  double grid_resolution;
+  Pose2 grid_origin;
+};
 
 struct BatchStepArgs {
   const BatchMember* members;     // device
@@ -451,22 +478,24 @@ struct BatchStepArgs {
   int* ticket;                    // pinned: stores `seq` once every member's summary is complete
   int seq;
   // The beam model (after the likelihood-field members so that those kernels keep their parameter offsets).
-  int path;                       // BatchReweightPath
+  int forms;                      // bit f: some member takes reweight form f (BatchReweightPath)
   OccupancyView occupancy;
   BeamParams beam;
   uint32_t* hits;                 // two-pass form: every member's hit words (BatchMember::hit_offset)
+  // Null when every member of the step reads one map, whose views are the fields above (field, free_cells ... beam);
+  // otherwise the device table of the batch's maps, and each member reads maps[BatchMember::map].
+  const BatchMap* maps;
 };
 static_assert(sizeof(BatchStepArgs) <= 1024, "the step's arguments travel as one kernel parameter block (4 KB at most)");
-/// Reweight | scan | finish: the likelihood field in one launch, the beam model's walk and mixture in two (two-pass form)
-/// or in one (fused form).
-enum BatchReweightPath : int { kBatchField = 0, kBatchBeamTwoPass = 1, kBatchBeamFused = 2 };
-/// Reset | propagate | reweight | quantise + scan | resample or normalise + moments.  Returns the number of launches: 5, or
-/// 6 for the beam model's two-pass form, whatever the members, their particle counts and their scans are.
+/// Reset | propagate | reweight | quantise + scan | resample or normalise + moments.  The reweight takes one launch for the
+/// likelihood field, two for the beam model's two-pass form (walk, mixture) and one for its fused form, each issued
+/// when some member takes that form.  Returns the number of launches: 4 plus those, so 5 to 8, whatever the members,
+/// their maps, their particle counts and their scans are.
 int launch_batch_step(const BatchStepArgs& args, cudaStream_t stream);
 /// Scan tiles of a member of n particles (the quantise-scan CTAs it needs).
 uint32_t batch_scan_tiles(uint64_t n);
-/// CTAs of a member in the launches of a batch step: propagate, reweight, scan, finish.
-void batch_member_ctas(const BatchMember& m, uint32_t out[kBatchLaunches]);
+/// CTAs of a member in each row of a batch step's ranges, for a member that takes reweight form `form`.
+void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunches]);
 
 /// Per-block raw weighted moments of (states, weights).
 uint32_t moments_block_count(uint64_t n);

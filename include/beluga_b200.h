@@ -524,23 +524,26 @@ int bb200_amcl_join_shards(bb200_amcl* a, int world, int rank, const void* handl
 int bb200_amcl_leave_shards(bb200_amcl* a);
 
 /* ---------------------------------------------------------------------------------------------
- * Many independent filters on one GPU: a batch of K beluga::Amcl members that share one device, one
- * map and one sensor model -- a fleet server localising many robots against one site
- * map, a simulator with many agents.  bb200_amcl_batch_update steps every member that has a new scan
- * with a fixed number of kernel launches and one host synchronisation, whatever K is; each member's
- * result and particles are bit-identical to what a standalone bb200_amcl with the same parameters returns
- * for the same inputs.
+ * Many independent filters on one GPU: a batch of K beluga::Amcl members that share one device -- a
+ * fleet server localising many robots on one or several site maps, a simulator with many agents.
+ * bb200_amcl_batch_update steps every member that has a new scan with a fixed number of kernel launches
+ * and one host synchronisation, whatever K is; each member's result and particles are bit-identical to
+ * what a standalone bb200_amcl with the same parameters returns for the same inputs.
  *
  * Every member has its own parameter block (seed, policies, resampling scheme, recovery override) and
  * motion model.  Members keep a fixed particle count: bb200_amcl_batch_create rejects, before touching a
  * device, with BB200_ERR_INVALID_ARGUMENT: n_members < 1, min_particles != max_particles (KLD), selective
  * resampling, non-zero shard fields, max_particles of 0 or above 32768, and members on different devices.
- * The map chooses the sensor model: either likelihood-field model (bb200_amcl_batch_set_likelihood_field_map)
- * or the beam model (bb200_amcl_batch_set_beam_map).  A step takes 5 kernel launches, or 6 for the beam model
- * on maps where a standalone filter walks its rays in two passes; there the batch does the same unless the
- * step's hit words (sum over the updating members of round_up(n, 32) x scan points x 4 bytes) exceed 3 GiB
- * or cannot be allocated, and then takes the fused beam kernel in 5 launches.  Either way every member's results stay
- * bit-identical to its standalone twin's.
+ *
+ * A batch holds a set of maps, each a grid with its sensor model: likelihood-field model or the beam model.
+ * Each member reads one of them or none.  bb200_amcl_batch_set_likelihood_field_map and _set_beam_map give every
+ * member one map; bb200_amcl_batch_add_*_map and bb200_amcl_batch_update_map let members read different maps and
+ * move between them, as a node's Amcl::update_map does.  Each reweight form that some updating member takes costs
+ * launches: the likelihood field 1, the beam model 2 on maps where a standalone filter walks its rays in two
+ * passes, and 1 otherwise.  A step takes 4 launches plus those, so 5 to 8, whatever K and the number of maps are;
+ * a step whose updating members read one map takes 5, or 6 for the two-pass beam form.  The two-pass members of a
+ * step take the fused beam kernel instead when their hit words (sum of round_up(n, 32) x scan points x 4 bytes)
+ * exceed 3 GiB or cannot be allocated.  Either way every member's results stay bit-identical to its standalone twin's.
  *
  * The fleet loop of a beluga_ros node per member is bb200_amcl_batch_update, then
  * bb200_amcl_batch_cluster_estimates for the members that updated: the estimate every node publishes, for all of them
@@ -553,13 +556,32 @@ void bb200_amcl_batch_destroy(bb200_amcl_batch* b);
 const char* bb200_amcl_batch_last_error(const bb200_amcl_batch* b);
 int bb200_amcl_batch_members(const bb200_amcl_batch* b);
 /* One likelihood field (prob != 0: the prob model) for every member, built and uploaded once.  Replaces any earlier
- * map, whichever sensor model it was for. */
+ * map, whichever sensor model it was for: removes every map, adds this one (it takes the next map id) and assigns
+ * every member to it. */
 int bb200_amcl_batch_set_likelihood_field_map(bb200_amcl_batch* b, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid,
                                               int prob);
 /* One beam-model map (BeamSensorModel) for every member, built and uploaded once; replaces any earlier map the same way.
  * BB200_ERR_INVALID_ARGUMENT for a null handle or argument. */
 int bb200_amcl_batch_set_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p, const bb200_occupancy_grid* grid);
-/* bb200_amcl_initialize / _initialize_from_map / _initialize_states / _force_update for member `member`. */
+/* Build and upload a map without assigning it to any member (LikelihoodFieldModel / LikelihoodFieldProbModel, or
+ * BeamSensorModel); *map_id receives its id.  Ids start at 0 over the batch's life, increase, and are never reused. */
+int bb200_amcl_batch_add_likelihood_field_map(bb200_amcl_batch* b, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid,
+                                              int prob, int* map_id);
+int bb200_amcl_batch_add_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p, const bb200_occupancy_grid* grid, int* map_id);
+/* Amcl::update_map (amcl_core.hpp:150) / beluga_ros::Amcl::update_map (beluga_ros/src/amcl.cpp:48-51) for one member:
+ * its particles and policies are kept; its next reweight, recovery injection and initialize_from_map use map_id. */
+int bb200_amcl_batch_update_map(bb200_amcl_batch* b, int member, int map_id);
+/* The map of a member (-1: none). */
+int bb200_amcl_batch_member_map(const bb200_amcl_batch* b, int member, int* map_id);
+/* Free a map; BB200_ERR_STATE while a member uses it. */
+int bb200_amcl_batch_remove_map(bb200_amcl_batch* b, int map_id);
+/* likelihood_field() of a likelihood-field map, height x width row-major (what a node publishes after a map update,
+ * amcl_node.cpp:473-476).  BB200_ERR_STATE for a beam-model map, BB200_ERR_CAPACITY when capacity is too small.
+ * Every call above returns BB200_ERR_INVALID_ARGUMENT for a null handle or argument, a bad member index or an unknown
+ * or removed map id, and then leaves the batch unchanged. */
+int bb200_amcl_batch_get_likelihood_field(const bb200_amcl_batch* b, int map_id, float* out, uint64_t capacity);
+/* bb200_amcl_initialize / _initialize_from_map / _initialize_states / _force_update for member `member`.
+ * _initialize_from_map samples the member's own map (BB200_ERR_STATE when it has none). */
 int bb200_amcl_batch_initialize(bb200_amcl_batch* b, int member, const double mean_xytheta[3], const double cov[9]);
 int bb200_amcl_batch_initialize_from_map(bb200_amcl_batch* b, int member);
 int bb200_amcl_batch_initialize_states(bb200_amcl_batch* b, int member, const double* states, const double* weights, uint64_t n);

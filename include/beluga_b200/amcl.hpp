@@ -15,6 +15,7 @@
 #pragma once
 
 #include <execution>
+#include <map>
 #include <optional>
 #include <utility>
 
@@ -205,8 +206,8 @@ template <class MotionModel, class SensorModel, class ExecutionPolicy>
   return std::make_pair(SE2d::from_data(e.mean), cov);
 }
 
-/// K independent filters on one GPU that share one map (bb200_amcl_batch), for a likelihood-field model or the beam model:
-/// update() steps every member with a new scan at once.  Member m behaves like an Amcl built from motions[m] and params[m]; members keep a fixed
+/// K independent filters on one GPU (bb200_amcl_batch) that read one or several maps, each for a likelihood-field model or
+/// the beam model: update() steps every member with a new scan at once.  Member m behaves like an Amcl built from motions[m] and params[m]; members keep a fixed
 /// particle count (min_particles == max_particles <= 32768).  Results are returned per member, std::nullopt where the
 /// reference's update would return it or where the member had no scan this step.
 class AmclBatch {
@@ -231,9 +232,47 @@ class AmclBatch {
   /// One likelihood field for every member (prob: the LikelihoodFieldProb model).
   void set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob = false) {
     check(bb200_amcl_batch_set_likelihood_field_map(handle_, &p, &grid, prob ? 1 : 0));
+    field_cells_.clear();
+    field_cells_[member_map(0)] = static_cast<std::size_t>(grid.width) * static_cast<std::size_t>(grid.height);
   }
   /// One beam-model map (BeamSensorModel) for every member; replaces the map set before, whichever model it was for.
-  void set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid) { check(bb200_amcl_batch_set_beam_map(handle_, &p, &grid)); }
+  void set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid) {
+    check(bb200_amcl_batch_set_beam_map(handle_, &p, &grid));
+    field_cells_.clear();
+  }
+  /// Adds a map that no member reads yet and returns its id (several floors or sites in one batch).
+  int add_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob = false) {
+    int id = -1;
+    check(bb200_amcl_batch_add_likelihood_field_map(handle_, &p, &grid, prob ? 1 : 0, &id));
+    field_cells_[id] = static_cast<std::size_t>(grid.width) * static_cast<std::size_t>(grid.height);
+    return id;
+  }
+  int add_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid) {
+    int id = -1;
+    check(bb200_amcl_batch_add_beam_map(handle_, &p, &grid, &id));
+    return id;
+  }
+  /// Amcl::update_map (amcl_core.hpp:150) for one member: it keeps its particles and reads map `map_id` from its next step.
+  void update_map(std::size_t member, int map_id) { check(bb200_amcl_batch_update_map(handle_, index(member), map_id)); }
+  /// The id of the map member m reads (-1: none).
+  [[nodiscard]] int member_map(std::size_t member) const {
+    int id = -1;
+    check(bb200_amcl_batch_member_map(handle_, index(member), &id));
+    return id;
+  }
+  /// Frees a map no member reads.
+  void remove_map(int map_id) {
+    check(bb200_amcl_batch_remove_map(handle_, map_id));
+    field_cells_.erase(map_id);
+  }
+  /// likelihood_field() of a likelihood-field map: height x width values, row-major.
+  [[nodiscard]] std::vector<float> likelihood_field(int map_id) const {
+    const auto it = field_cells_.find(map_id);
+    std::vector<float> out(it != field_cells_.end() ? it->second : 0);
+    float unused = 0.0f;  // an unknown id still reaches the batch, which refuses it
+    check(bb200_amcl_batch_get_likelihood_field(handle_, map_id, out.empty() ? &unused : out.data(), out.size()));
+    return out;
+  }
   void initialize(std::size_t member, const SE2d& pose, const Matrix3d& covariance) {
     const double mean[3] = {pose.x(), pose.y(), pose.theta()};
     check(bb200_amcl_batch_initialize(handle_, index(member), mean, covariance.data()));
@@ -323,6 +362,7 @@ class AmclBatch {
 
   bb200_amcl_batch* handle_{nullptr};
   std::vector<std::size_t> sizes_;
+  std::map<int, std::size_t> field_cells_;  // cells of each likelihood-field map, by id
 };
 
 }  // namespace beluga_b200

@@ -3,7 +3,8 @@
 `cloud`: 65 536-point lidar clouds at 10k and 1M particles.  `batch`: K node-sized filters (2000 particles x 100 points) stepped as one
 AmclBatch against K standalone Amcl stepped one after another.  `batch_cluster`: the same batches with the beluga_ros-shaped round
 update + cluster estimate, the estimate taken for all members in one call and member by member.  `batch_beam`: AmclBatch with the
-beam model (60 and 720 points per member) against the same members stepped as standalone Amcl.
+beam model (60 and 720 points per member) against the same members stepped as standalone Amcl.  `batch_maps`: one AmclBatch whose
+members read 1, 4 or 16 likelihood-field maps against one single-map batch per map, and a step mixing likelihood-field and beam members.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import json
@@ -187,6 +188,102 @@ def run_batch_beam():
     return res
 
 
+def batch_reweight_ms(batch, poses, scans, steps):
+    """Mean device time per step of the batch's reweight kernels (names containing batch_reweight or batch_beam), from
+    torch.profiler in a run of its own; poses[t] and scans[t] are step t's inputs of every member."""
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for t in range(steps):
+            batch.update(poses[t], scans[t])
+    total_us = sum(e.device_time_total for e in prof.key_averages() if "batch_reweight" in e.key or "batch_beam" in e.key)
+    return total_us / 1e3 / steps
+
+
+def run_batch_maps():
+    """K in {64, 256} members x 2000 particles x 100 points spread evenly (member m on map m % M) over M in {1, 4, 16}
+    likelihood-field maps of 2000^2, each a different synthetic scene, systematic resampling, every member updating every
+    step.  One AmclBatch with M maps against M single-map batches (K / M members each) stepped one after another, in the
+    same process, alternating step by step.  Also the batch's reweight kernel time per step (torch.profiler, separate
+    run), which shows what spreading the members' lookups over M tables (16 x 32 MB of fixed-point tables at M = 16,
+    beyond the 50 MB L2) costs; and one mixed step (likelihood-field and beam members) with its launch count."""
+    res = {}
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    n, steps, warmup = 2000, 20, 3
+    device = device_record()
+    scenes = [synthetic.make_scenario(grid_size=2000, n_beams=100, steps=warmup + steps, map_seed=42 + j) for j in range(16)]
+    grids = [bb.OccupancyGrid(s.cells, s.resolution) for s in scenes]
+
+    def make(members, maps):
+        """A batch whose member i reads maps[i % len(maps)] (scene indices), initialised on that scene."""
+        params = [bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m) for m in members]
+        b = bb.AmclBatch([bb.DifferentialDriveModelParam(*MOTION) for _ in members], params)
+        ids = [b.add_likelihood_field_map(lfm, grids[j]) for j in maps]
+        for i in range(len(members)):
+            b.update_map(i, ids[i % len(maps)])
+            s = scenes[maps[i % len(maps)]]
+            b.initialize(i, s.initial_mean, s.initial_cov)
+        return b
+
+    def inputs(members, maps, t):
+        return ([bb.se2(*scenes[maps[i % len(maps)]].poses[t]) for i in range(len(members))],
+                [scenes[maps[i % len(maps)]].scans[t] for i in range(len(members))])
+
+    for k in (64, 256):
+        for n_maps in (1, 4, 16):
+            maps = list(range(n_maps))
+            multi = make(list(range(k)), maps)
+            singles = [make(list(range(j, k, n_maps)), [j]) for j in maps]
+            wall_multi, wall_singles, launches = [], [], []
+            for t in range(warmup + steps):
+                # both arms' inputs are built before their timed windows, which hold only the update calls
+                poses, scans = inputs(range(k), maps, t)
+                single_inputs = [inputs(range(j, k, n_maps), [j], t) for j in maps]
+                before = multi.launch_count()
+                t0 = time.perf_counter()
+                r = multi.update(poses, scans)
+                t1 = time.perf_counter()
+                rs = [b.update(p, s) for b, (p, s) in zip(singles, single_inputs)]
+                t2 = time.perf_counter()
+                launches.append(multi.launch_count() - before)
+                assert all(x.updated for x in r) and all(x.updated for rr in rs for x in rr)
+                if t >= warmup:
+                    wall_multi.append((t1 - t0) * 1e3)
+                    wall_singles.append((t2 - t1) * 1e3)
+            mb, ms = float(np.median(wall_multi)), float(np.median(wall_singles))
+            prof_poses, prof_scans = zip(*[inputs(range(k), maps, t % (warmup + steps)) for t in range(10)])
+            res[f"batch_maps_{k}_x_{n}_x_100_lfm_2000_{n_maps}_maps"] = {
+                "members": k, "particles": n, "points": 100, "maps": n_maps, "steps": steps,
+                "ms_per_step_e2e": mb, "member_steps_per_s": k * 1e3 / mb, "launches_per_step": int(max(launches)),
+                "single_map_batches_ms_per_round": ms, "single_map_batches_member_steps_per_s": k * 1e3 / ms,
+                "reweight_kernel_ms_per_step": batch_reweight_ms(multi, prof_poses, prof_scans, 10),
+                "kernels_ms": {}, "device": device}
+            del multi, singles
+    # one mixed step: half the members on a likelihood field, half on a beam map of the same scene (two-pass walk)
+    k = 64
+    params = [bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m) for m in range(k)]
+    mixed = bb.AmclBatch([bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)], params)
+    ids = [mixed.add_likelihood_field_map(lfm, grids[0]), mixed.add_beam_map(bb.BeamModelParam(beam_max_range=60.0), grids[0])]
+    for m in range(k):
+        mixed.update_map(m, ids[m % 2])
+        mixed.initialize(m, scenes[0].initial_mean, scenes[0].initial_cov)
+    wall, launches = [], []
+    for t in range(warmup + steps):
+        pose = bb.se2(*scenes[0].poses[t])
+        t0 = time.perf_counter()
+        before = mixed.launch_count()
+        assert all(x.updated for x in mixed.update([pose] * k, [scenes[0].scans[t]] * k))
+        t1 = time.perf_counter()
+        launches.append(mixed.launch_count() - before)
+        if t >= warmup:
+            wall.append((t1 - t0) * 1e3)
+    mb = float(np.median(wall))
+    res[f"batch_maps_mixed_{k}_x_{n}_x_100_lfm_and_beam_2000"] = {
+        "members": k, "particles": n, "points": 100, "maps": 2, "steps": steps, "ms_per_step_e2e": mb,
+        "member_steps_per_s": k * 1e3 / mb, "launches_per_step": int(max(launches)), "kernels_ms": {}, "device": device}
+    return res
+
+
 def select_host_ms(states, weights, repeats=50):
     """Host time of the select_cluster pass alone (bb200_cluster_select_host) on the cells of one member's particles at the
     default clusterizer parameters; the records come from a standalone filter's device histogram."""
@@ -332,6 +429,8 @@ def main():
         out.update(run_batch_cluster())
     if "batch_beam" in which:
         out.update(run_batch_beam())
+    if "batch_maps" in which:
+        out.update(run_batch_maps())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}

@@ -731,6 +731,9 @@ class ShardedAmcl:
         return st, w
 
 
+_CELL_DTYPE = np.dtype([("rep", "<f8", 4), ("hash", "<u8"), ("first", "<u4"), ("count", "<u4"), ("weight", "<f8"), ("m", "<f8", 9)])
+
+
 class AmclBatch:
     """bb200_amcl_batch: K independent beluga::Amcl filters on one GPU, each reading one of the batch's maps -- a
     likelihood field or a beam-model map, one for every member (set_*_map) or several (add_*_map and update_map, which
@@ -871,6 +874,42 @@ class AmclBatch:
             e = (np.array(est[m].mean), np.array(est[m].cov).reshape(3, 3))
             out.append((*e, cells[m], clusters[m]) if with_counts else e)
         return out
+
+    def _mask(self, present):
+        k = len(self.params)
+        if present is not None and len(present) != k:
+            raise ValueError("one presence flag per member")
+        return None if present is None else (C.c_uint8 * k)(*[1 if x else 0 for x in present])
+
+    def particle_histograms(self, present=None, linear: float = 1e-3, angular: float = 1e-3):
+        """Filter.particle_histogram of every member whose `present` entry is true (None: all), in one call with a fixed
+        number of kernel launches -> per member (bins, max_bin_weight), None for members not selected.  `bins` is a
+        structured array of bb200_cluster_cell records (fields rep[4], hash, first, count, weight, m[9]) in first-occurrence order."""
+        mask = self._mask(present)
+        k = len(self.params)
+        # A member has at most as many bins as particles: buffers of max_particles bins take every histogram in one pass.
+        bufs = [np.empty(q.max_particles, dtype=_CELL_DTYPE) for q in self.params]
+        bins = (C.POINTER(_capi.ClusterCell) * k)(*[b.ctypes.data_as(C.POINTER(_capi.ClusterCell)) for b in bufs])
+        capacity = (C.c_uint64 * k)(*[len(b) for b in bufs])
+        n_bins, top = (C.c_uint64 * k)(), (C.c_double * k)()
+        self._check(self._lib.bb200_amcl_batch_particle_histograms(self._h, linear, angular, mask, bins, capacity, n_bins, top))
+        return [None if present is not None and not present[m] else (bufs[m][:n_bins[m]].copy(), top[m]) for m in range(k)]
+
+    def sample_states(self, count, step: int = 0xFFFFFFFF, present=None):
+        """Filter.sample_states(count, step) of every member whose `present` entry is true (None: all), in one call ->
+        per member a (count, 4) array [cos, sin, x, y], None for members not selected.  `count`: one number for every
+        member or one per member."""
+        mask = self._mask(present)
+        k = len(self.params)
+        counts = [int(count)] * k if np.isscalar(count) else [int(c) for c in count]
+        if len(counts) != k:
+            raise ValueError("one sample count per member")
+        if any(c < 0 for c in counts):
+            raise ValueError("sample counts must not be negative")
+        outs = [np.zeros((c, 4)) for c in counts]
+        ptrs = (C.POINTER(C.c_double) * k)(*[_dptr(o) if len(o) else None for o in outs])
+        self._check(self._lib.bb200_amcl_batch_sample_states(self._h, (C.c_uint64 * k)(*counts), step, mask, ptrs))
+        return [None if present is not None and not present[m] else outs[m] for m in range(k)]
 
     def update(self, control_poses, points, present=None) -> list:
         """Amcl::update for every member whose `present` entry is true (None: all).  `control_poses`: K poses [c, s, x, y];

@@ -223,6 +223,9 @@ SIGNATURES = {
     "bb200_amcl_batch_ancestors": (C.c_int, [_vp, C.c_int, _P(C.c_int64), C.c_uint64]),
     "bb200_amcl_batch_cluster_estimate": (C.c_int, [_vp, C.c_int, _P(ClusterParam), _P(Estimate)]),
     "bb200_amcl_batch_cluster_estimates": (C.c_int, [_vp, _P(ClusterParam), _P(C.c_uint8), _P(Estimate), _P(C.c_uint32), _P(C.c_uint32)]),
+    "bb200_amcl_batch_particle_histograms": (C.c_int, [_vp, C.c_double, C.c_double, _P(C.c_uint8), _P(_P(ClusterCell)), _P(C.c_uint64),
+                                                       _P(C.c_uint64), _dbl]),
+    "bb200_amcl_batch_sample_states": (C.c_int, [_vp, _P(C.c_uint64), C.c_uint32, _P(C.c_uint8), _P(_dbl)]),
     "bb200_amcl_batch_update": (C.c_int, [_vp, _dbl, _P(_dbl), _P(C.c_uint64), _P(C.c_uint8), _P(UpdateResult)]),
     "bb200_amcl_batch_launch_count": (C.c_uint64, [_vp]),
     "bb200_amcl_plan_update": (C.c_int, [_vp, _dbl, _P(StepPlan)]),

@@ -94,10 +94,10 @@ Batch::~Batch() {
   if (stream_ != nullptr) cudaStreamSynchronize(stream_);
   for (void* p : std::initializer_list<void*>{states_[0], states_[1], weights_, cdf_, ancestors_, scalars_, tile_state_, partials_, table_, first_,
                                               points_, hits_, map_table_, members_done_, cl_hashes_, cl_keys_, cl_first_, cl_ids_, cl_cell_of_, cl_sort_[0], cl_sort_[1],
-                                              cl_starts_, cl_records_, cl_table_, cl_cells_})
+                                              cl_starts_, cl_records_, cl_table_, cl_cells_, sm_table_, samples_})
     cudaFree(p);
   for (void* p : std::initializer_list<void*>{table_host_, first_host_, points_host_, summary_host_, ticket_host_, cl_table_host_, cl_cells_host_,
-                                              cl_records_host_})
+                                              cl_records_host_, sm_table_host_, samples_host_})
     cudaFreeHost(p);
   if (stream_ != nullptr) cudaStreamDestroy(stream_);
 }
@@ -251,6 +251,7 @@ int Batch::initialize(int member, const double mean[3], const double cov[9]) {
   std::string message;
   if (!normal_transform(cov, transform, &message)) return fail(BB200_ERR_INVALID_ARGUMENT, message);
   BB_CHECK(cudaSetDevice(device_));
+  m.cdf_total = 0;
   launch_initialize_normal(states_[m.cur] + m.offset, weights_ + m.offset, m.capacity, mean, transform, m.policy.params().seed, 0, stream_);
   ++launches_;
   BB_CHECK(cudaGetLastError());
@@ -269,6 +270,7 @@ int Batch::initialize_from_map(int member) {
   const DeviceMap& map = maps_.at(m.map).map;
   if (map.n_free == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
   BB_CHECK(cudaSetDevice(device_));
+  m.cdf_total = 0;
   launch_initialize_uniform(states_[m.cur] + m.offset, weights_ + m.offset, m.capacity, map.free_cells, map.n_free, map.grid_width,
                             map.grid_resolution, map.grid_origin, m.policy.params().seed, 0, stream_);
   ++launches_;
@@ -287,6 +289,7 @@ int Batch::initialize_states(int member, const double* states, const double* wei
   if (n > 0 && states == nullptr) return fail(BB200_ERR_INVALID_ARGUMENT, "states is null");
   BB_CHECK(cudaSetDevice(device_));
   BB_CHECK(cudaStreamSynchronize(stream_));
+  m.cdf_total = 0;
   if (n > 0) {
     BB_CHECK(cudaMemcpy(states_[m.cur] + m.offset, states, n * sizeof(Pose2), cudaMemcpyHostToDevice));
     const std::vector<double> ones(weights == nullptr ? n : 0, 1.0);
@@ -372,13 +375,36 @@ int Batch::cluster_estimates(const bb200_cluster_param& p, const uint8_t* presen
   if (!(p.linear_hash_resolution > 0.0) || !(p.angular_hash_resolution > 0.0) || !(p.weight_cap_percentile >= 0.0) ||
       !(p.weight_cap_percentile < 1.0))
     return fail(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)");
-  std::vector<uint32_t> selected;  // in member order
+  std::vector<uint32_t> selected;
+  if (const int st = select_members(present, &selected)) return st;
+  if (selected.empty()) return BB200_OK;
+  if (const int st = cell_records(p.linear_hash_resolution, p.angular_hash_resolution, selected)) return st;
+
+  // Host pass per member (Clusterizer::estimate's): the flood over the cells, then the estimate about the member's pivot.
+  const HostCell* cells = reinterpret_cast<const HostCell*>(cl_records_host_);
+  for (size_t j = 0; j < selected.size(); ++j) {
+    const uint32_t k = selected[j];
+    const Member& m = members_[k];
+    const uint32_t count = cl_cells_host_[j];
+    const ClusterSelection sel = select_cluster(cells, count, m.n, p.linear_hash_resolution, p.angular_hash_resolution, p.weight_cap_percentile);
+    if (out != nullptr) estimate_from_moments(sel.moments, m.pivot, &out[k]);
+    if (n_cells != nullptr) n_cells[k] = count;
+    if (n_clusters != nullptr) n_clusters[k] = sel.clusters;
+    cells += count;
+  }
+  return BB200_OK;
+}
+
+int Batch::select_members(const uint8_t* present, std::vector<uint32_t>* selected) {
   for (size_t k = 0; k < members_.size(); ++k) {
     if (present != nullptr && present[k] == 0) continue;
     if (members_[k].n == 0) return fail(BB200_ERR_STATE, "member " + std::to_string(k) + ": no particles");
-    selected.push_back(static_cast<uint32_t>(k));
+    selected->push_back(static_cast<uint32_t>(k));
   }
-  if (selected.empty()) return BB200_OK;
+  return BB200_OK;
+}
+
+int Batch::cell_records(double linear, double angular, const std::vector<uint32_t>& selected) {
   BB_CHECK(cudaSetDevice(device_));
   if (const int st = ensure_cluster_scratch()) return st;  // every batch call ends synchronised: the pinned buffers are free
 
@@ -404,8 +430,8 @@ int Batch::cluster_estimates(const bb200_cluster_param& p, const uint8_t* presen
   a.states[0] = states_[0];
   a.states[1] = states_[1];
   a.weights = weights_;
-  a.linear = p.linear_hash_resolution;
-  a.angular = p.angular_hash_resolution;
+  a.linear = linear;
+  a.angular = angular;
   a.hashes = cl_hashes_;
   a.keys = cl_keys_;
   a.first = cl_first_;
@@ -426,19 +452,134 @@ int Batch::cluster_estimates(const bb200_cluster_param& p, const uint8_t* presen
   launch_batch_cluster_compact(cl_table_, cl_cells_, cl_records_, n_sel, cl_records_host_, stream);
   BB_LAUNCHED("batch_cluster_compact");
   BB_CHECK(cudaStreamSynchronize(stream));  // 2: every record is in pinned memory
-
-  // Host pass per member (Clusterizer::estimate's): the flood over the cells, then the estimate about the member's pivot.
   static_assert(sizeof(HostCell) == sizeof(CellRecord), "record layouts must agree");
-  const HostCell* cells = reinterpret_cast<const HostCell*>(cl_records_host_);
-  for (uint32_t j = 0; j < n_sel; ++j) {
+  return BB200_OK;
+}
+
+int Batch::particle_histograms(double linear, double angular, const uint8_t* present, bb200_cluster_cell* const* bins, const uint64_t* capacity,
+                               uint64_t* n_bins, double* max_bin_weight) {
+  error_.clear();
+  if (!(linear > 0.0) || !(angular > 0.0)) return fail(BB200_ERR_INVALID_ARGUMENT, "histogram resolutions must be positive");
+  if (bins != nullptr && capacity == nullptr) return fail(BB200_ERR_INVALID_ARGUMENT, "capacity is null");
+  std::vector<uint32_t> selected;
+  if (const int st = select_members(present, &selected)) return st;
+  if (selected.empty()) return BB200_OK;
+  if (const int st = cell_records(linear, angular, selected)) return st;
+
+  // Filter::particle_histogram's host half per member.
+  static_assert(sizeof(bb200_cluster_cell) == sizeof(CellRecord), "public and internal cell records must agree");
+  const CellRecord* cells = cl_records_host_;
+  bool short_buffer = false;
+  for (size_t j = 0; j < selected.size(); ++j) {
     const uint32_t k = selected[j];
-    const Member& m = members_[k];
     const uint32_t count = cl_cells_host_[j];
-    const ClusterSelection sel = select_cluster(cells, count, m.n, p.linear_hash_resolution, p.angular_hash_resolution, p.weight_cap_percentile);
-    if (out != nullptr) estimate_from_moments(sel.moments, m.pivot, &out[k]);
-    if (n_cells != nullptr) n_cells[k] = count;
-    if (n_clusters != nullptr) n_clusters[k] = sel.clusters;
+    double top = 1e-3;  // beluga_ros/particle_cloud.hpp:197
+    for (uint32_t c = 0; c < count; ++c) top = cells[c].weight > top ? cells[c].weight : top;
+    if (n_bins != nullptr) n_bins[k] = count;
+    if (max_bin_weight != nullptr) max_bin_weight[k] = top;
+    if (bins != nullptr && bins[k] != nullptr) {
+      if (capacity[k] < count) {
+        short_buffer = true;
+      } else {
+        std::memcpy(bins[k], cells, count * sizeof(CellRecord));
+      }
+    }
     cells += count;
+  }
+  if (short_buffer) return fail(BB200_ERR_CAPACITY, "histogram bin buffer too small for some member (n_bins has the counts)");
+  return BB200_OK;
+}
+
+int Batch::ensure_samples(uint64_t draws) {
+  if (sm_table_host_ == nullptr) {
+    const size_t k = members_.size();
+    sample_header_ = (k * sizeof(unsigned long long) + sizeof(Pose2) - 1) / sizeof(Pose2);
+    BB_CHECK(dev_alloc(&sm_table_, k));
+    BB_CHECK(host_alloc(&sm_table_host_, k));  // marks the table as allocated
+  }
+  if (draws <= samples_capacity_) return BB200_OK;
+  cudaFree(samples_);
+  cudaFreeHost(samples_host_);
+  samples_ = samples_host_ = nullptr;
+  samples_capacity_ = 0;
+  const uint64_t want = std::min<uint64_t>(total_, std::max<uint64_t>(4096, 2 * draws));  // draws <= total_
+  BB_CHECK(realloc_staged(&samples_, &samples_host_, sample_header_ + want));
+  samples_capacity_ = want;
+  return BB200_OK;
+}
+
+int Batch::sample_states(const uint64_t* counts, uint32_t step, const uint8_t* present, double* const* states_out) {
+  error_.clear();
+  // Filter::sample_states's checks per member, all before anything reaches the device.
+  std::vector<uint32_t> drawn;  // selected members with something to draw, in member order
+  uint64_t draws = 0;
+  for (size_t k = 0; k < members_.size(); ++k) {
+    if (present != nullptr && present[k] == 0) continue;
+    const Member& m = members_[k];
+    const std::string who = "member " + std::to_string(k) + ": ";
+    if (m.n == 0) return fail(BB200_ERR_STATE, who + "no particles");
+    if (counts[k] > m.capacity) return fail(BB200_ERR_CAPACITY, who + "more samples than its max_particles");
+    if (counts[k] > 0 && states_out[k] == nullptr) return fail(BB200_ERR_INVALID_ARGUMENT, who + "states_out is null");
+    if (counts[k] == 0) continue;
+    drawn.push_back(static_cast<uint32_t>(k));
+    draws += counts[k];
+  }
+  if (drawn.empty()) return BB200_OK;
+  BB_CHECK(cudaSetDevice(device_));
+  if (const int st = ensure_samples(draws)) return st;  // every batch call ends synchronised: the pinned buffers are free
+
+  const uint32_t n_sel = static_cast<uint32_t>(drawn.size());
+  BatchSampleArgs a{};
+  a.n_members = n_sel;
+  uint64_t out_offset = 0;
+  for (uint32_t j = 0; j < n_sel; ++j) {
+    const uint32_t k = drawn[j];
+    const Member& m = members_[k];
+    BatchSampleMember& s = sm_table_host_[j];
+    s = BatchSampleMember{};
+    s.offset = m.offset;
+    s.n = m.n;
+    s.count = counts[k];
+    s.out_offset = out_offset;
+    s.seed = m.policy.params().seed;
+    s.total = m.cdf_total;
+    s.cur = m.cur;
+    s.ceil_log2_count = ceil_log2_count(m.capacity);
+    out_offset += s.count;
+    uint32_t ctas[kSampleLaunches];
+    batch_sample_ctas(s, s.total == 0, ctas);
+    for (int l = 0; l < kSampleLaunches; ++l) {
+      first_host_[static_cast<size_t>(l) * (n_sel + 1) + j] = a.ctas[l];  // the step's range buffers are free between calls
+      a.ctas[l] += ctas[l];
+    }
+  }
+  for (int l = 0; l < kSampleLaunches; ++l) first_host_[static_cast<size_t>(l) * (n_sel + 1) + n_sel] = a.ctas[l];
+  cudaStream_t stream = stream_;
+  BB_CHECK(cudaMemcpyAsync(sm_table_, sm_table_host_, n_sel * sizeof(BatchSampleMember), cudaMemcpyHostToDevice, stream));
+  BB_CHECK(cudaMemcpyAsync(first_, first_host_, kSampleLaunches * (n_sel + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+  a.members = sm_table_;
+  a.first = first_;
+  a.step = step;
+  a.states[0] = states_[0];
+  a.states[1] = states_[1];
+  a.weights = weights_;
+  a.cdf = cdf_;
+  a.scalars = scalars_;
+  a.tile_state = tile_state_;
+  a.partials = partials_;  // the step's moment rows are free between calls
+  a.totals = reinterpret_cast<unsigned long long*>(samples_);
+  a.out = samples_ + sample_header_;
+  launches_ += static_cast<uint64_t>(launch_batch_sample(a, stream));
+  BB_CHECK(cudaGetLastError());
+  BB_CHECK(cudaMemcpyAsync(samples_host_, samples_, (sample_header_ + draws) * sizeof(Pose2), cudaMemcpyDeviceToHost, stream));
+  BB_CHECK(cudaStreamSynchronize(stream));
+
+  const unsigned long long* totals = reinterpret_cast<const unsigned long long*>(samples_host_);
+  const Pose2* out = samples_host_ + sample_header_;
+  for (uint32_t j = 0; j < n_sel; ++j) {
+    const BatchSampleMember& s = sm_table_host_[j];
+    members_[drawn[j]].cdf_total = totals[j];  // a rebuilt CDF is current until the member's particles or weights change
+    std::memcpy(states_out[drawn[j]], out + s.out_offset, s.count * sizeof(Pose2));
   }
   return BB200_OK;
 }
@@ -571,6 +712,7 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   for (int l = 0; l < kBatchLaunches; ++l) first_host_[static_cast<size_t>(l) * (n_active + 1) + n_active] = a.ctas[l];
 
   cudaStream_t stream = stream_;
+  for (const uint32_t k : active) members_[k].cdf_total = 0;  // from here on the step may have rewritten their CDFs
   seq_ = seq_ == 0x7fffffff ? 1 : seq_ + 1;
   *ticket_host_ = 0;
   st = check(cudaMemcpyAsync(table_, table_host_, n_active * sizeof(BatchMember), cudaMemcpyHostToDevice, stream), "upload member table");
@@ -632,6 +774,8 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
       m.cur ^= 1;
       m.n = m.capacity;
       m.ancestors_n = m.n;
+    } else {
+      m.cdf_total = s.total;  // the step's scan, over the weights before normalisation
     }
     r.updated = 1;
     r.resampled = plan.resample;

@@ -58,6 +58,16 @@ class Batch {
   /// kernel launches and two host synchronisations whatever K and the cell counts are.  out[m], n_cells[m] and
   /// n_clusters[m] (either may be nullptr) are written for selected members only.
   int cluster_estimates(const bb200_cluster_param& p, const uint8_t* present, bb200_estimate* out, uint32_t* n_cells, uint32_t* n_clusters);
+  /// Filter::particle_histogram of every selected member: the device half of cluster_estimates with these resolutions (two
+  /// launches, two synchronisations).  n_bins[m] and max_bin_weight[m] (either may be nullptr) are written for selected
+  /// members; bins[m] (bins or bins[m] nullptr: counts only) receives member m's bins when capacity[m] holds them, and
+  /// BB200_ERR_CAPACITY is returned when some selected member's buffer does not.
+  int particle_histograms(double linear, double angular, const uint8_t* present, bb200_cluster_cell* const* bins, const uint64_t* capacity,
+                          uint64_t* n_bins, double* max_bin_weight);
+  /// Filter::sample_states(counts[m], step, states_out[m]) for every selected member with counts[m] > 0, one launch when
+  /// every such member's CDF is current and four when some CDF has to be rebuilt, and one host synchronisation.  No particle
+  /// set changes.
+  int sample_states(const uint64_t* counts, uint32_t step, const uint8_t* present, double* const* states_out);
   /// Amcl::update for every member whose present[m] is non-zero (present == nullptr: all of them).  Atomic for the whole
   /// batch: when the device half fails, every member's host state is rolled back.
   int update(const double* control_poses, const double* const* points_xy, const uint64_t* n_points, const uint8_t* present,
@@ -75,6 +85,10 @@ class Batch {
     uint64_t table_offset{0};  // its hash table in the cluster scratch
     uint32_t table_slots{0};   // a power of two >= 2 * capacity
     int map{-1};               // id of the map it reads (-1: none)
+    // Total of the CDF in its cdf_ slice while that CDF is the one a standalone filter would sample from (Filter's
+    // cdf_valid_): set by a step that normalised and by a rebuild in sample_states; 0 (stale) after a resampling step,
+    // an initialisation or a failed step.
+    unsigned long long cdf_total{0};
   };
   struct MapEntry {
     DeviceMap map;
@@ -94,6 +108,13 @@ class Batch {
   int ensure_map_table();
   int ensure_cluster_scratch();
   int ensure_cluster_records(uint64_t cells);
+  /// The members whose present[m] is non-zero (present == nullptr: all of them), in member order; BB200_ERR_STATE when one
+  /// of them has no particles.
+  int select_members(const uint8_t* present, std::vector<uint32_t>* selected);
+  /// Clusterizer::cell_records of every member in `selected` (non-empty): their records back to back in cl_records_host_,
+  /// member selected[j]'s count in cl_cells_host_[j].  Two launches and two host synchronisations.
+  int cell_records(double linear, double angular, const std::vector<uint32_t>& selected);
+  int ensure_samples(uint64_t draws);
 
   std::vector<Member> members_;
   int device_{0};
@@ -148,6 +169,15 @@ class Batch {
   uint32_t* cl_cells_host_{nullptr};            // pinned
   CellRecord* cl_records_host_{nullptr};        // pinned, written by the compaction kernel
   uint64_t cl_records_host_capacity_{0};
+
+  // Pose-sample scratch (allocated on first use): the member table, and the draws after a header of one CDF total per
+  // member (sample_header_ poses' worth), so that one copy brings both back.
+  BatchSampleMember* sm_table_{nullptr};       // device
+  BatchSampleMember* sm_table_host_{nullptr};  // pinned
+  uint64_t sample_header_{0};
+  Pose2* samples_{nullptr};                    // device
+  Pose2* samples_host_{nullptr};               // pinned
+  uint64_t samples_capacity_{0};               // draws
 };
 
 }  // namespace bb200

@@ -886,6 +886,15 @@ int bb200_amcl_batch_cluster_estimates(bb200_amcl_batch* b, const bb200_cluster_
   BB_REQUIRE(b && p && out);
   return guarded(b->impl, [&] { return b->impl.cluster_estimates(*p, present, out, n_cells, n_clusters); });
 }
+int bb200_amcl_batch_particle_histograms(bb200_amcl_batch* b, double linear_resolution, double angular_resolution, const uint8_t* present,
+                                         bb200_cluster_cell* const* bins, const uint64_t* capacity, uint64_t* n_bins, double* max_bin_weight) {
+  BB_REQUIRE(b);
+  return guarded(b->impl, [&] { return b->impl.particle_histograms(linear_resolution, angular_resolution, present, bins, capacity, n_bins, max_bin_weight); });
+}
+int bb200_amcl_batch_sample_states(bb200_amcl_batch* b, const uint64_t* counts, uint32_t step, const uint8_t* present, double* const* states_out) {
+  BB_REQUIRE(b && counts && states_out);
+  return guarded(b->impl, [&] { return b->impl.sample_states(counts, step, present, states_out); });
+}
 int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, const double* const* points_xy, const uint64_t* n_points,
                             const uint8_t* present, bb200_update_result* out) {
   BB_REQUIRE(b && control_poses && points_xy && n_points && out);

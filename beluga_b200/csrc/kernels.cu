@@ -1277,15 +1277,22 @@ __global__ void __launch_bounds__(kMixThreads)
   beam_mixture_block(states, weights, n, slot_base, slot_count, perm, grid, params, points, n_points, hits, hit_stride, scalars, blockIdx.x);
 }
 
-__global__ void __launch_bounds__(512) max_weight_kernel(const double* __restrict__ weights, uint64_t n, Scalars* scalars) {
-  __shared__ unsigned long long s_red[512 / kWarp];
+constexpr int kMaxThreads = 512;
+
+/// Block `block` of `grid` of max_weight_kernel: the largest positive finite weight into scalars->wmax_bits.
+__device__ __forceinline__ void max_weight_block(const double* __restrict__ weights, uint64_t n, Scalars* scalars, uint32_t block, uint32_t grid) {
+  __shared__ unsigned long long s_red[kMaxThreads / kWarp];
   unsigned long long m = 0;
-  for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * 512 + threadIdx.x; i < n; i += static_cast<uint64_t>(gridDim.x) * 512) {
+  for (uint64_t i = static_cast<uint64_t>(block) * kMaxThreads + threadIdx.x; i < n; i += static_cast<uint64_t>(grid) * kMaxThreads) {
     const unsigned long long b = weight_order_bits(weights[i]);
     m = b > m ? b : m;
   }
-  m = block_max_u64<512>(m, s_red);
+  m = block_max_u64<kMaxThreads>(m, s_red);
   if (threadIdx.x == 0 && m != 0) atomicMax(&scalars->wmax_bits, m);
+}
+
+__global__ void __launch_bounds__(kMaxThreads) max_weight_kernel(const double* __restrict__ weights, uint64_t n, Scalars* scalars) {
+  max_weight_block(weights, n, scalars, blockIdx.x, gridDim.x);
 }
 
 // ---- fixed-point CDF ------------------------------------------------------------------------------
@@ -1974,7 +1981,8 @@ __global__ void __launch_bounds__(256) fill_kernel(double* __restrict__ out, uin
 
 /// The member owning CTA `cta` of `launch` (the last one whose range starts at or before it: members without CTAs in this
 /// launch have empty ranges), the CTA's index inside that range and the range's length.
-__device__ __forceinline__ uint32_t batch_member_of(const BatchStepArgs& s, int launch, uint32_t cta, uint32_t& local, uint32_t& count) {
+template <class Args>
+__device__ __forceinline__ uint32_t batch_member_of(const Args& s, int launch, uint32_t cta, uint32_t& local, uint32_t& count) {
   const uint32_t* first = s.first + static_cast<size_t>(launch) * (s.n_members + 1);
   uint32_t lo = 0, hi = s.n_members;  // first[lo] <= cta < first[hi]
   while (hi - lo > 1) {
@@ -2033,7 +2041,8 @@ __device__ __forceinline__ void batch_recovery_map(const BatchStepArgs& s, const
 }
 
 /// The per-step scalars of every member (what begin_fused_step_kernel resets for one filter) and the scan state.
-__global__ void __launch_bounds__(256) batch_begin_kernel(BatchStepArgs s) {
+template <class Args>
+__device__ __forceinline__ void batch_reset_grid(const Args& s, uint32_t scan_tiles) {
   const uint32_t stride = gridDim.x * 256;
   for (uint32_t t = blockIdx.x * 256 + threadIdx.x; t < s.n_members; t += stride) {
     Scalars* sc = s.scalars + t;
@@ -2044,8 +2053,10 @@ __global__ void __launch_bounds__(256) batch_begin_kernel(BatchStepArgs s) {
     sc->valid = 0;
     sc->blocks_done = 0;
   }
-  for (uint32_t t = blockIdx.x * 256 + threadIdx.x; t < s.ctas[kBatchScan]; t += stride) s.tile_state[t] = 0;
+  for (uint32_t t = blockIdx.x * 256 + threadIdx.x; t < scan_tiles; t += stride) s.tile_state[t] = 0;
 }
+
+__global__ void __launch_bounds__(256) batch_begin_kernel(BatchStepArgs s) { batch_reset_grid(s, s.ctas[kBatchScan]); }
 
 /// propagate_kernel's per-particle body (counter RNG keyed by the member's seed, local index and step).
 __global__ void __launch_bounds__(kPrThreads) batch_propagate_kernel(BatchStepArgs s) {
@@ -2206,6 +2217,49 @@ __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs 
   } else {
     resample_block(a, scalars, partials, local, count, tail);
   }
+}
+
+// ---- pose samples of a batch (Filter::sample_states per member) --------------------------------------------------
+// A member whose CDF is stale gets the CDF Filter::build_cdf would build: scalars and scan state reset, the largest weight
+// (max_weight_kernel's block body), then the quantise + scan with the exponent derived from it exactly as prepare_cdf
+// derives it (a degenerate weight set gets the uniform CDF).
+
+__global__ void __launch_bounds__(256) batch_sample_reset_kernel(BatchSampleArgs s) { batch_reset_grid(s, s.ctas[kSampleScan]); }
+
+__global__ void __launch_bounds__(kMaxThreads) batch_sample_max_kernel(BatchSampleArgs s) {
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kSampleMax, blockIdx.x, local, count);
+  const BatchSampleMember& m = s.members[k];
+  max_weight_block(s.weights + m.offset, m.n, s.scalars + k, local, count);
+}
+
+__global__ void __launch_bounds__(kQsThreads) batch_sample_scan_kernel(BatchSampleArgs s) {
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kSampleScan, blockIdx.x, local, count);
+  const BatchSampleMember& m = s.members[k];
+  quantize_scan_tile(s.weights + m.offset, m.n, s.cdf + m.offset, s.scalars + k, s.tile_state + (blockIdx.x - local), local, 1,
+                     m.ceil_log2_count);
+}
+
+/// resample_kernel's multinomial draws of `count` slots without weights, ancestors or tail, into the member's run of `out`.
+__global__ void __launch_bounds__(kRsThreads) batch_sample_kernel(BatchSampleArgs s) {
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kSampleDraw, blockIdx.x, local, count);
+  const BatchSampleMember& m = s.members[k];
+  Scalars* scalars = s.scalars + k;
+  ResampleArgs a{};
+  a.states_in = (m.cur != 0 ? s.states[1] : s.states[0]) + m.offset;
+  a.cdf = s.cdf + m.offset;
+  a.n_in = m.n;
+  a.states_out = s.out + m.out_offset;
+  a.slot_count = m.count;
+  a.total_slots = m.count;
+  a.global_total = m.total;  // 0: the rebuilt CDF's, in scalars->total
+  a.scheme = BB200_RESAMPLE_MULTINOMIAL;
+  a.seed = m.seed;
+  a.step = s.step;
+  resample_block(a, scalars, s.partials + static_cast<size_t>(blockIdx.x - local) * kMomentCount, local, count, a.tail);
+  if (local == 0 && threadIdx.x == 0) s.totals[k] = m.total != 0 ? m.total : scalars->total;
 }
 
 // ---- shard exchange ------------------------------------------------------------------------------------
@@ -2587,6 +2641,25 @@ int launch_batch_step_from(const BatchStepArgs& s, cudaStream_t stream) {
 
 int launch_batch_step(const BatchStepArgs& s, cudaStream_t stream) {
   return s.maps != nullptr ? launch_batch_step_from<true>(s, stream) : launch_batch_step_from<false>(s, stream);
+}
+
+void batch_sample_ctas(const BatchSampleMember& m, bool rebuilt, uint32_t out[kSampleLaunches]) {
+  out[kSampleMax] = rebuilt ? static_cast<uint32_t>(std::min<uint64_t>((m.n + kMaxThreads - 1) / kMaxThreads, kStreamMaxBlocks)) : 0u;  // launch_max_weight's grid
+  out[kSampleScan] = rebuilt ? scan_tile_count(m.n) : 0u;
+  out[kSampleDraw] = resample_block_count(m.count);
+}
+
+int launch_batch_sample(const BatchSampleArgs& s, cudaStream_t stream) {
+  int launches = 1;
+  if (s.ctas[kSampleScan] > 0) {
+    const uint32_t reset = std::max(s.n_members, s.ctas[kSampleScan]);
+    batch_sample_reset_kernel<<<std::max(1u, std::min((reset + 255u) / 256u, kSmCount * 4u)), 256, 0, stream>>>(s);
+    batch_sample_max_kernel<<<s.ctas[kSampleMax], kMaxThreads, 0, stream>>>(s);
+    batch_sample_scan_kernel<<<s.ctas[kSampleScan], kQsThreads, 0, stream>>>(s);
+    launches += 3;
+  }
+  batch_sample_kernel<<<s.ctas[kSampleDraw], kRsThreads, 0, stream>>>(s);
+  return launches;
 }
 
 uint32_t launch_resample(const ResampleArgs& args, Scalars* scalars, double* moment_partials, cudaStream_t stream) {

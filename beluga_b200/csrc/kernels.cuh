@@ -497,6 +497,43 @@ uint32_t batch_scan_tiles(uint64_t n);
 /// CTAs of a member in each row of a batch step's ranges, for a member that takes reweight form `form`.
 void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunches]);
 
+/// One member of a batch's pose-sample draw (Filter::sample_states per member).
+struct BatchSampleMember {
+  uint64_t offset;           // first particle of the member in the batch buffers (also its CDF slice)
+  uint64_t n;                // particles: the length of its CDF
+  uint64_t count;            // states to draw (> 0)
+  uint64_t out_offset;       // first of its draws in BatchSampleArgs::out
+  uint64_t seed;
+  unsigned long long total;  // total of the member's current CDF; 0: the CDF is rebuilt in this call
+  int cur;                   // state buffer holding the member's particles
+  int ceil_log2_count;       // of max_particles: the fixed-point exponent's headroom
+};
+
+/// Rows of a sample call's CTA ranges: the rebuild of the stale members' CDFs (largest weight, quantise + scan) and the draw.
+enum BatchSampleLaunch : int { kSampleMax = 0, kSampleScan = 1, kSampleDraw = 2, kSampleLaunches = 3 };
+
+struct BatchSampleArgs {
+  const BatchSampleMember* members;  // device
+  const uint32_t* first;             // device: kSampleLaunches x (n_members + 1) CTA prefixes
+  uint32_t n_members;
+  uint32_t ctas[kSampleLaunches];
+  uint32_t step;                     // counter-RNG step of the draws
+  const Pose2* states[2];
+  const double* weights;
+  unsigned long long* cdf;
+  Scalars* scalars;                  // one per member of the table (the rebuild's)
+  unsigned long long* tile_state;    // one word per scan tile of the rebuild
+  double* partials;                  // kMomentCount per draw CTA: scratch for resample_block's moment rows, never read
+  Pose2* out;                        // the draws of every member, back to back
+  unsigned long long* totals;        // one per member of the table: the total of the CDF its draws used
+};
+/// The multinomial draws of Filter::sample_states for every member of the table, from its current CDF, or from one rebuilt
+/// first as Filter::build_cdf would (members with total == 0).  Returns the number of launches: 1 when no member is
+/// rebuilt, 4 otherwise (reset, largest weight, quantise + scan, draw), whatever the members and their counts are.
+int launch_batch_sample(const BatchSampleArgs& args, cudaStream_t stream);
+/// CTAs of a member in each row of a sample call's ranges (rebuilt: whether its CDF is rebuilt in the call).
+void batch_sample_ctas(const BatchSampleMember& m, bool rebuilt, uint32_t out[kSampleLaunches]);
+
 /// Per-block raw weighted moments of (states, weights).
 uint32_t moments_block_count(uint64_t n);
 void launch_moments(const Pose2* states, const double* weights, uint64_t n, double pivot_x, double pivot_y, double* moment_partials,

@@ -547,7 +547,10 @@ int bb200_amcl_leave_shards(bb200_amcl* a);
  *
  * The fleet loop of a beluga_ros node per member is bb200_amcl_batch_update, then
  * bb200_amcl_batch_cluster_estimates for the members that updated: the estimate every node publishes, for all of them
- * with two kernel launches and two host synchronisations, whatever K and the members' cell counts are.
+ * with two kernel launches and two host synchronisations, whatever K and the members' cell counts are.  On the publish
+ * timer a node also publishes its particle cloud, as markers and as a pose array: bb200_amcl_batch_particle_histograms
+ * (2 launches, 2 synchronisations) and bb200_amcl_batch_sample_states (1 launch, or 4 when some member's CDF has to
+ * be rebuilt; 1 synchronisation) do that for every selected member at once.
  * ------------------------------------------------------------------------------------------- */
 typedef struct bb200_amcl_batch bb200_amcl_batch;
 /* params[m] and motions[m] configure member m (params[m].device must be the same for all). */
@@ -601,6 +604,27 @@ int bb200_amcl_batch_cluster_estimate(bb200_amcl_batch* b, int member, const bb2
  * bad parameters and with BB200_ERR_STATE when a selected member holds no particles. */
 int bb200_amcl_batch_cluster_estimates(bb200_amcl_batch* b, const bb200_cluster_param* p, const uint8_t* present,
                                        bb200_estimate* out, uint32_t* n_cells, uint32_t* n_clusters);
+/* bb200_filter_particle_histogram for every member m with present[m] != 0 (present NULL: all members), with two kernel
+ * launches and two host synchronisations whatever K and the bin counts are.  bins[m] receives member m's bins in
+ * first-occurrence order when capacity[m] holds them; bins or bins[m] may be NULL to query the counts only (capacity may
+ * then be NULL too).  n_bins[m] and max_bin_weight[m] (max(1e-3, heaviest bin)) are written for selected members; either
+ * array may be NULL.  Entries of members not selected are not written.  Every selected member's output is bit-identical
+ * to a standalone filter's bb200_filter_particle_histogram over the same particles.  BB200_ERR_CAPACITY when some
+ * selected member's buffer is too small (n_bins is still filled, and the members whose buffers fit get their bins).
+ * Fails before any launch with BB200_ERR_INVALID_ARGUMENT for non-positive resolutions or a null handle, or bins without
+ * capacity, and with BB200_ERR_STATE when a selected member holds no particles. */
+int bb200_amcl_batch_particle_histograms(bb200_amcl_batch* b, double linear_resolution, double angular_resolution, const uint8_t* present,
+                                         bb200_cluster_cell* const* bins, const uint64_t* capacity, uint64_t* n_bins, double* max_bin_weight);
+/* bb200_filter_sample_states(counts[m], step) for every member m with present[m] != 0 (present NULL: all members):
+ * counts[m] states drawn by weight into states_out[m] (counts[m] x {cos, sin, x, y}), bit-identical to what a standalone
+ * filter draws; no member's particle set is modified.  A member samples from the CDF a standalone filter would use: the
+ * one its last step built when that step normalised instead of resampling, otherwise one rebuilt from its weights in
+ * this call (and kept for later calls until its particles or weights change).  One kernel launch when no CDF has to be
+ * rebuilt, four otherwise, and one host synchronisation, whatever K and the counts are.  counts[m] == 0 draws nothing.
+ * Fails before any launch with BB200_ERR_STATE when a selected member holds no particles, BB200_ERR_CAPACITY when
+ * counts[m] exceeds its max_particles, and BB200_ERR_INVALID_ARGUMENT for a null handle, counts or states_out, or a null
+ * states_out[m] with counts[m] > 0. */
+int bb200_amcl_batch_sample_states(bb200_amcl_batch* b, const uint64_t* counts, uint32_t step, const uint8_t* present, double* const* states_out);
 /* Amcl::update for every member m with present[m] != 0 (present NULL: all members).  control_poses holds K poses of 4
  * doubles, points_xy[m] member m's n_points[m] (x, y) pairs (NULL when n_points[m] == 0), out[m] its result.  An absent
  * member is left untouched -- no policy is evaluated -- and gets out[m].updated = 0.  Present members go through their
@@ -608,8 +632,8 @@ int bb200_amcl_batch_cluster_estimates(bb200_amcl_batch* b, const bb200_cluster_
  * every member's host state is as if it had not been made. */
 int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, const double* const* points_xy, const uint64_t* n_points,
                             const uint8_t* present, bb200_update_result* out);
-/* Kernel launches issued by this batch so far (steps, initialisations, cluster estimates and the beam model's map
- * uploads). */
+/* Kernel launches issued by this batch so far (steps, initialisations, cluster estimates, particle-cloud histograms and
+ * pose samples, and the beam model's map uploads). */
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b);
 
 /* The two host halves of bb200_amcl_update for callers that drive the filter themselves. */

@@ -349,6 +349,60 @@ class AmclBatch {
     return out;
   }
 
+  /// One member's particle-cloud histogram: its bins in first-occurrence order and max(1e-3, heaviest bin).
+  using histogram_type = std::pair<std::vector<bb200_cluster_cell>, double>;
+
+  /// The particle-cloud histogram (bb200_filter_particle_histogram) of every member whose present[m] is true (present ==
+  /// nullptr: all of them) in one call; std::nullopt for members not selected.  Each member's buffer holds max_particles
+  /// bins (a member never has more bins than particles), so one device pass fills them all.
+  [[nodiscard]] auto particle_histograms(const std::vector<bool>* present = nullptr, double linear_resolution = 1e-3,
+                                         double angular_resolution = 1e-3) const -> std::vector<std::optional<histogram_type>> {
+    const std::vector<std::uint8_t> mask = presence_mask(present);
+    const std::size_t k = size();
+    std::vector<std::vector<bb200_cluster_cell>> bins(k);
+    std::vector<bb200_cluster_cell*> ptrs(k, nullptr);
+    std::vector<std::uint64_t> capacity(k, 0), n_bins(k, 0);
+    std::vector<double> top(k, 0.0);
+    for (std::size_t m = 0; m < k; ++m) {
+      if (present != nullptr && !(*present)[m]) continue;
+      bins[m].resize(sizes_[m]);
+      ptrs[m] = bins[m].data();
+      capacity[m] = sizes_[m];
+    }
+    check(bb200_amcl_batch_particle_histograms(handle_, linear_resolution, angular_resolution, present != nullptr ? mask.data() : nullptr, ptrs.data(),
+                                               capacity.data(), n_bins.data(), top.data()));
+    std::vector<std::optional<histogram_type>> out(k);
+    for (std::size_t m = 0; m < k; ++m) {
+      if (ptrs[m] == nullptr) continue;
+      bins[m].resize(n_bins[m]);
+      out[m] = std::make_pair(std::move(bins[m]), top[m]);
+    }
+    return out;
+  }
+
+  /// counts[m] states {cos, sin, x, y} drawn by weight from every member whose present[m] is true (present == nullptr: all
+  /// of them), the multinomial counter-RNG draws of `step` (bb200_filter_sample_states); std::nullopt for members not
+  /// selected.  No particle set changes.
+  [[nodiscard]] auto sample_states(const std::vector<std::size_t>& counts, uint32_t step, const std::vector<bool>* present = nullptr) const
+      -> std::vector<std::optional<std::vector<double>>> {
+    const std::vector<std::uint8_t> mask = presence_mask(present);
+    const std::size_t k = size();
+    if (counts.size() != k) throw Error(BB200_ERR_INVALID_ARGUMENT, "one sample count per member");
+    std::vector<std::vector<double>> raw(k);
+    std::vector<double*> ptrs(k, nullptr);
+    std::vector<std::uint64_t> n(k, 0);
+    for (std::size_t m = 0; m < k; ++m) {
+      n[m] = counts[m];
+      raw[m].resize(4 * counts[m]);
+      ptrs[m] = raw[m].empty() ? nullptr : raw[m].data();
+    }
+    check(bb200_amcl_batch_sample_states(handle_, n.data(), step, present != nullptr ? mask.data() : nullptr, ptrs.data()));
+    std::vector<std::optional<std::vector<double>>> out(k);
+    for (std::size_t m = 0; m < k; ++m)
+      if (present == nullptr || (*present)[m]) out[m] = std::move(raw[m]);
+    return out;
+  }
+
   [[nodiscard]] bb200_amcl_batch* handle() const { return handle_; }
 
  private:
@@ -358,6 +412,12 @@ class AmclBatch {
   }
   void check(int status) const {
     if (status != BB200_OK) throw Error(status, bb200_amcl_batch_last_error(handle_));
+  }
+  std::vector<std::uint8_t> presence_mask(const std::vector<bool>* present) const {
+    if (present != nullptr && present->size() != size()) throw Error(BB200_ERR_INVALID_ARGUMENT, "one presence flag per member");
+    std::vector<std::uint8_t> mask(present != nullptr ? size() : 0);
+    for (std::size_t m = 0; m < mask.size(); ++m) mask[m] = (*present)[m] ? 1 : 0;
+    return mask;
   }
 
   bb200_amcl_batch* handle_{nullptr};

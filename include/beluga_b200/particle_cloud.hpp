@@ -6,10 +6,12 @@
 //   beluga_ros::assign_likelihood_field(field, origin, OccupancyGrid)      -> beluga_b200::likelihood_field_cells(amcl)
 //
 // The histogram behind the markers runs on the device (bb200_filter_particle_histogram): a publish of a million
-// particles moves a few thousand bins, not 40 MB of states.
+// particles moves a few thousand bins, not 40 MB of states.  The AmclBatch overloads publish every selected member of a
+// batch with one histogram call and one sample call (bb200_amcl_batch_particle_histograms / _sample_states).
 #pragma once
 
 #include <cstdint>
+#include <optional>
 #include <vector>
 
 #include "../beluga_b200.h"
@@ -57,6 +59,41 @@ std::vector<Pose2d> sample_poses(AmclT& amcl, std::size_t size, uint32_t draw = 
   detail_io::check_filter(f, bb200_filter_sample_states(f, size, 0xFFFFFFFFu - draw, raw.data()));
   std::vector<Pose2d> out(size);
   for (std::size_t i = 0; i < size; ++i) out[i] = Pose2d{raw[4 * i + 2], raw[4 * i + 3], raw[4 * i], raw[4 * i + 1]};
+  return out;
+}
+
+/// The markers of every member of a batch whose present[m] is true (present == nullptr: all of them), from one batched
+/// histogram call; std::nullopt for members not selected.
+inline std::vector<std::optional<ParticleCloudMarkers>> particle_cloud_markers(AmclBatch& batch, const std::vector<bool>* present = nullptr,
+                                                                                double linear_resolution = 1e-3, double angular_resolution = 1e-3) {
+  const auto histograms = batch.particle_histograms(present, linear_resolution, angular_resolution);
+  std::vector<std::optional<ParticleCloudMarkers>> out(histograms.size());
+  for (std::size_t m = 0; m < histograms.size(); ++m) {
+    if (!histograms[m]) continue;
+    const std::vector<bb200_cluster_cell>& bins = histograms[m]->first;
+    ParticleCloudMarkers markers;
+    markers.bodies.resize(2 * bins.size());
+    markers.heads.resize(3 * bins.size());
+    const int st = bb200_particle_cloud_markers(bins.data(), bins.size(), markers.bodies.data(), markers.heads.data(), &markers.body_scale_x);
+    if (st != BB200_OK) throw Error(st, "bb200_particle_cloud_markers");
+    out[m] = std::move(markers);
+  }
+  return out;
+}
+
+/// `size` poses drawn by weight from every member of a batch whose present[m] is true (present == nullptr: all of them),
+/// with the step convention of sample_poses above; std::nullopt for members not selected.
+inline std::vector<std::optional<std::vector<Pose2d>>> sample_poses(AmclBatch& batch, std::size_t size, uint32_t draw = 0,
+                                                                     const std::vector<bool>* present = nullptr) {
+  const auto raw = batch.sample_states(std::vector<std::size_t>(batch.size(), size), 0xFFFFFFFFu - draw, present);
+  std::vector<std::optional<std::vector<Pose2d>>> out(raw.size());
+  for (std::size_t m = 0; m < raw.size(); ++m) {
+    if (!raw[m]) continue;
+    const std::vector<double>& r = *raw[m];
+    std::vector<Pose2d> poses(size);
+    for (std::size_t i = 0; i < size; ++i) poses[i] = Pose2d{r[4 * i + 2], r[4 * i + 3], r[4 * i], r[4 * i + 1]};
+    out[m] = std::move(poses);
+  }
   return out;
 }
 

@@ -5,6 +5,8 @@ AmclBatch against K standalone Amcl stepped one after another.  `batch_cluster`:
 update + cluster estimate, the estimate taken for all members in one call and member by member.  `batch_beam`: AmclBatch with the
 beam model (60 and 720 points per member) against the same members stepped as standalone Amcl.  `batch_maps`: one AmclBatch whose
 members read 1, 4 or 16 likelihood-field maps against one single-map batch per map, and a step mixing likelihood-field and beam members.
+`batch_cloud`: the `batch` members' particle-cloud publish round (histograms and pose samples) in one batched call each against
+K standalone filters publishing in turn.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import json
@@ -370,6 +372,88 @@ def run_batch_cluster():
     return res
 
 
+def run_batch_cloud():
+    """The `batch` workload (K in {1, 16, 64, 256} members x 2000 particles x 100 points, 2000^2 map, systematic resampling)
+    and K standalone Amcl fed the same inputs, timed as one particle-cloud publish round after each update: the batched form
+    is one particle_histograms call and one sample_states call of 2000 poses per member; the per-node form is each standalone
+    filter's particle_histogram and sample_states in turn.  The two forms alternate which goes first from round to round,
+    their outputs are compared byte for byte, and the host marker geometry (bb200_particle_cloud_markers over every member's
+    bins) is timed on its own."""
+    import ctypes as C
+
+    from beluga_b200 import _capi
+
+    lib = _capi.load()
+    res = {}
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=100, steps=100)
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    steps, warmup, n = 20, 3, 2000
+    device = device_record()
+    for k in (1, 16, 64, 256):
+        params = [bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m) for m in range(k)]
+        motions = [bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)]
+        batch = bb.AmclBatch(motions, params)
+        batch.set_likelihood_field_map(lfm, grid)
+        nodes = []
+        for m in range(k):
+            batch.initialize(m, sc.initial_mean, sc.initial_cov)
+            a = bb.Amcl(motions[m], params[m])
+            a.update_map(bb.SENSOR_LIKELIHOOD_FIELD, lfm, grid)
+            a.initialize(sc.initial_mean, sc.initial_cov)
+            nodes.append(a)
+        batched_ms, node_ms, markers_ms, batched_launches = [], [], [], []
+        for t in range(warmup + steps):
+            pose = bb.se2(*sc.poses[t])
+            assert all(x.updated for x in batch.update([pose] * k, [sc.scans[t]] * k))
+            for a in nodes:
+                a.update(pose, sc.scans[t])
+            step = 0xFFFFFFFF - t
+
+            def batched():
+                before = batch.launch_count()
+                t0 = time.perf_counter()
+                hists = batch.particle_histograms()
+                poses = batch.sample_states(n, step)
+                t1 = time.perf_counter()
+                batched_launches.append(batch.launch_count() - before)
+                return (t1 - t0) * 1e3, hists, poses
+
+            def per_node():
+                t0 = time.perf_counter()
+                out = [(a.filter.particle_histogram(), a.filter.sample_states(n, step)) for a in nodes]
+                return (time.perf_counter() - t0) * 1e3, out
+
+            if t % 2 == 0:
+                b_ms, hists, poses = batched()
+                p_ms, each = per_node()
+            else:
+                p_ms, each = per_node()
+                b_ms, hists, poses = batched()
+            for m in range(k):
+                (rep, w, _, _, top), s = each[m]
+                assert hists[m][0]["rep"].tobytes() == rep.tobytes() and hists[m][0]["weight"].tobytes() == w.tobytes()
+                assert hists[m][1] == top and poses[m].tobytes() == s.tobytes()
+            t0 = time.perf_counter()
+            for bins, _ in hists:
+                cells = bins.ctypes.data_as(C.POINTER(_capi.ClusterCell))
+                bodies, heads = (_capi.MarkerVertex * (2 * len(bins)))(), (_capi.MarkerVertex * (3 * len(bins)))()
+                scale = C.c_double(0.0)
+                assert lib.bb200_particle_cloud_markers(cells, len(bins), bodies, heads, C.byref(scale)) == 0
+            t1 = time.perf_counter()
+            if t >= warmup:
+                batched_ms.append(b_ms)
+                node_ms.append(p_ms)
+                markers_ms.append((t1 - t0) * 1e3)
+        res[f"batch_cloud_{k}_x_{n}_x_100_lfm_2000"] = {
+            "members": k, "particles": n, "points": 100, "samples_per_member": n, "steps": steps,
+            "batched_publish_ms": float(np.median(batched_ms)), "batched_publish_ms_min_max": [float(np.min(batched_ms)), float(np.max(batched_ms))],
+            "per_node_publish_ms": float(np.median(node_ms)), "per_node_publish_ms_min_max": [float(np.min(node_ms)), float(np.max(node_ms))],
+            "host_marker_geometry_ms": float(np.median(markers_ms)), "launches_per_batched_round": int(max(batched_launches)),
+            "ms_per_step_e2e": float(np.median(batched_ms)), "kernels_ms": {}, "device": device}
+    return res
+
+
 def main():
     out = {}
     which = sys.argv[1:] or ["c1", "c3", "c4"]
@@ -427,6 +511,8 @@ def main():
         out.update(run_batch())
     if "batch_cluster" in which:
         out.update(run_batch_cluster())
+    if "batch_cloud" in which:
+        out.update(run_batch_cloud())
     if "batch_beam" in which:
         out.update(run_batch_beam())
     if "batch_maps" in which:

@@ -768,8 +768,7 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     const bb200_step_plan& plan = plans[k];
     bb200_update_result& r = out[k];
     estimate_from_moments(s.moments, m.pivot, &r.estimate);
-    m.pivot[0] = r.estimate.mean[2];
-    m.pivot[1] = r.estimate.mean[3];
+    pivot_to_estimate(r.estimate, m.pivot);
     if (plan.resample) {
       m.cur ^= 1;
       m.n = m.capacity;

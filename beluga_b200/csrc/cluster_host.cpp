@@ -147,4 +147,10 @@ void estimate_from_moments(const double m[9], const double pivot[2], bb200_estim
   }
 }
 
+void pivot_to_estimate(const bb200_estimate& e, double pivot[2]) {
+  if (!std::isfinite(e.mean[2]) || !std::isfinite(e.mean[3])) return;
+  pivot[0] = e.mean[2];
+  pivot[1] = e.mean[3];
+}
+
 }  // namespace bb200

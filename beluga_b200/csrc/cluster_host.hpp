@@ -40,4 +40,8 @@ ClusterSelection select_cluster(const HostCell* cells, std::size_t n_cells, std:
 /// kernels.cuh): what every estimate ends with, of the whole set or of the selected cluster.
 void estimate_from_moments(const double m[9], const double pivot[2], bb200_estimate* out);
 
+/// Moves the moments' pivot to the estimate's position -- unless that is not finite (a normalising step over weights that
+/// sum to 0, NaN or inf), which would make every later estimate NaN.
+void pivot_to_estimate(const bb200_estimate& e, double pivot[2]);
+
 }  // namespace bb200

@@ -773,8 +773,7 @@ int Filter::step_end(bb200_estimate* est, double* weight_sum, uint64_t* new_size
   bb200_estimate local{};
   if (est == nullptr) est = &local;
   estimate_from_moments(moments, pivot_, est);
-  pivot_[0] = est->mean[2];
-  pivot_[1] = est->mean[3];
+  pivot_to_estimate(*est, pivot_);
   cloud_ = *est;
   cloud_known_ = step_.resampled;  // unit weights: the estimate describes the raw cloud, the next step can predict its pose bins
   return BB200_OK;
@@ -1090,8 +1089,7 @@ int Filter::estimate(bb200_estimate* out) {
   const int st = moments(pivot_, m);
   if (st != BB200_OK) return st;
   estimate_from_moments(m, pivot_, out);
-  pivot_[0] = out->mean[2];
-  pivot_[1] = out->mean[3];
+  pivot_to_estimate(*out, pivot_);
   return BB200_OK;
 }
 

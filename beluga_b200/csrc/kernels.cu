@@ -95,9 +95,13 @@ __device__ __forceinline__ unsigned long long block_max_u64(unsigned long long v
   return m;
 }
 
+/// The one rule for which weights can be selected: 0 < w <= DBL_MAX.  Zero, negative, NaN and +-inf weights never enter
+/// the largest weight and quantise to 0 (a +inf weight would otherwise saturate to 2^64 - 1 and wrap the CDF).
+__device__ __forceinline__ bool weight_selectable(double w) { return w > 0.0 && w <= DBL_MAX; }
+
 /// Positive finite weights order like their bit patterns; anything else counts as 0.
 __device__ __forceinline__ unsigned long long weight_order_bits(double w) {
-  return (w > 0.0 && w <= DBL_MAX) ? static_cast<unsigned long long>(__double_as_longlong(w)) : 0ull;
+  return weight_selectable(w) ? static_cast<unsigned long long>(__double_as_longlong(w)) : 0ull;
 }
 
 // ---- TMA 1-D bulk copy of the scan points into shared memory ------------------------------------
@@ -1308,7 +1312,7 @@ constexpr unsigned long long kFlagAggregate = 1ull << 62, kFlagPrefix = 2ull << 
 
 __device__ __forceinline__ void prepare_cdf_scalars(Scalars* s, double wmax, int ceil_log2_count) {
   int ex = 0;
-  const bool ok = wmax > 0.0 && wmax <= DBL_MAX;
+  const bool ok = weight_selectable(wmax);
   if (ok) (void)frexp(wmax, &ex);
   const int p = min(52, 62 - ceil_log2_count);
   s->exponent = p - ex;
@@ -1398,8 +1402,7 @@ __device__ __forceinline__ double pow2_double(int e) {  // |e| <= 1000
   return __longlong_as_double(static_cast<long long>(e + 1023) << 52);
 }
 __device__ __forceinline__ unsigned long long quantize_mul(double w, double f1, double f2) {
-  const double scaled = (w * f1) * f2;
-  return scaled > 0.0 ? __double2ull_rd(scaled) : 0ull;  // zero / negative / NaN weights are never selected
+  return weight_selectable(w) ? __double2ull_rd((w * f1) * f2) : 0ull;
 }
 
 /// derive_exponent: the fused step -- the exponent comes from scalars->wmax_bits here (no prepare_cdf launch; the
@@ -1414,7 +1417,7 @@ __device__ __forceinline__ void quantize_scan_tile(const double* __restrict__ we
   if (derive_exponent) {  // every thread derives the exponent itself: a broadcast load and a few integer operations
     const double wmax = __longlong_as_double(static_cast<long long>(scalars->wmax_bits));
     int ex = 0;
-    const bool ok = wmax > 0.0 && wmax <= DBL_MAX;
+    const bool ok = weight_selectable(wmax);
     if (ok) (void)frexp(wmax, &ex);
     exponent = min(52, 62 - ceil_log2_count) - ex;
     valid_flag = ok ? 1 : 0;

@@ -221,6 +221,7 @@ class Amcl {
       // reproducible for any summation order / rank count).
       cdf_ = fixed_point_cdf(weights_);
       const double factor = std::ldexp(static_cast<double>(cdf_.total), -cdf_.exponent);
+      if (!cdf_.valid) return factor;  // no weight can be selected: weights kept, resampling draws from the uniform CDF
       const std::int64_t n = static_cast<std::int64_t>(weights_.size());
 #pragma omp parallel for num_threads(params_.threads) schedule(static) if (params_.threads > 1)
       for (std::int64_t i = 0; i < n; ++i) weights_[static_cast<std::size_t>(i)] = weights_[static_cast<std::size_t>(i)] / factor;

@@ -1053,32 +1053,41 @@ struct FixedPointCdf {
   int exponent{0};                 // q = floor(w * 2^exponent)
   std::vector<std::uint64_t> cdf;  // inclusive
   std::uint64_t total{0};
+  bool valid{true};  // false: no weight can be selected and `cdf` is the uniform fallback
 };
 
+/// The one rule for which weights can be selected: 0 < w <= DBL_MAX.  Zero, negative, NaN and +-inf weights never are.
+inline bool weight_selectable(double w) { return w > 0.0 && w <= std::numeric_limits<double>::max(); }
+
+/// What every particle quantises to when no weight can be selected: a uniform CDF.
+constexpr std::uint64_t kUniformFallbackWeight = std::uint64_t{1} << 20;
+
+/// wmax = 0 (no weight can be selected) counts as 2^0: the exponent is then P.
 inline int fixed_point_exponent(double wmax, std::uint64_t n_total) {
   const int p = std::min(52, 62 - ceil_log2(n_total));
   int ex = 0;
-  (void)std::frexp(wmax, &ex);  // wmax = m * 2^ex, m in [0.5, 1)
+  if (weight_selectable(wmax)) (void)std::frexp(wmax, &ex);  // wmax = m * 2^ex, m in [0.5, 1)
   return p - ex;
 }
 
 inline std::uint64_t quantize_weight(double w, int exponent) {
-  const double scaled = std::ldexp(w, exponent);
-  if (!(scaled > 0.0)) return 0;  // zero, negative or NaN weights never get selected
-  return static_cast<std::uint64_t>(scaled);
+  if (!weight_selectable(w)) return 0;  // zero, negative, NaN or infinite weights never get selected
+  return static_cast<std::uint64_t>(std::ldexp(w, exponent));
 }
 
+/// With no weight that can be selected, every particle gets kUniformFallbackWeight and `valid` is false (the reference
+/// would divide by zero in normalize.hpp:82).
 inline FixedPointCdf fixed_point_cdf(const std::vector<double>& weights, std::uint64_t n_total = 0) {
   FixedPointCdf out;
   double wmax = 0.0;
   for (const double w : weights)
-    if (w > wmax) wmax = w;
-  if (!(wmax > 0.0) || !std::isfinite(wmax)) throw std::runtime_error("no positive finite weight");
+    if (weight_selectable(w) && w > wmax) wmax = w;
+  out.valid = wmax > 0.0;
   out.exponent = fixed_point_exponent(wmax, n_total == 0 ? weights.size() : n_total);
   out.cdf.resize(weights.size());
   std::uint64_t acc = 0;
   for (std::size_t i = 0; i < weights.size(); ++i) {
-    acc += quantize_weight(weights[i], out.exponent);
+    acc += out.valid ? quantize_weight(weights[i], out.exponent) : kUniformFallbackWeight;
     out.cdf[i] = acc;
   }
   out.total = acc;

@@ -371,13 +371,14 @@ int orc_normal_transform(const double* cov9, double* transform9) {
 }
 
 /// Mode-B resampling of a weight vector: indices[j] for j < m (no injection, no KLD).
-int orc_resample_indices(const double* weights, std::uint64_t n, std::uint64_t n_total, int scheme, std::uint64_t seed, std::uint32_t step, std::uint64_t m, std::int64_t* indices, std::uint64_t* cdf_out, int* exponent_out) {
+int orc_resample_indices(const double* weights, std::uint64_t n, std::uint64_t n_total, int scheme, std::uint64_t seed, std::uint32_t step, std::uint64_t m, std::int64_t* indices, std::uint64_t* cdf_out, int* exponent_out, int* valid_out) {
   try {
     const FixedPointCdf cdf = fixed_point_cdf(std::vector<double>(weights, weights + n), n_total);
     const CounterResampler rs{seed, step, static_cast<ResampleScheme>(scheme), cdf.total, m};
     for (std::uint64_t j = 0; j < m; ++j) indices[j] = static_cast<std::int64_t>(cdf_search(cdf.cdf, rs.position(j)));
     if (cdf_out != nullptr) std::memcpy(cdf_out, cdf.cdf.data(), n * sizeof(std::uint64_t));
     if (exponent_out != nullptr) *exponent_out = cdf.exponent;
+    if (valid_out != nullptr) *valid_out = cdf.valid ? 1 : 0;
     return 0;
   } catch (const std::exception& e) {
     g_error = e.what();

@@ -418,18 +418,19 @@ def normal_transform(cov) -> np.ndarray:
 MULTINOMIAL, SYSTEMATIC = 0, 1
 
 
-def resample_indices(weights, scheme: int, seed: int, step: int, m: int | None = None, n_total: int = 0):
-    """Mode-B indices plus the fixed-point CDF and exponent."""
+def resample_indices(weights, scheme: int, seed: int, step: int, m: int | None = None, n_total: int = 0, return_valid: bool = False):
+    """Mode-B indices plus the fixed-point CDF and exponent; return_valid adds whether any weight could be selected
+    (False: the CDF is the uniform fallback, 2^20 per particle)."""
     w = _f64(weights)
     m = len(w) if m is None else m
     idx = np.zeros(m, dtype=np.int64)
     cdf = np.zeros(len(w), dtype=np.uint64)
-    ex = C.c_int(0)
+    ex, valid = C.c_int(0), C.c_int(0)
     rc = lib().orc_resample_indices(_p(w, C.c_double), C.c_uint64(len(w)), C.c_uint64(n_total), C.c_int(scheme), C.c_uint64(seed),
-                                    C.c_uint32(step), C.c_uint64(m), _p(idx, C.c_int64), _p(cdf, C.c_uint64), C.byref(ex))
+                                    C.c_uint32(step), C.c_uint64(m), _p(idx, C.c_int64), _p(cdf, C.c_uint64), C.byref(ex), C.byref(valid))
     if rc != 0:
         raise RuntimeError(lib().orc_last_error().decode())
-    return idx, cdf, ex.value
+    return (idx, cdf, ex.value, bool(valid.value)) if return_valid else (idx, cdf, ex.value)
 
 
 def resample_indices_std(weights, seed: int, m: int) -> np.ndarray:

@@ -14,8 +14,11 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbeluga_b200.so")
-SOURCES = ["kernels.cu", "cluster.cu", "device_map.cu", "filter.cu", "amcl.cu", "batch.cu", "c_api.cu", "map_host.cpp", "cluster_host.cpp"]
-HEADERS = ["kernels.cuh", "cluster.cuh", "cluster_host.hpp", "se2_math.cuh", "device_map.hpp", "filter.hpp", "amcl.hpp", "batch.hpp", "map_host.hpp", os.path.join("..", "..", "include", "beluga_b200.h")]
+SOURCES = ["step.cu", "propagate.cu", "reweight_lfm.cu", "reweight_beam.cu", "cdf.cu", "kld.cu", "resample.cu", "batch_kernels.cu",
+           "shard_exchange.cu", "cluster.cu", "device_map.cu", "filter.cu", "amcl.cu", "batch.cu", "c_api.cu", "map_host.cpp", "cluster_host.cpp"]
+HEADERS = ["kernels.cuh", "device_common.cuh", "bucket_set.cuh", "propagate.cuh", "reweight_lfm.cuh", "reweight_beam.cuh", "cdf.cuh", "resample.cuh",
+           "cluster.cuh", "cluster_host.hpp", "se2_math.cuh", "device_map.hpp", "filter.hpp", "amcl.hpp", "batch.hpp", "map_host.hpp",
+           os.path.join("..", "..", "include", "beluga_b200.h")]
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [

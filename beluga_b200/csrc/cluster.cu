@@ -6,7 +6,9 @@
 //   batch_cluster_cells / _compact  the same stages for every selected member of a batch, one CTA per member
 // Nothing here uses floating-point atomics: every sum has a fixed order, so results are reproducible
 // run to run and the per-cell weight is the reference's sequential sum bit for bit.
+#include "bucket_set.cuh"
 #include "cluster.cuh"
+#include "device_common.cuh"
 
 #include <algorithm>
 #include <initializer_list>
@@ -14,20 +16,6 @@
 namespace bb200 {
 
 namespace {
-
-constexpr int kWarp = 32;
-constexpr unsigned long long kEmpty = ~0ull;
-
-__device__ __forceinline__ Pose2 load_state(const Pose2* p) {
-  const double2 a = *reinterpret_cast<const double2*>(p);
-  const double2 b = *(reinterpret_cast<const double2*>(p) + 1);
-  return Pose2{a.x, a.y, b.x, b.y};
-}
-
-__device__ __forceinline__ uint64_t probe_start(unsigned long long key, uint64_t mask) {
-  const unsigned long long h = key * 0x9E3779B97F4A7C15ull;
-  return (h ^ (h >> 29)) & mask;
-}
 
 // ---- cells -------------------------------------------------------------------------------------------
 
@@ -38,18 +26,9 @@ __global__ void __launch_bounds__(256) cluster_insert_kernel(const Pose2* __rest
                                                              unsigned int* first, uint64_t mask) {
   const uint64_t i = static_cast<uint64_t>(blockIdx.x) * 256 + threadIdx.x;
   if (i >= n) return;
-  const unsigned long long hash = spatial_hash(load_state(states + i), linear, linear, angular);
+  const unsigned long long hash = spatial_hash(load_pose(states + i), linear, linear, angular);
   hashes[i] = hash;
-  const unsigned long long key = hash == kEmpty ? kEmpty - 1 : hash;  // the sentinel itself cannot be stored (2^-64 event)
-  uint64_t pos = probe_start(key, mask);
-  for (;;) {
-    const unsigned long long prev = atomicCAS(keys + pos, kEmpty, key);
-    if (prev == kEmpty || prev == key) {
-      atomicMin(first + pos, static_cast<unsigned int>(i));
-      return;
-    }
-    pos = (pos + 1) & mask;
-  }
+  bucket_set::insert_min(keys, first, mask, hash, static_cast<unsigned int>(i));
 }
 
 /// flags[i] = 1 when particle i is the first of its cell (try_emplace inserted, :151-156).
@@ -58,10 +37,7 @@ __global__ void __launch_bounds__(256) cluster_flag_kernel(const unsigned long l
                                                            uint64_t mask, uint32_t* __restrict__ slot_of, uint32_t* __restrict__ flags) {
   const uint64_t i = static_cast<uint64_t>(blockIdx.x) * 256 + threadIdx.x;
   if (i >= n) return;
-  const unsigned long long hash = hashes[i];
-  const unsigned long long key = hash == kEmpty ? kEmpty - 1 : hash;
-  uint64_t pos = probe_start(key, mask);
-  while (keys[pos] != key) pos = (pos + 1) & mask;
+  const uint64_t pos = bucket_set::find(keys, mask, hashes[i]);
   slot_of[i] = static_cast<uint32_t>(pos);
   flags[i] = first[pos] == static_cast<unsigned int>(i) ? 1u : 0u;
 }
@@ -175,7 +151,7 @@ __device__ __forceinline__ void cell_record_warp(const Pose2* states, const doub
   for (; p + 3 * kWarp < end; p += 4 * kWarp) {  // four gathers in flight per lane
     const uint32_t i0 = sorted_idx[p], i1 = sorted_idx[p + kWarp], i2 = sorted_idx[p + 2 * kWarp], i3 = sorted_idx[p + 3 * kWarp];
     const double w0 = weights[i0], w1 = weights[i1], w2 = weights[i2], w3 = weights[i3];
-    const Pose2 s0 = load_state(states + i0), s1 = load_state(states + i1), s2 = load_state(states + i2), s3 = load_state(states + i3);
+    const Pose2 s0 = load_pose(states + i0), s1 = load_pose(states + i1), s2 = load_pose(states + i2), s3 = load_pose(states + i3);
     add(s0, w0);
     add(s1, w1);
     add(s2, w2);
@@ -183,7 +159,7 @@ __device__ __forceinline__ void cell_record_warp(const Pose2* states, const doub
   }
   for (; p < end; p += kWarp) {
     const uint32_t i = sorted_idx[p];
-    add(load_state(states + i), weights[i]);
+    add(load_pose(states + i), weights[i]);
   }
 #pragma unroll
   for (int k = 0; k < kMomentCount; ++k) {
@@ -214,7 +190,7 @@ __device__ __forceinline__ void cell_record_warp(const Pose2* states, const doub
     r.first_index = first;
     r.count = end - begin;
     r.weight = total;
-    r.representative = load_state(states + first);
+    r.representative = load_pose(states + first);
 #pragma unroll
     for (int k = 0; k < kMomentCount; ++k) r.moments[k] = m[k];
     *record = r;
@@ -260,24 +236,15 @@ __global__ void __launch_bounds__(kBatchCellThreads) batch_cluster_cells_kernel(
   const unsigned lanes_below = (1u << lane) - 1u;
 
   for (uint64_t s = tid; s <= mask; s += kBatchCellThreads) {
-    keys[s] = kEmpty;
+    keys[s] = bucket_set::kEmpty;
     first[s] = ~0u;
   }
   __syncthreads();
   // spatial_hash<SE2d>{linear, linear, angular} of every state into the set "cell -> smallest particle index".
   for (uint32_t i = tid; i < n; i += kBatchCellThreads) {
-    const unsigned long long hash = spatial_hash(load_state(states + i), a.linear, a.linear, a.angular);
+    const unsigned long long hash = spatial_hash(load_pose(states + i), a.linear, a.linear, a.angular);
     hashes[i] = hash;
-    const unsigned long long key = hash == kEmpty ? kEmpty - 1 : hash;
-    uint64_t pos = probe_start(key, mask);
-    for (;;) {
-      const unsigned long long prev = atomicCAS(keys + pos, kEmpty, key);
-      if (prev == kEmpty || prev == key) {
-        atomicMin(first + pos, i);
-        break;
-      }
-      pos = (pos + 1) & mask;
-    }
+    bucket_set::insert_min(keys, first, mask, hash, i);
   }
   __syncthreads();
   // Cells numbered by first occurrence: chunk by chunk in particle order, a cell's first particle takes the next number.
@@ -287,10 +254,7 @@ __global__ void __launch_bounds__(kBatchCellThreads) batch_cluster_cells_kernel(
     uint32_t pos = 0;
     bool head = false;
     if (i < n) {
-      const unsigned long long hash = hashes[i];
-      const unsigned long long key = hash == kEmpty ? kEmpty - 1 : hash;
-      pos = static_cast<uint32_t>(probe_start(key, mask));
-      while (keys[pos] != key) pos = (pos + 1) & mask;
+      pos = static_cast<uint32_t>(bucket_set::find(keys, mask, hashes[i]));
       head = first[pos] == i;
       cell_of[i] = pos;  // the slot for now, the cell id below
     }

@@ -1,4 +1,24 @@
-// Kernel launch interface of the CUDA MCL backend (see kernels.cu for the kernels themselves).
+// Kernel launch interface of the CUDA MCL backend.  The kernels are hand-written for sm_90a, one source per stage of a
+// filter step on the device (fixed particle count, resample every step):
+//
+//   step.cu               begin_step: zero the per-filter scalars; the summary block of a finished step
+//   propagate.cu          a2 + a6 of SURVEY.md section 8(a): Philox normals, SE2 compose; cloud moments; initialisation;
+//                         schedule_*: counting sort of the particles over pose bins (execution order only)
+//   reweight_lfm.cu       a3 + a5: B likelihood-field lookups per particle in schedule order, w *= L written to the
+//                         particle's own slot, block max of w
+//   reweight_beam.cu      a4 + a5: the same with ray casts (beam model)
+//   cdf.cu                prepare_cdf: exponent of the fixed-point grid from the largest weight; quantize_scan:
+//                         q = floor(w * 2^e), single-pass decoupled look-back inclusive scan (u64); scan_u32
+//   kld.cu                a12: KLD-adaptive sample size over a spatial-hash bucket set (bucket_set.cuh)
+//   resample.cu           a10 + a11 + a13: one thread per output slot (or per particle, scatter form); counter draw,
+//                         CDF search, 32-byte state gather, w = 1, per-block raw moments for a14; normalise;
+//                         reduce_partials: fixed-order sum of the per-block moments
+//   batch_kernels.cu      the same stages for a batch of filters, one CTA range per member
+//   shard_exchange.cu     step scalars exchanged between the shards of one filter
+//
+// Block bodies that a batch kernel shares with a single-filter kernel live in the stage's .cuh; device_common.cuh holds
+// what every stage uses.  All floating-point arithmetic that decides a likelihood-field cell or a weight follows the
+// reference's operation order without FMA contraction (every source is compiled with -fmad=false).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -49,7 +69,7 @@ BB_HD uint32_t bordered_index(uint32_t px, uint32_t py, int kx) {
 /// Largest padded grid side the fixed-point kernel accepts (cell coordinates below 2^13).
 constexpr int kFixedMaxSide = 8000;
 /// What the fixed-point lookup's element index gains, modulo 2^32, when its coordinates keep the bias of their magic
-/// constants (kernels.cu, fixed_lookup).
+/// constants (reweight_lfm.cuh, fixed_lookup).
 uint32_t fixed_index_bias(uint32_t border_pitch);
 
 /// Device view of the occupancy grid (beam model).
@@ -316,6 +336,10 @@ void launch_prepare_cdf(Scalars* scalars, double host_wmax, uint64_t global_coun
 /// `ticket` is one device word, `tile_state` holds scan_tile_count(n) words; both are reset here.
 void launch_scan_u32(const uint32_t* in, uint32_t* out, uint32_t n, unsigned long long* ticket, unsigned long long* tile_state,
                      unsigned long long* total_out, cudaStream_t stream);
+/// The same scan without the resets: the caller has zeroed the (n + 4095) / 4096 tile words of `tile_state` already, and
+/// n must not be 0.  For launch sequences that reset the scan state together with other state.
+void launch_scan_u32_prepared(const uint32_t* in, uint32_t* out, uint32_t n, unsigned long long* ticket, unsigned long long* tile_state,
+                              unsigned long long* total_out, cudaStream_t stream);
 uint32_t scan_tile_count(uint64_t n);
 /// Fixed-point quantisation + single-pass inclusive scan (decoupled look-back).
 /// derive_exponent: take the exponent from scalars->wmax_bits inside the kernel (needs the scan state already reset,

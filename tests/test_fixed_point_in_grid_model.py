@@ -1,4 +1,4 @@
-"""Executable version of the argument behind the unclamped lookup of the fixed-point reweight kernels (csrc/kernels.cu,
+"""Executable version of the argument behind the unclamped lookup of the fixed-point reweight kernels (csrc/reweight_lfm.cuh,
 fixed_lookup<true>): a warp whose particles pass the in-grid test reads the table without clamping its cell coordinates and
 without removing their bias, from a base pointer moved back by fixed_index_bias(pitch).
 

@@ -1,4 +1,4 @@
-"""Executable version of the argument behind reweight_lfm_fixed_*_kernel (csrc/kernels.cu): the kernel finds the
+"""Executable version of the argument behind reweight_lfm_fixed_*_kernel (csrc/reweight_lfm.cuh): the kernel finds the
 likelihood-field CELL of a beam end point with two FMAs per coordinate and a magic-number add instead of the
 reference's rounded operation sequence -- the magic number riding in the FMAs' addend -- and claims the same cell
 whenever the fraction word it reads is at least 5.

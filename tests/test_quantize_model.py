@@ -1,4 +1,4 @@
-"""Executable version of the argument behind quantize_scan_kernel's arithmetic (csrc/kernels.cu): the fixed-point weight
+"""Executable version of the argument behind quantize_scan_kernel's arithmetic (csrc/cdf.cuh): the fixed-point weight
 q = floor(w * 2^e), with e from the largest weight and the particle count (oracle/beluga_oracle.hpp: fixed_point_exponent,
 quantize_weight -- std::ldexp), is computed on the device as floor((w * 2^e1) * 2^(e - e1)), e1 = e / 2: two multiplications
 by exact powers of two instead of scalbn.  The claims checked here, with exact rationals:
@@ -29,7 +29,7 @@ def fixed_point_exponent(wmax: float, n_total: int) -> int:
 
 
 def pow2_double(e: int) -> float:
-    """kernels.cu: pow2_double -- the bit pattern (e + 1023) << 52; needs a normal result."""
+    """cdf.cuh: pow2_double -- the bit pattern (e + 1023) << 52; needs a normal result."""
     assert -1022 <= e <= 1023, e
     return math.ldexp(1.0, e)
 
@@ -48,12 +48,12 @@ def double2ull_rd(x: float) -> int:
 
 
 def weight_selectable(w: float) -> bool:
-    """kernels.cu: weight_selectable -- the rule weight_order_bits and quantize_mul share."""
+    """device_common.cuh: weight_selectable -- the rule weight_order_bits and quantize_mul share."""
     return 0.0 < w <= DBL_MAX
 
 
 def kernel_quantize(w: float, exponent: int) -> int:
-    """kernels.cu: quantize_mul with the factors quantize_scan_tile builds."""
+    """cdf.cuh: quantize_mul with the factors quantize_scan_tile builds."""
     if not weight_selectable(w):
         return 0
     e1 = int(exponent / 2)  # C++ integer division truncates towards zero

@@ -1,4 +1,4 @@
-"""Integer model of the empty-space skipping in cast_ray (csrc/kernels.cu): the beam kernel walks the reference's
+"""Integer model of the empty-space skipping in cast_ray (csrc/reweight_beam.cuh): the beam kernel walks the reference's
 standard Bresenham line (algorithm/raycasting/bresenham.hpp:84-160) but advances d steps at once where the
 Chebyshev free-distance map says the next d - 1 cells cannot stop the ray, updating (x, y, error) in closed form
 (with the 32-bit reciprocal-multiply-and-correct quotient the kernel uses).  Checked here against a plain cell-by-cell

@@ -1,4 +1,4 @@
-"""Integer model of resample_scatter_kernel (csrc/kernels.cu): with the systematic comb t_j = offset + j*stride the
+"""Integer model of resample_scatter_kernel (csrc/resample.cuh): with the systematic comb t_j = offset + j*stride the
 slots that select particle i are [ja_i, jb_i) with ja/jb from two integer divisions.  Checked here against the
 per-slot definition (smallest i with cdf[i] > t_j, what resample_kernel and the oracle compute), on one shard and
 split over ranks, with python integers.  CPU only."""
@@ -9,7 +9,7 @@ from beluga_b200.distributed import cdf_offsets, slot_ranges
 
 
 def comb_slots_before(position, offset, stride, total_slots):
-    """Number of slots j with offset + j * stride < position (kernels.cu: comb_slots_before)."""
+    """Number of slots j with offset + j * stride < position (resample.cuh: comb_slots_before)."""
     if position <= offset:
         return 0
     return min((position - offset + stride - 1) // stride, total_slots)
@@ -84,7 +84,7 @@ def test_sharded_scatter_covers_every_slot_once(world):
 
 
 def comb_slots_before_magic(position, offset, stride, magic, total_slots):
-    """kernels.cu: comb_slots_before_magic -- the division replaced by __umul64hi with magic = floor((2^64 - 1) / stride) and one
+    """resample.cuh: comb_slots_before_magic -- the division replaced by __umul64hi with magic = floor((2^64 - 1) / stride) and one
     remainder check.  64-bit wrap-around arithmetic is modelled with masks."""
     mask = (1 << 64) - 1
     if position <= offset:

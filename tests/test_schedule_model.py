@@ -1,5 +1,5 @@
 """Executable version of the argument behind the execution schedule of the reweight kernel (csrc/kernels.cuh:
-schedule_from_moments, csrc/kernels.cu: schedule_bin): particles are counting-sorted over pose bins and every warp takes 32
+schedule_from_moments, csrc/propagate.cu: schedule_bin): particles are counting-sorted over pose bins and every warp takes 32
 neighbours of that order, so the 32 end points of one beam land in a few cache lines.  The schedule decides only WHICH
 THREAD handles a particle -- any permutation gives the same results -- so what there is to check is that the bin function
 always yields a valid bin, that consecutive bins are neighbours (boustrophedon order), and that the equal-mass bins do what

@@ -20,10 +20,25 @@ struct BeamRay {
   double short_decay;   // exp(-lambda_short * z) of the short-reading term (:137-141)
 };
 
-/// regular_grid.hpp:75-78.  Clamped to +-2^28 cells so that spans of far-away end points cannot
-/// overflow 32-bit integers (the reference's cast<int>() is undefined out there).
-__device__ __forceinline__ int cell_near(double p, double inv_resolution) {
-  return max(-(1 << 28), min(1 << 28, __double2int_rd(p * inv_resolution)));
+/// The largest span, in cells along either axis, for which the reference's int Bresenham arithmetic (bresenham.hpp:84-160)
+/// cannot overflow: error + dyspan <= 4 * span < 2^31.
+constexpr int kMaxRaySpan = (1 << 29) - 1;
+
+/// regular_grid.hpp:75-78 for the source cell of a ray: floor(p * inv_resolution), or -1 when that is NaN or outside
+/// [0, 2^31).  Such a source lies outside every grid (the reference's cast<int>() gives INT_MIN there on x86-64), so
+/// every ray from it is a miss.
+__device__ __forceinline__ int source_cell(double p, double inv_resolution) {
+  const double c = floor(p * inv_resolution);
+  return c >= 0.0 && c < 0x1p31 ? static_cast<int>(c) : -1;
+}
+
+/// The far-end cell of coordinate e (regular_grid.hpp:75-78, raycasting.hpp:81-85) as a span from the source cell s,
+/// clamped to +-kMaxRaySpan.  Within the clamp this is the reference's span exactly (floor(e * inv_resolution) and s are
+/// integers below 2^53); beyond it the reference's arithmetic overflows, and the far end is pulled back per axis.  A ray
+/// with a non-finite end point is a miss: the caller decides that (for NaN this still returns a span within the clamp).
+__device__ __forceinline__ int far_span(double e, double inv_resolution, int s) {
+  const double span = floor(e * inv_resolution) - static_cast<double>(s);
+  return static_cast<int>(fmin(fmax(span, -static_cast<double>(kMaxRaySpan)), static_cast<double>(kMaxRaySpan)));
 }
 
 /// One ray of Ray2d::cast (raycasting.hpp:79-107) over the standard Bresenham2i iterator (bresenham.hpp:84-160) as a
@@ -171,7 +186,7 @@ __device__ __forceinline__ void reweight_beam_block(const Pose2* __restrict__ st
   }
   // Ray2d: source pose in the grid frame and its cell (raycasting.hpp:67-70).
   const Pose2 src = pose_mul(grid.world_to_grid, st);
-  const int sx = cell_near(src.x, grid.inv_resolution), sy = cell_near(src.y, grid.inv_resolution);
+  const int sx = source_cell(src.x, grid.inv_resolution), sy = source_cell(src.y, grid.inv_resolution);
   const double n_norm = 1. / (sqrt(2. * 3.14159265358979323846) * params.sigma_hit);  // beam_model.hpp:107
 
   // The mixture value of one beam given its ray walk (beam_model.hpp:116-147).
@@ -193,7 +208,8 @@ __device__ __forceinline__ void reweight_beam_block(const Pose2* __restrict__ st
     // far end = r1 * t2 + t1 (raycasting.hpp:81-85)
     const double ex = (src.c * ray.far_x - src.s * ray.far_y) + src.x;
     const double ey = (src.s * ray.far_x + src.c * ray.far_y) + src.y;
-    ray_begin(walk, sx, sy, cell_near(ex, grid.inv_resolution), cell_near(ey, grid.inv_resolution));
+    ray_begin(walk, sx, sy, sx + far_span(ex, grid.inv_resolution, sx), sy + far_span(ey, grid.inv_resolution, sy));
+    if (!(isfinite(ex) && isfinite(ey))) walk.active = false;  // e.g. a NaN heading: the end point lies outside the grid, a miss
   };
   auto walk_ray = [&](const BeamRay& ray) {
     RayWalk walk;
@@ -266,8 +282,11 @@ __device__ __forceinline__ void beam_walk_block(const Pose2* __restrict__ states
   const uint64_t i = active ? (perm != nullptr ? perm[slot] : slot) : 0;
   // Ray2d: source pose in the grid frame and its cell (raycasting.hpp:67-70).
   const Pose2 src = pose_mul(grid.world_to_grid, active ? load_pose(states + i) : Pose2{1.0, 0.0, 0.0, 0.0});
-  const int sx = cell_near(src.x, grid.inv_resolution), sy = cell_near(src.y, grid.inv_resolution);
-  const bool source_inside = static_cast<unsigned>(sx) < static_cast<unsigned>(grid.width) && static_cast<unsigned>(sy) < static_cast<unsigned>(grid.height);
+  const int sx = source_cell(src.x, grid.inv_resolution), sy = source_cell(src.y, grid.inv_resolution);
+  // A source outside the grid sees nothing: the first cell already fails cell_is_valid.  Nor does a non-finite heading: its
+  // end points are not finite, so they lie outside the grid.
+  const bool source_inside = static_cast<unsigned>(sx) < static_cast<unsigned>(grid.width) && static_cast<unsigned>(sy) < static_cast<unsigned>(grid.height) &&
+                             isfinite(src.c) && isfinite(src.s);
   const int shift = grid.pad_shift;
   const int pitch = 1 << shift;
   const uint8_t* __restrict__ map = grid.free_padded;
@@ -284,12 +303,16 @@ __device__ __forceinline__ void beam_walk_block(const Pose2* __restrict__ states
     if (!active) continue;
     for (uint32_t b = 0; b < count; ++b) {
       uint32_t word = kHitMiss;
-      if (source_inside) {  // a source outside the grid sees nothing: the first cell already fails cell_is_valid
-        // far end = r1 * t2 + t1 (raycasting.hpp:81-85)
-        const double2 f = s_far[b];
-        const double ex = (src.c * f.x - src.s * f.y) + src.x;
-        const double ey = (src.s * f.x + src.c * f.y) + src.y;
-        int span = cell_near(ex, grid.inv_resolution) - sx, minor = cell_near(ey, grid.inv_resolution) - sy;
+      // far end = r1 * t2 + t1 (raycasting.hpp:81-85)
+      const double2 f = s_far[b];
+      const double ex = (src.c * f.x - src.s * f.y) + src.x;
+      const double ey = (src.s * f.x + src.c * f.y) + src.y;
+      // From a source inside the grid with a finite heading, an end point is NaN exactly when the beam's bearing is (a
+      // zero or non-finite scan point): it lies outside the grid, a miss.
+      if (source_inside && ex == ex && ey == ey) {
+        // far_span without its clamp: finite far ends lie within 2^21 cells of a source inside a grid of at most 65535
+        // cells a side, so the floor fits an int and the spans stay far below kMaxRaySpan
+        int span = __double2int_rd(ex * grid.inv_resolution) - sx, minor = __double2int_rd(ey * grid.inv_resolution) - sy;
         int stride_major = 1, stride_minor = pitch;
         if (span < 0) {
           span = -span;
@@ -353,7 +376,7 @@ __device__ __forceinline__ void beam_mixture_block(const Pose2* __restrict__ sta
   const bool active = local < slot_count && slot < n;
   const uint64_t i = active ? (perm != nullptr ? perm[slot] : slot) : 0;
   const Pose2 src = pose_mul(grid.world_to_grid, active ? load_pose(states + i) : Pose2{1.0, 0.0, 0.0, 0.0});
-  const int sx = cell_near(src.x, grid.inv_resolution), sy = cell_near(src.y, grid.inv_resolution);
+  const int sx = source_cell(src.x, grid.inv_resolution), sy = source_cell(src.y, grid.inv_resolution);
   const double source_x = (static_cast<double>(sx) + 0.5) * grid.resolution, source_y = (static_cast<double>(sy) + 0.5) * grid.resolution;
   const double n_norm = 1. / (sqrt(2. * 3.14159265358979323846) * params.sigma_hit);  // beam_model.hpp:107
 

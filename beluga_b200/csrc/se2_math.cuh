@@ -224,8 +224,15 @@ __device__ __forceinline__ double box_muller_first(const Draw& d) {
 #endif
 
 // ---- spatial hash (algorithm/spatial_hash.hpp:45-94,190-193) ------------------------------------
+/// floor(v) as an int64, or INT64_MIN when floor(v) is NaN or outside [-2^63, 2^63).  The reference's
+/// static_cast<int64_t>(std::floor(v)) is undefined out there; on x86-64 (cvttsd2si) it yields INT64_MIN, which this
+/// states explicitly, so that host and device agree (the device conversion saturates and turns NaN into 0).
+BB_HD int64_t floor_to_int64(double v) {
+  const double f = floor(v);
+  return f >= -0x1p63 && f < 0x1p63 ? static_cast<int64_t>(f) : INT64_MIN;
+}
 BB_HD uint64_t floor_and_fibo_hash(double value, unsigned shift) {
-  const int64_t signed_value = static_cast<int64_t>(floor(value));
+  const int64_t signed_value = floor_to_int64(value);
   const uint64_t h = 11400714819323198485ull * static_cast<uint64_t>(signed_value);
   return shift != 0 ? ((h << shift) | (h >> (64 - shift))) : h;
 }

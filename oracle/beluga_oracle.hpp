@@ -74,11 +74,17 @@ struct OccupancyGrid {
   [[nodiscard]] bool free_at(int xi, int yi) const { return free_at(index_at(xi, yi)); }
 };
 
-/// regular_grid.hpp:75-78: floor(p * (1/resolution)) cast to int.
+/// regular_grid.hpp:75-78: floor(p * (1/resolution)) cast to int.  The cast is undefined for NaN and outside
+/// [-2^31, 2^31); x86-64 gives INT_MIN there, stated here explicitly.  INT_MIN lies outside every grid.
 inline int cell_coord_near(double p, double resolution) {
   const double inv_resolution = 1. / resolution;
-  return static_cast<int>(std::floor(p * inv_resolution));
+  const double floored = std::floor(p * inv_resolution);
+  return floored >= -0x1p31 && floored < 0x1p31 ? static_cast<int>(floored) : std::numeric_limits<int>::min();
 }
+
+/// The largest span, in cells along either axis, for which Ray2d's int Bresenham arithmetic (bresenham.hpp:84-160)
+/// cannot overflow: error + dyspan <= 4 * span < 2^31.
+constexpr int kMaxRaySpan = (1 << 29) - 1;
 
 /// regular_grid.hpp:87-89: (cell + 0.5) * resolution.
 inline double cell_centroid(int cell, double resolution) { return (static_cast<double>(cell) + 0.5) * resolution; }
@@ -392,19 +398,32 @@ struct Ray2d {
         max_range(range),
         modified(modified_variant) {}
 
-  /// :79-88 far end cell for a bearing.
-  void far_end_cell(const SO2& bearing, int& fx, int& fy) const {
+  /// :79-88 far end cell for a bearing, for a source cell inside the grid.  Returns false when the far end is not
+  /// finite: the ray is then a miss.  Where the span from the source reaches kMaxRaySpan + 1 cells, the reference's
+  /// int arithmetic overflows; the far end is then pulled back, per axis, to kMaxRaySpan cells from the source.
+  /// Below that the far end is the reference's cell.
+  [[nodiscard]] bool far_end_cell(const SO2& bearing, int& fx, int& fy) const {
     const SO2& r1 = source_pose_in_local_frame.r;
     const Vec2 t2{bearing.c * max_range, bearing.s * max_range};
     const Vec2 rt = r1 * t2;
-    fx = cell_coord_near(rt.x + source_pose_in_local_frame.x, grid.resolution);
-    fy = cell_coord_near(rt.y + source_pose_in_local_frame.y, grid.resolution);
+    const double ex = rt.x + source_pose_in_local_frame.x;
+    const double ey = rt.y + source_pose_in_local_frame.y;
+    if (!std::isfinite(ex) || !std::isfinite(ey)) return false;
+    const double inv_resolution = 1. / grid.resolution;
+    const auto span = [](double e, int source) {  // exact: both terms are integers far below 2^53, or the clamp applies
+      const double s = std::floor(e) - static_cast<double>(source);
+      return static_cast<int>(std::min(std::max(s, -static_cast<double>(kMaxRaySpan)), static_cast<double>(kMaxRaySpan)));
+    };
+    fx = source_x + span(ex * inv_resolution, source_x);
+    fy = source_y + span(ey * inv_resolution, source_y);
+    return true;
   }
 
   /// :97-107.  `visited` (optional) counts the cells inspected (for the algorithmic-bytes figure).
   [[nodiscard]] std::optional<double> cast(const SO2& bearing, std::uint64_t* visited = nullptr) const {
+    if (!grid.contains(source_x, source_y)) return std::nullopt;  // the first cell of the line fails cell_is_valid
     int fx = 0, fy = 0;
-    far_end_cell(bearing, fx, fy);
+    if (!far_end_cell(bearing, fx, fy)) return std::nullopt;
     for (BresenhamLine line(source_x, source_y, fx, fy, modified); !line.done(); line.next()) {
       if (!grid.contains(line.cx, line.cy)) break;  // take_while(cell_is_valid), :86-87
       if (visited != nullptr) ++*visited;
@@ -820,7 +839,11 @@ struct RollingWindow2 {
 /// algorithm/spatial_hash.hpp:45-75 with N=21 bits per axis on 64-bit size_t (:93).
 inline std::uint64_t floor_and_fibo_hash(double value, unsigned shift) {
   constexpr std::uint64_t kFib = 11400714819323198485LLU;
-  const auto signed_value = static_cast<std::int64_t>(std::floor(value));
+  // The reference casts std::floor(value) to int64; for NaN and values outside [-2^63, 2^63) the cast is undefined and
+  // x86-64 gives INT64_MIN.  That result is stated here, so that the oracle gives it on every host.
+  const double floored = std::floor(value);
+  const std::int64_t signed_value = floored >= -0x1p63 && floored < 0x1p63 ? static_cast<std::int64_t>(floored)
+                                                                            : std::numeric_limits<std::int64_t>::min();
   const auto unsigned_value = static_cast<std::uint64_t>(signed_value);
   const std::uint64_t h = kFib * unsigned_value;
   if (shift != 0) return (h << shift) | (h >> (64 - shift));

@@ -2,6 +2,7 @@
 // tests (tests/test_schedule_model.py, tests/test_fixed_point_lookup_model.py) are checked against the code the kernels
 // are built from, not only against their own restatement.  Compiled with nvcc, runs without a GPU (no CUDA call).
 #include <cstdio>
+#include <cstring>
 
 #include "kernels.cuh"
 
@@ -46,6 +47,37 @@ int main() {
                 static_cast<unsigned long long>(spatial_hash(st, 0.5, 0.5, 0.17453292519943295)),
                 static_cast<unsigned long long>(spatial_hash(st, 0.05, 0.1, 0.01)), z0, z1,
                 static_cast<unsigned long long>(mulhi64(d.a, d.b)));
+  }
+  // the spatial hash where floor() leaves the int64 range (tests/test_integer_edges_cpu.py): values as bit patterns
+  const uint64_t edges[] = {
+      0x0000000000000000ull, 0x8000000000000000ull,  // +-0
+      0x0000000000000001ull, 0x8000000000000001ull, 0x000fffffffffffffull, 0x800fffffffffffffull,  // subnormals
+      0x3ff0000000000000ull, 0x3fefffffffffffffull, 0x3ff0000000000001ull,  // 1 and one ulp either side
+      0xbff0000000000000ull, 0xbfefffffffffffffull, 0xbff0000000000001ull,  // -1 and one ulp either side
+      0x4059000000000000ull, 0x4058ffffffffffffull, 0x4059000000000001ull,  // 100 and one ulp either side
+      0xbfe0000000000000ull, 0xbf847ae147ae147bull, 0x8000000000000010ull,  // -0.5, -0.01, a negative subnormal
+      0x4340000000000000ull, 0xc340000000000000ull, 0x4340000000000001ull,  // +-2^53, 2^53 + 2
+      0x43dfffffffffffffull, 0xc3dfffffffffffffull,  // +-(2^63 - 1024)
+      0x43e0000000000000ull, 0xc3e0000000000000ull,  // +-2^63
+      0x43e0000000000001ull, 0xc3e0000000000001ull,  // one ulp beyond +-2^63
+      0x7e37e43c8800759cull, 0xfe37e43c8800759cull,  // +-1e300
+      0x7fefffffffffffffull, 0xffefffffffffffffull,  // +-DBL_MAX
+      0x7ff0000000000000ull, 0xfff0000000000000ull,  // +-inf
+      0x7ff8000000000000ull, 0xfff8000000000000ull, 0x7ff0000000000001ull,  // NaNs
+  };
+  for (const uint64_t bits : edges) {
+    double v;
+    std::memcpy(&v, &bits, sizeof v);
+    std::printf("floor %016llx %lld %llu %llu\n", static_cast<unsigned long long>(bits), static_cast<long long>(floor_to_int64(v)),
+                static_cast<unsigned long long>(floor_and_fibo_hash(v, 0)), static_cast<unsigned long long>(floor_and_fibo_hash(v, 21)));
+    // the value as x, as y, and as the heading's cosine and sine (the bucket of atan2(s, c)), at resolutions that keep
+    // the quotient exact (1, 0.5) or push it past the int64 range (rtheta = 5e-324)
+    const Pose2 poses[] = {{1.0, 0.0, v, 0.25}, {1.0, 0.0, 0.25, v}, {v, 0.0, 0.25, 0.25}, {-1.0, v, 0.25, 0.25}, {1.0, v, 0.25, 0.25}};
+    for (const Pose2& st : poses)
+      std::printf("pose %016llx %.17g %.17g %.17g %.17g %llu %llu %llu\n", static_cast<unsigned long long>(bits), st.c, st.s, st.x, st.y,
+                  static_cast<unsigned long long>(spatial_hash(st, 1.0, 1.0, 0.1)),
+                  static_cast<unsigned long long>(spatial_hash(st, 0.5, 0.5, 0.17453292519943295)),
+                  static_cast<unsigned long long>(spatial_hash(st, 0.5, 0.5, 5e-324)));
   }
   return 0;
 }

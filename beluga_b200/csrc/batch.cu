@@ -3,7 +3,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
-#include <initializer_list>
+#include <utility>
 
 namespace bb200 {
 
@@ -68,38 +68,32 @@ Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, 
   const size_t k1 = static_cast<size_t>(n_members) + 1;
   BB_TRY(cudaSetDevice(device_));
   BB_TRY(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-  BB_TRY(dev_alloc(&states_[0], total_));
-  BB_TRY(dev_alloc(&states_[1], total_));
-  BB_TRY(dev_alloc(&weights_, total_));
-  BB_TRY(dev_alloc(&cdf_, total_));
-  if (record_ancestors_) BB_TRY(dev_alloc(&ancestors_, total_));
-  BB_TRY(dev_alloc(&scalars_, members_.size()));
-  BB_TRY(dev_alloc(&tile_state_, tiles));
-  BB_TRY(dev_alloc(&partials_, rows * kMomentCount));
-  BB_TRY(dev_alloc(&table_, members_.size()));
-  BB_TRY(host_alloc(&table_host_, members_.size()));
-  BB_TRY(dev_alloc(&first_, kBatchLaunches * k1));
-  BB_TRY(host_alloc(&first_host_, kBatchLaunches * k1));
-  BB_TRY(host_alloc(&summary_host_, members_.size()));
-  BB_TRY(host_alloc(&ticket_host_, 1));
-  BB_TRY(dev_alloc(&members_done_, 1));
-  *ticket_host_ = 0;  // pinned allocations are recycled with their old contents
-  BB_TRY(cudaMemsetAsync(scalars_, 0, members_.size() * sizeof(Scalars), stream_));
-  BB_TRY(cudaMemsetAsync(members_done_, 0, sizeof(unsigned int), stream_));
+  BB_TRY(states_[0].allocate(total_));
+  BB_TRY(states_[1].allocate(total_));
+  BB_TRY(weights_.allocate(total_));
+  BB_TRY(cdf_.allocate(total_));
+  if (record_ancestors_) BB_TRY(ancestors_.allocate(total_));
+  BB_TRY(scalars_.allocate(members_.size()));
+  BB_TRY(tile_state_.allocate(tiles));
+  BB_TRY(partials_.allocate(rows * kMomentCount));
+  BB_TRY(table_.allocate(members_.size()));
+  BB_TRY(table_host_.allocate(members_.size()));
+  BB_TRY(first_.allocate(kBatchLaunches * k1));
+  BB_TRY(first_host_.allocate(kBatchLaunches * k1));
+  BB_TRY(summary_host_.allocate(members_.size()));
+  BB_TRY(ticket_host_.allocate(1));
+  BB_TRY(members_done_.allocate(1));
+  *ticket_host_.get() = 0;  // pinned allocations are recycled with their old contents
+  BB_TRY(cudaMemsetAsync(scalars_.get(), 0, members_.size() * sizeof(Scalars), stream_));
+  BB_TRY(cudaMemsetAsync(members_done_.get(), 0, sizeof(unsigned int), stream_));
   BB_TRY(cudaStreamSynchronize(stream_));
   created_ = true;
 }
 
 Batch::~Batch() {
-  if (stream_ != nullptr) cudaStreamSynchronize(stream_);
-  for (void* p : std::initializer_list<void*>{states_[0], states_[1], weights_, cdf_, ancestors_, scalars_, tile_state_, partials_, table_, first_,
-                                              points_, hits_, map_table_, members_done_, cl_hashes_, cl_keys_, cl_first_, cl_ids_, cl_cell_of_, cl_sort_[0], cl_sort_[1],
-                                              cl_starts_, cl_records_, cl_table_, cl_cells_, sm_table_, samples_})
-    cudaFree(p);
-  for (void* p : std::initializer_list<void*>{table_host_, first_host_, points_host_, summary_host_, ticket_host_, cl_table_host_, cl_cells_host_,
-                                              cl_records_host_, sm_table_host_, samples_host_})
-    cudaFreeHost(p);
-  if (stream_ != nullptr) cudaStreamDestroy(stream_);
+  if (stream_ == nullptr) return;
+  cudaStreamSynchronize(stream_);  // nothing in flight reads the buffers the members free
+  cudaStreamDestroy(stream_);
 }
 
 int Batch::member_ok(int member) const {
@@ -230,16 +224,10 @@ int Batch::ensure_map_table() {
     e.slot = static_cast<int>(host.size());
     host.push_back(BatchMap{d.field, d.occupancy, d.beam, d.free_cells, d.n_free, d.grid_width, d.grid_resolution, d.grid_origin});
   }
-  if (host.size() > map_table_capacity_) {
-    BB_CHECK(cudaFree(map_table_));  // every batch call ends synchronised: no step reads the old table
-    map_table_ = nullptr;
-    map_table_capacity_ = 0;
-    BB_CHECK(dev_alloc(&map_table_, host.size()));
-    map_table_capacity_ = host.size();
-  }
+  BB_CHECK(map_table_.grow(host.size()));  // every batch call ends synchronised: no step reads the old table
   // On the batch's stream, so that the step's launches follow the copy in order; the pageable source is staged before the
   // call returns.
-  BB_CHECK(cudaMemcpyAsync(map_table_, host.data(), host.size() * sizeof(BatchMap), cudaMemcpyHostToDevice, stream_));
+  BB_CHECK(cudaMemcpyAsync(map_table_.get(), host.data(), host.size() * sizeof(BatchMap), cudaMemcpyHostToDevice, stream_));
   map_table_current_ = true;
   return BB200_OK;
 }
@@ -252,7 +240,7 @@ int Batch::initialize(int member, const double mean[3], const double cov[9]) {
   if (!normal_transform(cov, transform, &message)) return fail(BB200_ERR_INVALID_ARGUMENT, message);
   BB_CHECK(cudaSetDevice(device_));
   m.cdf_total = 0;
-  launch_initialize_normal(states_[m.cur] + m.offset, weights_ + m.offset, m.capacity, mean, transform, m.policy.params().seed, 0, stream_);
+  launch_initialize_normal(states_[m.cur].get() + m.offset, weights_.get() + m.offset, m.capacity, mean, transform, m.policy.params().seed, 0, stream_);
   ++launches_;
   BB_CHECK(cudaGetLastError());
   BB_CHECK(cudaStreamSynchronize(stream_));
@@ -271,7 +259,7 @@ int Batch::initialize_from_map(int member) {
   if (map.n_free == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
   BB_CHECK(cudaSetDevice(device_));
   m.cdf_total = 0;
-  launch_initialize_uniform(states_[m.cur] + m.offset, weights_ + m.offset, m.capacity, map.free_cells, map.n_free, map.grid_width,
+  launch_initialize_uniform(states_[m.cur].get() + m.offset, weights_.get() + m.offset, m.capacity, map.free_cells, map.n_free, map.grid_width,
                             map.grid_resolution, map.grid_origin, m.policy.params().seed, 0, stream_);
   ++launches_;
   BB_CHECK(cudaGetLastError());
@@ -291,9 +279,9 @@ int Batch::initialize_states(int member, const double* states, const double* wei
   BB_CHECK(cudaStreamSynchronize(stream_));
   m.cdf_total = 0;
   if (n > 0) {
-    BB_CHECK(cudaMemcpy(states_[m.cur] + m.offset, states, n * sizeof(Pose2), cudaMemcpyHostToDevice));
+    BB_CHECK(cudaMemcpy(states_[m.cur].get() + m.offset, states, n * sizeof(Pose2), cudaMemcpyHostToDevice));
     const std::vector<double> ones(weights == nullptr ? n : 0, 1.0);
-    BB_CHECK(cudaMemcpy(weights_ + m.offset, weights != nullptr ? weights : ones.data(), n * sizeof(double), cudaMemcpyHostToDevice));
+    BB_CHECK(cudaMemcpy(weights_.get() + m.offset, weights != nullptr ? weights : ones.data(), n * sizeof(double), cudaMemcpyHostToDevice));
     m.pivot[0] = states[2];
     m.pivot[1] = states[3];
   }
@@ -314,8 +302,8 @@ int Batch::get_particles(int member, double* states, double* weights, uint64_t c
   BB_CHECK(cudaSetDevice(device_));
   BB_CHECK(cudaStreamSynchronize(stream_));
   const uint64_t n = std::min(capacity, m.n);
-  if (states != nullptr && n > 0) BB_CHECK(cudaMemcpy(states, states_[m.cur] + m.offset, n * sizeof(Pose2), cudaMemcpyDeviceToHost));
-  if (weights != nullptr && n > 0) BB_CHECK(cudaMemcpy(weights, weights_ + m.offset, n * sizeof(double), cudaMemcpyDeviceToHost));
+  if (states != nullptr && n > 0) BB_CHECK(cudaMemcpy(states, states_[m.cur].get() + m.offset, n * sizeof(Pose2), cudaMemcpyDeviceToHost));
+  if (weights != nullptr && n > 0) BB_CHECK(cudaMemcpy(weights, weights_.get() + m.offset, n * sizeof(double), cudaMemcpyDeviceToHost));
   return BB200_OK;
 }
 
@@ -326,7 +314,7 @@ int Batch::ancestors(int member, int64_t* out, uint64_t capacity) {
   BB_CHECK(cudaSetDevice(device_));
   BB_CHECK(cudaStreamSynchronize(stream_));
   const uint64_t n = std::min(capacity, m.ancestors_n);
-  if (out != nullptr && n > 0) BB_CHECK(cudaMemcpy(out, ancestors_ + m.offset, n * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  if (out != nullptr && n > 0) BB_CHECK(cudaMemcpy(out, ancestors_.get() + m.offset, n * sizeof(int64_t), cudaMemcpyDeviceToHost));
   return BB200_OK;
 }
 
@@ -341,32 +329,28 @@ int Batch::cluster_estimate(int member, const bb200_cluster_param& p, bb200_esti
 }
 
 int Batch::ensure_cluster_scratch() {
-  if (cl_cells_host_ != nullptr) return BB200_OK;
+  if (cl_.hashes.get() != nullptr) return BB200_OK;
   const size_t k = members_.size();
-  BB_CHECK(dev_alloc(&cl_hashes_, total_));
-  BB_CHECK(dev_alloc(&cl_keys_, table_total_));
-  BB_CHECK(dev_alloc(&cl_first_, table_total_));
-  BB_CHECK(dev_alloc(&cl_ids_, table_total_));
-  BB_CHECK(dev_alloc(&cl_cell_of_, total_));
-  BB_CHECK(dev_alloc(&cl_sort_[0], total_));
-  BB_CHECK(dev_alloc(&cl_sort_[1], total_));
-  BB_CHECK(dev_alloc(&cl_starts_, total_ + k));
-  BB_CHECK(dev_alloc(&cl_records_, total_));
-  BB_CHECK(dev_alloc(&cl_table_, k));
-  BB_CHECK(host_alloc(&cl_table_host_, k));
-  BB_CHECK(dev_alloc(&cl_cells_, k));
-  BB_CHECK(host_alloc(&cl_cells_host_, k));  // last: marks the scratch as allocated
+  ClusterBuffers c;
+  BB_CHECK(c.hashes.allocate(total_));
+  BB_CHECK(c.keys.allocate(table_total_));
+  BB_CHECK(c.first.allocate(table_total_));
+  BB_CHECK(c.ids.allocate(table_total_));
+  BB_CHECK(c.cell_of.allocate(total_));
+  BB_CHECK(c.sort[0].allocate(total_));
+  BB_CHECK(c.sort[1].allocate(total_));
+  BB_CHECK(c.starts.allocate(total_ + k));
+  BB_CHECK(c.records.allocate(total_));
+  BB_CHECK(c.table.allocate(k));
+  BB_CHECK(c.table_host.allocate(k));
+  BB_CHECK(c.cells.allocate(k));
+  BB_CHECK(c.cells_host.allocate(k));
+  cl_ = std::move(c);
   return BB200_OK;
 }
 
 int Batch::ensure_cluster_records(uint64_t cells) {
-  if (cells <= cl_records_host_capacity_) return BB200_OK;
-  cudaFreeHost(cl_records_host_);
-  cl_records_host_ = nullptr;
-  cl_records_host_capacity_ = 0;
-  const uint64_t want = std::min<uint64_t>(total_, std::max<uint64_t>(4096, 2 * cells));
-  BB_CHECK(host_alloc(&cl_records_host_, want));
-  cl_records_host_capacity_ = want;
+  BB_CHECK(cl_records_host_.grow(cells, std::min<uint64_t>(total_, std::max<uint64_t>(4096, 2 * cells))));
   return BB200_OK;
 }
 
@@ -381,11 +365,11 @@ int Batch::cluster_estimates(const bb200_cluster_param& p, const uint8_t* presen
   if (const int st = cell_records(p.linear_hash_resolution, p.angular_hash_resolution, selected)) return st;
 
   // Host pass per member (Clusterizer::estimate's): the flood over the cells, then the estimate about the member's pivot.
-  const HostCell* cells = reinterpret_cast<const HostCell*>(cl_records_host_);
+  const HostCell* cells = reinterpret_cast<const HostCell*>(cl_records_host_.get());
   for (size_t j = 0; j < selected.size(); ++j) {
     const uint32_t k = selected[j];
     const Member& m = members_[k];
-    const uint32_t count = cl_cells_host_[j];
+    const uint32_t count = cl_.cells_host.get()[j];
     const ClusterSelection sel = select_cluster(cells, count, m.n, p.linear_hash_resolution, p.angular_hash_resolution, p.weight_cap_percentile);
     if (out != nullptr) estimate_from_moments(sel.moments, m.pivot, &out[k]);
     if (n_cells != nullptr) n_cells[k] = count;
@@ -412,7 +396,7 @@ int Batch::cell_records(double linear, double angular, const std::vector<uint32_
   for (uint32_t j = 0; j < n_sel; ++j) {
     const uint32_t k = selected[j];
     const Member& m = members_[k];
-    BatchClusterMember& c = cl_table_host_[j];
+    BatchClusterMember& c = cl_.table_host.get()[j];
     c = BatchClusterMember{};
     c.offset = m.offset;
     c.table_offset = m.table_offset;
@@ -424,32 +408,32 @@ int Batch::cell_records(double linear, double angular, const std::vector<uint32_
     c.pivot_y = m.pivot[1];
   }
   cudaStream_t stream = stream_;
-  BB_CHECK(cudaMemcpyAsync(cl_table_, cl_table_host_, n_sel * sizeof(BatchClusterMember), cudaMemcpyHostToDevice, stream));
+  BB_CHECK(cudaMemcpyAsync(cl_.table.get(), cl_.table_host.get(), n_sel * sizeof(BatchClusterMember), cudaMemcpyHostToDevice, stream));
   BatchClusterArgs a{};
-  a.members = cl_table_;
-  a.states[0] = states_[0];
-  a.states[1] = states_[1];
-  a.weights = weights_;
+  a.members = cl_.table.get();
+  a.states[0] = states_[0].get();
+  a.states[1] = states_[1].get();
+  a.weights = weights_.get();
   a.linear = linear;
   a.angular = angular;
-  a.hashes = cl_hashes_;
-  a.keys = cl_keys_;
-  a.first = cl_first_;
-  a.ids = cl_ids_;
-  a.cell_of = cl_cell_of_;
-  a.sort_a = cl_sort_[0];
-  a.sort_b = cl_sort_[1];
-  a.starts = cl_starts_;
-  a.records = cl_records_;
-  a.cells = cl_cells_;
+  a.hashes = cl_.hashes.get();
+  a.keys = cl_.keys.get();
+  a.first = cl_.first.get();
+  a.ids = cl_.ids.get();
+  a.cell_of = cl_.cell_of.get();
+  a.sort_a = cl_.sort[0].get();
+  a.sort_b = cl_.sort[1].get();
+  a.starts = cl_.starts.get();
+  a.records = cl_.records.get();
+  a.cells = cl_.cells.get();
   launch_batch_cluster_cells(a, n_sel, stream);
   BB_LAUNCHED("batch_cluster_cells");
-  BB_CHECK(cudaMemcpyAsync(cl_cells_host_, cl_cells_, n_sel * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+  BB_CHECK(cudaMemcpyAsync(cl_.cells_host.get(), cl_.cells.get(), n_sel * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
   BB_CHECK(cudaStreamSynchronize(stream));  // 1: the cell counts size the records' read-back
   uint64_t total_cells = 0;
-  for (uint32_t j = 0; j < n_sel; ++j) total_cells += cl_cells_host_[j];
+  for (uint32_t j = 0; j < n_sel; ++j) total_cells += cl_.cells_host.get()[j];
   if (const int st = ensure_cluster_records(total_cells)) return st;
-  launch_batch_cluster_compact(cl_table_, cl_cells_, cl_records_, n_sel, cl_records_host_, stream);
+  launch_batch_cluster_compact(cl_.table.get(), cl_.cells.get(), cl_.records.get(), n_sel, cl_records_host_.get(), stream);
   BB_LAUNCHED("batch_cluster_compact");
   BB_CHECK(cudaStreamSynchronize(stream));  // 2: every record is in pinned memory
   static_assert(sizeof(HostCell) == sizeof(CellRecord), "record layouts must agree");
@@ -468,11 +452,11 @@ int Batch::particle_histograms(double linear, double angular, const uint8_t* pre
 
   // Filter::particle_histogram's host half per member.
   static_assert(sizeof(bb200_cluster_cell) == sizeof(CellRecord), "public and internal cell records must agree");
-  const CellRecord* cells = cl_records_host_;
+  const CellRecord* cells = cl_records_host_.get();
   bool short_buffer = false;
   for (size_t j = 0; j < selected.size(); ++j) {
     const uint32_t k = selected[j];
-    const uint32_t count = cl_cells_host_[j];
+    const uint32_t count = cl_.cells_host.get()[j];
     double top = 1e-3;  // beluga_ros/particle_cloud.hpp:197
     for (uint32_t c = 0; c < count; ++c) top = cells[c].weight > top ? cells[c].weight : top;
     if (n_bins != nullptr) n_bins[k] = count;
@@ -491,20 +475,17 @@ int Batch::particle_histograms(double linear, double angular, const uint8_t* pre
 }
 
 int Batch::ensure_samples(uint64_t draws) {
-  if (sm_table_host_ == nullptr) {
+  if (sm_table_.host.get() == nullptr) {
     const size_t k = members_.size();
     sample_header_ = (k * sizeof(unsigned long long) + sizeof(Pose2) - 1) / sizeof(Pose2);
-    BB_CHECK(dev_alloc(&sm_table_, k));
-    BB_CHECK(host_alloc(&sm_table_host_, k));  // marks the table as allocated
+    SampleTable t;
+    BB_CHECK(t.device.allocate(k));
+    BB_CHECK(t.host.allocate(k));
+    sm_table_ = std::move(t);
   }
-  if (draws <= samples_capacity_) return BB200_OK;
-  cudaFree(samples_);
-  cudaFreeHost(samples_host_);
-  samples_ = samples_host_ = nullptr;
-  samples_capacity_ = 0;
   const uint64_t want = std::min<uint64_t>(total_, std::max<uint64_t>(4096, 2 * draws));  // draws <= total_
-  BB_CHECK(realloc_staged(&samples_, &samples_host_, sample_header_ + want));
-  samples_capacity_ = want;
+  BB_CHECK(samples_.grow(sample_header_ + draws, sample_header_ + want));
+  BB_CHECK(samples_host_.grow(sample_header_ + draws, sample_header_ + want));
   return BB200_OK;
 }
 
@@ -535,7 +516,7 @@ int Batch::sample_states(const uint64_t* counts, uint32_t step, const uint8_t* p
   for (uint32_t j = 0; j < n_sel; ++j) {
     const uint32_t k = drawn[j];
     const Member& m = members_[k];
-    BatchSampleMember& s = sm_table_host_[j];
+    BatchSampleMember& s = sm_table_.host.get()[j];
     s = BatchSampleMember{};
     s.offset = m.offset;
     s.n = m.n;
@@ -549,35 +530,35 @@ int Batch::sample_states(const uint64_t* counts, uint32_t step, const uint8_t* p
     uint32_t ctas[kSampleLaunches];
     batch_sample_ctas(s, s.total == 0, ctas);
     for (int l = 0; l < kSampleLaunches; ++l) {
-      first_host_[static_cast<size_t>(l) * (n_sel + 1) + j] = a.ctas[l];  // the step's range buffers are free between calls
+      first_host_.get()[static_cast<size_t>(l) * (n_sel + 1) + j] = a.ctas[l];  // the step's range buffers are free between calls
       a.ctas[l] += ctas[l];
     }
   }
-  for (int l = 0; l < kSampleLaunches; ++l) first_host_[static_cast<size_t>(l) * (n_sel + 1) + n_sel] = a.ctas[l];
+  for (int l = 0; l < kSampleLaunches; ++l) first_host_.get()[static_cast<size_t>(l) * (n_sel + 1) + n_sel] = a.ctas[l];
   cudaStream_t stream = stream_;
-  BB_CHECK(cudaMemcpyAsync(sm_table_, sm_table_host_, n_sel * sizeof(BatchSampleMember), cudaMemcpyHostToDevice, stream));
-  BB_CHECK(cudaMemcpyAsync(first_, first_host_, kSampleLaunches * (n_sel + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-  a.members = sm_table_;
-  a.first = first_;
+  BB_CHECK(cudaMemcpyAsync(sm_table_.device.get(), sm_table_.host.get(), n_sel * sizeof(BatchSampleMember), cudaMemcpyHostToDevice, stream));
+  BB_CHECK(cudaMemcpyAsync(first_.get(), first_host_.get(), kSampleLaunches * (n_sel + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+  a.members = sm_table_.device.get();
+  a.first = first_.get();
   a.step = step;
-  a.states[0] = states_[0];
-  a.states[1] = states_[1];
-  a.weights = weights_;
-  a.cdf = cdf_;
-  a.scalars = scalars_;
-  a.tile_state = tile_state_;
-  a.partials = partials_;  // the step's moment rows are free between calls
-  a.totals = reinterpret_cast<unsigned long long*>(samples_);
-  a.out = samples_ + sample_header_;
+  a.states[0] = states_[0].get();
+  a.states[1] = states_[1].get();
+  a.weights = weights_.get();
+  a.cdf = cdf_.get();
+  a.scalars = scalars_.get();
+  a.tile_state = tile_state_.get();
+  a.partials = partials_.get();  // the step's moment rows are free between calls
+  a.totals = reinterpret_cast<unsigned long long*>(samples_.get());
+  a.out = samples_.get() + sample_header_;
   launches_ += static_cast<uint64_t>(launch_batch_sample(a, stream));
   BB_CHECK(cudaGetLastError());
-  BB_CHECK(cudaMemcpyAsync(samples_host_, samples_, (sample_header_ + draws) * sizeof(Pose2), cudaMemcpyDeviceToHost, stream));
+  BB_CHECK(cudaMemcpyAsync(samples_host_.get(), samples_.get(), (sample_header_ + draws) * sizeof(Pose2), cudaMemcpyDeviceToHost, stream));
   BB_CHECK(cudaStreamSynchronize(stream));
 
-  const unsigned long long* totals = reinterpret_cast<const unsigned long long*>(samples_host_);
-  const Pose2* out = samples_host_ + sample_header_;
+  const unsigned long long* totals = reinterpret_cast<const unsigned long long*>(samples_host_.get());
+  const Pose2* out = samples_host_.get() + sample_header_;
   for (uint32_t j = 0; j < n_sel; ++j) {
-    const BatchSampleMember& s = sm_table_host_[j];
+    const BatchSampleMember& s = sm_table_.host.get()[j];
     members_[drawn[j]].cdf_total = totals[j];  // a rebuilt CDF is current until the member's particles or weights change
     std::memcpy(states_out[drawn[j]], out + s.out_offset, s.count * sizeof(Pose2));
   }
@@ -585,28 +566,22 @@ int Batch::sample_states(const uint64_t* counts, uint32_t step, const uint8_t* p
 }
 
 int Batch::ensure_points(uint64_t n_points) {
-  if (n_points <= points_capacity_) return BB200_OK;
+  if (2 * n_points <= std::min(points_.size(), points_host_.size())) return BB200_OK;
   BB_CHECK(cudaStreamSynchronize(stream_));
-  points_capacity_ = 0;
-  const uint64_t cap = std::max<uint64_t>(n_points + n_points / 2, 4096);
-  BB_CHECK(realloc_staged(&points_, &points_host_, 2 * cap));
-  points_capacity_ = cap;
+  const uint64_t room = 2 * std::max<uint64_t>(n_points + n_points / 2, 4096);
+  BB_CHECK(points_.grow(2 * n_points, room));
+  BB_CHECK(points_host_.grow(2 * n_points, room));
   return BB200_OK;
 }
 
 bool Batch::ensure_hits(uint64_t words) {
-  if (words <= hits_capacity_) return true;
   // Every batch call ends synchronised: nothing in flight reads the old buffer.
-  cudaFree(hits_);
-  hits_ = nullptr;
-  hits_capacity_ = 0;
   // words is at most one pass's worth (the caller checks), so the slack never takes the buffer past that
-  const uint64_t want = std::min<uint64_t>(std::max<uint64_t>(words + words / 2, 4096), kBeamHitPassBytes / sizeof(uint32_t));
-  if (dev_alloc(&hits_, want) != cudaSuccess) {
+  const uint64_t room = std::min<uint64_t>(std::max<uint64_t>(words + words / 2, 4096), kBeamHitPassBytes / sizeof(uint32_t));
+  if (hits_.grow(words, room) != cudaSuccess) {
     (void)cudaGetLastError();  // no room for the hit words: the fused kernel needs none
     return false;
   }
-  hits_capacity_ = want;
   return true;
 }
 
@@ -666,7 +641,7 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     const uint32_t k = active[j];
     const Member& m = members_[k];
     const bb200_step_plan& plan = plans[k];
-    BatchMember& b = table_host_[j];
+    BatchMember& b = table_host_.get()[j];
     b = BatchMember{};
     b.offset = m.offset;
     b.n = m.n;
@@ -685,7 +660,7 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     b.point_offset = point_offset;
     b.n_points = static_cast<uint32_t>(n_points[k]);
     b.points_radius = scan_radius(points_xy[k], n_points[k]);
-    if (n_points[k] > 0) std::memcpy(points_host_ + 2 * point_offset, points_xy[k], 2 * n_points[k] * sizeof(double));
+    if (n_points[k] > 0) std::memcpy(points_host_.get() + 2 * point_offset, points_xy[k], 2 * n_points[k] * sizeof(double));
     point_offset += n_points[k];
     b.hit_stride = (m.n + 31) / 32 * 32;
     if (forms[k] == kBatchBeamTwoPass) {
@@ -703,36 +678,36 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     const int form = forms[active[j]];
     a.forms |= 1 << form;
     uint32_t ctas[kBatchLaunches];
-    batch_member_ctas(table_host_[j], form, ctas);
+    batch_member_ctas(table_host_.get()[j], form, ctas);
     for (int l = 0; l < kBatchLaunches; ++l) {
-      first_host_[static_cast<size_t>(l) * (n_active + 1) + j] = a.ctas[l];
+      first_host_.get()[static_cast<size_t>(l) * (n_active + 1) + j] = a.ctas[l];
       a.ctas[l] += ctas[l];
     }
   }
-  for (int l = 0; l < kBatchLaunches; ++l) first_host_[static_cast<size_t>(l) * (n_active + 1) + n_active] = a.ctas[l];
+  for (int l = 0; l < kBatchLaunches; ++l) first_host_.get()[static_cast<size_t>(l) * (n_active + 1) + n_active] = a.ctas[l];
 
   cudaStream_t stream = stream_;
   for (const uint32_t k : active) members_[k].cdf_total = 0;  // from here on the step may have rewritten their CDFs
   seq_ = seq_ == 0x7fffffff ? 1 : seq_ + 1;
-  *ticket_host_ = 0;
-  st = check(cudaMemcpyAsync(table_, table_host_, n_active * sizeof(BatchMember), cudaMemcpyHostToDevice, stream), "upload member table");
+  *ticket_host_.get() = 0;
+  st = check(cudaMemcpyAsync(table_.get(), table_host_.get(), n_active * sizeof(BatchMember), cudaMemcpyHostToDevice, stream), "upload member table");
   if (st == BB200_OK)
-    st = check(cudaMemcpyAsync(first_, first_host_, kBatchLaunches * (n_active + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), "upload ranges");
+    st = check(cudaMemcpyAsync(first_.get(), first_host_.get(), kBatchLaunches * (n_active + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), "upload ranges");
   if (st == BB200_OK && points_total > 0)
-    st = check(cudaMemcpyAsync(points_, points_host_, 2 * points_total * sizeof(double), cudaMemcpyHostToDevice, stream), "upload points");
+    st = check(cudaMemcpyAsync(points_.get(), points_host_.get(), 2 * points_total * sizeof(double), cudaMemcpyHostToDevice, stream), "upload points");
   if (st != BB200_OK) return rollback(st);
-  a.members = table_;
-  a.first = first_;
+  a.members = table_.get();
+  a.first = first_.get();
   a.max_points = max_points;
-  a.states[0] = states_[0];
-  a.states[1] = states_[1];
-  a.weights = weights_;
-  a.cdf = cdf_;
-  a.ancestors = ancestors_;
-  a.tile_state = tile_state_;
-  a.scalars = scalars_;
-  a.partials = partials_;
-  a.points = points_;
+  a.states[0] = states_[0].get();
+  a.states[1] = states_[1].get();
+  a.weights = weights_.get();
+  a.cdf = cdf_.get();
+  a.ancestors = ancestors_.get();
+  a.tile_state = tile_state_.get();
+  a.scalars = scalars_.get();
+  a.partials = partials_.get();
+  a.points = points_.get();
   if (step_map >= 0) {
     const DeviceMap& map = maps_.at(step_map).map;
     a.field = map.field;
@@ -744,27 +719,27 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     a.occupancy = map.occupancy;
     a.beam = map.beam;
   } else {
-    a.maps = map_table_;
+    a.maps = map_table_.get();
   }
-  a.hits = hits_;
-  a.summary = summary_host_;
-  a.members_done = members_done_;
-  a.ticket = ticket_host_;
+  a.hits = hits_.get();
+  a.summary = summary_host_.get();
+  a.members_done = members_done_.get();
+  a.ticket = ticket_host_.get();
   a.seq = seq_;
   launches_ += static_cast<uint64_t>(launch_batch_step(a, stream));
   st = check(cudaGetLastError(), "batch step launch");
   if (st != BB200_OK) return rollback(st);
 
   // The last member to finish stores the ticket into pinned memory.
-  const bool done = wait_for_ticket(ticket_host_, seq_, stream);
+  const bool done = wait_for_ticket(ticket_host_.get(), seq_, stream);
   if (!done) st = check(cudaStreamSynchronize(stream), "batch step");
-  if (st == BB200_OK && !done && *static_cast<volatile int*>(ticket_host_) != seq_) st = fail(BB200_ERR_CUDA, "the batch step ended without its completion ticket");
+  if (st == BB200_OK && !done && *static_cast<volatile int*>(ticket_host_.get()) != seq_) st = fail(BB200_ERR_CUDA, "the batch step ended without its completion ticket");
   if (st != BB200_OK) return rollback(st);
 
   for (uint32_t j = 0; j < n_active; ++j) {
     const uint32_t k = active[j];
     Member& m = members_[k];
-    const StepSummary& s = summary_host_[j];
+    const StepSummary& s = summary_host_.get()[j];
     const bb200_step_plan& plan = plans[k];
     bb200_update_result& r = out[k];
     estimate_from_moments(s.moments, m.pivot, &r.estimate);

@@ -10,6 +10,7 @@
 
 #include "amcl.hpp"
 #include "cluster.cuh"
+#include "device_buffer.hpp"
 #include "device_map.hpp"
 
 namespace bb200 {
@@ -112,7 +113,7 @@ class Batch {
   /// of them has no particles.
   int select_members(const uint8_t* present, std::vector<uint32_t>* selected);
   /// Clusterizer::cell_records of every member in `selected` (non-empty): their records back to back in cl_records_host_,
-  /// member selected[j]'s count in cl_cells_host_[j].  Two launches and two host synchronisations.
+  /// member selected[j]'s count in cl_.cells_host[j].  Two launches and two host synchronisations.
   int cell_records(double linear, double angular, const std::vector<uint32_t>& selected);
   int ensure_samples(uint64_t draws);
 
@@ -121,63 +122,64 @@ class Batch {
   cudaStream_t stream_{nullptr};
   std::map<int, MapEntry> maps_;  // by id
   int next_map_id_{0};
-  BatchMap* map_table_{nullptr};  // device: one entry per map (MapEntry::slot), for steps whose members read several maps
-  size_t map_table_capacity_{0};
-  bool map_table_current_{false};  // the table and the slots match maps_
+  DeviceBuffer<BatchMap> map_table_;  // one entry per map (MapEntry::slot), for steps whose members read several maps
+  bool map_table_current_{false};     // the table and the slots match maps_
   bool created_{false};
   int create_status_{BB200_OK};
   mutable std::string error_;
   bool record_ancestors_{false};
 
   uint64_t total_{0};
-  Pose2* states_[2]{nullptr, nullptr};
-  double* weights_{nullptr};
-  unsigned long long* cdf_{nullptr};
-  long long* ancestors_{nullptr};
-  Scalars* scalars_{nullptr};
-  unsigned long long* tile_state_{nullptr};
-  double* partials_{nullptr};
-  BatchMember* table_{nullptr};       // device
-  BatchMember* table_host_{nullptr};  // pinned
-  uint32_t* first_{nullptr};          // device: kBatchLaunches x (K + 1)
-  uint32_t* first_host_{nullptr};     // pinned
-  double* points_{nullptr};
-  double* points_host_{nullptr};      // pinned
-  uint64_t points_capacity_{0};       // points (pairs)
-  uint32_t* hits_{nullptr};           // beam model, two-pass form: the step's hit words (grows only)
-  uint64_t hits_capacity_{0};         // words
-  StepSummary* summary_host_{nullptr};  // pinned, one per member of the step's table
-  int* ticket_host_{nullptr};           // pinned
-  unsigned int* members_done_{nullptr};
+  DeviceBuffer<Pose2> states_[2];
+  DeviceBuffer<double> weights_;
+  DeviceBuffer<unsigned long long> cdf_;
+  DeviceBuffer<long long> ancestors_;
+  DeviceBuffer<Scalars> scalars_;
+  DeviceBuffer<unsigned long long> tile_state_;
+  DeviceBuffer<double> partials_;
+  DeviceBuffer<BatchMember> table_;
+  PinnedBuffer<BatchMember> table_host_;
+  DeviceBuffer<uint32_t> first_;  // kBatchLaunches x (K + 1)
+  PinnedBuffer<uint32_t> first_host_;
+  DeviceBuffer<double> points_;   // (x, y) pairs
+  PinnedBuffer<double> points_host_;
+  DeviceBuffer<uint32_t> hits_;   // beam model, two-pass form: the step's hit words (grows only)
+  PinnedBuffer<StepSummary> summary_host_;  // one per member of the step's table
+  PinnedBuffer<int> ticket_host_;
+  DeviceBuffer<unsigned int> members_done_;
   int seq_{0};
   uint64_t launches_{0};
 
   // Cluster estimate scratch (allocated on first use): per-member slices of the particle-sized buffers, and the hash
   // tables back to back.
   uint64_t table_total_{0};
-  unsigned long long* cl_hashes_{nullptr};
-  unsigned long long* cl_keys_{nullptr};
-  unsigned int* cl_first_{nullptr};
-  uint32_t* cl_ids_{nullptr};
-  uint32_t* cl_cell_of_{nullptr};
-  uint32_t* cl_sort_[2]{nullptr, nullptr};
-  uint32_t* cl_starts_{nullptr};
-  CellRecord* cl_records_{nullptr};
-  BatchClusterMember* cl_table_{nullptr};       // device
-  BatchClusterMember* cl_table_host_{nullptr};  // pinned
-  uint32_t* cl_cells_{nullptr};                 // device
-  uint32_t* cl_cells_host_{nullptr};            // pinned
-  CellRecord* cl_records_host_{nullptr};        // pinned, written by the compaction kernel
-  uint64_t cl_records_host_capacity_{0};
+  struct ClusterBuffers {
+    DeviceBuffer<unsigned long long> hashes;
+    DeviceBuffer<unsigned long long> keys;
+    DeviceBuffer<unsigned int> first;
+    DeviceBuffer<uint32_t> ids;
+    DeviceBuffer<uint32_t> cell_of;
+    DeviceBuffer<uint32_t> sort[2];
+    DeviceBuffer<uint32_t> starts;
+    DeviceBuffer<CellRecord> records;
+    DeviceBuffer<BatchClusterMember> table;
+    PinnedBuffer<BatchClusterMember> table_host;
+    DeviceBuffer<uint32_t> cells;
+    PinnedBuffer<uint32_t> cells_host;
+  };
+  ClusterBuffers cl_;
+  PinnedBuffer<CellRecord> cl_records_host_;  // written by the compaction kernel
 
   // Pose-sample scratch (allocated on first use): the member table, and the draws after a header of one CDF total per
   // member (sample_header_ poses' worth), so that one copy brings both back.
-  BatchSampleMember* sm_table_{nullptr};       // device
-  BatchSampleMember* sm_table_host_{nullptr};  // pinned
+  struct SampleTable {
+    DeviceBuffer<BatchSampleMember> device;
+    PinnedBuffer<BatchSampleMember> host;
+  };
+  SampleTable sm_table_;
   uint64_t sample_header_{0};
-  Pose2* samples_{nullptr};                    // device
-  Pose2* samples_host_{nullptr};               // pinned
-  uint64_t samples_capacity_{0};               // draws
+  DeviceBuffer<Pose2> samples_;
+  PinnedBuffer<Pose2> samples_host_;
 };
 
 }  // namespace bb200

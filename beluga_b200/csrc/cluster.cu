@@ -11,7 +11,7 @@
 #include "device_common.cuh"
 
 #include <algorithm>
-#include <initializer_list>
+#include <utility>
 
 namespace bb200 {
 
@@ -389,34 +389,36 @@ uint32_t cluster_sort_tiles(uint64_t n) { return static_cast<uint32_t>((n + kSor
 void launch_cluster_cells_begin(const Pose2* states, uint64_t n, double linear_resolution, double angular_resolution, const ClusterScratch& s,
                                 cudaStream_t stream) {
   const unsigned blocks = static_cast<unsigned>((n + 255) / 256);
-  cudaMemsetAsync(s.keys, 0xFF, s.table_size * sizeof(unsigned long long), stream);
-  cudaMemsetAsync(s.first, 0xFF, s.table_size * sizeof(unsigned int), stream);
-  cluster_insert_kernel<<<blocks, 256, 0, stream>>>(states, n, linear_resolution, angular_resolution, s.hashes, s.keys, s.first, s.table_size - 1);
-  cluster_flag_kernel<<<blocks, 256, 0, stream>>>(s.hashes, n, s.keys, s.first, s.table_size - 1, s.slot_of, s.flags);
-  launch_scan_u32(s.flags, s.flags, static_cast<uint32_t>(n), s.words + 0, s.tile_state, s.words + 1, stream);
+  const uint64_t table_size = s.keys.size();
+  cudaMemsetAsync(s.keys.get(), 0xFF, table_size * sizeof(unsigned long long), stream);
+  cudaMemsetAsync(s.first.get(), 0xFF, table_size * sizeof(unsigned int), stream);
+  cluster_insert_kernel<<<blocks, 256, 0, stream>>>(states, n, linear_resolution, angular_resolution, s.hashes.get(), s.keys.get(), s.first.get(),
+                                                    table_size - 1);
+  cluster_flag_kernel<<<blocks, 256, 0, stream>>>(s.hashes.get(), n, s.keys.get(), s.first.get(), table_size - 1, s.slot_of.get(), s.flags.get());
+  launch_scan_u32(s.flags.get(), s.flags.get(), static_cast<uint32_t>(n), s.words.get() + 0, s.tile_state.get(), s.words.get() + 1, stream);
 }
 
 const uint32_t* launch_cluster_sort(uint64_t n, uint32_t cells, const ClusterScratch& s, cudaStream_t stream, int* launches) {
   const unsigned blocks = static_cast<unsigned>((n + 255) / 256);
   const uint32_t n32 = static_cast<uint32_t>(n);
-  cudaMemsetAsync(s.starts, 0, (static_cast<size_t>(cells) + 1) * sizeof(uint32_t), stream);
-  cluster_cell_of_kernel<<<blocks, 256, 0, stream>>>(s.slot_of, s.first, s.flags, n, s.cell_of, s.starts);
-  launch_scan_u32(s.starts, s.starts, cells + 1, s.words + 0, s.tile_state, nullptr, stream);
+  cudaMemsetAsync(s.starts.get(), 0, (static_cast<size_t>(cells) + 1) * sizeof(uint32_t), stream);
+  cluster_cell_of_kernel<<<blocks, 256, 0, stream>>>(s.slot_of.get(), s.first.get(), s.flags.get(), n, s.cell_of.get(), s.starts.get());
+  launch_scan_u32(s.starts.get(), s.starts.get(), cells + 1, s.words.get() + 0, s.tile_state.get(), nullptr, stream);
 
   const uint32_t tiles = cluster_sort_tiles(n);
   const int passes = std::max(1, (bits_for(cells) + 7) / 8);
-  const uint32_t* keys_in = s.cell_of;
+  const uint32_t* keys_in = s.cell_of.get();
   const uint32_t* idx_in = nullptr;  // first pass: the identity
-  uint32_t* keys_out = s.keys_a;
-  uint32_t* idx_out = s.idx_a;
+  uint32_t* keys_out = s.keys_a.get();
+  uint32_t* idx_out = s.idx_a.get();
   for (int pass = 0; pass < passes; ++pass) {
-    radix_histogram_kernel<<<tiles, kSortThreads, 0, stream>>>(keys_in, n32, 8 * pass, tiles, s.histogram);
-    launch_scan_u32(s.histogram, s.histogram, kRadix * tiles, s.words + 0, s.tile_state, nullptr, stream);
-    radix_scatter_kernel<<<tiles, kSortThreads, 0, stream>>>(keys_in, idx_in, n32, 8 * pass, tiles, s.histogram, keys_out, idx_out);
+    radix_histogram_kernel<<<tiles, kSortThreads, 0, stream>>>(keys_in, n32, 8 * pass, tiles, s.histogram.get());
+    launch_scan_u32(s.histogram.get(), s.histogram.get(), kRadix * tiles, s.words.get() + 0, s.tile_state.get(), nullptr, stream);
+    radix_scatter_kernel<<<tiles, kSortThreads, 0, stream>>>(keys_in, idx_in, n32, 8 * pass, tiles, s.histogram.get(), keys_out, idx_out);
     keys_in = keys_out;
     idx_in = idx_out;
-    keys_out = keys_out == s.keys_a ? s.keys_b : s.keys_a;
-    idx_out = idx_out == s.idx_a ? s.idx_b : s.idx_a;
+    keys_out = keys_out == s.keys_a.get() ? s.keys_b.get() : s.keys_a.get();
+    idx_out = idx_out == s.idx_a.get() ? s.idx_b.get() : s.idx_a.get();
   }
   if (launches != nullptr) *launches = 2 + 3 * passes;
   return idx_in;
@@ -425,7 +427,8 @@ const uint32_t* launch_cluster_sort(uint64_t n, uint32_t cells, const ClusterScr
 void launch_cluster_records(const Pose2* states, const double* weights, const uint32_t* sorted_idx, uint32_t cells, double pivot_x, double pivot_y,
                             const ClusterScratch& s, cudaStream_t stream) {
   const unsigned cell_blocks = static_cast<unsigned>((static_cast<uint64_t>(cells) * kWarp + kCellThreads - 1) / kCellThreads);
-  cluster_cells_kernel<<<cell_blocks, kCellThreads, 0, stream>>>(states, weights, s.hashes, sorted_idx, s.starts, cells, pivot_x, pivot_y, s.records);
+  cluster_cells_kernel<<<cell_blocks, kCellThreads, 0, stream>>>(states, weights, s.hashes.get(), sorted_idx, s.starts.get(), cells, pivot_x, pivot_y,
+                                                                  s.records.get());
 }
 
 void launch_batch_cluster_cells(const BatchClusterArgs& a, uint32_t n_members, cudaStream_t stream) {
@@ -439,44 +442,32 @@ void launch_batch_cluster_compact(const BatchClusterMember* members, const uint3
 
 // ---- Clusterizer -------------------------------------------------------------------------------------
 
-Clusterizer::~Clusterizer() {
-  for (void* p : std::initializer_list<void*>{s_.hashes, s_.keys, s_.first, s_.slot_of, s_.flags, s_.cell_of, s_.starts, s_.keys_a, s_.keys_b, s_.idx_a,
-                                              s_.idx_b, s_.histogram, s_.tile_state, s_.words, s_.records})
-    cudaFree(p);
-}
-
 int Clusterizer::ensure_scratch(uint32_t cells, std::string* error) {
   auto check = [error](cudaError_t e, const char* what) { return cuda_check(e, what, error); };
-  ClusterScratch& c = s_;
-  if (c.hashes == nullptr) {
-    if (c.capacity >= (1ull << 31)) return reject(BB200_ERR_CAPACITY, "cluster estimate: more than 2^31 particles per filter", error);
+  if (s_.hashes.get() == nullptr) {  // then the records are not allocated either
+    const uint64_t capacity = capacity_;
+    if (capacity >= (1ull << 31)) return reject(BB200_ERR_CAPACITY, "cluster estimate: more than 2^31 particles per filter", error);
     uint64_t table = 2;
-    while (table < 2 * c.capacity) table <<= 1;
-    const uint32_t tiles = cluster_sort_tiles(c.capacity);
-    BB_CHECK(dev_alloc(&c.keys, table));
-    BB_CHECK(dev_alloc(&c.first, table));
-    BB_CHECK(dev_alloc(&c.slot_of, c.capacity));
-    BB_CHECK(dev_alloc(&c.flags, c.capacity));
-    BB_CHECK(dev_alloc(&c.cell_of, c.capacity));
-    BB_CHECK(dev_alloc(&c.starts, c.capacity + 1));
-    BB_CHECK(dev_alloc(&c.keys_a, c.capacity));
-    BB_CHECK(dev_alloc(&c.keys_b, c.capacity));
-    BB_CHECK(dev_alloc(&c.idx_a, c.capacity));
-    BB_CHECK(dev_alloc(&c.idx_b, c.capacity));
-    BB_CHECK(dev_alloc(&c.histogram, static_cast<size_t>(256) * tiles));
-    BB_CHECK(dev_alloc(&c.tile_state, static_cast<size_t>(scan_tile_count(std::max<uint64_t>(c.capacity + 1, 256ull * tiles)) + 1)));
-    BB_CHECK(dev_alloc(&c.words, 4));
-    BB_CHECK(dev_alloc(&c.hashes, c.capacity));  // last: marks the scratch as allocated
-    c.table_size = table;
+    while (table < 2 * capacity) table <<= 1;
+    const uint32_t tiles = cluster_sort_tiles(capacity);
+    ClusterScratch c;
+    BB_CHECK(c.keys.allocate(table));
+    BB_CHECK(c.first.allocate(table));
+    BB_CHECK(c.slot_of.allocate(capacity));
+    BB_CHECK(c.flags.allocate(capacity));
+    BB_CHECK(c.cell_of.allocate(capacity));
+    BB_CHECK(c.starts.allocate(capacity + 1));
+    BB_CHECK(c.keys_a.allocate(capacity));
+    BB_CHECK(c.keys_b.allocate(capacity));
+    BB_CHECK(c.idx_a.allocate(capacity));
+    BB_CHECK(c.idx_b.allocate(capacity));
+    BB_CHECK(c.histogram.allocate(static_cast<size_t>(256) * tiles));
+    BB_CHECK(c.tile_state.allocate(static_cast<size_t>(scan_tile_count(std::max<uint64_t>(capacity + 1, 256ull * tiles)) + 1)));
+    BB_CHECK(c.words.allocate(4));
+    BB_CHECK(c.hashes.allocate(capacity));
+    s_ = std::move(c);
   }
-  if (cells > c.records_capacity) {
-    cudaFree(c.records);
-    c.records = nullptr;
-    c.records_capacity = 0;
-    const uint64_t want = std::min<uint64_t>(c.capacity, std::max<uint64_t>(1024, 2ull * cells));
-    BB_CHECK(dev_alloc(&c.records, want));
-    c.records_capacity = want;
-  }
+  BB_CHECK(s_.records.grow(cells, std::min<uint64_t>(capacity_, std::max<uint64_t>(1024, 2ull * cells))));
   return BB200_OK;
 }
 
@@ -494,7 +485,7 @@ int Clusterizer::cell_records(const Pose2* states, const double* weights, uint64
   launch_cluster_cells_begin(states, n, linear_resolution, angular_resolution, s_, stream);
   BB_LAUNCHED_N("cluster_cells_begin", 3);
   unsigned long long cells64 = 0;
-  BB_CHECK(cudaMemcpyAsync(&cells64, s_.words + 1, sizeof(cells64), cudaMemcpyDeviceToHost, stream));
+  BB_CHECK(cudaMemcpyAsync(&cells64, s_.words.get() + 1, sizeof(cells64), cudaMemcpyDeviceToHost, stream));
   BB_CHECK(cudaStreamSynchronize(stream));
   const uint32_t cells = static_cast<uint32_t>(cells64);
   {
@@ -510,7 +501,7 @@ int Clusterizer::cell_records(const Pose2* states, const double* weights, uint64
   BB_LAUNCHED("cluster_records");
   host->resize(cells);
   static_assert(sizeof(HostCell) == sizeof(CellRecord), "record layouts must agree");
-  BB_CHECK(cudaMemcpyAsync(host->data(), s_.records, static_cast<size_t>(cells) * sizeof(CellRecord), cudaMemcpyDeviceToHost, stream));
+  BB_CHECK(cudaMemcpyAsync(host->data(), s_.records.get(), static_cast<size_t>(cells) * sizeof(CellRecord), cudaMemcpyDeviceToHost, stream));
   BB_CHECK(cudaStreamSynchronize(stream));
   stage("end");
   return BB200_OK;
@@ -520,7 +511,7 @@ int Clusterizer::estimate(const Pose2* states, const double* weights, uint64_t n
                           bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells, uint32_t* n_clusters, std::string* error) {
   auto check = [error](cudaError_t e, const char* what) { return cuda_check(e, what, error); };
   if (n == 0) return reject(BB200_ERR_STATE, "no particles", error);
-  if (n > s_.capacity) return reject(BB200_ERR_CAPACITY, "cluster estimate: more particles than the scratch holds", error);
+  if (n > capacity_) return reject(BB200_ERR_CAPACITY, "cluster estimate: more particles than the scratch holds", error);
   if (!(p.linear_hash_resolution > 0.0) || !(p.angular_hash_resolution > 0.0) || !(p.weight_cap_percentile >= 0.0) ||
       !(p.weight_cap_percentile < 1.0))
     return reject(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)", error);
@@ -537,7 +528,7 @@ int Clusterizer::estimate(const Pose2* states, const double* weights, uint64_t n
   if (n_clusters != nullptr) *n_clusters = sel.clusters;
   if (cluster_ids != nullptr) {
     std::vector<uint32_t> cell_of(n);
-    BB_CHECK(cudaMemcpy(cell_of.data(), s_.cell_of, n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    BB_CHECK(cudaMemcpy(cell_of.data(), s_.cell_of.get(), n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     for (uint64_t i = 0; i < n; ++i) cluster_ids[i] = sel.cluster_of_cell[cell_of[i]];
   }
   return BB200_OK;

@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "cluster_host.hpp"
+#include "device_buffer.hpp"
 #include "kernels.cuh"
 
 namespace bb200 {
@@ -31,26 +32,21 @@ struct CellRecord {
 };
 static_assert(sizeof(CellRecord) == 128, "CellRecord is copied to the host as raw bytes");
 
-/// Scratch buffers of the clusterizer (owned by Clusterizer, sized for `capacity` particles).
+/// Scratch buffers of the clusterizer (owned by Clusterizer, sized for its `capacity` particles).
 struct ClusterScratch {
-  uint64_t capacity{0};
-  uint64_t table_size{0};              // power of two >= 2 * capacity
-  unsigned long long* hashes{nullptr}; // [capacity]
-  unsigned long long* keys{nullptr};   // [table_size]
-  unsigned int* first{nullptr};        // [table_size] smallest particle index per key
-  uint32_t* slot_of{nullptr};          // [capacity] table slot of each particle's cell
-  uint32_t* flags{nullptr};            // [capacity] first-occurrence flags, scanned in place
-  uint32_t* cell_of{nullptr};          // [capacity] dense cell id per particle
-  uint32_t* starts{nullptr};           // [capacity + 1] cell counts, scanned in place into segment starts
-  uint32_t* keys_a{nullptr};           // radix sort ping-pong: keys and particle indices
-  uint32_t* keys_b{nullptr};
-  uint32_t* idx_a{nullptr};
-  uint32_t* idx_b{nullptr};
-  uint32_t* histogram{nullptr};        // [256 * sort tiles]
-  unsigned long long* tile_state{nullptr};
-  unsigned long long* words{nullptr};  // [4]: scan ticket, cell count, spare
-  CellRecord* records{nullptr};
-  uint64_t records_capacity{0};
+  DeviceBuffer<unsigned long long> hashes;  // [capacity]
+  DeviceBuffer<unsigned long long> keys;    // [table size]: a power of two >= 2 * capacity
+  DeviceBuffer<unsigned int> first;         // [table size] smallest particle index per key
+  DeviceBuffer<uint32_t> slot_of;           // [capacity] table slot of each particle's cell
+  DeviceBuffer<uint32_t> flags;             // [capacity] first-occurrence flags, scanned in place
+  DeviceBuffer<uint32_t> cell_of;           // [capacity] dense cell id per particle
+  DeviceBuffer<uint32_t> starts;            // [capacity + 1] cell counts, scanned in place into segment starts
+  DeviceBuffer<uint32_t> keys_a, keys_b;    // radix sort ping-pong: keys and particle indices
+  DeviceBuffer<uint32_t> idx_a, idx_b;
+  DeviceBuffer<uint32_t> histogram;         // [256 * sort tiles]
+  DeviceBuffer<unsigned long long> tile_state;
+  DeviceBuffer<unsigned long long> words;   // [4]: scan ticket, cell count, spare
+  DeviceBuffer<CellRecord> records;         // grows with the cell count
 };
 
 uint32_t cluster_sort_tiles(uint64_t n);
@@ -114,8 +110,7 @@ void launch_batch_cluster_compact(const BatchClusterMember* members, const uint3
 /// `stream`, and returns a bb200_status with the message in *error.
 class Clusterizer {
  public:
-  explicit Clusterizer(uint64_t capacity) { s_.capacity = capacity; }
-  ~Clusterizer();
+  explicit Clusterizer(uint64_t capacity) : capacity_(capacity) {}
   Clusterizer(const Clusterizer&) = delete;
   Clusterizer& operator=(const Clusterizer&) = delete;
 
@@ -135,7 +130,8 @@ class Clusterizer {
  private:
   int ensure_scratch(uint32_t cells, std::string* error);
 
-  ClusterScratch s_{};  // allocated once `hashes` is set
+  uint64_t capacity_;
+  ClusterScratch s_;  // allocated (all but the records) once `hashes` is set
   uint64_t launches_{0};
 };
 

@@ -116,22 +116,19 @@ bool beam_two_pass_map(const MapLayout& map) {
 // ---------------------------------------------------------------------------------------------------
 
 void DeviceMap::release() {
-  for (void* p : buffers_) cudaFree(p);
-  buffers_.clear();
+  tables_ = Tables{};
   static_cast<MapLayout&>(*this) = MapLayout{};
   field_host.clear();
   free_cells = nullptr;
 }
 
 template <class T>
-cudaError_t DeviceMap::copy(const std::vector<T>& v, const T** out, cudaStream_t stream) {
-  T* p = nullptr;
-  *out = nullptr;
+cudaError_t DeviceMap::copy(const std::vector<T>& v, DeviceBuffer<T>* table, const T** view, cudaStream_t stream) {
+  *view = nullptr;
   if (v.empty()) return cudaSuccess;
-  if (const cudaError_t e = dev_alloc(&p, v.size())) return e;
-  buffers_.push_back(p);
-  *out = p;
-  return cudaMemcpyAsync(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, stream);
+  if (const cudaError_t e = table->allocate(v.size())) return e;
+  *view = table->get();
+  return cudaMemcpyAsync(table->get(), v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, stream);
 }
 
 int DeviceMap::upload(const MapTables& t, cudaStream_t stream, std::string* error) {
@@ -140,7 +137,7 @@ int DeviceMap::upload(const MapTables& t, cudaStream_t stream, std::string* erro
   release();
   static_cast<MapLayout&>(*this) = t;
   sensor = -1;  // until every table is in place
-  BB_CHECK(copy(t.bordered, &field.bordered, stream));
+  BB_CHECK(copy(t.bordered, &tables_.bordered, &field.bordered, stream));
   if (field.bordered != nullptr) {
     // The biased index of element e is e + bias modulo 2^32; it equals e + bias, and the moved-back base then finds the
     // element, only if no element's biased index passes 2^32.
@@ -148,19 +145,17 @@ int DeviceMap::upload(const MapTables& t, cudaStream_t stream, std::string* erro
     if (static_cast<uint64_t>(bias) + t.bordered.size() <= (1ull << 32))
       field.bordered_biased = reinterpret_cast<const double*>(reinterpret_cast<uintptr_t>(field.bordered) - uintptr_t{bias} * sizeof(double));
   }
-  BB_CHECK(copy(t.tiled, &field.tiled, stream));
-  BB_CHECK(copy(t.cells, &occupancy.cells, stream));
-  BB_CHECK(copy(t.free_distance, &occupancy.free_distance, stream));
-  BB_CHECK(copy(t.free_padded, &occupancy.free_padded, stream));
-  BB_CHECK(copy(t.free_cells, &free_cells, stream));
+  BB_CHECK(copy(t.tiled, &tables_.tiled, &field.tiled, stream));
+  BB_CHECK(copy(t.cells, &tables_.cells, &occupancy.cells, stream));
+  BB_CHECK(copy(t.free_distance, &tables_.free_distance, &occupancy.free_distance, stream));
+  BB_CHECK(copy(t.free_padded, &tables_.free_padded, &occupancy.free_padded, stream));
+  BB_CHECK(copy(t.free_cells, &tables_.free_cells, &free_cells, stream));
   if (t.sensor == BB200_SENSOR_BEAM) {
     if (const uint32_t entries = beam_eta_entries(beam.beam_max_range, grid_resolution)) {
-      double2* eta = nullptr;
-      BB_CHECK(dev_alloc(&eta, entries));
-      buffers_.push_back(eta);
-      launch_beam_eta_table(beam, grid_resolution, eta, entries, stream);
+      BB_CHECK(tables_.eta.allocate(entries));
+      launch_beam_eta_table(beam, grid_resolution, tables_.eta.get(), entries, stream);
       BB_LAUNCHED("beam_eta_table");
-      beam.eta = eta;
+      beam.eta = tables_.eta.get();
       beam.eta_entries = entries;
     }
   }

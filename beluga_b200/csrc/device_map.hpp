@@ -7,6 +7,7 @@
 #include <string>
 #include <vector>
 
+#include "device_buffer.hpp"
 #include "kernels.cuh"
 
 namespace bb200 {
@@ -49,7 +50,6 @@ bool beam_two_pass_map(const MapLayout& map);
 /// One device's copy of the current map.
 struct DeviceMap : MapLayout {
   DeviceMap() = default;
-  ~DeviceMap() { release(); }
   DeviceMap(const DeviceMap&) = delete;
   DeviceMap& operator=(const DeviceMap&) = delete;
 
@@ -66,9 +66,16 @@ struct DeviceMap : MapLayout {
  private:
   void release();
   template <class T>
-  cudaError_t copy(const std::vector<T>& v, const T** out, cudaStream_t stream);
+  cudaError_t copy(const std::vector<T>& v, DeviceBuffer<T>* table, const T** view, cudaStream_t stream);
 
-  std::vector<void*> buffers_;  // every device allocation of the current map
+  struct Tables {  // the device tables of the current map, one per view (an empty host table leaves both null)
+    DeviceBuffer<double> bordered, tiled;
+    DeviceBuffer<int8_t> cells;
+    DeviceBuffer<uint8_t> free_distance, free_padded;
+    DeviceBuffer<uint32_t> free_cells;
+    DeviceBuffer<double2> eta;  // beam model: normaliser table
+  };
+  Tables tables_;
   uint64_t launches_{0};
 };
 

@@ -4,7 +4,7 @@
 #include <atomic>
 #include <cmath>
 #include <cstring>
-#include <initializer_list>
+#include <utility>
 
 #include "cluster_host.hpp"
 
@@ -116,47 +116,43 @@ Filter::Filter(const bb200_filter_config& config) : config_(config), cluster_(co
   first_index_ = config.first_index;
   BB_TRY(cudaSetDevice(config.device));
   BB_TRY(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-  BB_TRY(dev_alloc(&states_[0], capacity_));
-  BB_TRY(dev_alloc(&states_[1], capacity_));
-  BB_TRY(dev_alloc(&weights_, capacity_));
-  BB_TRY(dev_alloc(&cdf_, capacity_));
-  if (config.record_ancestors) BB_TRY(dev_alloc(&ancestors_, capacity_));
-  BB_TRY(dev_alloc(&scalars_, 1));
-  BB_TRY(cudaMallocHost(reinterpret_cast<void**>(&scalars_host_), sizeof(Scalars)));
-  tile_capacity_ = scan_tile_count(capacity_) + 1;
-  BB_TRY(dev_alloc(&tile_state_, tile_capacity_));
-  partials_rows_ = std::max(std::max(resample_block_count(capacity_), moments_block_count(capacity_)), kSmCount * 8u);
-  BB_TRY(dev_alloc(&partials_, static_cast<size_t>(partials_rows_) * kMomentCount));
-  BB_TRY(dev_alloc(&results_, 16));
-  BB_TRY(cudaMallocHost(reinterpret_cast<void**>(&results_host_), 16 * sizeof(double)));
-  BB_TRY(dev_alloc(&sched_, 1));
-  BB_TRY(dev_alloc(&bins_, capacity_));
-  BB_TRY(dev_alloc(&bin_rank_, capacity_));
-  BB_TRY(dev_alloc(&perm_, capacity_));
-  BB_TRY(dev_alloc(&counters_, schedule_max_bins()));
-  BB_TRY(dev_alloc(&sched_tiles_, schedule_tile_count()));
-  BB_TRY(dev_alloc(&mail_, 1));  // its own allocation: exported to peer processes through CUDA IPC
-  BB_TRY(dev_alloc(&shard_totals_, kMaxShards));
-  BB_TRY(dev_alloc(&summary_, 1));
-  BB_TRY(cudaMallocHost(reinterpret_cast<void**>(&summary_host_), sizeof(StepSummary)));
-  std::memset(summary_host_, 0, sizeof(StepSummary));  // pinned allocations are recycled with their old contents (a stale completion ticket)
-  BB_TRY(cudaMemsetAsync(mail_, 0, sizeof(ShardMail), stream_));
-  BB_TRY(cudaMemsetAsync(summary_, 0, sizeof(StepSummary), stream_));
-  BB_TRY(cudaMemsetAsync(scalars_, 0, sizeof(Scalars), stream_));
+  BB_TRY(states_[0].allocate(capacity_));
+  BB_TRY(states_[1].allocate(capacity_));
+  BB_TRY(weights_.allocate(capacity_));
+  BB_TRY(cdf_.allocate(capacity_));
+  if (config.record_ancestors) BB_TRY(ancestors_.allocate(capacity_));
+  BB_TRY(scalars_.allocate(1));
+  BB_TRY(scalars_host_.allocate(1));
+  BB_TRY(tile_state_.allocate(scan_tile_count(capacity_) + 1));
+  const uint32_t partial_rows = std::max(std::max(resample_block_count(capacity_), moments_block_count(capacity_)), kSmCount * 8u);
+  BB_TRY(partials_.allocate(static_cast<size_t>(partial_rows) * kMomentCount));
+  BB_TRY(results_.allocate(16));
+  BB_TRY(results_host_.allocate(16));
+  BB_TRY(sched_.allocate(1));
+  BB_TRY(bins_.allocate(capacity_));
+  BB_TRY(bin_rank_.allocate(capacity_));
+  BB_TRY(perm_.allocate(capacity_));
+  BB_TRY(counters_.allocate(schedule_max_bins()));
+  BB_TRY(sched_tiles_.allocate(schedule_tile_count()));
+  BB_TRY(mail_.allocate(1));  // its own allocation: exported to peer processes through CUDA IPC
+  BB_TRY(shard_totals_.allocate(kMaxShards));
+  BB_TRY(summary_.allocate(1));
+  BB_TRY(summary_host_.allocate(1));
+  std::memset(summary_host_.get(), 0, sizeof(StepSummary));  // pinned allocations are recycled with their old contents (a stale completion ticket)
+  BB_TRY(cudaMemsetAsync(mail_.get(), 0, sizeof(ShardMail), stream_));
+  BB_TRY(cudaMemsetAsync(summary_.get(), 0, sizeof(StepSummary), stream_));
+  BB_TRY(cudaMemsetAsync(scalars_.get(), 0, sizeof(Scalars), stream_));
   BB_TRY(cudaStreamSynchronize(stream_));
   global_size_ = config_.global_count;
   created_ = true;
 }
 
 Filter::~Filter() {
+  // Before the members free this filter's buffers (after this body): nothing in flight may read them, and the peers'
+  // buffers mapped here are closed first (CUDA IPC requires importers to close before the exporter frees).
   if (stream_ != nullptr) cudaStreamSynchronize(stream_);
   release_peers();
   for (auto& e : event_pool_) cudaEventDestroy(e);
-  for (void* p : std::initializer_list<void*>{mail_, shard_totals_, summary_, states_[0], states_[1], weights_, cdf_, ancestors_, hashes_, scalars_,
-                                              sched_, bins_, bin_rank_, perm_, counters_, sched_tiles_, tile_state_, partials_, results_, kld_keys_,
-                                              kld_vals_, kld_flags_, kld_scan_, kld_tile_state_, kld_hashes_global_, points_, beam_hits_})
-    cudaFree(p);
-  for (void* p : std::initializer_list<void*>{summary_host_, scalars_host_, results_host_, points_host_}) cudaFreeHost(p);
   if (stream_ != nullptr && owns_stream_) cudaStreamDestroy(stream_);
 }
 
@@ -224,7 +220,7 @@ int Filter::enqueue_propagate_reweight(const bb200_motion_sampling* sampling, ui
   MotionSampling s{};
   if (sampling != nullptr) s = to_kernel_sampling(*sampling);
   mark("begin_step");
-  launch_begin_step(scalars_, stream_);
+  launch_begin_step(scalars_.get(), stream_);
   BB_LAUNCHED("begin_step");
   const int st = enqueue_propagate_reweight_kernels(sampling != nullptr ? &s : nullptr, step, do_reweight, n_points, false);
   cdf_valid_ = false;
@@ -235,9 +231,9 @@ int Filter::enqueue_propagate_reweight(const bb200_motion_sampling* sampling, ui
 int Filter::enqueue_max_weight() {
   if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
   BB_CHECK(cudaSetDevice(config_.device));
-  launch_begin_step(scalars_, stream_);
+  launch_begin_step(scalars_.get(), stream_);
   BB_LAUNCHED("begin_step");
-  launch_max_weight(weights_, n_, scalars_, stream_);
+  launch_max_weight(weights_.get(), n_, scalars_.get(), stream_);
   BB_LAUNCHED("max_weight");
   return BB200_OK;
 }
@@ -246,10 +242,10 @@ int Filter::enqueue_build_cdf(double global_wmax) {
   if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
   BB_CHECK(cudaSetDevice(config_.device));
   mark("prepare_cdf");
-  launch_prepare_cdf(scalars_, global_wmax, config_.global_count, tile_state_, scan_tile_count(n_), stream_);
+  launch_prepare_cdf(scalars_.get(), global_wmax, config_.global_count, tile_state_.get(), scan_tile_count(n_), stream_);
   BB_LAUNCHED("prepare_cdf");
   mark("quantize_scan");
-  launch_quantize_scan(weights_, n_, cdf_, scalars_, tile_state_, stream_);
+  launch_quantize_scan(weights_.get(), n_, cdf_.get(), scalars_.get(), tile_state_.get(), stream_);
   BB_LAUNCHED("quantize_scan");
   cdf_valid_ = true;
   return BB200_OK;
@@ -271,7 +267,7 @@ int Filter::enqueue_resample_range(const bb200_resample_opts& o, uint64_t global
     a.cdf_offset = cdf_offset;
     a.weights_out = nullptr;  // the current weights stay untouched; adopt() writes the ones
     mark("resample_range");
-    launch_resample(a, scalars_, partials_, stream_);
+    launch_resample(a, scalars_.get(), partials_.get(), stream_);
     BB_LAUNCHED("resample_range");
   }
   return BB200_OK;
@@ -287,7 +283,7 @@ int Filter::enqueue_adopt(uint64_t n) {
   cdf_valid_ = false;
   if (n > 0) {
     mark("fill_weights");
-    launch_fill(weights_, n, 1.0, stream_);
+    launch_fill(weights_.get(), n, 1.0, stream_);
     BB_LAUNCHED("fill_weights");
   }
   return BB200_OK;
@@ -301,9 +297,9 @@ int Filter::enqueue_moments(const double pivot[2]) {
 
 int Filter::enqueue_moment_kernels(const double pivot[2]) {
   mark("moments");
-  launch_moments(states_[cur_], weights_, n_, pivot[0], pivot[1], partials_, stream_);
+  launch_moments(states_[cur_].get(), weights_.get(), n_, pivot[0], pivot[1], partials_.get(), stream_);
   BB_LAUNCHED("moments");
-  launch_reduce_partials(partials_, moments_block_count(n_), kMomentCount, results_, stream_);
+  launch_reduce_partials(partials_.get(), moments_block_count(n_), kMomentCount, results_.get(), stream_);
   BB_LAUNCHED("reduce_partials");
   return BB200_OK;
 }
@@ -335,10 +331,10 @@ int Filter::leave_shards() {
 }
 
 int Filter::enable_shard_kld() {
-  if (kld_hashes_global_ != nullptr) return BB200_OK;
+  if (kld_hashes_global_.get() != nullptr) return BB200_OK;
   if (peer_world_ != 0) return fail(BB200_ERR_STATE, "KLD on shards must be enabled before the shards are joined");
   BB_CHECK(cudaSetDevice(config_.device));
-  BB_CHECK(dev_alloc(&kld_hashes_global_, config_.global_count));  // one spatial hash per candidate slot of the WHOLE filter
+  BB_CHECK(kld_hashes_global_.allocate(config_.global_count));  // one spatial hash per candidate slot of the WHOLE filter
   return BB200_OK;
 }
 
@@ -347,10 +343,10 @@ int Filter::export_shard(void* out256) {
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "four IPC handles are exported as 256 bytes");
   cudaIpcMemHandle_t h[4];
   std::memset(h, 0, sizeof(h));
-  BB_CHECK(cudaIpcGetMemHandle(&h[0], states_[0]));
-  BB_CHECK(cudaIpcGetMemHandle(&h[1], states_[1]));
-  BB_CHECK(cudaIpcGetMemHandle(&h[2], mail_));
-  if (kld_hashes_global_ != nullptr) BB_CHECK(cudaIpcGetMemHandle(&h[3], kld_hashes_global_));
+  BB_CHECK(cudaIpcGetMemHandle(&h[0], states_[0].get()));
+  BB_CHECK(cudaIpcGetMemHandle(&h[1], states_[1].get()));
+  BB_CHECK(cudaIpcGetMemHandle(&h[2], mail_.get()));
+  if (kld_hashes_global_.get() != nullptr) BB_CHECK(cudaIpcGetMemHandle(&h[3], kld_hashes_global_.get()));
   std::memcpy(out256, h, sizeof(h));
   return BB200_OK;
 }
@@ -367,16 +363,16 @@ int Filter::join_shards_ipc(int world, int rank, const void* handles) {
   peer_rank_ = rank;
   for (int r = 0; r < world; ++r) {
     if (r == rank) {
-      peer_states_[0][r] = states_[0];
-      peer_states_[1][r] = states_[1];
-      peer_mail_[r] = mail_;
-      peer_kld_hashes_[r] = kld_hashes_global_;
+      peer_states_[0][r] = states_[0].get();
+      peer_states_[1][r] = states_[1].get();
+      peer_mail_[r] = mail_.get();
+      peer_kld_hashes_[r] = kld_hashes_global_.get();
       continue;
     }
     static const cudaIpcMemHandle_t kNoHandle{};
     void* p[4] = {nullptr, nullptr, nullptr, nullptr};
     for (int b = 0; b < 4; ++b) {
-      if (b == 3 && (kld_hashes_global_ == nullptr || std::memcmp(&all[4 * r + 3], &kNoHandle, sizeof(kNoHandle)) == 0)) continue;  // no KLD on this filter
+      if (b == 3 && (kld_hashes_global_.get() == nullptr || std::memcmp(&all[4 * r + 3], &kNoHandle, sizeof(kNoHandle)) == 0)) continue;  // no KLD on this filter
       const int st = check(cudaIpcOpenMemHandle(&p[b], all[4 * r + b], cudaIpcMemLazyEnablePeerAccess), "cudaIpcOpenMemHandle");
       if (st != BB200_OK) {
         peer_states_[0][r] = static_cast<Pose2*>(p[0]);
@@ -391,7 +387,7 @@ int Filter::join_shards_ipc(int world, int rank, const void* handles) {
     peer_mail_[r] = static_cast<ShardMail*>(p[2]);
     peer_kld_hashes_[r] = static_cast<unsigned long long*>(p[3]);
   }
-  shard_kld_ = kld_hashes_global_ != nullptr;
+  shard_kld_ = kld_hashes_global_.get() != nullptr;
   for (int r = 0; r < world; ++r) shard_kld_ = shard_kld_ && peer_kld_hashes_[r] != nullptr;
   split_posts_ = false;  // every rank has its own host thread: post and wait travel in one launch
   return BB200_OK;
@@ -420,13 +416,13 @@ int Filter::join_shards_local(Filter* const* filters, int world) {
         if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) return fa->check(e, "cudaDeviceEnablePeerAccess");
         (void)cudaGetLastError();
       }
-      fa->peer_states_[0][b] = fb->states_[0];
-      fa->peer_states_[1][b] = fb->states_[1];
-      fa->peer_mail_[b] = fb->mail_;
-      fa->peer_kld_hashes_[b] = fb->kld_hashes_global_;
+      fa->peer_states_[0][b] = fb->states_[0].get();
+      fa->peer_states_[1][b] = fb->states_[1].get();
+      fa->peer_mail_[b] = fb->mail_.get();
+      fa->peer_kld_hashes_[b] = fb->kld_hashes_global_.get();
     }
     fa->shard_kld_ = true;
-    for (int b = 0; b < world; ++b) fa->shard_kld_ = fa->shard_kld_ && filters[b]->kld_hashes_global_ != nullptr;
+    for (int b = 0; b < world; ++b) fa->shard_kld_ = fa->shard_kld_ && filters[b]->kld_hashes_global_.get() != nullptr;
     fa->peer_world_ = world;
     fa->peer_rank_ = a;
     fa->peers_ipc_ = false;
@@ -444,12 +440,12 @@ int Filter::enqueue_exchange(int kind, bool post, bool wait) {
   a.world = peer_world_;
   a.epoch = epoch_;
   for (int r = 0; r < peer_world_; ++r) a.peers[r] = peer_mail_[r];
-  a.scalars = scalars_;
-  a.results = results_;
-  a.summary = summary_host_;  // pinned host memory: the step's results need no copy
-  a.rank_totals = shard_totals_;
+  a.scalars = scalars_.get();
+  a.results = results_.get();
+  a.summary = summary_host_.get();  // pinned host memory: the step's results need no copy
+  a.rank_totals = shard_totals_.get();
   a.ceil_log2_count = ceil_log2_count(config_.global_count);
-  a.tile_state = tile_state_;
+  a.tile_state = tile_state_.get();
   a.n_tiles = scan_tile_count(n_);
   launch_shard_exchange(a, stream_);
   BB_LAUNCHED("shard_exchange");
@@ -475,7 +471,7 @@ int Filter::step_begin(const bb200_motion_sampling& sampling, uint32_t step, con
   const int st = upload_points(points_xy, n_points);
   if (st != BB200_OK) return st;
   step_ = StepContext{};
-  summary_host_->error = 0;
+  summary_host_.get()->error = 0;
   step_.active = true;
   step_.sampling = to_kernel_sampling(sampling);
   step_.step = step;
@@ -499,8 +495,9 @@ int Filter::step_phase(int phase) {
       {
         const bool scheduled = n_ >= kScheduleMinParticles;
         const bool warm = map_.sensor != BB200_SENSOR_BEAM && map_.field.use_fixed && map_.bordered_bytes <= (96ull << 20);
-        launch_begin_fused_step(scalars_, tile_state_, scan_tile_count(n_), sched_, scheduled ? counters_ : nullptr, schedule_max_bins(), sched_tiles_,
-                                schedule_tile_count(), warm ? map_.field.bordered : nullptr, map_.bordered_bytes, stream_);
+        launch_begin_fused_step(scalars_.get(), tile_state_.get(), scan_tile_count(n_), sched_.get(), scheduled ? counters_.get() : nullptr,
+                                schedule_max_bins(), sched_tiles_.get(), schedule_tile_count(), warm ? map_.field.bordered : nullptr,
+                                map_.bordered_bytes, stream_);
         BB_LAUNCHED("begin_step");
         st = enqueue_propagate_reweight_kernels(&step_.sampling, step_.step, true, step_.n_points, scheduled);
       }
@@ -523,12 +520,12 @@ int Filter::step_phase(int phase) {
       mark("quantize_scan");
       // one GPU: the exponent comes from the shard's own largest weight inside the kernel (scan state reset by begin_step);
       // sharded: the exchange above has set the common exponent and reset the scan state
-      launch_quantize_scan(weights_, n_, cdf_, scalars_, tile_state_, stream_, !sharded, config_.global_count);
+      launch_quantize_scan(weights_.get(), n_, cdf_.get(), scalars_.get(), tile_state_.get(), stream_, !sharded, config_.global_count);
       BB_LAUNCHED("quantize_scan");
       if (sharded) {
         if (step_.resample_planned) {  // the CDF holds what sampling needs; every new particle weighs 1 (overlaps the wait for the peers' totals)
           mark("fill_weights");
-          launch_fill(weights_, capacity_, 1.0, stream_);
+          launch_fill(weights_.get(), capacity_, 1.0, stream_);
           BB_LAUNCHED("fill_weights");
           step_.weights_filled = true;
         }
@@ -558,7 +555,7 @@ int Filter::step_phase(int phase) {
         a.ancestors = nullptr;
         a.peer_count = peer_world_;
         a.peer_shard = accepted != 0 ? (accepted + static_cast<uint64_t>(peer_world_) - 1) / static_cast<uint64_t>(peer_world_) : capacity_;
-        a.rank_totals = shard_totals_;
+        a.rank_totals = shard_totals_.get();
         a.rank = peer_rank_;
         a.world = peer_world_;
         if (accepted != 0) {  // the comb still spans max_particles slots; only [0, accepted) are kept
@@ -574,7 +571,7 @@ int Filter::step_phase(int phase) {
         for (int r = 0; r < peer_world_; ++r) a.peer_out[r] = peer_states_[cur_ ^ 1][r];
         if (!step_.weights_filled) {
           mark("fill_weights");
-          launch_fill(weights_, capacity_, 1.0, stream_);  // the CDF holds what sampling needs; every new particle weighs 1
+          launch_fill(weights_.get(), capacity_, 1.0, stream_);  // the CDF holds what sampling needs; every new particle weighs 1
           BB_LAUNCHED("fill_weights");
           step_.weights_filled = true;
         }
@@ -588,10 +585,10 @@ int Filter::step_phase(int phase) {
       if (!sharded && !timing_) {
         step_seq_ = step_seq_ == 0x7fffffff ? 1 : step_seq_ + 1;
         step_.poll_seq = step_seq_;
-        summary_host_->seq = 0;  // nothing of this filter is in flight: the previous step was seen to end
+        summary_host_.get()->seq = 0;  // nothing of this filter is in flight: the previous step was seen to end
       }
-      a.tail = StepTail{1, results_, sharded ? nullptr : summary_host_, step_.poll_seq};
-      step_.partial_rows = launch_resample(a, scalars_, partials_, stream_);
+      a.tail = StepTail{1, results_.get(), sharded ? nullptr : summary_host_.get(), step_.poll_seq};
+      step_.partial_rows = launch_resample(a, scalars_.get(), partials_.get(), stream_);
       BB_LAUNCHED("resample");
       step_.resampled = true;
       if (sharded && split_posts_) {
@@ -607,7 +604,7 @@ int Filter::step_phase(int phase) {
         if (st != BB200_OK) return st;
       } else if (!step_.resampled) {  // kPhaseNormalize left the moments in results_: hand them to the host block
         mark("readback");
-        launch_write_summary(results_, scalars_, summary_host_, stream_);
+        launch_write_summary(results_.get(), scalars_.get(), summary_host_.get(), stream_);
         BB_LAUNCHED("write_summary");
       }
       mark("end");
@@ -623,7 +620,7 @@ int Filter::step_phase(int phase) {
       }
       uint32_t rows = 0;
       mark("normalize");
-      launch_normalize(weights_, n_, scalars_, sharded ? ~0ull : 0ull, partials_, &rows, stream_);  // actions/normalize.hpp:82
+      launch_normalize(weights_.get(), n_, scalars_.get(), sharded ? ~0ull : 0ull, partials_.get(), &rows, stream_);  // actions/normalize.hpp:82
       BB_LAUNCHED("normalize");
       st = enqueue_moment_kernels(pivot_);  // a KLD-sized shard may be empty here
       if (st != BB200_OK) return st;
@@ -645,26 +642,18 @@ int Filter::kld_sharded_candidates(uint64_t begin, uint64_t end) {
   if (end <= begin || end > config_.global_count) return fail(BB200_ERR_INVALID_ARGUMENT, "KLD on shards: bad slot window");
   BB_CHECK(cudaSetDevice(config_.device));
   const bb200_resample_opts& o = step_.opts;
-  if (kld_keys_ == nullptr) {  // the counting pass runs over ALL slots on every rank: tables sized for the whole filter
-    const uint64_t n = config_.global_count;
-    BB_CHECK(dev_alloc(&kld_flags_, n));
-    BB_CHECK(dev_alloc(&kld_scan_, n));
-    kld_table_size_ = 2;
-    while (kld_table_size_ < 2 * n) kld_table_size_ <<= 1;
-    BB_CHECK(dev_alloc(&kld_keys_, kld_table_size_));
-    BB_CHECK(dev_alloc(&kld_vals_, kld_table_size_));
-    BB_CHECK(dev_alloc(&kld_tile_state_, static_cast<size_t>(scan_tile_count(n)) + 1));
-  }
+  // the counting pass runs over ALL slots on every rank: tables sized for the whole filter
+  if (const int st = ensure_kld_tables(config_.global_count, true)) return st;
   if (begin == 0) {
     mark("kld");
-    launch_kld_clear(kld_keys_, kld_vals_, kld_table_size_, stream_);
+    launch_kld_clear(kld_.keys.get(), kld_.vals.get(), kld_.keys.size(), stream_);
   }
   const bool systematic = o.scheme == BB200_RESAMPLE_SYSTEMATIC;
   ResampleArgs a = make_resample_args(o, 0, std::min<uint64_t>(end - begin, capacity_), false);
   a.states_out = nullptr;
   a.weights_out = nullptr;
   a.ancestors = nullptr;
-  a.rank_totals = shard_totals_;
+  a.rank_totals = shard_totals_.get();
   a.rank = peer_rank_;
   a.world = peer_world_;
   a.window_begin = begin;
@@ -679,7 +668,7 @@ int Filter::kld_sharded_candidates(uint64_t begin, uint64_t end) {
     a.slot_count = end - begin;
   }
   mark("kld_candidates");
-  launch_resample(a, scalars_, partials_, stream_);
+  launch_resample(a, scalars_.get(), partials_.get(), stream_);
   BB_LAUNCHED("kld_candidates");
   ++epoch_;
   if (split_posts_) return enqueue_exchange(kExchangeKld, true, false);
@@ -694,19 +683,19 @@ int Filter::kld_sharded_count(uint64_t begin, uint64_t end, uint64_t k_before) {
   const int st = enqueue_exchange(kExchangeKld, !split_posts_, true);  // every rank's hashes of this window have arrived
   if (st != BB200_OK) return st;
   mark("kld");
-  KldArgs k{kld_hashes_global_ + begin, end - begin, begin, k_before, o.min_particles, o.kld_epsilon, o.kld_z};
-  launch_kld_chunk(k, kld_keys_, kld_vals_, kld_table_size_, kld_flags_, kld_scan_, scalars_, kld_tile_state_, stream_);
+  KldArgs k{kld_hashes_global_.get() + begin, end - begin, begin, k_before, o.min_particles, o.kld_epsilon, o.kld_z};
+  launch_kld_chunk(k, kld_.keys.get(), kld_.vals.get(), kld_.keys.size(), kld_.flags.get(), kld_.scan.get(), scalars_.get(), kld_.tile_state.get(), stream_);
   BB_LAUNCHED_N("kld", 5);
-  BB_CHECK(cudaMemcpyAsync(scalars_host_, scalars_, sizeof(Scalars), cudaMemcpyDeviceToHost, stream_));
+  BB_CHECK(cudaMemcpyAsync(scalars_host_.get(), scalars_.get(), sizeof(Scalars), cudaMemcpyDeviceToHost, stream_));
   return BB200_OK;
 }
 
 int Filter::kld_sharded_read(uint64_t* cutoff, uint64_t* new_buckets) {
   BB_CHECK(cudaSetDevice(config_.device));
   BB_CHECK(cudaStreamSynchronize(stream_));
-  if (scalars_host_->exchange_error != 0) return fail(BB200_ERR_STATE, "shard exchange timed out during the KLD count");
-  *cutoff = scalars_host_->kld_cutoff;
-  *new_buckets = scalars_host_->pad[1];
+  if (scalars_host_.get()->exchange_error != 0) return fail(BB200_ERR_STATE, "shard exchange timed out during the KLD count");
+  *cutoff = scalars_host_.get()->kld_cutoff;
+  *new_buckets = scalars_host_.get()->pad[1];
   return BB200_OK;
 }
 
@@ -721,9 +710,9 @@ int Filter::step_totals(uint64_t* rank_totals, int* exponent) {
   }
   if (rank_totals == nullptr) return BB200_OK;  // enqueue only
   BB_CHECK(cudaStreamSynchronize(stream_));
-  if (summary_host_->error != 0) return fail(BB200_ERR_STATE, "shard exchange timed out");
-  for (int r = 0; r < peer_world_; ++r) rank_totals[r] = summary_host_->rank_totals[r];
-  if (exponent != nullptr) *exponent = summary_host_->exponent;
+  if (summary_host_.get()->error != 0) return fail(BB200_ERR_STATE, "shard exchange timed out");
+  for (int r = 0; r < peer_world_; ++r) rank_totals[r] = summary_host_.get()->rank_totals[r];
+  if (exponent != nullptr) *exponent = summary_host_.get()->exponent;
   return BB200_OK;
 }
 
@@ -734,19 +723,19 @@ int Filter::step_end(bb200_estimate* est, double* weight_sum, uint64_t* new_size
   BB_CHECK(cudaSetDevice(config_.device));
   // The resample kernel's last block stores the summary to pinned memory and then the step's ticket.  Everything later on
   // this stream is ordered behind that kernel anyway.
-  const bool done = step_.poll_seq != 0 && step_.resampled && wait_for_ticket(&summary_host_->seq, step_.poll_seq, stream_);
+  const bool done = step_.poll_seq != 0 && step_.resampled && wait_for_ticket(&summary_host_.get()->seq, step_.poll_seq, stream_);
   if (!done) BB_CHECK(cudaStreamSynchronize(stream_));
   step_.poll_seq = 0;
   finish_marks();
   const bool sharded = peer_world_ > 1;
-  if (summary_host_->error != 0) {
+  if (summary_host_.get()->error != 0) {
     step_.active = false;
     return fail(BB200_ERR_STATE, "shard exchange timed out: a peer rank never posted its value for this step");
   }
-  const double* moments = summary_host_->moments;
-  step_.total = summary_host_->total;
-  step_.exponent = summary_host_->exponent;
-  weights_valid_ = summary_host_->valid != 0;
+  const double* moments = summary_host_.get()->moments;
+  step_.total = summary_host_.get()->total;
+  step_.exponent = summary_host_.get()->exponent;
+  weights_valid_ = summary_host_.get()->valid != 0;
   if (step_.resampled) {
     cur_ ^= 1;
     n_ = sharded ? capacity_ : step_.opts.max_particles;
@@ -788,12 +777,12 @@ int Filter::synchronize() {
 
 int Filter::device_pointer(int which, void** ptr, uint64_t* bytes) {
   switch (which) {
-    case 0: *ptr = states_[cur_]; *bytes = capacity_ * sizeof(Pose2); return BB200_OK;
-    case 1: *ptr = weights_; *bytes = capacity_ * sizeof(double); return BB200_OK;
-    case 2: *ptr = cdf_; *bytes = capacity_ * sizeof(unsigned long long); return BB200_OK;
-    case 3: *ptr = states_[cur_ ^ 1]; *bytes = capacity_ * sizeof(Pose2); return BB200_OK;
-    case 4: *ptr = scalars_; *bytes = sizeof(Scalars); return BB200_OK;
-    case 5: *ptr = results_; *bytes = 16 * sizeof(double); return BB200_OK;
+    case 0: *ptr = states_[cur_].get(); *bytes = capacity_ * sizeof(Pose2); return BB200_OK;
+    case 1: *ptr = weights_.get(); *bytes = capacity_ * sizeof(double); return BB200_OK;
+    case 2: *ptr = cdf_.get(); *bytes = capacity_ * sizeof(unsigned long long); return BB200_OK;
+    case 3: *ptr = states_[cur_ ^ 1].get(); *bytes = capacity_ * sizeof(Pose2); return BB200_OK;
+    case 4: *ptr = scalars_.get(); *bytes = sizeof(Scalars); return BB200_OK;
+    case 5: *ptr = results_.get(); *bytes = 16 * sizeof(double); return BB200_OK;
     default: return fail(BB200_ERR_INVALID_ARGUMENT, "unknown device pointer id");
   }
 }
@@ -833,12 +822,12 @@ int Filter::set_particles(const double* states, const double* weights, uint64_t 
   BB_CHECK(cudaSetDevice(config_.device));
   BB_CHECK(cudaStreamSynchronize(stream_));
   if (n > 0) {
-    BB_CHECK(cudaMemcpy(states_[cur_], states, n * sizeof(Pose2), cudaMemcpyHostToDevice));
+    BB_CHECK(cudaMemcpy(states_[cur_].get(), states, n * sizeof(Pose2), cudaMemcpyHostToDevice));
     if (weights != nullptr) {
-      BB_CHECK(cudaMemcpy(weights_, weights, n * sizeof(double), cudaMemcpyHostToDevice));
+      BB_CHECK(cudaMemcpy(weights_.get(), weights, n * sizeof(double), cudaMemcpyHostToDevice));
     } else {
       const std::vector<double> ones(n, 1.0);
-      BB_CHECK(cudaMemcpy(weights_, ones.data(), n * sizeof(double), cudaMemcpyHostToDevice));
+      BB_CHECK(cudaMemcpy(weights_.get(), ones.data(), n * sizeof(double), cudaMemcpyHostToDevice));
     }
   }
   n_ = n;
@@ -855,8 +844,8 @@ int Filter::get_particles(double* states, double* weights, uint64_t capacity) {
   BB_CHECK(cudaSetDevice(config_.device));
   BB_CHECK(cudaStreamSynchronize(stream_));
   const uint64_t n = std::min(capacity, n_);
-  if (states != nullptr && n > 0) BB_CHECK(cudaMemcpy(states, states_[cur_], n * sizeof(Pose2), cudaMemcpyDeviceToHost));
-  if (weights != nullptr && n > 0) BB_CHECK(cudaMemcpy(weights, weights_, n * sizeof(double), cudaMemcpyDeviceToHost));
+  if (states != nullptr && n > 0) BB_CHECK(cudaMemcpy(states, states_[cur_].get(), n * sizeof(Pose2), cudaMemcpyDeviceToHost));
+  if (weights != nullptr && n > 0) BB_CHECK(cudaMemcpy(weights, weights_.get(), n * sizeof(double), cudaMemcpyDeviceToHost));
   return BB200_OK;
 }
 
@@ -866,7 +855,7 @@ int Filter::initialize_normal(const double mean[3], const double cov[9], uint64_
   std::string message;
   if (!normal_transform(cov, transform, &message)) return fail(BB200_ERR_INVALID_ARGUMENT, message);
   BB_CHECK(cudaSetDevice(config_.device));
-  launch_initialize_normal(states_[cur_], weights_, n, mean, transform, config_.seed, first_index_, stream_);
+  launch_initialize_normal(states_[cur_].get(), weights_.get(), n, mean, transform, config_.seed, first_index_, stream_);
   BB_LAUNCHED("initialize_normal");
   BB_CHECK(cudaStreamSynchronize(stream_));
   n_ = n;
@@ -886,7 +875,7 @@ int Filter::initialize_uniform(uint64_t n) {
   if (map_.sensor < 0) return fail(BB200_ERR_STATE, "initialize_from_map needs a map (set_*_map first)");
   if (map_.n_free == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
   BB_CHECK(cudaSetDevice(config_.device));
-  launch_initialize_uniform(states_[cur_], weights_, n, map_.free_cells, map_.n_free, map_.grid_width, map_.grid_resolution, map_.grid_origin,
+  launch_initialize_uniform(states_[cur_].get(), weights_.get(), n, map_.free_cells, map_.n_free, map_.grid_width, map_.grid_resolution, map_.grid_origin,
                             config_.seed, first_index_, stream_);
   BB_LAUNCHED("initialize_uniform");
   BB_CHECK(cudaStreamSynchronize(stream_));
@@ -900,12 +889,9 @@ int Filter::initialize_uniform(uint64_t n) {
 // ---- per-step operations -----------------------------------------------------------------------------
 
 int Filter::upload_points(const double* points_xy, uint64_t n_points) {
-  if (n_points > points_capacity_) {
-    points_capacity_ = 0;
-    const uint64_t cap = std::max<uint64_t>(n_points, 2048);
-    BB_CHECK(realloc_staged(&points_, &points_host_, 2 * cap));
-    points_capacity_ = cap;
-  }
+  const uint64_t room = 2 * std::max<uint64_t>(n_points, 2048);
+  BB_CHECK(points_.grow(2 * n_points, room));
+  BB_CHECK(points_host_.grow(2 * n_points, room));
   double range_sum = 0.0;
   for (uint64_t i = 0; i < n_points; ++i) {
     const double e = std::hypot(points_xy[2 * i], points_xy[2 * i + 1]);
@@ -915,8 +901,8 @@ int Filter::upload_points(const double* points_xy, uint64_t n_points) {
   points_mean_range_ = n_points > 0 ? range_sum / static_cast<double>(n_points) : 1.0;  // lever arm of the heading in the schedule
   if (n_points > 0) {
     // The previous step's copy must have left the staging buffer before it is overwritten.
-    std::memcpy(points_host_, points_xy, 2 * n_points * sizeof(double));
-    BB_CHECK(cudaMemcpyAsync(points_, points_host_, 2 * n_points * sizeof(double), cudaMemcpyHostToDevice, stream_));
+    std::memcpy(points_host_.get(), points_xy, 2 * n_points * sizeof(double));
+    BB_CHECK(cudaMemcpyAsync(points_.get(), points_host_.get(), 2 * n_points * sizeof(double), cudaMemcpyHostToDevice, stream_));
   }
   return BB200_OK;
 }
@@ -946,23 +932,24 @@ int Filter::enqueue_propagate_reweight_kernels(const MotionSampling* sampling, u
   if (scheduled && counters_reset && sampling != nullptr && predict_schedule(*sampling, &grid)) {
     // Bin grid predicted on the host: propagate histograms its own output, two more launches turn it into the order.
     mark("propagate");
-    launch_propagate_binned(states_[cur_], n_, *sampling, config_.seed, step, first_index_, grid, bin_rank_, counters_, sched_, stream_);
+    launch_propagate_binned(states_[cur_].get(), n_, *sampling, config_.seed, step, first_index_, grid, bin_rank_.get(), counters_.get(), sched_.get(), stream_);
     BB_LAUNCHED("propagate");
     mark("schedule");
-    launch_finish_schedule(bin_rank_, n_, grid.n_bins, sched_, counters_, perm_, sched_tiles_, stream_);
+    launch_finish_schedule(bin_rank_.get(), n_, grid.n_bins, sched_.get(), counters_.get(), perm_.get(), sched_tiles_.get(), stream_);
     BB_LAUNCHED_N("schedule", 2);
-    perm = perm_;
+    perm = perm_.get();
   } else if (sampling != nullptr || scheduled) {
     mark("propagate");
-    launch_propagate(states_[cur_], n_, sampling != nullptr, sampling != nullptr ? *sampling : MotionSampling{}, config_.seed, step,
-                     first_index_, scheduled ? sched_ : nullptr, stream_);
+    launch_propagate(states_[cur_].get(), n_, sampling != nullptr, sampling != nullptr ? *sampling : MotionSampling{}, config_.seed, step,
+                     first_index_, scheduled ? sched_.get() : nullptr, stream_);
     BB_LAUNCHED_N("propagate", scheduled ? 2 : 1);
   }
   if (scheduled && perm == nullptr) {
     mark("schedule");
-    launch_build_schedule(states_[cur_], n_, sched_, bins_, counters_, perm_, sched_tiles_, points_mean_range_, 0.5 * map_.grid_resolution, stream_);
+    launch_build_schedule(states_[cur_].get(), n_, sched_.get(), bins_.get(), counters_.get(), perm_.get(), sched_tiles_.get(), points_mean_range_,
+                          0.5 * map_.grid_resolution, stream_);
     BB_LAUNCHED_N("schedule", 4);
-    perm = perm_;
+    perm = perm_.get();
   }
   if (do_reweight) {
     if (map_.sensor == BB200_SENSOR_BEAM) {
@@ -972,34 +959,30 @@ int Filter::enqueue_propagate_reweight_kernels(const MotionSampling* sampling, u
         // hit words of one pass: at most kBeamHitPassBytes, whole warps of particles
         pass = std::min<uint64_t>(n_, std::max<uint64_t>(32, (kBeamHitPassBytes / (4ull * n_points)) / 32 * 32));
         const uint64_t words = beam_hit_words(pass, static_cast<uint32_t>(n_points));
-        if (words > beam_hits_words_) {
+        if (words > beam_hits_.size()) {
           BB_CHECK(cudaStreamSynchronize(stream_));
-          cudaFree(beam_hits_);
-          beam_hits_ = nullptr;
-          beam_hits_words_ = 0;
           // sized for the filter's capacity so that a growing particle count (KLD) does not reallocate every step
           const uint64_t pass_cap = std::min<uint64_t>(capacity_, std::max<uint64_t>(32, (kBeamHitPassBytes / (4ull * n_points)) / 32 * 32));
           const uint64_t want = beam_hit_words(std::max(pass, pass_cap), static_cast<uint32_t>(n_points));
-          if (dev_alloc(&beam_hits_, want) == cudaSuccess) {
-            beam_hits_words_ = want;
-          } else {
+          if (beam_hits_.grow(words, want) != cudaSuccess) {
             (void)cudaGetLastError();  // no room for the intermediate: the fused kernel needs none
             pass = 0;
           }
         }
       }
       if (pass > 0) {
-        launch_reweight_beam_two_pass(states_[cur_], weights_, n_, perm, map_.occupancy, map_.beam, points_, static_cast<uint32_t>(n_points), beam_hits_, pass,
-                                      scalars_, stream_);
+        launch_reweight_beam_two_pass(states_[cur_].get(), weights_.get(), n_, perm, map_.occupancy, map_.beam, points_.get(), static_cast<uint32_t>(n_points),
+                                      beam_hits_.get(), pass, scalars_.get(), stream_);
         BB_LAUNCHED_N("reweight_beam", 2 * static_cast<int>((n_ + pass - 1) / pass));
       } else {
-        launch_reweight_beam(states_[cur_], weights_, n_, perm, map_.occupancy, map_.beam, points_, static_cast<uint32_t>(n_points), scalars_, stream_);
+        launch_reweight_beam(states_[cur_].get(), weights_.get(), n_, perm, map_.occupancy, map_.beam, points_.get(), static_cast<uint32_t>(n_points),
+                             scalars_.get(), stream_);
         BB_LAUNCHED("reweight_beam");
       }
     } else {
       mark("reweight_lfm");
-      launch_reweight_lfm(states_[cur_], weights_, n_, perm, map_.field, points_, points_host_, static_cast<uint32_t>(n_points),
-                          points_radius_, scalars_, stream_);
+      launch_reweight_lfm(states_[cur_].get(), weights_.get(), n_, perm, map_.field, points_.get(), points_host_.get(), static_cast<uint32_t>(n_points),
+                          points_radius_, scalars_.get(), stream_);
       BB_LAUNCHED("reweight_lfm");
     }
   }
@@ -1018,10 +1001,10 @@ int Filter::propagate_reweight(const bb200_motion_sampling* sampling, uint32_t s
 int Filter::max_weight(double* wmax) {
   const int st = enqueue_max_weight();
   if (st != BB200_OK) return st;
-  BB_CHECK(cudaMemcpyAsync(scalars_host_, scalars_, sizeof(Scalars), cudaMemcpyDeviceToHost, stream_));
+  BB_CHECK(cudaMemcpyAsync(scalars_host_.get(), scalars_.get(), sizeof(Scalars), cudaMemcpyDeviceToHost, stream_));
   BB_CHECK(cudaStreamSynchronize(stream_));
   double v;
-  std::memcpy(&v, &scalars_host_->wmax_bits, sizeof(double));
+  std::memcpy(&v, &scalars_host_.get()->wmax_bits, sizeof(double));
   *wmax = v;
   return BB200_OK;
 }
@@ -1031,14 +1014,14 @@ int Filter::build_cdf(double global_wmax, uint64_t* local_total, int* exponent) 
   if (global_wmax < 0.0) st = enqueue_max_weight();  // no global value: the exponent from this filter's own largest weight
   if (st == BB200_OK) st = enqueue_build_cdf(global_wmax);
   if (st != BB200_OK) return st;
-  BB_CHECK(cudaMemcpyAsync(scalars_host_, scalars_, sizeof(Scalars), cudaMemcpyDeviceToHost, stream_));
+  BB_CHECK(cudaMemcpyAsync(scalars_host_.get(), scalars_.get(), sizeof(Scalars), cudaMemcpyDeviceToHost, stream_));
   BB_CHECK(cudaStreamSynchronize(stream_));
   finish_marks();
-  if (local_total != nullptr) *local_total = scalars_host_->total;
-  if (exponent != nullptr) *exponent = scalars_host_->exponent;
+  if (local_total != nullptr) *local_total = scalars_host_.get()->total;
+  if (exponent != nullptr) *exponent = scalars_host_.get()->exponent;
   // No positive finite weight (the reference would divide by zero in normalize.hpp:82): a uniform CDF
   // has been substituted and the weights are left as they are; reported through last_error only.
-  weights_valid_ = scalars_host_->valid != 0;
+  weights_valid_ = scalars_host_.get()->valid != 0;
   if (!weights_valid_) error_ = "no positive finite weight (uniform CDF substituted)";
   return BB200_OK;
 }
@@ -1049,14 +1032,14 @@ int Filter::normalize_by(uint64_t global_total, double* local_sum_sq) {
   BB_CHECK(cudaSetDevice(config_.device));
   uint32_t rows = 0;
   mark("normalize");
-  launch_normalize(weights_, n_, scalars_, global_total, partials_, &rows, stream_);
+  launch_normalize(weights_.get(), n_, scalars_.get(), global_total, partials_.get(), &rows, stream_);
   BB_LAUNCHED("normalize");
-  launch_reduce_partials(partials_, rows, 1, results_, stream_);
+  launch_reduce_partials(partials_.get(), rows, 1, results_.get(), stream_);
   BB_LAUNCHED("reduce_partials");
-  BB_CHECK(cudaMemcpyAsync(results_host_, results_, sizeof(double), cudaMemcpyDeviceToHost, stream_));
+  BB_CHECK(cudaMemcpyAsync(results_host_.get(), results_.get(), sizeof(double), cudaMemcpyDeviceToHost, stream_));
   BB_CHECK(cudaStreamSynchronize(stream_));
   finish_marks();
-  if (local_sum_sq != nullptr) *local_sum_sq = results_host_[0];
+  if (local_sum_sq != nullptr) *local_sum_sq = results_host_.get()[0];
   return BB200_OK;
 }
 
@@ -1077,10 +1060,10 @@ int Filter::ensure_cdf_ready() {
 int Filter::moments(const double pivot[2], double out[9]) {
   const int st = enqueue_moments(pivot);
   if (st != BB200_OK) return st;
-  BB_CHECK(cudaMemcpyAsync(results_host_, results_, kMomentCount * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+  BB_CHECK(cudaMemcpyAsync(results_host_.get(), results_.get(), kMomentCount * sizeof(double), cudaMemcpyDeviceToHost, stream_));
   BB_CHECK(cudaStreamSynchronize(stream_));
   finish_marks();
-  std::memcpy(out, results_host_, kMomentCount * sizeof(double));
+  std::memcpy(out, results_host_.get(), kMomentCount * sizeof(double));
   return BB200_OK;
 }
 
@@ -1098,7 +1081,7 @@ int Filter::estimate(bb200_estimate* out) {
 int Filter::cluster_estimate(const bb200_cluster_param& p, bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity, uint32_t* n_cells,
                              uint32_t* n_clusters) {
   BB_CHECK(cudaSetDevice(config_.device));
-  const int st = cluster_.estimate(states_[cur_], weights_, n_, pivot_, p, stream_, out, cluster_ids, ids_capacity, n_cells, n_clusters, &error_);
+  const int st = cluster_.estimate(states_[cur_].get(), weights_.get(), n_, pivot_, p, stream_, out, cluster_ids, ids_capacity, n_cells, n_clusters, &error_);
   if (st == BB200_OK) finish_marks();
   return st;
 }
@@ -1109,7 +1092,7 @@ int Filter::particle_histogram(double linear_resolution, double angular_resoluti
   if (!(linear_resolution > 0.0) || !(angular_resolution > 0.0)) return fail(BB200_ERR_INVALID_ARGUMENT, "histogram resolutions must be positive");
   BB_CHECK(cudaSetDevice(config_.device));
   std::vector<HostCell> host;
-  const int st = cluster_.cell_records(states_[cur_], weights_, n_, pivot_, linear_resolution, angular_resolution, stream_, &host, &error_);
+  const int st = cluster_.cell_records(states_[cur_].get(), weights_.get(), n_, pivot_, linear_resolution, angular_resolution, stream_, &host, &error_);
   if (st != BB200_OK) return st;
   finish_marks();
   if (n_bins != nullptr) *n_bins = host.size();
@@ -1142,22 +1125,22 @@ int Filter::sample_states(uint64_t count, uint32_t step, double* states_out) {
   ResampleArgs a = make_resample_args(o, 0, count, false);
   a.weights_out = nullptr;  // the weights stay what they are
   a.ancestors = nullptr;
-  launch_resample(a, scalars_, partials_, stream_);  // into the staging state buffer; no flip
+  launch_resample(a, scalars_.get(), partials_.get(), stream_);  // into the staging state buffer; no flip
   BB_LAUNCHED("sample_states");
-  BB_CHECK(cudaMemcpyAsync(states_out, states_[cur_ ^ 1], count * sizeof(Pose2), cudaMemcpyDeviceToHost, stream_));
+  BB_CHECK(cudaMemcpyAsync(states_out, states_[cur_ ^ 1].get(), count * sizeof(Pose2), cudaMemcpyDeviceToHost, stream_));
   BB_CHECK(cudaStreamSynchronize(stream_));
   return BB200_OK;
 }
 
 ResampleArgs Filter::make_resample_args(const bb200_resample_opts& o, uint64_t slot_begin, uint64_t slot_end, bool with_hashes) const {
   ResampleArgs a{};
-  a.states_in = states_[cur_];
-  a.cdf = cdf_;
+  a.states_in = states_[cur_].get();
+  a.cdf = cdf_.get();
   a.n_in = n_;
-  a.states_out = states_[cur_ ^ 1] + slot_begin;
-  a.weights_out = weights_ + slot_begin;
-  a.ancestors = ancestors_ != nullptr ? ancestors_ + slot_begin : nullptr;
-  a.hashes = with_hashes ? hashes_ + slot_begin : nullptr;
+  a.states_out = states_[cur_ ^ 1].get() + slot_begin;
+  a.weights_out = weights_.get() + slot_begin;
+  a.ancestors = ancestors_.get() != nullptr ? ancestors_.get() + slot_begin : nullptr;
+  a.hashes = with_hashes ? kld_.hashes.get() + slot_begin : nullptr;
   a.slot_first = first_index_ + slot_begin;
   a.slot_count = slot_end - slot_begin;
   a.total_slots = o.max_particles;
@@ -1188,7 +1171,7 @@ int Filter::resample(const bb200_resample_opts& o, uint64_t* new_size) {
   if (o.min_particles >= o.max_particles) {
     // take_while_kld never stops before max when min == max (take_while_kld.hpp:86-87,136).
     mark("resample");
-    launch_resample(make_resample_args(o, 0, o.max_particles, false), scalars_, partials_, stream_);
+    launch_resample(make_resample_args(o, 0, o.max_particles, false), scalars_.get(), partials_.get(), stream_);
     BB_LAUNCHED("resample");
     BB_CHECK(cudaStreamSynchronize(stream_));
   } else {
@@ -1222,38 +1205,46 @@ int Filter::adopt(uint64_t n, int from_staging) {
   return BB200_OK;
 }
 
+int Filter::ensure_kld_tables(uint64_t slots, bool sharded) {
+  // A filter takes one of the two paths for its whole life (one GPU: global_count == capacity; shards: more).
+  if ((sharded ? kld_.tile_state : kld_.hashes).get() != nullptr) return BB200_OK;
+  KldTables t;
+  if (!sharded) BB_CHECK(t.hashes.allocate(slots));
+  BB_CHECK(t.flags.allocate(slots));
+  BB_CHECK(t.scan.allocate(slots));
+  uint64_t table_size = 2;
+  while (table_size < 2 * slots) table_size <<= 1;
+  BB_CHECK(t.keys.allocate(table_size));
+  BB_CHECK(t.vals.allocate(table_size));
+  if (sharded) BB_CHECK(t.tile_state.allocate(static_cast<size_t>(scan_tile_count(slots)) + 1));
+  kld_ = std::move(t);
+  return BB200_OK;
+}
+
 int Filter::resample_kld(const bb200_resample_opts& o, uint64_t* accepted) {
   if (config_.global_count != capacity_ || first_index_ != 0) return fail(BB200_ERR_STATE, "KLD-adaptive resampling runs on a single shard");
   if (o.max_particles >= (1ull << 32)) return fail(BB200_ERR_CAPACITY, "KLD-adaptive resampling keeps 32-bit slot indices: max_particles must be below 2^32");
-  if (hashes_ == nullptr) {
-    BB_CHECK(dev_alloc(&hashes_, capacity_));
-    BB_CHECK(dev_alloc(&kld_flags_, capacity_));
-    BB_CHECK(dev_alloc(&kld_scan_, capacity_));
-    kld_table_size_ = 2;
-    while (kld_table_size_ < 2 * capacity_) kld_table_size_ <<= 1;
-    BB_CHECK(dev_alloc(&kld_keys_, kld_table_size_));
-    BB_CHECK(dev_alloc(&kld_vals_, kld_table_size_));
-  }
+  if (const int st = ensure_kld_tables(capacity_, false)) return st;
   mark("kld");
-  launch_kld_clear(kld_keys_, kld_vals_, kld_table_size_, stream_);
+  launch_kld_clear(kld_.keys.get(), kld_.vals.get(), kld_.keys.size(), stream_);
   const uint64_t max = o.max_particles;
   uint64_t begin = 0, k_before = 0;
   uint64_t end = std::min<uint64_t>(max, std::max<uint64_t>(2 * o.min_particles, 65536));
   *accepted = max;
   while (begin < max) {
-    launch_resample(make_resample_args(o, begin, end, true), scalars_, partials_, stream_);
+    launch_resample(make_resample_args(o, begin, end, true), scalars_.get(), partials_.get(), stream_);
     BB_LAUNCHED("resample");
-    KldArgs k{hashes_ + begin, end - begin, begin, k_before, o.min_particles, o.kld_epsilon, o.kld_z};
-    launch_kld_chunk(k, kld_keys_, kld_vals_, kld_table_size_, kld_flags_, kld_scan_, scalars_, tile_state_, stream_);
+    KldArgs k{kld_.hashes.get() + begin, end - begin, begin, k_before, o.min_particles, o.kld_epsilon, o.kld_z};
+    launch_kld_chunk(k, kld_.keys.get(), kld_.vals.get(), kld_.keys.size(), kld_.flags.get(), kld_.scan.get(), scalars_.get(), tile_state_.get(), stream_);
     BB_LAUNCHED_N("kld", 5);
-    BB_CHECK(cudaMemcpyAsync(scalars_host_, scalars_, sizeof(Scalars), cudaMemcpyDeviceToHost, stream_));
+    BB_CHECK(cudaMemcpyAsync(scalars_host_.get(), scalars_.get(), sizeof(Scalars), cudaMemcpyDeviceToHost, stream_));
     BB_CHECK(cudaStreamSynchronize(stream_));
-    if (scalars_host_->kld_cutoff != ~0ull) {
+    if (scalars_host_.get()->kld_cutoff != ~0ull) {
       // take_while drops the first element whose condition fails (take_while_kld.hpp:134-136).
-      *accepted = std::min<uint64_t>(scalars_host_->kld_cutoff - 1, max);
+      *accepted = std::min<uint64_t>(scalars_host_.get()->kld_cutoff - 1, max);
       break;
     }
-    k_before += scalars_host_->pad[1];
+    k_before += scalars_host_.get()->pad[1];
     begin = end;
     end = std::min<uint64_t>(max, end * 2);
   }
@@ -1272,11 +1263,11 @@ int Filter::step_resample(const bb200_motion_sampling& sampling, uint32_t step, 
 }
 
 int Filter::ancestors(int64_t* out, uint64_t capacity) {
-  if (ancestors_ == nullptr) return fail(BB200_ERR_STATE, "filter was created without record_ancestors");
+  if (ancestors_.get() == nullptr) return fail(BB200_ERR_STATE, "filter was created without record_ancestors");
   BB_CHECK(cudaSetDevice(config_.device));
   BB_CHECK(cudaStreamSynchronize(stream_));
   const uint64_t n = std::min(capacity, ancestors_n_);
-  if (n > 0) BB_CHECK(cudaMemcpy(out, ancestors_, n * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  if (n > 0) BB_CHECK(cudaMemcpy(out, ancestors_.get(), n * sizeof(int64_t), cudaMemcpyDeviceToHost));
   return BB200_OK;
 }
 
@@ -1285,7 +1276,7 @@ int Filter::cdf(uint64_t* out, uint64_t capacity) {
   BB_CHECK(cudaSetDevice(config_.device));
   BB_CHECK(cudaStreamSynchronize(stream_));
   const uint64_t n = std::min(capacity, n_);
-  if (n > 0) BB_CHECK(cudaMemcpy(out, cdf_, n * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+  if (n > 0) BB_CHECK(cudaMemcpy(out, cdf_.get(), n * sizeof(uint64_t), cudaMemcpyDeviceToHost));
   return BB200_OK;
 }
 

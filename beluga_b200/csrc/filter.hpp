@@ -12,6 +12,7 @@
 
 #include "../../include/beluga_b200.h"
 #include "cluster.cuh"
+#include "device_buffer.hpp"
 #include "device_map.hpp"
 #include "kernels.cuh"
 
@@ -154,6 +155,8 @@ class Filter {
   bool predict_schedule(const MotionSampling& s, Schedule* grid) const;
   int ensure_cdf_ready();
   int resample_kld(const bb200_resample_opts& o, uint64_t* accepted);
+  /// The KLD tables for `slots` candidate slots, all or none (the one-GPU hashes, or the shards' scan state).
+  int ensure_kld_tables(uint64_t slots, bool sharded);
   ResampleArgs make_resample_args(const bb200_resample_opts& o, uint64_t slot_begin, uint64_t slot_end, bool with_hashes) const;
   void mark(const char* name);  // timing: record an event before the next kernel
   void finish_marks();
@@ -188,71 +191,68 @@ class Filter {
   bool owns_stream_{true};
   int peer_world_{0}, peer_rank_{0};
   Pose2* peer_states_[2][8]{};  // [buffer][rank]: the peers' ping-pong state buffers mapped into this process
-  ShardMail* mail_{nullptr};                 // this rank's mail block
+  DeviceBuffer<ShardMail> mail_;             // this rank's mail block
   ShardMail* peer_mail_[kMaxShards]{};       // every rank's mail block as seen from here ([rank] = mail_)
   bool peers_ipc_{false};                    // the peer pointers came from cudaIpcOpenMemHandle
   bool split_posts_{false};                  // post and wait as separate launches (several shards enqueued by one thread)
   unsigned long long epoch_{0};              // sequence number of the next exchange (all ranks count alike)
-  unsigned long long* shard_totals_{nullptr};  // device: the ranks' fixed-point totals of this step
-  StepSummary* summary_{nullptr};            // device
-  StepSummary* summary_host_{nullptr};       // pinned
+  DeviceBuffer<unsigned long long> shard_totals_;  // the ranks' fixed-point totals of this step
+  DeviceBuffer<StepSummary> summary_;
+  PinnedBuffer<StepSummary> summary_host_;
 
   // particle set (ping-pong states for the resample gather)
   uint64_t capacity_{0}, n_{0};
   uint64_t first_index_{0};   // global index of local particle 0 (moves when a KLD-sized filter re-splits its particles)
   uint64_t global_size_{0};   // particles over all shards
-  Pose2* states_[2]{nullptr, nullptr};
+  DeviceBuffer<Pose2> states_[2];
   int cur_{0};
-  double* weights_{nullptr};
-  unsigned long long* cdf_{nullptr};
-  long long* ancestors_{nullptr};
+  DeviceBuffer<double> weights_;
+  DeviceBuffer<unsigned long long> cdf_;
+  DeviceBuffer<long long> ancestors_;
   uint64_t ancestors_n_{0};
-  unsigned long long* hashes_{nullptr};
   bool cdf_valid_{false};
   bool weights_valid_{true};
 
   // scratch
-  Scalars* scalars_{nullptr};
-  Scalars* scalars_host_{nullptr};  // pinned
-  unsigned long long* tile_state_{nullptr};
-  uint32_t tile_capacity_{0};
-  double* partials_{nullptr};
-  uint32_t partials_rows_{0};
-  double* results_{nullptr};       // device: kMomentCount + extras
-  double* results_host_{nullptr};  // pinned
+  DeviceBuffer<Scalars> scalars_;
+  PinnedBuffer<Scalars> scalars_host_;
+  DeviceBuffer<unsigned long long> tile_state_;
+  DeviceBuffer<double> partials_;
+  DeviceBuffer<double> results_;      // kMomentCount + extras
+  PinnedBuffer<double> results_host_;
 
   Clusterizer cluster_;
 
-  // KLD scratch
-  unsigned long long* kld_keys_{nullptr};
-  unsigned int* kld_vals_{nullptr};
-  uint64_t kld_table_size_{0};
-  uint32_t* kld_flags_{nullptr};
-  uint32_t* kld_scan_{nullptr};
-  unsigned long long* kld_tile_state_{nullptr};
-  unsigned long long* kld_hashes_global_{nullptr};          // KLD on shards: spatial hash of every candidate slot (all ranks hold all)
+  // KLD scratch, allocated on first use for the slots of one pass (capacity_ on one GPU, global_count on shards)
+  struct KldTables {
+    DeviceBuffer<unsigned long long> hashes;      // one GPU: spatial hash of each candidate slot
+    DeviceBuffer<uint32_t> flags, scan;
+    DeviceBuffer<unsigned long long> keys;        // hash set of a power of two >= 2 * slots entries
+    DeviceBuffer<unsigned int> vals;
+    DeviceBuffer<unsigned long long> tile_state;  // shards: scan state of the count (one GPU uses tile_state_)
+  };
+  KldTables kld_;
+  DeviceBuffer<unsigned long long> kld_hashes_global_;  // KLD on shards: spatial hash of every candidate slot (all ranks hold all)
   unsigned long long* peer_kld_hashes_[kMaxShards]{};
   bool shard_kld_{false};
 
   // measurement
-  double* points_{nullptr};
-  double* points_host_{nullptr};  // pinned staging
-  uint64_t points_capacity_{0};
+  DeviceBuffer<double> points_;
+  PinnedBuffer<double> points_host_;  // staging
   double points_radius_{0.0};
   double points_mean_range_{1.0};
 
   // execution schedule (pose-sorted processing order of the reweight kernels)
   static constexpr uint64_t kScheduleMinParticles = 32768;
-  Schedule* sched_{nullptr};
-  uint32_t* bins_{nullptr};
-  uint2* bin_rank_{nullptr};
-  uint32_t* perm_{nullptr};
-  uint32_t* counters_{nullptr};
-  unsigned long long* sched_tiles_{nullptr};
+  DeviceBuffer<Schedule> sched_;
+  DeviceBuffer<uint32_t> bins_;
+  DeviceBuffer<uint2> bin_rank_;
+  DeviceBuffer<uint32_t> perm_;
+  DeviceBuffer<uint32_t> counters_;
+  DeviceBuffer<unsigned long long> sched_tiles_;
 
   DeviceMap map_;
-  uint32_t* beam_hits_{nullptr};   // two-pass beam model: hit word per (beam, particle) of one pass
-  uint64_t beam_hits_words_{0};
+  DeviceBuffer<uint32_t> beam_hits_;  // two-pass beam model: hit word per (beam, particle) of one pass
 
   double pivot_[2]{0.0, 0.0};
   bb200_estimate cloud_{};     // last estimate, when it describes the raw (unit-weight) cloud

@@ -171,26 +171,8 @@ constexpr int kMomentCount = 9;  // sum w, sum w^2, sum w c, sum w s, sum w dx, 
 /// that the per-block partial sums (and with them the rounding of the moments) do not depend on the part.
 constexpr uint32_t kSmCount = 132;
 
-// ---- host side of the owners of device buffers (Filter, Batch, DeviceMap, Clusterizer) ---------------------
+// ---- host side of the owners of device buffers (Filter, Batch, DeviceMap, Clusterizer; device_buffer.hpp) ---------
 
-/// cudaMalloc / cudaMallocHost of `count` elements (at least one, so that an empty table still has an address).
-template <class T>
-cudaError_t dev_alloc(T** p, size_t count) {
-  return cudaMalloc(reinterpret_cast<void**>(p), (count > 1 ? count : 1) * sizeof(T));
-}
-template <class T>
-cudaError_t host_alloc(T** p, size_t count) {
-  return cudaMallocHost(reinterpret_cast<void**>(p), (count > 1 ? count : 1) * sizeof(T));
-}
-/// A device buffer and its pinned staging copy with room for `count` elements each; the old contents are dropped.
-template <class T>
-cudaError_t realloc_staged(T** dev, T** host, size_t count) {
-  cudaFree(*dev);
-  cudaFreeHost(*host);
-  *dev = *host = nullptr;
-  const cudaError_t e = dev_alloc(dev, count);
-  return e != cudaSuccess ? e : host_alloc(host, count);
-}
 /// `status` with `message` in *error.
 inline int reject(int status, const char* message, std::string* error) {
   *error = message;

@@ -58,7 +58,7 @@ __global__ void __launch_bounds__(256) begin_fused_step_kernel(StepReset r) {
   }
   for (uint32_t k = t; k < r.n_tiles; k += stride) r.tile_state[k] = 0;
   if (r.counters != nullptr) {
-    uint4* c4 = reinterpret_cast<uint4*>(r.counters);  // cudaMalloc alignment; n_counters is a multiple of 4
+    uint4* c4 = reinterpret_cast<uint4*>(r.counters);  // device allocations are 256-byte aligned; n_counters is a multiple of 4
     for (uint32_t k = t; k < r.n_counters / 4; k += stride) c4[k] = make_uint4(0u, 0u, 0u, 0u);
     for (uint32_t k = t; k < r.n_sched_tiles; k += stride) r.sched_tiles[k] = 0;
   }

@@ -158,7 +158,7 @@ Amcl::Amcl(const bb200_amcl_param& p, const bb200_motion_param& motion)
     : policy_(p, motion),
       filter_(bb200_filter_config{p.device, p.shard_capacity != 0 ? p.shard_capacity : p.max_particles, p.seed, p.shard_first_index, p.max_particles,
                                   p.record_ancestors}) {
-  if (sharded() && p.min_particles < p.max_particles && filter_.ok()) (void)filter_.enable_shard_kld();
+  if (sharded() && p.min_particles < p.max_particles && filter_.ok()) (void)filter_.link().enable_kld();
 }
 
 int Amcl::initialized(int status, bool has_particles) {
@@ -200,10 +200,10 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
   const bool kld = lead.params().min_particles < lead.params().max_particles;
   if (kld)
     for (int r = 0; r < count; ++r)
-      if (!ranks[r]->filter_.shard_kld())
+      if (!ranks[r]->filter_.link().kld())
         return ranks[r]->filter_.fail_with(BB200_ERR_STATE, "KLD-adaptive resampling on shards: the hash arrays were not exported (create the shards with min_particles < max_particles before joining them)");
   for (int r = 0; r < count; ++r)
-    if (ranks[r]->sharded() && ranks[r]->filter_.shard_world() <= 1)
+    if (ranks[r]->sharded() && ranks[r]->filter_.link().world() <= 1)
       return ranks[r]->filter_.fail_with(BB200_ERR_STATE, "this shard has not joined its peers (bb200_amcl_join_shards / bb200_sharded_amcl_create)");
   std::vector<AmclPolicy> before;
   before.reserve(static_cast<size_t>(count));
@@ -263,7 +263,7 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
   auto kld_size = [&](uint64_t* accepted) {
     const uint64_t max = lead.params().max_particles;
     for (int r = 0; r < count; ++r) {
-      const int st = ranks[r]->filter_.step_totals(nullptr, nullptr);  // enqueue the totals exchange on every shard
+      const int st = ranks[r]->filter_.step_totals();  // on every shard
       if (st != BB200_OK) return st;
     }
     uint64_t begin = 0, k_before = 0;

@@ -600,15 +600,18 @@ int bb200_amcl_update_point_cloud(bb200_amcl* a, const double control_pose[4], c
 
 int bb200_amcl_export_shard(bb200_amcl* a, void* out256) {
   BB_REQUIRE(a && out256);
-  return guarded(a->impl, [&] { return a->impl.filter().export_shard(out256); });
+  return guarded(a->impl, [&] { return a->impl.filter().link().export_handles(out256); });
 }
 int bb200_amcl_join_shards(bb200_amcl* a, int world, int rank, const void* handles) {
   BB_REQUIRE(a && handles);
-  return guarded(a->impl, [&] { return a->impl.filter().join_shards_ipc(world, rank, handles); });
+  return guarded(a->impl, [&] { return a->impl.filter().link().join_ipc(world, rank, handles); });
 }
 int bb200_amcl_leave_shards(bb200_amcl* a) {
   BB_REQUIRE(a);
-  return guarded(a->impl, [&] { return a->impl.filter().leave_shards(); });
+  return guarded(a->impl, [&] {
+    bb200::Filter& f = a->impl.filter();
+    return f.link().leave(f.stream());
+  });
 }
 
 int bb200_sharded_amcl_create(const bb200_amcl_param* p, const bb200_motion_param* motion, int n_shards, const int* devices, bb200_sharded_amcl** out) {
@@ -625,6 +628,7 @@ int bb200_sharded_amcl_create(const bb200_amcl_param* p, const bb200_motion_para
     auto group = std::make_unique<bb200_sharded_amcl>();
     const uint64_t shard = p->max_particles / static_cast<uint64_t>(n_shards);
     std::vector<bb200::Filter*> filters;
+    std::vector<bb200::ShardLink*> links;
     for (int r = 0; r < n_shards; ++r) {
       bb200_amcl_param q = *p;
       q.device = devices[r];
@@ -635,8 +639,9 @@ int bb200_sharded_amcl_create(const bb200_amcl_param* p, const bb200_motion_para
       if (st != BB200_OK) return st;
       group->ranks.push_back(a);
       filters.push_back(&a->impl.filter());
+      links.push_back(&a->impl.filter().link());
     }
-    const int st = bb200::Filter::join_shards_local(filters.data(), n_shards);
+    const int st = bb200::ShardLink::join_local(links.data(), n_shards);
     if (st != BB200_OK) {
       g_create_error = "joining the shards failed (peer access between the devices?)";
       for (bb200::Filter* f : filters)

@@ -134,13 +134,9 @@ Filter::Filter(const bb200_filter_config& config) : config_(config), cluster_(co
   BB_TRY(perm_.allocate(capacity_));
   BB_TRY(counters_.allocate(schedule_max_bins()));
   BB_TRY(sched_tiles_.allocate(schedule_tile_count()));
-  BB_TRY(mail_.allocate(1));  // its own allocation: exported to peer processes through CUDA IPC
-  BB_TRY(shard_totals_.allocate(kMaxShards));
-  BB_TRY(summary_.allocate(1));
+  BB_TRY(link_.create(config_, states_[0].get(), states_[1].get(), stream_));
   BB_TRY(summary_host_.allocate(1));
   std::memset(summary_host_.get(), 0, sizeof(StepSummary));  // pinned allocations are recycled with their old contents (a stale completion ticket)
-  BB_TRY(cudaMemsetAsync(mail_.get(), 0, sizeof(ShardMail), stream_));
-  BB_TRY(cudaMemsetAsync(summary_.get(), 0, sizeof(StepSummary), stream_));
   BB_TRY(cudaMemsetAsync(scalars_.get(), 0, sizeof(Scalars), stream_));
   BB_TRY(cudaStreamSynchronize(stream_));
   global_size_ = config_.global_count;
@@ -148,10 +144,8 @@ Filter::Filter(const bb200_filter_config& config) : config_(config), cluster_(co
 }
 
 Filter::~Filter() {
-  // Before the members free this filter's buffers (after this body): nothing in flight may read them, and the peers'
-  // buffers mapped here are closed first (CUDA IPC requires importers to close before the exporter frees).
+  // Before the members free this filter's buffers (after this body): nothing in flight may read them.
   if (stream_ != nullptr) cudaStreamSynchronize(stream_);
-  release_peers();
   for (auto& e : event_pool_) cudaEventDestroy(e);
   if (stream_ != nullptr && owns_stream_) cudaStreamDestroy(stream_);
 }
@@ -304,165 +298,24 @@ int Filter::enqueue_moment_kernels(const double pivot[2]) {
   return BB200_OK;
 }
 
-void Filter::release_peers() {
-  if (peers_ipc_) {  // unmap what cudaIpcOpenMemHandle mapped; local peers are plain pointers owned by their filters
-    for (int r = 0; r < peer_world_; ++r) {
-      if (r == peer_rank_) continue;
-      for (int b = 0; b < 2; ++b)
-        if (peer_states_[b][r] != nullptr) cudaIpcCloseMemHandle(peer_states_[b][r]);
-      if (peer_mail_[r] != nullptr) cudaIpcCloseMemHandle(peer_mail_[r]);
-      if (peer_kld_hashes_[r] != nullptr) cudaIpcCloseMemHandle(peer_kld_hashes_[r]);
-    }
-  }
-  for (int r = 0; r < kMaxShards; ++r) {
-    peer_states_[0][r] = peer_states_[1][r] = nullptr;
-    peer_mail_[r] = nullptr;
-    peer_kld_hashes_[r] = nullptr;
-  }
-  peer_world_ = 0;
-  peers_ipc_ = false;
-}
-
-int Filter::leave_shards() {
-  BB_CHECK(cudaSetDevice(config_.device));
-  BB_CHECK(cudaStreamSynchronize(stream_));
-  release_peers();
-  return BB200_OK;
-}
-
-int Filter::enable_shard_kld() {
-  if (kld_hashes_global_.get() != nullptr) return BB200_OK;
-  if (peer_world_ != 0) return fail(BB200_ERR_STATE, "KLD on shards must be enabled before the shards are joined");
-  BB_CHECK(cudaSetDevice(config_.device));
-  BB_CHECK(kld_hashes_global_.allocate(config_.global_count));  // one spatial hash per candidate slot of the WHOLE filter
-  return BB200_OK;
-}
-
-int Filter::export_shard(void* out256) {
-  BB_CHECK(cudaSetDevice(config_.device));
-  static_assert(sizeof(cudaIpcMemHandle_t) == 64, "four IPC handles are exported as 256 bytes");
-  cudaIpcMemHandle_t h[4];
-  std::memset(h, 0, sizeof(h));
-  BB_CHECK(cudaIpcGetMemHandle(&h[0], states_[0].get()));
-  BB_CHECK(cudaIpcGetMemHandle(&h[1], states_[1].get()));
-  BB_CHECK(cudaIpcGetMemHandle(&h[2], mail_.get()));
-  if (kld_hashes_global_.get() != nullptr) BB_CHECK(cudaIpcGetMemHandle(&h[3], kld_hashes_global_.get()));
-  std::memcpy(out256, h, sizeof(h));
-  return BB200_OK;
-}
-
-int Filter::join_shards_ipc(int world, int rank, const void* handles) {
-  if (world < 1 || world > kMaxShards || rank < 0 || rank >= world) return fail(BB200_ERR_INVALID_ARGUMENT, "shard groups hold 1..8 ranks");
-  if (peer_world_ != 0) return fail(BB200_ERR_STATE, "the peers' buffers are already mapped");
-  if (config_.first_index != static_cast<uint64_t>(rank) * capacity_ || config_.global_count != static_cast<uint64_t>(world) * capacity_)
-    return fail(BB200_ERR_INVALID_ARGUMENT, "shard r of R holds the global indices [r * capacity, (r + 1) * capacity) of R * capacity particles");
-  BB_CHECK(cudaSetDevice(config_.device));
-  const auto* all = static_cast<const cudaIpcMemHandle_t*>(handles);
-  peers_ipc_ = true;
-  peer_world_ = world;
-  peer_rank_ = rank;
-  for (int r = 0; r < world; ++r) {
-    if (r == rank) {
-      peer_states_[0][r] = states_[0].get();
-      peer_states_[1][r] = states_[1].get();
-      peer_mail_[r] = mail_.get();
-      peer_kld_hashes_[r] = kld_hashes_global_.get();
-      continue;
-    }
-    static const cudaIpcMemHandle_t kNoHandle{};
-    void* p[4] = {nullptr, nullptr, nullptr, nullptr};
-    for (int b = 0; b < 4; ++b) {
-      if (b == 3 && (kld_hashes_global_.get() == nullptr || std::memcmp(&all[4 * r + 3], &kNoHandle, sizeof(kNoHandle)) == 0)) continue;  // no KLD on this filter
-      const int st = check(cudaIpcOpenMemHandle(&p[b], all[4 * r + b], cudaIpcMemLazyEnablePeerAccess), "cudaIpcOpenMemHandle");
-      if (st != BB200_OK) {
-        peer_states_[0][r] = static_cast<Pose2*>(p[0]);
-        peer_states_[1][r] = static_cast<Pose2*>(p[1]);
-        peer_mail_[r] = static_cast<ShardMail*>(p[2]);
-        release_peers();
-        return st;
-      }
-    }
-    peer_states_[0][r] = static_cast<Pose2*>(p[0]);
-    peer_states_[1][r] = static_cast<Pose2*>(p[1]);
-    peer_mail_[r] = static_cast<ShardMail*>(p[2]);
-    peer_kld_hashes_[r] = static_cast<unsigned long long*>(p[3]);
-  }
-  shard_kld_ = kld_hashes_global_.get() != nullptr;
-  for (int r = 0; r < world; ++r) shard_kld_ = shard_kld_ && peer_kld_hashes_[r] != nullptr;
-  split_posts_ = false;  // every rank has its own host thread: post and wait travel in one launch
-  return BB200_OK;
-}
-
-int Filter::join_shards_local(Filter* const* filters, int world) {
-  if (filters == nullptr || world < 1 || world > kMaxShards) return BB200_ERR_INVALID_ARGUMENT;
-  for (int r = 0; r < world; ++r) {
-    Filter* f = filters[r];
-    if (f == nullptr || !f->ok()) return BB200_ERR_INVALID_ARGUMENT;
-    if (f->peer_world_ != 0) return f->fail(BB200_ERR_STATE, "the peers' buffers are already mapped");
-    if (f->capacity_ != filters[0]->capacity_ || f->config_.first_index != static_cast<uint64_t>(r) * f->capacity_ ||
-        f->config_.global_count != static_cast<uint64_t>(world) * f->capacity_ || f->config_.seed != filters[0]->config_.seed)
-      return f->fail(BB200_ERR_INVALID_ARGUMENT, "shard r of R holds the global indices [r * capacity, (r + 1) * capacity) of R * capacity particles, same seed");
-  }
-  for (int a = 0; a < world; ++a) {
-    Filter* fa = filters[a];
-    for (int b = 0; b < world; ++b) {
-      const Filter* fb = filters[b];
-      if (fa->config_.device != fb->config_.device) {
-        int can = 0;
-        if (cudaDeviceCanAccessPeer(&can, fa->config_.device, fb->config_.device) != cudaSuccess || !can)
-          return fa->fail(BB200_ERR_CUDA, "no peer access between the devices of two shards");
-        if (fa->check(cudaSetDevice(fa->config_.device), "cudaSetDevice") != BB200_OK) return BB200_ERR_CUDA;
-        const cudaError_t e = cudaDeviceEnablePeerAccess(fb->config_.device, 0);
-        if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) return fa->check(e, "cudaDeviceEnablePeerAccess");
-        (void)cudaGetLastError();
-      }
-      fa->peer_states_[0][b] = fb->states_[0].get();
-      fa->peer_states_[1][b] = fb->states_[1].get();
-      fa->peer_mail_[b] = fb->mail_.get();
-      fa->peer_kld_hashes_[b] = fb->kld_hashes_global_.get();
-    }
-    fa->shard_kld_ = true;
-    for (int b = 0; b < world; ++b) fa->shard_kld_ = fa->shard_kld_ && filters[b]->kld_hashes_global_.get() != nullptr;
-    fa->peer_world_ = world;
-    fa->peer_rank_ = a;
-    fa->peers_ipc_ = false;
-    fa->split_posts_ = true;  // one thread enqueues all shards: every post must be enqueued before any wait that needs it
-  }
-  return BB200_OK;
-}
-
 int Filter::enqueue_exchange(int kind, bool post, bool wait) {
-  ShardExchangeArgs a{};
-  a.kind = kind;
-  a.post = post ? 1 : 0;
-  a.wait = wait ? 1 : 0;
-  a.rank = peer_rank_;
-  a.world = peer_world_;
-  a.epoch = epoch_;
-  for (int r = 0; r < peer_world_; ++r) a.peers[r] = peer_mail_[r];
-  a.scalars = scalars_.get();
-  a.results = results_.get();
-  a.summary = summary_host_.get();  // pinned host memory: the step's results need no copy
-  a.rank_totals = shard_totals_.get();
-  a.ceil_log2_count = ceil_log2_count(config_.global_count);
-  a.tile_state = tile_state_.get();
-  a.n_tiles = scan_tile_count(n_);
-  launch_shard_exchange(a, stream_);
+  // the summary is pinned host memory: the step's results need no copy
+  link_.exchange(kind, post, wait, scalars_.get(), results_.get(), summary_host_.get(), tile_state_.get(), scan_tile_count(n_), stream_);
   BB_LAUNCHED("shard_exchange");
   return BB200_OK;
 }
 
 int Filter::step_begin(const bb200_motion_sampling& sampling, uint32_t step, const double* points_xy, uint64_t n_points, const bb200_resample_opts& o,
                        bool resample_planned) {
-  const uint64_t world = peer_world_ > 1 ? static_cast<uint64_t>(peer_world_) : 1;
+  const uint64_t world = link_.world() > 1 ? static_cast<uint64_t>(link_.world()) : 1;
   const bool kld = o.min_particles < o.max_particles;
-  if (n_ == 0 && !(world > 1 && shard_kld_)) return fail(BB200_ERR_STATE, "no particles");  // a KLD-sized filter may leave a shard empty
+  if (n_ == 0 && !(world > 1 && link_.kld())) return fail(BB200_ERR_STATE, "no particles");  // a KLD-sized filter may leave a shard empty
   if (map_.sensor < 0) return fail(BB200_ERR_STATE, "no sensor model map set");
-  if (kld && !(world > 1 && shard_kld_)) return fail(BB200_ERR_STATE, "the fused step does not run KLD on one GPU; use resample()");
+  if (kld && !(world > 1 && link_.kld())) return fail(BB200_ERR_STATE, "the fused step does not run KLD on one GPU; use resample()");
   if (n_points > 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, "too many points");
   if (o.random_state_probability > 0.0 && map_.n_free == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
   if (world > 1) {
-    if ((!shard_kld_ && n_ != capacity_) || n_ > capacity_ || o.max_particles != world * capacity_)
+    if ((!link_.kld() && n_ != capacity_) || n_ > capacity_ || o.max_particles != world * capacity_)
       return fail(BB200_ERR_STATE, "a sharded filter keeps `capacity` particles on every rank (fewer only under KLD)");
   } else if (o.max_particles == 0 || o.max_particles > capacity_) {
     return fail(BB200_ERR_CAPACITY, "max_particles exceeds the filter capacity");
@@ -486,7 +339,8 @@ void Filter::step_abort() { step_.active = false; }
 int Filter::step_phase(int phase) {
   if (!step_.active) return fail(BB200_ERR_STATE, "step_begin must run first");
   BB_CHECK(cudaSetDevice(config_.device));
-  const bool sharded = peer_world_ > 1;
+  const bool sharded = link_.world() > 1;
+  const bool split = link_.split_posts();
   const bb200_resample_opts& o = step_.opts;
   int st = BB200_OK;
   switch (phase) {
@@ -503,8 +357,8 @@ int Filter::step_phase(int phase) {
       }
       if (st != BB200_OK) return st;
       if (sharded) {
-        ++epoch_;  // one sequence number per batch of exchanges
-        if (split_posts_) {
+        link_.begin_batch();
+        if (split) {
           mark("exchange");
           st = enqueue_exchange(kExchangeWmax, true, false);
         }
@@ -514,7 +368,7 @@ int Filter::step_phase(int phase) {
     case kPhaseCdf: {
       if (sharded) {
         mark("exchange_wmax");
-        st = enqueue_exchange(kExchangeWmax, !split_posts_, true);  // global largest weight -> exponent; resets the scan state
+        st = enqueue_exchange(kExchangeWmax, !split, true);  // global largest weight -> exponent; resets the scan state
         if (st != BB200_OK) return st;
       }
       mark("quantize_scan");
@@ -529,7 +383,7 @@ int Filter::step_phase(int phase) {
           BB_LAUNCHED("fill_weights");
           step_.weights_filled = true;
         }
-        if (split_posts_) {
+        if (split) {
           mark("exchange");
           st = enqueue_exchange(kExchangeTotal, true, false);
         }
@@ -542,7 +396,7 @@ int Filter::step_phase(int phase) {
       if (sharded) {
         if (!step_.totals_exchanged) {
           mark("exchange_total");
-          st = enqueue_exchange(kExchangeTotal, !split_posts_, true);  // every rank's fixed-point total -> CDF offsets
+          st = enqueue_exchange(kExchangeTotal, !split, true);  // every rank's fixed-point total -> CDF offsets
           if (st != BB200_OK) return st;
           step_.totals_exchanged = true;
         }
@@ -553,22 +407,19 @@ int Filter::step_phase(int phase) {
         a.slot_first = 0;
         a.weights_out = nullptr;
         a.ancestors = nullptr;
-        a.peer_count = peer_world_;
-        a.peer_shard = accepted != 0 ? (accepted + static_cast<uint64_t>(peer_world_) - 1) / static_cast<uint64_t>(peer_world_) : capacity_;
-        a.rank_totals = shard_totals_.get();
-        a.rank = peer_rank_;
-        a.world = peer_world_;
+        const uint64_t world = static_cast<uint64_t>(link_.world());
+        link_.target_states(&a, cur_ ^ 1);
+        a.peer_shard = accepted != 0 ? (accepted + world - 1) / world : capacity_;
         if (accepted != 0) {  // the comb still spans max_particles slots; only [0, accepted) are kept
           a.window_begin = 0;
           a.window_end = accepted;
-          a.inject_mod = peer_world_;
+          a.inject_mod = link_.world();
         }
         if (!systematic) {  // draws are independent: walk all global slots, keep those landing in this rank's CDF span
           a.span_filter = 1;
           a.owner_first = first_index_;
           a.owner_count = capacity_;
         }
-        for (int r = 0; r < peer_world_; ++r) a.peer_out[r] = peer_states_[cur_ ^ 1][r];
         if (!step_.weights_filled) {
           mark("fill_weights");
           launch_fill(weights_.get(), capacity_, 1.0, stream_);  // the CDF holds what sampling needs; every new particle weighs 1
@@ -591,7 +442,7 @@ int Filter::step_phase(int phase) {
       step_.partial_rows = launch_resample(a, scalars_.get(), partials_.get(), stream_);
       BB_LAUNCHED("resample");
       step_.resampled = true;
-      if (sharded && split_posts_) {
+      if (sharded && split) {
         mark("exchange");
         st = enqueue_exchange(kExchangeMoments, true, false);
       }
@@ -600,32 +451,28 @@ int Filter::step_phase(int phase) {
     case kPhaseFinish: {
       if (sharded) {
         mark("exchange_moments");
-        st = enqueue_exchange(kExchangeMoments, !split_posts_, true);  // also the barrier: the peers' stores into this rank's buffer are complete
+        st = enqueue_exchange(kExchangeMoments, !split, true);  // also the barrier: the peers' stores into this rank's buffer are complete
         if (st != BB200_OK) return st;
-      } else if (!step_.resampled) {  // kPhaseNormalize left the moments in results_: hand them to the host block
-        mark("readback");
-        launch_write_summary(results_.get(), scalars_.get(), summary_host_.get(), stream_);
-        BB_LAUNCHED("write_summary");
       }
       mark("end");
       return BB200_OK;
     }
     case kPhaseNormalize: {
+      // The moments reach the host block through the moments exchange of kPhaseFinish: a filter of one rank has none.
+      if (!sharded) return fail(BB200_ERR_STATE, "normalising without resampling is a step of joined shards");
       if (step_.normalized) return fail(BB200_ERR_STATE, "the weights of this step are already normalised");
-      if (sharded) {
-        mark("exchange");
-        st = enqueue_exchange(kExchangeTotal, !split_posts_, true);
-        if (st != BB200_OK) return st;
-        step_.totals_exchanged = true;
-      }
+      mark("exchange");
+      st = enqueue_exchange(kExchangeTotal, !split, true);
+      if (st != BB200_OK) return st;
+      step_.totals_exchanged = true;
       uint32_t rows = 0;
       mark("normalize");
-      launch_normalize(weights_.get(), n_, scalars_.get(), sharded ? ~0ull : 0ull, partials_.get(), &rows, stream_);  // actions/normalize.hpp:82
+      launch_normalize(weights_.get(), n_, scalars_.get(), ~0ull, partials_.get(), &rows, stream_);  // actions/normalize.hpp:82
       BB_LAUNCHED("normalize");
       st = enqueue_moment_kernels(pivot_);  // a KLD-sized shard may be empty here
       if (st != BB200_OK) return st;
       step_.normalized = true;
-      if (sharded && split_posts_) {
+      if (split) {
         mark("exchange");
         st = enqueue_exchange(kExchangeMoments, true, false);
       }
@@ -637,7 +484,7 @@ int Filter::step_phase(int phase) {
 }
 
 int Filter::kld_sharded_candidates(uint64_t begin, uint64_t end) {
-  if (!step_.active || !shard_kld_ || peer_world_ < 2) return fail(BB200_ERR_STATE, "KLD on shards: no step in progress on a KLD-enabled shard group");
+  if (!step_.active || !link_.kld() || link_.world() < 2) return fail(BB200_ERR_STATE, "KLD on shards: no step in progress on a KLD-enabled shard group");
   if (!step_.totals_exchanged) return fail(BB200_ERR_STATE, "KLD on shards: the totals exchange must run first");
   if (end <= begin || end > config_.global_count) return fail(BB200_ERR_INVALID_ARGUMENT, "KLD on shards: bad slot window");
   BB_CHECK(cudaSetDevice(config_.device));
@@ -653,14 +500,10 @@ int Filter::kld_sharded_candidates(uint64_t begin, uint64_t end) {
   a.states_out = nullptr;
   a.weights_out = nullptr;
   a.ancestors = nullptr;
-  a.rank_totals = shard_totals_.get();
-  a.rank = peer_rank_;
-  a.world = peer_world_;
+  link_.target_hashes(&a);
   a.window_begin = begin;
   a.window_end = end;
-  a.peer_hash_count = peer_world_;
-  for (int r = 0; r < peer_world_; ++r) a.peer_hashes[r] = peer_kld_hashes_[r];
-  a.inject_mod = peer_world_;
+  a.inject_mod = link_.world();
   a.slot_first = 0;
   if (!systematic) {
     a.span_filter = 1;
@@ -670,20 +513,20 @@ int Filter::kld_sharded_candidates(uint64_t begin, uint64_t end) {
   mark("kld_candidates");
   launch_resample(a, scalars_.get(), partials_.get(), stream_);
   BB_LAUNCHED("kld_candidates");
-  ++epoch_;
-  if (split_posts_) return enqueue_exchange(kExchangeKld, true, false);
+  link_.begin_batch();
+  if (link_.split_posts()) return enqueue_exchange(kExchangeKld, true, false);
   return BB200_OK;
 }
 
 int Filter::kld_sharded_count(uint64_t begin, uint64_t end, uint64_t k_before) {
-  if (!step_.active || !shard_kld_) return fail(BB200_ERR_STATE, "KLD on shards: no step in progress");
+  if (!step_.active || !link_.kld()) return fail(BB200_ERR_STATE, "KLD on shards: no step in progress");
   BB_CHECK(cudaSetDevice(config_.device));
   const bb200_resample_opts& o = step_.opts;
   mark("exchange_kld");
-  const int st = enqueue_exchange(kExchangeKld, !split_posts_, true);  // every rank's hashes of this window have arrived
+  const int st = enqueue_exchange(kExchangeKld, !link_.split_posts(), true);  // every rank's hashes of this window have arrived
   if (st != BB200_OK) return st;
   mark("kld");
-  KldArgs k{kld_hashes_global_.get() + begin, end - begin, begin, k_before, o.min_particles, o.kld_epsilon, o.kld_z};
+  KldArgs k{link_.kld_hashes() + begin, end - begin, begin, k_before, o.min_particles, o.kld_epsilon, o.kld_z};
   launch_kld_chunk(k, kld_.keys.get(), kld_.vals.get(), kld_.keys.size(), kld_.flags.get(), kld_.scan.get(), scalars_.get(), kld_.tile_state.get(), stream_);
   BB_LAUNCHED_N("kld", 5);
   BB_CHECK(cudaMemcpyAsync(scalars_host_.get(), scalars_.get(), sizeof(Scalars), cudaMemcpyDeviceToHost, stream_));
@@ -695,24 +538,19 @@ int Filter::kld_sharded_read(uint64_t* cutoff, uint64_t* new_buckets) {
   BB_CHECK(cudaStreamSynchronize(stream_));
   if (scalars_host_.get()->exchange_error != 0) return fail(BB200_ERR_STATE, "shard exchange timed out during the KLD count");
   *cutoff = scalars_host_.get()->kld_cutoff;
-  *new_buckets = scalars_host_.get()->pad[1];
+  *new_buckets = scalars_host_.get()->kld_new_buckets;
   return BB200_OK;
 }
 
-int Filter::step_totals(uint64_t* rank_totals, int* exponent) {
-  if (!step_.active || peer_world_ < 2) return fail(BB200_ERR_STATE, "no sharded step in progress");
+int Filter::step_totals() {
+  if (!step_.active || link_.world() < 2) return fail(BB200_ERR_STATE, "no sharded step in progress");
   BB_CHECK(cudaSetDevice(config_.device));
   if (!step_.totals_exchanged) {
     mark("exchange_total");
-    const int st = enqueue_exchange(kExchangeTotal, !split_posts_, true);
+    const int st = enqueue_exchange(kExchangeTotal, !link_.split_posts(), true);
     if (st != BB200_OK) return st;
     step_.totals_exchanged = true;
   }
-  if (rank_totals == nullptr) return BB200_OK;  // enqueue only
-  BB_CHECK(cudaStreamSynchronize(stream_));
-  if (summary_host_.get()->error != 0) return fail(BB200_ERR_STATE, "shard exchange timed out");
-  for (int r = 0; r < peer_world_; ++r) rank_totals[r] = summary_host_.get()->rank_totals[r];
-  if (exponent != nullptr) *exponent = summary_host_.get()->exponent;
   return BB200_OK;
 }
 
@@ -727,7 +565,8 @@ int Filter::step_end(bb200_estimate* est, double* weight_sum, uint64_t* new_size
   if (!done) BB_CHECK(cudaStreamSynchronize(stream_));
   step_.poll_seq = 0;
   finish_marks();
-  const bool sharded = peer_world_ > 1;
+  const int world = link_.world(), rank = link_.rank();
+  const bool sharded = world > 1;
   if (summary_host_.get()->error != 0) {
     step_.active = false;
     return fail(BB200_ERR_STATE, "shard exchange timed out: a peer rank never posted its value for this step");
@@ -740,10 +579,10 @@ int Filter::step_end(bb200_estimate* est, double* weight_sum, uint64_t* new_size
     cur_ ^= 1;
     n_ = sharded ? capacity_ : step_.opts.max_particles;
     if (sharded && step_.kld_accepted != 0) {  // the new set of `accepted` particles in equal contiguous shards
-      const uint64_t shard = (step_.kld_accepted + static_cast<uint64_t>(peer_world_) - 1) / static_cast<uint64_t>(peer_world_);
-      const uint64_t begin = std::min<uint64_t>(static_cast<uint64_t>(peer_rank_) * shard, step_.kld_accepted);
+      const uint64_t shard = (step_.kld_accepted + static_cast<uint64_t>(world) - 1) / static_cast<uint64_t>(world);
+      const uint64_t begin = std::min<uint64_t>(static_cast<uint64_t>(rank) * shard, step_.kld_accepted);
       n_ = std::min<uint64_t>(shard, step_.kld_accepted - begin);
-      first_index_ = static_cast<uint64_t>(peer_rank_) * shard;
+      first_index_ = static_cast<uint64_t>(rank) * shard;
     } else if (sharded) {
       first_index_ = config_.first_index;
     }
@@ -752,7 +591,7 @@ int Filter::step_end(bb200_estimate* est, double* weight_sum, uint64_t* new_size
     step_.active = false;
   } else {
     cdf_valid_ = true;  // kPhaseResample may still follow (selective resampling)
-    ++epoch_;           // ... as a new batch of exchanges
+    link_.begin_batch();  // ... as a new batch of exchanges
   }
   if (new_size != nullptr) *new_size = !sharded ? n_ : (step_.resampled && step_.kld_accepted != 0 ? step_.kld_accepted : global_size_);
   if (sharded && step_.resampled) global_size_ = step_.kld_accepted != 0 ? step_.kld_accepted : config_.global_count;
@@ -1244,7 +1083,7 @@ int Filter::resample_kld(const bb200_resample_opts& o, uint64_t* accepted) {
       *accepted = std::min<uint64_t>(scalars_host_.get()->kld_cutoff - 1, max);
       break;
     }
-    k_before += scalars_host_.get()->pad[1];
+    k_before += scalars_host_.get()->kld_new_buckets;
     begin = end;
     end = std::min<uint64_t>(max, end * 2);
   }

@@ -15,6 +15,7 @@
 #include "device_buffer.hpp"
 #include "device_map.hpp"
 #include "kernels.cuh"
+#include "shard_link.hpp"
 
 namespace bb200 {
 
@@ -79,19 +80,9 @@ class Filter {
   int enqueue_moments(const double pivot[2]);   // raw moments stay in the device result block
 
   // ---- one filter over several shards, exchanges through peer memory (no NCCL, no host round trip) ----
-  /// CUDA IPC handles of the two state buffers and the mail block (3 x 64 bytes) for peers in OTHER processes.
-  int export_shard(void* out256);
-  /// KLD-adaptive resampling on shards needs one hash array of the WHOLE filter's slot count on every rank, exported
-  /// with the other buffers: call before export_shard / join_shards_local.
-  int enable_shard_kld();
-  /// Map the peers' buffers from their exported handles (world x 256 bytes, rank order); one process per GPU.
-  int join_shards_ipc(int world, int rank, const void* handles);
-  /// Shards living in THIS process (one per device, or several on one device): direct pointers, peer access enabled
-  /// between distinct devices.  filters[r] becomes rank r.
-  static int join_shards_local(Filter* const* filters, int world);
-  int shard_world() const { return peer_world_; }
-  /// Unmaps the peers' buffers (before any rank frees its own: CUDA IPC requires importers to close first).
-  int leave_shards();
+  /// Export, join and leave go through the link; its views stay valid because the state buffers are never reallocated.
+  ShardLink& link() { return link_; }
+  cudaStream_t stream() const { return stream_; }
   /// The fused resampling step (propagate | reweight | normalize | resample | estimate), any number of shards.
   /// step_begin validates and stages the inputs; step_phase(1..4) only enqueues; step_end synchronises once.
   /// A driver holding several shards in one thread enqueues phase k of every shard before phase k+1 of any.
@@ -102,23 +93,22 @@ class Filter {
     kPhaseCdf = 2,        // common exponent | fixed-point CDF                                 (posts the shard's total)
     kPhaseResample = 3,   // resample (+ redistribution over peer memory) | moments of the new set (posts them)
     kPhaseFinish = 4,     // global moments, read-back
-    kPhaseNormalize = 5   // instead of kPhaseResample on a step that keeps its particles: w /= S | moments
+    kPhaseNormalize = 5   // joined shards, instead of kPhaseResample on a step that keeps its particles: w /= S | moments
   };
   int step_phase(int phase);
   void step_abort();
   // KLD on shards (views/take_while_kld.hpp:72-137 over the globally ordered candidate stream).  After kPhaseCdf:
-  //   step_totals            the ranks' fixed-point totals (also enqueues their exchange)
+  //   step_totals            enqueues the exchange of the ranks' fixed-point totals
   //   kld_sharded_candidates hashes of this rank's candidates among the slots [begin, end) -> every rank's hash array
   //   kld_sharded_count      (after all ranks' candidates) distinct-bucket count over the window, on every rank alike
   //   kld_sharded_read       first failing count (~0: none in this window), new buckets of the window
   //   step_set_kld_accepted  the count the loop settled on; kPhaseResample then produces exactly those slots
-  int step_totals(uint64_t* rank_totals, int* exponent);
+  int step_totals();
   int kld_sharded_candidates(uint64_t begin, uint64_t end);
   int kld_sharded_count(uint64_t begin, uint64_t end, uint64_t k_before);
   int kld_sharded_read(uint64_t* cutoff, uint64_t* new_buckets);
   void step_set_kld_accepted(uint64_t accepted);
-  bool shard_kld() const { return shard_kld_; }
-  uint64_t global_size() const { return peer_world_ > 1 ? global_size_ : n_; }
+  uint64_t global_size() const { return link_.world() > 1 ? global_size_ : n_; }
   uint64_t first_index() const { return first_index_; }
   const double* pivot() const { return pivot_; }
   /// Synchronises and closes the batch of phases enqueued so far.  After kPhaseNormalize a caller may still run
@@ -175,13 +165,12 @@ class Filter {
     bool weights_filled{false};
     bool totals_exchanged{false};
     int poll_seq{0};  // != 0: the resample kernel stores this ticket to the pinned summary when the step is complete
-    uint64_t kld_accepted{0};  // KLD on shards: particle count of the new set (0: fixed size)  // the ranks' totals of this step are in shard_totals_
+    uint64_t kld_accepted{0};  // KLD on shards: particle count of the new set (0: fixed size)
     unsigned long long total{0};
     int exponent{0};
   };
   StepContext step_{};
   int enqueue_exchange(int kind, bool post, bool wait);
-  void release_peers();
 
   bb200_filter_config config_{};
   bool created_{false};
@@ -189,15 +178,6 @@ class Filter {
   mutable std::string error_;
   cudaStream_t stream_{nullptr};
   bool owns_stream_{true};
-  int peer_world_{0}, peer_rank_{0};
-  Pose2* peer_states_[2][8]{};  // [buffer][rank]: the peers' ping-pong state buffers mapped into this process
-  DeviceBuffer<ShardMail> mail_;             // this rank's mail block
-  ShardMail* peer_mail_[kMaxShards]{};       // every rank's mail block as seen from here ([rank] = mail_)
-  bool peers_ipc_{false};                    // the peer pointers came from cudaIpcOpenMemHandle
-  bool split_posts_{false};                  // post and wait as separate launches (several shards enqueued by one thread)
-  unsigned long long epoch_{0};              // sequence number of the next exchange (all ranks count alike)
-  DeviceBuffer<unsigned long long> shard_totals_;  // the ranks' fixed-point totals of this step
-  DeviceBuffer<StepSummary> summary_;
   PinnedBuffer<StepSummary> summary_host_;
 
   // particle set (ping-pong states for the resample gather)
@@ -232,9 +212,6 @@ class Filter {
     DeviceBuffer<unsigned long long> tile_state;  // shards: scan state of the count (one GPU uses tile_state_)
   };
   KldTables kld_;
-  DeviceBuffer<unsigned long long> kld_hashes_global_;  // KLD on shards: spatial hash of every candidate slot (all ranks hold all)
-  unsigned long long* peer_kld_hashes_[kMaxShards]{};
-  bool shard_kld_{false};
 
   // measurement
   DeviceBuffer<double> points_;
@@ -270,6 +247,10 @@ class Filter {
   size_t events_used_{0};
   std::vector<std::pair<const char*, float>> timings_;
   uint64_t launches_{0};
+
+  // Declared last, so destroyed first: the peers' buffers mapped into this process are closed before this filter's own
+  // buffers are freed.
+  ShardLink link_{&error_};
 };
 
 /// bb200_motion_sampling -> the kernels' MotionSampling.

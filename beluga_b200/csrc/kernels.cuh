@@ -1,7 +1,7 @@
 // Kernel launch interface of the CUDA MCL backend.  The kernels are hand-written for sm_90a, one source per stage of a
 // filter step on the device (fixed particle count, resample every step):
 //
-//   step.cu               begin_step: zero the per-filter scalars; the summary block of a finished step
+//   step.cu               begin_step: zero the per-filter scalars
 //   propagate.cu          a2 + a6 of SURVEY.md section 8(a): Philox normals, SE2 compose; cloud moments; initialisation;
 //                         schedule_*: counting sort of the particles over pose bins (execution order only)
 //   reweight_lfm.cu       a3 + a5: B likelihood-field lookups per particle in schedule order, w *= L written to the
@@ -112,7 +112,9 @@ struct Scalars {
   int exponent;                   // q = floor(w * 2^exponent)
   int valid;                      // 0 when no positive finite weight exists
   unsigned long long kld_cutoff;  // first slot (1-based count) at which the KLD condition fails
-  unsigned long long pad[3];
+  unsigned long long kld_scan_ticket;  // KLD chunk: tile ticket of the flag scan
+  unsigned long long kld_new_buckets;  // KLD chunk: distinct buckets that first occur in the chunk
+  unsigned long long pad;
   unsigned long long work_ticket;  // persistent reweight kernel: next 32-particle task (rewound by the last warp out)
   unsigned long long work_done;    // warps that have left that kernel
   int exchange_error;              // sticky: a shard exchange timed out
@@ -154,7 +156,7 @@ struct ShardExchangeArgs {
   ShardMail* peers[kMaxShards];  // every rank's mail block (peers[rank] is this rank's own)
   struct Scalars* scalars;
   double* results;               // kMomentCount local sums in, global sums out (kExchangeMoments)
-  StepSummary* summary;          // device copy, filled as the exchanges complete
+  StepSummary* summary;          // the host's block (pinned memory), filled as the exchanges complete
   unsigned long long* rank_totals;  // device array of kMaxShards totals (kExchangeTotal)
   // kExchangeWmax also prepares the CDF build (what prepare_cdf does on one GPU)
   int ceil_log2_count;
@@ -162,8 +164,6 @@ struct ShardExchangeArgs {
   uint32_t n_tiles;
 };
 void launch_shard_exchange(const ShardExchangeArgs& args, cudaStream_t stream);
-/// results (9 moments) + the CDF scalars -> the host's StepSummary block (pinned memory).
-void launch_write_summary(const double* results, const struct Scalars* scalars, StepSummary* summary, cudaStream_t stream);
 int ceil_log2_count(uint64_t n);
 
 constexpr int kMomentCount = 9;  // sum w, sum w^2, sum w c, sum w s, sum w dx, sum w dy, sum w dx^2, sum w dx dy, sum w dy^2
@@ -550,7 +550,7 @@ void launch_reduce_partials(const double* partials, uint32_t n_partials, int wid
 
 /// KLD (views/take_while_kld.hpp:72-137) over one chunk of candidate slots [slot_base, slot_base + n):
 /// device hash set of buckets -> first-occurrence flags -> prefix count -> first failing count in
-/// scalars->kld_cutoff (1-based; ~0 when every count in the chunk passes); scalars->pad[1] receives
+/// scalars->kld_cutoff (1-based; ~0 when every count in the chunk passes); scalars->kld_new_buckets receives
 /// the number of new buckets of the chunk.
 struct KldArgs {
   const unsigned long long* hashes;  // spatial hash of each candidate of the chunk

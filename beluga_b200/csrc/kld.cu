@@ -59,8 +59,8 @@ __global__ void __launch_bounds__(256) kld_check_kernel(const uint32_t* __restri
 
 __global__ void kld_reset_kernel(Scalars* scalars) {
   scalars->kld_cutoff = ~0ull;
-  scalars->pad[0] = 0;  // tile ticket of the flag scan
-  scalars->pad[1] = 0;  // distinct buckets in the chunk
+  scalars->kld_scan_ticket = 0;
+  scalars->kld_new_buckets = 0;
 }
 
 }  // namespace
@@ -79,7 +79,7 @@ void launch_kld_chunk(const KldArgs& a, unsigned long long* keys, unsigned int* 
   cudaMemsetAsync(tile_state, 0, static_cast<size_t>(tiles) * sizeof(unsigned long long), stream);
   kld_insert_kernel<<<blocks, 256, 0, stream>>>(a.hashes, a.n, a.slot_base, keys, vals, table_size - 1);
   kld_flag_kernel<<<blocks, 256, 0, stream>>>(a.hashes, a.n, a.slot_base, keys, vals, table_size - 1, flags);
-  launch_scan_u32_prepared(flags, exclusive, static_cast<uint32_t>(a.n), &scalars->pad[0], tile_state, &scalars->pad[1], stream);
+  launch_scan_u32_prepared(flags, exclusive, static_cast<uint32_t>(a.n), &scalars->kld_scan_ticket, tile_state, &scalars->kld_new_buckets, stream);
   kld_check_kernel<<<blocks, 256, 0, stream>>>(flags, exclusive, a.n, a.slot_base, a.k_before, a.min_particles, 2 * a.epsilon, a.z, scalars);
 }
 

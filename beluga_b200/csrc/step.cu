@@ -1,5 +1,4 @@
-// Start and end of a filter step: the reset of the per-step scalars (and, in the fused step, of the scan and schedule
-// state) and the copy of a step's results into the host's summary block.
+// Start of a filter step: the reset of the per-step scalars (and, in the fused step, of the scan and schedule state).
 #include "kernels.cuh"
 
 #include <algorithm>
@@ -69,17 +68,6 @@ __global__ void __launch_bounds__(256) begin_fused_step_kernel(StepReset r) {
   for (uint64_t k = t; k < r.prefetch_lines; k += stride) asm volatile("prefetch.global.L2 [%0];" ::"l"(r.prefetch + k * 128));
 }
 
-__global__ void write_summary_kernel(const double* __restrict__ results, const Scalars* __restrict__ scalars, StepSummary* summary) {
-  if (threadIdx.x < kMomentCount) summary->moments[threadIdx.x] = results[threadIdx.x];
-  if (threadIdx.x == 0) {
-    summary->total = scalars->total;
-    summary->exponent = scalars->exponent;
-    summary->valid = scalars->valid;
-    summary->error = 0;
-  }
-  __threadfence_system();
-}
-
 }  // namespace
 
 int ceil_log2_count(uint64_t n) {
@@ -89,10 +77,6 @@ int ceil_log2_count(uint64_t n) {
 }
 
 void launch_begin_step(Scalars* scalars, cudaStream_t stream) { begin_step_kernel<<<1, 1, 0, stream>>>(scalars); }
-
-void launch_write_summary(const double* results, const Scalars* scalars, StepSummary* summary, cudaStream_t stream) {
-  write_summary_kernel<<<1, 32, 0, stream>>>(results, scalars, summary);
-}
 
 void launch_begin_fused_step(Scalars* scalars, unsigned long long* tile_state, uint32_t n_tiles, Schedule* sched, uint32_t* counters,
                              uint32_t n_counters, unsigned long long* sched_tiles, uint32_t n_sched_tiles, const void* prefetch,

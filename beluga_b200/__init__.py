@@ -33,7 +33,7 @@ from ._capi import (RESAMPLE_MULTINOMIAL, RESAMPLE_SYSTEMATIC, SENSOR_BEAM, SENS
 __all__ = [
     "Amcl", "AmclBatch", "AmclParams", "BeamModelParam", "DifferentialDriveModelParam", "OmnidirectionalDriveModelParam", "StationaryModelParam",
     "Filter", "LikelihoodFieldModelParam", "motion_sampling", "scan_to_points", "point_cloud_to_points", "take_evenly_indices",
-    "OccupancyGrid", "BelugaB200Error", "device_count", "se2",
+    "OccupancyGrid", "BelugaB200Error", "device_count", "se2", "LaserScan", "PointCloud",
     "RESAMPLE_MULTINOMIAL", "RESAMPLE_SYSTEMATIC", "SENSOR_BEAM", "SENSOR_LIKELIHOOD_FIELD", "SENSOR_LIKELIHOOD_FIELD_PROB",
 ]
 
@@ -188,6 +188,43 @@ def point_cloud_to_points(data, point_step: int, x_offset: int, dtype, origin=No
     if st != _capi.OK:
         raise BelugaB200Error(st, "bb200_point_cloud_to_points: datatype must be 7 (FLOAT32) or 8 (FLOAT64) and x, y, z must fit in point_step")
     return out[: n.value]
+
+
+@dataclass
+class LaserScan:
+    """A laser scan as Amcl.update_scan takes it (sensor_msgs/LaserScan with the node's range limits and max_beams), one member's
+    measurement in AmclBatch.update_measurements."""
+    ranges: object
+    angle_min: float
+    angle_increment: float
+    min_range: float = 0.0
+    max_range: float = float("inf")
+    max_beams: int = 0
+    laser_origin: object = None
+
+
+@dataclass
+class PointCloud:
+    """A packed PointCloud2 buffer as Amcl.update_point_cloud takes it (arguments as point_cloud_to_points), one member's
+    measurement in AmclBatch.update_measurements."""
+    data: object
+    point_step: int
+    x_offset: int
+    dtype: object
+    origin: object = None
+    n_points: int | None = None
+
+
+def _measurement(m):
+    """bb200_measurement of a LaserScan, a PointCloud or an (n, 2) array of points, and the objects that must outlive the call."""
+    if isinstance(m, LaserScan):
+        scan, keep = _laser_scan(m.ranges, m.angle_min, m.angle_increment, m.min_range, m.max_range, m.max_beams, m.laser_origin)
+        return _capi.Measurement(_capi.MEASUREMENT_SCAN, None, 0, C.pointer(scan), None), (scan, keep)
+    if isinstance(m, PointCloud):
+        cloud, keep = _point_cloud(m.data, m.point_step, m.x_offset, m.dtype, m.origin, m.n_points)
+        return _capi.Measurement(_capi.MEASUREMENT_CLOUD, None, 0, None, C.pointer(cloud)), (cloud, keep)
+    pts = _f64(m).reshape(-1, 2)
+    return _capi.Measurement(_capi.MEASUREMENT_POINTS, _dptr(pts) if len(pts) else None, len(pts), None, None), pts
 
 
 def _dptr(a: np.ndarray):
@@ -923,6 +960,33 @@ class AmclBatch:
         res = (_capi.UpdateResult * k)()
         self._check(self._lib.bb200_amcl_batch_update(self._h, _dptr(poses), ptrs, counts, mask, res))
         return list(res)
+
+    def update_measurements(self, control_poses, measurements, present=None) -> list:
+        """update() with each member's measurement as base-frame points ((n, 2) array), a LaserScan or a PointCloud, as
+        Amcl.update, Amcl.update_scan and Amcl.update_point_cloud take them; scans and clouds are converted on the device.
+        Results are bit-identical to those of update() given scan_to_points / point_cloud_to_points of the same messages."""
+        k = len(self.params)
+        if len(measurements) != k:
+            raise ValueError("one measurement per member")
+        mask = self._mask(present)
+        poses = _f64(control_poses).reshape(k, 4)
+        built = [_measurement(m) for m in measurements]
+        table = (_capi.Measurement * k)(*[b[0] for b in built])
+        res = (_capi.UpdateResult * k)()
+        self._check(self._lib.bb200_amcl_batch_update_measurements(self._h, _dptr(poses), table, mask, res))
+        return list(res)
+
+    def update_scans(self, control_poses, scans, present=None) -> list:
+        """update_measurements with a LaserScan for every member."""
+        if any(not isinstance(s, LaserScan) for s in scans):
+            raise TypeError("update_scans takes one LaserScan per member")
+        return self.update_measurements(control_poses, scans, present)
+
+    def update_point_clouds(self, control_poses, clouds, present=None) -> list:
+        """update_measurements with a PointCloud for every member."""
+        if any(not isinstance(c, PointCloud) for c in clouds):
+            raise TypeError("update_point_clouds takes one PointCloud per member")
+        return self.update_measurements(control_poses, clouds, present)
 
     def launch_count(self) -> int:
         return self._lib.bb200_amcl_batch_launch_count(self._h)

@@ -111,6 +111,14 @@ class MarkerVertex(C.Structure):
     _fields_ = [("x", C.c_double), ("y", C.c_double), ("z", C.c_double), ("r", C.c_float), ("g", C.c_float), ("b", C.c_float), ("a", C.c_float)]
 
 
+MEASUREMENT_POINTS, MEASUREMENT_SCAN, MEASUREMENT_CLOUD = 0, 1, 2
+
+
+class Measurement(C.Structure):
+    _fields_ = [("kind", C.c_int), ("points_xy", C.POINTER(C.c_double)), ("n_points", C.c_uint64), ("scan", C.POINTER(LaserScan)),
+                ("cloud", C.POINTER(PointCloud))]
+
+
 class UpdateResult(C.Structure):
     _fields_ = [("updated", C.c_int), ("resampled", C.c_int), ("n_particles", C.c_uint64), ("estimate", Estimate),
                 ("random_state_probability", C.c_double), ("weight_sum", C.c_double), ("weights_degenerate", C.c_int)]
@@ -227,6 +235,7 @@ SIGNATURES = {
                                                        _P(C.c_uint64), _dbl]),
     "bb200_amcl_batch_sample_states": (C.c_int, [_vp, _P(C.c_uint64), C.c_uint32, _P(C.c_uint8), _P(_dbl)]),
     "bb200_amcl_batch_update": (C.c_int, [_vp, _dbl, _P(_dbl), _P(C.c_uint64), _P(C.c_uint8), _P(UpdateResult)]),
+    "bb200_amcl_batch_update_measurements": (C.c_int, [_vp, _dbl, _P(Measurement), _P(C.c_uint8), _P(UpdateResult)]),
     "bb200_amcl_batch_launch_count": (C.c_uint64, [_vp]),
     "bb200_amcl_plan_update": (C.c_int, [_vp, _dbl, _P(StepPlan)]),
     "bb200_amcl_commit_update": (None, [_vp, C.c_int, C.c_double]),

@@ -1,4 +1,5 @@
 #include "batch.hpp"
+#include "measurement_host.hpp"
 
 #include <algorithm>
 #include <cmath>
@@ -78,8 +79,8 @@ Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, 
   BB_TRY(partials_.allocate(rows * kMomentCount));
   BB_TRY(table_.allocate(members_.size()));
   BB_TRY(table_host_.allocate(members_.size()));
-  BB_TRY(first_.allocate(kBatchLaunches * k1));
-  BB_TRY(first_host_.allocate(kBatchLaunches * k1));
+  BB_TRY(first_.allocate((kBatchLaunches + 1) * k1));
+  BB_TRY(first_host_.allocate((kBatchLaunches + 1) * k1));
   BB_TRY(summary_host_.allocate(members_.size()));
   BB_TRY(ticket_host_.allocate(1));
   BB_TRY(members_done_.allocate(1));
@@ -585,8 +586,108 @@ bool Batch::ensure_hits(uint64_t words) {
   return true;
 }
 
+int Batch::ensure_inputs(uint64_t floats) {
+  if (inputs_.host.get() == nullptr) {
+    InputTable t;
+    BB_CHECK(t.device.allocate(members_.size()));
+    BB_CHECK(t.host.allocate(members_.size()));
+    inputs_ = std::move(t);
+  }
+  // Every batch call ends synchronised: nothing in flight reads the old buffers.
+  const uint64_t room = std::max<uint64_t>(floats + floats / 2, 4096);
+  BB_CHECK(input_.grow(floats, room));
+  BB_CHECK(input_host_.grow(floats, room));
+  return BB200_OK;
+}
+
+int Batch::ensure_scan_table(Member& m, const bb200_laser_scan& scan) {
+  uint32_t angle_min_bits, angle_increment_bits;
+  std::memcpy(&angle_min_bits, &scan.angle_min, sizeof(float));
+  std::memcpy(&angle_increment_bits, &scan.angle_increment, sizeof(float));
+  Member::ScanTable& t = m.scan;
+  if (t.valid && t.n_ranges == scan.n_ranges && t.max_beams == scan.max_beams && t.angle_min_bits == angle_min_bits &&
+      t.angle_increment_bits == angle_increment_bits)
+    return BB200_OK;
+  const uint64_t kept = scan_beam_count(scan);
+  std::vector<uint64_t> indices(kept);
+  std::vector<double2> directions(kept);
+  for (uint64_t pos = 0; pos < kept; ++pos) {
+    const ScanBeam beam = scan_beam(scan, pos);
+    indices[pos] = beam.index;
+    directions[pos] = double2{beam.c, beam.s};
+  }
+  t.valid = false;  // until the new table is on the device
+  BB_CHECK(t.directions.grow(kept));  // every batch call ends synchronised: no step reads the old table
+  // Pageable source: staged before the call returns, and ordered before the step's launches on the batch's stream.
+  if (kept > 0) BB_CHECK(cudaMemcpyAsync(t.directions.get(), directions.data(), kept * sizeof(double2), cudaMemcpyHostToDevice, stream_));
+  t.indices = std::move(indices);
+  t.n_ranges = scan.n_ranges;
+  t.max_beams = scan.max_beams;
+  t.angle_min_bits = angle_min_bits;
+  t.angle_increment_bits = angle_increment_bits;
+  t.valid = true;
+  return BB200_OK;
+}
+
+namespace {
+
+/// Why the single filter would refuse member k's measurement (bb200_amcl_update / _update_scan / _update_point_cloud), or
+/// an empty string.
+std::string measurement_error(const bb200_measurement& in) {
+  switch (in.kind) {
+    case BB200_MEASUREMENT_POINTS:
+      return in.points_xy == nullptr && in.n_points > 0 ? "points_xy is null" : "";
+    case BB200_MEASUREMENT_SCAN:
+      if (in.scan == nullptr) return "scan is null";
+      return in.scan->ranges == nullptr && in.scan->n_ranges > 0 ? "scan ranges are null" : "";
+    case BB200_MEASUREMENT_CLOUD:
+      if (in.cloud == nullptr) return "cloud is null";
+      return cloud_valid(*in.cloud) ? ""
+                                    : "point cloud: datatype must be 7 (FLOAT32) or 8 (FLOAT64), x, y and z must fit in point_step, data must be set";
+    default:
+      return "unknown measurement kind";
+  }
+}
+
+/// The points a member's measurement can yield: the exact count for points and clouds, the kept beams for a scan.
+uint64_t measurement_bound(const bb200_measurement& in) {
+  return in.kind == BB200_MEASUREMENT_SCAN ? scan_beam_count(*in.scan) : in.kind == BB200_MEASUREMENT_CLOUD ? in.cloud->n_points : in.n_points;
+}
+
+/// A sensor origin's rows 0 and 1 in a BatchPointsMember (none: has_origin stays 0).
+void set_origin(BatchPointsMember& d, const double* origin) {
+  d.has_origin = origin != nullptr;
+  if (origin != nullptr) std::memcpy(d.origin, origin, sizeof(d.origin));
+}
+
+/// Packs the x, y, z of every point of a valid cloud as floats, read as bb200_point_cloud_to_points reads them.
+template <class Scalar>
+void pack_cloud(const bb200_point_cloud& c, float* out) {
+  for (uint64_t i = 0; i < c.n_points; ++i) cloud_point<Scalar>(c, i, out + 3 * i);
+}
+
+}  // namespace
+
 int Batch::update(const double* control_poses, const double* const* points_xy, const uint64_t* n_points, const uint8_t* present,
                   bb200_update_result* out) {
+  std::vector<bb200_measurement> in(members_.size());
+  for (size_t k = 0; k < members_.size(); ++k) in[k] = bb200_measurement{BB200_MEASUREMENT_POINTS, points_xy[k], n_points[k], nullptr, nullptr};
+  return step(control_poses, in.data(), present, out);
+}
+
+int Batch::update_measurements(const double* control_poses, const bb200_measurement* measurements, const uint8_t* present,
+                               bb200_update_result* out) {
+  error_.clear();
+  for (size_t k = 0; k < members_.size(); ++k) out[k] = bb200_update_result{};
+  for (size_t k = 0; k < members_.size(); ++k) {
+    if (present != nullptr && present[k] == 0) continue;
+    const std::string why = measurement_error(measurements[k]);
+    if (!why.empty()) return fail(BB200_ERR_INVALID_ARGUMENT, "member " + std::to_string(k) + ": " + why);
+  }
+  return step(control_poses, measurements, present, out);
+}
+
+int Batch::step(const double* control_poses, const bb200_measurement* in, const uint8_t* present, bb200_update_result* out) {
   error_.clear();
   const size_t count = members_.size();
   for (size_t k = 0; k < count; ++k) out[k] = bb200_update_result{};
@@ -608,15 +709,19 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   }
   if (active.empty()) return BB200_OK;
 
-  uint64_t points_total = 0;
+  // Points sent by the host come first in the point buffer, in member order; the points of scans and clouds, written by
+  // batch_points_kernel, follow them.  Scans and clouds are sized by their bounds (measurement_bound).
+  uint64_t points_total = 0, host_points = 0, input_floats = 0;
   uint32_t max_points = 0;
   int step_map = -1;            // the map every updating member reads, or -1 when they read several
   std::vector<int> forms(count, kBatchField);
   for (const uint32_t k : active)
     if (members_[k].map < 0) return rollback(fail(BB200_ERR_STATE, maps_.empty() ? "no map set" : "member " + std::to_string(k) + " has no map"));
   for (const uint32_t k : active) {
-    if (n_points[k] > 0xffffffffull) return rollback(fail(BB200_ERR_INVALID_ARGUMENT, "too many points"));
-    if (n_points[k] > 0 && points_xy[k] == nullptr) return rollback(fail(BB200_ERR_INVALID_ARGUMENT, "points_xy is null"));
+    const uint64_t bound = measurement_bound(in[k]);
+    if (bound > 0xffffffffull) return rollback(fail(BB200_ERR_INVALID_ARGUMENT, "too many points"));
+    if (in[k].kind == BB200_MEASUREMENT_POINTS && in[k].n_points > 0 && in[k].points_xy == nullptr)
+      return rollback(fail(BB200_ERR_INVALID_ARGUMENT, "points_xy is null"));
     const int id = members_[k].map;
     const DeviceMap& map = maps_.at(id).map;
     if (plans[k].resample && plans[k].random_state_probability > 0.0 && map.n_free == 0)
@@ -624,23 +729,31 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     // The beam model walks a member's rays in two passes when its map allows it (the rule of the single filter).
     if (map.sensor == BB200_SENSOR_BEAM) forms[k] = beam_two_pass_map(map) ? kBatchBeamTwoPass : kBatchBeamFused;
     step_map = k == active.front() || step_map == id ? id : -1;
-    points_total += n_points[k];
-    max_points = std::max(max_points, static_cast<uint32_t>(n_points[k]));
+    points_total += bound;
+    if (in[k].kind == BB200_MEASUREMENT_POINTS) host_points += bound;
+    input_floats += in[k].kind == BB200_MEASUREMENT_CLOUD ? 3 * bound : in[k].kind == BB200_MEASUREMENT_SCAN ? bound : 0;
+    max_points = std::max(max_points, static_cast<uint32_t>(bound));
   }
+  const bool convert = std::any_of(active.begin(), active.end(), [&](uint32_t k) { return in[k].kind != BB200_MEASUREMENT_POINTS; });
   int st = check(cudaSetDevice(device_), "cudaSetDevice");
   if (st == BB200_OK) st = ensure_points(points_total);  // the previous step has ended: the staging buffers are free
   if (st == BB200_OK && step_map < 0) st = ensure_map_table();
+  if (st == BB200_OK && convert) st = ensure_inputs(input_floats);
+  for (auto k = active.begin(); st == BB200_OK && k != active.end(); ++k)
+    if (in[*k].kind == BB200_MEASUREMENT_SCAN) st = ensure_scan_table(members_[*k], *in[*k].scan);
   if (st != BB200_OK) return rollback(st);
 
   // The step's member table and the concatenated scans.
   const uint32_t n_active = static_cast<uint32_t>(active.size());
   BatchStepArgs a{};
   a.n_members = n_active;
-  uint64_t point_offset = 0, hit_words = 0;
+  uint64_t point_offset = 0, device_offset = host_points, input_offset = 0, hit_words = 0;
   for (uint32_t j = 0; j < n_active; ++j) {
     const uint32_t k = active[j];
     const Member& m = members_[k];
     const bb200_step_plan& plan = plans[k];
+    const bb200_measurement& meas = in[k];
+    const uint64_t bound = measurement_bound(meas);
     BatchMember& b = table_host_.get()[j];
     b = BatchMember{};
     b.offset = m.offset;
@@ -657,15 +770,49 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     b.pivot_x = m.pivot[0];
     b.pivot_y = m.pivot[1];
     b.sampling = to_kernel_sampling(plan.sampling);
-    b.point_offset = point_offset;
-    b.n_points = static_cast<uint32_t>(n_points[k]);
-    b.points_radius = scan_radius(points_xy[k], n_points[k]);
-    if (n_points[k] > 0) std::memcpy(points_host_.get() + 2 * point_offset, points_xy[k], 2 * n_points[k] * sizeof(double));
-    point_offset += n_points[k];
+    if (meas.kind == BB200_MEASUREMENT_POINTS) {
+      b.point_offset = point_offset;
+      b.n_points = static_cast<uint32_t>(meas.n_points);
+      b.points_radius = scan_radius(meas.points_xy, meas.n_points);
+      if (meas.n_points > 0) std::memcpy(points_host_.get() + 2 * point_offset, meas.points_xy, 2 * meas.n_points * sizeof(double));
+      point_offset += meas.n_points;
+    } else {
+      b.point_offset = device_offset;
+      b.n_points = static_cast<uint32_t>(bound);  // a scan's survivors replace it on the device
+      b.points_radius = 0.0;                      // raised to the points' largest |x| + |y| on the device
+      device_offset += bound;
+    }
+    if (convert) {
+      BatchPointsMember& d = inputs_.host.get()[j];
+      d = BatchPointsMember{};
+      d.kind = meas.kind;
+      d.input_offset = input_offset;
+      d.count = static_cast<uint32_t>(bound);
+      float* raw = input_host_.get() + input_offset;
+      if (meas.kind == BB200_MEASUREMENT_SCAN) {
+        const bb200_laser_scan& scan = *meas.scan;
+        const std::vector<uint64_t>& indices = m.scan.indices;
+        for (uint64_t pos = 0; pos < bound; ++pos) raw[pos] = scan.ranges[indices[pos]];
+        d.min_range = scan.min_range;
+        d.max_range = scan.max_range;
+        d.directions = m.scan.directions.get();
+        set_origin(d, scan.laser_origin);
+        input_offset += bound;
+      } else if (meas.kind == BB200_MEASUREMENT_CLOUD) {
+        const bb200_point_cloud& cloud = *meas.cloud;
+        if (cloud.datatype == BB200_POINT_FLOAT32) {
+          pack_cloud<float>(cloud, raw);
+        } else {
+          pack_cloud<double>(cloud, raw);
+        }
+        set_origin(d, cloud.origin);
+        input_offset += 3 * bound;
+      }
+    }
     b.hit_stride = (m.n + 31) / 32 * 32;
     if (forms[k] == kBatchBeamTwoPass) {
       b.hit_offset = hit_words;
-      hit_words += b.hit_stride * n_points[k];
+      hit_words += b.hit_stride * bound;
     }
   }
   // The two-pass members keep that form when their hit words fit under the single filter's bound for one pass and in
@@ -685,6 +832,16 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
     }
   }
   for (int l = 0; l < kBatchLaunches; ++l) first_host_.get()[static_cast<size_t>(l) * (n_active + 1) + n_active] = a.ctas[l];
+  BatchPointsArgs pa{};
+  if (convert) {
+    uint32_t* row = first_host_.get() + static_cast<size_t>(kBatchPointsRow) * (n_active + 1);
+    for (uint32_t j = 0; j < n_active; ++j) {
+      row[j] = pa.ctas;
+      pa.ctas += batch_points_ctas(inputs_.host.get()[j]);
+    }
+    row[n_active] = pa.ctas;
+  }
+  const int rows = convert ? kBatchLaunches + 1 : kBatchLaunches;
 
   cudaStream_t stream = stream_;
   for (const uint32_t k : active) members_[k].cdf_total = 0;  // from here on the step may have rewritten their CDFs
@@ -692,10 +849,24 @@ int Batch::update(const double* control_poses, const double* const* points_xy, c
   *ticket_host_.get() = 0;
   st = check(cudaMemcpyAsync(table_.get(), table_host_.get(), n_active * sizeof(BatchMember), cudaMemcpyHostToDevice, stream), "upload member table");
   if (st == BB200_OK)
-    st = check(cudaMemcpyAsync(first_.get(), first_host_.get(), kBatchLaunches * (n_active + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), "upload ranges");
-  if (st == BB200_OK && points_total > 0)
-    st = check(cudaMemcpyAsync(points_.get(), points_host_.get(), 2 * points_total * sizeof(double), cudaMemcpyHostToDevice, stream), "upload points");
+    st = check(cudaMemcpyAsync(first_.get(), first_host_.get(), rows * (n_active + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), "upload ranges");
+  if (st == BB200_OK && host_points > 0)
+    st = check(cudaMemcpyAsync(points_.get(), points_host_.get(), 2 * host_points * sizeof(double), cudaMemcpyHostToDevice, stream), "upload points");
+  if (st == BB200_OK && convert)
+    st = check(cudaMemcpyAsync(inputs_.device.get(), inputs_.host.get(), n_active * sizeof(BatchPointsMember), cudaMemcpyHostToDevice, stream),
+               "upload measurement table");
+  if (st == BB200_OK && input_floats > 0)
+    st = check(cudaMemcpyAsync(input_.get(), input_host_.get(), input_floats * sizeof(float), cudaMemcpyHostToDevice, stream), "upload measurements");
   if (st != BB200_OK) return rollback(st);
+  if (convert) {
+    pa.members = table_.get();
+    pa.first = first_.get() + static_cast<size_t>(kBatchPointsRow) * (n_active + 1);
+    pa.n_members = n_active;
+    pa.inputs = inputs_.device.get();
+    pa.input = input_.get();
+    pa.points = points_.get();
+    launches_ += static_cast<uint64_t>(launch_batch_points(pa, stream));
+  }
   a.members = table_.get();
   a.first = first_.get();
   a.max_points = max_points;

@@ -73,6 +73,10 @@ class Batch {
   /// batch: when the device half fails, every member's host state is rolled back.
   int update(const double* control_poses, const double* const* points_xy, const uint64_t* n_points, const uint8_t* present,
              bb200_update_result* out);
+  /// update with each member's measurement as base-frame points, a laser scan or a point cloud
+  /// (bb200_amcl_batch_update_measurements): every present member's measurement is checked first, and scans and clouds
+  /// are converted on the device by one more launch.
+  int update_measurements(const double* control_poses, const bb200_measurement* measurements, const uint8_t* present, bb200_update_result* out);
 
  private:
   struct Member {
@@ -90,6 +94,16 @@ class Batch {
     // cdf_valid_): set by a step that normalised and by a rebuild in sample_states; 0 (stale) after a resampling step,
     // an initialisation or a failed step.
     unsigned long long cdf_total{0};
+    // The beam directions of the last scan it passed (update_measurements), kept until the scan geometry changes: the
+    // key, the kept readings' indices and their (cos, sin) on the device.
+    struct ScanTable {
+      bool valid{false};
+      uint64_t n_ranges{0}, max_beams{0};
+      uint32_t angle_min_bits{0}, angle_increment_bits{0};
+      std::vector<uint64_t> indices;
+      DeviceBuffer<double2> directions;
+    };
+    ScanTable scan;
   };
   struct MapEntry {
     DeviceMap map;
@@ -103,6 +117,10 @@ class Batch {
   int member_ok(int member) const;
   const MapEntry* find_map(int id) const;
   int ensure_points(uint64_t n_points);
+  int ensure_inputs(uint64_t floats);
+  int ensure_scan_table(Member& m, const bb200_laser_scan& scan);
+  /// The step of update and update_measurements: in[m] is member m's measurement, already checked when it is a scan or a cloud.
+  int step(const double* control_poses, const bb200_measurement* in, const uint8_t* present, bb200_update_result* out);
   bool ensure_hits(uint64_t words);
   int set_map(const MapTables& tables);
   int add_map(const MapTables& tables, int* id);
@@ -139,10 +157,19 @@ class Batch {
   DeviceBuffer<double> partials_;
   DeviceBuffer<BatchMember> table_;
   PinnedBuffer<BatchMember> table_host_;
-  DeviceBuffer<uint32_t> first_;  // kBatchLaunches x (K + 1)
+  DeviceBuffer<uint32_t> first_;  // (kBatchLaunches + 1) x (K + 1): the step's rows, then batch_points_kernel's
   PinnedBuffer<uint32_t> first_host_;
   DeviceBuffer<double> points_;   // (x, y) pairs
   PinnedBuffer<double> points_host_;
+  // Scans and clouds of update_measurements (allocated on first use): batch_points_kernel's member table and the raw
+  // measurements (kept ranges, or x, y, z per cloud point).
+  struct InputTable {
+    DeviceBuffer<BatchPointsMember> device;
+    PinnedBuffer<BatchPointsMember> host;
+  };
+  InputTable inputs_;
+  DeviceBuffer<float> input_;
+  PinnedBuffer<float> input_host_;
   DeviceBuffer<uint32_t> hits_;   // beam model, two-pass form: the step's hit words (grows only)
   PinnedBuffer<StepSummary> summary_host_;  // one per member of the step's table
   PinnedBuffer<int> ticket_host_;

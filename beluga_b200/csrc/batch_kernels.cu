@@ -294,6 +294,114 @@ __global__ void __launch_bounds__(kRsThreads) batch_sample_kernel(BatchSampleArg
   if (local == 0 && threadIdx.x == 0) s.totals[k] = m.total != 0 ? m.total : scalars->total;
 }
 
+// ---- scans and point clouds of a batch step (before the step's launches) -------------------------------------------
+
+constexpr int kPtThreads = 256;
+constexpr uint32_t kBatchCloudPointsPerCta = 16 * kPtThreads;
+
+/// Bit pattern of |x| + |y| that orders like scan_radius's result (filter.cu): non-negative doubles order like their bits,
+/// and every NaN becomes the one pattern above +inf, so that the largest pattern is NaN when some term is.
+__device__ __forceinline__ unsigned long long radius_bits(double x, double y) {
+  const double r = fabs(x) + fabs(y);
+  return isnan(r) ? 0x7ff8000000000000ull : static_cast<unsigned long long>(__double_as_longlong(r));
+}
+
+/// The largest of every thread's `bits`, in thread 0.
+__device__ __forceinline__ unsigned long long block_max_bits(unsigned long long bits) {
+  __shared__ unsigned long long s_max[kPtThreads / kWarp];
+#pragma unroll
+  for (int o = kWarp / 2; o > 0; o >>= 1) bits = max(bits, __shfl_xor_sync(0xffffffffu, bits, o));
+  if ((threadIdx.x & (kWarp - 1)) == 0) s_max[threadIdx.x / kWarp] = bits;
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (int w = 1; w < kPtThreads / kWarp; ++w) bits = max(bits, s_max[w]);
+  return bits;
+}
+
+/// A scan member (one CTA): bb200_scan_to_points's loop over the kept beams with the directions given, the survivors
+/// compacted in beam order, chunk by chunk; n_points and points_radius of the member follow.
+__device__ __forceinline__ void scan_points_block(const BatchPointsMember& in, const float* __restrict__ ranges, double2* __restrict__ out,
+                                                  BatchMember& m) {
+  __shared__ uint32_t s_warp[kPtThreads / kWarp];
+  const uint32_t lane = threadIdx.x & (kWarp - 1), warp = threadIdx.x / kWarp;
+  const double* o = in.origin;
+  uint32_t kept = 0;
+  unsigned long long bits = 0;
+  for (uint64_t base = 0; base < in.count; base += kPtThreads) {
+    const uint64_t i = base + threadIdx.x;
+    bool keep = false;
+    double px = 0.0, py = 0.0;
+    if (i < in.count) {
+      const double r = static_cast<double>(ranges[i]);
+      keep = !(isnan(r) || !(r >= in.min_range) || !(r <= in.max_range));  // laser_scan.hpp:80-84
+      if (keep) {
+        const double2 d = in.directions[i];
+        const double x = r * d.x, y = r * d.y;
+        px = x;
+        py = y;
+        if (in.has_origin) {  // origin * (x, y, 0), keep (x, y)  (beluga_ros/src/amcl.cpp:59-61)
+          px = (o[0] * x + o[1] * y) + o[3];
+          py = (o[4] * x + o[5] * y) + o[7];
+        }
+      }
+    }
+    const uint32_t ballot = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) s_warp[warp] = __popc(ballot);
+    __syncthreads();
+    uint32_t before = 0, total = 0;
+#pragma unroll
+    for (int w = 0; w < kPtThreads / kWarp; ++w) {
+      before += w < static_cast<int>(warp) ? s_warp[w] : 0u;
+      total += s_warp[w];
+    }
+    if (keep) {
+      out[kept + before + __popc(ballot & ((1u << lane) - 1u))] = make_double2(px, py);
+      bits = max(bits, radius_bits(px, py));
+    }
+    kept += total;
+    __syncthreads();  // every warp has read s_warp before the next chunk writes it
+  }
+  bits = block_max_bits(bits);
+  if (threadIdx.x == 0) {
+    m.n_points = kept;
+    m.points_radius = __longlong_as_double(static_cast<long long>(bits));
+  }
+}
+
+/// CTA `local` of a cloud member: cloud_to_points (c_api.cu) on its kBatchCloudPointsPerCta points, from the packed floats;
+/// the member's points_radius (0 when the step began) takes the CTA's largest term.
+__device__ __forceinline__ void cloud_points_block(const BatchPointsMember& in, const float* __restrict__ xyz, double2* __restrict__ out,
+                                                   BatchMember& m, uint32_t local) {
+  const double* o = in.origin;
+  unsigned long long bits = 0;
+  const uint64_t end = min(static_cast<uint64_t>(in.count), (static_cast<uint64_t>(local) + 1) * kBatchCloudPointsPerCta);
+  for (uint64_t i = static_cast<uint64_t>(local) * kBatchCloudPointsPerCta + threadIdx.x; i < end; i += kPtThreads) {
+    const double x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
+    double px = x, py = y;
+    if (in.has_origin) {
+      px = ((o[0] * x + o[1] * y) + o[2] * z) + o[3];
+      py = ((o[4] * x + o[5] * y) + o[6] * z) + o[7];
+    }
+    out[i] = make_double2(px, py);
+    bits = max(bits, radius_bits(px, py));
+  }
+  bits = block_max_bits(bits);
+  if (threadIdx.x == 0 && bits != 0) atomicMax(reinterpret_cast<unsigned long long*>(&m.points_radius), bits);
+}
+
+__global__ void __launch_bounds__(kPtThreads) batch_points_kernel(BatchPointsArgs s) {
+  uint32_t local, count;
+  const uint32_t j = batch_member_of(s, 0, blockIdx.x, local, count);
+  const BatchPointsMember& in = s.inputs[j];
+  BatchMember& m = s.members[j];
+  double2* out = reinterpret_cast<double2*>(s.points) + m.point_offset;
+  if (in.kind == kBatchInputScan) {
+    scan_points_block(in, s.input + in.input_offset, out, m);
+  } else {
+    cloud_points_block(in, s.input + in.input_offset, out, m, local);
+  }
+}
+
 template <bool kTable>
 int launch_batch_step_from(const BatchStepArgs& s, cudaStream_t stream) {
   const uint32_t reset = std::max(s.n_members, s.ctas[kBatchScan]);
@@ -340,6 +448,18 @@ void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunch
 
 int launch_batch_step(const BatchStepArgs& s, cudaStream_t stream) {
   return s.maps != nullptr ? launch_batch_step_from<true>(s, stream) : launch_batch_step_from<false>(s, stream);
+}
+
+uint32_t batch_points_ctas(const BatchPointsMember& m) {
+  if (m.kind == kBatchInputScan) return 1;
+  if (m.kind == kBatchInputCloud)
+    return std::max(1u, static_cast<uint32_t>((static_cast<uint64_t>(m.count) + kBatchCloudPointsPerCta - 1) / kBatchCloudPointsPerCta));
+  return 0;
+}
+
+int launch_batch_points(const BatchPointsArgs& s, cudaStream_t stream) {
+  batch_points_kernel<<<s.ctas, kPtThreads, 0, stream>>>(s);
+  return 1;
 }
 
 void batch_sample_ctas(const BatchSampleMember& m, bool rebuilt, uint32_t out[kSampleLaunches]) {

@@ -14,6 +14,7 @@
 #include "batch.hpp"
 #include "cluster_host.hpp"
 #include "filter.hpp"
+#include "measurement_host.hpp"
 
 using bb200::Amcl;
 using bb200::Batch;
@@ -87,23 +88,14 @@ int guarded_create(Body&& body) noexcept {
   return guarded(c, body);
 }
 
-/// One coordinate of a packed point cloud record.  The record has no alignment guarantee (PointCloud2 packs its fields),
-/// hence the copy.  float64 values are narrowed to float: SparsePointCloud3f casts them (sparse_point_cloud.hpp:106-116).
-template <class Scalar>
-double cloud_scalar(const unsigned char* p) {
-  Scalar v;
-  std::memcpy(&v, p, sizeof(Scalar));
-  return static_cast<double>(static_cast<float>(v));
-}
-
 /// SparsePointCloud3f::points() | transform(origin * p, keep (x, y))  (beluga_ros/src/amcl.cpp:73-78)
 template <class Scalar>
 void cloud_to_points(const bb200_point_cloud& c, double* points_xy) {
-  const unsigned char* base = static_cast<const unsigned char*>(c.data) + c.x_offset;
   const double* m = c.origin;
   for (uint64_t i = 0; i < c.n_points; ++i) {
-    const unsigned char* p = base + i * c.point_step;
-    const double x = cloud_scalar<Scalar>(p), y = cloud_scalar<Scalar>(p + sizeof(Scalar)), z = cloud_scalar<Scalar>(p + 2 * sizeof(Scalar));
+    float xyz[3];
+    bb200::cloud_point<Scalar>(c, i, xyz);
+    const double x = xyz[0], y = xyz[1], z = xyz[2];
     double px = x, py = y;
     if (m != nullptr) {
       px = ((m[0] * x + m[1] * y) + m[2] * z) + m[3];
@@ -524,21 +516,13 @@ int bb200_take_evenly_indices(uint64_t size, uint64_t count, uint64_t* indices, 
 
 int bb200_scan_to_points(const bb200_laser_scan* scan, double* points_xy, uint64_t capacity, uint64_t* n_points) {
   BB_REQUIRE(scan && points_xy && n_points && (scan->ranges || scan->n_ranges == 0));
-  const uint64_t size = scan->n_ranges;
-  const uint64_t count = scan->max_beams == 0 ? size : scan->max_beams;
-  const uint64_t kept = size == 0 ? 0 : (count > size ? size : count);
+  const uint64_t kept = bb200::scan_beam_count(*scan);
   uint64_t n = 0;
   for (uint64_t pos = 0; pos < kept; ++pos) {
-    uint64_t i = pos;
-    if (count <= size && pos != 0) {
-      const uint64_t a = pos * (size - 1), b = count - 1;
-      i = a / b + ((a % b == 0) ? 0 : 1);
-    }
-    const double range = static_cast<double>(scan->ranges[i]);
-    // beluga_ros/laser_scan.hpp:73-74: float arithmetic, then widened.
-    const double theta = static_cast<double>(scan->angle_min + static_cast<float>(static_cast<int>(i)) * scan->angle_increment);
-    if (std::isnan(range) || !(range >= scan->min_range) || !(range <= scan->max_range)) continue;  // laser_scan.hpp:80-84
-    const double x = range * std::cos(theta), y = range * std::sin(theta);                           // laser_scan.hpp:66-69
+    const bb200::ScanBeam beam = bb200::scan_beam(*scan, pos);
+    const double range = static_cast<double>(scan->ranges[beam.index]);
+    if (!bb200::scan_range_kept(range, *scan)) continue;
+    const double x = range * beam.c, y = range * beam.s;
     double px = x, py = y;
     if (scan->laser_origin != nullptr) {  // origin * (x, y, 0), keep (x, y)  (beluga_ros/src/amcl.cpp:59-61)
       const double* m = scan->laser_origin;
@@ -567,13 +551,9 @@ int bb200_amcl_update_scan(bb200_amcl* a, const double control_pose[4], const bb
 
 int bb200_point_cloud_to_points(const bb200_point_cloud* cloud, double* points_xy, uint64_t capacity, uint64_t* n_points) {
   BB_REQUIRE(cloud && n_points && (points_xy || capacity == 0));
-  const bool f32 = cloud->datatype == BB200_POINT_FLOAT32;
-  BB_REQUIRE(f32 || cloud->datatype == BB200_POINT_FLOAT64);
-  const uint64_t scalar = f32 ? sizeof(float) : sizeof(double);
-  BB_REQUIRE(static_cast<uint64_t>(cloud->x_offset) + 3 * scalar <= cloud->point_step);
-  BB_REQUIRE(cloud->data || cloud->n_points == 0);
+  BB_REQUIRE(bb200::cloud_valid(*cloud));
   if (cloud->n_points > capacity) return BB200_ERR_CAPACITY;
-  if (f32) {
+  if (cloud->datatype == BB200_POINT_FLOAT32) {
     cloud_to_points<float>(*cloud, points_xy);
   } else {
     cloud_to_points<double>(*cloud, points_xy);
@@ -904,6 +884,11 @@ int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, co
                             const uint8_t* present, bb200_update_result* out) {
   BB_REQUIRE(b && control_poses && points_xy && n_points && out);
   return guarded(b->impl, [&] { return b->impl.update(control_poses, points_xy, n_points, present, out); });
+}
+int bb200_amcl_batch_update_measurements(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements,
+                                         const uint8_t* present, bb200_update_result* out) {
+  BB_REQUIRE(b && control_poses && measurements && out);
+  return guarded(b->impl, [&] { return b->impl.update_measurements(control_poses, measurements, present, out); });
 }
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.launch_count() : 0; }
 

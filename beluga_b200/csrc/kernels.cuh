@@ -500,6 +500,38 @@ static_assert(sizeof(BatchStepArgs) <= 1024, "the step's arguments travel as one
 int launch_batch_step(const BatchStepArgs& args, cudaStream_t stream);
 /// Scan tiles of a member of n particles (the quantise-scan CTAs it needs).
 uint32_t batch_scan_tiles(uint64_t n);
+
+// ---- batches: laser scans and point clouds converted on the device ------------------------------------------
+// A step whose members pass scans or clouds runs batch_points_kernel first: it writes each such member's base-frame points
+// at its point_offset, and its n_points and points_radius into the step's member table, which the step's kernels then read
+// in stream order.  Its CTA ranges are one more row of the step's `first` buffer, after the kBatchLaunches rows.
+constexpr int kBatchPointsRow = kBatchLaunches;
+/// How a member's measurement reaches a batch step (the values of bb200_measurement_kind).
+enum BatchInputKind : int { kBatchInputPoints = 0, kBatchInputScan = 1, kBatchInputCloud = 2 };
+/// One member of batch_points_kernel, built on the host every step (one per entry of the step's member table).
+struct BatchPointsMember {
+  int kind;                   // BatchInputKind; kBatchInputPoints: the host wrote the points, no CTA
+  int has_origin;             // 0: no sensor origin, the sensor frame's (x, y) pass unchanged
+  uint64_t input_offset;      // first float of the member in BatchPointsArgs::input: kept ranges, or x, y, z per cloud point
+  uint32_t count;             // kept beams or cloud points
+  double min_range, max_range;
+  double origin[8];           // rows 0 and 1 of the sensor origin's [R | t]
+  const double2* directions;  // scans: (cos, sin) of each kept beam, computed on the host (measurement_host.hpp)
+};
+struct BatchPointsArgs {
+  BatchMember* members;             // the step's member table: point_offset read, n_points and points_radius written
+  const uint32_t* first;            // device: one row of n_members + 1 CTA prefixes
+  uint32_t n_members;
+  uint32_t ctas;
+  const BatchPointsMember* inputs;  // device, one per member of the table
+  const float* input;               // device: every converted member's raw measurement
+  double* points;                   // the step's (x, y) pairs
+};
+/// CTAs of a member in batch_points_kernel: none for points, one for a scan (its beams in order, compacted by a block scan),
+/// one per kBatchCloudPointsPerCta points of a cloud (at least one).
+uint32_t batch_points_ctas(const BatchPointsMember& m);
+/// One launch converting every scan and cloud member of the step's table.  Returns the number of launches (1).
+int launch_batch_points(const BatchPointsArgs& args, cudaStream_t stream);
 /// CTAs of a member in each row of a batch step's ranges, for a member that takes reweight form `form`.
 void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunches]);
 

@@ -632,6 +632,33 @@ int bb200_amcl_batch_sample_states(bb200_amcl_batch* b, const uint64_t* counts, 
  * every member's host state is as if it had not been made. */
 int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, const double* const* points_xy, const uint64_t* n_points,
                             const uint8_t* present, bb200_update_result* out);
+/* One member's measurement in a step: base-frame points, a laser scan or a point cloud, each as the single filter's
+ * bb200_amcl_update, bb200_amcl_update_scan and bb200_amcl_update_point_cloud take it.  Only the fields of `kind` are read. */
+typedef enum bb200_measurement_kind { BB200_MEASUREMENT_POINTS = 0, BB200_MEASUREMENT_SCAN = 1, BB200_MEASUREMENT_CLOUD = 2 } bb200_measurement_kind;
+typedef struct bb200_measurement {
+  int kind;                        /* bb200_measurement_kind */
+  const double* points_xy;         /* POINTS: n_points (x, y) pairs (NULL when n_points == 0) */
+  uint64_t n_points;
+  const bb200_laser_scan* scan;    /* SCAN */
+  const bb200_point_cloud* cloud;  /* CLOUD */
+} bb200_measurement;
+/* bb200_amcl_batch_update with measurements[m] as member m's input, so that members with 2-D lidars, 3-D lidars and
+ * points step in one call.  Scans and clouds are converted on the device: the host sends 4 bytes per kept beam (the
+ * range) or 12 bytes per cloud point (x, y, z as floats), and the beam directions, computed on the host as
+ * bb200_scan_to_points computes them, are uploaded once per scan geometry (n_ranges, max_beams, angle_min,
+ * angle_increment) and member.  A step in which some updating member passes a scan or a cloud takes one kernel launch
+ * more than bb200_amcl_batch_update's count; a step whose updating members all pass points takes the same launches.
+ *
+ * Bit-identity: every present member's out[m], particles, ancestors and later steps are bit-identical to a standalone
+ * bb200_amcl with the same parameters fed bb200_amcl_update_scan / bb200_amcl_update_point_cloud / bb200_amcl_update,
+ * and to bb200_amcl_batch_update given the points bb200_scan_to_points / bb200_point_cloud_to_points return.
+ * Validation: BB200_ERR_INVALID_ARGUMENT, before anything reaches the device, for a null handle, control_poses,
+ * measurements or out, and for a present member whose measurement the single filter refuses: an unknown kind, a null
+ * scan or cloud, null ranges or points with a non-zero count, a cloud datatype other than 7 or 8, or
+ * x_offset + 3 * sizeof(scalar) > point_step.  Every present member is checked, whether it updates in this step or not.
+ * Atomicity: as bb200_amcl_batch_update -- on failure every member's host state is as if the call had not been made. */
+int bb200_amcl_batch_update_measurements(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements,
+                                         const uint8_t* present, bb200_update_result* out);
 /* Kernel launches issued by this batch so far (steps, initialisations, cluster estimates, particle-cloud histograms and
  * pose samples, and the beam model's map uploads). */
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b);

@@ -18,6 +18,7 @@
 #include <map>
 #include <optional>
 #include <utility>
+#include <variant>
 
 #include "models.hpp"
 
@@ -299,15 +300,72 @@ class AmclBatch {
     }
     std::vector<bb200_update_result> r(k);
     check(bb200_amcl_batch_update(handle_, controls.front().data(), pts.data(), counts.data(), present != nullptr ? mask.data() : nullptr, r.data()));
-    std::vector<std::optional<estimation_type>> out(k);
-    for (std::size_t m = 0; m < k; ++m) {
-      if (!r[m].updated) continue;
-      Matrix3d cov;
-      for (int i = 0; i < 9; ++i) cov[i] = r[m].estimate.cov[i];
-      out[m] = std::make_pair(SE2d::from_data(r[m].estimate.mean), cov);
-    }
-    return out;
+    return estimates_of(r);
   }
+
+  /// One member's measurement in a step: base-frame points, a laser scan or a point cloud, as Amcl::update takes them.  The
+  /// constructors are explicit, so that a braced list of point vectors still selects the points overload above.
+  struct Measurement {
+    explicit Measurement(std::vector<std::pair<double, double>> points) : value(std::move(points)) {}
+    explicit Measurement(const LaserScanView& scan) : value(scan) {}
+    explicit Measurement(const PointCloudView& cloud) : value(cloud) {}
+    std::variant<std::vector<std::pair<double, double>>, LaserScanView, PointCloudView> value;
+  };
+  /// update with member m's measurement in measurements[m], so that members with 2-D and 3-D lidars step in one call; scans
+  /// and clouds are converted on the device (bb200_amcl_batch_update_measurements).  Every member's result equals its
+  /// standalone Amcl::update's with the same measurement.  Throws Error(BB200_ERR_INVALID_ARGUMENT) before any member
+  /// changes when some present member's scan or cloud is unusable.
+  auto update(const std::vector<SE2d>& controls, const std::vector<Measurement>& measurements, const std::vector<bool>* present = nullptr)
+      -> std::vector<std::optional<estimation_type>> {
+    const std::size_t k = size();
+    if (controls.size() != k || measurements.size() != k || (present != nullptr && present->size() != k))
+      throw Error(BB200_ERR_INVALID_ARGUMENT, "one control, one measurement (and one presence flag) per member");
+    static_assert(sizeof(SE2d) == 4 * sizeof(double), "SE2d must be four packed doubles");
+    std::vector<bb200_laser_scan> scans(k);
+    std::vector<bb200_point_cloud> clouds(k);
+    std::vector<bb200_measurement> in(k);
+    std::vector<std::uint8_t> mask(present != nullptr ? k : 0);
+    for (std::size_t m = 0; m < k; ++m) {
+      const auto& v = measurements[m].value;
+      if (const auto* points = std::get_if<0>(&v)) {
+        in[m] = bb200_measurement{BB200_MEASUREMENT_POINTS, points->empty() ? nullptr : &points->front().first, points->size(), nullptr, nullptr};
+      } else if (const auto* scan = std::get_if<LaserScanView>(&v)) {
+        scans[m] = scan->c_view();
+        in[m] = bb200_measurement{BB200_MEASUREMENT_SCAN, nullptr, 0, &scans[m], nullptr};
+      } else {
+        clouds[m] = std::get<PointCloudView>(v).c_view();
+        in[m] = bb200_measurement{BB200_MEASUREMENT_CLOUD, nullptr, 0, nullptr, &clouds[m]};
+      }
+      if (present != nullptr) mask[m] = (*present)[m] ? 1 : 0;
+    }
+    std::vector<bb200_update_result> r(k);
+    check(bb200_amcl_batch_update_measurements(handle_, controls.front().data(), in.data(), present != nullptr ? mask.data() : nullptr, r.data()));
+    return estimates_of(r);
+  }
+  /// update with a laser scan for every member (beluga_ros::Amcl::update(base_pose_in_odom, laser_scan) per member).
+  auto update(const std::vector<SE2d>& controls, const std::vector<LaserScanView>& scans, const std::vector<bool>* present = nullptr)
+      -> std::vector<std::optional<estimation_type>> {
+    return update(controls, std::vector<Measurement>(scans.begin(), scans.end()), present);
+  }
+  /// update with a point cloud for every member (beluga_ros::Amcl::update(base_pose_in_odom, point_cloud) per member).
+  auto update(const std::vector<SE2d>& controls, const std::vector<PointCloudView>& clouds, const std::vector<bool>* present = nullptr)
+      -> std::vector<std::optional<estimation_type>> {
+    return update(controls, std::vector<Measurement>(clouds.begin(), clouds.end()), present);
+  }
+#ifdef BELUGA_B200_WITH_SOPHUS
+  /// The same for any beluga::BaseSparsePointCloud-shaped clouds, e.g. beluga_ros::SparsePointCloud3f.
+  template <class SparsePointCloud, std::enable_if_t<is_sparse_point_cloud_v<SparsePointCloud>, int> = 0>
+  auto update(const std::vector<SE2d>& controls, const std::vector<SparsePointCloud>& clouds, const std::vector<bool>* present = nullptr)
+      -> std::vector<std::optional<estimation_type>> {
+    std::vector<PackedPointCloud> packed;
+    packed.reserve(clouds.size());
+    for (const auto& c : clouds) packed.emplace_back(c);
+    std::vector<Measurement> views;
+    views.reserve(packed.size());
+    for (const auto& p : packed) views.emplace_back(p.view());
+    return update(controls, views, present);
+  }
+#endif
 
   /// Member m's particle set, copied from the device.
   [[nodiscard]] ParticleSet particles(std::size_t member) const {
@@ -406,6 +464,16 @@ class AmclBatch {
   [[nodiscard]] bb200_amcl_batch* handle() const { return handle_; }
 
  private:
+  static std::vector<std::optional<estimation_type>> estimates_of(const std::vector<bb200_update_result>& r) {
+    std::vector<std::optional<estimation_type>> out(r.size());
+    for (std::size_t m = 0; m < r.size(); ++m) {
+      if (!r[m].updated) continue;
+      Matrix3d cov;
+      for (int i = 0; i < 9; ++i) cov[i] = r[m].estimate.cov[i];
+      out[m] = std::make_pair(SE2d::from_data(r[m].estimate.mean), cov);
+    }
+    return out;
+  }
   int index(std::size_t member) const {
     if (member >= size()) throw Error(BB200_ERR_INVALID_ARGUMENT, "member index out of range");
     return static_cast<int>(member);

@@ -263,6 +263,25 @@ struct PointCloudView {
   [[nodiscard]] bb200_point_cloud c_view() const { return bb200_point_cloud{data, size, point_step, x_offset, datatype, origin}; }
 };
 
+/// A sensor_msgs/LaserScan as beluga_ros::LaserScan reads it (beluga_ros/include/beluga_ros/laser_scan.hpp:69-80): the ranges,
+/// angle_min and angle_increment of the message, the range limits already combined with the node's, the max_beams of
+/// take_evenly (0: every reading) and the laser's frame in the base frame as a 3x4 row-major [R | t] (nullptr: the
+/// identity).  A view: the buffers must outlive it.
+struct LaserScanView {
+  const float* ranges = nullptr;
+  std::uint64_t size = 0;
+  float angle_min = 0.0f;
+  float angle_increment = 0.0f;
+  double min_range = 0.0;
+  double max_range = HUGE_VAL;
+  std::uint64_t max_beams = 0;
+  const double* origin = nullptr;
+
+  [[nodiscard]] bb200_laser_scan c_view() const {
+    return bb200_laser_scan{ranges, size, angle_min, angle_increment, min_range, max_range, max_beams, origin};
+  }
+};
+
 /// The base-frame (x, y) of every point, in order (beluga_ros/src/amcl.cpp:67-78); host only, needs no GPU.
 /// Throws Error(BB200_ERR_INVALID_ARGUMENT) where SparsePointCloud3 throws std::invalid_argument on the layout.
 [[nodiscard]] inline std::vector<std::pair<double, double>> point_cloud_points(const PointCloudView& cloud) {

@@ -6,7 +6,8 @@ update + cluster estimate, the estimate taken for all members in one call and me
 beam model (60 and 720 points per member) against the same members stepped as standalone Amcl.  `batch_maps`: one AmclBatch whose
 members read 1, 4 or 16 likelihood-field maps against one single-map batch per map, and a step mixing likelihood-field and beam members.
 `batch_cloud`: the `batch` members' particle-cloud publish round (histograms and pose samples) in one batched call each against
-K standalone filters publishing in turn.
+K standalone filters publishing in turn.  `batch_measurements`: AmclBatch fed laser scans and point clouds converted on the
+device against host conversion plus the points update.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import json
@@ -454,6 +455,89 @@ def run_batch_cloud():
     return res
 
 
+def run_batch_measurements():
+    """AmclBatch fed sensor messages: K in {1, 16, 64, 256} members x 2000 particles with {100, 1080}-beam laser scans, and 16
+    members with 64 x 1024 = 65 536-point lidar clouds, on the 2000^2 synthetic map.  Two batches step the same members in
+    turn: one with bb200_amcl_batch_update_measurements (scans and clouds converted on the device), one with K calls of
+    bb200_scan_to_points / bb200_point_cloud_to_points and bb200_amcl_batch_update.  The ctypes arguments of every step
+    are built before the timing, so each time is the C calls alone, end to end (median of 20 steps)."""
+    import ctypes as C
+
+    from beluga_b200 import _capi
+
+    lib = _capi.load()
+    res = {}
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    n, steps, warmup = 2000, 20, 3
+    device = device_record()
+    cases = [("scan", k, beams) for beams in (100, 1080) for k in (1, 16, 64, 256)] + [("cloud", 16, 65_536)]
+    scenes = {}
+    for kind, k, size in cases:
+        key = 1080 if kind == "cloud" else size
+        if key not in scenes:
+            scenes[key] = synthetic.make_scenario(grid_size=2000, n_beams=key, steps=warmup + steps + 1)
+        sc = scenes[key]
+        grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+        params = [bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m) for m in range(k)]
+        motions = [bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)]
+        batches = {}
+        for form in ("device", "host"):
+            b = bb.AmclBatch(motions, params)
+            b.set_likelihood_field_map(lfm, grid)
+            for m in range(k):
+                b.initialize(m, sc.initial_mean, sc.initial_cov)
+            batches[form] = b
+        # Every step's messages, one per member (the members of a step share the scene's message).
+        msgs, keep = [], []
+        for t in range(warmup + steps):
+            if kind == "scan":
+                r = np.hypot(*sc.scans[t].T).astype(np.float32)
+                m, kept = bb._laser_scan(r, np.float32(-np.pi), np.float32(2 * np.pi / size), 0.0, float("inf"), 0, None)
+                meas = _capi.Measurement(_capi.MEASUREMENT_SCAN, None, 0, C.pointer(m), None)
+            else:
+                pc = synthetic.make_point_cloud(sc, t, rows=64, azimuths=1024)
+                m, kept = bb._point_cloud(pc.data, pc.point_step, pc.x_offset, pc.datatype, pc.origin, None)
+                meas = _capi.Measurement(_capi.MEASUREMENT_CLOUD, None, 0, None, C.pointer(m))
+            msgs.append((m, (_capi.Measurement * k)(*([meas] * k)), bb.se2(*sc.poses[t])))
+            keep.append(kept)
+        bufs = [np.zeros((size + 1, 2)) for _ in range(k)]
+        ptrs = (C.POINTER(C.c_double) * k)(*[b.ctypes.data_as(C.POINTER(C.c_double)) for b in bufs])
+        counts = (C.c_uint64 * k)()
+        results = (_capi.UpdateResult * k)()
+        wall = {"device": [], "host": []}
+        launches = []
+        for t, (m, table, pose) in enumerate(msgs):
+            poses = np.tile(pose, (k, 1))
+            pp = poses.ctypes.data_as(C.POINTER(C.c_double))
+            before = batches["device"].launch_count()
+            t0 = time.perf_counter()
+            assert lib.bb200_amcl_batch_update_measurements(batches["device"]._h, pp, table, None, results) == 0
+            t1 = time.perf_counter()
+            launches.append(batches["device"].launch_count() - before)
+            assert all(x.updated for x in results)
+            cn = C.c_uint64()
+            for j in range(k):
+                if kind == "scan":
+                    assert lib.bb200_scan_to_points(C.byref(m), ptrs[j], size + 1, C.byref(cn)) == 0
+                else:
+                    assert lib.bb200_point_cloud_to_points(C.byref(m), ptrs[j], size + 1, C.byref(cn)) == 0
+                counts[j] = cn.value
+            assert lib.bb200_amcl_batch_update(batches["host"]._h, pp, ptrs, counts, None, results) == 0
+            t2 = time.perf_counter()
+            if t >= warmup:
+                wall["device"].append((t1 - t0) * 1e3)
+                wall["host"].append((t2 - t1) * 1e3)
+        md, mh = float(np.median(wall["device"])), float(np.median(wall["host"]))
+        per_point = 4 if kind == "scan" else 12
+        res[f"batch_measurements_{kind}_{k}_x_{n}_x_{size}_lfm_2000"] = {
+            "members": k, "particles": n, "kind": kind, "points": size, "steps": steps,
+            "ms_per_step_e2e": md, "ms_per_step_e2e_min_max": [float(np.min(wall["device"])), float(np.max(wall["device"]))],
+            "host_converted_ms_per_step": mh, "host_converted_ms_min_max": [float(np.min(wall["host"])), float(np.max(wall["host"]))],
+            "upload_bytes_per_member": per_point * size, "host_converted_upload_bytes_per_member": 16 * size,
+            "launches_per_step": int(max(launches)), "kernels_ms": {}, "device": device}
+    return res
+
+
 def main():
     out = {}
     which = sys.argv[1:] or ["c1", "c3", "c4"]
@@ -517,6 +601,8 @@ def main():
         out.update(run_batch_beam())
     if "batch_maps" in which:
         out.update(run_batch_maps())
+    if "batch_measurements" in which:
+        out.update(run_batch_measurements())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}

@@ -778,8 +778,11 @@ class AmclBatch:
     number of kernel launches and one synchronisation.  Member m's results and particles equal those of a standalone Amcl
     built from params[m] and motions[m] and fed the same inputs."""
 
-    def __init__(self, motions, params):
-        """`motions[m]`, `params[m]`: member m's motion model and AmclParams (min_particles == max_particles <= 32768)."""
+    def __init__(self, motions, params, adaptive: bool = False):
+        """`motions[m]`, `params[m]`: member m's motion model and AmclParams (max_particles <= 32768, and
+        min_particles == max_particles unless `adaptive`).  adaptive=True (bb200_amcl_batch_create_adaptive) lets members
+        have min_particles < max_particles: they resize their particle sets with KLD on every resampling step, and
+        particles() and ancestors() then return member_size(m) rows."""
         self._lib = _capi.load()
         k = len(params)
         if len(motions) != k:
@@ -787,11 +790,13 @@ class AmclBatch:
         p = (_capi.AmclParam * max(k, 1))(*[q.c() for q in params])
         m = (_capi.MotionParam * max(k, 1))(*[q.c_motion() for q in motions])
         h = C.c_void_p()
-        st = self._lib.bb200_amcl_batch_create(p, m, k, C.byref(h))
+        create = self._lib.bb200_amcl_batch_create_adaptive if adaptive else self._lib.bb200_amcl_batch_create
+        st = create(p, m, k, C.byref(h))
         if st != _capi.OK:
             raise BelugaB200Error(st, self._lib.bb200_create_error().decode())
         self._h = h
         self.params = list(params)
+        self.adaptive = bool(adaptive)
         self._field_shapes = {}  # (height, width) of each likelihood-field map, by id
 
     def close(self):
@@ -872,15 +877,25 @@ class AmclBatch:
     def force_update(self, member: int):
         self._check(self._lib.bb200_amcl_batch_force_update(self._h, member))
 
+    def member_size(self, member: int) -> int:
+        """Member m's current particle count."""
+        n = C.c_uint64(0)
+        self._check(self._lib.bb200_amcl_batch_member_size(self._h, member, C.byref(n)))
+        return n.value
+
+    def _rows(self, member: int) -> int:
+        # a fixed batch keeps its max_particles-row buffers; an adaptive one returns the member's current count
+        return self.member_size(member) if self.adaptive else self.params[member].max_particles
+
     def particles(self, member: int):
-        n = self.params[member].max_particles
+        n = self._rows(member)
         st = np.zeros((n, 4))
         w = np.zeros(n)
-        self._check(self._lib.bb200_amcl_batch_get_particles(self._h, member, _dptr(st), _dptr(w), n))
+        self._check(self._lib.bb200_amcl_batch_get_particles(self._h, member, _dptr(st) if n else None, _dptr(w) if n else None, n))
         return st, w
 
     def ancestors(self, member: int) -> np.ndarray:
-        out = np.zeros(self.params[member].max_particles, dtype=np.int64)
+        out = np.zeros(self._rows(member), dtype=np.int64)
         self._check(self._lib.bb200_amcl_batch_ancestors(self._h, member, out.ctypes.data_as(C.POINTER(C.c_int64)), len(out)))
         return out
 

@@ -212,6 +212,8 @@ SIGNATURES = {
     "bb200_amcl_join_shards": (C.c_int, [_vp, C.c_int, C.c_int, _vp]),
     "bb200_amcl_leave_shards": (C.c_int, [_vp]),
     "bb200_amcl_batch_create": (C.c_int, [_P(AmclParam), _P(MotionParam), C.c_int, _P(_vp)]),
+    "bb200_amcl_batch_create_adaptive": (C.c_int, [_P(AmclParam), _P(MotionParam), C.c_int, _P(_vp)]),
+    "bb200_amcl_batch_member_size": (C.c_int, [_vp, C.c_int, _P(C.c_uint64)]),
     "bb200_amcl_batch_destroy": (None, [_vp]),
     "bb200_amcl_batch_last_error": (C.c_char_p, [_vp]),
     "bb200_amcl_batch_members": (C.c_int, [_vp]),

@@ -20,7 +20,7 @@ uint64_t finish_rows(uint64_t capacity) {
 
 }  // namespace
 
-int Batch::validate(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, std::string* error) {
+int Batch::validate(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bool adaptive, std::string* error) {
   auto reject = [&](const std::string& m) {
     if (error != nullptr) *error = m;
     return static_cast<int>(BB200_ERR_INVALID_ARGUMENT);
@@ -32,7 +32,9 @@ int Batch::validate(const bb200_amcl_param* params, const bb200_motion_param* mo
     const std::string who = "member " + std::to_string(k) + ": ";
     if (p.device != params[0].device) return reject(who + "all members of a batch share one device");
     if (p.max_particles == 0 || p.max_particles > kBatchMaxParticles) return reject(who + "max_particles must lie in [1, 32768]");
-    if (p.min_particles != p.max_particles) return reject(who + "a batch member keeps a fixed particle count (min_particles == max_particles)");
+    if (!adaptive && p.min_particles != p.max_particles)
+      return reject(who + "a batch member keeps a fixed particle count (min_particles == max_particles)");
+    if (p.min_particles > p.max_particles) return reject(who + "need 0 < min_particles <= max_particles");  // bb200_amcl_create's check
     if (p.selective_resampling) return reject(who + "selective resampling is not supported in a batch");
     if (p.shard_first_index != 0 || p.shard_capacity != 0) return reject(who + "a batch member is not sharded");
     if (!(p.alpha_slow >= 0.0) || !(p.alpha_slow <= p.alpha_fast)) return reject(who + "need 0 <= alpha_slow <= alpha_fast");
@@ -41,8 +43,8 @@ int Batch::validate(const bb200_amcl_param* params, const bb200_motion_param* mo
   return BB200_OK;
 }
 
-Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members) {
-  create_status_ = validate(params, motions, n_members, &error_);
+Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bool adaptive) {
+  create_status_ = validate(params, motions, n_members, adaptive, &error_);
   if (create_status_ != BB200_OK) return;
   uint64_t tiles = 0, rows = 0;
   members_.reserve(static_cast<size_t>(n_members));
@@ -79,8 +81,8 @@ Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, 
   BB_TRY(partials_.allocate(rows * kMomentCount));
   BB_TRY(table_.allocate(members_.size()));
   BB_TRY(table_host_.allocate(members_.size()));
-  BB_TRY(first_.allocate((kBatchLaunches + 1) * k1));
-  BB_TRY(first_host_.allocate((kBatchLaunches + 1) * k1));
+  BB_TRY(first_.allocate(kBatchRows * k1));
+  BB_TRY(first_host_.allocate(kBatchRows * k1));
   BB_TRY(summary_host_.allocate(members_.size()));
   BB_TRY(ticket_host_.allocate(1));
   BB_TRY(members_done_.allocate(1));
@@ -308,6 +310,12 @@ int Batch::get_particles(int member, double* states, double* weights, uint64_t c
   return BB200_OK;
 }
 
+int Batch::member_size(int member, uint64_t* n) const {
+  BB_MEMBER(member);
+  *n = members_[static_cast<size_t>(member)].n;
+  return BB200_OK;
+}
+
 int Batch::ancestors(int member, int64_t* out, uint64_t capacity) {
   BB_MEMBER(member);
   const Member& m = members_[static_cast<size_t>(member)];
@@ -347,6 +355,16 @@ int Batch::ensure_cluster_scratch() {
   BB_CHECK(c.cells.allocate(k));
   BB_CHECK(c.cells_host.allocate(k));
   cl_ = std::move(c);
+  return BB200_OK;
+}
+
+int Batch::ensure_kld_scratch() {
+  if (const int st = ensure_cluster_scratch()) return st;
+  if (kld_.host.get() != nullptr) return BB200_OK;
+  KldTable t;
+  BB_CHECK(t.device.allocate(members_.size()));
+  BB_CHECK(t.host.allocate(members_.size()));
+  kld_ = std::move(t);
   return BB200_OK;
 }
 
@@ -735,10 +753,15 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     max_points = std::max(max_points, static_cast<uint32_t>(bound));
   }
   const bool convert = std::any_of(active.begin(), active.end(), [&](uint32_t k) { return in[k].kind != BB200_MEASUREMENT_POINTS; });
+  // Amcl::update_device's KLD path: a resampling member with min_particles < max_particles sizes its new set with
+  // take_while_kld (Filter::resample_kld).
+  auto resamples_kld = [&](uint32_t k) { return plans[k].resample != 0 && plans[k].opts.min_particles < plans[k].opts.max_particles; };
+  const bool kld = std::any_of(active.begin(), active.end(), resamples_kld);
   int st = check(cudaSetDevice(device_), "cudaSetDevice");
   if (st == BB200_OK) st = ensure_points(points_total);  // the previous step has ended: the staging buffers are free
   if (st == BB200_OK && step_map < 0) st = ensure_map_table();
   if (st == BB200_OK && convert) st = ensure_inputs(input_floats);
+  if (st == BB200_OK && kld) st = ensure_kld_scratch();
   for (auto k = active.begin(); st == BB200_OK && k != active.end(); ++k)
     if (in[*k].kind == BB200_MEASUREMENT_SCAN) st = ensure_scan_table(members_[*k], *in[*k].scan);
   if (st != BB200_OK) return rollback(st);
@@ -770,6 +793,17 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     b.pivot_x = m.pivot[0];
     b.pivot_y = m.pivot[1];
     b.sampling = to_kernel_sampling(plan.sampling);
+    b.kld = resamples_kld(k) ? 1 : 0;
+    if (b.kld) {
+      BatchKldMember& q = kld_.host.get()[j];
+      q = BatchKldMember{};
+      q.min_particles = plan.opts.min_particles;
+      q.two_epsilon = 2 * plan.opts.kld_epsilon;
+      q.z = plan.opts.kld_z;
+      for (int d = 0; d < 3; ++d) q.hash_resolution[d] = plan.opts.spatial_resolution[d];
+      q.table_offset = m.table_offset;
+      q.table_mask = m.table_slots - 1;
+    }
     if (meas.kind == BB200_MEASUREMENT_POINTS) {
       b.point_offset = point_offset;
       b.n_points = static_cast<uint32_t>(meas.n_points);
@@ -841,7 +875,20 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     }
     row[n_active] = pa.ctas;
   }
-  const int rows = convert ? kBatchLaunches + 1 : kBatchLaunches;
+  if (kld) {
+    uint32_t* rows_kld[2] = {first_host_.get() + static_cast<size_t>(kBatchKldRow) * (n_active + 1),
+                             first_host_.get() + static_cast<size_t>(kBatchKldMomentsRow) * (n_active + 1)};
+    for (uint32_t j = 0; j < n_active; ++j) {
+      uint32_t ctas[2];
+      batch_kld_ctas(table_host_.get()[j], ctas);
+      for (int l = 0; l < 2; ++l) {
+        rows_kld[l][j] = a.kld_ctas[l];
+        a.kld_ctas[l] += ctas[l];
+      }
+    }
+    for (int l = 0; l < 2; ++l) rows_kld[l][n_active] = a.kld_ctas[l];
+  }
+  const int rows = kld ? kBatchRows : convert ? kBatchLaunches + 1 : kBatchLaunches;
 
   cudaStream_t stream = stream_;
   for (const uint32_t k : active) members_[k].cdf_total = 0;  // from here on the step may have rewritten their CDFs
@@ -857,6 +904,8 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
                "upload measurement table");
   if (st == BB200_OK && input_floats > 0)
     st = check(cudaMemcpyAsync(input_.get(), input_host_.get(), input_floats * sizeof(float), cudaMemcpyHostToDevice, stream), "upload measurements");
+  if (st == BB200_OK && kld)
+    st = check(cudaMemcpyAsync(kld_.device.get(), kld_.host.get(), n_active * sizeof(BatchKldMember), cudaMemcpyHostToDevice, stream), "upload KLD table");
   if (st != BB200_OK) return rollback(st);
   if (convert) {
     pa.members = table_.get();
@@ -893,6 +942,12 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     a.maps = map_table_.get();
   }
   a.hits = hits_.get();
+  if (kld) {
+    a.kld = kld_.device.get();
+    a.hashes = cl_.hashes.get();
+    a.keys = cl_.keys.get();
+    a.vals = cl_.first.get();
+  }
   a.summary = summary_host_.get();
   a.members_done = members_done_.get();
   a.ticket = ticket_host_.get();
@@ -917,7 +972,7 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     pivot_to_estimate(r.estimate, m.pivot);
     if (plan.resample) {
       m.cur ^= 1;
-      m.n = m.capacity;
+      m.n = table_host_.get()[j].kld ? s.accepted : m.capacity;
       m.ancestors_n = m.n;
     } else {
       m.cdf_total = s.total;  // the step's scan, over the weights before normalisation

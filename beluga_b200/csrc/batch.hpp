@@ -15,18 +15,21 @@
 
 namespace bb200 {
 
-/// Largest particle count of a batch member: one member's kernels then run in at most 128 CTAs of each launch.
+/// Largest particle count of a batch member: one member's kernels then run in at most 128 CTAs of each launch, and a
+/// KLD-adaptive member's resample_kld takes one chunk (its first chunk of min(max, max(2 min, 65536)) slots is all of them).
 constexpr uint64_t kBatchMaxParticles = 32768;
 
 class Batch {
  public:
-  Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members);
+  /// adaptive: members may have min_particles < max_particles (KLD-adaptive particle counts, as a standalone filter);
+  /// otherwise every member keeps a fixed count.  The flag changes validation only.
+  Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bool adaptive = false);
   ~Batch();
   Batch(const Batch&) = delete;
   Batch& operator=(const Batch&) = delete;
 
   /// The configurations a batch rejects, checked without touching a device (BB200_OK or BB200_ERR_INVALID_ARGUMENT).
-  static int validate(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, std::string* error);
+  static int validate(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bool adaptive, std::string* error);
 
   bool ok() const { return created_; }
   int create_status() const { return create_status_; }
@@ -52,6 +55,8 @@ class Batch {
   int initialize_states(int member, const double* states, const double* weights, uint64_t n);
   int force_update(int member);
   int get_particles(int member, double* states, double* weights, uint64_t capacity);
+  /// Member m's current particle count.
+  int member_size(int member, uint64_t* n) const;
   int ancestors(int member, int64_t* out, uint64_t capacity);
   /// The cluster estimate of one member: cluster_estimates with that member alone selected.
   int cluster_estimate(int member, const bb200_cluster_param& p, bb200_estimate* out);
@@ -126,6 +131,8 @@ class Batch {
   int add_map(const MapTables& tables, int* id);
   int ensure_map_table();
   int ensure_cluster_scratch();
+  /// The cluster scratch, whose hashes and tables a KLD count reuses, and the step's KLD parameter table.
+  int ensure_kld_scratch();
   int ensure_cluster_records(uint64_t cells);
   /// The members whose present[m] is non-zero (present == nullptr: all of them), in member order; BB200_ERR_STATE when one
   /// of them has no particles.
@@ -157,7 +164,7 @@ class Batch {
   DeviceBuffer<double> partials_;
   DeviceBuffer<BatchMember> table_;
   PinnedBuffer<BatchMember> table_host_;
-  DeviceBuffer<uint32_t> first_;  // (kBatchLaunches + 1) x (K + 1): the step's rows, then batch_points_kernel's
+  DeviceBuffer<uint32_t> first_;  // kBatchRows x (K + 1): the step's rows, then batch_points_kernel's and the two KLD rows
   PinnedBuffer<uint32_t> first_host_;
   DeviceBuffer<double> points_;   // (x, y) pairs
   PinnedBuffer<double> points_host_;
@@ -196,6 +203,13 @@ class Batch {
   };
   ClusterBuffers cl_;
   PinnedBuffer<CellRecord> cl_records_host_;  // written by the compaction kernel
+  // KLD parameters of a step's members (allocated on first use, one entry per member of the step's table).  The count
+  // itself runs in the cluster scratch: per-slot hashes in cl_.hashes, bucket sets in cl_.keys and cl_.first.
+  struct KldTable {
+    DeviceBuffer<BatchKldMember> device;
+    PinnedBuffer<BatchKldMember> host;
+  };
+  KldTable kld_;
 
   // Pose-sample scratch (allocated on first use): the member table, and the draws after a header of one CDF total per
   // member (sample_header_ poses' worth), so that one copy brings both back.

@@ -1,6 +1,8 @@
 // ---- batches of filters ----------------------------------------------------------------------------------
 // Each kernel below runs, per CTA, the block body of the single-filter kernel it stands for, on the CTA's member.
+#include "bucket_set.cuh"
 #include "cdf.cuh"
+#include "kld.cuh"
 #include "resample.cuh"
 #include "reweight_beam.cuh"
 #include "reweight_lfm.cuh"
@@ -173,12 +175,14 @@ struct BatchTail {
   uint32_t n_members;
   int* ticket;
   int seq;
+  unsigned long long accepted;  // StepSummary::accepted
 };
 __device__ __forceinline__ bool tail_enabled(const BatchTail&) { return true; }
 __device__ __forceinline__ void tail_publish(const BatchTail& tail, const double* v, Scalars* scalars) {
 #pragma unroll
   for (int k = 0; k < kMomentCount; ++k) tail.summary->moments[k] = v[k];
   scalars->blocks_done = 0;
+  tail.summary->accepted = tail.accepted;
   tail.summary->total = scalars->total;
   tail.summary->exponent = scalars->exponent;
   tail.summary->valid = scalars->valid;
@@ -215,7 +219,9 @@ __device__ __forceinline__ void normalize_moments_block(const Pose2* __restrict_
 }
 
 /// Per member: resample_scatter_kernel or resample_kernel (recovery injection, multinomial draws) on a resampling step,
-/// normalisation otherwise; then the member's moments, summed by its last CTA.
+/// normalisation otherwise; then the member's moments, summed by its last CTA.  A member that resamples under KLD draws
+/// every one of its max_particles slots with their spatial hashes, as Filter::resample_kld's one chunk does, and leaves
+/// its summary to batch_kld_moments_kernel.
 template <bool kTable>
 __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs s) {
   uint32_t local, count;
@@ -223,7 +229,7 @@ __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs 
   const BatchMember& m = s.members[k];
   Scalars* scalars = s.scalars + k;
   double* partials = s.partials + static_cast<size_t>(blockIdx.x - local) * kMomentCount;
-  const BatchTail tail{s.summary + k, s.members_done, s.n_members, s.ticket, s.seq};
+  const BatchTail tail{s.summary + k, s.members_done, s.n_members, s.ticket, s.seq, 0};
   if (!m.resample) {
     normalize_moments_block(batch_states(s, m, 0), s.weights + m.offset, m.n, m.pivot_x, m.pivot_y, scalars, partials, local, count, tail);
     return;
@@ -244,11 +250,108 @@ __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs 
   batch_recovery_map<kTable>(s, m, a);
   a.pivot_x = m.pivot_x;
   a.pivot_y = m.pivot_y;
-  if (m.scheme == 1 && m.random_state_probability <= 0.0) {  // systematic, nothing drawn per slot: launch_resample's scatter form
+  if (m.kld) {  // launch_resample with hashes: always the per-slot form; a.tail is the disabled one (no summary, no arrival)
+    const BatchKldMember& q = s.kld[k];
+    a.hashes = s.hashes + m.offset;
+    for (int d = 0; d < 3; ++d) a.hash_resolution[d] = q.hash_resolution[d];
+    resample_block(a, scalars, partials, local, count, a.tail);
+  } else if (m.scheme == 1 && m.random_state_probability <= 0.0) {  // systematic, nothing drawn per slot: launch_resample's scatter form
     resample_scatter_block(a, scalars, partials, local, count, tail);
   } else {
     resample_block(a, scalars, partials, local, count, tail);
   }
+}
+
+// ---- KLD-adaptive members (Filter::resample_kld's one chunk, then Filter::estimate) ---------------------------------
+// A member holds at most kBatchMaxParticles = 32768 particles, so resample_kld's first chunk, min(max, max(2 min, 65536))
+// slots, is all of them: one draw (batch_finish_kernel), one count with no buckets before it, accepted =
+// min(cutoff - 1, max).  The count is kld_check_kernel's: a bucket set that keeps each bucket's smallest slot makes "slot
+// j is the first of its bucket" an order-independent fact, so k after every slot is a prefix sum of those flags in slot
+// order, and the cutoff is the smallest count whose condition fails.
+
+constexpr int kBatchKldThreads = 1024;
+constexpr int kBatchKldWarps = kBatchKldThreads / kWarp;
+
+/// One CTA per KLD member: clear its bucket set, insert every slot's hash, then flag first occurrences and scan them
+/// chunk by chunk in slot order; scalars->kld_cutoff receives the first failing count (~0 when every count passes).
+__global__ void __launch_bounds__(kBatchKldThreads) batch_kld_kernel(BatchStepArgs s) {
+  __shared__ uint32_t s_warp[kBatchKldWarps];
+  __shared__ unsigned long long s_min[kBatchKldWarps];
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kBatchKldRow, blockIdx.x, local, count);
+  const BatchMember& m = s.members[k];
+  const BatchKldMember& q = s.kld[k];
+  const unsigned long long* hashes = s.hashes + m.offset;
+  unsigned long long* keys = s.keys + q.table_offset;
+  unsigned int* vals = s.vals + q.table_offset;
+  const uint64_t mask = q.table_mask;
+  const uint32_t slots = static_cast<uint32_t>(m.slots);
+  const int tid = threadIdx.x, lane = tid % kWarp, warp = tid / kWarp;
+
+  for (uint64_t t = tid; t <= mask; t += kBatchKldThreads) {  // launch_kld_clear
+    keys[t] = bucket_set::kEmpty;
+    vals[t] = ~0u;
+  }
+  __syncthreads();
+  for (uint32_t j = tid; j < slots; j += kBatchKldThreads) bucket_set::insert_min(keys, vals, mask, hashes[j], j);  // kld_insert_kernel
+  __syncthreads();
+  unsigned long long failing = ~0ull, k_before = 0;
+  for (uint32_t base = 0; base < slots; base += kBatchKldThreads) {
+    const uint32_t j = base + tid;
+    bool head = false;
+    if (j < slots) head = vals[bucket_set::find(keys, mask, hashes[j])] == j;  // kld_flag_kernel
+    const unsigned heads = __ballot_sync(0xffffffffu, head);
+    if (lane == 0) s_warp[warp] = __popc(heads);
+    __syncthreads();
+    unsigned long long before = k_before;
+    for (int w = 0; w < kBatchKldWarps; ++w) {
+      const uint32_t c = s_warp[w];
+      if (w < warp) before += c;
+      k_before += c;
+    }
+    // kld_check_kernel: k = buckets up to and including slot j
+    if (j < slots && !kld_count_allowed(j + 1ull, before + __popc(heads & ((1u << lane) - 1u)) + (head ? 1u : 0u), q.min_particles,
+                                        q.two_epsilon, q.z))
+      failing = j + 1ull;
+    // Counts only grow: once a chunk holds a failing count, no later chunk holds a smaller one.  (Also the barrier
+    // before the next chunk writes s_warp.)
+    if (__syncthreads_or(failing != ~0ull)) break;
+  }
+#pragma unroll
+  for (int off = kWarp / 2; off > 0; off >>= 1) {
+    const unsigned long long o = __shfl_down_sync(0xffffffffu, failing, off);
+    failing = o < failing ? o : failing;
+  }
+  if (lane == 0) s_min[warp] = failing;
+  __syncthreads();
+  if (tid == 0) {
+    for (int w = 1; w < kBatchKldWarps; ++w) failing = s_min[w] < failing ? s_min[w] : failing;
+    s.scalars[k].kld_cutoff = failing;
+  }
+}
+
+/// moments_kernel over the particles a KLD member keeps (unit weights, the partition of moments_block_count(accepted)
+/// blocks), summed like reduce_partials_kernel by the last of those CTAs, which publishes the member's summary.  Each KLD
+/// member has moments_block_count(max_particles) CTAs; those beyond moments_block_count(accepted) only leave.
+__global__ void __launch_bounds__(kStreamThreads) batch_kld_moments_kernel(BatchStepArgs s) {
+  __shared__ double s_red[kMomentCount * kStreamThreads / kWarp];
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kBatchKldMomentsRow, blockIdx.x, local, count);
+  const BatchMember& m = s.members[k];
+  Scalars* scalars = s.scalars + k;
+  const unsigned long long cutoff = scalars->kld_cutoff;
+  // take_while drops the first element whose condition fails (take_while_kld.hpp:134-136)
+  const uint64_t accepted = cutoff != ~0ull ? (cutoff - 1 < m.slots ? cutoff - 1 : m.slots) : m.slots;
+  const uint32_t grid = moments_blocks(accepted);
+  if (local >= grid) return;
+  const Pose2* states = batch_states(s, m, 1);  // the new set (the host flips cur once the step has ended)
+  double v[kMomentCount];
+#pragma unroll
+  for (int c = 0; c < kMomentCount; ++c) v[c] = 0.0;
+  for (uint64_t i = static_cast<uint64_t>(local) * kStreamThreads + threadIdx.x; i < accepted; i += static_cast<uint64_t>(grid) * kStreamThreads)
+    accumulate_moments(v, load_pose(states + i), 1.0, m.pivot_x, m.pivot_y);  // the draw wrote w = 1 to every slot
+  const BatchTail tail{s.summary + k, s.members_done, s.n_members, s.ticket, s.seq, accepted};
+  finish_block_moments<kStreamThreads>(v, s_red, s.partials + static_cast<size_t>(blockIdx.x - local) * kMomentCount, scalars, local, grid, tail);
 }
 
 // ---- pose samples of a batch (Filter::sample_states per member) --------------------------------------------------
@@ -424,6 +527,11 @@ int launch_batch_step_from(const BatchStepArgs& s, cudaStream_t stream) {
   }
   batch_scan_kernel<<<s.ctas[kBatchScan], kQsThreads, 0, stream>>>(s);
   batch_finish_kernel<kTable><<<s.ctas[kBatchFinish], kRsThreads, 0, stream>>>(s);
+  if (s.kld != nullptr) {
+    batch_kld_kernel<<<s.kld_ctas[0], kBatchKldThreads, 0, stream>>>(s);
+    batch_kld_moments_kernel<<<s.kld_ctas[1], kStreamThreads, 0, stream>>>(s);
+    launches += 2;
+  }
   return launches;
 }
 
@@ -439,11 +547,16 @@ void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunch
   // the partition launch_resample / launch_moments would use for a single filter of this size
   if (!m.resample) {
     out[kBatchFinish] = moments_block_count(m.n);
-  } else if (m.scheme == 1 && m.random_state_probability <= 0.0) {
+  } else if (m.scheme == 1 && m.random_state_probability <= 0.0 && !m.kld) {
     out[kBatchFinish] = resample_scatter_block_count(m.n);
   } else {
     out[kBatchFinish] = resample_block_count(m.slots);
   }
+}
+
+void batch_kld_ctas(const BatchMember& m, uint32_t out[2]) {
+  out[0] = m.kld ? 1u : 0u;
+  out[1] = m.kld ? moments_blocks(m.slots) : 0u;
 }
 
 int launch_batch_step(const BatchStepArgs& s, cudaStream_t stream) {

@@ -33,7 +33,7 @@ struct bb200_amcl {
 
 struct bb200_amcl_batch {
   Batch impl;
-  bb200_amcl_batch(const bb200_amcl_param* p, const bb200_motion_param* m, int n) : impl(p, m, n) {}
+  bb200_amcl_batch(const bb200_amcl_param* p, const bb200_motion_param* m, int n, bool adaptive) : impl(p, m, n, adaptive) {}
 };
 
 /// One filter over several shards driven by ONE host thread (the shape of beluga_ros's single-process node).
@@ -118,6 +118,27 @@ int set_sharded_map(bb200_sharded_amcl* g, Prepare&& prepare) {
     if (st != BB200_OK) return g->ranks[0]->impl.filter().fail_with(st, message);
     for (auto a = g->ranks.begin(); st == BB200_OK && a != g->ranks.end(); ++a) st = (*a)->impl.filter().set_map(tables);
     return st;
+  });
+}
+
+int create_batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bool adaptive, bb200_amcl_batch** out) {
+  if (out == nullptr) {
+    g_create_error = "null argument";
+    return BB200_ERR_INVALID_ARGUMENT;
+  }
+  *out = nullptr;
+  {
+    const int st = Batch::validate(params, motions, n_members, adaptive, &g_create_error);  // before any device is touched
+    if (st != BB200_OK) return st;
+  }
+  return guarded_create([&] {
+    auto b = std::make_unique<bb200_amcl_batch>(params, motions, n_members, adaptive);
+    if (!b->impl.ok()) {
+      g_create_error = b->impl.last_error();
+      return b->impl.create_status();
+    }
+    *out = b.release();
+    return static_cast<int>(BB200_OK);
   });
 }
 }  // namespace
@@ -782,24 +803,14 @@ int bb200_sharded_amcl_get_particles(bb200_sharded_amcl* g, double* states, doub
 // ---- batches ------------------------------------------------------------------------------------------
 
 int bb200_amcl_batch_create(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bb200_amcl_batch** out) {
-  if (out == nullptr) {
-    g_create_error = "null argument";
-    return BB200_ERR_INVALID_ARGUMENT;
-  }
-  *out = nullptr;
-  {
-    const int st = Batch::validate(params, motions, n_members, &g_create_error);  // before any device is touched
-    if (st != BB200_OK) return st;
-  }
-  return guarded_create([&] {
-    auto b = std::make_unique<bb200_amcl_batch>(params, motions, n_members);
-    if (!b->impl.ok()) {
-      g_create_error = b->impl.last_error();
-      return b->impl.create_status();
-    }
-    *out = b.release();
-    return static_cast<int>(BB200_OK);
-  });
+  return create_batch(params, motions, n_members, false, out);
+}
+int bb200_amcl_batch_create_adaptive(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bb200_amcl_batch** out) {
+  return create_batch(params, motions, n_members, true, out);
+}
+int bb200_amcl_batch_member_size(const bb200_amcl_batch* b, int member, uint64_t* n) {
+  BB_REQUIRE(b && n);
+  return guarded(b->impl, [&] { return b->impl.member_size(member, n); });
 }
 void bb200_amcl_batch_destroy(bb200_amcl_batch* b) { delete b; }
 const char* bb200_amcl_batch_last_error(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.last_error() : "null batch"; }

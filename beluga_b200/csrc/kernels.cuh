@@ -148,6 +148,7 @@ struct StepSummary {
   int valid;                      // 0: no positive finite weight anywhere
   int error;                      // 1: a peer never posted (bounded spin ran out)
   int seq;                        // completion ticket of the step that wrote this block (written last; the host may poll it)
+  unsigned long long accepted;    // batch members resampled under KLD: the particles take_while_kld kept (0 otherwise)
 };
 struct ShardExchangeArgs {
   int kind, post, wait;
@@ -424,6 +425,7 @@ struct BatchMember {
   MotionSampling sampling;
   uint64_t point_offset;    // first point of the member's scan in the batch's point buffer
   uint32_t n_points;
+  int kld;                  // 1: resamples under KLD in this step (BatchStepArgs::kld[member] holds the parameters)
   double points_radius;     // largest |x| + |y| of the scan (NaN: some point is not finite)
   uint64_t hit_offset;      // beam model, two-pass form: first hit word of the member in the batch's hit buffer ...
   uint64_t hit_stride;      // ... beam-major, round_up(n, 32) words per beam (the single filter's layout)
@@ -459,6 +461,17 @@ struct BatchMap {
   Pose2 grid_origin;
 };
 
+/// The KLD parameters of a member that resamples under KLD in a batch step (BatchMember::kld), one entry per member of the
+/// step's table: what Filter::resample_kld takes from the member's resample options, and its bucket set.
+struct BatchKldMember {
+  uint64_t min_particles;
+  double two_epsilon;         // 2 * kld_epsilon, as launch_kld_chunk passes it
+  double z;                   // kld_z
+  double hash_resolution[3];  // spatial_resolution
+  uint64_t table_offset;      // its bucket set in BatchStepArgs::keys / vals (the cluster scratch's hash table)
+  uint64_t table_mask;        // the set's slots - 1 (a power of two >= 2 * max_particles, as Filter's KLD tables)
+};
+
 struct BatchStepArgs {
   const BatchMember* members;     // device
   const uint32_t* first;          // device: kBatchLaunches x (n_members + 1) CTA prefixes
@@ -491,12 +504,21 @@ struct BatchStepArgs {
   // Null when every member of the step reads one map, whose views are the fields above (field, free_cells ... beam);
   // otherwise the device table of the batch's maps, and each member reads maps[BatchMember::map].
   const BatchMap* maps;
+  // KLD-adaptive members (after every field the other kernels read, so that they keep their parameter offsets).  Null
+  // when no member of the step resamples under KLD.
+  const BatchKldMember* kld;      // device, one per member of the table
+  unsigned long long* hashes;     // the per-slot spatial hashes of the draw, at each member's offset
+  unsigned long long* keys;       // the members' bucket sets (BatchKldMember::table_offset)
+  unsigned int* vals;
+  uint32_t kld_ctas[2];           // total CTAs of batch_kld_kernel and batch_kld_moments_kernel
 };
 static_assert(sizeof(BatchStepArgs) <= 1024, "the step's arguments travel as one kernel parameter block (4 KB at most)");
 /// Reset | propagate | reweight | quantise + scan | resample or normalise + moments.  The reweight takes one launch for the
 /// likelihood field, two for the beam model's two-pass form (walk, mixture) and one for its fused form, each issued
-/// when some member takes that form.  Returns the number of launches: 4 plus those, so 5 to 8, whatever the members,
-/// their maps, their particle counts and their scans are.
+/// when some member takes that form.  When some member resamples under KLD (args.kld set), two launches follow: the
+/// KLD count of each such member and the moments of the particles it keeps.  Returns the number of launches: 4 plus
+/// those, so 5 to 8 without KLD members and 7 to 10 with them, whatever the members, their maps, their particle counts,
+/// their accepted counts and their scans are.
 int launch_batch_step(const BatchStepArgs& args, cudaStream_t stream);
 /// Scan tiles of a member of n particles (the quantise-scan CTAs it needs).
 uint32_t batch_scan_tiles(uint64_t n);
@@ -506,6 +528,11 @@ uint32_t batch_scan_tiles(uint64_t n);
 // at its point_offset, and its n_points and points_radius into the step's member table, which the step's kernels then read
 // in stream order.  Its CTA ranges are one more row of the step's `first` buffer, after the kBatchLaunches rows.
 constexpr int kBatchPointsRow = kBatchLaunches;
+/// The rows of batch_kld_kernel (one CTA per KLD member) and batch_kld_moments_kernel (moments_block_count(max_particles)
+/// CTAs per KLD member), after batch_points_kernel's; a step's `first` buffer holds kBatchRows rows.
+constexpr int kBatchKldRow = kBatchLaunches + 1;
+constexpr int kBatchKldMomentsRow = kBatchLaunches + 2;
+constexpr int kBatchRows = kBatchLaunches + 3;
 /// How a member's measurement reaches a batch step (the values of bb200_measurement_kind).
 enum BatchInputKind : int { kBatchInputPoints = 0, kBatchInputScan = 1, kBatchInputCloud = 2 };
 /// One member of batch_points_kernel, built on the host every step (one per entry of the step's member table).
@@ -534,6 +561,8 @@ uint32_t batch_points_ctas(const BatchPointsMember& m);
 int launch_batch_points(const BatchPointsArgs& args, cudaStream_t stream);
 /// CTAs of a member in each row of a batch step's ranges, for a member that takes reweight form `form`.
 void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunches]);
+/// CTAs of a member in the rows kBatchKldRow and kBatchKldMomentsRow (none unless it resamples under KLD).
+void batch_kld_ctas(const BatchMember& m, uint32_t out[2]);
 
 /// One member of a batch's pose-sample draw (Filter::sample_states per member).
 struct BatchSampleMember {

@@ -7,6 +7,7 @@
 // k after every slot and the first failing count is a min-reduction.
 #include "bucket_set.cuh"
 #include "cdf.cuh"
+#include "kld.cuh"
 
 namespace bb200 {
 
@@ -25,16 +26,6 @@ __global__ void __launch_bounds__(256) kld_flag_kernel(const unsigned long long*
   const uint64_t j = static_cast<uint64_t>(blockIdx.x) * 256 + threadIdx.x;
   if (j >= n) return;
   flags[j] = vals[bucket_set::find(keys, mask, hashes[j])] == static_cast<unsigned int>(slot_base + j) ? 1u : 0u;
-}
-
-/// kld_condition target size (views/take_while_kld.hpp:73-80), same operation order as the reference.
-__device__ __forceinline__ bool kld_count_allowed(unsigned long long count, unsigned long long k, unsigned long long min_count, double two_epsilon, double z) {
-  if (count <= min_count || k <= 2ull) return true;
-  const double common = 2. / static_cast<double>(9 * (k - 1));
-  const double base = 1. - common + sqrt(common) * z;
-  const double result = (static_cast<double>(k - 1) / two_epsilon) * base * base * base;
-  const double target = ceil(result);
-  return target >= 18446744073709551615.0 || count <= static_cast<unsigned long long>(target);
 }
 
 __global__ void __launch_bounds__(256) kld_check_kernel(const uint32_t* __restrict__ flags, const uint32_t* __restrict__ exclusive, uint64_t n,

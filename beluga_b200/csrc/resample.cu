@@ -105,9 +105,7 @@ uint32_t launch_resample(const ResampleArgs& args, Scalars* scalars, double* mom
   return blocks;
 }
 
-uint32_t moments_block_count(uint64_t n) {
-  return static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>((n + kStreamThreads - 1) / kStreamThreads, kStreamMaxBlocks)));
-}
+uint32_t moments_block_count(uint64_t n) { return moments_blocks(n); }
 
 void launch_moments(const Pose2* states, const double* weights, uint64_t n, double pivot_x, double pivot_y, double* moment_partials,
                     cudaStream_t stream) {

@@ -10,6 +10,12 @@ namespace {
 
 constexpr int kStreamThreads = 256;
 
+/// Blocks of moments_kernel over n particles (moments_block_count), on the host and on the device.
+BB_HD uint32_t moments_blocks(uint64_t n) {
+  const uint64_t blocks = (n + kStreamThreads - 1) / kStreamThreads;
+  return static_cast<uint32_t>(blocks < 1 ? 1 : blocks > kStreamMaxBlocks ? kStreamMaxBlocks : blocks);
+}
+
 // ---- resample -------------------------------------------------------------------------------------
 
 constexpr int kRsThreads = 256;

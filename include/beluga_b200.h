@@ -531,9 +531,13 @@ int bb200_amcl_leave_shards(bb200_amcl* a);
  * what a standalone bb200_amcl with the same parameters returns for the same inputs.
  *
  * Every member has its own parameter block (seed, policies, resampling scheme, recovery override) and
- * motion model.  Members keep a fixed particle count: bb200_amcl_batch_create rejects, before touching a
- * device, with BB200_ERR_INVALID_ARGUMENT: n_members < 1, min_particles != max_particles (KLD), selective
+ * motion model.  Members of a batch made by bb200_amcl_batch_create keep a fixed particle count: it rejects, before
+ * touching a device, with BB200_ERR_INVALID_ARGUMENT: n_members < 1, min_particles != max_particles (KLD), selective
  * resampling, non-zero shard fields, max_particles of 0 or above 32768, and members on different devices.
+ * bb200_amcl_batch_create_adaptive accepts min_particles <= max_particles as bb200_amcl_create does: a member with
+ * min_particles < max_particles resizes its particle set on every resampling step with KLD (take_while_kld), exactly
+ * as a standalone bb200_amcl; bb200_amcl_batch_member_size returns its current count.  Such a step takes 2 launches
+ * more (the members' KLD counts and the moments of the particles they keep), whatever K and the counts are.
  *
  * A batch holds a set of maps, each a grid with its sensor model: likelihood-field model or the beam model.
  * Each member reads one of them or none.  bb200_amcl_batch_set_likelihood_field_map and _set_beam_map give every
@@ -555,6 +559,13 @@ int bb200_amcl_leave_shards(bb200_amcl* a);
 typedef struct bb200_amcl_batch bb200_amcl_batch;
 /* params[m] and motions[m] configure member m (params[m].device must be the same for all). */
 int bb200_amcl_batch_create(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bb200_amcl_batch** out);
+/* bb200_amcl_batch_create whose members may have min_particles < max_particles (KLD-adaptive particle counts); it
+ * rejects min_particles > max_particles and keeps the other refusals.  A member with min_particles == max_particles
+ * keeps a fixed count, and a batch whose members all do computes what a bb200_amcl_batch_create batch computes. */
+int bb200_amcl_batch_create_adaptive(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bb200_amcl_batch** out);
+/* Member m's current particle count in *n (any batch): max_particles after a fixed-size resample, the count KLD kept
+ * after an adaptive one, n after bb200_amcl_batch_initialize_states. */
+int bb200_amcl_batch_member_size(const bb200_amcl_batch* b, int member, uint64_t* n);
 void bb200_amcl_batch_destroy(bb200_amcl_batch* b);
 const char* bb200_amcl_batch_last_error(const bb200_amcl_batch* b);
 int bb200_amcl_batch_members(const bb200_amcl_batch* b);

@@ -209,17 +209,20 @@ template <class MotionModel, class SensorModel, class ExecutionPolicy>
 
 /// K independent filters on one GPU (bb200_amcl_batch) that read one or several maps, each for a likelihood-field model or
 /// the beam model: update() steps every member with a new scan at once.  Member m behaves like an Amcl built from motions[m] and params[m]; members keep a fixed
-/// particle count (min_particles == max_particles <= 32768).  Results are returned per member, std::nullopt where the
-/// reference's update would return it or where the member had no scan this step.
+/// particle count (min_particles == max_particles <= 32768) unless the batch is adaptive, whose members may have
+/// min_particles < max_particles and resize their particle sets with KLD as a standalone Amcl does.  Results are returned
+/// per member, std::nullopt where the reference's update would return it or where the member had no scan this step.
 class AmclBatch {
  public:
   using estimation_type = std::pair<SE2d, Matrix3d>;
 
-  AmclBatch(const std::vector<bb200_motion_param>& motions, const std::vector<AmclParams>& params) {
+  /// adaptive: bb200_amcl_batch_create_adaptive (members may have min_particles < max_particles); particles(m) then
+  /// returns member_size(m) particles.
+  AmclBatch(const std::vector<bb200_motion_param>& motions, const std::vector<AmclParams>& params, bool adaptive = false) : adaptive_{adaptive} {
     if (motions.size() != params.size()) throw Error(BB200_ERR_INVALID_ARGUMENT, "one motion model per member");
     std::vector<bb200_amcl_param> p;
     for (const AmclParams& q : params) p.push_back(c_amcl_param(q));
-    const int st = bb200_amcl_batch_create(p.data(), motions.data(), static_cast<int>(p.size()), &handle_);
+    const int st = (adaptive ? bb200_amcl_batch_create_adaptive : bb200_amcl_batch_create)(p.data(), motions.data(), static_cast<int>(p.size()), &handle_);
     if (st != BB200_OK) throw Error(st, bb200_create_error());
     sizes_.reserve(params.size());
     for (const AmclParams& q : params) sizes_.push_back(q.max_particles);
@@ -367,11 +370,20 @@ class AmclBatch {
   }
 #endif
 
-  /// Member m's particle set, copied from the device.
+  /// Member m's current particle count.
+  [[nodiscard]] std::size_t member_size(std::size_t member) const {
+    std::uint64_t n = 0;
+    check(bb200_amcl_batch_member_size(handle_, index(member), &n));
+    return static_cast<std::size_t>(n);
+  }
+
+  /// Member m's particle set, copied from the device: max_particles entries in a fixed batch, member_size(m)
+  /// in an adaptive one.
   [[nodiscard]] ParticleSet particles(std::size_t member) const {
+    const std::size_t n = adaptive_ ? member_size(member) : sizes_.at(member);
     ParticleSet out;
-    out.states.resize(sizes_.at(member));
-    out.weights.resize(sizes_.at(member));
+    out.states.resize(n);
+    out.weights.resize(n);
     check(bb200_amcl_batch_get_particles(handle_, index(member), reinterpret_cast<double*>(out.states.data()), out.weights.data(), out.size()));
     return out;
   }
@@ -488,8 +500,9 @@ class AmclBatch {
     return mask;
   }
 
+  bool adaptive_{false};
   bb200_amcl_batch* handle_{nullptr};
-  std::vector<std::size_t> sizes_;
+  std::vector<std::size_t> sizes_;  // max_particles: upper bounds of every member's particle, histogram and sample counts
   std::map<int, std::size_t> field_cells_;  // cells of each likelihood-field map, by id
 };
 

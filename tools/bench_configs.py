@@ -7,7 +7,8 @@ beam model (60 and 720 points per member) against the same members stepped as st
 members read 1, 4 or 16 likelihood-field maps against one single-map batch per map, and a step mixing likelihood-field and beam members.
 `batch_cloud`: the `batch` members' particle-cloud publish round (histograms and pose samples) in one batched call each against
 K standalone filters publishing in turn.  `batch_measurements`: AmclBatch fed laser scans and point clouds converted on the
-device against host conversion plus the points update.
+device against host conversion plus the points update.  `batch_kld`: the `batch` workload with KLD-adaptive members (min 500,
+max 2000) against K standalone KLD Amcl.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import json
@@ -133,6 +134,53 @@ def run_batch():
             "members": k, "particles": n, "points": 100, "steps": steps,
             "ms_per_step_e2e": mb, "member_steps_per_s": k * 1e3 / mb, "launches_per_step": int(max(launches)),
             "standalone_ms_per_round": ms, "standalone_member_steps_per_s": k * 1e3 / ms,
+            "kernels_ms": {}, "device": device}
+    return res
+
+
+def run_batch_kld():
+    """`batch` with KLD-adaptive members: K in {1, 16, 64, 256} members of min 500 / max 2000 particles (beluga_ros's defaults)
+    x 100 points on the 2000^2 synthetic map, every member updating every step; beside it K standalone KLD Amcl stepped one
+    after another in the same process."""
+    res = {}
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=100, steps=100)
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    steps, warmup = 20, 3
+    device = device_record()
+    for k in (1, 16, 64, 256):
+        params = [bb.AmclParams(min_particles=500, max_particles=2000, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m) for m in range(k)]
+        motions = [bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)]
+        batch = bb.AmclBatch(motions, params, adaptive=True)
+        batch.set_likelihood_field_map(lfm, grid)
+        singles = []
+        for m in range(k):
+            batch.initialize(m, sc.initial_mean, sc.initial_cov)
+            a = bb.Amcl(motions[m], params[m])
+            a.update_map(bb.SENSOR_LIKELIHOOD_FIELD, lfm, grid)
+            a.initialize(sc.initial_mean, sc.initial_cov)
+            singles.append(a)
+        wall_batch, wall_single, launches, sizes = [], [], [], []
+        for t in range(warmup + steps):
+            pose = bb.se2(*sc.poses[t])
+            t0 = time.perf_counter()
+            before = batch.launch_count()
+            r = batch.update([pose] * k, [sc.scans[t]] * k)
+            t1 = time.perf_counter()
+            assert all(x.updated for x in r)
+            launches.append(batch.launch_count() - before)
+            for a, x in zip(singles, r):
+                assert a.update(pose, sc.scans[t]).n_particles == x.n_particles
+            t2 = time.perf_counter()
+            if t >= warmup:
+                wall_batch.append((t1 - t0) * 1e3)
+                wall_single.append((t2 - t1) * 1e3)
+                sizes.extend(x.n_particles for x in r)
+        mb, ms = float(np.median(wall_batch)), float(np.median(wall_single))
+        res[f"batch_kld_{k}_x_500_2000_x_100_lfm_2000"] = {
+            "members": k, "min_particles": 500, "max_particles": 2000, "points": 100, "steps": steps,
+            "mean_particles": float(np.mean(sizes)), "ms_per_step_e2e": mb, "member_steps_per_s": k * 1e3 / mb,
+            "launches_per_step": int(max(launches)), "standalone_ms_per_round": ms, "standalone_member_steps_per_s": k * 1e3 / ms,
             "kernels_ms": {}, "device": device}
     return res
 
@@ -593,6 +641,8 @@ def main():
         out.update(run_cloud())
     if "batch" in which:
         out.update(run_batch())
+    if "batch_kld" in which:
+        out.update(run_batch_kld())
     if "batch_cluster" in which:
         out.update(run_batch_cluster())
     if "batch_cloud" in which:

@@ -778,11 +778,13 @@ class AmclBatch:
     number of kernel launches and one synchronisation.  Member m's results and particles equal those of a standalone Amcl
     built from params[m] and motions[m] and fed the same inputs."""
 
-    def __init__(self, motions, params, adaptive: bool = False):
+    def __init__(self, motions, params, adaptive: bool = False, selective: bool = False):
         """`motions[m]`, `params[m]`: member m's motion model and AmclParams (max_particles <= 32768, and
-        min_particles == max_particles unless `adaptive`).  adaptive=True (bb200_amcl_batch_create_adaptive) lets members
+        min_particles == max_particles unless `adaptive`).  adaptive=True (BB200_BATCH_ADAPTIVE) lets members
         have min_particles < max_particles: they resize their particle sets with KLD on every resampling step, and
-        particles() and ancestors() then return member_size(m) rows."""
+        particles() and ancestors() then return member_size(m) rows.  selective=True (BB200_BATCH_SELECTIVE) lets members
+        have selective_resampling: they resample only when their effective sample size drops below half their particles,
+        and each result's `resampled` reports the decision."""
         self._lib = _capi.load()
         k = len(params)
         if len(motions) != k:
@@ -790,13 +792,14 @@ class AmclBatch:
         p = (_capi.AmclParam * max(k, 1))(*[q.c() for q in params])
         m = (_capi.MotionParam * max(k, 1))(*[q.c_motion() for q in motions])
         h = C.c_void_p()
-        create = self._lib.bb200_amcl_batch_create_adaptive if adaptive else self._lib.bb200_amcl_batch_create
-        st = create(p, m, k, C.byref(h))
+        flags = (_capi.BATCH_ADAPTIVE if adaptive else 0) | (_capi.BATCH_SELECTIVE if selective else 0)
+        st = self._lib.bb200_amcl_batch_create_with_flags(p, m, k, flags, C.byref(h))
         if st != _capi.OK:
             raise BelugaB200Error(st, self._lib.bb200_create_error().decode())
         self._h = h
         self.params = list(params)
         self.adaptive = bool(adaptive)
+        self.selective = bool(selective)
         self._field_shapes = {}  # (height, width) of each likelihood-field map, by id
 
     def close(self):

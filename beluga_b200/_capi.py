@@ -13,6 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libbeluga_b200.so")
 
 OK, ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_NO_DEVICE, ERR_STATE, ERR_CAPACITY = 0, -1, -2, -3, -4, -5
+BATCH_ADAPTIVE, BATCH_SELECTIVE = 1, 2  # bb200_batch_flags
 
 SENSOR_LIKELIHOOD_FIELD, SENSOR_LIKELIHOOD_FIELD_PROB, SENSOR_BEAM = 0, 1, 2
 RESAMPLE_MULTINOMIAL, RESAMPLE_SYSTEMATIC = 0, 1
@@ -213,6 +214,7 @@ SIGNATURES = {
     "bb200_amcl_leave_shards": (C.c_int, [_vp]),
     "bb200_amcl_batch_create": (C.c_int, [_P(AmclParam), _P(MotionParam), C.c_int, _P(_vp)]),
     "bb200_amcl_batch_create_adaptive": (C.c_int, [_P(AmclParam), _P(MotionParam), C.c_int, _P(_vp)]),
+    "bb200_amcl_batch_create_with_flags": (C.c_int, [_P(AmclParam), _P(MotionParam), C.c_int, C.c_uint32, _P(_vp)]),
     "bb200_amcl_batch_member_size": (C.c_int, [_vp, C.c_int, _P(C.c_uint64)]),
     "bb200_amcl_batch_destroy": (None, [_vp]),
     "bb200_amcl_batch_last_error": (C.c_char_p, [_vp]),

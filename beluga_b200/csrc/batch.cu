@@ -20,11 +20,13 @@ uint64_t finish_rows(uint64_t capacity) {
 
 }  // namespace
 
-int Batch::validate(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bool adaptive, std::string* error) {
+int Batch::validate(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, uint32_t flags, std::string* error) {
   auto reject = [&](const std::string& m) {
     if (error != nullptr) *error = m;
     return static_cast<int>(BB200_ERR_INVALID_ARGUMENT);
   };
+  if ((flags & ~static_cast<uint32_t>(BB200_BATCH_ADAPTIVE | BB200_BATCH_SELECTIVE)) != 0) return reject("unknown batch flags");
+  const bool adaptive = (flags & BB200_BATCH_ADAPTIVE) != 0, selective = (flags & BB200_BATCH_SELECTIVE) != 0;
   if (params == nullptr || motions == nullptr) return reject("null argument");
   if (n_members < 1) return reject("a batch needs at least one member");
   for (int k = 0; k < n_members; ++k) {
@@ -35,7 +37,7 @@ int Batch::validate(const bb200_amcl_param* params, const bb200_motion_param* mo
     if (!adaptive && p.min_particles != p.max_particles)
       return reject(who + "a batch member keeps a fixed particle count (min_particles == max_particles)");
     if (p.min_particles > p.max_particles) return reject(who + "need 0 < min_particles <= max_particles");  // bb200_amcl_create's check
-    if (p.selective_resampling) return reject(who + "selective resampling is not supported in a batch");
+    if (p.selective_resampling && !selective) return reject(who + "selective resampling is not supported in a batch");
     if (p.shard_first_index != 0 || p.shard_capacity != 0) return reject(who + "a batch member is not sharded");
     if (!(p.alpha_slow >= 0.0) || !(p.alpha_slow <= p.alpha_fast)) return reject(who + "need 0 <= alpha_slow <= alpha_fast");
     if (motions[k].model < BB200_MOTION_DIFFERENTIAL || motions[k].model > BB200_MOTION_STATIONARY) return reject(who + "unknown motion model");
@@ -43,8 +45,8 @@ int Batch::validate(const bb200_amcl_param* params, const bb200_motion_param* mo
   return BB200_OK;
 }
 
-Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bool adaptive) {
-  create_status_ = validate(params, motions, n_members, adaptive, &error_);
+Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, uint32_t flags) {
+  create_status_ = validate(params, motions, n_members, flags, &error_);
   if (create_status_ != BB200_OK) return;
   uint64_t tiles = 0, rows = 0;
   members_.reserve(static_cast<size_t>(n_members));
@@ -757,6 +759,9 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
   // take_while_kld (Filter::resample_kld).
   auto resamples_kld = [&](uint32_t k) { return plans[k].resample != 0 && plans[k].opts.min_particles < plans[k].opts.max_particles; };
   const bool kld = std::any_of(active.begin(), active.end(), resamples_kld);
+  // on_effective_size_drop: a selective member whose every_n fired resamples only when its effective sample size drops
+  // below n / 2, decided on the device (batch_ess_kernel).
+  const bool ess = std::any_of(active.begin(), active.end(), [&](uint32_t k) { return plans[k].needs_ess != 0; });
   int st = check(cudaSetDevice(device_), "cudaSetDevice");
   if (st == BB200_OK) st = ensure_points(points_total);  // the previous step has ended: the staging buffers are free
   if (st == BB200_OK && step_map < 0) st = ensure_map_table();
@@ -784,7 +789,7 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     b.slots = m.capacity;
     b.seed = m.policy.params().seed;
     b.step = plan.step;
-    b.resample = plan.resample;
+    b.resample = plan.needs_ess ? kBatchResampleEss : plan.resample;
     b.scheme = plan.opts.scheme;
     b.cur = m.cur;
     b.ceil_log2_count = ceil_log2_count(m.capacity);
@@ -875,20 +880,25 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     }
     row[n_active] = pa.ctas;
   }
-  if (kld) {
-    uint32_t* rows_kld[2] = {first_host_.get() + static_cast<size_t>(kBatchKldRow) * (n_active + 1),
-                             first_host_.get() + static_cast<size_t>(kBatchKldMomentsRow) * (n_active + 1)};
+  if (kld || ess) {
+    uint32_t* post_rows[3] = {first_host_.get() + static_cast<size_t>(kBatchKldRow) * (n_active + 1),
+                              first_host_.get() + static_cast<size_t>(kBatchMomentsRow) * (n_active + 1),
+                              first_host_.get() + static_cast<size_t>(kBatchEssRow) * (n_active + 1)};
+    uint32_t totals[3] = {0, 0, 0};
     for (uint32_t j = 0; j < n_active; ++j) {
-      uint32_t ctas[2];
-      batch_kld_ctas(table_host_.get()[j], ctas);
-      for (int l = 0; l < 2; ++l) {
-        rows_kld[l][j] = a.kld_ctas[l];
-        a.kld_ctas[l] += ctas[l];
+      uint32_t ctas[3];
+      batch_post_ctas(table_host_.get()[j], ctas);
+      for (int l = 0; l < 3; ++l) {
+        post_rows[l][j] = totals[l];
+        totals[l] += ctas[l];
       }
     }
-    for (int l = 0; l < 2; ++l) rows_kld[l][n_active] = a.kld_ctas[l];
+    for (int l = 0; l < 3; ++l) post_rows[l][n_active] = totals[l];
+    a.post_ctas[0] = totals[0];
+    a.post_ctas[1] = totals[1];
+    a.ess_ctas = totals[2];
   }
-  const int rows = kld ? kBatchRows : convert ? kBatchLaunches + 1 : kBatchLaunches;
+  const int rows = kld || ess ? kBatchRows : convert ? kBatchLaunches + 1 : kBatchLaunches;
 
   cudaStream_t stream = stream_;
   for (const uint32_t k : active) members_[k].cdf_total = 0;  // from here on the step may have rewritten their CDFs
@@ -970,7 +980,8 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     bb200_update_result& r = out[k];
     estimate_from_moments(s.moments, m.pivot, &r.estimate);
     pivot_to_estimate(r.estimate, m.pivot);
-    if (plan.resample) {
+    const bool resampled = plan.needs_ess ? s.resampled != 0 : plan.resample != 0;  // the device's decision for a selective member
+    if (resampled) {
       m.cur ^= 1;
       m.n = table_host_.get()[j].kld ? s.accepted : m.capacity;
       m.ancestors_n = m.n;
@@ -978,7 +989,7 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
       m.cdf_total = s.total;  // the step's scan, over the weights before normalisation
     }
     r.updated = 1;
-    r.resampled = plan.resample;
+    r.resampled = resampled ? 1 : 0;
     r.n_particles = m.n;
     r.random_state_probability = plan.random_state_probability;
     r.weight_sum = std::ldexp(static_cast<double>(s.total), -s.exponent);

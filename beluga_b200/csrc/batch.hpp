@@ -21,15 +21,16 @@ constexpr uint64_t kBatchMaxParticles = 32768;
 
 class Batch {
  public:
-  /// adaptive: members may have min_particles < max_particles (KLD-adaptive particle counts, as a standalone filter);
-  /// otherwise every member keeps a fixed count.  The flag changes validation only.
-  Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bool adaptive = false);
+  /// flags (bb200_batch_flags): BB200_BATCH_ADAPTIVE lets members have min_particles < max_particles (KLD-adaptive
+  /// particle counts, as a standalone filter), otherwise every member keeps a fixed count; BB200_BATCH_SELECTIVE lets
+  /// members have selective_resampling.  The flags change validation only.
+  Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, uint32_t flags = 0);
   ~Batch();
   Batch(const Batch&) = delete;
   Batch& operator=(const Batch&) = delete;
 
   /// The configurations a batch rejects, checked without touching a device (BB200_OK or BB200_ERR_INVALID_ARGUMENT).
-  static int validate(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bool adaptive, std::string* error);
+  static int validate(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, uint32_t flags, std::string* error);
 
   bool ok() const { return created_; }
   int create_status() const { return create_status_; }
@@ -96,8 +97,8 @@ class Batch {
     uint32_t table_slots{0};   // a power of two >= 2 * capacity
     int map{-1};               // id of the map it reads (-1: none)
     // Total of the CDF in its cdf_ slice while that CDF is the one a standalone filter would sample from (Filter's
-    // cdf_valid_): set by a step that normalised and by a rebuild in sample_states; 0 (stale) after a resampling step,
-    // an initialisation or a failed step.
+    // cdf_valid_): set by a step that kept the particles (normalised, or selective with a high effective sample size)
+    // and by a rebuild in sample_states; 0 (stale) after a resampling step, an initialisation or a failed step.
     unsigned long long cdf_total{0};
     // The beam directions of the last scan it passed (update_measurements), kept until the scan geometry changes: the
     // key, the kept readings' indices and their (cos, sin) on the device.
@@ -164,7 +165,9 @@ class Batch {
   DeviceBuffer<double> partials_;
   DeviceBuffer<BatchMember> table_;
   PinnedBuffer<BatchMember> table_host_;
-  DeviceBuffer<uint32_t> first_;  // kBatchRows x (K + 1): the step's rows, then batch_points_kernel's and the two KLD rows
+  // kBatchRows x (K + 1): the step's rows, then those of batch_points_kernel, batch_kld_kernel, batch_resampled_moments_kernel
+  // and batch_ess_kernel
+  DeviceBuffer<uint32_t> first_;
   PinnedBuffer<uint32_t> first_host_;
   DeviceBuffer<double> points_;   // (x, y) pairs
   PinnedBuffer<double> points_host_;

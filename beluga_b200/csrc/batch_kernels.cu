@@ -176,6 +176,7 @@ struct BatchTail {
   int* ticket;
   int seq;
   unsigned long long accepted;  // StepSummary::accepted
+  int resampled;                // StepSummary::resampled
 };
 __device__ __forceinline__ bool tail_enabled(const BatchTail&) { return true; }
 __device__ __forceinline__ void tail_publish(const BatchTail& tail, const double* v, Scalars* scalars) {
@@ -183,6 +184,7 @@ __device__ __forceinline__ void tail_publish(const BatchTail& tail, const double
   for (int k = 0; k < kMomentCount; ++k) tail.summary->moments[k] = v[k];
   scalars->blocks_done = 0;
   tail.summary->accepted = tail.accepted;
+  tail.summary->resampled = tail.resampled;
   tail.summary->total = scalars->total;
   tail.summary->exponent = scalars->exponent;
   tail.summary->valid = scalars->valid;
@@ -196,14 +198,45 @@ __device__ __forceinline__ void tail_publish(const BatchTail& tail, const double
   }
 }
 
-/// A step that keeps its particles: normalize_kernel's w /= S and moments_kernel's rows over the same partition
-/// (moments_block_count blocks), the rows summed like reduce_partials_kernel does.
+/// normalize_kernel's blocks (launch_normalize's partition, moments_block_count(n) blocks) for each member that runs the
+/// effective-sample-size test; the last of a member's blocks to arrive sums their rows as reduce_partials_kernel does and
+/// stores on_effective_size_drop's decision, ESS = 1 / sum w~^2 < n / 2, in scalars->ess_resample (a sum that is not
+/// positive, NaN included, gives ESS 0: resample).  The same double arithmetic as Amcl::update_device on the host.
+__global__ void __launch_bounds__(kStreamThreads) batch_ess_kernel(BatchStepArgs s) {
+  __shared__ double s_red[kStreamThreads / kWarp];
+  __shared__ int s_last;
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kBatchEssRow, blockIdx.x, local, count);
+  const BatchMember& m = s.members[k];
+  Scalars* scalars = s.scalars + k;
+  double* rows = s.partials + (blockIdx.x - local);  // one sum of squares per CTA
+  normalize_block(s.weights + m.offset, m.n, scalars, 0, rows, RangeBlocks{local, count});
+  if (threadIdx.x == 0) {
+    __threadfence();  // the row before the arrival count
+    s_last = atomicAdd(&scalars->blocks_done, 1u) + 1u == count ? 1 : 0;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  double v = 0.0;
+  for (uint32_t r = threadIdx.x; r < count; r += kStreamThreads) v = v + __ldcg(rows + r);
+  const double sum_sq = block_sum<kStreamThreads>(v, s_red);
+  if (threadIdx.x == 0) {
+    const double ess = sum_sq > 0.0 ? 1.0 / sum_sq : 0.0;
+    scalars->ess_resample = ess < static_cast<double>(m.n) * 0.5 ? 1 : 0;
+    scalars->blocks_done = 0;  // free for the arrivals of the finish launch
+  }
+}
+
+/// A step that keeps its particles: normalize_kernel's w /= S (unless batch_ess_kernel has divided already) and
+/// moments_kernel's rows over the same partition (moments_block_count blocks), the rows summed like
+/// reduce_partials_kernel does.
 __device__ __forceinline__ void normalize_moments_block(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n, double px,
                                                         double py, Scalars* scalars, double* __restrict__ moment_partials, uint32_t block,
-                                                        uint32_t grid, const BatchTail& tail) {
+                                                        uint32_t grid, const BatchTail& tail, bool divide) {
   __shared__ double s_red[kMomentCount * kStreamThreads / kWarp];
   const double factor = scalbn(static_cast<double>(scalars->total), -scalars->exponent);
-  const bool valid = scalars->valid != 0 && factor > 0.0;
+  const bool valid = divide && scalars->valid != 0 && factor > 0.0;
   double m[kMomentCount];
 #pragma unroll
   for (int k = 0; k < kMomentCount; ++k) m[k] = 0.0;
@@ -221,7 +254,10 @@ __device__ __forceinline__ void normalize_moments_block(const Pose2* __restrict_
 /// Per member: resample_scatter_kernel or resample_kernel (recovery injection, multinomial draws) on a resampling step,
 /// normalisation otherwise; then the member's moments, summed by its last CTA.  A member that resamples under KLD draws
 /// every one of its max_particles slots with their spatial hashes, as Filter::resample_kld's one chunk does, and leaves
-/// its summary to batch_kld_moments_kernel.
+/// its summary to batch_resampled_moments_kernel.  A member that ran the effective-sample-size test follows its
+/// decision: it draws and leaves its summary to that kernel too (Filter::resample, then Filter::estimate), or it sums the
+/// moments of the weights batch_ess_kernel normalised (Filter::estimate).  Its range fits either partition; the CTAs
+/// beyond the one it takes only leave.
 template <bool kTable>
 __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs s) {
   uint32_t local, count;
@@ -229,9 +265,12 @@ __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs 
   const BatchMember& m = s.members[k];
   Scalars* scalars = s.scalars + k;
   double* partials = s.partials + static_cast<size_t>(blockIdx.x - local) * kMomentCount;
-  const BatchTail tail{s.summary + k, s.members_done, s.n_members, s.ticket, s.seq, 0};
-  if (!m.resample) {
-    normalize_moments_block(batch_states(s, m, 0), s.weights + m.offset, m.n, m.pivot_x, m.pivot_y, scalars, partials, local, count, tail);
+  const bool ess = m.resample == kBatchResampleEss;
+  const BatchTail tail{s.summary + k, s.members_done, s.n_members, s.ticket, s.seq, 0, m.resample == 1 ? 1 : 0};
+  if (!m.resample || (ess && scalars->ess_resample == 0)) {
+    const uint32_t grid = ess ? moments_blocks(m.n) : count;
+    if (local >= grid) return;
+    normalize_moments_block(batch_states(s, m, 0), s.weights + m.offset, m.n, m.pivot_x, m.pivot_y, scalars, partials, local, grid, tail, !ess);
     return;
   }
   ResampleArgs a{};
@@ -250,12 +289,22 @@ __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs 
   batch_recovery_map<kTable>(s, m, a);
   a.pivot_x = m.pivot_x;
   a.pivot_y = m.pivot_y;
-  if (m.kld) {  // launch_resample with hashes: always the per-slot form; a.tail is the disabled one (no summary, no arrival)
+  if (m.kld) {  // launch_resample with hashes: always the per-slot form
     const BatchKldMember& q = s.kld[k];
     a.hashes = s.hashes + m.offset;
     for (int d = 0; d < 3; ++d) a.hash_resolution[d] = q.hash_resolution[d];
-    resample_block(a, scalars, partials, local, count, a.tail);
-  } else if (m.scheme == 1 && m.random_state_probability <= 0.0) {  // systematic, nothing drawn per slot: launch_resample's scatter form
+  }
+  // systematic, nothing drawn per slot and no hashes: launch_resample's scatter form
+  const bool scatter = !m.kld && m.scheme == 1 && m.random_state_probability <= 0.0;
+  if (m.kld || ess) {  // a.tail is the disabled one (no summary, no arrival): batch_resampled_moments_kernel publishes
+    const uint32_t grid = scatter ? resample_scatter_blocks(m.n) : resample_blocks(m.slots);
+    if (local >= grid) return;
+    if (scatter) {
+      resample_scatter_block(a, scalars, partials, local, grid, a.tail);
+    } else {
+      resample_block(a, scalars, partials, local, grid, a.tail);
+    }
+  } else if (scatter) {
     resample_scatter_block(a, scalars, partials, local, count, tail);
   } else {
     resample_block(a, scalars, partials, local, count, tail);
@@ -272,14 +321,22 @@ __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs 
 constexpr int kBatchKldThreads = 1024;
 constexpr int kBatchKldWarps = kBatchKldThreads / kWarp;
 
+/// Whether a member of the step drew a new particle set: every resampling member, except a selective one whose effective
+/// sample size stayed at n / 2 or above.
+__device__ __forceinline__ bool batch_resampled(const BatchMember& m, const Scalars* scalars) {
+  return m.resample == 1 || (m.resample == kBatchResampleEss && scalars->ess_resample != 0);
+}
+
 /// One CTA per KLD member: clear its bucket set, insert every slot's hash, then flag first occurrences and scan them
-/// chunk by chunk in slot order; scalars->kld_cutoff receives the first failing count (~0 when every count passes).
+/// chunk by chunk in slot order; scalars->kld_cutoff receives the first failing count (~0 when every count passes).  A
+/// selective member that kept its particles has nothing to count.
 __global__ void __launch_bounds__(kBatchKldThreads) batch_kld_kernel(BatchStepArgs s) {
   __shared__ uint32_t s_warp[kBatchKldWarps];
   __shared__ unsigned long long s_min[kBatchKldWarps];
   uint32_t local, count;
   const uint32_t k = batch_member_of(s, kBatchKldRow, blockIdx.x, local, count);
   const BatchMember& m = s.members[k];
+  if (!batch_resampled(m, s.scalars + k)) return;
   const BatchKldMember& q = s.kld[k];
   const unsigned long long* hashes = s.hashes + m.offset;
   unsigned long long* keys = s.keys + q.table_offset;
@@ -330,18 +387,25 @@ __global__ void __launch_bounds__(kBatchKldThreads) batch_kld_kernel(BatchStepAr
   }
 }
 
-/// moments_kernel over the particles a KLD member keeps (unit weights, the partition of moments_block_count(accepted)
-/// blocks), summed like reduce_partials_kernel by the last of those CTAs, which publishes the member's summary.  Each KLD
-/// member has moments_block_count(max_particles) CTAs; those beyond moments_block_count(accepted) only leave.
-__global__ void __launch_bounds__(kStreamThreads) batch_kld_moments_kernel(BatchStepArgs s) {
+/// Filter::estimate after Filter::resample: moments_kernel over the new particle set of a member that resampled under KLD
+/// or after the effective-sample-size test (unit weights, the partition of moments_block_count(accepted) blocks), summed
+/// like reduce_partials_kernel by the last of those CTAs, which publishes the member's summary.  accepted is the KLD count
+/// of a KLD member and max_particles otherwise.  Each such member has moments_block_count(max_particles) CTAs; those
+/// beyond moments_block_count(accepted) only leave, and so do all of those of a selective member that kept its particles
+/// (batch_finish_kernel published its summary).
+__global__ void __launch_bounds__(kStreamThreads) batch_resampled_moments_kernel(BatchStepArgs s) {
   __shared__ double s_red[kMomentCount * kStreamThreads / kWarp];
   uint32_t local, count;
-  const uint32_t k = batch_member_of(s, kBatchKldMomentsRow, blockIdx.x, local, count);
+  const uint32_t k = batch_member_of(s, kBatchMomentsRow, blockIdx.x, local, count);
   const BatchMember& m = s.members[k];
   Scalars* scalars = s.scalars + k;
-  const unsigned long long cutoff = scalars->kld_cutoff;
-  // take_while drops the first element whose condition fails (take_while_kld.hpp:134-136)
-  const uint64_t accepted = cutoff != ~0ull ? (cutoff - 1 < m.slots ? cutoff - 1 : m.slots) : m.slots;
+  if (!batch_resampled(m, scalars)) return;
+  uint64_t accepted = m.slots;
+  if (m.kld) {
+    const unsigned long long cutoff = scalars->kld_cutoff;
+    // take_while drops the first element whose condition fails (take_while_kld.hpp:134-136)
+    accepted = cutoff != ~0ull ? (cutoff - 1 < m.slots ? cutoff - 1 : m.slots) : m.slots;
+  }
   const uint32_t grid = moments_blocks(accepted);
   if (local >= grid) return;
   const Pose2* states = batch_states(s, m, 1);  // the new set (the host flips cur once the step has ended)
@@ -350,7 +414,7 @@ __global__ void __launch_bounds__(kStreamThreads) batch_kld_moments_kernel(Batch
   for (int c = 0; c < kMomentCount; ++c) v[c] = 0.0;
   for (uint64_t i = static_cast<uint64_t>(local) * kStreamThreads + threadIdx.x; i < accepted; i += static_cast<uint64_t>(grid) * kStreamThreads)
     accumulate_moments(v, load_pose(states + i), 1.0, m.pivot_x, m.pivot_y);  // the draw wrote w = 1 to every slot
-  const BatchTail tail{s.summary + k, s.members_done, s.n_members, s.ticket, s.seq, accepted};
+  const BatchTail tail{s.summary + k, s.members_done, s.n_members, s.ticket, s.seq, m.kld ? accepted : 0, 1};
   finish_block_moments<kStreamThreads>(v, s_red, s.partials + static_cast<size_t>(blockIdx.x - local) * kMomentCount, scalars, local, grid, tail);
 }
 
@@ -526,11 +590,18 @@ int launch_batch_step_from(const BatchStepArgs& s, cudaStream_t stream) {
     launches += 1;
   }
   batch_scan_kernel<<<s.ctas[kBatchScan], kQsThreads, 0, stream>>>(s);
+  if (s.ess_ctas > 0) {
+    batch_ess_kernel<<<s.ess_ctas, kStreamThreads, 0, stream>>>(s);
+    launches += 1;
+  }
   batch_finish_kernel<kTable><<<s.ctas[kBatchFinish], kRsThreads, 0, stream>>>(s);
   if (s.kld != nullptr) {
-    batch_kld_kernel<<<s.kld_ctas[0], kBatchKldThreads, 0, stream>>>(s);
-    batch_kld_moments_kernel<<<s.kld_ctas[1], kStreamThreads, 0, stream>>>(s);
-    launches += 2;
+    batch_kld_kernel<<<s.post_ctas[0], kBatchKldThreads, 0, stream>>>(s);
+    launches += 1;
+  }
+  if (s.kld != nullptr || s.ess_ctas > 0) {
+    batch_resampled_moments_kernel<<<s.post_ctas[1], kStreamThreads, 0, stream>>>(s);
+    launches += 1;
   }
   return launches;
 }
@@ -547,16 +618,18 @@ void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunch
   // the partition launch_resample / launch_moments would use for a single filter of this size
   if (!m.resample) {
     out[kBatchFinish] = moments_block_count(m.n);
-  } else if (m.scheme == 1 && m.random_state_probability <= 0.0 && !m.kld) {
-    out[kBatchFinish] = resample_scatter_block_count(m.n);
-  } else {
-    out[kBatchFinish] = resample_block_count(m.slots);
+    return;
   }
+  const uint32_t draw = m.scheme == 1 && m.random_state_probability <= 0.0 && !m.kld ? resample_scatter_block_count(m.n) : resample_block_count(m.slots);
+  // a selective member's range fits the draw and the moments of the weights it keeps, whichever the device decides
+  out[kBatchFinish] = m.resample == kBatchResampleEss ? std::max(draw, moments_block_count(m.n)) : draw;
 }
 
-void batch_kld_ctas(const BatchMember& m, uint32_t out[2]) {
+void batch_post_ctas(const BatchMember& m, uint32_t out[3]) {
+  const bool ess = m.resample == kBatchResampleEss;
   out[0] = m.kld ? 1u : 0u;
-  out[1] = m.kld ? moments_blocks(m.slots) : 0u;
+  out[1] = m.kld || ess ? moments_blocks(m.slots) : 0u;
+  out[2] = ess ? moments_blocks(m.n) : 0u;  // launch_normalize's partition
 }
 
 int launch_batch_step(const BatchStepArgs& s, cudaStream_t stream) {

@@ -33,7 +33,7 @@ struct bb200_amcl {
 
 struct bb200_amcl_batch {
   Batch impl;
-  bb200_amcl_batch(const bb200_amcl_param* p, const bb200_motion_param* m, int n, bool adaptive) : impl(p, m, n, adaptive) {}
+  bb200_amcl_batch(const bb200_amcl_param* p, const bb200_motion_param* m, int n, uint32_t flags) : impl(p, m, n, flags) {}
 };
 
 /// One filter over several shards driven by ONE host thread (the shape of beluga_ros's single-process node).
@@ -121,18 +121,18 @@ int set_sharded_map(bb200_sharded_amcl* g, Prepare&& prepare) {
   });
 }
 
-int create_batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bool adaptive, bb200_amcl_batch** out) {
+int create_batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, uint32_t flags, bb200_amcl_batch** out) {
   if (out == nullptr) {
     g_create_error = "null argument";
     return BB200_ERR_INVALID_ARGUMENT;
   }
   *out = nullptr;
   {
-    const int st = Batch::validate(params, motions, n_members, adaptive, &g_create_error);  // before any device is touched
+    const int st = Batch::validate(params, motions, n_members, flags, &g_create_error);  // before any device is touched
     if (st != BB200_OK) return st;
   }
   return guarded_create([&] {
-    auto b = std::make_unique<bb200_amcl_batch>(params, motions, n_members, adaptive);
+    auto b = std::make_unique<bb200_amcl_batch>(params, motions, n_members, flags);
     if (!b->impl.ok()) {
       g_create_error = b->impl.last_error();
       return b->impl.create_status();
@@ -803,10 +803,14 @@ int bb200_sharded_amcl_get_particles(bb200_sharded_amcl* g, double* states, doub
 // ---- batches ------------------------------------------------------------------------------------------
 
 int bb200_amcl_batch_create(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bb200_amcl_batch** out) {
-  return create_batch(params, motions, n_members, false, out);
+  return create_batch(params, motions, n_members, 0, out);
 }
 int bb200_amcl_batch_create_adaptive(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bb200_amcl_batch** out) {
-  return create_batch(params, motions, n_members, true, out);
+  return create_batch(params, motions, n_members, BB200_BATCH_ADAPTIVE, out);
+}
+int bb200_amcl_batch_create_with_flags(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, uint32_t flags,
+                                       bb200_amcl_batch** out) {
+  return create_batch(params, motions, n_members, flags, out);
 }
 int bb200_amcl_batch_member_size(const bb200_amcl_batch* b, int member, uint64_t* n) {
   BB_REQUIRE(b && n);

@@ -114,7 +114,7 @@ struct Scalars {
   unsigned long long kld_cutoff;  // first slot (1-based count) at which the KLD condition fails
   unsigned long long kld_scan_ticket;  // KLD chunk: tile ticket of the flag scan
   unsigned long long kld_new_buckets;  // KLD chunk: distinct buckets that first occur in the chunk
-  unsigned long long pad;
+  unsigned long long ess_resample;  // selective batch members: 1 when the step's effective sample size asks for a resample
   unsigned long long work_ticket;  // persistent reweight kernel: next 32-particle task (rewound by the last warp out)
   unsigned long long work_done;    // warps that have left that kernel
   int exchange_error;              // sticky: a shard exchange timed out
@@ -149,6 +149,7 @@ struct StepSummary {
   int error;                      // 1: a peer never posted (bounded spin ran out)
   int seq;                        // completion ticket of the step that wrote this block (written last; the host may poll it)
   unsigned long long accepted;    // batch members resampled under KLD: the particles take_while_kld kept (0 otherwise)
+  int resampled;                  // batch members: 1 when the step replaced the particle set, 0 when it kept it
 };
 struct ShardExchangeArgs {
   int kind, post, wait;
@@ -408,6 +409,10 @@ uint32_t resample_scatter_block_count(uint64_t n_in);
 // and the range's length as the grid.  Each member therefore sees the CTA partition -- and the moment partials, and so
 // the rounding -- of a single filter of its size.
 
+/// BatchMember::resample of a selective member whose every_n fired: normalise, then resample only when ESS = 1 / sum w~^2
+/// falls below n / 2 (on_effective_size_drop), a decision made on the device.
+constexpr int kBatchResampleEss = 2;
+
 /// What one member does in a batch step (built on the host every step).
 struct BatchMember {
   uint64_t offset;          // first particle of the member in the batch buffers
@@ -415,7 +420,8 @@ struct BatchMember {
   uint64_t slots;           // max_particles: particles after a resample
   uint64_t seed;
   uint32_t step;
-  int resample;             // 1: resample (every_n fired); 0: normalise the weights and keep the particles
+  int resample;             // 1: resample (every_n fired); 0: normalise the weights and keep the particles; kBatchResampleEss:
+                            // every_n fired on a selective member, the effective sample size decides on the device
   int scheme;               // bb200_resample_scheme
   int cur;                  // state buffer holding the member's particles
   int ceil_log2_count;      // of max_particles: the fixed-point exponent's headroom
@@ -510,15 +516,20 @@ struct BatchStepArgs {
   unsigned long long* hashes;     // the per-slot spatial hashes of the draw, at each member's offset
   unsigned long long* keys;       // the members' bucket sets (BatchKldMember::table_offset)
   unsigned int* vals;
-  uint32_t kld_ctas[2];           // total CTAs of batch_kld_kernel and batch_kld_moments_kernel
+  uint32_t post_ctas[2];          // total CTAs of batch_kld_kernel and batch_resampled_moments_kernel
+  // Selective members (BatchMember::resample == kBatchResampleEss): total CTAs of batch_ess_kernel, 0 when the step has none.
+  uint32_t ess_ctas;
 };
 static_assert(sizeof(BatchStepArgs) <= 1024, "the step's arguments travel as one kernel parameter block (4 KB at most)");
 /// Reset | propagate | reweight | quantise + scan | resample or normalise + moments.  The reweight takes one launch for the
 /// likelihood field, two for the beam model's two-pass form (walk, mixture) and one for its fused form, each issued
-/// when some member takes that form.  When some member resamples under KLD (args.kld set), two launches follow: the
-/// KLD count of each such member and the moments of the particles it keeps.  Returns the number of launches: 4 plus
-/// those, so 5 to 8 without KLD members and 7 to 10 with them, whatever the members, their maps, their particle counts,
-/// their accepted counts and their scans are.
+/// when some member takes that form.  When some member runs the effective-sample-size test (args.ess_ctas > 0), one
+/// launch before the resample normalises its weights and decides.  After the resample, when some member resamples under
+/// KLD (args.kld set), one launch counts each such member's particles; and when some member resamples under KLD or runs
+/// the test, one launch sums the moments of every new particle set that a separate estimate pass reads in a standalone
+/// filter.  Returns the number of launches: 4 plus those, so 5 to 8 without either kind of member, 7 to 10 with KLD
+/// members or with selective ones, and 8 to 11 with both, whatever the members, their maps, their particle counts,
+/// their decisions, their accepted counts and their scans are.
 int launch_batch_step(const BatchStepArgs& args, cudaStream_t stream);
 /// Scan tiles of a member of n particles (the quantise-scan CTAs it needs).
 uint32_t batch_scan_tiles(uint64_t n);
@@ -528,11 +539,13 @@ uint32_t batch_scan_tiles(uint64_t n);
 // at its point_offset, and its n_points and points_radius into the step's member table, which the step's kernels then read
 // in stream order.  Its CTA ranges are one more row of the step's `first` buffer, after the kBatchLaunches rows.
 constexpr int kBatchPointsRow = kBatchLaunches;
-/// The rows of batch_kld_kernel (one CTA per KLD member) and batch_kld_moments_kernel (moments_block_count(max_particles)
-/// CTAs per KLD member), after batch_points_kernel's; a step's `first` buffer holds kBatchRows rows.
+/// The rows of batch_kld_kernel (one CTA per KLD member), batch_resampled_moments_kernel (moments_block_count(max_particles)
+/// CTAs per KLD or selective member) and batch_ess_kernel (moments_block_count(n) CTAs per selective member), after
+/// batch_points_kernel's; a step's `first` buffer holds kBatchRows rows.
 constexpr int kBatchKldRow = kBatchLaunches + 1;
-constexpr int kBatchKldMomentsRow = kBatchLaunches + 2;
-constexpr int kBatchRows = kBatchLaunches + 3;
+constexpr int kBatchMomentsRow = kBatchLaunches + 2;
+constexpr int kBatchEssRow = kBatchLaunches + 3;
+constexpr int kBatchRows = kBatchLaunches + 4;
 /// How a member's measurement reaches a batch step (the values of bb200_measurement_kind).
 enum BatchInputKind : int { kBatchInputPoints = 0, kBatchInputScan = 1, kBatchInputCloud = 2 };
 /// One member of batch_points_kernel, built on the host every step (one per entry of the step's member table).
@@ -561,8 +574,9 @@ uint32_t batch_points_ctas(const BatchPointsMember& m);
 int launch_batch_points(const BatchPointsArgs& args, cudaStream_t stream);
 /// CTAs of a member in each row of a batch step's ranges, for a member that takes reweight form `form`.
 void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunches]);
-/// CTAs of a member in the rows kBatchKldRow and kBatchKldMomentsRow (none unless it resamples under KLD).
-void batch_kld_ctas(const BatchMember& m, uint32_t out[2]);
+/// CTAs of a member in the rows kBatchKldRow, kBatchMomentsRow and kBatchEssRow: a KLD count when it may resample under KLD,
+/// the moments of a new set when it may resample under KLD or runs the effective-sample-size test, and that test.
+void batch_post_ctas(const BatchMember& m, uint32_t out[3]);
 
 /// One member of a batch's pose-sample draw (Filter::sample_states per member).
 struct BatchSampleMember {

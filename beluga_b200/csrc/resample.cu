@@ -11,23 +11,7 @@ namespace {
 
 __global__ void __launch_bounds__(kStreamThreads) normalize_kernel(double* __restrict__ weights, uint64_t n, const Scalars* scalars,
                                                                    unsigned long long global_total, double* __restrict__ partials) {
-  __shared__ double s_red[kStreamThreads / kWarp];
-  // S = T * 2^-e: the normalisation factor derived from the exact integer total.
-  // 0: single GPU, the total is on the device; ~0: sharded, the sum of the ranks' totals is on the device
-  const unsigned long long t = global_total == ~0ull ? scalars->global_total : (global_total != 0 ? global_total : scalars->total);
-  const double factor = scalbn(static_cast<double>(t), -scalars->exponent);
-  const bool valid = scalars->valid != 0 && factor > 0.0;
-  double sq = 0.0;
-  for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kStreamThreads + threadIdx.x; i < n; i += static_cast<uint64_t>(gridDim.x) * kStreamThreads) {
-    double w = weights[i];
-    if (valid) {
-      w = w / factor;  // actions/normalize.hpp:82
-      weights[i] = w;
-    }
-    sq = sq + w * w;
-  }
-  const double total = block_sum<kStreamThreads>(sq, s_red);
-  if (threadIdx.x == 0) partials[blockIdx.x] = total;
+  normalize_block(weights, n, scalars, global_total, partials, LaunchBlocks{});
 }
 
 // ---- resample -------------------------------------------------------------------------------------
@@ -78,14 +62,9 @@ void launch_normalize(double* weights, uint64_t n, const Scalars* scalars, unsig
   normalize_kernel<<<blocks, kStreamThreads, 0, stream>>>(weights, n, scalars, global_total, partials);
 }
 
-uint32_t resample_block_count(uint64_t slots) {
-  return static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>((slots + kRsThreads - 1) / kRsThreads, kSmCount * 16)));
-}
+uint32_t resample_block_count(uint64_t slots) { return resample_blocks(slots); }
 
-uint32_t resample_scatter_block_count(uint64_t n_in) {
-  // one pass over the input particles; a few particles per thread amortise the block reduction of the moments
-  return static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>((n_in + kRsThreads - 1) / kRsThreads, kSmCount * kRsBlocksPerSm)));
-}
+uint32_t resample_scatter_block_count(uint64_t n_in) { return resample_scatter_blocks(n_in); }
 
 uint32_t launch_resample(const ResampleArgs& args, Scalars* scalars, double* moment_partials, cudaStream_t stream) {
   // The whole set on one GPU with the systematic comb and nothing per slot to draw: scatter form.

@@ -16,9 +16,65 @@ BB_HD uint32_t moments_blocks(uint64_t n) {
   return static_cast<uint32_t>(blocks < 1 ? 1 : blocks > kStreamMaxBlocks ? kStreamMaxBlocks : blocks);
 }
 
+// ---- normalize -------------------------------------------------------------------------------------
+
+/// The block index and block count a block body runs with: the launch's own (a single-filter kernel; read where they are
+/// used, so that the kernel compiles as it did with the body written inside it) ...
+struct LaunchBlocks {
+  __device__ __forceinline__ uint32_t block() const { return blockIdx.x; }
+  __device__ __forceinline__ uint32_t grid() const { return gridDim.x; }
+};
+/// ... or a batch member's range of the launch.
+struct RangeBlocks {
+  uint32_t index, count;
+  __device__ __forceinline__ uint32_t block() const { return index; }
+  __device__ __forceinline__ uint32_t grid() const { return count; }
+};
+
+/// One block of normalize_kernel: w /= S (S = T * 2^-e, T = global_total, or scalars->global_total when it is ~0, or
+/// scalars->total when it is 0) when the weights are valid, and the block's sum of w^2 into partials[block].
+template <class Blocks>
+__device__ __forceinline__ void normalize_block(double* __restrict__ weights, uint64_t n, const Scalars* scalars, unsigned long long global_total,
+                                                double* __restrict__ partials, const Blocks& blocks) {
+  __shared__ double s_red[kStreamThreads / kWarp];
+  // S = T * 2^-e: the normalisation factor derived from the exact integer total.
+  // 0: single GPU, the total is on the device; ~0: sharded, the sum of the ranks' totals is on the device
+  const unsigned long long t = global_total == ~0ull ? scalars->global_total : (global_total != 0 ? global_total : scalars->total);
+  const double factor = scalbn(static_cast<double>(t), -scalars->exponent);
+  const bool valid = scalars->valid != 0 && factor > 0.0;
+  double sq = 0.0;
+  for (uint64_t i = static_cast<uint64_t>(blocks.block()) * kStreamThreads + threadIdx.x; i < n;
+       i += static_cast<uint64_t>(blocks.grid()) * kStreamThreads) {
+    double w = weights[i];
+    if (valid) {
+      w = w / factor;  // actions/normalize.hpp:82
+      weights[i] = w;
+    }
+    sq = sq + w * w;
+  }
+  const double total = block_sum<kStreamThreads>(sq, s_red);
+  if (threadIdx.x == 0) partials[blocks.block()] = total;
+}
+
 // ---- resample -------------------------------------------------------------------------------------
 
 constexpr int kRsThreads = 256;
+// (CTAs per SM, particles per thread and round) = (3, 2) was chosen by a sweep at 1M on a B200, carried over to the H100
+// without re-measuring.
+constexpr int kRsBlocksPerSm = 3;  // resident CTAs per SM the kernel is compiled for (register cap)
+constexpr int kRsUnroll = 2;       // particles per thread and round
+
+/// Blocks of resample_kernel over `slots` output slots (resample_block_count), on the host and on the device.
+BB_HD uint32_t resample_blocks(uint64_t slots) {
+  const uint64_t blocks = (slots + kRsThreads - 1) / kRsThreads;
+  return static_cast<uint32_t>(blocks < 1 ? 1 : blocks > kSmCount * 16 ? kSmCount * 16 : blocks);
+}
+/// Blocks of resample_scatter_kernel over n_in particles (resample_scatter_block_count), on the host and on the device.
+BB_HD uint32_t resample_scatter_blocks(uint64_t n_in) {
+  // one pass over the input particles; a few particles per thread amortise the block reduction of the moments
+  const uint64_t blocks = (n_in + kRsThreads - 1) / kRsThreads;
+  return static_cast<uint32_t>(blocks < 1 ? 1 : blocks > kSmCount * kRsBlocksPerSm ? kSmCount * kRsBlocksPerSm : blocks);
+}
 
 /// Smallest i in [0, n) with cdf[i] > t.
 __device__ __forceinline__ uint64_t cdf_upper_bound(const unsigned long long* __restrict__ cdf, uint64_t n, unsigned long long t) {
@@ -210,11 +266,6 @@ __device__ __forceinline__ void resample_block(const ResampleArgs& a, Scalars* _
 // CDF entries and stores its state jb - ja times.  Same ancestors as resample_kernel by construction
 // (the parity tests compare them with the oracle's lower_bound search); the raw moments are summed per
 // particle (count * term) instead of per slot, which moves the estimate at rounding level only.
-
-// (CTAs per SM, particles per thread and round) = (3, 2) was chosen by a sweep at 1M on a B200, carried over to the H100
-// without re-measuring.
-constexpr int kRsBlocksPerSm = 3;  // resident CTAs per SM the kernel is compiled for (register cap)
-constexpr int kRsUnroll = 2;       // particles per thread and round
 
 /// Number of slots j with offset + j * stride < position, i.e. ceil((position - offset) / stride) capped at total_slots, with
 /// the division replaced by a multiplication with magic = floor((2^64 - 1) / stride): the high word of x * magic is the

@@ -536,8 +536,23 @@ int bb200_amcl_leave_shards(bb200_amcl* a);
  * resampling, non-zero shard fields, max_particles of 0 or above 32768, and members on different devices.
  * bb200_amcl_batch_create_adaptive accepts min_particles <= max_particles as bb200_amcl_create does: a member with
  * min_particles < max_particles resizes its particle set on every resampling step with KLD (take_while_kld), exactly
- * as a standalone bb200_amcl; bb200_amcl_batch_member_size returns its current count.  Such a step takes 2 launches
- * more (the members' KLD counts and the moments of the particles they keep), whatever K and the counts are.
+ * as a standalone bb200_amcl; bb200_amcl_batch_member_size returns its current count.
+ * bb200_amcl_batch_create_with_flags takes the same checks as a set of flags: 0 is bb200_amcl_batch_create,
+ * BB200_BATCH_ADAPTIVE is bb200_amcl_batch_create_adaptive, and BB200_BATCH_SELECTIVE (alone or with
+ * BB200_BATCH_ADAPTIVE) accepts members with selective_resampling: when such a member's resample_interval fires, it
+ * normalises its weights and resamples only when the effective sample size 1 / sum w^2 drops below n / 2 (beluga's
+ * on_effective_size_drop), exactly as a standalone bb200_amcl, and bb200_update_result::resampled reports the decision.
+ * The decision is made on the device, so the step keeps its one host synchronisation.
+ *
+ * A step takes 4 launches, plus those of the reweight forms (below), plus:
+ *  - 1 when some updating member passes a laser scan or a point cloud (bb200_amcl_batch_update_measurements);
+ *  - 2 when some updating member resamples under KLD (the members' KLD counts and the moments of the particles they
+ *    keep) and no updating member runs the effective-sample-size test;
+ *  - 2 when some updating member runs that test and none resamples under KLD (the test, and the moments of the new
+ *    sets of those that resample);
+ *  - 3 when both happen (the test, the KLD counts, the moments).
+ * These counts are fixed before the step runs: they depend on neither K, nor the particle counts, nor the
+ * members' decisions.
  *
  * A batch holds a set of maps, each a grid with its sensor model: likelihood-field model or the beam model.
  * Each member reads one of them or none.  bb200_amcl_batch_set_likelihood_field_map and _set_beam_map give every
@@ -563,6 +578,16 @@ int bb200_amcl_batch_create(const bb200_amcl_param* params, const bb200_motion_p
  * rejects min_particles > max_particles and keeps the other refusals.  A member with min_particles == max_particles
  * keeps a fixed count, and a batch whose members all do computes what a bb200_amcl_batch_create batch computes. */
 int bb200_amcl_batch_create_adaptive(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, bb200_amcl_batch** out);
+/* Flags of bb200_amcl_batch_create_with_flags; any other bit is BB200_ERR_INVALID_ARGUMENT. */
+typedef enum bb200_batch_flags {
+  BB200_BATCH_ADAPTIVE = 1,  /* members may have min_particles < max_particles (KLD) */
+  BB200_BATCH_SELECTIVE = 2  /* members may have selective_resampling */
+} bb200_batch_flags;
+/* bb200_amcl_batch_create with the refusals that `flags` lifts: 0 and BB200_BATCH_ADAPTIVE check exactly what
+ * bb200_amcl_batch_create and bb200_amcl_batch_create_adaptive check.  A BB200_BATCH_SELECTIVE batch whose members
+ * have no selective_resampling computes what a batch without the flag computes, with the same launches. */
+int bb200_amcl_batch_create_with_flags(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, uint32_t flags,
+                                       bb200_amcl_batch** out);
 /* Member m's current particle count in *n (any batch): max_particles after a fixed-size resample, the count KLD kept
  * after an adaptive one, n after bb200_amcl_batch_initialize_states. */
 int bb200_amcl_batch_member_size(const bb200_amcl_batch* b, int member, uint64_t* n);

@@ -210,19 +210,22 @@ template <class MotionModel, class SensorModel, class ExecutionPolicy>
 /// K independent filters on one GPU (bb200_amcl_batch) that read one or several maps, each for a likelihood-field model or
 /// the beam model: update() steps every member with a new scan at once.  Member m behaves like an Amcl built from motions[m] and params[m]; members keep a fixed
 /// particle count (min_particles == max_particles <= 32768) unless the batch is adaptive, whose members may have
-/// min_particles < max_particles and resize their particle sets with KLD as a standalone Amcl does.  Results are returned
+/// min_particles < max_particles and resize their particle sets with KLD as a standalone Amcl does; members of a selective
+/// batch may use selective_resampling, deciding on the device as a standalone Amcl does on the host.  Results are returned
 /// per member, std::nullopt where the reference's update would return it or where the member had no scan this step.
 class AmclBatch {
  public:
   using estimation_type = std::pair<SE2d, Matrix3d>;
 
-  /// adaptive: bb200_amcl_batch_create_adaptive (members may have min_particles < max_particles); particles(m) then
-  /// returns member_size(m) particles.
-  AmclBatch(const std::vector<bb200_motion_param>& motions, const std::vector<AmclParams>& params, bool adaptive = false) : adaptive_{adaptive} {
+  /// adaptive: BB200_BATCH_ADAPTIVE (members may have min_particles < max_particles); particles(m) then returns
+  /// member_size(m) particles.  selective: BB200_BATCH_SELECTIVE (members may have selective_resampling).
+  AmclBatch(const std::vector<bb200_motion_param>& motions, const std::vector<AmclParams>& params, bool adaptive = false, bool selective = false)
+      : adaptive_{adaptive} {
     if (motions.size() != params.size()) throw Error(BB200_ERR_INVALID_ARGUMENT, "one motion model per member");
     std::vector<bb200_amcl_param> p;
     for (const AmclParams& q : params) p.push_back(c_amcl_param(q));
-    const int st = (adaptive ? bb200_amcl_batch_create_adaptive : bb200_amcl_batch_create)(p.data(), motions.data(), static_cast<int>(p.size()), &handle_);
+    const uint32_t flags = (adaptive ? uint32_t{BB200_BATCH_ADAPTIVE} : 0u) | (selective ? uint32_t{BB200_BATCH_SELECTIVE} : 0u);
+    const int st = bb200_amcl_batch_create_with_flags(p.data(), motions.data(), static_cast<int>(p.size()), flags, &handle_);
     if (st != BB200_OK) throw Error(st, bb200_create_error());
     sizes_.reserve(params.size());
     for (const AmclParams& q : params) sizes_.push_back(q.max_particles);

@@ -8,7 +8,8 @@ members read 1, 4 or 16 likelihood-field maps against one single-map batch per m
 `batch_cloud`: the `batch` members' particle-cloud publish round (histograms and pose samples) in one batched call each against
 K standalone filters publishing in turn.  `batch_measurements`: AmclBatch fed laser scans and point clouds converted on the
 device against host conversion plus the points update.  `batch_kld`: the `batch` workload with KLD-adaptive members (min 500,
-max 2000) against K standalone KLD Amcl.
+max 2000) against K standalone KLD Amcl.  `batch_selective`: the `batch` workload with selective-resampling members, fixed-size
+and KLD-adaptive (min 500, max 2000), against K standalone selective Amcl.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import json
@@ -182,6 +183,58 @@ def run_batch_kld():
             "mean_particles": float(np.mean(sizes)), "ms_per_step_e2e": mb, "member_steps_per_s": k * 1e3 / mb,
             "launches_per_step": int(max(launches)), "standalone_ms_per_round": ms, "standalone_member_steps_per_s": k * 1e3 / ms,
             "kernels_ms": {}, "device": device}
+    return res
+
+
+def run_batch_selective():
+    """`batch` with selective-resampling members (on_effective_size_drop): K in {1, 16, 64, 256} members x 2000 particles x 100
+    points on the 2000^2 synthetic map, in one arm fixed-size and in the other KLD-adaptive (min 500, max 2000), every member
+    updating every step; beside it K standalone selective Amcl stepped one after another in the same process.  Also the share
+    of member-steps that resampled."""
+    res = {}
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=100, steps=100)
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    steps, warmup = 20, 3
+    device = device_record()
+    for arm, lo in (("fixed", 2000), ("kld", 500)):
+        for k in (1, 16, 64, 256):
+            params = [bb.AmclParams(min_particles=lo, max_particles=2000, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m, selective_resampling=True)
+                      for m in range(k)]
+            motions = [bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)]
+            batch = bb.AmclBatch(motions, params, adaptive=lo < 2000, selective=True)
+            batch.set_likelihood_field_map(lfm, grid)
+            singles = []
+            for m in range(k):
+                batch.initialize(m, sc.initial_mean, sc.initial_cov)
+                a = bb.Amcl(motions[m], params[m])
+                a.update_map(bb.SENSOR_LIKELIHOOD_FIELD, lfm, grid)
+                a.initialize(sc.initial_mean, sc.initial_cov)
+                singles.append(a)
+            wall_batch, wall_single, launches, resampled, sizes = [], [], [], [], []
+            for t in range(warmup + steps):
+                pose = bb.se2(*sc.poses[t])
+                t0 = time.perf_counter()
+                before = batch.launch_count()
+                r = batch.update([pose] * k, [sc.scans[t]] * k)
+                t1 = time.perf_counter()
+                assert all(x.updated for x in r)
+                launches.append(batch.launch_count() - before)
+                for a, x in zip(singles, r):
+                    y = a.update(pose, sc.scans[t])
+                    assert y.resampled == x.resampled and y.n_particles == x.n_particles
+                t2 = time.perf_counter()
+                if t >= warmup:
+                    wall_batch.append((t1 - t0) * 1e3)
+                    wall_single.append((t2 - t1) * 1e3)
+                    resampled.extend(x.resampled for x in r)
+                    sizes.extend(x.n_particles for x in r)
+            mb, ms = float(np.median(wall_batch)), float(np.median(wall_single))
+            res[f"batch_selective_{arm}_{k}_x_{lo}_2000_x_100_lfm_2000"] = {
+                "members": k, "min_particles": lo, "max_particles": 2000, "points": 100, "steps": steps,
+                "resampled_share": float(np.mean(resampled)), "mean_particles": float(np.mean(sizes)),
+                "ms_per_step_e2e": mb, "member_steps_per_s": k * 1e3 / mb, "launches_per_step": int(max(launches)),
+                "standalone_ms_per_round": ms, "standalone_member_steps_per_s": k * 1e3 / ms, "kernels_ms": {}, "device": device}
     return res
 
 
@@ -643,6 +696,8 @@ def main():
         out.update(run_batch())
     if "batch_kld" in which:
         out.update(run_batch_kld())
+    if "batch_selective" in which:
+        out.update(run_batch_selective())
     if "batch_cluster" in which:
         out.update(run_batch_cluster())
     if "batch_cloud" in which:

@@ -994,6 +994,34 @@ class AmclBatch:
         self._check(self._lib.bb200_amcl_batch_update_measurements(self._h, _dptr(poses), table, mask, res))
         return list(res)
 
+    def update_clustered(self, control_poses, measurements, present=None, linear: float = 0.20, angular: float = 0.524, percentile: float = 0.90,
+                         with_counts: bool = False):
+        """update_measurements, then the cluster-based estimate of every member that updated, in one call
+        (bb200_amcl_batch_update_clustered): what beluga_ros's Amcl::update returns per member.  Returns (results,
+        estimates): the K UpdateResult blocks update_measurements returns, and per member (mean[4], cov[3, 3]) -- with
+        with_counts, (mean, cov, n_cells, n_clusters) -- or None for a member that did not update.  The estimates equal
+        cluster_estimates(present=updated members) called right after update_measurements, byte for byte."""
+        k = len(self.params)
+        if len(measurements) != k:
+            raise ValueError("one measurement per member")
+        mask = self._mask(present)
+        poses = _f64(control_poses).reshape(k, 4)
+        built = [_measurement(m) for m in measurements]
+        table = (_capi.Measurement * k)(*[b[0] for b in built])
+        p = _capi.ClusterParam(linear, angular, percentile)
+        res = (_capi.UpdateResult * k)()
+        est = (_capi.Estimate * k)()
+        cells, clusters = (C.c_uint32 * k)(), (C.c_uint32 * k)()
+        self._check(self._lib.bb200_amcl_batch_update_clustered(self._h, _dptr(poses), table, mask, C.byref(p), res, est, cells, clusters))
+        out = []
+        for m in range(k):
+            if not res[m].updated:
+                out.append(None)
+                continue
+            e = (np.array(est[m].mean), np.array(est[m].cov).reshape(3, 3))
+            out.append((*e, cells[m], clusters[m]) if with_counts else e)
+        return list(res), out
+
     def update_scans(self, control_poses, scans, present=None) -> list:
         """update_measurements with a LaserScan for every member."""
         if any(not isinstance(s, LaserScan) for s in scans):

@@ -240,6 +240,8 @@ SIGNATURES = {
     "bb200_amcl_batch_sample_states": (C.c_int, [_vp, _P(C.c_uint64), C.c_uint32, _P(C.c_uint8), _P(_dbl)]),
     "bb200_amcl_batch_update": (C.c_int, [_vp, _dbl, _P(_dbl), _P(C.c_uint64), _P(C.c_uint8), _P(UpdateResult)]),
     "bb200_amcl_batch_update_measurements": (C.c_int, [_vp, _dbl, _P(Measurement), _P(C.c_uint8), _P(UpdateResult)]),
+    "bb200_amcl_batch_update_clustered": (C.c_int, [_vp, _dbl, _P(Measurement), _P(C.c_uint8), _P(ClusterParam), _P(UpdateResult), _P(Estimate),
+                                                    _P(C.c_uint32), _P(C.c_uint32)]),
     "bb200_amcl_batch_launch_count": (C.c_uint64, [_vp]),
     "bb200_amcl_plan_update": (C.c_int, [_vp, _dbl, _P(StepPlan)]),
     "bb200_amcl_commit_update": (None, [_vp, C.c_int, C.c_double]),

@@ -370,6 +370,30 @@ int Batch::ensure_kld_scratch() {
   return BB200_OK;
 }
 
+int Batch::ensure_select_scratch() {
+  if (const int st = ensure_cluster_scratch()) return st;
+  if (sel_.results.get() != nullptr) return BB200_OK;
+  const RehashTable& table = rehash_table();
+  const size_t k = members_.size();
+  SelectBuffers s;
+  s.offsets.resize(k);
+  uint64_t bytes = 0;
+  for (size_t m = 0; m < k; ++m) {
+    s.offsets[m] = bytes;
+    bytes += (select_scratch_bytes(members_[m].capacity) + 255) / 256 * 256;
+  }
+  BB_CHECK(s.schedule_start.allocate(table.start.size()));
+  BB_CHECK(s.schedule.allocate(table.steps.size()));
+  BB_CHECK(s.scratch.allocate(bytes));
+  BB_CHECK(s.post.allocate(k));
+  BB_CHECK(s.post_host.allocate(k));
+  BB_CHECK(s.results.allocate(k));
+  BB_CHECK(cudaMemcpy(s.schedule_start.get(), table.start.data(), table.start.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+  BB_CHECK(cudaMemcpy(s.schedule.get(), table.steps.data(), table.steps.size() * sizeof(RehashStep), cudaMemcpyHostToDevice));
+  sel_ = std::move(s);
+  return BB200_OK;
+}
+
 int Batch::ensure_cluster_records(uint64_t cells) {
   BB_CHECK(cl_records_host_.grow(cells, std::min<uint64_t>(total_, std::max<uint64_t>(4096, 2 * cells))));
   return BB200_OK;
@@ -707,7 +731,24 @@ int Batch::update_measurements(const double* control_poses, const bb200_measurem
   return step(control_poses, measurements, present, out);
 }
 
-int Batch::step(const double* control_poses, const bb200_measurement* in, const uint8_t* present, bb200_update_result* out) {
+int Batch::update_clustered(const double* control_poses, const bb200_measurement* measurements, const uint8_t* present, const bb200_cluster_param& p,
+                            bb200_update_result* out, bb200_estimate* clustered, uint32_t* n_cells, uint32_t* n_clusters) {
+  error_.clear();
+  for (size_t k = 0; k < members_.size(); ++k) out[k] = bb200_update_result{};
+  if (!(p.linear_hash_resolution > 0.0) || !(p.angular_hash_resolution > 0.0) || !(p.weight_cap_percentile >= 0.0) ||
+      !(p.weight_cap_percentile < 1.0))
+    return fail(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)");
+  for (size_t k = 0; k < members_.size(); ++k) {
+    if (present != nullptr && present[k] == 0) continue;
+    const std::string why = measurement_error(measurements[k]);
+    if (!why.empty()) return fail(BB200_ERR_INVALID_ARGUMENT, "member " + std::to_string(k) + ": " + why);
+  }
+  const ClusteredOut co{&p, clustered, n_cells, n_clusters};
+  return step(control_poses, measurements, present, out, &co);
+}
+
+int Batch::step(const double* control_poses, const bb200_measurement* in, const uint8_t* present, bb200_update_result* out,
+                const ClusteredOut* clustered) {
   error_.clear();
   const size_t count = members_.size();
   for (size_t k = 0; k < count; ++k) out[k] = bb200_update_result{};
@@ -767,6 +808,7 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
   if (st == BB200_OK && step_map < 0) st = ensure_map_table();
   if (st == BB200_OK && convert) st = ensure_inputs(input_floats);
   if (st == BB200_OK && kld) st = ensure_kld_scratch();
+  if (st == BB200_OK && clustered != nullptr) st = ensure_select_scratch();
   for (auto k = active.begin(); st == BB200_OK && k != active.end(); ++k)
     if (in[*k].kind == BB200_MEASUREMENT_SCAN) st = ensure_scan_table(members_[*k], *in[*k].scan);
   if (st != BB200_OK) return rollback(st);
@@ -899,6 +941,30 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     a.ess_ctas = totals[2];
   }
   const int rows = kld || ess ? kBatchRows : convert ? kBatchLaunches + 1 : kBatchLaunches;
+  // update_clustered: the pre-step cluster table and how the step may change each member (batch_cluster_table_kernel).
+  if (clustered != nullptr) {
+    for (uint32_t j = 0; j < n_active; ++j) {
+      const uint32_t k = active[j];
+      const Member& m = members_[k];
+      const bb200_step_plan& plan = plans[k];
+      BatchClusterMember& c = cl_.table_host.get()[j];
+      c = BatchClusterMember{};
+      c.offset = m.offset;
+      c.table_offset = m.table_offset;
+      c.starts_offset = m.offset + k;
+      c.n = static_cast<uint32_t>(m.n);
+      c.table_mask = m.table_slots - 1;
+      c.cur = static_cast<uint32_t>(m.cur);
+      c.pivot_x = m.pivot[0];
+      c.pivot_y = m.pivot[1];
+      BatchClusterPost& q = sel_.post_host.get()[j];
+      q = BatchClusterPost{};
+      q.scratch_offset = sel_.offsets[k];
+      q.capacity = static_cast<uint32_t>(m.capacity);
+      q.mode = plan.needs_ess ? 2 : plan.resample ? 1 : 0;
+      q.kld = resamples_kld(k) ? 1 : 0;
+    }
+  }
 
   cudaStream_t stream = stream_;
   for (const uint32_t k : active) members_[k].cdf_total = 0;  // from here on the step may have rewritten their CDFs
@@ -916,6 +982,12 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     st = check(cudaMemcpyAsync(input_.get(), input_host_.get(), input_floats * sizeof(float), cudaMemcpyHostToDevice, stream), "upload measurements");
   if (st == BB200_OK && kld)
     st = check(cudaMemcpyAsync(kld_.device.get(), kld_.host.get(), n_active * sizeof(BatchKldMember), cudaMemcpyHostToDevice, stream), "upload KLD table");
+  if (st == BB200_OK && clustered != nullptr)
+    st = check(cudaMemcpyAsync(cl_.table.get(), cl_.table_host.get(), n_active * sizeof(BatchClusterMember), cudaMemcpyHostToDevice, stream),
+               "upload cluster table");
+  if (st == BB200_OK && clustered != nullptr)
+    st = check(cudaMemcpyAsync(sel_.post.get(), sel_.post_host.get(), n_active * sizeof(BatchClusterPost), cudaMemcpyHostToDevice, stream),
+               "upload cluster steps");
   if (st != BB200_OK) return rollback(st);
   if (convert) {
     pa.members = table_.get();
@@ -965,36 +1037,164 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
   launches_ += static_cast<uint64_t>(launch_batch_step(a, stream));
   st = check(cudaGetLastError(), "batch step launch");
   if (st != BB200_OK) return rollback(st);
+  const bb200_cluster_param* cp = clustered != nullptr ? clustered->p : nullptr;
+  if (cp != nullptr) {
+    // After the step's last kernel: the post-step cluster table, the cells of every updated member, their selection.
+    BatchSelectArgs sa{};
+    sa.members = cl_.table.get();
+    sa.post = sel_.post.get();
+    sa.summary = summary_host_.get();
+    sa.n_members = n_active;
+    sa.records = cl_.records.get();
+    sa.cells = cl_.cells.get();
+    sa.keys = cl_.keys.get();
+    sa.ids = cl_.ids.get();
+    sa.schedule_start = sel_.schedule_start.get();
+    sa.schedule = sel_.schedule.get();
+    sa.scratch = sel_.scratch.get();
+    sa.linear = cp->linear_hash_resolution;
+    sa.angular = cp->angular_hash_resolution;
+    sa.percentile = cp->weight_cap_percentile;
+    const Rot2 zero = rot_exp(0.0), plus = rot_exp(+sa.angular), minus = rot_exp(-sa.angular);  // glibc, as select_cluster
+    const double lin = sa.linear;
+    const Pose2 adjacent[6] = {Pose2{zero.c, zero.s, +lin, 0.0}, Pose2{zero.c, zero.s, -lin, 0.0}, Pose2{zero.c, zero.s, 0.0, +lin},
+                               Pose2{zero.c, zero.s, 0.0, -lin}, Pose2{plus.c, plus.s, 0.0, 0.0},  Pose2{minus.c, minus.s, 0.0, 0.0}};
+    for (int s = 0; s < 6; ++s) sa.adjacent[s] = adjacent[s];
+    sa.results = sel_.results.get();
+    launch_batch_cluster_table(sa, stream);
+    BatchClusterArgs ca{};
+    ca.members = cl_.table.get();
+    ca.states[0] = states_[0].get();
+    ca.states[1] = states_[1].get();
+    ca.weights = weights_.get();
+    ca.linear = sa.linear;
+    ca.angular = sa.angular;
+    ca.hashes = cl_.hashes.get();
+    ca.keys = cl_.keys.get();
+    ca.first = cl_.first.get();
+    ca.ids = cl_.ids.get();
+    ca.cell_of = cl_.cell_of.get();
+    ca.sort_a = cl_.sort[0].get();
+    ca.sort_b = cl_.sort[1].get();
+    ca.starts = cl_.starts.get();
+    ca.records = cl_.records.get();
+    ca.cells = cl_.cells.get();
+    launch_batch_cluster_cells(ca, n_active, stream);
+    launch_batch_cluster_select(sa, stream);
+    launches_ += 3;
+    st = check(cudaGetLastError(), "batch cluster selection launch");
+    if (st != BB200_OK) return rollback(st);
+  }
 
-  // The last member to finish stores the ticket into pinned memory.
-  const bool done = wait_for_ticket(ticket_host_.get(), seq_, stream);
+  // The last member to finish stores the ticket into pinned memory; the cluster selection runs after it, so a step with
+  // one waits for the whole stream instead.
+  const bool done = cp == nullptr && wait_for_ticket(ticket_host_.get(), seq_, stream);
   if (!done) st = check(cudaStreamSynchronize(stream), "batch step");
   if (st == BB200_OK && !done && *static_cast<volatile int*>(ticket_host_.get()) != seq_) st = fail(BB200_ERR_CUDA, "the batch step ended without its completion ticket");
   if (st != BB200_OK) return rollback(st);
 
+  // What the step did to each member, committed once nothing can fail any more.
+  struct Outcome {
+    int cur;
+    uint64_t n;
+    double pivot[2];
+    bb200_update_result r;
+  };
+  std::vector<Outcome> outcome(n_active);
   for (uint32_t j = 0; j < n_active; ++j) {
     const uint32_t k = active[j];
-    Member& m = members_[k];
+    const Member& m = members_[k];
     const StepSummary& s = summary_host_.get()[j];
     const bb200_step_plan& plan = plans[k];
-    bb200_update_result& r = out[k];
+    Outcome& o = outcome[j];
+    bb200_update_result& r = o.r;
+    r = bb200_update_result{};
     estimate_from_moments(s.moments, m.pivot, &r.estimate);
-    pivot_to_estimate(r.estimate, m.pivot);
+    o.pivot[0] = m.pivot[0];
+    o.pivot[1] = m.pivot[1];
+    pivot_to_estimate(r.estimate, o.pivot);
     const bool resampled = plan.needs_ess ? s.resampled != 0 : plan.resample != 0;  // the device's decision for a selective member
-    if (resampled) {
-      m.cur ^= 1;
-      m.n = table_host_.get()[j].kld ? s.accepted : m.capacity;
-      m.ancestors_n = m.n;
-    } else {
-      m.cdf_total = s.total;  // the step's scan, over the weights before normalisation
-    }
+    o.cur = resampled ? m.cur ^ 1 : m.cur;
+    o.n = resampled ? (table_host_.get()[j].kld ? s.accepted : m.capacity) : m.n;
     r.updated = 1;
     r.resampled = resampled ? 1 : 0;
-    r.n_particles = m.n;
+    r.n_particles = o.n;
     r.random_state_probability = plan.random_state_probability;
     r.weight_sum = std::ldexp(static_cast<double>(s.total), -s.exponent);
     r.weights_degenerate = s.valid != 0 ? 0 : 1;
-    m.policy.commit_update(r.resampled, plan.random_state_probability);
+  }
+
+  if (cp != nullptr) {
+    // Members the device could not promise the host's bits for: their records back to back (batch_cluster_compact_kernel
+    // over those members alone), then select_cluster on the host.
+    const BatchClusterResult* res = sel_.results.get();
+    std::vector<uint32_t> flagged;
+    uint64_t flagged_cells = 0;
+    for (uint32_t j = 0; j < n_active; ++j) {
+      if (!res[j].fallback) continue;
+      BatchClusterMember& c = cl_.table_host.get()[flagged.size()];
+      c = BatchClusterMember{};
+      c.offset = members_[active[j]].offset;
+      cl_.cells_host.get()[flagged.size()] = res[j].cells;
+      flagged_cells += res[j].cells;
+      flagged.push_back(j);
+    }
+    std::vector<ClusterSelection> host_sel(flagged.size());
+    if (!flagged.empty()) {
+      const uint32_t n_flagged = static_cast<uint32_t>(flagged.size());
+      st = ensure_cluster_records(flagged_cells);
+      if (st == BB200_OK)
+        st = check(cudaMemcpyAsync(cl_.table.get(), cl_.table_host.get(), n_flagged * sizeof(BatchClusterMember), cudaMemcpyHostToDevice, stream),
+                   "upload fallback table");
+      if (st == BB200_OK)
+        st = check(cudaMemcpyAsync(cl_.cells.get(), cl_.cells_host.get(), n_flagged * sizeof(uint32_t), cudaMemcpyHostToDevice, stream),
+                   "upload fallback cells");
+      if (st == BB200_OK) {
+        launch_batch_cluster_compact(cl_.table.get(), cl_.cells.get(), cl_.records.get(), n_flagged, cl_records_host_.get(), stream);
+        ++launches_;
+        st = check(cudaGetLastError(), "batch_cluster_compact");
+      }
+      if (st == BB200_OK) st = check(cudaStreamSynchronize(stream), "batch cluster fallback");
+      if (st != BB200_OK) return rollback(st);
+      const HostCell* cells = reinterpret_cast<const HostCell*>(cl_records_host_.get());
+      for (size_t f = 0; f < flagged.size(); ++f) {
+        const uint32_t count = res[flagged[f]].cells;
+        host_sel[f] = select_cluster(cells, count, outcome[flagged[f]].n, cp->linear_hash_resolution, cp->angular_hash_resolution,
+                                     cp->weight_cap_percentile);
+        cells += count;
+      }
+    }
+    size_t f = 0;
+    for (uint32_t j = 0; j < n_active; ++j) {
+      const uint32_t k = active[j];
+      const double* moments = res[j].moments;
+      uint32_t clusters = res[j].clusters;
+      if (f < flagged.size() && flagged[f] == j) {
+        moments = host_sel[f].moments;
+        clusters = host_sel[f].clusters;
+        ++f;
+      }
+      if (clustered->estimates != nullptr) estimate_from_moments(moments, outcome[j].pivot, &clustered->estimates[k]);
+      if (clustered->n_cells != nullptr) clustered->n_cells[k] = res[j].cells;
+      if (clustered->n_clusters != nullptr) clustered->n_clusters[k] = clusters;
+    }
+  }
+
+  for (uint32_t j = 0; j < n_active; ++j) {
+    const uint32_t k = active[j];
+    Member& m = members_[k];
+    const Outcome& o = outcome[j];
+    if (o.r.resampled) {
+      m.ancestors_n = o.n;
+    } else {
+      m.cdf_total = summary_host_.get()[j].total;  // the step's scan, over the weights before normalisation
+    }
+    m.cur = o.cur;
+    m.n = o.n;
+    m.pivot[0] = o.pivot[0];
+    m.pivot[1] = o.pivot[1];
+    out[k] = o.r;
+    m.policy.commit_update(o.r.resampled, plans[k].random_state_probability);
   }
   return BB200_OK;
 }

@@ -83,8 +83,22 @@ class Batch {
   /// (bb200_amcl_batch_update_measurements): every present member's measurement is checked first, and scans and clouds
   /// are converted on the device by one more launch.
   int update_measurements(const double* control_poses, const bb200_measurement* measurements, const uint8_t* present, bb200_update_result* out);
+  /// update_measurements, then the cluster estimate of every member that updated, byte-identical to cluster_estimates
+  /// over those members right after it (bb200_amcl_batch_update_clustered): three more launches after the step
+  /// (batch_cluster_table, batch_cluster_cells, batch_cluster_select) and the step's one synchronisation, plus one launch
+  /// and one synchronisation when some member falls back to the host pass.  clustered[m], n_cells[m] and n_clusters[m]
+  /// (either may be nullptr) are written for the members with out[m].updated.
+  int update_clustered(const double* control_poses, const bb200_measurement* measurements, const uint8_t* present, const bb200_cluster_param& p,
+                       bb200_update_result* out, bb200_estimate* clustered, uint32_t* n_cells, uint32_t* n_clusters);
 
  private:
+  /// Where update_clustered's step writes the cluster estimates.
+  struct ClusteredOut {
+    const bb200_cluster_param* p;
+    bb200_estimate* estimates;
+    uint32_t* n_cells;
+    uint32_t* n_clusters;
+  };
   struct Member {
     AmclPolicy policy;
     uint64_t offset{0};    // first particle in the batch buffers
@@ -126,7 +140,9 @@ class Batch {
   int ensure_inputs(uint64_t floats);
   int ensure_scan_table(Member& m, const bb200_laser_scan& scan);
   /// The step of update and update_measurements: in[m] is member m's measurement, already checked when it is a scan or a cloud.
-  int step(const double* control_poses, const bb200_measurement* in, const uint8_t* present, bb200_update_result* out);
+  /// With `clustered`, the step also selects every updated member's cluster estimate on the device (update_clustered).
+  int step(const double* control_poses, const bb200_measurement* in, const uint8_t* present, bb200_update_result* out,
+           const ClusteredOut* clustered = nullptr);
   bool ensure_hits(uint64_t words);
   int set_map(const MapTables& tables);
   int add_map(const MapTables& tables, int* id);
@@ -135,6 +151,8 @@ class Batch {
   /// The cluster scratch, whose hashes and tables a KLD count reuses, and the step's KLD parameter table.
   int ensure_kld_scratch();
   int ensure_cluster_records(uint64_t cells);
+  /// The cluster scratch and the selection's: rehash schedules, per-member scratch, tables and results.
+  int ensure_select_scratch();
   /// The members whose present[m] is non-zero (present == nullptr: all of them), in member order; BB200_ERR_STATE when one
   /// of them has no particles.
   int select_members(const uint8_t* present, std::vector<uint32_t>* selected);
@@ -213,6 +231,18 @@ class Batch {
     PinnedBuffer<BatchKldMember> host;
   };
   KldTable kld_;
+  // The device selection of update_clustered (allocated on first use): the probed rehash schedules, one scratch slice per
+  // member (select_scratch_bytes of its max_particles, at offsets[k]), the post-step table inputs and the results.
+  struct SelectBuffers {
+    DeviceBuffer<uint32_t> schedule_start;
+    DeviceBuffer<RehashStep> schedule;
+    DeviceBuffer<unsigned char> scratch;
+    std::vector<uint64_t> offsets;
+    DeviceBuffer<BatchClusterPost> post;
+    PinnedBuffer<BatchClusterPost> post_host;
+    PinnedBuffer<BatchClusterResult> results;
+  };
+  SelectBuffers sel_;
 
   // Pose-sample scratch (allocated on first use): the member table, and the draws after a header of one CDF total per
   // member (sample_header_ poses' worth), so that one copy brings both back.

@@ -905,6 +905,12 @@ int bb200_amcl_batch_update_measurements(bb200_amcl_batch* b, const double* cont
   BB_REQUIRE(b && control_poses && measurements && out);
   return guarded(b->impl, [&] { return b->impl.update_measurements(control_poses, measurements, present, out); });
 }
+int bb200_amcl_batch_update_clustered(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements,
+                                      const uint8_t* present, const bb200_cluster_param* p, bb200_update_result* out, bb200_estimate* clustered,
+                                      uint32_t* n_cells, uint32_t* n_clusters) {
+  BB_REQUIRE(b && control_poses && measurements && p && out && clustered);
+  return guarded(b->impl, [&] { return b->impl.update_clustered(control_poses, measurements, present, *p, out, clustered, n_cells, n_clusters); });
+}
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.launch_count() : 0; }
 
 int bb200_amcl_plan_update(bb200_amcl* a, const double control_pose[4], bb200_step_plan* plan) {

@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "cluster_host.hpp"
+#include "cluster_select.cuh"
 #include "device_buffer.hpp"
 #include "kernels.cuh"
 
@@ -104,6 +105,53 @@ void launch_batch_cluster_cells(const BatchClusterArgs& a, uint32_t n_members, c
 /// Member j's cells[j] records to out[cells[0] + ... + cells[j - 1]]: the records of all members back to back.  One launch.
 void launch_batch_cluster_compact(const BatchClusterMember* members, const uint32_t* cells, const CellRecord* records, uint32_t n_members,
                                   CellRecord* out, cudaStream_t stream);
+
+// ---- the cluster estimate of every member that a batch step updated, selected on the device -----------------------
+// After the step: batch_cluster_table_kernel turns the pre-step member table into the post-step one (state buffer, count
+// and pivot, from the step's summaries), batch_cluster_cells_kernel runs on it, and batch_cluster_select_kernel restates
+// select_cluster per member (cluster_select.cuh), one CTA each.
+
+static_assert(kBatchClusterMaxParticles == kSelectMaxCells, "the rehash schedules cover every count a batch member can reach");
+
+/// What the table kernel needs besides the pre-step BatchClusterMember: how the step may have changed the member.
+struct BatchClusterPost {
+  uint64_t scratch_offset;  // bytes: the member's selection scratch when it does not fit in shared memory
+  uint32_t capacity;        // max_particles: the count after a fixed-size resample
+  int mode;                 // 0: kept its particles, 1: resampled, 2: the step decides (StepSummary::resampled)
+  int kld;                  // 1: a resample keeps StepSummary::accepted particles
+  int pad;
+};
+
+/// One member's selection, written to pinned memory.  fallback: the device cannot promise the host's bits (a NaN cell
+/// weight, or a neighbour heading at an angular bucket edge); the host then runs select_cluster on the member's records.
+struct BatchClusterResult {
+  uint32_t found;
+  uint32_t clusters;
+  uint32_t cells;
+  uint32_t fallback;
+  double moments[kMomentCount];  // of the heaviest cluster, or of every cell
+};
+
+struct BatchSelectArgs {
+  BatchClusterMember* members;        // pre-step table in, post-step table out (table kernel); one per CTA
+  const BatchClusterPost* post;
+  const StepSummary* summary;         // the step's, one per member of its table (pinned)
+  uint32_t n_members;
+  const CellRecord* records;          // the member slices batch_cluster_cells_kernel wrote
+  const uint32_t* cells;              // their cell counts
+  const unsigned long long* keys;     // their bucket sets: key -> cell id
+  const uint32_t* ids;
+  const uint32_t* schedule_start;     // RehashTable::start, by n / 5
+  const RehashStep* schedule;         // RehashTable::steps
+  unsigned char* scratch;             // BatchClusterPost::scratch_offset
+  double linear, angular, percentile;
+  Pose2 adjacent[6];                  // ParticleClusterizer::adjacent_grid_cells_, rot_exp on the host
+  BatchClusterResult* results;        // one per member (pinned)
+};
+
+/// One launch each.
+void launch_batch_cluster_table(const BatchSelectArgs& a, cudaStream_t stream);
+void launch_batch_cluster_select(const BatchSelectArgs& a, cudaStream_t stream);
 
 /// The clusterizer of a filter: scratch for up to `capacity` particles on one device, allocated on first use,
 /// run over any particle set of that size in that device's memory.  Every call works on the current device, ordered on

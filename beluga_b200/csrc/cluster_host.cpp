@@ -3,6 +3,7 @@
 #include <algorithm>
 #include <cmath>
 #include <limits>
+#include <map>
 #include <queue>
 #include <unordered_map>
 
@@ -120,6 +121,51 @@ ClusterSelection select_cluster(const HostCell* cells, std::size_t n_cells, std:
       for (int j = 0; j < 9; ++j) out.moments[j] += cells[k].moments[j];
   }
   return out;
+}
+
+const RehashTable& rehash_table() {
+  static const RehashTable table = [] {
+    RehashTable t;
+    const uint32_t max_want = kSelectMaxCells / 5;
+    std::vector<std::size_t> reserved(max_want + 1);
+    std::map<std::size_t, uint32_t> top_want;  // largest want per bucket count after reserve
+    for (uint32_t w = 0; w <= max_want; ++w) {
+      std::unordered_map<std::size_t, double> map;
+      map.reserve(w);
+      reserved[w] = map.bucket_count();
+      top_want[reserved[w]] = w;
+    }
+    std::map<std::size_t, uint32_t> first;  // schedule start per bucket count after reserve
+    for (const auto& [buckets, w] : top_want) {
+      first[buckets] = static_cast<uint32_t>(t.steps.size());
+      std::unordered_map<std::size_t, double> map;
+      map.reserve(w);
+      t.steps.push_back(RehashStep{0, static_cast<uint32_t>(map.bucket_count())});
+      const uint32_t cells = static_cast<uint32_t>(std::min<uint64_t>(5ull * w + 4, kSelectMaxCells));
+      for (uint32_t k = 0; k < cells; ++k) {
+        const std::size_t before = map.bucket_count();
+        map.emplace(k, 0.0);
+        if (map.bucket_count() != before) t.steps.push_back(RehashStep{k, static_cast<uint32_t>(map.bucket_count())});
+      }
+      t.steps.push_back(RehashStep{kSelectNone, 0});
+    }
+    t.start.resize(max_want + 1);
+    for (uint32_t w = 0; w <= max_want; ++w) t.start[w] = first[reserved[w]];
+    return t;
+  }();
+  return table;
+}
+
+uint64_t select_scratch_bytes(uint64_t capacity) {
+  const RehashTable& t = rehash_table();
+  uint64_t bytes = 0;
+  for (uint64_t w = 0; w <= capacity / 5; ++w) {
+    const uint32_t cells = static_cast<uint32_t>(std::min<uint64_t>(capacity, 5 * w + 4));
+    uint32_t max_buckets = 0;
+    const int phases = rehash_phases(t.steps.data() + t.start[w], cells, &max_buckets);
+    bytes = std::max(bytes, select_layout(cells, phases, max_buckets).bytes);
+  }
+  return bytes;
 }
 
 void estimate_from_moments(const double m[9], const double pivot[2], bb200_estimate* out) {

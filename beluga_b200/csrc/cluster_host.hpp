@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "../../include/beluga_b200.h"
+#include "cluster_select.cuh"
 
 namespace bb200 {
 
@@ -35,6 +36,18 @@ struct ClusterSelection {
 /// n_particles sizes the map's initial reserve like make_cluster_map (:146).
 ClusterSelection select_cluster(const HostCell* cells, std::size_t n_cells, std::uint64_t n_particles, double linear_resolution,
                                 double angular_resolution, double weight_cap_percentile);
+
+/// The bucket counts select_cluster's map passes through, probed from this process's libstdc++: for every
+/// want = n_particles / 5 with n_particles <= kSelectMaxCells, start[want] is the first entry of the schedule (RehashStep,
+/// cluster_select.cuh) of a map after reserve(want), which covers up to min(5 want + 4, kSelectMaxCells) insertions.
+/// Wants whose reserve gives the same bucket count share one schedule.
+struct RehashTable {
+  std::vector<uint32_t> start;
+  std::vector<RehashStep> steps;
+};
+const RehashTable& rehash_table();
+/// Bytes of scratch a member of at most `capacity` particles needs for its selection (select_layout at its largest).
+uint64_t select_scratch_bytes(uint64_t capacity);
 
 /// Mean and covariance (estimation.hpp:436-475) from the nine raw moments about `pivot` (layout of kMomentCount in
 /// kernels.cuh): what every estimate ends with, of the whole set or of the selected cluster.

@@ -695,6 +695,21 @@ typedef struct bb200_measurement {
  * Atomicity: as bb200_amcl_batch_update -- on failure every member's host state is as if the call had not been made. */
 int bb200_amcl_batch_update_measurements(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements,
                                          const uint8_t* present, bb200_update_result* out);
+/* bb200_amcl_batch_update_measurements, then beluga::cluster_based_estimate (cluster_based_estimation.hpp:415-432) of
+ * every member that updated: what beluga_ros::Amcl::update returns (beluga_ros/src/amcl.cpp:125), for the whole batch in
+ * one call.  out[m] is exactly what bb200_amcl_batch_update_measurements writes.  clustered[m], n_cells[m] and
+ * n_clusters[m] (n_cells and n_clusters may be NULL) are written for the members with out[m].updated, and they are
+ * byte-identical to bb200_amcl_batch_cluster_estimates(b, p, mask of updated members, ...) called right after the update.
+ *
+ * The per-cell flood of the estimate runs on the device, one CTA per member: the call takes the update's launches plus 3
+ * and one host synchronisation, whatever K and the cell counts are.  A member for which the device cannot promise the
+ * host's result -- a NaN cell weight, or a neighbour heading within a few ulps of an angular bucket edge -- gets the host
+ * pass instead; a call in which that happens takes 1 launch and 1 synchronisation more.  The cluster parameters are
+ * checked as bb200_amcl_batch_cluster_estimates checks them, before anything reaches the device (BB200_ERR_INVALID_ARGUMENT),
+ * and the call is atomic as bb200_amcl_batch_update_measurements is. */
+int bb200_amcl_batch_update_clustered(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements,
+                                      const uint8_t* present, const bb200_cluster_param* p, bb200_update_result* out,
+                                      bb200_estimate* clustered, uint32_t* n_cells, uint32_t* n_clusters);
 /* Kernel launches issued by this batch so far (steps, initialisations, cluster estimates, particle-cloud histograms and
  * pose samples, and the beam model's map uploads). */
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b);

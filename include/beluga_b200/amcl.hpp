@@ -358,6 +358,58 @@ class AmclBatch {
       -> std::vector<std::optional<estimation_type>> {
     return update(controls, std::vector<Measurement>(clouds.begin(), clouds.end()), present);
   }
+  /// update, then beluga::cluster_based_estimate of every member that updated, in one call
+  /// (bb200_amcl_batch_update_clustered): per member what beluga_ros::Amcl::update returns, the cluster-based estimate,
+  /// or std::nullopt when the member did not update.  The per-cell flood runs on the device.
+  auto update_clustered(const std::vector<SE2d>& controls, const std::vector<Measurement>& measurements, const std::vector<bool>* present = nullptr,
+                        ParticleClusterizerParam parameters = {}) -> std::vector<std::optional<estimation_type>> {
+    const std::size_t k = size();
+    if (controls.size() != k || measurements.size() != k || (present != nullptr && present->size() != k))
+      throw Error(BB200_ERR_INVALID_ARGUMENT, "one control, one measurement (and one presence flag) per member");
+    std::vector<bb200_laser_scan> scans(k);
+    std::vector<bb200_point_cloud> clouds(k);
+    std::vector<bb200_measurement> in(k);
+    const std::vector<std::uint8_t> mask = presence_mask(present);
+    for (std::size_t m = 0; m < k; ++m) {
+      const auto& v = measurements[m].value;
+      if (const auto* points = std::get_if<0>(&v)) {
+        in[m] = bb200_measurement{BB200_MEASUREMENT_POINTS, points->empty() ? nullptr : &points->front().first, points->size(), nullptr, nullptr};
+      } else if (const auto* scan = std::get_if<LaserScanView>(&v)) {
+        scans[m] = scan->c_view();
+        in[m] = bb200_measurement{BB200_MEASUREMENT_SCAN, nullptr, 0, &scans[m], nullptr};
+      } else {
+        clouds[m] = std::get<PointCloudView>(v).c_view();
+        in[m] = bb200_measurement{BB200_MEASUREMENT_CLOUD, nullptr, 0, nullptr, &clouds[m]};
+      }
+    }
+    const bb200_cluster_param p{parameters.linear_hash_resolution, parameters.angular_hash_resolution, parameters.weight_cap_percentile};
+    std::vector<bb200_update_result> r(k);
+    std::vector<bb200_estimate> e(k);
+    check(bb200_amcl_batch_update_clustered(handle_, controls.front().data(), in.data(), present != nullptr ? mask.data() : nullptr, &p, r.data(),
+                                            e.data(), nullptr, nullptr));
+    std::vector<std::optional<estimation_type>> out(k);
+    for (std::size_t m = 0; m < k; ++m) {
+      if (!r[m].updated) continue;
+      Matrix3d cov;
+      for (int i = 0; i < 9; ++i) cov[i] = e[m].cov[i];
+      out[m] = std::make_pair(SE2d::from_data(e[m].mean), cov);
+    }
+    return out;
+  }
+  /// update_clustered with base-frame points for every member.
+  auto update_clustered(const std::vector<SE2d>& controls, const std::vector<std::vector<std::pair<double, double>>>& points,
+                        const std::vector<bool>* present = nullptr, ParticleClusterizerParam parameters = {})
+      -> std::vector<std::optional<estimation_type>> {
+    std::vector<Measurement> views;
+    views.reserve(points.size());
+    for (const auto& p : points) views.emplace_back(p);
+    return update_clustered(controls, views, present, parameters);
+  }
+  /// update_clustered with a laser scan for every member.
+  auto update_clustered(const std::vector<SE2d>& controls, const std::vector<LaserScanView>& scans, const std::vector<bool>* present = nullptr,
+                        ParticleClusterizerParam parameters = {}) -> std::vector<std::optional<estimation_type>> {
+    return update_clustered(controls, std::vector<Measurement>(scans.begin(), scans.end()), present, parameters);
+  }
 #ifdef BELUGA_B200_WITH_SOPHUS
   /// The same for any beluga::BaseSparsePointCloud-shaped clouds, e.g. beluga_ros::SparsePointCloud3f.
   template <class SparsePointCloud, std::enable_if_t<is_sparse_point_cloud_v<SparsePointCloud>, int> = 0>

@@ -474,6 +474,58 @@ def run_batch_cluster():
     return res
 
 
+def run_batch_clustered():
+    """One beluga_ros node cycle for every member, two ways, on the `batch_cluster` shapes (K in {1, 16, 64, 256} members x
+    2000 particles x 100 points on the 2000^2 map, and K = 1 x 32 768): update_clustered (the update and every updated
+    member's cluster-based estimate in one call, the per-cell flood on the device) against update_measurements followed by
+    cluster_estimates (the flood on the host, member after member).  Two batches built alike take the same inputs; the two
+    forms alternate which goes first from round to round, and their results and estimates are compared byte for byte."""
+    res = {}
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=100, steps=100)
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    steps, warmup = 20, 3
+    device = device_record()
+    for k, n in ((1, 2000), (16, 2000), (64, 2000), (256, 2000), (1, 32768)):
+        params = [bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m) for m in range(k)]
+        batches = {}
+        for form in ("clustered", "separate"):
+            batch = bb.AmclBatch([bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)], params)
+            batch.set_likelihood_field_map(lfm, grid)
+            for m in range(k):
+                batch.initialize(m, sc.initial_mean, sc.initial_cov)
+            batches[form] = batch
+        times = {"clustered": [], "separate": []}
+        launches = {"clustered": [], "separate": []}
+        for t in range(warmup + steps):
+            pose = bb.se2(*sc.poses[t])
+            out = {}
+            for form in (("clustered", "separate") if t % 2 == 0 else ("separate", "clustered")):
+                batch = batches[form]
+                before = batch.launch_count()
+                t0 = time.perf_counter()
+                if form == "clustered":
+                    out[form] = batch.update_clustered([pose] * k, [sc.scans[t]] * k)
+                else:
+                    r = batch.update_measurements([pose] * k, [sc.scans[t]] * k)
+                    out[form] = (r, batch.cluster_estimates(present=[bool(x.updated) for x in r]))
+                t1 = time.perf_counter()
+                launches[form].append(batch.launch_count() - before)
+                if t >= warmup:
+                    times[form].append((t1 - t0) * 1e3)
+            for a, b in zip(out["clustered"][1], out["separate"][1]):
+                assert a[0].tobytes() == b[0].tobytes() and a[1].tobytes() == b[1].tobytes()
+        row = {"members": k, "particles": n, "points": 100, "steps": steps, "device": device, "kernels_ms": {},
+               "ms_per_step_e2e": float(np.median(times["clustered"]))}
+        for form in times:
+            row[f"{form}_round_ms_median"] = float(np.median(times[form]))
+            row[f"{form}_round_ms_range"] = [float(np.min(times[form])), float(np.max(times[form]))]
+            row[f"{form}_launches_per_round"] = int(max(launches[form]))
+        row["speedup_median"] = row["separate_round_ms_median"] / row["clustered_round_ms_median"]
+        res[f"batch_clustered_{k}_x_{n}_x_100_lfm_2000"] = row
+    return res
+
+
 def run_batch_cloud():
     """The `batch` workload (K in {1, 16, 64, 256} members x 2000 particles x 100 points, 2000^2 map, systematic resampling)
     and K standalone Amcl fed the same inputs, timed as one particle-cloud publish round after each update: the batched form
@@ -700,6 +752,8 @@ def main():
         out.update(run_batch_selective())
     if "batch_cluster" in which:
         out.update(run_batch_cluster())
+    if "batch_clustered" in which:
+        out.update(run_batch_clustered())
     if "batch_cloud" in which:
         out.update(run_batch_cloud())
     if "batch_beam" in which:

@@ -776,7 +776,11 @@ class AmclBatch:
     likelihood field or a beam-model map, one for every member (set_*_map) or several (add_*_map and update_map, which
     moves a member to another map as a node's Amcl::update_map does); update() steps every member with a new scan with a fixed
     number of kernel launches and one synchronisation.  Member m's results and particles equal those of a standalone Amcl
-    built from params[m] and motions[m] and fed the same inputs."""
+    built from params[m] and motions[m] and fed the same inputs.
+
+    Member indices are slots: add_member and remove_member let robots join and leave the running batch without
+    disturbing the others.  len() counts the slots, occupied and vacant, and every per-member list keeps that length;
+    `params[m]` is None for a vacant slot, whose entries of those lists are not read."""
 
     def __init__(self, motions, params, adaptive: bool = False, selective: bool = False):
         """`motions[m]`, `params[m]`: member m's motion model and AmclParams (max_particles <= 32768, and
@@ -817,11 +821,39 @@ class AmclBatch:
         if st != _capi.OK:
             raise BelugaB200Error(st, self._lib.bb200_amcl_batch_last_error(self._h).decode())
 
+    def add_member(self, motion, params) -> int:
+        """Adds a member configured by `motion` and `params` (AmclParams), validated as the constructor validates one under
+        this batch's flags; it takes the lowest vacant slot or appends one, and starts with no map and no particles, as a
+        member of a freshly created batch.  Returns its slot.  The other members keep their particles, policies and maps."""
+        p, m = params.c(), motion.c_motion()
+        i = C.c_int(-1)
+        self._check(self._lib.bb200_amcl_batch_add_member(self._h, C.byref(p), C.byref(m), C.byref(i)))
+        if i.value == len(self.params):
+            self.params.append(None)
+        self.params[i.value] = params
+        return i.value
+
+    def remove_member(self, member: int):
+        """Makes slot `member` vacant and frees its share of the device buffers; the last member cannot be removed."""
+        self._check(self._lib.bb200_amcl_batch_remove_member(self._h, member))
+        self.params[member] = None
+
+    def member_active(self, member: int) -> bool:
+        """Whether slot `member` holds a member."""
+        a = C.c_int(0)
+        self._check(self._lib.bb200_amcl_batch_member_active(self._h, member, C.byref(a)))
+        return bool(a.value)
+
+    def _skipped(self, present, m) -> bool:
+        # not selected: absent from `present`, or a vacant slot when present is None
+        return not present[m] if present is not None else self.params[m] is None
+
     def set_likelihood_field_map(self, params: LikelihoodFieldModelParam, grid: OccupancyGrid, prob: bool = False):
         """One likelihood field for every member: removes every map, adds this one and assigns every member to it."""
         p, g = params.c(), grid.c()
         self._check(self._lib.bb200_amcl_batch_set_likelihood_field_map(self._h, C.byref(p), C.byref(g), int(prob)))
-        self._field_shapes = {self.member_map(0): grid.cells.shape}
+        occupied = next(m for m, q in enumerate(self.params) if q is not None)
+        self._field_shapes = {self.member_map(occupied): grid.cells.shape}
 
     def set_beam_map(self, params: BeamModelParam, grid: OccupancyGrid):
         """The beam model (BeamSensorModel) on `grid` for every member; replaces the map set before, of either model."""
@@ -888,7 +920,8 @@ class AmclBatch:
 
     def _rows(self, member: int) -> int:
         # a fixed batch keeps its max_particles-row buffers; an adaptive one returns the member's current count
-        return self.member_size(member) if self.adaptive else self.params[member].max_particles
+        # (a vacant slot asks the library, which refuses it)
+        return self.member_size(member) if self.adaptive or self.params[member] is None else self.params[member].max_particles
 
     def particles(self, member: int):
         n = self._rows(member)
@@ -923,7 +956,7 @@ class AmclBatch:
         self._check(self._lib.bb200_amcl_batch_cluster_estimates(self._h, C.byref(p), mask, est, cells, clusters))
         out = []
         for m in range(k):
-            if present is not None and not present[m]:
+            if self._skipped(present, m):
                 out.append(None)
                 continue
             e = (np.array(est[m].mean), np.array(est[m].cov).reshape(3, 3))
@@ -943,12 +976,12 @@ class AmclBatch:
         mask = self._mask(present)
         k = len(self.params)
         # A member has at most as many bins as particles: buffers of max_particles bins take every histogram in one pass.
-        bufs = [np.empty(q.max_particles, dtype=_CELL_DTYPE) for q in self.params]
+        bufs = [np.empty(0 if q is None else q.max_particles, dtype=_CELL_DTYPE) for q in self.params]
         bins = (C.POINTER(_capi.ClusterCell) * k)(*[b.ctypes.data_as(C.POINTER(_capi.ClusterCell)) for b in bufs])
         capacity = (C.c_uint64 * k)(*[len(b) for b in bufs])
         n_bins, top = (C.c_uint64 * k)(), (C.c_double * k)()
         self._check(self._lib.bb200_amcl_batch_particle_histograms(self._h, linear, angular, mask, bins, capacity, n_bins, top))
-        return [None if present is not None and not present[m] else (bufs[m][:n_bins[m]].copy(), top[m]) for m in range(k)]
+        return [None if self._skipped(present, m) else (bufs[m][:n_bins[m]].copy(), top[m]) for m in range(k)]
 
     def sample_states(self, count, step: int = 0xFFFFFFFF, present=None):
         """Filter.sample_states(count, step) of every member whose `present` entry is true (None: all), in one call ->
@@ -964,14 +997,14 @@ class AmclBatch:
         outs = [np.zeros((c, 4)) for c in counts]
         ptrs = (C.POINTER(C.c_double) * k)(*[_dptr(o) if len(o) else None for o in outs])
         self._check(self._lib.bb200_amcl_batch_sample_states(self._h, (C.c_uint64 * k)(*counts), step, mask, ptrs))
-        return [None if present is not None and not present[m] else outs[m] for m in range(k)]
+        return [None if self._skipped(present, m) else outs[m] for m in range(k)]
 
     def update(self, control_poses, points, present=None) -> list:
         """Amcl::update for every member whose `present` entry is true (None: all).  `control_poses`: K poses [c, s, x, y];
         `points[m]`: member m's (x, y) points.  Returns K UpdateResult blocks; `.updated == 0` for absent members."""
         k = len(self.params)
         poses = _f64(control_poses).reshape(k, 4)
-        pts = [_f64(p).reshape(-1, 2) for p in points]
+        pts = [_f64(() if p is None else p).reshape(-1, 2) for p in points]
         ptrs = (C.POINTER(C.c_double) * k)(*[_dptr(p) if len(p) else None for p in pts])
         counts = (C.c_uint64 * k)(*[len(p) for p in pts])
         mask = None if present is None else (C.c_uint8 * k)(*[1 if x else 0 for x in present])
@@ -988,7 +1021,7 @@ class AmclBatch:
             raise ValueError("one measurement per member")
         mask = self._mask(present)
         poses = _f64(control_poses).reshape(k, 4)
-        built = [_measurement(m) for m in measurements]
+        built = [_measurement(() if m is None else m) for m in measurements]
         table = (_capi.Measurement * k)(*[b[0] for b in built])
         res = (_capi.UpdateResult * k)()
         self._check(self._lib.bb200_amcl_batch_update_measurements(self._h, _dptr(poses), table, mask, res))
@@ -1006,7 +1039,7 @@ class AmclBatch:
             raise ValueError("one measurement per member")
         mask = self._mask(present)
         poses = _f64(control_poses).reshape(k, 4)
-        built = [_measurement(m) for m in measurements]
+        built = [_measurement(() if m is None else m) for m in measurements]
         table = (_capi.Measurement * k)(*[b[0] for b in built])
         p = _capi.ClusterParam(linear, angular, percentile)
         res = (_capi.UpdateResult * k)()

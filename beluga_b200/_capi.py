@@ -243,6 +243,9 @@ SIGNATURES = {
     "bb200_amcl_batch_update_clustered": (C.c_int, [_vp, _dbl, _P(Measurement), _P(C.c_uint8), _P(ClusterParam), _P(UpdateResult), _P(Estimate),
                                                     _P(C.c_uint32), _P(C.c_uint32)]),
     "bb200_amcl_batch_launch_count": (C.c_uint64, [_vp]),
+    "bb200_amcl_batch_add_member": (C.c_int, [_vp, _P(AmclParam), _P(MotionParam), _P(C.c_int)]),
+    "bb200_amcl_batch_remove_member": (C.c_int, [_vp, C.c_int]),
+    "bb200_amcl_batch_member_active": (C.c_int, [_vp, C.c_int, _P(C.c_int)]),
     "bb200_amcl_plan_update": (C.c_int, [_vp, _dbl, _P(StepPlan)]),
     "bb200_amcl_commit_update": (None, [_vp, C.c_int, C.c_double]),
     "bb200_amcl_create_with_motion": (C.c_int, [_P(AmclParam), _P(MotionParam), _P(_vp)]),

@@ -20,79 +20,266 @@ uint64_t finish_rows(uint64_t capacity) {
 
 }  // namespace
 
+int Batch::validate_member(const bb200_amcl_param& p, const bb200_motion_param& motion, int k, int device, uint32_t flags, std::string* error) {
+  auto reject = [&](const std::string& m) {
+    if (error != nullptr) *error = m;
+    return static_cast<int>(BB200_ERR_INVALID_ARGUMENT);
+  };
+  const bool adaptive = (flags & BB200_BATCH_ADAPTIVE) != 0, selective = (flags & BB200_BATCH_SELECTIVE) != 0;
+  const std::string who = "member " + std::to_string(k) + ": ";
+  if (p.device != device) return reject(who + "all members of a batch share one device");
+  if (p.max_particles == 0 || p.max_particles > kBatchMaxParticles) return reject(who + "max_particles must lie in [1, 32768]");
+  if (!adaptive && p.min_particles != p.max_particles)
+    return reject(who + "a batch member keeps a fixed particle count (min_particles == max_particles)");
+  if (p.min_particles > p.max_particles) return reject(who + "need 0 < min_particles <= max_particles");  // bb200_amcl_create's check
+  if (p.selective_resampling && !selective) return reject(who + "selective resampling is not supported in a batch");
+  if (p.shard_first_index != 0 || p.shard_capacity != 0) return reject(who + "a batch member is not sharded");
+  if (!(p.alpha_slow >= 0.0) || !(p.alpha_slow <= p.alpha_fast)) return reject(who + "need 0 <= alpha_slow <= alpha_fast");
+  if (motion.model < BB200_MOTION_DIFFERENTIAL || motion.model > BB200_MOTION_STATIONARY) return reject(who + "unknown motion model");
+  return BB200_OK;
+}
+
 int Batch::validate(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, uint32_t flags, std::string* error) {
   auto reject = [&](const std::string& m) {
     if (error != nullptr) *error = m;
     return static_cast<int>(BB200_ERR_INVALID_ARGUMENT);
   };
   if ((flags & ~static_cast<uint32_t>(BB200_BATCH_ADAPTIVE | BB200_BATCH_SELECTIVE)) != 0) return reject("unknown batch flags");
-  const bool adaptive = (flags & BB200_BATCH_ADAPTIVE) != 0, selective = (flags & BB200_BATCH_SELECTIVE) != 0;
   if (params == nullptr || motions == nullptr) return reject("null argument");
   if (n_members < 1) return reject("a batch needs at least one member");
-  for (int k = 0; k < n_members; ++k) {
-    const bb200_amcl_param& p = params[k];
-    const std::string who = "member " + std::to_string(k) + ": ";
-    if (p.device != params[0].device) return reject(who + "all members of a batch share one device");
-    if (p.max_particles == 0 || p.max_particles > kBatchMaxParticles) return reject(who + "max_particles must lie in [1, 32768]");
-    if (!adaptive && p.min_particles != p.max_particles)
-      return reject(who + "a batch member keeps a fixed particle count (min_particles == max_particles)");
-    if (p.min_particles > p.max_particles) return reject(who + "need 0 < min_particles <= max_particles");  // bb200_amcl_create's check
-    if (p.selective_resampling && !selective) return reject(who + "selective resampling is not supported in a batch");
-    if (p.shard_first_index != 0 || p.shard_capacity != 0) return reject(who + "a batch member is not sharded");
-    if (!(p.alpha_slow >= 0.0) || !(p.alpha_slow <= p.alpha_fast)) return reject(who + "need 0 <= alpha_slow <= alpha_fast");
-    if (motions[k].model < BB200_MOTION_DIFFERENTIAL || motions[k].model > BB200_MOTION_STATIONARY) return reject(who + "unknown motion model");
-  }
+  for (int k = 0; k < n_members; ++k)
+    if (const int st = validate_member(params[k], motions[k], k, params[0].device, flags, error)) return st;
   return BB200_OK;
+}
+
+Batch::Layout Batch::lay_out(const std::vector<const bb200_amcl_param*>& slots) {
+  Layout l;
+  l.offset.assign(slots.size(), 0);
+  l.table_offset.assign(slots.size(), 0);
+  l.table_slots.assign(slots.size(), 0);
+  for (size_t k = 0; k < slots.size(); ++k) {
+    if (slots[k] == nullptr) continue;
+    const uint64_t capacity = slots[k]->max_particles;
+    // The CDF build reads weights and writes the CDF 16 bytes at a time from the slice's start: slices begin on whole
+    // 256-byte lines.
+    l.total = (l.total + kSliceAlign - 1) / kSliceAlign * kSliceAlign;
+    l.offset[k] = l.total;
+    l.total += capacity;
+    l.table_offset[k] = l.table_total;
+    uint32_t table_slots = 2;
+    while (table_slots < 2 * capacity) table_slots <<= 1;
+    l.table_slots[k] = table_slots;
+    l.table_total += table_slots;
+    l.tiles += batch_scan_tiles(capacity);
+    l.rows += finish_rows(capacity);
+    l.record_ancestors = l.record_ancestors || slots[k]->record_ancestors != 0;
+  }
+  return l;
+}
+
+void Batch::place(const Layout& l) {
+  for (size_t k = 0; k < members_.size(); ++k) {
+    Member& m = members_[k];
+    if (!m.active) continue;
+    m.offset = l.offset[k];
+    m.table_offset = l.table_offset[k];
+    m.table_slots = l.table_slots[k];
+  }
+  total_ = l.total;
+  table_total_ = l.table_total;
+  record_ancestors_ = l.record_ancestors;
+}
+
+int Batch::allocate(const Layout& l, size_t slots, Storage* s) {
+  const size_t k1 = slots + 1;
+  BB_CHECK(s->states[0].allocate(l.total));
+  BB_CHECK(s->states[1].allocate(l.total));
+  BB_CHECK(s->weights.allocate(l.total));
+  BB_CHECK(s->cdf.allocate(l.total));
+  if (l.record_ancestors) BB_CHECK(s->ancestors.allocate(l.total));
+  BB_CHECK(s->scalars.allocate(slots));
+  BB_CHECK(s->tile_state.allocate(l.tiles));
+  BB_CHECK(s->partials.allocate(l.rows * kMomentCount));
+  BB_CHECK(s->table.allocate(slots));
+  BB_CHECK(s->table_host.allocate(slots));
+  BB_CHECK(s->first.allocate(kBatchRows * k1));
+  BB_CHECK(s->first_host.allocate(kBatchRows * k1));
+  BB_CHECK(s->summary_host.allocate(slots));
+  BB_CHECK(cudaMemsetAsync(s->scalars.get(), 0, slots * sizeof(Scalars), stream_));
+  return BB200_OK;
+}
+
+void Batch::adopt(Storage&& s) {
+  states_[0] = std::move(s.states[0]);
+  states_[1] = std::move(s.states[1]);
+  weights_ = std::move(s.weights);
+  cdf_ = std::move(s.cdf);
+  ancestors_ = std::move(s.ancestors);
+  scalars_ = std::move(s.scalars);
+  tile_state_ = std::move(s.tile_state);
+  partials_ = std::move(s.partials);
+  table_ = std::move(s.table);
+  table_host_ = std::move(s.table_host);
+  first_ = std::move(s.first);
+  first_host_ = std::move(s.first_host);
+  summary_host_ = std::move(s.summary_host);
 }
 
 Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, uint32_t flags) {
   create_status_ = validate(params, motions, n_members, flags, &error_);
   if (create_status_ != BB200_OK) return;
-  uint64_t tiles = 0, rows = 0;
+  flags_ = flags;
   members_.reserve(static_cast<size_t>(n_members));
+  std::vector<const bb200_amcl_param*> slots;
   for (int k = 0; k < n_members; ++k) {
     members_.push_back(Member{AmclPolicy(params[k], motions[k])});
-    Member& m = members_.back();
-    // The CDF build reads weights and writes the CDF 16 bytes at a time from the slice's start: slices begin on whole
-    // 256-byte lines.
-    total_ = (total_ + kSliceAlign - 1) / kSliceAlign * kSliceAlign;
-    m.offset = total_;
-    m.capacity = params[k].max_particles;
-    total_ += m.capacity;
-    m.table_offset = table_total_;
-    m.table_slots = 2;
-    while (m.table_slots < 2 * m.capacity) m.table_slots <<= 1;
-    table_total_ += m.table_slots;
-    tiles += batch_scan_tiles(m.capacity);
-    rows += finish_rows(m.capacity);
-    record_ancestors_ = record_ancestors_ || params[k].record_ancestors != 0;
+    members_.back().capacity = params[k].max_particles;
+    slots.push_back(&params[k]);
   }
+  const Layout layout = lay_out(slots);
+  place(layout);
   device_ = params[0].device;
   create_status_ = check_device(device_, &error_);
   if (create_status_ != BB200_OK) return;
-  const size_t k1 = static_cast<size_t>(n_members) + 1;
   BB_TRY(cudaSetDevice(device_));
   BB_TRY(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-  BB_TRY(states_[0].allocate(total_));
-  BB_TRY(states_[1].allocate(total_));
-  BB_TRY(weights_.allocate(total_));
-  BB_TRY(cdf_.allocate(total_));
-  if (record_ancestors_) BB_TRY(ancestors_.allocate(total_));
-  BB_TRY(scalars_.allocate(members_.size()));
-  BB_TRY(tile_state_.allocate(tiles));
-  BB_TRY(partials_.allocate(rows * kMomentCount));
-  BB_TRY(table_.allocate(members_.size()));
-  BB_TRY(table_host_.allocate(members_.size()));
-  BB_TRY(first_.allocate(kBatchRows * k1));
-  BB_TRY(first_host_.allocate(kBatchRows * k1));
-  BB_TRY(summary_host_.allocate(members_.size()));
+  Storage s;
+  create_status_ = allocate(layout, members_.size(), &s);
+  if (create_status_ != BB200_OK) return;
+  adopt(std::move(s));
   BB_TRY(ticket_host_.allocate(1));
   BB_TRY(members_done_.allocate(1));
   *ticket_host_.get() = 0;  // pinned allocations are recycled with their old contents
-  BB_TRY(cudaMemsetAsync(scalars_.get(), 0, members_.size() * sizeof(Scalars), stream_));
   BB_TRY(cudaMemsetAsync(members_done_.get(), 0, sizeof(unsigned int), stream_));
   BB_TRY(cudaStreamSynchronize(stream_));
   created_ = true;
+}
+
+int Batch::relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* layout) {
+  BB_CHECK(cudaSetDevice(device_));
+  *layout = lay_out(slots);
+  // Every allocation before anything moves: a failure frees the attempt and leaves the batch as it was.
+  Storage s;
+  if (const int st = allocate(*layout, slots.size(), &s)) return st;
+  std::vector<BatchRelayoutMember> moves;
+  uint32_t ctas = 0;
+  for (size_t k = 0; k < members_.size(); ++k) {
+    const Member& m = members_[k];
+    if (!m.active || slots[k] == nullptr) continue;
+    BatchRelayoutMember r{};
+    r.from = m.offset;
+    r.to = layout->offset[k];
+    r.n = m.n;
+    r.cdf_n = m.cdf_total != 0 ? m.n : 0;
+    r.ancestors_n = m.policy.params().record_ancestors && ancestors_.get() != nullptr ? m.ancestors_n : 0;
+    r.cur = m.cur;
+    const uint32_t c = batch_relayout_ctas(r);
+    if (c == 0) continue;
+    s.first_host.get()[moves.size()] = ctas;
+    ctas += c;
+    moves.push_back(r);
+  }
+  DeviceBuffer<BatchRelayoutMember> table;
+  if (!moves.empty()) {
+    BB_CHECK(table.allocate(moves.size()));
+    const uint32_t n = static_cast<uint32_t>(moves.size());
+    s.first_host.get()[n] = ctas;
+    // Pageable table: staged before the call returns; the pinned prefixes stay untouched until the synchronisation below.
+    BB_CHECK(cudaMemcpyAsync(table.get(), moves.data(), n * sizeof(BatchRelayoutMember), cudaMemcpyHostToDevice, stream_));
+    BB_CHECK(cudaMemcpyAsync(s.first.get(), s.first_host.get(), (n + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream_));
+    BatchRelayoutArgs a{};
+    a.members = table.get();
+    a.first = s.first.get();
+    a.n_members = n;
+    a.ctas = ctas;
+    a.states_from[0] = states_[0].get();
+    a.states_from[1] = states_[1].get();
+    a.weights_from = weights_.get();
+    a.cdf_from = cdf_.get();
+    a.ancestors_from = ancestors_.get();
+    a.states_to = s.states[0].get();
+    a.weights_to = s.weights.get();
+    a.cdf_to = s.cdf.get();
+    a.ancestors_to = s.ancestors.get();
+    launches_ += static_cast<uint64_t>(launch_batch_relayout(a, stream_));
+    BB_CHECK(cudaGetLastError());
+  }
+  BB_CHECK(cudaStreamSynchronize(stream_));  // the moves have landed; nothing in flight reads the old buffers
+
+  // Nothing can fail from here on.
+  adopt(std::move(s));
+  for (size_t k = 0; k < members_.size(); ++k)
+    if (members_[k].active && slots[k] != nullptr) members_[k].cur = 0;  // the kernel wrote every survivor's states to buffer 0
+  // Scratch allocated on first use and sized by the layout or the slot count: re-created, all or nothing, on next use.
+  cl_ = ClusterBuffers{};
+  kld_ = KldTable{};
+  sel_ = SelectBuffers{};
+  sm_table_ = SampleTable{};
+  sample_header_ = 0;
+  inputs_ = InputTable{};
+  return BB200_OK;
+}
+
+int Batch::add_member(const bb200_amcl_param& params, const bb200_motion_param& motion, int* member) {
+  error_.clear();
+  size_t slot = 0;
+  while (slot < members_.size() && members_[slot].active) ++slot;
+  if (const int st = validate_member(params, motion, static_cast<int>(slot), device_, flags_, &error_)) return st;
+  Member joiner{AmclPolicy(params, motion)};
+  joiner.capacity = params.max_particles;
+  members_.reserve(members_.size() + 1);  // the host allocations that could fail come before the device work
+  std::vector<const bb200_amcl_param*> slots(std::max(members_.size(), slot + 1), nullptr);
+  for (size_t k = 0; k < members_.size(); ++k)
+    if (members_[k].active) slots[k] = &members_[k].policy.params();
+  slots[slot] = &params;
+  Layout layout;
+  if (const int st = relayout(slots, &layout)) return st;
+  if (slot == members_.size()) {
+    members_.push_back(std::move(joiner));
+  } else {
+    members_[slot] = std::move(joiner);
+  }
+  place(layout);
+  *member = static_cast<int>(slot);
+  return BB200_OK;
+}
+
+int Batch::remove_member(int member) {
+  error_.clear();
+  if (const int st = member_ok(member)) return st;
+  const size_t slot = static_cast<size_t>(member);
+  std::vector<const bb200_amcl_param*> slots(members_.size(), nullptr);
+  size_t occupied = 0;
+  for (size_t k = 0; k < members_.size(); ++k) {
+    if (!members_[k].active || k == slot) continue;
+    slots[k] = &members_[k].policy.params();
+    ++occupied;
+  }
+  if (occupied == 0) return fail(BB200_ERR_STATE, "a batch keeps at least one member: member " + std::to_string(member) + " is the last");
+  Layout layout;
+  if (const int st = relayout(slots, &layout)) return st;
+  Member vacant{members_[slot].policy};  // its scan table's device buffer goes with the old member
+  vacant.active = false;
+  members_[slot] = std::move(vacant);
+  place(layout);
+  return BB200_OK;
+}
+
+int Batch::member_active(int member, int* active) const {
+  error_.clear();
+  if (member < 0 || member >= members()) {
+    error_ = "member index out of range";
+    return BB200_ERR_INVALID_ARGUMENT;
+  }
+  *active = members_[static_cast<size_t>(member)].active ? 1 : 0;
+  return BB200_OK;
+}
+
+int Batch::check_present(const uint8_t* present) {
+  if (present == nullptr) return BB200_OK;
+  for (size_t k = 0; k < members_.size(); ++k)
+    if (present[k] != 0 && !members_[k].active) return fail(BB200_ERR_INVALID_ARGUMENT, "member " + std::to_string(k) + " is a vacant slot");
+  return BB200_OK;
 }
 
 Batch::~Batch() {
@@ -104,6 +291,10 @@ Batch::~Batch() {
 int Batch::member_ok(int member) const {
   if (member < 0 || member >= members()) {
     error_ = "member index out of range";
+    return BB200_ERR_INVALID_ARGUMENT;
+  }
+  if (!members_[static_cast<size_t>(member)].active) {
+    error_ = "member " + std::to_string(member) + " is a vacant slot";
     return BB200_ERR_INVALID_ARGUMENT;
   }
   return BB200_OK;
@@ -157,7 +348,8 @@ int Batch::set_map(const MapTables& tables) {
   int id = -1;
   const int st = add_map(tables, &id);
   if (st != BB200_OK) return st;
-  for (Member& m : members_) m.map = id;
+  for (Member& m : members_)
+    if (m.active) m.map = id;
   return BB200_OK;
 }
 
@@ -195,7 +387,7 @@ int Batch::remove_map(int id) {
   error_.clear();
   if (find_map(id) == nullptr) return BB200_ERR_INVALID_ARGUMENT;
   for (size_t k = 0; k < members_.size(); ++k)
-    if (members_[k].map == id) return fail(BB200_ERR_STATE, "member " + std::to_string(k) + " reads map " + std::to_string(id));
+    if (members_[k].active && members_[k].map == id) return fail(BB200_ERR_STATE, "member " + std::to_string(k) + " reads map " + std::to_string(id));
   BB_CHECK(cudaSetDevice(device_));
   BB_CHECK(cudaStreamSynchronize(stream_));  // nothing in flight reads its tables
   maps_.erase(id);
@@ -380,7 +572,7 @@ int Batch::ensure_select_scratch() {
   uint64_t bytes = 0;
   for (size_t m = 0; m < k; ++m) {
     s.offsets[m] = bytes;
-    bytes += (select_scratch_bytes(members_[m].capacity) + 255) / 256 * 256;
+    if (members_[m].active) bytes += (select_scratch_bytes(members_[m].capacity) + 255) / 256 * 256;
   }
   BB_CHECK(s.schedule_start.allocate(table.start.size()));
   BB_CHECK(s.schedule.allocate(table.steps.size()));
@@ -425,8 +617,9 @@ int Batch::cluster_estimates(const bb200_cluster_param& p, const uint8_t* presen
 }
 
 int Batch::select_members(const uint8_t* present, std::vector<uint32_t>* selected) {
+  if (const int st = check_present(present)) return st;
   for (size_t k = 0; k < members_.size(); ++k) {
-    if (present != nullptr && present[k] == 0) continue;
+    if (!selected_member(present, k)) continue;
     if (members_[k].n == 0) return fail(BB200_ERR_STATE, "member " + std::to_string(k) + ": no particles");
     selected->push_back(static_cast<uint32_t>(k));
   }
@@ -539,8 +732,9 @@ int Batch::sample_states(const uint64_t* counts, uint32_t step, const uint8_t* p
   // Filter::sample_states's checks per member, all before anything reaches the device.
   std::vector<uint32_t> drawn;  // selected members with something to draw, in member order
   uint64_t draws = 0;
+  if (const int st = check_present(present)) return st;
   for (size_t k = 0; k < members_.size(); ++k) {
-    if (present != nullptr && present[k] == 0) continue;
+    if (!selected_member(present, k)) continue;
     const Member& m = members_[k];
     const std::string who = "member " + std::to_string(k) + ": ";
     if (m.n == 0) return fail(BB200_ERR_STATE, who + "no particles");
@@ -715,7 +909,8 @@ void pack_cloud(const bb200_point_cloud& c, float* out) {
 int Batch::update(const double* control_poses, const double* const* points_xy, const uint64_t* n_points, const uint8_t* present,
                   bb200_update_result* out) {
   std::vector<bb200_measurement> in(members_.size());
-  for (size_t k = 0; k < members_.size(); ++k) in[k] = bb200_measurement{BB200_MEASUREMENT_POINTS, points_xy[k], n_points[k], nullptr, nullptr};
+  for (size_t k = 0; k < members_.size(); ++k)
+    if (members_[k].active) in[k] = bb200_measurement{BB200_MEASUREMENT_POINTS, points_xy[k], n_points[k], nullptr, nullptr};
   return step(control_poses, in.data(), present, out);
 }
 
@@ -723,8 +918,9 @@ int Batch::update_measurements(const double* control_poses, const bb200_measurem
                                bb200_update_result* out) {
   error_.clear();
   for (size_t k = 0; k < members_.size(); ++k) out[k] = bb200_update_result{};
+  if (const int st = check_present(present)) return st;
   for (size_t k = 0; k < members_.size(); ++k) {
-    if (present != nullptr && present[k] == 0) continue;
+    if (!selected_member(present, k)) continue;
     const std::string why = measurement_error(measurements[k]);
     if (!why.empty()) return fail(BB200_ERR_INVALID_ARGUMENT, "member " + std::to_string(k) + ": " + why);
   }
@@ -738,8 +934,9 @@ int Batch::update_clustered(const double* control_poses, const bb200_measurement
   if (!(p.linear_hash_resolution > 0.0) || !(p.angular_hash_resolution > 0.0) || !(p.weight_cap_percentile >= 0.0) ||
       !(p.weight_cap_percentile < 1.0))
     return fail(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)");
+  if (const int st = check_present(present)) return st;
   for (size_t k = 0; k < members_.size(); ++k) {
-    if (present != nullptr && present[k] == 0) continue;
+    if (!selected_member(present, k)) continue;
     const std::string why = measurement_error(measurements[k]);
     if (!why.empty()) return fail(BB200_ERR_INVALID_ARGUMENT, "member " + std::to_string(k) + ": " + why);
   }
@@ -752,6 +949,7 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
   error_.clear();
   const size_t count = members_.size();
   for (size_t k = 0; k < count; ++k) out[k] = bb200_update_result{};
+  if (const int st = check_present(present)) return st;
   std::vector<AmclPolicy> before;
   before.reserve(count);
   for (const Member& m : members_) before.push_back(m.policy);
@@ -764,7 +962,7 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
   std::vector<bb200_step_plan> plans(count);
   std::vector<uint32_t> active;  // members that update in this step, in member order
   for (size_t k = 0; k < count; ++k) {
-    if (present != nullptr && present[k] == 0) continue;
+    if (!selected_member(present, k)) continue;
     members_[k].policy.plan_update(control_poses + 4 * k, members_[k].n, &plans[k]);
     if (plans[k].update) active.push_back(static_cast<uint32_t>(k));
   }

@@ -36,7 +36,17 @@ class Batch {
   int create_status() const { return create_status_; }
   const char* last_error() const { return error_.c_str(); }
   void record_error(const std::string& message) const { error_ = message; }  // the C-ABI exception guard
+  /// Slots, occupied and vacant: the length of every per-member array a call takes.
   int members() const { return static_cast<int>(members_.size()); }
+
+  /// A new member in the lowest vacant slot, or in a new slot after the last; *member receives the slot.  The member is
+  /// validated as create validates one under this batch's flags and device, and starts as a created member does: no map,
+  /// no particles.  Every other member keeps its particles, weights, CDF, ancestors, policies and map: their live data
+  /// moves to the new layout in one launch (none when no other member holds particles).
+  int add_member(const bb200_amcl_param& params, const bb200_motion_param& motion, int* member);
+  /// Makes slot `member` vacant and frees its share of the particle buffers (BB200_ERR_STATE for the last occupied slot).
+  int remove_member(int member);
+  int member_active(int member, int* active) const;
   uint64_t launch_count() const { return launches_; }  // including the map uploads' (the beam model's normaliser tables)
 
   /// One map for every member: removes every map, adds this one and assigns every member to it.
@@ -100,7 +110,8 @@ class Batch {
     uint32_t* n_clusters;
   };
   struct Member {
-    AmclPolicy policy;
+    AmclPolicy policy;     // in a vacant slot, its last occupant's (never read)
+    bool active{true};     // false: a vacant slot
     uint64_t offset{0};    // first particle in the batch buffers
     uint64_t capacity{0};  // max_particles
     uint64_t n{0};
@@ -129,6 +140,45 @@ class Batch {
     DeviceMap map;
     int slot{0};  // its entry in the device map table
   };
+  /// Where the occupied slots' data lie in the batch buffers, and the sizes of the buffers that hold it.
+  struct Layout {
+    std::vector<uint64_t> offset, table_offset;  // per slot (vacant: 0)
+    std::vector<uint32_t> table_slots;
+    uint64_t total{0}, table_total{0}, tiles{0}, rows{0};
+    bool record_ancestors{false};
+  };
+  /// The buffers a layout and the slot count size: the particle slices, the step's scan tiles, finish rows, per-member
+  /// scalars and tables.
+  struct Storage {
+    DeviceBuffer<Pose2> states[2];
+    DeviceBuffer<double> weights;
+    DeviceBuffer<unsigned long long> cdf;
+    DeviceBuffer<long long> ancestors;
+    DeviceBuffer<Scalars> scalars;
+    DeviceBuffer<unsigned long long> tile_state;
+    DeviceBuffer<double> partials;
+    DeviceBuffer<BatchMember> table;
+    PinnedBuffer<BatchMember> table_host;
+    DeviceBuffer<uint32_t> first;
+    PinnedBuffer<uint32_t> first_host;
+    PinnedBuffer<StepSummary> summary_host;
+  };
+  /// The layout of the slots' params (nullptr: vacant): particle slices 32-aligned in slot order, hash tables back to back,
+  /// and the tiles and rows of every occupied slot.  The one rule of the constructor and of every membership change.
+  static Layout lay_out(const std::vector<const bb200_amcl_param*>& slots);
+  /// The checks validate makes on member k (a member of a batch on `device` with `flags`).
+  static int validate_member(const bb200_amcl_param& p, const bb200_motion_param& motion, int k, int device, uint32_t flags, std::string* error);
+  int allocate(const Layout& layout, size_t slots, Storage* s);
+  void adopt(Storage&& s);
+  /// Assigns every occupied member its place in `layout`.
+  void place(const Layout& layout);
+  /// The device half of a membership change to `slots`: new buffers, every surviving member's live data moved into them
+  /// (batch_relayout_kernel), the old buffers freed and the scratch sized by the old layout dropped.  A survivor is a slot
+  /// occupied now and in `slots`.  On failure the batch is unchanged.
+  int relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* layout);
+  /// BB200_ERR_INVALID_ARGUMENT when present (nullptr: every occupied slot) selects a vacant slot.
+  int check_present(const uint8_t* present);
+  bool selected_member(const uint8_t* present, size_t k) const { return members_[k].active && (present == nullptr || present[k] != 0); }
   int fail(int status, const std::string& message) {
     error_ = message;
     return status;
@@ -161,7 +211,8 @@ class Batch {
   int cell_records(double linear, double angular, const std::vector<uint32_t>& selected);
   int ensure_samples(uint64_t draws);
 
-  std::vector<Member> members_;
+  std::vector<Member> members_;  // by slot
+  uint32_t flags_{0};
   int device_{0};
   cudaStream_t stream_{nullptr};
   std::map<int, MapEntry> maps_;  // by id

@@ -569,6 +569,24 @@ __global__ void __launch_bounds__(kPtThreads) batch_points_kernel(BatchPointsArg
   }
 }
 
+// ---- membership changes: the surviving members' live data, from the old layout to the new one ------------------
+
+constexpr int kRelayoutThreads = 256;
+
+__global__ void __launch_bounds__(kRelayoutThreads) batch_relayout_kernel(BatchRelayoutArgs s) {
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, 0, blockIdx.x, local, count);
+  const BatchRelayoutMember& m = s.members[k];
+  const uint64_t i = static_cast<uint64_t>(local) * kRelayoutThreads + threadIdx.x;
+  if (i < m.n) {
+    const Pose2* from = (m.cur != 0 ? s.states_from[1] : s.states_from[0]) + m.from;
+    s.states_to[m.to + i] = from[i];
+    s.weights_to[m.to + i] = s.weights_from[m.from + i];
+  }
+  if (i < m.cdf_n) s.cdf_to[m.to + i] = s.cdf_from[m.from + i];
+  if (i < m.ancestors_n) s.ancestors_to[m.to + i] = s.ancestors_from[m.from + i];
+}
+
 template <bool kTable>
 int launch_batch_step_from(const BatchStepArgs& s, cudaStream_t stream) {
   const uint32_t reset = std::max(s.n_members, s.ctas[kBatchScan]);
@@ -665,6 +683,16 @@ int launch_batch_sample(const BatchSampleArgs& s, cudaStream_t stream) {
   }
   batch_sample_kernel<<<s.ctas[kSampleDraw], kRsThreads, 0, stream>>>(s);
   return launches;
+}
+
+uint32_t batch_relayout_ctas(const BatchRelayoutMember& m) {
+  const uint64_t n = std::max({m.n, m.cdf_n, m.ancestors_n});
+  return static_cast<uint32_t>((n + kRelayoutThreads - 1) / kRelayoutThreads);
+}
+
+int launch_batch_relayout(const BatchRelayoutArgs& s, cudaStream_t stream) {
+  batch_relayout_kernel<<<s.ctas, kRelayoutThreads, 0, stream>>>(s);
+  return 1;
 }
 
 }  // namespace bb200

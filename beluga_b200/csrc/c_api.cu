@@ -912,6 +912,18 @@ int bb200_amcl_batch_update_clustered(bb200_amcl_batch* b, const double* control
   return guarded(b->impl, [&] { return b->impl.update_clustered(control_poses, measurements, present, *p, out, clustered, n_cells, n_clusters); });
 }
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.launch_count() : 0; }
+int bb200_amcl_batch_add_member(bb200_amcl_batch* b, const bb200_amcl_param* params, const bb200_motion_param* motion, int* member) {
+  BB_REQUIRE(b && params && motion && member);
+  return guarded(b->impl, [&] { return b->impl.add_member(*params, *motion, member); });
+}
+int bb200_amcl_batch_remove_member(bb200_amcl_batch* b, int member) {
+  BB_REQUIRE(b);
+  return guarded(b->impl, [&] { return b->impl.remove_member(member); });
+}
+int bb200_amcl_batch_member_active(const bb200_amcl_batch* b, int member, int* active) {
+  BB_REQUIRE(b && active);
+  return guarded(b->impl, [&] { return b->impl.member_active(member, active); });
+}
 
 int bb200_amcl_plan_update(bb200_amcl* a, const double control_pose[4], bb200_step_plan* plan) {
   BB_REQUIRE(a && control_pose && plan);

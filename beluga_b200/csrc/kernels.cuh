@@ -615,6 +615,35 @@ int launch_batch_sample(const BatchSampleArgs& args, cudaStream_t stream);
 /// CTAs of a member in each row of a sample call's ranges (rebuilt: whether its CDF is rebuilt in the call).
 void batch_sample_ctas(const BatchSampleMember& m, bool rebuilt, uint32_t out[kSampleLaunches]);
 
+// ---- batches: members that join and leave ------------------------------------------------------------------
+/// One surviving member of a membership change: the live part of its slice, moved from the old buffers to the new ones.
+struct BatchRelayoutMember {
+  uint64_t from;         // first particle of its slice in the old buffers
+  uint64_t to;           // ... in the new buffers
+  uint64_t n;            // states and weights
+  uint64_t cdf_n;        // CDF entries: n while its CDF is current, 0 otherwise
+  uint64_t ancestors_n;  // ancestors (0 when the member does not record them)
+  int cur;               // old state buffer holding its particles; the new buffer is always states_to
+};
+struct BatchRelayoutArgs {
+  const BatchRelayoutMember* members;  // device
+  const uint32_t* first;               // device: n_members + 1 CTA prefixes
+  uint32_t n_members;
+  uint32_t ctas;
+  const Pose2* states_from[2];
+  const double* weights_from;
+  const unsigned long long* cdf_from;
+  const long long* ancestors_from;     // null when the old buffers record no ancestors
+  Pose2* states_to;
+  double* weights_to;
+  unsigned long long* cdf_to;
+  long long* ancestors_to;             // null when the new buffers record no ancestors
+};
+/// CTAs of a member in batch_relayout_kernel: one thread per particle of max(n, cdf_n, ancestors_n).
+uint32_t batch_relayout_ctas(const BatchRelayoutMember& m);
+/// Moves every member of the table in one launch; returns the number of launches (1).
+int launch_batch_relayout(const BatchRelayoutArgs& args, cudaStream_t stream);
+
 /// Per-block raw weighted moments of (states, weights).
 uint32_t moments_block_count(uint64_t n);
 void launch_moments(const Pose2* states, const double* weights, uint64_t n, double pivot_x, double pivot_y, double* moment_partials,

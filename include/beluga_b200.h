@@ -711,8 +711,40 @@ int bb200_amcl_batch_update_clustered(bb200_amcl_batch* b, const double* control
                                       const uint8_t* present, const bb200_cluster_param* p, bb200_update_result* out,
                                       bb200_estimate* clustered, uint32_t* n_cells, uint32_t* n_clusters);
 /* Kernel launches issued by this batch so far (steps, initialisations, cluster estimates, particle-cloud histograms and
- * pose samples, and the beam model's map uploads). */
+ * pose samples, membership changes, and the beam model's map uploads). */
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b);
+
+/* Members that join and leave a running batch (a fleet server whose robots connect, disconnect and reconnect with new
+ * parameters).  Member indices are slots: a slot is occupied or vacant, and an index keeps its meaning while its member
+ * lives.  bb200_amcl_batch_members returns the number of slots, occupied and vacant; slots are never removed, so every
+ * per-member array a call takes (control_poses, measurements, present, out, counts, ...) keeps that length.
+ *  - present == NULL selects every occupied slot.  present[m] != 0 on a vacant slot is BB200_ERR_INVALID_ARGUMENT before
+ *    anything reaches the device, and the batch is unchanged (bb200_amcl_batch_update, _update_measurements,
+ *    _update_clustered, _cluster_estimates, _particle_histograms, _sample_states).  A vacant slot's inputs are not read,
+ *    and its out[m] is written as an absent member's (updated = 0).
+ *  - Every per-member call (_initialize*, _force_update, _get_particles, _ancestors, _member_size, _update_map,
+ *    _member_map, _cluster_estimate, _remove_member) refuses a vacant slot with BB200_ERR_INVALID_ARGUMENT, as it refuses
+ *    an unknown index.
+ *  - _set_*_map assigns the map to every occupied slot; a vacant slot reads no map and never blocks _remove_map.
+ * Each call below is atomic -- when it fails, for validation or allocation, the batch is exactly as before -- and ends
+ * synchronised.  Every member's results stay byte-identical to those of a standalone bb200_amcl created when it joined
+ * (or when the batch was created) and fed the same inputs; after any sequence of joins and leaves, a step, cluster
+ * estimate, histogram or pose draw launches exactly what it launches on a freshly created batch of the same members. */
+
+/* Adds a member configured by params and motion, validated exactly as bb200_amcl_batch_create_with_flags validates a
+ * member under this batch's flags and device (the same messages, naming the slot it would take).  It takes the lowest
+ * vacant slot, or appends a new one; *member receives the slot.  The new member inherits nothing from the slot's earlier
+ * occupant: it reads no map and holds no particles, ancestors or CDF, and its policies start fresh, as those of a member
+ * of a freshly created batch.  Every other member's particles, weights, valid CDF, ancestors, policies and map are kept.
+ * The particle buffers are laid out again as create lays them out for the members now present: one kernel launch moves
+ * the other members' live data (none when no other member holds particles). */
+int bb200_amcl_batch_add_member(bb200_amcl_batch* b, const bb200_amcl_param* params, const bb200_motion_param* motion, int* member);
+/* Makes slot `member` vacant and frees its share of the device buffers (one kernel launch moves the other members' live
+ * data, none when none of them holds particles).  BB200_ERR_STATE when it is the last occupied slot: a batch always
+ * holds at least one member, as create requires. */
+int bb200_amcl_batch_remove_member(bb200_amcl_batch* b, int member);
+/* *active = 1 for an occupied slot, 0 for a vacant one (BB200_ERR_INVALID_ARGUMENT for an index out of range). */
+int bb200_amcl_batch_member_active(const bb200_amcl_batch* b, int member, int* active);
 
 /* The two host halves of bb200_amcl_update for callers that drive the filter themselves. */
 int bb200_amcl_plan_update(bb200_amcl* a, const double control_pose[4], bb200_step_plan* plan);

@@ -14,6 +14,7 @@
 // policy argument is accepted and ignored (everything per-particle runs on the device).
 #pragma once
 
+#include <algorithm>
 #include <execution>
 #include <map>
 #include <optional>
@@ -234,13 +235,39 @@ class AmclBatch {
   AmclBatch(const AmclBatch&) = delete;
   AmclBatch& operator=(const AmclBatch&) = delete;
 
+  /// Slots, occupied and vacant: the length of every per-member vector a call takes.
   [[nodiscard]] std::size_t size() const { return sizes_.size(); }
+
+  /// Adds a member (bb200_amcl_batch_add_member): it takes the lowest vacant slot or a new one after the last, and starts
+  /// as a member of a freshly created batch does, with no map and no particles.  Returns its slot.  The other members
+  /// keep their particles, policies and maps.
+  std::size_t add_member(const bb200_motion_param& motion, const AmclParams& params) {
+    const bb200_amcl_param p = c_amcl_param(params);
+    int slot = -1;
+    check(bb200_amcl_batch_add_member(handle_, &p, &motion, &slot));
+    const std::size_t m = static_cast<std::size_t>(slot);
+    if (m == sizes_.size()) sizes_.push_back(0);
+    sizes_[m] = params.max_particles;
+    return m;
+  }
+  /// Makes slot m vacant (bb200_amcl_batch_remove_member); the last occupied slot cannot be removed.
+  void remove_member(std::size_t member) {
+    check(bb200_amcl_batch_remove_member(handle_, index(member)));
+    sizes_[member] = 0;
+  }
+  /// Whether slot m holds a member.
+  [[nodiscard]] bool member_active(std::size_t member) const {
+    int active = 0;
+    check(bb200_amcl_batch_member_active(handle_, index(member), &active));
+    return active != 0;
+  }
 
   /// One likelihood field for every member (prob: the LikelihoodFieldProb model).
   void set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob = false) {
     check(bb200_amcl_batch_set_likelihood_field_map(handle_, &p, &grid, prob ? 1 : 0));
     field_cells_.clear();
-    field_cells_[member_map(0)] = static_cast<std::size_t>(grid.width) * static_cast<std::size_t>(grid.height);
+    const std::size_t occupied = static_cast<std::size_t>(std::find_if(sizes_.begin(), sizes_.end(), [](std::size_t n) { return n != 0; }) - sizes_.begin());
+    field_cells_[member_map(occupied)] = static_cast<std::size_t>(grid.width) * static_cast<std::size_t>(grid.height);
   }
   /// One beam-model map (BeamSensorModel) for every member; replaces the map set before, whichever model it was for.
   void set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid) {
@@ -466,7 +493,7 @@ class AmclBatch {
     check(bb200_amcl_batch_cluster_estimates(handle_, &p, present != nullptr ? mask.data() : nullptr, e.data(), nullptr, nullptr));
     std::vector<std::optional<estimation_type>> out(k);
     for (std::size_t m = 0; m < k; ++m) {
-      if (present != nullptr && !(*present)[m]) continue;
+      if ((present != nullptr && !(*present)[m]) || sizes_[m] == 0) continue;
       Matrix3d cov;
       for (int i = 0; i < 9; ++i) cov[i] = e[m].cov[i];
       out[m] = std::make_pair(SE2d::from_data(e[m].mean), cov);
@@ -489,7 +516,7 @@ class AmclBatch {
     std::vector<std::uint64_t> capacity(k, 0), n_bins(k, 0);
     std::vector<double> top(k, 0.0);
     for (std::size_t m = 0; m < k; ++m) {
-      if (present != nullptr && !(*present)[m]) continue;
+      if ((present != nullptr && !(*present)[m]) || sizes_[m] == 0) continue;
       bins[m].resize(sizes_[m]);
       ptrs[m] = bins[m].data();
       capacity[m] = sizes_[m];
@@ -524,7 +551,7 @@ class AmclBatch {
     check(bb200_amcl_batch_sample_states(handle_, n.data(), step, present != nullptr ? mask.data() : nullptr, ptrs.data()));
     std::vector<std::optional<std::vector<double>>> out(k);
     for (std::size_t m = 0; m < k; ++m)
-      if (present == nullptr || (*present)[m]) out[m] = std::move(raw[m]);
+      if ((present == nullptr || (*present)[m]) && sizes_[m] != 0) out[m] = std::move(raw[m]);
     return out;
   }
 
@@ -557,7 +584,7 @@ class AmclBatch {
 
   bool adaptive_{false};
   bb200_amcl_batch* handle_{nullptr};
-  std::vector<std::size_t> sizes_;  // max_particles: upper bounds of every member's particle, histogram and sample counts
+  std::vector<std::size_t> sizes_;  // per slot, max_particles (0: vacant): upper bounds of every member's particle, histogram and sample counts
   std::map<int, std::size_t> field_cells_;  // cells of each likelihood-field map, by id
 };
 

@@ -9,7 +9,8 @@ members read 1, 4 or 16 likelihood-field maps against one single-map batch per m
 K standalone filters publishing in turn.  `batch_measurements`: AmclBatch fed laser scans and point clouds converted on the
 device against host conversion plus the points update.  `batch_kld`: the `batch` workload with KLD-adaptive members (min 500,
 max 2000) against K standalone KLD Amcl.  `batch_selective`: the `batch` workload with selective-resampling members, fixed-size
-and KLD-adaptive (min 500, max 2000), against K standalone selective Amcl.
+and KLD-adaptive (min 500, max 2000), against K standalone selective Amcl.  `batch_members`: add_member and remove_member at
+K = 16 and 256 members, alone and next to a 32 768-particle member, and a step after churn against the same step on a fresh batch.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import json
@@ -235,6 +236,78 @@ def run_batch_selective():
                 "resampled_share": float(np.mean(resampled)), "mean_particles": float(np.mean(sizes)),
                 "ms_per_step_e2e": mb, "member_steps_per_s": k * 1e3 / mb, "launches_per_step": int(max(launches)),
                 "standalone_ms_per_round": ms, "standalone_member_steps_per_s": k * 1e3 / ms, "kernels_ms": {}, "device": device}
+    return res
+
+
+def run_batch_members():
+    """Members that join and leave: the host-clock time of add_member (a 2000-particle member) and of remove_member, each of
+    which ends synchronised, with K in {16, 256} members x 2000 particles holding particles, alone and next to a
+    32 768-particle member; and a step of a batch after churn (slot 0 vacated, one member appended) against the same step on
+    a freshly created batch of the same members, the two alternated in one session."""
+    res = {}
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=100, steps=100)
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    repeats, steps, warmup = 20, 20, 3
+    device = device_record()
+
+    def member(m, n=2000):
+        return bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m)
+
+    def make(params):
+        b = bb.AmclBatch([bb.DifferentialDriveModelParam(*MOTION) for _ in params], params)
+        b.set_likelihood_field_map(lfm, grid)
+        for m in range(len(params)):
+            b.initialize(m, sc.initial_mean, sc.initial_cov)
+        return b
+
+    for k in (16, 256):
+        for big in (False, True):
+            params = [member(m) for m in range(k)] + ([member(k, 32768)] if big else [])
+            batch = make(params)
+            batch.update([bb.se2(*sc.poses[0])] * len(params), [sc.scans[0]] * len(params))
+            add_ms, remove_ms, launches = [], [], []
+            for r in range(repeats + 1):
+                before = batch.launch_count()
+                t0 = time.perf_counter()
+                slot = batch.add_member(bb.DifferentialDriveModelParam(*MOTION), member(1000 + r))
+                t1 = time.perf_counter()
+                batch.remove_member(slot)
+                t2 = time.perf_counter()
+                launches.append(batch.launch_count() - before)
+                if r > 0:
+                    add_ms.append((t1 - t0) * 1e3)
+                    remove_ms.append((t2 - t1) * 1e3)
+            live = sum(q.max_particles for q in params)
+            res[f"batch_members_change_{k}_x_2000" + ("_and_32768" if big else "")] = {
+                "members": len(params), "live_particles": live, "moved_bytes_per_change": 40 * live,  # states and weights: the step resampled, so no CDF is current, and none records ancestors
+               
+                "add_member_ms": float(np.median(add_ms)), "remove_member_ms": float(np.median(remove_ms)),
+                "launches_per_add_and_remove": int(max(launches)), "repeats": repeats,
+                "ms_per_step_e2e": float(np.median(add_ms)), "kernels_ms": {}, "device": device}
+        churned = make([member(m) for m in range(k)])
+        map_id = churned.member_map(0)
+        slot = churned.add_member(bb.DifferentialDriveModelParam(*MOTION), member(k))
+        churned.remove_member(0)
+        churned.update_map(slot, map_id)
+        churned.initialize(slot, sc.initial_mean, sc.initial_cov)
+        fresh = make([member(m) for m in range(1, k + 1)])
+        wall_churned, wall_fresh = [], []
+        for t in range(warmup + steps):
+            pose = bb.se2(*sc.poses[t])
+            t0 = time.perf_counter()
+            a = churned.update([pose] * (k + 1), [None] + [sc.scans[t]] * k)
+            t1 = time.perf_counter()
+            b = fresh.update([pose] * k, [sc.scans[t]] * k)
+            t2 = time.perf_counter()
+            assert all(x.updated for x in a[1:]) and all(x.updated for x in b)
+            if t >= warmup:
+                wall_churned.append((t1 - t0) * 1e3)
+                wall_fresh.append((t2 - t1) * 1e3)
+        mc, mf = float(np.median(wall_churned)), float(np.median(wall_fresh))
+        res[f"batch_members_step_after_churn_{k}_x_2000_x_100_lfm_2000"] = {
+            "members": k, "steps": steps, "ms_per_step_e2e": mc, "fresh_batch_ms_per_step": mf, "churned_over_fresh": mc / mf,
+            "kernels_ms": {}, "device": device}
     return res
 
 
@@ -756,6 +829,8 @@ def main():
         out.update(run_batch_clustered())
     if "batch_cloud" in which:
         out.update(run_batch_cloud())
+    if "batch_members" in which:
+        out.update(run_batch_members())
     if "batch_beam" in which:
         out.update(run_batch_beam())
     if "batch_maps" in which:

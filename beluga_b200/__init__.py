@@ -350,6 +350,28 @@ class AmclParams:
                                self.recovery_probability_override)
 
 
+def state_params(blob: bytes):
+    """The parameters of a state blob (bb200_amcl_state_params, no device needed) -> (AmclParams, motion model param)."""
+    lib = _capi.load()
+    p, m = _capi.AmclParam(), _capi.MotionParam()
+    st = lib.bb200_amcl_state_params(blob, len(blob), C.byref(p), C.byref(m))
+    if st != _capi.OK:
+        raise BelugaB200Error(st, lib.bb200_create_error().decode())
+    params = AmclParams(p.update_min_d, p.update_min_a, p.resample_interval, bool(p.selective_resampling), p.min_particles,
+                        p.max_particles, p.alpha_slow, p.alpha_fast, p.kld_epsilon, p.kld_z, tuple(p.spatial_resolution),
+                        p.resample_scheme, p.seed, p.device, bool(p.record_ancestors), p.shard_first_index, p.shard_capacity,
+                        p.recovery_probability_override)
+    noise = (m.rotation_noise_from_rotation, m.rotation_noise_from_translation, m.translation_noise_from_translation,
+             m.translation_noise_from_rotation)
+    if m.model == _capi.MOTION_OMNIDIRECTIONAL:
+        motion = OmnidirectionalDriveModelParam(*noise, m.strafe_noise_from_translation, m.distance_threshold)
+    elif m.model == _capi.MOTION_STATIONARY:
+        motion = StationaryModelParam()
+    else:
+        motion = DifferentialDriveModelParam(*noise, m.distance_threshold)
+    return params, motion
+
+
 @dataclass
 class OccupancyGrid:
     """Occupancy grid with ROS trinary values: int8 [height, width], 0 free / 100 occupied / -1 unknown."""
@@ -609,6 +631,29 @@ class Amcl:
         self.params = params
         self.filter = Filter(_handle=self._lib.bb200_amcl_filter(self._h), _owner=self)
 
+    @classmethod
+    def from_state(cls, blob: bytes, device: int = 0) -> "Amcl":
+        """The filter a state blob holds (bb200_amcl_create_from_state) on `device`, without a map: update_map before updating."""
+        self = cls.__new__(cls)
+        self._lib = _capi.load()
+        h = C.c_void_p()
+        st = self._lib.bb200_amcl_create_from_state(blob, len(blob), device, C.byref(h))
+        if st != _capi.OK:
+            raise BelugaB200Error(st, self._lib.bb200_create_error().decode())
+        self._h = h
+        self.params = state_params(blob)[0]
+        self.params.device = device
+        self.filter = Filter(_handle=self._lib.bb200_amcl_filter(self._h), _owner=self)
+        return self
+
+    def export_state(self) -> bytes:
+        """This filter's state blob (bb200_amcl_export_state): parameters, policies, particles, weights, CDF and ancestors."""
+        size = C.c_uint64(0)
+        self._check(self._lib.bb200_amcl_export_state(self._h, None, 0, C.byref(size)))
+        buf = C.create_string_buffer(size.value)
+        self._check(self._lib.bb200_amcl_export_state(self._h, buf, size.value, C.byref(size)))
+        return buf.raw
+
     def close(self):
         if getattr(self, "_h", None):
             self.filter._h = None
@@ -828,6 +873,58 @@ class AmclBatch:
         p, m = params.c(), motion.c_motion()
         i = C.c_int(-1)
         self._check(self._lib.bb200_amcl_batch_add_member(self._h, C.byref(p), C.byref(m), C.byref(i)))
+        if i.value == len(self.params):
+            self.params.append(None)
+        self.params[i.value] = params
+        return i.value
+
+    @classmethod
+    def from_states(cls, blobs, adaptive: bool = False, selective: bool = False, device: int = 0) -> "AmclBatch":
+        """The batch whose member m is the filter of state blob blobs[m] (bb200_amcl_batch_create_from_states), on `device`,
+        validated with the constructor's flags; it has no map (add_*_map, then update_map)."""
+        self = cls.__new__(cls)
+        self._lib = _capi.load()
+        k = len(blobs)
+        data = (C.c_void_p * max(k, 1))(*[C.cast(C.c_char_p(b), C.c_void_p) for b in blobs])
+        sizes = (C.c_uint64 * max(k, 1))(*[len(b) for b in blobs])
+        flags = (_capi.BATCH_ADAPTIVE if adaptive else 0) | (_capi.BATCH_SELECTIVE if selective else 0)
+        h = C.c_void_p()
+        st = self._lib.bb200_amcl_batch_create_from_states(data, sizes, k, flags, device, C.byref(h))
+        if st != _capi.OK:
+            raise BelugaB200Error(st, self._lib.bb200_create_error().decode())
+        self._h = h
+        self.params = [state_params(b)[0] for b in blobs]
+        self.adaptive = bool(adaptive)
+        self.selective = bool(selective)
+        self._field_shapes = {}
+        return self
+
+    def export_member(self, member: int) -> bytes:
+        """Member `member`'s state blob (bb200_amcl_batch_export_member)."""
+        size = C.c_uint64(0)
+        self._check(self._lib.bb200_amcl_batch_export_member(self._h, member, None, 0, C.byref(size)))
+        buf = C.create_string_buffer(size.value)
+        self._check(self._lib.bb200_amcl_batch_export_member(self._h, member, buf, size.value, C.byref(size)))
+        return buf.raw
+
+    def export_members(self, present=None) -> list:
+        """The fleet checkpoint (bb200_amcl_batch_export_members): the state blob of every member whose `present` entry is
+        true (None: every occupied slot), None for the others, with one kernel launch and one synchronisation."""
+        mask = self._mask(present)
+        k = len(self.params)
+        sizes = (C.c_uint64 * k)()
+        self._check(self._lib.bb200_amcl_batch_export_members(self._h, mask, None, None, sizes))
+        bufs = [C.create_string_buffer(sizes[m]) if sizes[m] else None for m in range(k)]
+        out = (C.c_void_p * k)(*[C.cast(b, C.c_void_p) if b is not None else None for b in bufs])
+        self._check(self._lib.bb200_amcl_batch_export_members(self._h, mask, out, sizes, sizes))
+        return [None if self._skipped(present, m) else bufs[m].raw for m in range(k)]
+
+    def import_member(self, blob: bytes, map_id: int = -1) -> int:
+        """add_member with a history (bb200_amcl_batch_import_member): the blob's filter joins in the lowest vacant slot or a
+        new one and reads map `map_id` (-1: none).  Returns its slot."""
+        params = state_params(blob)[0]
+        i = C.c_int(-1)
+        self._check(self._lib.bb200_amcl_batch_import_member(self._h, blob, len(blob), map_id, C.byref(i)))
         if i.value == len(self.params):
             self.params.append(None)
         self.params[i.value] = params

@@ -246,6 +246,13 @@ SIGNATURES = {
     "bb200_amcl_batch_add_member": (C.c_int, [_vp, _P(AmclParam), _P(MotionParam), _P(C.c_int)]),
     "bb200_amcl_batch_remove_member": (C.c_int, [_vp, C.c_int]),
     "bb200_amcl_batch_member_active": (C.c_int, [_vp, C.c_int, _P(C.c_int)]),
+    "bb200_amcl_batch_export_members": (C.c_int, [_vp, _P(C.c_uint8), _P(_vp), _P(C.c_uint64), _P(C.c_uint64)]),
+    "bb200_amcl_batch_export_member": (C.c_int, [_vp, C.c_int, _vp, C.c_uint64, _P(C.c_uint64)]),
+    "bb200_amcl_batch_import_member": (C.c_int, [_vp, _vp, C.c_uint64, C.c_int, _P(C.c_int)]),
+    "bb200_amcl_batch_create_from_states": (C.c_int, [_P(_vp), _P(C.c_uint64), C.c_int, C.c_uint32, C.c_int, _P(_vp)]),
+    "bb200_amcl_export_state": (C.c_int, [_vp, _vp, C.c_uint64, _P(C.c_uint64)]),
+    "bb200_amcl_create_from_state": (C.c_int, [_vp, C.c_uint64, C.c_int, _P(_vp)]),
+    "bb200_amcl_state_params": (C.c_int, [_vp, C.c_uint64, _P(AmclParam), _P(MotionParam)]),
     "bb200_amcl_plan_update": (C.c_int, [_vp, _dbl, _P(StepPlan)]),
     "bb200_amcl_commit_update": (None, [_vp, C.c_int, C.c_double]),
     "bb200_amcl_create_with_motion": (C.c_int, [_P(AmclParam), _P(MotionParam), _P(_vp)]),

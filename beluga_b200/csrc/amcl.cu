@@ -2,6 +2,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <initializer_list>
 #include <limits>
 #include <vector>
@@ -89,6 +90,32 @@ bb200_motion_sampling motion_sampling(const bb200_motion_param& p, const Pose2& 
 
 AmclPolicy::AmclPolicy(const bb200_amcl_param& p, const bb200_motion_param& motion) : params_(p), motion_(motion) {
   if (params_.resample_interval == 0) params_.resample_interval = 1;
+}
+
+PolicyState AmclPolicy::save() const {
+  PolicyState s{};
+  s.has_latest_pose = latest_pose_.has_value() ? 1 : 0;
+  if (latest_pose_) std::memcpy(s.latest_pose, &*latest_pose_, sizeof(s.latest_pose));
+  std::memcpy(s.window, window_, sizeof(s.window));
+  s.every_n_current = every_n_current_;
+  s.slow_output = slow_output_;
+  s.fast_output = fast_output_;
+  s.step = step_;
+  s.window_size = window_size_;
+  s.force_update = force_update_ ? 1 : 0;
+  return s;
+}
+
+void AmclPolicy::restore(const PolicyState& s) {
+  latest_pose_.reset();
+  if (s.has_latest_pose) latest_pose_ = Pose2{s.latest_pose[0], s.latest_pose[1], s.latest_pose[2], s.latest_pose[3]};
+  std::memcpy(window_, s.window, sizeof(window_));
+  every_n_current_ = s.every_n_current;
+  slow_output_ = s.slow_output;
+  fast_output_ = s.fast_output;
+  step_ = s.step;
+  window_size_ = s.window_size;
+  force_update_ = s.force_update != 0;
 }
 
 void AmclPolicy::plan_update(const double control[4], uint64_t n, bb200_step_plan* plan) {
@@ -182,6 +209,36 @@ int Amcl::initialize_from_map() {
 int Amcl::initialize_states(const double* states, const double* weights, uint64_t n) {
   error_.clear();
   return initialized(filter_.set_particles(states, weights, n), n > 0);
+}
+
+int Amcl::export_state(void* out, uint64_t capacity, uint64_t* size) {
+  error_.clear();
+  if (sharded() || filter_.link().world() > 1) return filter_.fail_with(BB200_ERR_STATE, "a sharded filter has no state blob");
+  FilterState s{};
+  s.params = params();
+  s.motion = policy_.motion();
+  s.policy = policy_.save();
+  const bool record = params().record_ancestors != 0;
+  if (const int st = filter_.particle_set(&s.set, nullptr, size, record)) return st;
+  if (out == nullptr) return BB200_OK;
+  if (capacity < *size) return filter_.fail_with(BB200_ERR_CAPACITY, "state blob buffer too small (size has the blob's size)");
+  ParticleArrays arrays;
+  if (const int st = filter_.particle_set(&s.set, &arrays, size, record)) return st;
+  s.states = arrays.states.data();
+  s.weights = arrays.weights.data();
+  s.cdf = arrays.cdf.data();
+  s.ancestors = arrays.ancestors.data();
+  write_state_blob(s, out);
+  return BB200_OK;
+}
+
+int Amcl::restore_state(const FilterState& s) {
+  error_.clear();
+  const int st = filter_.restore_particle_set(s);
+  if (st != BB200_OK) return st;
+  policy_.restore(s.policy);
+  initialized_ = s.set.n > 0;
+  return BB200_OK;
 }
 
 int Amcl::plan_update(const double control[4], bb200_step_plan* plan) {

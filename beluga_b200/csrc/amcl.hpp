@@ -7,6 +7,7 @@
 #include <string>
 
 #include "filter.hpp"
+#include "state_blob.hpp"
 
 namespace bb200 {
 
@@ -24,6 +25,11 @@ class AmclPolicy {
   AmclPolicy(const bb200_amcl_param& p, const bb200_motion_param& motion);
 
   const bb200_amcl_param& params() const { return params_; }
+  const bb200_motion_param& motion() const { return motion_; }
+  /// Everything of the policy that decides its later steps, apart from its parameters (a state blob's policy section) ...
+  PolicyState save() const;
+  /// ... and the policy that saved it, given the same parameters.
+  void restore(const PolicyState& state);
   /// The next update runs whether or not the robot moved (amcl_core.hpp:136, after every initialisation).
   void force_update() { force_update_ = true; }
   /// Host half of update() for a filter of n particles (0: not initialised, no update): what to run this step.
@@ -63,6 +69,11 @@ class Amcl {
   int initialize(const double mean[3], const double cov[9]);
   int initialize_from_map();
   int initialize_states(const double* states, const double* weights, uint64_t n);
+  /// This filter's state blob (state_blob.hpp) into out[0, capacity), its size in *size; out == nullptr: the size only.
+  /// BB200_ERR_STATE for a shard, BB200_ERR_CAPACITY when capacity is below the size.
+  int export_state(void* out, uint64_t capacity, uint64_t* size);
+  /// Adopts a decoded state whose params and motion this filter was created with (bb200_amcl_create_from_state).
+  int restore_state(const FilterState& s);
   void force_update() { policy_.force_update(); }
   int update(const double control[4], const double* points_xy, uint64_t n_points, bb200_update_result* out);
   /// AmclPolicy::plan_update over this filter's particle count (a shard: the global count once initialised).

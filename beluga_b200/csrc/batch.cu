@@ -155,7 +155,7 @@ Batch::Batch(const bb200_amcl_param* params, const bb200_motion_param* motions, 
   created_ = true;
 }
 
-int Batch::relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* layout) {
+int Batch::relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* layout, const Arrival* arrival) {
   BB_CHECK(cudaSetDevice(device_));
   *layout = lay_out(slots);
   // Every allocation before anything moves: a failure frees the attempt and leaves the batch as it was.
@@ -204,6 +204,9 @@ int Batch::relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* l
     launches_ += static_cast<uint64_t>(launch_batch_relayout(a, stream_));
     BB_CHECK(cudaGetLastError());
   }
+  if (arrival != nullptr)
+    if (const int st = unpack({arrival->state}, {layout->offset[arrival->slot]}, s.states[0].get(), s.weights.get(), s.cdf.get(), s.ancestors.get()))
+      return st;
   BB_CHECK(cudaStreamSynchronize(stream_));  // the moves have landed; nothing in flight reads the old buffers
 
   // Nothing can fail from here on.
@@ -241,6 +244,255 @@ int Batch::add_member(const bb200_amcl_param& params, const bb200_motion_param& 
   }
   place(layout);
   *member = static_cast<int>(slot);
+  return BB200_OK;
+}
+
+namespace {
+
+/// Where a transfer's staging buffer holds the moved members' arrays: one region per array, each indexed by the members'
+/// staging offsets (a member takes max(n, ancestors) entries), so that one batch_relayout_kernel launch fills or empties it.
+struct StageLayout {
+  uint64_t states{0}, weights{0}, cdf{0}, ancestors{0}, bytes{0};  // byte offsets of the regions, and the total
+};
+
+StageLayout stage_layout(uint64_t entries, bool cdf, bool ancestors) {
+  StageLayout l;
+  l.weights = entries * sizeof(Pose2);
+  l.cdf = l.weights + entries * sizeof(double);
+  l.ancestors = l.cdf + (cdf ? entries * sizeof(unsigned long long) : 0);
+  l.bytes = l.ancestors + (ancestors ? entries * sizeof(long long) : 0);
+  return l;
+}
+
+}  // namespace
+
+ParticleSetState Batch::particle_set(const Member& m) {
+  ParticleSetState s{};
+  s.n = m.n;
+  s.ancestors_n = m.policy.params().record_ancestors ? m.ancestors_n : 0;
+  s.pivot[0] = m.pivot[0];
+  s.pivot[1] = m.pivot[1];
+  s.cdf_current = m.cdf_total != 0 ? 1 : 0;
+  s.cdf_total = m.cdf_total;
+  return s;
+}
+
+void Batch::adopt_state(Member& m, const FilterState& s) {
+  m.policy.restore(s.policy);
+  m.capacity = s.params.max_particles;
+  m.n = s.set.n;
+  m.cur = 0;
+  m.pivot[0] = s.set.pivot[0];
+  m.pivot[1] = s.set.pivot[1];
+  m.ancestors_n = s.set.ancestors_n;
+  m.cdf_total = s.set.cdf_current != 0 ? s.set.cdf_total : 0;
+}
+
+int Batch::launch_moves(const std::vector<BatchRelayoutMember>& moves, BatchRelayoutArgs a) {
+  const uint32_t n = static_cast<uint32_t>(moves.size());
+  std::vector<uint32_t> first(n + 1, 0);
+  for (uint32_t j = 0; j < n; ++j) first[j + 1] = first[j] + batch_relayout_ctas(moves[j]);
+  BB_CHECK(xfer_.table.grow(n));  // every batch call ends synchronised: nothing in flight reads the old tables
+  BB_CHECK(xfer_.first.grow(n + 1));
+  // Pageable sources: staged before the calls return.
+  BB_CHECK(cudaMemcpyAsync(xfer_.table.get(), moves.data(), n * sizeof(BatchRelayoutMember), cudaMemcpyHostToDevice, stream_));
+  BB_CHECK(cudaMemcpyAsync(xfer_.first.get(), first.data(), (n + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream_));
+  a.members = xfer_.table.get();
+  a.first = xfer_.first.get();
+  a.n_members = n;
+  a.ctas = first[n];
+  launches_ += static_cast<uint64_t>(launch_batch_relayout(a, stream_));
+  BB_CHECK(cudaGetLastError());
+  return BB200_OK;
+}
+
+int Batch::unpack(const std::vector<const FilterState*>& states, const std::vector<uint64_t>& to, Pose2* states_to, double* weights_to,
+                  unsigned long long* cdf_to, long long* ancestors_to) {
+  std::vector<BatchRelayoutMember> moves;
+  std::vector<const FilterState*> moved;
+  uint64_t entries = 0;
+  bool cdf = false, ancestors = false;
+  for (size_t j = 0; j < states.size(); ++j) {
+    const ParticleSetState& set = states[j]->set;
+    BatchRelayoutMember r{};
+    r.from = entries;
+    r.to = to[j];
+    r.n = set.n;
+    r.cdf_n = set.cdf_current != 0 ? set.n : 0;
+    r.ancestors_n = ancestors_to != nullptr ? set.ancestors_n : 0;
+    if (batch_relayout_ctas(r) == 0) continue;
+    entries += std::max(r.n, r.ancestors_n);
+    cdf = cdf || r.cdf_n > 0;
+    ancestors = ancestors || r.ancestors_n > 0;
+    moves.push_back(r);
+    moved.push_back(states[j]);
+  }
+  if (moves.empty()) return BB200_OK;
+  const StageLayout l = stage_layout(entries, cdf, ancestors);
+  BB_CHECK(xfer_.stage.grow(l.bytes));  // every batch call ends synchronised: the staging buffers are free
+  BB_CHECK(xfer_.stage_host.grow(l.bytes));
+  unsigned char* host = xfer_.stage_host.get();
+  for (size_t j = 0; j < moves.size(); ++j) {
+    const BatchRelayoutMember& r = moves[j];
+    const FilterState& s = *moved[j];
+    if (r.n > 0) std::memcpy(host + l.states + r.from * sizeof(Pose2), s.states, r.n * sizeof(Pose2));
+    if (r.n > 0) std::memcpy(host + l.weights + r.from * sizeof(double), s.weights, r.n * sizeof(double));
+    if (r.cdf_n > 0) std::memcpy(host + l.cdf + r.from * sizeof(unsigned long long), s.cdf, r.cdf_n * sizeof(unsigned long long));
+    if (r.ancestors_n > 0) std::memcpy(host + l.ancestors + r.from * sizeof(long long), s.ancestors, r.ancestors_n * sizeof(long long));
+  }
+  unsigned char* stage = xfer_.stage.get();
+  BB_CHECK(cudaMemcpyAsync(stage, host, l.bytes, cudaMemcpyHostToDevice, stream_));
+  BatchRelayoutArgs a{};
+  a.states_from[0] = a.states_from[1] = reinterpret_cast<const Pose2*>(stage + l.states);
+  a.weights_from = reinterpret_cast<const double*>(stage + l.weights);
+  a.cdf_from = reinterpret_cast<const unsigned long long*>(stage + l.cdf);
+  a.ancestors_from = reinterpret_cast<const long long*>(stage + l.ancestors);
+  a.states_to = states_to;
+  a.weights_to = weights_to;
+  a.cdf_to = cdf_to;
+  a.ancestors_to = ancestors_to;
+  return launch_moves(moves, a);
+}
+
+int Batch::export_members(const uint8_t* present, void* const* out, const uint64_t* capacity, uint64_t* size) {
+  error_.clear();
+  if (out != nullptr && capacity == nullptr) return fail(BB200_ERR_INVALID_ARGUMENT, "capacity is null");
+  if (const int st = check_present(present)) return st;
+  std::vector<uint32_t> written;  // selected members whose blobs are written, in member order
+  bool short_buffer = false;
+  for (size_t k = 0; k < members_.size(); ++k) {
+    if (!selected_member(present, k)) continue;
+    const Member& m = members_[k];
+    size[k] = state_blob_size(particle_set(m), m.policy.params().record_ancestors != 0);
+    if (out == nullptr || out[k] == nullptr) continue;
+    if (capacity[k] < size[k]) {
+      short_buffer = true;
+    } else {
+      written.push_back(static_cast<uint32_t>(k));
+    }
+  }
+  if (short_buffer) return fail(BB200_ERR_CAPACITY, "state blob buffer too small for some member (size has the sizes)");
+  if (written.empty()) return BB200_OK;
+
+  // The written members' live slices, gathered into the staging buffer by one launch and brought back by one copy.
+  std::vector<BatchRelayoutMember> moves;
+  std::vector<uint64_t> staged(written.size(), 0);
+  uint64_t entries = 0;
+  bool cdf = false, ancestors = false;
+  for (size_t j = 0; j < written.size(); ++j) {
+    const Member& m = members_[written[j]];
+    const ParticleSetState set = particle_set(m);
+    BatchRelayoutMember r{};
+    r.from = m.offset;
+    r.to = entries;
+    r.n = set.n;
+    r.cdf_n = set.cdf_current != 0 ? set.n : 0;
+    r.ancestors_n = set.ancestors_n;
+    r.cur = m.cur;
+    staged[j] = entries;
+    if (batch_relayout_ctas(r) == 0) continue;
+    entries += std::max(r.n, r.ancestors_n);
+    cdf = cdf || r.cdf_n > 0;
+    ancestors = ancestors || r.ancestors_n > 0;
+    moves.push_back(r);
+  }
+  const StageLayout l = stage_layout(entries, cdf, ancestors);
+  if (!moves.empty()) {
+    BB_CHECK(cudaSetDevice(device_));
+    BB_CHECK(xfer_.stage.grow(l.bytes));  // every batch call ends synchronised: the staging buffers are free
+    BB_CHECK(xfer_.stage_host.grow(l.bytes));
+    unsigned char* stage = xfer_.stage.get();
+    BatchRelayoutArgs a{};
+    a.states_from[0] = states_[0].get();
+    a.states_from[1] = states_[1].get();
+    a.weights_from = weights_.get();
+    a.cdf_from = cdf_.get();
+    a.ancestors_from = ancestors_.get();
+    a.states_to = reinterpret_cast<Pose2*>(stage + l.states);
+    a.weights_to = reinterpret_cast<double*>(stage + l.weights);
+    a.cdf_to = reinterpret_cast<unsigned long long*>(stage + l.cdf);
+    a.ancestors_to = reinterpret_cast<long long*>(stage + l.ancestors);
+    if (const int st = launch_moves(moves, a)) return st;
+    BB_CHECK(cudaMemcpyAsync(xfer_.stage_host.get(), stage, l.bytes, cudaMemcpyDeviceToHost, stream_));
+    BB_CHECK(cudaStreamSynchronize(stream_));
+  }
+
+  // The blobs, written from pinned memory.
+  const unsigned char* host = xfer_.stage_host.get();
+  for (size_t j = 0; j < written.size(); ++j) {
+    const uint32_t k = written[j];
+    const Member& m = members_[k];
+    FilterState s{};
+    s.params = m.policy.params();
+    s.motion = m.policy.motion();
+    s.policy = m.policy.save();
+    s.set = particle_set(m);
+    s.states = host + l.states + staged[j] * sizeof(Pose2);
+    s.weights = host + l.weights + staged[j] * sizeof(double);
+    s.cdf = host + l.cdf + staged[j] * sizeof(unsigned long long);
+    s.ancestors = host + l.ancestors + staged[j] * sizeof(long long);
+    write_state_blob(s, out[k]);
+  }
+  return BB200_OK;
+}
+
+int Batch::export_member(int member, void* out, uint64_t capacity, uint64_t* size) {
+  error_.clear();
+  if (const int st = member_ok(member)) return st;
+  const size_t k = static_cast<size_t>(member);
+  std::vector<uint8_t> present(members_.size(), 0);
+  std::vector<void*> outs(members_.size(), nullptr);
+  std::vector<uint64_t> capacities(members_.size(), 0), sizes(members_.size(), 0);
+  present[k] = 1;
+  outs[k] = out;
+  capacities[k] = capacity;
+  const int st = export_members(present.data(), outs.data(), capacities.data(), sizes.data());
+  *size = sizes[k];
+  return st;
+}
+
+int Batch::import_member(const void* blob, uint64_t size, int map, int* member) {
+  error_.clear();
+  FilterState s;
+  if (const int st = read_state_blob(blob, size, &s, &error_)) return st;
+  s.params.device = device_;  // the receiver's device
+  size_t slot = 0;
+  while (slot < members_.size() && members_[slot].active) ++slot;
+  if (const int st = validate_member(s.params, s.motion, static_cast<int>(slot), device_, flags_, &error_)) return st;
+  if (map != -1 && find_map(map) == nullptr) return BB200_ERR_INVALID_ARGUMENT;
+  Member joiner{AmclPolicy(s.params, s.motion)};
+  adopt_state(joiner, s);
+  joiner.map = map;
+  members_.reserve(members_.size() + 1);  // the host allocations that could fail come before the device work
+  std::vector<const bb200_amcl_param*> slots(std::max(members_.size(), slot + 1), nullptr);
+  for (size_t k = 0; k < members_.size(); ++k)
+    if (members_[k].active) slots[k] = &members_[k].policy.params();
+  slots[slot] = &s.params;
+  Layout layout;
+  const Arrival arrival{slot, &s};
+  if (const int st = relayout(slots, &layout, &arrival)) return st;
+  if (slot == members_.size()) {
+    members_.push_back(std::move(joiner));
+  } else {
+    members_[slot] = std::move(joiner);
+  }
+  place(layout);
+  *member = static_cast<int>(slot);
+  return BB200_OK;
+}
+
+int Batch::restore_members(const std::vector<FilterState>& states) {
+  error_.clear();
+  BB_CHECK(cudaSetDevice(device_));
+  std::vector<const FilterState*> from;
+  std::vector<uint64_t> to;
+  for (size_t k = 0; k < members_.size(); ++k) {
+    adopt_state(members_[k], states[k]);
+    from.push_back(&states[k]);
+    to.push_back(members_[k].offset);
+  }
+  if (const int st = unpack(from, to, states_[0].get(), weights_.get(), cdf_.get(), ancestors_.get())) return st;
+  BB_CHECK(cudaStreamSynchronize(stream_));
   return BB200_OK;
 }
 

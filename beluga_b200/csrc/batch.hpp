@@ -12,6 +12,7 @@
 #include "cluster.cuh"
 #include "device_buffer.hpp"
 #include "device_map.hpp"
+#include "state_blob.hpp"
 
 namespace bb200 {
 
@@ -47,6 +48,21 @@ class Batch {
   /// Makes slot `member` vacant and frees its share of the particle buffers (BB200_ERR_STATE for the last occupied slot).
   int remove_member(int member);
   int member_active(int member, int* active) const;
+  /// The state blob (state_blob.hpp) of every member whose present[m] is non-zero (present == nullptr: every occupied
+  /// slot).  size[m] receives the size of member m's blob; out[m] receives the blob when out and out[m] are set and
+  /// capacity[m] holds it (BB200_ERR_CAPACITY, before anything reaches the device, when some selected buffer does not).
+  /// One batch_relayout_kernel launch gathers every written member's arrays into one staging buffer, one copy brings it to
+  /// pinned memory and one synchronisation ends the call, whatever K is; none of them when no written member holds data.
+  int export_members(const uint8_t* present, void* const* out, const uint64_t* capacity, uint64_t* size);
+  /// export_members with member `member` alone selected.
+  int export_member(int member, void* out, uint64_t capacity, uint64_t* size);
+  /// add_member with a history: the member of a state blob, validated as add_member validates it (the blob's device is
+  /// not read), in the lowest vacant slot or a new one, reading map `map` (-1: none).  Its arrays reach the new layout
+  /// with one copy and one launch more than add_member's; on failure the batch is unchanged.
+  int import_member(const void* blob, uint64_t size, int map, int* member);
+  /// Gives the members of a batch just created from these states' params and motions their particle sets and policies
+  /// (bb200_amcl_batch_create_from_states): one copy and one launch, whatever K is.
+  int restore_members(const std::vector<FilterState>& states);
   uint64_t launch_count() const { return launches_; }  // including the map uploads' (the beam model's normaliser tables)
 
   /// One map for every member: removes every map, adds this one and assigns every member to it.
@@ -175,7 +191,24 @@ class Batch {
   /// The device half of a membership change to `slots`: new buffers, every surviving member's live data moved into them
   /// (batch_relayout_kernel), the old buffers freed and the scratch sized by the old layout dropped.  A survivor is a slot
   /// occupied now and in `slots`.  On failure the batch is unchanged.
-  int relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* layout);
+  /// `arrival` (nullable): a member joining in slot arrival->slot with the arrays of a decoded state, moved into the new
+  /// buffers before they are adopted (unpack).
+  struct Arrival {
+    size_t slot;
+    const FilterState* state;
+  };
+  int relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* layout, const Arrival* arrival = nullptr);
+  /// The scalars of member m's state blob.
+  static ParticleSetState particle_set(const Member& m);
+  /// Member m as the member a decoded state describes: its policy, count, pivot, CDF total and ancestors count (its
+  /// particles go to state buffer 0).
+  static void adopt_state(Member& m, const FilterState& s);
+  /// The arrays of states[j] into the staging buffer (host), one copy to the device, then one batch_relayout_kernel launch
+  /// into the buffers `*_to` at offsets to[j] (none when no state holds arrays).  Nothing is synchronised.
+  int unpack(const std::vector<const FilterState*>& states, const std::vector<uint64_t>& to, Pose2* states_to, double* weights_to,
+             unsigned long long* cdf_to, long long* ancestors_to);
+  /// One batch_relayout_kernel launch over `moves` (non-empty) with the ends in `a`; its table goes through the transfer scratch.
+  int launch_moves(const std::vector<BatchRelayoutMember>& moves, BatchRelayoutArgs a);
   /// BB200_ERR_INVALID_ARGUMENT when present (nullptr: every occupied slot) selects a vacant slot.
   int check_present(const uint8_t* present);
   bool selected_member(const uint8_t* present, size_t k) const { return members_[k].active && (present == nullptr || present[k] != 0); }
@@ -303,6 +336,15 @@ class Batch {
   };
   SampleTable sm_table_;
   uint64_t sample_header_{0};
+  // State blob transfers (grown on use): the move table of export and import, and the staging buffer that holds the moved
+  // members' arrays, on the device and in pinned memory (StageLayout, batch.cu).
+  struct TransferBuffers {
+    DeviceBuffer<BatchRelayoutMember> table;
+    DeviceBuffer<uint32_t> first;
+    DeviceBuffer<unsigned char> stage;
+    PinnedBuffer<unsigned char> stage_host;
+  };
+  TransferBuffers xfer_;
   DeviceBuffer<Pose2> samples_;
   PinnedBuffer<Pose2> samples_host_;
 };

@@ -15,6 +15,7 @@
 #include "cluster_host.hpp"
 #include "filter.hpp"
 #include "measurement_host.hpp"
+#include "state_blob.hpp"
 
 using bb200::Amcl;
 using bb200::Batch;
@@ -923,6 +924,95 @@ int bb200_amcl_batch_remove_member(bb200_amcl_batch* b, int member) {
 int bb200_amcl_batch_member_active(const bb200_amcl_batch* b, int member, int* active) {
   BB_REQUIRE(b && active);
   return guarded(b->impl, [&] { return b->impl.member_active(member, active); });
+}
+
+int bb200_amcl_batch_export_members(bb200_amcl_batch* b, const uint8_t* present, void* const* out, const uint64_t* capacity, uint64_t* size) {
+  BB_REQUIRE(b && size);
+  return guarded(b->impl, [&] { return b->impl.export_members(present, out, capacity, size); });
+}
+int bb200_amcl_batch_export_member(bb200_amcl_batch* b, int member, void* out, uint64_t capacity, uint64_t* size) {
+  BB_REQUIRE(b && size);
+  return guarded(b->impl, [&] { return b->impl.export_member(member, out, capacity, size); });
+}
+int bb200_amcl_batch_import_member(bb200_amcl_batch* b, const void* blob, uint64_t size, int map_id, int* member) {
+  BB_REQUIRE(b && blob && member);
+  return guarded(b->impl, [&] { return b->impl.import_member(blob, size, map_id, member); });
+}
+int bb200_amcl_batch_create_from_states(const void* const* blobs, const uint64_t* sizes, int n_members, uint32_t flags, int device,
+                                        bb200_amcl_batch** out) {
+  if (blobs == nullptr || sizes == nullptr || out == nullptr) {
+    g_create_error = "null argument";
+    return BB200_ERR_INVALID_ARGUMENT;
+  }
+  *out = nullptr;
+  if (n_members < 1) {
+    g_create_error = "a batch needs at least one member";
+    return BB200_ERR_INVALID_ARGUMENT;
+  }
+  return guarded_create([&] {
+    std::vector<bb200::FilterState> states(static_cast<size_t>(n_members));
+    std::vector<bb200_amcl_param> params(states.size());
+    std::vector<bb200_motion_param> motions(states.size());
+    for (size_t k = 0; k < states.size(); ++k) {
+      std::string message;
+      if (const int st = bb200::read_state_blob(blobs[k], sizes[k], &states[k], &message)) {
+        g_create_error = "member " + std::to_string(k) + ": " + message;
+        return st;
+      }
+      states[k].params.device = device;  // the receiver's device
+      params[k] = states[k].params;
+      motions[k] = states[k].motion;
+    }
+    bb200_amcl_batch* b = nullptr;
+    if (const int st = create_batch(params.data(), motions.data(), n_members, flags, &b)) return st;
+    if (const int st = b->impl.restore_members(states)) {
+      g_create_error = b->impl.last_error();
+      delete b;
+      return st;
+    }
+    *out = b;
+    return static_cast<int>(BB200_OK);
+  });
+}
+
+int bb200_amcl_state_params(const void* blob, uint64_t size, bb200_amcl_param* params, bb200_motion_param* motion) {
+  if (params == nullptr || motion == nullptr) {
+    g_create_error = "null argument";
+    return BB200_ERR_INVALID_ARGUMENT;
+  }
+  return guarded_create([&] {
+    bb200::FilterState s;
+    if (const int st = bb200::read_state_blob(blob, size, &s, &g_create_error)) return st;
+    *params = s.params;
+    *motion = s.motion;
+    return static_cast<int>(BB200_OK);
+  });
+}
+int bb200_amcl_export_state(bb200_amcl* a, void* out, uint64_t capacity, uint64_t* size) {
+  BB_REQUIRE(a && size);
+  return guarded(a->impl, [&] { return a->impl.export_state(out, capacity, size); });
+}
+int bb200_amcl_create_from_state(const void* blob, uint64_t size, int device, bb200_amcl** out) {
+  if (out == nullptr) {
+    g_create_error = "null argument";
+    return BB200_ERR_INVALID_ARGUMENT;
+  }
+  *out = nullptr;
+  bb200::FilterState s;
+  int st = guarded_create([&] { return bb200::read_state_blob(blob, size, &s, &g_create_error); });
+  if (st != BB200_OK) return st;
+  s.params.device = device;  // the receiver's device
+  bb200_amcl* a = nullptr;
+  st = bb200_amcl_create_with_motion(&s.params, &s.motion, &a);
+  if (st != BB200_OK) return st;
+  st = guarded(a->impl, [&] { return a->impl.restore_state(s); });
+  if (st != BB200_OK) {
+    g_create_error = a->impl.last_error();
+    bb200_amcl_destroy(a);
+    return st;
+  }
+  *out = a;
+  return BB200_OK;
 }
 
 int bb200_amcl_plan_update(bb200_amcl* a, const double control_pose[4], bb200_step_plan* plan) {

@@ -1119,4 +1119,58 @@ int Filter::cdf(uint64_t* out, uint64_t capacity) {
   return BB200_OK;
 }
 
+int Filter::particle_set(ParticleSetState* set, ParticleArrays* arrays, uint64_t* size, bool record_ancestors) {
+  *set = ParticleSetState{};
+  set->n = n_;
+  set->ancestors_n = record_ancestors && ancestors_.get() != nullptr ? ancestors_n_ : 0;
+  set->pivot[0] = pivot_[0];
+  set->pivot[1] = pivot_[1];
+  set->cdf_current = cdf_valid_ && n_ > 0 ? 1 : 0;
+  *size = state_blob_size(*set, record_ancestors);
+  if (arrays == nullptr) return BB200_OK;
+  BB_CHECK(cudaSetDevice(config_.device));
+  BB_CHECK(cudaStreamSynchronize(stream_));
+  arrays->states.resize(4 * n_);
+  arrays->weights.resize(n_);
+  arrays->cdf.resize(set->cdf_current != 0 ? n_ : 0);
+  arrays->ancestors.resize(set->ancestors_n);
+  if (n_ > 0) {
+    BB_CHECK(cudaMemcpy(arrays->states.data(), states_[cur_].get(), n_ * sizeof(Pose2), cudaMemcpyDeviceToHost));
+    BB_CHECK(cudaMemcpy(arrays->weights.data(), weights_.get(), n_ * sizeof(double), cudaMemcpyDeviceToHost));
+  }
+  if (set->cdf_current != 0) {
+    BB_CHECK(cudaMemcpy(arrays->cdf.data(), cdf_.get(), n_ * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    BB_CHECK(cudaMemcpy(&set->cdf_total, &scalars_.get()->total, sizeof(set->cdf_total), cudaMemcpyDeviceToHost));
+    if (set->cdf_total == 0) return fail(BB200_ERR_STATE, "the current CDF has a zero total");
+  }
+  if (set->ancestors_n > 0)
+    BB_CHECK(cudaMemcpy(arrays->ancestors.data(), ancestors_.get(), set->ancestors_n * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  return BB200_OK;
+}
+
+int Filter::restore_particle_set(const FilterState& s) {
+  const ParticleSetState& set = s.set;
+  if (set.n > capacity_ || set.ancestors_n > capacity_) return fail(BB200_ERR_CAPACITY, "more particles than the filter capacity");
+  BB_CHECK(cudaSetDevice(config_.device));
+  BB_CHECK(cudaStreamSynchronize(stream_));
+  if (set.n > 0) {
+    BB_CHECK(cudaMemcpy(states_[cur_].get(), s.states, set.n * sizeof(Pose2), cudaMemcpyHostToDevice));
+    BB_CHECK(cudaMemcpy(weights_.get(), s.weights, set.n * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  if (set.cdf_current != 0) {
+    // The draws of sample_states and resample read the CDF's total from the scalars, where the CDF build left it.
+    BB_CHECK(cudaMemcpy(cdf_.get(), s.cdf, set.n * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    BB_CHECK(cudaMemcpy(&scalars_.get()->total, &set.cdf_total, sizeof(set.cdf_total), cudaMemcpyHostToDevice));
+  }
+  if (set.ancestors_n > 0 && ancestors_.get() != nullptr)
+    BB_CHECK(cudaMemcpy(ancestors_.get(), s.ancestors, set.ancestors_n * sizeof(int64_t), cudaMemcpyHostToDevice));
+  n_ = set.n;
+  ancestors_n_ = ancestors_.get() != nullptr ? set.ancestors_n : 0;
+  pivot_[0] = set.pivot[0];
+  pivot_[1] = set.pivot[1];
+  cdf_valid_ = set.cdf_current != 0;
+  cloud_known_ = false;
+  return BB200_OK;
+}
+
 }  // namespace bb200

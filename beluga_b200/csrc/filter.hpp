@@ -16,8 +16,16 @@
 #include "device_map.hpp"
 #include "kernels.cuh"
 #include "shard_link.hpp"
+#include "state_blob.hpp"
 
 namespace bb200 {
+
+/// The particle arrays of a state blob, copied to the host.
+struct ParticleArrays {
+  std::vector<double> states, weights;
+  std::vector<uint64_t> cdf;
+  std::vector<int64_t> ancestors;
+};
 
 class Filter {
  public:
@@ -50,6 +58,11 @@ class Filter {
   int adopt(uint64_t n, int from_staging);
   int ancestors(int64_t* out, uint64_t capacity);
   int cdf(uint64_t* out, uint64_t capacity);
+  /// The particle set's part of a state blob: its scalars, and *size the blob's size with them.  With `arrays`, also its
+  /// arrays (the CDF while it is current, the ancestors when `record_ancestors`) and the current CDF's total.
+  int particle_set(ParticleSetState* set, ParticleArrays* arrays, uint64_t* size, bool record_ancestors);
+  /// Makes the particle set of a decoded state this filter's (its params' max_particles fit the capacity).
+  int restore_particle_set(const FilterState& s);
   int estimate(bb200_estimate* out);
   int moments(const double pivot[2], double out[9]);
   /// beluga::cluster_based_estimate (algorithm/cluster_based_estimation.hpp:415-432); cluster_ids

@@ -746,6 +746,46 @@ int bb200_amcl_batch_remove_member(bb200_amcl_batch* b, int member);
 /* *active = 1 for an occupied slot, 0 for a vacant one (BB200_ERR_INVALID_ARGUMENT for an index out of range). */
 int bb200_amcl_batch_member_active(const bb200_amcl_batch* b, int member, int* active);
 
+/* A filter's complete state as a byte string (a "state blob"): checkpoint a fleet before a restart, move a robot between
+ * batches, processes, devices and standalone filters, or capture one robot's filter to replay its logged scans offline.
+ * A blob holds the filter's parameters and motion model, its policies' state (on_motion pose, every_n phase, recovery
+ * filters, control window, forced update, step counter), its particles, weights, pivot, its CDF while that is current,
+ * and its ancestors when it records them.  It does not hold a map: the receiver attaches one.  A filter restored from a
+ * blob computes, step for step, exactly what the filter that wrote it would have computed (counter RNG keyed by seed,
+ * step and particle index).  The layout is versioned and described in DESIGN.md; it is in the byte order of the machine
+ * that wrote it, so blobs move between machines of the same endianness only.  params.device is not read on import: the
+ * receiver's device wins.  A blob that is truncated, padded, of another magic, blob version or ABI version, whose section
+ * lengths do not match its scalars, or whose scalars no filter holds is refused with BB200_ERR_INVALID_ARGUMENT.
+ *
+ * Size query: with out == NULL, *size receives the blob's size; BB200_ERR_CAPACITY (and *size) when capacity is below it.
+ * Sharded filters have no state blob: a shard (inside bb200_sharded_amcl, or with shard fields set) is BB200_ERR_STATE. */
+int bb200_amcl_export_state(bb200_amcl* a, void* out, uint64_t capacity, uint64_t* size);
+/* A standalone filter on `device` with the blob's parameters and state.  It has no map: an update before
+ * bb200_filter_set_*_map fails as on a newly created filter.  Failures are reported by bb200_create_error. */
+int bb200_amcl_create_from_state(const void* blob, uint64_t size, int device, bb200_amcl** out);
+/* Host only: checks a blob and returns its parameters and motion model (BB200_ERR_INVALID_ARGUMENT with the reason in
+ * bb200_create_error for a blob the calls here refuse). */
+int bb200_amcl_state_params(const void* blob, uint64_t size, bb200_amcl_param* params, bb200_motion_param* motion);
+/* The fleet checkpoint: the blob of every member m with present[m] != 0 (present NULL: every occupied slot).  size[m]
+ * receives member m's blob size; out[m] receives the blob when out and out[m] are not NULL and capacity[m] holds it.
+ * BB200_ERR_CAPACITY, before anything reaches the device, when some selected member's buffer is too small (size is still
+ * filled).  One kernel launch gathers the members' particle data, one copy brings it to the host and one synchronisation
+ * ends the call, whatever K is.  A vacant selected slot is BB200_ERR_INVALID_ARGUMENT. */
+int bb200_amcl_batch_export_members(bb200_amcl_batch* b, const uint8_t* present, void* const* out, const uint64_t* capacity, uint64_t* size);
+/* bb200_amcl_batch_export_members with member `member` alone selected. */
+int bb200_amcl_batch_export_member(bb200_amcl_batch* b, int member, void* out, uint64_t capacity, uint64_t* size);
+/* bb200_amcl_batch_add_member with a history: the blob's member joins in the lowest vacant slot or a new one (*member),
+ * validated exactly as bb200_amcl_batch_add_member validates its params under this batch's flags and device, and reads
+ * map map_id (-1: none, then it behaves as a joined member without a map).  The other members are kept as add_member keeps
+ * them.  One kernel launch more than add_member puts the blob's particle data in place.  Atomic: on failure the batch is
+ * unchanged. */
+int bb200_amcl_batch_import_member(bb200_amcl_batch* b, const void* blob, uint64_t size, int map_id, int* member);
+/* A batch whose member m is blobs[m]'s filter (sizes[m] bytes), on `device`, validated as bb200_amcl_batch_create_with_flags
+ * validates the blobs' parameters with `flags`.  One copy and one kernel launch restore every member's particle data,
+ * whatever K is.  The batch has no map: add them and assign them with bb200_amcl_batch_update_map. */
+int bb200_amcl_batch_create_from_states(const void* const* blobs, const uint64_t* sizes, int n_members, uint32_t flags, int device,
+                                        bb200_amcl_batch** out);
+
 /* The two host halves of bb200_amcl_update for callers that drive the filter themselves. */
 int bb200_amcl_plan_update(bb200_amcl* a, const double control_pose[4], bb200_step_plan* plan);
 void bb200_amcl_commit_update(bb200_amcl* a, int resampled, double random_state_probability);

@@ -69,6 +69,33 @@ inline bb200_amcl_param c_amcl_param(const AmclParams& params) {
   return p;
 }
 
+/// The parameters of a state blob (bb200_amcl_state_params), as AmclParams.
+inline AmclParams amcl_params_of_state(const std::vector<std::uint8_t>& blob, bb200_motion_param* motion = nullptr) {
+  bb200_amcl_param p{};
+  bb200_motion_param m{};
+  const int st = bb200_amcl_state_params(blob.data(), blob.size(), &p, &m);
+  if (st != BB200_OK) throw Error(st, bb200_create_error());
+  if (motion != nullptr) *motion = m;
+  AmclParams q;
+  q.update_min_d = p.update_min_d;
+  q.update_min_a = p.update_min_a;
+  q.resample_interval = p.resample_interval;
+  q.selective_resampling = p.selective_resampling != 0;
+  q.min_particles = p.min_particles;
+  q.max_particles = p.max_particles;
+  q.alpha_slow = p.alpha_slow;
+  q.alpha_fast = p.alpha_fast;
+  q.kld_epsilon = p.kld_epsilon;
+  q.kld_z = p.kld_z;
+  q.spatial_resolution_x = p.spatial_resolution[0];
+  q.spatial_resolution_y = p.spatial_resolution[1];
+  q.spatial_resolution_theta = p.spatial_resolution[2];
+  q.resample_scheme = static_cast<bb200_resample_scheme>(p.resample_scheme);
+  q.seed = p.seed;
+  q.device = p.device;
+  return q;
+}
+
 /// Particle set copy: the two vectors of beluga::TupleVector<std::tuple<SE2d, Weight>>.
 struct ParticleSet {
   std::vector<SE2d> states;
@@ -99,6 +126,25 @@ class Amcl {
   Amcl(Amcl&& other) noexcept
       : params_{other.params_}, motion_model_{std::move(other.motion_model_)}, sensor_model_{std::move(other.sensor_model_)}, handle_{other.handle_} {
     other.handle_ = nullptr;
+  }
+
+  /// The filter a state blob holds (bb200_amcl_create_from_state) on `device`, reading the sensor model's map: it continues
+  /// exactly where the filter that wrote the blob stopped.  The motion model must be the one the blob was written with.
+  static Amcl from_state(const std::vector<std::uint8_t>& blob, MotionModel motion_model, SensorModel sensor_model, int device = 0) {
+    AmclParams params = amcl_params_of_state(blob);
+    params.device = device;
+    bb200_amcl* handle = nullptr;
+    const int st = bb200_amcl_create_from_state(blob.data(), blob.size(), device, &handle);
+    if (st != BB200_OK) throw Error(st, bb200_create_error());
+    return Amcl(handle, params, std::move(motion_model), std::move(sensor_model));
+  }
+  /// This filter's state blob (bb200_amcl_export_state): parameters, policies, particles, weights, CDF and ancestors.
+  [[nodiscard]] std::vector<std::uint8_t> export_state() const {
+    std::uint64_t size = 0;
+    check(bb200_amcl_export_state(handle_, nullptr, 0, &size));
+    std::vector<std::uint8_t> blob(size);
+    check(bb200_amcl_export_state(handle_, blob.data(), blob.size(), &size));
+    return blob;
   }
 
   /// amcl_core.hpp:128 -- copies the particle set back from the device.
@@ -165,6 +211,10 @@ class Amcl {
   [[nodiscard]] bb200_amcl* handle() const { return handle_; }
 
  private:
+  Amcl(bb200_amcl* handle, const AmclParams& params, MotionModel motion_model, SensorModel sensor_model)
+      : params_{params}, motion_model_{std::move(motion_model)}, sensor_model_{std::move(sensor_model)}, handle_{handle} {
+    check(sensor_model_.attach(bb200_amcl_filter(handle_)));
+  }
   void check(int status) const {
     if (status != BB200_OK) throw Error(status, bb200_amcl_last_error(handle_));
   }
@@ -234,6 +284,10 @@ class AmclBatch {
   ~AmclBatch() { bb200_amcl_batch_destroy(handle_); }
   AmclBatch(const AmclBatch&) = delete;
   AmclBatch& operator=(const AmclBatch&) = delete;
+  /// Moves the handle (e.g. the batch from_states returns into the owner a server keeps).
+  AmclBatch(AmclBatch&& other) noexcept
+      : adaptive_{other.adaptive_}, handle_{std::exchange(other.handle_, nullptr)}, sizes_{std::move(other.sizes_)},
+        field_cells_{std::move(other.field_cells_)} {}
 
   /// Slots, occupied and vacant: the length of every per-member vector a call takes.
   [[nodiscard]] std::size_t size() const { return sizes_.size(); }
@@ -260,6 +314,59 @@ class AmclBatch {
     int active = 0;
     check(bb200_amcl_batch_member_active(handle_, index(member), &active));
     return active != 0;
+  }
+
+  /// The batch whose members are the filters of these state blobs (bb200_amcl_batch_create_from_states), on `device`,
+  /// with the batch flags as in the constructor.  It has no map: add maps and assign them with update_map.
+  static AmclBatch from_states(const std::vector<std::vector<std::uint8_t>>& blobs, bool adaptive = false, bool selective = false, int device = 0) {
+    std::vector<const void*> data;
+    std::vector<std::uint64_t> sizes;
+    std::vector<std::size_t> slots;
+    for (const auto& b : blobs) {
+      data.push_back(b.data());
+      sizes.push_back(b.size());
+      slots.push_back(amcl_params_of_state(b).max_particles);
+    }
+    const uint32_t flags = (adaptive ? uint32_t{BB200_BATCH_ADAPTIVE} : 0u) | (selective ? uint32_t{BB200_BATCH_SELECTIVE} : 0u);
+    bb200_amcl_batch* handle = nullptr;
+    const int st = bb200_amcl_batch_create_from_states(data.data(), sizes.data(), static_cast<int>(data.size()), flags, device, &handle);
+    if (st != BB200_OK) throw Error(st, bb200_create_error());
+    return AmclBatch(handle, std::move(slots), adaptive);
+  }
+  /// Member m's state blob (bb200_amcl_batch_export_member).
+  [[nodiscard]] std::vector<std::uint8_t> export_member(std::size_t member) const {
+    std::uint64_t size = 0;
+    check(bb200_amcl_batch_export_member(handle_, index(member), nullptr, 0, &size));
+    std::vector<std::uint8_t> blob(size);
+    check(bb200_amcl_batch_export_member(handle_, index(member), blob.data(), blob.size(), &size));
+    return blob;
+  }
+  /// The fleet checkpoint (bb200_amcl_batch_export_members): the state blob of every member selected by `present`
+  /// (nullptr: every occupied slot), an empty vector for the others, with one kernel launch and one synchronisation.
+  [[nodiscard]] std::vector<std::vector<std::uint8_t>> export_members(const std::vector<bool>* present = nullptr) const {
+    const std::vector<std::uint8_t> mask = presence_mask(present);
+    const std::uint8_t* m = present != nullptr ? mask.data() : nullptr;
+    std::vector<std::uint64_t> sizes(size(), 0);
+    check(bb200_amcl_batch_export_members(handle_, m, nullptr, nullptr, sizes.data()));
+    std::vector<std::vector<std::uint8_t>> blobs(size());
+    std::vector<void*> out(size(), nullptr);
+    for (std::size_t k = 0; k < size(); ++k) {
+      blobs[k].resize(sizes[k]);
+      if (sizes[k] > 0) out[k] = blobs[k].data();
+    }
+    check(bb200_amcl_batch_export_members(handle_, m, out.data(), sizes.data(), sizes.data()));
+    return blobs;
+  }
+  /// add_member with a history (bb200_amcl_batch_import_member): the blob's filter joins in the lowest vacant slot or a
+  /// new one, reading map `map_id` (-1: none).  Returns its slot.
+  std::size_t import_member(const std::vector<std::uint8_t>& blob, int map_id = -1) {
+    const std::size_t max_particles = amcl_params_of_state(blob).max_particles;
+    int slot = -1;
+    check(bb200_amcl_batch_import_member(handle_, blob.data(), blob.size(), map_id, &slot));
+    const std::size_t m = static_cast<std::size_t>(slot);
+    if (m == sizes_.size()) sizes_.push_back(0);
+    sizes_[m] = max_particles;
+    return m;
   }
 
   /// One likelihood field for every member (prob: the LikelihoodFieldProb model).
@@ -558,6 +665,7 @@ class AmclBatch {
   [[nodiscard]] bb200_amcl_batch* handle() const { return handle_; }
 
  private:
+  AmclBatch(bb200_amcl_batch* handle, std::vector<std::size_t> sizes, bool adaptive) : adaptive_{adaptive}, handle_{handle}, sizes_{std::move(sizes)} {}
   static std::vector<std::optional<estimation_type>> estimates_of(const std::vector<bb200_update_result>& r) {
     std::vector<std::optional<estimation_type>> out(r.size());
     for (std::size_t m = 0; m < r.size(); ++m) {

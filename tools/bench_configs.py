@@ -11,8 +11,10 @@ device against host conversion plus the points update.  `batch_kld`: the `batch`
 max 2000) against K standalone KLD Amcl.  `batch_selective`: the `batch` workload with selective-resampling members, fixed-size
 and KLD-adaptive (min 500, max 2000), against K standalone selective Amcl.  `batch_members`: add_member and remove_member at
 K = 16 and 256 members, alone and next to a 32 768-particle member, and a step after churn against the same step on a fresh batch.
+`batch_state`: export_members and AmclBatch.from_states (the fleet checkpoint and its restore) with the same members.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
+import ctypes
 import json
 import os
 import subprocess
@@ -308,6 +310,71 @@ def run_batch_members():
         res[f"batch_members_step_after_churn_{k}_x_2000_x_100_lfm_2000"] = {
             "members": k, "steps": steps, "ms_per_step_e2e": mc, "fresh_batch_ms_per_step": mf, "churned_over_fresh": mc / mf,
             "kernels_ms": {}, "device": device}
+    return res
+
+
+def run_batch_state():
+    """State blobs: the host-clock time of export_members (every member's blob, one launch, one copy and one
+    synchronisation) and of AmclBatch.from_states (a new batch from those blobs: its allocations, one copy and one launch),
+    with K in {16, 256} members x 2000 particles that have stepped once, alone and next to a 32 768-particle member; through
+    the Python wrappers (bytes in and out) and through the C ABI into buffers allocated once."""
+    res = {}
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=100, steps=10)
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    repeats = 20
+    device = device_record()
+
+    def member(m, n=2000):
+        return bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=m)
+
+    for k in (16, 256):
+        for big in (False, True):
+            params = [member(m) for m in range(k)] + ([member(k, 32768)] if big else [])
+            batch = bb.AmclBatch([bb.DifferentialDriveModelParam(*MOTION) for _ in params], params)
+            batch.set_likelihood_field_map(lfm, grid)
+            for m in range(len(params)):
+                batch.initialize(m, sc.initial_mean, sc.initial_cov)
+            batch.update([bb.se2(*sc.poses[0])] * len(params), [sc.scans[0]] * len(params))
+            export_ms, create_ms, launches = [], [], []
+            for r in range(repeats + 1):
+                before = batch.launch_count()
+                t0 = time.perf_counter()
+                blobs = batch.export_members()
+                t1 = time.perf_counter()
+                restored = bb.AmclBatch.from_states(blobs)
+                t2 = time.perf_counter()
+                launches.append((batch.launch_count() - before, restored.launch_count()))
+                restored.close()
+                if r > 0:
+                    export_ms.append((t1 - t0) * 1e3)
+                    create_ms.append((t2 - t1) * 1e3)
+            # The same two calls through the C ABI into buffers allocated once: the library's share of the times above.
+            lib, kk = batch._lib, len(params)
+            sizes = (ctypes.c_uint64 * kk)(*[len(b) for b in blobs])
+            bufs = [ctypes.create_string_buffer(len(b)) for b in blobs]
+            out = (ctypes.c_void_p * kk)(*[ctypes.cast(b, ctypes.c_void_p) for b in bufs])
+            data = (ctypes.c_void_p * kk)(*[ctypes.cast(b, ctypes.c_void_p) for b in bufs])
+            c_export_ms, c_create_ms = [], []
+            for r in range(repeats + 1):
+                h = ctypes.c_void_p()
+                t0 = time.perf_counter()
+                assert lib.bb200_amcl_batch_export_members(batch._h, None, out, sizes, sizes) == 0
+                t1 = time.perf_counter()
+                assert lib.bb200_amcl_batch_create_from_states(data, sizes, kk, 0, 0, ctypes.byref(h)) == 0
+                t2 = time.perf_counter()
+                lib.bb200_amcl_batch_destroy(h)
+                if r > 0:
+                    c_export_ms.append((t1 - t0) * 1e3)
+                    c_create_ms.append((t2 - t1) * 1e3)
+            live = sum(q.max_particles for q in params)
+            res[f"batch_state_{k}_x_2000" + ("_and_32768" if big else "")] = {
+                "members": len(params), "live_particles": live, "blob_bytes": sum(len(b) for b in blobs),
+                "moved_bytes": 40 * live,  # states and weights: the step resampled, so no CDF is current, and none records ancestors
+                "export_members_ms": float(np.median(export_ms)), "create_from_states_ms": float(np.median(create_ms)),
+                "export_members_c_ms": float(np.median(c_export_ms)), "create_from_states_c_ms": float(np.median(c_create_ms)),
+                "launches_export_and_create": [int(x) for x in max(launches)], "repeats": repeats,
+                "ms_per_step_e2e": float(np.median(export_ms)), "kernels_ms": {}, "device": device}
     return res
 
 
@@ -831,6 +898,8 @@ def main():
         out.update(run_batch_cloud())
     if "batch_members" in which:
         out.update(run_batch_members())
+    if "batch_state" in which:
+        out.update(run_batch_state())
     if "batch_beam" in which:
         out.update(run_batch_beam())
     if "batch_maps" in which:

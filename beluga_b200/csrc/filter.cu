@@ -820,7 +820,7 @@ int Filter::enqueue_propagate_reweight_kernels(const MotionSampling* sampling, u
       }
     } else {
       mark("reweight_lfm");
-      launch_reweight_lfm(states_[cur_].get(), weights_.get(), n_, perm, map_.field, points_.get(), points_host_.get(), static_cast<uint32_t>(n_points),
+      launch_reweight_lfm(states_[cur_].get(), weights_.get(), n_, perm, map_.field, points_.get(), static_cast<uint32_t>(n_points),
                           points_radius_, scalars_.get(), stream_);
       BB_LAUNCHED("reweight_lfm");
     }

@@ -292,11 +292,8 @@ uint32_t schedule_tile_count();
 void launch_build_schedule(const Pose2* states, uint64_t n, Schedule* sched, uint32_t* bins, uint32_t* counters, uint32_t* perm,
                            unsigned long long* tile_state, double mean_range, double min_bin, cudaStream_t stream);
 /// reweight with the likelihood-field table in schedule order (perm may be null) | block max.
-/// points_xy_host (optional): the same points in host memory; scans of up to 1920 points then travel as
-/// kernel parameters (constant bank) instead of being staged through shared memory.
 void launch_reweight_lfm(const Pose2* states, double* weights, uint64_t n, const uint32_t* perm, const FieldView& field,
-                         const double* points_xy_device, const double* points_xy_host, uint32_t n_points, double points_radius, Scalars* scalars,
-                         cudaStream_t stream);
+                         const double* points_xy_device, uint32_t n_points, double points_radius, Scalars* scalars, cudaStream_t stream);
 /// reweight with the beam model (Bresenham ray casting) in schedule order | block max.
 void launch_reweight_beam(const Pose2* states, double* weights, uint64_t n, const uint32_t* perm, const OccupancyView& grid,
                           const BeamParams& params, const double* points_xy_device, uint32_t n_points, Scalars* scalars, cudaStream_t stream);

@@ -144,6 +144,24 @@ __device__ __forceinline__ void staged_scan_block(const double2* __restrict__ po
   publish_weight_max(weight_bits(), &s_max, &s_arrived, kRwThreads / kWarp, scalars);
 }
 
+/// Copies the whole scan (n_points <= kChunkBeams) into the CTA's dynamic shared memory by one TMA bulk copy and returns
+/// it once every thread may read it.  Completion on an mbarrier, as in staged_scan_block.
+__device__ __forceinline__ const double2* stage_scan(const double2* __restrict__ points, uint32_t n_points) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  double2* s_pts = reinterpret_cast<double2*>(smem_raw);
+  __shared__ __align__(8) uint64_t s_bar;
+  if (threadIdx.x == 0) {
+    const uint32_t bytes = n_points * static_cast<uint32_t>(sizeof(double2));
+    mbarrier_init(&s_bar, 1);
+    mbarrier_init_fence();
+    mbarrier_expect_tx(&s_bar, bytes);  // an empty scan completes the phase here
+    if (bytes != 0) bulk_copy_g2s(s_pts, points, bytes, &s_bar);
+  }
+  __syncthreads();  // barrier initialised
+  mbarrier_wait(&s_bar, 0);
+  return s_pts;
+}
+
 /// One CTA of the general likelihood-field reweight: the particles in schedule slots [slot_base, slot_base + kRwThreads).
 __device__ __forceinline__ void reweight_lfm_block(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n,
                                                    const uint32_t* __restrict__ perm, const FieldView& field, const double2* __restrict__ points,
@@ -312,7 +330,7 @@ __device__ __forceinline__ void fixed_beams(const double2* pts, uint32_t count, 
 
 /// Adds the field values of pts[0, count) to the P sums acc: the fixed-point loop, then the reference's own operation
 /// sequence from the sum it started with for a particle whose margin ends at or below kFixedAmbiguous.  `pts` is the
-/// ScanParam in the constant bank or a chunk in shared memory.
+/// scan, or a chunk of it, in shared memory.
 template <int P>
 __device__ __forceinline__ void fixed_sum(const FieldView& field, const Pose2* __restrict__ states, const FixedGrid& grid,
                                           const FixedPose (&q)[P], const uint32_t (&margin_start)[P], const uint64_t (&i)[P],
@@ -367,7 +385,7 @@ __device__ __forceinline__ FixedGrid fixed_grid_setup(const FieldView& field, bo
   return g;
 }
 
-/// Scan staged in shared memory by TMA (scans longer than kParamBeams points): one CTA per kRwThreads particles, the
+/// Scan staged in shared memory by TMA chunk by chunk (scans longer than kChunkBeams points): one CTA per kRwThreads particles, the
 /// schedule slots [slot_base, slot_base + kRwThreads).
 __device__ __forceinline__ void reweight_lfm_fixed_block(const Pose2* __restrict__ states, double* __restrict__ weights, uint64_t n,
                                                          const uint32_t* __restrict__ perm, const FieldView& field, const double2* __restrict__ points,

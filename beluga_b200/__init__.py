@@ -32,7 +32,8 @@ from ._capi import (RESAMPLE_MULTINOMIAL, RESAMPLE_SYSTEMATIC, SENSOR_BEAM, SENS
 
 __all__ = [
     "Amcl", "AmclBatch", "AmclParams", "BeamModelParam", "DifferentialDriveModelParam", "OmnidirectionalDriveModelParam", "StationaryModelParam",
-    "Filter", "LikelihoodFieldModelParam", "motion_sampling", "scan_to_points", "point_cloud_to_points", "take_evenly_indices",
+    "Filter", "LikelihoodFieldModelParam", "motion_sampling", "scan_to_points", "scan_bearings", "point_cloud_to_points",
+    "take_evenly_indices",
     "OccupancyGrid", "BelugaB200Error", "device_count", "se2", "LaserScan", "PointCloud",
     "RESAMPLE_MULTINOMIAL", "RESAMPLE_SYSTEMATIC", "SENSOR_BEAM", "SENSOR_LIKELIHOOD_FIELD", "SENSOR_LIKELIHOOD_FIELD_PROB",
 ]
@@ -153,6 +154,27 @@ def scan_to_points(ranges, angle_min: float, angle_increment: float, min_range: 
     if st != _capi.OK:
         raise BelugaB200Error(st, "bb200_scan_to_points")
     return out[: n.value]
+
+
+def scan_bearings(angle_min: float, angle_increment: float, n_ranges: int, max_beams: int = 0) -> np.ndarray:
+    """The (n, 2) directions [cos, sin] of the beams a laser scan of this geometry keeps (take_evenly(max_beams)), exactly as
+    scan_to_points computes them and without dropping readings by range: the bearings of the scan's expected ranges
+    (Filter.cast_rays)."""
+    lib = _capi.load()
+    n = C.c_uint64()
+    st = lib.bb200_scan_bearings(angle_min, angle_increment, n_ranges, max_beams, None, 0, C.byref(n))
+    if st not in (_capi.OK, _capi.ERR_CAPACITY):
+        raise BelugaB200Error(st, "bb200_scan_bearings")
+    out = np.zeros((n.value, 2))
+    st = lib.bb200_scan_bearings(angle_min, angle_increment, n_ranges, max_beams, _dptr(out) if n.value else None, n.value, C.byref(n))
+    if st != _capi.OK:
+        raise BelugaB200Error(st, "bb200_scan_bearings")
+    return out
+
+
+def _rays(poses, bearings):
+    """Contiguous (n, 4) poses and (m, 2) bearings for a ray cast."""
+    return _f64(poses).reshape(-1, 4), _f64(bearings).reshape(-1, 2)
 
 
 def _point_cloud(data, point_step: int, x_offset: int, dtype, origin, n_points):
@@ -586,6 +608,15 @@ class Filter:
         self._check(self._lib.bb200_filter_sample_states(self._h, count, step, _dptr(out) if count else None))
         return out
 
+    def cast_rays(self, poses, bearings, max_range: float) -> np.ndarray:
+        """Ray2d::cast on the current map (bb200_filter_cast_rays): sensor poses (n, 4) [cos, sin, x, y] in the map frame
+        times bearings (m, 2) [cos, sin] taken as given -> (n, m) ranges, min(distance, max_range) on a hit, inf on a miss."""
+        p, b = _rays(poses, bearings)
+        out = np.zeros((len(p), len(b)))
+        self._check(self._lib.bb200_filter_cast_rays(self._h, _dptr(p) if len(p) else None, len(p), _dptr(b) if len(b) else None, len(b),
+                                                     max_range, _dptr(out) if out.size else None))
+        return out
+
     def moments(self, pivot=(0.0, 0.0)) -> np.ndarray:
         out = np.zeros(9)
         self._check(self._lib.bb200_filter_moments(self._h, _dptr(_f64(pivot)), _dptr(out)))
@@ -691,6 +722,10 @@ class Amcl:
 
     def particles(self):
         return self.filter.particles()
+
+    def cast_rays(self, poses, bearings, max_range: float) -> np.ndarray:
+        """Filter.cast_rays on the map of update_map."""
+        return self.filter.cast_rays(poses, bearings, max_range)
 
     def update_scan(self, control_pose, ranges, angle_min: float, angle_increment: float, min_range: float = 0.0,
                     max_range: float = float("inf"), max_beams: int = 0, laser_origin=None) -> _capi.UpdateResult:
@@ -1095,6 +1130,31 @@ class AmclBatch:
         ptrs = (C.POINTER(C.c_double) * k)(*[_dptr(o) if len(o) else None for o in outs])
         self._check(self._lib.bb200_amcl_batch_sample_states(self._h, (C.c_uint64 * k)(*counts), step, mask, ptrs))
         return [None if self._skipped(present, m) else outs[m] for m in range(k)]
+
+    def cast_rays(self, poses, bearings, max_range, present=None, map_ids=None) -> list:
+        """Filter.cast_rays for every member whose `present` entry is true (None: every occupied slot), in one launch ->
+        per member an (n_poses, n_bearings) array, None for members not selected.  `poses`: per member an (n, 4) array
+        (None where not selected); `bearings`: one (m, 2) array for every member, or one per member; `max_range`: one
+        number for every member, or one per member; `map_ids`: per member a map id of the batch to cast on, -1 (or
+        map_ids None) for the member's own map."""
+        mask = self._mask(present)
+        k = len(self.params)
+        shared = isinstance(bearings, np.ndarray) and bearings.ndim == 2
+        if len(poses) != k or (not shared and len(bearings) != k):
+            raise ValueError("one pose array and one bearing array per member")
+        ranges = [float(max_range)] * k if np.isscalar(max_range) else [float(r) for r in max_range]
+        if len(ranges) != k or (map_ids is not None and len(map_ids) != k):
+            raise ValueError("one maximum range and one map id per member")
+        sel = [not self._skipped(present, m) for m in range(k)]
+        rays = [_rays(poses[m], bearings if shared else bearings[m]) if sel[m] else (np.zeros((0, 4)), np.zeros((0, 2))) for m in range(k)]
+        outs = [np.zeros((len(p), len(b))) for p, b in rays]
+        ptr = lambda a: _dptr(a) if a.size else None  # noqa: E731
+        self._check(self._lib.bb200_amcl_batch_cast_rays(
+            self._h, mask, None if map_ids is None else (C.c_int * k)(*[int(i) for i in map_ids]),
+            (C.POINTER(C.c_double) * k)(*[ptr(p) for p, _ in rays]), (C.c_uint64 * k)(*[len(p) for p, _ in rays]),
+            (C.POINTER(C.c_double) * k)(*[ptr(b) for _, b in rays]), (C.c_uint64 * k)(*[len(b) for _, b in rays]),
+            (C.c_double * k)(*ranges), (C.POINTER(C.c_double) * k)(*[ptr(o) for o in outs])))
+        return [outs[m] if sel[m] else None for m in range(k)]
 
     def update(self, control_poses, points, present=None) -> list:
         """Amcl::update for every member whose `present` entry is true (None: all).  `control_poses`: K poses [c, s, x, y];

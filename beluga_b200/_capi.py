@@ -172,6 +172,7 @@ SIGNATURES = {
     "bb200_filter_cluster_estimate": (C.c_int, [_vp, _P(ClusterParam), _P(Estimate), _P(C.c_uint32), C.c_uint64, _P(C.c_uint32), _P(C.c_uint32)]),
     "bb200_filter_particle_histogram": (C.c_int, [_vp, C.c_double, C.c_double, _P(ClusterCell), C.c_uint64, _P(C.c_uint64), _dbl]),
     "bb200_filter_sample_states": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _dbl]),
+    "bb200_filter_cast_rays": (C.c_int, [_vp, _dbl, C.c_uint64, _dbl, C.c_uint64, C.c_double, _dbl]),
     "bb200_particle_cloud_markers": (C.c_int, [_P(ClusterCell), C.c_uint64, _P(MarkerVertex), _P(MarkerVertex), _dbl]),
     "bb200_likelihood_field_to_occupancy": (C.c_int, [_P(C.c_float), C.c_uint64, _P(C.c_int8)]),
     "bb200_filter_moments": (C.c_int, [_vp, _dbl, _dbl]),
@@ -191,6 +192,7 @@ SIGNATURES = {
     "bb200_amcl_force_update": (None, [_vp]),
     "bb200_amcl_update": (C.c_int, [_vp, _dbl, _dbl, C.c_uint64, _P(UpdateResult)]),
     "bb200_scan_to_points": (C.c_int, [_P(LaserScan), _dbl, C.c_uint64, _P(C.c_uint64)]),
+    "bb200_scan_bearings": (C.c_int, [C.c_float, C.c_float, C.c_uint64, C.c_uint64, _dbl, C.c_uint64, _P(C.c_uint64)]),
     "bb200_take_evenly_indices": (C.c_int, [C.c_uint64, C.c_uint64, _P(C.c_uint64), C.c_uint64, _P(C.c_uint64)]),
     "bb200_amcl_update_scan": (C.c_int, [_vp, _dbl, _P(LaserScan), _P(UpdateResult)]),
     "bb200_point_cloud_to_points": (C.c_int, [_P(PointCloud), _dbl, C.c_uint64, _P(C.c_uint64)]),
@@ -238,6 +240,7 @@ SIGNATURES = {
     "bb200_amcl_batch_particle_histograms": (C.c_int, [_vp, C.c_double, C.c_double, _P(C.c_uint8), _P(_P(ClusterCell)), _P(C.c_uint64),
                                                        _P(C.c_uint64), _dbl]),
     "bb200_amcl_batch_sample_states": (C.c_int, [_vp, _P(C.c_uint64), C.c_uint32, _P(C.c_uint8), _P(_dbl)]),
+    "bb200_amcl_batch_cast_rays": (C.c_int, [_vp, _P(C.c_uint8), _P(C.c_int), _P(_dbl), _P(C.c_uint64), _P(_dbl), _P(C.c_uint64), _dbl, _P(_dbl)]),
     "bb200_amcl_batch_update": (C.c_int, [_vp, _dbl, _P(_dbl), _P(C.c_uint64), _P(C.c_uint8), _P(UpdateResult)]),
     "bb200_amcl_batch_update_measurements": (C.c_int, [_vp, _dbl, _P(Measurement), _P(C.c_uint8), _P(UpdateResult)]),
     "bb200_amcl_batch_update_clustered": (C.c_int, [_vp, _dbl, _P(Measurement), _P(C.c_uint8), _P(ClusterParam), _P(UpdateResult), _P(Estimate),

@@ -1056,6 +1056,103 @@ int Batch::sample_states(const uint64_t* counts, uint32_t step, const uint8_t* p
   return BB200_OK;
 }
 
+int Batch::ensure_rays(size_t members, uint64_t doubles) {
+  const RayBuffers& r = rays_;
+  if (members <= std::min(r.table.size(), r.table_host.size()) && doubles <= std::min(r.data.size(), r.data_host.size())) return BB200_OK;
+  // Every batch call ends synchronised: nothing in flight reads the old buffers.
+  RayBuffers t;
+  const uint64_t room = std::max<uint64_t>(doubles + doubles / 2, 4096);
+  BB_CHECK(t.table.allocate(members_.size()));
+  BB_CHECK(t.table_host.allocate(members_.size()));
+  BB_CHECK(t.data.allocate(room));
+  BB_CHECK(t.data_host.allocate(room));
+  rays_ = std::move(t);
+  return BB200_OK;
+}
+
+int Batch::cast_rays(const uint8_t* present, const int* map_ids, const double* const* poses, const uint64_t* n_poses, const double* const* bearings,
+                     const uint64_t* n_bearings, const double* max_range, double* const* ranges) {
+  error_.clear();
+  // Filter::cast_rays's checks per member, all before anything reaches the device.
+  if (const int st = check_present(present)) return st;
+  struct Cast {
+    size_t k;
+    DeviceMap* map;
+    uint64_t n_rays;
+  };
+  std::vector<Cast> casts;  // selected members with rays to cast, in member order
+  uint64_t pose_doubles = 0, bearing_doubles = 0, total_rays = 0, ctas = 0;
+  for (size_t k = 0; k < members_.size(); ++k) {
+    if (!selected_member(present, k)) continue;
+    const std::string who = "member " + std::to_string(k) + ": ";
+    const bool override_map = map_ids != nullptr && map_ids[k] != -1;
+    const int id = override_map ? map_ids[k] : members_[k].map;
+    if (override_map && find_map(id) == nullptr) return fail(BB200_ERR_INVALID_ARGUMENT, who + error_);
+    if (id < 0) return fail(BB200_ERR_STATE, who + "no map");
+    uint64_t n_rays = 0;
+    if (!cast_ray_count(n_poses[k], n_bearings[k], &n_rays)) return fail(BB200_ERR_INVALID_ARGUMENT, who + "n_poses * n_bearings overflows");
+    if ((poses[k] == nullptr && n_poses[k] > 0) || (bearings[k] == nullptr && n_bearings[k] > 0) || (ranges[k] == nullptr && n_rays > 0))
+      return fail(BB200_ERR_INVALID_ARGUMENT, who + "null array with a non-zero count");
+    if (n_rays == 0) continue;
+    if (n_rays > kMaxCastRays) return fail(BB200_ERR_CAPACITY, who + "too many rays for one launch");
+    ctas += cast_rays_ctas(n_rays);
+    if (ctas > kMaxCastRays / 256) return fail(BB200_ERR_CAPACITY, "too many rays for one launch");
+    // n_poses and n_bearings are at most n_rays here, and the CTA bound keeps every sum far from overflowing
+    pose_doubles += 4 * n_poses[k];
+    bearing_doubles += 2 * n_bearings[k];
+    total_rays += n_rays;
+    casts.push_back(Cast{k, &maps_.at(id).map, n_rays});
+  }
+  if (casts.empty()) return BB200_OK;
+  BB_CHECK(cudaSetDevice(device_));
+  const uint32_t n_sel = static_cast<uint32_t>(casts.size());
+  if (const int st = ensure_rays(n_sel, pose_doubles + bearing_doubles + total_rays)) return st;
+  double* staged = rays_.data_host.get();
+  uint64_t pose_offset = 0, bearing_offset = 0, ray_offset = 0;
+  BatchRayArgs a{};
+  a.n_members = n_sel;
+  for (uint32_t j = 0; j < n_sel; ++j) {
+    const size_t k = casts[j].k;
+    BatchRayMember& r = rays_.table_host.get()[j];
+    r = BatchRayMember{};
+    if (const int st = casts[j].map->ray_view(stream_, &r.grid, &error_)) return st;  // a likelihood-field map's first cast uploads its table
+    r.pose_offset = pose_offset;
+    r.bearing_offset = bearing_offset;
+    r.ray_offset = ray_offset;
+    r.n_bearings = n_bearings[k];
+    r.n_rays = casts[j].n_rays;
+    r.max_range = max_range[k];
+    std::memcpy(staged + 4 * pose_offset, poses[k], 4 * n_poses[k] * sizeof(double));
+    std::memcpy(staged + pose_doubles + 2 * bearing_offset, bearings[k], 2 * n_bearings[k] * sizeof(double));
+    pose_offset += n_poses[k];
+    bearing_offset += n_bearings[k];
+    ray_offset += r.n_rays;
+    first_host_.get()[j] = a.ctas;  // the step's range buffers are free between calls
+    a.ctas += cast_rays_ctas(r.n_rays);
+  }
+  first_host_.get()[n_sel] = a.ctas;
+  cudaStream_t stream = stream_;
+  double* d = rays_.data.get();
+  BB_CHECK(cudaMemcpyAsync(d, staged, (pose_doubles + bearing_doubles) * sizeof(double), cudaMemcpyHostToDevice, stream));
+  BB_CHECK(cudaMemcpyAsync(rays_.table.get(), rays_.table_host.get(), n_sel * sizeof(BatchRayMember), cudaMemcpyHostToDevice, stream));
+  BB_CHECK(cudaMemcpyAsync(first_.get(), first_host_.get(), (n_sel + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+  a.members = rays_.table.get();
+  a.first = first_.get();
+  a.poses = reinterpret_cast<const Pose2*>(d);
+  a.bearings = reinterpret_cast<const double2*>(d + pose_doubles);
+  a.ranges = d + pose_doubles + bearing_doubles;
+  launches_ += static_cast<uint64_t>(launch_batch_cast_rays(a, stream));
+  BB_CHECK(cudaGetLastError());
+  double* out = staged + pose_doubles + bearing_doubles;
+  BB_CHECK(cudaMemcpyAsync(out, a.ranges, total_rays * sizeof(double), cudaMemcpyDeviceToHost, stream));
+  BB_CHECK(cudaStreamSynchronize(stream));
+  for (uint32_t j = 0; j < n_sel; ++j) {
+    const BatchRayMember& r = rays_.table_host.get()[j];
+    std::memcpy(ranges[casts[j].k], out + r.ray_offset, r.n_rays * sizeof(double));
+  }
+  return BB200_OK;
+}
+
 int Batch::ensure_points(uint64_t n_points) {
   if (2 * n_points <= std::min(points_.size(), points_host_.size())) return BB200_OK;
   BB_CHECK(cudaStreamSynchronize(stream_));

@@ -101,6 +101,12 @@ class Batch {
   /// every such member's CDF is current and four when some CDF has to be rebuilt, and one host synchronisation.  No particle
   /// set changes.
   int sample_states(const uint64_t* counts, uint32_t step, const uint8_t* present, double* const* states_out);
+  /// Filter::cast_rays for every selected member on its own map, or on map map_ids[m] when map_ids is set and the entry is
+  /// not -1: n_poses[m] x n_bearings[m] rays from poses[m] along bearings[m] up to max_range[m] into ranges[m].  One launch
+  /// (none without rays) and one host synchronisation, whatever K and the maps are.  Every check is made before anything
+  /// reaches the device, and no member changes.
+  int cast_rays(const uint8_t* present, const int* map_ids, const double* const* poses, const uint64_t* n_poses, const double* const* bearings,
+                const uint64_t* n_bearings, const double* max_range, double* const* ranges);
   /// Amcl::update for every member whose present[m] is non-zero (present == nullptr: all of them).  Atomic for the whole
   /// batch: when the device half fails, every member's host state is rolled back.
   int update(const double* control_poses, const double* const* points_xy, const uint64_t* n_points, const uint8_t* present,
@@ -243,6 +249,8 @@ class Batch {
   /// member selected[j]'s count in cl_.cells_host[j].  Two launches and two host synchronisations.
   int cell_records(double linear, double angular, const std::vector<uint32_t>& selected);
   int ensure_samples(uint64_t draws);
+  /// The ray-cast scratch for `members` table entries and `doubles` of poses, bearings and ranges.
+  int ensure_rays(size_t members, uint64_t doubles);
 
   std::vector<Member> members_;  // by slot
   uint32_t flags_{0};
@@ -347,6 +355,15 @@ class Batch {
   TransferBuffers xfer_;
   DeviceBuffer<Pose2> samples_;
   PinnedBuffer<Pose2> samples_host_;
+  // Ray-cast scratch (grown on use): the member table, and every casting member's poses, then bearings, then ranges, on the
+  // device and in pinned memory.
+  struct RayBuffers {
+    DeviceBuffer<BatchRayMember> table;
+    PinnedBuffer<BatchRayMember> table_host;
+    DeviceBuffer<double> data;
+    PinnedBuffer<double> data_host;
+  };
+  RayBuffers rays_;
 };
 
 }  // namespace bb200

@@ -3,6 +3,7 @@
 #include "bucket_set.cuh"
 #include "cdf.cuh"
 #include "kld.cuh"
+#include "raycast.cuh"
 #include "resample.cuh"
 #include "reweight_beam.cuh"
 #include "reweight_lfm.cuh"
@@ -587,6 +588,15 @@ __global__ void __launch_bounds__(kRelayoutThreads) batch_relayout_kernel(BatchR
   if (i < m.ancestors_n) s.ancestors_to[m.to + i] = s.ancestors_from[m.from + i];
 }
 
+// ---- ray casts: each member's rays on its map --------------------------------------------------------------------
+
+__global__ void __launch_bounds__(kRayThreads) batch_cast_rays_kernel(BatchRayArgs s) {
+  uint32_t local, count;
+  const BatchRayMember& m = s.members[batch_member_of(s, 0, blockIdx.x, local, count)];
+  const OccupancyView grid = m.grid;
+  cast_rays_block(grid, s.poses + m.pose_offset, s.bearings + m.bearing_offset, m.n_bearings, m.n_rays, m.max_range, s.ranges + m.ray_offset, local);
+}
+
 template <bool kTable>
 int launch_batch_step_from(const BatchStepArgs& s, cudaStream_t stream) {
   const uint32_t reset = std::max(s.n_members, s.ctas[kBatchScan]);
@@ -692,6 +702,11 @@ uint32_t batch_relayout_ctas(const BatchRelayoutMember& m) {
 
 int launch_batch_relayout(const BatchRelayoutArgs& s, cudaStream_t stream) {
   batch_relayout_kernel<<<s.ctas, kRelayoutThreads, 0, stream>>>(s);
+  return 1;
+}
+
+int launch_batch_cast_rays(const BatchRayArgs& s, cudaStream_t stream) {
+  batch_cast_rays_kernel<<<s.ctas, kRayThreads, 0, stream>>>(s);
   return 1;
 }
 

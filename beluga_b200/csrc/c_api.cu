@@ -350,6 +350,11 @@ int bb200_filter_sample_states(bb200_filter* f, uint64_t count, uint32_t step, d
   BB_REQUIRE(f);
   return guarded(f->impl, [&] { return f->impl.sample_states(count, step, states_out); });
 }
+int bb200_filter_cast_rays(bb200_filter* f, const double* poses, uint64_t n_poses, const double* bearings_cs, uint64_t n_bearings, double max_range,
+                           double* ranges) {
+  BB_REQUIRE(f);
+  return guarded(f->impl, [&] { return f->impl.cast_rays(poses, n_poses, bearings_cs, n_bearings, max_range, ranges); });
+}
 
 namespace {
 // detail::alphaHueToRGBA (beluga_ros/particle_cloud.hpp:56-70): single-precision HSV -> RGB for V = S = 1.
@@ -569,6 +574,25 @@ int bb200_amcl_update_scan(bb200_amcl* a, const double control_pose[4], const bb
     if (st != BB200_OK) return st;
     return bb200_amcl_update(a, control_pose, points.data(), n, out);
   });
+}
+
+int bb200_scan_bearings(float angle_min, float angle_increment, uint64_t n_ranges, uint64_t max_beams, double* bearings_cs, uint64_t capacity,
+                        uint64_t* n) {
+  BB_REQUIRE(n && (bearings_cs || capacity == 0));
+  bb200_laser_scan scan{};
+  scan.n_ranges = n_ranges;
+  scan.angle_min = angle_min;
+  scan.angle_increment = angle_increment;
+  scan.max_beams = max_beams;
+  const uint64_t kept = bb200::scan_beam_count(scan);
+  *n = kept;
+  if (kept > capacity) return BB200_ERR_CAPACITY;
+  for (uint64_t pos = 0; pos < kept; ++pos) {
+    const bb200::ScanBeam beam = bb200::scan_beam(scan, pos);
+    bearings_cs[2 * pos] = beam.c;
+    bearings_cs[2 * pos + 1] = beam.s;
+  }
+  return BB200_OK;
 }
 
 int bb200_point_cloud_to_points(const bb200_point_cloud* cloud, double* points_xy, uint64_t capacity, uint64_t* n_points) {
@@ -911,6 +935,11 @@ int bb200_amcl_batch_update_clustered(bb200_amcl_batch* b, const double* control
                                       uint32_t* n_cells, uint32_t* n_clusters) {
   BB_REQUIRE(b && control_poses && measurements && p && out && clustered);
   return guarded(b->impl, [&] { return b->impl.update_clustered(control_poses, measurements, present, *p, out, clustered, n_cells, n_clusters); });
+}
+int bb200_amcl_batch_cast_rays(bb200_amcl_batch* b, const uint8_t* present, const int* map_ids, const double* const* poses, const uint64_t* n_poses,
+                               const double* const* bearings_cs, const uint64_t* n_bearings, const double* max_range, double* const* ranges) {
+  BB_REQUIRE(b && poses && n_poses && bearings_cs && n_bearings && max_range && ranges);
+  return guarded(b->impl, [&] { return b->impl.cast_rays(present, map_ids, poses, n_poses, bearings_cs, n_bearings, max_range, ranges); });
 }
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.launch_count() : 0; }
 int bb200_amcl_batch_add_member(bb200_amcl_batch* b, const bb200_amcl_param* params, const bb200_motion_param* motion, int* member) {

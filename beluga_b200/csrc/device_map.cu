@@ -32,6 +32,7 @@ int prepare_likelihood_field_map(const bb200_likelihood_field_param& p, const bb
   if (!(p.sigma_hit > 0.0) || !(p.max_laser_distance > 0.0)) return reject(BB200_ERR_INVALID_ARGUMENT, "invalid likelihood field parameters", error);
   const char* too_large = "map too large for 32-bit cell indices";
   t->field_host = make_likelihood_field(p, g);
+  t->ray_grid.assign(g.cells, g.cells + static_cast<size_t>(g.width) * static_cast<size_t>(g.height));
   const size_t count = t->field_host.size();
   if (count + 64 >= (1ull << 32)) return reject(BB200_ERR_CAPACITY, too_large, error);
   // The lookup table the reweight kernel gathers from: f(pz) per cell as double, f = pz^3 (LikelihoodFieldModel) or
@@ -117,6 +118,7 @@ bool beam_two_pass_map(const MapLayout& map) {
 
 void DeviceMap::release() {
   tables_ = Tables{};
+  ray_ = RayTables{};
   static_cast<MapLayout&>(*this) = MapLayout{};
   field_host.clear();
   free_cells = nullptr;
@@ -161,7 +163,37 @@ int DeviceMap::upload(const MapTables& t, cudaStream_t stream, std::string* erro
   }
   BB_CHECK(cudaStreamSynchronize(stream));  // the host tables may go once this returns
   field_host = t.field_host;
+  ray_.grid = t.ray_grid;
   sensor = t.sensor;
+  return BB200_OK;
+}
+
+int DeviceMap::ray_view(cudaStream_t stream, OccupancyView* view, std::string* error) {
+  auto check = [error](cudaError_t e, const char* what) { return cuda_check(e, what, error); };
+  if (sensor < 0) return reject(BB200_ERR_STATE, "no map", error);
+  if (sensor == BB200_SENSOR_BEAM) {
+    *view = occupancy;
+    return BB200_OK;
+  }
+  if (ray_.free_distance.get() == nullptr) {
+    const bb200_occupancy_grid g{ray_.grid.data(), grid_width, grid_height, grid_resolution, {grid_origin.c, grid_origin.s, grid_origin.x, grid_origin.y}};
+    const std::vector<uint8_t> free_distance = make_free_distance(g);
+    DeviceBuffer<uint8_t> table;
+    BB_CHECK(table.allocate(free_distance.size()));
+    // pageable source: staged before the call returns, and the launch that reads the table follows the copy on `stream`
+    BB_CHECK(cudaMemcpyAsync(table.get(), free_distance.data(), free_distance.size(), cudaMemcpyHostToDevice, stream));
+    OccupancyView& v = ray_.view;
+    v = OccupancyView{};
+    v.free_distance = table.get();
+    v.width = grid_width;
+    v.height = grid_height;
+    v.resolution = grid_resolution;
+    v.inv_resolution = 1. / grid_resolution;
+    v.world_to_grid = pose_inverse(grid_origin);
+    ray_.free_distance = std::move(table);
+    ray_.grid = std::vector<int8_t>{};  // the table is made from it once
+  }
+  *view = ray_.view;
   return BB200_OK;
 }
 

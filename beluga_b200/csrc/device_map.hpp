@@ -35,6 +35,7 @@ struct MapTables : MapLayout {
   std::vector<uint8_t> free_distance;
   std::vector<uint8_t> free_padded;
   std::vector<uint32_t> free_cells;  // recovery injection and initialize_from_map
+  std::vector<int8_t> ray_grid;      // likelihood-field models: the grid, kept for ray casts (DeviceMap::ray_view)
 };
 
 /// Host preparation of a likelihood-field map (LikelihoodFieldModel, or LikelihoodFieldProbModel when prob).  Returns a
@@ -59,6 +60,10 @@ struct DeviceMap : MapLayout {
   /// The middle of the map in the global frame: the pivot of the raw moments after initialize_from_map.
   void centre(double pivot[2]) const;
   uint64_t launches() const { return launches_; }  // the beam model's normaliser tables
+  /// The occupancy view ray casts walk (raycast.cuh): the beam model's own, or, for a likelihood-field map, one made the
+  /// first time it is asked for: the free-distance map is built on the host from the grid kept at upload and copied on
+  /// `stream`, with no launch.  BB200_ERR_STATE without a map.
+  int ray_view(cudaStream_t stream, OccupancyView* view, std::string* error);
 
   std::vector<float> field_host;
   const uint32_t* free_cells{nullptr};
@@ -76,6 +81,14 @@ struct DeviceMap : MapLayout {
     DeviceBuffer<double2> eta;  // beam model: normaliser table
   };
   Tables tables_;
+  // Ray casts on a likelihood-field map, apart from tables_ so that upload copies exactly what the sensor model reads: the
+  // grid until the first cast, then the free-distance map on the device and its view.
+  struct RayTables {
+    std::vector<int8_t> grid;
+    DeviceBuffer<uint8_t> free_distance;
+    OccupancyView view{};
+  };
+  RayTables ray_;
   uint64_t launches_{0};
 };
 

@@ -971,6 +971,30 @@ int Filter::sample_states(uint64_t count, uint32_t step, double* states_out) {
   return BB200_OK;
 }
 
+int Filter::cast_rays(const double* poses, uint64_t n_poses, const double* bearings, uint64_t n_bearings, double max_range, double* ranges) {
+  if (map_.sensor < 0) return fail(BB200_ERR_STATE, "no map");
+  uint64_t n_rays = 0;
+  if (!cast_ray_count(n_poses, n_bearings, &n_rays)) return fail(BB200_ERR_INVALID_ARGUMENT, "n_poses * n_bearings overflows");
+  if ((poses == nullptr && n_poses > 0) || (bearings == nullptr && n_bearings > 0) || (ranges == nullptr && n_rays > 0))
+    return fail(BB200_ERR_INVALID_ARGUMENT, "null array with a non-zero count");
+  if (n_rays == 0) return BB200_OK;
+  if (n_rays > kMaxCastRays) return fail(BB200_ERR_CAPACITY, "too many rays for one launch");
+  BB_CHECK(cudaSetDevice(config_.device));
+  OccupancyView grid;
+  if (const int st = map_.ray_view(stream_, &grid, &error_)) return st;
+  const uint64_t pose_doubles = 4 * n_poses, bearing_doubles = 2 * n_bearings;
+  BB_CHECK(rays_.grow(pose_doubles + bearing_doubles + n_rays));  // every cast ends synchronised: no launch reads the old buffer
+  double* d = rays_.get();
+  BB_CHECK(cudaMemcpyAsync(d, poses, pose_doubles * sizeof(double), cudaMemcpyHostToDevice, stream_));
+  BB_CHECK(cudaMemcpyAsync(d + pose_doubles, bearings, bearing_doubles * sizeof(double), cudaMemcpyHostToDevice, stream_));
+  double* out = d + pose_doubles + bearing_doubles;
+  launch_cast_rays(grid, reinterpret_cast<const Pose2*>(d), reinterpret_cast<const double2*>(d + pose_doubles), n_bearings, n_rays, max_range, out, stream_);
+  BB_LAUNCHED("cast_rays");
+  BB_CHECK(cudaMemcpyAsync(ranges, out, n_rays * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+  BB_CHECK(cudaStreamSynchronize(stream_));
+  return BB200_OK;
+}
+
 ResampleArgs Filter::make_resample_args(const bb200_resample_opts& o, uint64_t slot_begin, uint64_t slot_end, bool with_hashes) const {
   ResampleArgs a{};
   a.states_in = states_[cur_].get();

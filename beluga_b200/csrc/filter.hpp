@@ -75,6 +75,10 @@ class Filter {
                          double* max_bin_weight);
   /// `count` states drawn by weight without touching the set (views::sample | take_exactly, particle_cloud.hpp:141-147).
   int sample_states(uint64_t count, uint32_t step, double* states_out);
+  /// Ray2d::cast (algorithm/raycasting.hpp:79-107) on the current map for n_poses sensor poses {cos, sin, x, y} (map frame)
+  /// and n_bearings bearings {cos, sin}, pose major: ranges[i * n_bearings + j] = min(distance, max_range) on a hit, +inf on
+  /// a miss.  One launch and one synchronisation (none without rays); the particle set is not touched.
+  int cast_rays(const double* poses, uint64_t n_poses, const double* bearings, uint64_t n_bearings, double max_range, double* ranges);
 
   /// Fused single-GPU step: propagate | reweight | normalize | resample | estimate with one
   /// host synchronisation at the end (the composition Amcl::update performs every step).
@@ -242,6 +246,7 @@ class Filter {
   DeviceBuffer<unsigned long long> sched_tiles_;
 
   DeviceMap map_;
+  DeviceBuffer<double> rays_;  // ray casts (grown on use): the poses, the bearings, then the ranges
   DeviceBuffer<uint32_t> beam_hits_;  // two-pass beam model: hit word per (beam, particle) of one pass
 
   double pivot_[2]{0.0, 0.0};

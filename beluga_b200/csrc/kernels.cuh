@@ -13,6 +13,7 @@
 //   resample.cu           a10 + a11 + a13: one thread per output slot (or per particle, scatter form); counter draw,
 //                         CDF search, 32-byte state gather, w = 1, per-block raw moments for a14; normalise;
 //                         reduce_partials: fixed-order sum of the per-block moments
+//   raycast.cu            Ray2d::cast for given sensor poses and bearings (no step stage: what a caller asks of a map)
 //   batch_kernels.cu      the same stages for a batch of filters, one CTA range per member
 //   shard_exchange.cu     step scalars exchanged between the shards of one filter
 //
@@ -611,6 +612,43 @@ struct BatchSampleArgs {
 int launch_batch_sample(const BatchSampleArgs& args, cudaStream_t stream);
 /// CTAs of a member in each row of a sample call's ranges (rebuilt: whether its CDF is rebuilt in the call).
 void batch_sample_ctas(const BatchSampleMember& m, bool rebuilt, uint32_t out[kSampleLaunches]);
+
+// ---- ray casts: Ray2d::cast (algorithm/raycasting.hpp:79-107) for n_poses x n_bearings rays ---------------------------
+// One thread per ray, pose major (ray i * n_bearings + j: pose i, bearing j), over the beam model's ray walk
+// (reweight_beam.cuh) on an OccupancyView.  ranges[ray] = min(distance, max_range) on a hit, +inf on a miss.
+
+/// Most rays of one launch (2^31 - 1 CTAs of 256 threads).
+constexpr uint64_t kMaxCastRays = 0x7FFFFFFFull * 256;
+/// n_poses * n_bearings in *n_rays; false when the product overflows.
+inline bool cast_ray_count(uint64_t n_poses, uint64_t n_bearings, uint64_t* n_rays) {
+  if (n_bearings != 0 && n_poses > UINT64_MAX / n_bearings) return false;
+  *n_rays = n_poses * n_bearings;
+  return true;
+}
+/// CTAs of n_rays rays (n_rays <= kMaxCastRays).
+uint32_t cast_rays_ctas(uint64_t n_rays);
+void launch_cast_rays(const OccupancyView& grid, const Pose2* poses, const double2* bearings, uint64_t n_bearings, uint64_t n_rays, double max_range,
+                      double* ranges, cudaStream_t stream);
+/// One member of a batch's ray casts (built on the host every call).
+struct BatchRayMember {
+  OccupancyView grid;       // the map it casts on
+  uint64_t pose_offset;     // first pose in BatchRayArgs::poses
+  uint64_t bearing_offset;  // first bearing in BatchRayArgs::bearings
+  uint64_t ray_offset;      // first range in BatchRayArgs::ranges
+  uint64_t n_bearings, n_rays;
+  double max_range;
+};
+struct BatchRayArgs {
+  const BatchRayMember* members;  // device
+  const uint32_t* first;          // device: n_members + 1 CTA prefixes (cast_rays_ctas of each member's rays)
+  uint32_t n_members;
+  uint32_t ctas;
+  const Pose2* poses;
+  const double2* bearings;
+  double* ranges;
+};
+/// Every member of the table in one launch; returns the number of launches (1).
+int launch_batch_cast_rays(const BatchRayArgs& args, cudaStream_t stream);
 
 // ---- batches: members that join and leave ------------------------------------------------------------------
 /// One surviving member of a membership change: the live part of its slice, moved from the old buffers to the new ones.

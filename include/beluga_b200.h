@@ -308,6 +308,17 @@ int bb200_filter_particle_histogram(bb200_filter* f, double linear_resolution, d
  * (views::sample | take_exactly) -- multinomial counter-RNG draws of `step` -- into states_out (count x {cos, sin, x, y});
  * the particle set is not modified. */
 int bb200_filter_sample_states(bb200_filter* f, uint64_t count, uint32_t step, double* states_out);
+/* Ray2d::cast (algorithm/raycasting.hpp:79-107, standard Bresenham) on the filter's current map, whichever sensor model it
+ * is for: n_poses sensor poses {cos, sin, x, y} in the map frame times n_bearings bearings {cos, sin}, taken as given
+ * (SO2::raw: not normalised; the library computes no trigonometry).  ranges receives n_poses x n_bearings doubles, pose
+ * major (ray i * n_bearings + j is pose i, bearing j): min(distance, max_range) where the ray hits a non-free cell, +inf
+ * where Ray2d::cast returns std::nullopt.  max_range is any double, as Ray2d takes it; a NaN makes every ray a miss.  One
+ * kernel launch and one host synchronisation (none when there are no rays); the particle set is not touched.  A
+ * likelihood-field map's first cast also builds the map's free-distance table on the host and uploads it (no launch); a
+ * map that is never cast keeps only its likelihood field on the device.  BB200_ERR_STATE without a map,
+ * BB200_ERR_INVALID_ARGUMENT for a null array with a non-zero count or when n_poses * n_bearings overflows. */
+int bb200_filter_cast_rays(bb200_filter* f, const double* poses, uint64_t n_poses, const double* bearings_cs, uint64_t n_bearings, double max_range,
+                           double* ranges);
 /* Host only.  The marker geometry of assign_particle_cloud(..., MarkerArray) (particle_cloud.hpp:212-294) from the
  * histogram bins: 2 vertices per bin for the LINE_LIST "bodies" marker, 3 per bin for the TRIANGLE_LIST "heads"
  * marker, each with its RGBA colour (detail::alphaHueToRGBA, :56-70), and arrow_bodies.scale.x. */
@@ -428,6 +439,12 @@ typedef struct bb200_laser_scan {
 } bb200_laser_scan;
 /* Writes at most `capacity` points (x, y pairs) and their count. */
 int bb200_scan_to_points(const bb200_laser_scan* scan, double* points_xy, uint64_t capacity, uint64_t* n_points);
+/* Host only.  The directions {cos, sin} of the beams a bb200_laser_scan with these fields keeps (take_evenly(max_beams)),
+ * computed exactly as bb200_scan_to_points computes them, without dropping any reading by its range: the bearings of a
+ * scan geometry's expected scan (bb200_filter_cast_rays).  *n receives the count; BB200_ERR_CAPACITY, with nothing
+ * written, when it exceeds capacity (bearings_cs may be NULL with capacity 0 to query it). */
+int bb200_scan_bearings(float angle_min, float angle_increment, uint64_t n_ranges, uint64_t max_beams, double* bearings_cs, uint64_t capacity,
+                        uint64_t* n);
 /* take_evenly (beluga/views/take_evenly.hpp:118-145): the indices kept out of `size` elements. */
 int bb200_take_evenly_indices(uint64_t size, uint64_t count, uint64_t* indices, uint64_t capacity, uint64_t* n_indices);
 /* Amcl::update(base_pose_in_odom, laser_scan) -- beluga_ros/src/amcl.cpp:54-64. */
@@ -661,6 +678,16 @@ int bb200_amcl_batch_particle_histograms(bb200_amcl_batch* b, double linear_reso
  * counts[m] exceeds its max_particles, and BB200_ERR_INVALID_ARGUMENT for a null handle, counts or states_out, or a null
  * states_out[m] with counts[m] > 0. */
 int bb200_amcl_batch_sample_states(bb200_amcl_batch* b, const uint64_t* counts, uint32_t step, const uint8_t* present, double* const* states_out);
+/* bb200_filter_cast_rays for every member m with present[m] != 0 (present NULL: every occupied slot): n_poses[m] x
+ * n_bearings[m] rays from poses[m] along bearings_cs[m] up to max_range[m] into ranges[m], on member m's own map, or on
+ * map map_ids[m] of the batch when map_ids is not NULL and map_ids[m] != -1 (e.g. a simulator's world map).  Every
+ * member's ranges are bit-identical to bb200_filter_cast_rays on the same map.  One kernel launch and one host
+ * synchronisation whatever K, the maps and the ray counts are (none when no selected member has a ray).  Refused before
+ * anything reaches the device, with the batch unchanged: a vacant selected slot, an unknown or removed map id, a null
+ * array with a non-zero count or an overflowing n_poses[m] * n_bearings[m] (BB200_ERR_INVALID_ARGUMENT), and a selected
+ * member without a map and no map id (BB200_ERR_STATE).  No member is modified. */
+int bb200_amcl_batch_cast_rays(bb200_amcl_batch* b, const uint8_t* present, const int* map_ids, const double* const* poses, const uint64_t* n_poses,
+                               const double* const* bearings_cs, const uint64_t* n_bearings, const double* max_range, double* const* ranges);
 /* Amcl::update for every member m with present[m] != 0 (present NULL: all members).  control_poses holds K poses of 4
  * doubles, points_xy[m] member m's n_points[m] (x, y) pairs (NULL when n_points[m] == 0), out[m] its result.  An absent
  * member is left untouched -- no policy is evaluated -- and gets out[m].updated = 0.  Present members go through their
@@ -711,7 +738,7 @@ int bb200_amcl_batch_update_clustered(bb200_amcl_batch* b, const double* control
                                       const uint8_t* present, const bb200_cluster_param* p, bb200_update_result* out,
                                       bb200_estimate* clustered, uint32_t* n_cells, uint32_t* n_clusters);
 /* Kernel launches issued by this batch so far (steps, initialisations, cluster estimates, particle-cloud histograms and
- * pose samples, membership changes, and the beam model's map uploads). */
+ * pose samples, ray casts, membership changes, and the beam model's map uploads). */
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b);
 
 /* Members that join and leave a running batch (a fleet server whose robots connect, disconnect and reconnect with new

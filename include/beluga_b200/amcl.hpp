@@ -15,7 +15,9 @@
 #pragma once
 
 #include <algorithm>
+#include <array>
 #include <execution>
+#include <limits>
 #include <map>
 #include <optional>
 #include <utility>
@@ -103,6 +105,33 @@ struct ParticleSet {
   [[nodiscard]] std::size_t size() const { return states.size(); }
   [[nodiscard]] bool empty() const { return states.empty(); }
 };
+
+/// A bearing {cos, sin} of a ray cast, taken as given (Sophus::SO2d's unit complex, not normalised).
+using Bearing = std::array<double, 2>;
+
+/// The directions of the beams a laser scan of this geometry keeps (take_evenly(max_beams), beluga_ros/laser_scan.hpp:69-80),
+/// computed as bb200_scan_to_points computes them and without dropping readings by range (bb200_scan_bearings): the
+/// bearings of the scan a sensor at some pose is expected to see (Amcl::cast_rays).
+inline std::vector<Bearing> scan_bearings(float angle_min, float angle_increment, std::uint64_t n_ranges, std::uint64_t max_beams = 0) {
+  std::uint64_t n = 0;
+  int st = bb200_scan_bearings(angle_min, angle_increment, n_ranges, max_beams, nullptr, 0, &n);
+  if (st != BB200_OK && st != BB200_ERR_CAPACITY) throw Error(st, "bb200_scan_bearings");
+  std::vector<Bearing> out(n);
+  static_assert(sizeof(Bearing) == 2 * sizeof(double), "bearings must be packed");
+  st = bb200_scan_bearings(angle_min, angle_increment, n_ranges, max_beams, n > 0 ? out.front().data() : nullptr, n, &n);
+  if (st != BB200_OK) throw Error(st, "bb200_scan_bearings");
+  return out;
+}
+
+namespace detail {
+/// The ranges of a ray cast as Ray2d::cast returns them: +inf (a miss) becomes std::nullopt.
+inline std::vector<std::optional<double>> cast_results(const double* ranges, std::size_t n) {
+  std::vector<std::optional<double>> out(n);
+  for (std::size_t i = 0; i < n; ++i)
+    if (ranges[i] != std::numeric_limits<double>::infinity()) out[i] = ranges[i];
+  return out;
+}
+}  // namespace detail
 
 template <class MotionModel, class SensorModel, class ExecutionPolicy = std::execution::sequenced_policy>
 class Amcl {
@@ -207,6 +236,17 @@ class Amcl {
 
   /// amcl_core.hpp:204
   void force_update() { bb200_amcl_force_update(handle_); }
+
+  /// Ray2d::cast (algorithm/raycasting.hpp:79-107) on the sensor model's map for every sensor pose (map frame) and bearing,
+  /// pose major: entry i * bearings.size() + j is what Ray2d{map, poses[i], max_range}.cast(bearings[j]) returns.  One
+  /// kernel launch (bb200_filter_cast_rays); the particle set is not touched.
+  [[nodiscard]] std::vector<std::optional<double>> cast_rays(const std::vector<state_type>& poses, const std::vector<Bearing>& bearings,
+                                                             double max_range) const {
+    std::vector<double> ranges(poses.size() * bearings.size());
+    check(bb200_filter_cast_rays(bb200_amcl_filter(handle_), poses.empty() ? nullptr : poses.front().data(), poses.size(),
+                                 bearings.empty() ? nullptr : bearings.front().data(), bearings.size(), max_range, ranges.empty() ? nullptr : ranges.data()));
+    return detail::cast_results(ranges.data(), ranges.size());
+  }
 
   [[nodiscard]] bb200_amcl* handle() const { return handle_; }
 
@@ -659,6 +699,37 @@ class AmclBatch {
     std::vector<std::optional<std::vector<double>>> out(k);
     for (std::size_t m = 0; m < k; ++m)
       if ((present == nullptr || (*present)[m]) && sizes_[m] != 0) out[m] = std::move(raw[m]);
+    return out;
+  }
+
+  /// Amcl::cast_rays for every member whose present[m] is true (present == nullptr: every occupied slot): poses[m] x
+  /// bearings[m] rays up to max_range[m], pose major, on the member's own map or on map (*map_ids)[m] of the batch when
+  /// map_ids is set and that entry is not -1; std::nullopt for members not selected.  One kernel launch whatever K is
+  /// (bb200_amcl_batch_cast_rays); no member changes.
+  [[nodiscard]] auto cast_rays(const std::vector<std::vector<SE2d>>& poses, const std::vector<std::vector<Bearing>>& bearings,
+                               const std::vector<double>& max_range, const std::vector<bool>* present = nullptr,
+                               const std::vector<int>* map_ids = nullptr) const -> std::vector<std::optional<std::vector<std::optional<double>>>> {
+    const std::vector<std::uint8_t> mask = presence_mask(present);
+    const std::size_t k = size();
+    if (poses.size() != k || bearings.size() != k || max_range.size() != k || (map_ids != nullptr && map_ids->size() != k))
+      throw Error(BB200_ERR_INVALID_ARGUMENT, "one pose list, bearing list, maximum range and map id per member");
+    std::vector<std::vector<double>> raw(k);
+    std::vector<const double*> p(k, nullptr), b(k, nullptr);
+    std::vector<double*> r(k, nullptr);
+    std::vector<std::uint64_t> np(k), nb(k);
+    for (std::size_t m = 0; m < k; ++m) {
+      np[m] = poses[m].size();
+      nb[m] = bearings[m].size();
+      p[m] = poses[m].empty() ? nullptr : poses[m].front().data();
+      b[m] = bearings[m].empty() ? nullptr : bearings[m].front().data();
+      raw[m].resize(poses[m].size() * bearings[m].size());
+      r[m] = raw[m].empty() ? nullptr : raw[m].data();
+    }
+    check(bb200_amcl_batch_cast_rays(handle_, present != nullptr ? mask.data() : nullptr, map_ids != nullptr ? map_ids->data() : nullptr, p.data(),
+                                     np.data(), b.data(), nb.data(), max_range.data(), r.data()));
+    std::vector<std::optional<std::vector<std::optional<double>>>> out(k);
+    for (std::size_t m = 0; m < k; ++m)
+      if ((present == nullptr || (*present)[m]) && sizes_[m] != 0) out[m] = detail::cast_results(raw[m].data(), raw[m].size());
     return out;
   }
 

@@ -12,6 +12,8 @@ max 2000) against K standalone KLD Amcl.  `batch_selective`: the `batch` workloa
 and KLD-adaptive (min 500, max 2000), against K standalone selective Amcl.  `batch_members`: add_member and remove_member at
 K = 16 and 256 members, alone and next to a 32 768-particle member, and a step after churn against the same step on a fresh batch.
 `batch_state`: export_members and AmclBatch.from_states (the fleet checkpoint and its restore) with the same members.
+`raycast`: device ray casts (Ray2d::cast) for 256 batch members x 1 pose x 1080 bearings and for 1M rays of one filter, against
+the CPU oracle's Ray2d on the same rays.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import ctypes
@@ -375,6 +377,81 @@ def run_batch_state():
                 "export_members_c_ms": float(np.median(c_export_ms)), "create_from_states_c_ms": float(np.median(c_create_ms)),
                 "launches_export_and_create": [int(x) for x in max(launches)], "repeats": repeats,
                 "ms_per_step_e2e": float(np.median(export_ms)), "kernels_ms": {}, "device": device}
+    return res
+
+
+def run_raycast():
+    """Ray casts on the 2000^2 synthetic map (likelihood-field map, 5 cm cells) at 30 m and 60 m: the expected scans of 256
+    batch members, one pose x 1080 bearings each (a fleet's health check, or a simulator's tick), in one
+    AmclBatch.cast_rays call; and 1M rays (1000 poses x 1000 bearings) through one bb200_filter_cast_rays.  Host clock around
+    each call (it ends synchronised; inputs and outputs cross PCIe inside it), median of `repeats` after one warm-up call that
+    also builds and uploads the map's free-distance table.  Beside them the CPU oracle's Ray2d::cast on the same rays, one
+    thread (tests/_raycast_oracle.py, -O3)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import _raycast_oracle  # noqa: E402
+
+    _raycast_oracle.lib()  # compiled before anything is timed
+
+    res = {}
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=100, steps=100)
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    lfm = bb.LikelihoodFieldModelParam(**LFM)
+    rng = np.random.default_rng(5)
+    device = device_record()
+    repeats = 20
+    bearings = bb.scan_bearings(-np.pi, 2 * np.pi / 1080, 1080)
+    k = 256
+    params = [bb.AmclParams(min_particles=500, max_particles=500, seed=m) for m in range(k)]
+    batch = bb.AmclBatch([bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)], params)
+    batch.set_likelihood_field_map(lfm, grid)
+    member_poses = [bb.se2(*sc.poses[rng.integers(0, 100)])[None] for _ in range(k)]
+    f = bb.Filter(capacity=16)
+    f.set_likelihood_field_map(lfm, grid)
+    poses_1m = np.stack([bb.se2(*sc.poses[i % 100]) for i in range(1000)])
+    bearings_1m = np.stack([[np.cos(t), np.sin(t)] for t in np.linspace(-np.pi, np.pi, 1000, endpoint=False)])
+    # The batch call through the C ABI into arrays built once: the library's share of the Python wrapper's time.
+    d = ctypes.POINTER(ctypes.c_double)
+    flat = np.ascontiguousarray(np.concatenate(member_poses))
+    ranges_c = np.zeros((k, 1080))
+    c_args = ((d * k)(*[flat[m:].ctypes.data_as(d) for m in range(k)]), (ctypes.c_uint64 * k)(*[1] * k),
+              (d * k)(*[bearings.ctypes.data_as(d)] * k), (ctypes.c_uint64 * k)(*[1080] * k),
+              (d * k)(*[ranges_c[m].ctypes.data_as(d) for m in range(k)]))
+
+    def batch_c(max_range):
+        p, n_p, b, n_b, r = c_args
+        assert batch._lib.bb200_amcl_batch_cast_rays(batch._h, None, None, p, n_p, b, n_b, (ctypes.c_double * k)(*[max_range] * k), r) == 0
+
+    for max_range in (30.0, 60.0):
+        batch_c(max_range)
+        c_ms = []
+        for _ in range(repeats):
+            t0 = time.perf_counter()
+            batch_c(max_range)
+            c_ms.append((time.perf_counter() - t0) * 1e3)
+        cases = (("batch_256_x_1_x_1080", lambda: batch.cast_rays(member_poses, bearings, max_range), batch.launch_count, k * 1080,
+                  np.concatenate(member_poses), bearings),
+                 ("filter_1000_x_1000", lambda: f.cast_rays(poses_1m, bearings_1m, max_range), f.launch_count, 1000 * 1000, poses_1m, bearings_1m))
+        for name, call, launches, rays, p, b in cases:
+            out = call()  # warm-up (the first call on this map builds its free-distance table)
+            times, counts = [], []
+            for _ in range(repeats):
+                before = launches()
+                t0 = time.perf_counter()
+                call()
+                times.append((time.perf_counter() - t0) * 1e3)
+                counts.append(launches() - before)
+            t0 = time.perf_counter()
+            want = _raycast_oracle.cast_rays(grid.cells, grid.resolution, grid.origin, p, b, max_range)
+            cpu_ms = (time.perf_counter() - t0) * 1e3
+            got = np.concatenate(out) if isinstance(out, list) else out
+            ms = float(np.median(times))
+            res[f"raycast_{name}_{int(max_range)}m_2000"] = {
+                "rays": rays, "ms_per_call": ms, "ms_per_call_min_max": [float(min(times)), float(max(times))],
+                "rays_per_s": rays / (ms * 1e-3), "launches_per_call": int(max(counts)), "repeats": repeats,
+                "hit_fraction": float(np.isfinite(got).mean()), "equal_to_oracle": bool(np.array_equal(got.reshape(want.shape), want)),
+                "cpu_oracle_ms_one_thread": cpu_ms, "cpu_oracle_rays_per_s": rays / (cpu_ms * 1e-3),
+                "ms_per_step_e2e": ms, "kernels_ms": {}, "device": device}
+        res[f"raycast_batch_256_x_1_x_1080_{int(max_range)}m_2000"]["ms_per_call_c"] = float(np.median(c_ms))
     return res
 
 
@@ -906,6 +983,8 @@ def main():
         out.update(run_batch_maps())
     if "batch_measurements" in which:
         out.update(run_batch_measurements())
+    if "raycast" in which:
+        out.update(run_raycast())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}

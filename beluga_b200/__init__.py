@@ -838,6 +838,48 @@ class ShardedAmcl:
         self._check(self._lib.bb200_sharded_amcl_cluster_estimate(self._h, C.byref(p), C.byref(est), C.byref(cells), C.byref(clusters)))
         return np.array(est.mean), np.array(est.cov).reshape(3, 3), cells.value, clusters.value
 
+    def update_scan(self, control_pose, ranges, angle_min: float, angle_increment: float, min_range: float = 0.0,
+                    max_range: float = float("inf"), max_beams: int = 0, laser_origin=None) -> _capi.UpdateResult:
+        """Amcl.update_scan over all shards (bb200_sharded_amcl_update_scan)."""
+        scan, keep = _laser_scan(ranges, angle_min, angle_increment, min_range, max_range, max_beams, laser_origin)
+        res = _capi.UpdateResult()
+        self._check(self._lib.bb200_sharded_amcl_update_scan(self._h, _dptr(_f64(control_pose)), C.byref(scan), C.byref(res)))
+        return res
+
+    def update_point_cloud(self, control_pose, data, point_step: int, x_offset: int, dtype, origin=None,
+                           n_points: int | None = None) -> _capi.UpdateResult:
+        """Amcl.update_point_cloud over all shards (bb200_sharded_amcl_update_point_cloud); arguments as point_cloud_to_points."""
+        cloud, keep = _point_cloud(data, point_step, x_offset, dtype, origin, n_points)
+        res = _capi.UpdateResult()
+        self._check(self._lib.bb200_sharded_amcl_update_point_cloud(self._h, _dptr(_f64(control_pose)), C.byref(cloud), C.byref(res)))
+        return res
+
+    def particle_histogram(self, linear: float = 1e-3, angular: float = 1e-3):
+        """Filter.particle_histogram over all shards, merged in rank order (bb200_sharded_amcl_particle_histogram).
+        -> (representatives [m, 4], weights [m], counts [m], first_index [m], max_bin_weight)."""
+        n_bins, top = C.c_uint64(0), C.c_double(0.0)
+        self._check(self._lib.bb200_sharded_amcl_particle_histogram(self._h, linear, angular, None, 0, C.byref(n_bins), C.byref(top)))
+        m = n_bins.value
+        arr = (_capi.ClusterCell * max(m, 1))()
+        self._check(self._lib.bb200_sharded_amcl_particle_histogram(self._h, linear, angular, arr, m, C.byref(n_bins), C.byref(top)))
+        raw = np.frombuffer(arr, dtype=_CELL_DTYPE, count=m)
+        return raw["rep"].copy(), raw["weight"].copy(), raw["count"].copy(), raw["first"].copy(), top.value
+
+    def sample_states(self, count: int, step: int = 0xFFFFFFFF) -> np.ndarray:
+        """Filter.sample_states over the global particle set (bb200_sharded_amcl_sample_states): the draws one filter holding
+        the same particles and weights returns, whatever the shard count."""
+        out = np.zeros((count, 4))
+        self._check(self._lib.bb200_sharded_amcl_sample_states(self._h, count, step, _dptr(out) if count else None))
+        return out
+
+    def cast_rays(self, poses, bearings, max_range: float) -> np.ndarray:
+        """Filter.cast_rays on the shards' copies of the map (bb200_sharded_amcl_cast_rays), the poses split over the devices."""
+        p, b = _rays(poses, bearings)
+        out = np.zeros((len(p), len(b)))
+        self._check(self._lib.bb200_sharded_amcl_cast_rays(self._h, _dptr(p) if len(p) else None, len(p), _dptr(b) if len(b) else None, len(b),
+                                                           max_range, _dptr(out) if out.size else None))
+        return out
+
     def particles(self):
         """The particle set in global index order (a KLD-sized filter holds fewer than max_particles)."""
         n = sum(f.size() for f in self.shards)

@@ -210,6 +210,11 @@ SIGNATURES = {
     "bb200_sharded_amcl_update": (C.c_int, [_vp, _dbl, _dbl, C.c_uint64, _P(UpdateResult)]),
     "bb200_sharded_amcl_get_particles": (C.c_int, [_vp, _dbl, _dbl, C.c_uint64]),
     "bb200_sharded_amcl_cluster_estimate": (C.c_int, [_vp, _P(ClusterParam), _P(Estimate), _P(C.c_uint32), _P(C.c_uint32)]),
+    "bb200_sharded_amcl_update_scan": (C.c_int, [_vp, _dbl, _P(LaserScan), _P(UpdateResult)]),
+    "bb200_sharded_amcl_update_point_cloud": (C.c_int, [_vp, _dbl, _P(PointCloud), _P(UpdateResult)]),
+    "bb200_sharded_amcl_particle_histogram": (C.c_int, [_vp, C.c_double, C.c_double, _P(ClusterCell), C.c_uint64, _P(C.c_uint64), _dbl]),
+    "bb200_sharded_amcl_sample_states": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _dbl]),
+    "bb200_sharded_amcl_cast_rays": (C.c_int, [_vp, _dbl, C.c_uint64, _dbl, C.c_uint64, C.c_double, _dbl]),
     "bb200_cluster_merge_host": (C.c_int, [_P(_P(ClusterCell)), _P(C.c_uint64), _P(C.c_uint64), C.c_int, _P(ClusterCell), C.c_uint64, _P(C.c_uint64)]),
     "bb200_amcl_export_shard": (C.c_int, [_vp, _vp]),
     "bb200_amcl_join_shards": (C.c_int, [_vp, C.c_int, C.c_int, _vp]),

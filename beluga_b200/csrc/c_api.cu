@@ -565,12 +565,27 @@ int bb200_scan_to_points(const bb200_laser_scan* scan, double* points_xy, uint64
   return BB200_OK;
 }
 
+namespace {
+/// The base-frame points an update takes from a laser scan (bb200_scan_to_points): the standalone and the sharded filter
+/// convert alike.
+int scan_points(const bb200_laser_scan& scan, std::vector<double>* points, uint64_t* n) {
+  points->assign(2 * (scan.n_ranges + 1), 0.0);
+  return bb200_scan_to_points(&scan, points->data(), scan.n_ranges + 1, n);
+}
+/// ... and from a point cloud (bb200_point_cloud_to_points).
+int cloud_points(const bb200_point_cloud& cloud, std::vector<double>* points, uint64_t* n) {
+  points->assign(2 * cloud.n_points, 0.0);
+  return bb200_point_cloud_to_points(&cloud, points->data(), cloud.n_points, n);
+}
+const char* const kCloudRefused = "point cloud: datatype must be 7 (FLOAT32) or 8 (FLOAT64), x, y and z must fit in point_step, data must be set";
+}  // namespace
+
 int bb200_amcl_update_scan(bb200_amcl* a, const double control_pose[4], const bb200_laser_scan* scan, bb200_update_result* out) {
   BB_REQUIRE(a && control_pose && scan && out);
   return guarded(a->impl, [&] {
-    std::vector<double> points(2 * (scan->n_ranges + 1));
+    std::vector<double> points;
     uint64_t n = 0;
-    const int st = bb200_scan_to_points(scan, points.data(), scan->n_ranges + 1, &n);
+    const int st = scan_points(*scan, &points, &n);
     if (st != BB200_OK) return st;
     return bb200_amcl_update(a, control_pose, points.data(), n, out);
   });
@@ -611,11 +626,11 @@ int bb200_point_cloud_to_points(const bb200_point_cloud* cloud, double* points_x
 int bb200_amcl_update_point_cloud(bb200_amcl* a, const double control_pose[4], const bb200_point_cloud* cloud, bb200_update_result* out) {
   BB_REQUIRE(a && control_pose && cloud && out);
   return guarded(a->impl, [&] {
-    std::vector<double> points(2 * cloud->n_points);
+    std::vector<double> points;
     uint64_t n = 0;
-    const int st = bb200_point_cloud_to_points(cloud, points.data(), cloud->n_points, &n);
+    const int st = cloud_points(*cloud, &points, &n);
     if (st != BB200_OK) {
-      a->impl.record_error("point cloud: datatype must be 7 (FLOAT32) or 8 (FLOAT64), x, y and z must fit in point_step, data must be set");
+      a->impl.record_error(kCloudRefused);
       return st;
     }
     return bb200_amcl_update(a, control_pose, points.data(), n, out);
@@ -738,6 +753,9 @@ int bb200_cluster_merge_host(const bb200_cluster_cell* const* shard_cells, const
     // ITS first-occurrence order -- visits the cells in the global first-occurrence order; a cell met again adds its count,
     // weight and raw moments to the record opened by the lower rank (whose representative is the globally first particle).
     std::unordered_map<uint64_t, uint64_t> slot_of;
+    uint64_t listed = 0;
+    for (int r = 0; r < shards; ++r) listed += shard_counts[r];
+    slot_of.reserve(listed);  // no rehash while the map grows to the merged count
     uint64_t n = 0;
     for (int r = 0; r < shards; ++r) {
       for (uint64_t k = 0; k < shard_counts[r]; ++k) {
@@ -763,46 +781,58 @@ int bb200_cluster_merge_host(const bb200_cluster_cell* const* shard_cells, const
   });
 }
 
+namespace {
+/// Every shard's cell records (Filter::cell_records, one device pass per shard) merged in rank order
+/// (bb200_cluster_merge_host): the cells of the whole particle set in its global first-occurrence order.  BB200_ERR_STATE
+/// when no shard holds a particle.
+int merged_cells(bb200_sharded_amcl* g, double linear_resolution, double angular_resolution, std::vector<bb200_cluster_cell>* merged,
+                 uint64_t* n_particles) {
+  static_assert(sizeof(bb200_cluster_cell) == sizeof(bb200::HostCell), "public and internal cell records must agree");
+  const int shards = static_cast<int>(g->ranks.size());
+  std::vector<std::vector<bb200::HostCell>> cells(static_cast<size_t>(shards));
+  std::vector<const bb200_cluster_cell*> ptrs;
+  std::vector<uint64_t> counts, firsts;
+  uint64_t total_cells = 0;
+  *n_particles = 0;
+  for (int r = 0; r < shards; ++r) {
+    Filter& f = g->ranks[static_cast<size_t>(r)]->impl.filter();
+    std::vector<bb200::HostCell>& c = cells[static_cast<size_t>(r)];
+    if (f.size() > 0)
+      if (const int st = f.cell_records(linear_resolution, angular_resolution, &c)) return st;
+    const uint64_t n = c.size();
+    ptrs.push_back(reinterpret_cast<const bb200_cluster_cell*>(c.data()));
+    counts.push_back(n);
+    firsts.push_back(f.first_index());
+    total_cells += n;
+    *n_particles += f.size();
+  }
+  if (*n_particles == 0) {
+    g->error = "no particles";
+    return static_cast<int>(BB200_ERR_STATE);
+  }
+  merged->resize(total_cells);
+  uint64_t n_merged = 0;
+  const int st = bb200_cluster_merge_host(ptrs.data(), counts.data(), firsts.data(), shards, merged->data(), merged->size(), &n_merged);
+  if (st != BB200_OK) return st;
+  merged->resize(n_merged);
+  return static_cast<int>(BB200_OK);
+}
+}  // namespace
+
 int bb200_sharded_amcl_cluster_estimate(bb200_sharded_amcl* g, const bb200_cluster_param* p, bb200_estimate* out, uint32_t* n_cells,
                                         uint32_t* n_clusters) {
   BB_REQUIRE(g && p && out);
   g->error.clear();
   return guarded(*g, [&] {
-    const int shards = static_cast<int>(g->ranks.size());
-    std::vector<std::vector<bb200_cluster_cell>> cells(static_cast<size_t>(shards));
-    std::vector<const bb200_cluster_cell*> ptrs;
-    std::vector<uint64_t> counts, firsts;
-    uint64_t total_cells = 0, n_particles = 0;
-    for (int r = 0; r < shards; ++r) {
-      Filter& f = g->ranks[static_cast<size_t>(r)]->impl.filter();
-      uint64_t n = 0;
-      double top = 0.0;
-      if (f.size() > 0) {
-        int st = f.particle_histogram(p->linear_hash_resolution, p->angular_hash_resolution, nullptr, 0, &n, &top);
-        if (st != BB200_OK) return st;
-        cells[static_cast<size_t>(r)].resize(n);
-        st = f.particle_histogram(p->linear_hash_resolution, p->angular_hash_resolution, cells[static_cast<size_t>(r)].data(), n, &n, &top);
-        if (st != BB200_OK) return st;
-      }
-      ptrs.push_back(cells[static_cast<size_t>(r)].data());
-      counts.push_back(n);
-      firsts.push_back(f.first_index());
-      total_cells += n;
-      n_particles += f.size();
-    }
-    if (n_particles == 0) {
-      g->error = "no particles";
-      return static_cast<int>(BB200_ERR_STATE);
-    }
-    std::vector<bb200_cluster_cell> merged(total_cells);
-    uint64_t n_merged = 0;
-    const int st = bb200_cluster_merge_host(ptrs.data(), counts.data(), firsts.data(), shards, merged.data(), merged.size(), &n_merged);
+    std::vector<bb200_cluster_cell> merged;
+    uint64_t n_particles = 0;
+    const int st = merged_cells(g, p->linear_hash_resolution, p->angular_hash_resolution, &merged, &n_particles);
     if (st != BB200_OK) return st;
     static_assert(sizeof(bb200_cluster_cell) == sizeof(bb200::HostCell), "public and internal cell records must agree");
-    const bb200::ClusterSelection sel = bb200::select_cluster(reinterpret_cast<const bb200::HostCell*>(merged.data()), n_merged, n_particles,
+    const bb200::ClusterSelection sel = bb200::select_cluster(reinterpret_cast<const bb200::HostCell*>(merged.data()), merged.size(), n_particles,
                                                               p->linear_hash_resolution, p->angular_hash_resolution, p->weight_cap_percentile);
     bb200::estimate_from_moments(sel.moments, g->ranks[0]->impl.filter().pivot(), out);  // every shard accumulates about the same pivot
-    if (n_cells != nullptr) *n_cells = static_cast<uint32_t>(n_merged);
+    if (n_cells != nullptr) *n_cells = static_cast<uint32_t>(merged.size());
     if (n_clusters != nullptr) *n_clusters = sel.clusters;
     return static_cast<int>(BB200_OK);
   });
@@ -820,6 +850,156 @@ int bb200_sharded_amcl_get_particles(bb200_sharded_amcl* g, double* states, doub
       if (st != BB200_OK) return st;
       done += n;
       if (done >= capacity) break;
+    }
+    return static_cast<int>(BB200_OK);
+  });
+}
+
+int bb200_sharded_amcl_update_scan(bb200_sharded_amcl* g, const double control_pose[4], const bb200_laser_scan* scan, bb200_update_result* out) {
+  BB_REQUIRE(g && control_pose && scan && out);
+  g->error.clear();
+  return guarded(*g, [&] {
+    std::vector<double> points;
+    uint64_t n = 0;
+    const int st = scan_points(*scan, &points, &n);
+    if (st != BB200_OK) return st;
+    return bb200_sharded_amcl_update(g, control_pose, points.data(), n, out);
+  });
+}
+
+int bb200_sharded_amcl_update_point_cloud(bb200_sharded_amcl* g, const double control_pose[4], const bb200_point_cloud* cloud,
+                                          bb200_update_result* out) {
+  BB_REQUIRE(g && control_pose && cloud && out);
+  g->error.clear();
+  return guarded(*g, [&] {
+    std::vector<double> points;
+    uint64_t n = 0;
+    const int st = cloud_points(*cloud, &points, &n);
+    if (st != BB200_OK) {
+      g->error = kCloudRefused;
+      return st;
+    }
+    return bb200_sharded_amcl_update(g, control_pose, points.data(), n, out);
+  });
+}
+
+int bb200_sharded_amcl_particle_histogram(bb200_sharded_amcl* g, double linear_resolution, double angular_resolution, bb200_cluster_cell* bins,
+                                          uint64_t capacity, uint64_t* n_bins, double* max_bin_weight) {
+  BB_REQUIRE(g);
+  g->error.clear();
+  return guarded(*g, [&] {
+    std::vector<bb200_cluster_cell> merged;
+    uint64_t n_particles = 0;
+    const int st = merged_cells(g, linear_resolution, angular_resolution, &merged, &n_particles);
+    if (st != BB200_OK) return st;
+    if (n_bins != nullptr) *n_bins = merged.size();
+    double top = 1e-3;  // beluga_ros/particle_cloud.hpp:197
+    for (const bb200_cluster_cell& c : merged) top = c.weight > top ? c.weight : top;
+    if (max_bin_weight != nullptr) *max_bin_weight = top;
+    if (bins != nullptr) {
+      if (capacity < merged.size()) {
+        g->error = "histogram bin buffer too small (n_bins has the count)";
+        return static_cast<int>(BB200_ERR_CAPACITY);
+      }
+      std::copy(merged.begin(), merged.end(), bins);
+    }
+    return static_cast<int>(BB200_OK);
+  });
+}
+
+int bb200_sharded_amcl_sample_states(bb200_sharded_amcl* g, uint64_t count, uint32_t step, double* states_out) {
+  BB_REQUIRE(g);
+  g->error.clear();
+  return guarded(*g, [&] {
+    const size_t shards = g->ranks.size();
+    std::vector<Filter*> f(shards);
+    uint64_t n_particles = 0;
+    for (size_t r = 0; r < shards; ++r) {
+      f[r] = &g->ranks[r]->impl.filter();
+      n_particles += f[r]->size();
+    }
+    const uint64_t max_particles = g->ranks[0]->impl.params().max_particles;
+    if (n_particles == 0) {
+      g->error = "no particles";
+      return static_cast<int>(BB200_ERR_STATE);
+    }
+    if (count > max_particles) {
+      g->error = "more samples than the filter capacity";
+      return static_cast<int>(BB200_ERR_CAPACITY);
+    }
+    if (count > 0 && states_out == nullptr) {
+      g->error = "states_out is null";
+      return static_cast<int>(BB200_ERR_INVALID_ARGUMENT);
+    }
+    if (count == 0) return static_cast<int>(BB200_OK);
+    // The global CDF: the one the last step left when it kept its particles, or one built as a sharded step builds it --
+    // the exponent from the largest weight of all shards, the offsets from the shards' fixed-point totals in rank order.
+    // Current CDFs quantised with different exponents were built shard by shard (e.g. bb200_filter_build_cdf on one shard):
+    // together they are no global CDF.  With one exponent on every shard they are the global build's bit for bit, since
+    // the global largest weight is some shard's largest weight.
+    std::vector<uint64_t> totals(shards, 0);
+    bool current = true, first = true;
+    int exponent = 0;
+    for (size_t r = 0; r < shards; ++r) {
+      if (f[r]->size() == 0) continue;
+      int e = 0;
+      if (const int st = f[r]->current_cdf(&totals[r], &e)) return st;
+      current = current && totals[r] != 0 && (first || e == exponent);
+      exponent = e;
+      first = false;
+    }
+    if (!current) {
+      double wmax = 0.0;
+      for (size_t r = 0; r < shards; ++r) {
+        if (f[r]->size() == 0) continue;
+        double w = 0.0;
+        if (const int st = f[r]->max_weight(&w)) return st;
+        wmax = w > wmax ? w : wmax;
+      }
+      for (size_t r = 0; r < shards; ++r)
+        if (f[r]->size() > 0)
+          if (const int st = f[r]->build_cdf(wmax, &totals[r], nullptr)) return st;
+    }
+    uint64_t total = 0;
+    std::vector<uint64_t> offsets(shards, 0);
+    for (size_t r = 0; r < shards; ++r) {
+      offsets[r] = total;
+      total += totals[r];
+    }
+    for (size_t r = 0; r < shards; ++r)
+      if (const int st = f[r]->sample_range(count, step, total, offsets[r])) return st;
+    for (Filter* s : f)  // every shard's draws have reached their slots' staging buffers
+      if (const int st = s->synchronize()) return st;
+    const uint64_t shard = max_particles / shards;  // slot j lies in the staging buffer of shard j / shard
+    for (size_t r = 0; r < shards && r * shard < count; ++r)
+      if (const int st = f[r]->staging_states(states_out + 4 * r * shard, std::min<uint64_t>(shard, count - r * shard))) return st;
+    return static_cast<int>(BB200_OK);
+  });
+}
+
+int bb200_sharded_amcl_cast_rays(bb200_sharded_amcl* g, const double* poses, uint64_t n_poses, const double* bearings_cs, uint64_t n_bearings,
+                                 double max_range, double* ranges) {
+  BB_REQUIRE(g);
+  g->error.clear();
+  return guarded(*g, [&] {
+    uint64_t n_rays = 0;
+    if (const int st = g->ranks[0]->impl.filter().check_cast_rays(poses, n_poses, bearings_cs, n_bearings, ranges, &n_rays)) return st;
+    if (n_rays == 0) return static_cast<int>(BB200_OK);
+    // The poses are cut into contiguous ranges, one per shard, each cast on that shard's copy of the map; every shard
+    // launches before any reads back, so shards on different devices cast at the same time.
+    std::vector<Filter*> casters;
+    for (bb200_amcl* a : g->ranks) casters.push_back(&a->impl.filter());
+    const uint64_t k = casters.size();
+    auto first_pose = [&](uint64_t c) { return n_poses * c / k; };  // n_poses <= kMaxCastRays: no overflow
+    for (uint64_t c = 0; c < k; ++c) {
+      const uint64_t begin = first_pose(c), end = first_pose(c + 1);
+      if (end > begin)
+        if (const int st = casters[c]->enqueue_cast_rays(poses + 4 * begin, end - begin, bearings_cs, n_bearings, max_range)) return st;
+    }
+    for (uint64_t c = 0; c < k; ++c) {
+      const uint64_t begin = first_pose(c), end = first_pose(c + 1);
+      if (end > begin)
+        if (const int st = casters[c]->finish_cast_rays(ranges + begin * n_bearings, (end - begin) * n_bearings)) return st;
     }
     return static_cast<int>(BB200_OK);
   });

@@ -124,7 +124,10 @@ Filter::Filter(const bb200_filter_config& config) : config_(config), cluster_(co
   BB_TRY(scalars_.allocate(1));
   BB_TRY(scalars_host_.allocate(1));
   BB_TRY(tile_state_.allocate(scan_tile_count(capacity_) + 1));
-  const uint32_t partial_rows = std::max(std::max(resample_block_count(capacity_), moments_block_count(capacity_)), kSmCount * 8u);
+  // A shard's per-slot resample walks the GLOBAL slots (the multinomial step, the KLD count, sample_range): one moment row
+  // per block of the largest launch.
+  const uint64_t slots = std::max<uint64_t>(capacity_, config.global_count);
+  const uint32_t partial_rows = std::max(std::max(resample_block_count(slots), moments_block_count(capacity_)), kSmCount * 8u);
   BB_TRY(partials_.allocate(static_cast<size_t>(partial_rows) * kMomentCount));
   BB_TRY(results_.allocate(16));
   BB_TRY(results_host_.allocate(16));
@@ -925,15 +928,21 @@ int Filter::cluster_estimate(const bb200_cluster_param& p, bb200_estimate* out, 
   return st;
 }
 
-int Filter::particle_histogram(double linear_resolution, double angular_resolution, bb200_cluster_cell* bins, uint64_t capacity, uint64_t* n_bins,
-                               double* max_bin_weight) {
+int Filter::cell_records(double linear_resolution, double angular_resolution, std::vector<HostCell>* host) {
   if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
   if (!(linear_resolution > 0.0) || !(angular_resolution > 0.0)) return fail(BB200_ERR_INVALID_ARGUMENT, "histogram resolutions must be positive");
   BB_CHECK(cudaSetDevice(config_.device));
-  std::vector<HostCell> host;
-  const int st = cluster_.cell_records(states_[cur_].get(), weights_.get(), n_, pivot_, linear_resolution, angular_resolution, stream_, &host, &error_);
+  const int st = cluster_.cell_records(states_[cur_].get(), weights_.get(), n_, pivot_, linear_resolution, angular_resolution, stream_, host, &error_);
   if (st != BB200_OK) return st;
   finish_marks();
+  return BB200_OK;
+}
+
+int Filter::particle_histogram(double linear_resolution, double angular_resolution, bb200_cluster_cell* bins, uint64_t capacity, uint64_t* n_bins,
+                               double* max_bin_weight) {
+  std::vector<HostCell> host;
+  const int st = cell_records(linear_resolution, angular_resolution, &host);
+  if (st != BB200_OK) return st;
   if (n_bins != nullptr) *n_bins = host.size();
   double top = 1e-3;  // beluga_ros/particle_cloud.hpp:197
   for (const HostCell& c : host) top = c.weight > top ? c.weight : top;
@@ -971,14 +980,72 @@ int Filter::sample_states(uint64_t count, uint32_t step, double* states_out) {
   return BB200_OK;
 }
 
-int Filter::cast_rays(const double* poses, uint64_t n_poses, const double* bearings, uint64_t n_bearings, double max_range, double* ranges) {
+int Filter::sample_range(uint64_t count, uint32_t step, uint64_t global_total, uint64_t cdf_offset) {
+  if (link_.world() < 1 || count > static_cast<uint64_t>(link_.world()) * capacity_) return fail(BB200_ERR_CAPACITY, "more samples than the joined shards hold");
+  if (n_ == 0 || count == 0) return BB200_OK;  // an empty shard's span is empty
+  if (!cdf_valid_) return fail(BB200_ERR_STATE, "build_cdf must run before sample_range");
+  BB_CHECK(cudaSetDevice(config_.device));
+  bb200_resample_opts o{};
+  o.scheme = BB200_RESAMPLE_MULTINOMIAL;
+  o.step = step;
+  o.min_particles = o.max_particles = count;
+  ResampleArgs a = make_resample_args(o, 0, count, false);
+  a.slot_first = 0;  // global slot index
+  a.global_total = global_total;
+  a.cdf_offset = cdf_offset;
+  a.weights_out = nullptr;  // the weights stay what they are
+  a.ancestors = nullptr;
+  a.span_filter = 1;  // draws are independent: walk every slot, keep those landing in this shard's span
+  a.owner_first = first_index_;
+  a.owner_count = capacity_;
+  link_.target_states(&a, cur_ ^ 1);
+  a.rank_totals = nullptr;  // the offsets of the CDF the caller names, not the totals the last step exchanged
+  a.peer_shard = capacity_;
+  launch_resample(a, scalars_.get(), partials_.get(), stream_);
+  BB_LAUNCHED("sample_range");
+  return BB200_OK;
+}
+
+int Filter::current_cdf(uint64_t* total, int* exponent) {
+  *total = 0;
+  *exponent = 0;
+  if (!cdf_valid_ || n_ == 0) return BB200_OK;
+  BB_CHECK(cudaSetDevice(config_.device));
+  BB_CHECK(cudaStreamSynchronize(stream_));
+  Scalars s;
+  BB_CHECK(cudaMemcpy(&s, scalars_.get(), sizeof(Scalars), cudaMemcpyDeviceToHost));
+  *total = s.total;
+  *exponent = s.exponent;
+  return BB200_OK;
+}
+
+int Filter::staging_states(double* out, uint64_t n) {
+  if (n > capacity_) return fail(BB200_ERR_CAPACITY, "more states than the staging buffer holds");
+  BB_CHECK(cudaSetDevice(config_.device));
+  BB_CHECK(cudaStreamSynchronize(stream_));
+  if (n > 0) BB_CHECK(cudaMemcpy(out, states_[cur_ ^ 1].get(), n * sizeof(Pose2), cudaMemcpyDeviceToHost));
+  return BB200_OK;
+}
+
+int Filter::check_cast_rays(const double* poses, uint64_t n_poses, const double* bearings, uint64_t n_bearings, const double* ranges, uint64_t* n_rays) {
   if (map_.sensor < 0) return fail(BB200_ERR_STATE, "no map");
-  uint64_t n_rays = 0;
-  if (!cast_ray_count(n_poses, n_bearings, &n_rays)) return fail(BB200_ERR_INVALID_ARGUMENT, "n_poses * n_bearings overflows");
-  if ((poses == nullptr && n_poses > 0) || (bearings == nullptr && n_bearings > 0) || (ranges == nullptr && n_rays > 0))
+  if (!cast_ray_count(n_poses, n_bearings, n_rays)) return fail(BB200_ERR_INVALID_ARGUMENT, "n_poses * n_bearings overflows");
+  if ((poses == nullptr && n_poses > 0) || (bearings == nullptr && n_bearings > 0) || (ranges == nullptr && *n_rays > 0))
     return fail(BB200_ERR_INVALID_ARGUMENT, "null array with a non-zero count");
+  if (*n_rays > kMaxCastRays) return fail(BB200_ERR_CAPACITY, "too many rays for one launch");
+  return BB200_OK;
+}
+
+int Filter::cast_rays(const double* poses, uint64_t n_poses, const double* bearings, uint64_t n_bearings, double max_range, double* ranges) {
+  uint64_t n_rays = 0;
+  if (const int st = check_cast_rays(poses, n_poses, bearings, n_bearings, ranges, &n_rays)) return st;
   if (n_rays == 0) return BB200_OK;
-  if (n_rays > kMaxCastRays) return fail(BB200_ERR_CAPACITY, "too many rays for one launch");
+  if (const int st = enqueue_cast_rays(poses, n_poses, bearings, n_bearings, max_range)) return st;
+  return finish_cast_rays(ranges, n_rays);
+}
+
+int Filter::enqueue_cast_rays(const double* poses, uint64_t n_poses, const double* bearings, uint64_t n_bearings, double max_range) {
+  const uint64_t n_rays = n_poses * n_bearings;
   BB_CHECK(cudaSetDevice(config_.device));
   OccupancyView grid;
   if (const int st = map_.ray_view(stream_, &grid, &error_)) return st;
@@ -990,7 +1057,13 @@ int Filter::cast_rays(const double* poses, uint64_t n_poses, const double* beari
   double* out = d + pose_doubles + bearing_doubles;
   launch_cast_rays(grid, reinterpret_cast<const Pose2*>(d), reinterpret_cast<const double2*>(d + pose_doubles), n_bearings, n_rays, max_range, out, stream_);
   BB_LAUNCHED("cast_rays");
-  BB_CHECK(cudaMemcpyAsync(ranges, out, n_rays * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+  cast_out_ = pose_doubles + bearing_doubles;
+  return BB200_OK;
+}
+
+int Filter::finish_cast_rays(double* ranges, uint64_t n_rays) {
+  BB_CHECK(cudaSetDevice(config_.device));
+  BB_CHECK(cudaMemcpyAsync(ranges, rays_.get() + cast_out_, n_rays * sizeof(double), cudaMemcpyDeviceToHost, stream_));
   BB_CHECK(cudaStreamSynchronize(stream_));
   return BB200_OK;
 }

@@ -73,12 +73,32 @@ class Filter {
   /// record per occupied bucket in first-occurrence order.  bins may be null (count only).
   int particle_histogram(double linear_resolution, double angular_resolution, bb200_cluster_cell* bins, uint64_t capacity, uint64_t* n_bins,
                          double* max_bin_weight);
+  /// The records of particle_histogram, in first-occurrence order, as the host vector the clusterizer returns.
+  int cell_records(double linear_resolution, double angular_resolution, std::vector<HostCell>* host);
   /// `count` states drawn by weight without touching the set (views::sample | take_exactly, particle_cloud.hpp:141-147).
   int sample_states(uint64_t count, uint32_t step, double* states_out);
   /// Ray2d::cast (algorithm/raycasting.hpp:79-107) on the current map for n_poses sensor poses {cos, sin, x, y} (map frame)
   /// and n_bearings bearings {cos, sin}, pose major: ranges[i * n_bearings + j] = min(distance, max_range) on a hit, +inf on
   /// a miss.  One launch and one synchronisation (none without rays); the particle set is not touched.
   int cast_rays(const double* poses, uint64_t n_poses, const double* bearings, uint64_t n_bearings, double max_range, double* ranges);
+  /// cast_rays in three parts, so that a caller holding filters on several devices keeps them all casting at once: the
+  /// refusals (nothing reaches the device; *n_rays = n_poses * n_bearings), the upload and launch of n_rays > 0 rays, and
+  /// the read-back of the ranges with the one synchronisation.
+  int check_cast_rays(const double* poses, uint64_t n_poses, const double* bearings, uint64_t n_bearings, const double* ranges, uint64_t* n_rays);
+  int enqueue_cast_rays(const double* poses, uint64_t n_poses, const double* bearings, uint64_t n_bearings, double max_range);
+  int finish_cast_rays(double* ranges, uint64_t n_rays);
+
+  // ---- sample_states over joined shards (bb200_sharded_amcl_sample_states) ----
+  /// Enqueues the multinomial draws of `step` among the global slots [0, count) whose position lies in this shard's span
+  /// [cdf_offset, cdf_offset + local total) of the global CDF (global_total): resample_range's multinomial form.  Slot j's
+  /// state goes to the staging buffer of the shard that owns it (j / capacity), as the sharded resample pushes its
+  /// particles; no weight, ancestor or particle of any shard changes.  The CDF must be current.
+  int sample_range(uint64_t count, uint32_t step, uint64_t global_total, uint64_t cdf_offset);
+  /// The local total and the fixed-point exponent of the current CDF; total 0 when the CDF is not current (or there are no
+  /// particles).
+  int current_cdf(uint64_t* total, int* exponent);
+  /// The first n states of the staging buffer, after this filter's stream has drained.
+  int staging_states(double* out, uint64_t n);
 
   /// Fused single-GPU step: propagate | reweight | normalize | resample | estimate with one
   /// host synchronisation at the end (the composition Amcl::update performs every step).
@@ -247,6 +267,7 @@ class Filter {
 
   DeviceMap map_;
   DeviceBuffer<double> rays_;  // ray casts (grown on use): the poses, the bearings, then the ranges
+  uint64_t cast_out_{0};       // offset of the last cast's ranges in rays_
   DeviceBuffer<uint32_t> beam_hits_;  // two-pass beam model: hit word per (beam, particle) of one pass
 
   double pivot_[2]{0.0, 0.0};

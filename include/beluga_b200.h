@@ -474,8 +474,8 @@ typedef struct bb200_point_cloud {
  * x_offset + 3 * sizeof(scalar) > point_step, or data == NULL with n_points > 0 (the std::invalid_argument cases of the
  * reference that reach this layer); BB200_ERR_CAPACITY when n_points > capacity.  On failure nothing is written. */
 int bb200_point_cloud_to_points(const bb200_point_cloud* cloud, double* points_xy, uint64_t capacity, uint64_t* n_points);
-/* Amcl::update(base_pose_in_odom, point_cloud) -- beluga_ros/src/amcl.cpp:67-81.  A sharded filter converts with
- * bb200_point_cloud_to_points and calls bb200_sharded_amcl_update. */
+/* Amcl::update(base_pose_in_odom, point_cloud) -- beluga_ros/src/amcl.cpp:67-81.  A sharded filter takes it through
+ * bb200_sharded_amcl_update_point_cloud. */
 int bb200_amcl_update_point_cloud(bb200_amcl* a, const double control_pose[4], const bb200_point_cloud* cloud, bb200_update_result* out);
 
 /* ---------------------------------------------------------------------------------------------
@@ -530,6 +530,39 @@ int bb200_cluster_merge_host(const bb200_cluster_cell* const* shard_cells, const
                              bb200_cluster_cell* merged, uint64_t capacity, uint64_t* n_merged);
 /* particles() in global index order (rank 0's shard first). */
 int bb200_sharded_amcl_get_particles(bb200_sharded_amcl* g, double* states, double* weights, uint64_t capacity);
+/* bb200_amcl_update_scan and bb200_amcl_update_point_cloud on a sharded filter: the scan or cloud is converted on the host
+ * exactly as the standalone calls convert it (bb200_scan_to_points, bb200_point_cloud_to_points), then
+ * bb200_sharded_amcl_update runs.  A scan or cloud the standalone calls refuse is refused with the same status before any
+ * device work, and the filter is left unchanged. */
+int bb200_sharded_amcl_update_scan(bb200_sharded_amcl* g, const double control_pose[4], const bb200_laser_scan* scan, bb200_update_result* out);
+int bb200_sharded_amcl_update_point_cloud(bb200_sharded_amcl* g, const double control_pose[4], const bb200_point_cloud* cloud,
+                                          bb200_update_result* out);
+/* bb200_filter_particle_histogram over the whole filter: every shard that holds particles builds its cell records on its
+ * device (the launches of bb200_filter_particle_histogram, once per call), and the records are merged on the host in rank order
+ * (bb200_cluster_merge_host), as bb200_sharded_amcl_cluster_estimate merges them.  Same contract as the filter call: bins
+ * may be NULL to query the count, BB200_ERR_CAPACITY leaves n_bins filled, max_bin_weight is max(1e-3, heaviest bin).
+ * Hashes, first indices, representatives and counts are those of one filter holding the same particles.  A cell that spans
+ * shards has its weight and raw moments added shard by shard: the weight is exact for unit weights (the state after a
+ * resample), otherwise it equals the single sequential sum up to the grouping of the additions; the moments always
+ * follow the grouping. */
+int bb200_sharded_amcl_particle_histogram(bb200_sharded_amcl* g, double linear_resolution, double angular_resolution, bb200_cluster_cell* bins,
+                                          uint64_t capacity, uint64_t* n_bins, double* max_bin_weight);
+/* bb200_filter_sample_states over the GLOBAL particle set: `count` multinomial draws of `step`, byte-identical to what one
+ * filter holding the same particles and weights returns, whatever the shard count; no shard's particles or weights change.
+ * The global CDF is the one the last step left when it kept its particles; otherwise every shard builds its CDF with the
+ * exponent of the largest weight of all shards (bb200_filter_max_weight, bb200_filter_build_cdf: 2 + 2 launches and 2
+ * synchronisations per shard); current CDFs that were quantised with different exponents (built shard by shard) are
+ * rebuilt the same way.  Then every shard with particles draws the slots of [0, count) whose position lands in its
+ * span of the global CDF (1 launch) and stores each into the staging buffer of the shard that owns the slot; one
+ * synchronisation per shard, and the host reads the staging buffers back in slot order.  BB200_ERR_STATE without
+ * particles, BB200_ERR_CAPACITY for count > max_particles, BB200_ERR_INVALID_ARGUMENT for a NULL states_out with count > 0. */
+int bb200_sharded_amcl_sample_states(bb200_sharded_amcl* g, uint64_t count, uint32_t step, double* states_out);
+/* bb200_filter_cast_rays on the shards' copies of the map: every ray equals the filter call's on the same map.  The poses
+ * are cut into contiguous ranges, one per shard in rank order; every shard with poses casts its range (1 launch) before
+ * any reads back, then the host reads each range back with one synchronisation per such shard.  ranges is pose major.
+ * Refusals are those of bb200_filter_cast_rays, before any device work. */
+int bb200_sharded_amcl_cast_rays(bb200_sharded_amcl* g, const double* poses, uint64_t n_poses, const double* bearings_cs, uint64_t n_bearings,
+                                 double max_range, double* ranges);
 #define BB200_SHARD_HANDLE_BYTES 256
 /* One process per GPU: CUDA IPC handles of this shard's two state buffers, mail block and (KLD) hash array (256 bytes) ... */
 int bb200_amcl_export_shard(bb200_amcl* a, void* out256);

@@ -298,6 +298,140 @@ template <class MotionModel, class SensorModel, class ExecutionPolicy>
   return std::make_pair(SE2d::from_data(e.mean), cov);
 }
 
+/// One filter over several shards (bb200_sharded_amcl), driven like Amcl: the constructor takes Amcl's arguments and the
+/// CUDA ordinal of every shard (ordinals may repeat); params.max_particles is the global particle count, a multiple of the
+/// shard count.  Every method marshals one C call; results equal those of one Amcl with the same parameters and seed.
+template <class MotionModel, class SensorModel>
+class ShardedAmcl {
+ public:
+  using state_type = typename SensorModel::state_type;
+  using measurement_type = typename SensorModel::measurement_type;
+  using map_type = typename SensorModel::map_type;
+  using estimation_type = std::pair<state_type, Matrix3d>;
+  /// The particle-cloud histogram: the bins in global first-occurrence order and max(1e-3, heaviest bin).
+  using histogram_type = std::pair<std::vector<bb200_cluster_cell>, double>;
+
+  ShardedAmcl(MotionModel motion_model, SensorModel sensor_model, const AmclParams& params, const std::vector<int>& devices)
+      : params_{params}, motion_model_{std::move(motion_model)}, sensor_model_{std::move(sensor_model)} {
+    const bb200_amcl_param p = c_amcl_param(params);
+    const bb200_motion_param m = motion_model_.c_motion_param();
+    const int st = bb200_sharded_amcl_create(&p, &m, static_cast<int>(devices.size()), devices.data(), &handle_);
+    if (st != BB200_OK) throw Error(st, bb200_create_error());
+    check(sensor_model_.attach(handle_));
+  }
+  ~ShardedAmcl() { bb200_sharded_amcl_destroy(handle_); }
+  ShardedAmcl(const ShardedAmcl&) = delete;
+  ShardedAmcl& operator=(const ShardedAmcl&) = delete;
+
+  /// Amcl::particles in global index order.
+  [[nodiscard]] ParticleSet particles() const {
+    std::uint64_t n = 0;
+    for (int r = 0; r < bb200_sharded_amcl_shards(handle_); ++r) {
+      std::uint64_t k = 0;
+      check(bb200_filter_size(bb200_amcl_filter(bb200_sharded_amcl_shard(handle_, r)), &k));
+      n += k;
+    }
+    ParticleSet out;
+    out.states.resize(n);
+    out.weights.resize(n);
+    if (n > 0) check(bb200_sharded_amcl_get_particles(handle_, reinterpret_cast<double*>(out.states.data()), out.weights.data(), n));
+    return out;
+  }
+
+  void initialize(const state_type& pose, const Matrix3d& covariance) {
+    const double mean[3] = {pose.x(), pose.y(), pose.theta()};
+    check(bb200_sharded_amcl_initialize(handle_, mean, covariance.data()));
+  }
+  void initialize_from_map() { check(bb200_sharded_amcl_initialize_from_map(handle_)); }
+  void update_map(const map_type& map) {
+    sensor_model_.update_map(map);
+    check(sensor_model_.attach(handle_));
+  }
+  void force_update() { bb200_sharded_amcl_force_update(handle_); }
+
+  auto update(const state_type& control_action, measurement_type measurement) -> std::optional<estimation_type> {
+    const measurement_token token = sensor_model_(std::move(measurement));
+    bb200_update_result r{};
+    check(bb200_sharded_amcl_update(handle_, control_action.data(), token.points.empty() ? nullptr : &token.points.front().first, token.points.size(), &r));
+    return estimate_of(r);
+  }
+  /// beluga_ros::Amcl::update(base_pose_in_odom, laser_scan) (bb200_sharded_amcl_update_scan).
+  auto update(const state_type& control_action, const LaserScanView& scan) -> std::optional<estimation_type> {
+    const bb200_laser_scan s = scan.c_view();
+    bb200_update_result r{};
+    check(bb200_sharded_amcl_update_scan(handle_, control_action.data(), &s, &r));
+    return estimate_of(r);
+  }
+  /// beluga_ros::Amcl::update(base_pose_in_odom, point_cloud) (bb200_sharded_amcl_update_point_cloud).
+  auto update(const state_type& control_action, const PointCloudView& cloud) -> std::optional<estimation_type> {
+    const bb200_point_cloud c = cloud.c_view();
+    bb200_update_result r{};
+    check(bb200_sharded_amcl_update_point_cloud(handle_, control_action.data(), &c, &r));
+    return estimate_of(r);
+  }
+#ifdef BELUGA_B200_WITH_SOPHUS
+  template <class SparsePointCloud, std::enable_if_t<is_sparse_point_cloud_v<SparsePointCloud>, int> = 0>
+  auto update(const state_type& control_action, const SparsePointCloud& cloud) -> std::optional<estimation_type> {
+    const PackedPointCloud packed{cloud};
+    return update(control_action, packed.view());
+  }
+#endif
+
+  /// beluga::cluster_based_estimate over all shards (bb200_sharded_amcl_cluster_estimate).
+  [[nodiscard]] estimation_type cluster_estimate(ParticleClusterizerParam parameters = {}) const {
+    const bb200_cluster_param p{parameters.linear_hash_resolution, parameters.angular_hash_resolution, parameters.weight_cap_percentile};
+    bb200_estimate e{};
+    check(bb200_sharded_amcl_cluster_estimate(handle_, &p, &e, nullptr, nullptr));
+    return estimation_of(e);
+  }
+  /// The particle-cloud histogram over all shards (bb200_sharded_amcl_particle_histogram).
+  [[nodiscard]] histogram_type particle_histogram(double linear_resolution = 1e-3, double angular_resolution = 1e-3) const {
+    std::uint64_t n = 0;
+    double top = 0.0;
+    check(bb200_sharded_amcl_particle_histogram(handle_, linear_resolution, angular_resolution, nullptr, 0, &n, &top));
+    std::vector<bb200_cluster_cell> bins(n);
+    check(bb200_sharded_amcl_particle_histogram(handle_, linear_resolution, angular_resolution, bins.data(), n, &n, &top));
+    return std::make_pair(std::move(bins), top);
+  }
+  /// `count` states drawn by weight from the global particle set, the multinomial draws of `step`
+  /// (bb200_sharded_amcl_sample_states); no particle changes.
+  [[nodiscard]] std::vector<state_type> sample_states(std::size_t count, uint32_t step) const {
+    std::vector<state_type> out(count);
+    check(bb200_sharded_amcl_sample_states(handle_, count, step, out.empty() ? nullptr : reinterpret_cast<double*>(out.data())));
+    return out;
+  }
+  /// Amcl::cast_rays on the shards' copies of the map (bb200_sharded_amcl_cast_rays).
+  [[nodiscard]] std::vector<std::optional<double>> cast_rays(const std::vector<state_type>& poses, const std::vector<Bearing>& bearings,
+                                                             double max_range) const {
+    std::vector<double> ranges(poses.size() * bearings.size());
+    check(bb200_sharded_amcl_cast_rays(handle_, poses.empty() ? nullptr : poses.front().data(), poses.size(),
+                                       bearings.empty() ? nullptr : bearings.front().data(), bearings.size(), max_range,
+                                       ranges.empty() ? nullptr : ranges.data()));
+    return detail::cast_results(ranges.data(), ranges.size());
+  }
+
+  [[nodiscard]] bb200_sharded_amcl* handle() const { return handle_; }
+
+ private:
+  void check(int status) const {
+    if (status != BB200_OK) throw Error(status, bb200_sharded_amcl_last_error(handle_));
+  }
+  static estimation_type estimation_of(const bb200_estimate& e) {
+    Matrix3d cov;
+    for (int i = 0; i < 9; ++i) cov[i] = e.cov[i];
+    return std::make_pair(state_type::from_data(e.mean), cov);
+  }
+  static auto estimate_of(const bb200_update_result& r) -> std::optional<estimation_type> {
+    if (!r.updated) return std::nullopt;
+    return estimation_of(r.estimate);
+  }
+
+  AmclParams params_;
+  MotionModel motion_model_;
+  SensorModel sensor_model_;
+  bb200_sharded_amcl* handle_{nullptr};
+};
+
 /// K independent filters on one GPU (bb200_amcl_batch) that read one or several maps, each for a likelihood-field model or
 /// the beam model: update() steps every member with a new scan at once.  Member m behaves like an Amcl built from motions[m] and params[m]; members keep a fixed
 /// particle count (min_particles == max_particles <= 32768) unless the batch is adaptive, whose members may have

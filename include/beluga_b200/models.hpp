@@ -356,6 +356,13 @@ class LikelihoodFieldModelImpl {
     const bb200_occupancy_grid g = grid_.view();
     return bb200_filter_set_likelihood_field_map(f, &p, &g, kProb ? 1 : 0);
   }
+  // -- used by beluga_b200::ShardedAmcl --
+  [[nodiscard]] int attach(bb200_sharded_amcl* g) const {
+    const bb200_likelihood_field_param p{params_.max_obstacle_distance, params_.max_laser_distance, params_.z_hit,      params_.z_random,
+                                         params_.sigma_hit,             params_.model_unknown_space ? 1 : 0, params_.only_obstacle_boundaries ? 1 : 0};
+    const bb200_occupancy_grid g_view = grid_.view();
+    return bb200_sharded_amcl_set_likelihood_field_map(g, &p, &g_view, kProb ? 1 : 0);
+  }
   [[nodiscard]] unsigned map_version() const { return map_version_; }
 
  private:
@@ -391,6 +398,11 @@ class BeamSensorModel {
     const bb200_beam_param p{params_.z_hit, params_.z_short, params_.z_max, params_.z_rand, params_.sigma_hit, params_.lambda_short, params_.beam_max_range};
     const bb200_occupancy_grid g = grid_.view();
     return bb200_filter_set_beam_map(f, &p, &g);
+  }
+  [[nodiscard]] int attach(bb200_sharded_amcl* g) const {
+    const bb200_beam_param p{params_.z_hit, params_.z_short, params_.z_max, params_.z_rand, params_.sigma_hit, params_.lambda_short, params_.beam_max_range};
+    const bb200_occupancy_grid g_view = grid_.view();
+    return bb200_sharded_amcl_set_beam_map(g, &p, &g_view);
   }
   [[nodiscard]] unsigned map_version() const { return map_version_; }
 

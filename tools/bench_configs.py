@@ -14,6 +14,8 @@ K = 16 and 256 members, alone and next to a 32 768-particle member, and a step a
 `batch_state`: export_members and AmclBatch.from_states (the fleet checkpoint and its restore) with the same members.
 `raycast`: device ray casts (Ray2d::cast) for 256 batch members x 1 pose x 1080 bearings and for 1M rays of one filter, against
 the CPU oracle's Ray2d on the same rays.
+`sharded-publish`: a 1M-particle filter's publish round (particle-cloud histogram and 2000 pose samples) and 1M ray casts on 2
+and 4 shards of one device, next to the single filter (a filter of one shard does not step, so it has no posterior to publish).
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import ctypes
@@ -452,6 +454,56 @@ def run_raycast():
                 "cpu_oracle_ms_one_thread": cpu_ms, "cpu_oracle_rays_per_s": rays / (cpu_ms * 1e-3),
                 "ms_per_step_e2e": ms, "kernels_ms": {}, "device": device}
         res[f"raycast_batch_256_x_1_x_1080_{int(max_range)}m_2000"]["ms_per_call_c"] = float(np.median(c_ms))
+    return res
+
+
+def run_sharded_publish():
+    """What a node publishes around each update, on 1M particles of the 2000^2 map after one resampling step: the particle-cloud
+    histogram (1 mm / 1 mrad buckets, the marker array's) plus 2000 pose samples (the pose array's; the CDF is rebuilt inside
+    the call, as it is after every resample), and 1M rays (1000 poses x 1000 bearings, 30 m).  A single Amcl, then one
+    ShardedAmcl of 2 and 4 shards on device 0 (one shard refuses to step).  Host clock around each call (every call ends synchronised), median of
+    `repeats` after one warm-up call."""
+    res = {}
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=1080, steps=100)
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    device = device_record()
+    n, repeats = 1_000_000, 20
+    params = bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=1)
+    poses = np.stack([bb.se2(*sc.poses[i % 100]) for i in range(1000)])
+    bearings = np.stack([[np.cos(t), np.sin(t)] for t in np.linspace(-np.pi, np.pi, 1000, endpoint=False)])
+    reference = {}
+    for shards in (0, 2, 4):
+        if shards == 0:
+            f = bb.Amcl(bb.DifferentialDriveModelParam(*MOTION), params)
+            histogram, sample = f.filter.particle_histogram, f.filter.sample_states
+        else:
+            f = bb.ShardedAmcl(bb.DifferentialDriveModelParam(*MOTION), params, devices=[0] * shards)
+            histogram, sample = f.particle_histogram, f.sample_states
+        f.update_map(bb.SENSOR_LIKELIHOOD_FIELD, bb.LikelihoodFieldModelParam(**LFM), grid)
+        f.initialize(sc.initial_mean, sc.initial_cov)
+        assert f.update(bb.se2(*sc.poses[0]), sc.scans[0]).resampled == 1
+
+        def publish():
+            return histogram(1e-3, 1e-3), sample(2000, 0xFFFFFFFF)
+
+        cases = (("publish", publish), ("rays_1000_x_1000_30m", lambda: f.cast_rays(poses, bearings, 30.0)))
+        name = "single" if shards == 0 else f"{shards}_shards"
+        for case, call in cases:
+            out = call()
+            times = []
+            for _ in range(repeats):
+                t0 = time.perf_counter()
+                call()
+                times.append((time.perf_counter() - t0) * 1e3)
+            if shards == 0:
+                reference[case] = out
+            same = (all(np.array_equal(a, b) for a, b in zip(out[0][:4], reference[case][0][:4])) and np.array_equal(out[1], reference[case][1])
+                    if case == "publish" else np.array_equal(out, reference[case]))
+            ms = float(np.median(times))
+            res[f"sharded_publish_{case}_1M_{name}"] = {
+                "ms_per_call": ms, "ms_per_call_min_max": [float(min(times)), float(max(times))], "repeats": repeats,
+                "equal_to_single_filter": bool(same), "ms_per_step_e2e": ms, "kernels_ms": {}, "device": device}
+        f.close()
     return res
 
 
@@ -985,6 +1037,8 @@ def main():
         out.update(run_batch_measurements())
     if "raycast" in which:
         out.update(run_raycast())
+    if "sharded-publish" in which:
+        out.update(run_sharded_publish())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}

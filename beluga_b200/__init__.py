@@ -773,6 +773,44 @@ class Amcl:
         self._check(self._lib.bb200_amcl_update(self._h, _dptr(_f64(control_pose)), _dptr(pts), len(pts), C.byref(res)))
         return res
 
+    def update_weighted(self, control_pose, weigh) -> _capi.UpdateResult:
+        """Amcl::update with the caller's own sensor model (bb200_amcl_update_begin / _end).
+
+        `weigh(states, factors)` receives torch CUDA tensors over the step's device views, without a copy: the propagated
+        states, (n, 4) float64 rows {cos, sin, x, y}, and the factors, (n,) float64, which it fills with L(states[i]).  It
+        runs inside torch.cuda.stream(torch.cuda.ExternalStream(view.stream)), so torch work it issues is ordered before the
+        rest of the step; other work must be synchronised with that stream by `weigh`.  It is not called when the policies
+        skip the step.  When `weigh` raises, the step is closed with every factor 1 (a step without a measurement) and the
+        exception propagates."""
+        view = _capi.WeighView()
+        self._check(self._lib.bb200_amcl_update_begin(self._h, _dptr(_f64(control_pose)), C.byref(view)))
+        res = _capi.UpdateResult()
+        if not view.updated:
+            self._check(self._lib.bb200_amcl_update_end(self._h, C.byref(res)))
+            return res
+        import torch
+
+        device = torch.device("cuda", self.params.device)
+        states = torch.as_tensor(_CudaArray(view.states, (view.n, 4)), device=device)
+        factors = torch.as_tensor(_CudaArray(view.factors, (view.n,)), device=device)
+        with torch.cuda.stream(torch.cuda.ExternalStream(view.stream, device=device)):
+            try:
+                weigh(states, factors)
+            except BaseException:
+                factors.fill_(1.0)
+                self._lib.bb200_amcl_update_end(self._h, C.byref(res))
+                raise
+        self._check(self._lib.bb200_amcl_update_end(self._h, C.byref(res)))
+        return res
+
+
+class _CudaArray:
+    """A float64 device array in the __cuda_array_interface__ protocol (no stream to wait on: the consumer orders its work)."""
+
+    def __init__(self, ptr: int, shape: tuple):
+        self.__cuda_array_interface__ = {"shape": tuple(int(d) for d in shape), "typestr": "<f8", "data": (int(ptr), False), "version": 3,
+                                         "strides": None, "stream": None}
+
 
 class ShardedAmcl:
     """bb200_sharded_amcl: ONE filter over several shards driven by one host thread (include/beluga_b200.h).
@@ -1252,6 +1290,55 @@ class AmclBatch:
                 continue
             e = (np.array(est[m].mean), np.array(est[m].cov).reshape(3, 3))
             out.append((*e, cells[m], clusters[m]) if with_counts else e)
+        return list(res), out
+
+    def update_weighted(self, control_poses, measurements, weigh, present=None, cluster=None):
+        """update_measurements with members weighed by the caller's own sensor model (bb200_amcl_batch_update_begin / _end):
+        a None measurement marks a weighed member; the others pass points, a LaserScan or a PointCloud as in
+        update_measurements.  `weigh(members, states, factors)` is called once, with the indices of the weighed members that
+        update in this step and, per member, torch CUDA tensors over its views without a copy: its propagated states,
+        (n, 4) float64, and its factors, (n,) float64, which it fills with L(states[i]).  It runs inside
+        torch.cuda.stream(torch.cuda.ExternalStream(stream)) on the batch's stream and is not called when no weighed member
+        updates.  When it raises, the step is closed with every factor 1 and the exception propagates.  cluster: None, or
+        (linear, angular, percentile) for the cluster estimates of update_clustered; the return value is then (results,
+        estimates) as update_clustered returns it, otherwise the results."""
+        k = len(self.params)
+        if len(measurements) != k:
+            raise ValueError("one measurement per member")
+        mask = self._mask(present)
+        poses = _f64(control_poses).reshape(k, 4)
+        built = [(_capi.Measurement(kind=_capi.MEASUREMENT_WEIGHTS), None) if m is None else _measurement(m) for m in measurements]
+        table = (_capi.Measurement * k)(*[b[0] for b in built])
+        views = (_capi.WeighView * k)()
+        self._check(self._lib.bb200_amcl_batch_update_begin(self._h, _dptr(poses), table, mask, views))
+        res = (_capi.UpdateResult * k)()
+        est = (_capi.Estimate * k)()
+        cells, clusters = (C.c_uint32 * k)(), (C.c_uint32 * k)()
+        p = None if cluster is None else _capi.ClusterParam(*cluster)
+
+        def end():
+            return self._lib.bb200_amcl_batch_update_end(self._h, None if p is None else C.byref(p), res, None if p is None else est,
+                                                         None if p is None else cells, None if p is None else clusters)
+
+        members = [m for m in range(k) if measurements[m] is None and views[m].updated]
+        if members:
+            import torch
+
+            device = torch.device("cuda", next(q.device for q in self.params if q is not None))
+            states = [torch.as_tensor(_CudaArray(views[m].states, (views[m].n, 4)), device=device) for m in members]
+            factors = [torch.as_tensor(_CudaArray(views[m].factors, (views[m].n,)), device=device) for m in members]
+            with torch.cuda.stream(torch.cuda.ExternalStream(views[members[0]].stream, device=device)):
+                try:
+                    weigh(members, states, factors)
+                except BaseException:
+                    for f in factors:
+                        f.fill_(1.0)
+                    end()
+                    raise
+        self._check(end())
+        if p is None:
+            return list(res)
+        out = [None if not res[m].updated else (np.array(est[m].mean), np.array(est[m].cov).reshape(3, 3)) for m in range(k)]
         return list(res), out
 
     def update_scans(self, control_poses, scans, present=None) -> list:

@@ -112,7 +112,7 @@ class MarkerVertex(C.Structure):
     _fields_ = [("x", C.c_double), ("y", C.c_double), ("z", C.c_double), ("r", C.c_float), ("g", C.c_float), ("b", C.c_float), ("a", C.c_float)]
 
 
-MEASUREMENT_POINTS, MEASUREMENT_SCAN, MEASUREMENT_CLOUD = 0, 1, 2
+MEASUREMENT_POINTS, MEASUREMENT_SCAN, MEASUREMENT_CLOUD, MEASUREMENT_WEIGHTS = 0, 1, 2, 3
 
 
 class Measurement(C.Structure):
@@ -123,6 +123,10 @@ class Measurement(C.Structure):
 class UpdateResult(C.Structure):
     _fields_ = [("updated", C.c_int), ("resampled", C.c_int), ("n_particles", C.c_uint64), ("estimate", Estimate),
                 ("random_state_probability", C.c_double), ("weight_sum", C.c_double), ("weights_degenerate", C.c_int)]
+
+
+class WeighView(C.Structure):
+    _fields_ = [("updated", C.c_int), ("n", C.c_uint64), ("states", C.c_void_p), ("factors", C.c_void_p), ("stream", C.c_void_p)]
 
 
 _P = C.POINTER
@@ -197,6 +201,10 @@ SIGNATURES = {
     "bb200_amcl_update_scan": (C.c_int, [_vp, _dbl, _P(LaserScan), _P(UpdateResult)]),
     "bb200_point_cloud_to_points": (C.c_int, [_P(PointCloud), _dbl, C.c_uint64, _P(C.c_uint64)]),
     "bb200_amcl_update_point_cloud": (C.c_int, [_vp, _dbl, _P(PointCloud), _P(UpdateResult)]),
+    "bb200_amcl_update_begin": (C.c_int, [_vp, _dbl, _P(WeighView)]),
+    "bb200_amcl_batch_update_begin": (C.c_int, [_vp, _dbl, _P(Measurement), _P(C.c_uint8), _P(WeighView)]),
+    "bb200_amcl_batch_update_end": (C.c_int, [_vp, _P(ClusterParam), _P(UpdateResult), _P(Estimate), _P(C.c_uint32), _P(C.c_uint32)]),
+    "bb200_amcl_update_end": (C.c_int, [_vp, _P(UpdateResult)]),
     "bb200_sharded_amcl_create": (C.c_int, [_P(AmclParam), _P(MotionParam), C.c_int, _P(C.c_int), _P(_vp)]),
     "bb200_sharded_amcl_destroy": (None, [_vp]),
     "bb200_sharded_amcl_last_error": (C.c_char_p, [_vp]),

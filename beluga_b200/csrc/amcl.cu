@@ -412,27 +412,43 @@ int Amcl::update(const double control[4], const double* points_xy, uint64_t n_po
   return st;
 }
 
+bool Amcl::fused(const bb200_step_plan& plan) const {
+  return plan.resample != 0 && !plan.needs_ess && !(params().min_particles < params().max_particles);
+}
+
 int Amcl::update_device(const double control[4], const double* points_xy, uint64_t n_points, bb200_update_result* out) {
   *out = bb200_update_result{};
   bb200_step_plan plan;
   int st = plan_update(control, &plan);
   if (st != BB200_OK || !plan.update) return st;
-  out->random_state_probability = plan.random_state_probability;
-  const uint64_t n = filter_.size();
-  bool do_resample = plan.resample != 0;
-  const bool kld_active = params().min_particles < params().max_particles;
-  if (do_resample && !plan.needs_ess && !kld_active) {
+  if (fused(plan)) {
     // The whole step in one stream-ordered sequence with a single host synchronisation.
+    st = filter_.step_begin(plan.sampling, plan.step, points_xy, n_points, plan.opts, true);
+    if (st == BB200_OK) st = filter_.step_phase(Filter::kPhaseReweight);
+    if (st != BB200_OK) {
+      filter_.step_abort();
+      return st;
+    }
+  } else {
+    st = filter_.propagate_reweight(&plan.sampling, plan.step, points_xy, n_points);
+    if (st != BB200_OK) return st;
+  }
+  return finish_update(plan, out);
+}
+
+int Amcl::finish_update(const bb200_step_plan& plan, bb200_update_result* out) {
+  out->random_state_probability = plan.random_state_probability;
+  if (fused(plan)) {
     uint64_t new_size = 0;
-    st = filter_.step_resample(plan.sampling, plan.step, points_xy, n_points, plan.opts, &out->estimate, &out->weight_sum, &new_size);
+    const int st = filter_.finish_resample(&out->estimate, &out->weight_sum, &new_size);
     if (st != BB200_OK) return st;
     out->resampled = 1;
     out->n_particles = new_size;
   } else {
-    st = filter_.propagate_reweight(&plan.sampling, plan.step, points_xy, n_points);
-    if (st != BB200_OK) return st;
+    const uint64_t n = filter_.size();
+    bool do_resample = plan.resample != 0;
     double factor = 0.0, sum_sq = 0.0;
-    st = filter_.normalize(&factor, &sum_sq);
+    int st = filter_.normalize(&factor, &sum_sq);
     if (st != BB200_OK) return st;
     out->weight_sum = factor;
     if (plan.needs_ess) {
@@ -454,6 +470,49 @@ int Amcl::update_device(const double control[4], const double* points_xy, uint64
   commit_update(out->resampled, plan.random_state_probability);
   out->updated = 1;
   return BB200_OK;
+}
+
+int Amcl::update_begin(const double control[4], bb200_weigh_view* view) {
+  error_.clear();
+  if (filter_.weigh_open()) return filter_.fail_with(BB200_ERR_STATE, "a weighed step is already open (bb200_amcl_update_end closes it)");
+  *view = bb200_weigh_view{};
+  if (sharded() || filter_.link().world() > 1) return filter_.fail_with(BB200_ERR_STATE, "a sharded filter takes no weighed steps");
+  weighed_before_ = policy_;
+  bb200_step_plan& plan = weighed_plan_;
+  int st = plan_update(control, &plan);
+  if (st == BB200_OK && plan.update) {
+    const bool injects = plan.resample != 0 && plan.random_state_probability > 0.0;
+    st = filter_.weigh_begin(plan.sampling, plan.step, plan.opts, fused(plan), injects);
+  }
+  if (st != BB200_OK) {
+    policy_ = weighed_before_;  // as update(): policies, control window and recovery estimator as if the call had not happened
+    filter_.step_abort();
+    return st;
+  }
+  filter_.set_weigh_open(true);
+  view->updated = plan.update;
+  if (plan.update) {
+    view->n = filter_.size();
+    view->states = filter_.weigh_states();
+    view->factors = filter_.weigh_factors();
+    view->stream = filter_.stream();
+  }
+  return BB200_OK;
+}
+
+int Amcl::update_end(bb200_update_result* out) {
+  *out = bb200_update_result{};
+  if (!filter_.weigh_open()) return filter_.fail_with(BB200_ERR_STATE, "no weighed step is open (bb200_amcl_update_begin)");
+  filter_.set_weigh_open(false);
+  if (!weighed_plan_.update) return BB200_OK;
+  int st = filter_.weigh_apply();
+  if (st == BB200_OK) st = finish_update(weighed_plan_, out);
+  if (st != BB200_OK) {
+    *out = bb200_update_result{};
+    policy_ = weighed_before_;
+    filter_.step_abort();
+  }
+  return st;
 }
 
 }  // namespace bb200

@@ -86,15 +86,28 @@ class Amcl {
   /// before the next one, the exchanges between the shards happen on the devices (csrc/kernels.cuh: ShardMail).
   static int update_group(Amcl* const* ranks, int count, const double control[4], const double* points_xy, uint64_t n_points,
                           bb200_update_result* out);
+  /// The first half of update() for a sensor model the caller runs: plans the step and, unless the policies skip it,
+  /// enqueues the propagate; *view gets the device views the caller weighs.  The step stays open until update_end.
+  /// Atomic as update(); refused on shards.
+  int update_begin(const double control[4], bb200_weigh_view* view);
+  /// The second half: w *= factors and everything update() runs after its sensor model.  Atomic as update().
+  int update_end(bb200_update_result* out);
 
  private:
   int update_device(const double control[4], const double* points_xy, uint64_t n_points, bb200_update_result* out);
+  /// A step that resamples in the fused sequence with one host synchronisation (every_n fired, no ESS test, no KLD).
+  bool fused(const bb200_step_plan& plan) const;
+  /// What update() runs after the sensor model, up to the result and the policies' commit.
+  int finish_update(const bb200_step_plan& plan, bb200_update_result* out);
   int initialized(int status, bool has_particles);  // after initialize*(): the next update is forced
 
   AmclPolicy policy_;
   Filter filter_;
   mutable std::string error_;
   bool initialized_{false};
+  // the open weighed step: its plan, and the policy to put back when it fails
+  bb200_step_plan weighed_plan_{};
+  AmclPolicy weighed_before_{policy_};
 };
 
 }  // namespace bb200

@@ -1238,6 +1238,7 @@ std::string measurement_error(const bb200_measurement& in) {
 
 /// The points a member's measurement can yield: the exact count for points and clouds, the kept beams for a scan.
 uint64_t measurement_bound(const bb200_measurement& in) {
+  if (in.kind == BB200_MEASUREMENT_WEIGHTS) return 0;
   return in.kind == BB200_MEASUREMENT_SCAN ? scan_beam_count(*in.scan) : in.kind == BB200_MEASUREMENT_CLOUD ? in.cloud->n_points : in.n_points;
 }
 
@@ -1295,15 +1296,48 @@ int Batch::update_clustered(const double* control_poses, const bb200_measurement
 
 int Batch::step(const double* control_poses, const bb200_measurement* in, const uint8_t* present, bb200_update_result* out,
                 const ClusteredOut* clustered) {
+  for (size_t k = 0; k < members_.size(); ++k) out[k] = bb200_update_result{};
+  if (const int st = step_begin(control_poses, in, present, nullptr)) return st;
+  return step_end(clustered, out);
+}
+
+int Batch::update_begin(const double* control_poses, const bb200_measurement* measurements, const uint8_t* present, bb200_weigh_view* views) {
+  error_.clear();
+  if (open_.open) return fail(BB200_ERR_STATE, "a weighed step is already open (bb200_amcl_batch_update_end closes it)");
+  if (const int st = check_present(present)) return st;
+  for (size_t k = 0; k < members_.size(); ++k) {
+    if (!selected_member(present, k) || measurements[k].kind == BB200_MEASUREMENT_WEIGHTS) continue;
+    const std::string why = measurement_error(measurements[k]);
+    if (!why.empty()) return fail(BB200_ERR_INVALID_ARGUMENT, "member " + std::to_string(k) + ": " + why);
+  }
+  return step_begin(control_poses, measurements, present, views);
+}
+
+int Batch::update_end(const bb200_cluster_param* cluster, bb200_update_result* out, bb200_estimate* clustered, uint32_t* n_cells, uint32_t* n_clusters) {
+  error_.clear();
+  for (size_t k = 0; k < members_.size(); ++k) out[k] = bb200_update_result{};
+  if (!open_.open) return fail(BB200_ERR_STATE, "no weighed step is open (bb200_amcl_batch_update_begin)");
+  if (cluster != nullptr && (!(cluster->linear_hash_resolution > 0.0) || !(cluster->angular_hash_resolution > 0.0) ||
+                             !(cluster->weight_cap_percentile >= 0.0) || !(cluster->weight_cap_percentile < 1.0))) {
+    return fail(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)");
+  }
+  const ClusteredOut co{cluster, clustered, n_cells, n_clusters};
+  return step_end(cluster != nullptr ? &co : nullptr, out);
+}
+
+int Batch::step_begin(const double* control_poses, const bb200_measurement* in, const uint8_t* present, bb200_weigh_view* views) {
   error_.clear();
   const size_t count = members_.size();
-  for (size_t k = 0; k < count; ++k) out[k] = bb200_update_result{};
+  if (views != nullptr)
+    for (size_t k = 0; k < count; ++k) views[k] = bb200_weigh_view{};
   if (const int st = check_present(present)) return st;
   std::vector<AmclPolicy> before;
   before.reserve(count);
   for (const Member& m : members_) before.push_back(m.policy);
   auto rollback = [&](int st) {
     for (size_t k = 0; k < count; ++k) members_[k].policy = before[k];
+    if (views != nullptr)
+      for (size_t k = 0; k < count; ++k) views[k] = bb200_weigh_view{};
     return st;
   };
 
@@ -1315,34 +1349,47 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     members_[k].policy.plan_update(control_poses + 4 * k, members_[k].n, &plans[k]);
     if (plans[k].update) active.push_back(static_cast<uint32_t>(k));
   }
-  if (active.empty()) return BB200_OK;
+  auto weighed = [&](uint32_t k) { return in[k].kind == BB200_MEASUREMENT_WEIGHTS; };
+  const bool any_weighed = std::any_of(active.begin(), active.end(), weighed);
+  if (active.empty()) {
+    open_ = OpenStep{};
+    open_.open = true;
+    open_.before = std::move(before);
+    return BB200_OK;
+  }
 
   // Points sent by the host come first in the point buffer, in member order; the points of scans and clouds, written by
   // batch_points_kernel, follow them.  Scans and clouds are sized by their bounds (measurement_bound).
   uint64_t points_total = 0, host_points = 0, input_floats = 0;
   uint32_t max_points = 0;
-  int step_map = -1;            // the map every updating member reads, or -1 when they read several
+  // The map every updating member with a map reads, -1 when they read several, -2 when none has one (every updating
+  // member is weighed by the caller and none may inject).
+  int step_map = -2;
   std::vector<int> forms(count, kBatchField);
   for (const uint32_t k : active)
-    if (members_[k].map < 0) return rollback(fail(BB200_ERR_STATE, maps_.empty() ? "no map set" : "member " + std::to_string(k) + " has no map"));
+    if (members_[k].map < 0 && !weighed(k))
+      return rollback(fail(BB200_ERR_STATE, maps_.empty() ? "no map set" : "member " + std::to_string(k) + " has no map"));
   for (const uint32_t k : active) {
     const uint64_t bound = measurement_bound(in[k]);
     if (bound > 0xffffffffull) return rollback(fail(BB200_ERR_INVALID_ARGUMENT, "too many points"));
     if (in[k].kind == BB200_MEASUREMENT_POINTS && in[k].n_points > 0 && in[k].points_xy == nullptr)
       return rollback(fail(BB200_ERR_INVALID_ARGUMENT, "points_xy is null"));
     const int id = members_[k].map;
+    const bool injects = plans[k].resample && plans[k].random_state_probability > 0.0;
+    if (injects && (id < 0 || maps_.at(id).map.n_free == 0)) return rollback(fail(BB200_ERR_STATE, "recovery injection needs a map with free cells"));
+    if (weighed(k)) forms[k] = kBatchWeighed;
+    if (id < 0) continue;
     const DeviceMap& map = maps_.at(id).map;
-    if (plans[k].resample && plans[k].random_state_probability > 0.0 && map.n_free == 0)
-      return rollback(fail(BB200_ERR_STATE, "recovery injection needs a map with free cells"));
     // The beam model walks a member's rays in two passes when its map allows it (the rule of the single filter).
-    if (map.sensor == BB200_SENSOR_BEAM) forms[k] = beam_two_pass_map(map) ? kBatchBeamTwoPass : kBatchBeamFused;
-    step_map = k == active.front() || step_map == id ? id : -1;
+    if (map.sensor == BB200_SENSOR_BEAM && !weighed(k)) forms[k] = beam_two_pass_map(map) ? kBatchBeamTwoPass : kBatchBeamFused;
+    step_map = step_map == -2 || step_map == id ? id : -1;
     points_total += bound;
     if (in[k].kind == BB200_MEASUREMENT_POINTS) host_points += bound;
     input_floats += in[k].kind == BB200_MEASUREMENT_CLOUD ? 3 * bound : in[k].kind == BB200_MEASUREMENT_SCAN ? bound : 0;
     max_points = std::max(max_points, static_cast<uint32_t>(bound));
   }
-  const bool convert = std::any_of(active.begin(), active.end(), [&](uint32_t k) { return in[k].kind != BB200_MEASUREMENT_POINTS; });
+  const bool convert = std::any_of(active.begin(), active.end(),
+                                   [&](uint32_t k) { return in[k].kind == BB200_MEASUREMENT_SCAN || in[k].kind == BB200_MEASUREMENT_CLOUD; });
   // Amcl::update_device's KLD path: a resampling member with min_particles < max_particles sizes its new set with
   // take_while_kld (Filter::resample_kld).
   auto resamples_kld = [&](uint32_t k) { return plans[k].resample != 0 && plans[k].opts.min_particles < plans[k].opts.max_particles; };
@@ -1352,10 +1399,10 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
   const bool ess = std::any_of(active.begin(), active.end(), [&](uint32_t k) { return plans[k].needs_ess != 0; });
   int st = check(cudaSetDevice(device_), "cudaSetDevice");
   if (st == BB200_OK) st = ensure_points(points_total);  // the previous step has ended: the staging buffers are free
-  if (st == BB200_OK && step_map < 0) st = ensure_map_table();
+  if (st == BB200_OK && step_map == -1) st = ensure_map_table();
   if (st == BB200_OK && convert) st = ensure_inputs(input_floats);
   if (st == BB200_OK && kld) st = ensure_kld_scratch();
-  if (st == BB200_OK && clustered != nullptr) st = ensure_select_scratch();
+  if (st == BB200_OK && any_weighed) st = check(factors_.grow(weights_.size()), "factor buffer");  // laid out like the weights
   for (auto k = active.begin(); st == BB200_OK && k != active.end(); ++k)
     if (in[*k].kind == BB200_MEASUREMENT_SCAN) st = ensure_scan_table(members_[*k], *in[*k].scan);
   if (st != BB200_OK) return rollback(st);
@@ -1382,7 +1429,7 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     b.scheme = plan.opts.scheme;
     b.cur = m.cur;
     b.ceil_log2_count = ceil_log2_count(m.capacity);
-    b.map = step_map < 0 ? maps_.at(m.map).slot : 0;
+    b.map = step_map == -1 && m.map >= 0 ? maps_.at(m.map).slot : 0;
     b.random_state_probability = plan.random_state_probability;
     b.pivot_x = m.pivot[0];
     b.pivot_y = m.pivot[1];
@@ -1398,7 +1445,11 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
       q.table_offset = m.table_offset;
       q.table_mask = m.table_slots - 1;
     }
-    if (meas.kind == BB200_MEASUREMENT_POINTS) {
+    if (meas.kind == BB200_MEASUREMENT_WEIGHTS) {
+      b.point_offset = 0;  // no points: the caller's factors stand for the sensor model
+      b.n_points = 0;
+      b.points_radius = 0.0;
+    } else if (meas.kind == BB200_MEASUREMENT_POINTS) {
       b.point_offset = point_offset;
       b.n_points = static_cast<uint32_t>(meas.n_points);
       b.points_radius = scan_radius(meas.points_xy, meas.n_points);
@@ -1413,7 +1464,7 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     if (convert) {
       BatchPointsMember& d = inputs_.host.get()[j];
       d = BatchPointsMember{};
-      d.kind = meas.kind;
+      d.kind = meas.kind;  // points and weighed members have no CTA there
       d.input_offset = input_offset;
       d.count = static_cast<uint32_t>(bound);
       float* raw = input_host_.get() + input_offset;
@@ -1487,31 +1538,15 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     a.post_ctas[1] = totals[1];
     a.ess_ctas = totals[2];
   }
-  const int rows = kld || ess ? kBatchRows : convert ? kBatchLaunches + 1 : kBatchLaunches;
-  // update_clustered: the pre-step cluster table and how the step may change each member (batch_cluster_table_kernel).
-  if (clustered != nullptr) {
+  if (any_weighed) {
+    uint32_t* row = first_host_.get() + static_cast<size_t>(kBatchWeighRow) * (n_active + 1);
     for (uint32_t j = 0; j < n_active; ++j) {
-      const uint32_t k = active[j];
-      const Member& m = members_[k];
-      const bb200_step_plan& plan = plans[k];
-      BatchClusterMember& c = cl_.table_host.get()[j];
-      c = BatchClusterMember{};
-      c.offset = m.offset;
-      c.table_offset = m.table_offset;
-      c.starts_offset = m.offset + k;
-      c.n = static_cast<uint32_t>(m.n);
-      c.table_mask = m.table_slots - 1;
-      c.cur = static_cast<uint32_t>(m.cur);
-      c.pivot_x = m.pivot[0];
-      c.pivot_y = m.pivot[1];
-      BatchClusterPost& q = sel_.post_host.get()[j];
-      q = BatchClusterPost{};
-      q.scratch_offset = sel_.offsets[k];
-      q.capacity = static_cast<uint32_t>(m.capacity);
-      q.mode = plan.needs_ess ? 2 : plan.resample ? 1 : 0;
-      q.kld = resamples_kld(k) ? 1 : 0;
+      row[j] = a.weigh_ctas;
+      if (weighed(active[j])) a.weigh_ctas += batch_weigh_ctas(table_host_.get()[j]);
     }
+    row[n_active] = a.weigh_ctas;
   }
+  const int rows = kld || ess || any_weighed ? kBatchRows : convert ? kBatchLaunches + 1 : kBatchLaunches;
 
   cudaStream_t stream = stream_;
   for (const uint32_t k : active) members_[k].cdf_total = 0;  // from here on the step may have rewritten their CDFs
@@ -1529,12 +1564,6 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     st = check(cudaMemcpyAsync(input_.get(), input_host_.get(), input_floats * sizeof(float), cudaMemcpyHostToDevice, stream), "upload measurements");
   if (st == BB200_OK && kld)
     st = check(cudaMemcpyAsync(kld_.device.get(), kld_.host.get(), n_active * sizeof(BatchKldMember), cudaMemcpyHostToDevice, stream), "upload KLD table");
-  if (st == BB200_OK && clustered != nullptr)
-    st = check(cudaMemcpyAsync(cl_.table.get(), cl_.table_host.get(), n_active * sizeof(BatchClusterMember), cudaMemcpyHostToDevice, stream),
-               "upload cluster table");
-  if (st == BB200_OK && clustered != nullptr)
-    st = check(cudaMemcpyAsync(sel_.post.get(), sel_.post_host.get(), n_active * sizeof(BatchClusterPost), cudaMemcpyHostToDevice, stream),
-               "upload cluster steps");
   if (st != BB200_OK) return rollback(st);
   if (convert) {
     pa.members = table_.get();
@@ -1567,7 +1596,7 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
     a.grid_origin = map.grid_origin;
     a.occupancy = map.occupancy;
     a.beam = map.beam;
-  } else {
+  } else if (step_map == -1) {
     a.maps = map_table_.get();
   }
   a.hits = hits_.get();
@@ -1581,7 +1610,82 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
   a.members_done = members_done_.get();
   a.ticket = ticket_host_.get();
   a.seq = seq_;
-  launches_ += static_cast<uint64_t>(launch_batch_step(a, stream));
+  a.factors = factors_.get();
+  launches_ += static_cast<uint64_t>(launch_batch_step_head(a, stream));
+  st = check(cudaGetLastError(), "batch step launch");
+  if (st != BB200_OK) return rollback(st);
+  if (views != nullptr)
+    for (const uint32_t k : active) {
+      const Member& m = members_[k];
+      bb200_weigh_view& v = views[k];
+      v.updated = 1;
+      if (!weighed(k)) continue;
+      v.n = m.n;
+      v.states = reinterpret_cast<const double*>(states_[m.cur].get() + m.offset);
+      v.factors = factors_.get() + m.offset;
+      v.stream = stream;
+    }
+  open_ = OpenStep{};
+  open_.open = true;
+  open_.before = std::move(before);
+  open_.plans = std::move(plans);
+  open_.active = std::move(active);
+  open_.kld = kld;
+  open_.args = a;
+  return BB200_OK;
+}
+
+int Batch::step_end(const ClusteredOut* clustered, bb200_update_result* out) {
+  OpenStep step = std::move(open_);
+  open_ = OpenStep{};
+  const size_t count = members_.size();
+  auto rollback = [&](int st) {
+    for (size_t k = 0; k < count; ++k) members_[k].policy = step.before[k];
+    return st;
+  };
+  const std::vector<bb200_step_plan>& plans = step.plans;
+  const std::vector<uint32_t>& active = step.active;
+  if (active.empty()) return BB200_OK;
+  const uint32_t n_active = static_cast<uint32_t>(active.size());
+  auto resamples_kld = [&](uint32_t k) { return plans[k].resample != 0 && plans[k].opts.min_particles < plans[k].opts.max_particles; };
+  BatchStepArgs& a = step.args;
+  cudaStream_t stream = stream_;
+  int st = BB200_OK;
+  if (clustered != nullptr) st = ensure_select_scratch();
+  if (st != BB200_OK) return rollback(st);
+  // update_clustered: the pre-step cluster table and how the step may change each member (batch_cluster_table_kernel).
+  if (clustered != nullptr) {
+    for (uint32_t j = 0; j < n_active; ++j) {
+      const uint32_t k = active[j];
+      const Member& m = members_[k];
+      const bb200_step_plan& plan = plans[k];
+      BatchClusterMember& c = cl_.table_host.get()[j];
+      c = BatchClusterMember{};
+      c.offset = m.offset;
+      c.table_offset = m.table_offset;
+      c.starts_offset = m.offset + k;
+      c.n = static_cast<uint32_t>(m.n);
+      c.table_mask = m.table_slots - 1;
+      c.cur = static_cast<uint32_t>(m.cur);
+      c.pivot_x = m.pivot[0];
+      c.pivot_y = m.pivot[1];
+      BatchClusterPost& q = sel_.post_host.get()[j];
+      q = BatchClusterPost{};
+      q.scratch_offset = sel_.offsets[k];
+      q.capacity = static_cast<uint32_t>(m.capacity);
+      q.mode = plan.needs_ess ? 2 : plan.resample ? 1 : 0;
+      q.kld = resamples_kld(k) ? 1 : 0;
+    }
+  }
+
+  if (st == BB200_OK && clustered != nullptr)
+    st = check(cudaMemcpyAsync(cl_.table.get(), cl_.table_host.get(), n_active * sizeof(BatchClusterMember), cudaMemcpyHostToDevice, stream),
+               "upload cluster table");
+  if (st == BB200_OK && clustered != nullptr)
+    st = check(cudaMemcpyAsync(sel_.post.get(), sel_.post_host.get(), n_active * sizeof(BatchClusterPost), cudaMemcpyHostToDevice, stream),
+               "upload cluster steps");
+  if (st != BB200_OK) return rollback(st);
+  launches_ += static_cast<uint64_t>(launch_batch_step_tail(a, stream));
   st = check(cudaGetLastError(), "batch step launch");
   if (st != BB200_OK) return rollback(st);
   const bb200_cluster_param* cp = clustered != nullptr ? clustered->p : nullptr;

@@ -123,6 +123,17 @@ class Batch {
   int update_clustered(const double* control_poses, const bb200_measurement* measurements, const uint8_t* present, const bb200_cluster_param& p,
                        bb200_update_result* out, bb200_estimate* clustered, uint32_t* n_cells, uint32_t* n_clusters);
 
+  /// The first half of update_measurements / update_clustered for a step in which some members are weighed by the caller
+  /// (kind BB200_MEASUREMENT_WEIGHTS; bb200_amcl_batch_update_begin): the policies' decisions, the conversion of scans
+  /// and clouds, the propagate and the built-in reweight of the other members are enqueued, and views[m] gives member m's
+  /// propagated states and its slice of the factor buffer.  Nothing is synchronised; the step stays open until update_end.
+  int update_begin(const double* control_poses, const bb200_measurement* measurements, const uint8_t* present, bb200_weigh_view* views);
+  /// The second half: w *= factor for the weighed members, then the rest of the step and, with `cluster`, the cluster
+  /// estimates as update_clustered computes them; the step's one synchronisation.  Atomic as update.
+  int update_end(const bb200_cluster_param* cluster, bb200_update_result* out, bb200_estimate* clustered, uint32_t* n_cells, uint32_t* n_clusters);
+  /// Whether a step is open (update_begin .. update_end): the C ABI then refuses every other call but destroy.
+  bool step_open() const { return open_.open; }
+
  private:
   /// Where update_clustered's step writes the cluster estimates.
   struct ClusteredOut {
@@ -232,6 +243,22 @@ class Batch {
   /// With `clustered`, the step also selects every updated member's cluster estimate on the device (update_clustered).
   int step(const double* control_poses, const bb200_measurement* in, const uint8_t* present, bb200_update_result* out,
            const ClusteredOut* clustered = nullptr);
+  /// The halves of step: plans, uploads and launch_batch_step_head (views: written for update_begin), then the tail
+  /// launches, the synchronisation and the commit.  Between the two the step is open_.
+  int step_begin(const double* control_poses, const bb200_measurement* in, const uint8_t* present, bb200_weigh_view* views);
+  int step_end(const ClusteredOut* clustered, bb200_update_result* out);
+  /// A step between step_begin and step_end: the policies to put back on failure, the plans, the updating members and
+  /// the launch arguments.
+  struct OpenStep {
+    bool open{false};
+    std::vector<AmclPolicy> before;
+    std::vector<bb200_step_plan> plans;
+    std::vector<uint32_t> active;
+    bool kld{false};
+    BatchStepArgs args{};
+  };
+  OpenStep open_;
+  DeviceBuffer<double> factors_;  // weighed members' factors, laid out like weights_ (grown by the first such step)
   bool ensure_hits(uint64_t words);
   int set_map(const MapTables& tables);
   int add_map(const MapTables& tables, int* id);

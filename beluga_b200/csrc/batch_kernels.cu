@@ -160,6 +160,14 @@ __global__ void __launch_bounds__(kBeamThreads, kBeamBlocksPerSm) batch_reweight
                       m.n_points, s.scalars + k, local);
 }
 
+/// apply_factors_kernel per weighed member: w *= factor over the member's slice, the largest weight into its scalars.
+__global__ void __launch_bounds__(kMaxThreads) batch_weigh_kernel(BatchStepArgs s) {
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kBatchWeighRow, blockIdx.x, local, count);
+  const BatchMember& m = s.members[k];
+  apply_factors_block(s.weights + m.offset, s.factors + m.offset, m.n, s.scalars + k, local, count);
+}
+
 /// quantize_scan_kernel per member: the exponent from the member's own largest weight, its own look-back state.
 __global__ void __launch_bounds__(kQsThreads) batch_scan_kernel(BatchStepArgs s) {
   uint32_t local, count;
@@ -598,11 +606,11 @@ __global__ void __launch_bounds__(kRayThreads) batch_cast_rays_kernel(BatchRayAr
 }
 
 template <bool kTable>
-int launch_batch_step_from(const BatchStepArgs& s, cudaStream_t stream) {
+int launch_batch_step_head_from(const BatchStepArgs& s, cudaStream_t stream) {
   const uint32_t reset = std::max(s.n_members, s.ctas[kBatchScan]);
   batch_begin_kernel<<<std::max(1u, std::min((reset + 255u) / 256u, kSmCount * 4u)), 256, 0, stream>>>(s);
   batch_propagate_kernel<<<s.ctas[kBatchPropagate], kPrThreads, 0, stream>>>(s);
-  int launches = 4;
+  int launches = 2;
   if (s.forms & (1 << kBatchField)) {
     const size_t smem = static_cast<size_t>(std::min(s.max_points, kChunkBeams)) * sizeof(double2);
     batch_reweight_kernel<kTable><<<s.ctas[kBatchReweight], kRwThreads, smem, stream>>>(s);
@@ -615,6 +623,16 @@ int launch_batch_step_from(const BatchStepArgs& s, cudaStream_t stream) {
   }
   if (s.forms & (1 << kBatchBeamFused)) {
     batch_reweight_beam_kernel<kTable><<<s.ctas[kBatchReweightBeam], kBeamThreads, 0, stream>>>(s);
+    launches += 1;
+  }
+  return launches;
+}
+
+template <bool kTable>
+int launch_batch_step_tail_from(const BatchStepArgs& s, cudaStream_t stream) {
+  int launches = 2;
+  if (s.weigh_ctas > 0) {
+    batch_weigh_kernel<<<s.weigh_ctas, kMaxThreads, 0, stream>>>(s);
     launches += 1;
   }
   batch_scan_kernel<<<s.ctas[kBatchScan], kQsThreads, 0, stream>>>(s);
@@ -641,7 +659,7 @@ uint32_t batch_scan_tiles(uint64_t n) { return scan_tile_count(n); }
 void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunches]) {
   out[kBatchPropagate] = static_cast<uint32_t>((m.n + kPrThreads - 1) / kPrThreads);
   out[kBatchReweight] = out[kBatchReweightWalk] = out[kBatchReweightBeam] = 0;
-  out[batch_reweight_row(form)] = static_cast<uint32_t>((m.n + kRwThreads - 1) / kRwThreads);
+  if (form != kBatchWeighed) out[batch_reweight_row(form)] = static_cast<uint32_t>((m.n + kRwThreads - 1) / kRwThreads);
   out[kBatchScan] = scan_tile_count(m.n);
   // the partition launch_resample / launch_moments would use for a single filter of this size
   if (!m.resample) {
@@ -660,8 +678,14 @@ void batch_post_ctas(const BatchMember& m, uint32_t out[3]) {
   out[2] = ess ? moments_blocks(m.n) : 0u;  // launch_normalize's partition
 }
 
-int launch_batch_step(const BatchStepArgs& s, cudaStream_t stream) {
-  return s.maps != nullptr ? launch_batch_step_from<true>(s, stream) : launch_batch_step_from<false>(s, stream);
+uint32_t batch_weigh_ctas(const BatchMember& m) { return static_cast<uint32_t>(std::min<uint64_t>((m.n + kMaxThreads - 1) / kMaxThreads, kStreamMaxBlocks)); }
+
+int launch_batch_step_head(const BatchStepArgs& s, cudaStream_t stream) {
+  return s.maps != nullptr ? launch_batch_step_head_from<true>(s, stream) : launch_batch_step_head_from<false>(s, stream);
+}
+
+int launch_batch_step_tail(const BatchStepArgs& s, cudaStream_t stream) {
+  return s.maps != nullptr ? launch_batch_step_tail_from<true>(s, stream) : launch_batch_step_tail_from<false>(s, stream);
 }
 
 uint32_t batch_points_ctas(const BatchPointsMember& m) {

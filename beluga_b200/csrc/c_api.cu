@@ -185,81 +185,115 @@ const char* bb200_last_error(const bb200_filter* f) { return f != nullptr ? f->i
   do {                                                \
     if (!(cond)) return BB200_ERR_INVALID_ARGUMENT;   \
   } while (0)
+// While a weighed step is open (bb200_amcl_update_begin .. _end) a filter refuses every call but the step's end and destroy;
+// a batch likewise between bb200_amcl_batch_update_begin and _end.
+#define BB_REFUSE_OPEN(filter)                                                                              \
+  do {                                                                                                      \
+    if ((filter).weigh_open()) {                                                                            \
+      (filter).record_error("a weighed step is open: only bb200_amcl_update_end and destroy are accepted"); \
+      return BB200_ERR_STATE;                                                                               \
+    }                                                                                                       \
+  } while (0)
+#define BB_REFUSE_OPEN_BATCH(batch)                                                                              \
+  do {                                                                                                           \
+    if ((batch) != nullptr && (batch)->impl.step_open()) {                                                       \
+      (batch)->impl.record_error("a weighed step is open: only bb200_amcl_batch_update_end and destroy are accepted"); \
+      return BB200_ERR_STATE;                                                                                    \
+    }                                                                                                            \
+  } while (0)
 
 int bb200_filter_set_likelihood_field_map(bb200_filter* f, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid, int prob) {
   BB_REQUIRE(f && p && grid);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.set_likelihood_field_map(*p, *grid, prob != 0); });
 }
 int bb200_filter_set_beam_map(bb200_filter* f, const bb200_beam_param* p, const bb200_occupancy_grid* grid) {
   BB_REQUIRE(f && p && grid);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.set_beam_map(*p, *grid); });
 }
 int bb200_filter_get_likelihood_field(const bb200_filter* f, float* out, uint64_t capacity) {
   BB_REQUIRE(f && out);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.get_likelihood_field(out, capacity); });
 }
 int bb200_filter_set_particles(bb200_filter* f, const double* states, const double* weights, uint64_t n) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.set_particles(states, weights, n); });
 }
 int bb200_filter_size(const bb200_filter* f, uint64_t* n) {
   BB_REQUIRE(f && n);
+  BB_REFUSE_OPEN(f->impl);
   *n = f->impl.size();
   return BB200_OK;
 }
 int bb200_filter_get_particles(bb200_filter* f, double* states, double* weights, uint64_t capacity) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.get_particles(states, weights, capacity); });
 }
 int bb200_filter_initialize_normal(bb200_filter* f, const double mean_xytheta[3], const double cov[9], uint64_t n) {
   BB_REQUIRE(f && mean_xytheta && cov);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.initialize_normal(mean_xytheta, cov, n); });
 }
 int bb200_filter_initialize_uniform(bb200_filter* f, uint64_t n) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.initialize_uniform(n); });
 }
 int bb200_filter_propagate(bb200_filter* f, const bb200_motion_sampling* s, uint32_t step) {
   BB_REQUIRE(f && s);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.propagate_reweight(s, step, nullptr, 0); });
 }
 int bb200_filter_reweight(bb200_filter* f, const double* points_xy, uint64_t n_points) {
   BB_REQUIRE(f && (points_xy || n_points == 0));
+  BB_REFUSE_OPEN(f->impl);
   static const double kNoPoints[2] = {0.0, 0.0};
   return guarded(f->impl, [&] { return f->impl.propagate_reweight(nullptr, 0, points_xy != nullptr ? points_xy : kNoPoints, n_points); });
 }
 int bb200_filter_propagate_reweight(bb200_filter* f, const bb200_motion_sampling* s, uint32_t step, const double* points_xy, uint64_t n_points) {
   BB_REQUIRE(f && s && (points_xy || n_points == 0));
+  BB_REFUSE_OPEN(f->impl);
   static const double kNoPoints[2] = {0.0, 0.0};
   return guarded(f->impl, [&] { return f->impl.propagate_reweight(s, step, points_xy != nullptr ? points_xy : kNoPoints, n_points); });
 }
 int bb200_filter_max_weight(bb200_filter* f, double* wmax) {
   BB_REQUIRE(f && wmax);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.max_weight(wmax); });
 }
 int bb200_filter_build_cdf(bb200_filter* f, double global_wmax, uint64_t* local_total, int* exponent) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.build_cdf(global_wmax, local_total, exponent); });
 }
 int bb200_filter_normalize_by(bb200_filter* f, uint64_t global_total, double* local_sum_sq) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.normalize_by(global_total, local_sum_sq); });
 }
 int bb200_filter_normalize(bb200_filter* f, double* factor, double* sum_sq) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.normalize(factor, sum_sq); });
 }
 int bb200_filter_resample(bb200_filter* f, const bb200_resample_opts* o, uint64_t* new_size) {
   BB_REQUIRE(f && o);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.resample(*o, new_size); });
 }
 int bb200_filter_resample_range(bb200_filter* f, const bb200_resample_opts* o, uint64_t global_total, uint64_t cdf_offset, uint64_t slot_begin,
                                 uint64_t slot_end) {
   BB_REQUIRE(f && o);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.resample_range(*o, global_total, cdf_offset, slot_begin, slot_end); });
 }
 int bb200_filter_adopt(bb200_filter* f, uint64_t n, int from_staging) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.adopt(n, from_staging); });
 }
 int bb200_systematic_comb(uint64_t seed, uint32_t step, uint64_t global_total, uint64_t total_slots, uint64_t* stride, uint64_t* offset) {
@@ -276,39 +310,48 @@ int bb200_estimate_from_moments(const double moments[9], const double pivot_xy[2
 }
 int bb200_filter_set_stream(bb200_filter* f, void* cuda_stream) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.set_stream(cuda_stream); });
 }
 int bb200_filter_enqueue_propagate_reweight(bb200_filter* f, const bb200_motion_sampling* s, uint32_t step, const double* points_xy, uint64_t n_points) {
   BB_REQUIRE(f && s && points_xy);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.enqueue_propagate_reweight(s, step, points_xy, n_points); });
 }
 int bb200_filter_enqueue_build_cdf(bb200_filter* f) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.enqueue_build_cdf(-1.0); });
 }
 int bb200_filter_enqueue_resample_range(bb200_filter* f, const bb200_resample_opts* o, uint64_t global_total, uint64_t cdf_offset, uint64_t slot_begin,
                                         uint64_t slot_end) {
   BB_REQUIRE(f && o);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.enqueue_resample_range(*o, global_total, cdf_offset, slot_begin, slot_end); });
 }
 int bb200_filter_enqueue_adopt(bb200_filter* f, uint64_t n) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.enqueue_adopt(n); });
 }
 int bb200_filter_enqueue_moments(bb200_filter* f, const double pivot_xy[2]) {
   BB_REQUIRE(f && pivot_xy);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.enqueue_moments(pivot_xy); });
 }
 int bb200_filter_ancestors(bb200_filter* f, int64_t* out, uint64_t capacity) {
   BB_REQUIRE(f && out);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.ancestors(out, capacity); });
 }
 int bb200_filter_cdf(bb200_filter* f, uint64_t* out, uint64_t capacity) {
   BB_REQUIRE(f && out);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.cdf(out, capacity); });
 }
 int bb200_filter_estimate(bb200_filter* f, bb200_estimate* out) {
   BB_REQUIRE(f && out);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.estimate(out); });
 }
 void bb200_cluster_param_default(bb200_cluster_param* p) {
@@ -320,6 +363,7 @@ void bb200_cluster_param_default(bb200_cluster_param* p) {
 int bb200_filter_cluster_estimate(bb200_filter* f, const bb200_cluster_param* p, bb200_estimate* out, uint32_t* cluster_ids, uint64_t ids_capacity,
                                   uint32_t* n_cells, uint32_t* n_clusters) {
   BB_REQUIRE(f && p);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.cluster_estimate(*p, out, cluster_ids, ids_capacity, n_cells, n_clusters); });
 }
 int bb200_cluster_select_host(const bb200_cluster_cell* cells, uint64_t n_cells, uint64_t n_particles, const bb200_cluster_param* p,
@@ -344,15 +388,18 @@ int bb200_cluster_select_host(const bb200_cluster_cell* cells, uint64_t n_cells,
 int bb200_filter_particle_histogram(bb200_filter* f, double linear_resolution, double angular_resolution, bb200_cluster_cell* bins, uint64_t capacity,
                                     uint64_t* n_bins, double* max_bin_weight) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.particle_histogram(linear_resolution, angular_resolution, bins, capacity, n_bins, max_bin_weight); });
 }
 int bb200_filter_sample_states(bb200_filter* f, uint64_t count, uint32_t step, double* states_out) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.sample_states(count, step, states_out); });
 }
 int bb200_filter_cast_rays(bb200_filter* f, const double* poses, uint64_t n_poses, const double* bearings_cs, uint64_t n_bearings, double max_range,
                            double* ranges) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.cast_rays(poses, n_poses, bearings_cs, n_bearings, max_range, ranges); });
 }
 
@@ -425,15 +472,18 @@ int bb200_likelihood_field_to_occupancy(const float* field, uint64_t n, int8_t* 
 
 int bb200_filter_moments(bb200_filter* f, const double pivot_xy[2], double out[9]) {
   BB_REQUIRE(f && pivot_xy && out);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.moments(pivot_xy, out); });
 }
 int bb200_filter_set_timing(bb200_filter* f, int enabled) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   f->impl.set_timing(enabled != 0);
   return BB200_OK;
 }
 int bb200_filter_clear_timings(bb200_filter* f) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   f->impl.clear_timings();
   return BB200_OK;
 }
@@ -444,10 +494,12 @@ int bb200_filter_last_timings(const bb200_filter* f, const char** names, float* 
 uint64_t bb200_filter_launch_count(const bb200_filter* f) { return f != nullptr ? f->impl.launch_count() : 0; }
 int bb200_filter_synchronize(bb200_filter* f) {
   BB_REQUIRE(f);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.synchronize(); });
 }
 int bb200_filter_device_pointer(bb200_filter* f, int which, void** ptr, uint64_t* bytes) {
   BB_REQUIRE(f && ptr && bytes);
+  BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.device_pointer(which, ptr, bytes); });
 }
 
@@ -502,23 +554,35 @@ const char* bb200_amcl_last_error(const bb200_amcl* a) { return a != nullptr ? a
 bb200_filter* bb200_amcl_filter(bb200_amcl* a) { return a != nullptr ? a->filter_view : nullptr; }
 int bb200_amcl_initialize(bb200_amcl* a, const double mean_xytheta[3], const double cov[9]) {
   BB_REQUIRE(a && mean_xytheta && cov);
+  BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] { return a->impl.initialize(mean_xytheta, cov); });
 }
 int bb200_amcl_initialize_from_map(bb200_amcl* a) {
   BB_REQUIRE(a);
+  BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] { return a->impl.initialize_from_map(); });
 }
 int bb200_amcl_initialize_states(bb200_amcl* a, const double* states, const double* weights, uint64_t n) {
   BB_REQUIRE(a);
+  BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] { return a->impl.initialize_states(states, weights, n); });
 }
 void bb200_amcl_force_update(bb200_amcl* a) {
-  if (a != nullptr) a->impl.force_update();
+  if (a != nullptr && !a->impl.filter().weigh_open()) a->impl.force_update();
 }
 int bb200_amcl_update(bb200_amcl* a, const double control_pose[4], const double* points_xy, uint64_t n_points, bb200_update_result* out) {
   BB_REQUIRE(a && control_pose && out && (points_xy || n_points == 0));
+  BB_REFUSE_OPEN(a->impl.filter());
   static const double kNoPoints[2] = {0.0, 0.0};
   return guarded(a->impl, [&] { return a->impl.update(control_pose, points_xy != nullptr ? points_xy : kNoPoints, n_points, out); });
+}
+int bb200_amcl_update_begin(bb200_amcl* a, const double control_pose[4], bb200_weigh_view* view) {
+  BB_REQUIRE(a && control_pose && view);
+  return guarded(a->impl, [&] { return a->impl.update_begin(control_pose, view); });
+}
+int bb200_amcl_update_end(bb200_amcl* a, bb200_update_result* out) {
+  BB_REQUIRE(a && out);
+  return guarded(a->impl, [&] { return a->impl.update_end(out); });
 }
 int bb200_take_evenly_indices(uint64_t size, uint64_t count, uint64_t* indices, uint64_t capacity, uint64_t* n_indices) {
   BB_REQUIRE(indices && n_indices);
@@ -582,6 +646,7 @@ const char* const kCloudRefused = "point cloud: datatype must be 7 (FLOAT32) or 
 
 int bb200_amcl_update_scan(bb200_amcl* a, const double control_pose[4], const bb200_laser_scan* scan, bb200_update_result* out) {
   BB_REQUIRE(a && control_pose && scan && out);
+  BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] {
     std::vector<double> points;
     uint64_t n = 0;
@@ -625,6 +690,7 @@ int bb200_point_cloud_to_points(const bb200_point_cloud* cloud, double* points_x
 
 int bb200_amcl_update_point_cloud(bb200_amcl* a, const double control_pose[4], const bb200_point_cloud* cloud, bb200_update_result* out) {
   BB_REQUIRE(a && control_pose && cloud && out);
+  BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] {
     std::vector<double> points;
     uint64_t n = 0;
@@ -641,14 +707,17 @@ int bb200_amcl_update_point_cloud(bb200_amcl* a, const double control_pose[4], c
 
 int bb200_amcl_export_shard(bb200_amcl* a, void* out256) {
   BB_REQUIRE(a && out256);
+  BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] { return a->impl.filter().link().export_handles(out256); });
 }
 int bb200_amcl_join_shards(bb200_amcl* a, int world, int rank, const void* handles) {
   BB_REQUIRE(a && handles);
+  BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] { return a->impl.filter().link().join_ipc(world, rank, handles); });
 }
 int bb200_amcl_leave_shards(bb200_amcl* a) {
   BB_REQUIRE(a);
+  BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] {
     bb200::Filter& f = a->impl.filter();
     return f.link().leave(f.stream());
@@ -1018,6 +1087,7 @@ int bb200_amcl_batch_create_with_flags(const bb200_amcl_param* params, const bb2
   return create_batch(params, motions, n_members, flags, out);
 }
 int bb200_amcl_batch_member_size(const bb200_amcl_batch* b, int member, uint64_t* n) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && n);
   return guarded(b->impl, [&] { return b->impl.member_size(member, n); });
 }
@@ -1026,124 +1096,162 @@ const char* bb200_amcl_batch_last_error(const bb200_amcl_batch* b) { return b !=
 int bb200_amcl_batch_members(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.members() : 0; }
 int bb200_amcl_batch_set_likelihood_field_map(bb200_amcl_batch* b, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid,
                                               int prob) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && p && grid);
   return guarded(b->impl, [&] { return b->impl.set_likelihood_field_map(*p, *grid, prob != 0); });
 }
 int bb200_amcl_batch_set_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p, const bb200_occupancy_grid* grid) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && p && grid);
   return guarded(b->impl, [&] { return b->impl.set_beam_map(*p, *grid); });
 }
 int bb200_amcl_batch_add_likelihood_field_map(bb200_amcl_batch* b, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid,
                                               int prob, int* map_id) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && p && grid && map_id);
   return guarded(b->impl, [&] { return b->impl.add_likelihood_field_map(*p, *grid, prob != 0, map_id); });
 }
 int bb200_amcl_batch_add_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p, const bb200_occupancy_grid* grid, int* map_id) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && p && grid && map_id);
   return guarded(b->impl, [&] { return b->impl.add_beam_map(*p, *grid, map_id); });
 }
 int bb200_amcl_batch_update_map(bb200_amcl_batch* b, int member, int map_id) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.update_map(member, map_id); });
 }
 int bb200_amcl_batch_member_map(const bb200_amcl_batch* b, int member, int* map_id) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && map_id);
   return guarded(b->impl, [&] { return b->impl.member_map(member, map_id); });
 }
 int bb200_amcl_batch_remove_map(bb200_amcl_batch* b, int map_id) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.remove_map(map_id); });
 }
 int bb200_amcl_batch_get_likelihood_field(const bb200_amcl_batch* b, int map_id, float* out, uint64_t capacity) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && out);
   return guarded(b->impl, [&] { return b->impl.get_likelihood_field(map_id, out, capacity); });
 }
 int bb200_amcl_batch_initialize(bb200_amcl_batch* b, int member, const double mean_xytheta[3], const double cov[9]) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && mean_xytheta && cov);
   return guarded(b->impl, [&] { return b->impl.initialize(member, mean_xytheta, cov); });
 }
 int bb200_amcl_batch_initialize_from_map(bb200_amcl_batch* b, int member) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.initialize_from_map(member); });
 }
 int bb200_amcl_batch_initialize_states(bb200_amcl_batch* b, int member, const double* states, const double* weights, uint64_t n) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.initialize_states(member, states, weights, n); });
 }
 int bb200_amcl_batch_force_update(bb200_amcl_batch* b, int member) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b);
   return b->impl.force_update(member);
 }
 int bb200_amcl_batch_get_particles(bb200_amcl_batch* b, int member, double* states, double* weights, uint64_t capacity) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.get_particles(member, states, weights, capacity); });
 }
 int bb200_amcl_batch_ancestors(bb200_amcl_batch* b, int member, int64_t* out, uint64_t capacity) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && (out || capacity == 0));
   return guarded(b->impl, [&] { return b->impl.ancestors(member, out, capacity); });
 }
 int bb200_amcl_batch_cluster_estimate(bb200_amcl_batch* b, int member, const bb200_cluster_param* p, bb200_estimate* out) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && p && out);
   return guarded(b->impl, [&] { return b->impl.cluster_estimate(member, *p, out); });
 }
 int bb200_amcl_batch_cluster_estimates(bb200_amcl_batch* b, const bb200_cluster_param* p, const uint8_t* present, bb200_estimate* out,
                                        uint32_t* n_cells, uint32_t* n_clusters) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && p && out);
   return guarded(b->impl, [&] { return b->impl.cluster_estimates(*p, present, out, n_cells, n_clusters); });
 }
 int bb200_amcl_batch_particle_histograms(bb200_amcl_batch* b, double linear_resolution, double angular_resolution, const uint8_t* present,
                                          bb200_cluster_cell* const* bins, const uint64_t* capacity, uint64_t* n_bins, double* max_bin_weight) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.particle_histograms(linear_resolution, angular_resolution, present, bins, capacity, n_bins, max_bin_weight); });
 }
 int bb200_amcl_batch_sample_states(bb200_amcl_batch* b, const uint64_t* counts, uint32_t step, const uint8_t* present, double* const* states_out) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && counts && states_out);
   return guarded(b->impl, [&] { return b->impl.sample_states(counts, step, present, states_out); });
 }
 int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, const double* const* points_xy, const uint64_t* n_points,
                             const uint8_t* present, bb200_update_result* out) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && control_poses && points_xy && n_points && out);
   return guarded(b->impl, [&] { return b->impl.update(control_poses, points_xy, n_points, present, out); });
 }
 int bb200_amcl_batch_update_measurements(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements,
                                          const uint8_t* present, bb200_update_result* out) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && control_poses && measurements && out);
   return guarded(b->impl, [&] { return b->impl.update_measurements(control_poses, measurements, present, out); });
 }
 int bb200_amcl_batch_update_clustered(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements,
                                       const uint8_t* present, const bb200_cluster_param* p, bb200_update_result* out, bb200_estimate* clustered,
                                       uint32_t* n_cells, uint32_t* n_clusters) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && control_poses && measurements && p && out && clustered);
   return guarded(b->impl, [&] { return b->impl.update_clustered(control_poses, measurements, present, *p, out, clustered, n_cells, n_clusters); });
 }
+int bb200_amcl_batch_update_begin(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements, const uint8_t* present,
+                                  bb200_weigh_view* views) {
+  BB_REQUIRE(b && control_poses && measurements && views);
+  return guarded(b->impl, [&] { return b->impl.update_begin(control_poses, measurements, present, views); });
+}
+int bb200_amcl_batch_update_end(bb200_amcl_batch* b, const bb200_cluster_param* cluster, bb200_update_result* out, bb200_estimate* clustered,
+                                uint32_t* n_cells, uint32_t* n_clusters) {
+  BB_REQUIRE(b && out && (cluster == nullptr || clustered != nullptr));
+  return guarded(b->impl, [&] { return b->impl.update_end(cluster, out, clustered, n_cells, n_clusters); });
+}
 int bb200_amcl_batch_cast_rays(bb200_amcl_batch* b, const uint8_t* present, const int* map_ids, const double* const* poses, const uint64_t* n_poses,
                                const double* const* bearings_cs, const uint64_t* n_bearings, const double* max_range, double* const* ranges) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && poses && n_poses && bearings_cs && n_bearings && max_range && ranges);
   return guarded(b->impl, [&] { return b->impl.cast_rays(present, map_ids, poses, n_poses, bearings_cs, n_bearings, max_range, ranges); });
 }
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.launch_count() : 0; }
 int bb200_amcl_batch_add_member(bb200_amcl_batch* b, const bb200_amcl_param* params, const bb200_motion_param* motion, int* member) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && params && motion && member);
   return guarded(b->impl, [&] { return b->impl.add_member(*params, *motion, member); });
 }
 int bb200_amcl_batch_remove_member(bb200_amcl_batch* b, int member) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.remove_member(member); });
 }
 int bb200_amcl_batch_member_active(const bb200_amcl_batch* b, int member, int* active) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && active);
   return guarded(b->impl, [&] { return b->impl.member_active(member, active); });
 }
 
 int bb200_amcl_batch_export_members(bb200_amcl_batch* b, const uint8_t* present, void* const* out, const uint64_t* capacity, uint64_t* size) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && size);
   return guarded(b->impl, [&] { return b->impl.export_members(present, out, capacity, size); });
 }
 int bb200_amcl_batch_export_member(bb200_amcl_batch* b, int member, void* out, uint64_t capacity, uint64_t* size) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && size);
   return guarded(b->impl, [&] { return b->impl.export_member(member, out, capacity, size); });
 }
 int bb200_amcl_batch_import_member(bb200_amcl_batch* b, const void* blob, uint64_t size, int map_id, int* member) {
+  BB_REFUSE_OPEN_BATCH(b);
   BB_REQUIRE(b && blob && member);
   return guarded(b->impl, [&] { return b->impl.import_member(blob, size, map_id, member); });
 }
@@ -1199,6 +1307,7 @@ int bb200_amcl_state_params(const void* blob, uint64_t size, bb200_amcl_param* p
 }
 int bb200_amcl_export_state(bb200_amcl* a, void* out, uint64_t capacity, uint64_t* size) {
   BB_REQUIRE(a && size);
+  BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] { return a->impl.export_state(out, capacity, size); });
 }
 int bb200_amcl_create_from_state(const void* blob, uint64_t size, int device, bb200_amcl** out) {
@@ -1226,10 +1335,11 @@ int bb200_amcl_create_from_state(const void* blob, uint64_t size, int device, bb
 
 int bb200_amcl_plan_update(bb200_amcl* a, const double control_pose[4], bb200_step_plan* plan) {
   BB_REQUIRE(a && control_pose && plan);
+  BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] { return a->impl.plan_update(control_pose, plan); });
 }
 void bb200_amcl_commit_update(bb200_amcl* a, int resampled, double random_state_probability) {
-  if (a != nullptr) a->impl.commit_update(resampled, random_state_probability);
+  if (a != nullptr && !a->impl.filter().weigh_open()) a->impl.commit_update(resampled, random_state_probability);
 }
 int bb200_motion_sampling_from_control(const bb200_motion_param* p, const double pose[4], const double previous_pose[4], bb200_motion_sampling* out) {
   BB_REQUIRE(p && pose && previous_pose && out);

@@ -12,6 +12,11 @@ __global__ void __launch_bounds__(kMaxThreads) max_weight_kernel(const double* _
   max_weight_block(weights, n, scalars, blockIdx.x, gridDim.x);
 }
 
+__global__ void __launch_bounds__(kMaxThreads) apply_factors_kernel(double* __restrict__ weights, const double* __restrict__ factors, uint64_t n,
+                                                                    Scalars* scalars) {
+  apply_factors_block(weights, factors, n, scalars, blockIdx.x, gridDim.x);
+}
+
 __global__ void prepare_cdf_kernel(Scalars* s, double host_wmax, int ceil_log2_count, unsigned long long* tile_state, uint32_t n_tiles) {
   for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n_tiles; t += gridDim.x * blockDim.x) tile_state[t] = 0;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -62,6 +67,12 @@ void launch_max_weight(const double* weights, uint64_t n, Scalars* scalars, cuda
   if (n == 0) return;
   const unsigned blocks = static_cast<unsigned>(std::min<uint64_t>((n + 511) / 512, kStreamMaxBlocks));
   max_weight_kernel<<<blocks, 512, 0, stream>>>(weights, n, scalars);
+}
+
+void launch_apply_factors(double* weights, const double* factors, uint64_t n, Scalars* scalars, cudaStream_t stream) {
+  if (n == 0) return;
+  const unsigned blocks = static_cast<unsigned>(std::min<uint64_t>((n + kMaxThreads - 1) / kMaxThreads, kStreamMaxBlocks));
+  apply_factors_kernel<<<blocks, kMaxThreads, 0, stream>>>(weights, factors, n, scalars);
 }
 
 uint32_t scan_tile_count(uint64_t n) { return static_cast<uint32_t>((n + kQsTile - 1) / kQsTile); }

@@ -22,6 +22,22 @@ __device__ __forceinline__ void max_weight_block(const double* __restrict__ weig
   if (threadIdx.x == 0 && m != 0) atomicMax(&scalars->wmax_bits, m);
 }
 
+/// Block `block` of `grid` of apply_factors_kernel: w_i = w_i * factors_i, the multiply of the built-in reweight
+/// (store_reweighted), and the largest selectable product into scalars->wmax_bits.  24 bytes per particle.
+__device__ __forceinline__ void apply_factors_block(double* __restrict__ weights, const double* __restrict__ factors, uint64_t n, Scalars* scalars,
+                                                    uint32_t block, uint32_t grid) {
+  __shared__ unsigned long long s_red[kMaxThreads / kWarp];
+  unsigned long long m = 0;
+  for (uint64_t i = static_cast<uint64_t>(block) * kMaxThreads + threadIdx.x; i < n; i += static_cast<uint64_t>(grid) * kMaxThreads) {
+    const double updated = weights[i] * factors[i];
+    weights[i] = updated;
+    const unsigned long long b = weight_order_bits(updated);
+    m = b > m ? b : m;
+  }
+  m = block_max_u64<kMaxThreads>(m, s_red);
+  if (threadIdx.x == 0 && m != 0) atomicMax(&scalars->wmax_bits, m);
+}
+
 // ---- fixed-point CDF ------------------------------------------------------------------------------
 // q_i = floor(w_i * 2^e) with e chosen so that the largest weight lands in [2^(P-1), 2^P),
 // P = min(52, 62 - ceil(log2(N_global))): the total stays below 2^62 and integer addition is

@@ -1187,15 +1187,55 @@ int Filter::resample_kld(const bb200_resample_opts& o, uint64_t* accepted) {
   return BB200_OK;
 }
 
-int Filter::step_resample(const bb200_motion_sampling& sampling, uint32_t step, const double* points_xy, uint64_t n_points,
-                          const bb200_resample_opts& o, bb200_estimate* est, double* weight_sum, uint64_t* new_size) {
-  int st = step_begin(sampling, step, points_xy, n_points, o, true);
-  for (int phase = kPhaseReweight; st == BB200_OK && phase <= kPhaseFinish; ++phase) st = step_phase(phase);
+int Filter::finish_resample(bb200_estimate* est, double* weight_sum, uint64_t* new_size) {
+  int st = BB200_OK;
+  for (int phase = kPhaseCdf; st == BB200_OK && phase <= kPhaseFinish; ++phase) st = step_phase(phase);
   if (st != BB200_OK) {
     step_.active = false;
     return st;
   }
   return step_end(est, weight_sum, new_size, nullptr);
+}
+
+int Filter::weigh_begin(const bb200_motion_sampling& sampling, uint32_t step, const bb200_resample_opts& o, bool fused, bool injects) {
+  if (link_.world() > 1 || config_.global_count != capacity_) return fail(BB200_ERR_STATE, "a weighed step runs on one filter, not on shards");
+  if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
+  if (o.max_particles == 0 || o.max_particles > capacity_) return fail(BB200_ERR_CAPACITY, "max_particles exceeds the filter capacity");
+  if (injects && map_.n_free == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
+  BB_CHECK(cudaSetDevice(config_.device));
+  if (factors_.get() == nullptr) BB_CHECK(factors_.allocate(capacity_));
+  const MotionSampling s = to_kernel_sampling(sampling);
+  mark("begin_step");
+  if (fused) {
+    step_ = StepContext{};
+    summary_host_.get()->error = 0;
+    step_.active = true;
+    step_.sampling = s;
+    step_.step = step;
+    step_.opts = o;
+    step_.resample_planned = true;
+    // the scalars and the CDF's scan state, as kPhaseReweight resets them; no schedule and no table to prefetch
+    launch_begin_fused_step(scalars_.get(), tile_state_.get(), scan_tile_count(n_), sched_.get(), nullptr, 0, sched_tiles_.get(), 0, nullptr, 0, stream_);
+  } else {
+    launch_begin_step(scalars_.get(), stream_);
+  }
+  BB_LAUNCHED("begin_step");
+  mark("propagate");
+  launch_propagate(states_[cur_].get(), n_, true, s, config_.seed, step, first_index_, nullptr, stream_);
+  BB_LAUNCHED("propagate");
+  cdf_valid_ = false;
+  cloud_known_ = false;
+  return BB200_OK;
+}
+
+// On a step that does not take the fused path, normalize's build_cdf recomputes the largest weight this kernel posts (as
+// after the built-in reweight on that path); the fused path's quantize_scan reads it.
+int Filter::weigh_apply() {
+  BB_CHECK(cudaSetDevice(config_.device));
+  mark("apply_factors");
+  launch_apply_factors(weights_.get(), factors_.get(), n_, scalars_.get(), stream_);
+  BB_LAUNCHED("apply_factors");
+  return BB200_OK;
 }
 
 int Filter::ancestors(int64_t* out, uint64_t capacity) {

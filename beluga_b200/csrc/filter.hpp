@@ -100,10 +100,24 @@ class Filter {
   /// The first n states of the staging buffer, after this filter's stream has drained.
   int staging_states(double* out, uint64_t n);
 
-  /// Fused single-GPU step: propagate | reweight | normalize | resample | estimate with one
-  /// host synchronisation at the end (the composition Amcl::update performs every step).
-  int step_resample(const bb200_motion_sampling& sampling, uint32_t step, const double* points_xy, uint64_t n_points,
-                    const bb200_resample_opts& o, bb200_estimate* est, double* weight_sum, uint64_t* new_size);
+  /// The fused single-GPU step (propagate | reweight | normalize | resample | estimate with one host synchronisation) is
+  /// step_begin, kPhaseReweight and then this: CDF, resample, moments, and the synchronisation (step_end).
+  int finish_resample(bb200_estimate* est, double* weight_sum, uint64_t* new_size);
+
+  // ---- a step whose sensor model the caller runs (bb200_amcl_update_begin / _end) ----
+  /// Checks the step, allocates the factor buffer on first use and enqueues the reset and the propagate (the non-binned
+  /// propagate_kernel: no pose-bin schedule); no host synchronisation.  `fused`: the step then ends as the fused step
+  /// does (weigh_apply, then finish_resample); otherwise weigh_apply is followed by the blocking normalize / resample /
+  /// estimate.  `injects`: the plan may inject random states, which needs a map with free cells.
+  int weigh_begin(const bb200_motion_sampling& sampling, uint32_t step, const bb200_resample_opts& o, bool fused, bool injects);
+  /// Enqueues w *= factors over the particle set and the largest weight into the device scalars.
+  int weigh_apply();
+  /// Whether a weighed step is open on this filter: the C ABI then refuses every call but the step's end and destroy.
+  void set_weigh_open(bool open) { weigh_open_ = open; }
+  bool weigh_open() const { return weigh_open_; }
+  /// Device views of an open weighed step: the propagated states and the factors the caller writes, n of each.
+  const double* weigh_states() const { return reinterpret_cast<const double*>(states_[cur_].get()); }
+  double* weigh_factors() { return factors_.get(); }
 
   // Stream-ordered variants for callers that interleave collectives on the same stream (sharded
   // filters): nothing here synchronises with the host or reads results back.  Each blocking call
@@ -269,6 +283,8 @@ class Filter {
   DeviceBuffer<double> rays_;  // ray casts (grown on use): the poses, the bearings, then the ranges
   uint64_t cast_out_{0};       // offset of the last cast's ranges in rays_
   DeviceBuffer<uint32_t> beam_hits_;  // two-pass beam model: hit word per (beam, particle) of one pass
+  DeviceBuffer<double> factors_;      // weighed steps: the caller's likelihood per particle (capacity_, allocated on the first)
+  bool weigh_open_{false};
 
   double pivot_[2]{0.0, 0.0};
   bb200_estimate cloud_{};     // last estimate, when it describes the raw (unit-weight) cloud

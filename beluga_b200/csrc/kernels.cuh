@@ -310,6 +310,8 @@ void launch_reweight_beam_two_pass(const Pose2* states, double* weights, uint64_
 
 /// Largest weight only (when propagate/reweight ran separately or particles were set by hand).
 void launch_max_weight(const double* weights, uint64_t n, Scalars* scalars, cudaStream_t stream);
+/// A weighed step's sensor update: weights[i] *= factors[i] (the caller's likelihoods) | largest weight into the scalars.
+void launch_apply_factors(double* weights, const double* factors, uint64_t n, Scalars* scalars, cudaStream_t stream);
 
 /// Sets scalars->exponent from wmax (device value when host_wmax < 0) and resets the scan state.
 void launch_prepare_cdf(Scalars* scalars, double host_wmax, uint64_t global_count, unsigned long long* tile_state, uint32_t n_tiles,
@@ -447,7 +449,9 @@ enum BatchLaunch : int {
   kBatchLaunches = 6
 };
 /// The reweight forms of a batch step; BatchStepArgs::forms has bit f set when some member takes form f.
-enum BatchReweightPath : int { kBatchField = 0, kBatchBeamTwoPass = 1, kBatchBeamFused = 2 };
+/// kBatchWeighed: a member the caller weighs (bb200_amcl_batch_update_begin / _end); it has no CTA in the reweight rows and
+/// its CTAs in the kBatchWeighRow row instead.
+enum BatchReweightPath : int { kBatchField = 0, kBatchBeamTwoPass = 1, kBatchBeamFused = 2, kBatchWeighed = 3 };
 /// The CTA-range row of each reweight form.
 constexpr int batch_reweight_row(int form) {
   return form == kBatchField ? kBatchReweight : form == kBatchBeamTwoPass ? kBatchReweightWalk : kBatchReweightBeam;
@@ -517,18 +521,26 @@ struct BatchStepArgs {
   uint32_t post_ctas[2];          // total CTAs of batch_kld_kernel and batch_resampled_moments_kernel
   // Selective members (BatchMember::resample == kBatchResampleEss): total CTAs of batch_ess_kernel, 0 when the step has none.
   uint32_t ess_ctas;
+  // Members the caller weighs (after every field the other kernels read): total CTAs of batch_weigh_kernel (0 when the
+  // step has none) and the batch's factor buffer, laid out like the weights.
+  uint32_t weigh_ctas;
+  const double* factors;
 };
 static_assert(sizeof(BatchStepArgs) <= 1024, "the step's arguments travel as one kernel parameter block (4 KB at most)");
-/// Reset | propagate | reweight | quantise + scan | resample or normalise + moments.  The reweight takes one launch for the
-/// likelihood field, two for the beam model's two-pass form (walk, mixture) and one for its fused form, each issued
-/// when some member takes that form.  When some member runs the effective-sample-size test (args.ess_ctas > 0), one
-/// launch before the resample normalises its weights and decides.  After the resample, when some member resamples under
-/// KLD (args.kld set), one launch counts each such member's particles; and when some member resamples under KLD or runs
-/// the test, one launch sums the moments of every new particle set that a separate estimate pass reads in a standalone
-/// filter.  Returns the number of launches: 4 plus those, so 5 to 8 without either kind of member, 7 to 10 with KLD
-/// members or with selective ones, and 8 to 11 with both, whatever the members, their maps, their particle counts,
-/// their decisions, their accepted counts and their scans are.
-int launch_batch_step(const BatchStepArgs& args, cudaStream_t stream);
+/// Reset | propagate | reweight | [weigh] | quantise + scan | resample or normalise + moments, in two halves that each
+/// return their launch count: launch_batch_step_head enqueues the reset, the propagate and the reweight, and
+/// launch_batch_step_tail the rest.  The reweight takes one launch for the likelihood field, two for the beam model's
+/// two-pass form (walk, mixture) and one for its fused form, each issued when some member takes that form.  When some
+/// member is weighed by the caller (args.weigh_ctas > 0), the tail starts with one launch of w *= factor.  When some member
+/// runs the effective-sample-size test (args.ess_ctas > 0), one launch before the resample normalises its weights and
+/// decides.  After the resample, when some member resamples under KLD (args.kld set), one launch counts each such member's
+/// particles; and when some member resamples under KLD or runs the test, one launch sums the moments of every new particle
+/// set that a separate estimate pass reads in a standalone filter.  The two halves together: 4 launches plus those, so 5 to
+/// 8 without weighed, KLD or selective members, 7 to 10 with KLD members or with selective ones, and 8 to 11 with both,
+/// one more with weighed members, whatever the members, their maps, their particle counts, their decisions, their accepted
+/// counts and their scans are.
+int launch_batch_step_head(const BatchStepArgs& args, cudaStream_t stream);
+int launch_batch_step_tail(const BatchStepArgs& args, cudaStream_t stream);
 /// Scan tiles of a member of n particles (the quantise-scan CTAs it needs).
 uint32_t batch_scan_tiles(uint64_t n);
 
@@ -543,9 +555,11 @@ constexpr int kBatchPointsRow = kBatchLaunches;
 constexpr int kBatchKldRow = kBatchLaunches + 1;
 constexpr int kBatchMomentsRow = kBatchLaunches + 2;
 constexpr int kBatchEssRow = kBatchLaunches + 3;
-constexpr int kBatchRows = kBatchLaunches + 4;
+/// The row of batch_weigh_kernel: apply_factors_block's grid of a standalone filter of the member's size per weighed member.
+constexpr int kBatchWeighRow = kBatchLaunches + 4;
+constexpr int kBatchRows = kBatchLaunches + 5;
 /// How a member's measurement reaches a batch step (the values of bb200_measurement_kind).
-enum BatchInputKind : int { kBatchInputPoints = 0, kBatchInputScan = 1, kBatchInputCloud = 2 };
+enum BatchInputKind : int { kBatchInputPoints = 0, kBatchInputScan = 1, kBatchInputCloud = 2, kBatchInputWeights = 3 };
 /// One member of batch_points_kernel, built on the host every step (one per entry of the step's member table).
 struct BatchPointsMember {
   int kind;                   // BatchInputKind; kBatchInputPoints: the host wrote the points, no CTA
@@ -575,6 +589,8 @@ void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunch
 /// CTAs of a member in the rows kBatchKldRow, kBatchMomentsRow and kBatchEssRow: a KLD count when it may resample under KLD,
 /// the moments of a new set when it may resample under KLD or runs the effective-sample-size test, and that test.
 void batch_post_ctas(const BatchMember& m, uint32_t out[3]);
+/// CTAs of a weighed member in the kBatchWeighRow row.
+uint32_t batch_weigh_ctas(const BatchMember& m);
 
 /// One member of a batch's pose-sample draw (Filter::sample_states per member).
 struct BatchSampleMember {

@@ -478,6 +478,32 @@ int bb200_point_cloud_to_points(const bb200_point_cloud* cloud, double* points_x
  * bb200_sharded_amcl_update_point_cloud. */
 int bb200_amcl_update_point_cloud(bb200_amcl* a, const double control_pose[4], const bb200_point_cloud* cloud, bb200_update_result* out);
 
+/* A step weighed by the caller's own sensor model (the SensorModel template parameter of beluga::Amcl, amcl_core.hpp:74-81),
+ * in two calls.  bb200_amcl_update_begin makes the host decisions of bb200_amcl_update (update policy, every_n, control
+ * window, recovery probability, motion sampling), checks the step and enqueues the motion update on the filter's stream; it
+ * does not synchronise.  When the policies skip the step (updated = 0) nothing reaches the device.  Otherwise the caller
+ * writes factors[i] = L(states_i) for every particle, on `stream` or synchronised with it, and bb200_amcl_update_end then
+ * runs w_i *= factors_i (the built-in reweight's multiply) and everything bb200_amcl_update runs after its sensor model:
+ * normalize, the recovery estimator, every_n / selective / KLD resampling, injection and the estimate.  Factors that are
+ * 0, negative, NaN or +-inf follow the rules of a built-in weight of that value (weights_degenerate when none is left).
+ * With factors bit-equal to a stock model's likelihoods the step is byte-identical to bb200_amcl_update with that model.
+ *
+ * While a step is open every other call on the handle, and on its bb200_amcl_filter view, returns BB200_ERR_STATE;
+ * bb200_amcl_destroy is allowed.  bb200_amcl_update_end must follow every successful begin, skipped steps included, and
+ * returns BB200_ERR_STATE without one.  Both calls are atomic as bb200_amcl_update: on failure the policies, the control
+ * window and the recovery estimator are as before the begin, and the step is closed.  No map is needed, except for a step
+ * that may inject random states (BB200_ERR_STATE before any device work).  Sharded filters and shards refuse begin with
+ * BB200_ERR_STATE.  The factor buffer belongs to the filter and is allocated by the first begin. */
+typedef struct bb200_weigh_view {
+  int updated;           /* 0: the policies skip this step; end returns updated = 0 */
+  uint64_t n;            /* particles to weigh */
+  const double* states;  /* device: n x {cos, sin, x, y}, the propagated states */
+  double* factors;       /* device: n doubles the caller writes, L(state_i) */
+  void* stream;          /* cudaStream_t: order the weighing on it */
+} bb200_weigh_view;
+int bb200_amcl_update_begin(bb200_amcl* a, const double control_pose[4], bb200_weigh_view* view);
+int bb200_amcl_update_end(bb200_amcl* a, bb200_update_result* out);
+
 /* ---------------------------------------------------------------------------------------------
  * One filter over several GPUs (SURVEY 8e).  Particles are split into equal contiguous global index
  * ranges ("shards"); map and scan are replicated; the counter RNG is keyed by the GLOBAL particle /
@@ -730,7 +756,14 @@ int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, co
                             const uint8_t* present, bb200_update_result* out);
 /* One member's measurement in a step: base-frame points, a laser scan or a point cloud, each as the single filter's
  * bb200_amcl_update, bb200_amcl_update_scan and bb200_amcl_update_point_cloud take it.  Only the fields of `kind` are read. */
-typedef enum bb200_measurement_kind { BB200_MEASUREMENT_POINTS = 0, BB200_MEASUREMENT_SCAN = 1, BB200_MEASUREMENT_CLOUD = 2 } bb200_measurement_kind;
+/* BB200_MEASUREMENT_WEIGHTS: this member is weighed by the caller (bb200_amcl_batch_update_begin / _end only; the other
+ * update calls refuse it); no field of the measurement is read. */
+typedef enum bb200_measurement_kind {
+  BB200_MEASUREMENT_POINTS = 0,
+  BB200_MEASUREMENT_SCAN = 1,
+  BB200_MEASUREMENT_CLOUD = 2,
+  BB200_MEASUREMENT_WEIGHTS = 3
+} bb200_measurement_kind;
 typedef struct bb200_measurement {
   int kind;                        /* bb200_measurement_kind */
   const double* points_xy;         /* POINTS: n_points (x, y) pairs (NULL when n_points == 0) */
@@ -770,6 +803,25 @@ int bb200_amcl_batch_update_measurements(bb200_amcl_batch* b, const double* cont
 int bb200_amcl_batch_update_clustered(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements,
                                       const uint8_t* present, const bb200_cluster_param* p, bb200_update_result* out,
                                       bb200_estimate* clustered, uint32_t* n_cells, uint32_t* n_clusters);
+/* bb200_amcl_batch_update_measurements / _update_clustered in two calls, for a step in which some members are weighed by
+ * the caller's own sensor model (measurements[m].kind == BB200_MEASUREMENT_WEIGHTS): the semantics of
+ * bb200_amcl_update_begin / _end, per member.  begin makes every present member's host decisions, checks the step and
+ * enqueues the conversion of scans and clouds, the propagate and the built-in reweight of the members that pass points,
+ * scans or clouds, so that their sensor work overlaps the caller's; it does not synchronise.  views[m] (one per slot) is
+ * written for every slot: updated = 1 for a present member that updates in this step, and for a weighed one n, its current
+ * state slice and its slice of one batch-owned factor buffer laid out like the particle buffers, and the batch's stream.
+ * The caller writes factors[i] = L(state_i) for every particle of every weighed updating member, on that stream or
+ * synchronised with it.  end enqueues w *= factor for the weighed members (one launch, a CTA range per member), then the
+ * rest of the step and, with `cluster` (NULL: none), the cluster estimates of bb200_amcl_batch_update_clustered, and
+ * synchronises once.  A step without weighed members launches exactly what bb200_amcl_batch_update_measurements (or
+ * _update_clustered) launches.  Weighed members need no map unless their step may inject random states.  While a step is
+ * open every other call on the batch returns BB200_ERR_STATE, except bb200_amcl_batch_update_end and destroy; end without
+ * an open step returns BB200_ERR_STATE.  Both calls are atomic as bb200_amcl_batch_update_measurements; a failed end closes
+ * the step. */
+int bb200_amcl_batch_update_begin(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements, const uint8_t* present,
+                                  bb200_weigh_view* views);
+int bb200_amcl_batch_update_end(bb200_amcl_batch* b, const bb200_cluster_param* cluster, bb200_update_result* out, bb200_estimate* clustered,
+                                uint32_t* n_cells, uint32_t* n_clusters);
 /* Kernel launches issued by this batch so far (steps, initialisations, cluster estimates, particle-cloud histograms and
  * pose samples, ray casts, membership changes, and the beam model's map uploads). */
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b);

@@ -208,12 +208,21 @@ class Amcl {
     check(sensor_model_.attach(bb200_amcl_filter(handle_)));
   }
 
-  /// amcl_core.hpp:165-201
+  /// amcl_core.hpp:165-201.  With a caller's device sensor model (is_weighed_token_v of its token): begin, the token's
+  /// weigh on the views (not called when the policies skip the step) and end (bb200_amcl_update_begin / _end).  weigh must
+  /// not throw: the step would stay open and the filter then accepts nothing but its destruction.
   auto update(const state_type& control_action, measurement_type measurement) -> std::optional<estimation_type> {
-    const measurement_token token = sensor_model_(std::move(measurement));
-    static_assert(sizeof(std::pair<double, double>) == 2 * sizeof(double), "measurement points must be packed");
+    const auto token = sensor_model_(std::move(measurement));
     bb200_update_result r{};
-    check(bb200_amcl_update(handle_, control_action.data(), token.points.empty() ? nullptr : &token.points.front().first, token.points.size(), &r));
+    if constexpr (is_weighed_token_v<std::decay_t<decltype(token)>>) {
+      bb200_weigh_view view{};
+      check(bb200_amcl_update_begin(handle_, control_action.data(), &view));
+      if (view.updated) token.weigh(view.stream, view.states, view.n, view.factors);
+      check(bb200_amcl_update_end(handle_, &r));
+    } else {
+      static_assert(sizeof(std::pair<double, double>) == 2 * sizeof(double), "measurement points must be packed");
+      check(bb200_amcl_update(handle_, control_action.data(), token.points.empty() ? nullptr : &token.points.front().first, token.points.size(), &r));
+    }
     return estimate_of(r);
   }
 
@@ -625,6 +634,19 @@ class AmclBatch {
     explicit Measurement(const PointCloudView& cloud) : value(cloud) {}
     std::variant<std::vector<std::pair<double, double>>, LaserScanView, PointCloudView> value;
   };
+  /// The bb200_measurement of one member's measurement; a scan's or a cloud's C view goes to *scan or *cloud, which must
+  /// outlive the call it is passed to.
+  static bb200_measurement c_measurement(const Measurement& measurement, bb200_laser_scan* scan, bb200_point_cloud* cloud) {
+    const auto& v = measurement.value;
+    if (const auto* points = std::get_if<0>(&v))
+      return bb200_measurement{BB200_MEASUREMENT_POINTS, points->empty() ? nullptr : &points->front().first, points->size(), nullptr, nullptr};
+    if (const auto* s = std::get_if<LaserScanView>(&v)) {
+      *scan = s->c_view();
+      return bb200_measurement{BB200_MEASUREMENT_SCAN, nullptr, 0, scan, nullptr};
+    }
+    *cloud = std::get<PointCloudView>(v).c_view();
+    return bb200_measurement{BB200_MEASUREMENT_CLOUD, nullptr, 0, nullptr, cloud};
+  }
   /// update with member m's measurement in measurements[m], so that members with 2-D and 3-D lidars step in one call; scans
   /// and clouds are converted on the device (bb200_amcl_batch_update_measurements).  Every member's result equals its
   /// standalone Amcl::update's with the same measurement.  Throws Error(BB200_ERR_INVALID_ARGUMENT) before any member
@@ -640,20 +662,40 @@ class AmclBatch {
     std::vector<bb200_measurement> in(k);
     std::vector<std::uint8_t> mask(present != nullptr ? k : 0);
     for (std::size_t m = 0; m < k; ++m) {
-      const auto& v = measurements[m].value;
-      if (const auto* points = std::get_if<0>(&v)) {
-        in[m] = bb200_measurement{BB200_MEASUREMENT_POINTS, points->empty() ? nullptr : &points->front().first, points->size(), nullptr, nullptr};
-      } else if (const auto* scan = std::get_if<LaserScanView>(&v)) {
-        scans[m] = scan->c_view();
-        in[m] = bb200_measurement{BB200_MEASUREMENT_SCAN, nullptr, 0, &scans[m], nullptr};
-      } else {
-        clouds[m] = std::get<PointCloudView>(v).c_view();
-        in[m] = bb200_measurement{BB200_MEASUREMENT_CLOUD, nullptr, 0, nullptr, &clouds[m]};
-      }
+      in[m] = c_measurement(measurements[m], &scans[m], &clouds[m]);
       if (present != nullptr) mask[m] = (*present)[m] ? 1 : 0;
     }
     std::vector<bb200_update_result> r(k);
     check(bb200_amcl_batch_update_measurements(handle_, controls.front().data(), in.data(), present != nullptr ? mask.data() : nullptr, r.data()));
+    return estimates_of(r);
+  }
+  /// update with members weighed by the caller's own sensor model (bb200_amcl_batch_update_begin / _end): an empty
+  /// measurements[m] marks a weighed member, the others pass points, a scan or a cloud.  weigh(members, views) is called
+  /// once with the weighed members that update in this step and the views of every slot (views[m].states, .factors, .n,
+  /// .stream), and writes each such member's factors on views[m].stream; it is not called when none of them updates.
+  /// weigh must not throw: the step would stay open and the batch then accepts nothing but its destruction.
+  template <class Weigh>
+  auto update(const std::vector<SE2d>& controls, const std::vector<std::optional<Measurement>>& measurements, Weigh&& weigh,
+              const std::vector<bool>* present = nullptr) -> std::vector<std::optional<estimation_type>> {
+    const std::size_t k = size();
+    if (controls.size() != k || measurements.size() != k || (present != nullptr && present->size() != k))
+      throw Error(BB200_ERR_INVALID_ARGUMENT, "one control, one measurement (and one presence flag) per member");
+    std::vector<bb200_laser_scan> scans(k);
+    std::vector<bb200_point_cloud> clouds(k);
+    std::vector<bb200_measurement> in(k);
+    std::vector<std::uint8_t> mask(present != nullptr ? k : 0);
+    for (std::size_t m = 0; m < k; ++m) {
+      in[m] = measurements[m] ? c_measurement(*measurements[m], &scans[m], &clouds[m]) : bb200_measurement{BB200_MEASUREMENT_WEIGHTS, nullptr, 0, nullptr, nullptr};
+      if (present != nullptr) mask[m] = (*present)[m] ? 1 : 0;
+    }
+    std::vector<bb200_weigh_view> views(k);
+    check(bb200_amcl_batch_update_begin(handle_, controls.front().data(), in.data(), present != nullptr ? mask.data() : nullptr, views.data()));
+    std::vector<std::size_t> weighed;
+    for (std::size_t m = 0; m < k; ++m)
+      if (!measurements[m] && views[m].updated) weighed.push_back(m);
+    if (!weighed.empty()) weigh(static_cast<const std::vector<std::size_t>&>(weighed), static_cast<const std::vector<bb200_weigh_view>&>(views));
+    std::vector<bb200_update_result> r(k);
+    check(bb200_amcl_batch_update_end(handle_, nullptr, r.data(), nullptr, nullptr, nullptr));
     return estimates_of(r);
   }
   /// update with a laser scan for every member (beluga_ros::Amcl::update(base_pose_in_odom, laser_scan) per member).

@@ -246,6 +246,22 @@ struct measurement_token {
   std::vector<std::pair<double, double>> points;
 };
 
+/// A caller's device sensor model (the SensorModel parameter of beluga::Amcl for a sensor this library has no model for)
+/// has state_type (SE2d), measurement_type and map_type, `int attach(bb200_filter*) const` (BB200_OK, or the status of the
+/// bb200_filter_set_*_map call that gives the filter a map for initialize_from_map and recovery injection) and
+/// `update_map(map)`, and its operator()(measurement) returns a token with
+///   void weigh(void* stream, const double* states, std::uint64_t n, double* factors) const;
+/// which writes factors[i] = L(state_i) for the n propagated device states {cos, sin, x, y}, enqueued on `stream` (a
+/// cudaStream_t) or synchronised with it.  Amcl::update then runs bb200_amcl_update_begin, weigh and bb200_amcl_update_end.
+template <class T, class = void>
+struct is_weighed_token : std::false_type {};
+template <class T>
+struct is_weighed_token<T, std::void_t<decltype(std::declval<const T&>().weigh(std::declval<void*>(), std::declval<const double*>(),
+                                                                                std::declval<std::uint64_t>(), std::declval<double*>()))>>
+    : std::true_type {};
+template <class T>
+constexpr bool is_weighed_token_v = is_weighed_token<T>::value;
+
 // ---- point clouds --------------------------------------------------------------------------------
 
 /// A sensor_msgs/PointCloud2 buffer as beluga_ros::SparsePointCloud3f reads it

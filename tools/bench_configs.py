@@ -14,6 +14,10 @@ K = 16 and 256 members, alone and next to a 32 768-particle member, and a step a
 `batch_state`: export_members and AmclBatch.from_states (the fleet checkpoint and its restore) with the same members.
 `raycast`: device ray casts (Ray2d::cast) for 256 batch members x 1 pose x 1080 bearings and for 1M rays of one filter, against
 the CPU oracle's Ray2d on the same rays.
+`weighed`: a 1M-particle step at 1080 beams on the 2000^2 map through the built-in likelihood-field update, against the same
+step weighed by the caller (bb200_amcl_update_begin, a one-kernel torch weigh on the step's stream, bb200_amcl_update_end);
+and a 256 x 2000 batch through update_measurements (100 points per member) against bb200_amcl_batch_update_begin / _end
+with every member weighed by one torch kernel.
 `sharded-publish`: a 1M-particle filter's publish round (particle-cloud histogram and 2000 pose samples) and 1M ray casts on 2
 and 4 shards of one device, next to the single filter (a filter of one shard does not step, so it has no posterior to publish).
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
@@ -454,6 +458,99 @@ def run_raycast():
                 "cpu_oracle_ms_one_thread": cpu_ms, "cpu_oracle_rays_per_s": rays / (cpu_ms * 1e-3),
                 "ms_per_step_e2e": ms, "kernels_ms": {}, "device": device}
         res[f"raycast_batch_256_x_1_x_1080_{int(max_range)}m_2000"]["ms_per_call_c"] = float(np.median(c_ms))
+    return res
+
+
+def run_weighed():
+    """The built-in likelihood-field update against a weighed step (update_begin, torch.exp(x) into the factors on the step's
+    stream, update_end), 1M particles x 1080 beams on the 2000^2 map, systematic resampling every step: the fused path with
+    one synchronisation on both sides.  Two filters stepped alternately in one process, host clock around each call (both
+    end synchronised), median and range of `steps` after `warmup`.  Then a pass with the device timers on for the kernel
+    times; apply_factors moves 24 bytes per particle (w and the factor read, w written)."""
+    import torch
+
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=1080, steps=100)
+    n = 1_000_000
+    params = bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=1)
+    builtin, weighed = (bb.Amcl(bb.DifferentialDriveModelParam(*MOTION), params) for _ in range(2))
+    for a in (builtin, weighed):
+        a.update_map(bb.SENSOR_LIKELIHOOD_FIELD, bb.LikelihoodFieldModelParam(**LFM), bb.OccupancyGrid(sc.cells, sc.resolution))
+        a.initialize(sc.initial_mean, sc.initial_cov)
+
+    def weigh(states, factors):
+        torch.exp(states[:, 2], out=factors)
+
+    warmup, steps = 3, 30
+    times = {"builtin": [], "weighed": []}
+    for k in range(warmup + steps):
+        pose = bb.se2(*sc.poses[k % 100])
+        for name, call in (("builtin", lambda: builtin.update(pose, sc.scans[k % 100])), ("weighed", lambda: weighed.update_weighted(pose, weigh))):
+            t0 = time.perf_counter()
+            r = call()
+            dt = (time.perf_counter() - t0) * 1e3
+            assert r.updated == 1 and r.resampled == 1
+            if k >= warmup:
+                times[name].append(dt)
+    kernels = {"builtin": {}, "weighed": {}}
+    timed = 5
+    for a in (builtin, weighed):
+        a.filter.set_timing(True)
+    for k in range(timed):
+        pose = bb.se2(*sc.poses[(warmup + steps + k) % 100])
+        for name, a, call in (("builtin", builtin, lambda: builtin.update(pose, sc.scans[(warmup + steps + k) % 100])),
+                              ("weighed", weighed, lambda: weighed.update_weighted(pose, weigh))):
+            a.filter.clear_timings()
+            call()
+            for kname, ms in a.filter.last_timings():
+                kernels[name][kname] = kernels[name].get(kname, 0.0) + ms / timed
+    apply_ms = kernels["weighed"].get("apply_factors", float("nan"))
+    device = device_record()
+    res = {}
+    for name in ("builtin", "weighed"):
+        t = times[name]
+        res[f"weighed_1M_x_1080_lfm_2000_{name}"] = {
+            "ms_per_step_e2e": float(np.median(t)), "ms_per_step_min_max": [float(min(t)), float(max(t))], "steps": steps, "warmup": warmup,
+            "kernels_ms": {k: round(v, 4) for k, v in kernels[name].items()}, "device": device}
+    res["weighed_1M_x_1080_lfm_2000_weighed"].update({"apply_factors_bytes": 24 * n, "apply_factors_gbs": 24 * n / (apply_ms * 1e-3) / 1e9})
+
+    # A 256 x 2000 batch: update_measurements with 100 points per member against begin / end with every member weighed
+    # by one torch kernel per member, alternated in one session.
+    k, m_n = 256, 2000
+    bparams = [bb.AmclParams(min_particles=m_n, max_particles=m_n, seed=m, resample_scheme=bb.RESAMPLE_SYSTEMATIC) for m in range(k)]
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    batches = {}
+    for name in ("builtin", "weighed"):
+        b = bb.AmclBatch([bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)], bparams)
+        b.set_likelihood_field_map(bb.LikelihoodFieldModelParam(**LFM), grid)
+        for m in range(k):
+            b.initialize(m, sc.initial_mean, sc.initial_cov)
+        batches[name] = b
+    pts = [sc.scans[i % 100][::10] for i in range(100)]
+
+    def weigh_batch(members, states, factors):
+        for s, f in zip(states, factors):
+            torch.exp(s[:, 2], out=f)
+
+    btimes = {"builtin": [], "weighed": []}
+    blaunch = {}
+    for step in range(warmup + steps):
+        poses = np.stack([bb.se2(*sc.poses[step % 100])] * k)
+        calls = (("builtin", lambda: batches["builtin"].update_measurements(poses, [pts[step % 100]] * k)),
+                 ("weighed", lambda: batches["weighed"].update_weighted(poses, [None] * k, weigh_batch)))
+        for name, call in calls:
+            before = batches[name].launch_count()
+            t0 = time.perf_counter()
+            r = call()
+            dt = (time.perf_counter() - t0) * 1e3
+            assert all(x.updated == 1 for x in r)
+            blaunch[name] = batches[name].launch_count() - before
+            if step >= warmup:
+                btimes[name].append(dt)
+    for name in ("builtin", "weighed"):
+        t = btimes[name]
+        res[f"weighed_batch_256_x_2000_{name}"] = {
+            "ms_per_step_e2e": float(np.median(t)), "ms_per_step_min_max": [float(min(t)), float(max(t))], "steps": steps, "warmup": warmup,
+            "library_launches_per_step": blaunch[name], "kernels_ms": {}, "device": device}
     return res
 
 
@@ -1037,6 +1134,8 @@ def main():
         out.update(run_batch_measurements())
     if "raycast" in which:
         out.update(run_raycast())
+    if "weighed" in which:
+        out.update(run_weighed())
     if "sharded-publish" in which:
         out.update(run_sharded_publish())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)

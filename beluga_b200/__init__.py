@@ -828,6 +828,7 @@ class ShardedAmcl:
             raise BelugaB200Error(st, self._lib.bb200_create_error().decode())
         self._h = h
         self.params = params
+        self.devices = list(devices)
         self.shards = [Filter(_handle=self._lib.bb200_amcl_filter(self._lib.bb200_sharded_amcl_shard(self._h, r)), _owner=self)
                        for r in range(len(devices))]
 
@@ -867,6 +868,49 @@ class ShardedAmcl:
         res = _capi.UpdateResult()
         self._check(self._lib.bb200_sharded_amcl_update(self._h, _dptr(_f64(control_pose)), _dptr(pts) if len(pts) else None, len(pts), C.byref(res)))
         return res
+
+    def update_weighted(self, control_pose, weigh) -> _capi.UpdateResult:
+        """Amcl.update_weighted over all shards (bb200_sharded_amcl_update_begin / _end): the same `weigh(states, factors)`.
+
+        It is called once per shard that holds particles, in rank order, with shard r's slice of the global particle order,
+        inside torch.cuda.device(devices[r]) and torch.cuda.stream(torch.cuda.ExternalStream(view.stream)), so a model
+        written for one filter works unchanged.  It is not called when the policies skip the step.  When `weigh` raises,
+        every shard's factors are set to 1, the step is closed and the exception propagates."""
+        k = len(self.devices)
+        views = (_capi.WeighView * k)()
+        self._check(self._lib.bb200_sharded_amcl_update_begin(self._h, _dptr(_f64(control_pose)), views))
+        res = _capi.UpdateResult()
+        if not views[0].updated:
+            self._check(self._lib.bb200_sharded_amcl_update_end(self._h, C.byref(res)))
+            return res
+        try:  # the tensors are made in here too: whatever raises, the step is closed
+            import torch
+
+            for device, stream, states, factors in self._weigh_views(views):
+                with torch.cuda.device(device), torch.cuda.stream(stream):
+                    weigh(states, factors)
+        except BaseException:
+            try:  # a step without a measurement; end runs even when the fill cannot
+                import torch
+
+                for device, stream, _, factors in self._weigh_views(views):
+                    with torch.cuda.device(device), torch.cuda.stream(stream):
+                        factors.fill_(1.0)
+            finally:
+                self._lib.bb200_sharded_amcl_update_end(self._h, C.byref(res))
+            raise
+        self._check(self._lib.bb200_sharded_amcl_update_end(self._h, C.byref(res)))
+        return res
+
+    def _weigh_views(self, views):
+        """(device, stream, states, factors) of every shard whose view holds particles, in rank order, as torch objects."""
+        import torch
+
+        for r, v in enumerate(views):
+            if v.n > 0:
+                device = torch.device("cuda", self.devices[r])
+                yield (device, torch.cuda.ExternalStream(v.stream, device=device), torch.as_tensor(_CudaArray(v.states, (v.n, 4)), device=device),
+                       torch.as_tensor(_CudaArray(v.factors, (v.n,)), device=device))
 
     def cluster_estimate(self, linear: float = 0.20, angular: float = 0.524, percentile: float = 0.90):
         """beluga::cluster_based_estimate over all shards -> (mean[4], cov[3, 3], n_cells, n_clusters)."""

@@ -216,6 +216,8 @@ SIGNATURES = {
     "bb200_sharded_amcl_initialize_from_map": (C.c_int, [_vp]),
     "bb200_sharded_amcl_force_update": (None, [_vp]),
     "bb200_sharded_amcl_update": (C.c_int, [_vp, _dbl, _dbl, C.c_uint64, _P(UpdateResult)]),
+    "bb200_sharded_amcl_update_begin": (C.c_int, [_vp, _dbl, _P(WeighView)]),
+    "bb200_sharded_amcl_update_end": (C.c_int, [_vp, _P(UpdateResult)]),
     "bb200_sharded_amcl_get_particles": (C.c_int, [_vp, _dbl, _dbl, C.c_uint64]),
     "bb200_sharded_amcl_cluster_estimate": (C.c_int, [_vp, _P(ClusterParam), _P(Estimate), _P(C.c_uint32), _P(C.c_uint32)]),
     "bb200_sharded_amcl_update_scan": (C.c_int, [_vp, _dbl, _P(LaserScan), _P(UpdateResult)]),

@@ -249,10 +249,15 @@ int Amcl::plan_update(const double control[4], bb200_step_plan* plan) {
   return BB200_OK;
 }
 
-int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], const double* points_xy, uint64_t n_points,
-                       bb200_update_result* out) {
-  *out = bb200_update_result{};
-  if (ranks == nullptr || count < 1 || count > kMaxShards) return BB200_ERR_INVALID_ARGUMENT;
+int Amcl::rollback_group(Amcl* const* ranks, int count, int status) {
+  for (int r = 0; r < count; ++r) {
+    ranks[r]->policy_ = ranks[r]->weighed_before_;
+    ranks[r]->filter_.step_abort();
+  }
+  return status;
+}
+
+int Amcl::plan_group(Amcl* const* ranks, int count, const double control[4], bb200_step_plan* plan) {
   Amcl& lead = *ranks[0];
   const bool kld = lead.params().min_particles < lead.params().max_particles;
   if (kld)
@@ -262,26 +267,42 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
   for (int r = 0; r < count; ++r)
     if (ranks[r]->sharded() && ranks[r]->filter_.link().world() <= 1)
       return ranks[r]->filter_.fail_with(BB200_ERR_STATE, "this shard has not joined its peers (bb200_amcl_join_shards / bb200_sharded_amcl_create)");
-  std::vector<AmclPolicy> before;
-  before.reserve(static_cast<size_t>(count));
-  for (int r = 0; r < count; ++r) before.push_back(ranks[r]->policy_);
-  auto rollback = [&](int st) {
-    for (int r = 0; r < count; ++r) {
-      ranks[r]->policy_ = before[static_cast<size_t>(r)];
-      ranks[r]->filter_.step_abort();
-    }
-    return st;
-  };
+  for (int r = 0; r < count; ++r) ranks[r]->weighed_before_ = ranks[r]->policy_;
   // The host half is the same arithmetic on every shard (policies, control window, recovery estimator).
-  bb200_step_plan plan{};
+  *plan = bb200_step_plan{};
   for (int r = 0; r < count; ++r) {
     bb200_step_plan p{};
     const int st = ranks[r]->plan_update(control, &p);
-    if (st != BB200_OK) return rollback(st);
-    if (r == 0) plan = p;
-    if (p.update != plan.update || p.step != plan.step) return rollback(lead.filter_.fail_with(BB200_ERR_STATE, "the shards of a filter disagree on the step plan"));
+    if (st != BB200_OK) return rollback_group(ranks, count, st);
+    if (r == 0) *plan = p;
+    if (p.update != plan->update || p.step != plan->step)
+      return rollback_group(ranks, count, lead.filter_.fail_with(BB200_ERR_STATE, "the shards of a filter disagree on the step plan"));
   }
-  if (!plan.update) return BB200_OK;
+  return BB200_OK;
+}
+
+int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], const double* points_xy, uint64_t n_points,
+                       bb200_update_result* out) {
+  *out = bb200_update_result{};
+  if (ranks == nullptr || count < 1 || count > kMaxShards) return BB200_ERR_INVALID_ARGUMENT;
+  bb200_step_plan plan{};
+  int st = plan_group(ranks, count, control, &plan);
+  if (st != BB200_OK || !plan.update) return st;
+  const bool resample_now = plan.resample != 0 && plan.needs_ess == 0;
+  for (int r = 0; r < count; ++r) {
+    st = ranks[r]->filter_.step_begin(plan.sampling, plan.step, points_xy, n_points, plan.opts, resample_now);
+    if (st != BB200_OK) return rollback_group(ranks, count, st);
+  }
+  for (int r = 0; r < count; ++r) {
+    st = ranks[r]->filter_.step_phase(Filter::kPhaseReweight);
+    if (st != BB200_OK) return rollback_group(ranks, count, st);
+  }
+  return finish_group(ranks, count, plan, out);
+}
+
+int Amcl::finish_group(Amcl* const* ranks, int count, const bb200_step_plan& plan, bb200_update_result* out) {
+  Amcl& lead = *ranks[0];
+  const bool kld = lead.params().min_particles < lead.params().max_particles;
   out->random_state_probability = plan.random_state_probability;
 
   auto run_phases = [&](std::initializer_list<int> phases) {
@@ -308,12 +329,6 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
     }
     return static_cast<int>(BB200_OK);
   };
-
-  const bool resample_now = plan.resample != 0 && plan.needs_ess == 0;
-  for (int r = 0; r < count; ++r) {
-    const int st = ranks[r]->filter_.step_begin(plan.sampling, plan.step, points_xy, n_points, plan.opts, resample_now);
-    if (st != BB200_OK) return rollback(st);
-  }
   // views::take_while_kld over the shards (take_while_kld.hpp:72-137): the candidate stream is ordered by output slot, and
   // every rank sees the spatial hash of every candidate, so all ranks count distinct buckets over the same stream and
   // stop at the same slot.  Windows of slots double like the single-GPU chunks; one host decision per window.
@@ -358,9 +373,10 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
     return static_cast<int>(BB200_OK);
   };
 
+  const bool resample_now = plan.resample != 0 && plan.needs_ess == 0;
   int st = BB200_OK;
   if (resample_now && kld) {
-    st = run_phases({Filter::kPhaseReweight, Filter::kPhaseCdf});
+    st = run_phases({Filter::kPhaseCdf});
     uint64_t accepted = 0;
     if (st == BB200_OK) st = kld_size(&accepted);
     if (st == BB200_OK) {
@@ -368,12 +384,12 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
       st = run_phases({Filter::kPhaseResample, Filter::kPhaseFinish});
     }
   } else {
-    st = resample_now ? run_phases({Filter::kPhaseReweight, Filter::kPhaseCdf, Filter::kPhaseResample, Filter::kPhaseFinish})
-                      : run_phases({Filter::kPhaseReweight, Filter::kPhaseCdf, Filter::kPhaseNormalize, Filter::kPhaseFinish});
+    st = resample_now ? run_phases({Filter::kPhaseCdf, Filter::kPhaseResample, Filter::kPhaseFinish})
+                      : run_phases({Filter::kPhaseCdf, Filter::kPhaseNormalize, Filter::kPhaseFinish});
   }
   double sum_sq = 0.0;
   if (st == BB200_OK) st = close_batch(&sum_sq);
-  if (st != BB200_OK) return rollback(st);
+  if (st != BB200_OK) return rollback_group(ranks, count, st);
   bool resampled = resample_now;
   if (!resample_now && plan.resample != 0) {
     // on_effective_size_drop (on_effective_size_drop.hpp:45-49): ESS = 1 / sum w~^2 < N / 2
@@ -382,12 +398,12 @@ int Amcl::update_group(Amcl* const* ranks, int count, const double control[4], c
       if (kld) {
         uint64_t accepted = 0;
         st = kld_size(&accepted);
-        if (st != BB200_OK) return rollback(st);
+        if (st != BB200_OK) return rollback_group(ranks, count, st);
         for (int r = 0; r < count; ++r) ranks[r]->filter_.step_set_kld_accepted(accepted);
       }
       st = run_phases({Filter::kPhaseResample, Filter::kPhaseFinish});
       if (st == BB200_OK) st = close_batch(nullptr);
-      if (st != BB200_OK) return rollback(st);
+      if (st != BB200_OK) return rollback_group(ranks, count, st);
       resampled = true;
     }
   }
@@ -476,13 +492,15 @@ int Amcl::update_begin(const double control[4], bb200_weigh_view* view) {
   error_.clear();
   if (filter_.weigh_open()) return filter_.fail_with(BB200_ERR_STATE, "a weighed step is already open (bb200_amcl_update_end closes it)");
   *view = bb200_weigh_view{};
-  if (sharded() || filter_.link().world() > 1) return filter_.fail_with(BB200_ERR_STATE, "a sharded filter takes no weighed steps");
+  if (sharded() || filter_.link().world() > 1)
+    return filter_.fail_with(BB200_ERR_STATE, "a shard takes weighed steps only with its filter (bb200_sharded_amcl_update_begin)");
   weighed_before_ = policy_;
   bb200_step_plan& plan = weighed_plan_;
   int st = plan_update(control, &plan);
   if (st == BB200_OK && plan.update) {
     const bool injects = plan.resample != 0 && plan.random_state_probability > 0.0;
-    st = filter_.weigh_begin(plan.sampling, plan.step, plan.opts, fused(plan), injects);
+    st = filter_.weigh_prepare(plan.opts, injects);
+    if (st == BB200_OK) st = filter_.weigh_propagate(plan.sampling, plan.step, plan.opts, fused(plan));
   }
   if (st != BB200_OK) {
     policy_ = weighed_before_;  // as update(): policies, control window and recovery estimator as if the call had not happened
@@ -502,6 +520,9 @@ int Amcl::update_begin(const double control[4], bb200_weigh_view* view) {
 
 int Amcl::update_end(bb200_update_result* out) {
   *out = bb200_update_result{};
+  // A shard's weigh_open flag belongs to its filter's step: this call leaves it open.
+  if (sharded() || filter_.link().world() > 1)
+    return filter_.fail_with(BB200_ERR_STATE, "a shard's weighed step is closed with its filter (bb200_sharded_amcl_update_end)");
   if (!filter_.weigh_open()) return filter_.fail_with(BB200_ERR_STATE, "no weighed step is open (bb200_amcl_update_begin)");
   filter_.set_weigh_open(false);
   if (!weighed_plan_.update) return BB200_OK;
@@ -512,6 +533,68 @@ int Amcl::update_end(bb200_update_result* out) {
     policy_ = weighed_before_;
     filter_.step_abort();
   }
+  return st;
+}
+
+int Amcl::update_group_begin(Amcl* const* ranks, int count, const double control[4], bb200_weigh_view* views) {
+  if (ranks == nullptr || count < 1 || count > kMaxShards) return BB200_ERR_INVALID_ARGUMENT;
+  for (int r = 0; r < count; ++r)
+    if (ranks[r]->filter_.weigh_open())
+      return ranks[r]->filter_.fail_with(BB200_ERR_STATE, "a weighed step is already open (bb200_sharded_amcl_update_end closes it)");
+  for (int r = 0; r < count; ++r) views[r] = bb200_weigh_view{};
+  bb200_step_plan plan{};
+  int st = plan_group(ranks, count, control, &plan);
+  if (st != BB200_OK) return st;
+  if (plan.update) {
+    const bool resample_now = plan.resample != 0 && plan.needs_ess == 0;
+    const bool injects = plan.resample != 0 && plan.random_state_probability > 0.0;
+    // Every shard's checks and allocations before any shard's propagate: a refusal leaves every shard's particles as they were.
+    for (int r = 0; r < count; ++r) {
+      st = ranks[r]->filter_.weigh_prepare(plan.opts, injects);
+      if (st != BB200_OK) return rollback_group(ranks, count, st);
+    }
+    for (int r = 0; r < count; ++r) {
+      st = ranks[r]->filter_.weigh_propagate(plan.sampling, plan.step, plan.opts, resample_now);
+      if (st != BB200_OK) return rollback_group(ranks, count, st);
+    }
+  }
+  for (int r = 0; r < count; ++r) {
+    Filter& f = ranks[r]->filter_;
+    ranks[r]->weighed_plan_ = plan;
+    f.set_weigh_open(true);
+    views[r].updated = plan.update;
+    if (plan.update) {
+      views[r].n = f.size();
+      views[r].states = f.weigh_states();
+      views[r].factors = f.weigh_factors();
+      views[r].stream = f.stream();
+    }
+  }
+  return BB200_OK;
+}
+
+int Amcl::update_group_end(Amcl* const* ranks, int count, bb200_update_result* out) {
+  *out = bb200_update_result{};
+  if (ranks == nullptr || count < 1 || count > kMaxShards) return BB200_ERR_INVALID_ARGUMENT;
+  for (int r = 0; r < count; ++r)
+    if (!ranks[r]->filter_.weigh_open())
+      return ranks[r]->filter_.fail_with(BB200_ERR_STATE, "no weighed step is open (bb200_sharded_amcl_update_begin)");
+  for (int r = 0; r < count; ++r) ranks[r]->filter_.set_weigh_open(false);
+  const bb200_step_plan plan = ranks[0]->weighed_plan_;
+  if (!plan.update) return BB200_OK;
+  for (int r = 0; r < count; ++r) {
+    const int st = ranks[r]->filter_.step_phase(Filter::kPhaseApplyFactors);
+    if (st != BB200_OK) return rollback_group(ranks, count, st);
+  }
+  // Every shard's exchanges wait for the device, with a timeout: none may start while a peer's sensor model still runs.
+  for (int r = 0; r < count; ++r)
+    for (int q = 0; q < count; ++q)
+      if (q != r) {
+        const int st = ranks[r]->filter_.wait_for_factors(ranks[q]->filter_);
+        if (st != BB200_OK) return rollback_group(ranks, count, st);
+      }
+  const int st = finish_group(ranks, count, plan, out);
+  if (st != BB200_OK) *out = bb200_update_result{};
   return st;
 }
 

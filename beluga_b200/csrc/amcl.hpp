@@ -92,8 +92,24 @@ class Amcl {
   int update_begin(const double control[4], bb200_weigh_view* view);
   /// The second half: w *= factors and everything update() runs after its sensor model.  Atomic as update().
   int update_end(bb200_update_result* out);
+  /// update_begin over the `count` shards of ONE filter held by this thread: views[r] is shard r's slice of the global
+  /// particle order (n may be 0 on a KLD-sized shard).  Every shard's step stays open until update_group_end.  Atomic as
+  /// update_group.
+  static int update_group_begin(Amcl* const* ranks, int count, const double control[4], bb200_weigh_view* views);
+  /// The second half: w *= factors on every shard, then everything update_group runs after its sensor model.  No shard's
+  /// exchange starts before every shard's factors are applied (stream waits, no host synchronisation).  Atomic as
+  /// update_group.
+  static int update_group_end(Amcl* const* ranks, int count, bb200_update_result* out);
 
  private:
+  /// The checks and the host half of update_group, the same arithmetic on every shard: the plan, and every rank's policy
+  /// before it in weighed_before_.  On failure every policy is put back.
+  static int plan_group(Amcl* const* ranks, int count, const double control[4], bb200_step_plan* plan);
+  /// Everything update_group runs once the sensor phase is enqueued on every shard: the phases, the KLD window loop, the
+  /// selective resampling decision and the commit.  On failure every rank's policy is put back and the step is closed.
+  static int finish_group(Amcl* const* ranks, int count, const bb200_step_plan& plan, bb200_update_result* out);
+  /// Puts back every rank's policy from weighed_before_ and closes the step on every shard; returns `status`.
+  static int rollback_group(Amcl* const* ranks, int count, int status);
   int update_device(const double control[4], const double* points_xy, uint64_t n_points, bb200_update_result* out);
   /// A step that resamples in the fused sequence with one host synchronisation (every_n fired, no ESS test, no KLD).
   bool fused(const bb200_step_plan& plan) const;
@@ -105,7 +121,7 @@ class Amcl {
   Filter filter_;
   mutable std::string error_;
   bool initialized_{false};
-  // the open weighed step: its plan, and the policy to put back when it fails
+  // the open weighed step's plan, and the policy to put back when a step fails (a weighed step, or a step of shards)
   bb200_step_plan weighed_plan_{};
   AmclPolicy weighed_before_{policy_};
 };

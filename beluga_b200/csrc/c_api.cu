@@ -42,6 +42,13 @@ struct bb200_sharded_amcl {
   std::vector<bb200_amcl*> ranks;
   mutable std::string error;
   void record_error(const std::string& m) const { error = m; }
+  /// Whether a weighed step is open: bb200_sharded_amcl_update_begin opens it on every shard at once.
+  bool step_open() const { return !ranks.empty() && ranks[0]->impl.filter().weigh_open(); }
+  std::vector<Amcl*> impls() const {
+    std::vector<Amcl*> out;
+    for (bb200_amcl* a : ranks) out.push_back(&a->impl);
+    return out;
+  }
   ~bb200_sharded_amcl() {
     for (bb200_amcl* a : ranks) delete a;
   }
@@ -186,13 +193,20 @@ const char* bb200_last_error(const bb200_filter* f) { return f != nullptr ? f->i
     if (!(cond)) return BB200_ERR_INVALID_ARGUMENT;   \
   } while (0)
 // While a weighed step is open (bb200_amcl_update_begin .. _end) a filter refuses every call but the step's end and destroy;
-// a batch likewise between bb200_amcl_batch_update_begin and _end.
+// a sharded filter and a batch likewise between their update_begin and _end.
 #define BB_REFUSE_OPEN(filter)                                                                              \
   do {                                                                                                      \
     if ((filter).weigh_open()) {                                                                            \
       (filter).record_error("a weighed step is open: only bb200_amcl_update_end and destroy are accepted"); \
       return BB200_ERR_STATE;                                                                               \
     }                                                                                                       \
+  } while (0)
+#define BB_REFUSE_OPEN_SHARDED(g)                                                                                \
+  do {                                                                                                           \
+    if ((g) != nullptr && (g)->step_open()) {                                                                    \
+      (g)->record_error("a weighed step is open: only bb200_sharded_amcl_update_end and destroy are accepted"); \
+      return BB200_ERR_STATE;                                                                                    \
+    }                                                                                                            \
   } while (0)
 #define BB_REFUSE_OPEN_BATCH(batch)                                                                              \
   do {                                                                                                           \
@@ -787,30 +801,52 @@ bb200_amcl* bb200_sharded_amcl_shard(bb200_sharded_amcl* g, int rank) {
 
 int bb200_sharded_amcl_set_likelihood_field_map(bb200_sharded_amcl* g, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid, int prob) {
   BB_REQUIRE(g && p && grid);
+  BB_REFUSE_OPEN_SHARDED(g);
   return set_sharded_map(g, [&](bb200::MapTables* t, std::string* e) { return bb200::prepare_likelihood_field_map(*p, *grid, prob != 0, t, e); });
 }
 int bb200_sharded_amcl_set_beam_map(bb200_sharded_amcl* g, const bb200_beam_param* p, const bb200_occupancy_grid* grid) {
   BB_REQUIRE(g && p && grid);
+  BB_REFUSE_OPEN_SHARDED(g);
   return set_sharded_map(g, [&](bb200::MapTables* t, std::string* e) { return bb200::prepare_beam_map(*p, *grid, t, e); });
 }
 int bb200_sharded_amcl_initialize(bb200_sharded_amcl* g, const double mean_xytheta[3], const double cov[9]) {
   BB_REQUIRE(mean_xytheta && cov);
+  BB_REFUSE_OPEN_SHARDED(g);
   BB_EACH_SHARD(a->impl.initialize(mean_xytheta, cov));
 }
-int bb200_sharded_amcl_initialize_from_map(bb200_sharded_amcl* g) { BB_EACH_SHARD(a->impl.initialize_from_map()); }
+int bb200_sharded_amcl_initialize_from_map(bb200_sharded_amcl* g) {
+  BB_REFUSE_OPEN_SHARDED(g);
+  BB_EACH_SHARD(a->impl.initialize_from_map());
+}
 #undef BB_EACH_SHARD
 void bb200_sharded_amcl_force_update(bb200_sharded_amcl* g) {
-  if (g != nullptr)
+  if (g != nullptr && !g->step_open())
     for (bb200_amcl* a : g->ranks) a->impl.force_update();
 }
 int bb200_sharded_amcl_update(bb200_sharded_amcl* g, const double control_pose[4], const double* points_xy, uint64_t n_points, bb200_update_result* out) {
   BB_REQUIRE(g && control_pose && out && (points_xy || n_points == 0));
+  BB_REFUSE_OPEN_SHARDED(g);
   static const double kNoPoints[2] = {0.0, 0.0};
   g->error.clear();
   return guarded(*g, [&] {
-    std::vector<Amcl*> ranks;
-    for (bb200_amcl* a : g->ranks) ranks.push_back(&a->impl);
+    const std::vector<Amcl*> ranks = g->impls();
     return Amcl::update_group(ranks.data(), static_cast<int>(ranks.size()), control_pose, points_xy != nullptr ? points_xy : kNoPoints, n_points, out);
+  });
+}
+int bb200_sharded_amcl_update_begin(bb200_sharded_amcl* g, const double control_pose[4], bb200_weigh_view* views) {
+  BB_REQUIRE(g && control_pose && views);
+  g->error.clear();
+  return guarded(*g, [&] {
+    const std::vector<Amcl*> ranks = g->impls();
+    return Amcl::update_group_begin(ranks.data(), static_cast<int>(ranks.size()), control_pose, views);
+  });
+}
+int bb200_sharded_amcl_update_end(bb200_sharded_amcl* g, bb200_update_result* out) {
+  BB_REQUIRE(g && out);
+  g->error.clear();
+  return guarded(*g, [&] {
+    const std::vector<Amcl*> ranks = g->impls();
+    return Amcl::update_group_end(ranks.data(), static_cast<int>(ranks.size()), out);
   });
 }
 int bb200_cluster_merge_host(const bb200_cluster_cell* const* shard_cells, const uint64_t* shard_counts, const uint64_t* shard_first_index, int shards,
@@ -891,6 +927,7 @@ int merged_cells(bb200_sharded_amcl* g, double linear_resolution, double angular
 int bb200_sharded_amcl_cluster_estimate(bb200_sharded_amcl* g, const bb200_cluster_param* p, bb200_estimate* out, uint32_t* n_cells,
                                         uint32_t* n_clusters) {
   BB_REQUIRE(g && p && out);
+  BB_REFUSE_OPEN_SHARDED(g);
   g->error.clear();
   return guarded(*g, [&] {
     std::vector<bb200_cluster_cell> merged;
@@ -909,6 +946,7 @@ int bb200_sharded_amcl_cluster_estimate(bb200_sharded_amcl* g, const bb200_clust
 
 int bb200_sharded_amcl_get_particles(bb200_sharded_amcl* g, double* states, double* weights, uint64_t capacity) {
   BB_REQUIRE(g);
+  BB_REFUSE_OPEN_SHARDED(g);
   g->error.clear();
   return guarded(*g, [&] {
     uint64_t done = 0;
@@ -926,6 +964,7 @@ int bb200_sharded_amcl_get_particles(bb200_sharded_amcl* g, double* states, doub
 
 int bb200_sharded_amcl_update_scan(bb200_sharded_amcl* g, const double control_pose[4], const bb200_laser_scan* scan, bb200_update_result* out) {
   BB_REQUIRE(g && control_pose && scan && out);
+  BB_REFUSE_OPEN_SHARDED(g);
   g->error.clear();
   return guarded(*g, [&] {
     std::vector<double> points;
@@ -939,6 +978,7 @@ int bb200_sharded_amcl_update_scan(bb200_sharded_amcl* g, const double control_p
 int bb200_sharded_amcl_update_point_cloud(bb200_sharded_amcl* g, const double control_pose[4], const bb200_point_cloud* cloud,
                                           bb200_update_result* out) {
   BB_REQUIRE(g && control_pose && cloud && out);
+  BB_REFUSE_OPEN_SHARDED(g);
   g->error.clear();
   return guarded(*g, [&] {
     std::vector<double> points;
@@ -955,6 +995,7 @@ int bb200_sharded_amcl_update_point_cloud(bb200_sharded_amcl* g, const double co
 int bb200_sharded_amcl_particle_histogram(bb200_sharded_amcl* g, double linear_resolution, double angular_resolution, bb200_cluster_cell* bins,
                                           uint64_t capacity, uint64_t* n_bins, double* max_bin_weight) {
   BB_REQUIRE(g);
+  BB_REFUSE_OPEN_SHARDED(g);
   g->error.clear();
   return guarded(*g, [&] {
     std::vector<bb200_cluster_cell> merged;
@@ -978,6 +1019,7 @@ int bb200_sharded_amcl_particle_histogram(bb200_sharded_amcl* g, double linear_r
 
 int bb200_sharded_amcl_sample_states(bb200_sharded_amcl* g, uint64_t count, uint32_t step, double* states_out) {
   BB_REQUIRE(g);
+  BB_REFUSE_OPEN_SHARDED(g);
   g->error.clear();
   return guarded(*g, [&] {
     const size_t shards = g->ranks.size();
@@ -1049,6 +1091,7 @@ int bb200_sharded_amcl_sample_states(bb200_sharded_amcl* g, uint64_t count, uint
 int bb200_sharded_amcl_cast_rays(bb200_sharded_amcl* g, const double* poses, uint64_t n_poses, const double* bearings_cs, uint64_t n_bearings,
                                  double max_range, double* ranges) {
   BB_REQUIRE(g);
+  BB_REFUSE_OPEN_SHARDED(g);
   g->error.clear();
   return guarded(*g, [&] {
     uint64_t n_rays = 0;

@@ -150,6 +150,7 @@ Filter::~Filter() {
   // Before the members free this filter's buffers (after this body): nothing in flight may read them.
   if (stream_ != nullptr) cudaStreamSynchronize(stream_);
   for (auto& e : event_pool_) cudaEventDestroy(e);
+  if (factors_applied_ != nullptr) cudaEventDestroy(factors_applied_);
   if (stream_ != nullptr && owns_stream_) cudaStreamDestroy(stream_);
 }
 
@@ -318,8 +319,7 @@ int Filter::step_begin(const bb200_motion_sampling& sampling, uint32_t step, con
   if (n_points > 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, "too many points");
   if (o.random_state_probability > 0.0 && map_.n_free == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
   if (world > 1) {
-    if ((!link_.kld() && n_ != capacity_) || n_ > capacity_ || o.max_particles != world * capacity_)
-      return fail(BB200_ERR_STATE, "a sharded filter keeps `capacity` particles on every rank (fewer only under KLD)");
+    if (const int st = check_shard_size(o)) return st;
   } else if (o.max_particles == 0 || o.max_particles > capacity_) {
     return fail(BB200_ERR_CAPACITY, "max_particles exceeds the filter capacity");
   }
@@ -337,6 +337,13 @@ int Filter::step_begin(const bb200_motion_sampling& sampling, uint32_t step, con
   return BB200_OK;
 }
 
+int Filter::check_shard_size(const bb200_resample_opts& o) {
+  const uint64_t world = static_cast<uint64_t>(link_.world());
+  if ((!link_.kld() && n_ != capacity_) || n_ > capacity_ || o.max_particles != world * capacity_)
+    return fail(BB200_ERR_STATE, "a sharded filter keeps `capacity` particles on every rank (fewer only under KLD)");
+  return BB200_OK;
+}
+
 void Filter::step_abort() { step_.active = false; }
 
 int Filter::step_phase(int phase) {
@@ -347,9 +354,12 @@ int Filter::step_phase(int phase) {
   const bb200_resample_opts& o = step_.opts;
   int st = BB200_OK;
   switch (phase) {
-    case kPhaseReweight: {
-      mark("begin_step");
-      {
+    case kPhaseReweight:
+    case kPhaseApplyFactors: {
+      if (phase == kPhaseApplyFactors) {
+        st = weigh_apply();
+      } else {
+        mark("begin_step");
         const bool scheduled = n_ >= kScheduleMinParticles;
         const bool warm = map_.sensor != BB200_SENSOR_BEAM && map_.field.use_fixed && map_.bordered_bytes <= (96ull << 20);
         launch_begin_fused_step(scalars_.get(), tile_state_.get(), scan_tile_count(n_), sched_.get(), scheduled ? counters_.get() : nullptr,
@@ -365,6 +375,7 @@ int Filter::step_phase(int phase) {
           mark("exchange");
           st = enqueue_exchange(kExchangeWmax, true, false);
         }
+        if (st == BB200_OK && phase == kPhaseApplyFactors) BB_CHECK(cudaEventRecord(factors_applied_, stream_));
       }
       return st;
     }
@@ -1197,23 +1208,34 @@ int Filter::finish_resample(bb200_estimate* est, double* weight_sum, uint64_t* n
   return step_end(est, weight_sum, new_size, nullptr);
 }
 
-int Filter::weigh_begin(const bb200_motion_sampling& sampling, uint32_t step, const bb200_resample_opts& o, bool fused, bool injects) {
-  if (link_.world() > 1 || config_.global_count != capacity_) return fail(BB200_ERR_STATE, "a weighed step runs on one filter, not on shards");
-  if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
-  if (o.max_particles == 0 || o.max_particles > capacity_) return fail(BB200_ERR_CAPACITY, "max_particles exceeds the filter capacity");
+int Filter::weigh_prepare(const bb200_resample_opts& o, bool injects) {
+  const bool sharded = link_.world() > 1;
+  if (!sharded && config_.global_count != capacity_) return fail(BB200_ERR_STATE, "a weighed step runs on one filter or on joined shards");
+  if (n_ == 0 && !(sharded && link_.kld())) return fail(BB200_ERR_STATE, "no particles");  // a KLD-sized filter may leave a shard empty
+  if (sharded) {
+    if (const int st = check_shard_size(o)) return st;
+  } else if (o.max_particles == 0 || o.max_particles > capacity_) {
+    return fail(BB200_ERR_CAPACITY, "max_particles exceeds the filter capacity");
+  }
   if (injects && map_.n_free == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
   BB_CHECK(cudaSetDevice(config_.device));
   if (factors_.get() == nullptr) BB_CHECK(factors_.allocate(capacity_));
+  if (sharded && factors_applied_ == nullptr) BB_CHECK(cudaEventCreateWithFlags(&factors_applied_, cudaEventDisableTiming));
+  return BB200_OK;
+}
+
+int Filter::weigh_propagate(const bb200_motion_sampling& sampling, uint32_t step, const bb200_resample_opts& o, bool resample_planned) {
+  BB_CHECK(cudaSetDevice(config_.device));
   const MotionSampling s = to_kernel_sampling(sampling);
   mark("begin_step");
-  if (fused) {
+  if (resample_planned || link_.world() > 1) {
     step_ = StepContext{};
     summary_host_.get()->error = 0;
     step_.active = true;
     step_.sampling = s;
     step_.step = step;
     step_.opts = o;
-    step_.resample_planned = true;
+    step_.resample_planned = resample_planned;
     // the scalars and the CDF's scan state, as kPhaseReweight resets them; no schedule and no table to prefetch
     launch_begin_fused_step(scalars_.get(), tile_state_.get(), scan_tile_count(n_), sched_.get(), nullptr, 0, sched_tiles_.get(), 0, nullptr, 0, stream_);
   } else {
@@ -1229,12 +1251,19 @@ int Filter::weigh_begin(const bb200_motion_sampling& sampling, uint32_t step, co
 }
 
 // On a step that does not take the fused path, normalize's build_cdf recomputes the largest weight this kernel posts (as
-// after the built-in reweight on that path); the fused path's quantize_scan reads it.
+// after the built-in reweight on that path); the fused path's quantize_scan reads it, joined shards exchange it.
 int Filter::weigh_apply() {
   BB_CHECK(cudaSetDevice(config_.device));
   mark("apply_factors");
   launch_apply_factors(weights_.get(), factors_.get(), n_, scalars_.get(), stream_);
   BB_LAUNCHED("apply_factors");
+  return BB200_OK;
+}
+
+int Filter::wait_for_factors(const Filter& peer) {
+  if (peer.factors_applied_ == nullptr) return fail(BB200_ERR_STATE, "the peer shard has no weighed step");
+  BB_CHECK(cudaSetDevice(config_.device));
+  BB_CHECK(cudaStreamWaitEvent(stream_, peer.factors_applied_, 0));
   return BB200_OK;
 }
 

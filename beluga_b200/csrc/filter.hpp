@@ -104,14 +104,22 @@ class Filter {
   /// step_begin, kPhaseReweight and then this: CDF, resample, moments, and the synchronisation (step_end).
   int finish_resample(bb200_estimate* est, double* weight_sum, uint64_t* new_size);
 
-  // ---- a step whose sensor model the caller runs (bb200_amcl_update_begin / _end) ----
-  /// Checks the step, allocates the factor buffer on first use and enqueues the reset and the propagate (the non-binned
-  /// propagate_kernel: no pose-bin schedule); no host synchronisation.  `fused`: the step then ends as the fused step
-  /// does (weigh_apply, then finish_resample); otherwise weigh_apply is followed by the blocking normalize / resample /
-  /// estimate.  `injects`: the plan may inject random states, which needs a map with free cells.
-  int weigh_begin(const bb200_motion_sampling& sampling, uint32_t step, const bb200_resample_opts& o, bool fused, bool injects);
+  // ---- a step whose sensor model the caller runs (bb200_amcl_update_begin / _end, bb200_sharded_amcl_update_begin / _end) ----
+  /// The host half of a weighed step's begin: checks the step and allocates the factor buffer (and, on joined shards, the
+  /// event of kPhaseApplyFactors) on first use.  Nothing reaches the device, so a driver of several shards runs it on
+  /// every shard before weigh_propagate on any, and a refusal leaves every shard's particles as they were.  `injects`: the
+  /// plan may inject random states, which needs a map with free cells.
+  int weigh_prepare(const bb200_resample_opts& o, bool injects);
+  /// The device half, after weigh_prepare: enqueues the reset and the propagate (the non-binned propagate_kernel: no
+  /// pose-bin schedule); no host synchronisation.  `resample_planned`: kPhaseResample follows kPhaseCdf directly.  One
+  /// filter: the step then ends as the fused step does (weigh_apply, then finish_resample); otherwise weigh_apply is
+  /// followed by the blocking normalize / resample / estimate.  Joined shards: the step continues with kPhaseApplyFactors
+  /// and the phases after it, as step_begin's does after kPhaseReweight.
+  int weigh_propagate(const bb200_motion_sampling& sampling, uint32_t step, const bb200_resample_opts& o, bool resample_planned);
   /// Enqueues w *= factors over the particle set and the largest weight into the device scalars.
   int weigh_apply();
+  /// Orders this filter's stream behind the end of `peer`'s kPhaseApplyFactors (a stream wait, no host synchronisation).
+  int wait_for_factors(const Filter& peer);
   /// Whether a weighed step is open on this filter: the C ABI then refuses every call but the step's end and destroy.
   void set_weigh_open(bool open) { weigh_open_ = open; }
   bool weigh_open() const { return weigh_open_; }
@@ -144,7 +152,8 @@ class Filter {
     kPhaseCdf = 2,        // common exponent | fixed-point CDF                                 (posts the shard's total)
     kPhaseResample = 3,   // resample (+ redistribution over peer memory) | moments of the new set (posts them)
     kPhaseFinish = 4,     // global moments, read-back
-    kPhaseNormalize = 5   // joined shards, instead of kPhaseResample on a step that keeps its particles: w /= S | moments
+    kPhaseNormalize = 5,  // joined shards, instead of kPhaseResample on a step that keeps its particles: w /= S | moments
+    kPhaseApplyFactors = 6  // a weighed step (weigh_propagate), instead of kPhaseReweight: w *= factors   (posts the shard's largest weight)
   };
   int step_phase(int phase);
   void step_abort();
@@ -187,6 +196,8 @@ class Filter {
     return status;
   }
   int check(cudaError_t e, const char* what) { return cuda_check(e, what, &error_); }
+  /// A joined shard's particle count against the plan's: `capacity` particles (fewer only under KLD), world * capacity in all.
+  int check_shard_size(const bb200_resample_opts& o);
   int upload_points(const double* points_xy, uint64_t n_points);
   /// propagate | schedule | reweight on a staged step (points uploaded, scalars reset), no validation.
   int enqueue_propagate_reweight_kernels(const MotionSampling* sampling, uint32_t step, bool do_reweight, uint64_t n_points, bool counters_reset);
@@ -285,6 +296,7 @@ class Filter {
   DeviceBuffer<uint32_t> beam_hits_;  // two-pass beam model: hit word per (beam, particle) of one pass
   DeviceBuffer<double> factors_;      // weighed steps: the caller's likelihood per particle (capacity_, allocated on the first)
   bool weigh_open_{false};
+  cudaEvent_t factors_applied_{nullptr};  // weighed steps of shards: the end of kPhaseApplyFactors (created by the first)
 
   double pivot_[2]{0.0, 0.0};
   bb200_estimate cloud_{};     // last estimate, when it describes the raw (unit-weight) cloud

@@ -492,8 +492,9 @@ int bb200_amcl_update_point_cloud(bb200_amcl* a, const double control_pose[4], c
  * bb200_amcl_destroy is allowed.  bb200_amcl_update_end must follow every successful begin, skipped steps included, and
  * returns BB200_ERR_STATE without one.  Both calls are atomic as bb200_amcl_update: on failure the policies, the control
  * window and the recovery estimator are as before the begin, and the step is closed.  No map is needed, except for a step
- * that may inject random states (BB200_ERR_STATE before any device work).  Sharded filters and shards refuse begin with
- * BB200_ERR_STATE.  The factor buffer belongs to the filter and is allocated by the first begin. */
+ * that may inject random states (BB200_ERR_STATE before any device work).  Shards refuse begin and end with
+ * BB200_ERR_STATE: a sharded filter takes weighed steps through bb200_sharded_amcl_update_begin / _end.  The factor buffer
+ * belongs to the filter and is allocated by the first begin. */
 typedef struct bb200_weigh_view {
   int updated;           /* 0: the policies skip this step; end returns updated = 0 */
   uint64_t n;            /* particles to weigh */
@@ -541,6 +542,21 @@ void bb200_sharded_amcl_force_update(bb200_sharded_amcl* g);
 /* Amcl::update (amcl_core.hpp:165-201) over all shards. */
 int bb200_sharded_amcl_update(bb200_sharded_amcl* g, const double control_pose[4], const double* points_xy, uint64_t n_points,
                               bb200_update_result* out);
+/* bb200_amcl_update_begin / _end over all shards: a step weighed by the caller's own sensor model.  views has
+ * bb200_sharded_amcl_shards(g) entries; view r is shard r's contiguous slice of the global particle order, on devices[r] as
+ * passed to bb200_sharded_amcl_create, with that shard's stream (a KLD-sized shard may hold n = 0: nothing to weigh).  The
+ * caller writes every shard's factors on its stream or synchronised with it; end then runs w_i *= factors_i on every
+ * shard and everything bb200_sharded_amcl_update runs after its sensor model.  No shard's exchanges start before every
+ * shard's factors are applied: end makes each shard's stream wait for the others' (no host synchronisation), so a sensor
+ * model may take as long as it needs.  With factors bit-equal to a stock model's likelihoods the step is byte-identical to
+ * bb200_sharded_amcl_update with that model.  The rules are those of bb200_amcl_update_begin / _end: while a step is open
+ * every other bb200_sharded_amcl_* call, and every call on the shards' bb200_amcl handles and their bb200_amcl_filter
+ * views (bb200_amcl_update_end included), returns BB200_ERR_STATE; bb200_sharded_amcl_force_update is ignored and
+ * bb200_sharded_amcl_destroy is allowed.  A step the policies skip launches nothing, and end still closes it.  Both calls
+ * are atomic: on failure every shard's policies are as before the begin and the step is closed.  Factors that are 0,
+ * negative, NaN or +-inf follow the built-in rules, weights_degenerate included. */
+int bb200_sharded_amcl_update_begin(bb200_sharded_amcl* g, const double control_pose[4], bb200_weigh_view* views);
+int bb200_sharded_amcl_update_end(bb200_sharded_amcl* g, bb200_update_result* out);
 /* beluga::cluster_based_estimate over all shards: every shard builds its cell records on its device
  * (bb200_filter_particle_histogram with the clusterizer's resolutions), the records are merged on the host in rank
  * order (bb200_cluster_merge_host) and flooded like the single-GPU estimate.  Counts, weights and moments of a cell

@@ -358,10 +358,23 @@ class ShardedAmcl {
   }
   void force_update() { bb200_sharded_amcl_force_update(handle_); }
 
+  /// Amcl::update over all shards.  With a caller's device sensor model (is_weighed_token_v of its token; the model's
+  /// attach takes the bb200_sharded_amcl*): begin, the token's weigh once per shard that holds particles, in rank order,
+  /// and end (bb200_sharded_amcl_update_begin / _end).  The views of shard r live on devices[r], the device of its stream:
+  /// a token that launches kernels must make that device current (cudaSetDevice) first.  weigh must not throw: the step
+  /// would stay open and the filter then accepts nothing but its destruction.
   auto update(const state_type& control_action, measurement_type measurement) -> std::optional<estimation_type> {
-    const measurement_token token = sensor_model_(std::move(measurement));
+    const auto token = sensor_model_(std::move(measurement));
     bb200_update_result r{};
-    check(bb200_sharded_amcl_update(handle_, control_action.data(), token.points.empty() ? nullptr : &token.points.front().first, token.points.size(), &r));
+    if constexpr (is_weighed_token_v<std::decay_t<decltype(token)>>) {
+      std::vector<bb200_weigh_view> views(static_cast<std::size_t>(bb200_sharded_amcl_shards(handle_)));
+      check(bb200_sharded_amcl_update_begin(handle_, control_action.data(), views.data()));
+      for (const bb200_weigh_view& view : views)
+        if (view.updated && view.n > 0) token.weigh(view.stream, view.states, view.n, view.factors);
+      check(bb200_sharded_amcl_update_end(handle_, &r));
+    } else {
+      check(bb200_sharded_amcl_update(handle_, control_action.data(), token.points.empty() ? nullptr : &token.points.front().first, token.points.size(), &r));
+    }
     return estimate_of(r);
   }
   /// beluga_ros::Amcl::update(base_pose_in_odom, laser_scan) (bb200_sharded_amcl_update_scan).

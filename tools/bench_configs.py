@@ -20,6 +20,9 @@ and a 256 x 2000 batch through update_measurements (100 points per member) again
 with every member weighed by one torch kernel.
 `sharded-publish`: a 1M-particle filter's publish round (particle-cloud histogram and 2000 pose samples) and 1M ray casts on 2
 and 4 shards of one device, next to the single filter (a filter of one shard does not step, so it has no posterior to publish).
+`sharded-weighed`: a 1M-particle step at 1080 beams on the 2000^2 map through the built-in likelihood-field update against the
+same step weighed by the caller (update_weighted, one torch kernel per shard), on one filter and on 2 and 4 shards of device 0
+(and over devices 0..1 and 0..3 where there are that many).
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import ctypes
@@ -551,6 +554,60 @@ def run_weighed():
         res[f"weighed_batch_256_x_2000_{name}"] = {
             "ms_per_step_e2e": float(np.median(t)), "ms_per_step_min_max": [float(min(t)), float(max(t))], "steps": steps, "warmup": warmup,
             "library_launches_per_step": blaunch[name], "kernels_ms": {}, "device": device}
+    return res
+
+
+def run_sharded_weighed():
+    """The built-in sharded step against the weighed sharded step (update_weighted with torch.exp(x) into each shard's factors
+    on its stream), 1M particles x 1080 beams on the 2000^2 map, systematic resampling every step.  One shard does not step
+    (a filter of one shard has no peers to exchange with): the one-shard row is the standalone Amcl.  Then 2 and 4 shards of
+    device 0, and 2 and 4 devices when there are that many.  The built-in and the weighed filter are stepped alternately in
+    one process, host clock around each call (both end synchronised), median and range of `steps` after `warmup`; the
+    per-shard launch counts of the last step."""
+    import torch
+
+    sc = synthetic.make_scenario(grid_size=2000, n_beams=1080, steps=100)
+    grid = bb.OccupancyGrid(sc.cells, sc.resolution)
+    n, warmup, steps = 1_000_000, 3, 30
+    params = bb.AmclParams(min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=1)
+
+    def weigh(states, factors):
+        torch.exp(states[:, 2], out=factors)
+
+    layouts = [("1_shard", None), ("2_shards", [0, 0]), ("4_shards", [0, 0, 0, 0])]
+    layouts += [(f"{k}_devices", list(range(k))) for k in (2, 4) if bb.device_count() >= k]
+    device = device_record()
+    res = {}
+    for name, devices in layouts:
+        filters = {}
+        for kind in ("builtin", "weighed"):
+            f = bb.Amcl(bb.DifferentialDriveModelParam(*MOTION), params) if devices is None else bb.ShardedAmcl(bb.DifferentialDriveModelParam(*MOTION), params, devices)
+            f.update_map(bb.SENSOR_LIKELIHOOD_FIELD, bb.LikelihoodFieldModelParam(**LFM), grid)
+            f.initialize(sc.initial_mean, sc.initial_cov)
+            filters[kind] = f
+        shards = {k: [f.filter] if devices is None else f.shards for k, f in filters.items()}
+        times = {"builtin": [], "weighed": []}
+        launches = {}
+        for k in range(warmup + steps):
+            pose = bb.se2(*sc.poses[k % 100])
+            calls = (("builtin", lambda: filters["builtin"].update(pose, sc.scans[k % 100])), ("weighed", lambda: filters["weighed"].update_weighted(pose, weigh)))
+            for kind, call in calls:
+                before = [s.launch_count() for s in shards[kind]]
+                t0 = time.perf_counter()
+                r = call()
+                dt = (time.perf_counter() - t0) * 1e3
+                assert r.updated == 1 and r.resampled == 1
+                launches[kind] = [s.launch_count() - b for s, b in zip(shards[kind], before)]
+                if k >= warmup:
+                    times[kind].append(dt)
+        for kind in ("builtin", "weighed"):
+            t = times[kind]
+            res[f"sharded_weighed_1M_x_1080_lfm_2000_{name}_{kind}"] = {
+                "shards": 1 if devices is None else len(devices), "devices": [0] if devices is None else devices,
+                "ms_per_step_e2e": float(np.median(t)), "ms_per_step_min_max": [float(min(t)), float(max(t))], "steps": steps, "warmup": warmup,
+                "launches_per_shard": launches[kind], "kernels_ms": {}, "device": device}
+        for f in filters.values():
+            f.close()
     return res
 
 
@@ -1138,6 +1195,8 @@ def main():
         out.update(run_weighed())
     if "sharded-publish" in which:
         out.update(run_sharded_publish())
+    if "sharded-weighed" in which:
+        out.update(run_sharded_weighed())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}

@@ -27,7 +27,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from . import _capi
-from ._capi import (RESAMPLE_MULTINOMIAL, RESAMPLE_SYSTEMATIC, SENSOR_BEAM, SENSOR_LIKELIHOOD_FIELD,
+from ._capi import (RESAMPLE_MULTINOMIAL, RESAMPLE_SYSTEMATIC, SENSOR_BEAM, SENSOR_BEARING, SENSOR_LANDMARK, SENSOR_LIKELIHOOD_FIELD,
                     SENSOR_LIKELIHOOD_FIELD_PROB)
 
 __all__ = [
@@ -35,7 +35,7 @@ __all__ = [
     "Filter", "LikelihoodFieldModelParam", "motion_sampling", "scan_to_points", "scan_bearings", "point_cloud_to_points",
     "take_evenly_indices",
     "OccupancyGrid", "BelugaB200Error", "device_count", "se2", "LaserScan", "PointCloud",
-    "RESAMPLE_MULTINOMIAL", "RESAMPLE_SYSTEMATIC", "SENSOR_BEAM", "SENSOR_LIKELIHOOD_FIELD", "SENSOR_LIKELIHOOD_FIELD_PROB",
+    "LandmarkModelParam", "BearingModelParam", "LandmarkMap", "RESAMPLE_MULTINOMIAL", "RESAMPLE_SYSTEMATIC", "SENSOR_BEAM", "SENSOR_BEARING", "SENSOR_LANDMARK", "SENSOR_LIKELIHOOD_FIELD", "SENSOR_LIKELIHOOD_FIELD_PROB",
 ]
 
 
@@ -343,6 +343,54 @@ class BeamModelParam:
 
 
 @dataclass
+class LandmarkModelParam:
+    """beluga::LandmarkModelParam (sensor/landmark_sensor_model.hpp:44-48)."""
+    sigma_range: float = 1.0
+    sigma_bearing: float = 1.0
+    random_prob: float = 1e-4
+
+    def c(self) -> _capi.LandmarkParam:
+        return _capi.LandmarkParam(self.sigma_range, self.sigma_bearing, self.random_prob)
+
+
+@dataclass
+class BearingModelParam:
+    """beluga::BearingModelParam (sensor/bearing_sensor_model.hpp:42-45); sensor_pose_in_robot is a 3x4 [R | t]."""
+    sigma_bearing: float = 1.0
+    sensor_pose_in_robot: object = None  # None: the identity
+
+    def c(self) -> _capi.BearingParam:
+        m = np.eye(3, 4) if self.sensor_pose_in_robot is None else _f64(self.sensor_pose_in_robot).reshape(3, 4)
+        return _capi.BearingParam(self.sigma_bearing, (C.c_double * 12)(*m.reshape(12)))
+
+
+def _landmark_array(positions, categories):
+    pos = _f64(positions).reshape(-1, 3)
+    cat = np.ascontiguousarray(categories, dtype=np.uint32).reshape(-1)
+    if len(cat) != len(pos):
+        raise ValueError("one category per position")
+    arr = (_capi.Landmark * max(len(pos), 1))()
+    for k in range(len(pos)):
+        arr[k] = _capi.Landmark(pos[k, 0], pos[k, 1], pos[k, 2], int(cat[k]))
+    return arr, len(pos)
+
+
+class LandmarkMap:
+    """beluga::LandmarkMap (sensor/data/landmark_map.hpp:40-166): (n, 3) world positions and n categories, with explicit
+    bounds {x, y, z} or, when both are None, the landmarks' own (:61-71)."""
+
+    def __init__(self, positions, categories, bounds_min=None, bounds_max=None):
+        self.landmarks, self.n = _landmark_array(positions, categories)
+        self.bounds_min = None if bounds_min is None else _f64(bounds_min).reshape(3)
+        self.bounds_max = None if bounds_max is None else _f64(bounds_max).reshape(3)
+
+    def c(self) -> _capi.LandmarkMap:
+        lo = None if self.bounds_min is None else _dptr(self.bounds_min)
+        hi = None if self.bounds_max is None else _dptr(self.bounds_max)
+        return _capi.LandmarkMap(self.landmarks, self.n, lo, hi)
+
+
+@dataclass
 class AmclParams:
     """beluga::AmclParams (algorithm/amcl_core.hpp:34-55) + spatial hash resolutions + backend knobs."""
     update_min_d: float = 0.25
@@ -452,6 +500,22 @@ class Filter:
         p, g = params.c(), grid.c()
         self._grid_shape = grid.cells.shape
         self._check(self._lib.bb200_filter_set_beam_map(self._h, C.byref(p), C.byref(g)))
+
+    def set_landmark_map(self, params: LandmarkModelParam, landmark_map: LandmarkMap):
+        """LandmarkSensorModel2d on `landmark_map`; replaces the map set before, of any model."""
+        p, m = params.c(), landmark_map.c()
+        self._check(self._lib.bb200_filter_set_landmark_map(self._h, C.byref(p), C.byref(m)))
+
+    def set_bearing_map(self, params: BearingModelParam, landmark_map: LandmarkMap):
+        """BearingSensorModel2d on `landmark_map`; replaces the map set before, of any model."""
+        p, m = params.c(), landmark_map.c()
+        self._check(self._lib.bb200_filter_set_bearing_map(self._h, C.byref(p), C.byref(m)))
+
+    def reweight_landmarks(self, positions, categories):
+        """w *= L(state) of the landmark map's model for the detections: (n, 3) positions in the robot frame (landmark
+        model) or bearings in the sensor frame (bearing model), and n categories."""
+        arr, n = _landmark_array(positions, categories)
+        self._check(self._lib.bb200_filter_reweight_landmarks(self._h, arr, n))
 
     def likelihood_field(self) -> np.ndarray:
         out = np.zeros(self._grid_shape, dtype=np.float32)
@@ -698,9 +762,14 @@ class Amcl:
         if st != _capi.OK:
             raise BelugaB200Error(st, self._lib.bb200_amcl_last_error(self._h).decode())
 
-    def update_map(self, sensor: int, params, grid: OccupancyGrid):
-        """Amcl::update_map (amcl_core.hpp:150) / sensor model construction."""
-        if sensor == SENSOR_BEAM:
+    def update_map(self, sensor: int, params, grid):
+        """Amcl::update_map (amcl_core.hpp:150) / sensor model construction.  `grid` is an OccupancyGrid, or a LandmarkMap
+        for SENSOR_LANDMARK and SENSOR_BEARING."""
+        if sensor == SENSOR_LANDMARK:
+            self.filter.set_landmark_map(params, grid)
+        elif sensor == SENSOR_BEARING:
+            self.filter.set_bearing_map(params, grid)
+        elif sensor == SENSOR_BEAM:
             self.filter.set_beam_map(params, grid)
         else:
             self.filter.set_likelihood_field_map(params, grid, prob=(sensor == SENSOR_LIKELIHOOD_FIELD_PROB))
@@ -771,6 +840,14 @@ class Amcl:
         pts = _f64(points).reshape(-1, 2)
         res = _capi.UpdateResult()
         self._check(self._lib.bb200_amcl_update(self._h, _dptr(_f64(control_pose)), _dptr(pts), len(pts), C.byref(res)))
+        return res
+
+    def update_landmarks(self, control_pose, positions, categories) -> _capi.UpdateResult:
+        """Amcl::update with the landmark map's model: (n, 3) detection positions in the robot frame (SENSOR_LANDMARK) or
+        bearings in the sensor frame (SENSOR_BEARING), and n categories."""
+        arr, n = _landmark_array(positions, categories)
+        res = _capi.UpdateResult()
+        self._check(self._lib.bb200_amcl_update_landmarks(self._h, _dptr(_f64(control_pose)), arr, n, C.byref(res)))
         return res
 
     def update_weighted(self, control_pose, weigh) -> _capi.UpdateResult:

@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(HERE, "libbeluga_b200.so")
 OK, ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_NO_DEVICE, ERR_STATE, ERR_CAPACITY = 0, -1, -2, -3, -4, -5
 BATCH_ADAPTIVE, BATCH_SELECTIVE = 1, 2  # bb200_batch_flags
 
-SENSOR_LIKELIHOOD_FIELD, SENSOR_LIKELIHOOD_FIELD_PROB, SENSOR_BEAM = 0, 1, 2
+SENSOR_LIKELIHOOD_FIELD, SENSOR_LIKELIHOOD_FIELD_PROB, SENSOR_BEAM, SENSOR_LANDMARK, SENSOR_BEARING = 0, 1, 2, 3, 4
 RESAMPLE_MULTINOMIAL, RESAMPLE_SYSTEMATIC = 0, 1
 
 
@@ -50,6 +50,22 @@ class LikelihoodFieldParam(C.Structure):
 
 class BeamParam(C.Structure):
     _fields_ = [(n, C.c_double) for n in ("z_hit", "z_short", "z_max", "z_rand", "sigma_hit", "lambda_short", "beam_max_range")]
+
+
+class Landmark(C.Structure):  # also bb200_landmark_detection: the same layout
+    _fields_ = [("x", C.c_double), ("y", C.c_double), ("z", C.c_double), ("category", C.c_uint32)]
+
+
+class LandmarkMap(C.Structure):
+    _fields_ = [("landmarks", C.POINTER(Landmark)), ("n", C.c_uint64), ("bounds_min3", C.POINTER(C.c_double)), ("bounds_max3", C.POINTER(C.c_double))]
+
+
+class LandmarkParam(C.Structure):
+    _fields_ = [(n, C.c_double) for n in ("sigma_range", "sigma_bearing", "random_prob")]
+
+
+class BearingParam(C.Structure):
+    _fields_ = [("sigma_bearing", C.c_double), ("sensor_pose_in_robot", C.c_double * 12)]
 
 
 class OccupancyGrid(C.Structure):
@@ -143,6 +159,9 @@ SIGNATURES = {
     "bb200_last_error": (C.c_char_p, [_vp]),
     "bb200_filter_set_likelihood_field_map": (C.c_int, [_vp, _P(LikelihoodFieldParam), _P(OccupancyGrid), C.c_int]),
     "bb200_filter_set_beam_map": (C.c_int, [_vp, _P(BeamParam), _P(OccupancyGrid)]),
+    "bb200_filter_set_landmark_map": (C.c_int, [_vp, _P(LandmarkParam), _P(LandmarkMap)]),
+    "bb200_filter_set_bearing_map": (C.c_int, [_vp, _P(BearingParam), _P(LandmarkMap)]),
+    "bb200_filter_reweight_landmarks": (C.c_int, [_vp, _P(Landmark), C.c_uint64]),
     "bb200_filter_get_likelihood_field": (C.c_int, [_vp, _P(C.c_float), C.c_uint64]),
     "bb200_filter_set_particles": (C.c_int, [_vp, _dbl, _dbl, C.c_uint64]),
     "bb200_filter_size": (C.c_int, [_vp, _P(C.c_uint64)]),
@@ -195,6 +214,7 @@ SIGNATURES = {
     "bb200_amcl_initialize_from_map": (C.c_int, [_vp]),
     "bb200_amcl_force_update": (None, [_vp]),
     "bb200_amcl_update": (C.c_int, [_vp, _dbl, _dbl, C.c_uint64, _P(UpdateResult)]),
+    "bb200_amcl_update_landmarks": (C.c_int, [_vp, _dbl, _P(Landmark), C.c_uint64, _P(UpdateResult)]),
     "bb200_scan_to_points": (C.c_int, [_P(LaserScan), _dbl, C.c_uint64, _P(C.c_uint64)]),
     "bb200_scan_bearings": (C.c_int, [C.c_float, C.c_float, C.c_uint64, C.c_uint64, _dbl, C.c_uint64, _P(C.c_uint64)]),
     "bb200_take_evenly_indices": (C.c_int, [C.c_uint64, C.c_uint64, _P(C.c_uint64), C.c_uint64, _P(C.c_uint64)]),

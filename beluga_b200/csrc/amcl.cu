@@ -428,6 +428,12 @@ int Amcl::update(const double control[4], const double* points_xy, uint64_t n_po
   return st;
 }
 
+int Amcl::update_landmarks(const double control[4], const bb200_landmark_detection* detections, uint64_t n, bb200_update_result* out) {
+  if (sharded()) return filter_.fail_with(BB200_ERR_STATE, "detection steps run on one GPU; a filter joined to shards takes points");
+  if (const int st = filter_.stage_detections(detections, n)) return st;
+  return update(control, Filter::staged_detections(), 0, out);
+}
+
 bool Amcl::fused(const bb200_step_plan& plan) const {
   return plan.resample != 0 && !plan.needs_ess && !(params().min_particles < params().max_particles);
 }

@@ -226,6 +226,24 @@ int bb200_filter_set_beam_map(bb200_filter* f, const bb200_beam_param* p, const 
   BB_REFUSE_OPEN(f->impl);
   return guarded(f->impl, [&] { return f->impl.set_beam_map(*p, *grid); });
 }
+int bb200_filter_set_landmark_map(bb200_filter* f, const bb200_landmark_param* p, const bb200_landmark_map* map) {
+  BB_REQUIRE(f && p && map);
+  BB_REFUSE_OPEN(f->impl);
+  return guarded(f->impl, [&] { return f->impl.set_landmark_map(p, nullptr, *map); });
+}
+int bb200_filter_set_bearing_map(bb200_filter* f, const bb200_bearing_param* p, const bb200_landmark_map* map) {
+  BB_REQUIRE(f && p && map);
+  BB_REFUSE_OPEN(f->impl);
+  return guarded(f->impl, [&] { return f->impl.set_landmark_map(nullptr, p, *map); });
+}
+int bb200_filter_reweight_landmarks(bb200_filter* f, const bb200_landmark_detection* detections, uint64_t n) {
+  BB_REQUIRE(f && (detections || n == 0));
+  BB_REFUSE_OPEN(f->impl);
+  return guarded(f->impl, [&] {
+    const int st = f->impl.stage_detections(detections, n);
+    return st != BB200_OK ? st : f->impl.propagate_reweight(nullptr, 0, Filter::staged_detections(), 0);
+  });
+}
 int bb200_filter_get_likelihood_field(const bb200_filter* f, float* out, uint64_t capacity) {
   BB_REQUIRE(f && out);
   BB_REFUSE_OPEN(f->impl);
@@ -589,6 +607,12 @@ int bb200_amcl_update(bb200_amcl* a, const double control_pose[4], const double*
   BB_REFUSE_OPEN(a->impl.filter());
   static const double kNoPoints[2] = {0.0, 0.0};
   return guarded(a->impl, [&] { return a->impl.update(control_pose, points_xy != nullptr ? points_xy : kNoPoints, n_points, out); });
+}
+int bb200_amcl_update_landmarks(bb200_amcl* a, const double control_pose[4], const bb200_landmark_detection* detections, uint64_t n,
+                                bb200_update_result* out) {
+  BB_REQUIRE(a && control_pose && out && (detections || n == 0));
+  BB_REFUSE_OPEN(a->impl.filter());
+  return guarded(a->impl, [&] { return a->impl.update_landmarks(control_pose, detections, n, out); });
 }
 int bb200_amcl_update_begin(bb200_amcl* a, const double control_pose[4], bb200_weigh_view* view) {
   BB_REQUIRE(a && control_pose && view);

@@ -122,6 +122,7 @@ void DeviceMap::release() {
   static_cast<MapLayout&>(*this) = MapLayout{};
   field_host.clear();
   free_cells = nullptr;
+  landmark_slices.clear();
 }
 
 template <class T>
@@ -152,6 +153,7 @@ int DeviceMap::upload(const MapTables& t, cudaStream_t stream, std::string* erro
   BB_CHECK(copy(t.free_distance, &tables_.free_distance, &occupancy.free_distance, stream));
   BB_CHECK(copy(t.free_padded, &tables_.free_padded, &occupancy.free_padded, stream));
   BB_CHECK(copy(t.free_cells, &tables_.free_cells, &free_cells, stream));
+  BB_CHECK(copy(t.landmark_points, &tables_.landmarks, &landmarks, stream));
   if (t.sensor == BB200_SENSOR_BEAM) {
     if (const uint32_t entries = beam_eta_entries(beam.beam_max_range, grid_resolution)) {
       BB_CHECK(tables_.eta.allocate(entries));
@@ -163,6 +165,7 @@ int DeviceMap::upload(const MapTables& t, cudaStream_t stream, std::string* erro
   }
   BB_CHECK(cudaStreamSynchronize(stream));  // the host tables may go once this returns
   field_host = t.field_host;
+  landmark_slices = t.landmark_slices;
   ray_.grid = t.ray_grid;
   sensor = t.sensor;
   return BB200_OK;
@@ -171,6 +174,7 @@ int DeviceMap::upload(const MapTables& t, cudaStream_t stream, std::string* erro
 int DeviceMap::ray_view(cudaStream_t stream, OccupancyView* view, std::string* error) {
   auto check = [error](cudaError_t e, const char* what) { return cuda_check(e, what, error); };
   if (sensor < 0) return reject(BB200_ERR_STATE, "no map", error);
+  if (landmark_map()) return reject(BB200_ERR_STATE, "a landmark map has no grid to cast rays on", error);
   if (sensor == BB200_SENSOR_BEAM) {
     *view = occupancy;
     return BB200_OK;
@@ -198,6 +202,11 @@ int DeviceMap::ray_view(cudaStream_t stream, OccupancyView* view, std::string* e
 }
 
 void DeviceMap::centre(double pivot[2]) const {
+  if (landmark_map()) {
+    pivot[0] = 0.5 * (box[0] + box[1]);
+    pivot[1] = 0.5 * (box[2] + box[3]);
+    return;
+  }
   const double cx = 0.5 * grid_width * grid_resolution, cy = 0.5 * grid_height * grid_resolution;
   pivot[0] = (grid_origin.c * cx - grid_origin.s * cy) + grid_origin.x;
   pivot[1] = (grid_origin.s * cx + grid_origin.c * cy) + grid_origin.y;

@@ -209,6 +209,9 @@ int Filter::enqueue_propagate_reweight(const bb200_motion_sampling* sampling, ui
   if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
   const bool do_reweight = points_xy != nullptr;
   if (do_reweight && map_.sensor < 0) return fail(BB200_ERR_STATE, "no sensor model map set");
+  if (do_reweight) {
+    if (const int st = check_measurement(points_xy)) return st;
+  }
   if (do_reweight && n_points > 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, "too many points");
   BB_CHECK(cudaSetDevice(config_.device));
   if (do_reweight) {
@@ -255,7 +258,7 @@ int Filter::enqueue_resample_range(const bb200_resample_opts& o, uint64_t global
   if (!cdf_valid_) return fail(BB200_ERR_STATE, "build_cdf must run before resample_range");
   if (o.scheme != BB200_RESAMPLE_SYSTEMATIC || o.min_particles < o.max_particles)
     return fail(BB200_ERR_STATE, "range resampling supports the systematic comb without KLD (multinomial or KLD on shards: bb200_amcl_join_shards / bb200_sharded_amcl)");
-  if (o.random_state_probability > 0.0 && map_.n_free == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
+  if (o.random_state_probability > 0.0 && !map_.can_draw_states()) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells or a non-empty landmark box");
   if (slot_end < slot_begin || slot_end - slot_begin > capacity_) return fail(BB200_ERR_CAPACITY, "slot range exceeds the staging buffer");
   BB_CHECK(cudaSetDevice(config_.device));
   if (slot_end > slot_begin) {
@@ -265,7 +268,7 @@ int Filter::enqueue_resample_range(const bb200_resample_opts& o, uint64_t global
     a.cdf_offset = cdf_offset;
     a.weights_out = nullptr;  // the current weights stay untouched; adopt() writes the ones
     mark("resample_range");
-    launch_resample(a, scalars_.get(), partials_.get(), stream_);
+    launch_resample(a, random_box(), scalars_.get(), partials_.get(), stream_);
     BB_LAUNCHED("resample_range");
   }
   return BB200_OK;
@@ -315,9 +318,10 @@ int Filter::step_begin(const bb200_motion_sampling& sampling, uint32_t step, con
   const bool kld = o.min_particles < o.max_particles;
   if (n_ == 0 && !(world > 1 && link_.kld())) return fail(BB200_ERR_STATE, "no particles");  // a KLD-sized filter may leave a shard empty
   if (map_.sensor < 0) return fail(BB200_ERR_STATE, "no sensor model map set");
+  if (const int st = check_measurement(points_xy)) return st;
   if (kld && !(world > 1 && link_.kld())) return fail(BB200_ERR_STATE, "the fused step does not run KLD on one GPU; use resample()");
   if (n_points > 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, "too many points");
-  if (o.random_state_probability > 0.0 && map_.n_free == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
+  if (o.random_state_probability > 0.0 && !map_.can_draw_states()) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells or a non-empty landmark box");
   if (world > 1) {
     if (const int st = check_shard_size(o)) return st;
   } else if (o.max_particles == 0 || o.max_particles > capacity_) {
@@ -360,7 +364,7 @@ int Filter::step_phase(int phase) {
         st = weigh_apply();
       } else {
         mark("begin_step");
-        const bool scheduled = n_ >= kScheduleMinParticles;
+        const bool scheduled = n_ >= kScheduleMinParticles && !map_.landmark_map();
         const bool warm = map_.sensor != BB200_SENSOR_BEAM && map_.field.use_fixed && map_.bordered_bytes <= (96ull << 20);
         launch_begin_fused_step(scalars_.get(), tile_state_.get(), scan_tile_count(n_), sched_.get(), scheduled ? counters_.get() : nullptr,
                                 schedule_max_bins(), sched_tiles_.get(), schedule_tile_count(), warm ? map_.field.bordered : nullptr,
@@ -453,7 +457,7 @@ int Filter::step_phase(int phase) {
         summary_host_.get()->seq = 0;  // nothing of this filter is in flight: the previous step was seen to end
       }
       a.tail = StepTail{1, results_.get(), sharded ? nullptr : summary_host_.get(), step_.poll_seq};
-      step_.partial_rows = launch_resample(a, scalars_.get(), partials_.get(), stream_);
+      step_.partial_rows = launch_resample(a, random_box(), scalars_.get(), partials_.get(), stream_);
       BB_LAUNCHED("resample");
       step_.resampled = true;
       if (sharded && split) {
@@ -525,7 +529,7 @@ int Filter::kld_sharded_candidates(uint64_t begin, uint64_t end) {
     a.slot_count = end - begin;
   }
   mark("kld_candidates");
-  launch_resample(a, scalars_.get(), partials_.get(), stream_);
+  launch_resample(a, random_box(), scalars_.get(), partials_.get(), stream_);
   BB_LAUNCHED("kld_candidates");
   link_.begin_batch();
   if (link_.split_posts()) return enqueue_exchange(kExchangeKld, true, false);
@@ -654,6 +658,32 @@ int Filter::set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& 
   return st != BB200_OK ? st : set_map(tables);
 }
 
+int Filter::set_landmark_map(const bb200_landmark_param* lp, const bb200_bearing_param* bp, const bb200_landmark_map& map) {
+  MapTables tables;
+  const int st = prepare_landmark_map(lp, bp, map, &tables, &error_);
+  return st != BB200_OK ? st : set_map(tables);
+}
+
+const double Filter::kStagedDetections = 0.0;
+
+int Filter::stage_detections(const bb200_landmark_detection* detections, uint64_t n) {
+  if (!map_.landmark_map()) return fail(BB200_ERR_STATE, "detections need a landmark map (set_landmark_map / set_bearing_map)");
+  if (n >= 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, "too many detections");
+  std::vector<LandmarkDetection> prepared;
+  prepare_detections(map_.landmark_slices, detections, n, &prepared);
+  BB_CHECK(cudaSetDevice(config_.device));
+  BB_CHECK(cudaStreamSynchronize(stream_));  // the previous step's copy has left the staging buffer
+  const uint64_t room = std::max<uint64_t>(n, 64);
+  BB_CHECK(detections_.grow(n, room));
+  BB_CHECK(detections_host_.grow(n, room));
+  if (n > 0) {
+    std::memcpy(detections_host_.get(), prepared.data(), n * sizeof(LandmarkDetection));
+    BB_CHECK(cudaMemcpyAsync(detections_.get(), detections_host_.get(), n * sizeof(LandmarkDetection), cudaMemcpyHostToDevice, stream_));
+  }
+  n_detections_ = static_cast<uint32_t>(n);
+  return BB200_OK;
+}
+
 int Filter::set_map(const MapTables& tables) {
   BB_CHECK(cudaSetDevice(config_.device));
   return map_.upload(tables, stream_, &error_);
@@ -726,11 +756,16 @@ int Filter::initialize_normal(const double mean[3], const double cov[9], uint64_
 int Filter::initialize_uniform(uint64_t n) {
   if (n > capacity_) return fail(BB200_ERR_CAPACITY, "more particles than the filter capacity");
   if (map_.sensor < 0) return fail(BB200_ERR_STATE, "initialize_from_map needs a map (set_*_map first)");
-  if (map_.n_free == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
+  if (!map_.can_draw_states()) return fail(BB200_ERR_STATE, "the map has no free cell (or, for a landmark map, no non-empty box) to sample from");
   BB_CHECK(cudaSetDevice(config_.device));
-  launch_initialize_uniform(states_[cur_].get(), weights_.get(), n, map_.free_cells, map_.n_free, map_.grid_width, map_.grid_resolution, map_.grid_origin,
-                            config_.seed, first_index_, stream_);
-  BB_LAUNCHED("initialize_uniform");
+  if (map_.landmark_map()) {
+    launch_initialize_box(states_[cur_].get(), weights_.get(), n, map_.box, config_.seed, first_index_, stream_);
+    BB_LAUNCHED("initialize_box");
+  } else {
+    launch_initialize_uniform(states_[cur_].get(), weights_.get(), n, map_.free_cells, map_.n_free, map_.grid_width, map_.grid_resolution,
+                              map_.grid_origin, config_.seed, first_index_, stream_);
+    BB_LAUNCHED("initialize_uniform");
+  }
   BB_CHECK(cudaStreamSynchronize(stream_));
   n_ = n;
   cdf_valid_ = false;
@@ -779,7 +814,8 @@ bool Filter::predict_schedule(const MotionSampling& s, Schedule* grid) const {
 }
 
 int Filter::enqueue_propagate_reweight_kernels(const MotionSampling* sampling, uint32_t step, bool do_reweight, uint64_t n_points, bool counters_reset) {
-  const bool scheduled = do_reweight && n_ >= kScheduleMinParticles;
+  // The pose-sorted schedule is for the grid gathers' locality: a landmark map has no grid.
+  const bool scheduled = do_reweight && n_ >= kScheduleMinParticles && !map_.landmark_map();
   Schedule grid{};
   const uint32_t* perm = nullptr;
   if (scheduled && counters_reset && sampling != nullptr && predict_schedule(*sampling, &grid)) {
@@ -805,7 +841,12 @@ int Filter::enqueue_propagate_reweight_kernels(const MotionSampling* sampling, u
     perm = perm_.get();
   }
   if (do_reweight) {
-    if (map_.sensor == BB200_SENSOR_BEAM) {
+    if (map_.landmark_map()) {
+      mark("reweight_landmark");
+      launch_reweight_landmark(states_[cur_].get(), weights_.get(), n_, map_.landmark, map_.landmarks, detections_.get(), n_detections_,
+                               scalars_.get(), stream_);
+      BB_LAUNCHED("reweight_landmark");
+    } else if (map_.sensor == BB200_SENSOR_BEAM) {
       mark("reweight_beam");
       uint64_t pass = 0;
       if (n_points > 0 && beam_two_pass_map(map_)) {
@@ -984,7 +1025,7 @@ int Filter::sample_states(uint64_t count, uint32_t step, double* states_out) {
   ResampleArgs a = make_resample_args(o, 0, count, false);
   a.weights_out = nullptr;  // the weights stay what they are
   a.ancestors = nullptr;
-  launch_resample(a, scalars_.get(), partials_.get(), stream_);  // into the staging state buffer; no flip
+  launch_resample(a, random_box(), scalars_.get(), partials_.get(), stream_);  // into the staging state buffer; no flip
   BB_LAUNCHED("sample_states");
   BB_CHECK(cudaMemcpyAsync(states_out, states_[cur_ ^ 1].get(), count * sizeof(Pose2), cudaMemcpyDeviceToHost, stream_));
   BB_CHECK(cudaStreamSynchronize(stream_));
@@ -1012,7 +1053,7 @@ int Filter::sample_range(uint64_t count, uint32_t step, uint64_t global_total, u
   link_.target_states(&a, cur_ ^ 1);
   a.rank_totals = nullptr;  // the offsets of the CDF the caller names, not the totals the last step exchanged
   a.peer_shard = capacity_;
-  launch_resample(a, scalars_.get(), partials_.get(), stream_);
+  launch_resample(a, random_box(), scalars_.get(), partials_.get(), stream_);
   BB_LAUNCHED("sample_range");
   return BB200_OK;
 }
@@ -1040,6 +1081,7 @@ int Filter::staging_states(double* out, uint64_t n) {
 
 int Filter::check_cast_rays(const double* poses, uint64_t n_poses, const double* bearings, uint64_t n_bearings, const double* ranges, uint64_t* n_rays) {
   if (map_.sensor < 0) return fail(BB200_ERR_STATE, "no map");
+  if (map_.landmark_map()) return fail(BB200_ERR_STATE, "a landmark map has no grid to cast rays on");
   if (!cast_ray_count(n_poses, n_bearings, n_rays)) return fail(BB200_ERR_INVALID_ARGUMENT, "n_poses * n_bearings overflows");
   if ((poses == nullptr && n_poses > 0) || (bearings == nullptr && n_bearings > 0) || (ranges == nullptr && *n_rays > 0))
     return fail(BB200_ERR_INVALID_ARGUMENT, "null array with a non-zero count");
@@ -1109,7 +1151,7 @@ ResampleArgs Filter::make_resample_args(const bb200_resample_opts& o, uint64_t s
 int Filter::resample(const bb200_resample_opts& o, uint64_t* new_size) {
   if (n_ == 0) return fail(BB200_ERR_STATE, "no particles");
   if (o.max_particles == 0 || o.max_particles > capacity_) return fail(BB200_ERR_CAPACITY, "max_particles exceeds the filter capacity");
-  if (o.random_state_probability > 0.0 && map_.n_free == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
+  if (o.random_state_probability > 0.0 && !map_.can_draw_states()) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells or a non-empty landmark box");
   int st = ensure_cdf_ready();
   if (st != BB200_OK && !cdf_valid_) return st;
   BB_CHECK(cudaSetDevice(config_.device));
@@ -1118,7 +1160,7 @@ int Filter::resample(const bb200_resample_opts& o, uint64_t* new_size) {
   if (o.min_particles >= o.max_particles) {
     // take_while_kld never stops before max when min == max (take_while_kld.hpp:86-87,136).
     mark("resample");
-    launch_resample(make_resample_args(o, 0, o.max_particles, false), scalars_.get(), partials_.get(), stream_);
+    launch_resample(make_resample_args(o, 0, o.max_particles, false), random_box(), scalars_.get(), partials_.get(), stream_);
     BB_LAUNCHED("resample");
     BB_CHECK(cudaStreamSynchronize(stream_));
   } else {
@@ -1179,7 +1221,7 @@ int Filter::resample_kld(const bb200_resample_opts& o, uint64_t* accepted) {
   uint64_t end = std::min<uint64_t>(max, std::max<uint64_t>(2 * o.min_particles, 65536));
   *accepted = max;
   while (begin < max) {
-    launch_resample(make_resample_args(o, begin, end, true), scalars_.get(), partials_.get(), stream_);
+    launch_resample(make_resample_args(o, begin, end, true), random_box(), scalars_.get(), partials_.get(), stream_);
     BB_LAUNCHED("resample");
     KldArgs k{kld_.hashes.get() + begin, end - begin, begin, k_before, o.min_particles, o.kld_epsilon, o.kld_z};
     launch_kld_chunk(k, kld_.keys.get(), kld_.vals.get(), kld_.keys.size(), kld_.flags.get(), kld_.scan.get(), scalars_.get(), tile_state_.get(), stream_);
@@ -1217,7 +1259,7 @@ int Filter::weigh_prepare(const bb200_resample_opts& o, bool injects) {
   } else if (o.max_particles == 0 || o.max_particles > capacity_) {
     return fail(BB200_ERR_CAPACITY, "max_particles exceeds the filter capacity");
   }
-  if (injects && map_.n_free == 0) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells");
+  if (injects && !map_.can_draw_states()) return fail(BB200_ERR_STATE, "recovery injection needs a map with free cells or a non-empty landmark box");
   BB_CHECK(cudaSetDevice(config_.device));
   if (factors_.get() == nullptr) BB_CHECK(factors_.allocate(capacity_));
   if (sharded && factors_applied_ == nullptr) BB_CHECK(cudaEventCreateWithFlags(&factors_applied_, cudaEventDisableTiming));

@@ -37,6 +37,13 @@ class Filter {
   // Every method returns a bb200_status and records the message for last_error().
   int set_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob);
   int set_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid);
+  /// A landmark map for LandmarkSensorModel2d (lp) or, with lp null, BearingSensorModel2d (bp).
+  int set_landmark_map(const bb200_landmark_param* lp, const bb200_bearing_param* bp, const bb200_landmark_map& map);
+  /// Prepares a step's detections on a landmark map and enqueues their upload; BB200_ERR_STATE on any other map.  The
+  /// reweight of a step that passes staged_detections() as its points weighs them.
+  int stage_detections(const bb200_landmark_detection* detections, uint64_t n);
+  /// The `points_xy` of a step on a landmark map: the reweight weighs the staged detections instead of points.
+  static const double* staged_detections() { return &kStagedDetections; }
   /// Makes the prepared tables this filter's map (the upload half of set_*_map).
   int set_map(const MapTables& tables);
   int get_likelihood_field(float* out, uint64_t capacity) const;
@@ -209,6 +216,8 @@ class Filter {
   int resample_kld(const bb200_resample_opts& o, uint64_t* accepted);
   /// The KLD tables for `slots` candidate slots, all or none (the one-GPU hashes, or the shards' scan state).
   int ensure_kld_tables(uint64_t slots, bool sharded);
+  /// The box injected states are drawn from on a landmark map (launch_resample), null on a grid map.
+  const double* random_box() const { return map_.landmark_map() ? map_.box : nullptr; }
   ResampleArgs make_resample_args(const bb200_resample_opts& o, uint64_t slot_begin, uint64_t slot_end, bool with_hashes) const;
   void mark(const char* name);  // timing: record an event before the next kernel
   void finish_marks();
@@ -279,6 +288,16 @@ class Filter {
   DeviceBuffer<double> points_;
   PinnedBuffer<double> points_host_;  // staging
   double points_radius_{0.0};
+  static const double kStagedDetections;
+  /// A step's measurement against the map's kind: points on a grid map, staged detections on a landmark map.
+  int check_measurement(const double* points_xy) {
+    if (map_.landmark_map() != (points_xy == staged_detections()))
+      return fail(BB200_ERR_STATE, map_.landmark_map() ? "a landmark map weighs detections, not points" : "detections need a landmark map");
+    return BB200_OK;
+  }
+  DeviceBuffer<LandmarkDetection> detections_;    // landmark maps: the staged detections ...
+  PinnedBuffer<LandmarkDetection> detections_host_;
+  uint32_t n_detections_{0};                      // ... and their count
   double points_mean_range_{1.0};
 
   // execution schedule (pose-sorted processing order of the reweight kernels)

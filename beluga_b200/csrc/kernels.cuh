@@ -204,6 +204,9 @@ void launch_initialize_normal(Pose2* states, double* weights, uint64_t n, const 
 /// initialize_from_map: n states uniform over the free cells (centroids, global frame), yaw uniform, weights 1.
 void launch_initialize_uniform(Pose2* states, double* weights, uint64_t n, const uint32_t* free_cells, uint64_t n_free, int grid_width,
                                double grid_resolution, const Pose2& grid_origin, uint64_t seed, uint64_t first_index, cudaStream_t stream);
+/// initialize_from_map on a landmark map: n states uniform over the box {min_x, max_x, min_y, max_y} (random_box_state).
+void launch_initialize_box(Pose2* states, double* weights, uint64_t n, const double box[4], uint64_t seed, uint64_t first_index,
+                           cudaStream_t stream);
 
 /// Offset of cell (xi, yi) in the tiled table.
 BB_HD size_t tiled_index(int xi, int yi, int tiles_x) {
@@ -398,6 +401,9 @@ uint32_t resample_block_count(uint64_t slots);
 /// sample | random_intersperse | (hash) | assign, plus per-block raw moments of the new set.  Returns the number of
 /// blocks launched (= rows of moment_partials written).
 uint32_t launch_resample(const ResampleArgs& args, Scalars* scalars, double* moment_partials, cudaStream_t stream);
+/// launch_resample for a landmark map: injected states are drawn from `box` {min_x, max_x, min_y, max_y}
+/// (resample_box_kernel) instead of the free cells.  box null: launch_resample.
+uint32_t launch_resample(const ResampleArgs& args, const double* box, Scalars* scalars, double* moment_partials, cudaStream_t stream);
 
 /// Blocks of the scatter-form resample over n_in particles (launch_resample picks that form for a plain systematic comb).
 uint32_t resample_scatter_block_count(uint64_t n_in);

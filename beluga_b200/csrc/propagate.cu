@@ -40,6 +40,15 @@ __global__ void __launch_bounds__(256) initialize_uniform_kernel(Pose2* states, 
   weights[i] = 1.0;
 }
 
+// initialize_from_map on a landmark map: the same draw over the map's box (random_box_state).
+__global__ void __launch_bounds__(256) initialize_box_kernel(Pose2* states, double* weights, uint64_t n, BoxSpace box, uint64_t seed,
+                                                             uint64_t first_index) {
+  const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  store_pose(states + i, random_box_state(box, seed, first_index + i, 0));
+  weights[i] = 1.0;
+}
+
 // ---- propagate (a2 + a6) --------------------------------------------------------------------------
 // One thread per particle, original order.  Also accumulates the first and second moments of the
 // propagated cloud (block reduction + double atomics); they only feed the execution schedule below,
@@ -177,6 +186,13 @@ void launch_initialize_uniform(Pose2* states, double* weights, uint64_t n, const
   if (n == 0) return;
   const FreeSpace fs{free_cells, n_free, grid_width, grid_resolution, grid_origin};
   initialize_uniform_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(states, weights, n, fs, seed, first_index);
+}
+
+void launch_initialize_box(Pose2* states, double* weights, uint64_t n, const double box[4], uint64_t seed, uint64_t first_index,
+                           cudaStream_t stream) {
+  if (n == 0) return;
+  const BoxSpace b{box[0], box[1], box[2], box[3]};
+  initialize_box_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(states, weights, n, b, seed, first_index);
 }
 
 void launch_propagate(Pose2* states, uint64_t n, bool do_propagate, const MotionSampling& sampling, uint64_t seed, uint32_t step,

@@ -30,6 +30,25 @@ __device__ __forceinline__ Pose2 random_free_state(const FreeSpace& fs, const Dr
   return Pose2{rot.c, rot.s, (fs.origin.c * lx - fs.origin.s * ly) + fs.origin.x, (fs.origin.s * lx + fs.origin.c * ly) + fs.origin.y};
 }
 
+/// MultivariateUniformDistribution<SE2d, AlignedBox2d> (random/multivariate_uniform_distribution.hpp:43-73) over a
+/// landmark map's bounds: yaw ~ U[-pi, pi) first (SO2d::sampleUniform), then x, then y, each a
+/// std::uniform_real_distribution: u * (max - min) + min.  Counter stream 6 gives yaw (word a) and x (word b), stream 7 y
+/// (word a), both at the index and step of the free-cell draw.
+struct BoxSpace {
+  double min_x, max_x, min_y, max_y;
+};
+
+__device__ __forceinline__ Pose2 random_box_state(const BoxSpace& box, uint64_t seed, uint64_t index, uint32_t step) {
+  const Draw r = counter_draw(seed, index, step, kStreamRandomState);
+  const Draw q = counter_draw(seed, index, step, kStreamRandomBox);
+  const double pi = 3.14159265358979323846;
+  const double yaw = uniform01(r.a) * (pi - (-pi)) + (-pi);
+  const double x = uniform01(r.b) * (box.max_x - box.min_x) + box.min_x;
+  const double y = uniform01(q.a) * (box.max_y - box.min_y) + box.min_y;
+  const Rot2 rot = rot_exp(yaw);
+  return Pose2{rot.c, rot.s, x, y};
+}
+
 __device__ __forceinline__ Pose2 propagate_one(const Pose2& st, const MotionSampling& p, uint64_t seed, uint64_t index, uint32_t step) {
   double z0, z1;
   box_muller_fast(counter_draw(seed, index, step, kStreamMotion0), z0, z1);

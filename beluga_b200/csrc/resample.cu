@@ -20,6 +20,11 @@ __global__ void __launch_bounds__(kRsThreads) resample_kernel(ResampleArgs a, Sc
   resample_block(a, scalars, moment_partials, blockIdx.x, gridDim.x, a.tail);
 }
 
+__global__ void __launch_bounds__(kRsThreads) resample_box_kernel(ResampleArgs a, Scalars* __restrict__ scalars, double* __restrict__ moment_partials,
+                                                                  BoxSpace box) {
+  resample_block<StepTail, true>(a, scalars, moment_partials, blockIdx.x, gridDim.x, a.tail, box);
+}
+
 __global__ void __launch_bounds__(kRsThreads, kRsBlocksPerSm) resample_scatter_kernel(ResampleArgs a, Scalars* __restrict__ scalars,
                                                                      double* __restrict__ moment_partials) {
   resample_scatter_block(a, scalars, moment_partials, blockIdx.x, gridDim.x, a.tail);
@@ -81,6 +86,13 @@ uint32_t launch_resample(const ResampleArgs& args, Scalars* scalars, double* mom
   }
   const uint32_t blocks = resample_block_count(args.slot_count);
   resample_kernel<<<blocks, kRsThreads, 0, stream>>>(args, scalars, moment_partials);
+  return blocks;
+}
+
+uint32_t launch_resample(const ResampleArgs& args, const double* box, Scalars* scalars, double* moment_partials, cudaStream_t stream) {
+  if (box == nullptr || args.random_state_probability <= 0.0) return launch_resample(args, scalars, moment_partials, stream);
+  const uint32_t blocks = resample_block_count(args.slot_count);
+  resample_box_kernel<<<blocks, kRsThreads, 0, stream>>>(args, scalars, moment_partials, BoxSpace{box[0], box[1], box[2], box[3]});
   return blocks;
 }
 

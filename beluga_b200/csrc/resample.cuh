@@ -165,10 +165,11 @@ __device__ __forceinline__ void finish_block_moments(double* m, double* scratch,
   if (threadIdx.x == 0) tail_publish(tail, v, scalars);
 }
 
-/// Block `block` of `grid` of the per-slot resample (resample_kernel).
-template <class Tail>
+/// Block `block` of `grid` of the per-slot resample (resample_kernel; resample_box_kernel with kBox, whose injected
+/// states come from a landmark map's box).
+template <class Tail, bool kBox = false>
 __device__ __forceinline__ void resample_block(const ResampleArgs& a, Scalars* __restrict__ scalars, double* __restrict__ moment_partials,
-                                               uint32_t block, uint32_t grid, const Tail& tail) {
+                                               uint32_t block, uint32_t grid, const Tail& tail, const BoxSpace& box = BoxSpace{}) {
   __shared__ double s_red[kMomentCount * kRsThreads / kWarp];
   unsigned long long total = a.global_total != 0 ? a.global_total : scalars->total;
   unsigned long long cdf_offset = a.cdf_offset, span_end = 0;
@@ -231,8 +232,12 @@ __device__ __forceinline__ void resample_block(const ResampleArgs& a, Scalars* _
       if (!mine) continue;
     }
     if (inject) {
-      st = random_free_state(FreeSpace{a.free_cells, a.n_free, a.grid_width, a.grid_resolution, a.grid_origin},
-                             counter_draw(a.seed, j, a.step, kStreamRandomState));
+      if constexpr (kBox) {
+        st = random_box_state(box, a.seed, j, a.step);
+      } else {
+        st = random_free_state(FreeSpace{a.free_cells, a.n_free, a.grid_width, a.grid_resolution, a.grid_origin},
+                               counter_draw(a.seed, j, a.step, kStreamRandomState));
+      }
     } else {
       const uint64_t idx = cdf_upper_bound(a.cdf, a.n_in, t - cdf_offset);  // the caller guarantees t lies in this shard's span
       ancestor = static_cast<long long>(idx);

@@ -162,7 +162,8 @@ enum Stream : uint32_t {
   kStreamMotion1 = 3,
   kStreamResample = 4,
   kStreamSystematic = 5,
-  kStreamRandomState = 6
+  kStreamRandomState = 6,
+  kStreamRandomBox = 7  // the second draw of a state inside a landmark map's box (random_box_state)
 };
 
 struct Draw {

@@ -124,8 +124,48 @@ typedef struct bb200_occupancy_grid {
 typedef enum bb200_sensor_model {
   BB200_SENSOR_LIKELIHOOD_FIELD = 0,      /* sensor/likelihood_field_model.hpp:69-90: 1 + sum pz^3 */
   BB200_SENSOR_LIKELIHOOD_FIELD_PROB = 1, /* sensor/likelihood_field_prob_model.hpp:69-90: exp(sum log pz) */
-  BB200_SENSOR_BEAM = 2                   /* sensor/beam_model.hpp:104-150 */
+  BB200_SENSOR_BEAM = 2,                  /* sensor/beam_model.hpp:104-150 */
+  BB200_SENSOR_LANDMARK = 3,              /* sensor/landmark_sensor_model.hpp:96-156: range and bearing to the nearest landmark */
+  BB200_SENSOR_BEARING = 4                /* sensor/bearing_sensor_model.hpp:92-140: bearing to the best-aligned landmark */
 } bb200_sensor_model;
+
+/* One landmark of a beluga::LandmarkMap (sensor/data/landmark_map.hpp:40-166): its position in the world frame and its
+ * category (LandmarkPositionDetection, types/landmark_detection_types.hpp:39-42). */
+typedef struct bb200_landmark {
+  double x, y, z;
+  uint32_t category;
+} bb200_landmark;
+
+/* LandmarkMap{boundaries, landmarks} (landmark_map.hpp:49-51), or LandmarkMap{landmarks} with null bounds: the implicit
+ * bounds are the landmarks' componentwise minimum and maximum (:61-71).  Only x and y of the bounds are used: they are
+ * the box of MultivariateUniformDistribution<SE2d, AlignedBox2d> (random/multivariate_uniform_distribution.hpp:43-73). */
+typedef struct bb200_landmark_map {
+  const bb200_landmark* landmarks;
+  uint64_t n;
+  const double* bounds_min3; /* {x, y, z}, or NULL with bounds_max3 NULL */
+  const double* bounds_max3;
+} bb200_landmark_map;
+
+/* beluga::LandmarkModelParam -- sensor/landmark_sensor_model.hpp:44-48 */
+typedef struct bb200_landmark_param {
+  double sigma_range;   /* > 0 */
+  double sigma_bearing; /* > 0 */
+  double random_prob;   /* in [0, 1]; also the factor of a detection with no landmark of its category */
+} bb200_landmark_param;
+
+/* beluga::BearingModelParam -- sensor/bearing_sensor_model.hpp:42-45 */
+typedef struct bb200_bearing_param {
+  double sigma_bearing;             /* > 0 */
+  double sensor_pose_in_robot[12];  /* 3x4 row-major [R | t]; R a rotation (within 1e-9) */
+} bb200_bearing_param;
+
+/* One detection: LandmarkPositionDetection (a position in the robot frame) for BB200_SENSOR_LANDMARK, or
+ * LandmarkBearingDetection (a bearing vector in the sensor frame, any length) for BB200_SENSOR_BEARING
+ * (types/landmark_detection_types.hpp:39-48). */
+typedef struct bb200_landmark_detection {
+  double x, y, z;
+  uint32_t category;
+} bb200_landmark_detection;
 
 typedef enum bb200_resample_scheme {
   BB200_RESAMPLE_MULTINOMIAL = 0, /* views/sample.hpp:128-135 in counter-RNG form */
@@ -175,6 +215,18 @@ const char* bb200_last_error(const bb200_filter* f);
 int bb200_filter_set_likelihood_field_map(bb200_filter* f, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid, int prob);
 /* BeamSensorModel{params, grid} (beam_model.hpp:96) / update_map (:156). */
 int bb200_filter_set_beam_map(bb200_filter* f, const bb200_beam_param* p, const bb200_occupancy_grid* grid);
+/* LandmarkSensorModel2d<LandmarkMap>{params, map} (landmark_sensor_model.hpp:83-84) / update_map (:160) and
+ * BearingSensorModel2d<LandmarkMap>{params, map} (bearing_sensor_model.hpp:80-81) / update_map (:144).  A landmark map has
+ * no grid: ray casts, bb200_filter_get_likelihood_field and point steps return BB200_ERR_STATE on it, and a detections
+ * step on a grid map returns BB200_ERR_STATE.  initialize_from_map and recovery injection draw from
+ * MultivariateUniformDistribution<SE2d, AlignedBox2d> over the map's x-y bounds (multivariate_uniform_distribution.hpp:
+ * 43-73; counter streams 6 and 7, DESIGN.md §1); on an empty or non-finite box they return BB200_ERR_STATE.  The landmarks are kept stably sorted by category on the device, so every detection scans its
+ * category's landmarks in the map's order. */
+int bb200_filter_set_landmark_map(bb200_filter* f, const bb200_landmark_param* p, const bb200_landmark_map* map);
+int bb200_filter_set_bearing_map(bb200_filter* f, const bb200_bearing_param* p, const bb200_landmark_map* map);
+/* actions::reweight(sensor_model(detections)) (actions/reweight.hpp:54-60) on a landmark map: w *= L(state), with L the
+ * std::transform_reduce product over the detections (landmark_sensor_model.hpp:155, bearing_sensor_model.hpp:139). */
+int bb200_filter_reweight_landmarks(bb200_filter* f, const bb200_landmark_detection* detections, uint64_t n);
 /* likelihood_field() accessor (likelihood_field_model_base.hpp:102): width*height floats. */
 int bb200_filter_get_likelihood_field(const bb200_filter* f, float* out, uint64_t capacity);
 
@@ -422,6 +474,11 @@ void bb200_amcl_force_update(bb200_amcl* a);
 /* Amcl::update(control_action, measurement) -- amcl_core.hpp:165-201.  `points_xy` is the
  * measurement_type std::vector<std::pair<double,double>> flattened (x0, y0, x1, y1, ...). */
 int bb200_amcl_update(bb200_amcl* a, const double control_pose[4], const double* points_xy, uint64_t n_points, bb200_update_result* out);
+/* Amcl::update(control, detections) (amcl_core.hpp:165-200) with a landmark or bearing sensor model: the same step as
+ * bb200_amcl_update, with the map's model weighing the detections.  BB200_ERR_STATE on a grid map, on a filter joined
+ * to shards, and for bb200_amcl_update on a landmark map. */
+int bb200_amcl_update_landmarks(bb200_amcl* a, const double control_pose[4], const bb200_landmark_detection* detections, uint64_t n,
+                                bb200_update_result* out);
 /* Scan preprocessing in front of the path (SURVEY 8f): what beluga_ros does between the sensor message
  * and Amcl::update -- beluga_ros::LaserScan (beluga_ros/include/beluga_ros/laser_scan.hpp:69-80:
  * take_evenly(max_beams) over ranges and angles, angle = float(angle_min + float(i) * angle_increment)),

@@ -219,6 +219,9 @@ class Amcl {
       check(bb200_amcl_update_begin(handle_, control_action.data(), &view));
       if (view.updated) token.weigh(view.stream, view.states, view.n, view.factors);
       check(bb200_amcl_update_end(handle_, &r));
+    } else if constexpr (is_landmark_token_v<std::decay_t<decltype(token)>>) {
+      check(bb200_amcl_update_landmarks(handle_, control_action.data(), token.detections.empty() ? nullptr : token.detections.data(),
+                                        token.detections.size(), &r));
     } else {
       static_assert(sizeof(std::pair<double, double>) == 2 * sizeof(double), "measurement points must be packed");
       check(bb200_amcl_update(handle_, control_action.data(), token.points.empty() ? nullptr : &token.points.front().first, token.points.size(), &r));

@@ -6,6 +6,8 @@
 //   beluga::LikelihoodFieldModel<Grid>    (beluga/sensor/likelihood_field_model.hpp:41-92)
 //   beluga::LikelihoodFieldProbModel<Grid>(beluga/sensor/likelihood_field_prob_model.hpp:41-92)
 //   beluga::BeamSensorModel<Grid>         (beluga/sensor/beam_model.hpp:73-163)
+//   beluga::LandmarkSensorModel2d<LandmarkMap>, beluga::BearingSensorModel2d<LandmarkMap>
+//                                         (beluga/sensor/landmark_sensor_model.hpp, bearing_sensor_model.hpp)
 // keeps compiling when the namespace is switched to beluga_b200.  The reference models return
 // per-particle callables (state sampling / weighting functions); here `operator()` returns a small
 // token that beluga_b200::Amcl hands to the device kernels -- the per-particle loop lives on the GPU.
@@ -426,6 +428,162 @@ class BeamSensorModel {
   param_type params_;
   GridSnapshot grid_;
   unsigned map_version_{0};
+};
+
+
+// ---- landmark and bearing models ----------------------------------------------------------------------------------------
+
+/// A position in 3-D: beluga's LandmarkPosition3 / LandmarkBearing3 (types/landmark_detection_types.hpp:33-34).
+using LandmarkPosition3 = std::array<double, 3>;
+
+/// types/landmark_detection_types.hpp:39-42: a detection's position in the robot frame and its category.
+struct LandmarkPositionDetection {
+  LandmarkPosition3 detection_position_in_robot{};
+  std::uint32_t category{0};
+};
+
+/// types/landmark_detection_types.hpp:45-48: a detection's bearing vector in the sensor frame and its category.
+struct LandmarkBearingDetection {
+  LandmarkPosition3 detection_bearing_in_sensor{};
+  std::uint32_t category{0};
+};
+
+/// The axis-aligned bounds of a LandmarkMap (LandmarkMapBoundaries, types/landmark_detection_types.hpp:36).
+struct LandmarkMapBoundaries {
+  LandmarkPosition3 min{}, max{};
+};
+
+/// beluga::LandmarkMap (sensor/data/landmark_map.hpp:40-166): the landmarks, in the world frame, with explicit bounds
+/// or, without them, the landmarks' own (:61-71, computed by the library).  The library keeps a copy on the device.
+class LandmarkMap {
+ public:
+  using landmarks_set_position_data = std::vector<LandmarkPositionDetection>;
+  explicit LandmarkMap(const LandmarkMapBoundaries& boundaries, landmarks_set_position_data landmarks)
+      : landmarks_(std::move(landmarks)), boundaries_(boundaries), explicit_bounds_(true) {}
+  explicit LandmarkMap(landmarks_set_position_data landmarks) : landmarks_(std::move(landmarks)) {}
+
+  /// The C view of this map; valid while the map lives and is not modified.
+  [[nodiscard]] bb200_landmark_map view() const {
+    c_.resize(landmarks_.size());
+    for (std::size_t k = 0; k < landmarks_.size(); ++k) {
+      const auto& p = landmarks_[k].detection_position_in_robot;
+      c_[k] = bb200_landmark{p[0], p[1], p[2], landmarks_[k].category};
+    }
+    return bb200_landmark_map{c_.empty() ? nullptr : c_.data(), c_.size(), explicit_bounds_ ? boundaries_.min.data() : nullptr,
+                              explicit_bounds_ ? boundaries_.max.data() : nullptr};
+  }
+
+ private:
+  landmarks_set_position_data landmarks_;
+  LandmarkMapBoundaries boundaries_{};
+  bool explicit_bounds_{false};
+  mutable std::vector<bb200_landmark> c_;
+};
+
+/// A pose in 3-D as the C ABI takes it: a row-major 3x4 [R | t].  With BELUGA_B200_WITH_SOPHUS it converts from
+/// Sophus::SE3d (SE3d::matrix3x4()).
+struct SE3d {
+  std::array<double, 12> m{1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0};
+  SE3d() = default;
+  explicit SE3d(const std::array<double, 12>& matrix3x4) : m(matrix3x4) {}
+#ifdef BELUGA_B200_WITH_SOPHUS
+  SE3d(const Sophus::SE3d& p) {  // NOLINT(google-explicit-constructor)
+    const auto r = p.matrix3x4();
+    for (int row = 0; row < 3; ++row)
+      for (int col = 0; col < 4; ++col) m[4 * row + col] = r(row, col);
+  }
+#endif
+};
+
+/// Same members and defaults as beluga::LandmarkModelParam (sensor/landmark_sensor_model.hpp:44-48).
+struct LandmarkModelParam {
+  double sigma_range{1.0};
+  double sigma_bearing{1.0};
+  double random_prob{1e-4};
+};
+
+/// Same members and defaults as beluga::BearingModelParam (sensor/bearing_sensor_model.hpp:42-45).
+struct BearingModelParam {
+  double sigma_bearing{1.0};
+  SE3d sensor_pose_in_robot{};
+};
+
+/// Measurement token of the landmark and bearing models: the detections as the C ABI takes them.
+struct landmark_token {
+  std::vector<bb200_landmark_detection> detections;
+};
+
+template <class T, class = void>
+struct is_landmark_token : std::false_type {};
+template <class T>
+struct is_landmark_token<T, std::void_t<decltype(std::declval<const T&>().detections)>> : std::true_type {};
+template <class T>
+constexpr bool is_landmark_token_v = is_landmark_token<T>::value;
+
+/// beluga::LandmarkSensorModel2d<LandmarkMap> (sensor/landmark_sensor_model.hpp:63-172): range and bearing to the nearest
+/// landmark of each detection's category.
+template <class LandmarkMapT = LandmarkMap>
+class LandmarkSensorModel2d {
+ public:
+  using state_type = SE2d;
+  using weight_type = double;
+  using measurement_type = std::vector<LandmarkPositionDetection>;
+  using map_type = LandmarkMapT;
+  using param_type = LandmarkModelParam;
+
+  explicit LandmarkSensorModel2d(const param_type& params, map_type map) : params_{params}, map_{std::move(map)} {}
+  void update_map(const map_type& map) { map_ = map; }
+  [[nodiscard]] landmark_token operator()(measurement_type&& detections) const {
+    landmark_token t;
+    for (const auto& d : detections) {
+      const auto& p = d.detection_position_in_robot;
+      t.detections.push_back(bb200_landmark_detection{p[0], p[1], p[2], d.category});
+    }
+    return t;
+  }
+  [[nodiscard]] int attach(bb200_filter* f) const {
+    const bb200_landmark_param p{params_.sigma_range, params_.sigma_bearing, params_.random_prob};
+    const bb200_landmark_map m = map_.view();
+    return bb200_filter_set_landmark_map(f, &p, &m);
+  }
+
+ private:
+  param_type params_;
+  map_type map_;
+};
+
+/// beluga::BearingSensorModel2d<LandmarkMap> (sensor/bearing_sensor_model.hpp:59-156): bearing alone, from a sensor at
+/// params.sensor_pose_in_robot, to the best-aligned landmark of each detection's category.
+template <class LandmarkMapT = LandmarkMap>
+class BearingSensorModel2d {
+ public:
+  using state_type = SE2d;
+  using weight_type = double;
+  using measurement_type = std::vector<LandmarkBearingDetection>;
+  using map_type = LandmarkMapT;
+  using param_type = BearingModelParam;
+
+  explicit BearingSensorModel2d(const param_type& params, map_type map) : params_{params}, map_{std::move(map)} {}
+  void update_map(const map_type& map) { map_ = map; }
+  [[nodiscard]] landmark_token operator()(measurement_type&& detections) const {
+    landmark_token t;
+    for (const auto& d : detections) {
+      const auto& b = d.detection_bearing_in_sensor;
+      t.detections.push_back(bb200_landmark_detection{b[0], b[1], b[2], d.category});
+    }
+    return t;
+  }
+  [[nodiscard]] int attach(bb200_filter* f) const {
+    bb200_bearing_param p{};
+    p.sigma_bearing = params_.sigma_bearing;
+    for (int k = 0; k < 12; ++k) p.sensor_pose_in_robot[k] = params_.sensor_pose_in_robot.m[k];
+    const bb200_landmark_map m = map_.view();
+    return bb200_filter_set_bearing_map(f, &p, &m);
+  }
+
+ private:
+  param_type params_;
+  map_type map_;
 };
 
 }  // namespace beluga_b200

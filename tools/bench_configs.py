@@ -23,6 +23,8 @@ and 4 shards of one device, next to the single filter (a filter of one shard doe
 `sharded-weighed`: a 1M-particle step at 1080 beams on the 2000^2 map through the built-in likelihood-field update against the
 same step weighed by the caller (update_weighted, one torch kernel per shard), on one filter and on 2 and 4 shards of device 0
 (and over devices 0..1 and 0..3 where there are that many).
+`landmark`: the landmark and bearing models at 1M particles x 16 detections on a fiducial-like and a reflector-like map, with
+the reweight kernel's share of the FP64 bound and the Python oracle beside them.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import ctypes
@@ -715,6 +717,71 @@ def run_batch_beam():
     return res
 
 
+def run_landmark():
+    """The landmark and bearing models at 1M particles x 16 detections, on (a) 64 landmarks in 64 categories (fiducial-like:
+    one candidate per detection) and (b) 1000 landmarks in one category (reflector-like: every detection scans all 1000).
+    Amcl.update_landmarks with systematic resampling every step: the host clock around each step (it ends synchronised),
+    median of `steps` after `warmup`, with the device timers on for the reweight kernel's time.  The kernel's operation count
+    is computed from the shapes: per candidate, the FP64 add, subtract and multiply instructions of the search key (8 for the
+    landmark model; 28 for the bearing model, plus its sqrt and three divisions, which are counted once each), over the H100
+    SXM's 34 TFLOP/s FP64 rate (an FMA counts two flops there, and the library does not contract, so 17e12 instructions/s).
+    Beside it the Python oracle (tests/_landmark_oracle.py, one thread) on 20 particles, scaled to 1M (extrapolated)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import _landmark_oracle as lo  # noqa: E402
+
+    res = {}
+    device = device_record()
+    rng = np.random.default_rng(9)
+    n, nd, steps, warmup = 1 << 20, 16, 10, 2
+    sensor_pose = (0.0, 0.0, 1.0, 0.2, -1.0, 0.0, 0.0, 0.0, 0.0, -1.0, 0.0, 0.5)
+    for map_name, n_lm, n_cat in (("64_in_64_categories", 64, 64), ("1000_in_1_category", 1000, 1)):
+        pos = np.stack([rng.uniform(-20, 20, n_lm), rng.uniform(-20, 20, n_lm), rng.uniform(0, 2, n_lm)], axis=1)
+        cat = (np.arange(n_lm) % n_cat).astype(np.uint32)
+        det_pos = np.stack([rng.uniform(-5, 5, nd), rng.uniform(-5, 5, nd), rng.uniform(0, 2, nd)], axis=1)
+        det_cat = rng.integers(0, n_cat, nd).astype(np.uint32)
+        candidates = sum(int((cat == c).sum()) for c in det_cat)
+        for model in ("landmark", "bearing"):
+            a = bb.Amcl(bb.DifferentialDriveModelParam(*MOTION), bb.AmclParams(update_min_d=0.0, update_min_a=0.0, min_particles=n, max_particles=n,
+                                                                               resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=1))
+            lmap = bb.LandmarkMap(pos, cat)
+            if model == "landmark":
+                a.update_map(bb.SENSOR_LANDMARK, bb.LandmarkModelParam(0.5, 0.3, 1e-3), lmap)
+            else:
+                a.update_map(bb.SENSOR_BEARING, bb.BearingModelParam(0.3, sensor_pose), lmap)
+            a.initialize([0.0, 0.0, 0.0], np.diag([25.0, 25.0, 1.0]))
+            a.filter.set_timing(True)
+            wall, kernels = [], {}
+            for k in range(warmup + steps):
+                a.filter.clear_timings()
+                t0 = time.perf_counter()
+                r = a.update_landmarks([np.cos(0.01 * k), np.sin(0.01 * k), 0.05 * k, 0.0], det_pos, det_cat)
+                dt = time.perf_counter() - t0
+                assert r.updated == 1
+                if k >= warmup:
+                    wall.append(dt * 1e3)
+                    for name, ms in a.filter.last_timings():
+                        kernels[name] = kernels.get(name, 0.0) + ms / steps
+            kernel_ms = kernels.get("reweight_landmark", float("nan"))
+            ops = n * candidates * (8 if model == "landmark" else 32)
+            states = a.particles()[0][:20]
+            dets = [(*p, int(c)) for p, c in zip(det_pos.tolist(), det_cat.tolist())]
+            omap = lo.LandmarkMap([(*p, int(c)) for p, c in zip(pos.tolist(), cat.tolist())])
+            t0 = time.perf_counter()
+            for s in states.tolist():
+                if model == "landmark":
+                    lo.landmark_weight(s, dets, omap, 0.5, 0.3, 1e-3)
+                else:
+                    lo.bearing_weight(s, dets, omap, 0.3, sensor_pose)
+            cpu_ms = (time.perf_counter() - t0) * 1e3 * n / len(states)
+            res[f"landmark_{model}_1M_x_16_{map_name}"] = {
+                "ms_per_step_e2e": float(np.median(wall)), "ms_per_step_min_max": [float(min(wall)), float(max(wall))],
+                "reweight_kernel_ms": kernel_ms, "candidates_per_particle": candidates, "fp64_instructions": ops,
+                "fp64_bound_ms": ops / 17e12 * 1e3, "share_of_fp64_bound": ops / 17e12 * 1e3 / kernel_ms,
+                "cpu_oracle_ms_one_thread_extrapolated": cpu_ms, "kernels_ms": {k: round(v, 4) for k, v in kernels.items()}, "device": device}
+            a.close()
+    return res
+
+
 def batch_reweight_ms(batch, poses, scans, steps):
     """Mean device time per step of the batch's reweight kernels (names containing batch_reweight or batch_beam), from
     torch.profiler in a run of its own; poses[t] and scans[t] are step t's inputs of every member."""
@@ -1197,6 +1264,8 @@ def main():
         out.update(run_sharded_publish())
     if "sharded-weighed" in which:
         out.update(run_sharded_weighed())
+    if "landmark" in which:
+        out.update(run_landmark())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}

@@ -188,6 +188,19 @@ Amcl::Amcl(const bb200_amcl_param& p, const bb200_motion_param& motion)
   if (sharded() && p.min_particles < p.max_particles && filter_.ok()) (void)filter_.link().enable_kld();
 }
 
+int Amcl::validate(const bb200_amcl_param& p, const bb200_motion_param& motion, std::string* error) {
+  auto reject = [&](const char* m) {
+    if (error != nullptr) *error = m;
+    return static_cast<int>(BB200_ERR_INVALID_ARGUMENT);
+  };
+  if (motion.model < BB200_MOTION_DIFFERENTIAL || motion.model > BB200_MOTION_STATIONARY) return reject("unknown motion model");
+  if (p.shard_capacity != 0 && p.shard_first_index + p.shard_capacity > p.max_particles) return reject("a shard must lie inside [0, max_particles)");
+  if (p.max_particles == 0 || p.min_particles > p.max_particles) return reject("need 0 < min_particles <= max_particles");
+  if (!(p.alpha_slow >= 0.0) || !(p.alpha_slow <= p.alpha_fast))  // thrun_recovery_probability_estimator.hpp:49-50
+    return reject("need 0 <= alpha_slow <= alpha_fast");
+  return BB200_OK;
+}
+
 int Amcl::initialized(int status, bool has_particles) {
   if (status == BB200_OK) {
     policy_.force_update();  // amcl_core.hpp:136, beluga_ros/include/beluga_ros/amcl.hpp:193-199

@@ -60,6 +60,9 @@ class Amcl {
  public:
   Amcl(const bb200_amcl_param& p, const bb200_motion_param& motion);
 
+  /// The configurations a filter rejects, checked without touching a device (BB200_OK or BB200_ERR_INVALID_ARGUMENT).
+  static int validate(const bb200_amcl_param& p, const bb200_motion_param& motion, std::string* error);
+
   Filter& filter() { return filter_; }
   bool ok() const { return filter_.ok(); }
   int create_status() const { return filter_.create_status(); }

@@ -6,7 +6,6 @@
 #include <memory>
 #include <new>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "../../include/beluga_b200.h"
@@ -15,11 +14,13 @@
 #include "cluster_host.hpp"
 #include "filter.hpp"
 #include "measurement_host.hpp"
+#include "sharded_amcl.hpp"
 #include "state_blob.hpp"
 
 using bb200::Amcl;
 using bb200::Batch;
 using bb200::Filter;
+using bb200::ShardedAmcl;
 
 struct bb200_filter {
   Filter impl;
@@ -28,8 +29,7 @@ struct bb200_filter {
 
 struct bb200_amcl {
   Amcl impl;
-  bb200_filter* filter_view;  // non-owning alias handed out by bb200_amcl_filter
-  bb200_amcl(const bb200_amcl_param& p, const bb200_motion_param& m) : impl(p, m), filter_view(nullptr) {}
+  bb200_amcl(const bb200_amcl_param& p, const bb200_motion_param& m) : impl(p, m) {}
 };
 
 struct bb200_amcl_batch {
@@ -37,29 +37,18 @@ struct bb200_amcl_batch {
   bb200_amcl_batch(const bb200_amcl_param* p, const bb200_motion_param* m, int n, uint32_t flags) : impl(p, m, n, flags) {}
 };
 
-/// One filter over several shards driven by ONE host thread (the shape of beluga_ros's single-process node).
 struct bb200_sharded_amcl {
-  std::vector<bb200_amcl*> ranks;
-  mutable std::string error;
-  void record_error(const std::string& m) const { error = m; }
-  /// Whether a weighed step is open: bb200_sharded_amcl_update_begin opens it on every shard at once.
-  bool step_open() const { return !ranks.empty() && ranks[0]->impl.filter().weigh_open(); }
-  std::vector<Amcl*> impls() const {
-    std::vector<Amcl*> out;
-    for (bb200_amcl* a : ranks) out.push_back(&a->impl);
-    return out;
-  }
-  ~bb200_sharded_amcl() {
-    for (bb200_amcl* a : ranks) delete a;
-  }
+  ShardedAmcl impl;
+  bb200_sharded_amcl(const bb200_amcl_param& p, const bb200_motion_param& m, int n, const int* devices) : impl(p, m, n, devices) {}
 };
 
 namespace {
 thread_local std::string g_create_error;
 
-// bb200_filter is layout-compatible with its only member, so the Amcl-owned Filter can be viewed
-// through the same handle type without a second allocation.
+// bb200_filter and bb200_amcl are layout-compatible with their only member, so the Amcl-owned Filter and the
+// ShardedAmcl-owned shards can be viewed through the same handle types without a second allocation.
 static_assert(sizeof(bb200_filter) == sizeof(Filter), "bb200_filter must wrap Filter exactly");
+static_assert(sizeof(bb200_amcl) == sizeof(Amcl), "bb200_amcl must wrap Amcl exactly");
 
 // Nothing throws across the C boundary: the host side allocates (std::vector, std::string, unordered_map), so every
 // entry point runs its body under this guard and turns an exception into a status + last_error message.
@@ -114,19 +103,27 @@ void cloud_to_points(const bb200_point_cloud& c, double* points_xy) {
   }
 }
 
-/// Prepares the map's tables once and uploads them to every shard.  A failed preparation is reported by the first shard, as
-/// its own set_*_map call would.
-template <class Prepare>
-int set_sharded_map(bb200_sharded_amcl* g, Prepare&& prepare) {
-  g->error.clear();
-  return guarded(*g, [&] {
-    bb200::MapTables tables;
-    std::string message;
-    int st = prepare(&tables, &message);
-    if (st != BB200_OK) return g->ranks[0]->impl.filter().fail_with(st, message);
-    for (auto a = g->ranks.begin(); st == BB200_OK && a != g->ranks.end(); ++a) st = (*a)->impl.filter().set_map(tables);
+const char* const kCloudRefused = "point cloud: datatype must be 7 (FLOAT32) or 8 (FLOAT64), x, y and z must fit in point_step, data must be set";
+/// update(points_xy, n_points) on the base-frame points of a laser scan (bb200_scan_to_points): the standalone and the
+/// sharded filter convert alike.
+template <class Update>
+int with_scan_points(const bb200_laser_scan& scan, Update&& update) {
+  std::vector<double> points(2 * (scan.n_ranges + 1), 0.0);
+  uint64_t n = 0;
+  const int st = bb200_scan_to_points(&scan, points.data(), scan.n_ranges + 1, &n);
+  return st != BB200_OK ? st : update(points.data(), n);
+}
+/// ... and on those of a point cloud (bb200_point_cloud_to_points); a refused cloud is reported to `context`.
+template <class Context, class Update>
+int with_cloud_points(Context& context, const bb200_point_cloud& cloud, Update&& update) {
+  std::vector<double> points(2 * cloud.n_points, 0.0);
+  uint64_t n = 0;
+  const int st = bb200_point_cloud_to_points(&cloud, points.data(), cloud.n_points, &n);
+  if (st != BB200_OK) {
+    context.record_error(kCloudRefused);
     return st;
-  });
+  }
+  return update(points.data(), n);
 }
 
 int create_batch(const bb200_amcl_param* params, const bb200_motion_param* motions, int n_members, uint32_t flags, bb200_amcl_batch** out) {
@@ -201,20 +198,17 @@ const char* bb200_last_error(const bb200_filter* f) { return f != nullptr ? f->i
       return BB200_ERR_STATE;                                                                               \
     }                                                                                                       \
   } while (0)
-#define BB_REFUSE_OPEN_SHARDED(g)                                                                                \
-  do {                                                                                                           \
-    if ((g) != nullptr && (g)->step_open()) {                                                                    \
-      (g)->record_error("a weighed step is open: only bb200_sharded_amcl_update_end and destroy are accepted"); \
-      return BB200_ERR_STATE;                                                                                    \
-    }                                                                                                            \
+#define BB_REFUSE_OPEN_STEP(handle, message)                   \
+  do {                                                         \
+    if ((handle) != nullptr && (handle)->impl.step_open()) {   \
+      (handle)->impl.record_error(message);                    \
+      return BB200_ERR_STATE;                                  \
+    }                                                          \
   } while (0)
-#define BB_REFUSE_OPEN_BATCH(batch)                                                                              \
-  do {                                                                                                           \
-    if ((batch) != nullptr && (batch)->impl.step_open()) {                                                       \
-      (batch)->impl.record_error("a weighed step is open: only bb200_amcl_batch_update_end and destroy are accepted"); \
-      return BB200_ERR_STATE;                                                                                    \
-    }                                                                                                            \
-  } while (0)
+namespace {
+const char* const kShardedStepOpen = "a weighed step is open: only bb200_sharded_amcl_update_end and destroy are accepted";
+const char* const kBatchStepOpen = "a weighed step is open: only bb200_amcl_batch_update_end and destroy are accepted";
+}  // namespace
 
 int bb200_filter_set_likelihood_field_map(bb200_filter* f, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid, int prob) {
   BB_REQUIRE(f && p && grid);
@@ -543,22 +537,7 @@ int bb200_amcl_create_with_motion(const bb200_amcl_param* p, const bb200_motion_
     return BB200_ERR_INVALID_ARGUMENT;
   }
   *out = nullptr;
-  if (motion->model < BB200_MOTION_DIFFERENTIAL || motion->model > BB200_MOTION_STATIONARY) {
-    g_create_error = "unknown motion model";
-    return BB200_ERR_INVALID_ARGUMENT;
-  }
-  if (p->shard_capacity != 0 && p->shard_first_index + p->shard_capacity > p->max_particles) {
-    g_create_error = "a shard must lie inside [0, max_particles)";
-    return BB200_ERR_INVALID_ARGUMENT;
-  }
-  if (p->max_particles == 0 || p->min_particles > p->max_particles) {
-    g_create_error = "need 0 < min_particles <= max_particles";
-    return BB200_ERR_INVALID_ARGUMENT;
-  }
-  if (!(p->alpha_slow >= 0.0) || !(p->alpha_slow <= p->alpha_fast)) {  // thrun_recovery_probability_estimator.hpp:49-50
-    g_create_error = "need 0 <= alpha_slow <= alpha_fast";
-    return BB200_ERR_INVALID_ARGUMENT;
-  }
+  if (const int st = Amcl::validate(*p, *motion, &g_create_error)) return st;
   return guarded_create([&] {
     bb200_amcl* a = new bb200_amcl(*p, *motion);
     if (!a->impl.ok()) {
@@ -567,7 +546,6 @@ int bb200_amcl_create_with_motion(const bb200_amcl_param* p, const bb200_motion_
       delete a;
       return st;
     }
-    a->filter_view = reinterpret_cast<bb200_filter*>(&a->impl.filter());
     *out = a;
     return static_cast<int>(BB200_OK);
   });
@@ -583,7 +561,7 @@ int bb200_amcl_create(const bb200_amcl_param* p, const bb200_diff_drive_param* m
 }
 void bb200_amcl_destroy(bb200_amcl* a) { delete a; }
 const char* bb200_amcl_last_error(const bb200_amcl* a) { return a != nullptr ? a->impl.last_error() : "null amcl"; }
-bb200_filter* bb200_amcl_filter(bb200_amcl* a) { return a != nullptr ? a->filter_view : nullptr; }
+bb200_filter* bb200_amcl_filter(bb200_amcl* a) { return a != nullptr ? reinterpret_cast<bb200_filter*>(&a->impl.filter()) : nullptr; }
 int bb200_amcl_initialize(bb200_amcl* a, const double mean_xytheta[3], const double cov[9]) {
   BB_REQUIRE(a && mean_xytheta && cov);
   BB_REFUSE_OPEN(a->impl.filter());
@@ -667,30 +645,11 @@ int bb200_scan_to_points(const bb200_laser_scan* scan, double* points_xy, uint64
   return BB200_OK;
 }
 
-namespace {
-/// The base-frame points an update takes from a laser scan (bb200_scan_to_points): the standalone and the sharded filter
-/// convert alike.
-int scan_points(const bb200_laser_scan& scan, std::vector<double>* points, uint64_t* n) {
-  points->assign(2 * (scan.n_ranges + 1), 0.0);
-  return bb200_scan_to_points(&scan, points->data(), scan.n_ranges + 1, n);
-}
-/// ... and from a point cloud (bb200_point_cloud_to_points).
-int cloud_points(const bb200_point_cloud& cloud, std::vector<double>* points, uint64_t* n) {
-  points->assign(2 * cloud.n_points, 0.0);
-  return bb200_point_cloud_to_points(&cloud, points->data(), cloud.n_points, n);
-}
-const char* const kCloudRefused = "point cloud: datatype must be 7 (FLOAT32) or 8 (FLOAT64), x, y and z must fit in point_step, data must be set";
-}  // namespace
-
 int bb200_amcl_update_scan(bb200_amcl* a, const double control_pose[4], const bb200_laser_scan* scan, bb200_update_result* out) {
   BB_REQUIRE(a && control_pose && scan && out);
   BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] {
-    std::vector<double> points;
-    uint64_t n = 0;
-    const int st = scan_points(*scan, &points, &n);
-    if (st != BB200_OK) return st;
-    return bb200_amcl_update(a, control_pose, points.data(), n, out);
+    return with_scan_points(*scan, [&](const double* points, uint64_t n) { return bb200_amcl_update(a, control_pose, points, n, out); });
   });
 }
 
@@ -730,14 +689,7 @@ int bb200_amcl_update_point_cloud(bb200_amcl* a, const double control_pose[4], c
   BB_REQUIRE(a && control_pose && cloud && out);
   BB_REFUSE_OPEN(a->impl.filter());
   return guarded(a->impl, [&] {
-    std::vector<double> points;
-    uint64_t n = 0;
-    const int st = cloud_points(*cloud, &points, &n);
-    if (st != BB200_OK) {
-      a->impl.record_error(kCloudRefused);
-      return st;
-    }
-    return bb200_amcl_update(a, control_pose, points.data(), n, out);
+    return with_cloud_points(a->impl, *cloud, [&](const double* points, uint64_t n) { return bb200_amcl_update(a, control_pose, points, n, out); });
   });
 }
 
@@ -768,377 +720,120 @@ int bb200_sharded_amcl_create(const bb200_amcl_param* p, const bb200_motion_para
     return BB200_ERR_INVALID_ARGUMENT;
   }
   *out = nullptr;
-  if (n_shards < 1 || n_shards > bb200::kMaxShards || p->max_particles == 0 || p->max_particles % static_cast<uint64_t>(n_shards) != 0) {
-    g_create_error = "a filter splits into 1..8 equal shards: max_particles must be a multiple of n_shards";
-    return BB200_ERR_INVALID_ARGUMENT;
-  }
+  if (const int st = ShardedAmcl::validate(*p, *motion, n_shards, &g_create_error)) return st;  // before any device is touched
   return guarded_create([&] {
-    auto group = std::make_unique<bb200_sharded_amcl>();
-    const uint64_t shard = p->max_particles / static_cast<uint64_t>(n_shards);
-    std::vector<bb200::Filter*> filters;
-    std::vector<bb200::ShardLink*> links;
-    for (int r = 0; r < n_shards; ++r) {
-      bb200_amcl_param q = *p;
-      q.device = devices[r];
-      q.shard_capacity = shard;
-      q.shard_first_index = static_cast<uint64_t>(r) * shard;
-      bb200_amcl* a = nullptr;
-      const int st = bb200_amcl_create_with_motion(&q, motion, &a);
-      if (st != BB200_OK) return st;
-      group->ranks.push_back(a);
-      filters.push_back(&a->impl.filter());
-      links.push_back(&a->impl.filter().link());
+    auto g = std::make_unique<bb200_sharded_amcl>(*p, *motion, n_shards, devices);
+    if (!g->impl.ok()) {
+      g_create_error = g->impl.last_error();
+      return g->impl.create_status();
     }
-    const int st = bb200::ShardLink::join_local(links.data(), n_shards);
-    if (st != BB200_OK) {
-      g_create_error = "joining the shards failed (peer access between the devices?)";
-      for (bb200::Filter* f : filters)
-        if (f->last_error()[0] != '\0') g_create_error = f->last_error();
-      return st;
-    }
-    *out = group.release();
+    *out = g.release();
     return static_cast<int>(BB200_OK);
   });
 }
 void bb200_sharded_amcl_destroy(bb200_sharded_amcl* g) { delete g; }
-const char* bb200_sharded_amcl_last_error(const bb200_sharded_amcl* g) {
-  if (g == nullptr) return "null sharded amcl";
-  if (!g->error.empty()) return g->error.c_str();
-  for (const bb200_amcl* a : g->ranks)
-    if (a->impl.last_error()[0] != '\0') return a->impl.last_error();
-  return "";
-}
-int bb200_sharded_amcl_shards(const bb200_sharded_amcl* g) { return g != nullptr ? static_cast<int>(g->ranks.size()) : 0; }
+const char* bb200_sharded_amcl_last_error(const bb200_sharded_amcl* g) { return g != nullptr ? g->impl.last_error() : "null sharded amcl"; }
+int bb200_sharded_amcl_shards(const bb200_sharded_amcl* g) { return g != nullptr ? g->impl.shards() : 0; }
 bb200_amcl* bb200_sharded_amcl_shard(bb200_sharded_amcl* g, int rank) {
-  return (g != nullptr && rank >= 0 && rank < static_cast<int>(g->ranks.size())) ? g->ranks[static_cast<size_t>(rank)] : nullptr;
+  return g != nullptr ? reinterpret_cast<bb200_amcl*>(g->impl.shard(rank)) : nullptr;
 }
-#define BB_EACH_SHARD(call)                                   \
-  BB_REQUIRE(g);                                              \
-  g->error.clear();                                           \
-  return guarded(*g, [&] {                                    \
-    for (bb200_amcl* a : g->ranks) {                          \
-      const int st = (call);                                  \
-      if (st != BB200_OK) return st;                          \
-    }                                                         \
-    return static_cast<int>(BB200_OK);                        \
-  })
 
 int bb200_sharded_amcl_set_likelihood_field_map(bb200_sharded_amcl* g, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid, int prob) {
   BB_REQUIRE(g && p && grid);
-  BB_REFUSE_OPEN_SHARDED(g);
-  return set_sharded_map(g, [&](bb200::MapTables* t, std::string* e) { return bb200::prepare_likelihood_field_map(*p, *grid, prob != 0, t, e); });
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  return guarded(g->impl, [&] {
+    return g->impl.set_map([&](bb200::MapTables* t, std::string* e) { return bb200::prepare_likelihood_field_map(*p, *grid, prob != 0, t, e); });
+  });
 }
 int bb200_sharded_amcl_set_beam_map(bb200_sharded_amcl* g, const bb200_beam_param* p, const bb200_occupancy_grid* grid) {
   BB_REQUIRE(g && p && grid);
-  BB_REFUSE_OPEN_SHARDED(g);
-  return set_sharded_map(g, [&](bb200::MapTables* t, std::string* e) { return bb200::prepare_beam_map(*p, *grid, t, e); });
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  return guarded(g->impl, [&] { return g->impl.set_map([&](bb200::MapTables* t, std::string* e) { return bb200::prepare_beam_map(*p, *grid, t, e); }); });
 }
 int bb200_sharded_amcl_initialize(bb200_sharded_amcl* g, const double mean_xytheta[3], const double cov[9]) {
   BB_REQUIRE(mean_xytheta && cov);
-  BB_REFUSE_OPEN_SHARDED(g);
-  BB_EACH_SHARD(a->impl.initialize(mean_xytheta, cov));
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  BB_REQUIRE(g);
+  return guarded(g->impl, [&] { return g->impl.initialize(mean_xytheta, cov); });
 }
 int bb200_sharded_amcl_initialize_from_map(bb200_sharded_amcl* g) {
-  BB_REFUSE_OPEN_SHARDED(g);
-  BB_EACH_SHARD(a->impl.initialize_from_map());
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  BB_REQUIRE(g);
+  return guarded(g->impl, [&] { return g->impl.initialize_from_map(); });
 }
-#undef BB_EACH_SHARD
 void bb200_sharded_amcl_force_update(bb200_sharded_amcl* g) {
-  if (g != nullptr && !g->step_open())
-    for (bb200_amcl* a : g->ranks) a->impl.force_update();
+  if (g != nullptr && !g->impl.step_open()) g->impl.force_update();
 }
 int bb200_sharded_amcl_update(bb200_sharded_amcl* g, const double control_pose[4], const double* points_xy, uint64_t n_points, bb200_update_result* out) {
   BB_REQUIRE(g && control_pose && out && (points_xy || n_points == 0));
-  BB_REFUSE_OPEN_SHARDED(g);
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
   static const double kNoPoints[2] = {0.0, 0.0};
-  g->error.clear();
-  return guarded(*g, [&] {
-    const std::vector<Amcl*> ranks = g->impls();
-    return Amcl::update_group(ranks.data(), static_cast<int>(ranks.size()), control_pose, points_xy != nullptr ? points_xy : kNoPoints, n_points, out);
-  });
+  return guarded(g->impl, [&] { return g->impl.update(control_pose, points_xy != nullptr ? points_xy : kNoPoints, n_points, out); });
 }
 int bb200_sharded_amcl_update_begin(bb200_sharded_amcl* g, const double control_pose[4], bb200_weigh_view* views) {
   BB_REQUIRE(g && control_pose && views);
-  g->error.clear();
-  return guarded(*g, [&] {
-    const std::vector<Amcl*> ranks = g->impls();
-    return Amcl::update_group_begin(ranks.data(), static_cast<int>(ranks.size()), control_pose, views);
-  });
+  return guarded(g->impl, [&] { return g->impl.update_begin(control_pose, views); });
 }
 int bb200_sharded_amcl_update_end(bb200_sharded_amcl* g, bb200_update_result* out) {
   BB_REQUIRE(g && out);
-  g->error.clear();
-  return guarded(*g, [&] {
-    const std::vector<Amcl*> ranks = g->impls();
-    return Amcl::update_group_end(ranks.data(), static_cast<int>(ranks.size()), out);
-  });
+  return guarded(g->impl, [&] { return g->impl.update_end(out); });
 }
 int bb200_cluster_merge_host(const bb200_cluster_cell* const* shard_cells, const uint64_t* shard_counts, const uint64_t* shard_first_index, int shards,
                              bb200_cluster_cell* merged, uint64_t capacity, uint64_t* n_merged) {
   BB_REQUIRE(shard_cells && shard_counts && n_merged && shards >= 1);
-  return guarded_create([&] {
-    // The reference's cluster map is filled by ONE pass over the particles in order (cluster_based_estimation.hpp:141-161).
-    // Shards hold contiguous index ranges, so going through the shards in rank order -- and through each shard's cells in
-    // ITS first-occurrence order -- visits the cells in the global first-occurrence order; a cell met again adds its count,
-    // weight and raw moments to the record opened by the lower rank (whose representative is the globally first particle).
-    std::unordered_map<uint64_t, uint64_t> slot_of;
-    uint64_t listed = 0;
-    for (int r = 0; r < shards; ++r) listed += shard_counts[r];
-    slot_of.reserve(listed);  // no rehash while the map grows to the merged count
-    uint64_t n = 0;
-    for (int r = 0; r < shards; ++r) {
-      for (uint64_t k = 0; k < shard_counts[r]; ++k) {
-        const bb200_cluster_cell& c = shard_cells[r][k];
-        const auto it = slot_of.find(c.hash);
-        if (it == slot_of.end()) {
-          if (merged != nullptr) {
-            if (n >= capacity) return static_cast<int>(BB200_ERR_CAPACITY);
-            merged[n] = c;
-            merged[n].first_index = static_cast<uint32_t>(c.first_index + (shard_first_index != nullptr ? shard_first_index[r] : 0));
-          }
-          slot_of.emplace(c.hash, n++);
-        } else if (merged != nullptr) {
-          bb200_cluster_cell& m = merged[it->second];
-          m.count += c.count;
-          m.weight += c.weight;
-          for (int j = 0; j < 9; ++j) m.moments[j] += c.moments[j];
-        }
-      }
-    }
-    *n_merged = n;
-    return static_cast<int>(BB200_OK);
-  });
+  return guarded_create([&] { return bb200::merge_cells(shard_cells, shard_counts, shard_first_index, shards, merged, capacity, n_merged); });
 }
-
-namespace {
-/// Every shard's cell records (Filter::cell_records, one device pass per shard) merged in rank order
-/// (bb200_cluster_merge_host): the cells of the whole particle set in its global first-occurrence order.  BB200_ERR_STATE
-/// when no shard holds a particle.
-int merged_cells(bb200_sharded_amcl* g, double linear_resolution, double angular_resolution, std::vector<bb200_cluster_cell>* merged,
-                 uint64_t* n_particles) {
-  static_assert(sizeof(bb200_cluster_cell) == sizeof(bb200::HostCell), "public and internal cell records must agree");
-  const int shards = static_cast<int>(g->ranks.size());
-  std::vector<std::vector<bb200::HostCell>> cells(static_cast<size_t>(shards));
-  std::vector<const bb200_cluster_cell*> ptrs;
-  std::vector<uint64_t> counts, firsts;
-  uint64_t total_cells = 0;
-  *n_particles = 0;
-  for (int r = 0; r < shards; ++r) {
-    Filter& f = g->ranks[static_cast<size_t>(r)]->impl.filter();
-    std::vector<bb200::HostCell>& c = cells[static_cast<size_t>(r)];
-    if (f.size() > 0)
-      if (const int st = f.cell_records(linear_resolution, angular_resolution, &c)) return st;
-    const uint64_t n = c.size();
-    ptrs.push_back(reinterpret_cast<const bb200_cluster_cell*>(c.data()));
-    counts.push_back(n);
-    firsts.push_back(f.first_index());
-    total_cells += n;
-    *n_particles += f.size();
-  }
-  if (*n_particles == 0) {
-    g->error = "no particles";
-    return static_cast<int>(BB200_ERR_STATE);
-  }
-  merged->resize(total_cells);
-  uint64_t n_merged = 0;
-  const int st = bb200_cluster_merge_host(ptrs.data(), counts.data(), firsts.data(), shards, merged->data(), merged->size(), &n_merged);
-  if (st != BB200_OK) return st;
-  merged->resize(n_merged);
-  return static_cast<int>(BB200_OK);
-}
-}  // namespace
 
 int bb200_sharded_amcl_cluster_estimate(bb200_sharded_amcl* g, const bb200_cluster_param* p, bb200_estimate* out, uint32_t* n_cells,
                                         uint32_t* n_clusters) {
   BB_REQUIRE(g && p && out);
-  BB_REFUSE_OPEN_SHARDED(g);
-  g->error.clear();
-  return guarded(*g, [&] {
-    std::vector<bb200_cluster_cell> merged;
-    uint64_t n_particles = 0;
-    const int st = merged_cells(g, p->linear_hash_resolution, p->angular_hash_resolution, &merged, &n_particles);
-    if (st != BB200_OK) return st;
-    static_assert(sizeof(bb200_cluster_cell) == sizeof(bb200::HostCell), "public and internal cell records must agree");
-    const bb200::ClusterSelection sel = bb200::select_cluster(reinterpret_cast<const bb200::HostCell*>(merged.data()), merged.size(), n_particles,
-                                                              p->linear_hash_resolution, p->angular_hash_resolution, p->weight_cap_percentile);
-    bb200::estimate_from_moments(sel.moments, g->ranks[0]->impl.filter().pivot(), out);  // every shard accumulates about the same pivot
-    if (n_cells != nullptr) *n_cells = static_cast<uint32_t>(merged.size());
-    if (n_clusters != nullptr) *n_clusters = sel.clusters;
-    return static_cast<int>(BB200_OK);
-  });
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  return guarded(g->impl, [&] { return g->impl.cluster_estimate(*p, out, n_cells, n_clusters); });
 }
 
 int bb200_sharded_amcl_get_particles(bb200_sharded_amcl* g, double* states, double* weights, uint64_t capacity) {
   BB_REQUIRE(g);
-  BB_REFUSE_OPEN_SHARDED(g);
-  g->error.clear();
-  return guarded(*g, [&] {
-    uint64_t done = 0;
-    for (bb200_amcl* a : g->ranks) {  // rank order is global particle order
-      Filter& f = a->impl.filter();
-      const uint64_t n = std::min<uint64_t>(f.size(), capacity - done);
-      const int st = f.get_particles(states != nullptr ? states + 4 * done : nullptr, weights != nullptr ? weights + done : nullptr, n);
-      if (st != BB200_OK) return st;
-      done += n;
-      if (done >= capacity) break;
-    }
-    return static_cast<int>(BB200_OK);
-  });
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  return guarded(g->impl, [&] { return g->impl.get_particles(states, weights, capacity); });
 }
 
 int bb200_sharded_amcl_update_scan(bb200_sharded_amcl* g, const double control_pose[4], const bb200_laser_scan* scan, bb200_update_result* out) {
   BB_REQUIRE(g && control_pose && scan && out);
-  BB_REFUSE_OPEN_SHARDED(g);
-  g->error.clear();
-  return guarded(*g, [&] {
-    std::vector<double> points;
-    uint64_t n = 0;
-    const int st = scan_points(*scan, &points, &n);
-    if (st != BB200_OK) return st;
-    return bb200_sharded_amcl_update(g, control_pose, points.data(), n, out);
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  g->impl.record_error("");  // a refused measurement leaves no earlier message behind
+  return guarded(g->impl, [&] {
+    return with_scan_points(*scan, [&](const double* points, uint64_t n) { return bb200_sharded_amcl_update(g, control_pose, points, n, out); });
   });
 }
 
 int bb200_sharded_amcl_update_point_cloud(bb200_sharded_amcl* g, const double control_pose[4], const bb200_point_cloud* cloud,
                                           bb200_update_result* out) {
   BB_REQUIRE(g && control_pose && cloud && out);
-  BB_REFUSE_OPEN_SHARDED(g);
-  g->error.clear();
-  return guarded(*g, [&] {
-    std::vector<double> points;
-    uint64_t n = 0;
-    const int st = cloud_points(*cloud, &points, &n);
-    if (st != BB200_OK) {
-      g->error = kCloudRefused;
-      return st;
-    }
-    return bb200_sharded_amcl_update(g, control_pose, points.data(), n, out);
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  g->impl.record_error("");  // a refused measurement leaves no earlier message behind
+  return guarded(g->impl, [&] {
+    return with_cloud_points(g->impl, *cloud, [&](const double* points, uint64_t n) { return bb200_sharded_amcl_update(g, control_pose, points, n, out); });
   });
 }
 
 int bb200_sharded_amcl_particle_histogram(bb200_sharded_amcl* g, double linear_resolution, double angular_resolution, bb200_cluster_cell* bins,
                                           uint64_t capacity, uint64_t* n_bins, double* max_bin_weight) {
   BB_REQUIRE(g);
-  BB_REFUSE_OPEN_SHARDED(g);
-  g->error.clear();
-  return guarded(*g, [&] {
-    std::vector<bb200_cluster_cell> merged;
-    uint64_t n_particles = 0;
-    const int st = merged_cells(g, linear_resolution, angular_resolution, &merged, &n_particles);
-    if (st != BB200_OK) return st;
-    if (n_bins != nullptr) *n_bins = merged.size();
-    double top = 1e-3;  // beluga_ros/particle_cloud.hpp:197
-    for (const bb200_cluster_cell& c : merged) top = c.weight > top ? c.weight : top;
-    if (max_bin_weight != nullptr) *max_bin_weight = top;
-    if (bins != nullptr) {
-      if (capacity < merged.size()) {
-        g->error = "histogram bin buffer too small (n_bins has the count)";
-        return static_cast<int>(BB200_ERR_CAPACITY);
-      }
-      std::copy(merged.begin(), merged.end(), bins);
-    }
-    return static_cast<int>(BB200_OK);
-  });
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  return guarded(g->impl, [&] { return g->impl.particle_histogram(linear_resolution, angular_resolution, bins, capacity, n_bins, max_bin_weight); });
 }
 
 int bb200_sharded_amcl_sample_states(bb200_sharded_amcl* g, uint64_t count, uint32_t step, double* states_out) {
   BB_REQUIRE(g);
-  BB_REFUSE_OPEN_SHARDED(g);
-  g->error.clear();
-  return guarded(*g, [&] {
-    const size_t shards = g->ranks.size();
-    std::vector<Filter*> f(shards);
-    uint64_t n_particles = 0;
-    for (size_t r = 0; r < shards; ++r) {
-      f[r] = &g->ranks[r]->impl.filter();
-      n_particles += f[r]->size();
-    }
-    const uint64_t max_particles = g->ranks[0]->impl.params().max_particles;
-    if (n_particles == 0) {
-      g->error = "no particles";
-      return static_cast<int>(BB200_ERR_STATE);
-    }
-    if (count > max_particles) {
-      g->error = "more samples than the filter capacity";
-      return static_cast<int>(BB200_ERR_CAPACITY);
-    }
-    if (count > 0 && states_out == nullptr) {
-      g->error = "states_out is null";
-      return static_cast<int>(BB200_ERR_INVALID_ARGUMENT);
-    }
-    if (count == 0) return static_cast<int>(BB200_OK);
-    // The global CDF: the one the last step left when it kept its particles, or one built as a sharded step builds it --
-    // the exponent from the largest weight of all shards, the offsets from the shards' fixed-point totals in rank order.
-    // Current CDFs quantised with different exponents were built shard by shard (e.g. bb200_filter_build_cdf on one shard):
-    // together they are no global CDF.  With one exponent on every shard they are the global build's bit for bit, since
-    // the global largest weight is some shard's largest weight.
-    std::vector<uint64_t> totals(shards, 0);
-    bool current = true, first = true;
-    int exponent = 0;
-    for (size_t r = 0; r < shards; ++r) {
-      if (f[r]->size() == 0) continue;
-      int e = 0;
-      if (const int st = f[r]->current_cdf(&totals[r], &e)) return st;
-      current = current && totals[r] != 0 && (first || e == exponent);
-      exponent = e;
-      first = false;
-    }
-    if (!current) {
-      double wmax = 0.0;
-      for (size_t r = 0; r < shards; ++r) {
-        if (f[r]->size() == 0) continue;
-        double w = 0.0;
-        if (const int st = f[r]->max_weight(&w)) return st;
-        wmax = w > wmax ? w : wmax;
-      }
-      for (size_t r = 0; r < shards; ++r)
-        if (f[r]->size() > 0)
-          if (const int st = f[r]->build_cdf(wmax, &totals[r], nullptr)) return st;
-    }
-    uint64_t total = 0;
-    std::vector<uint64_t> offsets(shards, 0);
-    for (size_t r = 0; r < shards; ++r) {
-      offsets[r] = total;
-      total += totals[r];
-    }
-    for (size_t r = 0; r < shards; ++r)
-      if (const int st = f[r]->sample_range(count, step, total, offsets[r])) return st;
-    for (Filter* s : f)  // every shard's draws have reached their slots' staging buffers
-      if (const int st = s->synchronize()) return st;
-    const uint64_t shard = max_particles / shards;  // slot j lies in the staging buffer of shard j / shard
-    for (size_t r = 0; r < shards && r * shard < count; ++r)
-      if (const int st = f[r]->staging_states(states_out + 4 * r * shard, std::min<uint64_t>(shard, count - r * shard))) return st;
-    return static_cast<int>(BB200_OK);
-  });
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  return guarded(g->impl, [&] { return g->impl.sample_states(count, step, states_out); });
 }
 
 int bb200_sharded_amcl_cast_rays(bb200_sharded_amcl* g, const double* poses, uint64_t n_poses, const double* bearings_cs, uint64_t n_bearings,
                                  double max_range, double* ranges) {
   BB_REQUIRE(g);
-  BB_REFUSE_OPEN_SHARDED(g);
-  g->error.clear();
-  return guarded(*g, [&] {
-    uint64_t n_rays = 0;
-    if (const int st = g->ranks[0]->impl.filter().check_cast_rays(poses, n_poses, bearings_cs, n_bearings, ranges, &n_rays)) return st;
-    if (n_rays == 0) return static_cast<int>(BB200_OK);
-    // The poses are cut into contiguous ranges, one per shard, each cast on that shard's copy of the map; every shard
-    // launches before any reads back, so shards on different devices cast at the same time.
-    std::vector<Filter*> casters;
-    for (bb200_amcl* a : g->ranks) casters.push_back(&a->impl.filter());
-    const uint64_t k = casters.size();
-    auto first_pose = [&](uint64_t c) { return n_poses * c / k; };  // n_poses <= kMaxCastRays: no overflow
-    for (uint64_t c = 0; c < k; ++c) {
-      const uint64_t begin = first_pose(c), end = first_pose(c + 1);
-      if (end > begin)
-        if (const int st = casters[c]->enqueue_cast_rays(poses + 4 * begin, end - begin, bearings_cs, n_bearings, max_range)) return st;
-    }
-    for (uint64_t c = 0; c < k; ++c) {
-      const uint64_t begin = first_pose(c), end = first_pose(c + 1);
-      if (end > begin)
-        if (const int st = casters[c]->finish_cast_rays(ranges + begin * n_bearings, (end - begin) * n_bearings)) return st;
-    }
-    return static_cast<int>(BB200_OK);
-  });
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  return guarded(g->impl, [&] { return g->impl.cast_rays(poses, n_poses, bearings_cs, n_bearings, max_range, ranges); });
 }
 
 // ---- batches ------------------------------------------------------------------------------------------
@@ -1154,7 +849,7 @@ int bb200_amcl_batch_create_with_flags(const bb200_amcl_param* params, const bb2
   return create_batch(params, motions, n_members, flags, out);
 }
 int bb200_amcl_batch_member_size(const bb200_amcl_batch* b, int member, uint64_t* n) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && n);
   return guarded(b->impl, [&] { return b->impl.member_size(member, n); });
 }
@@ -1163,114 +858,114 @@ const char* bb200_amcl_batch_last_error(const bb200_amcl_batch* b) { return b !=
 int bb200_amcl_batch_members(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.members() : 0; }
 int bb200_amcl_batch_set_likelihood_field_map(bb200_amcl_batch* b, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid,
                                               int prob) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && p && grid);
   return guarded(b->impl, [&] { return b->impl.set_likelihood_field_map(*p, *grid, prob != 0); });
 }
 int bb200_amcl_batch_set_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p, const bb200_occupancy_grid* grid) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && p && grid);
   return guarded(b->impl, [&] { return b->impl.set_beam_map(*p, *grid); });
 }
 int bb200_amcl_batch_add_likelihood_field_map(bb200_amcl_batch* b, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid,
                                               int prob, int* map_id) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && p && grid && map_id);
   return guarded(b->impl, [&] { return b->impl.add_likelihood_field_map(*p, *grid, prob != 0, map_id); });
 }
 int bb200_amcl_batch_add_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p, const bb200_occupancy_grid* grid, int* map_id) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && p && grid && map_id);
   return guarded(b->impl, [&] { return b->impl.add_beam_map(*p, *grid, map_id); });
 }
 int bb200_amcl_batch_update_map(bb200_amcl_batch* b, int member, int map_id) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.update_map(member, map_id); });
 }
 int bb200_amcl_batch_member_map(const bb200_amcl_batch* b, int member, int* map_id) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && map_id);
   return guarded(b->impl, [&] { return b->impl.member_map(member, map_id); });
 }
 int bb200_amcl_batch_remove_map(bb200_amcl_batch* b, int map_id) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.remove_map(map_id); });
 }
 int bb200_amcl_batch_get_likelihood_field(const bb200_amcl_batch* b, int map_id, float* out, uint64_t capacity) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && out);
   return guarded(b->impl, [&] { return b->impl.get_likelihood_field(map_id, out, capacity); });
 }
 int bb200_amcl_batch_initialize(bb200_amcl_batch* b, int member, const double mean_xytheta[3], const double cov[9]) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && mean_xytheta && cov);
   return guarded(b->impl, [&] { return b->impl.initialize(member, mean_xytheta, cov); });
 }
 int bb200_amcl_batch_initialize_from_map(bb200_amcl_batch* b, int member) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.initialize_from_map(member); });
 }
 int bb200_amcl_batch_initialize_states(bb200_amcl_batch* b, int member, const double* states, const double* weights, uint64_t n) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.initialize_states(member, states, weights, n); });
 }
 int bb200_amcl_batch_force_update(bb200_amcl_batch* b, int member) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b);
   return b->impl.force_update(member);
 }
 int bb200_amcl_batch_get_particles(bb200_amcl_batch* b, int member, double* states, double* weights, uint64_t capacity) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.get_particles(member, states, weights, capacity); });
 }
 int bb200_amcl_batch_ancestors(bb200_amcl_batch* b, int member, int64_t* out, uint64_t capacity) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && (out || capacity == 0));
   return guarded(b->impl, [&] { return b->impl.ancestors(member, out, capacity); });
 }
 int bb200_amcl_batch_cluster_estimate(bb200_amcl_batch* b, int member, const bb200_cluster_param* p, bb200_estimate* out) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && p && out);
   return guarded(b->impl, [&] { return b->impl.cluster_estimate(member, *p, out); });
 }
 int bb200_amcl_batch_cluster_estimates(bb200_amcl_batch* b, const bb200_cluster_param* p, const uint8_t* present, bb200_estimate* out,
                                        uint32_t* n_cells, uint32_t* n_clusters) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && p && out);
   return guarded(b->impl, [&] { return b->impl.cluster_estimates(*p, present, out, n_cells, n_clusters); });
 }
 int bb200_amcl_batch_particle_histograms(bb200_amcl_batch* b, double linear_resolution, double angular_resolution, const uint8_t* present,
                                          bb200_cluster_cell* const* bins, const uint64_t* capacity, uint64_t* n_bins, double* max_bin_weight) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.particle_histograms(linear_resolution, angular_resolution, present, bins, capacity, n_bins, max_bin_weight); });
 }
 int bb200_amcl_batch_sample_states(bb200_amcl_batch* b, const uint64_t* counts, uint32_t step, const uint8_t* present, double* const* states_out) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && counts && states_out);
   return guarded(b->impl, [&] { return b->impl.sample_states(counts, step, present, states_out); });
 }
 int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, const double* const* points_xy, const uint64_t* n_points,
                             const uint8_t* present, bb200_update_result* out) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && control_poses && points_xy && n_points && out);
   return guarded(b->impl, [&] { return b->impl.update(control_poses, points_xy, n_points, present, out); });
 }
 int bb200_amcl_batch_update_measurements(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements,
                                          const uint8_t* present, bb200_update_result* out) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && control_poses && measurements && out);
   return guarded(b->impl, [&] { return b->impl.update_measurements(control_poses, measurements, present, out); });
 }
 int bb200_amcl_batch_update_clustered(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements,
                                       const uint8_t* present, const bb200_cluster_param* p, bb200_update_result* out, bb200_estimate* clustered,
                                       uint32_t* n_cells, uint32_t* n_clusters) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && control_poses && measurements && p && out && clustered);
   return guarded(b->impl, [&] { return b->impl.update_clustered(control_poses, measurements, present, *p, out, clustered, n_cells, n_clusters); });
 }
@@ -1286,39 +981,39 @@ int bb200_amcl_batch_update_end(bb200_amcl_batch* b, const bb200_cluster_param* 
 }
 int bb200_amcl_batch_cast_rays(bb200_amcl_batch* b, const uint8_t* present, const int* map_ids, const double* const* poses, const uint64_t* n_poses,
                                const double* const* bearings_cs, const uint64_t* n_bearings, const double* max_range, double* const* ranges) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && poses && n_poses && bearings_cs && n_bearings && max_range && ranges);
   return guarded(b->impl, [&] { return b->impl.cast_rays(present, map_ids, poses, n_poses, bearings_cs, n_bearings, max_range, ranges); });
 }
 uint64_t bb200_amcl_batch_launch_count(const bb200_amcl_batch* b) { return b != nullptr ? b->impl.launch_count() : 0; }
 int bb200_amcl_batch_add_member(bb200_amcl_batch* b, const bb200_amcl_param* params, const bb200_motion_param* motion, int* member) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && params && motion && member);
   return guarded(b->impl, [&] { return b->impl.add_member(*params, *motion, member); });
 }
 int bb200_amcl_batch_remove_member(bb200_amcl_batch* b, int member) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b);
   return guarded(b->impl, [&] { return b->impl.remove_member(member); });
 }
 int bb200_amcl_batch_member_active(const bb200_amcl_batch* b, int member, int* active) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && active);
   return guarded(b->impl, [&] { return b->impl.member_active(member, active); });
 }
 
 int bb200_amcl_batch_export_members(bb200_amcl_batch* b, const uint8_t* present, void* const* out, const uint64_t* capacity, uint64_t* size) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && size);
   return guarded(b->impl, [&] { return b->impl.export_members(present, out, capacity, size); });
 }
 int bb200_amcl_batch_export_member(bb200_amcl_batch* b, int member, void* out, uint64_t capacity, uint64_t* size) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && size);
   return guarded(b->impl, [&] { return b->impl.export_member(member, out, capacity, size); });
 }
 int bb200_amcl_batch_import_member(bb200_amcl_batch* b, const void* blob, uint64_t size, int map_id, int* member) {
-  BB_REFUSE_OPEN_BATCH(b);
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b && blob && member);
   return guarded(b->impl, [&] { return b->impl.import_member(blob, size, map_id, member); });
 }

@@ -123,6 +123,40 @@ ClusterSelection select_cluster(const HostCell* cells, std::size_t n_cells, std:
   return out;
 }
 
+int merge_cells(const bb200_cluster_cell* const* shard_cells, const uint64_t* shard_counts, const uint64_t* shard_first_index, int shards,
+                bb200_cluster_cell* merged, uint64_t capacity, uint64_t* n_merged) {
+  // The reference's cluster map is filled by ONE pass over the particles in order (cluster_based_estimation.hpp:141-161).
+  // Shards hold contiguous index ranges, so going through the shards in rank order -- and through each shard's cells in
+  // ITS first-occurrence order -- visits the cells in the global first-occurrence order; a cell met again adds its count,
+  // weight and raw moments to the record opened by the lower rank (whose representative is the globally first particle).
+  std::unordered_map<uint64_t, uint64_t> slot_of;
+  uint64_t listed = 0;
+  for (int r = 0; r < shards; ++r) listed += shard_counts[r];
+  slot_of.reserve(listed);  // no rehash while the map grows to the merged count
+  uint64_t n = 0;
+  for (int r = 0; r < shards; ++r) {
+    for (uint64_t k = 0; k < shard_counts[r]; ++k) {
+      const bb200_cluster_cell& c = shard_cells[r][k];
+      const auto it = slot_of.find(c.hash);
+      if (it == slot_of.end()) {
+        if (merged != nullptr) {
+          if (n >= capacity) return static_cast<int>(BB200_ERR_CAPACITY);
+          merged[n] = c;
+          merged[n].first_index = static_cast<uint32_t>(c.first_index + (shard_first_index != nullptr ? shard_first_index[r] : 0));
+        }
+        slot_of.emplace(c.hash, n++);
+      } else if (merged != nullptr) {
+        bb200_cluster_cell& m = merged[it->second];
+        m.count += c.count;
+        m.weight += c.weight;
+        for (int j = 0; j < 9; ++j) m.moments[j] += c.moments[j];
+      }
+    }
+  }
+  *n_merged = n;
+  return static_cast<int>(BB200_OK);
+}
+
 const RehashTable& rehash_table() {
   static const RehashTable table = [] {
     RehashTable t;

@@ -49,6 +49,11 @@ const RehashTable& rehash_table();
 /// Bytes of scratch a member of at most `capacity` particles needs for its selection (select_layout at its largest).
 uint64_t select_scratch_bytes(uint64_t capacity);
 
+/// bb200_cluster_merge_host (beluga_b200.h): per-shard cell records, shards in rank order, merged into the cells of the whole
+/// particle set in its global first-occurrence order.  merged == nullptr: *n_merged receives the count only.
+int merge_cells(const bb200_cluster_cell* const* shard_cells, const uint64_t* shard_counts, const uint64_t* shard_first_index, int shards,
+                bb200_cluster_cell* merged, uint64_t capacity, uint64_t* n_merged);
+
 /// Mean and covariance (estimation.hpp:436-475) from the nine raw moments about `pivot` (layout of kMomentCount in
 /// kernels.cuh): what every estimate ends with, of the whole set or of the selected cluster.
 void estimate_from_moments(const double m[9], const double pivot[2], bb200_estimate* out);

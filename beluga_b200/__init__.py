@@ -35,7 +35,7 @@ __all__ = [
     "Filter", "LikelihoodFieldModelParam", "motion_sampling", "scan_to_points", "scan_bearings", "point_cloud_to_points",
     "take_evenly_indices",
     "OccupancyGrid", "BelugaB200Error", "device_count", "se2", "LaserScan", "PointCloud",
-    "LandmarkModelParam", "BearingModelParam", "LandmarkMap", "RESAMPLE_MULTINOMIAL", "RESAMPLE_SYSTEMATIC", "SENSOR_BEAM", "SENSOR_BEARING", "SENSOR_LANDMARK", "SENSOR_LIKELIHOOD_FIELD", "SENSOR_LIKELIHOOD_FIELD_PROB",
+    "LandmarkModelParam", "BearingModelParam", "LandmarkMap", "Detections", "RESAMPLE_MULTINOMIAL", "RESAMPLE_SYSTEMATIC", "SENSOR_BEAM", "SENSOR_BEARING", "SENSOR_LANDMARK", "SENSOR_LIKELIHOOD_FIELD", "SENSOR_LIKELIHOOD_FIELD_PROB",
 ]
 
 
@@ -247,6 +247,15 @@ def _measurement(m):
         return _capi.Measurement(_capi.MEASUREMENT_CLOUD, None, 0, None, C.pointer(cloud)), (cloud, keep)
     pts = _f64(m).reshape(-1, 2)
     return _capi.Measurement(_capi.MEASUREMENT_POINTS, _dptr(pts) if len(pts) else None, len(pts), None, None), pts
+
+
+@dataclass
+class Detections:
+    """One member's landmark detections in AmclBatch.update_measurements, update_clustered and update_weighted, as
+    Amcl.update_landmarks takes them: (n, 3) positions in the robot frame (SENSOR_LANDMARK) or bearings in the sensor frame
+    (SENSOR_BEARING), and n categories."""
+    positions: object
+    categories: object
 
 
 def _dptr(a: np.ndarray):
@@ -1054,7 +1063,7 @@ _CELL_DTYPE = np.dtype([("rep", "<f8", 4), ("hash", "<u8"), ("first", "<u4"), ("
 
 class AmclBatch:
     """bb200_amcl_batch: K independent beluga::Amcl filters on one GPU, each reading one of the batch's maps -- a
-    likelihood field or a beam-model map, one for every member (set_*_map) or several (add_*_map and update_map, which
+    likelihood field, a beam-model map or a landmark map, one for every member (set_*_map) or several (add_*_map and update_map, which
     moves a member to another map as a node's Amcl::update_map does); update() steps every member with a new scan with a fixed
     number of kernel launches and one synchronisation.  Member m's results and particles equal those of a standalone Amcl
     built from params[m] and motions[m] and fed the same inputs.
@@ -1208,6 +1217,56 @@ class AmclBatch:
         i = C.c_int(-1)
         self._check(self._lib.bb200_amcl_batch_add_beam_map(self._h, C.byref(p), C.byref(g), C.byref(i)))
         return i.value
+
+    def set_landmark_map(self, params: LandmarkModelParam, landmark_map: LandmarkMap):
+        """The landmark model (LandmarkSensorModel2d) on `landmark_map` for every member; replaces every earlier map."""
+        p, m = params.c(), landmark_map.c()
+        self._check(self._lib.bb200_amcl_batch_set_landmark_map(self._h, C.byref(p), C.byref(m)))
+        self._field_shapes = {}
+
+    def set_bearing_map(self, params: BearingModelParam, landmark_map: LandmarkMap):
+        """The bearing model (BearingSensorModel2d) on `landmark_map` for every member; replaces every earlier map."""
+        p, m = params.c(), landmark_map.c()
+        self._check(self._lib.bb200_amcl_batch_set_bearing_map(self._h, C.byref(p), C.byref(m)))
+        self._field_shapes = {}
+
+    def add_landmark_map(self, params: LandmarkModelParam, landmark_map: LandmarkMap) -> int:
+        """Adds a landmark-model map that no member reads yet; returns its id."""
+        p, m = params.c(), landmark_map.c()
+        i = C.c_int(-1)
+        self._check(self._lib.bb200_amcl_batch_add_landmark_map(self._h, C.byref(p), C.byref(m), C.byref(i)))
+        return i.value
+
+    def add_bearing_map(self, params: BearingModelParam, landmark_map: LandmarkMap) -> int:
+        """Adds a bearing-model map that no member reads yet; returns its id."""
+        p, m = params.c(), landmark_map.c()
+        i = C.c_int(-1)
+        self._check(self._lib.bb200_amcl_batch_add_bearing_map(self._h, C.byref(p), C.byref(m), C.byref(i)))
+        return i.value
+
+    def _built(self, measurements, present, weighed: bool = False):
+        """The bb200_measurement table of a step (a None entry: weighed by the caller when `weighed`, no points otherwise),
+        with every selected Detections member's detections staged first, and the objects that must outlive the call."""
+        k = len(self.params)
+        if len(measurements) != k:
+            raise ValueError("one measurement per member")
+        staged = {m for m in range(k) if isinstance(measurements[m], Detections) and not self._skipped(present, m)}
+        if staged:
+            arrays = [_landmark_array(measurements[m].positions, measurements[m].categories) if m in staged else (None, 0) for m in range(k)]
+            ptrs = (C.POINTER(_capi.Landmark) * k)(*[a if n else None for a, n in arrays])
+            counts = (C.c_uint64 * k)(*[n for _, n in arrays])
+            mask = (C.c_uint8 * k)(*[1 if m in staged else 0 for m in range(k)])
+            self._check(self._lib.bb200_amcl_batch_set_detections(self._h, ptrs, counts, mask))
+
+        def one(m):
+            if isinstance(m, Detections):
+                return _capi.Measurement(kind=_capi.MEASUREMENT_LANDMARKS), None
+            if m is None and weighed:
+                return _capi.Measurement(kind=_capi.MEASUREMENT_WEIGHTS), None
+            return _measurement(() if m is None else m)
+
+        built = [one(m) for m in measurements]
+        return (_capi.Measurement * k)(*[b[0] for b in built]), built
 
     def update_map(self, member: int, map_id: int):
         """Amcl::update_map for one member: it keeps its particles and policies and reads `map_id` from its next step."""
@@ -1371,16 +1430,14 @@ class AmclBatch:
         return list(res)
 
     def update_measurements(self, control_poses, measurements, present=None) -> list:
-        """update() with each member's measurement as base-frame points ((n, 2) array), a LaserScan or a PointCloud, as
-        Amcl.update, Amcl.update_scan and Amcl.update_point_cloud take them; scans and clouds are converted on the device.
-        Results are bit-identical to those of update() given scan_to_points / point_cloud_to_points of the same messages."""
+        """update() with each member's measurement as base-frame points ((n, 2) array), a LaserScan, a PointCloud or, for a
+        member on a landmark map, Detections, as Amcl.update, Amcl.update_scan, Amcl.update_point_cloud and
+        Amcl.update_landmarks take them; scans and clouds are converted on the device.  Results are bit-identical to those
+        of update() given scan_to_points / point_cloud_to_points of the same messages."""
         k = len(self.params)
-        if len(measurements) != k:
-            raise ValueError("one measurement per member")
         mask = self._mask(present)
+        table, built = self._built(measurements, present)
         poses = _f64(control_poses).reshape(k, 4)
-        built = [_measurement(() if m is None else m) for m in measurements]
-        table = (_capi.Measurement * k)(*[b[0] for b in built])
         res = (_capi.UpdateResult * k)()
         self._check(self._lib.bb200_amcl_batch_update_measurements(self._h, _dptr(poses), table, mask, res))
         return list(res)
@@ -1393,12 +1450,9 @@ class AmclBatch:
         with_counts, (mean, cov, n_cells, n_clusters) -- or None for a member that did not update.  The estimates equal
         cluster_estimates(present=updated members) called right after update_measurements, byte for byte."""
         k = len(self.params)
-        if len(measurements) != k:
-            raise ValueError("one measurement per member")
         mask = self._mask(present)
+        table, built = self._built(measurements, present)
         poses = _f64(control_poses).reshape(k, 4)
-        built = [_measurement(() if m is None else m) for m in measurements]
-        table = (_capi.Measurement * k)(*[b[0] for b in built])
         p = _capi.ClusterParam(linear, angular, percentile)
         res = (_capi.UpdateResult * k)()
         est = (_capi.Estimate * k)()
@@ -1415,7 +1469,7 @@ class AmclBatch:
 
     def update_weighted(self, control_poses, measurements, weigh, present=None, cluster=None):
         """update_measurements with members weighed by the caller's own sensor model (bb200_amcl_batch_update_begin / _end):
-        a None measurement marks a weighed member; the others pass points, a LaserScan or a PointCloud as in
+        a None measurement marks a weighed member; the others pass points, a LaserScan, a PointCloud or Detections as in
         update_measurements.  `weigh(members, states, factors)` is called once, with the indices of the weighed members that
         update in this step and, per member, torch CUDA tensors over its views without a copy: its propagated states,
         (n, 4) float64, and its factors, (n,) float64, which it fills with L(states[i]).  It runs inside
@@ -1424,12 +1478,9 @@ class AmclBatch:
         (linear, angular, percentile) for the cluster estimates of update_clustered; the return value is then (results,
         estimates) as update_clustered returns it, otherwise the results."""
         k = len(self.params)
-        if len(measurements) != k:
-            raise ValueError("one measurement per member")
         mask = self._mask(present)
+        table, built = self._built(measurements, present, weighed=True)
         poses = _f64(control_poses).reshape(k, 4)
-        built = [(_capi.Measurement(kind=_capi.MEASUREMENT_WEIGHTS), None) if m is None else _measurement(m) for m in measurements]
-        table = (_capi.Measurement * k)(*[b[0] for b in built])
         views = (_capi.WeighView * k)()
         self._check(self._lib.bb200_amcl_batch_update_begin(self._h, _dptr(poses), table, mask, views))
         res = (_capi.UpdateResult * k)()

@@ -128,7 +128,7 @@ class MarkerVertex(C.Structure):
     _fields_ = [("x", C.c_double), ("y", C.c_double), ("z", C.c_double), ("r", C.c_float), ("g", C.c_float), ("b", C.c_float), ("a", C.c_float)]
 
 
-MEASUREMENT_POINTS, MEASUREMENT_SCAN, MEASUREMENT_CLOUD, MEASUREMENT_WEIGHTS = 0, 1, 2, 3
+MEASUREMENT_POINTS, MEASUREMENT_SCAN, MEASUREMENT_CLOUD, MEASUREMENT_WEIGHTS, MEASUREMENT_LANDMARKS = 0, 1, 2, 3, 4
 
 
 class Measurement(C.Structure):
@@ -260,6 +260,11 @@ SIGNATURES = {
     "bb200_amcl_batch_set_beam_map": (C.c_int, [_vp, _P(BeamParam), _P(OccupancyGrid)]),
     "bb200_amcl_batch_add_likelihood_field_map": (C.c_int, [_vp, _P(LikelihoodFieldParam), _P(OccupancyGrid), C.c_int, _P(C.c_int)]),
     "bb200_amcl_batch_add_beam_map": (C.c_int, [_vp, _P(BeamParam), _P(OccupancyGrid), _P(C.c_int)]),
+    "bb200_amcl_batch_set_landmark_map": (C.c_int, [_vp, _P(LandmarkParam), _P(LandmarkMap)]),
+    "bb200_amcl_batch_set_bearing_map": (C.c_int, [_vp, _P(BearingParam), _P(LandmarkMap)]),
+    "bb200_amcl_batch_add_landmark_map": (C.c_int, [_vp, _P(LandmarkParam), _P(LandmarkMap), _P(C.c_int)]),
+    "bb200_amcl_batch_add_bearing_map": (C.c_int, [_vp, _P(BearingParam), _P(LandmarkMap), _P(C.c_int)]),
+    "bb200_amcl_batch_set_detections": (C.c_int, [_vp, _P(_P(Landmark)), _P(C.c_uint64), _P(C.c_uint8)]),
     "bb200_amcl_batch_update_map": (C.c_int, [_vp, C.c_int, C.c_int]),
     "bb200_amcl_batch_member_map": (C.c_int, [_vp, C.c_int, _P(C.c_int)]),
     "bb200_amcl_batch_remove_map": (C.c_int, [_vp, C.c_int]),

@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbeluga_b200.so")
 SOURCES = ["step.cu", "propagate.cu", "reweight_lfm.cu", "reweight_beam.cu", "reweight_landmark.cu", "raycast.cu", "cdf.cu", "kld.cu", "resample.cu", "batch_kernels.cu",
            "shard_exchange.cu", "cluster.cu", "cluster_select.cu", "device_map.cu", "filter.cu", "amcl.cu", "sharded_amcl.cu", "batch.cu", "c_api.cu", "shard_link.cpp", "map_host.cpp", "cluster_host.cpp", "state_blob.cpp"]
-HEADERS = ["kernels.cuh", "device_common.cuh", "bucket_set.cuh", "kld.cuh", "propagate.cuh", "reweight_lfm.cuh", "reweight_beam.cuh", "reweight_landmark.cuh", "raycast.cuh", "cdf.cuh", "resample.cuh",
+HEADERS = ["kernels.cuh", "device_common.cuh", "bucket_set.cuh", "kld.cuh", "propagate.cuh", "reweight_lfm.cuh", "reweight_beam.cuh", "reweight_landmark.cuh", "reweight_landmark_block.cuh", "raycast.cuh", "cdf.cuh", "resample.cuh",
            "cluster.cuh", "cluster_select.cuh", "cluster_host.hpp", "se2_math.cuh", "device_buffer.hpp", "device_map.hpp", "shard_link.hpp", "filter.hpp", "amcl.hpp", "sharded_amcl.hpp", "batch.hpp", "map_host.hpp", "measurement_host.hpp", "state_blob.hpp",
            os.path.join("..", "..", "include", "beluga_b200.h")]
 

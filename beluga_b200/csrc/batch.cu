@@ -589,6 +589,20 @@ int Batch::add_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& g
   return st != BB200_OK ? st : add_map(tables, id);
 }
 
+int Batch::set_landmark_map(const bb200_landmark_param* lp, const bb200_bearing_param* bp, const bb200_landmark_map& map) {
+  error_.clear();
+  MapTables tables;
+  const int st = prepare_landmark_map(lp, bp, map, &tables, &error_);
+  return st != BB200_OK ? st : set_map(tables);
+}
+
+int Batch::add_landmark_map(const bb200_landmark_param* lp, const bb200_bearing_param* bp, const bb200_landmark_map& map, int* id) {
+  error_.clear();
+  MapTables tables;
+  const int st = prepare_landmark_map(lp, bp, map, &tables, &error_);
+  return st != BB200_OK ? st : add_map(tables, id);
+}
+
 int Batch::set_map(const MapTables& tables) {
   // The old maps go before the new one is uploaded, so that the device never holds both; a failed upload leaves the
   // batch without a map.
@@ -671,7 +685,8 @@ int Batch::ensure_map_table() {
   for (auto& [id, e] : maps_) {
     const DeviceMap& d = e.map;
     e.slot = static_cast<int>(host.size());
-    host.push_back(BatchMap{d.field, d.occupancy, d.beam, d.free_cells, d.n_free, d.grid_width, d.grid_resolution, d.grid_origin});
+    host.push_back(BatchMap{d.field, d.occupancy, d.beam, d.free_cells, d.n_free, d.grid_width, d.grid_resolution, d.grid_origin, d.landmark,
+                            d.landmarks, d.n_landmarks, {d.box[0], d.box[1], d.box[2], d.box[3]}});
   }
   BB_CHECK(map_table_.grow(host.size()));  // every batch call ends synchronised: no step reads the old table
   // On the batch's stream, so that the step's launches follow the copy in order; the pageable source is staged before the
@@ -705,11 +720,16 @@ int Batch::initialize_from_map(int member) {
   Member& m = members_[static_cast<size_t>(member)];
   if (m.map < 0) return fail(BB200_ERR_STATE, "initialize_from_map needs a map (set_*_map or update_map first)");
   const DeviceMap& map = maps_.at(m.map).map;
-  if (map.n_free == 0) return fail(BB200_ERR_STATE, "the map has no free cell to sample from");
+  if (!map.can_draw_states())
+    return fail(BB200_ERR_STATE, map.landmark_map() ? "the landmark map's box is empty or not finite" : "the map has no free cell to sample from");
   BB_CHECK(cudaSetDevice(device_));
   m.cdf_total = 0;
-  launch_initialize_uniform(states_[m.cur].get() + m.offset, weights_.get() + m.offset, m.capacity, map.free_cells, map.n_free, map.grid_width,
-                            map.grid_resolution, map.grid_origin, m.policy.params().seed, 0, stream_);
+  if (map.landmark_map()) {
+    launch_initialize_box(states_[m.cur].get() + m.offset, weights_.get() + m.offset, m.capacity, map.box, m.policy.params().seed, 0, stream_);
+  } else {
+    launch_initialize_uniform(states_[m.cur].get() + m.offset, weights_.get() + m.offset, m.capacity, map.free_cells, map.n_free, map.grid_width,
+                              map.grid_resolution, map.grid_origin, m.policy.params().seed, 0, stream_);
+  }
   ++launches_;
   BB_CHECK(cudaGetLastError());
   BB_CHECK(cudaStreamSynchronize(stream_));
@@ -1089,6 +1109,7 @@ int Batch::cast_rays(const uint8_t* present, const int* map_ids, const double* c
     const int id = override_map ? map_ids[k] : members_[k].map;
     if (override_map && find_map(id) == nullptr) return fail(BB200_ERR_INVALID_ARGUMENT, who + error_);
     if (id < 0) return fail(BB200_ERR_STATE, who + "no map");
+    if (maps_.at(id).map.landmark_map()) return fail(BB200_ERR_STATE, who + "a landmark map has no grid to cast rays on");
     uint64_t n_rays = 0;
     if (!cast_ray_count(n_poses[k], n_bearings[k], &n_rays)) return fail(BB200_ERR_INVALID_ARGUMENT, who + "n_poses * n_bearings overflows");
     if ((poses[k] == nullptr && n_poses[k] > 0) || (bearings[k] == nullptr && n_bearings[k] > 0) || (ranges[k] == nullptr && n_rays > 0))
@@ -1162,6 +1183,33 @@ int Batch::ensure_points(uint64_t n_points) {
   return BB200_OK;
 }
 
+int Batch::ensure_detections(uint64_t n) {
+  if (n <= std::min(detections_.size(), detections_host_.size())) return BB200_OK;
+  BB_CHECK(cudaStreamSynchronize(stream_));
+  const uint64_t room = std::max<uint64_t>(n + n / 2, 256);
+  BB_CHECK(detections_.grow(n, room));
+  BB_CHECK(detections_host_.grow(n, room));
+  return BB200_OK;
+}
+
+int Batch::set_detections(const bb200_landmark_detection* const* detections, const uint64_t* n, const uint8_t* present) {
+  error_.clear();
+  if (const int st = check_present(present)) return st;
+  for (size_t k = 0; k < members_.size(); ++k) {
+    if (!selected_member(present, k)) continue;
+    const std::string who = "member " + std::to_string(k) + ": ";
+    if (n[k] > 0 && (detections == nullptr || detections[k] == nullptr)) return fail(BB200_ERR_INVALID_ARGUMENT, who + "detections is null");
+    if (n[k] >= 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, who + "too many detections");
+  }
+  for (size_t k = 0; k < members_.size(); ++k) {
+    if (!selected_member(present, k)) continue;
+    Member& m = members_[k];
+    m.detections.assign(detections != nullptr && n[k] > 0 ? detections[k] : nullptr, detections != nullptr && n[k] > 0 ? detections[k] + n[k] : nullptr);
+    m.detections_staged = true;
+  }
+  return BB200_OK;
+}
+
 bool Batch::ensure_hits(uint64_t words) {
   // Every batch call ends synchronised: nothing in flight reads the old buffer.
   // words is at most one pass's worth (the caller checks), so the slack never takes the buffer past that
@@ -1231,6 +1279,8 @@ std::string measurement_error(const bb200_measurement& in) {
       if (in.cloud == nullptr) return "cloud is null";
       return cloud_valid(*in.cloud) ? ""
                                     : "point cloud: datatype must be 7 (FLOAT32) or 8 (FLOAT64), x, y and z must fit in point_step, data must be set";
+    case BB200_MEASUREMENT_LANDMARKS:
+      return "";  // the member's staged detections (set_detections), checked against its map by the step
     default:
       return "unknown measurement kind";
   }
@@ -1238,7 +1288,7 @@ std::string measurement_error(const bb200_measurement& in) {
 
 /// The points a member's measurement can yield: the exact count for points and clouds, the kept beams for a scan.
 uint64_t measurement_bound(const bb200_measurement& in) {
-  if (in.kind == BB200_MEASUREMENT_WEIGHTS) return 0;
+  if (in.kind == BB200_MEASUREMENT_WEIGHTS || in.kind == BB200_MEASUREMENT_LANDMARKS) return 0;
   return in.kind == BB200_MEASUREMENT_SCAN ? scan_beam_count(*in.scan) : in.kind == BB200_MEASUREMENT_CLOUD ? in.cloud->n_points : in.n_points;
 }
 
@@ -1331,6 +1381,17 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
   if (views != nullptr)
     for (size_t k = 0; k < count; ++k) views[k] = bb200_weigh_view{};
   if (const int st = check_present(present)) return st;
+  // A landmark map weighs detections and a grid map points, scans or clouds, as Filter::check_measurement decides.
+  for (size_t k = 0; k < count; ++k) {
+    if (!selected_member(present, k) || in[k].kind == BB200_MEASUREMENT_WEIGHTS) continue;
+    const Member& m = members_[k];
+    const bool detections = in[k].kind == BB200_MEASUREMENT_LANDMARKS;
+    const bool landmark_map = m.map >= 0 && maps_.at(m.map).map.landmark_map();
+    const std::string who = "member " + std::to_string(k) + ": ";
+    if (detections && m.map >= 0 && !landmark_map) return fail(BB200_ERR_STATE, who + "detections need a landmark map");
+    if (!detections && landmark_map) return fail(BB200_ERR_STATE, who + "a landmark map weighs detections, not points");
+    if (detections && !m.detections_staged) return fail(BB200_ERR_STATE, who + "no detections staged (bb200_amcl_batch_set_detections)");
+  }
   std::vector<AmclPolicy> before;
   before.reserve(count);
   for (const Member& m : members_) before.push_back(m.policy);
@@ -1360,7 +1421,8 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
 
   // Points sent by the host come first in the point buffer, in member order; the points of scans and clouds, written by
   // batch_points_kernel, follow them.  Scans and clouds are sized by their bounds (measurement_bound).
-  uint64_t points_total = 0, host_points = 0, input_floats = 0;
+  uint64_t points_total = 0, host_points = 0, input_floats = 0, detections_total = 0;
+  bool landmark_maps = false;
   uint32_t max_points = 0;
   // The map every updating member with a map reads, -1 when they read several, -2 when none has one (every updating
   // member is weighed by the caller and none may inject).
@@ -1376,12 +1438,19 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
       return rollback(fail(BB200_ERR_INVALID_ARGUMENT, "points_xy is null"));
     const int id = members_[k].map;
     const bool injects = plans[k].resample && plans[k].random_state_probability > 0.0;
-    if (injects && (id < 0 || maps_.at(id).map.n_free == 0)) return rollback(fail(BB200_ERR_STATE, "recovery injection needs a map with free cells"));
+    if (injects && (id < 0 || !maps_.at(id).map.can_draw_states()))
+      return rollback(fail(BB200_ERR_STATE, id >= 0 && maps_.at(id).map.landmark_map() ? "recovery injection needs a non-empty, finite landmark box"
+                                                                                       : "recovery injection needs a map with free cells"));
     if (weighed(k)) forms[k] = kBatchWeighed;
     if (id < 0) continue;
     const DeviceMap& map = maps_.at(id).map;
     // The beam model walks a member's rays in two passes when its map allows it (the rule of the single filter).
     if (map.sensor == BB200_SENSOR_BEAM && !weighed(k)) forms[k] = beam_two_pass_map(map) ? kBatchBeamTwoPass : kBatchBeamFused;
+    if (in[k].kind == BB200_MEASUREMENT_LANDMARKS) {
+      forms[k] = kBatchLandmark;
+      detections_total += members_[k].detections.size();
+    }
+    landmark_maps = landmark_maps || map.landmark_map();
     step_map = step_map == -2 || step_map == id ? id : -1;
     points_total += bound;
     if (in[k].kind == BB200_MEASUREMENT_POINTS) host_points += bound;
@@ -1399,6 +1468,7 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
   const bool ess = std::any_of(active.begin(), active.end(), [&](uint32_t k) { return plans[k].needs_ess != 0; });
   int st = check(cudaSetDevice(device_), "cudaSetDevice");
   if (st == BB200_OK) st = ensure_points(points_total);  // the previous step has ended: the staging buffers are free
+  if (st == BB200_OK && detections_total > 0) st = ensure_detections(detections_total);
   if (st == BB200_OK && step_map == -1) st = ensure_map_table();
   if (st == BB200_OK && convert) st = ensure_inputs(input_floats);
   if (st == BB200_OK && kld) st = ensure_kld_scratch();
@@ -1411,7 +1481,8 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
   const uint32_t n_active = static_cast<uint32_t>(active.size());
   BatchStepArgs a{};
   a.n_members = n_active;
-  uint64_t point_offset = 0, device_offset = host_points, input_offset = 0, hit_words = 0;
+  uint64_t point_offset = 0, device_offset = host_points, input_offset = 0, hit_words = 0, detection_offset = 0;
+  std::vector<LandmarkDetection> prepared;
   for (uint32_t j = 0; j < n_active; ++j) {
     const uint32_t k = active[j];
     const Member& m = members_[k];
@@ -1449,6 +1520,14 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
       b.point_offset = 0;  // no points: the caller's factors stand for the sensor model
       b.n_points = 0;
       b.points_radius = 0.0;
+    } else if (meas.kind == BB200_MEASUREMENT_LANDMARKS) {
+      // No points: point_offset and n_points index the step's prepared detections instead.
+      prepare_detections(maps_.at(m.map).map.landmark_slices, m.detections.data(), m.detections.size(), &prepared);
+      if (!prepared.empty()) std::memcpy(detections_host_.get() + detection_offset, prepared.data(), prepared.size() * sizeof(LandmarkDetection));
+      b.point_offset = detection_offset;
+      b.n_points = static_cast<uint32_t>(prepared.size());
+      b.points_radius = 0.0;
+      detection_offset += prepared.size();
     } else if (meas.kind == BB200_MEASUREMENT_POINTS) {
       b.point_offset = point_offset;
       b.n_points = static_cast<uint32_t>(meas.n_points);
@@ -1538,6 +1617,15 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
     a.post_ctas[1] = totals[1];
     a.ess_ctas = totals[2];
   }
+  const bool any_landmark = std::any_of(active.begin(), active.end(), [&](uint32_t k) { return forms[k] == kBatchLandmark; });
+  if (any_landmark) {
+    uint32_t* row = first_host_.get() + static_cast<size_t>(kBatchLandmarkRow) * (n_active + 1);
+    for (uint32_t j = 0; j < n_active; ++j) {
+      row[j] = a.landmark_ctas;
+      if (forms[active[j]] == kBatchLandmark) a.landmark_ctas += batch_landmark_ctas(table_host_.get()[j]);
+    }
+    row[n_active] = a.landmark_ctas;
+  }
   if (any_weighed) {
     uint32_t* row = first_host_.get() + static_cast<size_t>(kBatchWeighRow) * (n_active + 1);
     for (uint32_t j = 0; j < n_active; ++j) {
@@ -1546,7 +1634,7 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
     }
     row[n_active] = a.weigh_ctas;
   }
-  const int rows = kld || ess || any_weighed ? kBatchRows : convert ? kBatchLaunches + 1 : kBatchLaunches;
+  const int rows = any_landmark ? kBatchRows : kld || ess || any_weighed ? kBatchLandmarkRow : convert ? kBatchLaunches + 1 : kBatchLaunches;
 
   cudaStream_t stream = stream_;
   for (const uint32_t k : active) members_[k].cdf_total = 0;  // from here on the step may have rewritten their CDFs
@@ -1560,6 +1648,9 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
   if (st == BB200_OK && convert)
     st = check(cudaMemcpyAsync(inputs_.device.get(), inputs_.host.get(), n_active * sizeof(BatchPointsMember), cudaMemcpyHostToDevice, stream),
                "upload measurement table");
+  if (st == BB200_OK && detection_offset > 0)
+    st = check(cudaMemcpyAsync(detections_.get(), detections_host_.get(), detection_offset * sizeof(LandmarkDetection), cudaMemcpyHostToDevice, stream),
+               "upload detections");
   if (st == BB200_OK && input_floats > 0)
     st = check(cudaMemcpyAsync(input_.get(), input_host_.get(), input_floats * sizeof(float), cudaMemcpyHostToDevice, stream), "upload measurements");
   if (st == BB200_OK && kld)
@@ -1596,6 +1687,10 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
     a.grid_origin = map.grid_origin;
     a.occupancy = map.occupancy;
     a.beam = map.beam;
+    a.landmark = map.landmark;
+    a.landmarks = map.landmarks;
+    a.n_landmarks = map.n_landmarks;
+    for (int c = 0; c < 4; ++c) a.box[c] = map.box[c];
   } else if (step_map == -1) {
     a.maps = map_table_.get();
   }
@@ -1611,6 +1706,8 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
   a.ticket = ticket_host_.get();
   a.seq = seq_;
   a.factors = factors_.get();
+  a.detections = detections_.get();
+  a.landmark_maps = landmark_maps ? 1 : 0;
   launches_ += static_cast<uint64_t>(launch_batch_step_head(a, stream));
   st = check(cudaGetLastError(), "batch step launch");
   if (st != BB200_OK) return rollback(st);

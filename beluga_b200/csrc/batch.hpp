@@ -1,7 +1,8 @@
 // K independent beluga::Amcl filters that share one device, stepped together: one call runs every updating member's step
 // with a fixed sequence of launches (csrc/kernels.cuh: launch_batch_step) and one host synchronisation, whatever K is.
 // Each member keeps the host half of a bb200_amcl (AmclPolicy) and a slice of the batch's particle buffers, and reads one
-// of the batch's maps (each a grid with its sensor model: likelihood-field model or the beam model).
+// of the batch's maps (a grid with its sensor model, the likelihood-field model or the beam model, or a landmark map with
+// the landmark or bearing model).
 #pragma once
 
 #include <map>
@@ -71,6 +72,14 @@ class Batch {
   /// Adds a map without assigning it; *id receives its id (0, 1, ... over the batch's life, never reused).
   int add_likelihood_field_map(const bb200_likelihood_field_param& p, const bb200_occupancy_grid& grid, bool prob, int* id);
   int add_beam_map(const bb200_beam_param& p, const bb200_occupancy_grid& grid, int* id);
+  /// A landmark map for LandmarkSensorModel2d (lp) or, with lp null, BearingSensorModel2d (bp), prepared and checked as
+  /// Filter::set_landmark_map prepares it: set_* for every member, add_* without assigning it.
+  int set_landmark_map(const bb200_landmark_param* lp, const bb200_bearing_param* bp, const bb200_landmark_map& map);
+  int add_landmark_map(const bb200_landmark_param* lp, const bb200_bearing_param* bp, const bb200_landmark_map& map, int* id);
+  /// Replaces the staged detections of every member whose present[m] is non-zero (present == nullptr: every occupied
+  /// slot) with detections[m][0, n[m]): a host copy, no device call.  A BB200_MEASUREMENT_LANDMARKS member weighs its
+  /// staged detections in every step until they are replaced; remove_member drops them.
+  int set_detections(const bb200_landmark_detection* const* detections, const uint64_t* n, const uint8_t* present);
   /// Amcl::update_map for one member: its particles and policies stay; its later steps read map `id`.
   int update_map(int member, int id);
   int member_map(int member, int* id) const;
@@ -168,6 +177,10 @@ class Batch {
       DeviceBuffer<double2> directions;
     };
     ScanTable scan;
+    // The detections a BB200_MEASUREMENT_LANDMARKS step weighs (set_detections), as given: their category slices are
+    // resolved against the member's map at step time.
+    std::vector<bb200_landmark_detection> detections;
+    bool detections_staged{false};
   };
   struct MapEntry {
     DeviceMap map;
@@ -237,6 +250,7 @@ class Batch {
   int member_ok(int member) const;
   const MapEntry* find_map(int id) const;
   int ensure_points(uint64_t n_points);
+  int ensure_detections(uint64_t n);
   int ensure_inputs(uint64_t floats);
   int ensure_scan_table(Member& m, const bb200_laser_scan& scan);
   /// The step of update and update_measurements: in[m] is member m's measurement, already checked when it is a scan or a cloud.
@@ -308,6 +322,8 @@ class Batch {
   PinnedBuffer<uint32_t> first_host_;
   DeviceBuffer<double> points_;   // (x, y) pairs
   PinnedBuffer<double> points_host_;
+  DeviceBuffer<LandmarkDetection> detections_;  // the step's prepared detections, every kBatchLandmark member's in member order
+  PinnedBuffer<LandmarkDetection> detections_host_;
   // Scans and clouds of update_measurements (allocated on first use): batch_points_kernel's member table and the raw
   // measurements (kept ranges, or x, y, z per cloud point).
   struct InputTable {

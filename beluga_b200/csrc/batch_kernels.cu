@@ -6,6 +6,7 @@
 #include "raycast.cuh"
 #include "resample.cuh"
 #include "reweight_beam.cuh"
+#include "reweight_landmark_block.cuh"
 #include "reweight_lfm.cuh"
 
 #include <algorithm>
@@ -73,6 +74,23 @@ __device__ __forceinline__ void batch_recovery_map(const BatchStepArgs& s, const
     a.grid_resolution = s.grid_resolution;
     a.grid_origin = s.grid_origin;
   }
+}
+
+/// A member's landmark model constants, landmarks and box (landmark.model 0: a grid map).
+template <bool kTable>
+__device__ __forceinline__ const LandmarkParams& batch_landmark(const BatchStepArgs& s, const BatchMember& m) {
+  if constexpr (kTable) return s.maps[m.map].landmark;
+  else return s.landmark;
+}
+template <bool kTable>
+__device__ __forceinline__ const LandmarkPoint* batch_landmarks(const BatchStepArgs& s, const BatchMember& m) {
+  if constexpr (kTable) return s.maps[m.map].landmarks;
+  else return s.landmarks;
+}
+template <bool kTable>
+__device__ __forceinline__ BoxSpace batch_box(const BatchStepArgs& s, const BatchMember& m) {
+  const double* b = kTable ? s.maps[m.map].box : s.box;
+  return BoxSpace{b[0], b[1], b[2], b[3]};
 }
 
 /// The per-step scalars of every member (what begin_fused_step_kernel resets for one filter) and the scan state.
@@ -158,6 +176,24 @@ __global__ void __launch_bounds__(kBeamThreads, kBeamBlocksPerSm) batch_reweight
   const double2* points = reinterpret_cast<const double2*>(s.points) + m.point_offset;
   reweight_beam_block(batch_states(s, m, 0), s.weights + m.offset, m.n, nullptr, batch_occupancy<kTable>(s, m), batch_beam<kTable>(s, m), points,
                       m.n_points, s.scalars + k, local);
+}
+
+/// reweight_landmark_kernel per kBatchLandmark member: its detections at detections + point_offset.  The model is the
+/// member's map's, so it is uniform within a CTA.
+template <bool kTable>
+__global__ void __launch_bounds__(kLandmarkThreads) batch_reweight_landmark_kernel(BatchStepArgs s) {
+  uint32_t local, count;
+  const uint32_t k = batch_member_of(s, kBatchLandmarkRow, blockIdx.x, local, count);
+  const BatchMember& m = s.members[k];
+  const LandmarkParams& params = batch_landmark<kTable>(s, m);
+  const LandmarkDetection* detections = s.detections + m.point_offset;
+  if (params.model == BB200_SENSOR_BEARING) {
+    reweight_landmark_block<BB200_SENSOR_BEARING>(batch_states(s, m, 0), s.weights + m.offset, m.n, params, batch_landmarks<kTable>(s, m), detections,
+                                                  m.n_points, s.scalars + k, local);
+  } else {
+    reweight_landmark_block<BB200_SENSOR_LANDMARK>(batch_states(s, m, 0), s.weights + m.offset, m.n, params, batch_landmarks<kTable>(s, m), detections,
+                                                   m.n_points, s.scalars + k, local);
+  }
 }
 
 /// apply_factors_kernel per weighed member: w *= factor over the member's slice, the largest weight into its scalars.
@@ -266,8 +302,9 @@ __device__ __forceinline__ void normalize_moments_block(const Pose2* __restrict_
 /// its summary to batch_resampled_moments_kernel.  A member that ran the effective-sample-size test follows its
 /// decision: it draws and leaves its summary to that kernel too (Filter::resample, then Filter::estimate), or it sums the
 /// moments of the weights batch_ess_kernel normalised (Filter::estimate).  Its range fits either partition; the CTAs
-/// beyond the one it takes only leave.
-template <bool kTable>
+/// beyond the one it takes only leave.  kBox: some member of the step reads a landmark map, and such a member's injected
+/// states come from its map's box (resample_box_kernel's body).
+template <bool kTable, bool kBox>
 __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs s) {
   uint32_t local, count;
   const uint32_t k = batch_member_of(s, kBatchFinish, blockIdx.x, local, count);
@@ -310,11 +347,15 @@ __global__ void __launch_bounds__(kRsThreads) batch_finish_kernel(BatchStepArgs 
     if (local >= grid) return;
     if (scatter) {
       resample_scatter_block(a, scalars, partials, local, grid, a.tail);
+    } else if (kBox && batch_landmark<kTable>(s, m).model != 0) {
+      resample_block<StepTail, true>(a, scalars, partials, local, grid, a.tail, batch_box<kTable>(s, m));
     } else {
       resample_block(a, scalars, partials, local, grid, a.tail);
     }
   } else if (scatter) {
     resample_scatter_block(a, scalars, partials, local, count, tail);
+  } else if (kBox && batch_landmark<kTable>(s, m).model != 0) {
+    resample_block<BatchTail, true>(a, scalars, partials, local, count, tail, batch_box<kTable>(s, m));
   } else {
     resample_block(a, scalars, partials, local, count, tail);
   }
@@ -625,6 +666,10 @@ int launch_batch_step_head_from(const BatchStepArgs& s, cudaStream_t stream) {
     batch_reweight_beam_kernel<kTable><<<s.ctas[kBatchReweightBeam], kBeamThreads, 0, stream>>>(s);
     launches += 1;
   }
+  if (s.forms & (1 << kBatchLandmark)) {
+    batch_reweight_landmark_kernel<kTable><<<s.landmark_ctas, kLandmarkThreads, 0, stream>>>(s);
+    launches += 1;
+  }
   return launches;
 }
 
@@ -640,7 +685,11 @@ int launch_batch_step_tail_from(const BatchStepArgs& s, cudaStream_t stream) {
     batch_ess_kernel<<<s.ess_ctas, kStreamThreads, 0, stream>>>(s);
     launches += 1;
   }
-  batch_finish_kernel<kTable><<<s.ctas[kBatchFinish], kRsThreads, 0, stream>>>(s);
+  if (s.landmark_maps) {
+    batch_finish_kernel<kTable, true><<<s.ctas[kBatchFinish], kRsThreads, 0, stream>>>(s);
+  } else {
+    batch_finish_kernel<kTable, false><<<s.ctas[kBatchFinish], kRsThreads, 0, stream>>>(s);
+  }
   if (s.kld != nullptr) {
     batch_kld_kernel<<<s.post_ctas[0], kBatchKldThreads, 0, stream>>>(s);
     launches += 1;
@@ -659,7 +708,7 @@ uint32_t batch_scan_tiles(uint64_t n) { return scan_tile_count(n); }
 void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunches]) {
   out[kBatchPropagate] = static_cast<uint32_t>((m.n + kPrThreads - 1) / kPrThreads);
   out[kBatchReweight] = out[kBatchReweightWalk] = out[kBatchReweightBeam] = 0;
-  if (form != kBatchWeighed) out[batch_reweight_row(form)] = static_cast<uint32_t>((m.n + kRwThreads - 1) / kRwThreads);
+  if (form != kBatchWeighed && form != kBatchLandmark) out[batch_reweight_row(form)] = static_cast<uint32_t>((m.n + kRwThreads - 1) / kRwThreads);
   out[kBatchScan] = scan_tile_count(m.n);
   // the partition launch_resample / launch_moments would use for a single filter of this size
   if (!m.resample) {
@@ -679,6 +728,8 @@ void batch_post_ctas(const BatchMember& m, uint32_t out[3]) {
 }
 
 uint32_t batch_weigh_ctas(const BatchMember& m) { return static_cast<uint32_t>(std::min<uint64_t>((m.n + kMaxThreads - 1) / kMaxThreads, kStreamMaxBlocks)); }
+
+uint32_t batch_landmark_ctas(const BatchMember& m) { return static_cast<uint32_t>((m.n + kLandmarkThreads - 1) / kLandmarkThreads); }
 
 int launch_batch_step_head(const BatchStepArgs& s, cudaStream_t stream) {
   return s.maps != nullptr ? launch_batch_step_head_from<true>(s, stream) : launch_batch_step_head_from<false>(s, stream);

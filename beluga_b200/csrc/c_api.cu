@@ -878,6 +878,31 @@ int bb200_amcl_batch_add_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p
   BB_REQUIRE(b && p && grid && map_id);
   return guarded(b->impl, [&] { return b->impl.add_beam_map(*p, *grid, map_id); });
 }
+int bb200_amcl_batch_set_landmark_map(bb200_amcl_batch* b, const bb200_landmark_param* p, const bb200_landmark_map* map) {
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
+  BB_REQUIRE(b && p && map);
+  return guarded(b->impl, [&] { return b->impl.set_landmark_map(p, nullptr, *map); });
+}
+int bb200_amcl_batch_set_bearing_map(bb200_amcl_batch* b, const bb200_bearing_param* p, const bb200_landmark_map* map) {
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
+  BB_REQUIRE(b && p && map);
+  return guarded(b->impl, [&] { return b->impl.set_landmark_map(nullptr, p, *map); });
+}
+int bb200_amcl_batch_add_landmark_map(bb200_amcl_batch* b, const bb200_landmark_param* p, const bb200_landmark_map* map, int* map_id) {
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
+  BB_REQUIRE(b && p && map && map_id);
+  return guarded(b->impl, [&] { return b->impl.add_landmark_map(p, nullptr, *map, map_id); });
+}
+int bb200_amcl_batch_add_bearing_map(bb200_amcl_batch* b, const bb200_bearing_param* p, const bb200_landmark_map* map, int* map_id) {
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
+  BB_REQUIRE(b && p && map && map_id);
+  return guarded(b->impl, [&] { return b->impl.add_landmark_map(nullptr, p, *map, map_id); });
+}
+int bb200_amcl_batch_set_detections(bb200_amcl_batch* b, const bb200_landmark_detection* const* detections, const uint64_t* n, const uint8_t* present) {
+  BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
+  BB_REQUIRE(b && n);
+  return guarded(b->impl, [&] { return b->impl.set_detections(detections, n, present); });
+}
 int bb200_amcl_batch_update_map(bb200_amcl_batch* b, int member, int map_id) {
   BB_REFUSE_OPEN_STEP(b, kBatchStepOpen);
   BB_REQUIRE(b);

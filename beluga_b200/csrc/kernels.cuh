@@ -28,6 +28,7 @@
 #include <string>
 
 #include "../../include/beluga_b200.h"
+#include "reweight_landmark.cuh"
 #include "se2_math.cuh"
 
 namespace bb200 {
@@ -456,8 +457,9 @@ enum BatchLaunch : int {
 };
 /// The reweight forms of a batch step; BatchStepArgs::forms has bit f set when some member takes form f.
 /// kBatchWeighed: a member the caller weighs (bb200_amcl_batch_update_begin / _end); it has no CTA in the reweight rows and
-/// its CTAs in the kBatchWeighRow row instead.
-enum BatchReweightPath : int { kBatchField = 0, kBatchBeamTwoPass = 1, kBatchBeamFused = 2, kBatchWeighed = 3 };
+/// its CTAs in the kBatchWeighRow row instead.  kBatchLandmark: a member on a landmark map weighing its detections; its
+/// CTAs are in the kBatchLandmarkRow row.
+enum BatchReweightPath : int { kBatchField = 0, kBatchBeamTwoPass = 1, kBatchBeamFused = 2, kBatchWeighed = 3, kBatchLandmark = 4 };
 /// The CTA-range row of each reweight form.
 constexpr int batch_reweight_row(int form) {
   return form == kBatchField ? kBatchReweight : form == kBatchBeamTwoPass ? kBatchReweightWalk : kBatchReweightBeam;
@@ -473,6 +475,12 @@ struct BatchMap {
   int grid_width;
   double grid_resolution;
   Pose2 grid_origin;
+  // Landmark maps (after the grid fields, so that the grid kernels keep their offsets): the model constants, the
+  // landmarks sorted by category and the box injected states are drawn from; landmark.model is 0 on a grid map.
+  LandmarkParams landmark;
+  const LandmarkPoint* landmarks;
+  uint32_t n_landmarks;
+  double box[4];
 };
 
 /// The KLD parameters of a member that resamples under KLD in a batch step (BatchMember::kld), one entry per member of the
@@ -531,12 +539,23 @@ struct BatchStepArgs {
   // step has none) and the batch's factor buffer, laid out like the weights.
   uint32_t weigh_ctas;
   const double* factors;
+  // Members on landmark maps (after every field the other kernels read).  When every member of the step reads one map
+  // and it is a landmark map, its model, landmarks and box (landmark.model is 0 otherwise); with several maps they come
+  // from maps[BatchMember::map].  A kBatchLandmark member's detections are detections[point_offset, + n_points).
+  LandmarkParams landmark;
+  const LandmarkPoint* landmarks;
+  uint32_t n_landmarks;
+  double box[4];
+  const LandmarkDetection* detections;
+  uint32_t landmark_ctas;         // total CTAs of batch_reweight_landmark_kernel, 0 when no member takes kBatchLandmark
+  int landmark_maps;              // 1: some updating member reads a landmark map (its recovery injection draws from the box)
 };
 static_assert(sizeof(BatchStepArgs) <= 1024, "the step's arguments travel as one kernel parameter block (4 KB at most)");
 /// Reset | propagate | reweight | [weigh] | quantise + scan | resample or normalise + moments, in two halves that each
 /// return their launch count: launch_batch_step_head enqueues the reset, the propagate and the reweight, and
 /// launch_batch_step_tail the rest.  The reweight takes one launch for the likelihood field, two for the beam model's
-/// two-pass form (walk, mixture) and one for its fused form, each issued when some member takes that form.  When some
+/// two-pass form (walk, mixture), one for its fused form and one for the landmark and bearing models, each issued when some
+/// member takes that form.  When some
 /// member is weighed by the caller (args.weigh_ctas > 0), the tail starts with one launch of w *= factor.  When some member
 /// runs the effective-sample-size test (args.ess_ctas > 0), one launch before the resample normalises its weights and
 /// decides.  After the resample, when some member resamples under KLD (args.kld set), one launch counts each such member's
@@ -544,7 +563,7 @@ static_assert(sizeof(BatchStepArgs) <= 1024, "the step's arguments travel as one
 /// set that a separate estimate pass reads in a standalone filter.  The two halves together: 4 launches plus those, so 5 to
 /// 8 without weighed, KLD or selective members, 7 to 10 with KLD members or with selective ones, and 8 to 11 with both,
 /// one more with weighed members, whatever the members, their maps, their particle counts, their decisions, their accepted
-/// counts and their scans are.
+/// counts and their scans are.  The landmark form's launch raises each of these upper bounds by one.
 int launch_batch_step_head(const BatchStepArgs& args, cudaStream_t stream);
 int launch_batch_step_tail(const BatchStepArgs& args, cudaStream_t stream);
 /// Scan tiles of a member of n particles (the quantise-scan CTAs it needs).
@@ -563,7 +582,9 @@ constexpr int kBatchMomentsRow = kBatchLaunches + 2;
 constexpr int kBatchEssRow = kBatchLaunches + 3;
 /// The row of batch_weigh_kernel: apply_factors_block's grid of a standalone filter of the member's size per weighed member.
 constexpr int kBatchWeighRow = kBatchLaunches + 4;
-constexpr int kBatchRows = kBatchLaunches + 5;
+/// The row of batch_reweight_landmark_kernel: reweight_landmark_kernel's grid per kBatchLandmark member.
+constexpr int kBatchLandmarkRow = kBatchLaunches + 5;
+constexpr int kBatchRows = kBatchLaunches + 6;
 /// How a member's measurement reaches a batch step (the values of bb200_measurement_kind).
 enum BatchInputKind : int { kBatchInputPoints = 0, kBatchInputScan = 1, kBatchInputCloud = 2, kBatchInputWeights = 3 };
 /// One member of batch_points_kernel, built on the host every step (one per entry of the step's member table).
@@ -597,6 +618,8 @@ void batch_member_ctas(const BatchMember& m, int form, uint32_t out[kBatchLaunch
 void batch_post_ctas(const BatchMember& m, uint32_t out[3]);
 /// CTAs of a weighed member in the kBatchWeighRow row.
 uint32_t batch_weigh_ctas(const BatchMember& m);
+/// CTAs of a kBatchLandmark member in the kBatchLandmarkRow row.
+uint32_t batch_landmark_ctas(const BatchMember& m);
 
 /// One member of a batch's pose-sample draw (Filter::sample_states per member).
 struct BatchSampleMember {

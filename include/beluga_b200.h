@@ -703,12 +703,13 @@ int bb200_amcl_leave_shards(bb200_amcl* a);
  * These counts are fixed before the step runs: they depend on neither K, nor the particle counts, nor the
  * members' decisions.
  *
- * A batch holds a set of maps, each a grid with its sensor model: likelihood-field model or the beam model.
- * Each member reads one of them or none.  bb200_amcl_batch_set_likelihood_field_map and _set_beam_map give every
+ * A batch holds a set of maps, each a grid with its sensor model (likelihood-field model or the beam model) or a
+ * landmark map with the landmark or bearing model.  Each member reads one of them or none.  bb200_amcl_batch_set_likelihood_field_map and _set_beam_map give every
  * member one map; bb200_amcl_batch_add_*_map and bb200_amcl_batch_update_map let members read different maps and
  * move between them, as a node's Amcl::update_map does.  Each reweight form that some updating member takes costs
  * launches: the likelihood field 1, the beam model 2 on maps where a standalone filter walks its rays in two
- * passes, and 1 otherwise.  A step takes 4 launches plus those, so 5 to 8, whatever K and the number of maps are;
+ * passes, 1 otherwise, and the landmark and bearing models 1 together.  A step takes 4 launches plus those, so 5 to 9,
+ * whatever K and the number of maps are;
  * a step whose updating members read one map takes 5, or 6 for the two-pass beam form.  The two-pass members of a
  * step take the fused beam kernel instead when their hit words (sum of round_up(n, 32) x scan points x 4 bytes)
  * exceed 3 GiB or cannot be allocated.  Either way every member's results stay bit-identical to its standalone twin's.
@@ -756,6 +757,16 @@ int bb200_amcl_batch_set_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p
 int bb200_amcl_batch_add_likelihood_field_map(bb200_amcl_batch* b, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid,
                                               int prob, int* map_id);
 int bb200_amcl_batch_add_beam_map(bb200_amcl_batch* b, const bb200_beam_param* p, const bb200_occupancy_grid* grid, int* map_id);
+/* Landmark maps: LandmarkSensorModel2d<LandmarkMap> / BearingSensorModel2d<LandmarkMap> on `map`, prepared and checked
+ * exactly as bb200_filter_set_landmark_map / _set_bearing_map prepare them (the same statuses and messages).  _set_*
+ * replaces every map as bb200_amcl_batch_set_beam_map does; _add_* adds one without assigning it.  A member on a landmark
+ * map steps with BB200_MEASUREMENT_LANDMARKS (bb200_amcl_batch_set_detections); its initialize_from_map and recovery
+ * injection draw from the map's box.  bb200_amcl_batch_get_likelihood_field and bb200_amcl_batch_cast_rays refuse a
+ * landmark map with BB200_ERR_STATE. */
+int bb200_amcl_batch_set_landmark_map(bb200_amcl_batch* b, const bb200_landmark_param* p, const bb200_landmark_map* map);
+int bb200_amcl_batch_set_bearing_map(bb200_amcl_batch* b, const bb200_bearing_param* p, const bb200_landmark_map* map);
+int bb200_amcl_batch_add_landmark_map(bb200_amcl_batch* b, const bb200_landmark_param* p, const bb200_landmark_map* map, int* map_id);
+int bb200_amcl_batch_add_bearing_map(bb200_amcl_batch* b, const bb200_bearing_param* p, const bb200_landmark_map* map, int* map_id);
 /* Amcl::update_map (amcl_core.hpp:150) / beluga_ros::Amcl::update_map (beluga_ros/src/amcl.cpp:48-51) for one member:
  * its particles and policies are kept; its next reweight, recovery injection and initialize_from_map use map_id. */
 int bb200_amcl_batch_update_map(bb200_amcl_batch* b, int member, int map_id);
@@ -831,11 +842,16 @@ int bb200_amcl_batch_update(bb200_amcl_batch* b, const double* control_poses, co
  * bb200_amcl_update, bb200_amcl_update_scan and bb200_amcl_update_point_cloud take it.  Only the fields of `kind` are read. */
 /* BB200_MEASUREMENT_WEIGHTS: this member is weighed by the caller (bb200_amcl_batch_update_begin / _end only; the other
  * update calls refuse it); no field of the measurement is read. */
+/* BB200_MEASUREMENT_LANDMARKS: this member, on a landmark map, weighs the detections staged for it by
+ * bb200_amcl_batch_set_detections, as bb200_amcl_update_landmarks weighs them; no field of the measurement is read.  The
+ * update calls refuse with BB200_ERR_STATE, before anything reaches the device, a present LANDMARKS member on a grid map
+ * or without staged detections, and a present points, scan or cloud member on a landmark map. */
 typedef enum bb200_measurement_kind {
   BB200_MEASUREMENT_POINTS = 0,
   BB200_MEASUREMENT_SCAN = 1,
   BB200_MEASUREMENT_CLOUD = 2,
-  BB200_MEASUREMENT_WEIGHTS = 3
+  BB200_MEASUREMENT_WEIGHTS = 3,
+  BB200_MEASUREMENT_LANDMARKS = 4
 } bb200_measurement_kind;
 typedef struct bb200_measurement {
   int kind;                        /* bb200_measurement_kind */
@@ -893,6 +909,12 @@ int bb200_amcl_batch_update_clustered(bb200_amcl_batch* b, const double* control
  * the step. */
 int bb200_amcl_batch_update_begin(bb200_amcl_batch* b, const double* control_poses, const bb200_measurement* measurements, const uint8_t* present,
                                   bb200_weigh_view* views);
+/* Stages detections[m][0, n[m]) for every member m with present[m] != 0 (present NULL: every occupied slot), replacing
+ * what was staged for it; they stay staged, and every BB200_MEASUREMENT_LANDMARKS step of the member weighs them, until
+ * they are replaced or the member is removed.  A host copy: nothing reaches the device.  Each detection's category is
+ * resolved against the member's map when a step weighs it.  BB200_ERR_INVALID_ARGUMENT, with nothing staged, for a
+ * null handle or n, a vacant selected slot, a null detections or detections[m] with n[m] > 0, or n[m] >= 2^32 - 1. */
+int bb200_amcl_batch_set_detections(bb200_amcl_batch* b, const bb200_landmark_detection* const* detections, const uint64_t* n, const uint8_t* present);
 int bb200_amcl_batch_update_end(bb200_amcl_batch* b, const bb200_cluster_param* cluster, bb200_update_result* out, bb200_estimate* clustered,
                                 uint32_t* n_cells, uint32_t* n_clusters);
 /* Kernel launches issued by this batch so far (steps, initialisations, cluster estimates, particle-cloud histograms and

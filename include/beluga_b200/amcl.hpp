@@ -592,6 +592,34 @@ class AmclBatch {
     check(bb200_amcl_batch_add_beam_map(handle_, &p, &grid, &id));
     return id;
   }
+  /// A landmark map (LandmarkSensorModel2d / BearingSensorModel2d on `map`) for every member, or added without assigning
+  /// it; members on it step with landmark_token measurements.
+  void set_landmark_map(const LandmarkModelParam& p, const LandmarkMap& map) {
+    const bb200_landmark_param c = c_param(p);
+    const bb200_landmark_map m = map.view();
+    check(bb200_amcl_batch_set_landmark_map(handle_, &c, &m));
+    field_cells_.clear();
+  }
+  void set_bearing_map(const BearingModelParam& p, const LandmarkMap& map) {
+    const bb200_bearing_param c = c_param(p);
+    const bb200_landmark_map m = map.view();
+    check(bb200_amcl_batch_set_bearing_map(handle_, &c, &m));
+    field_cells_.clear();
+  }
+  int add_landmark_map(const LandmarkModelParam& p, const LandmarkMap& map) {
+    const bb200_landmark_param c = c_param(p);
+    const bb200_landmark_map m = map.view();
+    int id = -1;
+    check(bb200_amcl_batch_add_landmark_map(handle_, &c, &m, &id));
+    return id;
+  }
+  int add_bearing_map(const BearingModelParam& p, const LandmarkMap& map) {
+    const bb200_bearing_param c = c_param(p);
+    const bb200_landmark_map m = map.view();
+    int id = -1;
+    check(bb200_amcl_batch_add_bearing_map(handle_, &c, &m, &id));
+    return id;
+  }
   /// Amcl::update_map (amcl_core.hpp:150) for one member: it keeps its particles and reads map `map_id` from its next step.
   void update_map(std::size_t member, int map_id) { check(bb200_amcl_batch_update_map(handle_, index(member), map_id)); }
   /// The id of the map member m reads (-1: none).
@@ -642,16 +670,18 @@ class AmclBatch {
     return estimates_of(r);
   }
 
-  /// One member's measurement in a step: base-frame points, a laser scan or a point cloud, as Amcl::update takes them.  The
+  /// One member's measurement in a step: base-frame points, a laser scan or a point cloud, as Amcl::update takes them, or
+  /// the detections of a member on a landmark map (what LandmarkSensorModel2d / BearingSensorModel2d return).  The
   /// constructors are explicit, so that a braced list of point vectors still selects the points overload above.
   struct Measurement {
     explicit Measurement(std::vector<std::pair<double, double>> points) : value(std::move(points)) {}
     explicit Measurement(const LaserScanView& scan) : value(scan) {}
     explicit Measurement(const PointCloudView& cloud) : value(cloud) {}
-    std::variant<std::vector<std::pair<double, double>>, LaserScanView, PointCloudView> value;
+    explicit Measurement(landmark_token detections) : value(std::move(detections)) {}
+    std::variant<std::vector<std::pair<double, double>>, LaserScanView, PointCloudView, landmark_token> value;
   };
   /// The bb200_measurement of one member's measurement; a scan's or a cloud's C view goes to *scan or *cloud, which must
-  /// outlive the call it is passed to.
+  /// outlive the call it is passed to.  Detections reach the batch through stage_detections.
   static bb200_measurement c_measurement(const Measurement& measurement, bb200_laser_scan* scan, bb200_point_cloud* cloud) {
     const auto& v = measurement.value;
     if (const auto* points = std::get_if<0>(&v))
@@ -660,8 +690,27 @@ class AmclBatch {
       *scan = s->c_view();
       return bb200_measurement{BB200_MEASUREMENT_SCAN, nullptr, 0, scan, nullptr};
     }
+    if (std::holds_alternative<landmark_token>(v)) return bb200_measurement{BB200_MEASUREMENT_LANDMARKS, nullptr, 0, nullptr, nullptr};
     *cloud = std::get<PointCloudView>(v).c_view();
     return bb200_measurement{BB200_MEASUREMENT_CLOUD, nullptr, 0, nullptr, cloud};
+  }
+  /// bb200_amcl_batch_set_detections for every selected member whose measurement is a landmark_token (none: no call).
+  template <class At>
+  void stage_detections(std::size_t k, At measurement_at, const std::vector<bool>* present) {
+    std::vector<const bb200_landmark_detection*> dets(k, nullptr);
+    std::vector<std::uint64_t> counts(k, 0);
+    std::vector<std::uint8_t> mask(k, 0);
+    bool any = false;
+    for (std::size_t m = 0; m < k; ++m) {
+      const Measurement* meas = measurement_at(m);
+      const auto* token = meas != nullptr ? std::get_if<landmark_token>(&meas->value) : nullptr;
+      if (token == nullptr || (present != nullptr ? !(*present)[m] : sizes_[m] == 0)) continue;
+      dets[m] = token->detections.empty() ? nullptr : token->detections.data();
+      counts[m] = token->detections.size();
+      mask[m] = 1;
+      any = true;
+    }
+    if (any) check(bb200_amcl_batch_set_detections(handle_, dets.data(), counts.data(), mask.data()));
   }
   /// update with member m's measurement in measurements[m], so that members with 2-D and 3-D lidars step in one call; scans
   /// and clouds are converted on the device (bb200_amcl_batch_update_measurements).  Every member's result equals its
@@ -677,6 +726,7 @@ class AmclBatch {
     std::vector<bb200_point_cloud> clouds(k);
     std::vector<bb200_measurement> in(k);
     std::vector<std::uint8_t> mask(present != nullptr ? k : 0);
+    stage_detections(k, [&](std::size_t m) { return &measurements[m]; }, present);
     for (std::size_t m = 0; m < k; ++m) {
       in[m] = c_measurement(measurements[m], &scans[m], &clouds[m]);
       if (present != nullptr) mask[m] = (*present)[m] ? 1 : 0;
@@ -700,6 +750,7 @@ class AmclBatch {
     std::vector<bb200_point_cloud> clouds(k);
     std::vector<bb200_measurement> in(k);
     std::vector<std::uint8_t> mask(present != nullptr ? k : 0);
+    stage_detections(k, [&](std::size_t m) { return measurements[m] ? &*measurements[m] : nullptr; }, present);
     for (std::size_t m = 0; m < k; ++m) {
       in[m] = measurements[m] ? c_measurement(*measurements[m], &scans[m], &clouds[m]) : bb200_measurement{BB200_MEASUREMENT_WEIGHTS, nullptr, 0, nullptr, nullptr};
       if (present != nullptr) mask[m] = (*present)[m] ? 1 : 0;
@@ -736,18 +787,8 @@ class AmclBatch {
     std::vector<bb200_point_cloud> clouds(k);
     std::vector<bb200_measurement> in(k);
     const std::vector<std::uint8_t> mask = presence_mask(present);
-    for (std::size_t m = 0; m < k; ++m) {
-      const auto& v = measurements[m].value;
-      if (const auto* points = std::get_if<0>(&v)) {
-        in[m] = bb200_measurement{BB200_MEASUREMENT_POINTS, points->empty() ? nullptr : &points->front().first, points->size(), nullptr, nullptr};
-      } else if (const auto* scan = std::get_if<LaserScanView>(&v)) {
-        scans[m] = scan->c_view();
-        in[m] = bb200_measurement{BB200_MEASUREMENT_SCAN, nullptr, 0, &scans[m], nullptr};
-      } else {
-        clouds[m] = std::get<PointCloudView>(v).c_view();
-        in[m] = bb200_measurement{BB200_MEASUREMENT_CLOUD, nullptr, 0, nullptr, &clouds[m]};
-      }
-    }
+    stage_detections(k, [&](std::size_t m) { return &measurements[m]; }, present);
+    for (std::size_t m = 0; m < k; ++m) in[m] = c_measurement(measurements[m], &scans[m], &clouds[m]);
     const bb200_cluster_param p{parameters.linear_hash_resolution, parameters.angular_hash_resolution, parameters.weight_cap_percentile};
     std::vector<bb200_update_result> r(k);
     std::vector<bb200_estimate> e(k);
@@ -945,6 +986,13 @@ class AmclBatch {
   }
   void check(int status) const {
     if (status != BB200_OK) throw Error(status, bb200_amcl_batch_last_error(handle_));
+  }
+  static bb200_landmark_param c_param(const LandmarkModelParam& p) { return bb200_landmark_param{p.sigma_range, p.sigma_bearing, p.random_prob}; }
+  static bb200_bearing_param c_param(const BearingModelParam& p) {
+    bb200_bearing_param c{};
+    c.sigma_bearing = p.sigma_bearing;
+    for (int k = 0; k < 12; ++k) c.sensor_pose_in_robot[k] = p.sensor_pose_in_robot.m[k];
+    return c;
   }
   std::vector<std::uint8_t> presence_mask(const std::vector<bool>* present) const {
     if (present != nullptr && present->size() != size()) throw Error(BB200_ERR_INVALID_ARGUMENT, "one presence flag per member");

@@ -25,6 +25,8 @@ same step weighed by the caller (update_weighted, one torch kernel per shard), o
 (and over devices 0..1 and 0..3 where there are that many).
 `landmark`: the landmark and bearing models at 1M particles x 16 detections on a fiducial-like and a reflector-like map, with
 the reweight kernel's share of the FP64 bound and the Python oracle beside them.
+`batch_landmark`: AmclBatch with the landmark model, K in {1, 16, 64, 256} members x 2000 particles x 16 detections on the
+same two maps, against the same members stepped as standalone Amcl.update_landmarks.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import ctypes
@@ -782,6 +784,64 @@ def run_landmark():
     return res
 
 
+def run_batch_landmark():
+    """AmclBatch with the landmark model: K in {1, 16, 64, 256} members x 2000 particles x 16 detections on (a) 64 landmarks
+    in 64 categories (fiducial-like) and (b) 1000 landmarks in one category (reflector-like), systematic resampling, every
+    member updating every step with its own detections; beside it, in the same process and alternated step by step, the
+    same K members stepped as standalone Amcl.update_landmarks one after another.  Host clock around each round (both end
+    synchronised), median of `steps` after `warmup`."""
+    res = {}
+    device = device_record()
+    rng = np.random.default_rng(13)
+    n, nd, steps, warmup = 2000, 16, 20, 3
+    param = bb.LandmarkModelParam(0.5, 0.3, 1e-3)
+    for map_name, n_lm, n_cat in (("64_in_64_categories", 64, 64), ("1000_in_1_category", 1000, 1)):
+        pos = np.stack([rng.uniform(-20, 20, n_lm), rng.uniform(-20, 20, n_lm), rng.uniform(0, 2, n_lm)], axis=1)
+        cat = (np.arange(n_lm) % n_cat).astype(np.uint32)
+        lmap = bb.LandmarkMap(pos, cat)
+        for k in (1, 16, 64, 256):
+            params = [bb.AmclParams(update_min_d=0.0, update_min_a=0.0, min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC,
+                                    seed=m) for m in range(k)]
+            motions = [bb.DifferentialDriveModelParam(*MOTION) for _ in range(k)]
+            batch = bb.AmclBatch(motions, params)
+            batch.set_landmark_map(param, lmap)
+            singles = []
+            for m in range(k):
+                batch.initialize(m, [0.0, 0.0, 0.0], np.diag([4.0, 4.0, 0.5]))
+                a = bb.Amcl(motions[m], params[m])
+                a.update_map(bb.SENSOR_LANDMARK, param, lmap)
+                a.initialize([0.0, 0.0, 0.0], np.diag([4.0, 4.0, 0.5]))
+                singles.append(a)
+            wall_batch, wall_single, launches = [], [], []
+            for t in range(warmup + steps):
+                pose = [np.cos(0.01 * t), np.sin(0.01 * t), 0.05 * t, 0.0]
+                dets = [(np.stack([rng.uniform(-5, 5, nd), rng.uniform(-5, 5, nd), rng.uniform(0, 2, nd)], axis=1),
+                         rng.integers(0, n_cat, nd).astype(np.uint32)) for _ in range(k)]
+                meas = [bb.Detections(*d) for d in dets]
+                t0 = time.perf_counter()
+                before = batch.launch_count()
+                r = batch.update_measurements([pose] * k, meas)
+                assert all(x.updated for x in r)
+                launches.append(batch.launch_count() - before)
+                t1 = time.perf_counter()
+                for a, d in zip(singles, dets):
+                    assert a.update_landmarks(pose, *d).updated == 1
+                t2 = time.perf_counter()
+                if t >= warmup:
+                    wall_batch.append((t1 - t0) * 1e3)
+                    wall_single.append((t2 - t1) * 1e3)
+            mb, ms = float(np.median(wall_batch)), float(np.median(wall_single))
+            res[f"batch_landmark_{k}_x_{n}_x_{nd}_{map_name}"] = {
+                "members": k, "particles": n, "detections": nd, "landmarks": n_lm, "categories": n_cat, "steps": steps,
+                "ms_per_step_e2e": mb, "member_steps_per_s": k * 1e3 / mb, "launches_per_step": int(max(launches)),
+                "standalone_ms_per_round": ms, "standalone_member_steps_per_s": k * 1e3 / ms, "speedup": ms / mb, "kernels_ms": {},
+                "device": device}
+            batch.close()
+            for a in singles:
+                a.close()
+    return res
+
+
 def batch_reweight_ms(batch, poses, scans, steps):
     """Mean device time per step of the batch's reweight kernels (names containing batch_reweight or batch_beam), from
     torch.profiler in a run of its own; poses[t] and scans[t] are step t's inputs of every member."""
@@ -1266,6 +1326,8 @@ def main():
         out.update(run_sharded_weighed())
     if "landmark" in which:
         out.update(run_landmark())
+    if "batch_landmark" in which:
+        out.update(run_batch_landmark())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}

@@ -14,7 +14,8 @@ import math
 import numpy as np
 import pytest
 
-from test_fixed_point_lookup_model import BIAS_X, BIAS_Y, bordered_index, kernel_cells, kernel_index, reference_cells
+from _cell_edges import BIAS_X, BIAS_Y, kernel_cells, reference_cells
+from test_fixed_point_lookup_model import bordered_index, kernel_index
 
 M32 = 1 << 32
 

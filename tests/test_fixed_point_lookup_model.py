@@ -5,52 +5,16 @@ whenever the fraction word it reads is at least 5.
 
 This test replays both evaluations on the CPU -- IEEE doubles for the reference sequence, exact rationals rounded
 once for the FMAs -- on random and adversarial (cell-edge) inputs and checks the claim, plus how often the
-fallback would be taken.  CPU only; it models the arithmetic, it does not run the kernel."""
+fallback would be taken.  CPU only; it models the arithmetic, it does not run the kernel.  The model and the case
+generator live in tests/_cell_edges.py, which test_gpu_lfm_cell_edges.py runs on the device."""
 import math
-import struct
 from fractions import Fraction
 
 import numpy as np
 import pytest
 
-MAGIC_X, MAGIC_Y = 393216.0, 1572864.0  # 1.5 * 2^18, 1.5 * 2^20 (kFixedMagicX / kFixedMagicY)
-BIAS_X, BIAS_Y = 0x41180000, 0x41380000
-# Folding the magic add into the FMA chain costs three roundings at the magic's ulp (2^-34 for x, 2^-32 for y) instead of
-# one: the computed fixed-point value lies within 3 half-ulps + 2^-36 of the reference's.  Two ulps of guard are added to
-# the offset, so that the uncertainty interval sits entirely BELOW the computed value: the cell is the reference's
-# whenever the fraction word is at least 5 (kFixedGuardX / kFixedGuardY / kFixedAmbiguous in the kernel).
-GUARD_X, GUARD_Y = 2.0 ** -33, 2.0 ** -31
-AMBIGUOUS_BELOW = 4
-
-
-def fma(a: float, b: float, c: float) -> float:
-    return float(Fraction(a) * Fraction(b) + Fraction(c))  # one rounding, to nearest even
-
-
-def words(t: float):
-    bits = struct.unpack("<Q", struct.pack("<d", t))[0]
-    return bits >> 32, bits & 0xFFFFFFFF
-
-
-def reference_cells(px, py, c, s, tx, ty, inv):
-    x = (px * c - py * s) + tx  # likelihood_field_model.hpp:82-83, every operation rounded
-    y = (px * s + py * c) + ty
-    return math.floor(x * inv), math.floor(y * inv)  # regular_grid.hpp:75-78
-
-
-def kernel_cells(px, py, c, s, tx, ty, inv):
-    """-> (cell x, cell y, ambiguous) as fixed_lookup computes them (before clamping to the border)."""
-    cx, sx = c * inv, s * inv
-    # the magic constants ride in the FMAs' addend: (offset + 1 border cell) + (magic + guard), each sum rounded once
-    ox, oy = (tx * inv + 1.0) + (MAGIC_X + GUARD_X), (ty * inv + 1.0) + (MAGIC_Y + GUARD_Y)
-    gx = fma(px, cx, fma(-py, sx, ox))
-    gy = fma(px, sx, fma(py, cx, oy))
-    hx, lx = words(gx)
-    hy, ly = words(gy)
-    ux = (hx - BIAS_X) & 0xFFFFFFFF  # 4 * padded x + 2 fraction bits (padded x = cell + 1, for cells >= -1)
-    uy = (hy - BIAS_Y) & 0xFFFFFFFF  # padded y
-    to_signed = lambda u: u - (1 << 32) if u >= (1 << 31) else u  # noqa: E731
-    return (to_signed(ux) >> 2) - 1, to_signed(uy) - 1, (lx <= AMBIGUOUS_BELOW or ly <= AMBIGUOUS_BELOW)
+import _cell_edges as ce
+from _cell_edges import kernel_cells, reference_cells
 
 
 def random_case(rng, res):
@@ -158,6 +122,46 @@ def test_end_points_a_hair_either_side_of_an_edge_at_any_heading():
                     decided += 1
                     assert (xk, yk) == (xr, yr), (case, eps)
     assert flagged > 200 and decided > 200
+
+
+# The shared generator (tests/_cell_edges.py) at the edges of the argument: end points 500 cells from poses 7550 cells
+# along a 7998-cell strip (every term near 2^13 cells, where the error bound is largest), and a 1/3 m grid (an inverse that
+# is not exact).  Every edge counts as one that changes the value read.
+HAIR_MAPS = {"strip": ((96, 7998), 0.05, 25.0, ((500, 7550), (-300, 400))), "third": ((300, 300), 1.0 / 3.0, 20.0, ((63, 237), (63, 237)))}
+_hair = {}
+
+
+def hair_set(name):
+    if name not in _hair:
+        shape, res, radius, box = HAIR_MAPS[name]
+        rng = np.random.default_rng(list(HAIR_MAPS).index(name) + 1)
+        emap = ce.EdgeMap.from_values(np.zeros(shape), res, thresh=-1.0)
+        r = radius * np.sqrt(rng.uniform(0.0, 1.0, 181))
+        a = rng.uniform(-math.pi, math.pi, 181)
+        pts = np.stack([r * np.cos(a), r * np.sin(a)], axis=1)
+        pts *= np.minimum(1.0, radius / np.abs(pts).sum(axis=1))[:, None]
+        _, poses = ce.hair_cloud(rng, emap, pts, box, 500, quarter_share=0.3)
+        _hair[name] = emap, pts, poses
+    return _hair[name]
+
+
+@pytest.mark.parametrize("name", list(HAIR_MAPS))
+def test_hair_clouds_near_the_range_limit_and_at_an_inexact_inverse(name):
+    emap, pts, poses = hair_set(name)
+    reach = (np.abs(pts).sum(axis=1).max() + np.abs(poses[:, 2:]).max()) * emap.inv + 2.0
+    assert reach < ce.REACH_LIMIT and (name != "strip" or reach > 8000.0)
+    b = ce.cloud_bands(emap, pts, poses)
+    assert b.wrong == 0, b
+    assert min(b.guard_x, b.guard_y, b.flagged) >= 150 and b.decided_particles >= 150 and b.flagged_particles >= 150, b
+
+
+@pytest.mark.parametrize("mutation", ["no_guard", "no_ambiguity"])
+def test_the_hair_clouds_catch_a_weaker_lookup(mutation):
+    """Without the two ulps of guard, or with only a zero fraction word taken as ambiguous, the model predicts a wrong cell
+    for some decided lookup of the generated cases: the device test built on them fails under either change."""
+    guard, ambiguous = ((0.0, 0.0), ce.AMBIGUOUS_BELOW) if mutation == "no_guard" else ((ce.GUARD_X, ce.GUARD_Y), 0)
+    wrong = sum(ce.cloud_bands(emap, pts, poses, guard, ambiguous).wrong for emap, pts, poses in map(hair_set, HAIR_MAPS))
+    assert wrong >= 1
 
 
 def bordered_index(px: int, py: int, kx: int) -> int:

@@ -18,6 +18,23 @@ uint64_t finish_rows(uint64_t capacity) {
   return std::max<uint64_t>({resample_scatter_block_count(capacity), resample_block_count(capacity), moments_block_count(capacity)});
 }
 
+/// The CTA ranges of Rows launches over n members, through which their kernels find a CTA's member: ctas(j, c) writes
+/// member j's CTA count in row l to c[l].  Row l (first + l * (n + 1)) receives the exclusive prefix of its counts and
+/// then their total, which totals[l] receives too.
+template <int Rows, class Ctas>
+void write_cta_rows(uint32_t* first, uint32_t n, uint32_t* totals, Ctas ctas) {
+  for (int l = 0; l < Rows; ++l) totals[l] = 0;
+  for (uint32_t j = 0; j < n; ++j) {
+    uint32_t c[Rows];
+    ctas(j, c);
+    for (int l = 0; l < Rows; ++l) {
+      first[static_cast<size_t>(l) * (n + 1) + j] = totals[l];
+      totals[l] += c[l];
+    }
+  }
+  for (int l = 0; l < Rows; ++l) first[static_cast<size_t>(l) * (n + 1) + n] = totals[l];
+}
+
 }  // namespace
 
 int Batch::validate_member(const bb200_amcl_param& p, const bb200_motion_param& motion, int k, int device, uint32_t flags, std::string* error) {
@@ -100,10 +117,8 @@ int Batch::allocate(const Layout& l, size_t slots, Storage* s) {
   BB_CHECK(s->scalars.allocate(slots));
   BB_CHECK(s->tile_state.allocate(l.tiles));
   BB_CHECK(s->partials.allocate(l.rows * kMomentCount));
-  BB_CHECK(s->table.allocate(slots));
-  BB_CHECK(s->table_host.allocate(slots));
-  BB_CHECK(s->first.allocate(kBatchRows * k1));
-  BB_CHECK(s->first_host.allocate(kBatchRows * k1));
+  BB_CHECK(s->table.grow(slots));
+  BB_CHECK(s->first.grow(kBatchRows * k1));
   BB_CHECK(s->summary_host.allocate(slots));
   BB_CHECK(cudaMemsetAsync(s->scalars.get(), 0, slots * sizeof(Scalars), stream_));
   return BB200_OK;
@@ -119,9 +134,7 @@ void Batch::adopt(Storage&& s) {
   tile_state_ = std::move(s.tile_state);
   partials_ = std::move(s.partials);
   table_ = std::move(s.table);
-  table_host_ = std::move(s.table_host);
   first_ = std::move(s.first);
-  first_host_ = std::move(s.first_host);
   summary_host_ = std::move(s.summary_host);
 }
 
@@ -162,7 +175,6 @@ int Batch::relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* l
   Storage s;
   if (const int st = allocate(*layout, slots.size(), &s)) return st;
   std::vector<BatchRelayoutMember> moves;
-  uint32_t ctas = 0;
   for (size_t k = 0; k < members_.size(); ++k) {
     const Member& m = members_[k];
     if (!m.active || slots[k] == nullptr) continue;
@@ -173,25 +185,10 @@ int Batch::relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* l
     r.cdf_n = m.cdf_total != 0 ? m.n : 0;
     r.ancestors_n = m.policy.params().record_ancestors && ancestors_.get() != nullptr ? m.ancestors_n : 0;
     r.cur = m.cur;
-    const uint32_t c = batch_relayout_ctas(r);
-    if (c == 0) continue;
-    s.first_host.get()[moves.size()] = ctas;
-    ctas += c;
-    moves.push_back(r);
+    if (batch_relayout_ctas(r) > 0) moves.push_back(r);
   }
-  DeviceBuffer<BatchRelayoutMember> table;
   if (!moves.empty()) {
-    BB_CHECK(table.allocate(moves.size()));
-    const uint32_t n = static_cast<uint32_t>(moves.size());
-    s.first_host.get()[n] = ctas;
-    // Pageable table: staged before the call returns; the pinned prefixes stay untouched until the synchronisation below.
-    BB_CHECK(cudaMemcpyAsync(table.get(), moves.data(), n * sizeof(BatchRelayoutMember), cudaMemcpyHostToDevice, stream_));
-    BB_CHECK(cudaMemcpyAsync(s.first.get(), s.first_host.get(), (n + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream_));
     BatchRelayoutArgs a{};
-    a.members = table.get();
-    a.first = s.first.get();
-    a.n_members = n;
-    a.ctas = ctas;
     a.states_from[0] = states_[0].get();
     a.states_from[1] = states_[1].get();
     a.weights_from = weights_.get();
@@ -201,9 +198,9 @@ int Batch::relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* l
     a.weights_to = s.weights.get();
     a.cdf_to = s.cdf.get();
     a.ancestors_to = s.ancestors.get();
-    launches_ += static_cast<uint64_t>(launch_batch_relayout(a, stream_));
-    BB_CHECK(cudaGetLastError());
+    if (const int st = launch_moves(moves, a)) return st;
   }
+  // The arrival is one move: it fits the transfer tables the survivors' launch may have grown, so none is freed in flight.
   if (arrival != nullptr)
     if (const int st = unpack({arrival->state}, {layout->offset[arrival->slot]}, s.states[0].get(), s.weights.get(), s.cdf.get(), s.ancestors.get()))
       return st;
@@ -213,30 +210,32 @@ int Batch::relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* l
   adopt(std::move(s));
   for (size_t k = 0; k < members_.size(); ++k)
     if (members_[k].active && slots[k] != nullptr) members_[k].cur = 0;  // the kernel wrote every survivor's states to buffer 0
-  // Scratch allocated on first use and sized by the layout or the slot count: re-created, all or nothing, on next use.
+  // Scratch allocated on first use and sized by the layout or the slot count: re-created on next use.
   cl_ = ClusterBuffers{};
-  kld_ = KldTable{};
+  kld_ = {};
   sel_ = SelectBuffers{};
-  sm_table_ = SampleTable{};
-  sample_header_ = 0;
-  inputs_ = InputTable{};
+  sm_table_ = {};
+  inputs_ = {};
   return BB200_OK;
 }
 
-int Batch::add_member(const bb200_amcl_param& params, const bb200_motion_param& motion, int* member) {
-  error_.clear();
+int Batch::join(const bb200_amcl_param& params, const bb200_motion_param& motion, const FilterState* state, int map, int* member) {
   size_t slot = 0;
   while (slot < members_.size() && members_[slot].active) ++slot;
   if (const int st = validate_member(params, motion, static_cast<int>(slot), device_, flags_, &error_)) return st;
+  if (map != -1 && find_map(map) == nullptr) return BB200_ERR_INVALID_ARGUMENT;
   Member joiner{AmclPolicy(params, motion)};
   joiner.capacity = params.max_particles;
+  if (state != nullptr) adopt_state(joiner, *state);
+  joiner.map = map;
   members_.reserve(members_.size() + 1);  // the host allocations that could fail come before the device work
   std::vector<const bb200_amcl_param*> slots(std::max(members_.size(), slot + 1), nullptr);
   for (size_t k = 0; k < members_.size(); ++k)
     if (members_[k].active) slots[k] = &members_[k].policy.params();
   slots[slot] = &params;
   Layout layout;
-  if (const int st = relayout(slots, &layout)) return st;
+  const Arrival arrival{slot, state};
+  if (const int st = relayout(slots, &layout, state != nullptr ? &arrival : nullptr)) return st;
   if (slot == members_.size()) {
     members_.push_back(std::move(joiner));
   } else {
@@ -245,6 +244,11 @@ int Batch::add_member(const bb200_amcl_param& params, const bb200_motion_param& 
   place(layout);
   *member = static_cast<int>(slot);
   return BB200_OK;
+}
+
+int Batch::add_member(const bb200_amcl_param& params, const bb200_motion_param& motion, int* member) {
+  error_.clear();
+  return join(params, motion, nullptr, -1, member);
 }
 
 namespace {
@@ -290,8 +294,8 @@ void Batch::adopt_state(Member& m, const FilterState& s) {
 
 int Batch::launch_moves(const std::vector<BatchRelayoutMember>& moves, BatchRelayoutArgs a) {
   const uint32_t n = static_cast<uint32_t>(moves.size());
-  std::vector<uint32_t> first(n + 1, 0);
-  for (uint32_t j = 0; j < n; ++j) first[j + 1] = first[j] + batch_relayout_ctas(moves[j]);
+  std::vector<uint32_t> first(n + 1);
+  write_cta_rows<1>(first.data(), n, &a.ctas, [&](uint32_t j, uint32_t* c) { *c = batch_relayout_ctas(moves[j]); });
   BB_CHECK(xfer_.table.grow(n));  // every batch call ends synchronised: nothing in flight reads the old tables
   BB_CHECK(xfer_.first.grow(n + 1));
   // Pageable sources: staged before the calls return.
@@ -300,7 +304,6 @@ int Batch::launch_moves(const std::vector<BatchRelayoutMember>& moves, BatchRela
   a.members = xfer_.table.get();
   a.first = xfer_.first.get();
   a.n_members = n;
-  a.ctas = first[n];
   launches_ += static_cast<uint64_t>(launch_batch_relayout(a, stream_));
   BB_CHECK(cudaGetLastError());
   return BB200_OK;
@@ -330,8 +333,7 @@ int Batch::unpack(const std::vector<const FilterState*>& states, const std::vect
   if (moves.empty()) return BB200_OK;
   const StageLayout l = stage_layout(entries, cdf, ancestors);
   BB_CHECK(xfer_.stage.grow(l.bytes));  // every batch call ends synchronised: the staging buffers are free
-  BB_CHECK(xfer_.stage_host.grow(l.bytes));
-  unsigned char* host = xfer_.stage_host.get();
+  unsigned char* host = xfer_.stage.host.get();
   for (size_t j = 0; j < moves.size(); ++j) {
     const BatchRelayoutMember& r = moves[j];
     const FilterState& s = *moved[j];
@@ -340,8 +342,8 @@ int Batch::unpack(const std::vector<const FilterState*>& states, const std::vect
     if (r.cdf_n > 0) std::memcpy(host + l.cdf + r.from * sizeof(unsigned long long), s.cdf, r.cdf_n * sizeof(unsigned long long));
     if (r.ancestors_n > 0) std::memcpy(host + l.ancestors + r.from * sizeof(long long), s.ancestors, r.ancestors_n * sizeof(long long));
   }
-  unsigned char* stage = xfer_.stage.get();
-  BB_CHECK(cudaMemcpyAsync(stage, host, l.bytes, cudaMemcpyHostToDevice, stream_));
+  unsigned char* stage = xfer_.stage.device.get();
+  BB_CHECK(xfer_.stage.to_device(0, l.bytes, stream_));
   BatchRelayoutArgs a{};
   a.states_from[0] = a.states_from[1] = reinterpret_cast<const Pose2*>(stage + l.states);
   a.weights_from = reinterpret_cast<const double*>(stage + l.weights);
@@ -400,8 +402,7 @@ int Batch::export_members(const uint8_t* present, void* const* out, const uint64
   if (!moves.empty()) {
     BB_CHECK(cudaSetDevice(device_));
     BB_CHECK(xfer_.stage.grow(l.bytes));  // every batch call ends synchronised: the staging buffers are free
-    BB_CHECK(xfer_.stage_host.grow(l.bytes));
-    unsigned char* stage = xfer_.stage.get();
+    unsigned char* stage = xfer_.stage.device.get();
     BatchRelayoutArgs a{};
     a.states_from[0] = states_[0].get();
     a.states_from[1] = states_[1].get();
@@ -413,12 +414,12 @@ int Batch::export_members(const uint8_t* present, void* const* out, const uint64
     a.cdf_to = reinterpret_cast<unsigned long long*>(stage + l.cdf);
     a.ancestors_to = reinterpret_cast<long long*>(stage + l.ancestors);
     if (const int st = launch_moves(moves, a)) return st;
-    BB_CHECK(cudaMemcpyAsync(xfer_.stage_host.get(), stage, l.bytes, cudaMemcpyDeviceToHost, stream_));
+    BB_CHECK(xfer_.stage.to_host(0, l.bytes, stream_));
     BB_CHECK(cudaStreamSynchronize(stream_));
   }
 
   // The blobs, written from pinned memory.
-  const unsigned char* host = xfer_.stage_host.get();
+  const unsigned char* host = xfer_.stage.host.get();
   for (size_t j = 0; j < written.size(); ++j) {
     const uint32_t k = written[j];
     const Member& m = members_[k];
@@ -456,29 +457,7 @@ int Batch::import_member(const void* blob, uint64_t size, int map, int* member) 
   FilterState s;
   if (const int st = read_state_blob(blob, size, &s, &error_)) return st;
   s.params.device = device_;  // the receiver's device
-  size_t slot = 0;
-  while (slot < members_.size() && members_[slot].active) ++slot;
-  if (const int st = validate_member(s.params, s.motion, static_cast<int>(slot), device_, flags_, &error_)) return st;
-  if (map != -1 && find_map(map) == nullptr) return BB200_ERR_INVALID_ARGUMENT;
-  Member joiner{AmclPolicy(s.params, s.motion)};
-  adopt_state(joiner, s);
-  joiner.map = map;
-  members_.reserve(members_.size() + 1);  // the host allocations that could fail come before the device work
-  std::vector<const bb200_amcl_param*> slots(std::max(members_.size(), slot + 1), nullptr);
-  for (size_t k = 0; k < members_.size(); ++k)
-    if (members_[k].active) slots[k] = &members_[k].policy.params();
-  slots[slot] = &s.params;
-  Layout layout;
-  const Arrival arrival{slot, &s};
-  if (const int st = relayout(slots, &layout, &arrival)) return st;
-  if (slot == members_.size()) {
-    members_.push_back(std::move(joiner));
-  } else {
-    members_[slot] = std::move(joiner);
-  }
-  place(layout);
-  *member = static_cast<int>(slot);
-  return BB200_OK;
+  return join(s.params, s.motion, &s, map, member);
 }
 
 int Batch::restore_members(const std::vector<FilterState>& states) {
@@ -816,21 +795,15 @@ int Batch::ensure_cluster_scratch() {
   BB_CHECK(c.sort[1].allocate(total_));
   BB_CHECK(c.starts.allocate(total_ + k));
   BB_CHECK(c.records.allocate(total_));
-  BB_CHECK(c.table.allocate(k));
-  BB_CHECK(c.table_host.allocate(k));
-  BB_CHECK(c.cells.allocate(k));
-  BB_CHECK(c.cells_host.allocate(k));
+  BB_CHECK(c.table.grow(k));
+  BB_CHECK(c.cells.grow(k));
   cl_ = std::move(c);
   return BB200_OK;
 }
 
 int Batch::ensure_kld_scratch() {
   if (const int st = ensure_cluster_scratch()) return st;
-  if (kld_.host.get() != nullptr) return BB200_OK;
-  KldTable t;
-  BB_CHECK(t.device.allocate(members_.size()));
-  BB_CHECK(t.host.allocate(members_.size()));
-  kld_ = std::move(t);
+  BB_CHECK(kld_.grow(members_.size()));
   return BB200_OK;
 }
 
@@ -849,8 +822,7 @@ int Batch::ensure_select_scratch() {
   BB_CHECK(s.schedule_start.allocate(table.start.size()));
   BB_CHECK(s.schedule.allocate(table.steps.size()));
   BB_CHECK(s.scratch.allocate(bytes));
-  BB_CHECK(s.post.allocate(k));
-  BB_CHECK(s.post_host.allocate(k));
+  BB_CHECK(s.post.grow(k));
   BB_CHECK(s.results.allocate(k));
   BB_CHECK(cudaMemcpy(s.schedule_start.get(), table.start.data(), table.start.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
   BB_CHECK(cudaMemcpy(s.schedule.get(), table.steps.data(), table.steps.size() * sizeof(RehashStep), cudaMemcpyHostToDevice));
@@ -865,9 +837,7 @@ int Batch::ensure_cluster_records(uint64_t cells) {
 
 int Batch::cluster_estimates(const bb200_cluster_param& p, const uint8_t* present, bb200_estimate* out, uint32_t* n_cells, uint32_t* n_clusters) {
   error_.clear();
-  if (!(p.linear_hash_resolution > 0.0) || !(p.angular_hash_resolution > 0.0) || !(p.weight_cap_percentile >= 0.0) ||
-      !(p.weight_cap_percentile < 1.0))
-    return fail(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)");
+  if (const char* why = cluster_param_error(p)) return fail(BB200_ERR_INVALID_ARGUMENT, why);
   std::vector<uint32_t> selected;
   if (const int st = select_members(present, &selected)) return st;
   if (selected.empty()) return BB200_OK;
@@ -878,7 +848,7 @@ int Batch::cluster_estimates(const bb200_cluster_param& p, const uint8_t* presen
   for (size_t j = 0; j < selected.size(); ++j) {
     const uint32_t k = selected[j];
     const Member& m = members_[k];
-    const uint32_t count = cl_.cells_host.get()[j];
+    const uint32_t count = cl_.cells.host.get()[j];
     const ClusterSelection sel = select_cluster(cells, count, m.n, p.linear_hash_resolution, p.angular_hash_resolution, p.weight_cap_percentile);
     if (out != nullptr) estimate_from_moments(sel.moments, m.pivot, &out[k]);
     if (n_cells != nullptr) n_cells[k] = count;
@@ -903,24 +873,40 @@ int Batch::cell_records(double linear, double angular, const std::vector<uint32_
   if (const int st = ensure_cluster_scratch()) return st;  // every batch call ends synchronised: the pinned buffers are free
 
   const uint32_t n_sel = static_cast<uint32_t>(selected.size());
-  for (uint32_t j = 0; j < n_sel; ++j) {
-    const uint32_t k = selected[j];
-    const Member& m = members_[k];
-    BatchClusterMember& c = cl_.table_host.get()[j];
-    c = BatchClusterMember{};
-    c.offset = m.offset;
-    c.table_offset = m.table_offset;
-    c.starts_offset = m.offset + k;  // a member's cells + 1 starts end before the next member's slice begins
-    c.n = static_cast<uint32_t>(m.n);
-    c.table_mask = m.table_slots - 1;
-    c.cur = static_cast<uint32_t>(m.cur);
-    c.pivot_x = m.pivot[0];
-    c.pivot_y = m.pivot[1];
-  }
+  for (uint32_t j = 0; j < n_sel; ++j) cl_.table.host.get()[j] = cluster_member(selected[j]);
   cudaStream_t stream = stream_;
-  BB_CHECK(cudaMemcpyAsync(cl_.table.get(), cl_.table_host.get(), n_sel * sizeof(BatchClusterMember), cudaMemcpyHostToDevice, stream));
+  BB_CHECK(cl_.table.to_device(0, n_sel, stream));
+  launch_batch_cluster_cells(cluster_args(linear, angular), n_sel, stream);
+  BB_LAUNCHED("batch_cluster_cells");
+  BB_CHECK(cl_.cells.to_host(0, n_sel, stream));
+  BB_CHECK(cudaStreamSynchronize(stream));  // 1: the cell counts size the records' read-back
+  uint64_t total_cells = 0;
+  for (uint32_t j = 0; j < n_sel; ++j) total_cells += cl_.cells.host.get()[j];
+  if (const int st = ensure_cluster_records(total_cells)) return st;
+  launch_batch_cluster_compact(cl_.table.device.get(), cl_.cells.device.get(), cl_.records.get(), n_sel, cl_records_host_.get(), stream);
+  BB_LAUNCHED("batch_cluster_compact");
+  BB_CHECK(cudaStreamSynchronize(stream));  // 2: every record is in pinned memory
+  static_assert(sizeof(HostCell) == sizeof(CellRecord), "record layouts must agree");
+  return BB200_OK;
+}
+
+BatchClusterMember Batch::cluster_member(uint32_t k) const {
+  const Member& m = members_[k];
+  BatchClusterMember c{};
+  c.offset = m.offset;
+  c.table_offset = m.table_offset;
+  c.starts_offset = m.offset + k;  // a member's cells + 1 starts end before the next member's slice begins
+  c.n = static_cast<uint32_t>(m.n);
+  c.table_mask = m.table_slots - 1;
+  c.cur = static_cast<uint32_t>(m.cur);
+  c.pivot_x = m.pivot[0];
+  c.pivot_y = m.pivot[1];
+  return c;
+}
+
+BatchClusterArgs Batch::cluster_args(double linear, double angular) const {
   BatchClusterArgs a{};
-  a.members = cl_.table.get();
+  a.members = cl_.table.device.get();
   a.states[0] = states_[0].get();
   a.states[1] = states_[1].get();
   a.weights = weights_.get();
@@ -935,19 +921,8 @@ int Batch::cell_records(double linear, double angular, const std::vector<uint32_
   a.sort_b = cl_.sort[1].get();
   a.starts = cl_.starts.get();
   a.records = cl_.records.get();
-  a.cells = cl_.cells.get();
-  launch_batch_cluster_cells(a, n_sel, stream);
-  BB_LAUNCHED("batch_cluster_cells");
-  BB_CHECK(cudaMemcpyAsync(cl_.cells_host.get(), cl_.cells.get(), n_sel * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
-  BB_CHECK(cudaStreamSynchronize(stream));  // 1: the cell counts size the records' read-back
-  uint64_t total_cells = 0;
-  for (uint32_t j = 0; j < n_sel; ++j) total_cells += cl_.cells_host.get()[j];
-  if (const int st = ensure_cluster_records(total_cells)) return st;
-  launch_batch_cluster_compact(cl_.table.get(), cl_.cells.get(), cl_.records.get(), n_sel, cl_records_host_.get(), stream);
-  BB_LAUNCHED("batch_cluster_compact");
-  BB_CHECK(cudaStreamSynchronize(stream));  // 2: every record is in pinned memory
-  static_assert(sizeof(HostCell) == sizeof(CellRecord), "record layouts must agree");
-  return BB200_OK;
+  a.cells = cl_.cells.device.get();
+  return a;
 }
 
 int Batch::particle_histograms(double linear, double angular, const uint8_t* present, bb200_cluster_cell* const* bins, const uint64_t* capacity,
@@ -966,7 +941,7 @@ int Batch::particle_histograms(double linear, double angular, const uint8_t* pre
   bool short_buffer = false;
   for (size_t j = 0; j < selected.size(); ++j) {
     const uint32_t k = selected[j];
-    const uint32_t count = cl_.cells_host.get()[j];
+    const uint32_t count = cl_.cells.host.get()[j];
     double top = 1e-3;  // beluga_ros/particle_cloud.hpp:197
     for (uint32_t c = 0; c < count; ++c) top = cells[c].weight > top ? cells[c].weight : top;
     if (n_bins != nullptr) n_bins[k] = count;
@@ -981,21 +956,6 @@ int Batch::particle_histograms(double linear, double angular, const uint8_t* pre
     cells += count;
   }
   if (short_buffer) return fail(BB200_ERR_CAPACITY, "histogram bin buffer too small for some member (n_bins has the counts)");
-  return BB200_OK;
-}
-
-int Batch::ensure_samples(uint64_t draws) {
-  if (sm_table_.host.get() == nullptr) {
-    const size_t k = members_.size();
-    sample_header_ = (k * sizeof(unsigned long long) + sizeof(Pose2) - 1) / sizeof(Pose2);
-    SampleTable t;
-    BB_CHECK(t.device.allocate(k));
-    BB_CHECK(t.host.allocate(k));
-    sm_table_ = std::move(t);
-  }
-  const uint64_t want = std::min<uint64_t>(total_, std::max<uint64_t>(4096, 2 * draws));  // draws <= total_
-  BB_CHECK(samples_.grow(sample_header_ + draws, sample_header_ + want));
-  BB_CHECK(samples_host_.grow(sample_header_ + draws, sample_header_ + want));
   return BB200_OK;
 }
 
@@ -1018,7 +978,11 @@ int Batch::sample_states(const uint64_t* counts, uint32_t step, const uint8_t* p
   }
   if (drawn.empty()) return BB200_OK;
   BB_CHECK(cudaSetDevice(device_));
-  if (const int st = ensure_samples(draws)) return st;  // every batch call ends synchronised: the pinned buffers are free
+  // Every batch call ends synchronised: the pinned buffers are free.  The draws follow one CDF total per member.
+  const uint64_t header = (members_.size() * sizeof(unsigned long long) + sizeof(Pose2) - 1) / sizeof(Pose2);
+  const uint64_t want = std::min<uint64_t>(total_, std::max<uint64_t>(4096, 2 * draws));  // draws <= total_
+  BB_CHECK(sm_table_.grow(members_.size()));
+  BB_CHECK(samples_.grow(header + draws, header + want));
 
   const uint32_t n_sel = static_cast<uint32_t>(drawn.size());
   BatchSampleArgs a{};
@@ -1038,19 +1002,17 @@ int Batch::sample_states(const uint64_t* counts, uint32_t step, const uint8_t* p
     s.cur = m.cur;
     s.ceil_log2_count = ceil_log2_count(m.capacity);
     out_offset += s.count;
-    uint32_t ctas[kSampleLaunches];
-    batch_sample_ctas(s, s.total == 0, ctas);
-    for (int l = 0; l < kSampleLaunches; ++l) {
-      first_host_.get()[static_cast<size_t>(l) * (n_sel + 1) + j] = a.ctas[l];  // the step's range buffers are free between calls
-      a.ctas[l] += ctas[l];
-    }
   }
-  for (int l = 0; l < kSampleLaunches; ++l) first_host_.get()[static_cast<size_t>(l) * (n_sel + 1) + n_sel] = a.ctas[l];
+  // The step's range buffers are free between calls.
+  write_cta_rows<kSampleLaunches>(first_.host.get(), n_sel, a.ctas, [&](uint32_t j, uint32_t* c) {
+    const BatchSampleMember& s = sm_table_.host.get()[j];
+    batch_sample_ctas(s, s.total == 0, c);
+  });
   cudaStream_t stream = stream_;
-  BB_CHECK(cudaMemcpyAsync(sm_table_.device.get(), sm_table_.host.get(), n_sel * sizeof(BatchSampleMember), cudaMemcpyHostToDevice, stream));
-  BB_CHECK(cudaMemcpyAsync(first_.get(), first_host_.get(), kSampleLaunches * (n_sel + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+  BB_CHECK(sm_table_.to_device(0, n_sel, stream));
+  BB_CHECK(first_.to_device(0, kSampleLaunches * (n_sel + 1), stream));
   a.members = sm_table_.device.get();
-  a.first = first_.get();
+  a.first = first_.device.get();
   a.step = step;
   a.states[0] = states_[0].get();
   a.states[1] = states_[1].get();
@@ -1059,34 +1021,20 @@ int Batch::sample_states(const uint64_t* counts, uint32_t step, const uint8_t* p
   a.scalars = scalars_.get();
   a.tile_state = tile_state_.get();
   a.partials = partials_.get();  // the step's moment rows are free between calls
-  a.totals = reinterpret_cast<unsigned long long*>(samples_.get());
-  a.out = samples_.get() + sample_header_;
+  a.totals = reinterpret_cast<unsigned long long*>(samples_.device.get());
+  a.out = samples_.device.get() + header;
   launches_ += static_cast<uint64_t>(launch_batch_sample(a, stream));
   BB_CHECK(cudaGetLastError());
-  BB_CHECK(cudaMemcpyAsync(samples_host_.get(), samples_.get(), (sample_header_ + draws) * sizeof(Pose2), cudaMemcpyDeviceToHost, stream));
+  BB_CHECK(samples_.to_host(0, header + draws, stream));
   BB_CHECK(cudaStreamSynchronize(stream));
 
-  const unsigned long long* totals = reinterpret_cast<const unsigned long long*>(samples_host_.get());
-  const Pose2* out = samples_host_.get() + sample_header_;
+  const unsigned long long* totals = reinterpret_cast<const unsigned long long*>(samples_.host.get());
+  const Pose2* out = samples_.host.get() + header;
   for (uint32_t j = 0; j < n_sel; ++j) {
     const BatchSampleMember& s = sm_table_.host.get()[j];
     members_[drawn[j]].cdf_total = totals[j];  // a rebuilt CDF is current until the member's particles or weights change
     std::memcpy(states_out[drawn[j]], out + s.out_offset, s.count * sizeof(Pose2));
   }
-  return BB200_OK;
-}
-
-int Batch::ensure_rays(size_t members, uint64_t doubles) {
-  const RayBuffers& r = rays_;
-  if (members <= std::min(r.table.size(), r.table_host.size()) && doubles <= std::min(r.data.size(), r.data_host.size())) return BB200_OK;
-  // Every batch call ends synchronised: nothing in flight reads the old buffers.
-  RayBuffers t;
-  const uint64_t room = std::max<uint64_t>(doubles + doubles / 2, 4096);
-  BB_CHECK(t.table.allocate(members_.size()));
-  BB_CHECK(t.table_host.allocate(members_.size()));
-  BB_CHECK(t.data.allocate(room));
-  BB_CHECK(t.data_host.allocate(room));
-  rays_ = std::move(t);
   return BB200_OK;
 }
 
@@ -1127,14 +1075,17 @@ int Batch::cast_rays(const uint8_t* present, const int* map_ids, const double* c
   if (casts.empty()) return BB200_OK;
   BB_CHECK(cudaSetDevice(device_));
   const uint32_t n_sel = static_cast<uint32_t>(casts.size());
-  if (const int st = ensure_rays(n_sel, pose_doubles + bearing_doubles + total_rays)) return st;
-  double* staged = rays_.data_host.get();
+  // Every batch call ends synchronised: nothing in flight reads the old buffers.
+  const uint64_t doubles = pose_doubles + bearing_doubles + total_rays;
+  BB_CHECK(rays_.table.grow(n_sel, members_.size()));
+  BB_CHECK(rays_.data.grow(doubles, std::max<uint64_t>(doubles + doubles / 2, 4096)));
+  double* staged = rays_.data.host.get();
   uint64_t pose_offset = 0, bearing_offset = 0, ray_offset = 0;
   BatchRayArgs a{};
   a.n_members = n_sel;
   for (uint32_t j = 0; j < n_sel; ++j) {
     const size_t k = casts[j].k;
-    BatchRayMember& r = rays_.table_host.get()[j];
+    BatchRayMember& r = rays_.table.host.get()[j];
     r = BatchRayMember{};
     if (const int st = casts[j].map->ray_view(stream_, &r.grid, &error_)) return st;  // a likelihood-field map's first cast uploads its table
     r.pose_offset = pose_offset;
@@ -1148,47 +1099,28 @@ int Batch::cast_rays(const uint8_t* present, const int* map_ids, const double* c
     pose_offset += n_poses[k];
     bearing_offset += n_bearings[k];
     ray_offset += r.n_rays;
-    first_host_.get()[j] = a.ctas;  // the step's range buffers are free between calls
-    a.ctas += cast_rays_ctas(r.n_rays);
   }
-  first_host_.get()[n_sel] = a.ctas;
+  // The step's range buffers are free between calls.
+  write_cta_rows<1>(first_.host.get(), n_sel, &a.ctas, [&](uint32_t j, uint32_t* c) { *c = cast_rays_ctas(rays_.table.host.get()[j].n_rays); });
   cudaStream_t stream = stream_;
-  double* d = rays_.data.get();
-  BB_CHECK(cudaMemcpyAsync(d, staged, (pose_doubles + bearing_doubles) * sizeof(double), cudaMemcpyHostToDevice, stream));
-  BB_CHECK(cudaMemcpyAsync(rays_.table.get(), rays_.table_host.get(), n_sel * sizeof(BatchRayMember), cudaMemcpyHostToDevice, stream));
-  BB_CHECK(cudaMemcpyAsync(first_.get(), first_host_.get(), (n_sel + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-  a.members = rays_.table.get();
-  a.first = first_.get();
+  double* d = rays_.data.device.get();
+  BB_CHECK(rays_.data.to_device(0, pose_doubles + bearing_doubles, stream));
+  BB_CHECK(rays_.table.to_device(0, n_sel, stream));
+  BB_CHECK(first_.to_device(0, n_sel + 1, stream));
+  a.members = rays_.table.device.get();
+  a.first = first_.device.get();
   a.poses = reinterpret_cast<const Pose2*>(d);
   a.bearings = reinterpret_cast<const double2*>(d + pose_doubles);
   a.ranges = d + pose_doubles + bearing_doubles;
   launches_ += static_cast<uint64_t>(launch_batch_cast_rays(a, stream));
   BB_CHECK(cudaGetLastError());
-  double* out = staged + pose_doubles + bearing_doubles;
-  BB_CHECK(cudaMemcpyAsync(out, a.ranges, total_rays * sizeof(double), cudaMemcpyDeviceToHost, stream));
+  BB_CHECK(rays_.data.to_host(pose_doubles + bearing_doubles, total_rays, stream));
   BB_CHECK(cudaStreamSynchronize(stream));
+  const double* out = staged + pose_doubles + bearing_doubles;
   for (uint32_t j = 0; j < n_sel; ++j) {
-    const BatchRayMember& r = rays_.table_host.get()[j];
+    const BatchRayMember& r = rays_.table.host.get()[j];
     std::memcpy(ranges[casts[j].k], out + r.ray_offset, r.n_rays * sizeof(double));
   }
-  return BB200_OK;
-}
-
-int Batch::ensure_points(uint64_t n_points) {
-  if (2 * n_points <= std::min(points_.size(), points_host_.size())) return BB200_OK;
-  BB_CHECK(cudaStreamSynchronize(stream_));
-  const uint64_t room = 2 * std::max<uint64_t>(n_points + n_points / 2, 4096);
-  BB_CHECK(points_.grow(2 * n_points, room));
-  BB_CHECK(points_host_.grow(2 * n_points, room));
-  return BB200_OK;
-}
-
-int Batch::ensure_detections(uint64_t n) {
-  if (n <= std::min(detections_.size(), detections_host_.size())) return BB200_OK;
-  BB_CHECK(cudaStreamSynchronize(stream_));
-  const uint64_t room = std::max<uint64_t>(n + n / 2, 256);
-  BB_CHECK(detections_.grow(n, room));
-  BB_CHECK(detections_host_.grow(n, room));
   return BB200_OK;
 }
 
@@ -1219,20 +1151,6 @@ bool Batch::ensure_hits(uint64_t words) {
     return false;
   }
   return true;
-}
-
-int Batch::ensure_inputs(uint64_t floats) {
-  if (inputs_.host.get() == nullptr) {
-    InputTable t;
-    BB_CHECK(t.device.allocate(members_.size()));
-    BB_CHECK(t.host.allocate(members_.size()));
-    inputs_ = std::move(t);
-  }
-  // Every batch call ends synchronised: nothing in flight reads the old buffers.
-  const uint64_t room = std::max<uint64_t>(floats + floats / 2, 4096);
-  BB_CHECK(input_.grow(floats, room));
-  BB_CHECK(input_host_.grow(floats, room));
-  return BB200_OK;
 }
 
 int Batch::ensure_scan_table(Member& m, const bb200_laser_scan& scan) {
@@ -1306,6 +1224,16 @@ void pack_cloud(const bb200_point_cloud& c, float* out) {
 
 }  // namespace
 
+int Batch::check_measurements(const bb200_measurement* in, const uint8_t* present, bool weighed_by_caller) {
+  if (const int st = check_present(present)) return st;
+  for (size_t k = 0; k < members_.size(); ++k) {
+    if (!selected_member(present, k) || (weighed_by_caller && in[k].kind == BB200_MEASUREMENT_WEIGHTS)) continue;
+    const std::string why = measurement_error(in[k]);
+    if (!why.empty()) return fail(BB200_ERR_INVALID_ARGUMENT, "member " + std::to_string(k) + ": " + why);
+  }
+  return BB200_OK;
+}
+
 int Batch::update(const double* control_poses, const double* const* points_xy, const uint64_t* n_points, const uint8_t* present,
                   bb200_update_result* out) {
   std::vector<bb200_measurement> in(members_.size());
@@ -1318,12 +1246,7 @@ int Batch::update_measurements(const double* control_poses, const bb200_measurem
                                bb200_update_result* out) {
   error_.clear();
   for (size_t k = 0; k < members_.size(); ++k) out[k] = bb200_update_result{};
-  if (const int st = check_present(present)) return st;
-  for (size_t k = 0; k < members_.size(); ++k) {
-    if (!selected_member(present, k)) continue;
-    const std::string why = measurement_error(measurements[k]);
-    if (!why.empty()) return fail(BB200_ERR_INVALID_ARGUMENT, "member " + std::to_string(k) + ": " + why);
-  }
+  if (const int st = check_measurements(measurements, present, false)) return st;
   return step(control_poses, measurements, present, out);
 }
 
@@ -1331,15 +1254,8 @@ int Batch::update_clustered(const double* control_poses, const bb200_measurement
                             bb200_update_result* out, bb200_estimate* clustered, uint32_t* n_cells, uint32_t* n_clusters) {
   error_.clear();
   for (size_t k = 0; k < members_.size(); ++k) out[k] = bb200_update_result{};
-  if (!(p.linear_hash_resolution > 0.0) || !(p.angular_hash_resolution > 0.0) || !(p.weight_cap_percentile >= 0.0) ||
-      !(p.weight_cap_percentile < 1.0))
-    return fail(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)");
-  if (const int st = check_present(present)) return st;
-  for (size_t k = 0; k < members_.size(); ++k) {
-    if (!selected_member(present, k)) continue;
-    const std::string why = measurement_error(measurements[k]);
-    if (!why.empty()) return fail(BB200_ERR_INVALID_ARGUMENT, "member " + std::to_string(k) + ": " + why);
-  }
+  if (const char* why = cluster_param_error(p)) return fail(BB200_ERR_INVALID_ARGUMENT, why);
+  if (const int st = check_measurements(measurements, present, false)) return st;
   const ClusteredOut co{&p, clustered, n_cells, n_clusters};
   return step(control_poses, measurements, present, out, &co);
 }
@@ -1354,12 +1270,7 @@ int Batch::step(const double* control_poses, const bb200_measurement* in, const 
 int Batch::update_begin(const double* control_poses, const bb200_measurement* measurements, const uint8_t* present, bb200_weigh_view* views) {
   error_.clear();
   if (open_.open) return fail(BB200_ERR_STATE, "a weighed step is already open (bb200_amcl_batch_update_end closes it)");
-  if (const int st = check_present(present)) return st;
-  for (size_t k = 0; k < members_.size(); ++k) {
-    if (!selected_member(present, k) || measurements[k].kind == BB200_MEASUREMENT_WEIGHTS) continue;
-    const std::string why = measurement_error(measurements[k]);
-    if (!why.empty()) return fail(BB200_ERR_INVALID_ARGUMENT, "member " + std::to_string(k) + ": " + why);
-  }
+  if (const int st = check_measurements(measurements, present, true)) return st;
   return step_begin(control_poses, measurements, present, views);
 }
 
@@ -1367,10 +1278,8 @@ int Batch::update_end(const bb200_cluster_param* cluster, bb200_update_result* o
   error_.clear();
   for (size_t k = 0; k < members_.size(); ++k) out[k] = bb200_update_result{};
   if (!open_.open) return fail(BB200_ERR_STATE, "no weighed step is open (bb200_amcl_batch_update_begin)");
-  if (cluster != nullptr && (!(cluster->linear_hash_resolution > 0.0) || !(cluster->angular_hash_resolution > 0.0) ||
-                             !(cluster->weight_cap_percentile >= 0.0) || !(cluster->weight_cap_percentile < 1.0))) {
-    return fail(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)");
-  }
+  if (cluster != nullptr)
+    if (const char* why = cluster_param_error(*cluster)) return fail(BB200_ERR_INVALID_ARGUMENT, why);
   const ClusteredOut co{cluster, clustered, n_cells, n_clusters};
   return step_end(cluster != nullptr ? &co : nullptr, out);
 }
@@ -1466,11 +1375,18 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
   // on_effective_size_drop: a selective member whose every_n fired resamples only when its effective sample size drops
   // below n / 2, decided on the device (batch_ess_kernel).
   const bool ess = std::any_of(active.begin(), active.end(), [&](uint32_t k) { return plans[k].needs_ess != 0; });
+  // The staging buffers grow with room to spare, points and detections once the stream has drained.
+  const uint64_t point_room = 2 * std::max<uint64_t>(points_total + points_total / 2, 4096);
+  const uint64_t detection_room = std::max<uint64_t>(detections_total + detections_total / 2, 256);
+  const uint64_t input_room = std::max<uint64_t>(input_floats + input_floats / 2, 4096);
   int st = check(cudaSetDevice(device_), "cudaSetDevice");
-  if (st == BB200_OK) st = ensure_points(points_total);  // the previous step has ended: the staging buffers are free
-  if (st == BB200_OK && detections_total > 0) st = ensure_detections(detections_total);
+  if (st == BB200_OK && 2 * points_total > points_.size()) st = check(cudaStreamSynchronize(stream_), "cudaStreamSynchronize");
+  if (st == BB200_OK) st = check(points_.grow(2 * points_total, point_room), "point staging");
+  if (st == BB200_OK && detections_total > detections_.size()) st = check(cudaStreamSynchronize(stream_), "cudaStreamSynchronize");
+  if (st == BB200_OK) st = check(detections_.grow(detections_total, detection_room), "detection staging");
   if (st == BB200_OK && step_map == -1) st = ensure_map_table();
-  if (st == BB200_OK && convert) st = ensure_inputs(input_floats);
+  if (st == BB200_OK && convert) st = check(inputs_.grow(count), "measurement table");
+  if (st == BB200_OK && convert) st = check(input_.grow(input_floats, input_room), "measurement staging");
   if (st == BB200_OK && kld) st = ensure_kld_scratch();
   if (st == BB200_OK && any_weighed) st = check(factors_.grow(weights_.size()), "factor buffer");  // laid out like the weights
   for (auto k = active.begin(); st == BB200_OK && k != active.end(); ++k)
@@ -1489,7 +1405,7 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
     const bb200_step_plan& plan = plans[k];
     const bb200_measurement& meas = in[k];
     const uint64_t bound = measurement_bound(meas);
-    BatchMember& b = table_host_.get()[j];
+    BatchMember& b = table_.host.get()[j];
     b = BatchMember{};
     b.offset = m.offset;
     b.n = m.n;
@@ -1523,7 +1439,7 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
     } else if (meas.kind == BB200_MEASUREMENT_LANDMARKS) {
       // No points: point_offset and n_points index the step's prepared detections instead.
       prepare_detections(maps_.at(m.map).map.landmark_slices, m.detections.data(), m.detections.size(), &prepared);
-      if (!prepared.empty()) std::memcpy(detections_host_.get() + detection_offset, prepared.data(), prepared.size() * sizeof(LandmarkDetection));
+      if (!prepared.empty()) std::memcpy(detections_.host.get() + detection_offset, prepared.data(), prepared.size() * sizeof(LandmarkDetection));
       b.point_offset = detection_offset;
       b.n_points = static_cast<uint32_t>(prepared.size());
       b.points_radius = 0.0;
@@ -1532,7 +1448,7 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
       b.point_offset = point_offset;
       b.n_points = static_cast<uint32_t>(meas.n_points);
       b.points_radius = scan_radius(meas.points_xy, meas.n_points);
-      if (meas.n_points > 0) std::memcpy(points_host_.get() + 2 * point_offset, meas.points_xy, 2 * meas.n_points * sizeof(double));
+      if (meas.n_points > 0) std::memcpy(points_.host.get() + 2 * point_offset, meas.points_xy, 2 * meas.n_points * sizeof(double));
       point_offset += meas.n_points;
     } else {
       b.point_offset = device_offset;
@@ -1546,7 +1462,7 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
       d.kind = meas.kind;  // points and weighed members have no CTA there
       d.input_offset = input_offset;
       d.count = static_cast<uint32_t>(bound);
-      float* raw = input_host_.get() + input_offset;
+      float* raw = input_.host.get() + input_offset;
       if (meas.kind == BB200_MEASUREMENT_SCAN) {
         const bb200_laser_scan& scan = *meas.scan;
         const std::vector<uint64_t>& indices = m.scan.indices;
@@ -1579,94 +1495,53 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
     for (const uint32_t k : active)
       if (forms[k] == kBatchBeamTwoPass) forms[k] = kBatchBeamFused;
   // The CTA ranges of every row: each member in the reweight row of its form.
-  for (uint32_t j = 0; j < n_active; ++j) {
-    const int form = forms[active[j]];
-    a.forms |= 1 << form;
-    uint32_t ctas[kBatchLaunches];
-    batch_member_ctas(table_host_.get()[j], form, ctas);
-    for (int l = 0; l < kBatchLaunches; ++l) {
-      first_host_.get()[static_cast<size_t>(l) * (n_active + 1) + j] = a.ctas[l];
-      a.ctas[l] += ctas[l];
-    }
-  }
-  for (int l = 0; l < kBatchLaunches; ++l) first_host_.get()[static_cast<size_t>(l) * (n_active + 1) + n_active] = a.ctas[l];
+  auto row = [&](int l) { return first_.host.get() + static_cast<size_t>(l) * (n_active + 1); };
+  for (const uint32_t k : active) a.forms |= 1 << forms[k];
+  write_cta_rows<kBatchLaunches>(row(0), n_active, a.ctas,
+                                 [&](uint32_t j, uint32_t* c) { batch_member_ctas(table_.host.get()[j], forms[active[j]], c); });
   BatchPointsArgs pa{};
-  if (convert) {
-    uint32_t* row = first_host_.get() + static_cast<size_t>(kBatchPointsRow) * (n_active + 1);
-    for (uint32_t j = 0; j < n_active; ++j) {
-      row[j] = pa.ctas;
-      pa.ctas += batch_points_ctas(inputs_.host.get()[j]);
-    }
-    row[n_active] = pa.ctas;
-  }
+  if (convert) write_cta_rows<1>(row(kBatchPointsRow), n_active, &pa.ctas, [&](uint32_t j, uint32_t* c) { *c = batch_points_ctas(inputs_.host.get()[j]); });
   if (kld || ess) {
-    uint32_t* post_rows[3] = {first_host_.get() + static_cast<size_t>(kBatchKldRow) * (n_active + 1),
-                              first_host_.get() + static_cast<size_t>(kBatchMomentsRow) * (n_active + 1),
-                              first_host_.get() + static_cast<size_t>(kBatchEssRow) * (n_active + 1)};
-    uint32_t totals[3] = {0, 0, 0};
-    for (uint32_t j = 0; j < n_active; ++j) {
-      uint32_t ctas[3];
-      batch_post_ctas(table_host_.get()[j], ctas);
-      for (int l = 0; l < 3; ++l) {
-        post_rows[l][j] = totals[l];
-        totals[l] += ctas[l];
-      }
-    }
-    for (int l = 0; l < 3; ++l) post_rows[l][n_active] = totals[l];
+    static_assert(kBatchMomentsRow == kBatchKldRow + 1 && kBatchEssRow == kBatchKldRow + 2, "batch_post_ctas fills three adjacent rows");
+    uint32_t totals[3];
+    write_cta_rows<3>(row(kBatchKldRow), n_active, totals, [&](uint32_t j, uint32_t* c) { batch_post_ctas(table_.host.get()[j], c); });
     a.post_ctas[0] = totals[0];
     a.post_ctas[1] = totals[1];
     a.ess_ctas = totals[2];
   }
   const bool any_landmark = std::any_of(active.begin(), active.end(), [&](uint32_t k) { return forms[k] == kBatchLandmark; });
-  if (any_landmark) {
-    uint32_t* row = first_host_.get() + static_cast<size_t>(kBatchLandmarkRow) * (n_active + 1);
-    for (uint32_t j = 0; j < n_active; ++j) {
-      row[j] = a.landmark_ctas;
-      if (forms[active[j]] == kBatchLandmark) a.landmark_ctas += batch_landmark_ctas(table_host_.get()[j]);
-    }
-    row[n_active] = a.landmark_ctas;
-  }
-  if (any_weighed) {
-    uint32_t* row = first_host_.get() + static_cast<size_t>(kBatchWeighRow) * (n_active + 1);
-    for (uint32_t j = 0; j < n_active; ++j) {
-      row[j] = a.weigh_ctas;
-      if (weighed(active[j])) a.weigh_ctas += batch_weigh_ctas(table_host_.get()[j]);
-    }
-    row[n_active] = a.weigh_ctas;
-  }
+  if (any_landmark)
+    write_cta_rows<1>(row(kBatchLandmarkRow), n_active, &a.landmark_ctas, [&](uint32_t j, uint32_t* c) {
+      *c = forms[active[j]] == kBatchLandmark ? batch_landmark_ctas(table_.host.get()[j]) : 0;
+    });
+  if (any_weighed)
+    write_cta_rows<1>(row(kBatchWeighRow), n_active, &a.weigh_ctas,
+                      [&](uint32_t j, uint32_t* c) { *c = weighed(active[j]) ? batch_weigh_ctas(table_.host.get()[j]) : 0; });
   const int rows = any_landmark ? kBatchRows : kld || ess || any_weighed ? kBatchLandmarkRow : convert ? kBatchLaunches + 1 : kBatchLaunches;
 
   cudaStream_t stream = stream_;
   for (const uint32_t k : active) members_[k].cdf_total = 0;  // from here on the step may have rewritten their CDFs
   seq_ = seq_ == 0x7fffffff ? 1 : seq_ + 1;
   *ticket_host_.get() = 0;
-  st = check(cudaMemcpyAsync(table_.get(), table_host_.get(), n_active * sizeof(BatchMember), cudaMemcpyHostToDevice, stream), "upload member table");
-  if (st == BB200_OK)
-    st = check(cudaMemcpyAsync(first_.get(), first_host_.get(), rows * (n_active + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), "upload ranges");
-  if (st == BB200_OK && host_points > 0)
-    st = check(cudaMemcpyAsync(points_.get(), points_host_.get(), 2 * host_points * sizeof(double), cudaMemcpyHostToDevice, stream), "upload points");
-  if (st == BB200_OK && convert)
-    st = check(cudaMemcpyAsync(inputs_.device.get(), inputs_.host.get(), n_active * sizeof(BatchPointsMember), cudaMemcpyHostToDevice, stream),
-               "upload measurement table");
-  if (st == BB200_OK && detection_offset > 0)
-    st = check(cudaMemcpyAsync(detections_.get(), detections_host_.get(), detection_offset * sizeof(LandmarkDetection), cudaMemcpyHostToDevice, stream),
-               "upload detections");
-  if (st == BB200_OK && input_floats > 0)
-    st = check(cudaMemcpyAsync(input_.get(), input_host_.get(), input_floats * sizeof(float), cudaMemcpyHostToDevice, stream), "upload measurements");
-  if (st == BB200_OK && kld)
-    st = check(cudaMemcpyAsync(kld_.device.get(), kld_.host.get(), n_active * sizeof(BatchKldMember), cudaMemcpyHostToDevice, stream), "upload KLD table");
+  st = check(table_.to_device(0, n_active, stream), "upload member table");
+  if (st == BB200_OK) st = check(first_.to_device(0, rows * (n_active + 1), stream), "upload ranges");
+  if (st == BB200_OK && host_points > 0) st = check(points_.to_device(0, 2 * host_points, stream), "upload points");
+  if (st == BB200_OK && convert) st = check(inputs_.to_device(0, n_active, stream), "upload measurement table");
+  if (st == BB200_OK && detection_offset > 0) st = check(detections_.to_device(0, detection_offset, stream), "upload detections");
+  if (st == BB200_OK && input_floats > 0) st = check(input_.to_device(0, input_floats, stream), "upload measurements");
+  if (st == BB200_OK && kld) st = check(kld_.to_device(0, n_active, stream), "upload KLD table");
   if (st != BB200_OK) return rollback(st);
   if (convert) {
-    pa.members = table_.get();
-    pa.first = first_.get() + static_cast<size_t>(kBatchPointsRow) * (n_active + 1);
+    pa.members = table_.device.get();
+    pa.first = first_.device.get() + static_cast<size_t>(kBatchPointsRow) * (n_active + 1);
     pa.n_members = n_active;
     pa.inputs = inputs_.device.get();
-    pa.input = input_.get();
-    pa.points = points_.get();
+    pa.input = input_.device.get();
+    pa.points = points_.device.get();
     launches_ += static_cast<uint64_t>(launch_batch_points(pa, stream));
   }
-  a.members = table_.get();
-  a.first = first_.get();
+  a.members = table_.device.get();
+  a.first = first_.device.get();
   a.max_points = max_points;
   a.states[0] = states_[0].get();
   a.states[1] = states_[1].get();
@@ -1676,7 +1551,7 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
   a.tile_state = tile_state_.get();
   a.scalars = scalars_.get();
   a.partials = partials_.get();
-  a.points = points_.get();
+  a.points = points_.device.get();
   if (step_map >= 0) {
     const DeviceMap& map = maps_.at(step_map).map;
     a.field = map.field;
@@ -1706,7 +1581,7 @@ int Batch::step_begin(const double* control_poses, const bb200_measurement* in, 
   a.ticket = ticket_host_.get();
   a.seq = seq_;
   a.factors = factors_.get();
-  a.detections = detections_.get();
+  a.detections = detections_.device.get();
   a.landmark_maps = landmark_maps ? 1 : 0;
   launches_ += static_cast<uint64_t>(launch_batch_step_head(a, stream));
   st = check(cudaGetLastError(), "batch step launch");
@@ -1756,17 +1631,8 @@ int Batch::step_end(const ClusteredOut* clustered, bb200_update_result* out) {
       const uint32_t k = active[j];
       const Member& m = members_[k];
       const bb200_step_plan& plan = plans[k];
-      BatchClusterMember& c = cl_.table_host.get()[j];
-      c = BatchClusterMember{};
-      c.offset = m.offset;
-      c.table_offset = m.table_offset;
-      c.starts_offset = m.offset + k;
-      c.n = static_cast<uint32_t>(m.n);
-      c.table_mask = m.table_slots - 1;
-      c.cur = static_cast<uint32_t>(m.cur);
-      c.pivot_x = m.pivot[0];
-      c.pivot_y = m.pivot[1];
-      BatchClusterPost& q = sel_.post_host.get()[j];
+      cl_.table.host.get()[j] = cluster_member(k);
+      BatchClusterPost& q = sel_.post.host.get()[j];
       q = BatchClusterPost{};
       q.scratch_offset = sel_.offsets[k];
       q.capacity = static_cast<uint32_t>(m.capacity);
@@ -1775,12 +1641,8 @@ int Batch::step_end(const ClusteredOut* clustered, bb200_update_result* out) {
     }
   }
 
-  if (st == BB200_OK && clustered != nullptr)
-    st = check(cudaMemcpyAsync(cl_.table.get(), cl_.table_host.get(), n_active * sizeof(BatchClusterMember), cudaMemcpyHostToDevice, stream),
-               "upload cluster table");
-  if (st == BB200_OK && clustered != nullptr)
-    st = check(cudaMemcpyAsync(sel_.post.get(), sel_.post_host.get(), n_active * sizeof(BatchClusterPost), cudaMemcpyHostToDevice, stream),
-               "upload cluster steps");
+  if (st == BB200_OK && clustered != nullptr) st = check(cl_.table.to_device(0, n_active, stream), "upload cluster table");
+  if (st == BB200_OK && clustered != nullptr) st = check(sel_.post.to_device(0, n_active, stream), "upload cluster steps");
   if (st != BB200_OK) return rollback(st);
   launches_ += static_cast<uint64_t>(launch_batch_step_tail(a, stream));
   st = check(cudaGetLastError(), "batch step launch");
@@ -1789,12 +1651,12 @@ int Batch::step_end(const ClusteredOut* clustered, bb200_update_result* out) {
   if (cp != nullptr) {
     // After the step's last kernel: the post-step cluster table, the cells of every updated member, their selection.
     BatchSelectArgs sa{};
-    sa.members = cl_.table.get();
-    sa.post = sel_.post.get();
+    sa.members = cl_.table.device.get();
+    sa.post = sel_.post.device.get();
     sa.summary = summary_host_.get();
     sa.n_members = n_active;
     sa.records = cl_.records.get();
-    sa.cells = cl_.cells.get();
+    sa.cells = cl_.cells.device.get();
     sa.keys = cl_.keys.get();
     sa.ids = cl_.ids.get();
     sa.schedule_start = sel_.schedule_start.get();
@@ -1810,24 +1672,7 @@ int Batch::step_end(const ClusteredOut* clustered, bb200_update_result* out) {
     for (int s = 0; s < 6; ++s) sa.adjacent[s] = adjacent[s];
     sa.results = sel_.results.get();
     launch_batch_cluster_table(sa, stream);
-    BatchClusterArgs ca{};
-    ca.members = cl_.table.get();
-    ca.states[0] = states_[0].get();
-    ca.states[1] = states_[1].get();
-    ca.weights = weights_.get();
-    ca.linear = sa.linear;
-    ca.angular = sa.angular;
-    ca.hashes = cl_.hashes.get();
-    ca.keys = cl_.keys.get();
-    ca.first = cl_.first.get();
-    ca.ids = cl_.ids.get();
-    ca.cell_of = cl_.cell_of.get();
-    ca.sort_a = cl_.sort[0].get();
-    ca.sort_b = cl_.sort[1].get();
-    ca.starts = cl_.starts.get();
-    ca.records = cl_.records.get();
-    ca.cells = cl_.cells.get();
-    launch_batch_cluster_cells(ca, n_active, stream);
+    launch_batch_cluster_cells(cluster_args(sa.linear, sa.angular), n_active, stream);
     launch_batch_cluster_select(sa, stream);
     launches_ += 3;
     st = check(cudaGetLastError(), "batch cluster selection launch");
@@ -1863,7 +1708,7 @@ int Batch::step_end(const ClusteredOut* clustered, bb200_update_result* out) {
     pivot_to_estimate(r.estimate, o.pivot);
     const bool resampled = plan.needs_ess ? s.resampled != 0 : plan.resample != 0;  // the device's decision for a selective member
     o.cur = resampled ? m.cur ^ 1 : m.cur;
-    o.n = resampled ? (table_host_.get()[j].kld ? s.accepted : m.capacity) : m.n;
+    o.n = resampled ? (table_.host.get()[j].kld ? s.accepted : m.capacity) : m.n;
     r.updated = 1;
     r.resampled = resampled ? 1 : 0;
     r.n_particles = o.n;
@@ -1880,10 +1725,10 @@ int Batch::step_end(const ClusteredOut* clustered, bb200_update_result* out) {
     uint64_t flagged_cells = 0;
     for (uint32_t j = 0; j < n_active; ++j) {
       if (!res[j].fallback) continue;
-      BatchClusterMember& c = cl_.table_host.get()[flagged.size()];
+      BatchClusterMember& c = cl_.table.host.get()[flagged.size()];
       c = BatchClusterMember{};
       c.offset = members_[active[j]].offset;
-      cl_.cells_host.get()[flagged.size()] = res[j].cells;
+      cl_.cells.host.get()[flagged.size()] = res[j].cells;
       flagged_cells += res[j].cells;
       flagged.push_back(j);
     }
@@ -1891,14 +1736,10 @@ int Batch::step_end(const ClusteredOut* clustered, bb200_update_result* out) {
     if (!flagged.empty()) {
       const uint32_t n_flagged = static_cast<uint32_t>(flagged.size());
       st = ensure_cluster_records(flagged_cells);
-      if (st == BB200_OK)
-        st = check(cudaMemcpyAsync(cl_.table.get(), cl_.table_host.get(), n_flagged * sizeof(BatchClusterMember), cudaMemcpyHostToDevice, stream),
-                   "upload fallback table");
-      if (st == BB200_OK)
-        st = check(cudaMemcpyAsync(cl_.cells.get(), cl_.cells_host.get(), n_flagged * sizeof(uint32_t), cudaMemcpyHostToDevice, stream),
-                   "upload fallback cells");
+      if (st == BB200_OK) st = check(cl_.table.to_device(0, n_flagged, stream), "upload fallback table");
+      if (st == BB200_OK) st = check(cl_.cells.to_device(0, n_flagged, stream), "upload fallback cells");
       if (st == BB200_OK) {
-        launch_batch_cluster_compact(cl_.table.get(), cl_.cells.get(), cl_.records.get(), n_flagged, cl_records_host_.get(), stream);
+        launch_batch_cluster_compact(cl_.table.device.get(), cl_.cells.device.get(), cl_.records.get(), n_flagged, cl_records_host_.get(), stream);
         ++launches_;
         st = check(cudaGetLastError(), "batch_cluster_compact");
       }

@@ -203,10 +203,8 @@ class Batch {
     DeviceBuffer<Scalars> scalars;
     DeviceBuffer<unsigned long long> tile_state;
     DeviceBuffer<double> partials;
-    DeviceBuffer<BatchMember> table;
-    PinnedBuffer<BatchMember> table_host;
-    DeviceBuffer<uint32_t> first;
-    PinnedBuffer<uint32_t> first_host;
+    MirroredBuffer<BatchMember> table;
+    MirroredBuffer<uint32_t> first;
     PinnedBuffer<StepSummary> summary_host;
   };
   /// The layout of the slots' params (nullptr: vacant): particle slices 32-aligned in slot order, hash tables back to back,
@@ -228,6 +226,9 @@ class Batch {
     const FilterState* state;
   };
   int relayout(const std::vector<const bb200_amcl_param*>& slots, Layout* layout, const Arrival* arrival = nullptr);
+  /// add_member, or with `state` import_member: a member with these params in the lowest vacant slot or a new one after
+  /// the last, validated, then given its place by a relayout (with `state`'s arrays and reading map `map`).
+  int join(const bb200_amcl_param& params, const bb200_motion_param& motion, const FilterState* state, int map, int* member);
   /// The scalars of member m's state blob.
   static ParticleSetState particle_set(const Member& m);
   /// Member m as the member a decoded state describes: its policy, count, pivot, CDF total and ancestors count (its
@@ -241,6 +242,9 @@ class Batch {
   int launch_moves(const std::vector<BatchRelayoutMember>& moves, BatchRelayoutArgs a);
   /// BB200_ERR_INVALID_ARGUMENT when present (nullptr: every occupied slot) selects a vacant slot.
   int check_present(const uint8_t* present);
+  /// check_present, then every selected member's measurement as the single filter checks it (BB200_ERR_INVALID_ARGUMENT);
+  /// with `weighed_by_caller`, BB200_MEASUREMENT_WEIGHTS members are taken as they are.
+  int check_measurements(const bb200_measurement* in, const uint8_t* present, bool weighed_by_caller);
   bool selected_member(const uint8_t* present, size_t k) const { return members_[k].active && (present == nullptr || present[k] != 0); }
   int fail(int status, const std::string& message) {
     error_ = message;
@@ -249,9 +253,6 @@ class Batch {
   int check(cudaError_t e, const char* what) { return cuda_check(e, what, &error_); }
   int member_ok(int member) const;
   const MapEntry* find_map(int id) const;
-  int ensure_points(uint64_t n_points);
-  int ensure_detections(uint64_t n);
-  int ensure_inputs(uint64_t floats);
   int ensure_scan_table(Member& m, const bb200_laser_scan& scan);
   /// The step of update and update_measurements: in[m] is member m's measurement, already checked when it is a scan or a cloud.
   /// With `clustered`, the step also selects every updated member's cluster estimate on the device (update_clustered).
@@ -287,11 +288,12 @@ class Batch {
   /// of them has no particles.
   int select_members(const uint8_t* present, std::vector<uint32_t>* selected);
   /// Clusterizer::cell_records of every member in `selected` (non-empty): their records back to back in cl_records_host_,
-  /// member selected[j]'s count in cl_.cells_host[j].  Two launches and two host synchronisations.
+  /// member selected[j]'s count in cl_.cells.host[j].  Two launches and two host synchronisations.
   int cell_records(double linear, double angular, const std::vector<uint32_t>& selected);
-  int ensure_samples(uint64_t draws);
-  /// The ray-cast scratch for `members` table entries and `doubles` of poses, bearings and ranges.
-  int ensure_rays(size_t members, uint64_t doubles);
+  /// Member k's row of the cluster table: its slice, hash table, count, state buffer and pivot as they are now.
+  BatchClusterMember cluster_member(uint32_t k) const;
+  /// The arguments of batch_cluster_cells over the cluster table at these resolutions.
+  BatchClusterArgs cluster_args(double linear, double angular) const;
 
   std::vector<Member> members_;  // by slot
   uint32_t flags_{0};
@@ -314,25 +316,16 @@ class Batch {
   DeviceBuffer<Scalars> scalars_;
   DeviceBuffer<unsigned long long> tile_state_;
   DeviceBuffer<double> partials_;
-  DeviceBuffer<BatchMember> table_;
-  PinnedBuffer<BatchMember> table_host_;
+  MirroredBuffer<BatchMember> table_;
   // kBatchRows x (K + 1): the step's rows, then those of batch_points_kernel, batch_kld_kernel, batch_resampled_moments_kernel
   // and batch_ess_kernel
-  DeviceBuffer<uint32_t> first_;
-  PinnedBuffer<uint32_t> first_host_;
-  DeviceBuffer<double> points_;   // (x, y) pairs
-  PinnedBuffer<double> points_host_;
-  DeviceBuffer<LandmarkDetection> detections_;  // the step's prepared detections, every kBatchLandmark member's in member order
-  PinnedBuffer<LandmarkDetection> detections_host_;
-  // Scans and clouds of update_measurements (allocated on first use): batch_points_kernel's member table and the raw
-  // measurements (kept ranges, or x, y, z per cloud point).
-  struct InputTable {
-    DeviceBuffer<BatchPointsMember> device;
-    PinnedBuffer<BatchPointsMember> host;
-  };
-  InputTable inputs_;
-  DeviceBuffer<float> input_;
-  PinnedBuffer<float> input_host_;
+  MirroredBuffer<uint32_t> first_;
+  MirroredBuffer<double> points_;   // (x, y) pairs
+  MirroredBuffer<LandmarkDetection> detections_;  // the step's prepared detections, every kBatchLandmark member's in member order
+  // Scans and clouds of update_measurements (the table allocated on first use): batch_points_kernel's member table and
+  // the raw measurements (kept ranges, or x, y, z per cloud point).
+  MirroredBuffer<BatchPointsMember> inputs_;
+  MirroredBuffer<float> input_;
   DeviceBuffer<uint32_t> hits_;   // beam model, two-pass form: the step's hit words (grows only)
   PinnedBuffer<StepSummary> summary_host_;  // one per member of the step's table
   PinnedBuffer<int> ticket_host_;
@@ -352,20 +345,14 @@ class Batch {
     DeviceBuffer<uint32_t> sort[2];
     DeviceBuffer<uint32_t> starts;
     DeviceBuffer<CellRecord> records;
-    DeviceBuffer<BatchClusterMember> table;
-    PinnedBuffer<BatchClusterMember> table_host;
-    DeviceBuffer<uint32_t> cells;
-    PinnedBuffer<uint32_t> cells_host;
+    MirroredBuffer<BatchClusterMember> table;
+    MirroredBuffer<uint32_t> cells;
   };
   ClusterBuffers cl_;
   PinnedBuffer<CellRecord> cl_records_host_;  // written by the compaction kernel
   // KLD parameters of a step's members (allocated on first use, one entry per member of the step's table).  The count
   // itself runs in the cluster scratch: per-slot hashes in cl_.hashes, bucket sets in cl_.keys and cl_.first.
-  struct KldTable {
-    DeviceBuffer<BatchKldMember> device;
-    PinnedBuffer<BatchKldMember> host;
-  };
-  KldTable kld_;
+  MirroredBuffer<BatchKldMember> kld_;
   // The device selection of update_clustered (allocated on first use): the probed rehash schedules, one scratch slice per
   // member (select_scratch_bytes of its max_particles, at offsets[k]), the post-step table inputs and the results.
   struct SelectBuffers {
@@ -373,38 +360,27 @@ class Batch {
     DeviceBuffer<RehashStep> schedule;
     DeviceBuffer<unsigned char> scratch;
     std::vector<uint64_t> offsets;
-    DeviceBuffer<BatchClusterPost> post;
-    PinnedBuffer<BatchClusterPost> post_host;
+    MirroredBuffer<BatchClusterPost> post;
     PinnedBuffer<BatchClusterResult> results;
   };
   SelectBuffers sel_;
 
-  // Pose-sample scratch (allocated on first use): the member table, and the draws after a header of one CDF total per
-  // member (sample_header_ poses' worth), so that one copy brings both back.
-  struct SampleTable {
-    DeviceBuffer<BatchSampleMember> device;
-    PinnedBuffer<BatchSampleMember> host;
-  };
-  SampleTable sm_table_;
-  uint64_t sample_header_{0};
-  // State blob transfers (grown on use): the move table of export and import, and the staging buffer that holds the moved
-  // members' arrays, on the device and in pinned memory (StageLayout, batch.cu).
+  // Pose-sample scratch: the member table (allocated on first use), and the draws after a header of one CDF total per
+  // member, so that one copy brings both back.
+  MirroredBuffer<BatchSampleMember> sm_table_;
+  // Moves and state blob transfers (grown on use): the move table and CTA prefix of every batch_relayout_kernel launch
+  // (one entry per moved member), and the staging buffer that holds a transfer's members' arrays (StageLayout, batch.cu).
   struct TransferBuffers {
     DeviceBuffer<BatchRelayoutMember> table;
     DeviceBuffer<uint32_t> first;
-    DeviceBuffer<unsigned char> stage;
-    PinnedBuffer<unsigned char> stage_host;
+    MirroredBuffer<unsigned char> stage;
   };
   TransferBuffers xfer_;
-  DeviceBuffer<Pose2> samples_;
-  PinnedBuffer<Pose2> samples_host_;
-  // Ray-cast scratch (grown on use): the member table, and every casting member's poses, then bearings, then ranges, on the
-  // device and in pinned memory.
+  MirroredBuffer<Pose2> samples_;
+  // Ray-cast scratch (grown on use): the member table, and every casting member's poses, then bearings, then ranges.
   struct RayBuffers {
-    DeviceBuffer<BatchRayMember> table;
-    PinnedBuffer<BatchRayMember> table_host;
-    DeviceBuffer<double> data;
-    PinnedBuffer<double> data_host;
+    MirroredBuffer<BatchRayMember> table;
+    MirroredBuffer<double> data;
   };
   RayBuffers rays_;
 };

@@ -512,9 +512,7 @@ int Clusterizer::estimate(const Pose2* states, const double* weights, uint64_t n
   auto check = [error](cudaError_t e, const char* what) { return cuda_check(e, what, error); };
   if (n == 0) return reject(BB200_ERR_STATE, "no particles", error);
   if (n > capacity_) return reject(BB200_ERR_CAPACITY, "cluster estimate: more particles than the scratch holds", error);
-  if (!(p.linear_hash_resolution > 0.0) || !(p.angular_hash_resolution > 0.0) || !(p.weight_cap_percentile >= 0.0) ||
-      !(p.weight_cap_percentile < 1.0))
-    return reject(BB200_ERR_INVALID_ARGUMENT, "cluster parameters: resolutions must be positive and the percentile in [0, 1)", error);
+  if (const char* why = cluster_param_error(p)) return reject(BB200_ERR_INVALID_ARGUMENT, why, error);
   if (cluster_ids != nullptr && ids_capacity < n) return reject(BB200_ERR_CAPACITY, "cluster id buffer too small", error);
   std::vector<HostCell> host;
   {

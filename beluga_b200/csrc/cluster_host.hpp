@@ -32,6 +32,13 @@ struct ClusterSelection {
   double moments[9]{};                    // raw moments to estimate from: that cluster's, or the whole set's
 };
 
+/// Why a cluster estimate refuses `p` (BB200_ERR_INVALID_ARGUMENT), or nullptr when it takes it.
+inline const char* cluster_param_error(const bb200_cluster_param& p) {
+  if (p.linear_hash_resolution > 0.0 && p.angular_hash_resolution > 0.0 && p.weight_cap_percentile >= 0.0 && p.weight_cap_percentile < 1.0)
+    return nullptr;
+  return "cluster parameters: resolutions must be positive and the percentile in [0, 1)";
+}
+
 /// cells in first-occurrence order (the insertion order of the reference's unordered_map);
 /// n_particles sizes the map's initial reserve like make_cluster_map (:146).
 ClusterSelection select_cluster(const HostCell* cells, std::size_t n_cells, std::uint64_t n_particles, double linear_resolution,

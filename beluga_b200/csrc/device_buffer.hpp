@@ -72,4 +72,28 @@ using DeviceBuffer = Buffer<T, Memory::kDevice>;
 template <class T>
 using PinnedBuffer = Buffer<T, Memory::kPinned>;
 
+/// A device buffer and its pinned twin: a table the host fills and uploads, or one the device fills and the host reads.
+/// Callers fill host.get() and hand device.get() to launchers; the pair only sizes both halves together and copies
+/// between them.
+template <class T>
+struct MirroredBuffer {
+  DeviceBuffer<T> device;
+  PinnedBuffer<T> host;
+
+  /// Elements both halves hold: after a failed grow the pair is short, and the next grow retries the half that failed.
+  size_t size() const { return device.size() < host.size() ? device.size() : host.size(); }
+  /// Buffer::grow on the device half, then on the pinned half; the first error.
+  cudaError_t grow(size_t count, size_t room = 0) {
+    const cudaError_t e = device.grow(count, room);
+    return e != cudaSuccess ? e : host.grow(count, room);
+  }
+  /// One cudaMemcpyAsync of elements [first, first + count) from the pinned half to the device half, or back.
+  cudaError_t to_device(size_t first, size_t count, cudaStream_t stream) const {
+    return cudaMemcpyAsync(device.get() + first, host.get() + first, count * sizeof(T), cudaMemcpyHostToDevice, stream);
+  }
+  cudaError_t to_host(size_t first, size_t count, cudaStream_t stream) const {
+    return cudaMemcpyAsync(host.get() + first, device.get() + first, count * sizeof(T), cudaMemcpyDeviceToHost, stream);
+  }
+};
+
 }  // namespace bb200

@@ -1,6 +1,6 @@
 // csrc/device_buffer.hpp without a GPU: the four CUDA allocation functions are defined here over malloc, count the live
-// allocations of each kind and fail the k-th call on request.  Prints one line per failed check; exit status 0 when all
-// checks pass.
+// allocations of each kind and fail the k-th call on request, and cudaMemcpyAsync records each copy it is asked for.
+// Prints one line per failed check; exit status 0 when all checks pass.
 #include "../../beluga_b200/csrc/device_buffer.hpp"
 
 #include <cstdint>
@@ -8,6 +8,7 @@
 #include <cstdlib>
 #include <map>
 #include <utility>
+#include <vector>
 
 namespace {
 
@@ -16,6 +17,16 @@ int alloc_calls = 0;   // allocation calls so far
 int fail_call = -1;    // index of the allocation call that fails (-1: none)
 int bad_frees = 0;     // frees of a pointer that is not live in that kind (double frees, wrong kind, null)
 int failures = 0;
+
+struct Copy {
+  void* dst;
+  const void* src;
+  size_t bytes;
+  cudaMemcpyKind kind;
+  cudaStream_t stream;
+};
+std::vector<Copy> copies;                  // every cudaMemcpyAsync call, in order
+cudaError_t copy_result = cudaSuccess;  // what cudaMemcpyAsync returns
 
 cudaError_t fake_alloc(void** p, size_t bytes, std::map<void*, size_t>& live) {
   if (alloc_calls++ == fail_call) return cudaErrorMemoryAllocation;  // *p stays as it was, like the runtime's
@@ -49,8 +60,13 @@ cudaError_t cudaMalloc(void** p, size_t bytes) { return fake_alloc(p, bytes, dev
 cudaError_t cudaFree(void* p) { return fake_free(p, device_live); }
 cudaError_t cudaMallocHost(void** p, size_t bytes) { return fake_alloc(p, bytes, pinned_live); }
 cudaError_t cudaFreeHost(void* p) { return fake_free(p, pinned_live); }
+cudaError_t cudaMemcpyAsync(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind, cudaStream_t stream) {
+  copies.push_back(Copy{dst, src, bytes, kind, stream});
+  return copy_result;
+}
 
 using bb200::DeviceBuffer;
+using bb200::MirroredBuffer;
 using bb200::PinnedBuffer;
 
 namespace {
@@ -162,6 +178,77 @@ void test_group_all_or_nothing(bool filled) {
   EXPECT(live_count() == 0 && bad_frees == 0);
 }
 
+void test_mirrored_grow() {
+  {
+    MirroredBuffer<double> m;
+    EXPECT(m.size() == 0 && m.grow(0) == cudaSuccess && live_count() == 0);
+    EXPECT(m.grow(10, 16) == cudaSuccess && m.device.size() == 16 && m.host.size() == 16 && m.size() == 16);
+    EXPECT(device_live.size() == 1 && pinned_live.size() == 1);
+    double* d = m.device.get();
+    const int calls = alloc_calls;
+    EXPECT(m.grow(16, 100) == cudaSuccess && m.device.get() == d && alloc_calls == calls);  // room enough in both halves
+
+    fail_call = alloc_calls + 1;  // the pinned half fails
+    EXPECT(m.grow(20) == cudaErrorMemoryAllocation);
+    EXPECT(m.device.size() == 20 && m.host.get() == nullptr && m.size() == 0 && device_live.size() == 1 && pinned_live.empty());
+    fail_call = -1;
+    d = m.device.get();
+    const int before_retry = alloc_calls;
+    EXPECT(m.grow(20) == cudaSuccess && m.size() == 20);  // the short half alone grows again
+    EXPECT(m.device.get() == d && alloc_calls == before_retry + 1 && pinned_live.size() == 1);
+
+    fail_call = alloc_calls;  // the device half fails: the pinned half is left as it was
+    EXPECT(m.grow(40) == cudaErrorMemoryAllocation);
+    EXPECT(m.device.get() == nullptr && m.host.size() == 20 && m.size() == 0 && device_live.empty() && pinned_live.size() == 1);
+    fail_call = -1;
+    EXPECT(m.grow(40) == cudaSuccess && m.device.size() == 40 && m.host.size() == 40 && m.size() == 40 && live_count() == 2);
+  }
+  EXPECT(live_count() == 0 && bad_frees == 0);
+}
+
+void test_mirrored_move() {
+  {
+    MirroredBuffer<uint32_t> a;
+    EXPECT(a.grow(8) == cudaSuccess);
+    uint32_t* d = a.device.get();
+    uint32_t* h = a.host.get();
+    MirroredBuffer<uint32_t> b(std::move(a));
+    EXPECT(a.device.get() == nullptr && a.host.get() == nullptr && a.size() == 0);
+    EXPECT(b.device.get() == d && b.host.get() == h && b.size() == 8 && live_count() == 2);
+    MirroredBuffer<uint32_t> c;
+    EXPECT(c.grow(4) == cudaSuccess && live_count() == 4);
+    c = std::move(b);  // c's own halves are freed, b's move over
+    EXPECT(b.size() == 0 && c.device.get() == d && c.host.get() == h && live_count() == 2);
+    c = {};  // as a relayout drops a table sized by the old slot count
+    EXPECT(c.size() == 0 && live_count() == 0);
+  }
+  EXPECT(live_count() == 0 && bad_frees == 0);
+}
+
+void test_mirrored_copies() {
+  {
+    MirroredBuffer<uint64_t> m;
+    EXPECT(m.grow(16) == cudaSuccess);
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(static_cast<uintptr_t>(0x5a));
+    copies.clear();
+    EXPECT(m.to_device(2, 3, stream) == cudaSuccess);
+    EXPECT(m.to_host(5, 4, stream) == cudaSuccess);
+    EXPECT(copies.size() == 2);
+    if (copies.size() == 2) {
+      const Copy& up = copies[0];
+      EXPECT(up.dst == m.device.get() + 2 && up.src == m.host.get() + 2 && up.bytes == 3 * sizeof(uint64_t));
+      EXPECT(up.kind == cudaMemcpyHostToDevice && up.stream == stream);
+      const Copy& down = copies[1];
+      EXPECT(down.dst == m.host.get() + 5 && down.src == m.device.get() + 5 && down.bytes == 4 * sizeof(uint64_t));
+      EXPECT(down.kind == cudaMemcpyDeviceToHost && down.stream == stream);
+    }
+    copy_result = cudaErrorInvalidValue;  // the copy's error reaches the caller
+    EXPECT(m.to_device(0, 1, stream) == cudaErrorInvalidValue && m.to_host(0, 1, stream) == cudaErrorInvalidValue);
+    copy_result = cudaSuccess;
+  }
+  EXPECT(live_count() == 0 && bad_frees == 0);
+}
+
 }  // namespace
 
 int main() {
@@ -172,6 +259,9 @@ int main() {
   test_failure_leaves_empty();
   test_group_all_or_nothing(false);
   test_group_all_or_nothing(true);
+  test_mirrored_grow();
+  test_mirrored_move();
+  test_mirrored_copies();
   if (failures == 0) std::printf("all device buffer checks passed\n");
   return failures == 0 ? 0 : 1;
 }

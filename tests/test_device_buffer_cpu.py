@@ -1,14 +1,17 @@
 """csrc/device_buffer.hpp on the CPU: the owner of every device and pinned buffer of the library.
 
 The header needs nothing from CUDA but <cuda_runtime_api.h>, so g++ compiles it against a test (tests/cpp/test_device_buffer.cpp)
-that defines cudaMalloc, cudaFree, cudaMallocHost and cudaFreeHost itself, over malloc, and links no CUDA runtime.  The
-test counts the live allocations and fails the k-th allocation on request; it checks that
+that defines cudaMalloc, cudaFree, cudaMallocHost, cudaFreeHost and cudaMemcpyAsync itself, over malloc, and links no CUDA
+runtime.  The test counts the live allocations, fails the k-th allocation on request and records every copy; it checks that
 
 * the destructor and moves free every buffer exactly once, each with the free of its kind;
 * allocate(0) still allocates one element, and grow() reallocates only when the buffer holds fewer elements than asked;
 * a failed allocate() or grow() leaves the buffer null with size 0 and nothing live;
 * a group of buffers allocated into a local struct and moved into its owner on success is all or nothing: a failure at
-  any of its allocations leaves the owner's buffers as they were and frees whatever the attempt allocated.
+  any of its allocations leaves the owner's buffers as they were and frees whatever the attempt allocated;
+* a MirroredBuffer grows both halves, reports the smaller half's size after a failed one and grows that half again on
+  the next call, frees each half once through moves, and copies exactly the element range asked for, in the direction
+  asked for, returning the copy's error.
 """
 import os
 import subprocess

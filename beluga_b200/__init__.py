@@ -932,10 +932,15 @@ class ShardedAmcl:
         if st != _capi.OK:
             raise BelugaB200Error(st, self._lib.bb200_sharded_amcl_last_error(self._h).decode())
 
-    def update_map(self, sensor: int, params, grid: OccupancyGrid):
+    def update_map(self, sensor: int, params, grid):
+        """Amcl.update_map on every shard: `grid` is an OccupancyGrid, or a LandmarkMap for SENSOR_LANDMARK and SENSOR_BEARING."""
         g = grid.c()
         p = params.c()
-        if sensor == SENSOR_BEAM:
+        if sensor == SENSOR_LANDMARK:
+            self._check(self._lib.bb200_sharded_amcl_set_landmark_map(self._h, C.byref(p), C.byref(g)))
+        elif sensor == SENSOR_BEARING:
+            self._check(self._lib.bb200_sharded_amcl_set_bearing_map(self._h, C.byref(p), C.byref(g)))
+        elif sensor == SENSOR_BEAM:
             self._check(self._lib.bb200_sharded_amcl_set_beam_map(self._h, C.byref(p), C.byref(g)))
         else:
             self._check(self._lib.bb200_sharded_amcl_set_likelihood_field_map(self._h, C.byref(p), C.byref(g), int(sensor == SENSOR_LIKELIHOOD_FIELD_PROB)))
@@ -953,6 +958,13 @@ class ShardedAmcl:
         pts = _f64(points).reshape(-1, 2)
         res = _capi.UpdateResult()
         self._check(self._lib.bb200_sharded_amcl_update(self._h, _dptr(_f64(control_pose)), _dptr(pts) if len(pts) else None, len(pts), C.byref(res)))
+        return res
+
+    def update_landmarks(self, control_pose, positions, categories) -> _capi.UpdateResult:
+        """Amcl.update_landmarks over all shards (bb200_sharded_amcl_update_landmarks)."""
+        arr, n = _landmark_array(positions, categories)
+        res = _capi.UpdateResult()
+        self._check(self._lib.bb200_sharded_amcl_update_landmarks(self._h, _dptr(_f64(control_pose)), arr, n, C.byref(res)))
         return res
 
     def update_weighted(self, control_pose, weigh) -> _capi.UpdateResult:

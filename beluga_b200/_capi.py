@@ -232,10 +232,13 @@ SIGNATURES = {
     "bb200_sharded_amcl_shard": (_vp, [_vp, C.c_int]),
     "bb200_sharded_amcl_set_likelihood_field_map": (C.c_int, [_vp, _P(LikelihoodFieldParam), _P(OccupancyGrid), C.c_int]),
     "bb200_sharded_amcl_set_beam_map": (C.c_int, [_vp, _P(BeamParam), _P(OccupancyGrid)]),
+    "bb200_sharded_amcl_set_landmark_map": (C.c_int, [_vp, _P(LandmarkParam), _P(LandmarkMap)]),
+    "bb200_sharded_amcl_set_bearing_map": (C.c_int, [_vp, _P(BearingParam), _P(LandmarkMap)]),
     "bb200_sharded_amcl_initialize": (C.c_int, [_vp, _dbl, _dbl]),
     "bb200_sharded_amcl_initialize_from_map": (C.c_int, [_vp]),
     "bb200_sharded_amcl_force_update": (None, [_vp]),
     "bb200_sharded_amcl_update": (C.c_int, [_vp, _dbl, _dbl, C.c_uint64, _P(UpdateResult)]),
+    "bb200_sharded_amcl_update_landmarks": (C.c_int, [_vp, _dbl, _P(Landmark), C.c_uint64, _P(UpdateResult)]),
     "bb200_sharded_amcl_update_begin": (C.c_int, [_vp, _dbl, _P(WeighView)]),
     "bb200_sharded_amcl_update_end": (C.c_int, [_vp, _P(UpdateResult)]),
     "bb200_sharded_amcl_get_particles": (C.c_int, [_vp, _dbl, _dbl, C.c_uint64]),

@@ -442,7 +442,7 @@ int Amcl::update(const double control[4], const double* points_xy, uint64_t n_po
 }
 
 int Amcl::update_landmarks(const double control[4], const bb200_landmark_detection* detections, uint64_t n, bb200_update_result* out) {
-  if (sharded()) return filter_.fail_with(BB200_ERR_STATE, "detection steps run on one GPU; a filter joined to shards takes points");
+  if (sharded()) return filter_.fail_with(BB200_ERR_STATE, "detection steps on shards run through bb200_sharded_amcl_update_landmarks; a shard joined by bb200_amcl_join_shards takes points");
   if (const int st = filter_.stage_detections(detections, n)) return st;
   return update(control, Filter::staged_detections(), 0, out);
 }

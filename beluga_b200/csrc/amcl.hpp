@@ -79,7 +79,8 @@ class Amcl {
   int restore_state(const FilterState& s);
   void force_update() { policy_.force_update(); }
   int update(const double control[4], const double* points_xy, uint64_t n_points, bb200_update_result* out);
-  /// update() with a landmark or bearing model: the map's model weighs the detections.  One GPU only.
+  /// update() with a landmark or bearing model: the map's model weighs the detections.  Refused on a shard: a sharded
+  /// filter takes detection steps through ShardedAmcl::update_landmarks.
   int update_landmarks(const double control[4], const bb200_landmark_detection* detections, uint64_t n, bb200_update_result* out);
   /// AmclPolicy::plan_update over this filter's particle count (a shard: the global count once initialised).
   int plan_update(const double control[4], bb200_step_plan* plan);

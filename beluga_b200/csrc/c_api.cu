@@ -750,6 +750,16 @@ int bb200_sharded_amcl_set_beam_map(bb200_sharded_amcl* g, const bb200_beam_para
   BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
   return guarded(g->impl, [&] { return g->impl.set_map([&](bb200::MapTables* t, std::string* e) { return bb200::prepare_beam_map(*p, *grid, t, e); }); });
 }
+int bb200_sharded_amcl_set_landmark_map(bb200_sharded_amcl* g, const bb200_landmark_param* p, const bb200_landmark_map* map) {
+  BB_REQUIRE(g && p && map);
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  return guarded(g->impl, [&] { return g->impl.set_landmark_map(p, nullptr, *map); });
+}
+int bb200_sharded_amcl_set_bearing_map(bb200_sharded_amcl* g, const bb200_bearing_param* p, const bb200_landmark_map* map) {
+  BB_REQUIRE(g && p && map);
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  return guarded(g->impl, [&] { return g->impl.set_landmark_map(nullptr, p, *map); });
+}
 int bb200_sharded_amcl_initialize(bb200_sharded_amcl* g, const double mean_xytheta[3], const double cov[9]) {
   BB_REQUIRE(mean_xytheta && cov);
   BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
@@ -769,6 +779,12 @@ int bb200_sharded_amcl_update(bb200_sharded_amcl* g, const double control_pose[4
   BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
   static const double kNoPoints[2] = {0.0, 0.0};
   return guarded(g->impl, [&] { return g->impl.update(control_pose, points_xy != nullptr ? points_xy : kNoPoints, n_points, out); });
+}
+int bb200_sharded_amcl_update_landmarks(bb200_sharded_amcl* g, const double control_pose[4], const bb200_landmark_detection* detections, uint64_t n,
+                                        bb200_update_result* out) {
+  BB_REQUIRE(g && control_pose && out && (detections || n == 0));
+  BB_REFUSE_OPEN_STEP(g, kShardedStepOpen);
+  return guarded(g->impl, [&] { return g->impl.update_landmarks(control_pose, detections, n, out); });
 }
 int bb200_sharded_amcl_update_begin(bb200_sharded_amcl* g, const double control_pose[4], bb200_weigh_view* views) {
   BB_REQUIRE(g && control_pose && views);

@@ -667,10 +667,21 @@ int Filter::set_landmark_map(const bb200_landmark_param* lp, const bb200_bearing
 const double Filter::kStagedDetections = 0.0;
 
 int Filter::stage_detections(const bb200_landmark_detection* detections, uint64_t n) {
+  std::vector<LandmarkDetection> prepared;
+  if (const int st = prepare_step_detections(detections, n, &prepared)) return st;
+  return upload_detections(prepared);
+}
+
+int Filter::prepare_step_detections(const bb200_landmark_detection* detections, uint64_t n, std::vector<LandmarkDetection>* prepared) {
   if (!map_.landmark_map()) return fail(BB200_ERR_STATE, "detections need a landmark map (set_landmark_map / set_bearing_map)");
   if (n >= 0xffffffffull) return fail(BB200_ERR_INVALID_ARGUMENT, "too many detections");
-  std::vector<LandmarkDetection> prepared;
-  prepare_detections(map_.landmark_slices, detections, n, &prepared);
+  prepare_detections(map_.landmark_slices, detections, n, prepared);
+  return BB200_OK;
+}
+
+int Filter::upload_detections(const std::vector<LandmarkDetection>& prepared) {
+  if (!map_.landmark_map()) return fail(BB200_ERR_STATE, "detections need a landmark map (set_landmark_map / set_bearing_map)");
+  const uint64_t n = prepared.size();
   BB_CHECK(cudaSetDevice(config_.device));
   BB_CHECK(cudaStreamSynchronize(stream_));  // the previous step's copy has left the staging buffer
   const uint64_t room = std::max<uint64_t>(n, 64);

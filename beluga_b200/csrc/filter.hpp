@@ -40,8 +40,16 @@ class Filter {
   /// A landmark map for LandmarkSensorModel2d (lp) or, with lp null, BearingSensorModel2d (bp).
   int set_landmark_map(const bb200_landmark_param* lp, const bb200_bearing_param* bp, const bb200_landmark_map& map);
   /// Prepares a step's detections on a landmark map and enqueues their upload; BB200_ERR_STATE on any other map.  The
-  /// reweight of a step that passes staged_detections() as its points weighs them.
+  /// reweight of a step that passes staged_detections() as its points weighs them.  prepare_step_detections followed by
+  /// upload_detections.
   int stage_detections(const bb200_landmark_detection* detections, uint64_t n);
+  /// The host half of stage_detections: the detections prepared against this filter's landmark map (prepare_detections);
+  /// BB200_ERR_STATE on any other map, BB200_ERR_INVALID_ARGUMENT for n >= 2^32 - 1.  Nothing reaches the device.
+  int prepare_step_detections(const bb200_landmark_detection* detections, uint64_t n, std::vector<LandmarkDetection>* prepared);
+  /// The device half: enqueues the upload of detections prepared against this map's tables (or an identical copy of
+  /// them, as every shard of a filter holds) on this filter's stream, once the previous step's upload has left the
+  /// pinned staging buffer.
+  int upload_detections(const std::vector<LandmarkDetection>& prepared);
   /// The `points_xy` of a step on a landmark map: the reweight weighs the staged detections instead of points.
   static const double* staged_detections() { return &kStagedDetections; }
   /// Makes the prepared tables this filter's map (the upload half of set_*_map).

@@ -72,6 +72,10 @@ int ShardedAmcl::set_map(const std::function<int(MapTables*, std::string*)>& pre
   return st;
 }
 
+int ShardedAmcl::set_landmark_map(const bb200_landmark_param* lp, const bb200_bearing_param* bp, const bb200_landmark_map& map) {
+  return set_map([&](MapTables* t, std::string* e) { return prepare_landmark_map(lp, bp, map, t, e); });
+}
+
 int ShardedAmcl::initialize(const double mean[3], const double cov[9]) {
   error_.clear();
   for (Amcl* a : ranks_)
@@ -93,6 +97,22 @@ void ShardedAmcl::force_update() {
 int ShardedAmcl::update(const double control[4], const double* points_xy, uint64_t n_points, bb200_update_result* out) {
   error_.clear();
   return Amcl::update_group(ranks_.data(), shards(), control, points_xy, n_points, out);
+}
+
+int ShardedAmcl::update_landmarks(const double control[4], const bb200_landmark_detection* detections, uint64_t n, bb200_update_result* out) {
+  error_.clear();
+  *out = bb200_update_result{};
+  if (detections == nullptr && n > 0) {
+    error_ = "detections is null";
+    return static_cast<int>(BB200_ERR_INVALID_ARGUMENT);
+  }
+  // Every shard holds the same tables: the detections are prepared once, against rank 0's, and uploaded to every shard
+  // before any shard's step starts.  The uploads only enqueue copies, and no policy has moved yet.
+  std::vector<LandmarkDetection> prepared;
+  if (const int st = ranks_[0]->filter().prepare_step_detections(detections, n, &prepared)) return st;
+  for (Amcl* a : ranks_)
+    if (const int st = a->filter().upload_detections(prepared)) return st;
+  return Amcl::update_group(ranks_.data(), shards(), control, Filter::staged_detections(), 0, out);
 }
 
 int ShardedAmcl::update_begin(const double control[4], bb200_weigh_view* views) {

@@ -35,10 +35,16 @@ class ShardedAmcl {
   /// Prepares the map's tables once (prepare fills them, or a message) and uploads them to every shard.  A failed
   /// preparation is reported by the first shard, as its own set_*_map call would.
   int set_map(const std::function<int(MapTables*, std::string*)>& prepare);
+  /// set_map with the tables of Filter::set_landmark_map: the landmark model (lp) or, with lp null, the bearing model (bp).
+  int set_landmark_map(const bb200_landmark_param* lp, const bb200_bearing_param* bp, const bb200_landmark_map& map);
   int initialize(const double mean[3], const double cov[9]);
   int initialize_from_map();
   void force_update();
   int update(const double control[4], const double* points_xy, uint64_t n_points, bb200_update_result* out);
+  /// update() with the landmark map's model weighing the detections: prepared once, uploaded to every shard, then the
+  /// step of update().  Null detections with n > 0, n >= 2^32 - 1 and a grid map are refused before any device work; a
+  /// step the policies skip launches nothing beyond the uploads.  Atomic as update().
+  int update_landmarks(const double control[4], const bb200_landmark_detection* detections, uint64_t n, bb200_update_result* out);
   int update_begin(const double control[4], bb200_weigh_view* views);
   int update_end(bb200_update_result* out);
   int cluster_estimate(const bb200_cluster_param& p, bb200_estimate* out, uint32_t* n_cells, uint32_t* n_clusters);

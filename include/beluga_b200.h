@@ -593,12 +593,26 @@ int bb200_sharded_amcl_shards(const bb200_sharded_amcl* g);
 bb200_amcl* bb200_sharded_amcl_shard(bb200_sharded_amcl* g, int rank);
 int bb200_sharded_amcl_set_likelihood_field_map(bb200_sharded_amcl* g, const bb200_likelihood_field_param* p, const bb200_occupancy_grid* grid, int prob);
 int bb200_sharded_amcl_set_beam_map(bb200_sharded_amcl* g, const bb200_beam_param* p, const bb200_occupancy_grid* grid);
+/* bb200_filter_set_landmark_map / _set_bearing_map on every shard: the map is prepared once and uploaded to each.  A map
+ * or parameters the filter calls refuse get the same status and message, and every shard keeps its map.  On a sharded
+ * landmark map, bb200_sharded_amcl_update, _update_scan, _update_point_cloud and _cast_rays return BB200_ERR_STATE;
+ * initialize_from_map and recovery injection draw from the map's box, as on one filter. */
+int bb200_sharded_amcl_set_landmark_map(bb200_sharded_amcl* g, const bb200_landmark_param* p, const bb200_landmark_map* map);
+int bb200_sharded_amcl_set_bearing_map(bb200_sharded_amcl* g, const bb200_bearing_param* p, const bb200_landmark_map* map);
 int bb200_sharded_amcl_initialize(bb200_sharded_amcl* g, const double mean_xytheta[3], const double cov[9]);
 int bb200_sharded_amcl_initialize_from_map(bb200_sharded_amcl* g);
 void bb200_sharded_amcl_force_update(bb200_sharded_amcl* g);
 /* Amcl::update (amcl_core.hpp:165-201) over all shards. */
 int bb200_sharded_amcl_update(bb200_sharded_amcl* g, const double control_pose[4], const double* points_xy, uint64_t n_points,
                               bb200_update_result* out);
+/* bb200_amcl_update_landmarks over all shards: the detections are prepared once on the host and copied to every shard
+ * (no kernel launch), then every shard weighs its particles with the map's model and the step continues as
+ * bb200_sharded_amcl_update does.  Particles, weights and the result's decisions, counts and weight_sum equal those of
+ * one filter with the same parameters and seed, whatever the shard count.  BB200_ERR_INVALID_ARGUMENT for a NULL
+ * detections with n > 0 and for n >= 2^32 - 1, BB200_ERR_STATE on a grid map, all before any device work; atomic as
+ * bb200_sharded_amcl_update.  A shard joined by bb200_amcl_join_shards (one process per GPU) takes no detections. */
+int bb200_sharded_amcl_update_landmarks(bb200_sharded_amcl* g, const double control_pose[4], const bb200_landmark_detection* detections, uint64_t n,
+                                        bb200_update_result* out);
 /* bb200_amcl_update_begin / _end over all shards: a step weighed by the caller's own sensor model.  views has
  * bb200_sharded_amcl_shards(g) entries; view r is shard r's contiguous slice of the global particle order, on devices[r] as
  * passed to bb200_sharded_amcl_create, with that shard's stream (a KLD-sized shard may hold n = 0: nothing to weigh).  The

@@ -361,7 +361,7 @@ class ShardedAmcl {
   }
   void force_update() { bb200_sharded_amcl_force_update(handle_); }
 
-  /// Amcl::update over all shards.  With a caller's device sensor model (is_weighed_token_v of its token; the model's
+  /// Amcl::update over all shards (with a landmark or bearing model, bb200_sharded_amcl_update_landmarks).  With a caller's device sensor model (is_weighed_token_v of its token; the model's
   /// attach takes the bb200_sharded_amcl*): begin, the token's weigh once per shard that holds particles, in rank order,
   /// and end (bb200_sharded_amcl_update_begin / _end).  The views of shard r live on devices[r], the device of its stream:
   /// a token that launches kernels must make that device current (cudaSetDevice) first.  weigh must not throw: the step
@@ -375,6 +375,9 @@ class ShardedAmcl {
       for (const bb200_weigh_view& view : views)
         if (view.updated && view.n > 0) token.weigh(view.stream, view.states, view.n, view.factors);
       check(bb200_sharded_amcl_update_end(handle_, &r));
+    } else if constexpr (is_landmark_token_v<std::decay_t<decltype(token)>>) {
+      check(bb200_sharded_amcl_update_landmarks(handle_, control_action.data(), token.detections.empty() ? nullptr : token.detections.data(),
+                                                token.detections.size(), &r));
     } else {
       check(bb200_sharded_amcl_update(handle_, control_action.data(), token.points.empty() ? nullptr : &token.points.front().first, token.points.size(), &r));
     }

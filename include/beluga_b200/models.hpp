@@ -546,6 +546,11 @@ class LandmarkSensorModel2d {
     const bb200_landmark_map m = map_.view();
     return bb200_filter_set_landmark_map(f, &p, &m);
   }
+  [[nodiscard]] int attach(bb200_sharded_amcl* g) const {
+    const bb200_landmark_param p{params_.sigma_range, params_.sigma_bearing, params_.random_prob};
+    const bb200_landmark_map m = map_.view();
+    return bb200_sharded_amcl_set_landmark_map(g, &p, &m);
+  }
 
  private:
   param_type params_;
@@ -574,14 +579,24 @@ class BearingSensorModel2d {
     return t;
   }
   [[nodiscard]] int attach(bb200_filter* f) const {
-    bb200_bearing_param p{};
-    p.sigma_bearing = params_.sigma_bearing;
-    for (int k = 0; k < 12; ++k) p.sensor_pose_in_robot[k] = params_.sensor_pose_in_robot.m[k];
+    const bb200_bearing_param p = c_param();
     const bb200_landmark_map m = map_.view();
     return bb200_filter_set_bearing_map(f, &p, &m);
   }
+  [[nodiscard]] int attach(bb200_sharded_amcl* g) const {
+    const bb200_bearing_param p = c_param();
+    const bb200_landmark_map m = map_.view();
+    return bb200_sharded_amcl_set_bearing_map(g, &p, &m);
+  }
 
  private:
+  [[nodiscard]] bb200_bearing_param c_param() const {
+    bb200_bearing_param p{};
+    p.sigma_bearing = params_.sigma_bearing;
+    for (int k = 0; k < 12; ++k) p.sensor_pose_in_robot[k] = params_.sensor_pose_in_robot.m[k];
+    return p;
+  }
+
   param_type params_;
   map_type map_;
 };

@@ -27,6 +27,8 @@ same step weighed by the caller (update_weighted, one torch kernel per shard), o
 the reweight kernel's share of the FP64 bound and the Python oracle beside them.
 `batch_landmark`: AmclBatch with the landmark model, K in {1, 16, 64, 256} members x 2000 particles x 16 detections on the
 same two maps, against the same members stepped as standalone Amcl.update_landmarks.
+`sharded_landmark`: `landmark`'s 1M-particle steps on one filter and on 2, 4 and 8 shards of device 0 (what sharding costs),
+and over 2, 4 and 8 devices where there are that many (how it scales), with each shard's reweight kernel time.
 C1 10k x 180 LFM 500^2 multinomial (GPU and CPU oracle seq/par), C3 1M x 720 beam model 2000^2,
 C4 KLD-adaptive 100k..10M LFM.  Writes gpurun_out/configs.json."""
 import ctypes
@@ -719,6 +721,36 @@ def run_batch_beam():
     return res
 
 
+LANDMARK_SENSOR_POSE = (0.0, 0.0, 1.0, 0.2, -1.0, 0.0, 0.0, 0.0, 0.0, -1.0, 0.0, 0.5)
+
+
+def landmark_maps():
+    """The two maps of `landmark` and `sharded_landmark`, each with its 16 detections: (name, positions, categories,
+    detection positions, detection categories)."""
+    rng = np.random.default_rng(9)
+    nd = 16
+    for map_name, n_lm, n_cat in (("64_in_64_categories", 64, 64), ("1000_in_1_category", 1000, 1)):
+        pos = np.stack([rng.uniform(-20, 20, n_lm), rng.uniform(-20, 20, n_lm), rng.uniform(0, 2, n_lm)], axis=1)
+        cat = (np.arange(n_lm) % n_cat).astype(np.uint32)
+        det_pos = np.stack([rng.uniform(-5, 5, nd), rng.uniform(-5, 5, nd), rng.uniform(0, 2, nd)], axis=1)
+        det_cat = rng.integers(0, n_cat, nd).astype(np.uint32)
+        yield map_name, pos, cat, det_pos, det_cat
+
+
+def landmark_params(n):
+    return bb.AmclParams(update_min_d=0.0, update_min_a=0.0, min_particles=n, max_particles=n, resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=1)
+
+
+def landmark_setup(f, model, pos, cat):
+    """The map of `model` on an Amcl or ShardedAmcl, and the particles of a wide Gaussian."""
+    lmap = bb.LandmarkMap(pos, cat)
+    if model == "landmark":
+        f.update_map(bb.SENSOR_LANDMARK, bb.LandmarkModelParam(0.5, 0.3, 1e-3), lmap)
+    else:
+        f.update_map(bb.SENSOR_BEARING, bb.BearingModelParam(0.3, LANDMARK_SENSOR_POSE), lmap)
+    f.initialize([0.0, 0.0, 0.0], np.diag([25.0, 25.0, 1.0]))
+
+
 def run_landmark():
     """The landmark and bearing models at 1M particles x 16 detections, on (a) 64 landmarks in 64 categories (fiducial-like:
     one candidate per detection) and (b) 1000 landmarks in one category (reflector-like: every detection scans all 1000).
@@ -733,24 +765,12 @@ def run_landmark():
 
     res = {}
     device = device_record()
-    rng = np.random.default_rng(9)
-    n, nd, steps, warmup = 1 << 20, 16, 10, 2
-    sensor_pose = (0.0, 0.0, 1.0, 0.2, -1.0, 0.0, 0.0, 0.0, 0.0, -1.0, 0.0, 0.5)
-    for map_name, n_lm, n_cat in (("64_in_64_categories", 64, 64), ("1000_in_1_category", 1000, 1)):
-        pos = np.stack([rng.uniform(-20, 20, n_lm), rng.uniform(-20, 20, n_lm), rng.uniform(0, 2, n_lm)], axis=1)
-        cat = (np.arange(n_lm) % n_cat).astype(np.uint32)
-        det_pos = np.stack([rng.uniform(-5, 5, nd), rng.uniform(-5, 5, nd), rng.uniform(0, 2, nd)], axis=1)
-        det_cat = rng.integers(0, n_cat, nd).astype(np.uint32)
+    n, steps, warmup = 1 << 20, 10, 2
+    for map_name, pos, cat, det_pos, det_cat in landmark_maps():
         candidates = sum(int((cat == c).sum()) for c in det_cat)
         for model in ("landmark", "bearing"):
-            a = bb.Amcl(bb.DifferentialDriveModelParam(*MOTION), bb.AmclParams(update_min_d=0.0, update_min_a=0.0, min_particles=n, max_particles=n,
-                                                                               resample_scheme=bb.RESAMPLE_SYSTEMATIC, seed=1))
-            lmap = bb.LandmarkMap(pos, cat)
-            if model == "landmark":
-                a.update_map(bb.SENSOR_LANDMARK, bb.LandmarkModelParam(0.5, 0.3, 1e-3), lmap)
-            else:
-                a.update_map(bb.SENSOR_BEARING, bb.BearingModelParam(0.3, sensor_pose), lmap)
-            a.initialize([0.0, 0.0, 0.0], np.diag([25.0, 25.0, 1.0]))
+            a = bb.Amcl(bb.DifferentialDriveModelParam(*MOTION), landmark_params(n))
+            landmark_setup(a, model, pos, cat)
             a.filter.set_timing(True)
             wall, kernels = [], {}
             for k in range(warmup + steps):
@@ -773,7 +793,7 @@ def run_landmark():
                 if model == "landmark":
                     lo.landmark_weight(s, dets, omap, 0.5, 0.3, 1e-3)
                 else:
-                    lo.bearing_weight(s, dets, omap, 0.3, sensor_pose)
+                    lo.bearing_weight(s, dets, omap, 0.3, LANDMARK_SENSOR_POSE)
             cpu_ms = (time.perf_counter() - t0) * 1e3 * n / len(states)
             res[f"landmark_{model}_1M_x_16_{map_name}"] = {
                 "ms_per_step_e2e": float(np.median(wall)), "ms_per_step_min_max": [float(min(wall)), float(max(wall))],
@@ -781,6 +801,56 @@ def run_landmark():
                 "fp64_bound_ms": ops / 17e12 * 1e3, "share_of_fp64_bound": ops / 17e12 * 1e3 / kernel_ms,
                 "cpu_oracle_ms_one_thread_extrapolated": cpu_ms, "kernels_ms": {k: round(v, 4) for k, v in kernels.items()}, "device": device}
             a.close()
+    return res
+
+
+def run_sharded_landmark():
+    """`landmark`'s workload (the same two maps, 16 detections, 1M particles, systematic resampling every step) on one Amcl
+    and on one ShardedAmcl of 2, 4 and 8 shards of device 0, and of 2, 4 and 8 devices where there are that many.  Shards
+    of one device share its SMs: those rows measure what sharding costs, not how it scales.  Host clock around each
+    update_landmarks (it ends synchronised), median of `steps` after `warmup`; each shard's reweight_landmark time from
+    its device timers (averaged over the steps), and whether the last particle set equals the single filter's."""
+    res = {}
+    device = device_record()
+    n, steps, warmup = 1 << 20, 10, 2
+    layouts = [("single", None)] + [(f"{k}_shards_device_0", [0] * k) for k in (2, 4, 8)]
+    layouts += [(f"{k}_devices", list(range(k))) for k in (2, 4, 8) if bb.device_count() >= k]
+    for map_name, pos, cat, det_pos, det_cat in landmark_maps():
+        for model in ("landmark", "bearing"):
+            reference = None
+            for name, devices in layouts:
+                if devices is None:
+                    f = bb.Amcl(bb.DifferentialDriveModelParam(*MOTION), landmark_params(n))
+                    shards = [f.filter]
+                else:
+                    f = bb.ShardedAmcl(bb.DifferentialDriveModelParam(*MOTION), landmark_params(n), devices)
+                    shards = f.shards
+                landmark_setup(f, model, pos, cat)
+                for s in shards:
+                    s.set_timing(True)
+                wall, reweight = [], [0.0] * len(shards)
+                for k in range(warmup + steps):
+                    for s in shards:
+                        s.clear_timings()
+                    t0 = time.perf_counter()
+                    r = f.update_landmarks([np.cos(0.01 * k), np.sin(0.01 * k), 0.05 * k, 0.0], det_pos, det_cat)
+                    dt = time.perf_counter() - t0
+                    assert r.updated == 1 and r.resampled == 1
+                    if k >= warmup:
+                        wall.append(dt * 1e3)
+                        for i, s in enumerate(shards):
+                            reweight[i] += dict(s.last_timings()).get("reweight_landmark", float("nan")) / steps
+                states, weights = f.particles()
+                if reference is None:
+                    reference = (states, weights)
+                res[f"sharded_landmark_{model}_1M_x_16_{map_name}_{name}"] = {
+                    "shards": 1 if devices is None else len(devices), "devices": [0] if devices is None else devices,
+                    "scaling": "one filter" if devices is None else ("measured" if len(set(devices)) > 1 else "not measured: the shards share one device"),
+                    "ms_per_step_e2e": float(np.median(wall)), "ms_per_step_min_max": [float(min(wall)), float(max(wall))], "steps": steps,
+                    "warmup": warmup, "reweight_landmark_ms_per_shard": [round(x, 4) for x in reweight],
+                    "equal_to_single_filter": bool(states.tobytes() == reference[0].tobytes() and weights.tobytes() == reference[1].tobytes()),
+                    "kernels_ms": {}, "device": device}
+                f.close()
     return res
 
 
@@ -1328,6 +1398,8 @@ def main():
         out.update(run_landmark())
     if "batch_landmark" in which:
         out.update(run_batch_landmark())
+    if "sharded_landmark" in which:
+        out.update(run_sharded_landmark())
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     path = os.path.join(ROOT, "gpurun_out", "configs.json")
     merged = json.load(open(path)) if os.path.exists(path) else {}
